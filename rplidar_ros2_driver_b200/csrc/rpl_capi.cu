@@ -184,8 +184,11 @@ rpl_result enqueue_args(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, uint32_t flag
     const bool emit = a.nodes_out != nullptr;
     const bool aligned = (reinterpret_cast<uintptr_t>(a.nodes) & 15u) == 0 && (stride & 1u) == 0;
     const bool use_tma = !emit && aligned && ((flags & RPL_FLAG_NO_TMA) == 0 || a.xyzi != nullptr);
+    // LaserScan Mode B scans too large for the shared-memory kernels but no larger than two SMs can stage
+    const bool use_cluster = use_tma && !a.xyzi && !a.mode_a && rpl::scan_tma_cluster_applies(stride);
     const int tma_grid = c->tma_grid[a.xyzi ? 2 : a.mode_a ? 1 : 0];
-    const int grid = (int)std::min<uint32_t>(n_scans, (uint32_t)(use_tma ? tma_grid : c->fast_grid));
+    const int grid = use_cluster ? 2 * (int)std::min<uint32_t>(n_scans, (uint32_t)c->tma_clusters)
+                                 : (int)std::min<uint32_t>(n_scans, (uint32_t)(use_tma ? tma_grid : c->fast_grid));
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (c->profile) {
       cudaEventCreate(&e0);
@@ -202,6 +205,8 @@ rpl_result enqueue_args(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, uint32_t flag
                                          fuse ? post->voxel : 0.0f, c->num_sms, stream),
                RPL_RESULT_OPERATION_FAIL);
       if (post_fused) *post_fused = fuse;
+    } else if (use_cluster) {
+      RPL_CUDA(c, rpl::launch_scan_tma_cluster(a, l.fws, grid, stream), RPL_RESULT_OPERATION_FAIL);
     } else if (use_tma) {
       RPL_CUDA(c, rpl::launch_scan_tma(a, l.fws, grid, stream), RPL_RESULT_OPERATION_FAIL);
     } else {
@@ -273,6 +278,11 @@ rpl_result rpl_ctx_create(int device, uint32_t max_nodes, uint32_t max_scans, rp
   const int occ = std::max(1, rpl::scan_fast_max_ctas_per_sm());
   c->fast_grid = c->num_sms * occ;
   for (int m = 0; m < 3; ++m) c->tma_grid[m] = c->num_sms * std::max(1, rpl::scan_tma_max_ctas_per_sm(m));
+  c->tma_clusters = rpl::scan_tma_max_clusters();
+  if (c->tma_clusters < 1) {
+    c->err = "scan_tma_cluster_kernel: no two-CTA cluster fits the device";
+    return fail(RPL_RESULT_OPERATION_FAIL);
+  }
   c->general_grid = c->num_sms;
 
   for (int i = 0; i < kLanes; ++i) {

@@ -47,6 +47,7 @@ struct rpl_ctx {
   uint32_t max_nodes = 0, max_scans = 0;
   int num_sms = 0;
   int fast_grid = 0, tma_grid[3] = {0, 0, 0}, general_grid = 0;  // tma_grid by scan_tma mode (B, A, cloud)
+  int tma_clusters = 0;  // resident two-CTA clusters of scan_tma_cluster_kernel
   Lane lane[kLanes];
   std::string err;
   uint64_t launches = 0;

@@ -11,8 +11,6 @@ SRCS=("$HERE"/csrc/*.cu)
 CFLAGS=(-gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo --fmad=false \
         -Xcompiler -fPIC,-O2,-ffp-contract=off,-Wall,-Wno-address-of-packed-member)
 if [[ "${RPL_PTXAS_V:-0}" == "1" ]]; then CFLAGS+=(-Xptxas -v); fi
-# extra -D tuning switches for experiments, e.g. RPL_DEFS="-DRPL_TMA_CH=1024 -DRPL_TMA_STAGES=4"
-if [[ -n "${RPL_DEFS:-}" ]]; then CFLAGS+=(${RPL_DEFS}); fi
 # a change of flags or of any header rebuilds everything
 STAMP="$OBJ/.flags"
 NEWEST_HDR=$(ls -t "$HERE"/csrc/*.h "$HERE"/csrc/*.cuh "$HERE"/../include/*.h | head -1)

@@ -206,9 +206,9 @@ rpl_result enqueue_args(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, uint32_t flag
                RPL_RESULT_OPERATION_FAIL);
       if (post_fused) *post_fused = fuse;
     } else if (use_cluster) {
-      RPL_CUDA(c, rpl::launch_scan_tma_cluster(a, l.fws, grid, stream), RPL_RESULT_OPERATION_FAIL);
+      RPL_CUDA(c, rpl::launch_scan_tma_cluster(a, l.fws.max_nodes, grid, stream), RPL_RESULT_OPERATION_FAIL);
     } else if (use_tma) {
-      RPL_CUDA(c, rpl::launch_scan_tma(a, l.fws, grid, stream), RPL_RESULT_OPERATION_FAIL);
+      RPL_CUDA(c, rpl::launch_scan_tma(a, l.fws.max_nodes, grid, stream), RPL_RESULT_OPERATION_FAIL);
     } else {
       RPL_CUDA(c, rpl::launch_scan_fast(a, l.fws, grid, stream), RPL_RESULT_OPERATION_FAIL);
     }
@@ -290,7 +290,7 @@ rpl_result rpl_ctx_create(int device, uint32_t max_nodes, uint32_t max_scans, rp
     const rpl_result oom = RPL_RESULT_INSUFFICIENT_MEMORY;
     if (!cuda_ok(c, cudaStreamCreateWithFlags(&l.stream, cudaStreamNonBlocking), "cudaStreamCreate"))
       return fail(RPL_RESULT_OPERATION_FAIL);
-    const size_t fast_nodes = (size_t)std::max({c->fast_grid, c->tma_grid[0], c->tma_grid[1], c->tma_grid[2]}) * max_nodes;
+    const size_t fast_nodes = (size_t)c->fast_grid * max_nodes;  // launch_scan_fast never gets a larger grid
     const size_t gen_nodes = (size_t)c->general_grid * max_nodes;
     l.fws.max_nodes = max_nodes;
     l.gws.max_nodes = max_nodes;
@@ -625,7 +625,7 @@ rpl_result scan_single(rpl_ctx* c, const rpl_node_hq* nodes_in, size_t count, co
   if (!force_general) {
     const bool use_tma = !want_nodes && (p->flags & RPL_FLAG_NO_TMA) == 0;  // d_one and S keep bases 16-byte aligned
     if (use_tma)
-      RPL_CUDA(c, rpl::launch_scan_tma(a, l.fws, 1, l.stream), RPL_RESULT_OPERATION_FAIL);
+      RPL_CUDA(c, rpl::launch_scan_tma(a, l.fws.max_nodes, 1, l.stream), RPL_RESULT_OPERATION_FAIL);
     else
       RPL_CUDA(c, rpl::launch_scan_fast(a, l.fws, 1, l.stream), RPL_RESULT_OPERATION_FAIL);
     c->launches++;

@@ -12,6 +12,7 @@ namespace rpl {
 
 constexpr uint32_t kKeySpace = 65536;  // angle_z_q14 is a u16: 65536 units = 360 degrees
 constexpr uint32_t kResultOk = 0u;
+constexpr uint32_t kResultInvalidData = 0x80008000u;    // SL_RESULT_INVALID_DATA
 constexpr uint32_t kResultOperationFail = 0x80008001u;  // SL_RESULT_OPERATION_FAIL
 
 // A packed node (reference sl_lidar_cmd.h:272-278) seen as two little-endian words:
@@ -95,6 +96,14 @@ __device__ __forceinline__ float small_uint_to_float(uint32_t q) {
 __device__ __forceinline__ float quality_to_intensity(uint32_t q, bool new_protocol) {
   return small_uint_to_float(new_protocol ? q : (q >> 2));
 }
+// the same intensity taken straight from node word y, with the protocol's shift and mask fixed once per launch
+struct IntensityOf {
+  uint32_t shift, mask;
+  __device__ __forceinline__ explicit IntensityOf(bool new_protocol)
+      : shift(new_protocol ? 16u : 18u), mask(new_protocol ? 0xFFu : 0x3Fu) {}
+  __device__ __forceinline__ uint32_t units(uint32_t y) const { return (y >> shift) & mask; }
+  __device__ __forceinline__ float operator()(uint32_t y) const { return small_uint_to_float(units(y)); }
+};
 
 // LaserScan.angle_increment (reference rplidar_node.cpp:633-634 Mode A, :664-666 Mode B)
 __device__ __forceinline__ float angle_increment(uint32_t m, bool mode_a) {
@@ -170,14 +179,8 @@ __device__ __forceinline__ uint32_t warp_inclusive_scan(uint32_t v) {
 // The policies are the fixed encodings createpolicy.fractional.L2::evict_{last,first} (1.0)
 // produces (the same constants CUTLASS passes as TMA cache hints); as immediates they live in
 // uniform registers instead of being re-broadcast from a per-thread register at every access.
-#ifndef RPL_POLICY_KEEP
-#define RPL_POLICY_KEEP 0x14F0000000000000ull   /* evict_last */
-#endif
-#ifndef RPL_POLICY_STREAM
-#define RPL_POLICY_STREAM 0x12F0000000000000ull /* evict_first */
-#endif
-__device__ __forceinline__ uint64_t l2_policy_evict_last() { return RPL_POLICY_KEEP; }
-__device__ __forceinline__ uint64_t l2_policy_evict_first() { return RPL_POLICY_STREAM; }
+__device__ __forceinline__ uint64_t l2_policy_evict_last() { return 0x14F0000000000000ull; }
+__device__ __forceinline__ uint64_t l2_policy_evict_first() { return 0x12F0000000000000ull; }
 __device__ __forceinline__ uint4 ld_hint_v4(const void* p, uint64_t pol) {
   uint4 r;
   asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
@@ -191,9 +194,6 @@ __device__ __forceinline__ uint2 ld_hint_v2(const void* p, uint64_t pol) {
                : "=r"(r.x), "=r"(r.y)
                : "l"(p), "l"(pol));
   return r;
-}
-__device__ __forceinline__ void st_hint_f32(float* p, float v, uint64_t pol) {
-  asm volatile("st.global.L1::no_allocate.L2::cache_hint.f32 [%0], %1, %2;" ::"l"(p), "f"(v), "l"(pol));
 }
 __device__ __forceinline__ void st_hint_v2(uint2* p, uint2 v, uint64_t pol) {
   asm volatile("st.global.L1::no_allocate.L2::cache_hint.v2.u32 [%0], {%1,%2}, %3;" ::"l"(p), "r"(v.x), "r"(v.y), "l"(pol));
@@ -210,14 +210,7 @@ __device__ __forceinline__ bool cloud_keep(float dm, float inten, float rmin, fl
   return !(dm < rmin) && !(dm > rmax) && !(inten < imin);
 }
 
-// streaming global accesses: inputs are read at most twice, outputs written once
-__device__ __forceinline__ uint4 ld_stream_v4(const void* p) {
-  uint4 r;
-  asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
-               : "l"(p));
-  return r;
-}
+// streaming global load: inputs are read at most twice
 __device__ __forceinline__ uint2 ld_stream_v2(const void* p) {
   uint2 r;
   asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0,%1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));

@@ -89,13 +89,13 @@ cudaError_t scan_fast_configure();     // opt-in dynamic shared memory, once per
 cudaError_t scan_general_configure();
 int scan_fast_max_ctas_per_sm();
 // v2: TMA-ring kernel (scan_tma.cu); needs 16-byte aligned scan bases
-cudaError_t launch_scan_tma(const ScanBatchArgs& a, const FastWorkspace& ws, int grid, cudaStream_t stream);
+cudaError_t launch_scan_tma(const ScanBatchArgs& a, uint32_t max_nodes, int grid, cudaStream_t stream);
 cudaError_t scan_tma_configure();
 int scan_tma_max_ctas_per_sm(int mode);  // mode: 0 LaserScan Mode B, 1 Mode A, 2 PointCloud2
 // LaserScan Mode B without the ascended buffer for strides in (kSmallMaxNodes, 32768]: each scan staged whole
 // across a cluster of two CTAs (scan_tma.cu); 16-byte aligned scan bases, even grid of 2 x clusters
 bool scan_tma_cluster_applies(uint32_t stride);
-cudaError_t launch_scan_tma_cluster(const ScanBatchArgs& a, const FastWorkspace& ws, int grid, cudaStream_t stream);
+cudaError_t launch_scan_tma_cluster(const ScanBatchArgs& a, uint32_t max_nodes, int grid, cudaStream_t stream);
 int scan_tma_max_clusters();  // two-CTA clusters of that kernel resident at once on the current device
 
 }  // namespace rpl

@@ -1,10 +1,9 @@
-// scan_common.cuh -- device code shared by the two fast scan kernels (scan_fast.cu: register-
-// streamed v1, scan_tma.cu: TMA-ring v2): rank lookup in the key bitmap and the Mode A
-// bin-ownership logic.
+// scan_common.cuh -- device code used by more than one scan kernel (scan_small.cu, scan_fast.cu, and the ring and
+// cluster kernels of scan_tma.cu): the per-scan outcome record, the Mode B output slots, the 64 KB presence byte
+// map with its rank table, and the Mode A bin-ownership logic.
 #pragma once
-#include <type_traits>
-
 #include "rpl_device.cuh"
+#include "scan_args.h"
 
 namespace rpl {
 namespace {
@@ -12,28 +11,22 @@ namespace {
 constexpr uint32_t kWords = kKeySpace / 32;     // 2048 bitmap words
 constexpr uint32_t kMaxFastNodes = kKeySpace;   // more nodes cannot be tie-free
 
-__device__ __forceinline__ uint32_t rank_of(const uint2* rk, uint32_t key) {
-  const uint2 e = rk[key >> 5];
-  return e.y + __popc(e.x & ((1u << (key & 31)) - 1u));
+// ---- the per-scan outcome (one thread writes it) ----------------------------------------------------------------
+__device__ __forceinline__ void write_outcome(const ScanBatchArgs& a, uint32_t s, uint32_t status, uint32_t beams,
+                                              float inc) {
+  if (a.status) a.status[s] = status;
+  if (a.path) a.path[s] = 0u;
+  if (a.beam_counts) a.beam_counts[s] = beams;
+  if (a.angle_inc) a.angle_inc[s] = inc;
 }
-// largest set key < k (or -1) / smallest set key > k (or -1)
-__device__ __forceinline__ int prev_set(const uint2* rk, uint32_t k) {
-  int w = (int)(k >> 5);
-  uint32_t m = rk[w].x & ((1u << (k & 31)) - 1u);
-  for (;;) {
-    if (m) return (w << 5) + 31 - __clz(m);
-    if (w == 0) return -1;
-    m = rk[--w].x;
-  }
+// no measured node: ascendScanData returns OPERATION_FAIL and leaves the buffer untouched; publish_scan publishes
+// nothing
+__device__ __forceinline__ void write_outcome_empty(const ScanBatchArgs& a, uint32_t s) {
+  write_outcome(a, s, a.apply_ascend ? kResultOperationFail : kResultOk, 0u, 0.0f);
 }
-__device__ __forceinline__ int next_set(const uint2* rk, uint32_t k) {
-  uint32_t w = k >> 5;
-  uint32_t m = rk[w].x & ~((2u << (k & 31)) - 1u);
-  for (;;) {
-    if (m) return (int)((w << 5) + __ffs(m) - 1);
-    if (++w == kWords) return -1;
-    m = rk[w].x;
-  }
+// scan s goes to the general kernel, which runs after this one and follows the stable tie rule
+__device__ __forceinline__ void hand_to_general(const ScanBatchArgs& a, uint32_t s) {
+  a.fallback_list[atomicAdd(a.fallback_count, 1u)] = s;
 }
 
 // predicated streaming stores (no branch around them)
@@ -44,19 +37,118 @@ __device__ __forceinline__ void st_f32_if(float* p, float v, uint64_t pol, uint3
       "f"(v), "l"(pol), "r"(pred));
 }
 
+// ---- Mode B output (reference rplidar_node.cpp:661-677) ---------------------------------------------------------
+// The point of rank r among the M measured points goes to slot ob + os * r in wrapping u32 arithmetic (reference
+// :673); intensities[] sits at a fixed byte distance from ranges[].
+struct ModeBOut {
+  float* ranges;
+  ptrdiff_t i_minus_r;
+  uint32_t ob, os;
+  __device__ __forceinline__ ModeBOut(float* r, float* i, uint32_t M, bool inverted)
+      : ranges(r),
+        i_minus_r(reinterpret_cast<char*>(i) - reinterpret_cast<char*>(r)),
+        ob(inverted ? M - 1u : 0u),
+        os(inverted ? 0xFFFFFFFFu : 1u) {}
+  __device__ __forceinline__ void store(uint32_t rank, float dist_m, float intensity, uint32_t pred) const {
+    float* pr = ranges + (ob + os * rank);
+    st_f32_if(pr, dist_m, l2_policy_evict_first(), pred);
+    st_f32_if(reinterpret_cast<float*>(reinterpret_cast<char*>(pr) + i_minus_r), intensity, l2_policy_evict_first(),
+              pred);
+  }
+};
+
+// ---- the presence byte map of scan_fast.cu and scan_tma.cu --------------------------------------------------------
+// One byte per key, marked with plain byte stores, then folded to bit-words by kMapThreads threads: thread t owns
+// keys [128 t, 128 t + 128), a 128-byte row of eight 16-byte columns.
+constexpr int kMapThreads = 512;
+constexpr int kMapWarps = kMapThreads / 32;
+constexpr uint32_t kWordsPerThread = kWords / kMapThreads;  // 4 bit-words per row
+
+// barrier of the kMapThreads threads (named barrier 1: the TMA kernels' producer warp stays out)
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kMapThreads) : "memory"); }
+
+// address swizzle: within a row the 16-byte column is XORed with row & 7, so that the 128-bit reads of 8
+// neighbouring threads in the fold hit 8 different bank groups.  Takes the raw first word of a node (key in the
+// low 16 bits).
+__device__ __forceinline__ uint32_t swz_x(uint32_t x) { return (x ^ ((x >> 3) & 0x70u)) & 0xFFFFu; }
+// bit 0 of each of the four bytes of x -> bits 0..3
+__device__ __forceinline__ uint32_t gather4(uint32_t x) { return (x * 0x10204080u) >> 28; }
+
+__device__ __forceinline__ void bytemap_clear(uint8_t* bytemap, uint32_t tid) {
+  uint4* bm = reinterpret_cast<uint4*>(bytemap);
+  const uint4 z = make_uint4(0, 0, 0, 0);
+#pragma unroll
+  for (uint32_t j = 0; j < kKeySpace / 16 / kMapThreads; ++j) bm[j * kMapThreads + tid] = z;
+}
+
+// fold: thread tid gathers bit 0 of the presence bytes of its row into its kWordsPerThread bit-words
+__device__ __forceinline__ void fold_row(const uint8_t* bytemap, uint32_t tid, uint32_t (&wv)[kWordsPerThread]) {
+#pragma unroll
+  for (uint32_t j = 0; j < kWordsPerThread; ++j) wv[j] = 0;
+  const uint4* bm = reinterpret_cast<const uint4*>(bytemap);
+#pragma unroll
+  for (uint32_t c = 0; c < 8; ++c) {
+    const uint4 q = bm[tid * 8 + (c ^ (tid & 7u))];  // physical column of logical chunk c
+    const uint32_t x[4] = {q.x, q.y, q.z, q.w};
+    uint32_t bv = 0;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) bv |= gather4(x[j] & 0x01010101u) << (4 * j);
+    wv[c >> 1] |= bv << (16 * (c & 1));
+  }
+}
+
+// Rank table from the folded bit-words, by all kMapThreads threads (two consumer_sync barriers inside):
+// sm.rankV[w] = {bits of word w, set bits in the words below w}.  On entry sm.red[0 .. kMapWarps) holds the warps'
+// measured counts; sm.red[2 kMapWarps .. 3 kMapWarps) is scratch.  Sets sm.totV to the set bits of the whole table and
+// sm.valid_count to the measured count plus `extra_count`.  Read them after a further barrier.
+template <class Smem>
+__device__ __forceinline__ void rank_table(Smem& sm, const uint32_t (&wv)[kWordsPerThread], uint32_t tid,
+                                           uint32_t extra_count) {
+  const uint32_t lane = tid & 31, warp = tid >> 5;
+  uint32_t sv = 0;
+#pragma unroll
+  for (uint32_t j = 0; j < kWordsPerThread; ++j) sv += __popc(wv[j]);
+  const uint32_t iv = warp_inclusive_scan(sv);
+  if (lane == 31) sm.red[2 * kMapWarps + warp] = iv;
+  consumer_sync();
+  if (warp == 0) {
+    uint32_t tv = lane < kMapWarps ? sm.red[2 * kMapWarps + lane] : 0u;
+    uint32_t cc = lane < kMapWarps ? sm.red[lane] : 0u;
+    const uint32_t cv = warp_inclusive_scan(tv);
+    cc = warp_sum(cc);
+    if (lane < kMapWarps) sm.red[2 * kMapWarps + lane] = cv - tv;
+    if (lane == 31) {
+      sm.totV = cv;
+      sm.valid_count = cc + extra_count;
+    }
+  }
+  consumer_sync();
+  uint32_t pv = sm.red[2 * kMapWarps + warp] + iv - sv;
+#pragma unroll
+  for (uint32_t j = 0; j < kWordsPerThread; ++j) {
+    sm.rankV[tid * kWordsPerThread + j] = make_uint2(wv[j], pv);
+    pv += __popc(wv[j]);
+  }
+}
+
+__device__ __forceinline__ uint32_t rank_of(const uint2* rk, uint32_t key) {
+  const uint2 e = rk[key >> 5];
+  return e.y + __popc(e.x & ((1u << (key & 31)) - 1u));
+}
+
 // ---- Mode A (reference rplidar_node.cpp:630-660) ------------------------------------------
 // beam_count = M bins; every measured point goes to bin (int)(angle / angle_increment) and the
 // bin keeps the smallest dist_m (strict '<': on equal dist_m the first point in ascending key
 // order, i.e. the smallest key).
 //
 // Bins grow with the key -- for inverted scans along "key 0 first, then descending keys" -- so in
-// that order (the "u-order") the points of a bin are neighbours.  The place pass therefore
-// writes one packed entry per measured point at its u-rank into a per-CTA scratch
+// that order (the "u-order") the points of a bin are neighbours.  The place pass of scan_fast.cu
+// and scan_tma.cu therefore records every measured point at its u-rank, ordered by
 //     entry = dist_m bits << 32 | key << 8 | quality          (u64 min = min (dist_m, key))
-// and mode_a_emit() walks the entries in order: every warp owns a contiguous slice, finds the
-// runs of equal bins, takes their minimum with a segmented shuffle scan, and writes each bin
-// exactly once (empty bins included) with converged, mostly coalesced stores.  No atomics, no
-// block-wide barriers inside the walk.
+// and the emit pass (mode_a_emit, mode_a_emit_smem) walks the entries in order: every warp owns a
+// contiguous slice, finds the runs of equal bins, takes their minimum, and writes each bin exactly
+// once (empty bins included) with converged, mostly coalesced stores.  No atomics, no block-wide
+// barriers inside the walk.
 __device__ __forceinline__ uint32_t mode_a_urank(uint32_t key, uint32_t rank, uint32_t M, bool inverted,
                                                  bool has0) {
   if (!inverted) return rank;
@@ -89,206 +181,6 @@ __device__ __forceinline__ void mode_a_fill_empty(const ModeAOut& o, int from, i
   for (int e = from; e < to; ++e) {
     o.ranges[e] = kInf;
     o.intens[e] = 0.0f;
-  }
-}
-
-// One warp of `nwarps`; E = entries in u-order.  Call with all 32 lanes converged.
-//
-// Ownership: a run (maximal stretch of equal bins) belongs to the warp whose slice holds its
-// first entry.  The owner writes the run's bin and the empty bins in front of it; the owner of
-// the last run also writes the empty bins behind it.  A warp therefore may read past the end of
-// its slice to finish a run it owns, and skips leading entries that continue a run of the
-// previous slice.
-constexpr uint32_t kEmitBatch = 256;                 // entries a warp stages per batch
-constexpr uint32_t kEmitStage = kEmitBatch + 33;     // + the entry before and 32 after (look-ahead)
-constexpr uint32_t kEmitStageBytes = (kEmitStage * 12 + 15) & ~15u;  // u64 entry + i32 bin per staged entry
-
-// Every entry is handled by one lane, independently of all others: the lane that holds the
-// first entry of a run (bin differs from the previous entry's) takes the run's minimum by
-// looking ahead, writes the bin, and fills the empty bins in front of it; the lane holding the
-// very last entry fills the empty bins behind it.  A warp stages 256 entries (+ one before,
-// 32 after) and their bins in its private slice of shared memory, so all loads and bin
-// evaluations of a batch are in flight together and the per-entry work reads shared memory.
-// `stage`: kEmitStageBytes of shared memory private to this warp.  Call converged.
-__device__ __forceinline__ void mode_a_emit(const ModeAOut& o, const unsigned long long* E, uint32_t warp,
-                                            uint32_t nwarps, unsigned char* stage) {
-  const uint32_t lane = threadIdx.x & 31u;
-  const uint32_t M = o.M;
-  const uint32_t len = ((M + nwarps - 1u) / nwarps + kEmitBatch - 1u) & ~(kEmitBatch - 1u);  // whole batches
-  const uint32_t r_begin = min(M, warp * len), r_end = min(M, r_begin + len);
-  if (r_begin >= r_end) return;
-  unsigned long long* se = reinterpret_cast<unsigned long long*>(stage);
-  int* sb = reinterpret_cast<int*>(stage + kEmitStage * 8);
-  // (int)((angle - angle_min) / angle_increment) with the reference's own float angle from the
-  // table: exact, no double precision, no divergence
-  auto bin_of = [&](unsigned long long e) {
-    const float2 a = __ldg(o.angle + ((uint32_t)(e >> 8) & 0xFFFFu));
-    return __float2int_rz(__fdiv_rn(o.inverted ? a.y : a.x, o.inc));
-  };
-  const int kNoBin = 0x7fffffff;
-  const float kInf = __int_as_float(0x7f800000);
-
-  for (uint32_t base = r_begin; base < r_end; base += kEmitBatch) {
-    __syncwarp();
-    for (uint32_t t = lane; t < kEmitStage; t += 32) {  // staged index t <-> rank base - 1 + t
-      const long long r = (long long)base - 1 + t;
-      unsigned long long e = ~0ull;
-      int b = (r < 0) ? -1 : kNoBin;
-      if (r >= 0 && r < (long long)M) {
-        e = E[r];
-        b = bin_of(e);
-      }
-      se[t] = e;
-      sb[t] = b;
-    }
-    __syncwarp();
-#pragma unroll 2
-    for (uint32_t w = 0; w < kEmitBatch / 32; ++w) {
-      const uint32_t i = 1 + w * 32 + lane;
-      const uint32_t r = base + w * 32 + lane;
-      const bool live = r < M;
-      const int b = sb[i], bprev = sb[i - 1];
-      const bool head = live && (b != bprev);
-      unsigned long long v = se[i];
-      if (head && sb[i + 1] == b) {
-        v = min(v, se[i + 1]);
-        if (sb[i + 2] == b) {  // a run of three or more: walk it (rare with M points in M bins)
-          uint32_t j = i + 2;
-          while (j < kEmitStage && sb[j] == b) {
-            v = min(v, se[j]);
-            ++j;
-          }
-          if (j == kEmitStage) {
-            for (uint32_t rr = base - 1 + j; rr < M; ++rr) {
-              const unsigned long long ee = E[rr];
-              if (bin_of(ee) != b) break;
-              v = min(v, ee);
-            }
-          }
-        }
-      }
-      mode_a_store_bin(o, head ? b : 0, v, head ? 1u : 0u);
-      if (head && b - bprev > 1) {  // empty bins in front of this run
-        if (b - bprev == 2) {
-          o.ranges[b - 1] = kInf;
-          o.intens[b - 1] = 0.0f;
-        } else {
-          mode_a_fill_empty(o, bprev + 1, b);
-        }
-      }
-      if (live && r == M - 1u) mode_a_fill_empty(o, b + 1, (int)M);  // empty bins behind the last run
-    }
-  }
-}
-
-// ---- Mode A emit, shared-memory variant (scan_tma.cu) ----------------------------------------
-// ncu on the variant above showed the scratch doubling DRAM traffic (8 B written + 8 B read per
-// point through a 76 MB working set).  Here the place pass only records WHICH node sits at each
-// u-rank, as a u16 node index in the 64 KB the dead presence map leaves free (so M <= 32768),
-// and the emit pass gathers the nodes from the tile again (L2 hits, coalesced for a sorted
-// revolution).  Bins of a batch are staged per warp in the (equally dead) rank table.
-constexpr uint32_t kEmit2Batch = 256;
-constexpr uint32_t kEmit2Stage = kEmit2Batch + 33;  // staged bins: one entry before, 32 after
-constexpr uint32_t kModeASmemMaxPoints = kKeySpace / 2;
-
-__device__ __forceinline__ void mode_a_emit_smem(const ModeAOut& o, const uint16_t* sidx, const uint2* tile,
-                                                 uint32_t warp, uint32_t nwarps, uint16_t* sb) {
-  const uint32_t lane = threadIdx.x & 31u;
-  const uint32_t M = o.M;
-  const uint32_t len = ((M + nwarps - 1u) / nwarps + kEmit2Batch - 1u) & ~(kEmit2Batch - 1u);
-  const uint32_t r_begin = min(M, warp * len), r_end = min(M, r_begin + len);
-  if (r_begin >= r_end) return;
-  const bool inverted = o.inverted;
-  const float inc = o.inc;
-  // integer quotient where the float chain provably agrees, else the exact chain in registers
-  // (FP64, no memory access): this pass is bound by load latency, not by issue slots, so the
-  // table lookup of mode_a_emit would only add a dependent L2 access per entry
-  auto bin_of_key = [&](uint32_t key) { return (uint32_t)mode_a_bin_fast(key, M, inc, inverted); };
-  const uint32_t kNoBin = 0xFFFFu, kBeforeFirst = 0xFFFEu;  // real bins are < 32768
-  const float kInf = __int_as_float(0x7f800000);
-  auto entry_of = [&](uint2 nd) {
-    return mode_a_entry(dist_to_m(__funnelshift_r(nd.x, nd.y, 16)), nd.x & 0xFFFFu, (nd.y >> 16) & 0xFFu);
-  };
-  constexpr int kW = kEmit2Batch / 32;
-  using Checked = std::integral_constant<bool, true>;
-  using Unchecked = std::integral_constant<bool, false>;
-
-  auto batch = [&](auto checked, uint32_t base) {
-    constexpr bool CK = decltype(checked)::value;
-    __syncwarp();
-    // stage: this lane's own eight entries (kept in registers) plus one halo entry (the entry
-    // before the batch for lane 0, the 32 after it for the others); all gathers issued together
-    uint2 nd[kW];
-#pragma unroll
-    for (int w = 0; w < kW; ++w) {
-      const uint32_t r = base + w * 32 + lane;
-      nd[w] = (!CK || r < M) ? tile[sidx[r]] : make_uint2(0, 0);
-    }
-    const uint32_t th = (lane == 0) ? 0u : (kEmit2Batch + lane);  // lane 0 -> before; 1..31 -> after
-    const long long rh = (long long)base - 1 + th;
-    const bool halo_ok = !CK || (rh >= 0 && rh < (long long)M);
-    const uint2 ndh = halo_ok ? tile[sidx[halo_ok ? rh : 0]] : make_uint2(0, 0);
-    const uint32_t r2 = base - 1 + kEmit2Batch + 32;  // last look-ahead slot (lane 31)
-    const bool last_ok = (lane == 31) && (!CK || r2 < M);
-    const uint2 nd2 = last_ok ? tile[sidx[last_ok ? r2 : 0]] : make_uint2(0, 0);
-#pragma unroll
-    for (int w = 0; w < kW; ++w) {
-      const uint32_t r = base + w * 32 + lane;
-      sb[1 + w * 32 + lane] = (!CK || r < M) ? (uint16_t)bin_of_key(nd[w].x & 0xFFFFu) : (uint16_t)kNoBin;
-    }
-    {
-      uint32_t b = (CK && rh < 0) ? kBeforeFirst : kNoBin;
-      if (halo_ok) b = bin_of_key(ndh.x & 0xFFFFu);
-      sb[th] = (uint16_t)b;
-      if (lane == 31) sb[kEmit2Batch + 32] = last_ok ? (uint16_t)bin_of_key(nd2.x & 0xFFFFu) : (uint16_t)kNoBin;
-    }
-    __syncwarp();
-#pragma unroll
-    for (int w = 0; w < kW; ++w) {
-      const uint32_t i = 1 + w * 32 + lane;
-      const uint32_t r = base + w * 32 + lane;
-      const bool live = !CK || r < M;
-      const uint32_t b = sb[i], bprev = sb[i - 1];
-      const bool head = live && (b != bprev);
-      unsigned long long v = entry_of(nd[w]);
-      // the next entry's node sits in the neighbouring lane (or lane 0 of the next window):
-      // a bin shared by two points -- the usual collision -- costs two shuffles, no memory access
-      uint2 nxt;
-      nxt.x = __shfl_down_sync(0xffffffffu, nd[w].x, 1);
-      nxt.y = __shfl_down_sync(0xffffffffu, nd[w].y, 1);
-      if (w + 1 < kW) {
-        const uint32_t fx = __shfl_sync(0xffffffffu, nd[(w + 1) % kW].x, 0);
-        const uint32_t fy = __shfl_sync(0xffffffffu, nd[(w + 1) % kW].y, 0);
-        if (lane == 31) nxt = make_uint2(fx, fy);
-      }
-      if (head && sb[i + 1] == b) {
-        if (w + 1 == kW && lane == 31) nxt = tile[sidx[r + 1]];  // first entry of the next batch
-        v = min(v, entry_of(nxt));
-        if (sb[i + 2] == b) {  // three or more points in the bin: walk on (rare: M points, M bins)
-          for (uint32_t rr = r + 2; rr < M; ++rr) {
-            const uint2 other = tile[sidx[rr]];
-            if (bin_of_key(other.x & 0xFFFFu) != b) break;
-            v = min(v, entry_of(other));
-          }
-        }
-      }
-      mode_a_store_bin(o, head ? (int)b : 0, v, head ? 1u : 0u);
-      const int gap_from = (CK && bprev == kBeforeFirst) ? 0 : (int)bprev + 1;
-      if (head && (int)b > gap_from) {  // empty bins in front of this run
-        if ((int)b - gap_from == 1) {
-          o.ranges[gap_from] = kInf;
-          o.intens[gap_from] = 0.0f;
-        } else {
-          mode_a_fill_empty(o, gap_from, (int)b);
-        }
-      }
-      if (CK && live && r == M - 1u) mode_a_fill_empty(o, (int)b + 1, (int)M);  // empty bins behind the last run
-    }
-  };
-  for (uint32_t base = r_begin; base < r_end; base += kEmit2Batch) {
-    // interior batches (entry before and all 256 + 32 look-ahead entries exist) skip every range check
-    if (base >= 1u && base + kEmit2Batch + 32u <= M) batch(Unchecked{}, base);
-    else batch(Checked{}, base);
   }
 }
 

@@ -127,7 +127,7 @@ __global__ void __launch_bounds__(GT, 1)
 
     if (n > a.stride || n > ws.max_nodes) {  // caller error: report, touch nothing
       if (tid == 0) {
-        if (a.status) a.status[s] = 0x80008000u;  // SL_RESULT_INVALID_DATA
+        if (a.status) a.status[s] = kResultInvalidData;
         if (a.path) a.path[s] = 1u;
         if (a.beam_counts) a.beam_counts[s] = 0u;
         if (a.angle_inc) a.angle_inc[s] = 0.0f;

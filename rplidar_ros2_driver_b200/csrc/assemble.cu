@@ -1,5 +1,5 @@
 // assemble.cu -- scan assembly on the GPU (SURVEY.md 8(f) rank 2): cuts decoded node streams into
-// scans, the bridge between decode.cu and the scan kernels without a host round trip.
+// scans, the bridge between the decoders and the scan kernels without a host round trip.
 //
 // Replaces ScanDataHolder::pushScanNodeData / rewindCurrentScanData (reference
 // src/sdk/src/sl_lidar_driver.cpp:272-315) as a pure function of the node stream and the

@@ -1,4 +1,4 @@
-// decode_args.h -- argument block of the dense-capsule decode kernel (decode.cu).
+// decode_args.h -- argument blocks of the decode, framing, timestamp and assembly kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -7,36 +7,26 @@
 
 namespace rpl {
 
-struct DecodeArgs {
-  const uint8_t* capsules;        // [n_streams][stride_capsules][84], stream bases 4-byte aligned
-  const uint32_t* counts;         // [n_streams] capsules per stream
-  uint32_t n_streams;
-  uint32_t stride_capsules;
-  uint32_t sample_duration_us;    // SlamtecLidarTimingDesc::sample_duration_uS (jump threshold)
-  const uint32_t* sync_state_in;  // [n_streams] lastNodeSyncBit entering each stream (nullable: 0)
-  uint2* nodes_out;               // [n_streams][stride_capsules * 40]
-  uint32_t* node_counts;          // [n_streams]
-  uint32_t* capsule_status;       // [n_streams][stride_capsules] nullable
-  uint32_t* capsule_node_offset;  // [n_streams][stride_capsules] nullable
-  uint32_t* sync_state_out;       // [n_streams] nullable
-  // positions (node offsets) of the scan-start nodes of every stream, in no particular order (nullable): what
-  // rpl_assemble_scan_views_dev otherwise finds by reading every node again
-  uint32_t* scan_starts;          // [n_streams][starts_stride]
-  uint32_t* scan_start_counts;    // [n_streams] (may exceed starts_stride: the list is then incomplete)
-  uint32_t starts_stride;
-};
-
-// the other capsule formats (decode_formats.cu): 0x82 express, 0x83 HQ, 0x84 ultra, 0x86 ultra-dense
+// the capsule formats (decode_formats.cu): 0x82 express, 0x83 HQ, 0x84 ultra, 0x85 dense, 0x86 ultra-dense
 struct CapsuleDecodeArgs {
   const uint8_t* capsules;        // [n_streams][stride_capsules][capsule bytes]
   const uint32_t* counts;         // [n_streams]
-  uint32_t n_streams, stride_capsules, sample_duration_us;
-  const uint32_t* state_in;       // [n_streams][2] {last node sync bit, last distance} (nullable: 0)
+  uint32_t n_streams, stride_capsules;
+  uint32_t sample_duration_us;    // SlamtecLidarTimingDesc::sample_duration_uS (jump threshold)
+  // words per stream of state_in / state_out: 1 = {last node sync bit} (the dense entry points), 2 = {last node
+  // sync bit, last distance} (rpl_decode_capsules_batch_dev)
+  uint32_t state_words;
+  const uint32_t* state_in;       // [n_streams][state_words] (nullable: 0)
   uint2* nodes_out;               // [n_streams][stride_capsules * nodes per capsule]
   uint32_t* node_counts;          // [n_streams]
   uint32_t* capsule_status;       // nullable
   uint32_t* capsule_node_offset;  // nullable
-  uint32_t* state_out;            // [n_streams][2] nullable
+  uint32_t* state_out;            // [n_streams][state_words] nullable
+  // positions (node offsets) of the scan-start nodes of every stream, in no particular order (nullable; the dense
+  // entry points only): what rpl_assemble_scan_views_dev otherwise finds by reading every node again
+  uint32_t* scan_starts;          // [n_streams][starts_stride]
+  uint32_t* scan_start_counts;    // [n_streams] (may exceed starts_stride: the list is then incomplete)
+  uint32_t starts_stride;
 };
 
 // 5-byte standard nodes from raw byte streams
@@ -113,7 +103,5 @@ struct FrameArgs {
 };
 cudaError_t launch_frame_capsules(const FrameArgs& a, int grid, cudaStream_t stream);
 cudaError_t launch_assemble(const AssembleArgs& a, int grid, cudaStream_t stream);
-cudaError_t launch_decode_dense(const DecodeArgs& a, int grid, cudaStream_t stream);
-cudaError_t decode_configure();  // opt-in dynamic shared memory, once per device
 
 }  // namespace rpl

@@ -1,23 +1,28 @@
-// decode_formats.cu -- the other measurement answer formats on the GPU (SURVEY.md 8(f) rank 1).
+// decode_formats.cu -- the measurement answer formats on the GPU (SURVEY.md 8(f) rank 1).
 //
 // Replaces, for framed capsules (reference src/sdk/src/dataunpacker/unpacker/):
 //   0x82 express      UnpackerHandler_CapsuleNode            handler_capsules.cpp:109-266  (84 B -> 32 nodes)
 //   0x84 ultra        UnpackerHandler_UltraCapsuleNode       handler_capsules.cpp:324-580  (132 B -> 96 nodes)
+//   0x85 dense        UnpackerHandler_DenseCapsuleNode       handler_capsules.cpp:639-791  (84 B -> 40 nodes)
 //   0x86 ultra-dense  UnpackerHandler_UltraDenseCapsuleNode  handler_capsules.cpp:852-1047 (170 B -> 64 nodes)
 //   0x83 HQ           UnpackerHandler_HQNode                 handler_hqnode.cpp:93-172     (781 B -> 96 nodes)
 // and, for raw byte streams,
 //   0x81 standard     UnpackerHandler_NormalNode             handler_normalnode.cpp:88-141 (5 B -> 1 node)
-// (0x85 dense capsules: decode.cu.)
 //
-// Capsule formats share one skeleton (one CTA per stream, tiles of 256 capsules staged through shared
-// memory, one thread per capsule for frame / checksum / "does this capsule release its predecessor",
-// an exclusive block scan for the node offsets, then emission in the format's own grain -- a thread per
-// 5-byte cabin (two samples, one 16-byte store) for express, a warp per capsule with a lane per cabin
-// for ultra (3 samples) and ultra-dense (2 samples) -- into one contiguous run of the output).  What
-// differs besides is the state that crosses capsules:
+// The reference decodes capsules byte by byte in a state machine: a capsule's nodes are produced when the NEXT
+// capsule arrives (angles are interpolated between the two start angles), and only if both checksums hold and the
+// next capsule is not a scan start (dense, ultra-dense: and the angular step is below the 100 Hz bound).  Here the
+// capsule formats but HQ share one kernel, decode_capsule_kernel<F> (one CTA per stream, tiles of 256 capsules
+// staged through shared memory, one thread per capsule for frame / checksum / "does this capsule release its
+// predecessor", an exclusive block scan for the node offsets, then emission in the format's own grain -- a thread
+// per pair of samples (one 16-byte store) for express and dense, a warp per capsule with a lane per cabin for ultra
+// (3 samples) and ultra-dense (2 samples) -- into one contiguous run of the output).  What differs besides is the
+// state that crosses capsules:
 //   * express / ultra: none (the scan-start flag of a node is a function of its angle only);
-//   * ultra-dense: the last node's scan-start flag (a 2-bit transfer function per capsule, scanned
-//     under composition, as in decode.cu) and `_last_dist_q2`, a smoothing recurrence over
+//   * dense / ultra-dense: the last node's scan-start flag (the reference's lastNodeSyncBit,
+//     sync_i = raw_i & ~sync_{i-1}), carried across capsules as a 2-bit transfer function per capsule,
+//     scanned under composition;
+//   * ultra-dense besides: `_last_dist_q2`, a smoothing recurrence over
 //     neighbouring short-range samples.  A capsule's effect on that value is a function of at most
 //     nine candidate inputs (the first sample either ignores the incoming value or averages with
 //     one of 17 neighbours -> 9 results), so every capsule thread tabulates its nine outcomes, one
@@ -40,26 +45,34 @@ constexpr uint32_t kStOk = 1, kStSync = 2, kStEmit = 4, kStDiscard = 8, kStCheck
                    kStBadFrame = 64;
 constexpr int kFull = 360 << 16;
 
-enum { kExpress = 0, kUltra = 1, kUltraDense = 2 };
+enum { kExpress = 0, kUltra = 1, kUltraDense = 2, kDense = 3 };
 
+// CB bytes and NODES nodes per capsule, the start angle at byte START, BUFFERS tile buffers of DT capsules (= threads).
+// JUMP_CABINS: the cabin count in the reference's angular-jump discard threshold (0: no threshold).  SYNC_CHAIN: the
+// last node's scan-start flag crosses capsules; SMOOTH_CHAIN: so does the smoothed last distance.
 template <int F>
 struct Fmt;
 template <>
 struct Fmt<kExpress> {
-  static constexpr int CB = 84, NODES = 32, START = 2, BUFFERS = 2, DT = 256;
-  static constexpr bool THRESHOLD = false, STATE = false;
+  static constexpr int CB = 84, NODES = 32, START = 2, BUFFERS = 2, DT = 256, JUMP_CABINS = 0;
+  static constexpr bool SYNC_CHAIN = false, SMOOTH_CHAIN = false;
 };
 template <>
 struct Fmt<kUltra> {
   // one tile buffer (more CTAs per SM instead of a prefetch: the emission is instruction-bound)
-  static constexpr int CB = 132, NODES = 96, START = 2, BUFFERS = 1, DT = 256;
-  static constexpr bool THRESHOLD = false, STATE = false;
+  static constexpr int CB = 132, NODES = 96, START = 2, BUFFERS = 1, DT = 256, JUMP_CABINS = 0;
+  static constexpr bool SYNC_CHAIN = false, SMOOTH_CHAIN = false;
+};
+template <>
+struct Fmt<kDense> {
+  static constexpr int CB = 84, NODES = 40, START = 2, BUFFERS = 2, DT = 256, JUMP_CABINS = 40;
+  static constexpr bool SYNC_CHAIN = true, SMOOTH_CHAIN = false;
 };
 template <>
 struct Fmt<kUltraDense> {
   // one tile buffer: with the smoothing tables a second one would leave a single CTA (8 warps) per SM
-  static constexpr int CB = 170, NODES = 64, START = 8, BUFFERS = 1, DT = 128;
-  static constexpr bool THRESHOLD = true, STATE = true;
+  static constexpr int CB = 170, NODES = 64, START = 8, BUFFERS = 1, DT = 128, JUMP_CABINS = 32;
+  static constexpr bool SYNC_CHAIN = true, SMOOTH_CHAIN = true;
 };
 
 __device__ __forceinline__ uint32_t ld16(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8); }
@@ -78,6 +91,10 @@ __device__ __forceinline__ uint2 pack_node(int angle_q6, uint32_t dist_q2, uint3
   return nd;
 }
 
+__device__ __forceinline__ void cp_async4(void* dst, const void* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src)
+               : "memory");
+}
 __device__ __forceinline__ void cp_async16(void* dst, const void* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src)
                : "memory");
@@ -105,6 +122,49 @@ __device__ __forceinline__ void cabin_express(const uint8_t* prev, int prev_q8, 
   const uint32_t q0 = d0 & 0xFFFCu, q1 = d1 & 0xFFFCu;
   na = pack_node((a0 - (off0 << 13)) >> 10, q0, sync0, q0 ? (0x2Fu << 2) : 0u);
   nb = pack_node((a1 - (off1 << 13)) >> 10, q1, sync1, q1 ? (0x2Fu << 2) : 0u);
+}
+
+// ---- dense (handler_capsules.cpp:736-791) --------------------------------------------------------------
+// samples 2 * pair and 2 * pair + 1: one 32-bit word of 16-bit distances, the angle interpolated in q16 (inc: step
+// per sample), the two resolved scan-start flags in sync2
+__device__ __forceinline__ void pair_dense(const uint8_t* prev, int prev_q8, int inc, uint32_t pair, uint32_t sync2,
+                                           uint2& na, uint2& nb) {
+  const int a0 = (prev_q8 << 8) + (int)(2u * pair) * inc;
+  const uint32_t w = *reinterpret_cast<const uint32_t*>(prev + 4 + 4 * pair);
+  const uint32_t q0 = (w & 0xFFFFu) << 2, q1 = (w >> 16) << 2;
+  na = pack_node(a0 >> 10, q0, sync2 & 1u, q0 ? (0x2Fu << 2) : 0u);
+  nb = pack_node((a0 + inc) >> 10, q1, sync2 >> 1, q1 ? (0x2Fu << 2) : 0u);
+}
+
+// ---- the scan-start chain (dense :768-769, ultra-dense) ---------------------------------------------------
+// raw scan-start test of the N interpolated samples of a capsule as a bit mask.  One real modulo, then a running
+// remainder: inc_q16 < 360 deg (the jump threshold keeps the step per sample far below a revolution), so a single
+// conditional subtraction per step suffices.
+template <int N>
+__device__ __forceinline__ unsigned long long raw_sync_mask(int prev_q8, int inc_q16) {
+  unsigned long long m = 0;
+  int rem = ((prev_q8 << 8) + inc_q16) % kFull;  // (cur + inc) % full for pos = 0
+  const int lim = inc_q16 << 1;
+  // no wrap inside the capsule and already past the two steps after the last one: nothing to mark (most capsules)
+  if (rem >= lim && rem + (N - 1) * inc_q16 < kFull) return 0ull;
+#pragma unroll 8
+  for (int pos = 0; pos < N; ++pos) {
+    if (rem < lim) m |= 1ull << pos;
+    rem += inc_q16;
+    if (rem >= kFull) rem -= kFull;
+  }
+  return m;
+}
+// sync_i = raw_i & ~sync_{i-1}, sync_{-1} = s_in; only set raw bits matter
+__device__ __forceinline__ unsigned long long resolve_sync(unsigned long long raw, uint32_t s_in) {
+  unsigned long long s = 0, r = raw;
+  while (r) {
+    const int i = __ffsll((long long)r) - 1;
+    r &= r - 1;
+    const uint32_t prev = (i == 0) ? s_in : (uint32_t)((s >> (i - 1)) & 1ull);
+    if (!prev) s |= 1ull << i;
+  }
+  return s;
 }
 
 // ---- ultra (handler_capsules.cpp:422-580) --------------------------------------------------------------
@@ -199,34 +259,11 @@ __device__ __forceinline__ int ud_smooth(int raw, uint32_t scale, int last) {
   if (scale == 0 && last && abs(raw - last) <= 8) return (raw + last) >> 1;
   return raw;
 }
-// scan-start test of the 64 interpolated samples before the "not twice in a row" rule
-__device__ __forceinline__ unsigned long long raw_sync_mask64(int prev_q8, int inc_q16) {
-  unsigned long long m = 0;
-  int rem = ((prev_q8 << 8) + inc_q16) % kFull;
-  const int lim = inc_q16 << 1;
-  if (rem >= lim && rem + 63 * inc_q16 < kFull) return 0ull;  // no wrap inside this capsule: nothing to mark
-#pragma unroll 8
-  for (int pos = 0; pos < 64; ++pos) {
-    if (rem < lim) m |= 1ull << pos;
-    rem += inc_q16;
-    if (rem >= kFull) rem -= kFull;
-  }
-  return m;
-}
-__device__ __forceinline__ unsigned long long resolve_sync64(unsigned long long raw, uint32_t s_in) {
-  unsigned long long s = 0, r = raw;
-  while (r) {
-    const int i = __ffsll((long long)r) - 1;
-    r &= r - 1;
-    const uint32_t prev = (i == 0) ? s_in : (uint32_t)((s >> (i - 1)) & 1ull);
-    if (!prev) s |= 1ull << i;
-  }
-  return s;
-}
 
 template <int F>
 struct CapsuleSmem {
   static constexpr int CB = Fmt<F>::CB, DT = Fmt<F>::DT;
+  static constexpr int SYNC = Fmt<F>::SYNC_CHAIN ? DT : 1, SMOOTH = Fmt<F>::SMOOTH_CHAIN ? DT : 1;
   static constexpr int kTileBytes = (DT * CB + 15) & ~15;
   uint8_t cap[Fmt<F>::BUFFERS][kTileBytes];  // tiles (double-buffered: cp.async prefetch of the next one)
   uint8_t carry[(CB + 15) & ~15];      // last capsule of the previous tile
@@ -235,16 +272,18 @@ struct CapsuleSmem {
   uint32_t emit_list[DT];
   uint32_t warp_a[DT / 32], warp_b[DT / 32];
   uint32_t carry_nodes, tile_nodes;
-  // ultra-dense only
-  unsigned long long smask[Fmt<F>::STATE ? DT : 1];
-  uint32_t ud_out[Fmt<F>::STATE ? DT : 1][10];   // nine outcomes of the smoothing chain + first raw sample
-  uint32_t ud_first_scale[Fmt<F>::STATE ? DT : 1];  // bit 31: the capsule's outcome does not depend on its input
-  uint32_t ud_last_in[Fmt<F>::STATE ? DT : 1];
-  uint16_t ud_dist[Fmt<F>::STATE ? DT : 1][66];  // smoothed short-range distances (rows padded to 33 words: a thread per capsule walks a column)
-  uint32_t carry_sync, red_sync, carry_last, red_last;
+  unsigned long long smask[SYNC];      // scan-start chain: final flags of the nodes each capsule releases
+  // smoothing chain
+  uint32_t ud_out[SMOOTH][10];         // nine outcomes of the smoothing chain + first raw sample
+  uint32_t ud_first_scale[SMOOTH];     // bit 31: the capsule's outcome does not depend on its input
+  uint32_t ud_last_in[SMOOTH];
+  uint16_t ud_dist[SMOOTH][66];  // smoothed short-range distances (rows padded to 33 words: a thread per capsule walks a column)
+  uint32_t carry_sync, red_sync, n_starts, carry_last, red_last;
   // ultra only: angle-correction table and the per-warp staging rows of the emission
   int ultra_off[F == kUltra ? 496 : 1];
   uint2 wstage[F == kUltra ? DT / 32 : 1][F == kUltra ? 96 : 1];
+  // dense only: angular step per sample of the nodes each capsule releases
+  int inc_q16[F == kDense ? DT : 1];
 };
 
 template <int F>
@@ -255,7 +294,7 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
   CapsuleSmem<F>& sm = *reinterpret_cast<CapsuleSmem<F>*>(capsule_smem_raw);
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   int thr_q8 = 0;
-  if (T::THRESHOLD) thr_q8 = (360 * 100 * 32 / (int)(1000000u / a.sample_duration_us)) << 8;
+  if (T::JUMP_CABINS) thr_q8 = (360 * 100 * T::JUMP_CABINS / (int)(1000000u / a.sample_duration_us)) << 8;
   if constexpr (F == kUltra) {
     for (uint32_t i = tid; i < 493u; i += DT) sm.ultra_off[i] = g_ultra_offset[i];
     __syncthreads();
@@ -267,15 +306,19 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
     uint2* out = a.nodes_out + (size_t)s * a.stride_capsules * NODES;
     uint32_t* st_out = a.capsule_status ? a.capsule_status + (size_t)s * a.stride_capsules : nullptr;
     uint32_t* off_out = a.capsule_node_offset ? a.capsule_node_offset + (size_t)s * a.stride_capsules : nullptr;
+    uint32_t* starts = a.scan_starts ? a.scan_starts + (size_t)s * a.starts_stride : nullptr;
+    const uint32_t* state_in = a.state_in ? a.state_in + (size_t)s * a.state_words : nullptr;
     if (tid == 0) {
       sm.carry_nodes = 0;
       sm.okflag[0] = 0;
       sm.start_q8[0] = 0;
-      sm.carry_sync = a.state_in ? (a.state_in[2 * s] & 1u) : 0u;
-      sm.carry_last = a.state_in ? a.state_in[2 * s + 1] : 0u;
+      if constexpr (T::SYNC_CHAIN) sm.carry_sync = state_in ? (state_in[0] & 1u) : 0u;
+      if constexpr (F == kDense) sm.n_starts = 0;
+      if constexpr (T::SMOOTH_CHAIN) sm.carry_last = (state_in && a.state_words == 2) ? state_in[1] : 0u;
     }
     __syncthreads();
 
+    // stage a tile into buffer `b`: asynchronous 16-byte copies, 4-byte ones where the stream is only 4-byte aligned
     auto stage = [&](uint32_t c0, uint32_t b) {
       const uint32_t live = min((uint32_t)DT, n - c0);
       const uint32_t bytes = live * CB;
@@ -285,6 +328,10 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
         const uint32_t quads = bytes >> 4;
         for (uint32_t q = tid; q < quads; q += DT) cp_async16(&sm.cap[b][16 * q], g + 16 * q);
         done = quads << 4;
+      } else if ((reinterpret_cast<uintptr_t>(g) & 3u) == 0) {
+        const uint32_t words = bytes >> 2;
+        for (uint32_t w = tid; w < words; w += DT) cp_async4(&sm.cap[b][4 * w], g + 4 * w);
+        done = words << 2;
       }
       for (uint32_t w = done + tid; w < bytes; w += DT) sm.cap[b][w] = __ldg(g + w);
       asm volatile("cp.async.commit_group;" ::: "memory");
@@ -308,9 +355,17 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
           st = kStBadFrame;
         } else {
           uint32_t x = 0;
-          const uint16_t* h = reinterpret_cast<const uint16_t*>(c);
+          if constexpr (CB % 4 == 0) {  // 32-bit words (half the loads of the 16-bit loop)
+            const uint32_t* w = reinterpret_cast<const uint32_t*>(c);
+            x = w[0] >> 16;
+#pragma unroll
+            for (int k = 1; k < CB / 4; ++k) x ^= w[k];
+            x ^= x >> 16;
+          } else {
+            const uint16_t* h = reinterpret_cast<const uint16_t*>(c);
 #pragma unroll 8
-          for (int w = 1; w < CB / 2; ++w) x ^= h[w];
+            for (int k = 1; k < CB / 2; ++k) x ^= h[k];
+          }
           const uint32_t sum = (x ^ (x >> 8)) & 0xFFu;
           const uint32_t recv = ((b0 & 0xFu) | (b1 << 4)) & 0xFFu;
           if (recv != sum) {
@@ -338,7 +393,7 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
           prev_q8 = (int)sm.start_q8[tid];
           diff = cur_q8 - prev_q8;
           if (prev_q8 > cur_q8) diff += (360 << 8);
-          if (T::THRESHOLD && diff > thr_q8) {
+          if (T::JUMP_CABINS && diff > thr_q8) {
             st |= kStDiscard;
           } else {
             emit = 1;
@@ -348,17 +403,20 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
       }
       const uint32_t inc_scan = warp_inclusive_scan(emit);
       if (lane == 31) sm.warp_a[warp] = inc_scan;
-      // ultra-dense: transfer function of the scan-start flag through this capsule
+      // scan-start chain: transfer function of the flag through this capsule, f(s_in) = s_out
       unsigned long long raw = 0;
-      uint32_t Fsync = 0x2;  // identity
-      if constexpr (T::STATE) {
+      uint32_t Fsync = 0x2;  // identity: f(0) = 0 (bit 0), f(1) = 1 (bit 1)
+      if constexpr (T::SYNC_CHAIN) {
         uint32_t f = 0x2;
         if (emit) {
-          raw = raw_sync_mask64(prev_q8, (diff << 8) / 64);
-          const uint32_t o0 = (uint32_t)(resolve_sync64(raw, 0) >> 63) & 1u;
-          const uint32_t o1 = (uint32_t)(resolve_sync64(raw, 1) >> 63) & 1u;
+          const int inc_q16 = (diff << 8) / NODES;
+          raw = raw_sync_mask<NODES>(prev_q8, inc_q16);
+          if constexpr (F == kDense) sm.inc_q16[tid] = inc_q16;  // the emission's step, once per capsule
+          const uint32_t o0 = (uint32_t)(resolve_sync(raw, 0) >> (NODES - 1)) & 1u;
+          const uint32_t o1 = (uint32_t)(resolve_sync(raw, 1) >> (NODES - 1)) & 1u;
           f = o0 | (o1 << 1);
         }
+        // inclusive scan of the functions under composition: (g o f)(x) = g(f(x))
         Fsync = f;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) {
@@ -368,36 +426,49 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
         if (lane == 31) sm.warp_b[warp] = Fsync;
       }
       __syncthreads();
-      uint32_t base_off = 0, s_state = T::STATE ? sm.carry_sync : 0u;
+      uint32_t base_off = 0, s_state = T::SYNC_CHAIN ? sm.carry_sync : 0u;
       for (uint32_t w = 0; w < warp; ++w) {
         base_off += sm.warp_a[w];
-        if (T::STATE) s_state = (sm.warp_b[w] >> s_state) & 1u;
+        if (T::SYNC_CHAIN) s_state = (sm.warp_b[w] >> s_state) & 1u;
       }
       const uint32_t my_off = base_off + inc_scan - emit;
-      if constexpr (T::STATE) {
+      unsigned long long smask = 0;
+      if constexpr (T::SYNC_CHAIN) {
+        // flag entering this capsule: everything before it in the warp
         const uint32_t Fprev = __shfl_up_sync(0xffffffffu, Fsync, 1);
         const uint32_t s_in = (lane == 0) ? s_state : ((Fprev >> s_state) & 1u);
-        if (tid < live) sm.smask[tid] = emit ? resolve_sync64(raw, s_in) : 0ull;
+        if (emit) smask = resolve_sync(raw, s_in);
+        if (tid < live) sm.smask[tid] = smask;
       }
       if (tid < live) {
+        const uint32_t node_off = sm.carry_nodes + (uint32_t)NODES * my_off;
         if (emit) sm.emit_list[my_off] = tid;
         if (st_out) st_out[c0 + tid] = st;
-        if (off_out) off_out[c0 + tid] = sm.carry_nodes + (uint32_t)NODES * my_off;
+        if (off_out) off_out[c0 + tid] = node_off;
+        // this capsule's scan-start nodes (a few per revolution), for the assembler.  Only the dense entry points
+        // offer the list: compiled into ultra-dense, the loop alone takes that kernel from 40 to 32 registers and
+        // makes it slower
+        if (F == kDense && starts) {
+          for (; smask; smask &= smask - 1) {
+            const uint32_t idx = atomicAdd(&sm.n_starts, 1u);
+            if (idx < a.starts_stride) starts[idx] = node_off + (uint32_t)(__ffsll((long long)smask) - 1);
+          }
+        }
       }
       if (tid == DT - 1) {
-        uint32_t tot = 0, st2 = T::STATE ? sm.carry_sync : 0u;
+        uint32_t tot = 0, st2 = T::SYNC_CHAIN ? sm.carry_sync : 0u;
         for (uint32_t w = 0; w < DT / 32; ++w) {
           tot += sm.warp_a[w];
-          if (T::STATE) st2 = (sm.warp_b[w] >> st2) & 1u;
+          if (T::SYNC_CHAIN) st2 = (sm.warp_b[w] >> st2) & 1u;
         }
         sm.tile_nodes = (uint32_t)NODES * tot;
-        if (T::STATE) sm.red_sync = st2;
+        if (T::SYNC_CHAIN) sm.red_sync = st2;
       }
       // first sample position from which this capsule's smoothed distances no longer depend on the value that
       // enters the capsule (the nine candidates have merged): step 1 stores those directly, step 3 replays only
       // the positions before it
       uint32_t ud_pm = 64;
-      if constexpr (T::STATE) {
+      if constexpr (T::SMOOTH_CHAIN) {
         // ---- smoothing chain, step 1: the nine outcomes of this capsule's 64 samples ------------------
         if (emit) {
           const uint8_t* pc = (tid == 0) ? sm.carry : tile + (tid - 1) * CB;
@@ -446,7 +517,7 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
         }
       }
       __syncthreads();
-      if constexpr (T::STATE) {
+      if constexpr (T::SMOOTH_CHAIN) {
         // ---- step 2: the value entering every releasing capsule.  A capsule whose nine outcomes agree
         // (any far sample inside it) is a constant: each thread walks back to the nearest such capsule (or
         // to the tile's input) and applies the tables from there -- usually one or two steps.
@@ -536,21 +607,27 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
             dst[1] = nb;
           }
         }
-      } else if constexpr (F == kExpress) {
-        // a thread handles one 5-byte cabin (two samples): the capsule look-ups and the cabin bytes are shared and
-        // the two nodes leave as one 16-byte store (a capsule's run starts on a multiple of 256 bytes)
+      } else {
+        // express, dense: a thread handles one pair of samples (an express cabin, a dense distance word): the
+        // capsule look-ups and the capsule bytes are shared and the two nodes leave as one 16-byte store (a
+        // capsule's run starts on a multiple of 256 / 320 bytes)
+        constexpr uint32_t kPairs = NODES / 2;
         const uint32_t n_pairs = sm.tile_nodes / 2u;
         uint2* o = out + sm.carry_nodes;
         const bool wide = (reinterpret_cast<uintptr_t>(o) & 15u) == 0;
         for (uint32_t p = tid; p < n_pairs; p += DT) {
-          const uint32_t e = p >> 4, cabin = p & 15u;
+          const uint32_t e = p / kPairs, pair = p - e * kPairs;
           const uint32_t j = sm.emit_list[e];
           const uint8_t* pc = (j == 0) ? sm.carry : tile + (j - 1) * CB;
           const int pq8 = (int)sm.start_q8[j];
-          int d = (int)sm.start_q8[j + 1] - pq8;
-          if (pq8 > (int)sm.start_q8[j + 1]) d += (360 << 8);
           uint2 na, nb;
-          cabin_express(pc, pq8, d, cabin, na, nb);
+          if constexpr (F == kExpress) {
+            int d = (int)sm.start_q8[j + 1] - pq8;
+            if (pq8 > (int)sm.start_q8[j + 1]) d += (360 << 8);
+            cabin_express(pc, pq8, d, pair, na, nb);
+          } else {
+            pair_dense(pc, pq8, sm.inc_q16[j], pair, (uint32_t)(sm.smask[j] >> (2 * pair)) & 3u, na, nb);
+          }
           if (wide) {
             *reinterpret_cast<uint4*>(o + 2u * p) = make_uint4(na.x, na.y, nb.x, nb.y);
           } else {
@@ -566,16 +643,18 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
         sm.okflag[0] = sm.okflag[live];
         sm.start_q8[0] = sm.start_q8[live];
         sm.carry_nodes += sm.tile_nodes;
-        if (T::STATE) sm.carry_sync = sm.red_sync;
+        if (T::SYNC_CHAIN) sm.carry_sync = sm.red_sync;
       }
       __syncthreads();
     }
     if (tid == 0) {
       if (a.node_counts) a.node_counts[s] = sm.carry_nodes;
       if (a.state_out) {
-        a.state_out[2 * s] = T::STATE ? sm.carry_sync : 0u;
-        a.state_out[2 * s + 1] = T::STATE ? sm.carry_last : 0u;
+        uint32_t* state_out = a.state_out + (size_t)s * a.state_words;
+        state_out[0] = T::SYNC_CHAIN ? sm.carry_sync : 0u;
+        if (a.state_words == 2) state_out[1] = T::SMOOTH_CHAIN ? sm.carry_last : 0u;
       }
+      if (F == kDense && a.scan_start_counts) a.scan_start_counts[s] = sm.n_starts;
     }
     __syncthreads();
   }
@@ -935,6 +1014,7 @@ cudaError_t launch_decode_capsules(uint32_t ans_type, const CapsuleDecodeArgs& a
   switch (ans_type) {
     case 0x82: return launch_fmt<kExpress>(a, grid, stream);
     case 0x84: return launch_fmt<kUltra>(a, grid, stream);
+    case 0x85: return launch_fmt<kDense>(a, grid, stream);
     case 0x86: return launch_fmt<kUltraDense>(a, grid, stream);
     case 0x83:
       decode_hq_kernel<<<grid, HT, sizeof(HqSmem), stream>>>(a);
@@ -986,6 +1066,9 @@ cudaError_t decode_formats_configure() {
   if (e != cudaSuccess) return e;
   e = cudaFuncSetAttribute(decode_capsule_kernel<kUltra>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)sizeof(CapsuleSmem<kUltra>));
+  if (e != cudaSuccess) return e;
+  e = cudaFuncSetAttribute(decode_capsule_kernel<kDense>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)sizeof(CapsuleSmem<kDense>));
   if (e != cudaSuccess) return e;
   e = cudaFuncSetAttribute(decode_capsule_kernel<kUltraDense>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)sizeof(CapsuleSmem<kUltraDense>));

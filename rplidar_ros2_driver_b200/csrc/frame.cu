@@ -10,7 +10,7 @@
 //   collecting:          bytes 2 .. size-1 are taken blindly; the frame is then checked (checksum) and decoded
 // As a function of the stream this is a chain of jumps from one "waiting for byte 0" position to the next:
 // +1, +2 or +frame size.  This kernel walks that chain and writes the frames it visits back to back
-// ([capsules][frame size], the input format of decode.cu / decode_formats.cu); every stretch of skipped bytes
+// ([capsules][frame size], the input format of decode_formats.cu); every stretch of skipped bytes
 // becomes ONE all-zero capsule in the output.  The decoders report such a capsule as RPL_CAPSULE_BAD_FRAME and
 // forget the capsule before it -- precisely the effect the skipped bytes have in the SDK -- so framing + decoding
 // reproduces the SDK's node stream on damaged input (dropped, inserted, corrupted bytes), pinned against the

@@ -272,7 +272,6 @@ rpl_result rpl_ctx_create(int device, uint32_t max_nodes, uint32_t max_scans, rp
       !cuda_ok(c, rpl::scan_small_configure(), "scan_small_configure") ||
       !cuda_ok(c, rpl::scan_general_configure(), "scan_general_configure") ||
       !cuda_ok(c, rpl::cloud_configure(), "cloud_configure") ||
-      !cuda_ok(c, rpl::decode_configure(), "decode_configure") ||
       !cuda_ok(c, rpl::decode_formats_configure(), "decode_formats_configure"))
     return fail(RPL_RESULT_OPERATION_FAIL);
   const int occ = std::max(1, rpl::scan_fast_max_ctas_per_sm());
@@ -339,7 +338,6 @@ void rpl_ctx_destroy(rpl_ctx* c) {
     free_lane(c->lane[i]);
   }
   if (c->asm_done) cudaEventDestroy(c->asm_done);
-  cudaFree(c->d_state_tmp);
   cudaFree(c->d_reset_prefix);
   cudaFree(c->d_desc);
   if (c->h_one) cudaFreeHost(c->h_one);
@@ -691,6 +689,20 @@ rpl_result rpl_scan(rpl_ctx* c, rpl_node_hq* nodes, size_t count, const rpl_scan
 }
 
 // ---- dense-capsule decode (SURVEY.md 8(f) rank 1) ---------------------------------------------
+namespace {
+// one launch of the capsule decoder on arguments the entry point has checked (n_streams > 0)
+rpl_result decode_capsules_launch(rpl_ctx* c, uint32_t ans_type, const rpl::CapsuleDecodeArgs& a, void* stream) {
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : c->lane[0].stream;
+  // one CTA per stream, up to four (dense) or eight (the other formats) CTAs per SM; a CTA loops over the rest
+  const uint32_t ctas_per_sm = ans_type == 0x85 ? 4u : 8u;
+  const int grid = (int)std::min<uint32_t>(a.n_streams, (uint32_t)c->num_sms * ctas_per_sm);
+  RPL_CUDA(c, rpl::launch_decode_capsules(ans_type, a, grid, st), RPL_RESULT_OPERATION_FAIL);
+  c->launches++;
+  return RPL_RESULT_OK;
+}
+}  // namespace
+
 rpl_result rpl_decode_dense_batch_dev(rpl_ctx* c, const uint8_t* capsules, const uint32_t* capsule_counts,
                                       uint32_t n_streams, uint32_t stride_capsules, uint32_t sample_duration_us,
                                       const uint32_t* sync_state_in, rpl_node_hq* nodes_out,
@@ -722,67 +734,33 @@ rpl_result rpl_decode_dense_batch_starts_dev(rpl_ctx* c, const uint8_t* capsules
     return RPL_RESULT_INVALID_DATA;
   }
   if (n_streams == 0) return RPL_RESULT_OK;
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : c->lane[0].stream;
-  rpl::DecodeArgs a{};
+  rpl::CapsuleDecodeArgs a{};
   a.capsules = capsules;
   a.counts = capsule_counts;
   a.n_streams = n_streams;
   a.stride_capsules = stride_capsules;
   a.sample_duration_us = sample_duration_us;
-  a.sync_state_in = sync_state_in;
+  a.state_words = 1;
+  a.state_in = sync_state_in;
   a.nodes_out = reinterpret_cast<uint2*>(nodes_out);
   a.node_counts = node_counts;
   a.capsule_status = capsule_status;
   a.capsule_node_offset = capsule_node_offset;
-  a.sync_state_out = sync_state_out;
+  a.state_out = sync_state_out;
   a.scan_starts = scan_starts;
   a.scan_start_counts = scan_start_counts;
   a.starts_stride = starts_stride;
-  const int grid = (int)std::min<uint32_t>(n_streams, (uint32_t)c->num_sms * 4u);
-  RPL_CUDA(c, rpl::launch_decode_dense(a, grid, st), RPL_RESULT_OPERATION_FAIL);
-  c->launches++;
-  return RPL_RESULT_OK;
+  return decode_capsules_launch(c, 0x85, a, stream);
 }
 
 rpl_result rpl_decode_dense(rpl_ctx* c, const uint8_t* capsules, uint32_t n_capsules, uint32_t sample_duration_us,
                             uint32_t* sync_state, rpl_node_hq* nodes_out, uint32_t* node_count,
                             uint32_t* capsule_status, uint32_t* capsule_node_offset) {
-  if (!c || !node_count || (n_capsules && (!capsules || !nodes_out))) return RPL_RESULT_INVALID_DATA;
-  *node_count = 0;
-  if (n_capsules == 0) return RPL_RESULT_OK;
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  cudaStream_t st = c->lane[0].stream;
-  const size_t cb = (size_t)n_capsules * 84, nb = (size_t)n_capsules * 40 * 8, sb = (size_t)n_capsules * 4;
-  unsigned char* d = nullptr;  // [capsules | pad][nodes][status][offsets][count, n_nodes, sync in, sync out]
-  const size_t o_nodes = (cb + 15) & ~(size_t)15, o_st = o_nodes + nb, o_off = o_st + sb, o_small = o_off + sb;
-  RPL_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&d), o_small + 16), RPL_RESULT_INSUFFICIENT_MEMORY);
-  uint32_t small[4] = {n_capsules, 0u, sync_state ? (*sync_state & 1u) : 0u, 0u};
-  rpl_result r = RPL_RESULT_OK;
-  auto bail = [&](rpl_result code) {
-    cudaFree(d);
-    return code;
-  };
-  if (!cuda_ok(c, cudaMemcpyAsync(d, capsules, cb, cudaMemcpyHostToDevice, st), "H2D") ||
-      !cuda_ok(c, cudaMemcpyAsync(d + o_small, small, 16, cudaMemcpyHostToDevice, st), "H2D"))
-    return bail(RPL_RESULT_OPERATION_FAIL);
-  uint32_t* ds = reinterpret_cast<uint32_t*>(d + o_small);
-  r = rpl_decode_dense_batch_dev(c, d, ds, 1, n_capsules, sample_duration_us, ds + 2,
-                                 reinterpret_cast<rpl_node_hq*>(d + o_nodes), ds + 1,
-                                 reinterpret_cast<uint32_t*>(d + o_st), reinterpret_cast<uint32_t*>(d + o_off), ds + 3, st);
-  if (r != RPL_RESULT_OK) return bail(r);
-  if (!cuda_ok(c, cudaMemcpyAsync(small, ds, 16, cudaMemcpyDeviceToHost, st), "D2H") ||
-      !cuda_ok(c, cudaStreamSynchronize(st), "sync"))
-    return bail(RPL_RESULT_OPERATION_FAIL);
-  *node_count = small[1];
-  if (sync_state) *sync_state = small[3];
-  if (!cuda_ok(c, cudaMemcpy(nodes_out, d + o_nodes, (size_t)small[1] * 8, cudaMemcpyDeviceToHost), "D2H"))
-    return bail(RPL_RESULT_OPERATION_FAIL);
-  if (capsule_status && !cuda_ok(c, cudaMemcpy(capsule_status, d + o_st, sb, cudaMemcpyDeviceToHost), "D2H"))
-    return bail(RPL_RESULT_OPERATION_FAIL);
-  if (capsule_node_offset && !cuda_ok(c, cudaMemcpy(capsule_node_offset, d + o_off, sb, cudaMemcpyDeviceToHost), "D2H"))
-    return bail(RPL_RESULT_OPERATION_FAIL);
-  return bail(RPL_RESULT_OK);
+  uint32_t state[2] = {sync_state ? *sync_state : 0u, 0u};
+  const rpl_result r = rpl_decode_capsules(c, 0x85, capsules, n_capsules, sample_duration_us, state, nodes_out,
+                                           node_count, capsule_status, capsule_node_offset, nullptr, nullptr, nullptr);
+  if (r == RPL_RESULT_OK && sync_state) *sync_state = state[0];
+  return r;
 }
 
 // ---- the other answer formats (SURVEY.md 8(f) rank 1) ----------------------------------------------
@@ -807,21 +785,6 @@ uint32_t rpl_capsule_nodes(uint32_t ans_type) {
   }
 }
 
-namespace {
-// word 0 of every [2]-state pair, strided: the dense kernel keeps a single word per stream
-__global__ void gather_state_kernel(const uint32_t* in2, uint32_t* out1, uint32_t n) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out1[i] = in2[2 * i] & 1u;
-}
-__global__ void scatter_state_kernel(const uint32_t* in1, uint32_t* out2, uint32_t n) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) {
-    out2[2 * i] = in1[i];
-    out2[2 * i + 1] = 0u;
-  }
-}
-}  // namespace
-
 rpl_result rpl_decode_capsules_batch_dev(rpl_ctx* c, uint32_t ans_type, const uint8_t* capsules,
                                          const uint32_t* capsule_counts, uint32_t n_streams,
                                          uint32_t stride_capsules, uint32_t sample_duration_us,
@@ -842,29 +805,9 @@ rpl_result rpl_decode_capsules_batch_dev(rpl_ctx* c, uint32_t ans_type, const ui
     return RPL_RESULT_INVALID_DATA;
   }
   if (n_streams == 0) return RPL_RESULT_OK;
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : c->lane[0].stream;
-  if (ans_type == 0x85) {  // the dense kernel keeps one state word per stream
-    uint32_t* tmp = nullptr;
-    if (state_in || state_out) {
-      if (n_streams > c->state_tmp_cap) {
-        cudaFree(c->d_state_tmp);
-        c->d_state_tmp = nullptr;
-        RPL_CUDA(c, dev_alloc(&c->d_state_tmp, (size_t)2 * n_streams), RPL_RESULT_INSUFFICIENT_MEMORY);
-        c->state_tmp_cap = n_streams;
-      }
-      tmp = c->d_state_tmp;
-    }
-    const uint32_t blocks = (n_streams + 255) / 256;
-    if (state_in) gather_state_kernel<<<blocks, 256, 0, st>>>(state_in, tmp, n_streams);
-    rpl_result r = rpl_decode_dense_batch_dev(c, capsules, capsule_counts, n_streams, stride_capsules,
-                                              sample_duration_us, state_in ? tmp : nullptr, nodes_out, node_counts,
-                                              capsule_status, capsule_node_offset,
-                                              state_out ? tmp + n_streams : nullptr, st);
-    if (r != RPL_RESULT_OK) return r;
-    if (state_out) scatter_state_kernel<<<blocks, 256, 0, st>>>(tmp + n_streams, state_out, n_streams);
-    RPL_CUDA(c, cudaGetLastError(), RPL_RESULT_OPERATION_FAIL);
-    return RPL_RESULT_OK;
+  if (ans_type == 0x85 && (reinterpret_cast<uintptr_t>(capsules) & 3u) != 0) {
+    c->err = "dense capsule buffer must be 4-byte aligned";
+    return RPL_RESULT_INVALID_DATA;
   }
   rpl::CapsuleDecodeArgs a{};
   a.capsules = capsules;
@@ -872,17 +815,14 @@ rpl_result rpl_decode_capsules_batch_dev(rpl_ctx* c, uint32_t ans_type, const ui
   a.n_streams = n_streams;
   a.stride_capsules = stride_capsules;
   a.sample_duration_us = sample_duration_us;
+  a.state_words = 2;
   a.state_in = state_in;
   a.nodes_out = reinterpret_cast<uint2*>(nodes_out);
   a.node_counts = node_counts;
   a.capsule_status = capsule_status;
   a.capsule_node_offset = capsule_node_offset;
   a.state_out = state_out;
-  // one CTA per stream while they fit (express / ultra: five CTAs per SM by shared memory, ultra-dense two)
-  const int grid = (int)std::min<uint32_t>(n_streams, (uint32_t)c->num_sms * 8u);
-  RPL_CUDA(c, rpl::launch_decode_capsules(ans_type, a, grid, st), RPL_RESULT_OPERATION_FAIL);
-  c->launches++;
-  return RPL_RESULT_OK;
+  return decode_capsules_launch(c, ans_type, a, stream);
 }
 
 namespace {

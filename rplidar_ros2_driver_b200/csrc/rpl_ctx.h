@@ -66,8 +66,6 @@ struct rpl_ctx {
   uint2* d_desc = nullptr;
   size_t reset_prefix_cap = 0, desc_cap = 0;
   cudaEvent_t asm_done = nullptr;   // rpl_chain_dense_laserscan: the assemble scratch above is shared by the lanes
-  uint32_t* d_state_tmp = nullptr;  // dense decoder reached through the [2]-word state interface
-  size_t state_tmp_cap = 0;
   bool profile = false;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_fast, prof_general;
 };

@@ -327,10 +327,9 @@ def test_wire_bytes_to_laserscan_in_one_host_call(R, oracle, n_streams, max_node
 
 
 def test_stateful_decode_and_assembly_alternate_on_one_context(R, oracle):
-    """Regression (round-1 review): the dense decoder's per-stream state scratch and the assembler's reset-prefix
-    scratch live in the same context; growing one must not free the other.  Three rounds of
-    decode (0x85, state carried from round to round) -> assemble on ONE context, stream counts growing so that both
-    scratch buffers are reallocated in between, every round compared with the oracle."""
+    """Regression (round-1 review): stateful decodes and the assembler's reset-prefix scratch share one context.
+    Three rounds of decode (0x85, state carried from round to round) -> assemble on ONE context, stream counts
+    growing so that the assembler's scratch is reallocated in between, every round compared with the oracle."""
     import torch
 
     dev = torch.device("cuda")

@@ -86,21 +86,27 @@ def test_batched_streams_and_chain_into_the_scan_path(R, oracle, ctx):
     caps = torch.from_numpy(host).to(dev)
     counts = torch.full((n_streams,), n_caps, dtype=torch.int32, device=dev)
     counts[3] = 123  # ragged
+    sync_h = (np.arange(n_streams) % 3 == 0).astype(np.uint32)  # one state word per stream
+    sync_in = torch.from_numpy(sync_h.view(np.int32)).to(dev)
+    sync_out = torch.full((n_streams,), 7, dtype=torch.int32, device=dev)
     nodes = torch.zeros((n_streams, n_caps * 40, 8), dtype=torch.uint8, device=dev)
     ncount = torch.zeros(n_streams, dtype=torch.int32, device=dev)
     status = torch.zeros((n_streams, n_caps), dtype=torch.int32, device=dev)
     torch.cuda.synchronize()  # buffers were filled on torch's stream; the library runs on its own
     ctx.decode_dense_batch_dev(caps.data_ptr(), counts.data_ptr(), n_streams, n_caps, 31, nodes.data_ptr(),
-                               ncount.data_ptr(), capsule_status=status.data_ptr())
+                               ncount.data_ptr(), sync_state_in=sync_in.data_ptr(), capsule_status=status.data_ptr(),
+                               sync_state_out=sync_out.data_ptr())
     ctx.synchronize()
     torch.cuda.synchronize()
     hn = nodes.cpu().numpy().view(oracle.NODE_DTYPE).reshape(n_streams, n_caps * 40)
+    so = sync_out.cpu().numpy().astype(np.uint32)
     for s in range(n_streams):
         k = int(counts[s])
-        en, es, _, _ = oracle.dense_decode(host[s, :k], 31, 0)
+        en, es, _, est = oracle.dense_decode(host[s, :k], 31, int(sync_h[s]))
         assert int(ncount[s]) == len(en)
         assert (hn[s, : len(en)].view(np.uint64) == en.view(np.uint64)).all()
         assert (status[s, :k].cpu().numpy().astype(np.uint32) == es).all()
+        assert int(so[s]) == est
     # one revolution of stream 0: nodes between the first two scan-start flags
     en, _, _, _ = oracle.dense_decode(host[0], 31, 0)
     starts = np.flatnonzero(en["flag"] & 1)

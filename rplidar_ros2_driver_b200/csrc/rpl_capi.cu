@@ -97,14 +97,117 @@ rpl_result ensure_staging(rpl_ctx* c, Lane& l, uint32_t scans, size_t nodes, boo
   return RPL_RESULT_OK;
 }
 
-// PointCloud2 steps 4-5 a launch may fuse into the shared-memory kernel (scan_small.cu)
-struct PostParams {
-  uint32_t sor_k = 0;
-  float sor_alpha = 0.0f;
-  float voxel = 0.0f;
-};
+// The kernel that runs ahead of scan_general_kernel; the general kernel then serves only the scans it hands on.
+// kNone: the general kernel serves every scan.
+enum class FastKernel { kNone, kSmall, kCluster, kTma, kFast };
+
+// the kernel-selection rule of every scan entry point, batches and single scans alike
+FastKernel pick_fast(const rpl::ScanBatchArgs& a, uint32_t flags) {
+  // FORCE_GENERAL and status-only calls (no LaserScan, no ascended buffer) take the general kernel alone
+  if ((flags & RPL_FLAG_FORCE_GENERAL) != 0 || (!a.ranges && !a.nodes_out && !a.xyzi)) return FastKernel::kNone;
+  // revolutions that fit shared memory (what a lidar delivers) have their own kernels
+  if (rpl::scan_small_applies(a.stride) && (flags & RPL_FLAG_NO_SMALL) == 0) return FastKernel::kSmall;
+  // above that the TMA kernels need every scan base 16-byte aligned, and the PointCloud2 payload exists in the
+  // TMA kernel and the general kernel only
+  const bool aligned = (reinterpret_cast<uintptr_t>(a.nodes) & 15u) == 0 && (a.stride & 1u) == 0;
+  if (a.xyzi && !aligned) return FastKernel::kNone;
+  // the ascended buffer and NO_TMA (LaserScan only) take scan_fast_kernel
+  if (a.nodes_out || !aligned || ((flags & RPL_FLAG_NO_TMA) != 0 && !a.xyzi)) return FastKernel::kFast;
+  // LaserScan Mode B scans too large for the shared-memory kernels but no larger than two SMs can stage
+  if (!a.xyzi && !a.mode_a && rpl::scan_tma_cluster_applies(a.stride)) return FastKernel::kCluster;
+  return FastKernel::kTma;
+}
+
+// Launches fast kernel k on `stream` (k != kNone); the caller has zeroed a.fallback_count.  A PointCloud2 launch may
+// fuse the SOR / voxel-grid passes of `cloud` (steps 4-5) into the shared-memory kernel: *post_fused tells.
+rpl_result launch_fast(rpl_ctx* c, Lane& l, const rpl::ScanBatchArgs& a, FastKernel k, cudaStream_t stream,
+                       const rpl_cloud_params* cloud = nullptr, bool* post_fused = nullptr) {
+  const int tma_grid = c->tma_grid[a.xyzi ? 2 : a.mode_a ? 1 : 0];
+  const int grid = k == FastKernel::kCluster
+                       ? 2 * (int)std::min<uint32_t>(a.n_scans, (uint32_t)c->tma_clusters)
+                       : (int)std::min<uint32_t>(a.n_scans, (uint32_t)(k == FastKernel::kTma ? tma_grid : c->fast_grid));
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  if (c->profile) {
+    cudaEventCreate(&e0);
+    cudaEventCreate(&e1);
+    cudaEventRecord(e0, stream);
+  }
+  if (k == FastKernel::kSmall) {
+    // SOR / voxel grid run inside the kernel when the 32-bit cell keys and accumulators are exact:
+    // |cell index| < 32768 and voxel <= 4 m (scan_small.cu); otherwise as separate passes
+    bool fuse = false;
+    if (a.xyzi && cloud && (cloud->sor_k > 0 || cloud->voxel_size > 0.0f) && rpl::scan_small_post_applies(a.stride))
+      fuse = cloud->voxel_size == 0.0f || (cloud->voxel_size <= 4.0f && a.range_max / cloud->voxel_size < 32000.0f);
+    RPL_CUDA(c, rpl::launch_scan_small(a, l.fws.max_nodes, fuse ? cloud->sor_k : 0u, fuse ? cloud->sor_alpha : 0.0f,
+                                       fuse ? cloud->voxel_size : 0.0f, c->num_sms, stream),
+             RPL_RESULT_OPERATION_FAIL);
+    if (post_fused) *post_fused = fuse;
+  } else if (k == FastKernel::kCluster) {
+    RPL_CUDA(c, rpl::launch_scan_tma_cluster(a, l.fws.max_nodes, grid, stream), RPL_RESULT_OPERATION_FAIL);
+  } else if (k == FastKernel::kTma) {
+    RPL_CUDA(c, rpl::launch_scan_tma(a, l.fws.max_nodes, grid, stream), RPL_RESULT_OPERATION_FAIL);
+  } else {
+    RPL_CUDA(c, rpl::launch_scan_fast(a, l.fws, grid, stream), RPL_RESULT_OPERATION_FAIL);
+  }
+  if (c->profile) {
+    cudaEventRecord(e1, stream);
+    c->prof_fast.emplace_back(e0, e1);
+  }
+  c->launches++;
+  return RPL_RESULT_OK;
+}
+
+// launches scan_general_kernel on `stream` over every scan (all_scans) or over the scans in a.fallback_list
+rpl_result launch_general(rpl_ctx* c, Lane& l, const rpl::ScanBatchArgs& a, bool all_scans, cudaStream_t stream) {
+  const int grid = (int)std::min<uint32_t>(a.n_scans, (uint32_t)c->general_grid);
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  if (c->profile) {
+    cudaEventCreate(&e0);
+    cudaEventCreate(&e1);
+    cudaEventRecord(e0, stream);
+  }
+  RPL_CUDA(c, rpl::launch_scan_general(a, l.gws, grid, all_scans, stream), RPL_RESULT_OPERATION_FAIL);
+  if (c->profile) {
+    cudaEventRecord(e1, stream);
+    c->prof_general.emplace_back(e0, e1);
+  }
+  c->launches++;
+  return RPL_RESULT_OK;
+}
+
+// the fast kernel, then the general kernel for the scans it hands on (or for all), on `stream` with no host round trip
 rpl_result enqueue_args(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, uint32_t flags, cudaStream_t stream,
-                        const PostParams* post = nullptr, bool* post_fused = nullptr);
+                        const rpl_cloud_params* cloud = nullptr, bool* post_fused = nullptr) {
+  if (post_fused) *post_fused = false;
+  if (a.nodes_out && !a.apply_ascend) {
+    // no geometric correction requested: the buffer passes through unchanged
+    // (reference lidar_driver_wrapper.cpp:330-337); a plain device copy, not kernel work
+    RPL_CUDA(c, cudaMemcpy2DAsync(a.nodes_out, (size_t)a.stride * 8, a.nodes, (size_t)a.stride * 8,
+                                  (size_t)a.stride * 8, a.n_scans, cudaMemcpyDeviceToDevice, stream),
+             RPL_RESULT_OPERATION_FAIL);
+    a.nodes_out = nullptr;
+  }
+  const FastKernel k = pick_fast(a, flags);
+  if (k != FastKernel::kNone) {
+    RPL_CUDA(c, cudaMemsetAsync(l.fallback_count, 0, sizeof(uint32_t), stream), RPL_RESULT_OPERATION_FAIL);
+    const rpl_result r = launch_fast(c, l, a, k, stream, cloud, post_fused);
+    if (r != RPL_RESULT_OK) return r;
+  }
+  return launch_general(c, l, a, k == FastKernel::kNone, stream);
+}
+
+// the fields of a LaserScan launch that come from the parameters and the lane
+rpl::ScanBatchArgs scan_args(const rpl_scan_params* p, const Lane& l) {
+  rpl::ScanBatchArgs a{};
+  a.fallback_list = l.fallback_list;
+  a.fallback_count = l.fallback_count;
+  a.is_new_protocol = p->is_new_protocol;
+  a.mode_a = p->scan_processing;
+  a.inverted = p->inverted;
+  a.apply_ascend = p->apply_ascend;
+  a.angle = l.cws.angle;
+  return a;
+}
 
 // queue the scan kernels for one device-resident batch on `stream`
 rpl_result enqueue_scan(rpl_ctx* c, Lane& l, const rpl_node_hq* nodes, const uint32_t* counts,
@@ -133,10 +236,7 @@ rpl_result enqueue_scan(rpl_ctx* c, Lane& l, const rpl_node_hq* nodes, const uin
     c->err = "node buffers must be 8-byte aligned";
     return RPL_RESULT_INVALID_DATA;
   }
-  rpl::ScanBatchArgs a{};
-  a.xyzi = nullptr;
-  a.trig = nullptr;
-  a.angle = l.cws.angle;
+  rpl::ScanBatchArgs a = scan_args(p, l);
   a.nodes = reinterpret_cast<const uint2*>(nodes);
   a.nodes_out = reinterpret_cast<uint2*>(nodes_out);
   a.counts = counts;
@@ -148,90 +248,47 @@ rpl_result enqueue_scan(rpl_ctx* c, Lane& l, const rpl_node_hq* nodes, const uin
   a.angle_inc = inc;
   a.status = status;
   a.path = path;
-  a.fallback_list = l.fallback_list;
-  a.fallback_count = l.fallback_count;
-  a.is_new_protocol = p->is_new_protocol;
-  a.mode_a = p->scan_processing;
-  a.inverted = p->inverted;
-  a.apply_ascend = p->apply_ascend;
   a.views = views;
   a.nodes_total = nodes_total;
   return enqueue_args(c, l, a, p->flags, stream);
 }
 
-rpl_result enqueue_args(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, uint32_t flags, cudaStream_t stream,
-                        const PostParams* post, bool* post_fused) {
-  const uint32_t n_scans = a.n_scans, stride = a.stride;
-  bool force_general = (flags & RPL_FLAG_FORCE_GENERAL) != 0;
-  if (post_fused) *post_fused = false;
-  if (a.nodes_out && !a.apply_ascend) {
-    // no geometric correction requested: the buffer passes through unchanged
-    // (reference lidar_driver_wrapper.cpp:330-337); a plain device copy, not kernel work
-    RPL_CUDA(c, cudaMemcpy2DAsync(a.nodes_out, (size_t)stride * 8, a.nodes, (size_t)stride * 8,
-                                  (size_t)stride * 8, n_scans, cudaMemcpyDeviceToDevice, stream),
-             RPL_RESULT_OPERATION_FAIL);
-    a.nodes_out = nullptr;
-  }
-  // status-only calls (no LaserScan, no ascended buffer) take the general kernel
-  if (!a.ranges && !a.nodes_out && !a.xyzi) force_general = true;
-  // revolutions that fit shared memory (what a lidar delivers) have their own kernels
-  const bool small = !force_general && rpl::scan_small_applies(stride) && (flags & RPL_FLAG_NO_SMALL) == 0;
-  // above that the PointCloud2 payload exists in the TMA kernel and the general kernel only
-  if (a.xyzi && !small && ((reinterpret_cast<uintptr_t>(a.nodes) & 15u) != 0 || (stride & 1u) != 0)) force_general = true;
-  if (!force_general) {
-    RPL_CUDA(c, cudaMemsetAsync(l.fallback_count, 0, sizeof(uint32_t), stream), RPL_RESULT_OPERATION_FAIL);
-    // the TMA-ring kernel needs every scan base 16-byte aligned
-    const bool emit = a.nodes_out != nullptr;
-    const bool aligned = (reinterpret_cast<uintptr_t>(a.nodes) & 15u) == 0 && (stride & 1u) == 0;
-    const bool use_tma = !emit && aligned && ((flags & RPL_FLAG_NO_TMA) == 0 || a.xyzi != nullptr);
-    // LaserScan Mode B scans too large for the shared-memory kernels but no larger than two SMs can stage
-    const bool use_cluster = use_tma && !a.xyzi && !a.mode_a && rpl::scan_tma_cluster_applies(stride);
-    const int tma_grid = c->tma_grid[a.xyzi ? 2 : a.mode_a ? 1 : 0];
-    const int grid = use_cluster ? 2 * (int)std::min<uint32_t>(n_scans, (uint32_t)c->tma_clusters)
-                                 : (int)std::min<uint32_t>(n_scans, (uint32_t)(use_tma ? tma_grid : c->fast_grid));
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    if (c->profile) {
-      cudaEventCreate(&e0);
-      cudaEventCreate(&e1);
-      cudaEventRecord(e0, stream);
+// Runs fn(lane, first, n) over `total` items in chunks of `chunk`, round-robin over the lanes, and waits for every
+// lane.  A failure leaves the loop with copies possibly still in flight: nothing may still be writing into the
+// caller's buffers when the error is reported, so every lane is drained first and the first error kept.
+template <class F>
+rpl_result run_chunks(rpl_ctx* c, uint32_t total, uint32_t chunk, F fn) {
+  uint32_t ci = 0;
+  for (uint32_t s0 = 0; s0 < total; s0 += chunk, ++ci) {
+    const rpl_result r = fn(c->lane[ci % kLanes], s0, std::min(chunk, total - s0));
+    if (r != RPL_RESULT_OK) {
+      const std::string why = c->err;
+      for (int i = 0; i < kLanes; ++i) cudaStreamSynchronize(c->lane[i].stream);
+      c->err = why;
+      return r;
     }
-    if (small) {
-      // SOR / voxel grid run inside the kernel when the 32-bit cell keys and accumulators are exact:
-      // |cell index| < 32768 and voxel <= 4 m (scan_small.cu); otherwise as separate passes
-      bool fuse = false;
-      if (a.xyzi && post && (post->sor_k > 0 || post->voxel > 0.0f) && rpl::scan_small_post_applies(stride))
-        fuse = post->voxel == 0.0f || (post->voxel <= 4.0f && a.range_max / post->voxel < 32000.0f);
-      RPL_CUDA(c, rpl::launch_scan_small(a, l.fws.max_nodes, fuse ? post->sor_k : 0u, fuse ? post->sor_alpha : 0.0f,
-                                         fuse ? post->voxel : 0.0f, c->num_sms, stream),
-               RPL_RESULT_OPERATION_FAIL);
-      if (post_fused) *post_fused = fuse;
-    } else if (use_cluster) {
-      RPL_CUDA(c, rpl::launch_scan_tma_cluster(a, l.fws.max_nodes, grid, stream), RPL_RESULT_OPERATION_FAIL);
-    } else if (use_tma) {
-      RPL_CUDA(c, rpl::launch_scan_tma(a, l.fws.max_nodes, grid, stream), RPL_RESULT_OPERATION_FAIL);
-    } else {
-      RPL_CUDA(c, rpl::launch_scan_fast(a, l.fws, grid, stream), RPL_RESULT_OPERATION_FAIL);
-    }
-    if (c->profile) {
-      cudaEventRecord(e1, stream);
-      c->prof_fast.emplace_back(e0, e1);
-    }
-    c->launches++;
   }
-  const int ggrid = (int)std::min<uint32_t>(n_scans, (uint32_t)c->general_grid);
-  cudaEvent_t g0 = nullptr, g1 = nullptr;
-  if (c->profile) {
-    cudaEventCreate(&g0);
-    cudaEventCreate(&g1);
-    cudaEventRecord(g0, stream);
-  }
-  RPL_CUDA(c, rpl::launch_scan_general(a, l.gws, ggrid, force_general, stream), RPL_RESULT_OPERATION_FAIL);
-  if (c->profile) {
-    cudaEventRecord(g1, stream);
-    c->prof_general.emplace_back(g0, g1);
-  }
-  c->launches++;
-  return RPL_RESULT_OK;
+  return rpl_ctx_synchronize(c);
+}
+
+// argument checks shared by several entry points
+bool sample_duration_ok(rpl_ctx* c, uint32_t sample_duration_us) {
+  if (sample_duration_us != 0 && sample_duration_us <= 1000000u) return true;
+  c->err = "sample_duration_us must be in [1, 1000000]";
+  return false;
+}
+
+// bytes per capsule of a capsule answer type; 0, with the error set, for any other type
+uint32_t capsule_bytes(rpl_ctx* c, uint32_t ans_type) {
+  const uint32_t b = rpl_capsule_bytes(ans_type);
+  if (b == 0) c->err = "unknown answer type (capsule formats are 0x82..0x86)";
+  return b;
+}
+
+bool frame_id_length_ok(rpl_ctx* c, size_t len) {
+  if (len <= 255) return true;
+  c->err = "frame_id longer than 255 characters";
+  return false;
 }
 
 }  // namespace
@@ -300,8 +357,7 @@ rpl_result rpl_ctx_create(int device, uint32_t max_nodes, uint32_t max_scans, rp
         !cuda_ok(c, dev_alloc(&l.gws.idx0, gen_nodes), "cudaMalloc") ||
         !cuda_ok(c, dev_alloc(&l.gws.idx1, gen_nodes), "cudaMalloc") ||
         !cuda_ok(c, dev_alloc(&l.gws.vidx, gen_nodes), "cudaMalloc") ||
-        !cuda_ok(c, dev_alloc(&l.gws.cell, gen_nodes), "cudaMalloc") ||
-        false)
+        !cuda_ok(c, dev_alloc(&l.gws.cell, gen_nodes), "cudaMalloc"))
       return fail(oom);
     if (i == 0) {
       if (!cuda_ok(c, rpl::cloud_workspace_alloc(l.cws, c->num_sms, max_nodes), "cloud workspace")) return fail(oom);
@@ -404,14 +460,14 @@ rpl_result rpl_scan_batch_dev(rpl_ctx* c, const rpl_node_hq* nodes, const uint32
                               uint32_t* beam_counts, float* angle_increment, uint32_t* status,
                               uint32_t* path, void* stream) {
   if (!c) return RPL_RESULT_INVALID_DATA;
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   if (n_scans != 0 && stride == 0) {
     c->err = "stride == 0";
     return RPL_RESULT_INVALID_DATA;
   }
   // counts[] live on the device: a scan with counts[s] > stride or > the context's max_nodes is reported
   // through status[s] = RPL_RESULT_INVALID_DATA by the kernels (nothing else is written for it)
-  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : c->lane[0].stream;
   return enqueue_scan(c, c->lane[0], nodes, counts, n_scans, stride, params, nodes_out, ranges,
                       intensities, beam_counts, angle_increment, status, path, st);
 }
@@ -455,7 +511,7 @@ rpl_result rpl_scan_batch(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t* 
   uint32_t* hs_inc = c->h_small + c->max_scans;
   uint32_t* hs_status = c->h_small + 2 * (size_t)c->max_scans;
   uint32_t* hs_path = c->h_small + 3 * (size_t)c->max_scans;
-  // one chunk through one lane; any failure leaves the loop with copies possibly still in flight
+  // one chunk through one lane
   auto run_chunk = [&](Lane& l, uint32_t s0, uint32_t ns) -> rpl_result {
     const size_t off = (size_t)s0 * stride, cnt = (size_t)ns * stride;
     // the lane's previous chunk (2 chunks ago) must have left its staging buffers
@@ -498,19 +554,8 @@ rpl_result rpl_scan_batch(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t* 
                RPL_RESULT_OPERATION_FAIL);
     return RPL_RESULT_OK;
   };
-  uint32_t ci = 0;
-  for (uint32_t s0 = 0; s0 < n_scans; s0 += chunk, ++ci) {
-    const rpl_result r = run_chunk(c->lane[ci % kLanes], s0, std::min(chunk, n_scans - s0));
-    if (r != RPL_RESULT_OK) {
-      // nothing may still be writing into the caller's buffers when the error is reported
-      const std::string why = c->err;
-      for (int i = 0; i < kLanes; ++i) cudaStreamSynchronize(c->lane[i].stream);
-      c->err = why;
-      return r;
-    }
-  }
-  const rpl_result rs = rpl_ctx_synchronize(c);
-  if (rs != RPL_RESULT_OK) return rs;
+  const rpl_result r = run_chunks(c, n_scans, chunk, run_chunk);
+  if (r != RPL_RESULT_OK) return r;
   if (beam_counts) std::memcpy(beam_counts, hs_beams, (size_t)n_scans * 4);
   if (angle_increment) std::memcpy(angle_increment, hs_inc, (size_t)n_scans * 4);
   if (status) std::memcpy(status, hs_status, (size_t)n_scans * 4);
@@ -554,7 +599,8 @@ static_assert(sizeof(OneSmall) == 64, "control block");
 
 // One lidar revolution: the operating point of the reference (one scan thread, ~10 Hz).  What
 // matters here is latency, so the scan travels in one pinned block each way and the general
-// kernel is launched only when the fast kernel reports a duplicate-key scan.
+// kernel is launched only when the fast kernel reports a duplicate-key scan.  The fast kernel is
+// the one a batch of one scan at stride one_stride gets (pick_fast).
 rpl_result scan_single(rpl_ctx* c, const rpl_node_hq* nodes_in, size_t count, const rpl_scan_params* p,
                        rpl_node_hq* nodes_out, float* ranges, float* intensities, uint32_t* beam_count,
                        float* angle_increment, rpl_result* ascend_status) {
@@ -562,7 +608,6 @@ rpl_result scan_single(rpl_ctx* c, const rpl_node_hq* nodes_in, size_t count, co
   Lane& l = c->lane[0];
   const size_t S = c->one_stride, n = count;
   const size_t off_small = S * 8, off_nout = off_small + 64, off_r = off_nout + S * 8, off_i = off_r + S * 4;
-  const size_t total = off_i + S * 4;
   std::memcpy(c->h_one, nodes_in, n * 8);
   OneSmall* hs = reinterpret_cast<OneSmall*>(c->h_one + off_small);
   std::memset(hs, 0, sizeof(OneSmall));
@@ -579,8 +624,8 @@ rpl_result scan_single(rpl_ctx* c, const rpl_node_hq* nodes_in, size_t count, co
   OneSmall* ds = reinterpret_cast<OneSmall*>(c->d_one + off_small);
   const bool want_nodes = nodes_out != nullptr && p->apply_ascend;
   const bool want_scan = ranges != nullptr;
-  rpl::ScanBatchArgs a{};
-  a.nodes = reinterpret_cast<const uint2*>(c->d_one);
+  rpl::ScanBatchArgs a = scan_args(p, l);
+  a.nodes = reinterpret_cast<const uint2*>(c->d_one);  // d_one and S keep bases 16-byte aligned
   a.nodes_out = want_nodes ? reinterpret_cast<uint2*>(c->d_one + off_nout) : nullptr;
   a.counts = &ds->count;
   a.n_scans = 1;
@@ -591,20 +636,13 @@ rpl_result scan_single(rpl_ctx* c, const rpl_node_hq* nodes_in, size_t count, co
   a.angle_inc = &ds->inc;
   a.status = &ds->status;
   a.path = &ds->path;
-  a.fallback_list = &ds->fallback_list;
+  a.fallback_list = &ds->fallback_list;  // zeroed by the H2D copy
   a.fallback_count = &ds->fallback_count;
-  a.is_new_protocol = p->is_new_protocol;
-  a.mode_a = p->scan_processing;
-  a.inverted = p->inverted;
-  a.apply_ascend = p->apply_ascend;
-  a.angle = l.cws.angle;
-  const bool force_general = (p->flags & RPL_FLAG_FORCE_GENERAL) != 0 || (!want_nodes && !want_scan);
   // D2H extent: control block + whatever was produced, trimmed to the live part
   auto copy_back = [&]() -> rpl_result {
     size_t end = off_nout;
     if (want_nodes) end = off_nout + n * 8;
     if (want_scan) end = off_i + n * 4;
-    (void)total;
     if (want_scan && (end - off_small) > 3 * (64 + n * 16) + 8192) {
       // short scan in a large context: three small copies beat one copy across the gaps
       RPL_CUDA(c, cudaMemcpyAsync(hs, ds, 64 + (want_nodes ? n * 8 : 0), cudaMemcpyDeviceToHost, l.stream),
@@ -620,20 +658,15 @@ rpl_result scan_single(rpl_ctx* c, const rpl_node_hq* nodes_in, size_t count, co
     RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);
     return RPL_RESULT_OK;
   };
-  if (!force_general) {
-    const bool use_tma = !want_nodes && (p->flags & RPL_FLAG_NO_TMA) == 0;  // d_one and S keep bases 16-byte aligned
-    if (use_tma)
-      RPL_CUDA(c, rpl::launch_scan_tma(a, l.fws.max_nodes, 1, l.stream), RPL_RESULT_OPERATION_FAIL);
-    else
-      RPL_CUDA(c, rpl::launch_scan_fast(a, l.fws, 1, l.stream), RPL_RESULT_OPERATION_FAIL);
-    c->launches++;
-    rpl_result r = copy_back();
+  const FastKernel k = pick_fast(a, p->flags);
+  if (k != FastKernel::kNone) {
+    rpl_result r = launch_fast(c, l, a, k, l.stream);
+    if (r == RPL_RESULT_OK) r = copy_back();
     if (r != RPL_RESULT_OK) return r;
   }
-  if (force_general || hs->fallback_count != 0) {
-    RPL_CUDA(c, rpl::launch_scan_general(a, l.gws, 1, true, l.stream), RPL_RESULT_OPERATION_FAIL);
-    c->launches++;
-    rpl_result r = copy_back();
+  if (k == FastKernel::kNone || hs->fallback_count != 0) {
+    rpl_result r = launch_general(c, l, a, true, l.stream);
+    if (r == RPL_RESULT_OK) r = copy_back();
     if (r != RPL_RESULT_OK) return r;
   }
   const uint32_t m = hs->beams;
@@ -692,8 +725,8 @@ rpl_result rpl_scan(rpl_ctx* c, rpl_node_hq* nodes, size_t count, const rpl_scan
 namespace {
 // one launch of the capsule decoder on arguments the entry point has checked (n_streams > 0)
 rpl_result decode_capsules_launch(rpl_ctx* c, uint32_t ans_type, const rpl::CapsuleDecodeArgs& a, void* stream) {
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : c->lane[0].stream;
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   // one CTA per stream, up to four (dense) or eight (the other formats) CTAs per SM; a CTA loops over the rest
   const uint32_t ctas_per_sm = ans_type == 0x85 ? 4u : 8u;
   const int grid = (int)std::min<uint32_t>(a.n_streams, (uint32_t)c->num_sms * ctas_per_sm);
@@ -725,10 +758,7 @@ rpl_result rpl_decode_dense_batch_starts_dev(rpl_ctx* c, const uint8_t* capsules
     c->err = "scan_starts and scan_start_counts go together (starts_stride > 0)";
     return RPL_RESULT_INVALID_DATA;
   }
-  if (sample_duration_us == 0 || sample_duration_us > 1000000u) {
-    c->err = "sample_duration_us must be in [1, 1000000]";
-    return RPL_RESULT_INVALID_DATA;
-  }
+  if (!sample_duration_ok(c, sample_duration_us)) return RPL_RESULT_INVALID_DATA;
   if ((reinterpret_cast<uintptr_t>(capsules) & 3u) != 0 || misaligned8(nodes_out)) {
     c->err = "capsule buffer must be 4-byte aligned, nodes_out 8-byte aligned";
     return RPL_RESULT_INVALID_DATA;
@@ -792,18 +822,12 @@ rpl_result rpl_decode_capsules_batch_dev(rpl_ctx* c, uint32_t ans_type, const ui
                                          uint32_t* capsule_status, uint32_t* capsule_node_offset,
                                          uint32_t* state_out, void* stream) {
   if (!c || !capsules || !capsule_counts || !nodes_out) return RPL_RESULT_INVALID_DATA;
-  if (rpl_capsule_bytes(ans_type) == 0) {
-    c->err = "unknown answer type (capsule formats are 0x82..0x86)";
-    return RPL_RESULT_INVALID_DATA;
-  }
+  if (capsule_bytes(c, ans_type) == 0) return RPL_RESULT_INVALID_DATA;
   if (misaligned8(nodes_out)) {
     c->err = "nodes_out must be 8-byte aligned";
     return RPL_RESULT_INVALID_DATA;
   }
-  if (sample_duration_us == 0 || sample_duration_us > 1000000u) {
-    c->err = "sample_duration_us must be in [1, 1000000]";
-    return RPL_RESULT_INVALID_DATA;
-  }
+  if (!sample_duration_ok(c, sample_duration_us)) return RPL_RESULT_INVALID_DATA;
   if (n_streams == 0) return RPL_RESULT_OK;
   if (ans_type == 0x85 && (reinterpret_cast<uintptr_t>(capsules) & 3u) != 0) {
     c->err = "dense capsule buffer must be 4-byte aligned";
@@ -846,14 +870,11 @@ rpl_result rpl_decode_capsules(rpl_ctx* c, uint32_t ans_type, const uint8_t* cap
   }
   if (want_ts) sample_duration_us = timing->sample_duration_us;
   *node_count = 0;
-  const uint32_t cbytes = rpl_capsule_bytes(ans_type), per = rpl_capsule_nodes(ans_type);
-  if (cbytes == 0) {
-    c->err = "unknown answer type (capsule formats are 0x82..0x86)";
-    return RPL_RESULT_INVALID_DATA;
-  }
+  const uint32_t cbytes = capsule_bytes(c, ans_type), per = rpl_capsule_nodes(ans_type);
+  if (cbytes == 0) return RPL_RESULT_INVALID_DATA;
   if (n_capsules == 0) return RPL_RESULT_OK;
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  cudaStream_t st = c->lane[0].stream;
+  cudaStream_t st;
+  if (!enter_device(c, nullptr, &st)) return RPL_RESULT_OPERATION_FAIL;
   const size_t cb = (size_t)n_capsules * cbytes, nb = (size_t)n_capsules * per * 8, sb = (size_t)n_capsules * 4;
   HostDecode h;  // [capsules | pad][nodes][status][offsets][count, n_nodes, state in x2, state out x2][rx][ts]
   h.o_nodes = (cb + 15) & ~(size_t)15;
@@ -910,8 +931,8 @@ rpl_result rpl_frame_capsules_dev(rpl_ctx* c, uint32_t ans_type, const uint8_t* 
     return RPL_RESULT_INVALID_DATA;
   }
   if (n_streams == 0) return RPL_RESULT_OK;
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : c->lane[0].stream;
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   rpl::FrameArgs a{};
   a.bytes = bytes;
   a.byte_counts = byte_counts;
@@ -938,8 +959,8 @@ rpl_result rpl_decode_normal_batch_dev(rpl_ctx* c, const uint8_t* bytes, const u
     return RPL_RESULT_INVALID_DATA;
   }
   if (n_streams == 0) return RPL_RESULT_OK;
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : c->lane[0].stream;
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   rpl::NormalDecodeArgs a{};
   a.bytes = bytes;
   a.byte_counts = byte_counts;
@@ -960,8 +981,8 @@ rpl_result rpl_decode_normal(rpl_ctx* c, const uint8_t* bytes, uint32_t n_bytes,
   if (!c || !node_count || (n_bytes && (!bytes || !nodes_out))) return RPL_RESULT_INVALID_DATA;
   *node_count = 0;
   if (n_bytes < 5) return RPL_RESULT_OK;
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  cudaStream_t st = c->lane[0].stream;
+  cudaStream_t st;
+  if (!enter_device(c, nullptr, &st)) return RPL_RESULT_OPERATION_FAIL;
   HostDecode h;  // [bytes | pad][nodes][byte count, node count]
   h.o_nodes = ((size_t)n_bytes + 15) & ~(size_t)15;
   h.o_small = h.o_nodes + (size_t)(n_bytes / 5) * 8;
@@ -995,6 +1016,10 @@ rpl_result assemble_common(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t*
                                   uint64_t* scan_begin_ts_us, void* stream, const uint32_t* scan_starts = nullptr,
                                   uint32_t starts_stride = 0, const uint32_t* scan_start_counts = nullptr) {
   if (!c || !nodes || !node_counts || (!scans_out && !views_out) || !scan_len || !scans_per_stream) return RPL_RESULT_INVALID_DATA;
+  if (views_out && (unsigned long long)n_streams * stride_nodes > 0xFFFFFFFFull) {
+    c->err = "view mode addresses nodes with 32 bits: n_streams * stride_nodes must stay below 2^32";
+    return RPL_RESULT_INVALID_DATA;
+  }
   const bool any = capsule_status || capsule_node_offset || capsule_counts;
   if (any && !(capsule_status && capsule_node_offset && capsule_counts)) {
     c->err = "capsule_status, capsule_node_offset and capsule_counts go together";
@@ -1009,7 +1034,8 @@ rpl_result assemble_common(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t*
     return RPL_RESULT_INVALID_DATA;
   }
   if (n_streams == 0) return RPL_RESULT_OK;
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   const size_t need_rp = (size_t)n_streams * std::max<uint32_t>(stride_capsules, 1u);
   const size_t need_desc = (size_t)n_streams * max_scans;
   if (need_rp > c->reset_prefix_cap) {
@@ -1024,7 +1050,6 @@ rpl_result assemble_common(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t*
     RPL_CUDA(c, dev_alloc(&c->d_desc, need_desc), RPL_RESULT_INSUFFICIENT_MEMORY);
     c->desc_cap = need_desc;
   }
-  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : c->lane[0].stream;
   rpl::AssembleArgs a{};
   a.nodes = reinterpret_cast<const uint2*>(nodes);
   a.node_counts = node_counts;
@@ -1078,10 +1103,6 @@ rpl_result rpl_assemble_scan_views_dev(rpl_ctx* c, rpl_node_hq* nodes, const uin
                                        rpl_scan_view* views_out, uint32_t* scan_len, uint32_t* scans_per_stream,
                                        const uint64_t* node_ts_us, uint64_t* scan_begin_ts_us, void* stream) {
   if (!views_out) return RPL_RESULT_INVALID_DATA;
-  if ((unsigned long long)n_streams * stride_nodes > 0xFFFFFFFFull) {
-    if (c) c->err = "view mode addresses nodes with 32 bits: n_streams * stride_nodes must stay below 2^32";
-    return RPL_RESULT_INVALID_DATA;
-  }
   return assemble_common(c, nodes, node_counts, n_streams, stride_nodes, capsule_status, capsule_node_offset,
                          capsule_counts, stride_capsules, max_nodes, max_scans, max_nodes, nullptr, views_out, scan_len,
                          scans_per_stream, node_ts_us, scan_begin_ts_us, stream);
@@ -1096,10 +1117,6 @@ rpl_result rpl_assemble_scan_views_starts_dev(rpl_ctx* c, rpl_node_hq* nodes, co
                                               uint32_t* scan_len, uint32_t* scans_per_stream, const uint64_t* node_ts_us,
                                               uint64_t* scan_begin_ts_us, void* stream) {
   if (!views_out || !scan_starts || !scan_start_counts || starts_stride == 0) return RPL_RESULT_INVALID_DATA;
-  if ((unsigned long long)n_streams * stride_nodes > 0xFFFFFFFFull) {
-    if (c) c->err = "view mode addresses nodes with 32 bits: n_streams * stride_nodes must stay below 2^32";
-    return RPL_RESULT_INVALID_DATA;
-  }
   return assemble_common(c, nodes, node_counts, n_streams, stride_nodes, capsule_status, capsule_node_offset,
                          capsule_counts, stride_capsules, max_nodes, max_scans, max_nodes, nullptr, views_out, scan_len,
                          scans_per_stream, node_ts_us, scan_begin_ts_us, stream, scan_starts, starts_stride,
@@ -1119,8 +1136,8 @@ rpl_result rpl_scan_views_dev(rpl_ctx* c, const rpl_node_hq* nodes, uint64_t nod
     c->err = "the node buffer of a view batch must be 16-byte aligned";
     return RPL_RESULT_INVALID_DATA;
   }
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : c->lane[0].stream;
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   return enqueue_scan(c, c->lane[0], nodes, reinterpret_cast<const uint32_t*>(views), n_scans, stride, params, nodes_out,
                       ranges, intensities, beam_counts, angle_increment, status, path, st,
                       reinterpret_cast<const uint2*>(views), nodes_total);
@@ -1223,17 +1240,7 @@ rpl_result rpl_chain_dense_laserscan(rpl_ctx* c, const uint8_t* capsules, const 
     RPL_CUDA(c, cudaMemcpyAsync(scans_per_stream + s0, d + o_sps, (size_t)ns * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
     return RPL_RESULT_OK;
   };
-  uint32_t ci = 0;
-  for (uint32_t s0 = 0; s0 < n_streams; s0 += chunk, ++ci) {
-    const rpl_result r = run_chunk(c->lane[ci % kLanes], s0, std::min(chunk, n_streams - s0));
-    if (r != RPL_RESULT_OK) {
-      const std::string why = c->err;
-      for (int i = 0; i < kLanes; ++i) cudaStreamSynchronize(c->lane[i].stream);
-      c->err = why;
-      return r;
-    }
-  }
-  return rpl_ctx_synchronize(c);
+  return run_chunks(c, n_streams, chunk, run_chunk);
 }
 
 // ---- LaserScan / PointCloud2 -> CDR (SURVEY.md 8(f) rank 3) -------------------------------------
@@ -1281,18 +1288,15 @@ rpl_result rpl_laserscan_cdr_batch_dev(rpl_ctx* c, const rpl_laserscan_meta* met
                                        uint8_t* cdr_out, uint32_t cdr_stride, uint32_t* cdr_sizes, void* stream) {
   if (!c || !meta || !frame_id || !ranges || !intensities || !beam_counts || !cdr_out) return RPL_RESULT_INVALID_DATA;
   const size_t L = std::strlen(frame_id);
-  if (L > 255) {
-    c->err = "frame_id longer than 255 characters";
-    return RPL_RESULT_INVALID_DATA;
-  }
+  if (!frame_id_length_ok(c, L)) return RPL_RESULT_INVALID_DATA;
   if ((cdr_stride & 3u) || cdr_stride < rpl_laserscan_cdr_size((uint32_t)L, stride) ||
       (reinterpret_cast<uintptr_t>(cdr_out) & 3u)) {
     c->err = "cdr_out must be 4-byte aligned, cdr_stride a multiple of 4 and >= rpl_laserscan_cdr_size(len, stride)";
     return RPL_RESULT_INVALID_DATA;
   }
   if (n_scans == 0) return RPL_RESULT_OK;
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : c->lane[0].stream;
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   rpl::CdrTemplate t{};
   CdrWriter w(t.prefix);
   w.u32(0);  // stamp.sec     (patched)
@@ -1323,18 +1327,15 @@ rpl_result rpl_pointcloud2_cdr_batch_dev(rpl_ctx* c, const uint32_t* stamps, con
                                          uint32_t* cdr_sizes, void* stream) {
   if (!c || !stamps || !frame_id || !xyzi || !point_counts || !cdr_out) return RPL_RESULT_INVALID_DATA;
   const size_t L = std::strlen(frame_id);
-  if (L > 255) {
-    c->err = "frame_id longer than 255 characters";
-    return RPL_RESULT_INVALID_DATA;
-  }
+  if (!frame_id_length_ok(c, L)) return RPL_RESULT_INVALID_DATA;
   if ((cdr_stride & 15u) || cdr_stride < rpl_pointcloud2_cdr_size((uint32_t)L, stride) ||
       (reinterpret_cast<uintptr_t>(cdr_out) & 15u)) {
     c->err = "cdr_out must be 16-byte aligned, cdr_stride a multiple of 16 and >= rpl_pointcloud2_cdr_size(len, stride)";
     return RPL_RESULT_INVALID_DATA;
   }
   if (n_clouds == 0) return RPL_RESULT_OK;
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : c->lane[0].stream;
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   rpl::CdrTemplate t{};
   CdrWriter w(t.prefix);
   w.u32(0);
@@ -1384,13 +1385,10 @@ rpl_result rpl_node_timestamps_dev(rpl_ctx* c, uint32_t ans_type, const rpl_timi
     c->err = "timestamp buffers must be 8-byte aligned";
     return RPL_RESULT_INVALID_DATA;
   }
-  if (rpl_capsule_bytes(ans_type) == 0) {
-    c->err = "unknown answer type (capsule formats are 0x82..0x86)";
-    return RPL_RESULT_INVALID_DATA;
-  }
+  if (capsule_bytes(c, ans_type) == 0) return RPL_RESULT_INVALID_DATA;
   if (n_streams == 0) return RPL_RESULT_OK;
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : c->lane[0].stream;
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   rpl::TimingDesc t{timing->sample_duration_us, timing->native_baudrate, timing->linkage_delay_us,
                     timing->native_interface_type};
   rpl::TimestampArgs a{};
@@ -1417,8 +1415,8 @@ rpl_result rpl_normal_timestamps_dev(rpl_ctx* c, const rpl_timing* timing, const
     return RPL_RESULT_INVALID_DATA;
   }
   if (n_streams == 0) return RPL_RESULT_OK;
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : c->lane[0].stream;
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   rpl::TimingDesc t{timing->sample_duration_us, timing->native_baudrate, timing->linkage_delay_us,
                     timing->native_interface_type};
   rpl::NormalTimestampArgs a{};
@@ -1440,8 +1438,8 @@ rpl_result rpl_synth_batch_dev(rpl_ctx* c, uint64_t first_scan_id, uint32_t n_sc
                                uint32_t stride, int variant, rpl_node_hq* nodes, uint32_t* counts,
                                void* stream) {
   if (!c || !nodes || n > stride || variant < 0 || variant > 4) return RPL_RESULT_INVALID_DATA;
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : c->lane[0].stream;
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   RPL_CUDA(c, rpl::launch_synth(first_scan_id, n_scans, n, stride, variant,
                                 reinterpret_cast<uint2*>(nodes), counts, st),
            RPL_RESULT_OPERATION_FAIL);
@@ -1463,8 +1461,8 @@ rpl_result rpl_cloud_batch_dev(rpl_ctx* c, const rpl_node_hq* nodes, const uint3
     c->err = "voxel grid: voxel_size must be >= 1e-6 m and range_max < 1000 m (cell indices must fit 31 bits)";
     return RPL_RESULT_INVALID_DATA;
   }
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : c->lane[0].stream;
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   rpl::ScanBatchArgs a{};
   a.nodes = reinterpret_cast<const uint2*>(nodes);
   a.counts = counts;
@@ -1483,13 +1481,9 @@ rpl_result rpl_cloud_batch_dev(rpl_ctx* c, const rpl_node_hq* nodes, const uint3
   // Revolutions of at most 4096 nodes: the whole chain (window, xyz, SOR, voxel grid) in one kernel, in shared
   // memory (scan_small.cu); the separate in-place post passes then only see the duplicate-key scans that kernel
   // handed to the general kernel.  Larger revolutions: steps 1-3 inside the scan kernels, steps 4-5 as post passes.
-  PostParams pp;
-  pp.sor_k = params->sor_k;
-  pp.sor_alpha = params->sor_alpha;
-  pp.voxel = params->voxel_size;
   bool fused = false;
   const uint32_t flags = (params->flags & RPL_CLOUD_NO_FUSED) ? RPL_FLAG_NO_SMALL : 0u;
-  rpl_result r = enqueue_args(c, c->lane[0], a, flags, st, &pp, &fused);
+  rpl_result r = enqueue_args(c, c->lane[0], a, flags, st, params, &fused);
   if (r != RPL_RESULT_OK) return r;
   if (params->sor_k > 0 || params->voxel_size > 0.0f) {
     int launched = 0;
@@ -1532,8 +1526,8 @@ rpl_result rpl_cloud_fuse_dev(rpl_ctx* c, const float* xyzi, const uint32_t* poi
                               uint32_t n_scans, uint32_t stride, float* fused, uint32_t* offsets,
                               uint32_t* total, void* stream) {
   if (!c || !xyzi || !point_counts || !fused || !offsets || !total) return RPL_RESULT_INVALID_DATA;
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : c->lane[0].stream;
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   int launched = 0;
   RPL_CUDA(c, rpl::launch_cloud_fuse(reinterpret_cast<const float4*>(xyzi), point_counts, n_scans, stride,
                                      reinterpret_cast<float4*>(fused), 0xFFFFFFFFu, offsets, total, st, &launched),
@@ -1602,8 +1596,8 @@ rpl_result rpl_cloud_fuse_push_dev(rpl_ctx* c, const float* xyzi, const uint32_t
     }
     peers.base[p] = static_cast<unsigned char*>(peer_bases[p]);
   }
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : c->lane[0].stream;
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   int launched = 0;
   RPL_CUDA(c, rpl::launch_cloud_fuse_push(reinterpret_cast<const float4*>(xyzi), point_counts, n_scans, stride, peers,
                                           world, rank, slot_points, offsets, total, st, &launched),

@@ -82,5 +82,12 @@ inline bool cuda_ok(rpl_ctx* c, cudaError_t e, const char* what) {
     if (!cuda_ok((c), (call), #call)) return (code); \
   } while (0)
 
+// Selects the context's device for an entry point and resolves the stream it runs on: the caller's, or the
+// context's default stream (lane 0) when none is given.
+inline bool enter_device(rpl_ctx* c, void* stream, cudaStream_t* st) {
+  *st = stream ? static_cast<cudaStream_t>(stream) : c->lane[0].stream;
+  return cuda_ok(c, cudaSetDevice(c->device), "cudaSetDevice(c->device)");
+}
+
 // device buffers of 8-byte records (nodes, 64-bit stamps) are accessed with 8-byte loads and stores
 inline bool misaligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7u) != 0; }

@@ -1,9 +1,9 @@
 """The scan kernels across their whole size range, against the CPU oracle (stable rule) bit for bit, with the kernel
 that ran made visible.
 
-enqueue_args (rpl_capi.cu) picks one of five kernels per launch from the stride, the base alignment, the mode, the
-ascended buffer and the flags; scan_single picks the ring kernel or scan_fast_kernel for one scan.  Every kernel
-hands a scan it cannot serve to scan_general_kernel, so a change to the dispatch leaves every result correct and
+pick_fast (rpl_capi.cu) picks one of five kernels per launch from the stride, the base alignment, the mode, the
+ascended buffer and the flags, for batches and single scans alike (a single scan is a batch of one at the context's
+stride: max_nodes rounded up to even).  Every kernel hands a scan it cannot serve to scan_general_kernel, so a change to the dispatch leaves every result correct and
 moves a test case onto a different kernel without any parity test noticing.  Here each case runs under the CUDA
 profiler and asserts the kernel it expects (kernels_run, DISPATCH), then covers what the other tests never reach:
 
@@ -334,13 +334,13 @@ NS, NT, FG = 4, 2, 1  # RPL_FLAG_NO_SMALL, RPL_FLAG_NO_TMA, RPL_FLAG_FORCE_GENER
 # (entry, stride, count, base offset in bytes, mode_a, ascend, emit, flags, duplicate key) -> the fast kernel that
 # must run (None: none, the general kernel serves every scan).  Batches (batch = rpl_scan_batch, dev =
 # rpl_scan_batch_dev, status = rpl_scan_batch without LaserScan or ascended buffer, cloud = rpl_cloud_batch) run
-# scan_general_kernel after it, always; single scans (scan, laserscan, ascend_scan; the stride is the count) run it
-# only when a scan is handed on.  enqueue_args: FORCE_GENERAL or nothing to produce -> general only; stride <= 8192
-# and not NO_SMALL -> shared-memory kernel; PointCloud2 with an unaligned base or odd stride -> general only;
-# the ascended buffer (emit with ascend), NO_TMA (LaserScan only), an odd stride or a base not 16-byte aligned ->
-# scan_fast_kernel; LaserScan Mode B at strides in (8192, 32768] -> the cluster kernel; else the ring kernel.
-# scan_single: FORCE_GENERAL -> general only; the ascended buffer or NO_TMA -> scan_fast_kernel; else the ring kernel
-# on a grid of 1, any size, Mode B included.
+# scan_general_kernel after it, always; single scans (scan, laserscan, ascend_scan; the count is given, the stride is
+# the context's) run it only when a scan is handed on.  One rule for both: FORCE_GENERAL or nothing to produce ->
+# general only; stride <= 8192 and not NO_SMALL -> shared-memory kernel; PointCloud2 with an unaligned base or odd
+# stride -> general only; the ascended buffer (emit with ascend), NO_TMA (LaserScan only), an odd stride or a base not
+# 16-byte aligned -> scan_fast_kernel; LaserScan Mode B at strides in (8192, 32768] -> the cluster kernel; else the
+# ring kernel.  The single scans here run in a 70002-node context (stride 70002); SIZED_SINGLE below runs them in a
+# context of their own size.
 DISPATCH = [
     # stride <= 8192
     ("batch", 3200, 3200, 0, 0, 1, False, 0, False, SMALL),
@@ -442,12 +442,48 @@ def dispatch_ctx(R):
     c.close()
 
 
+# single scans in a context of exactly their size: the stride the rule sees is the count rounded up to even, so the
+# shared-memory and cluster kernels serve them as they serve a batch at that stride
+SIZED_SINGLE = [
+    ("laserscan", 3200, 3200, 0, 0, 0, False, 0, False, SMALL),
+    ("laserscan", 8192, 8192, 0, 1, 0, False, 0, False, SMALL),
+    ("laserscan", 8191, 8191, 0, 0, 0, False, 0, False, SMALL),      # stride 8192
+    ("scan", 3200, 3200, 0, 1, 0, False, 0, False, SMALL),
+    ("scan", 8192, 8192, 0, 0, 1, True, 0, False, SMALL),
+    ("scan", 3200, 3200, 0, 0, 0, False, NT, False, SMALL),         # NO_TMA does not keep it off the shared memory
+    ("scan", 3200, 3200, 0, 0, 1, True, 0, True, SMALL),            # duplicate: + the general kernel
+    ("scan", 3200, 3200, 0, 0, 1, True, NS, False, FAST_EMIT_B),
+    ("scan", 3200, 3200, 0, 0, 0, False, NS, False, RING_B),
+    ("ascend_scan", 3200, 3200, 0, 0, 1, True, 0, False, SMALL),
+    ("ascend_scan", 8192, 8192, 0, 0, 1, True, 0, False, SMALL),
+    ("laserscan", 20000, 20000, 0, 0, 0, False, 0, False, CLUSTER),
+    ("laserscan", 8193, 8193, 0, 0, 0, False, 0, False, CLUSTER),   # stride 8194
+    ("laserscan", 20000, 20000, 0, 0, 0, False, 0, True, CLUSTER),  # duplicate: + the general kernel
+    ("scan", 32768, 32768, 0, 0, 0, False, 0, False, CLUSTER),
+    ("laserscan", 20000, 20000, 0, 1, 0, False, 0, False, RING_A),
+    ("scan", 20000, 20000, 0, 0, 1, True, 0, False, FAST_EMIT_B),
+    ("laserscan", 20000, 20000, 0, 0, 0, False, NT, False, FAST_B),
+    ("ascend_scan", 20000, 20000, 0, 0, 1, True, 0, False, FAST_EMIT_B),
+]
+
+
 @gpu
 @pytest.mark.parametrize("row", DISPATCH, ids=[_row_id(r) for r in DISPATCH])
 def test_dispatch_table(R, oracle, dispatch_ctx, row):
+    check_dispatch(R, oracle, dispatch_ctx, row, DISPATCH.index(row))
+
+
+@gpu
+@pytest.mark.parametrize("row", SIZED_SINGLE, ids=[_row_id(r) for r in SIZED_SINGLE])
+def test_dispatch_single_scan_in_a_context_of_its_size(R, oracle, row):
+    with R.Context(0, row[2], 1) as ctx:
+        check_dispatch(R, oracle, ctx, row, len(DISPATCH) + SIZED_SINGLE.index(row))
+
+
+def check_dispatch(R, oracle, ctx, row, i):
+    """One row of the dispatch table in `ctx`: its results against the oracle and the kernels that ran.  i seeds the
+    scan and picks the protocol and the inversion."""
     entry, stride, n, off, mode_a, ascend, emit, flags, dup, kernel = row
-    ctx = dispatch_ctx
-    i = DISPATCH.index(row)
     newp, inv = i & 1, (i >> 1) & 1
     scan = tie_free(oracle, n, 60000 + i)
     if dup:
@@ -628,9 +664,12 @@ SINGLE_SIZES = (3200, 8192, 16385, 32768, 40000, KEYS)
 @gpu
 def test_single_scan_at_real_sizes(R, oracle):
     """ctx.scan (with and without the ascended buffer), ctx.laserscan and ctx.ascend_scan at revolution sizes up to
-    the full key space, on the ring kernel (grid of 1) and with NO_TMA on scan_fast_kernel, in a context much larger
-    than the scan (the result comes back in three copies) and in one exactly its size (one copy; an odd size rounds
-    the context's stride up to even).  A scan with a duplicated key is re-run by the general kernel."""
+    the full key space, with and without NO_TMA, in a context much larger than the scan (the result comes back in
+    three copies) and in one exactly its size (one copy; an odd size rounds the context's stride up to even).  The
+    kernel is the one a batch at the context's stride gets: in the large context the ring kernel (grid of 1) or, with
+    NO_TMA or the ascended buffer, scan_fast_kernel; in the exact one up to 8192 nodes the shared-memory kernel, and
+    Mode B without the ascended buffer up to 32768 nodes the cluster kernel (grid of 2).  A scan with a duplicated key
+    is re-run by the general kernel."""
     scans = {n: [oracle.synth_batch(5100 + n, 1, n, 1)[0]] for n in SINGLE_SIZES}
     for n in SINGLE_SIZES:
         scans[n].append(with_duplicate(measured_everywhere(scans[n][0]), 3, n - 2))
@@ -721,8 +760,9 @@ def test_case_builders_make_what_the_gpu_tests_rely_on(oracle):
         nothing = [p for p in range(POOL) if counts[p] == stride and not measured_keys(pool[p], counts[p]).size]
         tail = [p for p in range(POOL) if counts[p] == stride and (pool[p]["dist_mm_q2"][-3 * CH:] == 0).all()]
         assert len(nothing) == 1 and len(set(tail) - set(nothing)) == 1
-    for row in DISPATCH:
+    for i, row in enumerate(DISPATCH + SIZED_SINGLE):
         entry, stride, n, off, mode_a, ascend, emit, flags, dup, kernel = row
         assert n <= stride and (entry == "dev" or off == 0)
-        scan = tie_free(oracle, n, 60000 + DISPATCH.index(row))
+        assert i < len(DISPATCH) or (entry in ("scan", "laserscan", "ascend_scan") and n == stride)
+        scan = tie_free(oracle, n, 60000 + i)
         assert has_duplicate(scan) == (n > KEYS)

@@ -41,7 +41,7 @@ def oracle_batch(O, nodes, counts, newp, mode_a, inv, ascend, stable=True):
 def check_batch(R, O, ctx, nodes, counts, newp, mode_a, inv, ascend, flags=0, stable=True, expect_path=None,
                 emit=True):
     """rpl_scan_batch on the host arrays against the oracle, bit for bit.  Which kernel serves the batch is decided
-    by rpl_capi.cu enqueue_args; tests/test_gpu_scan_bands.py states the rule (DISPATCH) and asserts it case by
+    by rpl_capi.cu pick_fast; tests/test_gpu_scan_bands.py states the rule (DISPATCH) and asserts it case by
     case: flags & 1 the general kernel alone; stride <= 8192 and not flags & 4 the shared-memory kernels
     (scan_small.cu); else the ascended buffer (emit and ascend), flags & 2 or an odd stride scan_fast.cu; else Mode B
     at strides up to 32768 the two-CTA cluster kernel and everything else the TMA ring (scan_tma.cu).  The general

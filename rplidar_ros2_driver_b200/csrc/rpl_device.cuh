@@ -175,12 +175,14 @@ __device__ __forceinline__ uint32_t warp_inclusive_scan(uint32_t v) {
 // L2 residency control.  A scan tile is read twice (mark pass, place pass): the first read
 // asks L2 to keep the lines (evict_last), the second read and all output stores mark their
 // lines evict_first so that the 1 GB/launch output stream does not push tiles out of the
-// 50 MB L2 before their second read.
-// The policies are the fixed encodings createpolicy.fractional.L2::evict_{last,first} (1.0)
+// 50 MB L2 before their second read.  The two-CTA cluster kernel reads each node once and marks
+// its loads and stores evict_normal, which it measured faster than evict_first (scan_tma.cu).
+// The policies are the fixed encodings createpolicy.fractional.L2::evict_{last,first,normal} (1.0)
 // produces (the same constants CUTLASS passes as TMA cache hints); as immediates they live in
 // uniform registers instead of being re-broadcast from a per-thread register at every access.
 __device__ __forceinline__ uint64_t l2_policy_evict_last() { return 0x14F0000000000000ull; }
 __device__ __forceinline__ uint64_t l2_policy_evict_first() { return 0x12F0000000000000ull; }
+__device__ __forceinline__ uint64_t l2_policy_evict_normal() { return 0x1000000000000000ull; }
 __device__ __forceinline__ uint4 ld_hint_v4(const void* p, uint64_t pol) {
   uint4 r;
   asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"

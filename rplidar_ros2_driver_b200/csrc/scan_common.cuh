@@ -40,20 +40,23 @@ __device__ __forceinline__ void st_f32_if(float* p, float v, uint64_t pol, uint3
 // ---- Mode B output (reference rplidar_node.cpp:661-677) ---------------------------------------------------------
 // The point of rank r among the M measured points goes to slot ob + os * r in wrapping u32 arithmetic (reference
 // :673); intensities[] sits at a fixed byte distance from ranges[].
+// The stores carry L2 policy `pol` (evict_first unless the kernel passes another).
 struct ModeBOut {
   float* ranges;
   ptrdiff_t i_minus_r;
   uint32_t ob, os;
-  __device__ __forceinline__ ModeBOut(float* r, float* i, uint32_t M, bool inverted)
+  uint64_t pol;
+  __device__ __forceinline__ ModeBOut(float* r, float* i, uint32_t M, bool inverted,
+                                      uint64_t policy = l2_policy_evict_first())
       : ranges(r),
         i_minus_r(reinterpret_cast<char*>(i) - reinterpret_cast<char*>(r)),
         ob(inverted ? M - 1u : 0u),
-        os(inverted ? 0xFFFFFFFFu : 1u) {}
+        os(inverted ? 0xFFFFFFFFu : 1u),
+        pol(policy) {}
   __device__ __forceinline__ void store(uint32_t rank, float dist_m, float intensity, uint32_t pred) const {
     float* pr = ranges + (ob + os * rank);
-    st_f32_if(pr, dist_m, l2_policy_evict_first(), pred);
-    st_f32_if(reinterpret_cast<float*>(reinterpret_cast<char*>(pr) + i_minus_r), intensity, l2_policy_evict_first(),
-              pred);
+    st_f32_if(pr, dist_m, pol, pred);
+    st_f32_if(reinterpret_cast<float*>(reinterpret_cast<char*>(pr) + i_minus_r), intensity, pol, pred);
   }
 };
 

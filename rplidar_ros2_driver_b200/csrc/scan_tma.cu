@@ -399,35 +399,60 @@ __global__ void __launch_bounds__(kBlock, 2) scan_tma_kernel(ScanBatchArgs a, ui
 // =========================== two-CTA cluster kernel (LaserScan Mode B) ===========================
 // A scan of up to 32768 nodes does not fit one SM's shared memory next to its byte map, but it fits two.
 // scan_tma_cluster_kernel stages the whole scan across a cluster of two CTAs and reads every node from
-// global memory once: chunk c (CH nodes) goes to CTA c & 1, slot c >> 1, filled by one bulk copy with an
-// evict_first hint.  Each CTA marks its own nodes in its own byte map and folds it to bit-words; the CTAs
-// swap words and measured counts through distributed shared memory, both build the same rank table, and
-// each places its own slots from shared memory.  The ring kernel's second pass over global memory (an L2
-// re-read of 8 B per node, and the 34 MB of evict_last lines it keeps live) is gone.
+// global memory once: chunk c (CH nodes) goes to CTA c & 1, slot c >> 1, filled by one bulk copy.  Each
+// CTA marks its own nodes in its own byte map and folds it to bit-words; the CTAs swap words and measured
+// counts through distributed shared memory, both build the same rank table, and each places its own
+// chunks.  The ring kernel's second pass over global memory (an L2 re-read of 8 B per node, and the 34 MB
+// of evict_last lines it keeps live) is gone.
+//
+// L2 policy: the bulk copies and the output stores are marked evict_normal.  With nothing read twice there
+// is nothing to protect, and on the H100 evict_normal on both took about 1 % off the launch, while
+// evict_first on both (as in the ring kernel) or evict_normal on the stores alone were slower (DESIGN.md §5.1).
+//
+// Held slots: shared memory is full (216.6 KB), but the register file is not.  Each consumer thread keeps
+// its kRounds nodes of the chunks in slots j < kHeld in registers (4 registers per chunk) and hands those
+// slots back to its producer as soon as they are marked, so the producer loads the next scan's first
+// chunks while this scan folds, exchanges and builds its rank table -- a stretch in which the SM would
+// otherwise have no load in flight.  The other slots are handed back in the place pass, which takes them
+// first, in ascending order, and then places the held chunks from registers.  Each filled slot still gets
+// exactly one arrive per consumer warp per scan: held slots in the mark pass, the others in the place pass
+// or, for a scan handed on or with nothing measured, right after the exchange.
 //
 // Exchange: CTA r writes its words and count into the PEER's inbox with st.async, whose bytes complete on
 // the peer's inbox_full barrier; the peer arms that barrier for the scan with one arrive.expect_tx of
 // kInboxBytes.  Its phase completes once the arrive and all the bytes are in, in either order.  The data
 // is visible to every thread that waits on the phase.  No fence and no block barrier come before the
 // signal: a first version stored plainly and signalled with a fence.acq_rel.cluster + remote arrive, and
-// that fence alone made the kernel no faster than the ring kernel.  After reading its own inbox, a CTA
-// arrives on the peer's peer_free barrier (release, cluster scope): the peer waits there before it writes
-// this inbox for the next scan, so neither barrier can run more than one phase ahead of its waiter.  Both
-// barriers complete one phase per streamed scan.
+// that fence alone made the kernel no faster than the ring kernel.  Once every consumer thread has used what
+// it read from its own inbox -- the words and count are folded into the rank table behind rank_table's
+// barriers -- thread 0 arrives on the peer's peer_free barrier: the peer waits there before it writes this
+// inbox for the next scan, so neither barrier can run more than one phase ahead of its waiter.  That arrive
+// is a release at CTA scope (mbar_arrive_remote): the reads it hands back have returned their values
+// before it issues, and the cluster-scope form put a MEMBAR.ALL.GPU in front of it that held every consumer
+// warp for about 2 us per scan.  Both barriers complete one phase per streamed scan.
 //
 // Why this cannot deadlock: only the consumer threads touch the exchange barriers, and both CTAs walk
 // the same scans in the same order and take the same branches (every decision -- invalid, empty, no
 // measured node, duplicate key -- depends on counts[s] or on the exchanged totals, identical on both
-// sides).  In scan s a CTA publishes after its own mark pass, which waits only on its own producer; the
-// producer waits only on slots its own consumers release after the place pass of scan s - 1, which in
-// turn needs the peer's publish of s - 1 and the peer's read of the inbox of s - 1 -- both done before the
-// peer could start scan s.  The producer warp never takes part in a cluster barrier while the loop runs;
+// sides).  In scan s a CTA publishes after its own mark pass, which waits only on its own producer.  To
+// fill a slot for scan s the producer waits only on its own consumers: for a held slot (j < kHeld), on
+// their mark pass of scan s - 1, which needs nothing from the peer; for any other slot, on their place
+// pass of scan s - 1 (or their early exit after its exchange), which in turn needs the peer's publish of
+// s - 1 and the peer's read of the inbox of s - 1 -- both done before the peer could start scan s.  The
+// producer fills scan by scan, so while it waits on a slot for scan s + 1 every slot of scan s is filled,
+// and the mark pass of scan s (held slots included) can finish.  The producer warp never takes part in a
+// cluster barrier while the loop runs;
 // the whole cluster, producer warps included, meets in barrier.cluster exactly twice: after the barrier
 // init (no remote arrive may reach an uninitialised barrier) and before exit (no CTA may exit while the
 // peer can still store to its inbox or arrive on its barriers).
 constexpr int kClusterSlots = 16;
 constexpr uint32_t kClusterMaxNodes = 2u * kClusterSlots * CH;  // 32768
 static_assert(kClusterMaxNodes <= kMaxFastNodes, "every scan the cluster kernel serves must be streamable");
+// Slots per CTA whose chunks are held in registers from the mark to the place pass.  Timed on an H100 SXM (4096 x
+// 32768-node Mode B launches): 0 / 4 / 6 / 8 / 10 / 12 held slots take 0.788 / 0.780 / 0.782 / 0.790 / 0.788 /
+// 0.784-0.791 ms at 64 / 80 / 88 / 95 / 96 / 96 registers per thread, no spills (DESIGN.md §5.1).
+constexpr int kHeld = 4;
+static_assert(kHeld >= 0 && kHeld <= kClusterSlots, "held slots are a prefix of the tile");
 
 struct __align__(128) ClusterSmem {
   uint8_t bytemap[kKeySpace];                // presence map of this CTA's nodes (swizzled)
@@ -458,7 +483,7 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
   if (tid == 0) {
     for (int i = 0; i < kClusterSlots; ++i) {
       mbar_init(&sm.full[i], 1);         // the producer's arrive.expect_tx
-      mbar_init(&sm.empty[i], kCWarps);  // one arrive per consumer warp (after the place pass)
+      mbar_init(&sm.empty[i], kCWarps);  // one arrive per consumer warp (after the mark or the place pass)
     }
     mbar_init(&sm.inbox_full, 1);        // this CTA's arrive.expect_tx per scan + the peer's st.async bytes
     mbar_init(&sm.peer_free, 1);         // one remote arrive by the peer per scan
@@ -470,7 +495,7 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
   if (warp == kCWarps) {
     // =========================== producer warp =========================================
     if (lane == 0) {
-      const uint64_t pol_stream = l2_policy_evict_first();
+      const uint64_t pol_load = l2_policy_evict_normal();  // (see the L2 policy note above the kernel)
       uint32_t eph = 0xFFFFFFFFu;  // empty-barrier parity per slot: the first fill passes at once
       for (uint32_t s = s0; s < a.n_scans; s += s_step) {
         const uint32_t n = a.counts[s];
@@ -486,7 +511,7 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
           const uint32_t cn = min(CH, n - c * CH);
           const uint32_t bytes = ((cn + 1u) & ~1u) * 8u;
           mbar_expect_tx(&sm.full[j], bytes);
-          tma_load_1d(&sm.tile[j][0], base + (size_t)c * CH, bytes, &sm.full[j], pol_stream);
+          tma_load_1d(&sm.tile[j][0], base + (size_t)c * CH, bytes, &sm.full[j], pol_load);
         }
       }
     }
@@ -527,17 +552,25 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
       bytemap_clear(sm.bytemap, tid);
       consumer_sync();
 
-      // ---- mark this CTA's chunks (they stay in their slots for the place pass) ------------
+      // ---- mark this CTA's chunks ---------------------------------------------------------------
+      // Slots j < kHeld are copied into registers and handed back as soon as they are marked, so the producer
+      // loads the next scan into them during this scan's fold and exchange; the other slots stay in shared
+      // memory until the place pass.
+      uint2 held[kHeld > 0 ? kHeld : 1][kRounds];
       uint32_t cnt = 0;
       uint8_t* const bmap = sm.bytemap;
-      auto mark_chunk = [&](auto checked, uint32_t j) {
-        mbar_wait(&sm.full[j], (fph >> j) & 1u);
-        fph ^= 1u << j;
-        const uint32_t c = 2u * j + rank;
+      auto fetch = [&](uint32_t j, uint2 (&v)[kRounds]) {
         const uint2* slot = sm.tile[j];
-        uint2 v[kRounds];
 #pragma unroll
         for (int r = 0; r < kRounds; ++r) v[r] = slot[r * TC + tid];
+      };
+      auto wait_and_fetch = [&](uint32_t j, uint2 (&v)[kRounds]) {
+        mbar_wait(&sm.full[j], (fph >> j) & 1u);
+        fph ^= 1u << j;
+        fetch(j, v);
+      };
+      auto mark_chunk = [&](auto checked, const uint2 (&v)[kRounds], uint32_t j) {
+        const uint32_t c = 2u * j + rank;
 #pragma unroll
         for (int r = 0; r < kRounds; ++r) {
           const uint32_t dist = __funnelshift_r(v[r].x, v[r].y, 16);
@@ -550,8 +583,27 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
       // the partial chunk (c == nfull < nch) is the last of this CTA's chunks if it is this CTA's at all
       const bool tail = nfull < nch && (nfull & 1u) == rank;
       const uint32_t mine_full = tail ? mine - 1u : mine;
-      for (uint32_t j = 0; j < mine_full; ++j) mark_chunk(Unchecked{}, j);
-      if (tail) mark_chunk(Checked{}, mine_full);
+      const uint32_t nheld = min((uint32_t)kHeld, mine);
+      // held slots first: the producer fills them first.  Only constant indices into held[] (no local memory);
+      // every held chunk takes the tail mask, which is a no-op on the full ones.
+#pragma unroll
+      for (int j = 0; j < kHeld; ++j) {
+        if (j < (int)mine) {
+          wait_and_fetch(j, held[j]);
+          mark_chunk(Checked{}, held[j], j);
+          release(j);  // after the byte-map stores whose addresses depend on the slot's values
+        }
+      }
+      for (uint32_t j = nheld; j < mine_full; ++j) {
+        uint2 v[kRounds];
+        wait_and_fetch(j, v);
+        mark_chunk(Unchecked{}, v, j);
+      }
+      if (tail && mine_full >= nheld) {
+        uint2 v[kRounds];
+        wait_and_fetch(mine_full, v);
+        mark_chunk(Checked{}, v, mine_full);
+      }
       cnt = warp_sum(cnt);
       if (lane == 0) sm.red[warp] = cnt;
       consumer_sync();
@@ -578,7 +630,7 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
         wv[2] |= pw.z;
         wv[3] |= pw.w;
         rank_table(sm, wv, tid, other);
-        // every thread has read its inbox entry (rank_table's barriers): the peer may overwrite it
+        // every thread has used its inbox entry (rank_table's barriers): the peer may overwrite it
         if (tid == 0) mbar_arrive_remote(peer_peer_free);
       }
       consumer_sync();
@@ -589,18 +641,16 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
           if (M == 0) write_outcome_empty(a, s);
           else hand_to_general(a, s);  // duplicate keys, within a half or across the halves
         }
-        for (uint32_t j = 0; j < mine; ++j) release(j);
+        for (uint32_t j = nheld; j < mine; ++j) release(j);  // the held slots went back in the mark pass
         continue;
       }
 
-      // ---- place this CTA's chunks by rank, then hand the slots back ----------------------
-      const ModeBOut mode_b(a.ranges + (size_t)s * a.stride, a.intensities + (size_t)s * a.stride, M, inverted);
-      auto place_chunk = [&](auto checked, uint32_t j) {
+      // ---- place this CTA's chunks by rank: the slots still in shared memory first, handing each back, ----
+      // ---- so that the producer's next wait (on slot kHeld) is the first one met; then the held chunks ----
+      const ModeBOut mode_b(a.ranges + (size_t)s * a.stride, a.intensities + (size_t)s * a.stride, M, inverted,
+                            l2_policy_evict_normal());
+      auto place_chunk = [&](auto checked, const uint2 (&v)[kRounds], uint32_t j) {
         const uint32_t c = 2u * j + rank;
-        const uint2* slot = sm.tile[j];
-        uint2 v[kRounds];
-#pragma unroll
-        for (int r = 0; r < kRounds; ++r) v[r] = slot[r * TC + tid];
 #pragma unroll
         for (int r = 0; r < kRounds; ++r) {
           const uint2 nd = v[r];
@@ -610,10 +660,23 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
           if (decltype(checked)::value && c * CH + r * TC + tid >= n) measured = 0;
           mode_b.store(rank_of(sm.rankV, k), dist_to_m(dist), intensity_of(nd.y), measured);
         }
-        release(j);
       };
-      for (uint32_t j = 0; j < mine_full; ++j) place_chunk(Unchecked{}, j);
-      if (tail) place_chunk(Checked{}, mine_full);
+      for (uint32_t j = nheld; j < mine_full; ++j) {
+        uint2 v[kRounds];
+        fetch(j, v);
+        place_chunk(Unchecked{}, v, j);
+        release(j);
+      }
+      if (tail && mine_full >= nheld) {
+        uint2 v[kRounds];
+        fetch(mine_full, v);
+        place_chunk(Checked{}, v, mine_full);
+        release(mine_full);
+      }
+#pragma unroll
+      for (int j = 0; j < kHeld; ++j) {
+        if (j < (int)mine) place_chunk(Checked{}, held[j], j);
+      }
       if (writer) write_outcome(a, s, kResultOk, M, angle_increment(M, false));
     }
   }

@@ -89,8 +89,13 @@ __device__ __forceinline__ void st_async_u32(uint32_t addr, uint32_t v, uint32_t
                "r"(bar)
                : "memory");
 }
+// arrive on a barrier of the peer CTA, with the default semantics (release at CTA scope), as CUTLASS's cluster
+// pipelines hand a buffer back to a peer CTA.  The caller must have consumed every value it read from the buffer the
+// arrive hands back before a block barrier that precedes the arrive: nothing here orders those reads at cluster
+// scope.  The .release.cluster form compiles to MEMBAR.ALL.GPU before the arrive, and every consumer warp of the
+// cluster kernel waited behind that fence once per scan (DESIGN.md §5.1).
 __device__ __forceinline__ void mbar_arrive_remote(uint32_t addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(addr) : "memory");
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(addr) : "memory");
 }
 // wait for a phase completed by the peer's remote arrive: acquire at cluster scope, so that the peer's
 // shared-memory accesses before its arrive are visible (or complete) here

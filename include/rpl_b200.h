@@ -33,6 +33,8 @@
  *   rpl_node_timestamps_dev  the timestamp the unpackers attach to every node (_getSampleDelayOffsetIn*Mode)
  *   rpl_assemble_scans_dev   ScanDataHolder::pushScanNodeData / rewindCurrentScanData
  *                              src/sdk/src/sl_lidar_driver.cpp:272-315
+ *   rpl_dense_stream_*       the dense unpacker and the ScanDataHolder as live, per-stream state across calls:
+ *                              wire capsules pushed in any pieces publish the scans of the whole stream
  *   rpl_*_cdr_batch_dev      the serialised form of the message scan_pub_->publish hands to the RMW layer
  *                              src/rplidar_node.cpp:679
  *   rpl_cloud_fuse_push_dev  (with rpl_peer_*) the fused cloud's all-gather across GPUs, in the pack kernel
@@ -432,6 +434,43 @@ rpl_result rpl_chain_dense_laserscan(rpl_ctx* ctx, const uint8_t* capsules, cons
                                      const rpl_scan_params* params, uint32_t max_nodes, uint32_t max_scans,
                                      float* ranges, float* intensities, uint32_t* beam_counts, float* angle_increment,
                                      uint32_t* scans_per_stream);
+
+/* Dense-capsule stream session: rpl_chain_dense_laserscan for live streams.  The chain treats every call as a whole
+ * recording (the last capsule, which the unpacker holds until the next one arrives, and the revolution still open at
+ * the end are lost); a session keeps both per stream on the device, so that for ANY split of a stream's capsules
+ * into pushes the scans published over the pushes, in order, are the scans of the whole stream (the SDK's unpacker
+ * and ScanDataHolder fed the same bytes).  A scan is published by the push that delivers the scan-start node closing
+ * it -- with the held capsule, possibly one push after its capsule.  A stream with 0 capsules in a push keeps its
+ * state and publishes nothing.  The first push of a fresh session publishes what rpl_chain_dense_laserscan does.
+ *   create:  n_streams, stride_capsules (most capsules per stream in one push), max_nodes (even, <= 8192: the holder
+ *            capacity and the output row), max_scans (slots per stream per push); the context's max_scans must cover
+ *            one stream's max_scans.  The session borrows the context (its lanes and the assembler scratch) and is
+ *            destroyed before it.  Device memory: two node arenas of n_streams * (max_nodes + 40 * stride_capsules)
+ *            nodes each (DESIGN.md 5.7), plus per-capsule reports.
+ *   push:    host buffers, synchronous, chunked over the context's two lanes; layouts are the chain's: capsules
+ *            [n_streams][stride_capsules][84], capsule_counts [n_streams] (<= stride_capsules), outputs
+ *            [n_streams * max_scans][max_nodes] / [n_streams * max_scans] (slot k of stream s = the k-th scan this push
+ *            published for s), scans_per_stream [n_streams] (> max_scans: scans were dropped).
+ *   push_dev: the same on device buffers, asynchronous on `stream` (NULL = the context's stream).  Counts above the
+ *            stride are clamped to it.
+ *   reset:   the SDK's unpacker reset + holder reset (a reconnect): drop the held capsule, the decoder's scan-start
+ *            flag and the open revolution of every stream whose stream_mask entry is non-zero (NULL = all).
+ *   state:   synchronous; open_nodes [n_streams] = nodes in each stream's open revolution (capped at max_nodes),
+ *            held_capsule [n_streams] = 1 when a valid capsule is held for the next push (either pointer nullable). */
+typedef struct rpl_dense_stream rpl_dense_stream;
+rpl_result rpl_dense_stream_create(rpl_ctx* ctx, uint32_t n_streams, uint32_t stride_capsules, uint32_t max_nodes,
+                                   uint32_t max_scans, rpl_dense_stream** out);
+void rpl_dense_stream_destroy(rpl_dense_stream* s);
+rpl_result rpl_dense_stream_push(rpl_dense_stream* s, const uint8_t* capsules, const uint32_t* capsule_counts,
+                                 uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
+                                 float* intensities, uint32_t* beam_counts, float* angle_increment,
+                                 uint32_t* scans_per_stream);
+rpl_result rpl_dense_stream_push_dev(rpl_dense_stream* s, const uint8_t* capsules, const uint32_t* capsule_counts,
+                                     uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
+                                     float* intensities, uint32_t* beam_counts, float* angle_increment,
+                                     uint32_t* scans_per_stream, void* stream);
+rpl_result rpl_dense_stream_reset(rpl_dense_stream* s, const uint8_t* stream_mask);
+rpl_result rpl_dense_stream_state(rpl_dense_stream* s, uint32_t* open_nodes, uint32_t* held_capsule);
 
 /* ---- LaserScan / PointCloud2 -> wire (SURVEY.md 8(f) rank 3) ---------------------------- */
 /* The serialised message the RMW layer would produce from the message the reference publishes

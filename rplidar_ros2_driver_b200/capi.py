@@ -47,6 +47,8 @@ EXPORTS = [
     "rpl_decode_dense_batch_dev", "rpl_decode_dense", "rpl_assemble_scans_dev", "rpl_assemble_scan_views_dev",
     "rpl_scan_views_dev", "rpl_chain_dense_laserscan", "rpl_decode_dense_batch_starts_dev",
     "rpl_assemble_scan_views_starts_dev",
+    "rpl_dense_stream_create", "rpl_dense_stream_destroy", "rpl_dense_stream_push", "rpl_dense_stream_push_dev",
+    "rpl_dense_stream_reset", "rpl_dense_stream_state",
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -188,6 +190,12 @@ def lib() -> C.CDLL:
         "rpl_chain_dense_laserscan": ([vp, vp, vp, u32, u32, u32, PSP, u32, u32, vp, vp, vp, vp, vp], u32),
         "rpl_decode_dense_batch_starts_dev": ([vp, vp, vp, u32, u32, u32, vp, vp, vp, vp, vp, vp, vp, u32, vp, vp], u32),
         "rpl_assemble_scan_views_starts_dev": ([vp, vp, vp, u32, u32, vp, vp, vp, u32, vp, u32, vp, u32, u32, vp, vp, vp, vp, vp, vp], u32),
+        "rpl_dense_stream_create": ([vp, u32, u32, u32, u32, C.POINTER(vp)], u32),
+        "rpl_dense_stream_destroy": ([vp], None),
+        "rpl_dense_stream_push": ([vp, vp, vp, u32, PSP, vp, vp, vp, vp, vp], u32),
+        "rpl_dense_stream_push_dev": ([vp, vp, vp, u32, PSP, vp, vp, vp, vp, vp, vp], u32),
+        "rpl_dense_stream_reset": ([vp, vp], u32),
+        "rpl_dense_stream_state": ([vp, vp, vp], u32),
     }
     for name, (args, res) in sig.items():
         fn = getattr(L, name)  # AttributeError here = the library does not export the ABI
@@ -538,6 +546,73 @@ class Context:
     def cloud_fuse_dev(self, xyzi, point_counts, n_scans, stride, fused, offsets, total, stream=None):
         self._check(self._L.rpl_cloud_fuse_dev(self._h, _p(xyzi), _p(point_counts), n_scans, stride, _p(fused),
                                                _p(offsets), _p(total), _p(stream)))
+
+
+class DenseStreamSession:
+    """rpl_dense_stream wrapper: dense capsules pushed in pieces, scans published as the whole stream would publish
+    them.  Borrows `ctx`; close it before the context."""
+
+    def __init__(self, ctx: Context, n_streams: int, stride_capsules: int, max_nodes: int, max_scans: int):
+        self._L, self._ctx = ctx._L, ctx
+        h = C.c_void_p()
+        ctx._check(self._L.rpl_dense_stream_create(ctx._h, n_streams, stride_capsules, max_nodes, max_scans, C.byref(h)))
+        self._h = h
+        self.n_streams, self.stride_capsules, self.max_nodes, self.max_scans = n_streams, stride_capsules, max_nodes, max_scans
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._L.rpl_dense_stream_destroy(self._h)
+            self._h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def _outputs(self, out):
+        out = dict(out or {})
+        ns = self.n_streams * self.max_scans
+        for k, shape, dt in (("ranges", (ns, self.max_nodes), np.float32), ("intensities", (ns, self.max_nodes), np.float32),
+                             ("beam_counts", (ns,), np.uint32), ("angle_increment", (ns,), np.float32),
+                             ("scans_per_stream", (self.n_streams,), np.uint32)):
+            if k not in out:
+                out[k] = np.zeros(shape, dt)
+        return out
+
+    def push(self, capsules, capsule_counts, params: ScanParams, sample_duration_us=31, out=None):
+        """Host buffers: capsules [n_streams, stride_capsules, 84] uint8 -> the dict of Context.chain_dense_laserscan
+        holding the scans this push published."""
+        assert capsules.dtype == np.uint8 and capsules.shape == (self.n_streams, self.stride_capsules, 84)
+        assert capsules.flags.c_contiguous
+        cc = np.ascontiguousarray(capsule_counts, dtype=np.uint32)
+        assert cc.shape == (self.n_streams,)
+        out = self._outputs(out)
+        self._ctx._check(self._L.rpl_dense_stream_push(
+            self._h, _p(capsules), _p(cc), sample_duration_us, C.byref(params), _p(out["ranges"]),
+            _p(out["intensities"]), _p(out["beam_counts"]), _p(out["angle_increment"]), _p(out["scans_per_stream"])))
+        return out
+
+    def push_dev(self, capsules, capsule_counts, params: ScanParams, ranges, intensities, beam_counts,
+                 angle_increment, scans_per_stream, sample_duration_us=31, stream=None):
+        """Device addresses (the layouts of push), asynchronous on `stream` (None: the context's stream)."""
+        self._ctx._check(self._L.rpl_dense_stream_push_dev(
+            self._h, _p(capsules), _p(capsule_counts), sample_duration_us, C.byref(params), _p(ranges),
+            _p(intensities), _p(beam_counts), _p(angle_increment), _p(scans_per_stream), _p(stream)))
+
+    def reset(self, mask=None):
+        """Drops the held capsule, the decoder state and the open revolution of the streams where mask is true
+        (None: every stream)."""
+        m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
+        assert m is None or m.shape == (self.n_streams,)
+        self._ctx._check(self._L.rpl_dense_stream_reset(self._h, _p(m)))
+
+    def state(self):
+        """(open_nodes, held_capsule): nodes in each stream's open revolution, 1 where a valid capsule is held."""
+        open_nodes = np.zeros(self.n_streams, np.uint32)
+        held = np.zeros(self.n_streams, np.uint32)
+        self._ctx._check(self._L.rpl_dense_stream_state(self._h, _p(open_nodes), _p(held)))
+        return open_nodes, held
 
 
 EXCHANGE_NCCL, EXCHANGE_COPY = 0, 1

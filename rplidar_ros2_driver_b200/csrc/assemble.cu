@@ -56,6 +56,9 @@ __device__ __forceinline__ void rank_sort(const uint32_t* in, uint32_t* out, uin
   }
 }
 
+// STREAM: the dense stream session's instantiation (AssembleArgs::carry_len): positions count from the first node of
+// the revolution carried in front of the new nodes, which is a scan start like any other
+template <bool STREAM>
 __global__ void __launch_bounds__(AT) assemble_kernel(AssembleArgs a) {
   __shared__ uint32_t s_list[kListCap], s_sorted[kListCap];      // scan-start positions
   __shared__ uint32_t s_rlist[kResetCap], s_rsorted[kResetCap];  // reset positions
@@ -64,13 +67,16 @@ __global__ void __launch_bounds__(AT) assemble_kernel(AssembleArgs a) {
   __shared__ int s_wmax[AT / 32];
   __shared__ int s_last_sync;       // position of the latest scan-start node seen so far (-1: none)
   __shared__ uint32_t s_published;  // scans published so far
+  __shared__ int s_open;            // STREAM: first node of the revolution left open (-1: none, or a reset emptied it)
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 
   for (uint32_t s = blockIdx.x; s < a.n_streams; s += gridDim.x) {
-    const uint32_t n = a.node_counts[s];
-    const uint2* nodes = a.nodes + (size_t)s * a.stride_nodes;
+    const uint32_t L = STREAM ? a.carry_len[s] : 0u;           // carried nodes
+    const uint32_t base = STREAM ? a.max_nodes - L : 0u;        // position 0 within the stream's region
+    const uint32_t n = a.node_counts[s] + L;
+    const uint2* nodes = a.nodes + (size_t)s * a.stride_nodes + base;
     const bool have_resets = a.capsule_status != nullptr;
-    const uint32_t ncap = have_resets ? a.capsule_counts[s] : 0u;
+    const uint32_t ncap = !have_resets ? 0u : STREAM ? min(a.capsule_counts[s], a.stride_capsules) : a.capsule_counts[s];
     const uint32_t* cst = have_resets ? a.capsule_status + (size_t)s * a.stride_capsules : nullptr;
     const uint32_t* coff = have_resets ? a.capsule_node_offset + (size_t)s * a.stride_capsules : nullptr;
     uint32_t* rs = a.reset_prefix + (size_t)s * a.stride_capsules;  // inclusive count of reset capsules
@@ -89,16 +95,20 @@ __global__ void __launch_bounds__(AT) assemble_kernel(AssembleArgs a) {
     for (uint32_t j = tid; j < ncap; j += AT) {
       if (cst[j] & kStSync) {
         const uint32_t idx = atomicAdd(&s_rcnt, 1u);
-        if (idx < kResetCap) s_rlist[idx] = coff[j];
+        if (idx < kResetCap) s_rlist[idx] = coff[j] + L;
       }
     }
     // the decoder may have handed the scan-start positions over (rpl_decode_dense_batch_starts_dev): then the node
     // stream is not read again at all
     const uint32_t n_listed = (a.scan_starts && a.scan_start_counts) ? a.scan_start_counts[s] : 0xFFFFFFFFu;
-    if (n_listed <= a.starts_stride && n_listed <= kListCap) {
+    const uint32_t lead = (STREAM && L > 0) ? 1u : 0u;  // the carried revolution's scan start, at 0
+    if (n_listed <= a.starts_stride && n_listed + lead <= kListCap) {
       const uint32_t* lst = a.scan_starts + (size_t)s * a.starts_stride;
-      for (uint32_t e = tid; e < n_listed; e += AT) s_list[e] = lst[e];
-      if (tid == 0) s_cnt = n_listed;
+      for (uint32_t e = tid; e < n_listed; e += AT) s_list[e + lead] = lst[e] + L;
+      if (tid == 0) {
+        if (lead) s_list[0] = 0;
+        s_cnt = n_listed + lead;
+      }
     } else {
       const uint32_t* flags = reinterpret_cast<const uint32_t*>(nodes) + 1;  // word 1 of every node
       uint32_t i = tid;
@@ -157,6 +167,8 @@ __global__ void __launch_bounds__(AT) assemble_kernel(AssembleArgs a) {
         if (tid == 0) s_published += tot;
         __syncthreads();
       }
+      // the revolution after the last scan start stays open unless a reset follows its start
+      if (STREAM && tid == 0) s_open = (K > 0 && resets_upto(s_sorted[K - 1]) == RK) ? (int)s_sorted[K - 1] : -1;
     } else {
       // ---- many scan starts: chunked block scans over the flags ---------------------------------------
       uint32_t carry = 0;
@@ -174,7 +186,7 @@ __global__ void __launch_bounds__(AT) assemble_kernel(AssembleArgs a) {
         uint32_t lo = 0, hi = ncap;  // first capsule with offset > x
         while (lo < hi) {
           const uint32_t mid = (lo + hi) >> 1;
-          if (coff[mid] <= x) lo = mid + 1;
+          if (coff[mid] + L <= x) lo = mid + 1;
           else hi = mid;
         }
         return lo ? rs[lo - 1] : 0u;
@@ -213,6 +225,10 @@ __global__ void __launch_bounds__(AT) assemble_kernel(AssembleArgs a) {
         }
         __syncthreads();
       }
+      if (STREAM && tid == 0) {
+        const int ls = s_last_sync;
+        s_open = (ls >= 0 && resets_upto((uint32_t)ls) == carry) ? ls : -1;
+      }
     }
     __syncthreads();
     const uint32_t total = s_published;
@@ -229,14 +245,28 @@ __global__ void __launch_bounds__(AT) assemble_kernel(AssembleArgs a) {
         if (k < stored) {
           const uint2 d = desc[k];
           const uint32_t cnt = min(d.y, a.max_nodes);
-          if (d.y > cnt) a.nodes_mut[(size_t)s * a.stride_nodes + d.x + cnt - 1] = nodes[d.x + d.y - 1];
-          v = make_uint2((uint32_t)((size_t)s * a.stride_nodes + d.x), cnt);
+          if (d.y > cnt) a.nodes_mut[(size_t)s * a.stride_nodes + base + d.x + cnt - 1] = nodes[d.x + d.y - 1];
+          v = make_uint2((uint32_t)((size_t)s * a.stride_nodes + base + d.x), cnt);
           if (a.scan_begin_ts_us)
             a.scan_begin_ts_us[(size_t)s * a.max_scans + k] =
-                a.node_ts_us ? a.node_ts_us[(size_t)s * a.stride_nodes + d.x] : 0ull;
+                a.node_ts_us ? a.node_ts_us[(size_t)s * a.stride_nodes + base + d.x] : 0ull;
         }
         vout[k] = v;
         out_len[k] = v.y;
+      }
+      if constexpr (STREAM) {
+        // the open revolution, capped by the holder's rule, right-aligned into the other arena's carry slots (none of
+        // its nodes is a published scan's, so the in-place cap above never touches them)
+        const int ls = s_open;
+        const uint32_t t = ls >= 0 ? n - (uint32_t)ls : 0u, tc = min(t, a.max_nodes);
+        const uint2* src = nodes + (ls >= 0 ? ls : 0);
+        uint2* dst = a.carry_out + (size_t)s * a.stride_nodes + a.max_nodes - tc;
+        const uint32_t ncopy = t > tc ? tc - 1 : tc;
+        for (uint32_t q = tid; q < ncopy; q += AT) dst[q] = src[q];
+        if (tid == 0) {
+          if (t > tc) dst[tc - 1] = src[t - 1];
+          a.carry_len_out[s] = tc;
+        }
       }
       __syncthreads();
       continue;
@@ -277,7 +307,10 @@ __global__ void __launch_bounds__(AT) assemble_kernel(AssembleArgs a) {
 
 cudaError_t launch_assemble(const AssembleArgs& a, int grid, cudaStream_t stream) {
   if (a.n_streams == 0) return cudaSuccess;
-  assemble_kernel<<<grid, AT, 0, stream>>>(a);
+  if (a.carry_len)
+    assemble_kernel<true><<<grid, AT, 0, stream>>>(a);
+  else
+    assemble_kernel<false><<<grid, AT, 0, stream>>>(a);
   return cudaGetLastError();
 }
 

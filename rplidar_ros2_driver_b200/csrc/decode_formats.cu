@@ -45,7 +45,8 @@ constexpr uint32_t kStOk = 1, kStSync = 2, kStEmit = 4, kStDiscard = 8, kStCheck
                    kStBadFrame = 64;
 constexpr int kFull = 360 << 16;
 
-enum { kExpress = 0, kUltra = 1, kUltraDense = 2, kDense = 3 };
+// kDenseStream: the dense decoder of a stream session (CapsuleDecodeArgs::held)
+enum { kExpress = 0, kUltra = 1, kUltraDense = 2, kDense = 3, kDenseStream = 4 };
 
 // CB bytes and NODES nodes per capsule, the start angle at byte START, BUFFERS tile buffers of DT capsules (= threads).
 // JUMP_CABINS: the cabin count in the reference's angular-jump discard threshold (0: no threshold).  SYNC_CHAIN: the
@@ -68,6 +69,8 @@ struct Fmt<kDense> {
   static constexpr int CB = 84, NODES = 40, START = 2, BUFFERS = 2, DT = 256, JUMP_CABINS = 40;
   static constexpr bool SYNC_CHAIN = true, SMOOTH_CHAIN = false;
 };
+template <>
+struct Fmt<kDenseStream> : Fmt<kDense> {};
 template <>
 struct Fmt<kUltraDense> {
   // one tile buffer: with the smoothing tables a second one would leave a single CTA (8 warps) per SM
@@ -283,13 +286,14 @@ struct CapsuleSmem {
   int ultra_off[F == kUltra ? 496 : 1];
   uint2 wstage[F == kUltra ? DT / 32 : 1][F == kUltra ? 96 : 1];
   // dense only: angular step per sample of the nodes each capsule releases
-  int inc_q16[F == kDense ? DT : 1];
+  int inc_q16[(F == kDense || F == kDenseStream) ? DT : 1];
 };
 
 template <int F>
 __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecodeArgs a) {
   using T = Fmt<F>;
   constexpr int CB = T::CB, NODES = T::NODES, DT = T::DT;
+  constexpr bool DENSE = F == kDense || F == kDenseStream, STREAM = F == kDenseStream;
   extern __shared__ __align__(16) unsigned char capsule_smem_raw[];
   CapsuleSmem<F>& sm = *reinterpret_cast<CapsuleSmem<F>*>(capsule_smem_raw);
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -301,9 +305,10 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
   }
 
   for (uint32_t s = blockIdx.x; s < a.n_streams; s += gridDim.x) {
-    const uint32_t n = a.counts[s];
+    const uint32_t n = STREAM ? min(a.counts[s], a.stride_capsules) : a.counts[s];
     const uint8_t* src = a.capsules + (size_t)s * a.stride_capsules * CB;
-    uint2* out = a.nodes_out + (size_t)s * a.stride_capsules * NODES;
+    uint2* out = STREAM ? a.nodes_out + (size_t)s * a.node_stride + a.node_first
+                        : a.nodes_out + (size_t)s * a.stride_capsules * NODES;
     uint32_t* st_out = a.capsule_status ? a.capsule_status + (size_t)s * a.stride_capsules : nullptr;
     uint32_t* off_out = a.capsule_node_offset ? a.capsule_node_offset + (size_t)s * a.stride_capsules : nullptr;
     uint32_t* starts = a.scan_starts ? a.scan_starts + (size_t)s * a.starts_stride : nullptr;
@@ -313,9 +318,19 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
       sm.okflag[0] = 0;
       sm.start_q8[0] = 0;
       if constexpr (T::SYNC_CHAIN) sm.carry_sync = state_in ? (state_in[0] & 1u) : 0u;
-      if constexpr (F == kDense) sm.n_starts = 0;
+      if constexpr (DENSE) sm.n_starts = 0;
       if constexpr (T::SMOOTH_CHAIN) sm.carry_last = (state_in && a.state_words == 2) ? state_in[1] : 0u;
+      if constexpr (STREAM) {
+        const uint32_t* held = a.held + (size_t)s * kHeldWords;
+        sm.okflag[0] = held[kHeldOk];
+        sm.start_q8[0] = held[kHeldStart];
+        sm.carry_sync = held[kHeldSync];
+      }
     }
+    // the held capsule takes the place of a previous tile's last capsule: the first capsule releases it if both hold
+    if constexpr (STREAM)
+      for (uint32_t w = tid; w < (uint32_t)CB / 4; w += DT)
+        reinterpret_cast<uint32_t*>(sm.carry)[w] = a.held[(size_t)s * kHeldWords + w];
     __syncthreads();
 
     // stage a tile into buffer `b`: asynchronous 16-byte copies, 4-byte ones where the stream is only 4-byte aligned
@@ -411,7 +426,7 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
         if (emit) {
           const int inc_q16 = (diff << 8) / NODES;
           raw = raw_sync_mask<NODES>(prev_q8, inc_q16);
-          if constexpr (F == kDense) sm.inc_q16[tid] = inc_q16;  // the emission's step, once per capsule
+          if constexpr (DENSE) sm.inc_q16[tid] = inc_q16;  // the emission's step, once per capsule
           const uint32_t o0 = (uint32_t)(resolve_sync(raw, 0) >> (NODES - 1)) & 1u;
           const uint32_t o1 = (uint32_t)(resolve_sync(raw, 1) >> (NODES - 1)) & 1u;
           f = o0 | (o1 << 1);
@@ -448,7 +463,7 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
         // this capsule's scan-start nodes (a few per revolution), for the assembler.  Only the dense entry points
         // offer the list: compiled into ultra-dense, the loop alone takes that kernel from 40 to 32 registers and
         // makes it slower
-        if (F == kDense && starts) {
+        if (DENSE && starts) {
           for (; smask; smask &= smask - 1) {
             const uint32_t idx = atomicAdd(&sm.n_starts, 1u);
             if (idx < a.starts_stride) starts[idx] = node_off + (uint32_t)(__ffsll((long long)smask) - 1);
@@ -654,8 +669,18 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
         state_out[0] = T::SYNC_CHAIN ? sm.carry_sync : 0u;
         if (a.state_words == 2) state_out[1] = T::SMOOTH_CHAIN ? sm.carry_last : 0u;
       }
-      if (F == kDense && a.scan_start_counts) a.scan_start_counts[s] = sm.n_starts;
+      if (DENSE && a.scan_start_counts) a.scan_start_counts[s] = sm.n_starts;
+      if constexpr (STREAM) {
+        uint32_t* held = a.held + (size_t)s * kHeldWords;
+        held[kHeldOk] = sm.okflag[0];
+        held[kHeldStart] = sm.start_q8[0];
+        held[kHeldSync] = sm.carry_sync;
+      }
     }
+    // the last capsule is held for the next push (a stream without capsules writes back what it read)
+    if constexpr (STREAM)
+      for (uint32_t w = tid; w < (uint32_t)CB / 4; w += DT)
+        a.held[(size_t)s * kHeldWords + w] = reinterpret_cast<const uint32_t*>(sm.carry)[w];
     __syncthreads();
   }
 }
@@ -1014,7 +1039,7 @@ cudaError_t launch_decode_capsules(uint32_t ans_type, const CapsuleDecodeArgs& a
   switch (ans_type) {
     case 0x82: return launch_fmt<kExpress>(a, grid, stream);
     case 0x84: return launch_fmt<kUltra>(a, grid, stream);
-    case 0x85: return launch_fmt<kDense>(a, grid, stream);
+    case 0x85: return a.held ? launch_fmt<kDenseStream>(a, grid, stream) : launch_fmt<kDense>(a, grid, stream);
     case 0x86: return launch_fmt<kUltraDense>(a, grid, stream);
     case 0x83:
       decode_hq_kernel<<<grid, HT, sizeof(HqSmem), stream>>>(a);
@@ -1069,6 +1094,9 @@ cudaError_t decode_formats_configure() {
   if (e != cudaSuccess) return e;
   e = cudaFuncSetAttribute(decode_capsule_kernel<kDense>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)sizeof(CapsuleSmem<kDense>));
+  if (e != cudaSuccess) return e;
+  e = cudaFuncSetAttribute(decode_capsule_kernel<kDenseStream>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)sizeof(CapsuleSmem<kDenseStream>));
   if (e != cudaSuccess) return e;
   e = cudaFuncSetAttribute(decode_capsule_kernel<kUltraDense>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                            (int)sizeof(CapsuleSmem<kUltraDense>));

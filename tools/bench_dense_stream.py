@@ -1,0 +1,142 @@
+"""Dense stream session (rpl_dense_stream_*) timings on the GPU; prints one JSON line.
+
+  * per-push latency of push (host buffers, synchronous) and push_dev (device buffers, CUDA events on a torch stream)
+    for 512 streams x {8, 80, 800} capsules per push: a live aggregator's receive periods of ~2.5 ms, ~25 ms, ~250 ms
+    at 10 Hz, 80 capsules per revolution;
+  * device-resident throughput of push_dev on the shape of bench.py --workload chain (512 streams x 4096 capsules,
+    max_nodes 4096, max_scans 56), in nodes decoded per second: the figure to set next to that workload's.
+
+Each push continues the stream where the previous one ended (the capsules of a push follow on in angle), so the carry
+and the held capsule are exercised as in a live feed.  The GPU's name and power limit are part of the output.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+from bench import wire_dense_capsules  # noqa: E402
+
+
+def feed(n_streams, n_caps, seed=1):
+    """[n_streams, n_caps, 84]: 80 capsules per revolution, 5 % zero distances, every stream at its own angle"""
+    rng = np.random.default_rng(seed)
+    out = np.empty((n_streams, n_caps, 84), np.uint8)
+    for s in range(n_streams):
+        ang = (rng.uniform(0, 360) + np.arange(n_caps) * 4.5 + rng.normal(0, 0.03, n_caps)) % 360.0
+        q6 = np.round(ang * 64).astype(np.uint32) % (360 * 64)
+        dist = rng.integers(1, 40000, (n_caps, 40))
+        dist[rng.random((n_caps, 40)) < 0.05] = 0
+        out[s] = wire_dense_capsules(q6, np.zeros(n_caps, bool), dist)
+    return out
+
+
+def gpu_info():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True)
+    return q.stdout.strip().splitlines()[0] if q.returncode == 0 else "unknown"
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--pushes", type=int, default=40, help="timed pushes per latency point")
+    ap.add_argument("--steps", type=int, default=20, help="timed pushes of the throughput point")
+    args = ap.parse_args()
+    import torch
+
+    import rplidar_ros2_driver_b200 as R
+
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    params = R.scan_params(1, 0, 0, 1)
+    res = {"gpu": gpu_info(), "latency": [], "throughput": None}
+    n_streams, max_nodes, max_scans = 512, 4096, 16
+    ctx = R.Context(0, max_nodes, n_streams * max_scans)
+    for per in (8, 80, 800):
+        caps = feed(16, per * (args.pushes + 4), seed=per)  # 16 distinct streams, tiled over the 512
+        rep = n_streams // 16
+        counts = np.full(n_streams, per, np.uint32)
+        row = {"streams": n_streams, "capsules_per_push": per}
+        # host buffers: wall clock around the synchronous call (pinned buffers, as an aggregator would keep them)
+        with R.DenseStreamSession(ctx, n_streams, per, max_nodes, max_scans) as sess:
+            pin = torch.empty((n_streams, per, 84), dtype=torch.uint8).pin_memory().numpy()
+            out = {k: torch.zeros(shape, dtype=dt).pin_memory().numpy() for k, shape, dt in (
+                ("ranges", (n_streams * max_scans, max_nodes), torch.float32),
+                ("intensities", (n_streams * max_scans, max_nodes), torch.float32),
+                ("beam_counts", (n_streams * max_scans,), torch.int32), ("angle_increment", (n_streams * max_scans,), torch.float32),
+                ("scans_per_stream", (n_streams,), torch.int32))}
+            out["beam_counts"] = out["beam_counts"].view(np.uint32)
+            out["scans_per_stream"] = out["scans_per_stream"].view(np.uint32)
+            ts = []
+            for t in range(args.pushes + 4):
+                pin[:] = np.tile(caps[:, t * per:(t + 1) * per], (rep, 1, 1))
+                t0 = time.perf_counter()
+                sess.push(pin, counts, params, out=out)
+                ts.append(time.perf_counter() - t0)
+            ts = np.array(ts[4:]) * 1e3
+            row["push_ms_median"], row["push_ms_p90"] = float(np.median(ts)), float(np.percentile(ts, 90))
+        # device buffers: CUDA events around push_dev on a torch stream
+        with R.DenseStreamSession(ctx, n_streams, per, max_nodes, max_scans) as sess, torch.cuda.stream(stream):
+            d_caps = torch.from_numpy(caps).to(dev)
+            d_cnt = torch.full((n_streams,), per, dtype=torch.int32, device=dev)
+            NS = n_streams * max_scans
+            r = torch.empty((NS, max_nodes), device=dev)
+            it = torch.empty((NS, max_nodes), device=dev)
+            bc = torch.zeros(NS, dtype=torch.int32, device=dev)
+            inc = torch.zeros(NS, device=dev)
+            sps = torch.zeros(n_streams, dtype=torch.int32, device=dev)
+            evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.pushes + 4)]
+            for t in range(args.pushes + 4):
+                piece = d_caps[:, t * per:(t + 1) * per].repeat(rep, 1, 1)
+                evs[t][0].record(stream)
+                sess.push_dev(piece.data_ptr(), d_cnt.data_ptr(), params, r.data_ptr(), it.data_ptr(), bc.data_ptr(),
+                              inc.data_ptr(), sps.data_ptr(), stream=stream.cuda_stream)
+                evs[t][1].record(stream)
+            stream.synchronize()
+            ms = np.array([a.elapsed_time(b) for a, b in evs[4:]])
+            row["push_dev_ms_median"], row["push_dev_ms_p90"] = float(np.median(ms)), float(np.percentile(ms, 90))
+        res["latency"].append(row)
+    ctx.close()
+    # throughput on the chain workload's shape
+    n_caps, max_scans = 4096, 56
+    ctx = R.Context(0, max_nodes, n_streams * max_scans)
+    caps = feed(16, n_caps * 2, seed=7)
+    with R.DenseStreamSession(ctx, n_streams, n_caps, max_nodes, max_scans) as sess, torch.cuda.stream(stream):
+        halves = [torch.from_numpy(np.tile(caps[:, h * n_caps:(h + 1) * n_caps], (n_streams // 16, 1, 1))).to(dev)
+                  for h in (0, 1)]
+        d_cnt = torch.full((n_streams,), n_caps, dtype=torch.int32, device=dev)
+        NS = n_streams * max_scans
+        r = torch.empty((NS, max_nodes), device=dev)
+        it = torch.empty((NS, max_nodes), device=dev)
+        bc = torch.zeros(NS, dtype=torch.int32, device=dev)
+        inc = torch.zeros(NS, device=dev)
+        sps = torch.zeros(n_streams, dtype=torch.int32, device=dev)
+
+        def push(t):
+            sess.push_dev(halves[t % 2].data_ptr(), d_cnt.data_ptr(), params, r.data_ptr(), it.data_ptr(),
+                          bc.data_ptr(), inc.data_ptr(), sps.data_ptr(), stream=stream.cuda_stream)
+
+        for t in range(4):
+            push(t)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        for t in range(args.steps):
+            push(t)
+        e1.record(stream)
+        stream.synchronize()
+        ms = e0.elapsed_time(e1) / args.steps
+        scans = int(sps.cpu().sum())
+    res["throughput"] = {"streams": n_streams, "capsules_per_push": n_caps, "ms_per_push": ms,
+                         "gnodes_per_s": n_streams * n_caps * 40 / (ms * 1e-3) / 1e9, "scans_per_push": scans}
+    ctx.close()
+    print(json.dumps(res))
+
+
+if __name__ == "__main__":
+    main()

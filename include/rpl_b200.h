@@ -33,8 +33,9 @@
  *   rpl_node_timestamps_dev  the timestamp the unpackers attach to every node (_getSampleDelayOffsetIn*Mode)
  *   rpl_assemble_scans_dev   ScanDataHolder::pushScanNodeData / rewindCurrentScanData
  *                              src/sdk/src/sl_lidar_driver.cpp:272-315
- *   rpl_dense_stream_*       the dense unpacker and the ScanDataHolder as live, per-stream state across calls:
- *                              wire capsules pushed in any pieces publish the scans of the whole stream
+ *   rpl_capsule_stream_*     the capsule unpackers (express, HQ, ultra, dense, ultra-dense) and the ScanDataHolder
+ *                              as live, per-stream state across calls: wire capsules pushed in any pieces publish the
+ *                              scans of the whole stream (rpl_dense_stream_*: the same, fixed to dense capsules)
  *   rpl_*_cdr_batch_dev      the serialised form of the message scan_pub_->publish hands to the RMW layer
  *                              src/rplidar_node.cpp:679
  *   rpl_cloud_fuse_push_dev  (with rpl_peer_*) the fused cloud's all-gather across GPUs, in the pack kernel
@@ -435,28 +436,53 @@ rpl_result rpl_chain_dense_laserscan(rpl_ctx* ctx, const uint8_t* capsules, cons
                                      float* ranges, float* intensities, uint32_t* beam_counts, float* angle_increment,
                                      uint32_t* scans_per_stream);
 
-/* Dense-capsule stream session: rpl_chain_dense_laserscan for live streams.  The chain treats every call as a whole
- * recording (the last capsule, which the unpacker holds until the next one arrives, and the revolution still open at
- * the end are lost); a session keeps both per stream on the device, so that for ANY split of a stream's capsules
- * into pushes the scans published over the pushes, in order, are the scans of the whole stream (the SDK's unpacker
- * and ScanDataHolder fed the same bytes).  A scan is published by the push that delivers the scan-start node closing
- * it -- with the held capsule, possibly one push after its capsule.  A stream with 0 capsules in a push keeps its
- * state and publishes nothing.  The first push of a fresh session publishes what rpl_chain_dense_laserscan does.
- *   create:  n_streams, stride_capsules (most capsules per stream in one push), max_nodes (even, <= 8192: the holder
- *            capacity and the output row), max_scans (slots per stream per push); the context's max_scans must cover
- *            one stream's max_scans.  The session borrows the context (its lanes and the assembler scratch) and is
- *            destroyed before it.  Device memory: two node arenas of n_streams * (max_nodes + 40 * stride_capsules)
- *            nodes each (DESIGN.md 5.7), plus per-capsule reports.
- *   push:    host buffers, synchronous, chunked over the context's two lanes; layouts are the chain's: capsules
- *            [n_streams][stride_capsules][84], capsule_counts [n_streams] (<= stride_capsules), outputs
- *            [n_streams * max_scans][max_nodes] / [n_streams * max_scans] (slot k of stream s = the k-th scan this push
- *            published for s), scans_per_stream [n_streams] (> max_scans: scans were dropped).
+/* Capsule stream session: decode -> assemble -> LaserScan for live streams of one capsule answer type.  The stateless
+ * calls (rpl_chain_dense_laserscan; rpl_decode_capsules_batch_dev -> rpl_assemble_scan_views_dev -> rpl_scan_views_dev)
+ * treat every call as a whole recording: the last capsule, which the express, ultra, dense and ultra-dense unpackers
+ * hold until the next one arrives, and the revolution still open at the end are lost.  A session keeps both per stream
+ * on the device, so that for ANY split of a stream's capsules into pushes the scans published over the pushes, in
+ * order, are the scans of the whole stream (the SDK's unpacker and ScanDataHolder fed the same bytes).  A scan is
+ * published by the push that delivers the scan-start node closing it -- with the held capsule, possibly one push after
+ * its capsule.  A stream with 0 capsules in a push keeps its state and publishes nothing.  The first push of a fresh
+ * session publishes what the stateless device path does on the same capsules.
+ *   create:  ans_type 0x82 express, 0x83 HQ, 0x84 ultra, 0x85 dense or 0x86 ultra-dense (0x81 and anything else:
+ *            RPL_RESULT_INVALID_DATA); n_streams, stride_capsules (most capsules per stream in one push), max_nodes
+ *            (even, <= 8192: the holder capacity and the output row), max_scans (slots per stream per push); the
+ *            context's max_scans must cover one stream's max_scans.  The session borrows the context (its lanes and the
+ *            assembler scratch) and is destroyed before it.  Device memory: two node arenas of
+ *            n_streams * (max_nodes + rpl_capsule_nodes(ans_type) * stride_capsules) nodes each (DESIGN.md 5.7), which
+ *            must stay below 2^32 nodes, plus per-capsule reports.
+ *   push:    host buffers, synchronous, chunked (about 16 MiB of capsules) over the context's two lanes: capsules
+ *            [n_streams][stride_capsules][rpl_capsule_bytes(ans_type)], capsule_counts [n_streams] (<= stride_capsules),
+ *            outputs [n_streams * max_scans][max_nodes] / [n_streams * max_scans] (slot k of stream s = the k-th scan
+ *            this push published for s), scans_per_stream [n_streams] (> max_scans: scans were dropped).  Dense capsule
+ *            buffers must be 4-byte aligned, as for rpl_decode_capsules_batch_dev.
  *   push_dev: the same on device buffers, asynchronous on `stream` (NULL = the context's stream).  Counts above the
  *            stride are clamped to it.
  *   reset:   the SDK's unpacker reset + holder reset (a reconnect): drop the held capsule, the decoder's scan-start
- *            flag and the open revolution of every stream whose stream_mask entry is non-zero (NULL = all).
+ *            flag and smoothed last distance, and the open revolution of every stream whose stream_mask entry is
+ *            non-zero (NULL = all).
  *   state:   synchronous; open_nodes [n_streams] = nodes in each stream's open revolution (capped at max_nodes),
- *            held_capsule [n_streams] = 1 when a valid capsule is held for the next push (either pointer nullable). */
+ *            held_capsule [n_streams] = 1 when a valid capsule is held for the next push (always 0 for HQ, which holds
+ *            nothing); either pointer nullable. */
+typedef struct rpl_capsule_stream rpl_capsule_stream;
+rpl_result rpl_capsule_stream_create(rpl_ctx* ctx, uint32_t ans_type, uint32_t n_streams, uint32_t stride_capsules,
+                                     uint32_t max_nodes, uint32_t max_scans, rpl_capsule_stream** out);
+void rpl_capsule_stream_destroy(rpl_capsule_stream* s);
+rpl_result rpl_capsule_stream_push(rpl_capsule_stream* s, const uint8_t* capsules, const uint32_t* capsule_counts,
+                                   uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
+                                   float* intensities, uint32_t* beam_counts, float* angle_increment,
+                                   uint32_t* scans_per_stream);
+rpl_result rpl_capsule_stream_push_dev(rpl_capsule_stream* s, const uint8_t* capsules, const uint32_t* capsule_counts,
+                                       uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
+                                       float* intensities, uint32_t* beam_counts, float* angle_increment,
+                                       uint32_t* scans_per_stream, void* stream);
+rpl_result rpl_capsule_stream_reset(rpl_capsule_stream* s, const uint8_t* stream_mask);
+rpl_result rpl_capsule_stream_state(rpl_capsule_stream* s, uint32_t* open_nodes, uint32_t* held_capsule);
+
+/* Dense-capsule stream session: rpl_capsule_stream_* fixed to 0x85 (capsules [n_streams][stride_capsules][84], arenas
+ * of n_streams * (max_nodes + 40 * stride_capsules) nodes); the first push of a fresh session publishes what
+ * rpl_chain_dense_laserscan does. */
 typedef struct rpl_dense_stream rpl_dense_stream;
 rpl_result rpl_dense_stream_create(rpl_ctx* ctx, uint32_t n_streams, uint32_t stride_capsules, uint32_t max_nodes,
                                    uint32_t max_scans, rpl_dense_stream** out);

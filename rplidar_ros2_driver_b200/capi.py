@@ -49,6 +49,8 @@ EXPORTS = [
     "rpl_assemble_scan_views_starts_dev",
     "rpl_dense_stream_create", "rpl_dense_stream_destroy", "rpl_dense_stream_push", "rpl_dense_stream_push_dev",
     "rpl_dense_stream_reset", "rpl_dense_stream_state",
+    "rpl_capsule_stream_create", "rpl_capsule_stream_destroy", "rpl_capsule_stream_push", "rpl_capsule_stream_push_dev",
+    "rpl_capsule_stream_reset", "rpl_capsule_stream_state",
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -196,6 +198,12 @@ def lib() -> C.CDLL:
         "rpl_dense_stream_push_dev": ([vp, vp, vp, u32, PSP, vp, vp, vp, vp, vp, vp], u32),
         "rpl_dense_stream_reset": ([vp, vp], u32),
         "rpl_dense_stream_state": ([vp, vp, vp], u32),
+        "rpl_capsule_stream_create": ([vp, u32, u32, u32, u32, u32, C.POINTER(vp)], u32),
+        "rpl_capsule_stream_destroy": ([vp], None),
+        "rpl_capsule_stream_push": ([vp, vp, vp, u32, PSP, vp, vp, vp, vp, vp], u32),
+        "rpl_capsule_stream_push_dev": ([vp, vp, vp, u32, PSP, vp, vp, vp, vp, vp, vp], u32),
+        "rpl_capsule_stream_reset": ([vp, vp], u32),
+        "rpl_capsule_stream_state": ([vp, vp, vp], u32),
     }
     for name, (args, res) in sig.items():
         fn = getattr(L, name)  # AttributeError here = the library does not export the ABI
@@ -548,20 +556,32 @@ class Context:
                                                _p(offsets), _p(total), _p(stream)))
 
 
-class DenseStreamSession:
-    """rpl_dense_stream wrapper: dense capsules pushed in pieces, scans published as the whole stream would publish
-    them.  Borrows `ctx`; close it before the context."""
+class CapsuleStreamSession:
+    """rpl_capsule_stream wrapper: capsules of one answer type (0x82 express, 0x83 HQ, 0x84 ultra, 0x85 dense, 0x86
+    ultra-dense) pushed in pieces, scans published as the whole stream would publish them.  Borrows `ctx`; close it
+    before the context."""
 
-    def __init__(self, ctx: Context, n_streams: int, stride_capsules: int, max_nodes: int, max_scans: int):
+    _sym = "rpl_capsule_stream"
+
+    def __init__(self, ctx: Context, ans_type: int, n_streams: int, stride_capsules: int, max_nodes: int, max_scans: int):
+        self._init(ctx, ans_type, n_streams, stride_capsules, max_nodes, max_scans,
+                   lambda h: ctx._L.rpl_capsule_stream_create(ctx._h, ans_type, n_streams, stride_capsules, max_nodes,
+                                                               max_scans, C.byref(h)))
+
+    def _init(self, ctx, ans_type, n_streams, stride_capsules, max_nodes, max_scans, create):
         self._L, self._ctx = ctx._L, ctx
         h = C.c_void_p()
-        ctx._check(self._L.rpl_dense_stream_create(ctx._h, n_streams, stride_capsules, max_nodes, max_scans, C.byref(h)))
+        ctx._check(create(h))
         self._h = h
+        self.ans_type, self.capsule_bytes = ans_type, int(self._L.rpl_capsule_bytes(ans_type))
         self.n_streams, self.stride_capsules, self.max_nodes, self.max_scans = n_streams, stride_capsules, max_nodes, max_scans
+
+    def _fn(self, name):
+        return getattr(self._L, f"{self._sym}_{name}")
 
     def close(self):
         if getattr(self, "_h", None):
-            self._L.rpl_dense_stream_destroy(self._h)
+            self._fn("destroy")(self._h)
             self._h = None
 
     def __enter__(self):
@@ -581,14 +601,14 @@ class DenseStreamSession:
         return out
 
     def push(self, capsules, capsule_counts, params: ScanParams, sample_duration_us=31, out=None):
-        """Host buffers: capsules [n_streams, stride_capsules, 84] uint8 -> the dict of Context.chain_dense_laserscan
-        holding the scans this push published."""
-        assert capsules.dtype == np.uint8 and capsules.shape == (self.n_streams, self.stride_capsules, 84)
+        """Host buffers: capsules [n_streams, stride_capsules, capsule_bytes] uint8 -> the dict of
+        Context.chain_dense_laserscan holding the scans this push published."""
+        assert capsules.dtype == np.uint8 and capsules.shape == (self.n_streams, self.stride_capsules, self.capsule_bytes)
         assert capsules.flags.c_contiguous
         cc = np.ascontiguousarray(capsule_counts, dtype=np.uint32)
         assert cc.shape == (self.n_streams,)
         out = self._outputs(out)
-        self._ctx._check(self._L.rpl_dense_stream_push(
+        self._ctx._check(self._fn("push")(
             self._h, _p(capsules), _p(cc), sample_duration_us, C.byref(params), _p(out["ranges"]),
             _p(out["intensities"]), _p(out["beam_counts"]), _p(out["angle_increment"]), _p(out["scans_per_stream"])))
         return out
@@ -596,7 +616,7 @@ class DenseStreamSession:
     def push_dev(self, capsules, capsule_counts, params: ScanParams, ranges, intensities, beam_counts,
                  angle_increment, scans_per_stream, sample_duration_us=31, stream=None):
         """Device addresses (the layouts of push), asynchronous on `stream` (None: the context's stream)."""
-        self._ctx._check(self._L.rpl_dense_stream_push_dev(
+        self._ctx._check(self._fn("push_dev")(
             self._h, _p(capsules), _p(capsule_counts), sample_duration_us, C.byref(params), _p(ranges),
             _p(intensities), _p(beam_counts), _p(angle_increment), _p(scans_per_stream), _p(stream)))
 
@@ -605,14 +625,25 @@ class DenseStreamSession:
         (None: every stream)."""
         m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
         assert m is None or m.shape == (self.n_streams,)
-        self._ctx._check(self._L.rpl_dense_stream_reset(self._h, _p(m)))
+        self._ctx._check(self._fn("reset")(self._h, _p(m)))
 
     def state(self):
         """(open_nodes, held_capsule): nodes in each stream's open revolution, 1 where a valid capsule is held."""
         open_nodes = np.zeros(self.n_streams, np.uint32)
         held = np.zeros(self.n_streams, np.uint32)
-        self._ctx._check(self._L.rpl_dense_stream_state(self._h, _p(open_nodes), _p(held)))
+        self._ctx._check(self._fn("state")(self._h, _p(open_nodes), _p(held)))
         return open_nodes, held
+
+
+class DenseStreamSession(CapsuleStreamSession):
+    """rpl_dense_stream wrapper: the capsule session fixed to dense capsules (0x85, 84 bytes)."""
+
+    _sym = "rpl_dense_stream"
+
+    def __init__(self, ctx: Context, n_streams: int, stride_capsules: int, max_nodes: int, max_scans: int):
+        self._init(ctx, 0x85, n_streams, stride_capsules, max_nodes, max_scans,
+                   lambda h: ctx._L.rpl_dense_stream_create(ctx._h, n_streams, stride_capsules, max_nodes, max_scans,
+                                                             C.byref(h)))
 
 
 EXCHANGE_NCCL, EXCHANGE_COPY = 0, 1

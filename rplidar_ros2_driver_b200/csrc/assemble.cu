@@ -56,8 +56,9 @@ __device__ __forceinline__ void rank_sort(const uint32_t* in, uint32_t* out, uin
   }
 }
 
-// STREAM: the dense stream session's instantiation (AssembleArgs::carry_len): positions count from the first node of
-// the revolution carried in front of the new nodes, which is a scan start like any other
+// STREAM: a stream session's instantiation, any capsule format (AssembleArgs::carry_len): positions count from the first
+// node of the revolution carried in front of the new nodes, which is a scan start like any other -- listed first when
+// the decoder hands a scan-start list over (dense), found by the flag pass like the others when it does not
 template <bool STREAM>
 __global__ void __launch_bounds__(AT) assemble_kernel(AssembleArgs a) {
   __shared__ uint32_t s_list[kListCap], s_sorted[kListCap];      // scan-start positions

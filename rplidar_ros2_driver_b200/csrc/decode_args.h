@@ -27,17 +27,21 @@ struct CapsuleDecodeArgs {
   uint32_t* scan_starts;          // [n_streams][starts_stride]
   uint32_t* scan_start_counts;    // [n_streams] (may exceed starts_stride: the list is then incomplete)
   uint32_t starts_stride;
-  // dense stream session only (held != nullptr): the capsule each stream held back at the end of the previous push
-  // enters as the predecessor of its first capsule, and the nodes go to nodes_out + s * node_stride + node_first
-  // (behind the session's carry slots) instead of nodes_out + s * stride_capsules * 40.  state_in / state_out are
-  // unused: the scan-start flag travels in the held record.
-  uint32_t* held;                 // [n_streams][kHeldWords], read and rewritten in place
+  // stream session only (node_stride != 0, any capsule format): the nodes go to nodes_out + s * node_stride +
+  // node_first (behind the session's carry slots) instead of nodes_out + s * stride_capsules * nodes per capsule, and
+  // counts above stride_capsules are clamped to it.  Every format but HQ besides lets the capsule each stream held
+  // back at the end of the previous push enter as the predecessor of its first capsule; state_in / state_out are
+  // unused then: the decoder's cross-capsule state travels in the held record.
+  uint32_t* held;                 // [n_streams][kHeldWords], read and rewritten in place (HQ: unused)
   uint32_t node_stride, node_first;
 };
 
-// a held-capsule record: words 0..20 the capsule's 84 bytes, 21 its frame and checksum held (1) or not (0), 22 its
-// start angle (q8), 23 the last released node's scan-start flag.  All zero: nothing held, a fresh stream.
-constexpr uint32_t kHeldWords = 24, kHeldOk = 21, kHeldStart = 22, kHeldSync = 23;
+// a held-capsule record, sized for the largest capsule (ultra-dense, 170 bytes): words 0..42 the capsule's bytes,
+// 43 its frame and checksum held (1) or not (0), 44 its start angle (q8), 45 the last released node's scan-start flag
+// (dense, ultra-dense), 46 the smoothed last distance (ultra-dense's _last_dist_q2).  All zero: nothing held, a fresh
+// stream.
+constexpr uint32_t kHeldCapsuleWords = 43, kHeldOk = 43, kHeldStart = 44, kHeldSync = 45, kHeldLast = 46,
+                   kHeldWords = 48;
 
 // 5-byte standard nodes from raw byte streams
 struct NormalDecodeArgs {
@@ -98,7 +102,7 @@ struct AssembleArgs {
   uint32_t starts_stride;
   uint32_t* reset_prefix;             // scratch [n_streams][stride_capsules]
   uint2* desc;                        // scratch [n_streams][max_scans]
-  // dense stream session only (view mode, carry_len != nullptr): each stream's region of `nodes` is
+  // stream session only (view mode, carry_len != nullptr): each stream's region of `nodes` is
   // [max_nodes carry slots][new nodes]; the first carry_len[s] nodes in front of the new ones are the revolution left
   // open by the previous push.  The revolution this call leaves open goes, capped, right-aligned into the carry slots
   // of carry_out (the other arena: the scans closed here still read this one's), its length into carry_len_out.

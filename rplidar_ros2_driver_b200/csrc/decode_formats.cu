@@ -45,8 +45,7 @@ constexpr uint32_t kStOk = 1, kStSync = 2, kStEmit = 4, kStDiscard = 8, kStCheck
                    kStBadFrame = 64;
 constexpr int kFull = 360 << 16;
 
-// kDenseStream: the dense decoder of a stream session (CapsuleDecodeArgs::held)
-enum { kExpress = 0, kUltra = 1, kUltraDense = 2, kDense = 3, kDenseStream = 4 };
+enum { kExpress = 0, kUltra = 1, kUltraDense = 2, kDense = 3 };
 
 // CB bytes and NODES nodes per capsule, the start angle at byte START, BUFFERS tile buffers of DT capsules (= threads).
 // JUMP_CABINS: the cabin count in the reference's angular-jump discard threshold (0: no threshold).  SYNC_CHAIN: the
@@ -69,8 +68,6 @@ struct Fmt<kDense> {
   static constexpr int CB = 84, NODES = 40, START = 2, BUFFERS = 2, DT = 256, JUMP_CABINS = 40;
   static constexpr bool SYNC_CHAIN = true, SMOOTH_CHAIN = false;
 };
-template <>
-struct Fmt<kDenseStream> : Fmt<kDense> {};
 template <>
 struct Fmt<kUltraDense> {
   // one tile buffer: with the smoothing tables a second one would leave a single CTA (8 warps) per SM
@@ -286,14 +283,19 @@ struct CapsuleSmem {
   int ultra_off[F == kUltra ? 496 : 1];
   uint2 wstage[F == kUltra ? DT / 32 : 1][F == kUltra ? 96 : 1];
   // dense only: angular step per sample of the nodes each capsule releases
-  int inc_q16[(F == kDense || F == kDenseStream) ? DT : 1];
+  int inc_q16[F == kDense ? DT : 1];
 };
 
-template <int F>
+// STREAM: a stream session's instantiation (CapsuleDecodeArgs::node_stride != 0).  The held record stands in for the
+// previous tile's last capsule and its state (sm.carry, okflag[0], start_q8[0], carry_sync, carry_last), so a push
+// boundary is decoded as a tile boundary is.
+template <int F, bool STREAM>
 __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecodeArgs a) {
   using T = Fmt<F>;
   constexpr int CB = T::CB, NODES = T::NODES, DT = T::DT;
-  constexpr bool DENSE = F == kDense || F == kDenseStream, STREAM = F == kDenseStream;
+  constexpr bool DENSE = F == kDense;
+  constexpr uint32_t kCarryWords = (CB + 3) / 4;  // whole words of the held capsule (ultra-dense: 170 -> 172 bytes)
+  static_assert(kCarryWords <= kHeldCapsuleWords && 4 * kCarryWords <= sizeof(CapsuleSmem<F>::carry), "held capsule");
   extern __shared__ __align__(16) unsigned char capsule_smem_raw[];
   CapsuleSmem<F>& sm = *reinterpret_cast<CapsuleSmem<F>*>(capsule_smem_raw);
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -324,12 +326,14 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
         const uint32_t* held = a.held + (size_t)s * kHeldWords;
         sm.okflag[0] = held[kHeldOk];
         sm.start_q8[0] = held[kHeldStart];
-        sm.carry_sync = held[kHeldSync];
+        if constexpr (T::SYNC_CHAIN) sm.carry_sync = held[kHeldSync];
+        if constexpr (T::SMOOTH_CHAIN) sm.carry_last = held[kHeldLast];
       }
     }
     // the held capsule takes the place of a previous tile's last capsule: the first capsule releases it if both hold
+    // (ultra: its last cabin reads cabin 0 of that first capsule)
     if constexpr (STREAM)
-      for (uint32_t w = tid; w < (uint32_t)CB / 4; w += DT)
+      for (uint32_t w = tid; w < kCarryWords; w += DT)
         reinterpret_cast<uint32_t*>(sm.carry)[w] = a.held[(size_t)s * kHeldWords + w];
     __syncthreads();
 
@@ -674,12 +678,13 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
         uint32_t* held = a.held + (size_t)s * kHeldWords;
         held[kHeldOk] = sm.okflag[0];
         held[kHeldStart] = sm.start_q8[0];
-        held[kHeldSync] = sm.carry_sync;
+        if constexpr (T::SYNC_CHAIN) held[kHeldSync] = sm.carry_sync;
+        if constexpr (T::SMOOTH_CHAIN) held[kHeldLast] = sm.carry_last;
       }
     }
     // the last capsule is held for the next push (a stream without capsules writes back what it read)
     if constexpr (STREAM)
-      for (uint32_t w = tid; w < (uint32_t)CB / 4; w += DT)
+      for (uint32_t w = tid; w < kCarryWords; w += DT)
         a.held[(size_t)s * kHeldWords + w] = reinterpret_cast<const uint32_t*>(sm.carry)[w];
     __syncthreads();
   }
@@ -708,6 +713,9 @@ struct HqSmem {
   uint32_t carry_nodes, tile_nodes;
 };
 
+// STREAM: a stream session's instantiation.  HQ capsules carry nothing across capsules (handler_hqnode.cpp:93-172), so
+// it differs only in where the nodes go (behind the session's carry slots).
+template <bool STREAM>
 __global__ void __launch_bounds__(HT) decode_hq_kernel(CapsuleDecodeArgs a) {
   extern __shared__ __align__(16) unsigned char capsule_smem_raw[];
   HqSmem& sm = *reinterpret_cast<HqSmem*>(capsule_smem_raw);
@@ -734,9 +742,10 @@ __global__ void __launch_bounds__(HT) decode_hq_kernel(CapsuleDecodeArgs a) {
            sm.advance[which][3][v >> 24];
   };
   for (uint32_t s = blockIdx.x; s < a.n_streams; s += gridDim.x) {
-    const uint32_t n = a.counts[s];
+    const uint32_t n = STREAM ? min(a.counts[s], a.stride_capsules) : a.counts[s];
     const uint8_t* src = a.capsules + (size_t)s * a.stride_capsules * kHqBytes;
-    uint2* out = a.nodes_out + (size_t)s * a.stride_capsules * 96;
+    uint2* out = STREAM ? a.nodes_out + (size_t)s * a.node_stride + a.node_first
+                        : a.nodes_out + (size_t)s * a.stride_capsules * 96;
     uint32_t* st_out = a.capsule_status ? a.capsule_status + (size_t)s * a.stride_capsules : nullptr;
     uint32_t* off_out = a.capsule_node_offset ? a.capsule_node_offset + (size_t)s * a.stride_capsules : nullptr;
     if (tid == 0) sm.carry_nodes = 0;
@@ -1028,8 +1037,20 @@ __global__ void __launch_bounds__(NT, 5) decode_normal_kernel(NormalDecodeArgs a
 
 template <int F>
 cudaError_t launch_fmt(const CapsuleDecodeArgs& a, int grid, cudaStream_t stream) {
-  decode_capsule_kernel<F><<<grid, Fmt<F>::DT, sizeof(CapsuleSmem<F>), stream>>>(a);
+  if (a.node_stride)
+    decode_capsule_kernel<F, true><<<grid, Fmt<F>::DT, sizeof(CapsuleSmem<F>), stream>>>(a);
+  else
+    decode_capsule_kernel<F, false><<<grid, Fmt<F>::DT, sizeof(CapsuleSmem<F>), stream>>>(a);
   return cudaGetLastError();
+}
+
+template <int F>
+cudaError_t configure_fmt() {
+  cudaError_t e = cudaFuncSetAttribute(decode_capsule_kernel<F, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)sizeof(CapsuleSmem<F>));
+  if (e != cudaSuccess) return e;
+  return cudaFuncSetAttribute(decode_capsule_kernel<F, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              (int)sizeof(CapsuleSmem<F>));
 }
 
 }  // namespace
@@ -1039,10 +1060,13 @@ cudaError_t launch_decode_capsules(uint32_t ans_type, const CapsuleDecodeArgs& a
   switch (ans_type) {
     case 0x82: return launch_fmt<kExpress>(a, grid, stream);
     case 0x84: return launch_fmt<kUltra>(a, grid, stream);
-    case 0x85: return a.held ? launch_fmt<kDenseStream>(a, grid, stream) : launch_fmt<kDense>(a, grid, stream);
+    case 0x85: return launch_fmt<kDense>(a, grid, stream);
     case 0x86: return launch_fmt<kUltraDense>(a, grid, stream);
     case 0x83:
-      decode_hq_kernel<<<grid, HT, sizeof(HqSmem), stream>>>(a);
+      if (a.node_stride)
+        decode_hq_kernel<true><<<grid, HT, sizeof(HqSmem), stream>>>(a);
+      else
+        decode_hq_kernel<false><<<grid, HT, sizeof(HqSmem), stream>>>(a);
       return cudaGetLastError();
     default: return cudaErrorInvalidValue;
   }
@@ -1086,22 +1110,12 @@ cudaError_t decode_formats_configure() {
     e = cudaMemcpyToSymbol(g_hq_advance, adv, sizeof(adv));
     if (e != cudaSuccess) return e;
   }
-  e = cudaFuncSetAttribute(decode_capsule_kernel<kExpress>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           (int)sizeof(CapsuleSmem<kExpress>));
+  if ((e = configure_fmt<kExpress>()) != cudaSuccess || (e = configure_fmt<kUltra>()) != cudaSuccess ||
+      (e = configure_fmt<kDense>()) != cudaSuccess || (e = configure_fmt<kUltraDense>()) != cudaSuccess)
+    return e;
+  e = cudaFuncSetAttribute(decode_hq_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HqSmem));
   if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(decode_capsule_kernel<kUltra>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           (int)sizeof(CapsuleSmem<kUltra>));
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(decode_capsule_kernel<kDense>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           (int)sizeof(CapsuleSmem<kDense>));
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(decode_capsule_kernel<kDenseStream>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           (int)sizeof(CapsuleSmem<kDenseStream>));
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(decode_capsule_kernel<kUltraDense>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           (int)sizeof(CapsuleSmem<kUltraDense>));
-  if (e != cudaSuccess) return e;
-  return cudaFuncSetAttribute(decode_hq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HqSmem));
+  return cudaFuncSetAttribute(decode_hq_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HqSmem));
 }
 
 }  // namespace rpl

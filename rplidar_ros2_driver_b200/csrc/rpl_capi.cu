@@ -1250,14 +1250,16 @@ rpl_result rpl_chain_dense_laserscan(rpl_ctx* c, const uint8_t* capsules, const 
 
 }  // extern "C"
 
-// ---- dense-capsule stream session (DESIGN.md 5.7) ------------------------------------------------------------------
-// Per stream: the held capsule with the decoder's scan-start flag (one rpl::kHeldWords record), and the revolution left
-// open, kept in front of the next push's nodes so that a scan spanning pushes is one contiguous view.  Each stream's
-// region of an arena is [max_nodes carry slots][40 * stride_capsules new nodes]; push t decodes into arena t % 2 and
-// its assembler writes the new open revolution into the carry slots of the other arena, because the scans push t
-// closes are read from this arena's carry slots by the scan kernels after the assembler.
-struct rpl_dense_stream {
+// ---- capsule stream session (DESIGN.md 5.7) ------------------------------------------------------------------------
+// Per stream: the held capsule with the decoder's cross-capsule state (one rpl::kHeldWords record; HQ capsules hold
+// nothing), and the revolution left open, kept in front of the next push's nodes so that a scan spanning pushes is one
+// contiguous view.  Each stream's region of an arena is [max_nodes carry slots][nodes per capsule * stride_capsules new
+// nodes]; push t decodes into arena t % 2 and its assembler writes the new open revolution into the carry slots of the
+// other arena, because the scans push t closes are read from this arena's carry slots by the scan kernels after the
+// assembler.  rpl_dense_stream is this session fixed to 0x85.
+struct rpl_capsule_stream {
   rpl_ctx* c = nullptr;
+  uint32_t ans_type = 0, cap_bytes = 0;    // answer type, bytes per capsule
   uint32_t n_streams = 0, stride_capsules = 0, max_nodes = 0, max_scans = 0;
   uint32_t stride_nodes = 0, starts_stride = 0;
   uint32_t chunk_dev = 0, chunk_host = 0;  // streams per scan launch (context's max_scans), per host-push chunk
@@ -1265,7 +1267,8 @@ struct rpl_dense_stream {
   rpl_node_hq* arena[2] = {nullptr, nullptr};
   uint32_t* carry_len[2] = {nullptr, nullptr};  // [n_streams] open revolution in front of arena[p]'s new nodes
   uint32_t* held = nullptr;                     // [n_streams][kHeldWords]
-  uint32_t *status = nullptr, *offsets = nullptr, *node_counts = nullptr, *starts = nullptr, *start_counts = nullptr;
+  uint32_t *status = nullptr, *offsets = nullptr, *node_counts = nullptr;
+  uint32_t *starts = nullptr, *start_counts = nullptr;  // dense only: the decoder's scan-start list
   uint32_t* scan_len = nullptr;
   rpl_scan_view* views = nullptr;
   unsigned char* lane_buf[kLanes] = {nullptr, nullptr};  // host-push staging: capsules, counts and outputs of a chunk
@@ -1275,17 +1278,22 @@ struct rpl_dense_stream {
 
 namespace {
 
+// the dense session's handle is a capsule session's
+rpl_capsule_stream* capsule_session(rpl_dense_stream* ds) { return reinterpret_cast<rpl_capsule_stream*>(ds); }
+
 // decode -> assemble -> scan kernels for streams [s0, s0 + ns) on `st`; capsules / counts / outputs point at s0's
-rpl_result dense_stream_chunk(rpl_dense_stream* ds, Lane& l, cudaStream_t st, uint32_t s0, uint32_t ns,
-                              const uint8_t* capsules, const uint32_t* counts, uint32_t sample_duration_us,
-                              const rpl_scan_params* params, float* ranges, float* intens, uint32_t* beams, float* inc,
-                              uint32_t* scans_per_stream) {
-  rpl_ctx* c = ds->c;
-  const uint32_t p = ds->parity, sc = ds->stride_capsules;
-  rpl_node_hq* nodes = ds->arena[p] + (size_t)s0 * ds->stride_nodes;
-  uint32_t* status = ds->status + (size_t)s0 * sc;
-  uint32_t* offsets = ds->offsets + (size_t)s0 * sc;
-  uint32_t* starts = ds->starts + (size_t)s0 * ds->starts_stride;
+rpl_result capsule_stream_chunk(rpl_capsule_stream* cs, Lane& l, cudaStream_t st, uint32_t s0, uint32_t ns,
+                                const uint8_t* capsules, const uint32_t* counts, uint32_t sample_duration_us,
+                                const rpl_scan_params* params, float* ranges, float* intens, uint32_t* beams,
+                                float* inc, uint32_t* scans_per_stream) {
+  rpl_ctx* c = cs->c;
+  const uint32_t p = cs->parity, sc = cs->stride_capsules;
+  rpl_node_hq* nodes = cs->arena[p] + (size_t)s0 * cs->stride_nodes;
+  uint32_t* status = cs->status + (size_t)s0 * sc;
+  uint32_t* offsets = cs->offsets + (size_t)s0 * sc;
+  // only the dense decoder lists its scan starts; the assembler finds the others' with its flag pass
+  uint32_t* starts = cs->starts ? cs->starts + (size_t)s0 * cs->starts_stride : nullptr;
+  uint32_t* start_counts = cs->starts ? cs->start_counts + s0 : nullptr;
   rpl::CapsuleDecodeArgs a{};
   a.capsules = capsules;
   a.counts = counts;
@@ -1294,42 +1302,43 @@ rpl_result dense_stream_chunk(rpl_dense_stream* ds, Lane& l, cudaStream_t st, ui
   a.sample_duration_us = sample_duration_us;
   a.state_words = 1;
   a.nodes_out = reinterpret_cast<uint2*>(nodes);
-  a.node_counts = ds->node_counts + s0;
+  a.node_counts = cs->node_counts + s0;
   a.capsule_status = status;
   a.capsule_node_offset = offsets;
   a.scan_starts = starts;
-  a.scan_start_counts = ds->start_counts + s0;
-  a.starts_stride = ds->starts_stride;
-  a.held = ds->held + (size_t)s0 * rpl::kHeldWords;
-  a.node_stride = ds->stride_nodes;
-  a.node_first = ds->max_nodes;
-  rpl_result r = decode_capsules_launch(c, 0x85, a, st);
+  a.scan_start_counts = start_counts;
+  a.starts_stride = cs->starts_stride;
+  a.held = cs->held + (size_t)s0 * rpl::kHeldWords;
+  a.node_stride = cs->stride_nodes;
+  a.node_first = cs->max_nodes;
+  rpl_result r = decode_capsules_launch(c, cs->ans_type, a, st);
   if (r != RPL_RESULT_OK) return r;
   // the assembler's scratch belongs to the context: one assemble kernel at a time (as in the chain)
   if (!c->asm_done) RPL_CUDA(c, cudaEventCreateWithFlags(&c->asm_done, cudaEventDisableTiming), RPL_RESULT_OPERATION_FAIL);
   RPL_CUDA(c, cudaStreamWaitEvent(st, c->asm_done, 0), RPL_RESULT_OPERATION_FAIL);
-  const size_t so = (size_t)s0 * ds->max_scans;
-  r = assemble_common(c, nodes, ds->node_counts + s0, ns, ds->stride_nodes, status, offsets, counts, sc, ds->max_nodes,
-                      ds->max_scans, ds->max_nodes, nullptr, ds->views + so, ds->scan_len + so, scans_per_stream, nullptr,
-                      nullptr, st, starts, ds->starts_stride, ds->start_counts + s0, ds->carry_len[p] + s0,
-                      ds->arena[p ^ 1u] + (size_t)s0 * ds->stride_nodes, ds->carry_len[p ^ 1u] + s0);
+  const size_t so = (size_t)s0 * cs->max_scans;
+  r = assemble_common(c, nodes, cs->node_counts + s0, ns, cs->stride_nodes, status, offsets, counts, sc, cs->max_nodes,
+                      cs->max_scans, cs->max_nodes, nullptr, cs->views + so, cs->scan_len + so, scans_per_stream, nullptr,
+                      nullptr, st, starts, starts ? cs->starts_stride : 0u, start_counts, cs->carry_len[p] + s0,
+                      cs->arena[p ^ 1u] + (size_t)s0 * cs->stride_nodes, cs->carry_len[p ^ 1u] + s0);
   if (r != RPL_RESULT_OK) return r;
   RPL_CUDA(c, cudaEventRecord(c->asm_done, st), RPL_RESULT_OPERATION_FAIL);
-  return enqueue_scan(c, l, nodes, ds->scan_len + so, ns * ds->max_scans, ds->max_nodes, params, nullptr, ranges, intens,
-                      beams, inc, nullptr, nullptr, st, reinterpret_cast<const uint2*>(ds->views + so),
-                      (unsigned long long)ns * ds->stride_nodes);
+  return enqueue_scan(c, l, nodes, cs->scan_len + so, ns * cs->max_scans, cs->max_nodes, params, nullptr, ranges, intens,
+                      beams, inc, nullptr, nullptr, st, reinterpret_cast<const uint2*>(cs->views + so),
+                      (unsigned long long)ns * cs->stride_nodes);
 }
 
-bool dense_stream_args_ok(rpl_dense_stream* ds, const uint8_t* capsules, const uint32_t* capsule_counts,
-                          uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges, float* intensities,
-                          uint32_t* beam_counts, uint32_t* scans_per_stream) {
-  rpl_ctx* c = ds->c;
+bool capsule_stream_args_ok(rpl_capsule_stream* cs, const uint8_t* capsules, const uint32_t* capsule_counts,
+                            uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
+                            float* intensities, uint32_t* beam_counts, uint32_t* scans_per_stream) {
+  rpl_ctx* c = cs->c;
   if (!capsules || !capsule_counts || !params || !ranges || !intensities || !beam_counts || !scans_per_stream) {
     c->err = "null capsules, counts, params or output buffer";
     return false;
   }
   if (!sample_duration_ok(c, sample_duration_us)) return false;
-  if ((reinterpret_cast<uintptr_t>(capsules) & 3u) != 0) {
+  // the alignment rule of rpl_decode_capsules_batch_dev: only dense capsules are read in 4-byte words
+  if (cs->ans_type == 0x85 && (reinterpret_cast<uintptr_t>(capsules) & 3u) != 0) {
     c->err = "capsule buffer must be 4-byte aligned";
     return false;
   }
@@ -1340,10 +1349,15 @@ bool dense_stream_args_ok(rpl_dense_stream* ds, const uint8_t* capsules, const u
 
 extern "C" {
 
-rpl_result rpl_dense_stream_create(rpl_ctx* c, uint32_t n_streams, uint32_t stride_capsules, uint32_t max_nodes,
-                                   uint32_t max_scans, rpl_dense_stream** out) {
+rpl_result rpl_capsule_stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint32_t stride_capsules,
+                                     uint32_t max_nodes, uint32_t max_scans, rpl_capsule_stream** out) {
   if (!c || !out) return RPL_RESULT_INVALID_DATA;
   *out = nullptr;
+  const uint32_t cap_bytes = rpl_capsule_bytes(ans_type), cap_nodes = rpl_capsule_nodes(ans_type);
+  if (cap_bytes == 0) {
+    c->err = "a stream session takes the capsule answer types 0x82..0x86 (0x81 standard nodes are no capsules)";
+    return RPL_RESULT_INVALID_DATA;
+  }
   if (n_streams == 0 || stride_capsules == 0 || max_scans == 0 || max_nodes == 0 || max_nodes > rpl::kSmallMaxNodes ||
       (max_nodes & 1u)) {
     c->err = "need n_streams > 0, stride_capsules > 0, max_scans > 0 and an even max_nodes in [2, 8192]";
@@ -1353,197 +1367,236 @@ rpl_result rpl_dense_stream_create(rpl_ctx* c, uint32_t n_streams, uint32_t stri
     c->err = "the context's max_scans is smaller than max_scans of one stream";
     return RPL_RESULT_INVALID_DATA;
   }
-  const unsigned long long stride_nodes = (unsigned long long)max_nodes + 40ull * stride_capsules;
+  const unsigned long long stride_nodes = (unsigned long long)max_nodes + (unsigned long long)cap_nodes * stride_capsules;
   if (stride_nodes * n_streams > 0xFFFFFFFFull) {
-    c->err = "n_streams * (max_nodes + 40 * stride_capsules) must stay below 2^32 (32-bit scan views)";
+    c->err = "n_streams * (max_nodes + nodes per capsule * stride_capsules) must stay below 2^32 (32-bit scan views)";
     return RPL_RESULT_INVALID_DATA;
   }
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  rpl_dense_stream* ds = new (std::nothrow) rpl_dense_stream();
-  if (!ds) return RPL_RESULT_INSUFFICIENT_MEMORY;
-  ds->c = c;
-  ds->n_streams = n_streams;
-  ds->stride_capsules = stride_capsules;
-  ds->max_nodes = max_nodes;
-  ds->max_scans = max_scans;
-  ds->stride_nodes = (uint32_t)stride_nodes;  // even: every region starts 16-byte aligned
-  ds->starts_stride = 2 * max_scans + 64;     // scan starts per stream the decoder may list (as in the chain)
-  ds->chunk_dev = std::min(n_streams, c->max_scans / max_scans);
+  rpl_capsule_stream* cs = new (std::nothrow) rpl_capsule_stream();
+  if (!cs) return RPL_RESULT_INSUFFICIENT_MEMORY;
+  cs->c = c;
+  cs->ans_type = ans_type;
+  cs->cap_bytes = cap_bytes;
+  cs->n_streams = n_streams;
+  cs->stride_capsules = stride_capsules;
+  cs->max_nodes = max_nodes;
+  cs->max_scans = max_scans;
+  cs->stride_nodes = (uint32_t)stride_nodes;  // even: every region starts 16-byte aligned
+  cs->starts_stride = 2 * max_scans + 64;     // scan starts per stream the decoder may list (as in the chain)
+  cs->chunk_dev = std::min(n_streams, c->max_scans / max_scans);
   // host pushes: about 16 MiB of capsules per chunk, whole streams (as in the chain)
-  const size_t cap_bytes_stream = (size_t)stride_capsules * 84;
-  ds->chunk_host = std::min<uint32_t>(ds->chunk_dev, (uint32_t)std::max<size_t>(1, ((size_t)16 << 20) / cap_bytes_stream));
+  const size_t cap_bytes_stream = (size_t)stride_capsules * cap_bytes;
+  cs->chunk_host = std::min<uint32_t>(cs->chunk_dev, (uint32_t)std::max<size_t>(1, ((size_t)16 << 20) / cap_bytes_stream));
   auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
-  const size_t NS = (size_t)ds->chunk_host * max_scans;
-  ds->o_ccnt = up((size_t)ds->chunk_host * cap_bytes_stream);
-  ds->o_r = ds->o_ccnt + up((size_t)ds->chunk_host * 4);
-  ds->o_i = ds->o_r + up(NS * max_nodes * 4);
-  ds->o_b = ds->o_i + up(NS * max_nodes * 4);
-  ds->o_inc = ds->o_b + up(NS * 4);
-  ds->o_sps = ds->o_inc + up(NS * 4);
-  ds->lane_bytes = ds->o_sps + up((size_t)ds->chunk_host * 4);
+  const size_t NS = (size_t)cs->chunk_host * max_scans;
+  cs->o_ccnt = up((size_t)cs->chunk_host * cap_bytes_stream);
+  cs->o_r = cs->o_ccnt + up((size_t)cs->chunk_host * 4);
+  cs->o_i = cs->o_r + up(NS * max_nodes * 4);
+  cs->o_b = cs->o_i + up(NS * max_nodes * 4);
+  cs->o_inc = cs->o_b + up(NS * 4);
+  cs->o_sps = cs->o_inc + up(NS * 4);
+  cs->lane_bytes = cs->o_sps + up((size_t)cs->chunk_host * 4);
   const size_t n = n_streams, ncap = n * stride_capsules;
   const rpl_result oom = RPL_RESULT_INSUFFICIENT_MEMORY;
   auto fail = [&](rpl_result r) {
-    rpl_dense_stream_destroy(ds);
+    rpl_capsule_stream_destroy(cs);
     return r;
   };
   for (int p = 0; p < 2; ++p)
-    if (!cuda_ok(c, dev_alloc(&ds->arena[p], n * ds->stride_nodes), "cudaMalloc") ||
-        !cuda_ok(c, dev_alloc(&ds->carry_len[p], n), "cudaMalloc") ||
-        !cuda_ok(c, cudaMemset(ds->carry_len[p], 0, n * 4), "cudaMemset"))
+    if (!cuda_ok(c, dev_alloc(&cs->arena[p], n * cs->stride_nodes), "cudaMalloc") ||
+        !cuda_ok(c, dev_alloc(&cs->carry_len[p], n), "cudaMalloc") ||
+        !cuda_ok(c, cudaMemset(cs->carry_len[p], 0, n * 4), "cudaMemset"))
       return fail(oom);
   for (int i = 0; i < kLanes; ++i)
-    if (!cuda_ok(c, dev_alloc(&ds->lane_buf[i], ds->lane_bytes), "cudaMalloc")) return fail(oom);
-  if (!cuda_ok(c, dev_alloc(&ds->held, n * rpl::kHeldWords), "cudaMalloc") ||
-      !cuda_ok(c, cudaMemset(ds->held, 0, n * rpl::kHeldWords * 4), "cudaMemset") ||
-      !cuda_ok(c, dev_alloc(&ds->status, ncap), "cudaMalloc") || !cuda_ok(c, dev_alloc(&ds->offsets, ncap), "cudaMalloc") ||
-      !cuda_ok(c, dev_alloc(&ds->node_counts, n), "cudaMalloc") ||
-      !cuda_ok(c, dev_alloc(&ds->starts, n * ds->starts_stride), "cudaMalloc") ||
-      !cuda_ok(c, dev_alloc(&ds->start_counts, n), "cudaMalloc") ||
-      !cuda_ok(c, dev_alloc(&ds->scan_len, n * max_scans), "cudaMalloc") ||
-      !cuda_ok(c, dev_alloc(&ds->views, n * max_scans), "cudaMalloc") ||
-      !cuda_ok(c, cudaEventCreateWithFlags(&ds->done, cudaEventDisableTiming), "cudaEventCreate") ||
+    if (!cuda_ok(c, dev_alloc(&cs->lane_buf[i], cs->lane_bytes), "cudaMalloc")) return fail(oom);
+  if (ans_type == 0x85 && (!cuda_ok(c, dev_alloc(&cs->starts, n * cs->starts_stride), "cudaMalloc") ||
+                           !cuda_ok(c, dev_alloc(&cs->start_counts, n), "cudaMalloc")))
+    return fail(oom);
+  if (!cuda_ok(c, dev_alloc(&cs->held, n * rpl::kHeldWords), "cudaMalloc") ||
+      !cuda_ok(c, cudaMemset(cs->held, 0, n * rpl::kHeldWords * 4), "cudaMemset") ||
+      !cuda_ok(c, dev_alloc(&cs->status, ncap), "cudaMalloc") || !cuda_ok(c, dev_alloc(&cs->offsets, ncap), "cudaMalloc") ||
+      !cuda_ok(c, dev_alloc(&cs->node_counts, n), "cudaMalloc") ||
+      !cuda_ok(c, dev_alloc(&cs->scan_len, n * max_scans), "cudaMalloc") ||
+      !cuda_ok(c, dev_alloc(&cs->views, n * max_scans), "cudaMalloc") ||
+      !cuda_ok(c, cudaEventCreateWithFlags(&cs->done, cudaEventDisableTiming), "cudaEventCreate") ||
       !cuda_ok(c, cudaDeviceSynchronize(), "cudaDeviceSynchronize"))  // the zeroed state is in place before any push
     return fail(oom);
-  *out = ds;
+  *out = cs;
   return RPL_RESULT_OK;
 }
 
-void rpl_dense_stream_destroy(rpl_dense_stream* ds) {
-  if (!ds) return;
-  cudaSetDevice(ds->c->device);
-  if (ds->done) cudaEventSynchronize(ds->done);
-  for (int i = 0; i < kLanes; ++i) cudaStreamSynchronize(ds->c->lane[i].stream);
+void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
+  if (!cs) return;
+  cudaSetDevice(cs->c->device);
+  if (cs->done) cudaEventSynchronize(cs->done);
+  for (int i = 0; i < kLanes; ++i) cudaStreamSynchronize(cs->c->lane[i].stream);
   for (int p = 0; p < 2; ++p) {
-    cudaFree(ds->arena[p]);
-    cudaFree(ds->carry_len[p]);
+    cudaFree(cs->arena[p]);
+    cudaFree(cs->carry_len[p]);
   }
-  for (int i = 0; i < kLanes; ++i) cudaFree(ds->lane_buf[i]);
-  cudaFree(ds->held);
-  cudaFree(ds->status);
-  cudaFree(ds->offsets);
-  cudaFree(ds->node_counts);
-  cudaFree(ds->starts);
-  cudaFree(ds->start_counts);
-  cudaFree(ds->scan_len);
-  cudaFree(ds->views);
-  if (ds->done) cudaEventDestroy(ds->done);
-  delete ds;
+  for (int i = 0; i < kLanes; ++i) cudaFree(cs->lane_buf[i]);
+  cudaFree(cs->held);
+  cudaFree(cs->status);
+  cudaFree(cs->offsets);
+  cudaFree(cs->node_counts);
+  cudaFree(cs->starts);
+  cudaFree(cs->start_counts);
+  cudaFree(cs->scan_len);
+  cudaFree(cs->views);
+  if (cs->done) cudaEventDestroy(cs->done);
+  delete cs;
 }
 
-rpl_result rpl_dense_stream_push(rpl_dense_stream* ds, const uint8_t* capsules, const uint32_t* capsule_counts,
-                                 uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
-                                 float* intensities, uint32_t* beam_counts, float* angle_increment,
-                                 uint32_t* scans_per_stream) {
-  if (!ds) return RPL_RESULT_INVALID_DATA;
-  rpl_ctx* c = ds->c;
-  if (!dense_stream_args_ok(ds, capsules, capsule_counts, sample_duration_us, params, ranges, intensities, beam_counts,
-                            scans_per_stream))
+rpl_result rpl_capsule_stream_push(rpl_capsule_stream* cs, const uint8_t* capsules, const uint32_t* capsule_counts,
+                                   uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
+                                   float* intensities, uint32_t* beam_counts, float* angle_increment,
+                                   uint32_t* scans_per_stream) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!capsule_stream_args_ok(cs, capsules, capsule_counts, sample_duration_us, params, ranges, intensities,
+                              beam_counts, scans_per_stream))
     return RPL_RESULT_INVALID_DATA;
-  for (uint32_t s = 0; s < ds->n_streams; ++s)
-    if (capsule_counts[s] > ds->stride_capsules) {
+  for (uint32_t s = 0; s < cs->n_streams; ++s)
+    if (capsule_counts[s] > cs->stride_capsules) {
       c->err = "capsule_counts[s] exceeds stride_capsules";
       return RPL_RESULT_INVALID_DATA;
     }
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  for (int i = 0; i < kLanes; ++i) RPL_CUDA(c, cudaStreamWaitEvent(c->lane[i].stream, ds->done, 0), RPL_RESULT_OPERATION_FAIL);
-  const size_t cap_bytes_stream = (size_t)ds->stride_capsules * 84, row = (size_t)ds->max_scans * ds->max_nodes;
+  for (int i = 0; i < kLanes; ++i) RPL_CUDA(c, cudaStreamWaitEvent(c->lane[i].stream, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
+  const size_t cap_bytes_stream = (size_t)cs->stride_capsules * cs->cap_bytes, row = (size_t)cs->max_scans * cs->max_nodes;
   const cudaMemcpyKind h2d = cudaMemcpyHostToDevice, d2h = cudaMemcpyDeviceToHost;
   auto run_chunk = [&](Lane& l, uint32_t s0, uint32_t ns) -> rpl_result {
-    unsigned char* d = ds->lane_buf[&l - c->lane];
-    const size_t nsc = (size_t)ns * ds->max_scans;
+    unsigned char* d = cs->lane_buf[&l - c->lane];
+    const size_t nsc = (size_t)ns * cs->max_scans;
     RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);  // the lane's previous chunk has left
     RPL_CUDA(c, cudaMemcpyAsync(d, capsules + s0 * cap_bytes_stream, ns * cap_bytes_stream, h2d, l.stream),
              RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(d + ds->o_ccnt, capsule_counts + s0, (size_t)ns * 4, h2d, l.stream),
+    RPL_CUDA(c, cudaMemcpyAsync(d + cs->o_ccnt, capsule_counts + s0, (size_t)ns * 4, h2d, l.stream),
              RPL_RESULT_OPERATION_FAIL);
-    const rpl_result r = dense_stream_chunk(
-        ds, l, l.stream, s0, ns, d, reinterpret_cast<uint32_t*>(d + ds->o_ccnt), sample_duration_us, params,
-        reinterpret_cast<float*>(d + ds->o_r), reinterpret_cast<float*>(d + ds->o_i),
-        reinterpret_cast<uint32_t*>(d + ds->o_b), reinterpret_cast<float*>(d + ds->o_inc),
-        reinterpret_cast<uint32_t*>(d + ds->o_sps));
+    const rpl_result r = capsule_stream_chunk(
+        cs, l, l.stream, s0, ns, d, reinterpret_cast<uint32_t*>(d + cs->o_ccnt), sample_duration_us, params,
+        reinterpret_cast<float*>(d + cs->o_r), reinterpret_cast<float*>(d + cs->o_i),
+        reinterpret_cast<uint32_t*>(d + cs->o_b), reinterpret_cast<float*>(d + cs->o_inc),
+        reinterpret_cast<uint32_t*>(d + cs->o_sps));
     if (r != RPL_RESULT_OK) return r;
-    const size_t so = (size_t)s0 * ds->max_scans;
-    RPL_CUDA(c, cudaMemcpyAsync(ranges + so * ds->max_nodes, d + ds->o_r, ns * row * 4, d2h, l.stream),
+    const size_t so = (size_t)s0 * cs->max_scans;
+    RPL_CUDA(c, cudaMemcpyAsync(ranges + so * cs->max_nodes, d + cs->o_r, ns * row * 4, d2h, l.stream),
              RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(intensities + so * ds->max_nodes, d + ds->o_i, ns * row * 4, d2h, l.stream),
+    RPL_CUDA(c, cudaMemcpyAsync(intensities + so * cs->max_nodes, d + cs->o_i, ns * row * 4, d2h, l.stream),
              RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(beam_counts + so, d + ds->o_b, nsc * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(beam_counts + so, d + cs->o_b, nsc * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
     if (angle_increment)
-      RPL_CUDA(c, cudaMemcpyAsync(angle_increment + so, d + ds->o_inc, nsc * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(scans_per_stream + s0, d + ds->o_sps, (size_t)ns * 4, d2h, l.stream),
+      RPL_CUDA(c, cudaMemcpyAsync(angle_increment + so, d + cs->o_inc, nsc * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(scans_per_stream + s0, d + cs->o_sps, (size_t)ns * 4, d2h, l.stream),
              RPL_RESULT_OPERATION_FAIL);
     return RPL_RESULT_OK;
   };
-  const rpl_result r = run_chunks(c, ds->n_streams, ds->chunk_host, run_chunk);
-  ds->parity ^= 1u;
+  const rpl_result r = run_chunks(c, cs->n_streams, cs->chunk_host, run_chunk);
+  cs->parity ^= 1u;
   return r;
 }
 
-rpl_result rpl_dense_stream_push_dev(rpl_dense_stream* ds, const uint8_t* capsules, const uint32_t* capsule_counts,
-                                     uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
-                                     float* intensities, uint32_t* beam_counts, float* angle_increment,
-                                     uint32_t* scans_per_stream, void* stream) {
-  if (!ds) return RPL_RESULT_INVALID_DATA;
-  rpl_ctx* c = ds->c;
-  if (!dense_stream_args_ok(ds, capsules, capsule_counts, sample_duration_us, params, ranges, intensities, beam_counts,
-                            scans_per_stream))
+rpl_result rpl_capsule_stream_push_dev(rpl_capsule_stream* cs, const uint8_t* capsules, const uint32_t* capsule_counts,
+                                       uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
+                                       float* intensities, uint32_t* beam_counts, float* angle_increment,
+                                       uint32_t* scans_per_stream, void* stream) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!capsule_stream_args_ok(cs, capsules, capsule_counts, sample_duration_us, params, ranges, intensities,
+                              beam_counts, scans_per_stream))
     return RPL_RESULT_INVALID_DATA;
   cudaStream_t st;
   if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
-  RPL_CUDA(c, cudaStreamWaitEvent(st, ds->done, 0), RPL_RESULT_OPERATION_FAIL);
-  const size_t row = (size_t)ds->max_scans * ds->max_nodes;
+  RPL_CUDA(c, cudaStreamWaitEvent(st, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
+  const size_t row = (size_t)cs->max_scans * cs->max_nodes;
   rpl_result r = RPL_RESULT_OK;
-  for (uint32_t s0 = 0; s0 < ds->n_streams && r == RPL_RESULT_OK; s0 += ds->chunk_dev) {
-    const uint32_t ns = std::min(ds->chunk_dev, ds->n_streams - s0);
-    const size_t so = (size_t)s0 * ds->max_scans;
-    r = dense_stream_chunk(ds, c->lane[0], st, s0, ns, capsules + (size_t)s0 * ds->stride_capsules * 84,
-                           capsule_counts + s0, sample_duration_us, params, ranges + (size_t)s0 * row,
-                           intensities + (size_t)s0 * row, beam_counts + so, angle_increment ? angle_increment + so : nullptr,
-                           scans_per_stream + s0);
+  for (uint32_t s0 = 0; s0 < cs->n_streams && r == RPL_RESULT_OK; s0 += cs->chunk_dev) {
+    const uint32_t ns = std::min(cs->chunk_dev, cs->n_streams - s0);
+    const size_t so = (size_t)s0 * cs->max_scans;
+    r = capsule_stream_chunk(cs, c->lane[0], st, s0, ns, capsules + (size_t)s0 * cs->stride_capsules * cs->cap_bytes,
+                             capsule_counts + s0, sample_duration_us, params, ranges + (size_t)s0 * row,
+                             intensities + (size_t)s0 * row, beam_counts + so,
+                             angle_increment ? angle_increment + so : nullptr, scans_per_stream + s0);
   }
-  ds->parity ^= 1u;
-  RPL_CUDA(c, cudaEventRecord(ds->done, st), RPL_RESULT_OPERATION_FAIL);
+  cs->parity ^= 1u;
+  RPL_CUDA(c, cudaEventRecord(cs->done, st), RPL_RESULT_OPERATION_FAIL);
   return r;
 }
 
-rpl_result rpl_dense_stream_reset(rpl_dense_stream* ds, const uint8_t* stream_mask) {
-  if (!ds) return RPL_RESULT_INVALID_DATA;
-  rpl_ctx* c = ds->c;
+rpl_result rpl_capsule_stream_reset(rpl_capsule_stream* cs, const uint8_t* stream_mask) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
   cudaStream_t st = c->lane[0].stream;
-  RPL_CUDA(c, cudaStreamWaitEvent(st, ds->done, 0), RPL_RESULT_OPERATION_FAIL);
-  const uint32_t p = ds->parity;
-  for (uint32_t s = 0; s < ds->n_streams;) {  // one pair of clears per run of masked streams
+  RPL_CUDA(c, cudaStreamWaitEvent(st, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
+  const uint32_t p = cs->parity;
+  for (uint32_t s = 0; s < cs->n_streams;) {  // one pair of clears per run of masked streams
     if (stream_mask && !stream_mask[s]) {
       ++s;
       continue;
     }
     uint32_t e = s + 1;
-    while (e < ds->n_streams && (!stream_mask || stream_mask[e])) ++e;
-    RPL_CUDA(c, cudaMemsetAsync(ds->held + (size_t)s * rpl::kHeldWords, 0, (size_t)(e - s) * rpl::kHeldWords * 4, st),
+    while (e < cs->n_streams && (!stream_mask || stream_mask[e])) ++e;
+    RPL_CUDA(c, cudaMemsetAsync(cs->held + (size_t)s * rpl::kHeldWords, 0, (size_t)(e - s) * rpl::kHeldWords * 4, st),
              RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemsetAsync(ds->carry_len[p] + s, 0, (size_t)(e - s) * 4, st), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemsetAsync(cs->carry_len[p] + s, 0, (size_t)(e - s) * 4, st), RPL_RESULT_OPERATION_FAIL);
     s = e;
   }
   RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);
   return RPL_RESULT_OK;
 }
 
-rpl_result rpl_dense_stream_state(rpl_dense_stream* ds, uint32_t* open_nodes, uint32_t* held_capsule) {
-  if (!ds) return RPL_RESULT_INVALID_DATA;
-  rpl_ctx* c = ds->c;
+rpl_result rpl_capsule_stream_state(rpl_capsule_stream* cs, uint32_t* open_nodes, uint32_t* held_capsule) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  RPL_CUDA(c, cudaEventSynchronize(ds->done), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);
   if (open_nodes)
-    RPL_CUDA(c, cudaMemcpy(open_nodes, ds->carry_len[ds->parity], (size_t)ds->n_streams * 4, cudaMemcpyDeviceToHost),
+    RPL_CUDA(c, cudaMemcpy(open_nodes, cs->carry_len[cs->parity], (size_t)cs->n_streams * 4, cudaMemcpyDeviceToHost),
              RPL_RESULT_OPERATION_FAIL);
-  if (held_capsule) {
-    std::vector<uint32_t> h((size_t)ds->n_streams * rpl::kHeldWords);
-    RPL_CUDA(c, cudaMemcpy(h.data(), ds->held, h.size() * 4, cudaMemcpyDeviceToHost), RPL_RESULT_OPERATION_FAIL);
-    for (uint32_t s = 0; s < ds->n_streams; ++s) held_capsule[s] = h[(size_t)s * rpl::kHeldWords + rpl::kHeldOk];
+  if (held_capsule) {  // HQ: the record stays zero
+    std::vector<uint32_t> h((size_t)cs->n_streams * rpl::kHeldWords);
+    RPL_CUDA(c, cudaMemcpy(h.data(), cs->held, h.size() * 4, cudaMemcpyDeviceToHost), RPL_RESULT_OPERATION_FAIL);
+    for (uint32_t s = 0; s < cs->n_streams; ++s) held_capsule[s] = h[(size_t)s * rpl::kHeldWords + rpl::kHeldOk];
   }
   return RPL_RESULT_OK;
+}
+
+// ---- the dense session: the capsule session fixed to 0x85 ----
+rpl_result rpl_dense_stream_create(rpl_ctx* c, uint32_t n_streams, uint32_t stride_capsules, uint32_t max_nodes,
+                                   uint32_t max_scans, rpl_dense_stream** out) {
+  if (!c || !out) return RPL_RESULT_INVALID_DATA;
+  rpl_capsule_stream* cs = nullptr;
+  const rpl_result r = rpl_capsule_stream_create(c, 0x85, n_streams, stride_capsules, max_nodes, max_scans, &cs);
+  *out = reinterpret_cast<rpl_dense_stream*>(cs);
+  return r;
+}
+
+void rpl_dense_stream_destroy(rpl_dense_stream* ds) { rpl_capsule_stream_destroy(capsule_session(ds)); }
+
+rpl_result rpl_dense_stream_push(rpl_dense_stream* ds, const uint8_t* capsules, const uint32_t* capsule_counts,
+                                 uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
+                                 float* intensities, uint32_t* beam_counts, float* angle_increment,
+                                 uint32_t* scans_per_stream) {
+  return rpl_capsule_stream_push(capsule_session(ds), capsules, capsule_counts, sample_duration_us, params, ranges,
+                                 intensities, beam_counts, angle_increment, scans_per_stream);
+}
+
+rpl_result rpl_dense_stream_push_dev(rpl_dense_stream* ds, const uint8_t* capsules, const uint32_t* capsule_counts,
+                                     uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
+                                     float* intensities, uint32_t* beam_counts, float* angle_increment,
+                                     uint32_t* scans_per_stream, void* stream) {
+  return rpl_capsule_stream_push_dev(capsule_session(ds), capsules, capsule_counts, sample_duration_us, params, ranges,
+                                     intensities, beam_counts, angle_increment, scans_per_stream, stream);
+}
+
+rpl_result rpl_dense_stream_reset(rpl_dense_stream* ds, const uint8_t* stream_mask) {
+  return rpl_capsule_stream_reset(capsule_session(ds), stream_mask);
+}
+
+rpl_result rpl_dense_stream_state(rpl_dense_stream* ds, uint32_t* open_nodes, uint32_t* held_capsule) {
+  return rpl_capsule_stream_state(capsule_session(ds), open_nodes, held_capsule);
 }
 
 // ---- LaserScan / PointCloud2 -> CDR (SURVEY.md 8(f) rank 3) -------------------------------------

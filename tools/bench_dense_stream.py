@@ -1,10 +1,17 @@
-"""Dense stream session (rpl_dense_stream_*) timings on the GPU; prints one JSON line.
+"""Stream session timings on the GPU; prints one JSON line.
+
+With --format 0x85 (the default), the dense stream session (rpl_dense_stream_*):
 
   * per-push latency of push (host buffers, synchronous) and push_dev (device buffers, CUDA events on a torch stream)
     for 512 streams x {8, 80, 800} capsules per push: a live aggregator's receive periods of ~2.5 ms, ~25 ms, ~250 ms
     at 10 Hz, 80 capsules per revolution;
   * device-resident throughput of push_dev on the shape of bench.py --workload chain (512 streams x 4096 capsules,
     max_nodes 4096, max_scans 56), in nodes decoded per second: the figure to set next to that workload's.
+
+With --format 0x82 / 0x83 / 0x84 / 0x86, the capsule stream session (rpl_capsule_stream_*) of that format against the
+stateless device path on the same capsules (rpl_decode_capsules_batch_dev -> rpl_assemble_scan_views_dev ->
+rpl_scan_views_dev): a chain-like shape of 512 streams x about 163840 nodes per push (the chain's 4096 dense capsules
+x 40), revolutions of about 3200 nodes, max_nodes 4096, max_scans 56.
 
 Each push continues the stream where the previous one ended (the capsules of a push follow on in angle), so the carry
 and the held capsule are exercised as in a live feed.  The GPU's name and power limit are part of the output.
@@ -21,7 +28,11 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-from bench import wire_dense_capsules  # noqa: E402
+from bench import wire_dense_capsules, wire_seal_capsules  # noqa: E402
+
+# per format: bytes and nodes per capsule, capsules per push (about 163840 nodes), capsules per revolution (~3200 nodes)
+FORMATS = {0x82: (84, 32, 5120, 100.0), 0x83: (781, 96, 1707, 100.0 / 3), 0x84: (132, 96, 1707, 100.0 / 3),
+           0x86: (170, 64, 2560, 50.0)}
 
 
 def feed(n_streams, n_caps, seed=1):
@@ -37,6 +48,99 @@ def feed(n_streams, n_caps, seed=1):
     return out
 
 
+def feed_format(fmt, n_streams, n_caps, seed=1):
+    """[n_streams, n_caps, capsule bytes] of format `fmt`: random payloads, start angles (HQ: node angles and scan-start
+    flags) rising through revolutions of about 3200 nodes, every stream at its own angle"""
+    cb, per, _, cpr = FORMATS[fmt]
+    rng = np.random.default_rng(seed)
+    out = np.empty((n_streams, n_caps, cb), np.uint8)
+    for s in range(n_streams):
+        payload = rng.integers(0, 256, (n_caps, cb), dtype=np.uint8)
+        if fmt == 0x83:
+            # nodes: angle_z_q14 u16 | dist_mm_q2 u32 | quality u8 | flag u8 (scan start on each revolution's first)
+            m, npr = n_caps * per, int(round(cpr * per))
+            pos = (np.arange(m) + int(rng.integers(0, npr))) % npr
+            dist = rng.integers(4, 160000, m).astype(np.uint32)
+            w = np.empty((m, 2), np.uint32)
+            w[:, 0] = (pos * 65536 // npr).astype(np.uint32) | ((dist & 0xFFFF) << 16)
+            w[:, 1] = (dist >> 16) | (rng.integers(0, 256, m).astype(np.uint32) << 16) | \
+                (np.where(pos == 0, 1, 2).astype(np.uint32) << 24)
+            payload[:, 9:9 + 8 * per] = w.view(np.uint8).reshape(n_caps, 8 * per)
+            out[s] = wire_seal_capsules(fmt, payload)
+        else:
+            ang = (rng.uniform(0, 360) + np.arange(n_caps) * 360.0 / cpr + rng.normal(0, 0.03, n_caps)) % 360.0
+            q6 = np.round(ang * 64).astype(np.uint32) % (360 * 64)
+            out[s] = wire_seal_capsules(fmt, payload, q6, np.zeros(n_caps, bool))
+    return out
+
+
+def compare_stateless(R, torch, fmt, steps):
+    """ms per push of the session's push_dev and of the stateless device path, on the same capsules"""
+    _, per, n_caps, _ = FORMATS[fmt]
+    n_streams, max_nodes, max_scans = 512, 4096, 56
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    params = R.scan_params(1, 0, 0, 1)
+    ctx = R.Context(0, max_nodes, n_streams * max_scans)
+    caps = feed_format(fmt, 16, n_caps * 2, seed=7)
+    NS, stride_nodes = n_streams * max_scans, n_caps * per
+    res = {"format": hex(fmt), "streams": n_streams, "capsules_per_push": n_caps, "nodes_per_push_per_stream": stride_nodes,
+           "max_nodes": max_nodes, "max_scans": max_scans}
+    with torch.cuda.stream(stream):
+        halves = [torch.from_numpy(np.tile(caps[:, h * n_caps:(h + 1) * n_caps], (n_streams // 16, 1, 1))).to(dev)
+                  for h in (0, 1)]
+        d_cnt = torch.full((n_streams,), n_caps, dtype=torch.int32, device=dev)
+        r = torch.empty((NS, max_nodes), device=dev)
+        it = torch.empty((NS, max_nodes), device=dev)
+        bc = torch.zeros(NS, dtype=torch.int32, device=dev)
+        inc = torch.zeros(NS, device=dev)
+        sps = torch.zeros(n_streams, dtype=torch.int32, device=dev)
+        nodes = torch.empty(n_streams * stride_nodes, dtype=torch.int64, device=dev)
+        node_counts = torch.empty(n_streams, dtype=torch.int32, device=dev)
+        status = torch.empty(n_streams * n_caps, dtype=torch.int32, device=dev)
+        offs = torch.empty(n_streams * n_caps, dtype=torch.int32, device=dev)
+        views = torch.empty(NS, dtype=torch.int64, device=dev)
+        scan_len = torch.empty(NS, dtype=torch.int32, device=dev)
+    cs = stream.cuda_stream
+
+    def stateless(t):
+        ctx.decode_capsules_batch_dev(fmt, halves[t % 2].data_ptr(), d_cnt.data_ptr(), n_streams, n_caps, 31,
+                                      nodes.data_ptr(), node_counts.data_ptr(), capsule_status=status.data_ptr(),
+                                      capsule_node_offset=offs.data_ptr(), stream=cs)
+        ctx.assemble_scan_views_dev(nodes.data_ptr(), node_counts.data_ptr(), n_streams, stride_nodes, max_nodes,
+                                    max_scans, views.data_ptr(), scan_len.data_ptr(), sps.data_ptr(),
+                                    capsule_status=status.data_ptr(), capsule_node_offset=offs.data_ptr(),
+                                    capsule_counts=d_cnt.data_ptr(), stride_capsules=n_caps, stream=cs)
+        ctx.scan_views_dev(nodes.data_ptr(), n_streams * stride_nodes, views.data_ptr(), NS, max_nodes, params,
+                           ranges=r.data_ptr(), intensities=it.data_ptr(), beam_counts=bc.data_ptr(),
+                           angle_increment=inc.data_ptr(), stream=cs)
+
+    def timed(fn):
+        for t in range(4):
+            fn(t)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        for t in range(steps):
+            fn(t)
+        e1.record(stream)
+        stream.synchronize()
+        return e0.elapsed_time(e1) / steps
+
+    res["stateless_ms_per_push"] = timed(stateless)
+    res["stateless_scans_per_push"] = int(sps.cpu().sum())
+    with R.CapsuleStreamSession(ctx, fmt, n_streams, n_caps, max_nodes, max_scans) as sess:
+        def push(t):
+            sess.push_dev(halves[t % 2].data_ptr(), d_cnt.data_ptr(), params, r.data_ptr(), it.data_ptr(),
+                          bc.data_ptr(), inc.data_ptr(), sps.data_ptr(), stream=cs)
+
+        res["push_dev_ms_per_push"] = timed(push)
+        res["push_dev_scans_per_push"] = int(sps.cpu().sum())
+    res["push_dev_gnodes_per_s"] = n_streams * stride_nodes / (res["push_dev_ms_per_push"] * 1e-3) / 1e9
+    res["session_over_stateless"] = res["push_dev_ms_per_push"] / res["stateless_ms_per_push"] - 1.0
+    ctx.close()
+    return res
+
+
 def gpu_info():
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                        capture_output=True, text=True)
@@ -47,10 +151,16 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--pushes", type=int, default=40, help="timed pushes per latency point")
     ap.add_argument("--steps", type=int, default=20, help="timed pushes of the throughput point")
+    ap.add_argument("--format", type=lambda v: int(v, 0), default=0x85, choices=[0x82, 0x83, 0x84, 0x85, 0x86],
+                    help="capsule answer type (default 0x85: the dense session's latency and throughput points)")
     args = ap.parse_args()
     import torch
 
     import rplidar_ros2_driver_b200 as R
+
+    if args.format != 0x85:
+        print(json.dumps({"gpu": gpu_info(), "comparison": compare_stateless(R, torch, args.format, args.steps)}))
+        return
 
     dev = torch.device("cuda", 0)
     stream = torch.cuda.Stream(device=dev)

@@ -36,6 +36,7 @@
  *   rpl_capsule_stream_*     the capsule unpackers (express, HQ, ultra, dense, ultra-dense) and the ScanDataHolder
  *                              as live, per-stream state across calls: wire capsules pushed in any pieces publish the
  *                              scans of the whole stream (rpl_dense_stream_*: the same, fixed to dense capsules)
+ *   rpl_normal_stream_*      the same for the standard-node unpacker: raw 0x81 bytes pushed in any pieces
  *   rpl_*_cdr_batch_dev      the serialised form of the message scan_pub_->publish hands to the RMW layer
  *                              src/rplidar_node.cpp:679
  *   rpl_cloud_fuse_push_dev  (with rpl_peer_*) the fused cloud's all-gather across GPUs, in the pack kernel
@@ -497,6 +498,35 @@ rpl_result rpl_dense_stream_push_dev(rpl_dense_stream* s, const uint8_t* capsule
                                      uint32_t* scans_per_stream, void* stream);
 rpl_result rpl_dense_stream_reset(rpl_dense_stream* s, const uint8_t* stream_mask);
 rpl_result rpl_dense_stream_state(rpl_dense_stream* s, uint32_t* open_nodes, uint32_t* held_capsule);
+
+/* Standard-node stream session: rpl_capsule_stream_* on RAW 0x81 byte streams (the SDK's "Standard" scan mode, the
+ * only mode of the legacy A-series lidars).  Per stream the device keeps the unpacker's 0..4 bytes of an unfinished
+ * record and the open revolution, so that for ANY split of a stream's bytes into pushes -- through a record, a
+ * resynchronisation or a scan-start record -- the scans published over the pushes, in order, are the scans of the
+ * whole stream (UnpackerHandler_NormalNode and the ScanDataHolder fed the same bytes).  The standard unpacker requests
+ * no scan resets.  The first push of a fresh session publishes what rpl_decode_normal_batch_dev ->
+ * rpl_assemble_scan_views_dev -> rpl_scan_views_dev does on the same bytes.
+ *   create:  n_streams, stride_bytes (most bytes per stream in one push), max_nodes (even, <= 8192), max_scans, with
+ *            the rules of rpl_capsule_stream_create; the node arenas hold n_streams * (max_nodes + (stride_bytes + 4)
+ *            / 5 rounded up to even) nodes each, which must stay below 2^32.
+ *   push:    bytes [n_streams][stride_bytes] (any alignment), byte_counts [n_streams] (<= stride_bytes), outputs as
+ *            for rpl_capsule_stream_push.  push_dev: the same on device buffers (counts above the stride clamped).
+ *   reset:   the unpacker's reset (_cached_scan_node_buf_pos = 0) + holder reset of the masked streams (NULL = all).
+ *   state:   open_nodes as for rpl_capsule_stream_state; held_bytes [n_streams] = bytes of the unfinished record the
+ *            unpacker holds for the next push, 0..4. */
+typedef struct rpl_normal_stream rpl_normal_stream;
+rpl_result rpl_normal_stream_create(rpl_ctx* ctx, uint32_t n_streams, uint32_t stride_bytes, uint32_t max_nodes,
+                                    uint32_t max_scans, rpl_normal_stream** out);
+void rpl_normal_stream_destroy(rpl_normal_stream* s);
+rpl_result rpl_normal_stream_push(rpl_normal_stream* s, const uint8_t* bytes, const uint32_t* byte_counts,
+                                  const rpl_scan_params* params, float* ranges, float* intensities,
+                                  uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream);
+rpl_result rpl_normal_stream_push_dev(rpl_normal_stream* s, const uint8_t* bytes, const uint32_t* byte_counts,
+                                      const rpl_scan_params* params, float* ranges, float* intensities,
+                                      uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
+                                      void* stream);
+rpl_result rpl_normal_stream_reset(rpl_normal_stream* s, const uint8_t* stream_mask);
+rpl_result rpl_normal_stream_state(rpl_normal_stream* s, uint32_t* open_nodes, uint32_t* held_bytes);
 
 /* ---- LaserScan / PointCloud2 -> wire (SURVEY.md 8(f) rank 3) ---------------------------- */
 /* The serialised message the RMW layer would produce from the message the reference publishes

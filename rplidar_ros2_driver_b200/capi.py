@@ -51,6 +51,8 @@ EXPORTS = [
     "rpl_dense_stream_reset", "rpl_dense_stream_state",
     "rpl_capsule_stream_create", "rpl_capsule_stream_destroy", "rpl_capsule_stream_push", "rpl_capsule_stream_push_dev",
     "rpl_capsule_stream_reset", "rpl_capsule_stream_state",
+    "rpl_normal_stream_create", "rpl_normal_stream_destroy", "rpl_normal_stream_push", "rpl_normal_stream_push_dev",
+    "rpl_normal_stream_reset", "rpl_normal_stream_state",
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -204,6 +206,12 @@ def lib() -> C.CDLL:
         "rpl_capsule_stream_push_dev": ([vp, vp, vp, u32, PSP, vp, vp, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_reset": ([vp, vp], u32),
         "rpl_capsule_stream_state": ([vp, vp, vp], u32),
+        "rpl_normal_stream_create": ([vp, u32, u32, u32, u32, C.POINTER(vp)], u32),
+        "rpl_normal_stream_destroy": ([vp], None),
+        "rpl_normal_stream_push": ([vp, vp, vp, PSP, vp, vp, vp, vp, vp], u32),
+        "rpl_normal_stream_push_dev": ([vp, vp, vp, PSP, vp, vp, vp, vp, vp, vp], u32),
+        "rpl_normal_stream_reset": ([vp, vp], u32),
+        "rpl_normal_stream_state": ([vp, vp, vp], u32),
     }
     for name, (args, res) in sig.items():
         fn = getattr(L, name)  # AttributeError here = the library does not export the ABI
@@ -644,6 +652,41 @@ class DenseStreamSession(CapsuleStreamSession):
         self._init(ctx, 0x85, n_streams, stride_capsules, max_nodes, max_scans,
                    lambda h: ctx._L.rpl_dense_stream_create(ctx._h, n_streams, stride_capsules, max_nodes, max_scans,
                                                              C.byref(h)))
+
+
+class NormalStreamSession(CapsuleStreamSession):
+    """rpl_normal_stream wrapper: raw 0x81 standard-node byte streams pushed in any pieces, scans published as the
+    whole stream would publish them.  close, reset and state are the capsule session's; state() returns
+    (open_nodes, held_bytes), held_bytes = bytes of the unfinished record held for the next push (0..4)."""
+
+    _sym = "rpl_normal_stream"
+
+    def __init__(self, ctx: Context, n_streams: int, stride_bytes: int, max_nodes: int, max_scans: int):
+        self._L, self._ctx = ctx._L, ctx
+        h = C.c_void_p()
+        ctx._check(ctx._L.rpl_normal_stream_create(ctx._h, n_streams, stride_bytes, max_nodes, max_scans, C.byref(h)))
+        self._h = h
+        self.ans_type = 0x81
+        self.n_streams, self.stride_bytes, self.max_nodes, self.max_scans = n_streams, stride_bytes, max_nodes, max_scans
+
+    def push(self, stream_bytes, byte_counts, params: ScanParams, out=None):
+        """Host buffers: stream_bytes [n_streams, stride_bytes] uint8 -> the dict of CapsuleStreamSession.push."""
+        assert stream_bytes.dtype == np.uint8 and stream_bytes.shape == (self.n_streams, self.stride_bytes)
+        assert stream_bytes.flags.c_contiguous
+        bc = np.ascontiguousarray(byte_counts, dtype=np.uint32)
+        assert bc.shape == (self.n_streams,)
+        out = self._outputs(out)
+        self._ctx._check(self._fn("push")(
+            self._h, _p(stream_bytes), _p(bc), C.byref(params), _p(out["ranges"]), _p(out["intensities"]),
+            _p(out["beam_counts"]), _p(out["angle_increment"]), _p(out["scans_per_stream"])))
+        return out
+
+    def push_dev(self, stream_bytes, byte_counts, params: ScanParams, ranges, intensities, beam_counts,
+                 angle_increment, scans_per_stream, stream=None):
+        """Device addresses (the layouts of push), asynchronous on `stream` (None: the context's stream)."""
+        self._ctx._check(self._fn("push_dev")(
+            self._h, _p(stream_bytes), _p(byte_counts), C.byref(params), _p(ranges), _p(intensities),
+            _p(beam_counts), _p(angle_increment), _p(scans_per_stream), _p(stream)))
 
 
 EXCHANGE_NCCL, EXCHANGE_COPY = 0, 1

@@ -39,7 +39,8 @@ struct CapsuleDecodeArgs {
 // a held-capsule record, sized for the largest capsule (ultra-dense, 170 bytes): words 0..42 the capsule's bytes,
 // 43 its frame and checksum held (1) or not (0), 44 its start angle (q8), 45 the last released node's scan-start flag
 // (dense, ultra-dense), 46 the smoothed last distance (ultra-dense's _last_dist_q2).  All zero: nothing held, a fresh
-// stream.
+// stream.  The standard-node session (0x81) uses the same record for its byte machine: word 0 the last four bytes of
+// the stream so far (oldest in the low byte), 43 the machine's state (bytes of the unfinished record, 0..4).
 constexpr uint32_t kHeldCapsuleWords = 43, kHeldOk = 43, kHeldStart = 44, kHeldSync = 45, kHeldLast = 46,
                    kHeldWords = 48;
 
@@ -52,6 +53,11 @@ struct NormalDecodeArgs {
   uint32_t* node_counts;          // [n_streams]
   uint32_t* fsm_state_out;        // [n_streams] nullable: bytes buffered when the stream ended
   uint32_t* node_end;             // [n_streams][stride_bytes / 5] nullable: index of each record's last byte
+  // stream session only (node_stride != 0): the nodes go to nodes_out + s * node_stride + node_first (behind the
+  // session's carry slots), counts above stride_bytes are clamped to it, and the stream enters in the state and with
+  // the last four bytes its held record keeps (written back at the end); fsm_state_out and node_end are unused then
+  uint32_t* held;                 // [n_streams][kHeldWords], read and rewritten in place
+  uint32_t node_stride, node_first;
 };
 
 // per-sample timestamps (timestamps.cu)

@@ -885,20 +885,35 @@ __device__ __forceinline__ uint32_t compose_map(uint32_t g, uint32_t f) {
   return r;
 }
 
+// STREAM: a stream session's instantiation (NormalDecodeArgs::node_stride != 0).  The held record's state and last four
+// bytes take the place of a previous tile's (carry_state and the halo), so a record begun in an earlier push completes
+// in this one's first bytes, read through the halo like a record spanning two tiles.
+template <bool STREAM>
 __global__ void __launch_bounds__(NT, 5) decode_normal_kernel(NormalDecodeArgs a) {
   __shared__ __align__(16) NormalSmem sm;
   uint8_t* const sm_bytes = sm.raw + 12;  // bytes[0..3] = halo, bytes + 4 = the tile
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (uint32_t s = blockIdx.x; s < a.n_streams; s += gridDim.x) {
-    const uint32_t n = a.byte_counts[s];
+    const uint32_t n = STREAM ? min(a.byte_counts[s], a.stride_bytes) : a.byte_counts[s];
     const uint8_t* src = a.bytes + (size_t)s * a.stride_bytes;
-    uint2* out = a.nodes_out + (size_t)s * (a.stride_bytes / 5u);
-    uint32_t* end_out = a.node_end ? a.node_end + (size_t)s * (a.stride_bytes / 5u) : nullptr;
-    if (tid == 0) {
-      sm.carry_state = 0;
-      sm.carry_nodes = 0;
+    uint2* out = STREAM ? a.nodes_out + (size_t)s * a.node_stride + a.node_first
+                        : a.nodes_out + (size_t)s * (a.stride_bytes / 5u);
+    uint32_t* end_out = (!STREAM && a.node_end) ? a.node_end + (size_t)s * (a.stride_bytes / 5u) : nullptr;
+    if constexpr (STREAM) {
+      // all zero (a fresh stream): state 0, whose first record ends at byte 5 at the earliest, never reading the halo
+      if (tid == 0) {
+        const uint32_t* held = a.held + (size_t)s * kHeldWords;
+        sm.carry_state = held[kHeldOk];
+        sm.carry_nodes = 0;
+        *reinterpret_cast<uint32_t*>(sm_bytes) = held[0];
+      }
+    } else {
+      if (tid == 0) {
+        sm.carry_state = 0;
+        sm.carry_nodes = 0;
+      }
+      if (tid < 4) sm_bytes[tid] = 0;
     }
-    if (tid < 4) sm_bytes[tid] = 0;
     __syncthreads();
     for (uint32_t t0 = 0; t0 < n; t0 += kNormTile) {
       const uint32_t live = min((uint32_t)kNormTile, n - t0);
@@ -1020,7 +1035,16 @@ __global__ void __launch_bounds__(NT, 5) decode_normal_kernel(NormalDecodeArgs a
         if (end_out) end_out[sm.carry_nodes + q] = t0 + sm.ends[q];
       }
       __syncthreads();
-      if (tid < 4) sm_bytes[tid] = sm_bytes[live + tid];  // last four bytes of this tile (live >= 4 or stream ends)
+      if constexpr (STREAM) {
+        // the next push reads the halo, and a last tile of live < 4 bytes shifts it onto itself: every read lands
+        // before any write
+        uint8_t last = 0;
+        if (tid < 4) last = sm_bytes[live + tid];
+        __syncwarp();
+        if (tid < 4) sm_bytes[tid] = last;
+      } else {
+        if (tid < 4) sm_bytes[tid] = sm_bytes[live + tid];  // last four bytes of this tile (live >= 4 or stream ends)
+      }
       if (tid == 0) {
         sm.carry_nodes += sm.tile_nodes;
         sm.carry_state = sm.red_state;
@@ -1029,7 +1053,13 @@ __global__ void __launch_bounds__(NT, 5) decode_normal_kernel(NormalDecodeArgs a
     }
     if (tid == 0) {
       if (a.node_counts) a.node_counts[s] = sm.carry_nodes;
-      if (a.fsm_state_out) a.fsm_state_out[s] = sm.carry_state;
+      if constexpr (STREAM) {  // a stream without bytes writes back what it read
+        uint32_t* held = a.held + (size_t)s * kHeldWords;
+        held[kHeldOk] = sm.carry_state;
+        held[0] = *reinterpret_cast<const uint32_t*>(sm_bytes);
+      } else {
+        if (a.fsm_state_out) a.fsm_state_out[s] = sm.carry_state;
+      }
     }
     __syncthreads();
   }
@@ -1074,7 +1104,10 @@ cudaError_t launch_decode_capsules(uint32_t ans_type, const CapsuleDecodeArgs& a
 
 cudaError_t launch_decode_normal(const NormalDecodeArgs& a, int grid, cudaStream_t stream) {
   if (a.n_streams == 0) return cudaSuccess;
-  decode_normal_kernel<<<grid, NT, 0, stream>>>(a);
+  if (a.node_stride)
+    decode_normal_kernel<true><<<grid, NT, 0, stream>>>(a);
+  else
+    decode_normal_kernel<false><<<grid, NT, 0, stream>>>(a);
   return cudaGetLastError();
 }
 

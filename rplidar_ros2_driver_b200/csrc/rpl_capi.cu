@@ -734,6 +734,16 @@ rpl_result decode_capsules_launch(rpl_ctx* c, uint32_t ans_type, const rpl::Caps
   c->launches++;
   return RPL_RESULT_OK;
 }
+
+// one launch of the standard-node decoder on arguments the entry point has checked (n_streams > 0)
+rpl_result decode_normal_launch(rpl_ctx* c, const rpl::NormalDecodeArgs& a, void* stream) {
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
+  const int grid = (int)std::min<uint32_t>(a.n_streams, (uint32_t)c->num_sms * 8u);
+  RPL_CUDA(c, rpl::launch_decode_normal(a, grid, st), RPL_RESULT_OPERATION_FAIL);
+  c->launches++;
+  return RPL_RESULT_OK;
+}
 }  // namespace
 
 rpl_result rpl_decode_dense_batch_dev(rpl_ctx* c, const uint8_t* capsules, const uint32_t* capsule_counts,
@@ -959,8 +969,6 @@ rpl_result rpl_decode_normal_batch_dev(rpl_ctx* c, const uint8_t* bytes, const u
     return RPL_RESULT_INVALID_DATA;
   }
   if (n_streams == 0) return RPL_RESULT_OK;
-  cudaStream_t st;
-  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   rpl::NormalDecodeArgs a{};
   a.bytes = bytes;
   a.byte_counts = byte_counts;
@@ -970,10 +978,7 @@ rpl_result rpl_decode_normal_batch_dev(rpl_ctx* c, const uint8_t* bytes, const u
   a.node_counts = node_counts;
   a.fsm_state_out = fsm_state_out;
   a.node_end = node_end;
-  const int grid = (int)std::min<uint32_t>(n_streams, (uint32_t)c->num_sms * 8u);
-  RPL_CUDA(c, rpl::launch_decode_normal(a, grid, st), RPL_RESULT_OPERATION_FAIL);
-  c->launches++;
-  return RPL_RESULT_OK;
+  return decode_normal_launch(c, a, stream);
 }
 
 rpl_result rpl_decode_normal(rpl_ctx* c, const uint8_t* bytes, uint32_t n_bytes, rpl_node_hq* nodes_out,
@@ -1256,18 +1261,20 @@ rpl_result rpl_chain_dense_laserscan(rpl_ctx* c, const uint8_t* capsules, const 
 // contiguous view.  Each stream's region of an arena is [max_nodes carry slots][nodes per capsule * stride_capsules new
 // nodes]; push t decodes into arena t % 2 and its assembler writes the new open revolution into the carry slots of the
 // other arena, because the scans push t closes are read from this arena's carry slots by the scan kernels after the
-// assembler.  rpl_dense_stream is this session fixed to 0x85.
+// assembler.  rpl_dense_stream is this session fixed to 0x85.  rpl_normal_stream is this session on 0x81 standard-node
+// bytes: a push's input counts bytes instead of capsules (cap_bytes 1), the held record keeps the byte machine, and
+// there are no capsule reports (the standard unpacker requests no scan resets).
 struct rpl_capsule_stream {
   rpl_ctx* c = nullptr;
-  uint32_t ans_type = 0, cap_bytes = 0;    // answer type, bytes per capsule
-  uint32_t n_streams = 0, stride_capsules = 0, max_nodes = 0, max_scans = 0;
+  uint32_t ans_type = 0, cap_bytes = 0;    // answer type, bytes per capsule (0x81: 1)
+  uint32_t n_streams = 0, stride_capsules = 0, max_nodes = 0, max_scans = 0;  // stride_capsules: 0x81, bytes
   uint32_t stride_nodes = 0, starts_stride = 0;
   uint32_t chunk_dev = 0, chunk_host = 0;  // streams per scan launch (context's max_scans), per host-push chunk
   uint32_t parity = 0;                     // arena of the next push
   rpl_node_hq* arena[2] = {nullptr, nullptr};
   uint32_t* carry_len[2] = {nullptr, nullptr};  // [n_streams] open revolution in front of arena[p]'s new nodes
   uint32_t* held = nullptr;                     // [n_streams][kHeldWords]
-  uint32_t *status = nullptr, *offsets = nullptr, *node_counts = nullptr;
+  uint32_t *status = nullptr, *offsets = nullptr, *node_counts = nullptr;  // status, offsets: capsule formats only
   uint32_t *starts = nullptr, *start_counts = nullptr;  // dense only: the decoder's scan-start list
   uint32_t* scan_len = nullptr;
   rpl_scan_view* views = nullptr;
@@ -1278,8 +1285,9 @@ struct rpl_capsule_stream {
 
 namespace {
 
-// the dense session's handle is a capsule session's
+// the dense and standard-node sessions' handles are a capsule session's
 rpl_capsule_stream* capsule_session(rpl_dense_stream* ds) { return reinterpret_cast<rpl_capsule_stream*>(ds); }
+rpl_capsule_stream* capsule_session(rpl_normal_stream* ns) { return reinterpret_cast<rpl_capsule_stream*>(ns); }
 
 // decode -> assemble -> scan kernels for streams [s0, s0 + ns) on `st`; capsules / counts / outputs point at s0's
 rpl_result capsule_stream_chunk(rpl_capsule_stream* cs, Lane& l, cudaStream_t st, uint32_t s0, uint32_t ns,
@@ -1289,37 +1297,54 @@ rpl_result capsule_stream_chunk(rpl_capsule_stream* cs, Lane& l, cudaStream_t st
   rpl_ctx* c = cs->c;
   const uint32_t p = cs->parity, sc = cs->stride_capsules;
   rpl_node_hq* nodes = cs->arena[p] + (size_t)s0 * cs->stride_nodes;
-  uint32_t* status = cs->status + (size_t)s0 * sc;
-  uint32_t* offsets = cs->offsets + (size_t)s0 * sc;
+  // capsule formats only: the per-capsule reports, which carry the scan-reset requests to the assembler
+  uint32_t* status = cs->status ? cs->status + (size_t)s0 * sc : nullptr;
+  uint32_t* offsets = cs->offsets ? cs->offsets + (size_t)s0 * sc : nullptr;
   // only the dense decoder lists its scan starts; the assembler finds the others' with its flag pass
   uint32_t* starts = cs->starts ? cs->starts + (size_t)s0 * cs->starts_stride : nullptr;
   uint32_t* start_counts = cs->starts ? cs->start_counts + s0 : nullptr;
-  rpl::CapsuleDecodeArgs a{};
-  a.capsules = capsules;
-  a.counts = counts;
-  a.n_streams = ns;
-  a.stride_capsules = sc;
-  a.sample_duration_us = sample_duration_us;
-  a.state_words = 1;
-  a.nodes_out = reinterpret_cast<uint2*>(nodes);
-  a.node_counts = cs->node_counts + s0;
-  a.capsule_status = status;
-  a.capsule_node_offset = offsets;
-  a.scan_starts = starts;
-  a.scan_start_counts = start_counts;
-  a.starts_stride = cs->starts_stride;
-  a.held = cs->held + (size_t)s0 * rpl::kHeldWords;
-  a.node_stride = cs->stride_nodes;
-  a.node_first = cs->max_nodes;
-  rpl_result r = decode_capsules_launch(c, cs->ans_type, a, st);
+  rpl_result r;
+  if (cs->ans_type == RPL_ANS_MEASUREMENT) {
+    rpl::NormalDecodeArgs a{};
+    a.bytes = capsules;
+    a.byte_counts = counts;
+    a.n_streams = ns;
+    a.stride_bytes = sc;
+    a.nodes_out = reinterpret_cast<uint2*>(nodes);
+    a.node_counts = cs->node_counts + s0;
+    a.held = cs->held + (size_t)s0 * rpl::kHeldWords;
+    a.node_stride = cs->stride_nodes;
+    a.node_first = cs->max_nodes;
+    r = decode_normal_launch(c, a, st);
+  } else {
+    rpl::CapsuleDecodeArgs a{};
+    a.capsules = capsules;
+    a.counts = counts;
+    a.n_streams = ns;
+    a.stride_capsules = sc;
+    a.sample_duration_us = sample_duration_us;
+    a.state_words = 1;
+    a.nodes_out = reinterpret_cast<uint2*>(nodes);
+    a.node_counts = cs->node_counts + s0;
+    a.capsule_status = status;
+    a.capsule_node_offset = offsets;
+    a.scan_starts = starts;
+    a.scan_start_counts = start_counts;
+    a.starts_stride = cs->starts_stride;
+    a.held = cs->held + (size_t)s0 * rpl::kHeldWords;
+    a.node_stride = cs->stride_nodes;
+    a.node_first = cs->max_nodes;
+    r = decode_capsules_launch(c, cs->ans_type, a, st);
+  }
   if (r != RPL_RESULT_OK) return r;
   // the assembler's scratch belongs to the context: one assemble kernel at a time (as in the chain)
   if (!c->asm_done) RPL_CUDA(c, cudaEventCreateWithFlags(&c->asm_done, cudaEventDisableTiming), RPL_RESULT_OPERATION_FAIL);
   RPL_CUDA(c, cudaStreamWaitEvent(st, c->asm_done, 0), RPL_RESULT_OPERATION_FAIL);
   const size_t so = (size_t)s0 * cs->max_scans;
-  r = assemble_common(c, nodes, cs->node_counts + s0, ns, cs->stride_nodes, status, offsets, counts, sc, cs->max_nodes,
-                      cs->max_scans, cs->max_nodes, nullptr, cs->views + so, cs->scan_len + so, scans_per_stream, nullptr,
-                      nullptr, st, starts, starts ? cs->starts_stride : 0u, start_counts, cs->carry_len[p] + s0,
+  r = assemble_common(c, nodes, cs->node_counts + s0, ns, cs->stride_nodes, status, offsets, status ? counts : nullptr,
+                      status ? sc : 0u, cs->max_nodes, cs->max_scans, cs->max_nodes, nullptr, cs->views + so,
+                      cs->scan_len + so, scans_per_stream, nullptr, nullptr, st, starts,
+                      starts ? cs->starts_stride : 0u, start_counts, cs->carry_len[p] + s0,
                       cs->arena[p ^ 1u] + (size_t)s0 * cs->stride_nodes, cs->carry_len[p ^ 1u] + s0);
   if (r != RPL_RESULT_OK) return r;
   RPL_CUDA(c, cudaEventRecord(c->asm_done, st), RPL_RESULT_OPERATION_FAIL);
@@ -1336,7 +1361,8 @@ bool capsule_stream_args_ok(rpl_capsule_stream* cs, const uint8_t* capsules, con
     c->err = "null capsules, counts, params or output buffer";
     return false;
   }
-  if (!sample_duration_ok(c, sample_duration_us)) return false;
+  // the standard decoder takes no sample duration (it tests no jump between capsules)
+  if (cs->ans_type != RPL_ANS_MEASUREMENT && !sample_duration_ok(c, sample_duration_us)) return false;
   // the alignment rule of rpl_decode_capsules_batch_dev: only dense capsules are read in 4-byte words
   if (cs->ans_type == 0x85 && (reinterpret_cast<uintptr_t>(capsules) & 3u) != 0) {
     c->err = "capsule buffer must be 4-byte aligned";
@@ -1345,31 +1371,32 @@ bool capsule_stream_args_ok(rpl_capsule_stream* cs, const uint8_t* capsules, con
   return true;
 }
 
-}  // namespace
-
-extern "C" {
-
-rpl_result rpl_capsule_stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint32_t stride_capsules,
-                                     uint32_t max_nodes, uint32_t max_scans, rpl_capsule_stream** out) {
-  if (!c || !out) return RPL_RESULT_INVALID_DATA;
-  *out = nullptr;
-  const uint32_t cap_bytes = rpl_capsule_bytes(ans_type), cap_nodes = rpl_capsule_nodes(ans_type);
-  if (cap_bytes == 0) {
-    c->err = "a stream session takes the capsule answer types 0x82..0x86 (0x81 standard nodes are no capsules)";
-    return RPL_RESULT_INVALID_DATA;
-  }
+// a session of a capsule answer type or of 0x81 standard nodes (the caller has checked ans_type); stride_capsules
+// counts bytes for 0x81
+rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint32_t stride_capsules,
+                         uint32_t max_nodes, uint32_t max_scans, rpl_capsule_stream** out) {
+  const bool normal = ans_type == RPL_ANS_MEASUREMENT;
+  const uint32_t cap_bytes = normal ? 1u : rpl_capsule_bytes(ans_type);
   if (n_streams == 0 || stride_capsules == 0 || max_scans == 0 || max_nodes == 0 || max_nodes > rpl::kSmallMaxNodes ||
       (max_nodes & 1u)) {
-    c->err = "need n_streams > 0, stride_capsules > 0, max_scans > 0 and an even max_nodes in [2, 8192]";
+    c->err = normal ? "need n_streams > 0, stride_bytes > 0, max_scans > 0 and an even max_nodes in [2, 8192]"
+                    : "need n_streams > 0, stride_capsules > 0, max_scans > 0 and an even max_nodes in [2, 8192]";
     return RPL_RESULT_INVALID_DATA;
   }
   if (max_scans > c->max_scans) {
     c->err = "the context's max_scans is smaller than max_scans of one stream";
     return RPL_RESULT_INVALID_DATA;
   }
-  const unsigned long long stride_nodes = (unsigned long long)max_nodes + (unsigned long long)cap_nodes * stride_capsules;
+  // 0x81: a push of n bytes completes up to (n + 4) / 5 records with the up to 4 bytes held before it; rounded up to
+  // even, as every capsule format's node count is, so that every region stays 16-byte aligned
+  const unsigned long long new_nodes = normal ? (((unsigned long long)stride_capsules + 4) / 5 + 1) & ~1ull
+                                              : (unsigned long long)rpl_capsule_nodes(ans_type) * stride_capsules;
+  const unsigned long long stride_nodes = (unsigned long long)max_nodes + new_nodes;
   if (stride_nodes * n_streams > 0xFFFFFFFFull) {
-    c->err = "n_streams * (max_nodes + nodes per capsule * stride_capsules) must stay below 2^32 (32-bit scan views)";
+    c->err = normal ? "n_streams * (max_nodes + (stride_bytes + 4) / 5 rounded up to even) must stay below 2^32 "
+                      "(32-bit scan views)"
+                    : "n_streams * (max_nodes + nodes per capsule * stride_capsules) must stay below 2^32 (32-bit scan "
+                      "views)";
     return RPL_RESULT_INVALID_DATA;
   }
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
@@ -1413,9 +1440,11 @@ rpl_result rpl_capsule_stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_s
   if (ans_type == 0x85 && (!cuda_ok(c, dev_alloc(&cs->starts, n * cs->starts_stride), "cudaMalloc") ||
                            !cuda_ok(c, dev_alloc(&cs->start_counts, n), "cudaMalloc")))
     return fail(oom);
+  if (!normal && (!cuda_ok(c, dev_alloc(&cs->status, ncap), "cudaMalloc") ||
+                  !cuda_ok(c, dev_alloc(&cs->offsets, ncap), "cudaMalloc")))
+    return fail(oom);
   if (!cuda_ok(c, dev_alloc(&cs->held, n * rpl::kHeldWords), "cudaMalloc") ||
       !cuda_ok(c, cudaMemset(cs->held, 0, n * rpl::kHeldWords * 4), "cudaMemset") ||
-      !cuda_ok(c, dev_alloc(&cs->status, ncap), "cudaMalloc") || !cuda_ok(c, dev_alloc(&cs->offsets, ncap), "cudaMalloc") ||
       !cuda_ok(c, dev_alloc(&cs->node_counts, n), "cudaMalloc") ||
       !cuda_ok(c, dev_alloc(&cs->scan_len, n * max_scans), "cudaMalloc") ||
       !cuda_ok(c, dev_alloc(&cs->views, n * max_scans), "cudaMalloc") ||
@@ -1424,6 +1453,21 @@ rpl_result rpl_capsule_stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_s
     return fail(oom);
   *out = cs;
   return RPL_RESULT_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+rpl_result rpl_capsule_stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint32_t stride_capsules,
+                                     uint32_t max_nodes, uint32_t max_scans, rpl_capsule_stream** out) {
+  if (!c || !out) return RPL_RESULT_INVALID_DATA;
+  *out = nullptr;
+  if (rpl_capsule_bytes(ans_type) == 0) {
+    c->err = "a stream session takes the capsule answer types 0x82..0x86 (0x81 standard nodes are no capsules)";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  return stream_create(c, ans_type, n_streams, stride_capsules, max_nodes, max_scans, out);
 }
 
 void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
@@ -1459,7 +1503,8 @@ rpl_result rpl_capsule_stream_push(rpl_capsule_stream* cs, const uint8_t* capsul
     return RPL_RESULT_INVALID_DATA;
   for (uint32_t s = 0; s < cs->n_streams; ++s)
     if (capsule_counts[s] > cs->stride_capsules) {
-      c->err = "capsule_counts[s] exceeds stride_capsules";
+      c->err = cs->ans_type == RPL_ANS_MEASUREMENT ? "byte_counts[s] exceeds stride_bytes"
+                                                   : "capsule_counts[s] exceeds stride_capsules";
       return RPL_RESULT_INVALID_DATA;
     }
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
@@ -1555,7 +1600,7 @@ rpl_result rpl_capsule_stream_state(rpl_capsule_stream* cs, uint32_t* open_nodes
   if (open_nodes)
     RPL_CUDA(c, cudaMemcpy(open_nodes, cs->carry_len[cs->parity], (size_t)cs->n_streams * 4, cudaMemcpyDeviceToHost),
              RPL_RESULT_OPERATION_FAIL);
-  if (held_capsule) {  // HQ: the record stays zero
+  if (held_capsule) {  // HQ: the record stays zero; 0x81: the byte machine's state, 0..4 bytes held
     std::vector<uint32_t> h((size_t)cs->n_streams * rpl::kHeldWords);
     RPL_CUDA(c, cudaMemcpy(h.data(), cs->held, h.size() * 4, cudaMemcpyDeviceToHost), RPL_RESULT_OPERATION_FAIL);
     for (uint32_t s = 0; s < cs->n_streams; ++s) held_capsule[s] = h[(size_t)s * rpl::kHeldWords + rpl::kHeldOk];
@@ -1597,6 +1642,41 @@ rpl_result rpl_dense_stream_reset(rpl_dense_stream* ds, const uint8_t* stream_ma
 
 rpl_result rpl_dense_stream_state(rpl_dense_stream* ds, uint32_t* open_nodes, uint32_t* held_capsule) {
   return rpl_capsule_stream_state(capsule_session(ds), open_nodes, held_capsule);
+}
+
+// ---- the standard-node session: the capsule session on 0x81 bytes ----
+rpl_result rpl_normal_stream_create(rpl_ctx* c, uint32_t n_streams, uint32_t stride_bytes, uint32_t max_nodes,
+                                    uint32_t max_scans, rpl_normal_stream** out) {
+  if (!c || !out) return RPL_RESULT_INVALID_DATA;
+  rpl_capsule_stream* cs = nullptr;
+  const rpl_result r = stream_create(c, RPL_ANS_MEASUREMENT, n_streams, stride_bytes, max_nodes, max_scans, &cs);
+  *out = reinterpret_cast<rpl_normal_stream*>(cs);
+  return r;
+}
+
+void rpl_normal_stream_destroy(rpl_normal_stream* ns) { rpl_capsule_stream_destroy(capsule_session(ns)); }
+
+rpl_result rpl_normal_stream_push(rpl_normal_stream* ns, const uint8_t* bytes, const uint32_t* byte_counts,
+                                  const rpl_scan_params* params, float* ranges, float* intensities,
+                                  uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream) {
+  return rpl_capsule_stream_push(capsule_session(ns), bytes, byte_counts, 0, params, ranges, intensities, beam_counts,
+                                 angle_increment, scans_per_stream);
+}
+
+rpl_result rpl_normal_stream_push_dev(rpl_normal_stream* ns, const uint8_t* bytes, const uint32_t* byte_counts,
+                                      const rpl_scan_params* params, float* ranges, float* intensities,
+                                      uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
+                                      void* stream) {
+  return rpl_capsule_stream_push_dev(capsule_session(ns), bytes, byte_counts, 0, params, ranges, intensities,
+                                     beam_counts, angle_increment, scans_per_stream, stream);
+}
+
+rpl_result rpl_normal_stream_reset(rpl_normal_stream* ns, const uint8_t* stream_mask) {
+  return rpl_capsule_stream_reset(capsule_session(ns), stream_mask);
+}
+
+rpl_result rpl_normal_stream_state(rpl_normal_stream* ns, uint32_t* open_nodes, uint32_t* held_bytes) {
+  return rpl_capsule_stream_state(capsule_session(ns), open_nodes, held_bytes);
 }
 
 // ---- LaserScan / PointCloud2 -> CDR (SURVEY.md 8(f) rank 3) -------------------------------------

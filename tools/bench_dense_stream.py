@@ -13,6 +13,12 @@ stateless device path on the same capsules (rpl_decode_capsules_batch_dev -> rpl
 rpl_scan_views_dev): a chain-like shape of 512 streams x about 163840 nodes per push (the chain's 4096 dense capsules
 x 40), revolutions of about 3200 nodes, max_nodes 4096, max_scans 56.
 
+With --format 0x81, the standard-node stream session (rpl_normal_stream_*) on raw byte streams: the same comparison
+against the stateless device path (rpl_decode_normal_batch_dev -> rpl_assemble_scan_views_dev -> rpl_scan_views_dev) on
+512 streams x 163840 five-byte records per push, revolutions of 3200 records, max_nodes 4096, max_scans 56; and the
+per-push latency of push and push_dev for 512 streams x {100, 1000, 10000} bytes (at 115200 baud a standard-mode lidar
+delivers about 11500 bytes per second).
+
 Each push continues the stream where the previous one ended (the capsules of a push follow on in angle), so the carry
 and the held capsule are exercised as in a live feed.  The GPU's name and power limit are part of the output.
 """
@@ -74,6 +80,148 @@ def feed_format(fmt, n_streams, n_caps, seed=1):
     return out
 
 
+def feed_normal(n_streams, n_bytes, seed=1):
+    """[n_streams, n_bytes] of 0x81 records: angles rising through revolutions of 3200 records whose first carries the
+    sync bit, 5 % zero distances, every stream at its own angle; a push may end inside a record"""
+    rng = np.random.default_rng(seed)
+    n_rec = (n_bytes + 4) // 5
+    out = np.empty((n_streams, n_rec * 5), np.uint8)
+    for s in range(n_streams):
+        pos = (np.arange(n_rec) + int(rng.integers(0, 3200))) % 3200
+        start = (pos == 0).astype(np.uint8)
+        rec = out[s].reshape(n_rec, 5)
+        rec[:, 0] = (rng.integers(0, 64, n_rec).astype(np.uint8) << 2) | ((1 - start) << 1) | start
+        w = ((pos * (360 * 64) // 3200) << 1) | 1
+        rec[:, 1], rec[:, 2] = w & 0xFF, w >> 8
+        dist = rng.integers(4, 65536, n_rec)
+        dist[rng.random(n_rec) < 0.05] = 0
+        rec[:, 3], rec[:, 4] = dist & 0xFF, dist >> 8
+    return out[:, :n_bytes]
+
+
+def compare_normal(R, torch, steps):
+    """ms per push of the standard-node session's push_dev and of the stateless device path, on the same bytes"""
+    n_streams, n_bytes, max_nodes, max_scans = 512, 163840 * 5, 4096, 56
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    params = R.scan_params(1, 0, 0, 1)
+    ctx = R.Context(0, max_nodes, n_streams * max_scans)
+    feed_ = feed_normal(16, 2 * n_bytes, seed=7)
+    NS, stride_nodes = n_streams * max_scans, n_bytes // 5
+    res = {"format": "0x81", "streams": n_streams, "bytes_per_push": n_bytes, "nodes_per_push_per_stream": stride_nodes,
+           "max_nodes": max_nodes, "max_scans": max_scans}
+    with torch.cuda.stream(stream):
+        halves = [torch.from_numpy(np.ascontiguousarray(feed_[:, h * n_bytes:(h + 1) * n_bytes])).to(dev)
+                  .repeat(n_streams // 16, 1) for h in (0, 1)]
+        d_cnt = torch.full((n_streams,), n_bytes, dtype=torch.int32, device=dev)
+        r = torch.empty((NS, max_nodes), device=dev)
+        it = torch.empty((NS, max_nodes), device=dev)
+        bc = torch.zeros(NS, dtype=torch.int32, device=dev)
+        inc = torch.zeros(NS, device=dev)
+        sps = torch.zeros(n_streams, dtype=torch.int32, device=dev)
+        nodes = torch.empty(n_streams * stride_nodes, dtype=torch.int64, device=dev)
+        node_counts = torch.empty(n_streams, dtype=torch.int32, device=dev)
+        views = torch.empty(NS, dtype=torch.int64, device=dev)
+        scan_len = torch.empty(NS, dtype=torch.int32, device=dev)
+    cs = stream.cuda_stream
+
+    def stateless(t):
+        ctx.decode_normal_batch_dev(halves[t % 2].data_ptr(), d_cnt.data_ptr(), n_streams, n_bytes, nodes.data_ptr(),
+                                    node_counts.data_ptr(), stream=cs)
+        ctx.assemble_scan_views_dev(nodes.data_ptr(), node_counts.data_ptr(), n_streams, stride_nodes, max_nodes,
+                                    max_scans, views.data_ptr(), scan_len.data_ptr(), sps.data_ptr(), stream=cs)
+        ctx.scan_views_dev(nodes.data_ptr(), n_streams * stride_nodes, views.data_ptr(), NS, max_nodes, params,
+                           ranges=r.data_ptr(), intensities=it.data_ptr(), beam_counts=bc.data_ptr(),
+                           angle_increment=inc.data_ptr(), stream=cs)
+
+    res["stateless_ms_per_push"] = timed(torch, stream, stateless, steps)
+    res["stateless_scans_per_push"] = int(sps.cpu().sum())
+    with R.NormalStreamSession(ctx, n_streams, n_bytes, max_nodes, max_scans) as sess:
+        def push(t):
+            sess.push_dev(halves[t % 2].data_ptr(), d_cnt.data_ptr(), params, r.data_ptr(), it.data_ptr(),
+                          bc.data_ptr(), inc.data_ptr(), sps.data_ptr(), stream=cs)
+
+        res["push_dev_ms_per_push"] = timed(torch, stream, push, steps)
+        res["push_dev_scans_per_push"] = int(sps.cpu().sum())
+    res["push_dev_gnodes_per_s"] = n_streams * stride_nodes / (res["push_dev_ms_per_push"] * 1e-3) / 1e9
+    res["session_over_stateless"] = res["push_dev_ms_per_push"] / res["stateless_ms_per_push"] - 1.0
+    ctx.close()
+    return res
+
+
+def normal_latency(R, torch, pushes):
+    """per-push latency of the standard-node session for 512 streams x {100, 1000, 10000} bytes per push"""
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    params = R.scan_params(1, 0, 0, 1)
+    n_streams, max_nodes, max_scans = 512, 4096, 16
+    rep = n_streams // 16
+    ctx = R.Context(0, max_nodes, n_streams * max_scans)
+    rows = []
+    for per in (100, 1000, 10000):
+        feed_ = feed_normal(16, per * (pushes + 4), seed=per)
+        counts = np.full(n_streams, per, np.uint32)
+        row = {"streams": n_streams, "bytes_per_push": per}
+        with R.NormalStreamSession(ctx, n_streams, per, max_nodes, max_scans) as sess:
+            pin = torch.empty((n_streams, per), dtype=torch.uint8).pin_memory().numpy()
+            out = pinned_outputs(torch, n_streams, max_nodes, max_scans)
+            ts = []
+            for t in range(pushes + 4):
+                pin[:] = np.tile(feed_[:, t * per:(t + 1) * per], (rep, 1))
+                t0 = time.perf_counter()
+                sess.push(pin, counts, params, out=out)
+                ts.append(time.perf_counter() - t0)
+            ts = np.array(ts[4:]) * 1e3
+            row["push_ms_median"], row["push_ms_p90"] = float(np.median(ts)), float(np.percentile(ts, 90))
+        with R.NormalStreamSession(ctx, n_streams, per, max_nodes, max_scans) as sess, torch.cuda.stream(stream):
+            d_feed = torch.from_numpy(feed_).to(dev)
+            d_cnt = torch.full((n_streams,), per, dtype=torch.int32, device=dev)
+            NS = n_streams * max_scans
+            r = torch.empty((NS, max_nodes), device=dev)
+            it = torch.empty((NS, max_nodes), device=dev)
+            bc = torch.zeros(NS, dtype=torch.int32, device=dev)
+            inc = torch.zeros(NS, device=dev)
+            sps = torch.zeros(n_streams, dtype=torch.int32, device=dev)
+            evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(pushes + 4)]
+            for t in range(pushes + 4):
+                piece = d_feed[:, t * per:(t + 1) * per].repeat(rep, 1)
+                evs[t][0].record(stream)
+                sess.push_dev(piece.data_ptr(), d_cnt.data_ptr(), params, r.data_ptr(), it.data_ptr(), bc.data_ptr(),
+                              inc.data_ptr(), sps.data_ptr(), stream=stream.cuda_stream)
+                evs[t][1].record(stream)
+            stream.synchronize()
+            ms = np.array([a.elapsed_time(b) for a, b in evs[4:]])
+            row["push_dev_ms_median"], row["push_dev_ms_p90"] = float(np.median(ms)), float(np.percentile(ms, 90))
+        rows.append(row)
+    ctx.close()
+    return rows
+
+
+def pinned_outputs(torch, n_streams, max_nodes, max_scans):
+    """the output dict of push in pinned host memory, as an aggregator would keep it"""
+    out = {k: torch.zeros(shape, dtype=dt).pin_memory().numpy() for k, shape, dt in (
+        ("ranges", (n_streams * max_scans, max_nodes), torch.float32),
+        ("intensities", (n_streams * max_scans, max_nodes), torch.float32),
+        ("beam_counts", (n_streams * max_scans,), torch.int32), ("angle_increment", (n_streams * max_scans,), torch.float32),
+        ("scans_per_stream", (n_streams,), torch.int32))}
+    out["beam_counts"] = out["beam_counts"].view(np.uint32)
+    out["scans_per_stream"] = out["scans_per_stream"].view(np.uint32)
+    return out
+
+
+def timed(torch, stream, fn, steps):
+    """ms per call of fn(t) on `stream`, CUDA events around `steps` calls after 4 warm-up calls"""
+    for t in range(4):
+        fn(t)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(stream)
+    for t in range(steps):
+        fn(t)
+    e1.record(stream)
+    stream.synchronize()
+    return e0.elapsed_time(e1) / steps
+
+
 def compare_stateless(R, torch, fmt, steps):
     """ms per push of the session's push_dev and of the stateless device path, on the same capsules"""
     _, per, n_caps, _ = FORMATS[fmt]
@@ -115,25 +263,14 @@ def compare_stateless(R, torch, fmt, steps):
                            ranges=r.data_ptr(), intensities=it.data_ptr(), beam_counts=bc.data_ptr(),
                            angle_increment=inc.data_ptr(), stream=cs)
 
-    def timed(fn):
-        for t in range(4):
-            fn(t)
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record(stream)
-        for t in range(steps):
-            fn(t)
-        e1.record(stream)
-        stream.synchronize()
-        return e0.elapsed_time(e1) / steps
-
-    res["stateless_ms_per_push"] = timed(stateless)
+    res["stateless_ms_per_push"] = timed(torch, stream, stateless, steps)
     res["stateless_scans_per_push"] = int(sps.cpu().sum())
     with R.CapsuleStreamSession(ctx, fmt, n_streams, n_caps, max_nodes, max_scans) as sess:
         def push(t):
             sess.push_dev(halves[t % 2].data_ptr(), d_cnt.data_ptr(), params, r.data_ptr(), it.data_ptr(),
                           bc.data_ptr(), inc.data_ptr(), sps.data_ptr(), stream=cs)
 
-        res["push_dev_ms_per_push"] = timed(push)
+        res["push_dev_ms_per_push"] = timed(torch, stream, push, steps)
         res["push_dev_scans_per_push"] = int(sps.cpu().sum())
     res["push_dev_gnodes_per_s"] = n_streams * stride_nodes / (res["push_dev_ms_per_push"] * 1e-3) / 1e9
     res["session_over_stateless"] = res["push_dev_ms_per_push"] / res["stateless_ms_per_push"] - 1.0
@@ -151,13 +288,17 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--pushes", type=int, default=40, help="timed pushes per latency point")
     ap.add_argument("--steps", type=int, default=20, help="timed pushes of the throughput point")
-    ap.add_argument("--format", type=lambda v: int(v, 0), default=0x85, choices=[0x82, 0x83, 0x84, 0x85, 0x86],
-                    help="capsule answer type (default 0x85: the dense session's latency and throughput points)")
+    ap.add_argument("--format", type=lambda v: int(v, 0), default=0x85, choices=[0x81, 0x82, 0x83, 0x84, 0x85, 0x86],
+                    help="answer type (default 0x85: the dense session's latency and throughput points)")
     args = ap.parse_args()
     import torch
 
     import rplidar_ros2_driver_b200 as R
 
+    if args.format == 0x81:
+        print(json.dumps({"gpu": gpu_info(), "comparison": compare_normal(R, torch, args.steps),
+                          "latency": normal_latency(R, torch, args.pushes)}))
+        return
     if args.format != 0x85:
         print(json.dumps({"gpu": gpu_info(), "comparison": compare_stateless(R, torch, args.format, args.steps)}))
         return
@@ -176,13 +317,7 @@ def main():
         # host buffers: wall clock around the synchronous call (pinned buffers, as an aggregator would keep them)
         with R.DenseStreamSession(ctx, n_streams, per, max_nodes, max_scans) as sess:
             pin = torch.empty((n_streams, per, 84), dtype=torch.uint8).pin_memory().numpy()
-            out = {k: torch.zeros(shape, dtype=dt).pin_memory().numpy() for k, shape, dt in (
-                ("ranges", (n_streams * max_scans, max_nodes), torch.float32),
-                ("intensities", (n_streams * max_scans, max_nodes), torch.float32),
-                ("beam_counts", (n_streams * max_scans,), torch.int32), ("angle_increment", (n_streams * max_scans,), torch.float32),
-                ("scans_per_stream", (n_streams,), torch.int32))}
-            out["beam_counts"] = out["beam_counts"].view(np.uint32)
-            out["scans_per_stream"] = out["scans_per_stream"].view(np.uint32)
+            out = pinned_outputs(torch, n_streams, max_nodes, max_scans)
             ts = []
             for t in range(args.pushes + 4):
                 pin[:] = np.tile(caps[:, t * per:(t + 1) * per], (rep, 1, 1))

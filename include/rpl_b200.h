@@ -193,7 +193,7 @@ rpl_result rpl_cloud_batch(rpl_ctx* ctx, const rpl_node_hq* nodes, const uint32_
                            float* xyzi, uint32_t* point_counts);
 /* Packs the per-scan clouds of a batch into one dense cloud (the per-GPU "fused cloud" that
  * is all-gathered across ranks): fused[0..*total) points, 16 B each; offsets[s] = first point
- * of scan s.  fused must hold n_scans*stride points. */
+ * of scan s.  fused must hold n_scans*stride points.  n_scans == 0 is an empty cloud: *total = 0. */
 rpl_result rpl_cloud_fuse_dev(rpl_ctx* ctx, const float* xyzi, const uint32_t* point_counts,
                               uint32_t n_scans, uint32_t stride, float* fused, uint32_t* offsets,
                               uint32_t* total, void* stream);
@@ -238,7 +238,9 @@ rpl_result rpl_cloud_fuse_push_dev(rpl_ctx* ctx, const float* xyzi, const uint32
  * `stream` is NOT made to wait for the transfer: the caller's next batch overlaps it.  *buffer_index (0/1) names
  * the buffer this step fills; a consumer calls rpl_exchange_wait(index, its stream) before reading the slots
  * (rpl_exchange_slot) and rpl_exchange_release(index, its stream) after its last read -- the exchange that reuses
- * the buffer two steps later waits for that.  A slot whose count exceeds slot_points overflowed (points dropped). */
+ * the buffer two steps later waits for that.  A slot whose count exceeds slot_points overflowed (points dropped).
+ * A step with n_scans == 0 (a rank with no streams, or none that closed a revolution) publishes an empty slot:
+ * count 0; rpl_cloud_fuse_push_dev likewise writes 0 into header word `rank` of every peer. */
 #define RPL_EXCHANGE_ID_BYTES 128u
 #define RPL_EXCHANGE_NCCL 0u
 #define RPL_EXCHANGE_COPY 1u

@@ -37,6 +37,7 @@
  *                              as live, per-stream state across calls: wire capsules pushed in any pieces publish the
  *                              scans of the whole stream (rpl_dense_stream_*: the same, fixed to dense capsules)
  *   rpl_normal_stream_*      the same for the standard-node unpacker: raw 0x81 bytes pushed in any pieces
+ *   rpl_*_stream_push_ts*    a session push that also stamps every published scan with its scan-begin time
  *   rpl_*_cdr_batch_dev      the serialised form of the message scan_pub_->publish hands to the RMW layer
  *                              src/rplidar_node.cpp:679
  *   rpl_cloud_fuse_push_dev  (with rpl_peer_*) the fused cloud's all-gather across GPUs, in the pack kernel
@@ -467,7 +468,21 @@ rpl_result rpl_chain_dense_laserscan(rpl_ctx* ctx, const uint8_t* capsules, cons
  *            non-zero (NULL = all).
  *   state:   synchronous; open_nodes [n_streams] = nodes in each stream's open revolution (capped at max_nodes),
  *            held_capsule [n_streams] = 1 when a valid capsule is held for the next push (always 0 for HQ, which holds
- *            nothing); either pointer nullable. */
+ *            nothing); either pointer nullable.
+ *   push_ts / push_ts_dev: a stamped push.  push / push_dev with the receive time of every capsule, capsule_rx_us
+ *            [n_streams][stride_capsules] (the time of the read that delivered the capsule's last byte, when the
+ *            SDK's unpacker calls getCurrentTimestamp_uS), and the timing of rpl_node_timestamps_dev, whose
+ *            sample_duration_us the decoder takes.  Also returns scan_begin_ts_us [n_streams * max_scans] (slots as
+ *            beam_counts, unused ones 0): the stamp of the scan-start node that opened each published scan, the
+ *            holder's _scan_begin_timestamp_uS (sl_lidar_driver.cpp:293).  For any split into pushes the stamps
+ *            published over the pushes, in order, are those of the whole stream (rpl_node_timestamps_dev ->
+ *            rpl_assemble_scans_dev on the concatenation).  A scan opened pushes ago keeps its stamp; for express and
+ *            ultra, a scan-start node in a capsule held over a push counts from the held capsule's receive time.
+ *            Stamped and unstamped pushes mix on one session (an unstamped push runs exactly the unstamped kernels and
+ *            keeps no stamp), so a stamp that depends on a receive time the session was not given or did not keep is
+ *            reported as 0: a scan opened in an unstamped push or still open across one, or (express, ultra) opened
+ *            by a node of a capsule an unstamped push held.  Null timing, receive times or scan_begin_ts_us, or 8-byte
+ *            buffers not 8-byte aligned: RPL_RESULT_INVALID_DATA. */
 typedef struct rpl_capsule_stream rpl_capsule_stream;
 rpl_result rpl_capsule_stream_create(rpl_ctx* ctx, uint32_t ans_type, uint32_t n_streams, uint32_t stride_capsules,
                                      uint32_t max_nodes, uint32_t max_scans, rpl_capsule_stream** out);
@@ -480,6 +495,16 @@ rpl_result rpl_capsule_stream_push_dev(rpl_capsule_stream* s, const uint8_t* cap
                                        uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
                                        float* intensities, uint32_t* beam_counts, float* angle_increment,
                                        uint32_t* scans_per_stream, void* stream);
+rpl_result rpl_capsule_stream_push_ts(rpl_capsule_stream* s, const uint8_t* capsules, const uint32_t* capsule_counts,
+                                      const rpl_timing* timing, const uint64_t* capsule_rx_us,
+                                      const rpl_scan_params* params, float* ranges, float* intensities,
+                                      uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
+                                      uint64_t* scan_begin_ts_us);
+rpl_result rpl_capsule_stream_push_ts_dev(rpl_capsule_stream* s, const uint8_t* capsules,
+                                          const uint32_t* capsule_counts, const rpl_timing* timing,
+                                          const uint64_t* capsule_rx_us, const rpl_scan_params* params, float* ranges,
+                                          float* intensities, uint32_t* beam_counts, float* angle_increment,
+                                          uint32_t* scans_per_stream, uint64_t* scan_begin_ts_us, void* stream);
 rpl_result rpl_capsule_stream_reset(rpl_capsule_stream* s, const uint8_t* stream_mask);
 rpl_result rpl_capsule_stream_state(rpl_capsule_stream* s, uint32_t* open_nodes, uint32_t* held_capsule);
 
@@ -498,6 +523,16 @@ rpl_result rpl_dense_stream_push_dev(rpl_dense_stream* s, const uint8_t* capsule
                                      uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
                                      float* intensities, uint32_t* beam_counts, float* angle_increment,
                                      uint32_t* scans_per_stream, void* stream);
+rpl_result rpl_dense_stream_push_ts(rpl_dense_stream* s, const uint8_t* capsules, const uint32_t* capsule_counts,
+                                    const rpl_timing* timing, const uint64_t* capsule_rx_us,
+                                    const rpl_scan_params* params, float* ranges, float* intensities,
+                                    uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
+                                    uint64_t* scan_begin_ts_us);
+rpl_result rpl_dense_stream_push_ts_dev(rpl_dense_stream* s, const uint8_t* capsules, const uint32_t* capsule_counts,
+                                        const rpl_timing* timing, const uint64_t* capsule_rx_us,
+                                        const rpl_scan_params* params, float* ranges, float* intensities,
+                                        uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
+                                        uint64_t* scan_begin_ts_us, void* stream);
 rpl_result rpl_dense_stream_reset(rpl_dense_stream* s, const uint8_t* stream_mask);
 rpl_result rpl_dense_stream_state(rpl_dense_stream* s, uint32_t* open_nodes, uint32_t* held_capsule);
 
@@ -515,7 +550,11 @@ rpl_result rpl_dense_stream_state(rpl_dense_stream* s, uint32_t* open_nodes, uin
  *            for rpl_capsule_stream_push.  push_dev: the same on device buffers (counts above the stride clamped).
  *   reset:   the unpacker's reset (_cached_scan_node_buf_pos = 0) + holder reset of the masked streams (NULL = all).
  *   state:   open_nodes as for rpl_capsule_stream_state; held_bytes [n_streams] = bytes of the unfinished record the
- *            unpacker holds for the next push, 0..4. */
+ *            unpacker holds for the next push, 0..4.
+ *   push_ts / push_ts_dev: a stamped push, as rpl_capsule_stream_push_ts: chunk_rx_us [n_streams][ceil(stride_bytes /
+ *            chunk_bytes)], chunk c the receive time of bytes [c * chunk_bytes, (c + 1) * chunk_bytes) of THIS push (the
+ *            rule of rpl_normal_timestamps_dev); a record is stamped by the chunk holding its last byte, also when it
+ *            began in an earlier push.  chunk_bytes == 0: RPL_RESULT_INVALID_DATA. */
 typedef struct rpl_normal_stream rpl_normal_stream;
 rpl_result rpl_normal_stream_create(rpl_ctx* ctx, uint32_t n_streams, uint32_t stride_bytes, uint32_t max_nodes,
                                     uint32_t max_scans, rpl_normal_stream** out);
@@ -527,6 +566,16 @@ rpl_result rpl_normal_stream_push_dev(rpl_normal_stream* s, const uint8_t* bytes
                                       const rpl_scan_params* params, float* ranges, float* intensities,
                                       uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
                                       void* stream);
+rpl_result rpl_normal_stream_push_ts(rpl_normal_stream* s, const uint8_t* bytes, const uint32_t* byte_counts,
+                                     const rpl_timing* timing, uint32_t chunk_bytes, const uint64_t* chunk_rx_us,
+                                     const rpl_scan_params* params, float* ranges, float* intensities,
+                                     uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
+                                     uint64_t* scan_begin_ts_us);
+rpl_result rpl_normal_stream_push_ts_dev(rpl_normal_stream* s, const uint8_t* bytes, const uint32_t* byte_counts,
+                                         const rpl_timing* timing, uint32_t chunk_bytes, const uint64_t* chunk_rx_us,
+                                         const rpl_scan_params* params, float* ranges, float* intensities,
+                                         uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
+                                         uint64_t* scan_begin_ts_us, void* stream);
 rpl_result rpl_normal_stream_reset(rpl_normal_stream* s, const uint8_t* stream_mask);
 rpl_result rpl_normal_stream_state(rpl_normal_stream* s, uint32_t* open_nodes, uint32_t* held_bytes);
 

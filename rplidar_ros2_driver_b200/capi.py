@@ -48,11 +48,12 @@ EXPORTS = [
     "rpl_scan_views_dev", "rpl_chain_dense_laserscan", "rpl_decode_dense_batch_starts_dev",
     "rpl_assemble_scan_views_starts_dev",
     "rpl_dense_stream_create", "rpl_dense_stream_destroy", "rpl_dense_stream_push", "rpl_dense_stream_push_dev",
-    "rpl_dense_stream_reset", "rpl_dense_stream_state",
+    "rpl_dense_stream_reset", "rpl_dense_stream_state", "rpl_dense_stream_push_ts", "rpl_dense_stream_push_ts_dev",
     "rpl_capsule_stream_create", "rpl_capsule_stream_destroy", "rpl_capsule_stream_push", "rpl_capsule_stream_push_dev",
-    "rpl_capsule_stream_reset", "rpl_capsule_stream_state",
+    "rpl_capsule_stream_reset", "rpl_capsule_stream_state", "rpl_capsule_stream_push_ts",
+    "rpl_capsule_stream_push_ts_dev",
     "rpl_normal_stream_create", "rpl_normal_stream_destroy", "rpl_normal_stream_push", "rpl_normal_stream_push_dev",
-    "rpl_normal_stream_reset", "rpl_normal_stream_state",
+    "rpl_normal_stream_reset", "rpl_normal_stream_state", "rpl_normal_stream_push_ts", "rpl_normal_stream_push_ts_dev",
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -136,7 +137,7 @@ def lib() -> C.CDLL:
         )
     L = C.CDLL(LIB_PATH)
     vp, u32, u64, sz, i32 = C.c_void_p, C.c_uint32, C.c_uint64, C.c_size_t, C.c_int
-    PSP, PCP = C.POINTER(ScanParams), C.POINTER(CloudParams)
+    PSP, PCP, PT = C.POINTER(ScanParams), C.POINTER(CloudParams), C.POINTER(Timing)
     sig = {
         "rpl_abi_version": ([], u32),
         "rpl_ctx_create": ([i32, u32, u32, C.POINTER(vp)], u32),
@@ -212,6 +213,12 @@ def lib() -> C.CDLL:
         "rpl_normal_stream_push_dev": ([vp, vp, vp, PSP, vp, vp, vp, vp, vp, vp], u32),
         "rpl_normal_stream_reset": ([vp, vp], u32),
         "rpl_normal_stream_state": ([vp, vp, vp], u32),
+        "rpl_capsule_stream_push_ts": ([vp, vp, vp, PT, vp, PSP, vp, vp, vp, vp, vp, vp], u32),
+        "rpl_capsule_stream_push_ts_dev": ([vp, vp, vp, PT, vp, PSP, vp, vp, vp, vp, vp, vp, vp], u32),
+        "rpl_dense_stream_push_ts": ([vp, vp, vp, PT, vp, PSP, vp, vp, vp, vp, vp, vp], u32),
+        "rpl_dense_stream_push_ts_dev": ([vp, vp, vp, PT, vp, PSP, vp, vp, vp, vp, vp, vp, vp], u32),
+        "rpl_normal_stream_push_ts": ([vp, vp, vp, PT, u32, vp, PSP, vp, vp, vp, vp, vp, vp], u32),
+        "rpl_normal_stream_push_ts_dev": ([vp, vp, vp, PT, u32, vp, PSP, vp, vp, vp, vp, vp, vp, vp], u32),
     }
     for name, (args, res) in sig.items():
         fn = getattr(L, name)  # AttributeError here = the library does not export the ABI
@@ -608,25 +615,53 @@ class CapsuleStreamSession:
                 out[k] = np.zeros(shape, dt)
         return out
 
-    def push(self, capsules, capsule_counts, params: ScanParams, sample_duration_us=31, out=None):
+    def _stamped_outputs(self, out):
+        out = self._outputs(out)
+        if "scan_begin_ts_us" not in out:
+            out["scan_begin_ts_us"] = np.zeros(self.n_streams * self.max_scans, np.uint64)
+        return out
+
+    def push(self, capsules, capsule_counts, params: ScanParams, sample_duration_us=31, out=None, rx_us=None,
+             timing: "Timing | None" = None):
         """Host buffers: capsules [n_streams, stride_capsules, capsule_bytes] uint8 -> the dict of
-        Context.chain_dense_laserscan holding the scans this push published."""
+        Context.chain_dense_laserscan holding the scans this push published.  With rx_us ([n_streams, stride_capsules]
+        receive time of every capsule) and timing, a stamped push (rpl_*_stream_push_ts, whose decoder takes
+        timing.sample_duration_us): the dict also holds scan_begin_ts_us [n_streams * max_scans] uint64."""
         assert capsules.dtype == np.uint8 and capsules.shape == (self.n_streams, self.stride_capsules, self.capsule_bytes)
         assert capsules.flags.c_contiguous
         cc = np.ascontiguousarray(capsule_counts, dtype=np.uint32)
         assert cc.shape == (self.n_streams,)
-        out = self._outputs(out)
-        self._ctx._check(self._fn("push")(
-            self._h, _p(capsules), _p(cc), sample_duration_us, C.byref(params), _p(out["ranges"]),
-            _p(out["intensities"]), _p(out["beam_counts"]), _p(out["angle_increment"]), _p(out["scans_per_stream"])))
+        if rx_us is None and timing is None:
+            out = self._outputs(out)
+            self._ctx._check(self._fn("push")(
+                self._h, _p(capsules), _p(cc), sample_duration_us, C.byref(params), _p(out["ranges"]),
+                _p(out["intensities"]), _p(out["beam_counts"]), _p(out["angle_increment"]),
+                _p(out["scans_per_stream"])))
+            return out
+        assert rx_us is not None and timing is not None, "a stamped push takes both rx_us and timing"
+        rx = np.ascontiguousarray(rx_us, dtype=np.uint64)
+        assert rx.shape == (self.n_streams, self.stride_capsules)
+        out = self._stamped_outputs(out)
+        self._ctx._check(self._fn("push_ts")(
+            self._h, _p(capsules), _p(cc), C.byref(timing), _p(rx), C.byref(params), _p(out["ranges"]),
+            _p(out["intensities"]), _p(out["beam_counts"]), _p(out["angle_increment"]), _p(out["scans_per_stream"]),
+            _p(out["scan_begin_ts_us"])))
         return out
 
     def push_dev(self, capsules, capsule_counts, params: ScanParams, ranges, intensities, beam_counts,
-                 angle_increment, scans_per_stream, sample_duration_us=31, stream=None):
-        """Device addresses (the layouts of push), asynchronous on `stream` (None: the context's stream)."""
-        self._ctx._check(self._fn("push_dev")(
-            self._h, _p(capsules), _p(capsule_counts), sample_duration_us, C.byref(params), _p(ranges),
-            _p(intensities), _p(beam_counts), _p(angle_increment), _p(scans_per_stream), _p(stream)))
+                 angle_increment, scans_per_stream, sample_duration_us=31, stream=None, rx_us=None,
+                 timing: "Timing | None" = None, scan_begin_ts_us=None):
+        """Device addresses (the layouts of push), asynchronous on `stream` (None: the context's stream).  With rx_us,
+        timing and scan_begin_ts_us (device addresses but timing), a stamped push."""
+        if rx_us is None and timing is None and scan_begin_ts_us is None:
+            self._ctx._check(self._fn("push_dev")(
+                self._h, _p(capsules), _p(capsule_counts), sample_duration_us, C.byref(params), _p(ranges),
+                _p(intensities), _p(beam_counts), _p(angle_increment), _p(scans_per_stream), _p(stream)))
+            return
+        self._ctx._check(self._fn("push_ts_dev")(
+            self._h, _p(capsules), _p(capsule_counts), C.byref(timing) if timing is not None else None, _p(rx_us),
+            C.byref(params), _p(ranges), _p(intensities), _p(beam_counts), _p(angle_increment), _p(scans_per_stream),
+            _p(scan_begin_ts_us), _p(stream)))
 
     def reset(self, mask=None):
         """Drops the held capsule, the decoder state and the open revolution of the streams where mask is true
@@ -669,24 +704,46 @@ class NormalStreamSession(CapsuleStreamSession):
         self.ans_type = 0x81
         self.n_streams, self.stride_bytes, self.max_nodes, self.max_scans = n_streams, stride_bytes, max_nodes, max_scans
 
-    def push(self, stream_bytes, byte_counts, params: ScanParams, out=None):
-        """Host buffers: stream_bytes [n_streams, stride_bytes] uint8 -> the dict of CapsuleStreamSession.push."""
+    def push(self, stream_bytes, byte_counts, params: ScanParams, out=None, chunk_bytes=None, chunk_rx_us=None,
+             timing: "Timing | None" = None):
+        """Host buffers: stream_bytes [n_streams, stride_bytes] uint8 -> the dict of CapsuleStreamSession.push.  With
+        chunk_bytes, chunk_rx_us ([n_streams, ceil(stride_bytes / chunk_bytes)]: receive time of each chunk_bytes piece
+        of this push) and timing, a stamped push: the dict also holds scan_begin_ts_us."""
         assert stream_bytes.dtype == np.uint8 and stream_bytes.shape == (self.n_streams, self.stride_bytes)
         assert stream_bytes.flags.c_contiguous
         bc = np.ascontiguousarray(byte_counts, dtype=np.uint32)
         assert bc.shape == (self.n_streams,)
-        out = self._outputs(out)
-        self._ctx._check(self._fn("push")(
-            self._h, _p(stream_bytes), _p(bc), C.byref(params), _p(out["ranges"]), _p(out["intensities"]),
-            _p(out["beam_counts"]), _p(out["angle_increment"]), _p(out["scans_per_stream"])))
+        if chunk_bytes is None and chunk_rx_us is None and timing is None:
+            out = self._outputs(out)
+            self._ctx._check(self._fn("push")(
+                self._h, _p(stream_bytes), _p(bc), C.byref(params), _p(out["ranges"]), _p(out["intensities"]),
+                _p(out["beam_counts"]), _p(out["angle_increment"]), _p(out["scans_per_stream"])))
+            return out
+        assert chunk_bytes is not None and chunk_rx_us is not None and timing is not None, \
+            "a stamped push takes chunk_bytes, chunk_rx_us and timing"
+        rx = np.ascontiguousarray(chunk_rx_us, dtype=np.uint64)
+        assert chunk_bytes == 0 or rx.shape == (self.n_streams, -(-self.stride_bytes // chunk_bytes))
+        out = self._stamped_outputs(out)
+        self._ctx._check(self._fn("push_ts")(
+            self._h, _p(stream_bytes), _p(bc), C.byref(timing), chunk_bytes, _p(rx), C.byref(params),
+            _p(out["ranges"]), _p(out["intensities"]), _p(out["beam_counts"]), _p(out["angle_increment"]),
+            _p(out["scans_per_stream"]), _p(out["scan_begin_ts_us"])))
         return out
 
     def push_dev(self, stream_bytes, byte_counts, params: ScanParams, ranges, intensities, beam_counts,
-                 angle_increment, scans_per_stream, stream=None):
-        """Device addresses (the layouts of push), asynchronous on `stream` (None: the context's stream)."""
-        self._ctx._check(self._fn("push_dev")(
-            self._h, _p(stream_bytes), _p(byte_counts), C.byref(params), _p(ranges), _p(intensities),
-            _p(beam_counts), _p(angle_increment), _p(scans_per_stream), _p(stream)))
+                 angle_increment, scans_per_stream, stream=None, chunk_bytes=None, chunk_rx_us=None,
+                 timing: "Timing | None" = None, scan_begin_ts_us=None):
+        """Device addresses (the layouts of push), asynchronous on `stream` (None: the context's stream).  With
+        chunk_bytes, chunk_rx_us, timing and scan_begin_ts_us, a stamped push."""
+        if chunk_bytes is None and chunk_rx_us is None and timing is None and scan_begin_ts_us is None:
+            self._ctx._check(self._fn("push_dev")(
+                self._h, _p(stream_bytes), _p(byte_counts), C.byref(params), _p(ranges), _p(intensities),
+                _p(beam_counts), _p(angle_increment), _p(scans_per_stream), _p(stream)))
+            return
+        self._ctx._check(self._fn("push_ts_dev")(
+            self._h, _p(stream_bytes), _p(byte_counts), C.byref(timing) if timing is not None else None,
+            chunk_bytes or 0, _p(chunk_rx_us), C.byref(params), _p(ranges), _p(intensities), _p(beam_counts),
+            _p(angle_increment), _p(scans_per_stream), _p(scan_begin_ts_us), _p(stream)))
 
 
 EXCHANGE_NCCL, EXCHANGE_COPY = 0, 1

@@ -16,6 +16,7 @@
 // compacted into descriptors and then copied coalesced.  A stream with more scan starts than the
 // list holds takes the chunked block-scan path instead (same result, more barriers).
 #include "decode_args.h"
+#include "delay_model.cuh"
 #include "rpl_device.cuh"
 
 namespace rpl {
@@ -58,9 +59,12 @@ __device__ __forceinline__ void rank_sort(const uint32_t* in, uint32_t* out, uin
 
 // STREAM: a stream session's instantiation, any capsule format (AssembleArgs::carry_len): positions count from the first
 // node of the revolution carried in front of the new nodes, which is a scan start like any other -- listed first when
-// the decoder hands a scan-start list over (dense), found by the flag pass like the others when it does not
-template <bool STREAM>
-__global__ void __launch_bounds__(AT) assemble_kernel(AssembleArgs a) {
+// the decoder hands a scan-start list over (dense), found by the flag pass like the others when it does not.
+// STAMPED (a stamped session push, STREAM only): also the stamp of every published scan's scan-start node and of the
+// open revolution's first node, computed for those nodes alone (sa, m)
+template <bool STREAM, bool STAMPED>
+__device__ __forceinline__ void assemble_body(const AssembleArgs& a, const AssembleStampArgs& sa, const DelayModel& m) {
+  static_assert(STREAM || !STAMPED, "stamps are a stream session's");
   __shared__ uint32_t s_list[kListCap], s_sorted[kListCap];      // scan-start positions
   __shared__ uint32_t s_rlist[kResetCap], s_rsorted[kResetCap];  // reset positions
   __shared__ uint32_t s_cnt, s_rcnt;
@@ -84,6 +88,44 @@ __global__ void __launch_bounds__(AT) assemble_kernel(AssembleArgs a) {
     uint2* desc = a.desc + (size_t)s * a.max_scans;                 // (start, length) of published scans
     uint2* out = a.scans_out + (size_t)s * a.max_scans * a.scan_stride;
     uint32_t* out_len = a.scan_len + (size_t)s * a.max_scans;
+    // STAMPED: the stamp of the scan-start node at position x (ScanDataHolder::_scan_begin_timestamp_uS), what the
+    // timestamp kernels would have written for it.  The only scan start among the carried nodes is the carried
+    // revolution's first, at 0.  A capsule-format node was released by the last capsule whose node offset is <= its
+    // index (a capsule that releases nothing shares the next release's offset); a 0x81 node takes the receive time of
+    // the chunk its record's last byte came in.
+    unsigned long long open_in = 0, held_rx_in = kRxUnknown;
+    if constexpr (STAMPED) {
+      if (sa.prev_stamped) {
+        open_in = sa.open_ts_in[s];
+        if (m.prev_base) held_rx_in = sa.held_rx[s];
+      }
+    }
+    const unsigned long long* crx = STAMPED && have_resets ? sa.capsule_rx_us + (size_t)s * a.stride_capsules : nullptr;
+    auto stamp_at = [&](uint32_t x) -> unsigned long long {
+      if constexpr (!STAMPED) {
+        return 0ull;
+      } else {
+        if (x < L) return open_in;
+        const uint32_t y = x - L;
+        if (!have_resets) {  // 0x81
+          const uint32_t e = sa.node_end[(size_t)s * sa.stride_ends + y];
+          return sa.chunk_rx_us[(size_t)s * sa.stride_chunks + e / sa.chunk_bytes] - m.base;
+        }
+        uint32_t lo = 0, hi = ncap;  // first capsule with offset > y (>= 1: node y was released)
+        while (lo < hi) {
+          const uint32_t mid = (lo + hi) >> 1;
+          if (coff[mid] <= y) lo = mid + 1;
+          else hi = mid;
+        }
+        const uint32_t j = lo - 1;
+        // express, ultra: the released capsule's own receive time, the held one's for capsule 0
+        if (m.prev_base && j == 0 && held_rx_in == kRxUnknown) return 0ull;
+        const unsigned long long rx = !m.prev_base ? crx[j] : j ? crx[j - 1] : held_rx_in;
+        unsigned long long d = m.base;
+        if (m.group >= 0) d += (unsigned long long)(m.group - (int)(y - coff[j])) * m.sd;
+        return rx - d;
+      }
+    };
 
     if (tid == 0) {
       s_cnt = 0;
@@ -248,10 +290,13 @@ __global__ void __launch_bounds__(AT) assemble_kernel(AssembleArgs a) {
           const uint32_t cnt = min(d.y, a.max_nodes);
           if (d.y > cnt) a.nodes_mut[(size_t)s * a.stride_nodes + base + d.x + cnt - 1] = nodes[d.x + d.y - 1];
           v = make_uint2((uint32_t)((size_t)s * a.stride_nodes + base + d.x), cnt);
-          if (a.scan_begin_ts_us)
-            a.scan_begin_ts_us[(size_t)s * a.max_scans + k] =
-                a.node_ts_us ? a.node_ts_us[(size_t)s * a.stride_nodes + base + d.x] : 0ull;
+          if constexpr (!STAMPED) {
+            if (a.scan_begin_ts_us)
+              a.scan_begin_ts_us[(size_t)s * a.max_scans + k] =
+                  a.node_ts_us ? a.node_ts_us[(size_t)s * a.stride_nodes + base + d.x] : 0ull;
+          }
         }
+        if constexpr (STAMPED) a.scan_begin_ts_us[(size_t)s * a.max_scans + k] = k < stored ? stamp_at(desc[k].x) : 0ull;
         vout[k] = v;
         out_len[k] = v.y;
       }
@@ -267,6 +312,11 @@ __global__ void __launch_bounds__(AT) assemble_kernel(AssembleArgs a) {
         if (tid == 0) {
           if (t > tc) dst[tc - 1] = src[t - 1];
           a.carry_len_out[s] = tc;
+          if constexpr (STAMPED) {
+            // every thread has read held_rx_in (before the first barrier of this stream)
+            sa.open_ts_out[s] = ls >= 0 ? stamp_at((uint32_t)ls) : 0ull;
+            if (m.prev_base) sa.held_rx[s] = ncap ? crx[ncap - 1] : held_rx_in;
+          }
         }
       }
       __syncthreads();
@@ -304,6 +354,15 @@ __global__ void __launch_bounds__(AT) assemble_kernel(AssembleArgs a) {
   }
 }
 
+template <bool STREAM>
+__global__ void __launch_bounds__(AT) assemble_kernel(AssembleArgs a) {
+  assemble_body<STREAM, false>(a, AssembleStampArgs{}, DelayModel{});
+}
+
+__global__ void __launch_bounds__(AT) assemble_stamped_kernel(AssembleArgs a, AssembleStampArgs sa, DelayModel m) {
+  assemble_body<true, true>(a, sa, m);
+}
+
 }  // namespace
 
 cudaError_t launch_assemble(const AssembleArgs& a, int grid, cudaStream_t stream) {
@@ -312,6 +371,12 @@ cudaError_t launch_assemble(const AssembleArgs& a, int grid, cudaStream_t stream
     assemble_kernel<true><<<grid, AT, 0, stream>>>(a);
   else
     assemble_kernel<false><<<grid, AT, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_assemble_stamped(const AssembleArgs& a, const AssembleStampArgs& sa, int grid, cudaStream_t stream) {
+  if (a.n_streams == 0) return cudaSuccess;
+  assemble_stamped_kernel<<<grid, AT, 0, stream>>>(a, sa, delay_model(sa.ans_type, sa.timing));
   return cudaGetLastError();
 }
 

@@ -55,7 +55,8 @@ struct NormalDecodeArgs {
   uint32_t* node_end;             // [n_streams][stride_bytes / 5] nullable: index of each record's last byte
   // stream session only (node_stride != 0): the nodes go to nodes_out + s * node_stride + node_first (behind the
   // session's carry slots), counts above stride_bytes are clamped to it, and the stream enters in the state and with
-  // the last four bytes its held record keeps (written back at the end); fsm_state_out and node_end are unused then
+  // the last four bytes its held record keeps (written back at the end); fsm_state_out is unused then, and node_end
+  // (nullable, [n_streams][node_stride - node_first]) is written for the scan-start records only
   uint32_t* held;                 // [n_streams][kHeldWords], read and rewritten in place
   uint32_t node_stride, node_first;
 };
@@ -117,6 +118,29 @@ struct AssembleArgs {
   uint32_t* carry_len_out;            // [n_streams]
 };
 
+// a stamped stream-session push (launch_assemble_stamped; AssembleArgs::scan_begin_ts_us is the output, every slot
+// written, unused ones 0): the stamp of each published scan's scan-start node, from the receive times of this push,
+// without a per-node stamp array.  Capsule formats read AssembleArgs' capsule report, 0x81 reads node_end.
+constexpr unsigned long long kRxUnknown = ~0ull;  // held_rx: the held capsule came in a push without receive times
+struct AssembleStampArgs {
+  uint32_t ans_type;
+  TimingDesc timing;
+  const unsigned long long* capsule_rx_us;  // capsule formats: [n_streams][AssembleArgs::stride_capsules]
+  // 0x81: [n_streams][stride_ends], at the new-node index of every scan-start record the push-relative index of its
+  // last byte (decode_normal's stamped instantiation; other entries undefined); chunk c covers bytes
+  // [c * chunk_bytes, (c + 1) * chunk_bytes) of the push
+  const uint32_t* node_end;
+  uint32_t stride_ends, chunk_bytes, stride_chunks;
+  const unsigned long long* chunk_rx_us;    // 0x81: [n_streams][stride_chunks]
+  // the stamp of the open revolution entering and leaving the push, beside carry_len (0: unknown)
+  const unsigned long long* open_ts_in;     // [n_streams]
+  unsigned long long* open_ts_out;          // [n_streams]
+  // express, ultra: receive time of the held capsule, read and rewritten in place (kRxUnknown: never given)
+  unsigned long long* held_rx;              // [n_streams]
+  // 0: the previous push had no receive times, so open_ts_in and held_rx are stale and count as unknown
+  uint32_t prev_stamped;
+};
+
 // byte-level framing with the SDK's resynchronisation (frame.cu)
 struct FrameArgs {
   const uint8_t* bytes;           // [n_streams][stride_bytes] raw capsule streams
@@ -130,5 +154,6 @@ struct FrameArgs {
 };
 cudaError_t launch_frame_capsules(const FrameArgs& a, int grid, cudaStream_t stream);
 cudaError_t launch_assemble(const AssembleArgs& a, int grid, cudaStream_t stream);
+cudaError_t launch_assemble_stamped(const AssembleArgs& a, const AssembleStampArgs& t, int grid, cudaStream_t stream);
 
 }  // namespace rpl

@@ -888,8 +888,11 @@ __device__ __forceinline__ uint32_t compose_map(uint32_t g, uint32_t f) {
 // STREAM: a stream session's instantiation (NormalDecodeArgs::node_stride != 0).  The held record's state and last four
 // bytes take the place of a previous tile's (carry_state and the halo), so a record begun in an earlier push completes
 // in this one's first bytes, read through the halo like a record spanning two tiles.
-template <bool STREAM>
-__global__ void __launch_bounds__(NT, 5) decode_normal_kernel(NormalDecodeArgs a) {
+// STARTS (a stamped session push, STREAM only): node_end [n_streams][node_stride - node_first] gets the push-relative
+// index of the last byte of the scan-start records alone, at their node index (a few stores per revolution)
+template <bool STREAM, bool STARTS>
+__device__ __forceinline__ void decode_normal_body(const NormalDecodeArgs& a) {
+  static_assert(STREAM || !STARTS, "the scan-start ends are a stream session's");
   __shared__ __align__(16) NormalSmem sm;
   uint8_t* const sm_bytes = sm.raw + 12;  // bytes[0..3] = halo, bytes + 4 = the tile
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -898,7 +901,8 @@ __global__ void __launch_bounds__(NT, 5) decode_normal_kernel(NormalDecodeArgs a
     const uint8_t* src = a.bytes + (size_t)s * a.stride_bytes;
     uint2* out = STREAM ? a.nodes_out + (size_t)s * a.node_stride + a.node_first
                         : a.nodes_out + (size_t)s * (a.stride_bytes / 5u);
-    uint32_t* end_out = (!STREAM && a.node_end) ? a.node_end + (size_t)s * (a.stride_bytes / 5u) : nullptr;
+    uint32_t* end_out = STARTS ? a.node_end + (size_t)s * (a.node_stride - a.node_first)
+                        : (!STREAM && a.node_end) ? a.node_end + (size_t)s * (a.stride_bytes / 5u) : nullptr;
     if constexpr (STREAM) {
       // all zero (a fresh stream): state 0, whose first record ends at byte 5 at the earliest, never reading the halo
       if (tid == 0) {
@@ -962,7 +966,7 @@ __global__ void __launch_bounds__(NT, 5) decode_normal_kernel(NormalDecodeArgs a
             const uint32_t q = tid + j * NT;
             if (q < n_rec) {
               o[q] = nd[j];
-              if (end_out) end_out[sm.carry_nodes + q] = t0 + 5 * q + 4;
+              if (end_out && (!STARTS || ((nd[j].y >> 24) & 1u))) end_out[sm.carry_nodes + q] = t0 + 5 * q + 4;
             }
           }
           __syncthreads();
@@ -1032,7 +1036,7 @@ __global__ void __launch_bounds__(NT, 5) decode_normal_kernel(NormalDecodeArgs a
         nd.x = key | (dist << 16);
         nd.y = (((sq >> 2) << 2) << 16) | ((sq & 1u) << 24);
         o[q] = nd;
-        if (end_out) end_out[sm.carry_nodes + q] = t0 + sm.ends[q];
+        if (end_out && (!STARTS || ((nd.y >> 24) & 1u))) end_out[sm.carry_nodes + q] = t0 + sm.ends[q];
       }
       __syncthreads();
       if constexpr (STREAM) {
@@ -1063,6 +1067,15 @@ __global__ void __launch_bounds__(NT, 5) decode_normal_kernel(NormalDecodeArgs a
     }
     __syncthreads();
   }
+}
+
+template <bool STREAM>
+__global__ void __launch_bounds__(NT, 5) decode_normal_kernel(NormalDecodeArgs a) {
+  decode_normal_body<STREAM, false>(a);
+}
+
+__global__ void __launch_bounds__(NT, 5) decode_normal_starts_kernel(NormalDecodeArgs a) {
+  decode_normal_body<true, true>(a);
 }
 
 template <int F>
@@ -1104,7 +1117,9 @@ cudaError_t launch_decode_capsules(uint32_t ans_type, const CapsuleDecodeArgs& a
 
 cudaError_t launch_decode_normal(const NormalDecodeArgs& a, int grid, cudaStream_t stream) {
   if (a.n_streams == 0) return cudaSuccess;
-  if (a.node_stride)
+  if (a.node_stride && a.node_end)
+    decode_normal_starts_kernel<<<grid, NT, 0, stream>>>(a);
+  else if (a.node_stride)
     decode_normal_kernel<true><<<grid, NT, 0, stream>>>(a);
   else
     decode_normal_kernel<false><<<grid, NT, 0, stream>>>(a);

@@ -1021,7 +1021,7 @@ rpl_result assemble_common(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t*
                                   uint64_t* scan_begin_ts_us, void* stream, const uint32_t* scan_starts = nullptr,
                                   uint32_t starts_stride = 0, const uint32_t* scan_start_counts = nullptr,
                                   const uint32_t* carry_len = nullptr, rpl_node_hq* carry_out = nullptr,
-                                  uint32_t* carry_len_out = nullptr) {
+                                  uint32_t* carry_len_out = nullptr, const rpl::AssembleStampArgs* stamp = nullptr) {
   if (!c || !nodes || !node_counts || (!scans_out && !views_out) || !scan_len || !scans_per_stream) return RPL_RESULT_INVALID_DATA;
   if (views_out && (unsigned long long)n_streams * stride_nodes > 0xFFFFFFFFull) {
     c->err = "view mode addresses nodes with 32 bits: n_streams * stride_nodes must stay below 2^32";
@@ -1085,7 +1085,10 @@ rpl_result assemble_common(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t*
   a.carry_out = reinterpret_cast<uint2*>(carry_out);
   a.carry_len_out = carry_len_out;
   const int grid = (int)std::min<uint32_t>(n_streams, (uint32_t)c->num_sms * 4u);
-  RPL_CUDA(c, rpl::launch_assemble(a, grid, st), RPL_RESULT_OPERATION_FAIL);
+  if (stamp)
+    RPL_CUDA(c, rpl::launch_assemble_stamped(a, *stamp, grid, st), RPL_RESULT_OPERATION_FAIL);
+  else
+    RPL_CUDA(c, rpl::launch_assemble(a, grid, st), RPL_RESULT_OPERATION_FAIL);
   c->launches++;
   return RPL_RESULT_OK;
 }
@@ -1264,6 +1267,9 @@ rpl_result rpl_chain_dense_laserscan(rpl_ctx* c, const uint8_t* capsules, const 
 // assembler.  rpl_dense_stream is this session fixed to 0x85.  rpl_normal_stream is this session on 0x81 standard-node
 // bytes: a push's input counts bytes instead of capsules (cap_bytes 1), the held record keeps the byte machine, and
 // there are no capsule reports (the standard unpacker requests no scan resets).
+// A stamped push (rpl_*_stream_push_ts*) runs the stamped decoder (0x81) and assembler instead; they keep, beside the
+// carry, the open revolution's stamp (open_ts, per arena like carry_len) and, for express and ultra, the held capsule's
+// receive time (held_rx).  An unstamped push leaves both stale, so the next stamped push counts them as unknown.
 struct rpl_capsule_stream {
   rpl_ctx* c = nullptr;
   uint32_t ans_type = 0, cap_bytes = 0;    // answer type, bytes per capsule (0x81: 1)
@@ -1280,7 +1286,12 @@ struct rpl_capsule_stream {
   rpl_scan_view* views = nullptr;
   unsigned char* lane_buf[kLanes] = {nullptr, nullptr};  // host-push staging: capsules, counts and outputs of a chunk
   size_t o_ccnt = 0, o_r = 0, o_i = 0, o_b = 0, o_inc = 0, o_sps = 0, lane_bytes = 0;
+  size_t o_ts = 0, o_rx = 0;                    // stamped host pushes: scan stamps, then receive times of a chunk
   cudaEvent_t done = nullptr;                   // the last push_dev: later calls on other streams wait for it
+  unsigned long long* open_ts[2] = {nullptr, nullptr};  // [n_streams] stamp of the open revolution (0: unknown)
+  unsigned long long* held_rx = nullptr;        // [n_streams] express, ultra: receive time of the held capsule
+  uint32_t* scan_ends = nullptr;                // 0x81: [n_streams][new nodes] end bytes of the scan-start records
+  bool prev_stamped = true;                     // the last push had receive times (a fresh session holds nothing)
 };
 
 namespace {
@@ -1289,13 +1300,22 @@ namespace {
 rpl_capsule_stream* capsule_session(rpl_dense_stream* ds) { return reinterpret_cast<rpl_capsule_stream*>(ds); }
 rpl_capsule_stream* capsule_session(rpl_normal_stream* ns) { return reinterpret_cast<rpl_capsule_stream*>(ns); }
 
-// decode -> assemble -> scan kernels for streams [s0, s0 + ns) on `st`; capsules / counts / outputs point at s0's
+// a stamped push's receive times and stamp output (rx, scan_ts: of the first stream of the call they are passed to)
+struct StampPush {
+  rpl::TimingDesc timing;
+  const unsigned long long* rx;         // capsule_rx_us [.][stride_capsules], 0x81: chunk_rx_us [.][stride_chunks]
+  uint32_t chunk_bytes, stride_chunks;  // 0x81
+  unsigned long long* scan_ts;          // scan_begin_ts_us [.][max_scans]
+};
+
+// decode -> assemble -> scan kernels for streams [s0, s0 + ns) on `st`; capsules / counts / outputs / sp point at s0's
 rpl_result capsule_stream_chunk(rpl_capsule_stream* cs, Lane& l, cudaStream_t st, uint32_t s0, uint32_t ns,
                                 const uint8_t* capsules, const uint32_t* counts, uint32_t sample_duration_us,
                                 const rpl_scan_params* params, float* ranges, float* intens, uint32_t* beams,
-                                float* inc, uint32_t* scans_per_stream) {
+                                float* inc, uint32_t* scans_per_stream, const StampPush* sp = nullptr) {
   rpl_ctx* c = cs->c;
-  const uint32_t p = cs->parity, sc = cs->stride_capsules;
+  const uint32_t p = cs->parity, sc = cs->stride_capsules, new_nodes = cs->stride_nodes - cs->max_nodes;
+  uint32_t* ends = sp && cs->scan_ends ? cs->scan_ends + (size_t)s0 * new_nodes : nullptr;
   rpl_node_hq* nodes = cs->arena[p] + (size_t)s0 * cs->stride_nodes;
   // capsule formats only: the per-capsule reports, which carry the scan-reset requests to the assembler
   uint32_t* status = cs->status ? cs->status + (size_t)s0 * sc : nullptr;
@@ -1315,6 +1335,7 @@ rpl_result capsule_stream_chunk(rpl_capsule_stream* cs, Lane& l, cudaStream_t st
     a.held = cs->held + (size_t)s0 * rpl::kHeldWords;
     a.node_stride = cs->stride_nodes;
     a.node_first = cs->max_nodes;
+    a.node_end = ends;
     r = decode_normal_launch(c, a, st);
   } else {
     rpl::CapsuleDecodeArgs a{};
@@ -1341,11 +1362,27 @@ rpl_result capsule_stream_chunk(rpl_capsule_stream* cs, Lane& l, cudaStream_t st
   if (!c->asm_done) RPL_CUDA(c, cudaEventCreateWithFlags(&c->asm_done, cudaEventDisableTiming), RPL_RESULT_OPERATION_FAIL);
   RPL_CUDA(c, cudaStreamWaitEvent(st, c->asm_done, 0), RPL_RESULT_OPERATION_FAIL);
   const size_t so = (size_t)s0 * cs->max_scans;
+  rpl::AssembleStampArgs t{};
+  if (sp) {
+    t.ans_type = cs->ans_type;
+    t.timing = sp->timing;
+    t.capsule_rx_us = status ? sp->rx : nullptr;
+    t.node_end = ends;
+    t.stride_ends = new_nodes;
+    t.chunk_bytes = sp->chunk_bytes;
+    t.stride_chunks = sp->stride_chunks;
+    t.chunk_rx_us = status ? nullptr : sp->rx;
+    t.open_ts_in = cs->open_ts[p] + s0;
+    t.open_ts_out = cs->open_ts[p ^ 1u] + s0;
+    t.held_rx = cs->held_rx + s0;
+    t.prev_stamped = cs->prev_stamped ? 1u : 0u;
+  }
   r = assemble_common(c, nodes, cs->node_counts + s0, ns, cs->stride_nodes, status, offsets, status ? counts : nullptr,
                       status ? sc : 0u, cs->max_nodes, cs->max_scans, cs->max_nodes, nullptr, cs->views + so,
-                      cs->scan_len + so, scans_per_stream, nullptr, nullptr, st, starts,
+                      cs->scan_len + so, scans_per_stream, nullptr,
+                      sp ? reinterpret_cast<uint64_t*>(sp->scan_ts) : nullptr, st, starts,
                       starts ? cs->starts_stride : 0u, start_counts, cs->carry_len[p] + s0,
-                      cs->arena[p ^ 1u] + (size_t)s0 * cs->stride_nodes, cs->carry_len[p ^ 1u] + s0);
+                      cs->arena[p ^ 1u] + (size_t)s0 * cs->stride_nodes, cs->carry_len[p ^ 1u] + s0, sp ? &t : nullptr);
   if (r != RPL_RESULT_OK) return r;
   RPL_CUDA(c, cudaEventRecord(c->asm_done, st), RPL_RESULT_OPERATION_FAIL);
   return enqueue_scan(c, l, nodes, cs->scan_len + so, ns * cs->max_scans, cs->max_nodes, params, nullptr, ranges, intens,
@@ -1423,7 +1460,10 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint
   cs->o_b = cs->o_i + up(NS * max_nodes * 4);
   cs->o_inc = cs->o_b + up(NS * 4);
   cs->o_sps = cs->o_inc + up(NS * 4);
-  cs->lane_bytes = cs->o_sps + up((size_t)cs->chunk_host * 4);
+  cs->o_ts = cs->o_sps + up((size_t)cs->chunk_host * 4);
+  cs->o_rx = cs->o_ts + up(NS * 8);
+  // 0x81: the receive times' count depends on each push's chunk_bytes, and a stamped push grows the buffers to it
+  cs->lane_bytes = cs->o_rx + (normal ? 0 : up((size_t)cs->chunk_host * stride_capsules * 8));
   const size_t n = n_streams, ncap = n * stride_capsules;
   const rpl_result oom = RPL_RESULT_INSUFFICIENT_MEMORY;
   auto fail = [&](rpl_result r) {
@@ -1433,8 +1473,14 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint
   for (int p = 0; p < 2; ++p)
     if (!cuda_ok(c, dev_alloc(&cs->arena[p], n * cs->stride_nodes), "cudaMalloc") ||
         !cuda_ok(c, dev_alloc(&cs->carry_len[p], n), "cudaMalloc") ||
-        !cuda_ok(c, cudaMemset(cs->carry_len[p], 0, n * 4), "cudaMemset"))
+        !cuda_ok(c, cudaMemset(cs->carry_len[p], 0, n * 4), "cudaMemset") ||
+        !cuda_ok(c, dev_alloc(&cs->open_ts[p], n), "cudaMalloc") ||
+        !cuda_ok(c, cudaMemset(cs->open_ts[p], 0, n * 8), "cudaMemset"))
       return fail(oom);
+  if (!cuda_ok(c, dev_alloc(&cs->held_rx, n), "cudaMalloc") ||
+      !cuda_ok(c, cudaMemset(cs->held_rx, 0, n * 8), "cudaMemset"))
+    return fail(oom);
+  if (normal && !cuda_ok(c, dev_alloc(&cs->scan_ends, n * (size_t)new_nodes), "cudaMalloc")) return fail(oom);
   for (int i = 0; i < kLanes; ++i)
     if (!cuda_ok(c, dev_alloc(&cs->lane_buf[i], cs->lane_bytes), "cudaMalloc")) return fail(oom);
   if (ans_type == 0x85 && (!cuda_ok(c, dev_alloc(&cs->starts, n * cs->starts_stride), "cudaMalloc") ||
@@ -1453,6 +1499,144 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint
     return fail(oom);
   *out = cs;
   return RPL_RESULT_OK;
+}
+
+// the stamped pushes' own arguments (chunk_bytes: 0x81 only, 1 for the capsule formats) into *sp
+bool stamp_args_ok(rpl_capsule_stream* cs, const rpl_timing* timing, const uint64_t* rx, uint32_t chunk_bytes,
+                   uint64_t* scan_begin_ts_us, StampPush* sp) {
+  if (!cs) return false;
+  rpl_ctx* c = cs->c;
+  if (!timing || !rx || !scan_begin_ts_us) {
+    c->err = "null timing, receive times or scan_begin_ts_us";
+    return false;
+  }
+  if (chunk_bytes == 0) {
+    c->err = "chunk_bytes must be > 0";
+    return false;
+  }
+  if (misaligned8(rx) || misaligned8(scan_begin_ts_us)) {
+    c->err = "timestamp buffers must be 8-byte aligned";
+    return false;
+  }
+  sp->timing = rpl::TimingDesc{timing->sample_duration_us, timing->native_baudrate, timing->linkage_delay_us,
+                               timing->native_interface_type};
+  sp->rx = reinterpret_cast<const unsigned long long*>(rx);
+  sp->chunk_bytes = chunk_bytes;
+  sp->stride_chunks = (cs->stride_capsules + chunk_bytes - 1) / chunk_bytes;
+  sp->scan_ts = reinterpret_cast<unsigned long long*>(scan_begin_ts_us);
+  return true;
+}
+
+// a host push; sp: a stamped one (its rx and scan_ts are host arrays of all streams)
+rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* capsules, const uint32_t* capsule_counts,
+                       uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges, float* intensities,
+                       uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
+                       const StampPush* sp) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!capsule_stream_args_ok(cs, capsules, capsule_counts, sample_duration_us, params, ranges, intensities,
+                              beam_counts, scans_per_stream))
+    return RPL_RESULT_INVALID_DATA;
+  for (uint32_t s = 0; s < cs->n_streams; ++s)
+    if (capsule_counts[s] > cs->stride_capsules) {
+      c->err = cs->ans_type == RPL_ANS_MEASUREMENT ? "byte_counts[s] exceeds stride_bytes"
+                                                   : "capsule_counts[s] exceeds stride_capsules";
+      return RPL_RESULT_INVALID_DATA;
+    }
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  // receive times per stream: one per capsule, 0x81 one per chunk_bytes piece (the lane buffers grow to them)
+  const size_t rx_stream = sp ? (cs->status ? cs->stride_capsules : sp->stride_chunks) : 0;
+  if (sp && cs->o_rx + (size_t)cs->chunk_host * rx_stream * 8 > cs->lane_bytes) {
+    const size_t need = cs->o_rx + (((size_t)cs->chunk_host * rx_stream * 8 + 255) & ~(size_t)255);
+    for (int i = 0; i < kLanes; ++i) {
+      RPL_CUDA(c, cudaStreamSynchronize(c->lane[i].stream), RPL_RESULT_OPERATION_FAIL);
+      cudaFree(cs->lane_buf[i]);
+      cs->lane_buf[i] = nullptr;
+    }
+    cs->lane_bytes = 0;
+    for (int i = 0; i < kLanes; ++i)
+      RPL_CUDA(c, dev_alloc(&cs->lane_buf[i], need), RPL_RESULT_INSUFFICIENT_MEMORY);
+    cs->lane_bytes = need;
+  }
+  for (int i = 0; i < kLanes; ++i) RPL_CUDA(c, cudaStreamWaitEvent(c->lane[i].stream, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
+  const size_t cap_bytes_stream = (size_t)cs->stride_capsules * cs->cap_bytes, row = (size_t)cs->max_scans * cs->max_nodes;
+  const cudaMemcpyKind h2d = cudaMemcpyHostToDevice, d2h = cudaMemcpyDeviceToHost;
+  auto run_chunk = [&](Lane& l, uint32_t s0, uint32_t ns) -> rpl_result {
+    unsigned char* d = cs->lane_buf[&l - c->lane];
+    const size_t nsc = (size_t)ns * cs->max_scans;
+    RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);  // the lane's previous chunk has left
+    RPL_CUDA(c, cudaMemcpyAsync(d, capsules + s0 * cap_bytes_stream, ns * cap_bytes_stream, h2d, l.stream),
+             RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(d + cs->o_ccnt, capsule_counts + s0, (size_t)ns * 4, h2d, l.stream),
+             RPL_RESULT_OPERATION_FAIL);
+    StampPush chunk_sp{};
+    if (sp) {
+      chunk_sp = *sp;
+      chunk_sp.rx = reinterpret_cast<const unsigned long long*>(d + cs->o_rx);
+      chunk_sp.scan_ts = reinterpret_cast<unsigned long long*>(d + cs->o_ts);
+      RPL_CUDA(c, cudaMemcpyAsync(d + cs->o_rx, sp->rx + s0 * rx_stream, ns * rx_stream * 8, h2d, l.stream),
+               RPL_RESULT_OPERATION_FAIL);
+    }
+    const rpl_result r = capsule_stream_chunk(
+        cs, l, l.stream, s0, ns, d, reinterpret_cast<uint32_t*>(d + cs->o_ccnt), sample_duration_us, params,
+        reinterpret_cast<float*>(d + cs->o_r), reinterpret_cast<float*>(d + cs->o_i),
+        reinterpret_cast<uint32_t*>(d + cs->o_b), reinterpret_cast<float*>(d + cs->o_inc),
+        reinterpret_cast<uint32_t*>(d + cs->o_sps), sp ? &chunk_sp : nullptr);
+    if (r != RPL_RESULT_OK) return r;
+    const size_t so = (size_t)s0 * cs->max_scans;
+    if (sp)
+      RPL_CUDA(c, cudaMemcpyAsync(sp->scan_ts + so, d + cs->o_ts, nsc * 8, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(ranges + so * cs->max_nodes, d + cs->o_r, ns * row * 4, d2h, l.stream),
+             RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(intensities + so * cs->max_nodes, d + cs->o_i, ns * row * 4, d2h, l.stream),
+             RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(beam_counts + so, d + cs->o_b, nsc * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
+    if (angle_increment)
+      RPL_CUDA(c, cudaMemcpyAsync(angle_increment + so, d + cs->o_inc, nsc * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(scans_per_stream + s0, d + cs->o_sps, (size_t)ns * 4, d2h, l.stream),
+             RPL_RESULT_OPERATION_FAIL);
+    return RPL_RESULT_OK;
+  };
+  const rpl_result r = run_chunks(c, cs->n_streams, cs->chunk_host, run_chunk);
+  cs->parity ^= 1u;
+  cs->prev_stamped = sp != nullptr;
+  return r;
+}
+
+// a device push; sp: a stamped one (its rx and scan_ts are device arrays of all streams)
+rpl_result stream_push_dev(rpl_capsule_stream* cs, const uint8_t* capsules, const uint32_t* capsule_counts,
+                           uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
+                           float* intensities, uint32_t* beam_counts, float* angle_increment,
+                           uint32_t* scans_per_stream, void* stream, const StampPush* sp) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!capsule_stream_args_ok(cs, capsules, capsule_counts, sample_duration_us, params, ranges, intensities,
+                              beam_counts, scans_per_stream))
+    return RPL_RESULT_INVALID_DATA;
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
+  RPL_CUDA(c, cudaStreamWaitEvent(st, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
+  const size_t row = (size_t)cs->max_scans * cs->max_nodes;
+  rpl_result r = RPL_RESULT_OK;
+  for (uint32_t s0 = 0; s0 < cs->n_streams && r == RPL_RESULT_OK; s0 += cs->chunk_dev) {
+    const uint32_t ns = std::min(cs->chunk_dev, cs->n_streams - s0);
+    const size_t so = (size_t)s0 * cs->max_scans;
+    StampPush chunk_sp{};
+    if (sp) {
+      chunk_sp = *sp;
+      chunk_sp.rx += (size_t)s0 * (cs->status ? cs->stride_capsules : sp->stride_chunks);
+      chunk_sp.scan_ts += so;
+    }
+    r = capsule_stream_chunk(cs, c->lane[0], st, s0, ns, capsules + (size_t)s0 * cs->stride_capsules * cs->cap_bytes,
+                             capsule_counts + s0, sample_duration_us, params, ranges + (size_t)s0 * row,
+                             intensities + (size_t)s0 * row, beam_counts + so,
+                             angle_increment ? angle_increment + so : nullptr, scans_per_stream + s0,
+                             sp ? &chunk_sp : nullptr);
+  }
+  cs->parity ^= 1u;
+  cs->prev_stamped = sp != nullptr;
+  RPL_CUDA(c, cudaEventRecord(cs->done, st), RPL_RESULT_OPERATION_FAIL);
+  return r;
 }
 
 }  // namespace
@@ -1478,7 +1662,10 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   for (int p = 0; p < 2; ++p) {
     cudaFree(cs->arena[p]);
     cudaFree(cs->carry_len[p]);
+    cudaFree(cs->open_ts[p]);
   }
+  cudaFree(cs->held_rx);
+  cudaFree(cs->scan_ends);
   for (int i = 0; i < kLanes; ++i) cudaFree(cs->lane_buf[i]);
   cudaFree(cs->held);
   cudaFree(cs->status);
@@ -1496,77 +1683,38 @@ rpl_result rpl_capsule_stream_push(rpl_capsule_stream* cs, const uint8_t* capsul
                                    uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
                                    float* intensities, uint32_t* beam_counts, float* angle_increment,
                                    uint32_t* scans_per_stream) {
-  if (!cs) return RPL_RESULT_INVALID_DATA;
-  rpl_ctx* c = cs->c;
-  if (!capsule_stream_args_ok(cs, capsules, capsule_counts, sample_duration_us, params, ranges, intensities,
-                              beam_counts, scans_per_stream))
-    return RPL_RESULT_INVALID_DATA;
-  for (uint32_t s = 0; s < cs->n_streams; ++s)
-    if (capsule_counts[s] > cs->stride_capsules) {
-      c->err = cs->ans_type == RPL_ANS_MEASUREMENT ? "byte_counts[s] exceeds stride_bytes"
-                                                   : "capsule_counts[s] exceeds stride_capsules";
-      return RPL_RESULT_INVALID_DATA;
-    }
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  for (int i = 0; i < kLanes; ++i) RPL_CUDA(c, cudaStreamWaitEvent(c->lane[i].stream, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
-  const size_t cap_bytes_stream = (size_t)cs->stride_capsules * cs->cap_bytes, row = (size_t)cs->max_scans * cs->max_nodes;
-  const cudaMemcpyKind h2d = cudaMemcpyHostToDevice, d2h = cudaMemcpyDeviceToHost;
-  auto run_chunk = [&](Lane& l, uint32_t s0, uint32_t ns) -> rpl_result {
-    unsigned char* d = cs->lane_buf[&l - c->lane];
-    const size_t nsc = (size_t)ns * cs->max_scans;
-    RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);  // the lane's previous chunk has left
-    RPL_CUDA(c, cudaMemcpyAsync(d, capsules + s0 * cap_bytes_stream, ns * cap_bytes_stream, h2d, l.stream),
-             RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(d + cs->o_ccnt, capsule_counts + s0, (size_t)ns * 4, h2d, l.stream),
-             RPL_RESULT_OPERATION_FAIL);
-    const rpl_result r = capsule_stream_chunk(
-        cs, l, l.stream, s0, ns, d, reinterpret_cast<uint32_t*>(d + cs->o_ccnt), sample_duration_us, params,
-        reinterpret_cast<float*>(d + cs->o_r), reinterpret_cast<float*>(d + cs->o_i),
-        reinterpret_cast<uint32_t*>(d + cs->o_b), reinterpret_cast<float*>(d + cs->o_inc),
-        reinterpret_cast<uint32_t*>(d + cs->o_sps));
-    if (r != RPL_RESULT_OK) return r;
-    const size_t so = (size_t)s0 * cs->max_scans;
-    RPL_CUDA(c, cudaMemcpyAsync(ranges + so * cs->max_nodes, d + cs->o_r, ns * row * 4, d2h, l.stream),
-             RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(intensities + so * cs->max_nodes, d + cs->o_i, ns * row * 4, d2h, l.stream),
-             RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(beam_counts + so, d + cs->o_b, nsc * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
-    if (angle_increment)
-      RPL_CUDA(c, cudaMemcpyAsync(angle_increment + so, d + cs->o_inc, nsc * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(scans_per_stream + s0, d + cs->o_sps, (size_t)ns * 4, d2h, l.stream),
-             RPL_RESULT_OPERATION_FAIL);
-    return RPL_RESULT_OK;
-  };
-  const rpl_result r = run_chunks(c, cs->n_streams, cs->chunk_host, run_chunk);
-  cs->parity ^= 1u;
-  return r;
+  return stream_push(cs, capsules, capsule_counts, sample_duration_us, params, ranges, intensities, beam_counts,
+                     angle_increment, scans_per_stream, nullptr);
 }
 
 rpl_result rpl_capsule_stream_push_dev(rpl_capsule_stream* cs, const uint8_t* capsules, const uint32_t* capsule_counts,
                                        uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
                                        float* intensities, uint32_t* beam_counts, float* angle_increment,
                                        uint32_t* scans_per_stream, void* stream) {
-  if (!cs) return RPL_RESULT_INVALID_DATA;
-  rpl_ctx* c = cs->c;
-  if (!capsule_stream_args_ok(cs, capsules, capsule_counts, sample_duration_us, params, ranges, intensities,
-                              beam_counts, scans_per_stream))
-    return RPL_RESULT_INVALID_DATA;
-  cudaStream_t st;
-  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
-  RPL_CUDA(c, cudaStreamWaitEvent(st, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
-  const size_t row = (size_t)cs->max_scans * cs->max_nodes;
-  rpl_result r = RPL_RESULT_OK;
-  for (uint32_t s0 = 0; s0 < cs->n_streams && r == RPL_RESULT_OK; s0 += cs->chunk_dev) {
-    const uint32_t ns = std::min(cs->chunk_dev, cs->n_streams - s0);
-    const size_t so = (size_t)s0 * cs->max_scans;
-    r = capsule_stream_chunk(cs, c->lane[0], st, s0, ns, capsules + (size_t)s0 * cs->stride_capsules * cs->cap_bytes,
-                             capsule_counts + s0, sample_duration_us, params, ranges + (size_t)s0 * row,
-                             intensities + (size_t)s0 * row, beam_counts + so,
-                             angle_increment ? angle_increment + so : nullptr, scans_per_stream + s0);
-  }
-  cs->parity ^= 1u;
-  RPL_CUDA(c, cudaEventRecord(cs->done, st), RPL_RESULT_OPERATION_FAIL);
-  return r;
+  return stream_push_dev(cs, capsules, capsule_counts, sample_duration_us, params, ranges, intensities, beam_counts,
+                         angle_increment, scans_per_stream, stream, nullptr);
+}
+
+rpl_result rpl_capsule_stream_push_ts(rpl_capsule_stream* cs, const uint8_t* capsules, const uint32_t* capsule_counts,
+                                      const rpl_timing* timing, const uint64_t* capsule_rx_us,
+                                      const rpl_scan_params* params, float* ranges, float* intensities,
+                                      uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
+                                      uint64_t* scan_begin_ts_us) {
+  StampPush sp{};
+  if (!stamp_args_ok(cs, timing, capsule_rx_us, 1, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
+  return stream_push(cs, capsules, capsule_counts, timing->sample_duration_us, params, ranges, intensities,
+                     beam_counts, angle_increment, scans_per_stream, &sp);
+}
+
+rpl_result rpl_capsule_stream_push_ts_dev(rpl_capsule_stream* cs, const uint8_t* capsules,
+                                          const uint32_t* capsule_counts, const rpl_timing* timing,
+                                          const uint64_t* capsule_rx_us, const rpl_scan_params* params, float* ranges,
+                                          float* intensities, uint32_t* beam_counts, float* angle_increment,
+                                          uint32_t* scans_per_stream, uint64_t* scan_begin_ts_us, void* stream) {
+  StampPush sp{};
+  if (!stamp_args_ok(cs, timing, capsule_rx_us, 1, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
+  return stream_push_dev(cs, capsules, capsule_counts, timing->sample_duration_us, params, ranges, intensities,
+                         beam_counts, angle_increment, scans_per_stream, stream, &sp);
 }
 
 rpl_result rpl_capsule_stream_reset(rpl_capsule_stream* cs, const uint8_t* stream_mask) {
@@ -1586,6 +1734,8 @@ rpl_result rpl_capsule_stream_reset(rpl_capsule_stream* cs, const uint8_t* strea
     RPL_CUDA(c, cudaMemsetAsync(cs->held + (size_t)s * rpl::kHeldWords, 0, (size_t)(e - s) * rpl::kHeldWords * 4, st),
              RPL_RESULT_OPERATION_FAIL);
     RPL_CUDA(c, cudaMemsetAsync(cs->carry_len[p] + s, 0, (size_t)(e - s) * 4, st), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemsetAsync(cs->open_ts[p] + s, 0, (size_t)(e - s) * 8, st), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemsetAsync(cs->held_rx + s, 0, (size_t)(e - s) * 8, st), RPL_RESULT_OPERATION_FAIL);
     s = e;
   }
   RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);
@@ -1636,6 +1786,26 @@ rpl_result rpl_dense_stream_push_dev(rpl_dense_stream* ds, const uint8_t* capsul
                                      intensities, beam_counts, angle_increment, scans_per_stream, stream);
 }
 
+rpl_result rpl_dense_stream_push_ts(rpl_dense_stream* ds, const uint8_t* capsules, const uint32_t* capsule_counts,
+                                    const rpl_timing* timing, const uint64_t* capsule_rx_us,
+                                    const rpl_scan_params* params, float* ranges, float* intensities,
+                                    uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
+                                    uint64_t* scan_begin_ts_us) {
+  return rpl_capsule_stream_push_ts(capsule_session(ds), capsules, capsule_counts, timing, capsule_rx_us, params,
+                                    ranges, intensities, beam_counts, angle_increment, scans_per_stream,
+                                    scan_begin_ts_us);
+}
+
+rpl_result rpl_dense_stream_push_ts_dev(rpl_dense_stream* ds, const uint8_t* capsules, const uint32_t* capsule_counts,
+                                        const rpl_timing* timing, const uint64_t* capsule_rx_us,
+                                        const rpl_scan_params* params, float* ranges, float* intensities,
+                                        uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
+                                        uint64_t* scan_begin_ts_us, void* stream) {
+  return rpl_capsule_stream_push_ts_dev(capsule_session(ds), capsules, capsule_counts, timing, capsule_rx_us, params,
+                                        ranges, intensities, beam_counts, angle_increment, scans_per_stream,
+                                        scan_begin_ts_us, stream);
+}
+
 rpl_result rpl_dense_stream_reset(rpl_dense_stream* ds, const uint8_t* stream_mask) {
   return rpl_capsule_stream_reset(capsule_session(ds), stream_mask);
 }
@@ -1669,6 +1839,30 @@ rpl_result rpl_normal_stream_push_dev(rpl_normal_stream* ns, const uint8_t* byte
                                       void* stream) {
   return rpl_capsule_stream_push_dev(capsule_session(ns), bytes, byte_counts, 0, params, ranges, intensities,
                                      beam_counts, angle_increment, scans_per_stream, stream);
+}
+
+rpl_result rpl_normal_stream_push_ts(rpl_normal_stream* ns, const uint8_t* bytes, const uint32_t* byte_counts,
+                                     const rpl_timing* timing, uint32_t chunk_bytes, const uint64_t* chunk_rx_us,
+                                     const rpl_scan_params* params, float* ranges, float* intensities,
+                                     uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
+                                     uint64_t* scan_begin_ts_us) {
+  rpl_capsule_stream* cs = capsule_session(ns);
+  StampPush sp{};
+  if (!stamp_args_ok(cs, timing, chunk_rx_us, chunk_bytes, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
+  return stream_push(cs, bytes, byte_counts, 0, params, ranges, intensities, beam_counts, angle_increment,
+                     scans_per_stream, &sp);
+}
+
+rpl_result rpl_normal_stream_push_ts_dev(rpl_normal_stream* ns, const uint8_t* bytes, const uint32_t* byte_counts,
+                                         const rpl_timing* timing, uint32_t chunk_bytes, const uint64_t* chunk_rx_us,
+                                         const rpl_scan_params* params, float* ranges, float* intensities,
+                                         uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
+                                         uint64_t* scan_begin_ts_us, void* stream) {
+  rpl_capsule_stream* cs = capsule_session(ns);
+  StampPush sp{};
+  if (!stamp_args_ok(cs, timing, chunk_rx_us, chunk_bytes, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
+  return stream_push_dev(cs, bytes, byte_counts, 0, params, ranges, intensities, beam_counts, angle_increment,
+                         scans_per_stream, stream, &sp);
 }
 
 rpl_result rpl_normal_stream_reset(rpl_normal_stream* ns, const uint8_t* stream_mask) {

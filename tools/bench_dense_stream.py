@@ -19,6 +19,11 @@ against the stateless device path (rpl_decode_normal_batch_dev -> rpl_assemble_s
 per-push latency of push and push_dev for 512 streams x {100, 1000, 10000} bytes (at 115200 baud a standard-mode lidar
 delivers about 11500 bytes per second).
 
+With --stamped (any --format), stamped pushes (rpl_*_stream_push_ts_dev, receive times in, scan-begin stamps out)
+against unstamped ones on the same data and shapes: the chain shape above for 0x85, the comparison shapes above for the
+other formats; two sessions, timed in alternating rounds in one run.  Also the host push of a 25 ms receive period
+(512 streams x 80 dense capsules, or the format's equivalent), stamped and unstamped, with the bytes each copies.
+
 Each push continues the stream where the previous one ended (the capsules of a push follow on in angle), so the carry
 and the held capsule are exercised as in a live feed.  The GPU's name and power limit are part of the output.
 """
@@ -278,6 +283,98 @@ def compare_stateless(R, torch, fmt, steps):
     return res
 
 
+def compare_stamped(R, torch, fmt, steps, rounds):
+    """ms per push_dev of a stamped and an unstamped session on the same data, alternating rounds of `steps` pushes;
+    and ms per host push of a 25 ms receive period, stamped and unstamped"""
+    n_streams, max_nodes, max_scans = 512, 4096, 56
+    if fmt == 0x81:
+        cb, n_units, host_units = 1, 163840 * 5, 1000
+        data = feed_normal(16, 2 * n_units, seed=7)
+    elif fmt == 0x85:
+        cb, n_units, host_units = 84, 4096, 80
+        data = feed(16, 2 * n_units, seed=7)
+    else:
+        cb, _, n_units, cpr = FORMATS[fmt]
+        host_units = int(round(cpr))  # one revolution, as the dense session's 80 capsules
+        data = feed_format(fmt, 16, 2 * n_units, seed=7)
+    chunk_bytes = 64  # 0x81: one receive time per 64 bytes
+    n_rx = -(-n_units // chunk_bytes) if fmt == 0x81 else n_units
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    params = R.scan_params(1, 0, 0, 1)
+    timing = R.Timing(31, 0, 0, 0)
+    ctx = R.Context(0, max_nodes, n_streams * max_scans)
+    NS = n_streams * max_scans
+    reps = (n_streams // 16,) + (1,) * (data.ndim - 1)
+    with torch.cuda.stream(stream):
+        halves = [torch.from_numpy(np.ascontiguousarray(np.tile(data[:, h * n_units:(h + 1) * n_units], reps))).to(dev)
+                  for h in (0, 1)]
+        d_cnt = torch.full((n_streams,), n_units, dtype=torch.int32, device=dev)
+        rx = [(torch.arange(n_streams * n_rx, device=dev, dtype=torch.int64) * 10 + 10_000_000 + h).reshape(n_streams, n_rx)
+              for h in (0, 1)]
+        r = torch.empty((NS, max_nodes), device=dev)
+        it = torch.empty((NS, max_nodes), device=dev)
+        bc = torch.zeros(NS, dtype=torch.int32, device=dev)
+        inc = torch.zeros(NS, device=dev)
+        sps = torch.zeros(n_streams, dtype=torch.int32, device=dev)
+        ts = torch.zeros(NS, dtype=torch.int64, device=dev)
+    cs = stream.cuda_stream
+
+    def session(stride):
+        if fmt == 0x81:
+            return R.NormalStreamSession(ctx, n_streams, stride, max_nodes, max_scans)
+        return R.CapsuleStreamSession(ctx, fmt, n_streams, stride, max_nodes, max_scans)
+
+    def stamp_kw(rx_ptr, ts_ptr):
+        if fmt == 0x81:
+            return dict(chunk_bytes=chunk_bytes, chunk_rx_us=rx_ptr, timing=timing, scan_begin_ts_us=ts_ptr)
+        return dict(rx_us=rx_ptr, timing=timing, scan_begin_ts_us=ts_ptr)
+
+    res = {"format": hex(fmt), "streams": n_streams, "units_per_push": n_units, "unit_bytes": cb, "max_nodes": max_nodes,
+           "max_scans": max_scans, "steps": steps, "rounds": rounds, "plain_ms": [], "stamped_ms": []}
+    with session(n_units) as plain, session(n_units) as stamped:
+        def push_plain(t):
+            plain.push_dev(halves[t % 2].data_ptr(), d_cnt.data_ptr(), params, r.data_ptr(), it.data_ptr(),
+                           bc.data_ptr(), inc.data_ptr(), sps.data_ptr(), stream=cs)
+
+        def push_stamped(t):
+            stamped.push_dev(halves[t % 2].data_ptr(), d_cnt.data_ptr(), params, r.data_ptr(), it.data_ptr(),
+                             bc.data_ptr(), inc.data_ptr(), sps.data_ptr(), stream=cs,
+                             **stamp_kw(rx[t % 2].data_ptr(), ts.data_ptr()))
+
+        for _ in range(rounds):
+            res["plain_ms"].append(timed(torch, stream, push_plain, steps))
+            res["stamped_ms"].append(timed(torch, stream, push_stamped, steps))
+        res["scans_per_push"] = int(sps.cpu().sum())
+    res["plain_ms_median"] = float(np.median(res["plain_ms"]))
+    res["stamped_ms_median"] = float(np.median(res["stamped_ms"]))
+    res["stamped_over_plain"] = res["stamped_ms_median"] / res["plain_ms_median"] - 1.0
+    # host pushes of one receive period: input bytes and the receive times' extra bytes, copied per push
+    h_data = np.ascontiguousarray(np.tile(data[:, :host_units], reps))
+    h_cnt = np.full(n_streams, host_units, np.uint32)
+    h_rx_n = -(-host_units // chunk_bytes) if fmt == 0x81 else host_units
+    h_rx = np.arange(n_streams * h_rx_n, dtype=np.uint64).reshape(n_streams, h_rx_n) + 10_000_000
+    out = pinned_outputs(torch, n_streams, max_nodes, max_scans)
+    out["scan_begin_ts_us"] = torch.zeros(NS, dtype=torch.int64).pin_memory().numpy().view(np.uint64)
+    host = {"units_per_push": host_units, "input_bytes": int(h_data.nbytes), "rx_bytes": int(h_rx.nbytes),
+            "plain_ms": [], "stamped_ms": []}
+    with session(host_units) as plain, session(host_units) as stamped:
+        kw = dict(chunk_bytes=chunk_bytes, chunk_rx_us=h_rx, timing=timing) if fmt == 0x81 else \
+            dict(rx_us=h_rx, timing=timing)
+        for t in range(4 + 2 * steps):
+            for sess, extra, key in ((plain, {}, "plain_ms"), (stamped, kw, "stamped_ms")):
+                t0 = time.perf_counter()
+                sess.push(h_data, h_cnt, params, out=out, **extra)
+                if t >= 4:
+                    host[key].append((time.perf_counter() - t0) * 1e3)
+    host["plain_ms_median"] = float(np.median(host.pop("plain_ms")))
+    host["stamped_ms_median"] = float(np.median(host.pop("stamped_ms")))
+    host["stamped_over_plain"] = host["stamped_ms_median"] / host["plain_ms_median"] - 1.0
+    res["host_push"] = host
+    ctx.close()
+    return res
+
+
 def gpu_info():
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                        capture_output=True, text=True)
@@ -290,10 +387,16 @@ def main():
     ap.add_argument("--steps", type=int, default=20, help="timed pushes of the throughput point")
     ap.add_argument("--format", type=lambda v: int(v, 0), default=0x85, choices=[0x81, 0x82, 0x83, 0x84, 0x85, 0x86],
                     help="answer type (default 0x85: the dense session's latency and throughput points)")
+    ap.add_argument("--stamped", action="store_true", help="stamped against unstamped pushes of --format")
+    ap.add_argument("--rounds", type=int, default=5, help="--stamped: alternating rounds of --steps pushes each")
     args = ap.parse_args()
     import torch
 
     import rplidar_ros2_driver_b200 as R
+
+    if args.stamped:
+        print(json.dumps({"gpu": gpu_info(), "stamped": compare_stamped(R, torch, args.format, args.steps, args.rounds)}))
+        return
 
     if args.format == 0x81:
         print(json.dumps({"gpu": gpu_info(), "comparison": compare_normal(R, torch, args.steps),

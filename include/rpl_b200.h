@@ -452,8 +452,9 @@ rpl_result rpl_chain_dense_laserscan(rpl_ctx* ctx, const uint8_t* capsules, cons
  *   create:  ans_type 0x82 express, 0x83 HQ, 0x84 ultra, 0x85 dense or 0x86 ultra-dense (0x81 and anything else:
  *            RPL_RESULT_INVALID_DATA); n_streams, stride_capsules (most capsules per stream in one push), max_nodes
  *            (even, <= 8192: the holder capacity and the output row), max_scans (slots per stream per push); the
- *            context's max_scans must cover one stream's max_scans.  The session borrows the context (its lanes and the
- *            assembler scratch) and is destroyed before it.  Device memory: two node arenas of
+ *            context's max_scans must cover one stream's max_scans.  The session borrows the context (its lanes, whose
+ *            staging memory a host push grows to what it needs, and the assembler scratch) and is destroyed before
+ *            it.  Device memory of its own: two node arenas of
  *            n_streams * (max_nodes + rpl_capsule_nodes(ans_type) * stride_capsules) nodes each (DESIGN.md 5.7), which
  *            must stay below 2^32 nodes, plus per-capsule reports.
  *   push:    host buffers, synchronous, chunked (about 16 MiB of capsules) over the context's two lanes: capsules

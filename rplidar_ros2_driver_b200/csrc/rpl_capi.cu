@@ -45,55 +45,41 @@ void free_lane(Lane& l) {
   cudaFree(l.gws.vidx);
   cudaFree(l.gws.cell);
   if (l.owns_cws) rpl::cloud_workspace_free(l.cws);
-  cudaFree(l.d_nodes);
-  cudaFree(l.d_nodes_out);
-  cudaFree(l.d_counts);
-  cudaFree(l.d_ranges);
-  cudaFree(l.d_intens);
-  cudaFree(l.d_beams);
-  cudaFree(l.d_inc);
-  cudaFree(l.d_status);
-  cudaFree(l.d_path);
-  cudaFree(l.d_xyzi);
-  cudaFree(l.d_pcount);
-  cudaFree(l.d_chain);
+  cudaFree(l.stage);
   if (l.stream) cudaStreamDestroy(l.stream);
   l = Lane{};
 }
 
-rpl_result ensure_staging(rpl_ctx* c, Lane& l, uint32_t scans, size_t nodes, bool cloud) {
-  if (l.staged_nodes < nodes || l.staged_scans < scans) {
-    cudaFree(l.d_nodes);
-    cudaFree(l.d_nodes_out);
-    cudaFree(l.d_ranges);
-    cudaFree(l.d_intens);
-    cudaFree(l.d_counts);
-    cudaFree(l.d_beams);
-    cudaFree(l.d_inc);
-    cudaFree(l.d_status);
-    cudaFree(l.d_path);
-    cudaFree(l.d_xyzi);
-    cudaFree(l.d_pcount);
-    l.d_nodes = l.d_nodes_out = nullptr;
-    l.d_ranges = l.d_intens = l.d_inc = l.d_xyzi = nullptr;
-    l.d_counts = l.d_beams = l.d_status = l.d_path = l.d_pcount = nullptr;
-    l.staged_nodes = 0;
-    l.staged_scans = 0;
-    const rpl_result oom = RPL_RESULT_INSUFFICIENT_MEMORY;
-    RPL_CUDA(c, dev_alloc(&l.d_nodes, nodes), oom);
-    RPL_CUDA(c, dev_alloc(&l.d_nodes_out, nodes), oom);
-    RPL_CUDA(c, dev_alloc(&l.d_ranges, nodes), oom);
-    RPL_CUDA(c, dev_alloc(&l.d_intens, nodes), oom);
-    RPL_CUDA(c, dev_alloc(&l.d_counts, scans), oom);
-    RPL_CUDA(c, dev_alloc(&l.d_beams, scans), oom);
-    RPL_CUDA(c, dev_alloc(&l.d_inc, scans), oom);
-    RPL_CUDA(c, dev_alloc(&l.d_status, scans), oom);
-    RPL_CUDA(c, dev_alloc(&l.d_path, scans), oom);
-    RPL_CUDA(c, dev_alloc(&l.d_pcount, scans), oom);
-    l.staged_nodes = nodes;
-    l.staged_scans = scans;
+// Carves consecutive 256-byte-aligned regions off a lane's staging block; with base == nullptr it only counts their
+// bytes, so that one layout function both sizes the block and lays it out.  Regions lie in the order they are taken;
+// a braced list is evaluated left to right, so a layout may take them all in the initializer of its Regions struct.
+struct Carve {
+  unsigned char* base = nullptr;
+  size_t bytes = 0;
+  template <class T>
+  T* take(size_t count) {
+    T* p = base ? reinterpret_cast<T*>(base + bytes) : nullptr;
+    bytes += (count * sizeof(T) + 255) & ~(size_t)255;
+    return p;
   }
-  if (cloud && !l.d_xyzi) RPL_CUDA(c, dev_alloc(&l.d_xyzi, l.staged_nodes * 4), RPL_RESULT_INSUFFICIENT_MEMORY);
+};
+
+// Grows the staging blocks of lanes [0, lanes) to what layout(Carve&) takes.  Called before a call's chunk loop only:
+// a lane's stream is drained before its block is replaced, since an earlier call's copies may still use it.
+template <class Layout>
+rpl_result grow_stage(rpl_ctx* c, int lanes, Layout layout) {
+  Carve k;
+  layout(k);
+  for (int i = 0; i < lanes; ++i) {
+    Lane& l = c->lane[i];
+    if (l.stage_bytes >= k.bytes) continue;
+    RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);
+    cudaFree(l.stage);
+    l.stage = nullptr;
+    l.stage_bytes = 0;
+    RPL_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&l.stage), k.bytes), RPL_RESULT_INSUFFICIENT_MEMORY);
+    l.stage_bytes = k.bytes;
+  }
   return RPL_RESULT_OK;
 }
 
@@ -501,10 +487,18 @@ rpl_result rpl_scan_batch(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t* 
   uint32_t chunk = (uint32_t)std::max<size_t>(1, target_nodes / stride);
   chunk = std::min(chunk, n_scans);
   const bool want_scan = ranges != nullptr;
-  for (int i = 0; i < kLanes; ++i) {
-    rpl_result r = ensure_staging(c, c->lane[i], chunk, (size_t)chunk * stride, false);
-    if (r != RPL_RESULT_OK) return r;
-  }
+  struct Regions {
+    rpl_node_hq *nodes, *nodes_out;
+    float *ranges, *intens, *inc;
+    uint32_t *counts, *beams, *status, *path;
+  };
+  auto layout = [&, cnt = (size_t)chunk * stride](Carve& k) {
+    const size_t scan = want_scan ? cnt : 0;
+    return Regions{k.take<rpl_node_hq>(cnt), k.take<rpl_node_hq>(nodes_out ? cnt : 0), k.take<float>(scan),
+                   k.take<float>(scan), k.take<float>(chunk), k.take<uint32_t>(chunk), k.take<uint32_t>(chunk),
+                   k.take<uint32_t>(chunk), k.take<uint32_t>(chunk)};
+  };
+  if (const rpl_result r = grow_stage(c, kLanes, layout); r != RPL_RESULT_OK) return r;
   const cudaMemcpyKind h2d = cudaMemcpyHostToDevice, d2h = cudaMemcpyDeviceToHost;
   std::memcpy(c->h_counts, counts, (size_t)n_scans * sizeof(uint32_t));
   uint32_t* hs_beams = c->h_small;
@@ -514,43 +508,44 @@ rpl_result rpl_scan_batch(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t* 
   // one chunk through one lane
   auto run_chunk = [&](Lane& l, uint32_t s0, uint32_t ns) -> rpl_result {
     const size_t off = (size_t)s0 * stride, cnt = (size_t)ns * stride;
+    Carve k{l.stage};
+    const Regions d = layout(k);
     // the lane's previous chunk (2 chunks ago) must have left its staging buffers
     RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(l.d_nodes, nodes + off, cnt * sizeof(rpl_node_hq), h2d, l.stream),
+    RPL_CUDA(c, cudaMemcpyAsync(d.nodes, nodes + off, cnt * sizeof(rpl_node_hq), h2d, l.stream),
              RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(l.d_counts, c->h_counts + s0, ns * sizeof(uint32_t), h2d, l.stream),
+    RPL_CUDA(c, cudaMemcpyAsync(d.counts, c->h_counts + s0, ns * sizeof(uint32_t), h2d, l.stream),
              RPL_RESULT_OPERATION_FAIL);
     // The kernels write only the first counts[s] nodes of a scan they ascend (nothing for an empty or
     // unmeasured scan: the reference leaves those buffers untouched).  The whole [ns][stride] region goes
     // back to the caller, so it starts out as the caller's own bytes, not as leftovers of an earlier chunk.
     if (nodes_out && params->apply_ascend)
-      RPL_CUDA(c, cudaMemcpyAsync(l.d_nodes_out, l.d_nodes, cnt * sizeof(rpl_node_hq), cudaMemcpyDeviceToDevice, l.stream),
+      RPL_CUDA(c, cudaMemcpyAsync(d.nodes_out, d.nodes, cnt * sizeof(rpl_node_hq), cudaMemcpyDeviceToDevice, l.stream),
                RPL_RESULT_OPERATION_FAIL);
-    rpl_result r = enqueue_scan(c, l, reinterpret_cast<rpl_node_hq*>(l.d_nodes), l.d_counts, ns, stride,
-                                params, nodes_out ? reinterpret_cast<rpl_node_hq*>(l.d_nodes_out) : nullptr,
-                                want_scan ? l.d_ranges : nullptr, want_scan ? l.d_intens : nullptr,
-                                l.d_beams, l.d_inc, l.d_status, l.d_path, l.stream);
+    rpl_result r = enqueue_scan(c, l, d.nodes, d.counts, ns, stride, params, nodes_out ? d.nodes_out : nullptr,
+                                want_scan ? d.ranges : nullptr, want_scan ? d.intens : nullptr, d.beams, d.inc,
+                                d.status, d.path, l.stream);
     if (r != RPL_RESULT_OK) return r;
     if (nodes_out)
-      RPL_CUDA(c, cudaMemcpyAsync(nodes_out + off, l.d_nodes_out, cnt * sizeof(rpl_node_hq), d2h, l.stream),
+      RPL_CUDA(c, cudaMemcpyAsync(nodes_out + off, d.nodes_out, cnt * sizeof(rpl_node_hq), d2h, l.stream),
                RPL_RESULT_OPERATION_FAIL);
     if (want_scan) {
-      RPL_CUDA(c, cudaMemcpyAsync(ranges + off, l.d_ranges, cnt * sizeof(float), d2h, l.stream),
+      RPL_CUDA(c, cudaMemcpyAsync(ranges + off, d.ranges, cnt * sizeof(float), d2h, l.stream),
                RPL_RESULT_OPERATION_FAIL);
-      RPL_CUDA(c, cudaMemcpyAsync(intensities + off, l.d_intens, cnt * sizeof(float), d2h, l.stream),
+      RPL_CUDA(c, cudaMemcpyAsync(intensities + off, d.intens, cnt * sizeof(float), d2h, l.stream),
                RPL_RESULT_OPERATION_FAIL);
     }
     if (beam_counts)
-      RPL_CUDA(c, cudaMemcpyAsync(hs_beams + s0, l.d_beams, ns * sizeof(uint32_t), d2h, l.stream),
+      RPL_CUDA(c, cudaMemcpyAsync(hs_beams + s0, d.beams, ns * sizeof(uint32_t), d2h, l.stream),
                RPL_RESULT_OPERATION_FAIL);
     if (angle_increment)
-      RPL_CUDA(c, cudaMemcpyAsync(hs_inc + s0, l.d_inc, ns * sizeof(float), d2h, l.stream),
+      RPL_CUDA(c, cudaMemcpyAsync(hs_inc + s0, d.inc, ns * sizeof(float), d2h, l.stream),
                RPL_RESULT_OPERATION_FAIL);
     if (status)
-      RPL_CUDA(c, cudaMemcpyAsync(hs_status + s0, l.d_status, ns * sizeof(uint32_t), d2h, l.stream),
+      RPL_CUDA(c, cudaMemcpyAsync(hs_status + s0, d.status, ns * sizeof(uint32_t), d2h, l.stream),
                RPL_RESULT_OPERATION_FAIL);
     if (path)
-      RPL_CUDA(c, cudaMemcpyAsync(hs_path + s0, l.d_path, ns * sizeof(uint32_t), d2h, l.stream),
+      RPL_CUDA(c, cudaMemcpyAsync(hs_path + s0, d.path, ns * sizeof(uint32_t), d2h, l.stream),
                RPL_RESULT_OPERATION_FAIL);
     return RPL_RESULT_OK;
   };
@@ -859,15 +854,6 @@ rpl_result rpl_decode_capsules_batch_dev(rpl_ctx* c, uint32_t ans_type, const ui
   return decode_capsules_launch(c, ans_type, a, stream);
 }
 
-namespace {
-// one stream from host buffers through a device-side entry: shared by the capsule and byte decoders
-struct HostDecode {
-  unsigned char* d = nullptr;
-  size_t o_nodes = 0, o_st = 0, o_off = 0, o_small = 0;
-  ~HostDecode() { cudaFree(d); }
-};
-}  // namespace
-
 rpl_result rpl_decode_capsules(rpl_ctx* c, uint32_t ans_type, const uint8_t* capsules, uint32_t n_capsules,
                                uint32_t sample_duration_us, uint32_t* state, rpl_node_hq* nodes_out,
                                uint32_t* node_count, uint32_t* capsule_status, uint32_t* capsule_node_offset,
@@ -885,33 +871,31 @@ rpl_result rpl_decode_capsules(rpl_ctx* c, uint32_t ans_type, const uint8_t* cap
   if (n_capsules == 0) return RPL_RESULT_OK;
   cudaStream_t st;
   if (!enter_device(c, nullptr, &st)) return RPL_RESULT_OPERATION_FAIL;
-  const size_t cb = (size_t)n_capsules * cbytes, nb = (size_t)n_capsules * per * 8, sb = (size_t)n_capsules * 4;
-  HostDecode h;  // [capsules | pad][nodes][status][offsets][count, n_nodes, state in x2, state out x2][rx][ts]
-  h.o_nodes = (cb + 15) & ~(size_t)15;
-  h.o_st = h.o_nodes + nb;
-  h.o_off = h.o_st + sb;
-  h.o_small = h.o_off + sb;
-  const size_t o_rx = (h.o_small + 32 + 7) & ~(size_t)7, o_ts = o_rx + (size_t)n_capsules * 8;
-  const size_t total_bytes = want_ts ? o_ts + (size_t)n_capsules * per * 8 : h.o_small + 32;
-  RPL_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&h.d), total_bytes), RPL_RESULT_INSUFFICIENT_MEMORY);
+  const size_t sb = (size_t)n_capsules * 4;
+  // small: count, n_nodes, state in x2, state out x2
+  struct Regions { uint8_t* caps; rpl_node_hq* nodes; uint32_t *status, *offsets, *small; uint64_t *rx, *ts; };
+  auto layout = [&](Carve& k) {
+    const size_t n = n_capsules, ts = want_ts ? n : 0;
+    return Regions{k.take<uint8_t>(n * cbytes), k.take<rpl_node_hq>(n * per), k.take<uint32_t>(n), k.take<uint32_t>(n),
+                   k.take<uint32_t>(8), k.take<uint64_t>(ts), k.take<uint64_t>(ts * per)};
+  };
+  if (const rpl_result r = grow_stage(c, 1, layout); r != RPL_RESULT_OK) return r;
+  Carve k{c->lane[0].stage};
+  const Regions d = layout(k);
   uint32_t small[8] = {n_capsules, 0u, state ? state[0] : 0u, state ? state[1] : 0u, 0u, 0u, 0u, 0u};
-  RPL_CUDA(c, cudaMemcpyAsync(h.d, capsules, cb, cudaMemcpyHostToDevice, st), RPL_RESULT_OPERATION_FAIL);
-  RPL_CUDA(c, cudaMemcpyAsync(h.d + h.o_small, small, 32, cudaMemcpyHostToDevice, st), RPL_RESULT_OPERATION_FAIL);
-  uint32_t* ds = reinterpret_cast<uint32_t*>(h.d + h.o_small);
-  rpl_result r = rpl_decode_capsules_batch_dev(c, ans_type, h.d, ds, 1, n_capsules, sample_duration_us, ds + 2,
-                                               reinterpret_cast<rpl_node_hq*>(h.d + h.o_nodes), ds + 1,
-                                               reinterpret_cast<uint32_t*>(h.d + h.o_st),
-                                               reinterpret_cast<uint32_t*>(h.d + h.o_off), ds + 4, st);
+  RPL_CUDA(c, cudaMemcpyAsync(d.caps, capsules, (size_t)n_capsules * cbytes, cudaMemcpyHostToDevice, st),
+           RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaMemcpyAsync(d.small, small, 32, cudaMemcpyHostToDevice, st), RPL_RESULT_OPERATION_FAIL);
+  rpl_result r = rpl_decode_capsules_batch_dev(c, ans_type, d.caps, d.small, 1, n_capsules, sample_duration_us,
+                                               d.small + 2, d.nodes, d.small + 1, d.status, d.offsets, d.small + 4, st);
   if (r != RPL_RESULT_OK) return r;
   if (want_ts) {
-    RPL_CUDA(c, cudaMemcpyAsync(h.d + o_rx, capsule_rx_us, (size_t)n_capsules * 8, cudaMemcpyHostToDevice, st),
+    RPL_CUDA(c, cudaMemcpyAsync(d.rx, capsule_rx_us, (size_t)n_capsules * 8, cudaMemcpyHostToDevice, st),
              RPL_RESULT_OPERATION_FAIL);
-    r = rpl_node_timestamps_dev(c, ans_type, timing, reinterpret_cast<const uint64_t*>(h.d + o_rx),
-                                reinterpret_cast<uint32_t*>(h.d + h.o_st), reinterpret_cast<uint32_t*>(h.d + h.o_off), ds,
-                                1, n_capsules, reinterpret_cast<uint64_t*>(h.d + o_ts), st);
+    r = rpl_node_timestamps_dev(c, ans_type, timing, d.rx, d.status, d.offsets, d.small, 1, n_capsules, d.ts, st);
     if (r != RPL_RESULT_OK) return r;
   }
-  RPL_CUDA(c, cudaMemcpyAsync(small, ds, 32, cudaMemcpyDeviceToHost, st), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaMemcpyAsync(small, d.small, 32, cudaMemcpyDeviceToHost, st), RPL_RESULT_OPERATION_FAIL);
   RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);
   *node_count = small[1];
   if (state) {
@@ -919,14 +903,12 @@ rpl_result rpl_decode_capsules(rpl_ctx* c, uint32_t ans_type, const uint8_t* cap
     state[1] = small[5];
   }
   if (want_ts)
-    RPL_CUDA(c, cudaMemcpy(node_ts_us, h.d + o_ts, (size_t)small[1] * 8, cudaMemcpyDeviceToHost),
-             RPL_RESULT_OPERATION_FAIL);
-  RPL_CUDA(c, cudaMemcpy(nodes_out, h.d + h.o_nodes, (size_t)small[1] * 8, cudaMemcpyDeviceToHost),
-           RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpy(node_ts_us, d.ts, (size_t)small[1] * 8, cudaMemcpyDeviceToHost), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaMemcpy(nodes_out, d.nodes, (size_t)small[1] * 8, cudaMemcpyDeviceToHost), RPL_RESULT_OPERATION_FAIL);
   if (capsule_status)
-    RPL_CUDA(c, cudaMemcpy(capsule_status, h.d + h.o_st, sb, cudaMemcpyDeviceToHost), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpy(capsule_status, d.status, sb, cudaMemcpyDeviceToHost), RPL_RESULT_OPERATION_FAIL);
   if (capsule_node_offset)
-    RPL_CUDA(c, cudaMemcpy(capsule_node_offset, h.d + h.o_off, sb, cudaMemcpyDeviceToHost), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpy(capsule_node_offset, d.offsets, sb, cudaMemcpyDeviceToHost), RPL_RESULT_OPERATION_FAIL);
   return RPL_RESULT_OK;
 }
 
@@ -988,22 +970,23 @@ rpl_result rpl_decode_normal(rpl_ctx* c, const uint8_t* bytes, uint32_t n_bytes,
   if (n_bytes < 5) return RPL_RESULT_OK;
   cudaStream_t st;
   if (!enter_device(c, nullptr, &st)) return RPL_RESULT_OPERATION_FAIL;
-  HostDecode h;  // [bytes | pad][nodes][byte count, node count]
-  h.o_nodes = ((size_t)n_bytes + 15) & ~(size_t)15;
-  h.o_small = h.o_nodes + (size_t)(n_bytes / 5) * 8;
-  RPL_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&h.d), h.o_small + 16), RPL_RESULT_INSUFFICIENT_MEMORY);
+  struct Regions { uint8_t* bytes; rpl_node_hq* nodes; uint32_t* small; };  // small: byte count, node count
+  auto layout = [&](Carve& k) {
+    return Regions{k.take<uint8_t>(n_bytes), k.take<rpl_node_hq>(n_bytes / 5), k.take<uint32_t>(2)};
+  };
+  if (const rpl_result r = grow_stage(c, 1, layout); r != RPL_RESULT_OK) return r;
+  Carve k{c->lane[0].stage};
+  const Regions d = layout(k);
   uint32_t small[2] = {n_bytes, 0u};
-  RPL_CUDA(c, cudaMemcpyAsync(h.d, bytes, n_bytes, cudaMemcpyHostToDevice, st), RPL_RESULT_OPERATION_FAIL);
-  RPL_CUDA(c, cudaMemcpyAsync(h.d + h.o_small, small, 8, cudaMemcpyHostToDevice, st), RPL_RESULT_OPERATION_FAIL);
-  uint32_t* ds = reinterpret_cast<uint32_t*>(h.d + h.o_small);
-  rpl_result r = rpl_decode_normal_batch_dev(c, h.d, ds, 1, n_bytes, reinterpret_cast<rpl_node_hq*>(h.d + h.o_nodes),
-                                             ds + 1, nullptr, nullptr, st);
+  RPL_CUDA(c, cudaMemcpyAsync(d.bytes, bytes, n_bytes, cudaMemcpyHostToDevice, st), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaMemcpyAsync(d.small, small, 8, cudaMemcpyHostToDevice, st), RPL_RESULT_OPERATION_FAIL);
+  const rpl_result r =
+      rpl_decode_normal_batch_dev(c, d.bytes, d.small, 1, n_bytes, d.nodes, d.small + 1, nullptr, nullptr, st);
   if (r != RPL_RESULT_OK) return r;
-  RPL_CUDA(c, cudaMemcpyAsync(small, ds, 8, cudaMemcpyDeviceToHost, st), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaMemcpyAsync(small, d.small, 8, cudaMemcpyDeviceToHost, st), RPL_RESULT_OPERATION_FAIL);
   RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);
   *node_count = small[1];
-  RPL_CUDA(c, cudaMemcpy(nodes_out, h.d + h.o_nodes, (size_t)small[1] * 8, cudaMemcpyDeviceToHost),
-           RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaMemcpy(nodes_out, d.nodes, (size_t)small[1] * 8, cudaMemcpyDeviceToHost), RPL_RESULT_OPERATION_FAIL);
   return RPL_RESULT_OK;
 }
 
@@ -1156,106 +1139,6 @@ rpl_result rpl_scan_views_dev(rpl_ctx* c, const rpl_node_hq* nodes, uint64_t nod
                       reinterpret_cast<const uint2*>(views), nodes_total);
 }
 
-// ---- wire bytes -> LaserScan in one host call --------------------------------------------------------------------
-rpl_result rpl_chain_dense_laserscan(rpl_ctx* c, const uint8_t* capsules, const uint32_t* capsule_counts,
-                                     uint32_t n_streams, uint32_t stride_capsules, uint32_t sample_duration_us,
-                                     const rpl_scan_params* params, uint32_t max_nodes, uint32_t max_scans,
-                                     float* ranges, float* intensities, uint32_t* beam_counts, float* angle_increment,
-                                     uint32_t* scans_per_stream) {
-  if (!c || !capsules || !capsule_counts || !params || !ranges || !intensities || !beam_counts || !scans_per_stream)
-    return RPL_RESULT_INVALID_DATA;
-  if (n_streams == 0) return RPL_RESULT_OK;
-  if (max_nodes == 0 || max_nodes > rpl::kSmallMaxNodes || (max_nodes & 1u) || max_scans == 0 || stride_capsules == 0) {
-    c->err = "need an even max_nodes in [2, 8192] (the longest revolution), max_scans > 0, stride_capsules > 0";
-    return RPL_RESULT_INVALID_DATA;
-  }
-  for (uint32_t s = 0; s < n_streams; ++s)
-    if (capsule_counts[s] > stride_capsules) {
-      c->err = "capsule_counts[s] exceeds stride_capsules";
-      return RPL_RESULT_INVALID_DATA;
-    }
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  // chunk: about 16 MiB of capsules (~64 MiB of decoded nodes), whole streams
-  const size_t cap_bytes_stream = (size_t)stride_capsules * 84;
-  uint32_t chunk = (uint32_t)std::max<size_t>(1, ((size_t)16 << 20) / cap_bytes_stream);
-  chunk = std::min(chunk, n_streams);
-  if ((size_t)chunk * max_scans > c->max_scans) chunk = c->max_scans / max_scans;
-  if (chunk == 0) {
-    c->err = "the context's max_scans is smaller than max_scans of one stream";
-    return RPL_RESULT_INVALID_DATA;
-  }
-  const size_t nodes_stream = (size_t)stride_capsules * 40;
-  if ((size_t)chunk * nodes_stream > 0xFFFFFFFFull) {
-    c->err = "chunk too large for 32-bit views";
-    return RPL_RESULT_INVALID_DATA;
-  }
-  auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
-  const size_t NS = (size_t)chunk * max_scans;
-  const uint32_t starts_stride = 2 * max_scans + 64;  // scan starts per stream the decoder may list
-  const size_t o_caps = 0, o_ccnt = o_caps + up(chunk * cap_bytes_stream), o_nodes = o_ccnt + up((size_t)chunk * 4),
-               o_ncnt = o_nodes + up(chunk * nodes_stream * 8), o_st = o_ncnt + up((size_t)chunk * 4),
-               o_off = o_st + up((size_t)chunk * stride_capsules * 4), o_views = o_off + up((size_t)chunk * stride_capsules * 4),
-               o_slen = o_views + up(NS * 8), o_sps = o_slen + up(NS * 4), o_r = o_sps + up((size_t)chunk * 4),
-               o_i = o_r + up(NS * max_nodes * 4), o_b = o_i + up(NS * max_nodes * 4), o_inc = o_b + up(NS * 4),
-               o_starts = o_inc + up(NS * 4), o_scnt = o_starts + up((size_t)chunk * starts_stride * 4),
-               total = o_scnt + up((size_t)chunk * 4);
-  for (int i = 0; i < kLanes; ++i) {
-    Lane& l = c->lane[i];
-    if (l.chain_bytes < total) {
-      RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);
-      cudaFree(l.d_chain);
-      l.d_chain = nullptr;
-      l.chain_bytes = 0;
-      RPL_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&l.d_chain), total), RPL_RESULT_INSUFFICIENT_MEMORY);
-      l.chain_bytes = total;
-    }
-  }
-  const cudaMemcpyKind h2d = cudaMemcpyHostToDevice, d2h = cudaMemcpyDeviceToHost;
-  auto run_chunk = [&](Lane& l, uint32_t s0, uint32_t ns) -> rpl_result {
-    unsigned char* d = l.d_chain;
-    const size_t nsc = (size_t)ns * max_scans;
-    RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);  // the lane's previous chunk has left
-    RPL_CUDA(c, cudaMemcpyAsync(d + o_caps, capsules + (size_t)s0 * cap_bytes_stream, ns * cap_bytes_stream, h2d, l.stream),
-             RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(d + o_ccnt, capsule_counts + s0, (size_t)ns * 4, h2d, l.stream), RPL_RESULT_OPERATION_FAIL);
-    rpl_result r = rpl_decode_dense_batch_starts_dev(
-        c, d + o_caps, reinterpret_cast<uint32_t*>(d + o_ccnt), ns, stride_capsules, sample_duration_us, nullptr,
-        reinterpret_cast<rpl_node_hq*>(d + o_nodes), reinterpret_cast<uint32_t*>(d + o_ncnt),
-        reinterpret_cast<uint32_t*>(d + o_st), reinterpret_cast<uint32_t*>(d + o_off), nullptr,
-        reinterpret_cast<uint32_t*>(d + o_starts), starts_stride, reinterpret_cast<uint32_t*>(d + o_scnt), l.stream);
-    if (r != RPL_RESULT_OK) return r;
-    // the assembler's scratch belongs to the context, not to the lane: one assemble kernel at a time
-    if (!c->asm_done) RPL_CUDA(c, cudaEventCreateWithFlags(&c->asm_done, cudaEventDisableTiming), RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaStreamWaitEvent(l.stream, c->asm_done, 0), RPL_RESULT_OPERATION_FAIL);
-    r = rpl_assemble_scan_views_starts_dev(c, reinterpret_cast<rpl_node_hq*>(d + o_nodes), reinterpret_cast<uint32_t*>(d + o_ncnt), ns,
-                                    (uint32_t)nodes_stream, reinterpret_cast<uint32_t*>(d + o_st),
-                                    reinterpret_cast<uint32_t*>(d + o_off), reinterpret_cast<uint32_t*>(d + o_ccnt),
-                                    stride_capsules, reinterpret_cast<uint32_t*>(d + o_starts), starts_stride,
-                                    reinterpret_cast<uint32_t*>(d + o_scnt), max_nodes, max_scans,
-                                    reinterpret_cast<rpl_scan_view*>(d + o_views),
-                                    reinterpret_cast<uint32_t*>(d + o_slen), reinterpret_cast<uint32_t*>(d + o_sps), nullptr,
-                                    nullptr, l.stream);
-    if (r != RPL_RESULT_OK) return r;
-    RPL_CUDA(c, cudaEventRecord(c->asm_done, l.stream), RPL_RESULT_OPERATION_FAIL);
-    r = enqueue_scan(c, l, reinterpret_cast<rpl_node_hq*>(d + o_nodes), reinterpret_cast<uint32_t*>(d + o_slen),
-                     (uint32_t)nsc, max_nodes, params, nullptr, reinterpret_cast<float*>(d + o_r),
-                     reinterpret_cast<float*>(d + o_i), reinterpret_cast<uint32_t*>(d + o_b),
-                     reinterpret_cast<float*>(d + o_inc), nullptr, nullptr, l.stream,
-                     reinterpret_cast<const uint2*>(d + o_views), (unsigned long long)ns * nodes_stream);
-    if (r != RPL_RESULT_OK) return r;
-    const size_t so = (size_t)s0 * max_scans;
-    RPL_CUDA(c, cudaMemcpyAsync(ranges + so * max_nodes, d + o_r, nsc * max_nodes * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(intensities + so * max_nodes, d + o_i, nsc * max_nodes * 4, d2h, l.stream),
-             RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(beam_counts + so, d + o_b, nsc * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
-    if (angle_increment)
-      RPL_CUDA(c, cudaMemcpyAsync(angle_increment + so, d + o_inc, nsc * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(scans_per_stream + s0, d + o_sps, (size_t)ns * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
-    return RPL_RESULT_OK;
-  };
-  return run_chunks(c, n_streams, chunk, run_chunk);
-}
-
 }  // extern "C"
 
 // ---- capsule stream session (DESIGN.md 5.7) ------------------------------------------------------------------------
@@ -1284,9 +1167,6 @@ struct rpl_capsule_stream {
   uint32_t *starts = nullptr, *start_counts = nullptr;  // dense only: the decoder's scan-start list
   uint32_t* scan_len = nullptr;
   rpl_scan_view* views = nullptr;
-  unsigned char* lane_buf[kLanes] = {nullptr, nullptr};  // host-push staging: capsules, counts and outputs of a chunk
-  size_t o_ccnt = 0, o_r = 0, o_i = 0, o_b = 0, o_inc = 0, o_sps = 0, lane_bytes = 0;
-  size_t o_ts = 0, o_rx = 0;                    // stamped host pushes: scan stamps, then receive times of a chunk
   cudaEvent_t done = nullptr;                   // the last push_dev: later calls on other streams wait for it
   unsigned long long* open_ts[2] = {nullptr, nullptr};  // [n_streams] stamp of the open revolution (0: unknown)
   unsigned long long* held_rx = nullptr;        // [n_streams] express, ultra: receive time of the held capsule
@@ -1308,33 +1188,78 @@ struct StampPush {
   unsigned long long* scan_ts;          // scan_begin_ts_us [.][max_scans]
 };
 
-// decode -> assemble -> scan kernels for streams [s0, s0 + ns) on `st`; capsules / counts / outputs / sp point at s0's
-rpl_result capsule_stream_chunk(rpl_capsule_stream* cs, Lane& l, cudaStream_t st, uint32_t s0, uint32_t ns,
+// Where a chunk of streams lives on the device between the kernels of capsule_stream_chunk, every pointer at the
+// chunk's first stream.  A session's chunk decodes behind node_first carry slots per stream (node_stride != 0),
+// keeps the held record and hands the open revolution to the other arena.  The chain's has no held record, no carry
+// and node_stride 0, so that the decoder and the assembler run their stateless kernels.
+struct WireChunk {
+  uint32_t ans_type, stride_capsules, max_nodes, max_scans, starts_stride;
+  uint32_t stride_nodes;             // each stream's region of `nodes`
+  uint32_t node_stride, node_first;  // the decoder's: a session's stride_nodes and max_nodes; 0, 0 for the chain
+  rpl_node_hq *nodes, *carry_out;
+  uint32_t *node_counts, *scan_len, *held, *carry_len_out;
+  const uint32_t* carry_len;
+  uint32_t *status, *offsets;       // capsule formats only: the per-capsule reports (scan-reset requests)
+  uint32_t *starts, *start_counts;  // dense only: the decoder's scan-start list (others: the assembler's flag pass)
+  rpl_scan_view* views;
+  // a stamped session push's: 0x81 scan-start record ends, the open revolution's stamp, the held capsule's rx
+  uint32_t* node_end;
+  unsigned long long *open_ts_in, *open_ts_out, *held_rx;
+  bool prev_stamped;
+};
+
+// session cs's chunk from stream s0 in the push under way (arena cs->parity)
+WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0) {
+  const uint32_t p = cs->parity, sc = cs->stride_capsules;
+  const size_t sn = (size_t)s0 * cs->stride_nodes, so = (size_t)s0 * cs->max_scans;
+  WireChunk w{};
+  w.ans_type = cs->ans_type;
+  w.stride_capsules = sc;
+  w.max_nodes = cs->max_nodes;
+  w.max_scans = cs->max_scans;
+  w.stride_nodes = w.node_stride = cs->stride_nodes;
+  w.node_first = cs->max_nodes;
+  w.starts_stride = cs->starts_stride;
+  w.nodes = cs->arena[p] + sn;
+  w.node_counts = cs->node_counts + s0;
+  w.status = cs->status ? cs->status + (size_t)s0 * sc : nullptr;
+  w.offsets = cs->offsets ? cs->offsets + (size_t)s0 * sc : nullptr;
+  w.starts = cs->starts ? cs->starts + (size_t)s0 * cs->starts_stride : nullptr;
+  w.start_counts = cs->starts ? cs->start_counts + s0 : nullptr;
+  w.views = cs->views + so;
+  w.scan_len = cs->scan_len + so;
+  w.held = cs->held + (size_t)s0 * rpl::kHeldWords;
+  w.carry_len = cs->carry_len[p] + s0;
+  w.carry_out = cs->arena[p ^ 1u] + sn;
+  w.carry_len_out = cs->carry_len[p ^ 1u] + s0;
+  w.node_end = cs->scan_ends ? cs->scan_ends + (size_t)s0 * (cs->stride_nodes - cs->max_nodes) : nullptr;
+  w.open_ts_in = cs->open_ts[p] + s0;
+  w.open_ts_out = cs->open_ts[p ^ 1u] + s0;
+  w.held_rx = cs->held_rx + s0;
+  w.prev_stamped = cs->prev_stamped;
+  return w;
+}
+
+// decode -> assemble -> scan kernels for the ns streams of chunk w on `st`; capsules / counts / outputs / sp point at
+// the chunk's first stream's
+rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const WireChunk& w, uint32_t ns,
                                 const uint8_t* capsules, const uint32_t* counts, uint32_t sample_duration_us,
                                 const rpl_scan_params* params, float* ranges, float* intens, uint32_t* beams,
                                 float* inc, uint32_t* scans_per_stream, const StampPush* sp = nullptr) {
-  rpl_ctx* c = cs->c;
-  const uint32_t p = cs->parity, sc = cs->stride_capsules, new_nodes = cs->stride_nodes - cs->max_nodes;
-  uint32_t* ends = sp && cs->scan_ends ? cs->scan_ends + (size_t)s0 * new_nodes : nullptr;
-  rpl_node_hq* nodes = cs->arena[p] + (size_t)s0 * cs->stride_nodes;
-  // capsule formats only: the per-capsule reports, which carry the scan-reset requests to the assembler
-  uint32_t* status = cs->status ? cs->status + (size_t)s0 * sc : nullptr;
-  uint32_t* offsets = cs->offsets ? cs->offsets + (size_t)s0 * sc : nullptr;
-  // only the dense decoder lists its scan starts; the assembler finds the others' with its flag pass
-  uint32_t* starts = cs->starts ? cs->starts + (size_t)s0 * cs->starts_stride : nullptr;
-  uint32_t* start_counts = cs->starts ? cs->start_counts + s0 : nullptr;
+  const uint32_t sc = w.stride_capsules;
+  uint32_t* ends = sp ? w.node_end : nullptr;
   rpl_result r;
-  if (cs->ans_type == RPL_ANS_MEASUREMENT) {
+  if (w.ans_type == RPL_ANS_MEASUREMENT) {
     rpl::NormalDecodeArgs a{};
     a.bytes = capsules;
     a.byte_counts = counts;
     a.n_streams = ns;
     a.stride_bytes = sc;
-    a.nodes_out = reinterpret_cast<uint2*>(nodes);
-    a.node_counts = cs->node_counts + s0;
-    a.held = cs->held + (size_t)s0 * rpl::kHeldWords;
-    a.node_stride = cs->stride_nodes;
-    a.node_first = cs->max_nodes;
+    a.nodes_out = reinterpret_cast<uint2*>(w.nodes);
+    a.node_counts = w.node_counts;
+    a.held = w.held;
+    a.node_stride = w.node_stride;
+    a.node_first = w.node_first;
     a.node_end = ends;
     r = decode_normal_launch(c, a, st);
   } else {
@@ -1345,49 +1270,120 @@ rpl_result capsule_stream_chunk(rpl_capsule_stream* cs, Lane& l, cudaStream_t st
     a.stride_capsules = sc;
     a.sample_duration_us = sample_duration_us;
     a.state_words = 1;
-    a.nodes_out = reinterpret_cast<uint2*>(nodes);
-    a.node_counts = cs->node_counts + s0;
-    a.capsule_status = status;
-    a.capsule_node_offset = offsets;
-    a.scan_starts = starts;
-    a.scan_start_counts = start_counts;
-    a.starts_stride = cs->starts_stride;
-    a.held = cs->held + (size_t)s0 * rpl::kHeldWords;
-    a.node_stride = cs->stride_nodes;
-    a.node_first = cs->max_nodes;
-    r = decode_capsules_launch(c, cs->ans_type, a, st);
+    a.nodes_out = reinterpret_cast<uint2*>(w.nodes);
+    a.node_counts = w.node_counts;
+    a.capsule_status = w.status;
+    a.capsule_node_offset = w.offsets;
+    a.scan_starts = w.starts;
+    a.scan_start_counts = w.start_counts;
+    a.starts_stride = w.starts_stride;
+    a.held = w.held;
+    a.node_stride = w.node_stride;
+    a.node_first = w.node_first;
+    r = decode_capsules_launch(c, w.ans_type, a, st);
   }
   if (r != RPL_RESULT_OK) return r;
-  // the assembler's scratch belongs to the context: one assemble kernel at a time (as in the chain)
+  // the assembler's scratch belongs to the context: one assemble kernel at a time, whatever lane or stream
   if (!c->asm_done) RPL_CUDA(c, cudaEventCreateWithFlags(&c->asm_done, cudaEventDisableTiming), RPL_RESULT_OPERATION_FAIL);
   RPL_CUDA(c, cudaStreamWaitEvent(st, c->asm_done, 0), RPL_RESULT_OPERATION_FAIL);
-  const size_t so = (size_t)s0 * cs->max_scans;
   rpl::AssembleStampArgs t{};
   if (sp) {
-    t.ans_type = cs->ans_type;
+    t.ans_type = w.ans_type;
     t.timing = sp->timing;
-    t.capsule_rx_us = status ? sp->rx : nullptr;
+    t.capsule_rx_us = w.status ? sp->rx : nullptr;
     t.node_end = ends;
-    t.stride_ends = new_nodes;
+    t.stride_ends = w.stride_nodes - w.node_first;
     t.chunk_bytes = sp->chunk_bytes;
     t.stride_chunks = sp->stride_chunks;
-    t.chunk_rx_us = status ? nullptr : sp->rx;
-    t.open_ts_in = cs->open_ts[p] + s0;
-    t.open_ts_out = cs->open_ts[p ^ 1u] + s0;
-    t.held_rx = cs->held_rx + s0;
-    t.prev_stamped = cs->prev_stamped ? 1u : 0u;
+    t.chunk_rx_us = w.status ? nullptr : sp->rx;
+    t.open_ts_in = w.open_ts_in;
+    t.open_ts_out = w.open_ts_out;
+    t.held_rx = w.held_rx;
+    t.prev_stamped = w.prev_stamped ? 1u : 0u;
   }
-  r = assemble_common(c, nodes, cs->node_counts + s0, ns, cs->stride_nodes, status, offsets, status ? counts : nullptr,
-                      status ? sc : 0u, cs->max_nodes, cs->max_scans, cs->max_nodes, nullptr, cs->views + so,
-                      cs->scan_len + so, scans_per_stream, nullptr,
-                      sp ? reinterpret_cast<uint64_t*>(sp->scan_ts) : nullptr, st, starts,
-                      starts ? cs->starts_stride : 0u, start_counts, cs->carry_len[p] + s0,
-                      cs->arena[p ^ 1u] + (size_t)s0 * cs->stride_nodes, cs->carry_len[p ^ 1u] + s0, sp ? &t : nullptr);
+  r = assemble_common(c, w.nodes, w.node_counts, ns, w.stride_nodes, w.status, w.offsets, w.status ? counts : nullptr,
+                      w.status ? sc : 0u, w.max_nodes, w.max_scans, w.max_nodes, nullptr, w.views, w.scan_len,
+                      scans_per_stream, nullptr, sp ? reinterpret_cast<uint64_t*>(sp->scan_ts) : nullptr, st, w.starts,
+                      w.starts ? w.starts_stride : 0u, w.start_counts, w.carry_len, w.carry_out, w.carry_len_out,
+                      sp ? &t : nullptr);
   if (r != RPL_RESULT_OK) return r;
   RPL_CUDA(c, cudaEventRecord(c->asm_done, st), RPL_RESULT_OPERATION_FAIL);
-  return enqueue_scan(c, l, nodes, cs->scan_len + so, ns * cs->max_scans, cs->max_nodes, params, nullptr, ranges, intens,
-                      beams, inc, nullptr, nullptr, st, reinterpret_cast<const uint2*>(cs->views + so),
-                      (unsigned long long)ns * cs->stride_nodes);
+  return enqueue_scan(c, l, w.nodes, w.scan_len, ns * w.max_scans, w.max_nodes, params, nullptr, ranges, intens, beams,
+                      inc, nullptr, nullptr, st, reinterpret_cast<const uint2*>(w.views),
+                      (unsigned long long)ns * w.stride_nodes);
+}
+
+// A host call's wire input and LaserScan outputs: host arrays of all its streams (the chain's, a session's host push)
+struct HostWire {
+  const uint8_t* capsules;  // [n_streams][in_stream bytes]
+  const uint32_t* counts;
+  size_t in_stream;
+  uint32_t sample_duration_us, max_nodes, max_scans;
+  const rpl_scan_params* params;
+  float *ranges, *intensities, *angle_increment;  // angle_increment nullable
+  uint32_t *beam_counts, *scans_per_stream;
+  const StampPush* sp;  // a stamped push: receive times in, scan stamps out
+  size_t rx_stream;     // receive times per stream of a stamped push
+};
+
+// Runs a host call's n_streams streams through capsule_stream_chunk, `chunk` streams at a time round-robin over the
+// lanes: H2D of a chunk's input (and receive times), its kernels, D2H of its LaserScans (and stamps).  A lane's
+// staging block holds one chunk's input and outputs, then whatever chunk_at(k, s0) carves off k for the device state
+// of the chunk from stream s0, which it returns (the chain's lives there; a session's in its arenas).
+template <class ChunkAt>
+rpl_result push_host(rpl_ctx* c, const HostWire& h, uint32_t n_streams, uint32_t chunk, ChunkAt chunk_at) {
+  const size_t NS = (size_t)chunk * h.max_scans, row = (size_t)h.max_scans * h.max_nodes;
+  using u64 = unsigned long long;
+  struct Regions {
+    uint8_t* in;
+    uint32_t* counts;
+    u64* rx;
+    float *ranges, *intens, *inc;
+    uint32_t *beams, *sps;
+    u64* ts;
+    WireChunk w;
+  };
+  auto layout = [&](Carve& k, uint32_t s0) {
+    return Regions{k.take<uint8_t>(chunk * h.in_stream), k.take<uint32_t>(chunk),
+                   k.take<u64>(h.sp ? chunk * h.rx_stream : 0), k.take<float>(NS * h.max_nodes),
+                   k.take<float>(NS * h.max_nodes), k.take<float>(NS), k.take<uint32_t>(NS), k.take<uint32_t>(chunk),
+                   k.take<u64>(h.sp ? NS : 0), chunk_at(k, s0)};
+  };
+  if (const rpl_result r = grow_stage(c, kLanes, [&](Carve& k) { layout(k, 0); }); r != RPL_RESULT_OK) return r;
+  const cudaMemcpyKind h2d = cudaMemcpyHostToDevice, d2h = cudaMemcpyDeviceToHost;
+  auto run_chunk = [&](Lane& l, uint32_t s0, uint32_t ns) -> rpl_result {
+    Carve k{l.stage};
+    const Regions d = layout(k, s0);
+    const size_t so = (size_t)s0 * h.max_scans, nsc = (size_t)ns * h.max_scans;
+    RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);  // the lane's previous chunk has left
+    RPL_CUDA(c, cudaMemcpyAsync(d.in, h.capsules + s0 * h.in_stream, ns * h.in_stream, h2d, l.stream),
+             RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(d.counts, h.counts + s0, (size_t)ns * 4, h2d, l.stream), RPL_RESULT_OPERATION_FAIL);
+    StampPush sp{};
+    if (h.sp) {
+      sp = *h.sp;
+      sp.rx = d.rx;
+      sp.scan_ts = d.ts;
+      RPL_CUDA(c, cudaMemcpyAsync(d.rx, h.sp->rx + s0 * h.rx_stream, ns * h.rx_stream * 8, h2d, l.stream),
+               RPL_RESULT_OPERATION_FAIL);
+    }
+    const rpl_result r = capsule_stream_chunk(c, l, l.stream, d.w, ns, d.in, d.counts, h.sample_duration_us, h.params,
+                                              d.ranges, d.intens, d.beams, d.inc, d.sps, h.sp ? &sp : nullptr);
+    if (r != RPL_RESULT_OK) return r;
+    if (h.sp)
+      RPL_CUDA(c, cudaMemcpyAsync(h.sp->scan_ts + so, d.ts, nsc * 8, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(h.ranges + so * h.max_nodes, d.ranges, ns * row * 4, d2h, l.stream),
+             RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(h.intensities + so * h.max_nodes, d.intens, ns * row * 4, d2h, l.stream),
+             RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(h.beam_counts + so, d.beams, nsc * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
+    if (h.angle_increment)
+      RPL_CUDA(c, cudaMemcpyAsync(h.angle_increment + so, d.inc, nsc * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(h.scans_per_stream + s0, d.sps, (size_t)ns * 4, d2h, l.stream),
+             RPL_RESULT_OPERATION_FAIL);
+    return RPL_RESULT_OK;
+  };
+  return run_chunks(c, n_streams, chunk, run_chunk);
 }
 
 bool capsule_stream_args_ok(rpl_capsule_stream* cs, const uint8_t* capsules, const uint32_t* capsule_counts,
@@ -1452,18 +1448,6 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint
   // host pushes: about 16 MiB of capsules per chunk, whole streams (as in the chain)
   const size_t cap_bytes_stream = (size_t)stride_capsules * cap_bytes;
   cs->chunk_host = std::min<uint32_t>(cs->chunk_dev, (uint32_t)std::max<size_t>(1, ((size_t)16 << 20) / cap_bytes_stream));
-  auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
-  const size_t NS = (size_t)cs->chunk_host * max_scans;
-  cs->o_ccnt = up((size_t)cs->chunk_host * cap_bytes_stream);
-  cs->o_r = cs->o_ccnt + up((size_t)cs->chunk_host * 4);
-  cs->o_i = cs->o_r + up(NS * max_nodes * 4);
-  cs->o_b = cs->o_i + up(NS * max_nodes * 4);
-  cs->o_inc = cs->o_b + up(NS * 4);
-  cs->o_sps = cs->o_inc + up(NS * 4);
-  cs->o_ts = cs->o_sps + up((size_t)cs->chunk_host * 4);
-  cs->o_rx = cs->o_ts + up(NS * 8);
-  // 0x81: the receive times' count depends on each push's chunk_bytes, and a stamped push grows the buffers to it
-  cs->lane_bytes = cs->o_rx + (normal ? 0 : up((size_t)cs->chunk_host * stride_capsules * 8));
   const size_t n = n_streams, ncap = n * stride_capsules;
   const rpl_result oom = RPL_RESULT_INSUFFICIENT_MEMORY;
   auto fail = [&](rpl_result r) {
@@ -1481,8 +1465,6 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint
       !cuda_ok(c, cudaMemset(cs->held_rx, 0, n * 8), "cudaMemset"))
     return fail(oom);
   if (normal && !cuda_ok(c, dev_alloc(&cs->scan_ends, n * (size_t)new_nodes), "cudaMalloc")) return fail(oom);
-  for (int i = 0; i < kLanes; ++i)
-    if (!cuda_ok(c, dev_alloc(&cs->lane_buf[i], cs->lane_bytes), "cudaMalloc")) return fail(oom);
   if (ans_type == 0x85 && (!cuda_ok(c, dev_alloc(&cs->starts, n * cs->starts_stride), "cudaMalloc") ||
                            !cuda_ok(c, dev_alloc(&cs->start_counts, n), "cudaMalloc")))
     return fail(oom);
@@ -1544,60 +1526,14 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* capsules, const ui
       return RPL_RESULT_INVALID_DATA;
     }
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  // receive times per stream: one per capsule, 0x81 one per chunk_bytes piece (the lane buffers grow to them)
-  const size_t rx_stream = sp ? (cs->status ? cs->stride_capsules : sp->stride_chunks) : 0;
-  if (sp && cs->o_rx + (size_t)cs->chunk_host * rx_stream * 8 > cs->lane_bytes) {
-    const size_t need = cs->o_rx + (((size_t)cs->chunk_host * rx_stream * 8 + 255) & ~(size_t)255);
-    for (int i = 0; i < kLanes; ++i) {
-      RPL_CUDA(c, cudaStreamSynchronize(c->lane[i].stream), RPL_RESULT_OPERATION_FAIL);
-      cudaFree(cs->lane_buf[i]);
-      cs->lane_buf[i] = nullptr;
-    }
-    cs->lane_bytes = 0;
-    for (int i = 0; i < kLanes; ++i)
-      RPL_CUDA(c, dev_alloc(&cs->lane_buf[i], need), RPL_RESULT_INSUFFICIENT_MEMORY);
-    cs->lane_bytes = need;
-  }
   for (int i = 0; i < kLanes; ++i) RPL_CUDA(c, cudaStreamWaitEvent(c->lane[i].stream, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
-  const size_t cap_bytes_stream = (size_t)cs->stride_capsules * cs->cap_bytes, row = (size_t)cs->max_scans * cs->max_nodes;
-  const cudaMemcpyKind h2d = cudaMemcpyHostToDevice, d2h = cudaMemcpyDeviceToHost;
-  auto run_chunk = [&](Lane& l, uint32_t s0, uint32_t ns) -> rpl_result {
-    unsigned char* d = cs->lane_buf[&l - c->lane];
-    const size_t nsc = (size_t)ns * cs->max_scans;
-    RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);  // the lane's previous chunk has left
-    RPL_CUDA(c, cudaMemcpyAsync(d, capsules + s0 * cap_bytes_stream, ns * cap_bytes_stream, h2d, l.stream),
-             RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(d + cs->o_ccnt, capsule_counts + s0, (size_t)ns * 4, h2d, l.stream),
-             RPL_RESULT_OPERATION_FAIL);
-    StampPush chunk_sp{};
-    if (sp) {
-      chunk_sp = *sp;
-      chunk_sp.rx = reinterpret_cast<const unsigned long long*>(d + cs->o_rx);
-      chunk_sp.scan_ts = reinterpret_cast<unsigned long long*>(d + cs->o_ts);
-      RPL_CUDA(c, cudaMemcpyAsync(d + cs->o_rx, sp->rx + s0 * rx_stream, ns * rx_stream * 8, h2d, l.stream),
-               RPL_RESULT_OPERATION_FAIL);
-    }
-    const rpl_result r = capsule_stream_chunk(
-        cs, l, l.stream, s0, ns, d, reinterpret_cast<uint32_t*>(d + cs->o_ccnt), sample_duration_us, params,
-        reinterpret_cast<float*>(d + cs->o_r), reinterpret_cast<float*>(d + cs->o_i),
-        reinterpret_cast<uint32_t*>(d + cs->o_b), reinterpret_cast<float*>(d + cs->o_inc),
-        reinterpret_cast<uint32_t*>(d + cs->o_sps), sp ? &chunk_sp : nullptr);
-    if (r != RPL_RESULT_OK) return r;
-    const size_t so = (size_t)s0 * cs->max_scans;
-    if (sp)
-      RPL_CUDA(c, cudaMemcpyAsync(sp->scan_ts + so, d + cs->o_ts, nsc * 8, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(ranges + so * cs->max_nodes, d + cs->o_r, ns * row * 4, d2h, l.stream),
-             RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(intensities + so * cs->max_nodes, d + cs->o_i, ns * row * 4, d2h, l.stream),
-             RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(beam_counts + so, d + cs->o_b, nsc * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
-    if (angle_increment)
-      RPL_CUDA(c, cudaMemcpyAsync(angle_increment + so, d + cs->o_inc, nsc * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(scans_per_stream + s0, d + cs->o_sps, (size_t)ns * 4, d2h, l.stream),
-             RPL_RESULT_OPERATION_FAIL);
-    return RPL_RESULT_OK;
-  };
-  const rpl_result r = run_chunks(c, cs->n_streams, cs->chunk_host, run_chunk);
+  // receive times per stream of a stamped push: one per capsule, 0x81 one per chunk_bytes piece
+  const size_t rx_stream = sp ? (cs->status ? cs->stride_capsules : sp->stride_chunks) : 0;
+  const HostWire h{capsules, capsule_counts, (size_t)cs->stride_capsules * cs->cap_bytes, sample_duration_us,
+                   cs->max_nodes, cs->max_scans, params, ranges, intensities, angle_increment, beam_counts,
+                   scans_per_stream, sp, rx_stream};
+  const rpl_result r =
+      push_host(c, h, cs->n_streams, cs->chunk_host, [&](Carve&, uint32_t s0) { return session_chunk(cs, s0); });
   cs->parity ^= 1u;
   cs->prev_stamped = sp != nullptr;
   return r;
@@ -1627,9 +1563,10 @@ rpl_result stream_push_dev(rpl_capsule_stream* cs, const uint8_t* capsules, cons
       chunk_sp.rx += (size_t)s0 * (cs->status ? cs->stride_capsules : sp->stride_chunks);
       chunk_sp.scan_ts += so;
     }
-    r = capsule_stream_chunk(cs, c->lane[0], st, s0, ns, capsules + (size_t)s0 * cs->stride_capsules * cs->cap_bytes,
-                             capsule_counts + s0, sample_duration_us, params, ranges + (size_t)s0 * row,
-                             intensities + (size_t)s0 * row, beam_counts + so,
+    r = capsule_stream_chunk(c, c->lane[0], st, session_chunk(cs, s0), ns,
+                             capsules + (size_t)s0 * cs->stride_capsules * cs->cap_bytes, capsule_counts + s0,
+                             sample_duration_us, params, ranges + (size_t)s0 * row, intensities + (size_t)s0 * row,
+                             beam_counts + so,
                              angle_increment ? angle_increment + so : nullptr, scans_per_stream + s0,
                              sp ? &chunk_sp : nullptr);
   }
@@ -1642,6 +1579,64 @@ rpl_result stream_push_dev(rpl_capsule_stream* cs, const uint8_t* capsules, cons
 }  // namespace
 
 extern "C" {
+
+// ---- wire bytes -> LaserScan in one host call: a fresh dense session's host push, with nothing kept ----------------
+rpl_result rpl_chain_dense_laserscan(rpl_ctx* c, const uint8_t* capsules, const uint32_t* capsule_counts,
+                                     uint32_t n_streams, uint32_t stride_capsules, uint32_t sample_duration_us,
+                                     const rpl_scan_params* params, uint32_t max_nodes, uint32_t max_scans,
+                                     float* ranges, float* intensities, uint32_t* beam_counts, float* angle_increment,
+                                     uint32_t* scans_per_stream) {
+  if (!c || !capsules || !capsule_counts || !params || !ranges || !intensities || !beam_counts || !scans_per_stream)
+    return RPL_RESULT_INVALID_DATA;
+  if (n_streams == 0) return RPL_RESULT_OK;
+  if (max_nodes == 0 || max_nodes > rpl::kSmallMaxNodes || (max_nodes & 1u) || max_scans == 0 || stride_capsules == 0) {
+    c->err = "need an even max_nodes in [2, 8192] (the longest revolution), max_scans > 0, stride_capsules > 0";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  for (uint32_t s = 0; s < n_streams; ++s)
+    if (capsule_counts[s] > stride_capsules) {
+      c->err = "capsule_counts[s] exceeds stride_capsules";
+      return RPL_RESULT_INVALID_DATA;
+    }
+  // chunk: about 16 MiB of capsules (~64 MiB of decoded nodes), whole streams
+  const size_t cap_bytes_stream = (size_t)stride_capsules * 84;
+  uint32_t chunk = (uint32_t)std::max<size_t>(1, ((size_t)16 << 20) / cap_bytes_stream);
+  chunk = std::min(chunk, n_streams);
+  if ((size_t)chunk * max_scans > c->max_scans) chunk = c->max_scans / max_scans;
+  if (chunk == 0) {
+    c->err = "the context's max_scans is smaller than max_scans of one stream";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  const size_t nodes_stream = (size_t)stride_capsules * 40;
+  if ((size_t)chunk * nodes_stream > 0xFFFFFFFFull) {
+    c->err = "chunk too large for 32-bit views";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  if (!sample_duration_ok(c, sample_duration_us)) return RPL_RESULT_INVALID_DATA;
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  // a chunk's decoded nodes, reports, scan-start lists and views sit in the lane block behind its input and outputs
+  auto chunk_at = [&](Carve& k, uint32_t) {
+    WireChunk w{};
+    w.ans_type = 0x85;
+    w.stride_capsules = stride_capsules;
+    w.max_nodes = max_nodes;
+    w.max_scans = max_scans;
+    w.stride_nodes = (uint32_t)nodes_stream;
+    w.starts_stride = 2 * max_scans + 64;  // scan starts per stream the decoder may list
+    w.nodes = k.take<rpl_node_hq>(chunk * nodes_stream);
+    w.node_counts = k.take<uint32_t>(chunk);
+    w.status = k.take<uint32_t>((size_t)chunk * stride_capsules);
+    w.offsets = k.take<uint32_t>((size_t)chunk * stride_capsules);
+    w.starts = k.take<uint32_t>((size_t)chunk * w.starts_stride);
+    w.start_counts = k.take<uint32_t>(chunk);
+    w.views = k.take<rpl_scan_view>((size_t)chunk * max_scans);
+    w.scan_len = k.take<uint32_t>((size_t)chunk * max_scans);
+    return w;
+  };
+  const HostWire h{capsules, capsule_counts, cap_bytes_stream, sample_duration_us, max_nodes, max_scans, params, ranges,
+                   intensities, angle_increment, beam_counts, scans_per_stream, nullptr, 0};
+  return push_host(c, h, n_streams, chunk, chunk_at);
+}
 
 rpl_result rpl_capsule_stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint32_t stride_capsules,
                                      uint32_t max_nodes, uint32_t max_scans, rpl_capsule_stream** out) {
@@ -1666,7 +1661,6 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   }
   cudaFree(cs->held_rx);
   cudaFree(cs->scan_ends);
-  for (int i = 0; i < kLanes; ++i) cudaFree(cs->lane_buf[i]);
   cudaFree(cs->held);
   cudaFree(cs->status);
   cudaFree(cs->offsets);
@@ -2134,19 +2128,25 @@ rpl_result rpl_cloud_batch(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t*
   if (n_scans > c->max_scans) return RPL_RESULT_INVALID_DATA;
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
   Lane& l = c->lane[0];
-  rpl_result r = ensure_staging(c, l, n_scans, (size_t)n_scans * stride, true);
-  if (r != RPL_RESULT_OK) return r;
   const size_t cnt = (size_t)n_scans * stride;
-  RPL_CUDA(c, cudaMemcpyAsync(l.d_nodes, nodes, cnt * sizeof(rpl_node_hq), cudaMemcpyHostToDevice, l.stream),
-           RPL_RESULT_OPERATION_FAIL);
-  RPL_CUDA(c, cudaMemcpyAsync(l.d_counts, counts, n_scans * sizeof(uint32_t), cudaMemcpyHostToDevice, l.stream),
-           RPL_RESULT_OPERATION_FAIL);
-  r = rpl_cloud_batch_dev(c, reinterpret_cast<rpl_node_hq*>(l.d_nodes), l.d_counts, n_scans, stride, params,
-                          l.d_xyzi, l.d_pcount, l.stream);
+  struct Regions { rpl_node_hq* nodes; float* xyzi; uint32_t *counts, *pcount; };
+  auto layout = [&](Carve& k) {
+    return Regions{k.take<rpl_node_hq>(cnt), k.take<float>(cnt * 4), k.take<uint32_t>(n_scans),
+                   k.take<uint32_t>(n_scans)};
+  };
+  rpl_result r = grow_stage(c, 1, layout);
   if (r != RPL_RESULT_OK) return r;
-  RPL_CUDA(c, cudaMemcpyAsync(xyzi, l.d_xyzi, cnt * 4 * sizeof(float), cudaMemcpyDeviceToHost, l.stream),
+  Carve k{l.stage};
+  const Regions d = layout(k);
+  RPL_CUDA(c, cudaMemcpyAsync(d.nodes, nodes, cnt * sizeof(rpl_node_hq), cudaMemcpyHostToDevice, l.stream),
            RPL_RESULT_OPERATION_FAIL);
-  RPL_CUDA(c, cudaMemcpyAsync(point_counts, l.d_pcount, n_scans * sizeof(uint32_t), cudaMemcpyDeviceToHost, l.stream),
+  RPL_CUDA(c, cudaMemcpyAsync(d.counts, counts, n_scans * sizeof(uint32_t), cudaMemcpyHostToDevice, l.stream),
+           RPL_RESULT_OPERATION_FAIL);
+  r = rpl_cloud_batch_dev(c, d.nodes, d.counts, n_scans, stride, params, d.xyzi, d.pcount, l.stream);
+  if (r != RPL_RESULT_OK) return r;
+  RPL_CUDA(c, cudaMemcpyAsync(xyzi, d.xyzi, cnt * 4 * sizeof(float), cudaMemcpyDeviceToHost, l.stream),
+           RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaMemcpyAsync(point_counts, d.pcount, n_scans * sizeof(uint32_t), cudaMemcpyDeviceToHost, l.stream),
            RPL_RESULT_OPERATION_FAIL);
   RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);
   return RPL_RESULT_OK;

@@ -22,24 +22,10 @@ struct Lane {
   rpl::GeneralWorkspace gws{};
   rpl::CloudWorkspace cws{};   // lane 0 owns the tables and the post-pass scratch; the others alias its tables
   bool owns_cws = false;
-  // device staging for host-buffer calls (lazy)
-  uint2* d_nodes = nullptr;
-  uint2* d_nodes_out = nullptr;
-  uint32_t* d_counts = nullptr;
-  float* d_ranges = nullptr;
-  float* d_intens = nullptr;
-  uint32_t* d_beams = nullptr;
-  float* d_inc = nullptr;
-  uint32_t* d_status = nullptr;
-  uint32_t* d_path = nullptr;
-  float* d_xyzi = nullptr;
-  uint32_t* d_pcount = nullptr;
-  size_t staged_nodes = 0;  // capacity in nodes of the staging buffers
-  uint32_t staged_scans = 0;
-  // device staging of rpl_chain_dense_laserscan (lazy): one block carved into capsules, decoded nodes,
-  // per-capsule reports, views and the LaserScan outputs of a chunk of streams
-  unsigned char* d_chain = nullptr;
-  size_t chain_bytes = 0;
+  // device staging of every host-buffer call (batches, the chain, the sessions' host pushes, the single-stream
+  // decoders): one block, grown before a call's chunk loop, that each call carves into the regions of one chunk
+  unsigned char* stage = nullptr;
+  size_t stage_bytes = 0;
 };
 
 struct rpl_ctx {
@@ -65,7 +51,7 @@ struct rpl_ctx {
   uint32_t* d_reset_prefix = nullptr;
   uint2* d_desc = nullptr;
   size_t reset_prefix_cap = 0, desc_cap = 0;
-  cudaEvent_t asm_done = nullptr;   // rpl_chain_dense_laserscan: the assemble scratch above is shared by the lanes
+  cudaEvent_t asm_done = nullptr;   // the wire-to-LaserScan chunks of every lane and stream share the assemble scratch
   bool profile = false;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_fast, prof_general;
 };

@@ -35,7 +35,9 @@
  *                              src/sdk/src/sl_lidar_driver.cpp:272-315
  *   rpl_capsule_stream_*     the capsule unpackers (express, HQ, ultra, dense, ultra-dense) and the ScanDataHolder
  *                              as live, per-stream state across calls: wire capsules pushed in any pieces publish the
- *                              scans of the whole stream (rpl_dense_stream_*: the same, fixed to dense capsules)
+ *                              scans of the whole stream (rpl_dense_stream_*: the same, fixed to dense capsules);
+ *                              rpl_capsule_stream_*_bytes: the raw serial bytes in any pieces, with the unpackers'
+ *                              search for the sync bytes carried across calls
  *   rpl_normal_stream_*      the same for the standard-node unpacker: raw 0x81 bytes pushed in any pieces
  *   rpl_*_stream_push_ts*    a session push that also stamps every published scan with its scan-begin time
  *   rpl_*_cdr_batch_dev      the serialised form of the message scan_pub_->publish hands to the RMW layer
@@ -508,6 +510,58 @@ rpl_result rpl_capsule_stream_push_ts_dev(rpl_capsule_stream* s, const uint8_t* 
                                           uint32_t* scans_per_stream, uint64_t* scan_begin_ts_us, void* stream);
 rpl_result rpl_capsule_stream_reset(rpl_capsule_stream* s, const uint8_t* stream_mask);
 rpl_result rpl_capsule_stream_state(rpl_capsule_stream* s, uint32_t* open_nodes, uint32_t* held_capsule);
+
+/* Byte session: the capsule session fed the RAW serial stream after the answer descriptor, any number of bytes per push,
+ * a push ending anywhere -- what the SDK's protocol codec hands LIDARSampleDataUnpacker::onSampleData.  Per stream the
+ * device also keeps the unpacker's search for the sync bytes (handler_capsules.cpp:107-135 express, :324-353 ultra,
+ * :639-668 dense, :852-880 ultra-dense; handler_hqnode.cpp:95-172 HQ): the search position, the bytes of the unfinished
+ * frame (up to the frame size - 1) and whether bytes were skipped since the last frame (which clears the handler's
+ * _is_previous_capsuledataRdy).  So for ANY split of a stream's bytes into pushes -- between the two sync bytes, inside
+ * a frame, inside a run of skipped bytes -- the scans (and, stamped, their scan-begin stamps) published over the pushes
+ * are those of the SDK's unpacker and ScanDataHolder fed the whole stream.  Each push is framed on the device
+ * (rpl_frame_capsules_dev's framing carried across pushes; HQ: a byte other than 0xA5 is skipped while waiting, a 0xA5
+ * and the 780 bytes behind it are a frame) and then decoded as a framed push of those capsules.
+ *   create_bytes: ans_type 0x82..0x86 (0x81: rpl_normal_stream; anything else RPL_RESULT_INVALID_DATA), stride_bytes
+ *            (most bytes per stream in one push), max_nodes, max_scans: the rules of rpl_capsule_stream_create.  With
+ *            F = ceil(stride_bytes / frame size) (the frames a push can complete) and S = 2 * F capsule slots (F for HQ:
+ *            every frame can follow a run of skipped bytes, reported as one all-zero capsule), the session's own device
+ *            memory is two node arenas of n_streams * (max_nodes + rpl_capsule_nodes(ans_type) * F) nodes of 8 bytes
+ *            (below 2^32 nodes), n_streams * S * (frame size + 16) bytes of framed capsules, their reports and receive
+ *            times, and an 800-byte framer record per stream.
+ *   push_bytes / push_bytes_dev: bytes [n_streams][stride_bytes] (any alignment), byte_counts [n_streams] (<= stride_bytes;
+ *            _dev: counts above it clamped), sample_duration_us and outputs as for rpl_capsule_stream_push.
+ *   push_bytes_ts / push_bytes_ts_dev: stamped, as rpl_normal_stream_push_ts: chunk_rx_us [n_streams][ceil(stride_bytes /
+ *            chunk_bytes)], chunk c the receive time of bytes [c * chunk_bytes, (c + 1) * chunk_bytes) of THIS push; a
+ *            capsule gets the time of the chunk holding its last byte (when the handler completes it), also when it began
+ *            in an earlier push.  chunk_bytes == 0: RPL_RESULT_INVALID_DATA.
+ *   reset:   rpl_capsule_stream_reset, which on a byte session also restarts the search (the handlers' reset()).
+ *   state_bytes: rpl_capsule_stream_state plus held_bytes [n_streams] = bytes of the unfinished frame held for the next
+ *            push (0..frame size - 1; always 0 on a framed session); held_capsule is 0 while skipped bytes wait to be
+ *            reported.  Any pointer nullable.
+ * A framed push (rpl_capsule_stream_push*) on a byte session, or a byte push on a framed session: RPL_RESULT_INVALID_DATA. */
+rpl_result rpl_capsule_stream_create_bytes(rpl_ctx* ctx, uint32_t ans_type, uint32_t n_streams, uint32_t stride_bytes,
+                                           uint32_t max_nodes, uint32_t max_scans, rpl_capsule_stream** out);
+rpl_result rpl_capsule_stream_push_bytes(rpl_capsule_stream* s, const uint8_t* bytes, const uint32_t* byte_counts,
+                                         uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
+                                         float* intensities, uint32_t* beam_counts, float* angle_increment,
+                                         uint32_t* scans_per_stream);
+rpl_result rpl_capsule_stream_push_bytes_dev(rpl_capsule_stream* s, const uint8_t* bytes, const uint32_t* byte_counts,
+                                             uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
+                                             float* intensities, uint32_t* beam_counts, float* angle_increment,
+                                             uint32_t* scans_per_stream, void* stream);
+rpl_result rpl_capsule_stream_push_bytes_ts(rpl_capsule_stream* s, const uint8_t* bytes, const uint32_t* byte_counts,
+                                            const rpl_timing* timing, uint32_t chunk_bytes, const uint64_t* chunk_rx_us,
+                                            const rpl_scan_params* params, float* ranges, float* intensities,
+                                            uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
+                                            uint64_t* scan_begin_ts_us);
+rpl_result rpl_capsule_stream_push_bytes_ts_dev(rpl_capsule_stream* s, const uint8_t* bytes,
+                                                const uint32_t* byte_counts, const rpl_timing* timing,
+                                                uint32_t chunk_bytes, const uint64_t* chunk_rx_us,
+                                                const rpl_scan_params* params, float* ranges, float* intensities,
+                                                uint32_t* beam_counts, float* angle_increment,
+                                                uint32_t* scans_per_stream, uint64_t* scan_begin_ts_us, void* stream);
+rpl_result rpl_capsule_stream_state_bytes(rpl_capsule_stream* s, uint32_t* open_nodes, uint32_t* held_capsule,
+                                          uint32_t* held_bytes);
 
 /* Dense-capsule stream session: rpl_capsule_stream_* fixed to 0x85 (capsules [n_streams][stride_capsules][84], arenas
  * of n_streams * (max_nodes + 40 * stride_capsules) nodes); the first push of a fresh session publishes what

@@ -52,6 +52,8 @@ EXPORTS = [
     "rpl_capsule_stream_create", "rpl_capsule_stream_destroy", "rpl_capsule_stream_push", "rpl_capsule_stream_push_dev",
     "rpl_capsule_stream_reset", "rpl_capsule_stream_state", "rpl_capsule_stream_push_ts",
     "rpl_capsule_stream_push_ts_dev",
+    "rpl_capsule_stream_create_bytes", "rpl_capsule_stream_push_bytes", "rpl_capsule_stream_push_bytes_dev",
+    "rpl_capsule_stream_push_bytes_ts", "rpl_capsule_stream_push_bytes_ts_dev", "rpl_capsule_stream_state_bytes",
     "rpl_normal_stream_create", "rpl_normal_stream_destroy", "rpl_normal_stream_push", "rpl_normal_stream_push_dev",
     "rpl_normal_stream_reset", "rpl_normal_stream_state", "rpl_normal_stream_push_ts", "rpl_normal_stream_push_ts_dev",
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
@@ -219,6 +221,12 @@ def lib() -> C.CDLL:
         "rpl_dense_stream_push_ts_dev": ([vp, vp, vp, PT, vp, PSP, vp, vp, vp, vp, vp, vp, vp], u32),
         "rpl_normal_stream_push_ts": ([vp, vp, vp, PT, u32, vp, PSP, vp, vp, vp, vp, vp, vp], u32),
         "rpl_normal_stream_push_ts_dev": ([vp, vp, vp, PT, u32, vp, PSP, vp, vp, vp, vp, vp, vp, vp], u32),
+        "rpl_capsule_stream_create_bytes": ([vp, u32, u32, u32, u32, u32, C.POINTER(vp)], u32),
+        "rpl_capsule_stream_push_bytes": ([vp, vp, vp, u32, PSP, vp, vp, vp, vp, vp], u32),
+        "rpl_capsule_stream_push_bytes_dev": ([vp, vp, vp, u32, PSP, vp, vp, vp, vp, vp, vp], u32),
+        "rpl_capsule_stream_push_bytes_ts": ([vp, vp, vp, PT, u32, vp, PSP, vp, vp, vp, vp, vp, vp], u32),
+        "rpl_capsule_stream_push_bytes_ts_dev": ([vp, vp, vp, PT, u32, vp, PSP, vp, vp, vp, vp, vp, vp, vp], u32),
+        "rpl_capsule_stream_state_bytes": ([vp, vp, vp, vp], u32),
     }
     for name, (args, res) in sig.items():
         fn = getattr(L, name)  # AttributeError here = the library does not export the ABI
@@ -744,6 +752,69 @@ class NormalStreamSession(CapsuleStreamSession):
             self._h, _p(stream_bytes), _p(byte_counts), C.byref(timing) if timing is not None else None,
             chunk_bytes or 0, _p(chunk_rx_us), C.byref(params), _p(ranges), _p(intensities), _p(beam_counts),
             _p(angle_increment), _p(scans_per_stream), _p(scan_begin_ts_us), _p(stream)))
+
+
+class CapsuleByteStreamSession(CapsuleStreamSession):
+    """rpl_capsule_stream byte session (rpl_capsule_stream_create_bytes): the raw serial bytes of a capsule answer type
+    (0x82..0x86, after the answer descriptor) pushed in any pieces, with the unpackers' search for the sync bytes carried
+    across pushes; scans published as the whole stream would publish them.  close and reset are the capsule session's;
+    state() returns (open_nodes, held_capsule, held_bytes), held_bytes = bytes of the unfinished frame held for the next
+    push."""
+
+    def __init__(self, ctx: Context, ans_type: int, n_streams: int, stride_bytes: int, max_nodes: int, max_scans: int):
+        self._init(ctx, ans_type, n_streams, 0, max_nodes, max_scans,
+                   lambda h: ctx._L.rpl_capsule_stream_create_bytes(ctx._h, ans_type, n_streams, stride_bytes, max_nodes,
+                                                                     max_scans, C.byref(h)))
+        self.stride_bytes = stride_bytes
+
+    def push(self, stream_bytes, byte_counts, params: ScanParams, sample_duration_us=31, out=None, chunk_bytes=None,
+             chunk_rx_us=None, timing: "Timing | None" = None):
+        """Host buffers: stream_bytes [n_streams, stride_bytes] uint8 -> the dict of CapsuleStreamSession.push.  With
+        chunk_bytes, chunk_rx_us ([n_streams, ceil(stride_bytes / chunk_bytes)]: receive time of each chunk_bytes piece
+        of this push) and timing, a stamped push (whose decoder takes timing.sample_duration_us): the dict also holds
+        scan_begin_ts_us."""
+        assert stream_bytes.dtype == np.uint8 and stream_bytes.shape == (self.n_streams, self.stride_bytes)
+        assert stream_bytes.flags.c_contiguous
+        bc = np.ascontiguousarray(byte_counts, dtype=np.uint32)
+        assert bc.shape == (self.n_streams,)
+        if chunk_bytes is None and chunk_rx_us is None and timing is None:
+            out = self._outputs(out)
+            self._ctx._check(self._L.rpl_capsule_stream_push_bytes(
+                self._h, _p(stream_bytes), _p(bc), sample_duration_us, C.byref(params), _p(out["ranges"]),
+                _p(out["intensities"]), _p(out["beam_counts"]), _p(out["angle_increment"]),
+                _p(out["scans_per_stream"])))
+            return out
+        assert chunk_bytes is not None and chunk_rx_us is not None and timing is not None, \
+            "a stamped push takes chunk_bytes, chunk_rx_us and timing"
+        rx = np.ascontiguousarray(chunk_rx_us, dtype=np.uint64)
+        assert chunk_bytes == 0 or rx.shape == (self.n_streams, -(-self.stride_bytes // chunk_bytes))
+        out = self._stamped_outputs(out)
+        self._ctx._check(self._L.rpl_capsule_stream_push_bytes_ts(
+            self._h, _p(stream_bytes), _p(bc), C.byref(timing), chunk_bytes, _p(rx), C.byref(params),
+            _p(out["ranges"]), _p(out["intensities"]), _p(out["beam_counts"]), _p(out["angle_increment"]),
+            _p(out["scans_per_stream"]), _p(out["scan_begin_ts_us"])))
+        return out
+
+    def push_dev(self, stream_bytes, byte_counts, params: ScanParams, ranges, intensities, beam_counts,
+                 angle_increment, scans_per_stream, sample_duration_us=31, stream=None, chunk_bytes=None,
+                 chunk_rx_us=None, timing: "Timing | None" = None, scan_begin_ts_us=None):
+        """Device addresses (the layouts of push), asynchronous on `stream` (None: the context's stream).  With
+        chunk_bytes, chunk_rx_us, timing and scan_begin_ts_us, a stamped push."""
+        if chunk_bytes is None and chunk_rx_us is None and timing is None and scan_begin_ts_us is None:
+            self._ctx._check(self._L.rpl_capsule_stream_push_bytes_dev(
+                self._h, _p(stream_bytes), _p(byte_counts), sample_duration_us, C.byref(params), _p(ranges),
+                _p(intensities), _p(beam_counts), _p(angle_increment), _p(scans_per_stream), _p(stream)))
+            return
+        self._ctx._check(self._L.rpl_capsule_stream_push_bytes_ts_dev(
+            self._h, _p(stream_bytes), _p(byte_counts), C.byref(timing) if timing is not None else None,
+            chunk_bytes or 0, _p(chunk_rx_us), C.byref(params), _p(ranges), _p(intensities), _p(beam_counts),
+            _p(angle_increment), _p(scans_per_stream), _p(scan_begin_ts_us), _p(stream)))
+
+    def state(self):
+        """(open_nodes, held_capsule, held_bytes)"""
+        open_nodes, held, held_bytes = (np.zeros(self.n_streams, np.uint32) for _ in range(3))
+        self._ctx._check(self._L.rpl_capsule_stream_state_bytes(self._h, _p(open_nodes), _p(held), _p(held_bytes)))
+        return open_nodes, held, held_bytes
 
 
 EXCHANGE_NCCL, EXCHANGE_COPY = 0, 1

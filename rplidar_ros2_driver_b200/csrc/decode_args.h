@@ -152,7 +152,22 @@ struct FrameArgs {
   uint32_t* capsule_counts_out;   // [n_streams]
   uint32_t* bytes_left_out;       // [n_streams] nullable: bytes of an unfinished frame at the end
 };
+// a byte session's framer record per stream: word kFramerPos the search position (0 waiting for byte 0, 1 waiting for
+// byte 1 -- HQ: collecting --, k >= 2 collecting), which is also the number of bytes of the unfinished frame held from
+// kFramerBytes on (up to the frame size - 1: 780 for HQ); kFramerLost 1 while skipped bytes wait for the next frame to
+// be reported as the all-zero capsule in front of it.  All zero: a fresh stream.
+constexpr uint32_t kFramerPos = 0, kFramerLost = 1, kFramerBytes = 2, kFramerWords = 200;
+// the session instantiation's own arguments (FrameArgs::stride_capsules then counts capsule slots, byte counts above
+// stride_bytes are clamped to it, and bytes_left_out is unused)
+struct FrameStreamArgs {
+  uint32_t* framer;                         // [n_streams][kFramerWords], read and rewritten in place
+  // nullable: chunk c the receive time of bytes [c * chunk_bytes, (c + 1) * chunk_bytes) of the push
+  const unsigned long long* chunk_rx_us;    // [n_streams][stride_chunks]
+  uint32_t chunk_bytes, stride_chunks;
+  unsigned long long* capsule_rx_out;       // [n_streams][stride_capsules] with chunk_rx_us: each capsule's
+};
 cudaError_t launch_frame_capsules(const FrameArgs& a, int grid, cudaStream_t stream);
+cudaError_t launch_frame_capsules_stream(const FrameArgs& a, const FrameStreamArgs& f, int grid, cudaStream_t stream);
 cudaError_t launch_assemble(const AssembleArgs& a, int grid, cudaStream_t stream);
 cudaError_t launch_assemble_stamped(const AssembleArgs& a, const AssembleStampArgs& t, int grid, cudaStream_t stream);
 

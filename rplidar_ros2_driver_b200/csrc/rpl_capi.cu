@@ -1153,6 +1153,10 @@ rpl_result rpl_scan_views_dev(rpl_ctx* c, const rpl_node_hq* nodes, uint64_t nod
 // A stamped push (rpl_*_stream_push_ts*) runs the stamped decoder (0x81) and assembler instead; they keep, beside the
 // carry, the open revolution's stamp (open_ts, per arena like carry_len) and, for express and ultra, the held capsule's
 // receive time (held_rx).  An unstamped push leaves both stale, so the next stamped push counts them as unknown.
+// A byte session (rpl_capsule_stream_create_bytes) takes the raw bytes of the serial stream instead of framed capsules:
+// each push is framed first (frame.cu's session instantiation, the search carried in the framer record) into the
+// session's own capsule slots, which the decoder then reads as a framed session's push; stride_capsules counts those
+// slots, and a stamped push's capsule receive times come out of the framer.
 struct rpl_capsule_stream {
   rpl_ctx* c = nullptr;
   uint32_t ans_type = 0, cap_bytes = 0;    // answer type, bytes per capsule (0x81: 1)
@@ -1172,6 +1176,11 @@ struct rpl_capsule_stream {
   unsigned long long* held_rx = nullptr;        // [n_streams] express, ultra: receive time of the held capsule
   uint32_t* scan_ends = nullptr;                // 0x81: [n_streams][new nodes] end bytes of the scan-start records
   bool prev_stamped = true;                     // the last push had receive times (a fresh session holds nothing)
+  uint32_t stride_bytes = 0;                    // byte session: most bytes per stream in one push (0: framed capsules)
+  uint32_t* framer = nullptr;                   // byte session: [n_streams][kFramerWords]
+  uint8_t* framed = nullptr;                    // byte session: [n_streams][stride_capsules][cap_bytes] this push's
+  uint32_t* framed_counts = nullptr;            // byte session: [n_streams]
+  unsigned long long* framed_rx = nullptr;      // byte session: [n_streams][stride_capsules] (stamped pushes)
 };
 
 namespace {
@@ -1206,6 +1215,11 @@ struct WireChunk {
   uint32_t* node_end;
   unsigned long long *open_ts_in, *open_ts_out, *held_rx;
   bool prev_stamped;
+  // a byte session's: the input is raw bytes [.][stride_bytes], framed into `framed` first
+  uint32_t stride_bytes;
+  uint32_t *framer, *framed_counts;
+  uint8_t* framed;
+  unsigned long long* framed_rx;
 };
 
 // session cs's chunk from stream s0 in the push under way (arena cs->parity)
@@ -1237,17 +1251,52 @@ WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0) {
   w.open_ts_out = cs->open_ts[p ^ 1u] + s0;
   w.held_rx = cs->held_rx + s0;
   w.prev_stamped = cs->prev_stamped;
+  if (cs->framer) {
+    w.stride_bytes = cs->stride_bytes;
+    w.framer = cs->framer + (size_t)s0 * rpl::kFramerWords;
+    w.framed = cs->framed + (size_t)s0 * sc * cs->cap_bytes;
+    w.framed_counts = cs->framed_counts + s0;
+    w.framed_rx = cs->framed_rx + (size_t)s0 * sc;
+  }
   return w;
 }
 
-// decode -> assemble -> scan kernels for the ns streams of chunk w on `st`; capsules / counts / outputs / sp point at
-// the chunk's first stream's
+// (frame ->) decode -> assemble -> scan kernels for the ns streams of chunk w on `st`; capsules / counts / outputs / sp
+// point at the chunk's first stream's (a byte session's capsules / counts: the raw bytes and byte counts)
 rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const WireChunk& w, uint32_t ns,
                                 const uint8_t* capsules, const uint32_t* counts, uint32_t sample_duration_us,
                                 const rpl_scan_params* params, float* ranges, float* intens, uint32_t* beams,
                                 float* inc, uint32_t* scans_per_stream, const StampPush* sp = nullptr) {
   const uint32_t sc = w.stride_capsules;
   uint32_t* ends = sp ? w.node_end : nullptr;
+  StampPush framed_sp{};
+  if (w.framer) {
+    rpl::FrameArgs a{};
+    a.bytes = capsules;
+    a.byte_counts = counts;
+    a.n_streams = ns;
+    a.stride_bytes = w.stride_bytes;
+    a.capsule_bytes = rpl_capsule_bytes(w.ans_type);
+    a.capsules_out = w.framed;
+    a.stride_capsules = sc;
+    a.capsule_counts_out = w.framed_counts;
+    rpl::FrameStreamArgs f{};
+    f.framer = w.framer;
+    if (sp) {  // the framer turns the chunk receive times into the capsule receive times the assembler reads
+      f.chunk_rx_us = sp->rx;
+      f.chunk_bytes = sp->chunk_bytes;
+      f.stride_chunks = sp->stride_chunks;
+      f.capsule_rx_out = w.framed_rx;
+      framed_sp = *sp;
+      framed_sp.rx = w.framed_rx;
+      sp = &framed_sp;
+    }
+    const int grid = (int)std::min<uint32_t>(ns, (uint32_t)c->num_sms * 8u);
+    RPL_CUDA(c, rpl::launch_frame_capsules_stream(a, f, grid, st), RPL_RESULT_OPERATION_FAIL);
+    c->launches++;
+    capsules = w.framed;
+    counts = w.framed_counts;
+  }
   rpl_result r;
   if (w.ans_type == RPL_ANS_MEASUREMENT) {
     rpl::NormalDecodeArgs a{};
@@ -1396,8 +1445,9 @@ bool capsule_stream_args_ok(rpl_capsule_stream* cs, const uint8_t* capsules, con
   }
   // the standard decoder takes no sample duration (it tests no jump between capsules)
   if (cs->ans_type != RPL_ANS_MEASUREMENT && !sample_duration_ok(c, sample_duration_us)) return false;
-  // the alignment rule of rpl_decode_capsules_batch_dev: only dense capsules are read in 4-byte words
-  if (cs->ans_type == 0x85 && (reinterpret_cast<uintptr_t>(capsules) & 3u) != 0) {
+  // the alignment rule of rpl_decode_capsules_batch_dev: only dense capsules are read in 4-byte words (a byte session's
+  // bytes have any alignment: its decoder reads the session's own capsule slots)
+  if (cs->ans_type == 0x85 && !cs->framer && (reinterpret_cast<uintptr_t>(capsules) & 3u) != 0) {
     c->err = "capsule buffer must be 4-byte aligned";
     return false;
   }
@@ -1405,15 +1455,19 @@ bool capsule_stream_args_ok(rpl_capsule_stream* cs, const uint8_t* capsules, con
 }
 
 // a session of a capsule answer type or of 0x81 standard nodes (the caller has checked ans_type); stride_capsules
-// counts bytes for 0x81
+// counts bytes for 0x81.  stride_bytes != 0: a byte session of a capsule answer type (stride_capsules is ignored)
 rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint32_t stride_capsules,
-                         uint32_t max_nodes, uint32_t max_scans, rpl_capsule_stream** out) {
-  const bool normal = ans_type == RPL_ANS_MEASUREMENT;
+                         uint32_t max_nodes, uint32_t max_scans, rpl_capsule_stream** out, uint32_t stride_bytes = 0) {
+  const bool normal = ans_type == RPL_ANS_MEASUREMENT, bytes = stride_bytes != 0;
   const uint32_t cap_bytes = normal ? 1u : rpl_capsule_bytes(ans_type);
+  // a byte push completes at most `frames` frames with the up to cap_bytes - 1 bytes held before it, each behind at most
+  // one all-zero capsule (none for HQ, whose skipped bytes are no loss)
+  const unsigned long long frames = bytes ? ((unsigned long long)stride_bytes + cap_bytes - 1) / cap_bytes : stride_capsules;
+  if (bytes) stride_capsules = (uint32_t)(ans_type == 0x83 ? frames : 2 * frames);
   if (n_streams == 0 || stride_capsules == 0 || max_scans == 0 || max_nodes == 0 || max_nodes > rpl::kSmallMaxNodes ||
       (max_nodes & 1u)) {
-    c->err = normal ? "need n_streams > 0, stride_bytes > 0, max_scans > 0 and an even max_nodes in [2, 8192]"
-                    : "need n_streams > 0, stride_capsules > 0, max_scans > 0 and an even max_nodes in [2, 8192]";
+    c->err = normal || bytes ? "need n_streams > 0, stride_bytes > 0, max_scans > 0 and an even max_nodes in [2, 8192]"
+                             : "need n_streams > 0, stride_capsules > 0, max_scans > 0 and an even max_nodes in [2, 8192]";
     return RPL_RESULT_INVALID_DATA;
   }
   if (max_scans > c->max_scans) {
@@ -1423,13 +1477,15 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint
   // 0x81: a push of n bytes completes up to (n + 4) / 5 records with the up to 4 bytes held before it; rounded up to
   // even, as every capsule format's node count is, so that every region stays 16-byte aligned
   const unsigned long long new_nodes = normal ? (((unsigned long long)stride_capsules + 4) / 5 + 1) & ~1ull
-                                              : (unsigned long long)rpl_capsule_nodes(ans_type) * stride_capsules;
+                                              : (unsigned long long)rpl_capsule_nodes(ans_type) * frames;
   const unsigned long long stride_nodes = (unsigned long long)max_nodes + new_nodes;
   if (stride_nodes * n_streams > 0xFFFFFFFFull) {
     c->err = normal ? "n_streams * (max_nodes + (stride_bytes + 4) / 5 rounded up to even) must stay below 2^32 "
                       "(32-bit scan views)"
-                    : "n_streams * (max_nodes + nodes per capsule * stride_capsules) must stay below 2^32 (32-bit scan "
-                      "views)";
+                    : bytes ? "n_streams * (max_nodes + nodes per capsule * ceil(stride_bytes / capsule bytes)) must stay "
+                              "below 2^32 (32-bit scan views)"
+                            : "n_streams * (max_nodes + nodes per capsule * stride_capsules) must stay below 2^32 (32-bit "
+                              "scan views)";
     return RPL_RESULT_INVALID_DATA;
   }
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
@@ -1445,8 +1501,9 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint
   cs->stride_nodes = (uint32_t)stride_nodes;  // even: every region starts 16-byte aligned
   cs->starts_stride = 2 * max_scans + 64;     // scan starts per stream the decoder may list (as in the chain)
   cs->chunk_dev = std::min(n_streams, c->max_scans / max_scans);
-  // host pushes: about 16 MiB of capsules per chunk, whole streams (as in the chain)
-  const size_t cap_bytes_stream = (size_t)stride_capsules * cap_bytes;
+  cs->stride_bytes = stride_bytes;
+  // host pushes: about 16 MiB of capsules (a byte session: bytes) per chunk, whole streams (as in the chain)
+  const size_t cap_bytes_stream = bytes ? (size_t)stride_bytes : (size_t)stride_capsules * cap_bytes;
   cs->chunk_host = std::min<uint32_t>(cs->chunk_dev, (uint32_t)std::max<size_t>(1, ((size_t)16 << 20) / cap_bytes_stream));
   const size_t n = n_streams, ncap = n * stride_capsules;
   const rpl_result oom = RPL_RESULT_INSUFFICIENT_MEMORY;
@@ -1470,6 +1527,12 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint
     return fail(oom);
   if (!normal && (!cuda_ok(c, dev_alloc(&cs->status, ncap), "cudaMalloc") ||
                   !cuda_ok(c, dev_alloc(&cs->offsets, ncap), "cudaMalloc")))
+    return fail(oom);
+  if (bytes && (!cuda_ok(c, dev_alloc(&cs->framer, n * rpl::kFramerWords), "cudaMalloc") ||
+                !cuda_ok(c, cudaMemset(cs->framer, 0, n * rpl::kFramerWords * 4), "cudaMemset") ||
+                !cuda_ok(c, dev_alloc(&cs->framed, ncap * cap_bytes), "cudaMalloc") ||
+                !cuda_ok(c, dev_alloc(&cs->framed_counts, n), "cudaMalloc") ||
+                !cuda_ok(c, dev_alloc(&cs->framed_rx, ncap), "cudaMalloc")))
     return fail(oom);
   if (!cuda_ok(c, dev_alloc(&cs->held, n * rpl::kHeldWords), "cudaMalloc") ||
       !cuda_ok(c, cudaMemset(cs->held, 0, n * rpl::kHeldWords * 4), "cudaMemset") ||
@@ -1504,32 +1567,44 @@ bool stamp_args_ok(rpl_capsule_stream* cs, const rpl_timing* timing, const uint6
                                timing->native_interface_type};
   sp->rx = reinterpret_cast<const unsigned long long*>(rx);
   sp->chunk_bytes = chunk_bytes;
-  sp->stride_chunks = (cs->stride_capsules + chunk_bytes - 1) / chunk_bytes;
+  const uint32_t stride_in = cs->framer ? cs->stride_bytes : cs->stride_capsules;  // bytes, or capsules
+  sp->stride_chunks = (uint32_t)(((unsigned long long)stride_in + chunk_bytes - 1) / chunk_bytes);
   sp->scan_ts = reinterpret_cast<unsigned long long*>(scan_begin_ts_us);
   return true;
+}
+
+// a byte push on a framed session or a framed push on a byte session
+bool push_kind_ok(rpl_capsule_stream* cs, bool bytes) {
+  if ((cs->framer != nullptr) == bytes) return true;
+  cs->c->err = bytes ? "a byte push needs a session made by rpl_capsule_stream_create_bytes"
+                     : "a session made by rpl_capsule_stream_create_bytes takes byte pushes (rpl_capsule_stream_push_bytes*)";
+  return false;
 }
 
 // a host push; sp: a stamped one (its rx and scan_ts are host arrays of all streams)
 rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* capsules, const uint32_t* capsule_counts,
                        uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges, float* intensities,
                        uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
-                       const StampPush* sp) {
+                       const StampPush* sp, bool bytes = false) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
   rpl_ctx* c = cs->c;
+  if (!push_kind_ok(cs, bytes)) return RPL_RESULT_INVALID_DATA;
   if (!capsule_stream_args_ok(cs, capsules, capsule_counts, sample_duration_us, params, ranges, intensities,
                               beam_counts, scans_per_stream))
     return RPL_RESULT_INVALID_DATA;
+  const uint32_t stride_in = bytes ? cs->stride_bytes : cs->stride_capsules;
   for (uint32_t s = 0; s < cs->n_streams; ++s)
-    if (capsule_counts[s] > cs->stride_capsules) {
-      c->err = cs->ans_type == RPL_ANS_MEASUREMENT ? "byte_counts[s] exceeds stride_bytes"
-                                                   : "capsule_counts[s] exceeds stride_capsules";
+    if (capsule_counts[s] > stride_in) {
+      c->err = cs->ans_type == RPL_ANS_MEASUREMENT || bytes ? "byte_counts[s] exceeds stride_bytes"
+                                                            : "capsule_counts[s] exceeds stride_capsules";
       return RPL_RESULT_INVALID_DATA;
     }
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
   for (int i = 0; i < kLanes; ++i) RPL_CUDA(c, cudaStreamWaitEvent(c->lane[i].stream, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
-  // receive times per stream of a stamped push: one per capsule, 0x81 one per chunk_bytes piece
-  const size_t rx_stream = sp ? (cs->status ? cs->stride_capsules : sp->stride_chunks) : 0;
-  const HostWire h{capsules, capsule_counts, (size_t)cs->stride_capsules * cs->cap_bytes, sample_duration_us,
+  // receive times per stream of a stamped push: one per capsule, 0x81 and byte pushes one per chunk_bytes piece
+  const size_t rx_stream = sp ? (cs->status && !bytes ? cs->stride_capsules : sp->stride_chunks) : 0;
+  const size_t in_stream = bytes ? (size_t)cs->stride_bytes : (size_t)cs->stride_capsules * cs->cap_bytes;
+  const HostWire h{capsules, capsule_counts, in_stream, sample_duration_us,
                    cs->max_nodes, cs->max_scans, params, ranges, intensities, angle_increment, beam_counts,
                    scans_per_stream, sp, rx_stream};
   const rpl_result r =
@@ -1543,9 +1618,10 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* capsules, const ui
 rpl_result stream_push_dev(rpl_capsule_stream* cs, const uint8_t* capsules, const uint32_t* capsule_counts,
                            uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
                            float* intensities, uint32_t* beam_counts, float* angle_increment,
-                           uint32_t* scans_per_stream, void* stream, const StampPush* sp) {
+                           uint32_t* scans_per_stream, void* stream, const StampPush* sp, bool bytes = false) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
   rpl_ctx* c = cs->c;
+  if (!push_kind_ok(cs, bytes)) return RPL_RESULT_INVALID_DATA;
   if (!capsule_stream_args_ok(cs, capsules, capsule_counts, sample_duration_us, params, ranges, intensities,
                               beam_counts, scans_per_stream))
     return RPL_RESULT_INVALID_DATA;
@@ -1560,11 +1636,12 @@ rpl_result stream_push_dev(rpl_capsule_stream* cs, const uint8_t* capsules, cons
     StampPush chunk_sp{};
     if (sp) {
       chunk_sp = *sp;
-      chunk_sp.rx += (size_t)s0 * (cs->status ? cs->stride_capsules : sp->stride_chunks);
+      chunk_sp.rx += (size_t)s0 * (cs->status && !bytes ? cs->stride_capsules : sp->stride_chunks);
       chunk_sp.scan_ts += so;
     }
     r = capsule_stream_chunk(c, c->lane[0], st, session_chunk(cs, s0), ns,
-                             capsules + (size_t)s0 * cs->stride_capsules * cs->cap_bytes, capsule_counts + s0,
+                             capsules + (size_t)s0 * (bytes ? cs->stride_bytes : cs->stride_capsules * cs->cap_bytes),
+                             capsule_counts + s0,
                              sample_duration_us, params, ranges + (size_t)s0 * row, intensities + (size_t)s0 * row,
                              beam_counts + so,
                              angle_increment ? angle_increment + so : nullptr, scans_per_stream + s0,
@@ -1669,6 +1746,10 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   cudaFree(cs->start_counts);
   cudaFree(cs->scan_len);
   cudaFree(cs->views);
+  cudaFree(cs->framer);
+  cudaFree(cs->framed);
+  cudaFree(cs->framed_counts);
+  cudaFree(cs->framed_rx);
   if (cs->done) cudaEventDestroy(cs->done);
   delete cs;
 }
@@ -1730,6 +1811,9 @@ rpl_result rpl_capsule_stream_reset(rpl_capsule_stream* cs, const uint8_t* strea
     RPL_CUDA(c, cudaMemsetAsync(cs->carry_len[p] + s, 0, (size_t)(e - s) * 4, st), RPL_RESULT_OPERATION_FAIL);
     RPL_CUDA(c, cudaMemsetAsync(cs->open_ts[p] + s, 0, (size_t)(e - s) * 8, st), RPL_RESULT_OPERATION_FAIL);
     RPL_CUDA(c, cudaMemsetAsync(cs->held_rx + s, 0, (size_t)(e - s) * 8, st), RPL_RESULT_OPERATION_FAIL);
+    if (cs->framer)  // the handlers' reset: _cached_scan_node_buf_pos = 0, _is_previous_capsuledataRdy = false
+      RPL_CUDA(c, cudaMemsetAsync(cs->framer + (size_t)s * rpl::kFramerWords, 0, (size_t)(e - s) * rpl::kFramerWords * 4, st),
+               RPL_RESULT_OPERATION_FAIL);
     s = e;
   }
   RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);
@@ -1737,6 +1821,11 @@ rpl_result rpl_capsule_stream_reset(rpl_capsule_stream* cs, const uint8_t* strea
 }
 
 rpl_result rpl_capsule_stream_state(rpl_capsule_stream* cs, uint32_t* open_nodes, uint32_t* held_capsule) {
+  return rpl_capsule_stream_state_bytes(cs, open_nodes, held_capsule, nullptr);
+}
+
+rpl_result rpl_capsule_stream_state_bytes(rpl_capsule_stream* cs, uint32_t* open_nodes, uint32_t* held_capsule,
+                                          uint32_t* held_bytes) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
   rpl_ctx* c = cs->c;
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
@@ -1744,12 +1833,79 @@ rpl_result rpl_capsule_stream_state(rpl_capsule_stream* cs, uint32_t* open_nodes
   if (open_nodes)
     RPL_CUDA(c, cudaMemcpy(open_nodes, cs->carry_len[cs->parity], (size_t)cs->n_streams * 4, cudaMemcpyDeviceToHost),
              RPL_RESULT_OPERATION_FAIL);
+  std::vector<uint32_t> fr;  // a byte session's framer records
+  if (cs->framer && (held_capsule || held_bytes)) {
+    fr.resize((size_t)cs->n_streams * rpl::kFramerWords);
+    RPL_CUDA(c, cudaMemcpy(fr.data(), cs->framer, fr.size() * 4, cudaMemcpyDeviceToHost), RPL_RESULT_OPERATION_FAIL);
+  }
   if (held_capsule) {  // HQ: the record stays zero; 0x81: the byte machine's state, 0..4 bytes held
     std::vector<uint32_t> h((size_t)cs->n_streams * rpl::kHeldWords);
     RPL_CUDA(c, cudaMemcpy(h.data(), cs->held, h.size() * 4, cudaMemcpyDeviceToHost), RPL_RESULT_OPERATION_FAIL);
-    for (uint32_t s = 0; s < cs->n_streams; ++s) held_capsule[s] = h[(size_t)s * rpl::kHeldWords + rpl::kHeldOk];
+    for (uint32_t s = 0; s < cs->n_streams; ++s) {
+      held_capsule[s] = h[(size_t)s * rpl::kHeldWords + rpl::kHeldOk];
+      // skipped bytes waiting to be reported: the next frame releases nothing (the SDK cleared its ready flag)
+      if (!fr.empty() && fr[(size_t)s * rpl::kFramerWords + rpl::kFramerLost]) held_capsule[s] = 0;
+    }
   }
+  if (held_bytes)
+    for (uint32_t s = 0; s < cs->n_streams; ++s)
+      held_bytes[s] = fr.empty() ? 0u : fr[(size_t)s * rpl::kFramerWords + rpl::kFramerPos];
   return RPL_RESULT_OK;
+}
+
+// ---- byte sessions: the capsule session fed the raw serial stream ----
+rpl_result rpl_capsule_stream_create_bytes(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint32_t stride_bytes,
+                                           uint32_t max_nodes, uint32_t max_scans, rpl_capsule_stream** out) {
+  if (!c || !out) return RPL_RESULT_INVALID_DATA;
+  *out = nullptr;
+  if (rpl_capsule_bytes(ans_type) == 0) {
+    c->err = "a byte session takes the capsule answer types 0x82..0x86 (0x81 standard-node bytes: rpl_normal_stream)";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  if (stride_bytes == 0) {
+    c->err = "need n_streams > 0, stride_bytes > 0, max_scans > 0 and an even max_nodes in [2, 8192]";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  return stream_create(c, ans_type, n_streams, 0, max_nodes, max_scans, out, stride_bytes);
+}
+
+rpl_result rpl_capsule_stream_push_bytes(rpl_capsule_stream* cs, const uint8_t* bytes, const uint32_t* byte_counts,
+                                         uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
+                                         float* intensities, uint32_t* beam_counts, float* angle_increment,
+                                         uint32_t* scans_per_stream) {
+  return stream_push(cs, bytes, byte_counts, sample_duration_us, params, ranges, intensities, beam_counts,
+                     angle_increment, scans_per_stream, nullptr, true);
+}
+
+rpl_result rpl_capsule_stream_push_bytes_dev(rpl_capsule_stream* cs, const uint8_t* bytes, const uint32_t* byte_counts,
+                                             uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
+                                             float* intensities, uint32_t* beam_counts, float* angle_increment,
+                                             uint32_t* scans_per_stream, void* stream) {
+  return stream_push_dev(cs, bytes, byte_counts, sample_duration_us, params, ranges, intensities, beam_counts,
+                         angle_increment, scans_per_stream, stream, nullptr, true);
+}
+
+rpl_result rpl_capsule_stream_push_bytes_ts(rpl_capsule_stream* cs, const uint8_t* bytes, const uint32_t* byte_counts,
+                                            const rpl_timing* timing, uint32_t chunk_bytes, const uint64_t* chunk_rx_us,
+                                            const rpl_scan_params* params, float* ranges, float* intensities,
+                                            uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
+                                            uint64_t* scan_begin_ts_us) {
+  StampPush sp{};
+  if (!stamp_args_ok(cs, timing, chunk_rx_us, chunk_bytes, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
+  return stream_push(cs, bytes, byte_counts, timing->sample_duration_us, params, ranges, intensities, beam_counts,
+                     angle_increment, scans_per_stream, &sp, true);
+}
+
+rpl_result rpl_capsule_stream_push_bytes_ts_dev(rpl_capsule_stream* cs, const uint8_t* bytes,
+                                                const uint32_t* byte_counts, const rpl_timing* timing,
+                                                uint32_t chunk_bytes, const uint64_t* chunk_rx_us,
+                                                const rpl_scan_params* params, float* ranges, float* intensities,
+                                                uint32_t* beam_counts, float* angle_increment,
+                                                uint32_t* scans_per_stream, uint64_t* scan_begin_ts_us, void* stream) {
+  StampPush sp{};
+  if (!stamp_args_ok(cs, timing, chunk_rx_us, chunk_bytes, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
+  return stream_push_dev(cs, bytes, byte_counts, timing->sample_duration_us, params, ranges, intensities, beam_counts,
+                         angle_increment, scans_per_stream, stream, &sp, true);
 }
 
 // ---- the dense session: the capsule session fixed to 0x85 ----

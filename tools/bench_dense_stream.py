@@ -24,11 +24,19 @@ against unstamped ones on the same data and shapes: the chain shape above for 0x
 other formats; two sessions, timed in alternating rounds in one run.  Also the host push of a 25 ms receive period
 (512 streams x 80 dense capsules, or the format's equivalent), stamped and unstamped, with the bytes each copies.
 
+With --bytes (--format 0x82..0x86), byte pushes (rpl_capsule_stream_push_bytes_dev: raw bytes framed on the device,
+the search for the sync bytes carried across pushes) against framed pushes (rpl_capsule_stream_push_dev) of the same
+clean stream: the chain shape for 0x85 (512 streams x 4096 capsules), the comparison shapes above for the other formats,
+and small pushes of 512 streams x about 2 KB (a 20 ms receive period at 1 Mbaud).  Two byte sessions: one pushed whole
+capsules (every push starts on a frame), one pushed a byte count that is no multiple of the frame size, so most pushes
+begin with held bytes and the stream sits off the word grid; three sessions timed in alternating rounds in one run.
+
 Each push continues the stream where the previous one ended (the capsules of a push follow on in angle), so the carry
 and the held capsule are exercised as in a live feed.  The GPU's name and power limit are part of the output.
 """
 import argparse
 import json
+import math
 import os
 import subprocess
 import sys
@@ -375,6 +383,89 @@ def compare_stamped(R, torch, fmt, steps, rounds):
     return res
 
 
+def byte_windows(torch, dev, caps, n_streams, P):
+    """caps [16, M, cb] read as a ring of M * cb bytes per stream (a whole number of pushes of P bytes): the device
+    buffers [n_streams, P] of the pushes that walk once around it, tiled over n_streams"""
+    flat = caps.reshape(caps.shape[0], -1)
+    W = flat.shape[1] // P
+    assert W * P == flat.shape[1]
+    return [torch.from_numpy(np.ascontiguousarray(np.tile(flat[:, w * P:(w + 1) * P], (n_streams // 16, 1)))).to(dev)
+            for w in range(W)]
+
+
+def compare_bytes(R, torch, fmt, steps, rounds, small):
+    """ms per push_dev of a framed session, a byte session pushed whole capsules and a byte session pushed a byte count
+    off the frame grid, on clean streams of `fmt`, alternating rounds of `steps` pushes"""
+    n_streams, max_nodes, max_scans = 512, 4096, 56
+    if fmt == 0x85:
+        cb, n_units = 84, 4096
+
+        def gen(m, seed):
+            return feed(16, m, seed)
+    else:
+        cb, _, n_units, _ = FORMATS[fmt]
+
+        def gen(m, seed):
+            return feed_format(fmt, 16, m, seed)
+    if small:  # about 2 KB per push: framed pushes carry the whole capsules in it, byte pushes 2048 bytes
+        n_units, P = max(1, 2048 // cb), 2048
+        W = cb // math.gcd(cb, P)
+    else:  # the byte count of W pushes is a whole number of frames: W - 1 of W pushes begin with held bytes
+        W = min(w for w in range(3, cb + 1) if cb % w == 0)
+        P = n_units * cb - cb // W
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    params = R.scan_params(1, 0, 0, 1)
+    ctx = R.Context(0, max_nodes, n_streams * max_scans)
+    NS = n_streams * max_scans
+    data = gen(2 * n_units, 7)
+    ring = gen(W * P // cb, 8)
+    with torch.cuda.stream(stream):
+        halves = [torch.from_numpy(np.ascontiguousarray(np.tile(data[:, h * n_units:(h + 1) * n_units],
+                                                                (n_streams // 16, 1, 1)))).to(dev) for h in (0, 1)]
+        windows = byte_windows(torch, dev, ring, n_streams, P)
+        cnt_caps = torch.full((n_streams,), n_units, dtype=torch.int32, device=dev)
+        cnt_al = torch.full((n_streams,), n_units * cb, dtype=torch.int32, device=dev)
+        cnt_mis = torch.full((n_streams,), P, dtype=torch.int32, device=dev)
+        r = torch.empty((NS, max_nodes), device=dev)
+        it = torch.empty((NS, max_nodes), device=dev)
+        bc = torch.zeros(NS, dtype=torch.int32, device=dev)
+        inc = torch.zeros(NS, device=dev)
+        sps = torch.zeros(n_streams, dtype=torch.int32, device=dev)
+    cs = stream.cuda_stream
+    outs = (r.data_ptr(), it.data_ptr(), bc.data_ptr(), inc.data_ptr(), sps.data_ptr())
+    res = {"format": hex(fmt), "streams": n_streams, "capsules_per_framed_push": n_units,
+           "bytes_per_aligned_push": n_units * cb, "bytes_per_offgrid_push": P, "offgrid_pushes_per_cycle": W,
+           "max_nodes": max_nodes, "max_scans": max_scans, "steps": steps, "rounds": rounds,
+           "framed_ms": [], "bytes_aligned_ms": [], "bytes_offgrid_ms": []}
+    scans = {}
+    with R.CapsuleStreamSession(ctx, fmt, n_streams, n_units, max_nodes, max_scans) as framed, \
+            R.CapsuleByteStreamSession(ctx, fmt, n_streams, n_units * cb, max_nodes, max_scans) as aligned, \
+            R.CapsuleByteStreamSession(ctx, fmt, n_streams, P, max_nodes, max_scans) as offgrid:
+        def push_framed(t):
+            framed.push_dev(halves[t % 2].data_ptr(), cnt_caps.data_ptr(), params, *outs, stream=cs)
+
+        def push_aligned(t):
+            aligned.push_dev(halves[t % 2].data_ptr(), cnt_al.data_ptr(), params, *outs, stream=cs)
+
+        def push_offgrid(t):
+            offgrid.push_dev(windows[t % W].data_ptr(), cnt_mis.data_ptr(), params, *outs, stream=cs)
+
+        for _ in range(rounds):
+            for key, fn in (("framed_ms", push_framed), ("bytes_aligned_ms", push_aligned),
+                            ("bytes_offgrid_ms", push_offgrid)):
+                res[key].append(timed(torch, stream, fn, steps))
+                scans[key] = int(sps.cpu().sum())
+        res["held_bytes_offgrid"] = sorted(set(offgrid.state()[2].tolist()))
+    res["scans_per_push"] = scans
+    for key in ("framed_ms", "bytes_aligned_ms", "bytes_offgrid_ms"):
+        res[key + "_median"] = float(np.median(res[key]))
+    res["aligned_over_framed"] = res["bytes_aligned_ms_median"] / res["framed_ms_median"] - 1.0
+    res["offgrid_over_framed"] = res["bytes_offgrid_ms_median"] / res["framed_ms_median"] - 1.0
+    ctx.close()
+    return res
+
+
 def gpu_info():
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                        capture_output=True, text=True)
@@ -388,11 +479,19 @@ def main():
     ap.add_argument("--format", type=lambda v: int(v, 0), default=0x85, choices=[0x81, 0x82, 0x83, 0x84, 0x85, 0x86],
                     help="answer type (default 0x85: the dense session's latency and throughput points)")
     ap.add_argument("--stamped", action="store_true", help="stamped against unstamped pushes of --format")
-    ap.add_argument("--rounds", type=int, default=5, help="--stamped: alternating rounds of --steps pushes each")
+    ap.add_argument("--rounds", type=int, default=5, help="--stamped, --bytes: alternating rounds of --steps pushes each")
+    ap.add_argument("--bytes", action="store_true", help="byte pushes against framed pushes of --format (not 0x81)")
     args = ap.parse_args()
     import torch
 
     import rplidar_ros2_driver_b200 as R
+
+    if args.bytes:
+        if args.format == 0x81:
+            ap.error("--bytes takes a capsule format: 0x81 bytes are the standard-node session's input already")
+        print(json.dumps({"gpu": gpu_info(), "bytes": [compare_bytes(R, torch, args.format, args.steps, args.rounds, small)
+                                                       for small in (False, True)]}))
+        return
 
     if args.stamped:
         print(json.dumps({"gpu": gpu_info(), "stamped": compare_stamped(R, torch, args.format, args.steps, args.rounds)}))

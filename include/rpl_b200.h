@@ -634,6 +634,38 @@ rpl_result rpl_normal_stream_push_ts_dev(rpl_normal_stream* s, const uint8_t* by
 rpl_result rpl_normal_stream_reset(rpl_normal_stream* s, const uint8_t* stream_mask);
 rpl_result rpl_normal_stream_state(rpl_normal_stream* s, uint32_t* open_nodes, uint32_t* held_bytes);
 
+/* Session clouds: the PointCloud2 chain of rpl_cloud_batch_dev over the scans the session's last successful push
+ * published, read in place from the session's node arenas (no copy of the scans, no second decode).
+ *   Which scans: xyzi [n_streams * max_scans][max_nodes][4] floats (the layout of rpl_cloud_batch_dev), point_counts
+ *            [n_streams * max_scans]; slot k of stream s is the scan whose LaserScan (and scan-begin stamp) that push
+ *            wrote to slot k of stream s; unused slots get point count 0 (their rows are not written).
+ *   Definition: each cloud is bit for bit what rpl_cloud_batch_dev returns with the same params for that scan's nodes,
+ *            the holder's scan after its capacity rule (the ascended buffer does not matter: the cloud drops
+ *            unmeasured nodes).  Flags 0 fuses SOR / voxel grid into the shared-memory kernel whenever the voxel rule
+ *            of rpl_cloud_batch_dev allows it, also for max_nodes above 4096 (a revolution longer than 4096 nodes then
+ *            takes the general kernel and the separate passes); RPL_CLOUD_NO_FUSED runs them as separate passes.
+ *   Every push flavour: framed or byte pushes, host or device, stamped or not (a byte session: the
+ *            rpl_capsule_stream_* pair).  The clouds can be taken any number of times between that push and the
+ *            next; a reset in between does not change them.  Before any push, after a push that failed, with
+ *            sor_k > 32, outside the voxel rule of rpl_cloud_batch_dev or with a null pointer:
+ *            RPL_RESULT_INVALID_DATA.
+ *   cloud_dev: device buffers, asynchronous on `stream` (NULL = the context's stream).  It waits for the session's
+ *            last push (on any stream) and the session's next push waits for it.  The SOR / voxel passes of every
+ *            session cloud on a context take turns on the context's cloud workspace, whatever their stream.
+ *   cloud:   host buffers, synchronous, chunked over the context's lanes as a host push is. */
+rpl_result rpl_capsule_stream_cloud_dev(rpl_capsule_stream* s, const rpl_cloud_params* params, float* xyzi,
+                                        uint32_t* point_counts, void* stream);
+rpl_result rpl_capsule_stream_cloud(rpl_capsule_stream* s, const rpl_cloud_params* params, float* xyzi,
+                                    uint32_t* point_counts);
+rpl_result rpl_dense_stream_cloud_dev(rpl_dense_stream* s, const rpl_cloud_params* params, float* xyzi,
+                                      uint32_t* point_counts, void* stream);
+rpl_result rpl_dense_stream_cloud(rpl_dense_stream* s, const rpl_cloud_params* params, float* xyzi,
+                                  uint32_t* point_counts);
+rpl_result rpl_normal_stream_cloud_dev(rpl_normal_stream* s, const rpl_cloud_params* params, float* xyzi,
+                                       uint32_t* point_counts, void* stream);
+rpl_result rpl_normal_stream_cloud(rpl_normal_stream* s, const rpl_cloud_params* params, float* xyzi,
+                                   uint32_t* point_counts);
+
 /* ---- LaserScan / PointCloud2 -> wire (SURVEY.md 8(f) rank 3) ---------------------------- */
 /* The serialised message the RMW layer would produce from the message the reference publishes
  * (scan_pub_->publish, reference src/rplidar_node.cpp:679): XCDR1 little endian, 4-byte

@@ -56,6 +56,8 @@ EXPORTS = [
     "rpl_capsule_stream_push_bytes_ts", "rpl_capsule_stream_push_bytes_ts_dev", "rpl_capsule_stream_state_bytes",
     "rpl_normal_stream_create", "rpl_normal_stream_destroy", "rpl_normal_stream_push", "rpl_normal_stream_push_dev",
     "rpl_normal_stream_reset", "rpl_normal_stream_state", "rpl_normal_stream_push_ts", "rpl_normal_stream_push_ts_dev",
+    "rpl_capsule_stream_cloud", "rpl_capsule_stream_cloud_dev", "rpl_dense_stream_cloud", "rpl_dense_stream_cloud_dev",
+    "rpl_normal_stream_cloud", "rpl_normal_stream_cloud_dev",
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -228,6 +230,9 @@ def lib() -> C.CDLL:
         "rpl_capsule_stream_push_bytes_ts_dev": ([vp, vp, vp, PT, u32, vp, PSP, vp, vp, vp, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_state_bytes": ([vp, vp, vp, vp], u32),
     }
+    for kind in ("capsule", "dense", "normal"):
+        sig[f"rpl_{kind}_stream_cloud"] = ([vp, PCP, vp, vp], u32)
+        sig[f"rpl_{kind}_stream_cloud_dev"] = ([vp, PCP, vp, vp, vp], u32)
     for name, (args, res) in sig.items():
         fn = getattr(L, name)  # AttributeError here = the library does not export the ABI
         fn.argtypes = args
@@ -670,6 +675,25 @@ class CapsuleStreamSession:
             self._h, _p(capsules), _p(capsule_counts), C.byref(timing) if timing is not None else None, _p(rx_us),
             C.byref(params), _p(ranges), _p(intensities), _p(beam_counts), _p(angle_increment), _p(scans_per_stream),
             _p(scan_begin_ts_us), _p(stream)))
+
+    def cloud(self, params: CloudParams, out=None):
+        """The PointCloud2 chain over the scans the last push published, read where the session keeps them:
+        {"xyzi": [n_streams * max_scans, max_nodes, 4] float32, "point_counts": [n_streams * max_scans] uint32}, slot k
+        of stream s the cloud of the scan in slot k of that push's outputs (unused slots: count 0, row untouched)."""
+        out = dict(out or {})
+        ns = self.n_streams * self.max_scans
+        if "xyzi" not in out:
+            out["xyzi"] = np.zeros((ns, self.max_nodes, 4), np.float32)
+        if "point_counts" not in out:
+            out["point_counts"] = np.zeros(ns, np.uint32)
+        assert out["xyzi"].shape == (ns, self.max_nodes, 4) and out["xyzi"].dtype == np.float32
+        assert out["point_counts"].shape == (ns,) and out["point_counts"].dtype == np.uint32
+        self._ctx._check(self._fn("cloud")(self._h, C.byref(params), _p(out["xyzi"]), _p(out["point_counts"])))
+        return out
+
+    def cloud_dev(self, params: CloudParams, xyzi, point_counts, stream=None):
+        """Device addresses (the layouts of cloud), asynchronous on `stream` (None: the context's stream)."""
+        self._ctx._check(self._fn("cloud_dev")(self._h, C.byref(params), _p(xyzi), _p(point_counts), _p(stream)))
 
     def reset(self, mask=None):
         """Drops the held capsule, the decoder state and the open revolution of the streams where mask is true

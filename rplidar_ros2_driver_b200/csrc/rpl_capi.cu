@@ -106,8 +106,10 @@ FastKernel pick_fast(const rpl::ScanBatchArgs& a, uint32_t flags) {
 
 // Launches fast kernel k on `stream` (k != kNone); the caller has zeroed a.fallback_count.  A PointCloud2 launch may
 // fuse the SOR / voxel-grid passes of `cloud` (steps 4-5) into the shared-memory kernel: *post_fused tells.
+// hand_off (scan views): above kSmallPostMaxNodes, fuse all the same with the shared memory sized for that many nodes,
+// the longer views going to the general kernel like duplicate-key scans.
 rpl_result launch_fast(rpl_ctx* c, Lane& l, const rpl::ScanBatchArgs& a, FastKernel k, cudaStream_t stream,
-                       const rpl_cloud_params* cloud = nullptr, bool* post_fused = nullptr) {
+                       const rpl_cloud_params* cloud = nullptr, bool* post_fused = nullptr, bool hand_off = false) {
   const int tma_grid = c->tma_grid[a.xyzi ? 2 : a.mode_a ? 1 : 0];
   const int grid = k == FastKernel::kCluster
                        ? 2 * (int)std::min<uint32_t>(a.n_scans, (uint32_t)c->tma_clusters)
@@ -121,11 +123,13 @@ rpl_result launch_fast(rpl_ctx* c, Lane& l, const rpl::ScanBatchArgs& a, FastKer
   if (k == FastKernel::kSmall) {
     // SOR / voxel grid run inside the kernel when the 32-bit cell keys and accumulators are exact:
     // |cell index| < 32768 and voxel <= 4 m (scan_small.cu); otherwise as separate passes
+    const bool fits = rpl::scan_small_post_applies(a.stride);
     bool fuse = false;
-    if (a.xyzi && cloud && (cloud->sor_k > 0 || cloud->voxel_size > 0.0f) && rpl::scan_small_post_applies(a.stride))
+    if (a.xyzi && cloud && (cloud->sor_k > 0 || cloud->voxel_size > 0.0f) && (fits || (hand_off && a.views)))
       fuse = cloud->voxel_size == 0.0f || (cloud->voxel_size <= 4.0f && a.range_max / cloud->voxel_size < 32000.0f);
+    const uint32_t cap = fuse && !fits ? rpl::kSmallPostMaxNodes : 0u;
     RPL_CUDA(c, rpl::launch_scan_small(a, l.fws.max_nodes, fuse ? cloud->sor_k : 0u, fuse ? cloud->sor_alpha : 0.0f,
-                                       fuse ? cloud->voxel_size : 0.0f, c->num_sms, stream),
+                                       fuse ? cloud->voxel_size : 0.0f, c->num_sms, stream, cap),
              RPL_RESULT_OPERATION_FAIL);
     if (post_fused) *post_fused = fuse;
   } else if (k == FastKernel::kCluster) {
@@ -163,7 +167,7 @@ rpl_result launch_general(rpl_ctx* c, Lane& l, const rpl::ScanBatchArgs& a, bool
 
 // the fast kernel, then the general kernel for the scans it hands on (or for all), on `stream` with no host round trip
 rpl_result enqueue_args(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, uint32_t flags, cudaStream_t stream,
-                        const rpl_cloud_params* cloud = nullptr, bool* post_fused = nullptr) {
+                        const rpl_cloud_params* cloud = nullptr, bool* post_fused = nullptr, bool hand_off = false) {
   if (post_fused) *post_fused = false;
   if (a.nodes_out && !a.apply_ascend) {
     // no geometric correction requested: the buffer passes through unchanged
@@ -176,7 +180,7 @@ rpl_result enqueue_args(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, uint32_t flag
   const FastKernel k = pick_fast(a, flags);
   if (k != FastKernel::kNone) {
     RPL_CUDA(c, cudaMemsetAsync(l.fallback_count, 0, sizeof(uint32_t), stream), RPL_RESULT_OPERATION_FAIL);
-    const rpl_result r = launch_fast(c, l, a, k, stream, cloud, post_fused);
+    const rpl_result r = launch_fast(c, l, a, k, stream, cloud, post_fused, hand_off);
     if (r != RPL_RESULT_OK) return r;
   }
   return launch_general(c, l, a, k == FastKernel::kNone, stream);
@@ -380,6 +384,7 @@ void rpl_ctx_destroy(rpl_ctx* c) {
     free_lane(c->lane[i]);
   }
   if (c->asm_done) cudaEventDestroy(c->asm_done);
+  if (c->cloud_done) cudaEventDestroy(c->cloud_done);
   cudaFree(c->d_reset_prefix);
   cudaFree(c->d_desc);
   if (c->h_one) cudaFreeHost(c->h_one);
@@ -1181,6 +1186,9 @@ struct rpl_capsule_stream {
   uint8_t* framed = nullptr;                    // byte session: [n_streams][stride_capsules][cap_bytes] this push's
   uint32_t* framed_counts = nullptr;            // byte session: [n_streams]
   unsigned long long* framed_rx = nullptr;      // byte session: [n_streams][stride_capsules] (stamped pushes)
+  // the last push, as the cloud calls replay it: its views count from the first stream of their chunk
+  uint32_t cloud_chunk = 0;                     // streams per chunk (chunk_host or chunk_dev); 0: no push, or it failed
+  uint32_t cloud_arena = 0;                     // the arena its views point into
 };
 
 namespace {
@@ -1588,6 +1596,7 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* capsules, const ui
                        const StampPush* sp, bool bytes = false) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
   rpl_ctx* c = cs->c;
+  cs->cloud_chunk = 0;
   if (!push_kind_ok(cs, bytes)) return RPL_RESULT_INVALID_DATA;
   if (!capsule_stream_args_ok(cs, capsules, capsule_counts, sample_duration_us, params, ranges, intensities,
                               beam_counts, scans_per_stream))
@@ -1611,6 +1620,10 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* capsules, const ui
       push_host(c, h, cs->n_streams, cs->chunk_host, [&](Carve&, uint32_t s0) { return session_chunk(cs, s0); });
   cs->parity ^= 1u;
   cs->prev_stamped = sp != nullptr;
+  if (r == RPL_RESULT_OK) {
+    cs->cloud_chunk = cs->chunk_host;
+    cs->cloud_arena = cs->parity ^ 1u;
+  }
   return r;
 }
 
@@ -1621,6 +1634,7 @@ rpl_result stream_push_dev(rpl_capsule_stream* cs, const uint8_t* capsules, cons
                            uint32_t* scans_per_stream, void* stream, const StampPush* sp, bool bytes = false) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
   rpl_ctx* c = cs->c;
+  cs->cloud_chunk = 0;
   if (!push_kind_ok(cs, bytes)) return RPL_RESULT_INVALID_DATA;
   if (!capsule_stream_args_ok(cs, capsules, capsule_counts, sample_duration_us, params, ranges, intensities,
                               beam_counts, scans_per_stream))
@@ -1650,7 +1664,130 @@ rpl_result stream_push_dev(rpl_capsule_stream* cs, const uint8_t* capsules, cons
   cs->parity ^= 1u;
   cs->prev_stamped = sp != nullptr;
   RPL_CUDA(c, cudaEventRecord(cs->done, st), RPL_RESULT_OPERATION_FAIL);
+  if (r == RPL_RESULT_OK) {
+    cs->cloud_chunk = cs->chunk_dev;
+    cs->cloud_arena = cs->parity ^ 1u;
+  }
   return r;
+}
+
+// the parameter rules of the PointCloud2 chain (rpl_cloud_batch_dev and the session clouds)
+bool cloud_params_ok(rpl_ctx* c, const rpl_cloud_params* p) {
+  if (p->sor_k > 32) {
+    c->err = "sor_k > 32";
+    return false;
+  }
+  if (p->voxel_size != 0.0f && !(p->voxel_size >= 1e-6f && p->range_max < 1000.0f)) {
+    c->err = "voxel grid: voxel_size must be >= 1e-6 m and range_max < 1000 m (cell indices must fit 31 bits)";
+    return false;
+  }
+  return true;
+}
+
+// The cloud chain over the scans of streams [s0, s0 + ns) of the session's last push, one chunk of that push: its
+// views count from node 0 of stream s0 in the push's arena.  xyzi / point_counts point at the chunk's first slot.
+// Flags 0: the shared-memory kernel with SOR / voxel grid fused, its arrays sized for at most kSmallPostMaxNodes nodes
+// (a longer view goes to the general kernel, then to the post passes restricted to the hand-off list);
+// RPL_CLOUD_NO_FUSED: the shared-memory kernel's window + xyz, then the post passes over every scan.
+rpl_result stream_cloud_chunk(rpl_capsule_stream* cs, Lane& l, uint32_t s0, uint32_t ns, const rpl_cloud_params* p,
+                              float* xyzi, uint32_t* point_counts, cudaStream_t st) {
+  rpl_ctx* c = cs->c;
+  rpl::ScanBatchArgs a{};
+  a.nodes = reinterpret_cast<const uint2*>(cs->arena[cs->cloud_arena] + (size_t)s0 * cs->stride_nodes);
+  a.views = reinterpret_cast<const uint2*>(cs->views + (size_t)s0 * cs->max_scans);
+  a.counts = reinterpret_cast<const uint32_t*>(a.views);
+  a.nodes_total = (unsigned long long)ns * cs->stride_nodes;
+  a.n_scans = ns * cs->max_scans;
+  a.stride = cs->max_nodes;
+  a.beam_counts = point_counts;
+  a.fallback_list = l.fallback_list;
+  a.fallback_count = l.fallback_count;
+  a.is_new_protocol = p->is_new_protocol;
+  a.xyzi = reinterpret_cast<float4*>(xyzi);
+  a.trig = c->lane[0].cws.trig;
+  a.angle = c->lane[0].cws.angle;
+  a.range_min = p->range_min;
+  a.range_max = p->range_max;
+  a.intensity_min = p->intensity_min;
+  const bool separate = (p->flags & RPL_CLOUD_NO_FUSED) != 0;
+  bool fused = false;
+  rpl_result r = enqueue_args(c, l, a, 0u, st, separate ? nullptr : p, &fused, true);
+  if (r != RPL_RESULT_OK || (p->sor_k == 0 && p->voxel_size == 0.0f)) return r;
+  if (!c->cloud_done)
+    RPL_CUDA(c, cudaEventCreateWithFlags(&c->cloud_done, cudaEventDisableTiming), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaStreamWaitEvent(st, c->cloud_done, 0), RPL_RESULT_OPERATION_FAIL);
+  int launched = 0;
+  RPL_CUDA(c, rpl::launch_cloud_post(a.xyzi, point_counts, a.n_scans, a.stride, p->sor_k, p->sor_alpha, p->voxel_size,
+                                     c->lane[0].cws, fused ? a.fallback_list : nullptr,
+                                     fused ? a.fallback_count : nullptr, st, &launched),
+           RPL_RESULT_OPERATION_FAIL);
+  c->launches += launched;
+  RPL_CUDA(c, cudaEventRecord(c->cloud_done, st), RPL_RESULT_OPERATION_FAIL);
+  return RPL_RESULT_OK;
+}
+
+bool stream_cloud_args_ok(rpl_capsule_stream* cs, const rpl_cloud_params* params, float* xyzi, uint32_t* point_counts) {
+  rpl_ctx* c = cs->c;
+  if (!params || !xyzi || !point_counts) {
+    c->err = "null params, xyzi or point_counts";
+    return false;
+  }
+  if (!cloud_params_ok(c, params)) return false;
+  if (cs->cloud_chunk == 0) {
+    c->err = "no clouds to take: the session has not pushed yet, or its last push failed";
+    return false;
+  }
+  return true;
+}
+
+rpl_result stream_cloud_dev(rpl_capsule_stream* cs, const rpl_cloud_params* params, float* xyzi,
+                            uint32_t* point_counts, void* stream) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!stream_cloud_args_ok(cs, params, xyzi, point_counts)) return RPL_RESULT_INVALID_DATA;
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
+  // the last push's kernels are done before these read its arena and views; the next push waits for these
+  RPL_CUDA(c, cudaStreamWaitEvent(st, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
+  const size_t row = (size_t)cs->max_scans * cs->max_nodes * 4;
+  rpl_result r = RPL_RESULT_OK;
+  for (uint32_t s0 = 0; s0 < cs->n_streams && r == RPL_RESULT_OK; s0 += cs->cloud_chunk)
+    r = stream_cloud_chunk(cs, c->lane[0], s0, std::min(cs->cloud_chunk, cs->n_streams - s0), params,
+                           xyzi + (size_t)s0 * row, point_counts + (size_t)s0 * cs->max_scans, st);
+  RPL_CUDA(c, cudaEventRecord(cs->done, st), RPL_RESULT_OPERATION_FAIL);
+  return r;
+}
+
+// the host variant: the last push's chunks round-robin over the lanes, each lane's clouds staged in its block and
+// copied back while the next chunk runs on the other lane
+rpl_result stream_cloud(rpl_capsule_stream* cs, const rpl_cloud_params* params, float* xyzi, uint32_t* point_counts) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!stream_cloud_args_ok(cs, params, xyzi, point_counts)) return RPL_RESULT_INVALID_DATA;
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  const uint32_t chunk = cs->cloud_chunk;
+  const size_t NS = (size_t)chunk * cs->max_scans, row = (size_t)cs->max_scans * cs->max_nodes * 4;
+  struct Regions {
+    float* xyzi;
+    uint32_t* counts;
+  };
+  auto layout = [&](Carve& k) { return Regions{k.take<float>(NS * cs->max_nodes * 4), k.take<uint32_t>(NS)}; };
+  if (const rpl_result r = grow_stage(c, kLanes, layout); r != RPL_RESULT_OK) return r;
+  for (int i = 0; i < kLanes; ++i) RPL_CUDA(c, cudaStreamWaitEvent(c->lane[i].stream, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
+  const cudaMemcpyKind d2h = cudaMemcpyDeviceToHost;
+  auto run_chunk = [&](Lane& l, uint32_t s0, uint32_t ns) -> rpl_result {
+    Carve k{l.stage};
+    const Regions d = layout(k);
+    RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);  // the lane's previous chunk has left
+    const rpl_result r = stream_cloud_chunk(cs, l, s0, ns, params, d.xyzi, d.counts, l.stream);
+    if (r != RPL_RESULT_OK) return r;
+    RPL_CUDA(c, cudaMemcpyAsync(xyzi + (size_t)s0 * row, d.xyzi, ns * row * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(point_counts + (size_t)s0 * cs->max_scans, d.counts, (size_t)ns * cs->max_scans * 4, d2h,
+                                l.stream),
+             RPL_RESULT_OPERATION_FAIL);
+    return RPL_RESULT_OK;
+  };
+  return run_chunks(c, cs->n_streams, chunk, run_chunk);
 }
 
 }  // namespace
@@ -2023,6 +2160,37 @@ rpl_result rpl_normal_stream_state(rpl_normal_stream* ns, uint32_t* open_nodes, 
   return rpl_capsule_stream_state(capsule_session(ns), open_nodes, held_bytes);
 }
 
+// ---- session clouds: the PointCloud2 chain over the scans the last push published, read in place ----
+rpl_result rpl_capsule_stream_cloud_dev(rpl_capsule_stream* cs, const rpl_cloud_params* params, float* xyzi,
+                                        uint32_t* point_counts, void* stream) {
+  return stream_cloud_dev(cs, params, xyzi, point_counts, stream);
+}
+
+rpl_result rpl_capsule_stream_cloud(rpl_capsule_stream* cs, const rpl_cloud_params* params, float* xyzi,
+                                    uint32_t* point_counts) {
+  return stream_cloud(cs, params, xyzi, point_counts);
+}
+
+rpl_result rpl_dense_stream_cloud_dev(rpl_dense_stream* ds, const rpl_cloud_params* params, float* xyzi,
+                                      uint32_t* point_counts, void* stream) {
+  return stream_cloud_dev(capsule_session(ds), params, xyzi, point_counts, stream);
+}
+
+rpl_result rpl_dense_stream_cloud(rpl_dense_stream* ds, const rpl_cloud_params* params, float* xyzi,
+                                  uint32_t* point_counts) {
+  return stream_cloud(capsule_session(ds), params, xyzi, point_counts);
+}
+
+rpl_result rpl_normal_stream_cloud_dev(rpl_normal_stream* ns, const rpl_cloud_params* params, float* xyzi,
+                                       uint32_t* point_counts, void* stream) {
+  return stream_cloud_dev(capsule_session(ns), params, xyzi, point_counts, stream);
+}
+
+rpl_result rpl_normal_stream_cloud(rpl_normal_stream* ns, const rpl_cloud_params* params, float* xyzi,
+                                   uint32_t* point_counts) {
+  return stream_cloud(capsule_session(ns), params, xyzi, point_counts);
+}
+
 // ---- LaserScan / PointCloud2 -> CDR (SURVEY.md 8(f) rank 3) -------------------------------------
 namespace {
 struct CdrWriter {  // XCDR1 little endian; alignment counts from the byte after the encapsulation header
@@ -2233,14 +2401,11 @@ rpl_result rpl_cloud_batch_dev(rpl_ctx* c, const rpl_node_hq* nodes, const uint3
                                float* xyzi, uint32_t* point_counts, void* stream) {
   if (!c || !nodes || !counts || !params || !xyzi || !point_counts) return RPL_RESULT_INVALID_DATA;
   if (n_scans == 0) return RPL_RESULT_OK;
-  if (n_scans > c->max_scans || params->sor_k > 32) {
-    c->err = "n_scans exceeds max_scans or sor_k > 32";
+  if (n_scans > c->max_scans) {
+    c->err = "n_scans exceeds max_scans";
     return RPL_RESULT_INVALID_DATA;
   }
-  if (params->voxel_size != 0.0f && !(params->voxel_size >= 1e-6f && params->range_max < 1000.0f)) {
-    c->err = "voxel grid: voxel_size must be >= 1e-6 m and range_max < 1000 m (cell indices must fit 31 bits)";
-    return RPL_RESULT_INVALID_DATA;
-  }
+  if (!cloud_params_ok(c, params)) return RPL_RESULT_INVALID_DATA;
   cudaStream_t st;
   if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   rpl::ScanBatchArgs a{};

@@ -52,6 +52,7 @@ struct rpl_ctx {
   uint2* d_desc = nullptr;
   size_t reset_prefix_cap = 0, desc_cap = 0;
   cudaEvent_t asm_done = nullptr;   // the wire-to-LaserScan chunks of every lane and stream share the assemble scratch
+  cudaEvent_t cloud_done = nullptr; // the session clouds' post passes of every lane and stream share lane 0's scratch
   bool profile = false;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_fast, prof_general;
 };

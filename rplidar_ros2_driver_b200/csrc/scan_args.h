@@ -61,7 +61,7 @@ struct FastWorkspace {
 constexpr uint32_t kSmallMaxNodes = 8192;
 constexpr uint32_t kSmallPostMaxNodes = 4096;
 struct SmallArgs {
-  uint32_t cap;        // stride rounded up to 64 nodes: capacity of the shared-memory arrays
+  uint32_t cap;        // stride (or cap_nodes) rounded up to 64 nodes: capacity of the shared-memory arrays
   uint32_t max_nodes;  // the context's max_nodes (a larger count is a caller error)
   uint32_t use_tma;    // every scan base is 16-byte aligned: stage with one bulk-TMA copy
   uint32_t sor_k;      // PointCloud2 chain: 0 = no outlier removal
@@ -73,8 +73,10 @@ bool scan_small_post_applies(uint32_t stride);
 cudaError_t scan_small_configure();
 // a.xyzi set: PointCloud2 (window + xyz, then SOR / voxel grid in shared memory when asked for); else LaserScan
 // Mode A/B with the ascended buffer when a.nodes_out is set.  Duplicate-key scans land in a.fallback_list.
+// cap_nodes (PointCloud2 chain with SOR / voxel grid fused, scan views): size the shared-memory arrays for this many
+// nodes instead of the stride; a view longer than that lands in a.fallback_list as well.  0: the stride.
 cudaError_t launch_scan_small(const ScanBatchArgs& a, uint32_t max_nodes, uint32_t sor_k, float sor_alpha, float voxel,
-                              int num_sms, cudaStream_t stream);
+                              int num_sms, cudaStream_t stream, uint32_t cap_nodes = 0);
 
 constexpr int kFastThreads = 512;
 constexpr int kGeneralThreads = 128;

@@ -331,6 +331,10 @@ __global__ void __launch_bounds__(TS, POST ? 2 : (EMIT ? 4 : (MODE == 0 ? 5 : 1)
       if (tid == 0) write_outcome(a, s, kResultInvalidData, 0u, 0.0f);
       continue;
     }
+    if (POST && n > cap) {  // a view longer than the shared-memory arrays (cap < stride): the general kernel's
+      if (tid == 0) hand_to_general(a, s);
+      continue;
+    }
     if (n == 0) {  // ascendScanData: OPERATION_FAIL; publish_scan: nodes.empty() -> return
       if (tid == 0) write_outcome_empty(a, s);
       continue;
@@ -1022,9 +1026,9 @@ cudaError_t scan_small_configure() {
 }
 
 cudaError_t launch_scan_small(const ScanBatchArgs& a, uint32_t max_nodes, uint32_t sor_k, float sor_alpha, float voxel,
-                              int num_sms, cudaStream_t stream) {
+                              int num_sms, cudaStream_t stream, uint32_t cap_nodes) {
   SmallArgs p{};
-  p.cap = (a.stride + 63u) & ~63u;
+  p.cap = ((cap_nodes ? cap_nodes : a.stride) + 63u) & ~63u;
   p.max_nodes = max_nodes;
   p.use_tma = ((reinterpret_cast<uintptr_t>(a.nodes) & 15u) == 0 && (a.stride & 1u) == 0) ? 1u : 0u;
   p.sor_k = sor_k;

@@ -31,6 +31,12 @@ and small pushes of 512 streams x about 2 KB (a 20 ms receive period at 1 Mbaud)
 capsules (every push starts on a frame), one pushed a byte count that is no multiple of the frame size, so most pushes
 begin with held bytes and the stream sits off the word grid; three sessions timed in alternating rounds in one run.
 
+With --cloud, the session clouds (rpl_capsule_stream_cloud_dev): push_dev alone against push_dev + cloud_dev with the
+window only, 5 cm voxels, and SOR k=8 + 5 cm voxels, the last two fused (flags 0) and as separate passes
+(RPL_CLOUD_NO_FUSED), at max_nodes 4096 and 8192 (at 8192 the fused kernel's shared memory is sized for 4096 nodes and
+longer revolutions go to the general kernel), on the chain shape of 0x85 and the comparison shape of 0x84 (or of
+--format): 512 streams, revolutions of about 3200 nodes; all timed in alternating rounds in one run.
+
 Each push continues the stream where the previous one ended (the capsules of a push follow on in angle), so the carry
 and the held capsule are exercised as in a live feed.  The GPU's name and power limit are part of the output.
 """
@@ -466,6 +472,75 @@ def compare_bytes(R, torch, fmt, steps, rounds, small):
     return res
 
 
+def compare_cloud(R, torch, fmt, steps, rounds):
+    """ms per push_dev alone and per push_dev + cloud_dev (window only; 5 cm voxels; SOR k=8 + 5 cm voxels; fused and
+    RPL_CLOUD_NO_FUSED) at max_nodes 4096 and 8192, on the chain-like shape of `fmt` (revolutions of about 3200 nodes),
+    alternating rounds of `steps` pushes"""
+    n_streams, max_scans = 512, 56
+    if fmt == 0x85:
+        n_units, data = 4096, feed(16, 2 * 4096, seed=7)
+    else:
+        n_units = FORMATS[fmt][2]
+        data = feed_format(fmt, 16, 2 * n_units, seed=7)
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    params = R.scan_params(1, 0, 0, 1)
+    cs = stream.cuda_stream
+    NS = n_streams * max_scans
+    configs = [("push", None), ("window", {}), ("voxel", dict(voxel_size=0.05)),
+               ("voxel_separate", dict(voxel_size=0.05, flags=R.CLOUD_NO_FUSED)),
+               ("sor_voxel", dict(sor_k=8, sor_alpha=1.0, voxel_size=0.05)),
+               ("sor_voxel_separate", dict(sor_k=8, sor_alpha=1.0, voxel_size=0.05, flags=R.CLOUD_NO_FUSED))]
+    res = {"format": hex(fmt), "streams": n_streams, "units_per_push": n_units, "max_scans": max_scans, "steps": steps,
+           "rounds": rounds, "by_max_nodes": []}
+    for max_nodes in (4096, 8192):
+        ctx = R.Context(0, max_nodes, NS)
+        with torch.cuda.stream(stream):
+            halves = [torch.from_numpy(np.ascontiguousarray(np.tile(data[:, h * n_units:(h + 1) * n_units],
+                                                                    (n_streams // 16, 1, 1)))).to(dev) for h in (0, 1)]
+            d_cnt = torch.full((n_streams,), n_units, dtype=torch.int32, device=dev)
+            r = torch.empty((NS, max_nodes), device=dev)
+            it = torch.empty((NS, max_nodes), device=dev)
+            bc = torch.zeros(NS, dtype=torch.int32, device=dev)
+            inc = torch.zeros(NS, device=dev)
+            sps = torch.zeros(n_streams, dtype=torch.int32, device=dev)
+            xyzi = torch.empty((NS, max_nodes, 4), device=dev)
+            pc = torch.zeros(NS, dtype=torch.int32, device=dev)
+        stream.synchronize()
+        row = {"max_nodes": max_nodes, "ms": {k: [] for k, _ in configs}}
+        points = {}
+        with R.CapsuleStreamSession(ctx, fmt, n_streams, n_units, max_nodes, max_scans) as sess:
+            def step_fn(prm):
+                def step(t):
+                    sess.push_dev(halves[t % 2].data_ptr(), d_cnt.data_ptr(), params, r.data_ptr(), it.data_ptr(),
+                                  bc.data_ptr(), inc.data_ptr(), sps.data_ptr(), stream=cs)
+                    if prm is not None:
+                        sess.cloud_dev(prm, xyzi.data_ptr(), pc.data_ptr(), stream=cs)
+                return step
+
+            fns = {k: step_fn(None if kw is None else R.cloud_params(range_min=0.15, range_max=40.0, **kw))
+                   for k, kw in configs}
+            for _ in range(rounds):
+                for k, _ in configs:
+                    row["ms"][k].append(timed(torch, stream, fns[k], steps))
+                    if k != "push":
+                        points[k] = int(pc.sum().item())
+            row["scans_per_push"] = int(sps.sum().item())
+            row["scan_nodes_per_push"] = int(bc.sum().item())
+        med = {k: float(np.median(v)) for k, v in row["ms"].items()}
+        row["ms_median"] = med
+        row["cloud_ms_median"] = {k: med[k] - med["push"] for k, _ in configs[1:]}
+        # points into the cloud chain (the window's points) and out of it, per push; points/s of push + cloud
+        row["points_in_per_push"] = points["window"]
+        row["points_out_per_push"] = points
+        row["gpoints_per_s"] = {k: points["window"] / (med[k] * 1e-3) / 1e9 for k, _ in configs[1:]}
+        row["fused_over_separate"] = {k: med[k] / med[k + "_separate"] - 1.0 for k in ("voxel", "sor_voxel")}
+        res["by_max_nodes"].append(row)
+        del halves, r, it, xyzi
+        ctx.close()
+    return res
+
+
 def gpu_info():
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                        capture_output=True, text=True)
@@ -481,10 +556,20 @@ def main():
     ap.add_argument("--stamped", action="store_true", help="stamped against unstamped pushes of --format")
     ap.add_argument("--rounds", type=int, default=5, help="--stamped, --bytes: alternating rounds of --steps pushes each")
     ap.add_argument("--bytes", action="store_true", help="byte pushes against framed pushes of --format (not 0x81)")
+    ap.add_argument("--cloud", action="store_true",
+                    help="push_dev alone against push_dev + cloud_dev (0x85 and 0x84 unless --format is given)")
     args = ap.parse_args()
     import torch
 
     import rplidar_ros2_driver_b200 as R
+
+    if args.cloud:
+        fmts = [args.format] if "--format" in " ".join(sys.argv) else [0x85, 0x84]
+        if 0x81 in fmts:
+            ap.error("--cloud takes a capsule format")
+        print(json.dumps({"gpu": gpu_info(), "cloud": [compare_cloud(R, torch, f, args.steps, args.rounds)
+                                                       for f in fmts]}))
+        return
 
     if args.bytes:
         if args.format == 0x81:

@@ -49,7 +49,10 @@
  * ordered on the stream passed in (NULL = the context's own stream).  The context's own stream is a non-blocking
  * stream: it does not wait for work the caller has in flight on other streams (the legacy default stream included).
  * A caller that fills its device buffers on a stream of its own either passes that stream, or synchronises before the
- * call and calls rpl_ctx_synchronize before it reads the results.
+ * call and calls rpl_ctx_synchronize before it reads the results.  One context's calls may be issued on several
+ * streams, device and host calls mixed: their scan kernels take turns on the context's scan scratch in the order the
+ * calls were made (each call waits on its stream for the previous call's scan kernels), so every call gives what it
+ * gives alone.
  *
  * Tie rule.  The reference sorts with std::sort (unstable); on equal angle_z_q14 its order
  * is whatever libstdc++'s introsort produces.  This library defines the order: equal keys
@@ -650,8 +653,8 @@ rpl_result rpl_normal_stream_state(rpl_normal_stream* s, uint32_t* open_nodes, u
  *            sor_k > 32, outside the voxel rule of rpl_cloud_batch_dev or with a null pointer:
  *            RPL_RESULT_INVALID_DATA.
  *   cloud_dev: device buffers, asynchronous on `stream` (NULL = the context's stream).  It waits for the session's
- *            last push (on any stream) and the session's next push waits for it.  The SOR / voxel passes of every
- *            session cloud on a context take turns on the context's cloud workspace, whatever their stream.
+ *            last push (on any stream) and the session's next push waits for it.  Its scan kernels and SOR / voxel
+ *            passes take turns with every other call of the context on its scan scratch, whatever their stream.
  *   cloud:   host buffers, synchronous, chunked over the context's lanes as a host push is. */
 rpl_result rpl_capsule_stream_cloud_dev(rpl_capsule_stream* s, const rpl_cloud_params* params, float* xyzi,
                                         uint32_t* point_counts, void* stream);

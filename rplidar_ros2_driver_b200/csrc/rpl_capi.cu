@@ -46,6 +46,7 @@ void free_lane(Lane& l) {
   cudaFree(l.gws.cell);
   if (l.owns_cws) rpl::cloud_workspace_free(l.cws);
   cudaFree(l.stage);
+  if (l.scratch_free) cudaEventDestroy(l.scratch_free);
   if (l.stream) cudaStreamDestroy(l.stream);
   l = Lane{};
 }
@@ -165,7 +166,20 @@ rpl_result launch_general(rpl_ctx* c, Lane& l, const rpl::ScanBatchArgs& a, bool
   return RPL_RESULT_OK;
 }
 
-// the fast kernel, then the general kernel for the scans it hands on (or for all), on `stream` with no host round trip
+// A lane's scan scratch (Lane::scratch_free) is taken by one section of kernels at a time: the device calls of every
+// stream run on lane 0's, the host calls' chunks on their lane's.  A section starts, on its stream, after the lane's
+// previous section has ended, and ends after its last kernel that reads the scratch.
+rpl_result scratch_enter(rpl_ctx* c, const Lane& l, cudaStream_t stream) {
+  RPL_CUDA(c, cudaStreamWaitEvent(stream, l.scratch_free, 0), RPL_RESULT_OPERATION_FAIL);
+  return RPL_RESULT_OK;
+}
+rpl_result scratch_leave(rpl_ctx* c, const Lane& l, cudaStream_t stream) {
+  RPL_CUDA(c, cudaEventRecord(l.scratch_free, stream), RPL_RESULT_OPERATION_FAIL);
+  return RPL_RESULT_OK;
+}
+
+// the fast kernel, then the general kernel for the scans it hands on (or for all), on `stream` with no host round trip;
+// the caller holds lane l's scratch (scratch_enter) from before this call to after the last reader of its fallback list
 rpl_result enqueue_args(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, uint32_t flags, cudaStream_t stream,
                         const rpl_cloud_params* cloud = nullptr, bool* post_fused = nullptr, bool hand_off = false) {
   if (post_fused) *post_fused = false;
@@ -240,7 +254,9 @@ rpl_result enqueue_scan(rpl_ctx* c, Lane& l, const rpl_node_hq* nodes, const uin
   a.path = path;
   a.views = views;
   a.nodes_total = nodes_total;
-  return enqueue_args(c, l, a, p->flags, stream);
+  rpl_result r = scratch_enter(c, l, stream);
+  if (r == RPL_RESULT_OK) r = enqueue_args(c, l, a, p->flags, stream);
+  return r == RPL_RESULT_OK ? scratch_leave(c, l, stream) : r;
 }
 
 // Runs fn(lane, first, n) over `total` items in chunks of `chunk`, round-robin over the lanes, and waits for every
@@ -334,7 +350,8 @@ rpl_result rpl_ctx_create(int device, uint32_t max_nodes, uint32_t max_scans, rp
   for (int i = 0; i < kLanes; ++i) {
     Lane& l = c->lane[i];
     const rpl_result oom = RPL_RESULT_INSUFFICIENT_MEMORY;
-    if (!cuda_ok(c, cudaStreamCreateWithFlags(&l.stream, cudaStreamNonBlocking), "cudaStreamCreate"))
+    if (!cuda_ok(c, cudaStreamCreateWithFlags(&l.stream, cudaStreamNonBlocking), "cudaStreamCreate") ||
+        !cuda_ok(c, cudaEventCreateWithFlags(&l.scratch_free, cudaEventDisableTiming), "cudaEventCreate"))
       return fail(RPL_RESULT_OPERATION_FAIL);
     const size_t fast_nodes = (size_t)c->fast_grid * max_nodes;  // launch_scan_fast never gets a larger grid
     const size_t gen_nodes = (size_t)c->general_grid * max_nodes;
@@ -384,7 +401,6 @@ void rpl_ctx_destroy(rpl_ctx* c) {
     free_lane(c->lane[i]);
   }
   if (c->asm_done) cudaEventDestroy(c->asm_done);
-  if (c->cloud_done) cudaEventDestroy(c->cloud_done);
   cudaFree(c->d_reset_prefix);
   cudaFree(c->d_desc);
   if (c->h_one) cudaFreeHost(c->h_one);
@@ -658,14 +674,19 @@ rpl_result scan_single(rpl_ctx* c, const rpl_node_hq* nodes_in, size_t count, co
     RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);
     return RPL_RESULT_OK;
   };
+  // the fallback list is the control block's; fws and gws are lane 0's, which device calls on other streams share
   const FastKernel k = pick_fast(a, p->flags);
   if (k != FastKernel::kNone) {
-    rpl_result r = launch_fast(c, l, a, k, l.stream);
+    rpl_result r = scratch_enter(c, l, l.stream);
+    if (r == RPL_RESULT_OK) r = launch_fast(c, l, a, k, l.stream);
+    if (r == RPL_RESULT_OK) r = scratch_leave(c, l, l.stream);
     if (r == RPL_RESULT_OK) r = copy_back();
     if (r != RPL_RESULT_OK) return r;
   }
   if (k == FastKernel::kNone || hs->fallback_count != 0) {
-    rpl_result r = launch_general(c, l, a, true, l.stream);
+    rpl_result r = scratch_enter(c, l, l.stream);
+    if (r == RPL_RESULT_OK) r = launch_general(c, l, a, true, l.stream);
+    if (r == RPL_RESULT_OK) r = scratch_leave(c, l, l.stream);
     if (r == RPL_RESULT_OK) r = copy_back();
     if (r != RPL_RESULT_OK) return r;
   }
@@ -1711,19 +1732,22 @@ rpl_result stream_cloud_chunk(rpl_capsule_stream* cs, Lane& l, uint32_t s0, uint
   a.intensity_min = p->intensity_min;
   const bool separate = (p->flags & RPL_CLOUD_NO_FUSED) != 0;
   bool fused = false;
-  rpl_result r = enqueue_args(c, l, a, 0u, st, separate ? nullptr : p, &fused, true);
-  if (r != RPL_RESULT_OK || (p->sor_k == 0 && p->voxel_size == 0.0f)) return r;
-  if (!c->cloud_done)
-    RPL_CUDA(c, cudaEventCreateWithFlags(&c->cloud_done, cudaEventDisableTiming), RPL_RESULT_OPERATION_FAIL);
-  RPL_CUDA(c, cudaStreamWaitEvent(st, c->cloud_done, 0), RPL_RESULT_OPERATION_FAIL);
-  int launched = 0;
-  RPL_CUDA(c, rpl::launch_cloud_post(a.xyzi, point_counts, a.n_scans, a.stride, p->sor_k, p->sor_alpha, p->voxel_size,
-                                     c->lane[0].cws, fused ? a.fallback_list : nullptr,
-                                     fused ? a.fallback_count : nullptr, st, &launched),
-           RPL_RESULT_OPERATION_FAIL);
-  c->launches += launched;
-  RPL_CUDA(c, cudaEventRecord(c->cloud_done, st), RPL_RESULT_OPERATION_FAIL);
-  return RPL_RESULT_OK;
+  rpl_result r = scratch_enter(c, l, st);
+  if (r == RPL_RESULT_OK) r = enqueue_args(c, l, a, 0u, st, separate ? nullptr : p, &fused, true);
+  if (r != RPL_RESULT_OK) return r;
+  if (p->sor_k > 0 || p->voxel_size > 0.0f) {
+    // the post passes read lane l's fallback list and run on lane 0's cws: a lane-1 chunk takes lane 0's scratch too
+    Lane& post = c->lane[0];
+    if (&l != &post && (r = scratch_enter(c, post, st)) != RPL_RESULT_OK) return r;
+    int launched = 0;
+    RPL_CUDA(c, rpl::launch_cloud_post(a.xyzi, point_counts, a.n_scans, a.stride, p->sor_k, p->sor_alpha, p->voxel_size,
+                                       post.cws, fused ? a.fallback_list : nullptr, fused ? a.fallback_count : nullptr,
+                                       st, &launched),
+             RPL_RESULT_OPERATION_FAIL);
+    c->launches += launched;
+    if (&l != &post && (r = scratch_leave(c, post, st)) != RPL_RESULT_OK) return r;
+  }
+  return scratch_leave(c, l, st);
 }
 
 bool stream_cloud_args_ok(rpl_capsule_stream* cs, const rpl_cloud_params* params, float* xyzi, uint32_t* point_counts) {
@@ -2428,7 +2452,8 @@ rpl_result rpl_cloud_batch_dev(rpl_ctx* c, const rpl_node_hq* nodes, const uint3
   // handed to the general kernel.  Larger revolutions: steps 1-3 inside the scan kernels, steps 4-5 as post passes.
   bool fused = false;
   const uint32_t flags = (params->flags & RPL_CLOUD_NO_FUSED) ? RPL_FLAG_NO_SMALL : 0u;
-  rpl_result r = enqueue_args(c, c->lane[0], a, flags, st, params, &fused);
+  rpl_result r = scratch_enter(c, c->lane[0], st);
+  if (r == RPL_RESULT_OK) r = enqueue_args(c, c->lane[0], a, flags, st, params, &fused);
   if (r != RPL_RESULT_OK) return r;
   if (params->sor_k > 0 || params->voxel_size > 0.0f) {
     int launched = 0;
@@ -2438,7 +2463,7 @@ rpl_result rpl_cloud_batch_dev(rpl_ctx* c, const rpl_node_hq* nodes, const uint3
              RPL_RESULT_OPERATION_FAIL);
     c->launches += launched;
   }
-  return RPL_RESULT_OK;
+  return scratch_leave(c, c->lane[0], st);
 }
 
 rpl_result rpl_cloud_batch(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t* counts,

@@ -22,6 +22,10 @@ struct Lane {
   rpl::GeneralWorkspace gws{};
   rpl::CloudWorkspace cws{};   // lane 0 owns the tables and the post-pass scratch; the others alias its tables
   bool owns_cws = false;
+  // The scan scratch above (fallback list and count, fws, gws; lane 0's also the post-pass cws) serves one call's
+  // kernels at a time, whatever stream the call runs on: each section that uses it waits on this event first and
+  // records it after its last reader (scratch_enter / scratch_leave in rpl_capi.cu).
+  cudaEvent_t scratch_free = nullptr;
   // device staging of every host-buffer call (batches, the chain, the sessions' host pushes, the single-stream
   // decoders): one block, grown before a call's chunk loop, that each call carves into the regions of one chunk
   unsigned char* stage = nullptr;
@@ -52,7 +56,6 @@ struct rpl_ctx {
   uint2* d_desc = nullptr;
   size_t reset_prefix_cap = 0, desc_cap = 0;
   cudaEvent_t asm_done = nullptr;   // the wire-to-LaserScan chunks of every lane and stream share the assemble scratch
-  cudaEvent_t cloud_done = nullptr; // the session clouds' post passes of every lane and stream share lane 0's scratch
   bool profile = false;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_fast, prof_general;
 };

@@ -40,6 +40,9 @@
  *                              search for the sync bytes carried across calls
  *   rpl_normal_stream_*      the same for the standard-node unpacker: raw 0x81 bytes pushed in any pieces
  *   rpl_*_stream_push_ts*    a session push that also stamps every published scan with its scan-begin time
+ *   rpl_*_stream_*_msgs*     (with rpl_*_stream_set_frames) the serialised LaserScan / PointCloud2 of every scan a
+ *                              session push published, packed: what scan_pub_->publish hands the RMW layer
+ *                              src/rplidar_node.cpp:616-679
  *   rpl_*_cdr_batch_dev      the serialised form of the message scan_pub_->publish hands to the RMW layer
  *                              src/rplidar_node.cpp:679
  *   rpl_cloud_fuse_push_dev  (with rpl_peer_*) the fused cloud's all-gather across GPUs, in the pack kernel
@@ -668,6 +671,88 @@ rpl_result rpl_normal_stream_cloud_dev(rpl_normal_stream* s, const rpl_cloud_par
                                        uint32_t* point_counts, void* stream);
 rpl_result rpl_normal_stream_cloud(rpl_normal_stream* s, const rpl_cloud_params* params, float* xyzi,
                                    uint32_t* point_counts);
+
+/* Session messages: the serialised sensor_msgs/LaserScan and PointCloud2 (XCDR1, as rpl_*_cdr_batch_dev below) of
+ * every scan the session's last successful push published, packed back to back, each ready for
+ * rclcpp::SerializedMessage (INTEGRATION.md 4c) -- what scan_pub_->publish (src/rplidar_node.cpp:679) hands the RMW
+ * layer, without the padded [n_streams * max_scans][max_nodes] arrays crossing the link.
+ *   set_frames: per stream the message settings, synchronous: frame_ids [n_streams] (each at most 255 characters),
+ *            range_max [n_streams] (nullable: keep the current values; the caller passes min(max_distance, hardware
+ *            limit) per lidar, as rplidar_node.cpp:389-393).  Before the first call: "laser_frame" and 12.0f, the
+ *            reference's defaults (rplidar_node.cpp:80, rplidar_node.hpp:328).
+ *   Which scans, repeat calls, ordering and errors: those of the session clouds above.  Slot i = s * max_scans + k.
+ *   laserscan_msgs[_dev]: slot k of stream s has a message iff k < min(scans_per_stream[s], max_scans) and its beam
+ *            count is > 0 (the reference does not publish an empty scan, :609-611).  With B / E the slot's scan-begin
+ *            stamp and the stamp of the scan-start node that closed it (the next scan's begin, whether that scan was
+ *            published, dropped past max_scans or reset), SDK microseconds, 0 when unknown:
+ *              ranges, intensities, angle_increment: what the push returned for the slot with the same params (the
+ *                scan kernels run again on the scans where the session keeps them);
+ *              header.stamp: t = B * 1000 + clock_offset_ns (int64 nanoseconds), sec = t / 10^9, nanosec = t % 10^9;
+ *                {0, 0} when B == 0, t < 0 or sec > INT32_MAX;
+ *              frame_id, range_max: the stream's settings; range_min 0.15f, angle_min 0.0f, angle_max (float)(2 pi);
+ *              scan_duration = (double)((E - B) * 1000) / 1e9 (rclcpp Duration::seconds()), scan_time =
+ *                (float)scan_duration, time_increment = (float)(scan_duration / denom), denom = beams in Mode A,
+ *                max(beams - 1, 1) in Mode B (:635, :667); both 0 when B or E is 0 or E <= B.
+ *            An unstamped push's messages have stamp {0, 0} and scan_time = time_increment = 0.
+ *   cloud_msgs[_dev]: one message for every published slot (k < min(scans_per_stream[s], max_scans)), empty clouds
+ *            included (the node publishes the cloud also when it drops the LaserScan): the session cloud of that slot
+ *            (rpl_*_stream_cloud with the same params) as rpl_pointcloud2_cdr_batch_dev writes it, with the stamp and
+ *            frame_id above.
+ *   Packing: message i starts at msgs + msg_offsets[i], a multiple of 16 (msg_offsets [n_streams * max_scans] is the
+ *            exclusive scan of the sizes, each rounded up to 16), msg_sizes[i] its bytes (0: no message), *total_bytes
+ *            the end of the last message.  When *total_bytes exceeds capacity no message is written and every size is
+ *            0; *total_bytes still reports the bytes needed (the host form then returns RPL_RESULT_INSUFFICIENT_MEMORY).
+ *            Nothing at or past msgs + *total_bytes is written; the padding between messages is unspecified.
+ *   _dev:    device buffers, asynchronous on `stream` (NULL = the context's stream); msgs 16-byte aligned, msg_offsets
+ *            and total_bytes 8-byte, msg_sizes 4-byte aligned.  The session keeps a device block of its own for the
+ *            scan outputs of every slot (8 bytes per node of max_nodes for LaserScan, 16 for PointCloud2), grown on
+ *            the first call.
+ *   host:    synchronous; copies back the tables, then only total_bytes of messages, chunked over the context's
+ *            lanes as the host cloud call is. */
+rpl_result rpl_capsule_stream_set_frames(rpl_capsule_stream* s, const char* const* frame_ids, const float* range_max);
+rpl_result rpl_capsule_stream_laserscan_msgs_dev(rpl_capsule_stream* s, const rpl_scan_params* params,
+                                                 int64_t clock_offset_ns, uint8_t* msgs, uint64_t capacity,
+                                                 uint64_t* msg_offsets, uint32_t* msg_sizes, uint64_t* total_bytes,
+                                                 void* stream);
+rpl_result rpl_capsule_stream_laserscan_msgs(rpl_capsule_stream* s, const rpl_scan_params* params,
+                                             int64_t clock_offset_ns, uint8_t* msgs, uint64_t capacity,
+                                             uint64_t* msg_offsets, uint32_t* msg_sizes, uint64_t* total_bytes);
+rpl_result rpl_capsule_stream_cloud_msgs_dev(rpl_capsule_stream* s, const rpl_cloud_params* params,
+                                             int64_t clock_offset_ns, uint8_t* msgs, uint64_t capacity,
+                                             uint64_t* msg_offsets, uint32_t* msg_sizes, uint64_t* total_bytes,
+                                             void* stream);
+rpl_result rpl_capsule_stream_cloud_msgs(rpl_capsule_stream* s, const rpl_cloud_params* params, int64_t clock_offset_ns,
+                                         uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
+                                         uint64_t* total_bytes);
+rpl_result rpl_dense_stream_set_frames(rpl_dense_stream* s, const char* const* frame_ids, const float* range_max);
+rpl_result rpl_dense_stream_laserscan_msgs_dev(rpl_dense_stream* s, const rpl_scan_params* params,
+                                               int64_t clock_offset_ns, uint8_t* msgs, uint64_t capacity,
+                                               uint64_t* msg_offsets, uint32_t* msg_sizes, uint64_t* total_bytes,
+                                               void* stream);
+rpl_result rpl_dense_stream_laserscan_msgs(rpl_dense_stream* s, const rpl_scan_params* params, int64_t clock_offset_ns,
+                                           uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
+                                           uint64_t* total_bytes);
+rpl_result rpl_dense_stream_cloud_msgs_dev(rpl_dense_stream* s, const rpl_cloud_params* params, int64_t clock_offset_ns,
+                                           uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
+                                           uint64_t* total_bytes, void* stream);
+rpl_result rpl_dense_stream_cloud_msgs(rpl_dense_stream* s, const rpl_cloud_params* params, int64_t clock_offset_ns,
+                                       uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
+                                       uint64_t* total_bytes);
+rpl_result rpl_normal_stream_set_frames(rpl_normal_stream* s, const char* const* frame_ids, const float* range_max);
+rpl_result rpl_normal_stream_laserscan_msgs_dev(rpl_normal_stream* s, const rpl_scan_params* params,
+                                                int64_t clock_offset_ns, uint8_t* msgs, uint64_t capacity,
+                                                uint64_t* msg_offsets, uint32_t* msg_sizes, uint64_t* total_bytes,
+                                                void* stream);
+rpl_result rpl_normal_stream_laserscan_msgs(rpl_normal_stream* s, const rpl_scan_params* params,
+                                            int64_t clock_offset_ns, uint8_t* msgs, uint64_t capacity,
+                                            uint64_t* msg_offsets, uint32_t* msg_sizes, uint64_t* total_bytes);
+rpl_result rpl_normal_stream_cloud_msgs_dev(rpl_normal_stream* s, const rpl_cloud_params* params,
+                                            int64_t clock_offset_ns, uint8_t* msgs, uint64_t capacity,
+                                            uint64_t* msg_offsets, uint32_t* msg_sizes, uint64_t* total_bytes,
+                                            void* stream);
+rpl_result rpl_normal_stream_cloud_msgs(rpl_normal_stream* s, const rpl_cloud_params* params, int64_t clock_offset_ns,
+                                        uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
+                                        uint64_t* total_bytes);
 
 /* ---- LaserScan / PointCloud2 -> wire (SURVEY.md 8(f) rank 3) ---------------------------- */
 /* The serialised message the RMW layer would produce from the message the reference publishes

@@ -21,6 +21,7 @@ RESULT_OK = 0
 RESULT_INVALID_DATA = 0x80008000
 RESULT_OPERATION_FAIL = 0x80008001
 RESULT_OPERATION_NOT_SUPPORT = 0x80008004
+RESULT_INSUFFICIENT_MEMORY = 0x80008006
 FLAG_FORCE_GENERAL = 1
 FLAG_NO_TMA = 2
 FLAG_NO_SMALL = 4
@@ -58,6 +59,8 @@ EXPORTS = [
     "rpl_normal_stream_reset", "rpl_normal_stream_state", "rpl_normal_stream_push_ts", "rpl_normal_stream_push_ts_dev",
     "rpl_capsule_stream_cloud", "rpl_capsule_stream_cloud_dev", "rpl_dense_stream_cloud", "rpl_dense_stream_cloud_dev",
     "rpl_normal_stream_cloud", "rpl_normal_stream_cloud_dev",
+    *[f"rpl_{kind}_stream_{fn}" for kind in ("capsule", "dense", "normal")
+      for fn in ("set_frames", "laserscan_msgs", "laserscan_msgs_dev", "cloud_msgs", "cloud_msgs_dev")],
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -233,6 +236,11 @@ def lib() -> C.CDLL:
     for kind in ("capsule", "dense", "normal"):
         sig[f"rpl_{kind}_stream_cloud"] = ([vp, PCP, vp, vp], u32)
         sig[f"rpl_{kind}_stream_cloud_dev"] = ([vp, PCP, vp, vp, vp], u32)
+        sig[f"rpl_{kind}_stream_set_frames"] = ([vp, vp, vp], u32)
+        sig[f"rpl_{kind}_stream_laserscan_msgs"] = ([vp, PSP, C.c_int64, vp, u64, vp, vp, vp], u32)
+        sig[f"rpl_{kind}_stream_laserscan_msgs_dev"] = ([vp, PSP, C.c_int64, vp, u64, vp, vp, vp, vp], u32)
+        sig[f"rpl_{kind}_stream_cloud_msgs"] = ([vp, PCP, C.c_int64, vp, u64, vp, vp, vp], u32)
+        sig[f"rpl_{kind}_stream_cloud_msgs_dev"] = ([vp, PCP, C.c_int64, vp, u64, vp, vp, vp, vp], u32)
     for name, (args, res) in sig.items():
         fn = getattr(L, name)  # AttributeError here = the library does not export the ABI
         fn.argtypes = args
@@ -694,6 +702,55 @@ class CapsuleStreamSession:
     def cloud_dev(self, params: CloudParams, xyzi, point_counts, stream=None):
         """Device addresses (the layouts of cloud), asynchronous on `stream` (None: the context's stream)."""
         self._ctx._check(self._fn("cloud_dev")(self._h, C.byref(params), _p(xyzi), _p(point_counts), _p(stream)))
+
+    def set_frames(self, frame_ids, range_max=None):
+        """Per stream the frame_id and LaserScan range_max of the messages (range_max None: keep the current ones)."""
+        assert len(frame_ids) == self.n_streams
+        ids = (C.c_char_p * self.n_streams)(*[f.encode() for f in frame_ids])
+        rm = None if range_max is None else np.ascontiguousarray(range_max, dtype=np.float32)
+        assert rm is None or rm.shape == (self.n_streams,)
+        self._ctx._check(self._fn("set_frames")(self._h, C.cast(ids, C.c_void_p), _p(rm)))
+
+    def _msgs(self, name, params, clock_offset_ns, msgs, packed):
+        ns = self.n_streams * self.max_scans
+        if msgs is None:  # room for every slot's largest message
+            per = 288 + (32 + 8 * self.max_nodes + 4 if name == "laserscan_msgs" else 116 + 16 * self.max_nodes + 1)
+            msgs = np.zeros(ns * ((per + 15) // 16 * 16), np.uint8)
+        assert msgs.dtype == np.uint8 and msgs.flags.c_contiguous
+        offs, sizes, total = np.zeros(ns, np.uint64), np.zeros(ns, np.uint32), np.zeros(1, np.uint64)
+        rc = self._fn(name)(self._h, C.byref(params), int(clock_offset_ns), _p(msgs), msgs.size, _p(offs), _p(sizes),
+                            _p(total))
+        if not packed or rc != RESULT_INSUFFICIENT_MEMORY:
+            self._ctx._check(rc)
+        if packed:
+            return dict(msgs=msgs, msg_offsets=offs, msg_sizes=sizes, total_bytes=int(total[0]), result=rc)
+        return [bytes(msgs[o: o + s]) if s else None for o, s in zip(offs.tolist(), sizes.tolist())]
+
+    def laserscan_msgs(self, params: ScanParams, clock_offset_ns=0, msgs=None, packed=False):
+        """The serialised sensor_msgs/LaserScan of every scan the last push published: per slot (n_streams *
+        max_scans) the message's bytes, None for no message.  msgs: the host buffer to pack into (its size is the
+        capacity; None: one that always fits).  packed: return {"msgs", "msg_offsets", "msg_sizes", "total_bytes",
+        "result"} instead, with result RESULT_INSUFFICIENT_MEMORY rather than an exception when msgs is too small."""
+        return self._msgs("laserscan_msgs", params, clock_offset_ns, msgs, packed)
+
+    def cloud_msgs(self, params: CloudParams, clock_offset_ns=0, msgs=None, packed=False):
+        """The serialised sensor_msgs/PointCloud2 of every published slot, as laserscan_msgs."""
+        return self._msgs("cloud_msgs", params, clock_offset_ns, msgs, packed)
+
+    def laserscan_msgs_dev(self, params: ScanParams, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
+                           total_bytes, stream=None):
+        """Device addresses (msgs [capacity] bytes, msg_offsets [n_streams * max_scans] uint64, msg_sizes uint32,
+        total_bytes one uint64), asynchronous on `stream` (None: the context's stream)."""
+        self._ctx._check(self._fn("laserscan_msgs_dev")(self._h, C.byref(params), int(clock_offset_ns), _p(msgs),
+                                                         int(capacity), _p(msg_offsets), _p(msg_sizes),
+                                                         _p(total_bytes), _p(stream)))
+
+    def cloud_msgs_dev(self, params: CloudParams, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
+                       total_bytes, stream=None):
+        """Device addresses, as laserscan_msgs_dev."""
+        self._ctx._check(self._fn("cloud_msgs_dev")(self._h, C.byref(params), int(clock_offset_ns), _p(msgs),
+                                                     int(capacity), _p(msg_offsets), _p(msg_sizes), _p(total_bytes),
+                                                     _p(stream)))
 
     def reset(self, mask=None):
         """Drops the held capsule, the decoder state and the open revolution of the streams where mask is true

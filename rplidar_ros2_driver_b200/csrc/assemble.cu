@@ -296,7 +296,15 @@ __device__ __forceinline__ void assemble_body(const AssembleArgs& a, const Assem
                   a.node_ts_us ? a.node_ts_us[(size_t)s * a.stride_nodes + base + d.x] : 0ull;
           }
         }
-        if constexpr (STAMPED) a.scan_begin_ts_us[(size_t)s * a.max_scans + k] = k < stored ? stamp_at(desc[k].x) : 0ull;
+        if constexpr (STAMPED) {
+          // the end: the closing scan-start node at desc.x + desc.y, also for the last stored slot of a stream that
+          // published more than max_scans (the first dropped scan's begin)
+          const size_t o = (size_t)s * a.max_scans + k;
+          const unsigned long long b = k < stored ? stamp_at(desc[k].x) : 0ull;
+          a.scan_begin_ts_us[o] = b;
+          sa.slot_begin_us[o] = b;
+          sa.slot_end_us[o] = k < stored ? stamp_at(desc[k].x + desc[k].y) : 0ull;
+        }
         vout[k] = v;
         out_len[k] = v.y;
       }

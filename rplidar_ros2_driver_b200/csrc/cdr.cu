@@ -93,7 +93,184 @@ __global__ void __launch_bounds__(CT) pointcloud2_cdr_kernel(PointCloudCdrArgs a
   }
 }
 
+// ---- packed messages of a stream session's push -----------------------------------------------------------------
+constexpr int MT = 1024;  // the sizes and offsets pass: one CTA
+
+__device__ __forceinline__ uint32_t msg_bytes(MsgKind kind, uint32_t header_bytes, uint32_t n) {
+  return kind == MsgKind::kLaserScan ? header_bytes + 32 + 8 * n + 4 : header_bytes + 116 + 16 * n + 1;
+}
+
+// One CTA, the slots in tiles of MT: sizes, the exclusive scan of the sizes rounded up to 16 (the carry passes from
+// tile to tile), the end of the last message; then every size again, or 0 when the messages do not fit.
+__global__ void __launch_bounds__(MT) msg_table_kernel(MsgTableArgs a) {
+  __shared__ unsigned long long s_warp[MT / 32];
+  __shared__ unsigned long long s_end;
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  if (tid == 0) s_end = 0;
+  unsigned long long carry = 0;
+  auto size_of = [&](uint32_t i) -> uint32_t {
+    const uint32_t n = a.counts[i];
+    const bool has = a.kind == MsgKind::kLaserScan ? n > 0 : a.views[i].y > 0;
+    return has ? msg_bytes(a.kind, a.hdr[i / a.max_scans].bytes, n) : 0u;
+  };
+  for (uint32_t t0 = 0; t0 < a.n_slots; t0 += MT) {
+    const uint32_t i = t0 + tid;
+    const uint32_t sz = i < a.n_slots ? size_of(i) : 0u;
+    const unsigned long long v = (sz + 15u) & ~15u;
+    unsigned long long inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned long long u = __shfl_up_sync(0xffffffffu, inc, o);
+      if (lane >= (uint32_t)o) inc += u;
+    }
+    if (lane == 31) s_warp[warp] = inc;
+    __syncthreads();
+    unsigned long long base = 0, tile = 0;
+    for (uint32_t w = 0; w < MT / 32; ++w) {
+      const unsigned long long x = s_warp[w];
+      if (w < warp) base += x;
+      tile += x;
+    }
+    const unsigned long long off = carry + base + inc - v;
+    if (i < a.n_slots) {
+      a.offsets[i] = off;
+      if (sz) atomicMax(&s_end, off + sz);
+    }
+    carry += tile;
+    __syncthreads();  // s_warp is rewritten by the next tile
+  }
+  const unsigned long long total = s_end;
+  const bool fits = total <= a.capacity;
+  for (uint32_t i = tid; i < a.n_slots; i += MT) a.sizes[i] = fits ? size_of(i) : 0u;
+  if (tid == 0) *a.total = total;
+}
+
+// header.stamp of a scan-begin stamp b (SDK us) on the caller's clock: {0, 0} when unknown or not representable
+__device__ __forceinline__ void msg_stamp(unsigned long long b, long long offset_ns, uint32_t* sec, uint32_t* nanosec) {
+  *sec = 0;
+  *nanosec = 0;
+  if (b == 0) return;
+  const long long t = (long long)(b * 1000ull + (unsigned long long)offset_ns);  // int64 ns, two's complement
+  if (t < 0) return;
+  const long long s = t / 1000000000ll;
+  if (s > 2147483647ll) return;
+  *sec = (uint32_t)s;
+  *nanosec = (uint32_t)(t - s * 1000000000ll);
+}
+
+// rclcpp's Duration::seconds() of the stamp-to-stamp period (0 when either stamp is unknown or the period is not > 0)
+__device__ __forceinline__ double msg_period(unsigned long long b, unsigned long long e) {
+  if (b == 0 || e == 0 || e <= b) return 0.0;
+  return (double)(long long)((e - b) * 1000ull) / 1e9;
+}
+
+// the header words of the stream's settings, stamp words left to the caller (no two threads write one word)
+__device__ __forceinline__ void put_header(uint8_t* msg, const StreamMsgHeader& h) {
+  for (uint32_t w = threadIdx.x; w < h.bytes / 4; w += CT)
+    if (w != 1 && w != 2) put32(msg + 4 * w, h.w[w]);
+}
+
+__global__ void __launch_bounds__(CT) laserscan_msgs_kernel(MsgWriteArgs a) {
+  const uint32_t i = a.slot0 + blockIdx.y;
+  const uint32_t size = a.sizes[i];
+  if (size == 0) return;
+  const uint32_t n = a.counts[i];
+  const StreamMsgHeader& h = a.hdr[i / a.max_scans];
+  const uint32_t P = h.bytes + 32;  // the 7 floats and the ranges count follow the header
+  uint8_t* msg = a.out + (a.offsets[i] - a.out_base);
+  if (blockIdx.x == 0) {
+    put_header(msg, h);
+    if (threadIdx.x == 0) {
+      const unsigned long long b = a.begin_us ? a.begin_us[i] : 0ull, e = a.end_us ? a.end_us[i] : 0ull;
+      uint32_t sec, nsec;
+      msg_stamp(b, a.clock_offset_ns, &sec, &nsec);
+      const double d = msg_period(b, e);
+      const double denom = a.mode_a ? (double)n : (double)(n > 1 ? n - 1 : 1);
+      put32(msg + 4, sec);
+      put32(msg + 8, nsec);
+      uint8_t* f = msg + h.bytes;
+      put32(f + 0, __float_as_uint(0.0f));                             // angle_min
+      put32(f + 4, __float_as_uint((float)(2.0 * 3.14159265358979323846)));  // angle_max
+      put32(f + 8, __float_as_uint(a.angle_increment[i]));
+      put32(f + 12, __float_as_uint(__double2float_rn(d / denom)));    // time_increment
+      put32(f + 16, __float_as_uint(__double2float_rn(d)));            // scan_time
+      put32(f + 20, __float_as_uint(0.15f));                           // range_min
+      put32(f + 24, __float_as_uint(h.range_max));
+      put32(f + 28, n);
+      put32(msg + P + 4 * (size_t)n, n);  // intensities count
+    }
+  }
+  uint32_t* r_out = reinterpret_cast<uint32_t*>(msg + P);
+  uint32_t* i_out = r_out + n + 1;
+  const uint32_t* r_in = reinterpret_cast<const uint32_t*>(a.ranges + (size_t)i * a.stride);
+  const uint32_t* i_in = reinterpret_cast<const uint32_t*>(a.intensities + (size_t)i * a.stride);
+  for (uint32_t j = blockIdx.x * CT + threadIdx.x; j < n; j += gridDim.x * CT) {
+    r_out[j] = __ldg(r_in + j);
+    i_out[j] = __ldg(i_in + j);
+  }
+}
+
+__global__ void __launch_bounds__(CT) pointcloud2_msgs_kernel(MsgWriteArgs a, CloudTail t) {
+  const uint32_t i = a.slot0 + blockIdx.y;
+  const uint32_t size = a.sizes[i];
+  if (size == 0) return;
+  const uint32_t n = a.counts[i];
+  const StreamMsgHeader& h = a.hdr[i / a.max_scans];
+  const uint32_t P = h.bytes + t.bytes;  // ends with the data length
+  uint8_t* msg = a.out + (a.offsets[i] - a.out_base);
+  if (blockIdx.x == 0) {
+    put_header(msg, h);
+    for (uint32_t w = threadIdx.x; w < t.bytes / 4; w += CT) {
+      const uint32_t v = w == t.at_width ? n : (w == t.at_row_step || w == t.at_data) ? 16u * n : t.w[w];
+      put32(msg + h.bytes + 4 * w, v);
+    }
+    if (threadIdx.x == 0) {
+      uint32_t sec, nsec;
+      msg_stamp(a.begin_us ? a.begin_us[i] : 0ull, a.clock_offset_ns, &sec, &nsec);
+      put32(msg + 4, sec);
+      put32(msg + 8, nsec);
+      msg[P + 16 * (size_t)n] = 1;  // is_dense: the cloud path drops unmeasured points
+    }
+  }
+  const uint4* d_in = reinterpret_cast<const uint4*>(a.xyzi + (size_t)i * a.stride * 4);
+  if ((P & 15u) == 0) {  // the message starts 16-aligned: the data is 16-aligned iff P is
+    uint4* d_out = reinterpret_cast<uint4*>(msg + P);
+    for (uint32_t j = blockIdx.x * CT + threadIdx.x; j < n; j += gridDim.x * CT) d_out[j] = __ldg(d_in + j);
+  } else {
+    uint32_t* o = reinterpret_cast<uint32_t*>(msg + P);
+    const uint32_t* in = reinterpret_cast<const uint32_t*>(d_in);
+    for (uint32_t j = blockIdx.x * CT + threadIdx.x; j < 4 * n; j += gridDim.x * CT) o[j] = __ldg(in + j);
+  }
+}
+
 }  // namespace
+
+cudaError_t launch_msg_table(const MsgTableArgs& a, cudaStream_t stream) {
+  if (a.n_slots == 0) return cudaSuccess;
+  msg_table_kernel<<<1, MT, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_laserscan_msgs(const MsgWriteArgs& a, uint32_t max_beams, cudaStream_t stream) {
+  const uint32_t bx = std::max(1u, std::min((max_beams + CT * 4 - 1) / (CT * 4), 32u));
+  for (uint32_t k = 0; k < a.n; k += 65535) {
+    MsgWriteArgs b = a;
+    b.slot0 = a.slot0 + k;
+    laserscan_msgs_kernel<<<dim3(bx, std::min(65535u, a.n - k)), CT, 0, stream>>>(b);
+  }
+  return cudaGetLastError();
+}
+
+cudaError_t launch_pointcloud2_msgs(const MsgWriteArgs& a, const CloudTail& t, uint32_t max_points,
+                                    cudaStream_t stream) {
+  const uint32_t bx = std::max(1u, std::min((max_points + CT * 4 - 1) / (CT * 4), 32u));
+  for (uint32_t k = 0; k < a.n; k += 65535) {
+    MsgWriteArgs b = a;
+    b.slot0 = a.slot0 + k;
+    pointcloud2_msgs_kernel<<<dim3(bx, std::min(65535u, a.n - k)), CT, 0, stream>>>(b, t);
+  }
+  return cudaGetLastError();
+}
 
 cudaError_t launch_laserscan_cdr(const LaserScanCdrArgs& a, const CdrTemplate& t, cudaStream_t stream) {
   if (a.n_scans == 0) return cudaSuccess;

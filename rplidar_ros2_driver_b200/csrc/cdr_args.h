@@ -46,4 +46,57 @@ struct PointCloudCdrArgs {
 cudaError_t launch_laserscan_cdr(const LaserScanCdrArgs& a, const CdrTemplate& t, cudaStream_t stream);
 cudaError_t launch_pointcloud2_cdr(const PointCloudCdrArgs& a, const CdrTemplate& t, cudaStream_t stream);
 
+// ---- packed messages of a stream session's last push (rpl_*_stream_{laserscan,cloud}_msgs*) ----------------------
+// One stream's message settings, built on the host by rpl_*_stream_set_frames: the bytes every message of the stream
+// starts with -- encapsulation header, stamp (zero here, patched per message), frame_id string padded to 4.
+constexpr uint32_t kMsgHeaderWords = 70;  // 4 + 8 + 4 + 256 (frame_id <= 255 characters + NUL) bytes, rounded up
+struct StreamMsgHeader {
+  uint32_t bytes;                  // multiple of 4
+  float range_max;                 // LaserScan range_max
+  uint32_t w[kMsgHeaderWords];
+};
+
+// The PointCloud2 members between the header and the data (height .. data length): identical bytes for every frame
+// id, since the header ends 4-aligned and nothing behind it is aligned to more than 4
+struct CloudTail {
+  uint32_t w[29];
+  uint32_t bytes;                          // 116
+  uint32_t at_width, at_row_step, at_data;  // word indices patched per message
+};
+
+enum class MsgKind : uint32_t { kLaserScan, kPointCloud2 };
+
+// sizes and offsets pass: one CTA over every slot
+struct MsgTableArgs {
+  MsgKind kind;
+  const StreamMsgHeader* hdr;      // [n_slots / max_scans]
+  const uint32_t* counts;          // [n_slots] beams / points
+  const uint2* views;              // [n_slots] PointCloud2: a slot has a message iff its view count is > 0
+  uint32_t n_slots, max_scans;
+  unsigned long long capacity;
+  unsigned long long* offsets;     // [n_slots] out: exclusive scan of the sizes rounded up to 16
+  uint32_t* sizes;                 // [n_slots] out: message bytes, 0 for no message or when the total exceeds capacity
+  unsigned long long* total;       // out: end of the last message
+};
+
+// the writers, over slots [slot0, slot0 + n) (slot indices count from the first slot of the call)
+struct MsgWriteArgs {
+  const StreamMsgHeader* hdr;
+  const unsigned long long *begin_us, *end_us;  // [n_slots] nullable together: an unstamped push (stamps 0)
+  long long clock_offset_ns;
+  const uint32_t* counts;          // [n_slots]
+  const float *ranges, *intensities, *angle_increment;  // LaserScan: [n_slots][stride], [n_slots]
+  const float* xyzi;               // PointCloud2: [n_slots][stride][4]
+  uint32_t stride, max_scans, mode_a;
+  uint32_t slot0, n;
+  const unsigned long long* offsets;
+  const uint32_t* sizes;
+  uint8_t* out;                    // message i at out + offsets[i] - out_base
+  unsigned long long out_base;
+};
+
+cudaError_t launch_msg_table(const MsgTableArgs& a, cudaStream_t stream);
+cudaError_t launch_laserscan_msgs(const MsgWriteArgs& a, uint32_t max_beams, cudaStream_t stream);
+cudaError_t launch_pointcloud2_msgs(const MsgWriteArgs& a, const CloudTail& t, uint32_t max_points, cudaStream_t stream);
+
 }  // namespace rpl

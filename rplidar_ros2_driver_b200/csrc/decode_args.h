@@ -139,6 +139,10 @@ struct AssembleStampArgs {
   unsigned long long* held_rx;              // [n_streams]
   // 0: the previous push had no receive times, so open_ts_in and held_rx are stale and count as unknown
   uint32_t prev_stamped;
+  // the session's own copy of every slot's scan-begin stamp, and its end stamp: the stamp of the scan-start node that
+  // closed the scan, which opens the next scan whether that one is published, dropped past max_scans or reset
+  unsigned long long* slot_begin_us;        // [n_streams][AssembleArgs::max_scans], unused slots 0
+  unsigned long long* slot_end_us;          // [n_streams][AssembleArgs::max_scans], unused slots 0
 };
 
 // byte-level framing with the SDK's resynchronisation (frame.cu)

@@ -1210,6 +1210,13 @@ struct rpl_capsule_stream {
   // the last push, as the cloud calls replay it: its views count from the first stream of their chunk
   uint32_t cloud_chunk = 0;                     // streams per chunk (chunk_host or chunk_dev); 0: no push, or it failed
   uint32_t cloud_arena = 0;                     // the arena its views point into
+  // the messages of the last push (rpl_*_stream_*_msgs*): a stamped push's slot stamps, the per-stream settings
+  unsigned long long* slot_begin = nullptr;     // [n_streams * max_scans] scan-begin stamps (0: unused, unknown)
+  unsigned long long* slot_end = nullptr;       // [n_streams * max_scans] the closing scan-start node's stamp
+  rpl::StreamMsgHeader* msg_hdr = nullptr;      // [n_streams] device
+  std::vector<rpl::StreamMsgHeader> msg_hdr_host;
+  unsigned char* msg_work = nullptr;            // the scan kernels' outputs and the tables of a messages call
+  size_t msg_work_bytes = 0;
 };
 
 namespace {
@@ -1243,6 +1250,7 @@ struct WireChunk {
   // a stamped session push's: 0x81 scan-start record ends, the open revolution's stamp, the held capsule's rx
   uint32_t* node_end;
   unsigned long long *open_ts_in, *open_ts_out, *held_rx;
+  unsigned long long *slot_begin, *slot_end;
   bool prev_stamped;
   // a byte session's: the input is raw bytes [.][stride_bytes], framed into `framed` first
   uint32_t stride_bytes;
@@ -1279,6 +1287,8 @@ WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0) {
   w.open_ts_in = cs->open_ts[p] + s0;
   w.open_ts_out = cs->open_ts[p ^ 1u] + s0;
   w.held_rx = cs->held_rx + s0;
+  w.slot_begin = cs->slot_begin + so;
+  w.slot_end = cs->slot_end + so;
   w.prev_stamped = cs->prev_stamped;
   if (cs->framer) {
     w.stride_bytes = cs->stride_bytes;
@@ -1378,6 +1388,8 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
     t.open_ts_out = w.open_ts_out;
     t.held_rx = w.held_rx;
     t.prev_stamped = w.prev_stamped ? 1u : 0u;
+    t.slot_begin_us = w.slot_begin;
+    t.slot_end_us = w.slot_end;
   }
   r = assemble_common(c, w.nodes, w.node_counts, ns, w.stride_nodes, w.status, w.offsets, w.status ? counts : nullptr,
                       w.status ? sc : 0u, w.max_nodes, w.max_scans, w.max_nodes, nullptr, w.views, w.scan_len,
@@ -1483,6 +1495,20 @@ bool capsule_stream_args_ok(rpl_capsule_stream* cs, const uint8_t* capsules, con
   return true;
 }
 
+// a stream's message settings: XCDR1 encapsulation {0x00, 0x01, 0x00, 0x00}, a zero stamp, frame_id as a string
+// (uint32 length with the NUL, the bytes, the NUL), zero padding to 4
+rpl::StreamMsgHeader msg_header(const char* frame_id, size_t len, float range_max) {
+  rpl::StreamMsgHeader h{};
+  uint8_t* b = reinterpret_cast<uint8_t*>(h.w);
+  b[1] = 0x01;
+  const uint32_t n = (uint32_t)len + 1;
+  std::memcpy(b + 12, &n, 4);
+  std::memcpy(b + 16, frame_id, len);
+  h.bytes = 4 + ((12 + (uint32_t)len + 1 + 3) & ~3u);
+  h.range_max = range_max;
+  return h;
+}
+
 // a session of a capsule answer type or of 0x81 standard nodes (the caller has checked ans_type); stride_capsules
 // counts bytes for 0x81.  stride_bytes != 0: a byte session of a capsule answer type (stride_capsules is ignored)
 rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint32_t stride_capsules,
@@ -1568,6 +1594,14 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint
       !cuda_ok(c, dev_alloc(&cs->node_counts, n), "cudaMalloc") ||
       !cuda_ok(c, dev_alloc(&cs->scan_len, n * max_scans), "cudaMalloc") ||
       !cuda_ok(c, dev_alloc(&cs->views, n * max_scans), "cudaMalloc") ||
+      !cuda_ok(c, dev_alloc(&cs->slot_begin, n * max_scans), "cudaMalloc") ||
+      !cuda_ok(c, dev_alloc(&cs->slot_end, n * max_scans), "cudaMalloc") ||
+      !cuda_ok(c, dev_alloc(&cs->msg_hdr, n), "cudaMalloc"))
+    return fail(oom);
+  // the reference's defaults: frame_id "laser_frame" (rplidar_node.cpp:80), range_max 12 m (rplidar_node.hpp:328)
+  cs->msg_hdr_host.assign(n, msg_header("laser_frame", 11, 12.0f));
+  if (!cuda_ok(c, cudaMemcpy(cs->msg_hdr, cs->msg_hdr_host.data(), n * sizeof(rpl::StreamMsgHeader),
+                             cudaMemcpyHostToDevice), "cudaMemcpy") ||
       !cuda_ok(c, cudaEventCreateWithFlags(&cs->done, cudaEventDisableTiming), "cudaEventCreate") ||
       !cuda_ok(c, cudaDeviceSynchronize(), "cudaDeviceSynchronize"))  // the zeroed state is in place before any push
     return fail(oom);
@@ -1814,6 +1848,280 @@ rpl_result stream_cloud(rpl_capsule_stream* cs, const rpl_cloud_params* params, 
   return run_chunks(c, cs->n_streams, chunk, run_chunk);
 }
 
+// ---- packed LaserScan / PointCloud2 messages of the last push (DESIGN.md 5.9) -------------------------------------
+// Per call: the scan kernels (LaserScan) or the session cloud chain (PointCloud2) over the last push's views into the
+// session's work block, the sizes and offsets pass over every slot, then the writers.  The device form writes every
+// message into the caller's buffer; the host form reads the tables back first and then writes and copies the
+// messages chunk by chunk over the lanes, so that only message bytes cross the link.
+
+rpl_result stream_set_frames(rpl_capsule_stream* cs, const char* const* frame_ids, const float* range_max) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!frame_ids) {
+    c->err = "null frame_ids";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  std::vector<rpl::StreamMsgHeader> h(cs->n_streams);
+  for (uint32_t s = 0; s < cs->n_streams; ++s) {
+    if (!frame_ids[s]) {
+      c->err = "null frame_ids[s]";
+      return RPL_RESULT_INVALID_DATA;
+    }
+    const size_t L = std::strlen(frame_ids[s]);
+    if (!frame_id_length_ok(c, L)) return RPL_RESULT_INVALID_DATA;
+    h[s] = msg_header(frame_ids[s], L, range_max ? range_max[s] : cs->msg_hdr_host[s].range_max);
+  }
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);  // a messages call may still read them
+  RPL_CUDA(c, cudaMemcpy(cs->msg_hdr, h.data(), h.size() * sizeof(rpl::StreamMsgHeader), cudaMemcpyHostToDevice),
+           RPL_RESULT_OPERATION_FAIL);
+  cs->msg_hdr_host = std::move(h);
+  return RPL_RESULT_OK;
+}
+
+// the PointCloud2 members between the header and the data: height 1, width, the fields x, y, z, intensity (float32,
+// count 1), is_bigendian 0, point_step 16, row_step, data length
+rpl::CloudTail cloud_tail() {
+  rpl::CloudTail t{};
+  uint8_t* b = reinterpret_cast<uint8_t*>(t.w);
+  uint32_t n = 0;
+  auto u32 = [&](uint32_t v) {
+    n = (n + 3) & ~3u;
+    std::memcpy(b + n, &v, 4);
+    n += 4;
+  };
+  u32(1);
+  t.at_width = n / 4;
+  u32(0);
+  u32(4);
+  const char* names[4] = {"x", "y", "z", "intensity"};
+  for (uint32_t f = 0; f < 4; ++f) {
+    const uint32_t L = (uint32_t)std::strlen(names[f]);
+    u32(L + 1);
+    std::memcpy(b + n, names[f], L + 1);
+    n += L + 1;
+    u32(4 * f);
+    b[n++] = 7;  // FLOAT32
+    u32(1);
+  }
+  b[n++] = 0;  // is_bigendian
+  u32(16);     // point_step
+  t.at_row_step = (n + 3) / 4;
+  u32(0);
+  t.at_data = n / 4;
+  u32(0);
+  t.bytes = n;
+  return t;
+}
+
+// the work block of a messages call: scan outputs of every slot (LaserScan ranges then intensities, or xyzi), their
+// counts and angle increments; the host form's tables behind them
+struct MsgWork {
+  float* data;
+  uint32_t* counts;
+  float* inc;
+  unsigned long long* offsets;
+  uint32_t* sizes;
+  unsigned long long* total;
+};
+MsgWork msg_work_layout(const rpl_capsule_stream* cs, rpl::MsgKind kind, bool tables, Carve& k) {
+  const size_t NS = (size_t)cs->n_streams * cs->max_scans;
+  const size_t floats = NS * cs->max_nodes * (kind == rpl::MsgKind::kLaserScan ? 2 : 4);
+  return MsgWork{k.take<float>(floats), k.take<uint32_t>(NS), k.take<float>(NS),
+                 k.take<unsigned long long>(tables ? NS : 0), k.take<uint32_t>(tables ? NS : 0),
+                 k.take<unsigned long long>(tables ? 1 : 0)};
+}
+
+bool stream_msgs_args_ok(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* params, const void* msgs,
+                         const void* offsets, const void* sizes, const void* total, bool dev) {
+  rpl_ctx* c = cs->c;
+  if (!params || !msgs || !offsets || !sizes || !total) {
+    c->err = "null params, msgs, msg_offsets, msg_sizes or total_bytes";
+    return false;
+  }
+  if (kind == rpl::MsgKind::kPointCloud2 && !cloud_params_ok(c, static_cast<const rpl_cloud_params*>(params)))
+    return false;
+  if (dev && ((reinterpret_cast<uintptr_t>(msgs) & 15u) || misaligned8(offsets) || misaligned8(total) ||
+              (reinterpret_cast<uintptr_t>(sizes) & 3u))) {
+    c->err = "msgs must be 16-byte aligned, msg_offsets and total_bytes 8-byte, msg_sizes 4-byte aligned";
+    return false;
+  }
+  if (cs->cloud_chunk == 0) {
+    c->err = "no messages to take: the session has not pushed yet, or its last push failed";
+    return false;
+  }
+  return true;
+}
+
+// grows the session's work block (an earlier messages call, on any stream, may still read it)
+rpl_result grow_msg_work(rpl_capsule_stream* cs, size_t bytes) {
+  rpl_ctx* c = cs->c;
+  if (cs->msg_work_bytes >= bytes) return RPL_RESULT_OK;
+  RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);
+  cudaFree(cs->msg_work);
+  cs->msg_work = nullptr;
+  cs->msg_work_bytes = 0;
+  RPL_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&cs->msg_work), bytes), RPL_RESULT_INSUFFICIENT_MEMORY);
+  cs->msg_work_bytes = bytes;
+  return RPL_RESULT_OK;
+}
+
+// on `st`, after the last push: the scan kernels or the cloud chain of every slot into w, then the tables
+rpl_result msgs_prepare(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* params, const MsgWork& w,
+                        unsigned long long capacity, unsigned long long* offsets, uint32_t* sizes,
+                        unsigned long long* total, cudaStream_t st) {
+  rpl_ctx* c = cs->c;
+  const size_t NS = (size_t)cs->n_streams * cs->max_scans, row = cs->max_nodes;
+  rpl_result r = RPL_RESULT_OK;
+  for (uint32_t s0 = 0; s0 < cs->n_streams && r == RPL_RESULT_OK; s0 += cs->cloud_chunk) {
+    const uint32_t ns = std::min(cs->cloud_chunk, cs->n_streams - s0);
+    const size_t so = (size_t)s0 * cs->max_scans;
+    if (kind == rpl::MsgKind::kLaserScan)
+      r = enqueue_scan(c, c->lane[0], cs->arena[cs->cloud_arena] + (size_t)s0 * cs->stride_nodes, cs->scan_len + so,
+                       ns * cs->max_scans, cs->max_nodes, static_cast<const rpl_scan_params*>(params), nullptr,
+                       w.data + so * row, w.data + (NS + so) * row, w.counts + so, w.inc + so, nullptr, nullptr, st,
+                       reinterpret_cast<const uint2*>(cs->views + so), (unsigned long long)ns * cs->stride_nodes);
+    else
+      r = stream_cloud_chunk(cs, c->lane[0], s0, ns, static_cast<const rpl_cloud_params*>(params),
+                             w.data + so * row * 4, w.counts + so, st);
+  }
+  if (r != RPL_RESULT_OK) return r;
+  rpl::MsgTableArgs t{};
+  t.kind = kind;
+  t.hdr = cs->msg_hdr;
+  t.counts = w.counts;
+  t.views = reinterpret_cast<const uint2*>(cs->views);
+  t.n_slots = (uint32_t)NS;
+  t.max_scans = cs->max_scans;
+  t.capacity = capacity;
+  t.offsets = offsets;
+  t.sizes = sizes;
+  t.total = total;
+  RPL_CUDA(c, rpl::launch_msg_table(t, st), RPL_RESULT_OPERATION_FAIL);
+  c->launches++;
+  return RPL_RESULT_OK;
+}
+
+// the writers over slots [slot0, slot0 + n), message i at out + offsets[i] - out_base
+rpl_result msgs_write(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* params, long long clock_offset_ns,
+                      const MsgWork& w, const unsigned long long* offsets, const uint32_t* sizes, uint32_t slot0,
+                      uint32_t n, uint8_t* out, unsigned long long out_base, cudaStream_t st) {
+  rpl_ctx* c = cs->c;
+  if (n == 0) return RPL_RESULT_OK;
+  const size_t NS = (size_t)cs->n_streams * cs->max_scans;
+  rpl::MsgWriteArgs a{};
+  a.hdr = cs->msg_hdr;
+  if (cs->prev_stamped) {  // the stamps of the last push (an unstamped one kept none)
+    a.begin_us = cs->slot_begin;
+    a.end_us = cs->slot_end;
+  }
+  a.clock_offset_ns = clock_offset_ns;
+  a.counts = w.counts;
+  a.stride = cs->max_nodes;
+  a.max_scans = cs->max_scans;
+  a.slot0 = slot0;
+  a.n = n;
+  a.offsets = offsets;
+  a.sizes = sizes;
+  a.out = out;
+  a.out_base = out_base;
+  if (kind == rpl::MsgKind::kLaserScan) {
+    a.ranges = w.data;
+    a.intensities = w.data + NS * cs->max_nodes;
+    a.angle_increment = w.inc;
+    a.mode_a = static_cast<const rpl_scan_params*>(params)->scan_processing ? 1u : 0u;
+    RPL_CUDA(c, rpl::launch_laserscan_msgs(a, cs->max_nodes, st), RPL_RESULT_OPERATION_FAIL);
+  } else {
+    a.xyzi = w.data;
+    static const rpl::CloudTail tail = cloud_tail();
+    RPL_CUDA(c, rpl::launch_pointcloud2_msgs(a, tail, cs->max_nodes, st), RPL_RESULT_OPERATION_FAIL);
+  }
+  c->launches += (n + 65534) / 65535;
+  return RPL_RESULT_OK;
+}
+
+rpl_result stream_msgs_dev(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* params, int64_t clock_offset_ns,
+                           uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
+                           uint64_t* total_bytes, void* stream) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!stream_msgs_args_ok(cs, kind, params, msgs, msg_offsets, msg_sizes, total_bytes, true))
+    return RPL_RESULT_INVALID_DATA;
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
+  Carve k;
+  msg_work_layout(cs, kind, false, k);
+  if (const rpl_result r = grow_msg_work(cs, k.bytes); r != RPL_RESULT_OK) return r;
+  Carve kw{cs->msg_work};
+  const MsgWork w = msg_work_layout(cs, kind, false, kw);
+  auto* offs = reinterpret_cast<unsigned long long*>(msg_offsets);
+  // the last push's kernels are done before these read its arena and views; the next push waits for these
+  RPL_CUDA(c, cudaStreamWaitEvent(st, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
+  rpl_result r = msgs_prepare(cs, kind, params, w, capacity, offs, msg_sizes,
+                              reinterpret_cast<unsigned long long*>(total_bytes), st);
+  if (r == RPL_RESULT_OK)
+    r = msgs_write(cs, kind, params, clock_offset_ns, w, offs, msg_sizes, 0, cs->n_streams * cs->max_scans, msgs, 0, st);
+  RPL_CUDA(c, cudaEventRecord(cs->done, st), RPL_RESULT_OPERATION_FAIL);
+  return r;
+}
+
+rpl_result stream_msgs(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* params, int64_t clock_offset_ns,
+                       uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
+                       uint64_t* total_bytes) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!stream_msgs_args_ok(cs, kind, params, msgs, msg_offsets, msg_sizes, total_bytes, false))
+    return RPL_RESULT_INVALID_DATA;
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  Carve k;
+  msg_work_layout(cs, kind, true, k);
+  if (const rpl_result r = grow_msg_work(cs, k.bytes); r != RPL_RESULT_OK) return r;
+  Carve kw{cs->msg_work};
+  const MsgWork w = msg_work_layout(cs, kind, true, kw);
+  const uint32_t NS = cs->n_streams * cs->max_scans;
+  cudaStream_t st = c->lane[0].stream;
+  for (int i = 0; i < kLanes; ++i) RPL_CUDA(c, cudaStreamWaitEvent(c->lane[i].stream, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
+  rpl_result r = msgs_prepare(cs, kind, params, w, capacity, w.offsets, w.sizes, w.total, st);
+  if (r != RPL_RESULT_OK) {
+    cudaStreamSynchronize(st);
+    return r;
+  }
+  const cudaMemcpyKind d2h = cudaMemcpyDeviceToHost;
+  RPL_CUDA(c, cudaMemcpyAsync(msg_offsets, w.offsets, (size_t)NS * 8, d2h, st), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaMemcpyAsync(msg_sizes, w.sizes, (size_t)NS * 4, d2h, st), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaMemcpyAsync(total_bytes, w.total, 8, d2h, st), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);
+  const uint64_t total = *total_bytes;
+  if (total > capacity) {
+    c->err = "the messages need more than capacity bytes (total_bytes tells how many)";
+    return RPL_RESULT_INSUFFICIENT_MEMORY;
+  }
+  // the chunks of the last push: each one's messages are one stretch [lo, hi) of the packed buffer
+  const uint32_t chunk = cs->cloud_chunk;
+  auto stretch = [&](uint32_t s0, uint32_t ns) {
+    const uint32_t i0 = s0 * cs->max_scans, i1 = (s0 + ns) * cs->max_scans;
+    const uint64_t hi = i1 < NS ? std::min<uint64_t>(msg_offsets[i1], total) : total;
+    return std::make_pair(std::min<uint64_t>(msg_offsets[i0], hi), hi);
+  };
+  size_t most = 0;
+  for (uint32_t s0 = 0; s0 < cs->n_streams; s0 += chunk) {
+    const auto [lo, hi] = stretch(s0, std::min(chunk, cs->n_streams - s0));
+    most = std::max<size_t>(most, hi - lo);
+  }
+  if (const rpl_result g = grow_stage(c, kLanes, [&](Carve& k) { k.take<uint8_t>(most); }); g != RPL_RESULT_OK) return g;
+  auto run_chunk = [&](Lane& l, uint32_t s0, uint32_t ns) -> rpl_result {
+    const auto [lo, hi] = stretch(s0, ns);
+    if (hi == lo) return RPL_RESULT_OK;
+    RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);  // the lane's previous chunk has left
+    const rpl_result wr = msgs_write(cs, kind, params, clock_offset_ns, w, w.offsets, w.sizes, s0 * cs->max_scans,
+                                     ns * cs->max_scans, l.stage, lo, l.stream);
+    if (wr != RPL_RESULT_OK) return wr;
+    RPL_CUDA(c, cudaMemcpyAsync(msgs + lo, l.stage, hi - lo, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
+    return RPL_RESULT_OK;
+  };
+  return run_chunks(c, cs->n_streams, chunk, run_chunk);
+}
+
 }  // namespace
 
 extern "C" {
@@ -1911,6 +2219,10 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   cudaFree(cs->framed);
   cudaFree(cs->framed_counts);
   cudaFree(cs->framed_rx);
+  cudaFree(cs->slot_begin);
+  cudaFree(cs->slot_end);
+  cudaFree(cs->msg_hdr);
+  cudaFree(cs->msg_work);
   if (cs->done) cudaEventDestroy(cs->done);
   delete cs;
 }
@@ -2214,6 +2526,40 @@ rpl_result rpl_normal_stream_cloud(rpl_normal_stream* ns, const rpl_cloud_params
                                    uint32_t* point_counts) {
   return stream_cloud(capsule_session(ns), params, xyzi, point_counts);
 }
+
+// ---- packed messages of the last push, one set per session handle type -------------------------------------------
+#define RPL_STREAM_MSGS(KIND, T, SESSION)                                                                              \
+  rpl_result rpl_##KIND##_stream_set_frames(T* s, const char* const* frame_ids, const float* range_max) {             \
+    return stream_set_frames(SESSION, frame_ids, range_max);                                                         \
+  }                                                                                                                  \
+  rpl_result rpl_##KIND##_stream_laserscan_msgs_dev(T* s, const rpl_scan_params* params, int64_t clock_offset_ns,    \
+                                                    uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,         \
+                                                    uint32_t* msg_sizes, uint64_t* total_bytes, void* stream) {      \
+    return stream_msgs_dev(SESSION, rpl::MsgKind::kLaserScan, params, clock_offset_ns, msgs, capacity, msg_offsets,  \
+                           msg_sizes, total_bytes, stream);                                                          \
+  }                                                                                                                  \
+  rpl_result rpl_##KIND##_stream_laserscan_msgs(T* s, const rpl_scan_params* params, int64_t clock_offset_ns,        \
+                                                uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,             \
+                                                uint32_t* msg_sizes, uint64_t* total_bytes) {                        \
+    return stream_msgs(SESSION, rpl::MsgKind::kLaserScan, params, clock_offset_ns, msgs, capacity, msg_offsets,      \
+                       msg_sizes, total_bytes);                                                                      \
+  }                                                                                                                  \
+  rpl_result rpl_##KIND##_stream_cloud_msgs_dev(T* s, const rpl_cloud_params* params, int64_t clock_offset_ns,       \
+                                                uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,             \
+                                                uint32_t* msg_sizes, uint64_t* total_bytes, void* stream) {          \
+    return stream_msgs_dev(SESSION, rpl::MsgKind::kPointCloud2, params, clock_offset_ns, msgs, capacity,             \
+                           msg_offsets, msg_sizes, total_bytes, stream);                                             \
+  }                                                                                                                  \
+  rpl_result rpl_##KIND##_stream_cloud_msgs(T* s, const rpl_cloud_params* params, int64_t clock_offset_ns,           \
+                                            uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,                 \
+                                            uint32_t* msg_sizes, uint64_t* total_bytes) {                            \
+    return stream_msgs(SESSION, rpl::MsgKind::kPointCloud2, params, clock_offset_ns, msgs, capacity, msg_offsets,    \
+                       msg_sizes, total_bytes);                                                                      \
+  }
+RPL_STREAM_MSGS(capsule, rpl_capsule_stream, s)
+RPL_STREAM_MSGS(dense, rpl_dense_stream, capsule_session(s))
+RPL_STREAM_MSGS(normal, rpl_normal_stream, capsule_session(s))
+#undef RPL_STREAM_MSGS
 
 // ---- LaserScan / PointCloud2 -> CDR (SURVEY.md 8(f) rank 3) -------------------------------------
 namespace {

@@ -27,8 +27,9 @@ def kernels(path):
     for line in txt.splitlines():
         m = re.match(r"\s*Function : (\S+)", line)
         if m:
-            # internal-linkage names carry a hash of the file's contents: _GLOBAL__N__<hash>_<file>
-            name = re.sub(r"_GLOBAL__N__[0-9a-f]+_", "_GLOBAL__N__", m.group(1))
+            # internal-linkage names carry two hashes, of the build and of the file's contents:
+            # _GLOBAL__N__<hash>_<len>_<file>_cu_<hash>
+            name = re.sub(r"_GLOBAL__N__[0-9a-f]+_(\d+_\w+?_cu)_[0-9a-f]{8}", r"_GLOBAL__N__\1", m.group(1))
             out[name] = []
             continue
         m = re.match(r"\s*/\*[0-9a-f]{4,}\*/\s*(.*?)\s*;", line)

@@ -108,6 +108,8 @@ typedef struct rpl_scan_params {
                                      TMA-ring kernel (scan_tma.cu) applies; for A/B measurements */
 #define RPL_FLAG_NO_SMALL 4u      /* do not use the shared-memory-resident kernels (scan_small.cu) for
                                      revolutions of at most 8192 nodes; for A/B measurements */
+#define RPL_FLAG_PER_STREAM 8u    /* stream sessions: every stream's own rpl_lidar_settings (rpl_*_stream_set_lidars)
+                                     instead of this struct's settings and the push's timing; other calls ignore it */
 
 /* per-scan path report (optional output) */
 #define RPL_PATH_FAST 0u    /* tie-free scan: bitmap-rank kernel */
@@ -126,6 +128,8 @@ typedef struct rpl_cloud_params {
 } rpl_cloud_params;
 #define RPL_CLOUD_NO_FUSED 1u /* run SOR / voxel grid as separate passes even where the shared-memory kernel
                                  could fuse them (A/B measurements, second implementation for the tests) */
+#define RPL_CLOUD_PER_STREAM 2u /* stream sessions: every stream's own is_new_protocol (rpl_*_stream_set_lidars) for
+                                   the intensity and the intensity_min window; other calls ignore it */
 
 typedef struct rpl_ctx rpl_ctx;
 
@@ -753,6 +757,41 @@ rpl_result rpl_normal_stream_cloud_msgs_dev(rpl_normal_stream* s, const rpl_clou
 rpl_result rpl_normal_stream_cloud_msgs(rpl_normal_stream* s, const rpl_cloud_params* params, int64_t clock_offset_ns,
                                         uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
                                         uint64_t* total_bytes);
+
+/* Per-stream lidar settings: each stream of a session is one lidar, the reference's one RPlidarNode, with its own
+ * intensity protocol (RealLidarDriver::is_new_type(), src/lidar_driver_wrapper.cpp:303-305), scan_processing and
+ * inverted parameters (src/rplidar_node.cpp:270, 278-279) and SlamtecLidarTimingDesc (which depends on the model, the
+ * scan mode and the link).  One session then serves a fleet that mixes them.
+ *   set_lidars: synchronous (it waits for the session's device calls in flight that may read the table).  Copies
+ *            settings[s] for every stream whose stream_mask entry is non-zero (NULL = all); the first call must set
+ *            every stream.  A null settings, a first call that leaves a stream out, or a masked entry whose
+ *            sample_duration_us is outside [1, 1000000] (the decoders' jump threshold divides by it):
+ *            RPL_RESULT_INVALID_DATA, and the table is unchanged.
+ *   RPL_FLAG_PER_STREAM in rpl_scan_params.flags (every push flavour: framed or byte, host or device, stamped or not;
+ *            laserscan_msgs[_dev]): stream s is decoded, stamped and converted with settings[s] -- is_new_protocol,
+ *            scan_processing, inverted, and timing for the decoder's discard threshold and the scan-begin stamps.  The
+ *            call's own is_new_protocol, scan_processing, inverted, sample_duration_us and timing are ignored; timing
+ *            may be NULL on a stamped push.  Each stream's outputs are bit for bit those of a session of that stream
+ *            alone pushed with uniform params and timing equal to its settings.  Before the first set_lidars:
+ *            RPL_RESULT_INVALID_DATA.
+ *   RPL_CLOUD_PER_STREAM in rpl_cloud_params.flags (cloud[_dev], cloud_msgs[_dev]): stream s takes
+ *            settings[s].is_new_protocol; before the first set_lidars: RPL_RESULT_INVALID_DATA.
+ *   Changes between pushes apply to everything the next push decodes and publishes; a scan-begin stamp a push already
+ *   computed (of a revolution still open) keeps its value.  Cloud and message calls read the table as it is when they
+ *   are made.  apply_ascend stays a call parameter: it moves only unmeasured nodes, which no session output keeps. */
+typedef struct rpl_lidar_settings {
+  uint8_t is_new_protocol; /* as rpl_scan_params */
+  uint8_t scan_processing; /* 1 Mode A, 0 Mode B */
+  uint8_t inverted;
+  uint8_t pad;
+  rpl_timing timing;       /* sample_duration_us must be in [1, 1000000] */
+} rpl_lidar_settings;
+rpl_result rpl_capsule_stream_set_lidars(rpl_capsule_stream* s, const rpl_lidar_settings* settings /* [n_streams] */,
+                                         const uint8_t* stream_mask /* nullable: all */);
+rpl_result rpl_dense_stream_set_lidars(rpl_dense_stream* s, const rpl_lidar_settings* settings,
+                                       const uint8_t* stream_mask);
+rpl_result rpl_normal_stream_set_lidars(rpl_normal_stream* s, const rpl_lidar_settings* settings,
+                                        const uint8_t* stream_mask);
 
 /* ---- LaserScan / PointCloud2 -> wire (SURVEY.md 8(f) rank 3) ---------------------------- */
 /* The serialised message the RMW layer would produce from the message the reference publishes

@@ -25,7 +25,9 @@ RESULT_INSUFFICIENT_MEMORY = 0x80008006
 FLAG_FORCE_GENERAL = 1
 FLAG_NO_TMA = 2
 FLAG_NO_SMALL = 4
+FLAG_PER_STREAM = 8
 CLOUD_NO_FUSED = 1
+CLOUD_PER_STREAM = 2
 CAPSULE_OK, CAPSULE_SYNC, CAPSULE_EMIT, CAPSULE_DISCARD = 1, 2, 4, 8
 CAPSULE_CHECKSUM_ERR, CAPSULE_ENCODER_RESET_ERR, CAPSULE_BAD_FRAME = 16, 32, 64
 PATH_FAST, PATH_GENERAL = 0, 1
@@ -60,7 +62,7 @@ EXPORTS = [
     "rpl_capsule_stream_cloud", "rpl_capsule_stream_cloud_dev", "rpl_dense_stream_cloud", "rpl_dense_stream_cloud_dev",
     "rpl_normal_stream_cloud", "rpl_normal_stream_cloud_dev",
     *[f"rpl_{kind}_stream_{fn}" for kind in ("capsule", "dense", "normal")
-      for fn in ("set_frames", "laserscan_msgs", "laserscan_msgs_dev", "cloud_msgs", "cloud_msgs_dev")],
+      for fn in ("set_frames", "set_lidars", "laserscan_msgs", "laserscan_msgs_dev", "cloud_msgs", "cloud_msgs_dev")],
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -87,6 +89,12 @@ class Timing(C.Structure):
     """rpl_timing == sl::SlamtecLidarTimingDesc without the bool."""
     _fields_ = [("sample_duration_us", C.c_uint32), ("native_baudrate", C.c_uint32),
                 ("linkage_delay_us", C.c_uint32), ("native_interface_type", C.c_uint32)]
+
+
+class LidarSettings(C.Structure):
+    """rpl_lidar_settings: one stream's lidar (is_new_type(), scan_processing, inverted, timing)."""
+    _fields_ = [("is_new_protocol", C.c_uint8), ("scan_processing", C.c_uint8), ("inverted", C.c_uint8),
+                ("pad", C.c_uint8), ("timing", Timing)]
 
 
 class ScanParams(C.Structure):
@@ -237,6 +245,7 @@ def lib() -> C.CDLL:
         sig[f"rpl_{kind}_stream_cloud"] = ([vp, PCP, vp, vp], u32)
         sig[f"rpl_{kind}_stream_cloud_dev"] = ([vp, PCP, vp, vp, vp], u32)
         sig[f"rpl_{kind}_stream_set_frames"] = ([vp, vp, vp], u32)
+        sig[f"rpl_{kind}_stream_set_lidars"] = ([vp, vp, vp], u32)
         sig[f"rpl_{kind}_stream_laserscan_msgs"] = ([vp, PSP, C.c_int64, vp, u64, vp, vp, vp], u32)
         sig[f"rpl_{kind}_stream_laserscan_msgs_dev"] = ([vp, PSP, C.c_int64, vp, u64, vp, vp, vp, vp], u32)
         sig[f"rpl_{kind}_stream_cloud_msgs"] = ([vp, PCP, C.c_int64, vp, u64, vp, vp, vp], u32)
@@ -253,10 +262,20 @@ def scan_params(is_new_protocol=0, scan_processing=1, inverted=0, apply_ascend=1
     return ScanParams(int(is_new_protocol), int(scan_processing), int(inverted), int(apply_ascend), int(flags))
 
 
+def lidar_settings(is_new_protocol=0, scan_processing=1, inverted=0, timing: "Timing | None" = None) -> LidarSettings:
+    """timing None: Timing(31, 0, 0, 0)"""
+    return LidarSettings(int(is_new_protocol), int(scan_processing), int(inverted), 0,
+                         timing if timing is not None else Timing(31, 0, 0, 0))
+
+
 def cloud_params(range_min=0.15, range_max=40.0, intensity_min=0.0, voxel_size=0.0, sor_k=0,
                  sor_alpha=1.0, is_new_protocol=0, flags=0) -> CloudParams:
     return CloudParams(float(range_min), float(range_max), float(intensity_min), float(voxel_size),
                        int(sor_k), float(sor_alpha), int(is_new_protocol), int(flags), (C.c_uint8 * 2)(0, 0))
+
+
+def _timing(t):
+    return C.byref(t) if t is not None else None
 
 
 def _p(a):
@@ -659,12 +678,13 @@ class CapsuleStreamSession:
                 _p(out["intensities"]), _p(out["beam_counts"]), _p(out["angle_increment"]),
                 _p(out["scans_per_stream"])))
             return out
-        assert rx_us is not None and timing is not None, "a stamped push takes both rx_us and timing"
+        assert rx_us is not None and (timing is not None or params.flags & FLAG_PER_STREAM), \
+            "a stamped push takes rx_us and timing (timing may be None with FLAG_PER_STREAM)"
         rx = np.ascontiguousarray(rx_us, dtype=np.uint64)
         assert rx.shape == (self.n_streams, self.stride_capsules)
         out = self._stamped_outputs(out)
         self._ctx._check(self._fn("push_ts")(
-            self._h, _p(capsules), _p(cc), C.byref(timing), _p(rx), C.byref(params), _p(out["ranges"]),
+            self._h, _p(capsules), _p(cc), _timing(timing), _p(rx), C.byref(params), _p(out["ranges"]),
             _p(out["intensities"]), _p(out["beam_counts"]), _p(out["angle_increment"]), _p(out["scans_per_stream"]),
             _p(out["scan_begin_ts_us"])))
         return out
@@ -710,6 +730,16 @@ class CapsuleStreamSession:
         rm = None if range_max is None else np.ascontiguousarray(range_max, dtype=np.float32)
         assert rm is None or rm.shape == (self.n_streams,)
         self._ctx._check(self._fn("set_frames")(self._h, C.cast(ids, C.c_void_p), _p(rm)))
+
+    def set_lidars(self, settings, mask=None):
+        """Per stream the lidar's settings (n_streams LidarSettings, see lidar_settings) that pushes and message calls
+        with FLAG_PER_STREAM, and cloud calls with CLOUD_PER_STREAM, use.  Only the entries where mask is true are
+        copied (None: all); the first call must set every stream."""
+        assert len(settings) == self.n_streams
+        arr = (LidarSettings * self.n_streams)(*settings)
+        m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
+        assert m is None or m.shape == (self.n_streams,)
+        self._ctx._check(self._fn("set_lidars")(self._h, C.cast(arr, C.c_void_p), _p(m)))
 
     def _msgs(self, name, params, clock_offset_ns, msgs, packed):
         ns = self.n_streams * self.max_scans
@@ -808,13 +838,13 @@ class NormalStreamSession(CapsuleStreamSession):
                 self._h, _p(stream_bytes), _p(bc), C.byref(params), _p(out["ranges"]), _p(out["intensities"]),
                 _p(out["beam_counts"]), _p(out["angle_increment"]), _p(out["scans_per_stream"])))
             return out
-        assert chunk_bytes is not None and chunk_rx_us is not None and timing is not None, \
-            "a stamped push takes chunk_bytes, chunk_rx_us and timing"
+        assert chunk_bytes is not None and chunk_rx_us is not None and (timing is not None or params.flags & FLAG_PER_STREAM), \
+            "a stamped push takes chunk_bytes, chunk_rx_us and timing (timing may be None with FLAG_PER_STREAM)"
         rx = np.ascontiguousarray(chunk_rx_us, dtype=np.uint64)
         assert chunk_bytes == 0 or rx.shape == (self.n_streams, -(-self.stride_bytes // chunk_bytes))
         out = self._stamped_outputs(out)
         self._ctx._check(self._fn("push_ts")(
-            self._h, _p(stream_bytes), _p(bc), C.byref(timing), chunk_bytes, _p(rx), C.byref(params),
+            self._h, _p(stream_bytes), _p(bc), _timing(timing), chunk_bytes, _p(rx), C.byref(params),
             _p(out["ranges"]), _p(out["intensities"]), _p(out["beam_counts"]), _p(out["angle_increment"]),
             _p(out["scans_per_stream"]), _p(out["scan_begin_ts_us"])))
         return out
@@ -865,13 +895,13 @@ class CapsuleByteStreamSession(CapsuleStreamSession):
                 _p(out["intensities"]), _p(out["beam_counts"]), _p(out["angle_increment"]),
                 _p(out["scans_per_stream"])))
             return out
-        assert chunk_bytes is not None and chunk_rx_us is not None and timing is not None, \
-            "a stamped push takes chunk_bytes, chunk_rx_us and timing"
+        assert chunk_bytes is not None and chunk_rx_us is not None and (timing is not None or params.flags & FLAG_PER_STREAM), \
+            "a stamped push takes chunk_bytes, chunk_rx_us and timing (timing may be None with FLAG_PER_STREAM)"
         rx = np.ascontiguousarray(chunk_rx_us, dtype=np.uint64)
         assert chunk_bytes == 0 or rx.shape == (self.n_streams, -(-self.stride_bytes // chunk_bytes))
         out = self._stamped_outputs(out)
         self._ctx._check(self._L.rpl_capsule_stream_push_bytes_ts(
-            self._h, _p(stream_bytes), _p(bc), C.byref(timing), chunk_bytes, _p(rx), C.byref(params),
+            self._h, _p(stream_bytes), _p(bc), _timing(timing), chunk_bytes, _p(rx), C.byref(params),
             _p(out["ranges"]), _p(out["intensities"]), _p(out["beam_counts"]), _p(out["angle_increment"]),
             _p(out["scans_per_stream"]), _p(out["scan_begin_ts_us"])))
         return out

@@ -61,9 +61,10 @@ __device__ __forceinline__ void rank_sort(const uint32_t* in, uint32_t* out, uin
 // node of the revolution carried in front of the new nodes, which is a scan start like any other -- listed first when
 // the decoder hands a scan-start list over (dense), found by the flag pass like the others when it does not.
 // STAMPED (a stamped session push, STREAM only): also the stamp of every published scan's scan-start node and of the
-// open revolution's first node, computed for those nodes alone (sa, m)
+// open revolution's first node, computed for those nodes alone (sa, and the delay model m0 or, with a per-stream table,
+// the stream's own)
 template <bool STREAM, bool STAMPED>
-__device__ __forceinline__ void assemble_body(const AssembleArgs& a, const AssembleStampArgs& sa, const DelayModel& m) {
+__device__ __forceinline__ void assemble_body(const AssembleArgs& a, const AssembleStampArgs& sa, const DelayModel& m0) {
   static_assert(STREAM || !STAMPED, "stamps are a stream session's");
   __shared__ uint32_t s_list[kListCap], s_sorted[kListCap];      // scan-start positions
   __shared__ uint32_t s_rlist[kResetCap], s_rsorted[kResetCap];  // reset positions
@@ -76,6 +77,9 @@ __device__ __forceinline__ void assemble_body(const AssembleArgs& a, const Assem
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 
   for (uint32_t s = blockIdx.x; s < a.n_streams; s += gridDim.x) {
+    DelayModel m = m0;
+    if constexpr (STAMPED)
+      if (sa.lidars) m = delay_model(sa.ans_type, sa.lidars[s].timing);
     const uint32_t L = STREAM ? a.carry_len[s] : 0u;           // carried nodes
     const uint32_t base = STREAM ? a.max_nodes - L : 0u;        // position 0 within the stream's region
     const uint32_t n = a.node_counts[s] + L;

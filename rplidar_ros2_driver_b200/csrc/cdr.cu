@@ -185,7 +185,8 @@ __global__ void __launch_bounds__(CT) laserscan_msgs_kernel(MsgWriteArgs a) {
       uint32_t sec, nsec;
       msg_stamp(b, a.clock_offset_ns, &sec, &nsec);
       const double d = msg_period(b, e);
-      const double denom = a.mode_a ? (double)n : (double)(n > 1 ? n - 1 : 1);
+      const bool mode_a = a.lidars ? a.lidars[i / a.max_scans].mode_a != 0 : a.mode_a != 0;
+      const double denom = mode_a ? (double)n : (double)(n > 1 ? n - 1 : 1);
       put32(msg + 4, sec);
       put32(msg + 8, nsec);
       uint8_t* f = msg + h.bytes;

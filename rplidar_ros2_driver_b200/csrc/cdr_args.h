@@ -5,6 +5,8 @@
 
 #include <algorithm>
 
+#include "lidar_args.h"
+
 namespace rpl {
 
 struct LaserScanMeta {  // == rpl_laserscan_meta
@@ -93,6 +95,7 @@ struct MsgWriteArgs {
   const uint32_t* sizes;
   uint8_t* out;                    // message i at out + offsets[i] - out_base
   unsigned long long out_base;
+  const LidarSettings* lidars;     // [n_slots / max_scans] nullable: LaserScan slot i takes its stream's mode, not mode_a
 };
 
 cudaError_t launch_msg_table(const MsgTableArgs& a, cudaStream_t stream);

@@ -5,6 +5,8 @@
 
 #include <algorithm>
 
+#include "lidar_args.h"
+
 namespace rpl {
 
 // the capsule formats (decode_formats.cu): 0x82 express, 0x83 HQ, 0x84 ultra, 0x85 dense, 0x86 ultra-dense
@@ -34,6 +36,9 @@ struct CapsuleDecodeArgs {
   // unused then: the decoder's cross-capsule state travels in the held record.
   uint32_t* held;                 // [n_streams][kHeldWords], read and rewritten in place (HQ: unused)
   uint32_t node_stride, node_first;
+  // stream session only, nullable: each stream's jump threshold from its own entry's sample duration instead of
+  // sample_duration_us
+  const LidarSettings* lidars;    // [n_streams]
 };
 
 // a held-capsule record, sized for the largest capsule (ultra-dense, 170 bytes): words 0..42 the capsule's bytes,
@@ -61,10 +66,7 @@ struct NormalDecodeArgs {
   uint32_t node_stride, node_first;
 };
 
-// per-sample timestamps (timestamps.cu)
-struct TimingDesc {  // sl::SlamtecLidarTimingDesc without the bool
-  uint32_t sample_duration_us, native_baudrate, linkage_delay_us, native_interface_type;
-};
+// per-sample timestamps (timestamps.cu; TimingDesc: lidar_args.h)
 struct TimestampArgs {
   const unsigned long long* capsule_rx_us;  // [n_streams][stride_capsules]
   const uint32_t* capsule_status;
@@ -143,6 +145,8 @@ struct AssembleStampArgs {
   // closed the scan, which opens the next scan whether that one is published, dropped past max_scans or reset
   unsigned long long* slot_begin_us;        // [n_streams][AssembleArgs::max_scans], unused slots 0
   unsigned long long* slot_end_us;          // [n_streams][AssembleArgs::max_scans], unused slots 0
+  // nullable: each stream's delay model from its own entry's timing instead of `timing`
+  const LidarSettings* lidars;              // [n_streams]
 };
 
 // byte-level framing with the SDK's resynchronisation (frame.cu)

@@ -307,6 +307,8 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
   }
 
   for (uint32_t s = blockIdx.x; s < a.n_streams; s += gridDim.x) {
+    if constexpr (STREAM && T::JUMP_CABINS != 0)
+      if (a.lidars) thr_q8 = (360 * 100 * T::JUMP_CABINS / (int)(1000000u / a.lidars[s].timing.sample_duration_us)) << 8;
     const uint32_t n = STREAM ? min(a.counts[s], a.stride_capsules) : a.counts[s];
     const uint8_t* src = a.capsules + (size_t)s * a.stride_capsules * CB;
     uint2* out = STREAM ? a.nodes_out + (size_t)s * a.node_stride + a.node_first

@@ -144,7 +144,8 @@ rpl_result launch_fast(rpl_ctx* c, Lane& l, const rpl::ScanBatchArgs& a, FastKer
     cudaEventRecord(e1, stream);
     c->prof_fast.emplace_back(e0, e1);
   }
-  c->launches++;
+  // a per-stream LaserScan launch of the shared-memory kernels is one launch per mode present
+  c->launches += k == FastKernel::kSmall && a.lidars && !a.xyzi ? __builtin_popcount(a.lidar_modes) : 1;
   return RPL_RESULT_OK;
 }
 
@@ -191,7 +192,9 @@ rpl_result enqueue_args(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, uint32_t flag
              RPL_RESULT_OPERATION_FAIL);
     a.nodes_out = nullptr;
   }
-  const FastKernel k = pick_fast(a, flags);
+  FastKernel k = pick_fast(a, flags);
+  // per-stream settings are read by the shared-memory kernels and the general kernel only
+  if (a.lidars && k != FastKernel::kSmall) k = FastKernel::kNone;
   if (k != FastKernel::kNone) {
     RPL_CUDA(c, cudaMemsetAsync(l.fallback_count, 0, sizeof(uint32_t), stream), RPL_RESULT_OPERATION_FAIL);
     const rpl_result r = launch_fast(c, l, a, k, stream, cloud, post_fused, hand_off);
@@ -213,12 +216,20 @@ rpl::ScanBatchArgs scan_args(const rpl_scan_params* p, const Lane& l) {
   return a;
 }
 
+// a session call's per-stream settings (RPL_FLAG_PER_STREAM): scan slot s of the call takes entry s / per of `at`,
+// which points at the call's first stream's entry; at == nullptr: the call's params serve every scan
+struct LidarTable {
+  const rpl::LidarSettings* at = nullptr;
+  uint32_t per = 0;    // scan slots per stream
+  uint32_t modes = 0;  // bit 0: some stream of the session in Mode B, bit 1: in Mode A
+};
+
 // queue the scan kernels for one device-resident batch on `stream`
 rpl_result enqueue_scan(rpl_ctx* c, Lane& l, const rpl_node_hq* nodes, const uint32_t* counts,
                         uint32_t n_scans, uint32_t stride, const rpl_scan_params* p,
                         rpl_node_hq* nodes_out, float* ranges, float* intens, uint32_t* beams,
                         float* inc, uint32_t* status, uint32_t* path, cudaStream_t stream,
-                        const uint2* views = nullptr, unsigned long long nodes_total = 0) {
+                        const uint2* views = nullptr, unsigned long long nodes_total = 0, LidarTable lt = {}) {
   if (n_scans == 0) return RPL_RESULT_OK;
   if (!nodes || !counts || !p) {
     c->err = "null nodes/counts/params";
@@ -254,6 +265,9 @@ rpl_result enqueue_scan(rpl_ctx* c, Lane& l, const rpl_node_hq* nodes, const uin
   a.path = path;
   a.views = views;
   a.nodes_total = nodes_total;
+  a.lidars = lt.at;
+  a.lidar_scans = lt.per;
+  a.lidar_modes = lt.modes;
   rpl_result r = scratch_enter(c, l, stream);
   if (r == RPL_RESULT_OK) r = enqueue_args(c, l, a, p->flags, stream);
   return r == RPL_RESULT_OK ? scratch_leave(c, l, stream) : r;
@@ -1217,7 +1231,19 @@ struct rpl_capsule_stream {
   std::vector<rpl::StreamMsgHeader> msg_hdr_host;
   unsigned char* msg_work = nullptr;            // the scan kernels' outputs and the tables of a messages call
   size_t msg_work_bytes = 0;
+  // the per-stream lidar settings (rpl_*_stream_set_lidars) that calls with RPL_FLAG_PER_STREAM / RPL_CLOUD_PER_STREAM
+  // read; empty until the first call sets every stream
+  rpl::LidarSettings* lidars = nullptr;         // [n_streams] device
+  std::vector<rpl::LidarSettings> lidars_host;
+  uint32_t lidar_modes = 0;                     // LidarTable::modes of the table
 };
+
+static_assert(sizeof(rpl::LidarSettings) == sizeof(rpl_lidar_settings) &&
+                  offsetof(rpl::LidarSettings, mode_a) == offsetof(rpl_lidar_settings, scan_processing) &&
+                  offsetof(rpl::LidarSettings, inverted) == offsetof(rpl_lidar_settings, inverted) &&
+                  offsetof(rpl::LidarSettings, timing) == offsetof(rpl_lidar_settings, timing) &&
+                  sizeof(rpl::TimingDesc) == sizeof(rpl_timing),
+              "rpl::LidarSettings must be rpl_lidar_settings byte for byte");
 
 namespace {
 
@@ -1257,10 +1283,13 @@ struct WireChunk {
   uint32_t *framer, *framed_counts;
   uint8_t* framed;
   unsigned long long* framed_rx;
+  // a session push with RPL_FLAG_PER_STREAM: the chunk's first stream's entry of the session's table (else nullptr)
+  const rpl::LidarSettings* lidars;
+  uint32_t lidar_modes;
 };
 
-// session cs's chunk from stream s0 in the push under way (arena cs->parity)
-WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0) {
+// session cs's chunk from stream s0 in the push under way (arena cs->parity); per_stream: RPL_FLAG_PER_STREAM
+WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0, bool per_stream) {
   const uint32_t p = cs->parity, sc = cs->stride_capsules;
   const size_t sn = (size_t)s0 * cs->stride_nodes, so = (size_t)s0 * cs->max_scans;
   WireChunk w{};
@@ -1296,6 +1325,10 @@ WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0) {
     w.framed = cs->framed + (size_t)s0 * sc * cs->cap_bytes;
     w.framed_counts = cs->framed_counts + s0;
     w.framed_rx = cs->framed_rx + (size_t)s0 * sc;
+  }
+  if (per_stream) {
+    w.lidars = cs->lidars + s0;
+    w.lidar_modes = cs->lidar_modes;
   }
   return w;
 }
@@ -1368,6 +1401,7 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
     a.held = w.held;
     a.node_stride = w.node_stride;
     a.node_first = w.node_first;
+    a.lidars = w.lidars;
     r = decode_capsules_launch(c, w.ans_type, a, st);
   }
   if (r != RPL_RESULT_OK) return r;
@@ -1390,6 +1424,7 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
     t.prev_stamped = w.prev_stamped ? 1u : 0u;
     t.slot_begin_us = w.slot_begin;
     t.slot_end_us = w.slot_end;
+    t.lidars = w.lidars;
   }
   r = assemble_common(c, w.nodes, w.node_counts, ns, w.stride_nodes, w.status, w.offsets, w.status ? counts : nullptr,
                       w.status ? sc : 0u, w.max_nodes, w.max_scans, w.max_nodes, nullptr, w.views, w.scan_len,
@@ -1400,7 +1435,7 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
   RPL_CUDA(c, cudaEventRecord(c->asm_done, st), RPL_RESULT_OPERATION_FAIL);
   return enqueue_scan(c, l, w.nodes, w.scan_len, ns * w.max_scans, w.max_nodes, params, nullptr, ranges, intens, beams,
                       inc, nullptr, nullptr, st, reinterpret_cast<const uint2*>(w.views),
-                      (unsigned long long)ns * w.stride_nodes);
+                      (unsigned long long)ns * w.stride_nodes, LidarTable{w.lidars, w.max_scans, w.lidar_modes});
 }
 
 // A host call's wire input and LaserScan outputs: host arrays of all its streams (the chain's, a session's host push)
@@ -1476,6 +1511,19 @@ rpl_result push_host(rpl_ctx* c, const HostWire& h, uint32_t n_streams, uint32_t
   return run_chunks(c, n_streams, chunk, run_chunk);
 }
 
+// a call with RPL_FLAG_PER_STREAM / RPL_CLOUD_PER_STREAM needs the table
+bool lidars_ok(rpl_capsule_stream* cs) {
+  if (!cs->lidars_host.empty()) return true;
+  cs->c->err = "per-stream settings requested before rpl_*_stream_set_lidars set every stream";
+  return false;
+}
+
+// the table of a session call: the stream s0's entry on, when per_stream
+LidarTable lidar_table(const rpl_capsule_stream* cs, bool per_stream, uint32_t s0) {
+  if (!per_stream) return LidarTable{};
+  return LidarTable{cs->lidars + s0, cs->max_scans, cs->lidar_modes};
+}
+
 bool capsule_stream_args_ok(rpl_capsule_stream* cs, const uint8_t* capsules, const uint32_t* capsule_counts,
                             uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
                             float* intensities, uint32_t* beam_counts, uint32_t* scans_per_stream) {
@@ -1484,8 +1532,12 @@ bool capsule_stream_args_ok(rpl_capsule_stream* cs, const uint8_t* capsules, con
     c->err = "null capsules, counts, params or output buffer";
     return false;
   }
-  // the standard decoder takes no sample duration (it tests no jump between capsules)
-  if (cs->ans_type != RPL_ANS_MEASUREMENT && !sample_duration_ok(c, sample_duration_us)) return false;
+  if ((params->flags & RPL_FLAG_PER_STREAM) != 0) {  // every stream's sample duration comes from the table
+    if (!lidars_ok(cs)) return false;
+  } else if (cs->ans_type != RPL_ANS_MEASUREMENT && !sample_duration_ok(c, sample_duration_us)) {
+    // (the standard decoder takes no sample duration: it tests no jump between capsules)
+    return false;
+  }
   // the alignment rule of rpl_decode_capsules_batch_dev: only dense capsules are read in 4-byte words (a byte session's
   // bytes have any alignment: its decoder reads the session's own capsule slots)
   if (cs->ans_type == 0x85 && !cs->framer && (reinterpret_cast<uintptr_t>(capsules) & 3u) != 0) {
@@ -1609,12 +1661,14 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint
   return RPL_RESULT_OK;
 }
 
-// the stamped pushes' own arguments (chunk_bytes: 0x81 only, 1 for the capsule formats) into *sp
-bool stamp_args_ok(rpl_capsule_stream* cs, const rpl_timing* timing, const uint64_t* rx, uint32_t chunk_bytes,
-                   uint64_t* scan_begin_ts_us, StampPush* sp) {
+// the stamped pushes' own arguments (chunk_bytes: 0x81 only, 1 for the capsule formats) into *sp; with
+// RPL_FLAG_PER_STREAM the table's timing serves and `timing` may be null
+bool stamp_args_ok(rpl_capsule_stream* cs, const rpl_scan_params* params, const rpl_timing* timing, const uint64_t* rx,
+                   uint32_t chunk_bytes, uint64_t* scan_begin_ts_us, StampPush* sp) {
   if (!cs) return false;
   rpl_ctx* c = cs->c;
-  if (!timing || !rx || !scan_begin_ts_us) {
+  const bool per_stream = params && (params->flags & RPL_FLAG_PER_STREAM) != 0;
+  if ((!timing && !per_stream) || !rx || !scan_begin_ts_us) {
     c->err = "null timing, receive times or scan_begin_ts_us";
     return false;
   }
@@ -1626,8 +1680,9 @@ bool stamp_args_ok(rpl_capsule_stream* cs, const rpl_timing* timing, const uint6
     c->err = "timestamp buffers must be 8-byte aligned";
     return false;
   }
-  sp->timing = rpl::TimingDesc{timing->sample_duration_us, timing->native_baudrate, timing->linkage_delay_us,
-                               timing->native_interface_type};
+  if (timing && !per_stream)
+    sp->timing = rpl::TimingDesc{timing->sample_duration_us, timing->native_baudrate, timing->linkage_delay_us,
+                                 timing->native_interface_type};
   sp->rx = reinterpret_cast<const unsigned long long*>(rx);
   sp->chunk_bytes = chunk_bytes;
   const uint32_t stride_in = cs->framer ? cs->stride_bytes : cs->stride_capsules;  // bytes, or capsules
@@ -1671,8 +1726,9 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* capsules, const ui
   const HostWire h{capsules, capsule_counts, in_stream, sample_duration_us,
                    cs->max_nodes, cs->max_scans, params, ranges, intensities, angle_increment, beam_counts,
                    scans_per_stream, sp, rx_stream};
-  const rpl_result r =
-      push_host(c, h, cs->n_streams, cs->chunk_host, [&](Carve&, uint32_t s0) { return session_chunk(cs, s0); });
+  const bool per_stream = (params->flags & RPL_FLAG_PER_STREAM) != 0;
+  const rpl_result r = push_host(c, h, cs->n_streams, cs->chunk_host,
+                                 [&](Carve&, uint32_t s0) { return session_chunk(cs, s0, per_stream); });
   cs->parity ^= 1u;
   cs->prev_stamped = sp != nullptr;
   if (r == RPL_RESULT_OK) {
@@ -1708,7 +1764,7 @@ rpl_result stream_push_dev(rpl_capsule_stream* cs, const uint8_t* capsules, cons
       chunk_sp.rx += (size_t)s0 * (cs->status && !bytes ? cs->stride_capsules : sp->stride_chunks);
       chunk_sp.scan_ts += so;
     }
-    r = capsule_stream_chunk(c, c->lane[0], st, session_chunk(cs, s0), ns,
+    r = capsule_stream_chunk(c, c->lane[0], st, session_chunk(cs, s0, (params->flags & RPL_FLAG_PER_STREAM) != 0), ns,
                              capsules + (size_t)s0 * (bytes ? cs->stride_bytes : cs->stride_capsules * cs->cap_bytes),
                              capsule_counts + s0,
                              sample_duration_us, params, ranges + (size_t)s0 * row, intensities + (size_t)s0 * row,
@@ -1764,6 +1820,10 @@ rpl_result stream_cloud_chunk(rpl_capsule_stream* cs, Lane& l, uint32_t s0, uint
   a.range_min = p->range_min;
   a.range_max = p->range_max;
   a.intensity_min = p->intensity_min;
+  if ((p->flags & RPL_CLOUD_PER_STREAM) != 0) {  // each stream's is_new_protocol (the window's intensity too)
+    a.lidars = cs->lidars + s0;
+    a.lidar_scans = cs->max_scans;
+  }
   const bool separate = (p->flags & RPL_CLOUD_NO_FUSED) != 0;
   bool fused = false;
   rpl_result r = scratch_enter(c, l, st);
@@ -1791,6 +1851,7 @@ bool stream_cloud_args_ok(rpl_capsule_stream* cs, const rpl_cloud_params* params
     return false;
   }
   if (!cloud_params_ok(c, params)) return false;
+  if ((params->flags & RPL_CLOUD_PER_STREAM) != 0 && !lidars_ok(cs)) return false;
   if (cs->cloud_chunk == 0) {
     c->err = "no clouds to take: the session has not pushed yet, or its last push failed";
     return false;
@@ -1879,6 +1940,42 @@ rpl_result stream_set_frames(rpl_capsule_stream* cs, const char* const* frame_id
   return RPL_RESULT_OK;
 }
 
+// the per-stream lidar settings: the masked entries of `settings` replace the table's, all or none
+rpl_result stream_set_lidars(rpl_capsule_stream* cs, const rpl_lidar_settings* settings, const uint8_t* stream_mask) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!settings) {
+    c->err = "null settings";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  std::vector<rpl::LidarSettings> t = cs->lidars_host;
+  if (t.empty()) {  // the first call sets every stream: no stream is left without a sample duration
+    for (uint32_t s = 0; s < cs->n_streams; ++s)
+      if (stream_mask && !stream_mask[s]) {
+        c->err = "the first rpl_*_stream_set_lidars call must set every stream";
+        return RPL_RESULT_INVALID_DATA;
+      }
+    t.resize(cs->n_streams);
+  }
+  for (uint32_t s = 0; s < cs->n_streams; ++s) {
+    if (stream_mask && !stream_mask[s]) continue;
+    // the decoders divide by it (the angular-jump threshold)
+    if (!sample_duration_ok(c, settings[s].timing.sample_duration_us)) return RPL_RESULT_INVALID_DATA;
+    std::memcpy(&t[s], &settings[s], sizeof(rpl::LidarSettings));
+  }
+  uint32_t modes = 0;
+  for (const rpl::LidarSettings& e : t) modes |= e.mode_a ? 2u : 1u;
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  if (!cs->lidars)
+    RPL_CUDA(c, dev_alloc(&cs->lidars, cs->n_streams), RPL_RESULT_INSUFFICIENT_MEMORY);
+  RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);  // a push or messages call may still read it
+  RPL_CUDA(c, cudaMemcpy(cs->lidars, t.data(), t.size() * sizeof(rpl::LidarSettings), cudaMemcpyHostToDevice),
+           RPL_RESULT_OPERATION_FAIL);
+  cs->lidars_host = std::move(t);
+  cs->lidar_modes = modes;
+  return RPL_RESULT_OK;
+}
+
 // the PointCloud2 members between the header and the data: height 1, width, the fields x, y, z, intensity (float32,
 // count 1), is_bigendian 0, point_step 16, row_step, data length
 rpl::CloudTail cloud_tail() {
@@ -1941,6 +2038,10 @@ bool stream_msgs_args_ok(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* 
   }
   if (kind == rpl::MsgKind::kPointCloud2 && !cloud_params_ok(c, static_cast<const rpl_cloud_params*>(params)))
     return false;
+  const bool per_stream = kind == rpl::MsgKind::kLaserScan
+                              ? (static_cast<const rpl_scan_params*>(params)->flags & RPL_FLAG_PER_STREAM) != 0
+                              : (static_cast<const rpl_cloud_params*>(params)->flags & RPL_CLOUD_PER_STREAM) != 0;
+  if (per_stream && !lidars_ok(cs)) return false;
   if (dev && ((reinterpret_cast<uintptr_t>(msgs) & 15u) || misaligned8(offsets) || misaligned8(total) ||
               (reinterpret_cast<uintptr_t>(sizes) & 3u))) {
     c->err = "msgs must be 16-byte aligned, msg_offsets and total_bytes 8-byte, msg_sizes 4-byte aligned";
@@ -1976,14 +2077,17 @@ rpl_result msgs_prepare(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* p
   for (uint32_t s0 = 0; s0 < cs->n_streams && r == RPL_RESULT_OK; s0 += cs->cloud_chunk) {
     const uint32_t ns = std::min(cs->cloud_chunk, cs->n_streams - s0);
     const size_t so = (size_t)s0 * cs->max_scans;
-    if (kind == rpl::MsgKind::kLaserScan)
+    if (kind == rpl::MsgKind::kLaserScan) {
+      const auto* p = static_cast<const rpl_scan_params*>(params);
       r = enqueue_scan(c, c->lane[0], cs->arena[cs->cloud_arena] + (size_t)s0 * cs->stride_nodes, cs->scan_len + so,
-                       ns * cs->max_scans, cs->max_nodes, static_cast<const rpl_scan_params*>(params), nullptr,
-                       w.data + so * row, w.data + (NS + so) * row, w.counts + so, w.inc + so, nullptr, nullptr, st,
-                       reinterpret_cast<const uint2*>(cs->views + so), (unsigned long long)ns * cs->stride_nodes);
-    else
+                       ns * cs->max_scans, cs->max_nodes, p, nullptr, w.data + so * row, w.data + (NS + so) * row,
+                       w.counts + so, w.inc + so, nullptr, nullptr, st, reinterpret_cast<const uint2*>(cs->views + so),
+                       (unsigned long long)ns * cs->stride_nodes,
+                       lidar_table(cs, (p->flags & RPL_FLAG_PER_STREAM) != 0, s0));
+    } else {
       r = stream_cloud_chunk(cs, c->lane[0], s0, ns, static_cast<const rpl_cloud_params*>(params),
                              w.data + so * row * 4, w.counts + so, st);
+    }
   }
   if (r != RPL_RESULT_OK) return r;
   rpl::MsgTableArgs t{};
@@ -2029,7 +2133,9 @@ rpl_result msgs_write(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* par
     a.ranges = w.data;
     a.intensities = w.data + NS * cs->max_nodes;
     a.angle_increment = w.inc;
-    a.mode_a = static_cast<const rpl_scan_params*>(params)->scan_processing ? 1u : 0u;
+    const auto* p = static_cast<const rpl_scan_params*>(params);
+    a.mode_a = p->scan_processing ? 1u : 0u;
+    if ((p->flags & RPL_FLAG_PER_STREAM) != 0) a.lidars = cs->lidars;
     RPL_CUDA(c, rpl::launch_laserscan_msgs(a, cs->max_nodes, st), RPL_RESULT_OPERATION_FAIL);
   } else {
     a.xyzi = w.data;
@@ -2223,6 +2329,7 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   cudaFree(cs->slot_end);
   cudaFree(cs->msg_hdr);
   cudaFree(cs->msg_work);
+  cudaFree(cs->lidars);
   if (cs->done) cudaEventDestroy(cs->done);
   delete cs;
 }
@@ -2249,8 +2356,8 @@ rpl_result rpl_capsule_stream_push_ts(rpl_capsule_stream* cs, const uint8_t* cap
                                       uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
                                       uint64_t* scan_begin_ts_us) {
   StampPush sp{};
-  if (!stamp_args_ok(cs, timing, capsule_rx_us, 1, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
-  return stream_push(cs, capsules, capsule_counts, timing->sample_duration_us, params, ranges, intensities,
+  if (!stamp_args_ok(cs, params, timing, capsule_rx_us, 1, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
+  return stream_push(cs, capsules, capsule_counts, timing ? timing->sample_duration_us : 0u, params, ranges, intensities,
                      beam_counts, angle_increment, scans_per_stream, &sp);
 }
 
@@ -2260,8 +2367,8 @@ rpl_result rpl_capsule_stream_push_ts_dev(rpl_capsule_stream* cs, const uint8_t*
                                           float* intensities, uint32_t* beam_counts, float* angle_increment,
                                           uint32_t* scans_per_stream, uint64_t* scan_begin_ts_us, void* stream) {
   StampPush sp{};
-  if (!stamp_args_ok(cs, timing, capsule_rx_us, 1, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
-  return stream_push_dev(cs, capsules, capsule_counts, timing->sample_duration_us, params, ranges, intensities,
+  if (!stamp_args_ok(cs, params, timing, capsule_rx_us, 1, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
+  return stream_push_dev(cs, capsules, capsule_counts, timing ? timing->sample_duration_us : 0u, params, ranges, intensities,
                          beam_counts, angle_increment, scans_per_stream, stream, &sp);
 }
 
@@ -2364,8 +2471,8 @@ rpl_result rpl_capsule_stream_push_bytes_ts(rpl_capsule_stream* cs, const uint8_
                                             uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
                                             uint64_t* scan_begin_ts_us) {
   StampPush sp{};
-  if (!stamp_args_ok(cs, timing, chunk_rx_us, chunk_bytes, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
-  return stream_push(cs, bytes, byte_counts, timing->sample_duration_us, params, ranges, intensities, beam_counts,
+  if (!stamp_args_ok(cs, params, timing, chunk_rx_us, chunk_bytes, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
+  return stream_push(cs, bytes, byte_counts, timing ? timing->sample_duration_us : 0u, params, ranges, intensities, beam_counts,
                      angle_increment, scans_per_stream, &sp, true);
 }
 
@@ -2376,8 +2483,8 @@ rpl_result rpl_capsule_stream_push_bytes_ts_dev(rpl_capsule_stream* cs, const ui
                                                 uint32_t* beam_counts, float* angle_increment,
                                                 uint32_t* scans_per_stream, uint64_t* scan_begin_ts_us, void* stream) {
   StampPush sp{};
-  if (!stamp_args_ok(cs, timing, chunk_rx_us, chunk_bytes, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
-  return stream_push_dev(cs, bytes, byte_counts, timing->sample_duration_us, params, ranges, intensities, beam_counts,
+  if (!stamp_args_ok(cs, params, timing, chunk_rx_us, chunk_bytes, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
+  return stream_push_dev(cs, bytes, byte_counts, timing ? timing->sample_duration_us : 0u, params, ranges, intensities, beam_counts,
                          angle_increment, scans_per_stream, stream, &sp, true);
 }
 
@@ -2471,7 +2578,7 @@ rpl_result rpl_normal_stream_push_ts(rpl_normal_stream* ns, const uint8_t* bytes
                                      uint64_t* scan_begin_ts_us) {
   rpl_capsule_stream* cs = capsule_session(ns);
   StampPush sp{};
-  if (!stamp_args_ok(cs, timing, chunk_rx_us, chunk_bytes, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
+  if (!stamp_args_ok(cs, params, timing, chunk_rx_us, chunk_bytes, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
   return stream_push(cs, bytes, byte_counts, 0, params, ranges, intensities, beam_counts, angle_increment,
                      scans_per_stream, &sp);
 }
@@ -2483,7 +2590,7 @@ rpl_result rpl_normal_stream_push_ts_dev(rpl_normal_stream* ns, const uint8_t* b
                                          uint64_t* scan_begin_ts_us, void* stream) {
   rpl_capsule_stream* cs = capsule_session(ns);
   StampPush sp{};
-  if (!stamp_args_ok(cs, timing, chunk_rx_us, chunk_bytes, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
+  if (!stamp_args_ok(cs, params, timing, chunk_rx_us, chunk_bytes, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
   return stream_push_dev(cs, bytes, byte_counts, 0, params, ranges, intensities, beam_counts, angle_increment,
                          scans_per_stream, stream, &sp);
 }
@@ -2527,10 +2634,13 @@ rpl_result rpl_normal_stream_cloud(rpl_normal_stream* ns, const rpl_cloud_params
   return stream_cloud(capsule_session(ns), params, xyzi, point_counts);
 }
 
-// ---- packed messages of the last push, one set per session handle type -------------------------------------------
+// ---- per-stream settings and packed messages of the last push, one set per session handle type ---------------------
 #define RPL_STREAM_MSGS(KIND, T, SESSION)                                                                              \
   rpl_result rpl_##KIND##_stream_set_frames(T* s, const char* const* frame_ids, const float* range_max) {             \
     return stream_set_frames(SESSION, frame_ids, range_max);                                                         \
+  }                                                                                                                  \
+  rpl_result rpl_##KIND##_stream_set_lidars(T* s, const rpl_lidar_settings* settings, const uint8_t* stream_mask) {  \
+    return stream_set_lidars(SESSION, settings, stream_mask);                                                        \
   }                                                                                                                  \
   rpl_result rpl_##KIND##_stream_laserscan_msgs_dev(T* s, const rpl_scan_params* params, int64_t clock_offset_ns,    \
                                                     uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,         \

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "lidar_args.h"
+
 namespace rpl {
 
 struct ScanBatchArgs {
@@ -36,6 +38,12 @@ struct ScanBatchArgs {
   // outputs stay at s * stride.  nodes_total = nodes in the buffer (bulk copies must not run past it).
   const uint2* views;
   unsigned long long nodes_total;
+  // per-stream settings (stream sessions, nullable): scan s takes is_new_protocol, inverted and (LaserScan) its Mode
+  // A / Mode B from lidars[s / lidar_scans] instead of the fields above.  The shared-memory kernels are launched once
+  // per mode in lidar_modes (bit 0 Mode B, bit 1 Mode A) and each serves its own mode's scans; the general kernel
+  // takes every scan's mode from the table.
+  const LidarSettings* lidars;
+  uint32_t lidar_scans, lidar_modes;
 };
 
 // per-CTA global workspace of the general kernel, sized for max_nodes

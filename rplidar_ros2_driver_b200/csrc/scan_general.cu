@@ -97,9 +97,9 @@ __global__ void __launch_bounds__(GT, 1)
   extern __shared__ __align__(16) unsigned char smem_raw[];
   GeneralSmem& sm = *reinterpret_cast<GeneralSmem*>(smem_raw);
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const bool new_proto = a.is_new_protocol != 0;
-  const bool mode_a = a.mode_a != 0;
-  const bool inverted = a.inverted != 0;
+  bool new_proto = a.is_new_protocol != 0;
+  bool mode_a = a.mode_a != 0;
+  bool inverted = a.inverted != 0;
   const bool ascend = a.apply_ascend != 0;
   const bool cloud = a.xyzi != nullptr;  // PointCloud2 payload: window filter + polar->xyz
   const bool want_scan = a.ranges != nullptr || cloud;
@@ -121,6 +121,12 @@ __global__ void __launch_bounds__(GT, 1)
   const uint32_t n_work = all_scans ? a.n_scans : *a.fallback_count;
   for (uint32_t work = blockIdx.x; work < n_work; work += gridDim.x) {
     const uint32_t s = all_scans ? work : a.fallback_list[work];
+    if (a.lidars) {  // the scan's stream's settings (the hand-off list mixes the modes of both shared-memory launches)
+      const LidarSettings& ls = a.lidars[s / a.lidar_scans];
+      new_proto = ls.is_new_protocol != 0;
+      mode_a = ls.mode_a != 0;
+      inverted = ls.inverted != 0;
+    }
     const uint32_t n = a.views ? a.views[s].y : a.counts[s];
     const uint2* base = a.views ? a.nodes + a.views[s].x : a.nodes + (size_t)s * a.stride;
     uint2* nodes_out = a.nodes_out ? a.nodes_out + (size_t)s * a.stride : nullptr;

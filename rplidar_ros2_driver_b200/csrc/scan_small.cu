@@ -311,10 +311,7 @@ __global__ void __launch_bounds__(TS, POST ? 2 : (EMIT ? 4 : (MODE == 0 ? 5 : 1)
 
 
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const bool new_proto = a.is_new_protocol != 0;
-  const bool inverted = a.inverted != 0;
   const uint64_t pol_stream = l2_policy_evict_first();
-  const IntensityOf intensity_of(new_proto);
   const float w_rmin = a.range_min, w_rmax = a.range_max, w_imin = a.intensity_min;
   const bool want_scan = CLOUD ? false : (EMIT ? (a.ranges != nullptr) : true);
 
@@ -326,6 +323,14 @@ __global__ void __launch_bounds__(TS, POST ? 2 : (EMIT ? 4 : (MODE == 0 ? 5 : 1)
   uint32_t parity = 0;
 
   for (uint32_t s = blockIdx.x; s < a.n_scans; s += gridDim.x) {
+    bool new_proto = a.is_new_protocol != 0, inverted = a.inverted != 0;
+    if (a.lidars) {  // the scan's stream's settings; a LaserScan scan of the other mode is the other launch's
+      const LidarSettings& ls = a.lidars[s / a.lidar_scans];
+      if (!CLOUD && (ls.mode_a != 0) != MODE_A) continue;
+      new_proto = ls.is_new_protocol != 0;
+      inverted = ls.inverted != 0;
+    }
+    const IntensityOf intensity_of(new_proto);
     const uint32_t n = a.views ? a.views[s].y : a.counts[s];
     if (n > a.stride || n > p.max_nodes) {  // caller error: report, touch nothing
       if (tid == 0) write_outcome(a, s, kResultInvalidData, 0u, 0.0f);
@@ -1037,18 +1042,26 @@ cudaError_t launch_scan_small(const ScanBatchArgs& a, uint32_t max_nodes, uint32
   const bool cloud = a.xyzi != nullptr;
   const bool emit = !cloud && a.nodes_out != nullptr && a.apply_ascend != 0;
   const bool post = cloud && (sor_k > 0 || voxel > 0.0f);
-  const int mode = cloud ? 2 : (a.mode_a ? 1 : 0);
-  const size_t sh = scan_small_smem_bytes(p.cap, mode, emit, post);
   if (cloud) {
+    const size_t sh = scan_small_smem_bytes(p.cap, 2, false, post);
     if (post) return launch_one<2, false, true, kSmallPostThreads>(a, p, sh, num_sms, stream);
     return launch_one<2, false, false, kSmallThreads>(a, p, sh, num_sms, stream);
   }
-  if (mode == 1) {
-    if (emit) return launch_one<1, true, false, kSmallThreads>(a, p, sh, num_sms, stream);
-    return launch_one<1, false, false, kSmallThreads>(a, p, sh, num_sms, stream);
-  }
-  if (emit) return launch_one<0, true, false, kSmallThreads>(a, p, sh, num_sms, stream);
-  return launch_one<0, false, false, kSmallThreads>(a, p, sh, num_sms, stream);
+  auto launch_mode = [&](int mode) {
+    const size_t sh = scan_small_smem_bytes(p.cap, mode, emit, false);
+    if (mode == 1) {
+      if (emit) return launch_one<1, true, false, kSmallThreads>(a, p, sh, num_sms, stream);
+      return launch_one<1, false, false, kSmallThreads>(a, p, sh, num_sms, stream);
+    }
+    if (emit) return launch_one<0, true, false, kSmallThreads>(a, p, sh, num_sms, stream);
+    return launch_one<0, false, false, kSmallThreads>(a, p, sh, num_sms, stream);
+  };
+  if (!a.lidars) return launch_mode(a.mode_a ? 1 : 0);
+  // per-stream settings: one launch per mode present, each skipping the other mode's scans
+  cudaError_t e = cudaSuccess;
+  for (int mode = 0; mode < 2 && e == cudaSuccess; ++mode)
+    if ((a.lidar_modes >> mode) & 1u) e = launch_mode(mode);
+  return e;
 }
 
 }  // namespace rpl

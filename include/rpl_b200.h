@@ -676,6 +676,58 @@ rpl_result rpl_normal_stream_cloud_dev(rpl_normal_stream* s, const rpl_cloud_par
 rpl_result rpl_normal_stream_cloud(rpl_normal_stream* s, const rpl_cloud_params* params, float* xyzi,
                                    uint32_t* point_counts);
 
+/* Session nodes: the node buffer RealLidarDriver::grab_scan_data returns (src/lidar_driver_wrapper.cpp:307-342) for
+ * every scan the session's last successful push published -- the holder's scan, run through ascendScanData when
+ * angle_compensate is set (:326-329, return value ignored) -- packed one behind the other.
+ *   Which scans, repeat calls, ordering and errors: those of the session clouds above.  Slot i = s * max_scans + k is
+ *            the scan whose LaserScan and scan-begin stamp that push wrote to slot k of stream s.  Every push flavour;
+ *            callable any number of times between that push and the next, a reset in between changes nothing.  Before
+ *            any push, after a push that failed, or with a null nodes, node_offsets, node_counts, status or
+ *            total_nodes: RPL_RESULT_INVALID_DATA.
+ *   Definition: with H the holder's scan (the view's nodes after the assembler's capacity rule), node_counts[i] =
+ *            len(H), 0 for an unused slot.  Where ascend applies to the stream, the buffer is ascendScanData(H) under
+ *            this library's tie rule (equal final keys keep buffer order): bit for bit what rpl_scan_batch_dev writes
+ *            to nodes_out for H with apply_ascend = 1, and on tie-free revolutions the SDK's own result.  status[i] is
+ *            the SDK's return value: RPL_RESULT_OK, or RPL_RESULT_OPERATION_FAIL when H has no measured node, the
+ *            buffer then being H unchanged (src/sdk/src/sl_lidar_driver.cpp:150-151; the wrapper still returns the
+ *            nodes).  Where ascend does not apply, the buffer is H unchanged and the status RPL_RESULT_OK.  A slot
+ *            without a buffer (unused, or every slot when the buffers do not fit) has status RPL_RESULT_OK.
+ *   Which streams are ascended: ascend_per_stream == NULL: every stream iff apply_ascend != 0.  Otherwise stream s iff
+ *            ascend_per_stream[s] != 0 ([n_streams], host memory in both forms), and apply_ascend is ignored:
+ *            angle_compensate is a parameter of each node in the reference (connect(port, baud,
+ *            use_geometric_compensation)).  rpl_lidar_settings.pad plays no part.
+ *   Packing: buffer i starts at nodes + node_offsets[i]; node_offsets [n_streams * max_scans] is the exclusive scan, in
+ *            slot order, of the counts each rounded up to even, so every buffer is 16-byte aligned when nodes is.
+ *            *total_nodes is the end of the last buffer.  When *total_nodes exceeds capacity_nodes nothing is written
+ *            to nodes and every count is 0; *total_nodes still reports the nodes needed (the host form then returns
+ *            RPL_RESULT_INSUFFICIENT_MEMORY).  Nothing at or past nodes + *total_nodes is written; the one padding
+ *            node behind an odd-length buffer is unspecified.
+ *   _dev:    device buffers, asynchronous on `stream` (NULL = the context's stream); nodes 16-byte aligned,
+ *            node_offsets and total_nodes 8-byte, node_counts and status 4-byte aligned, else RPL_RESULT_INVALID_DATA.
+ *            It waits for the session's last push (on any stream) and the session's next push waits for it; its scan
+ *            kernels take turns with every other call of the context on its scan scratch.  No LaserScan is computed
+ *            and nothing a push, a cloud or a message call returned is touched.
+ *   host:    synchronous; copies back the tables, then only total_nodes * 8 bytes of nodes, chunked over the context's
+ *            lanes as the host message calls are. */
+rpl_result rpl_capsule_stream_nodes_dev(rpl_capsule_stream* s, uint32_t apply_ascend,
+    const uint8_t* ascend_per_stream /* nullable, [n_streams], host */, rpl_node_hq* nodes, uint64_t capacity_nodes,
+    uint64_t* node_offsets, uint32_t* node_counts, uint32_t* status, uint64_t* total_nodes, void* stream);
+rpl_result rpl_capsule_stream_nodes(rpl_capsule_stream* s, uint32_t apply_ascend, const uint8_t* ascend_per_stream,
+    rpl_node_hq* nodes, uint64_t capacity_nodes, uint64_t* node_offsets, uint32_t* node_counts, uint32_t* status,
+    uint64_t* total_nodes);
+rpl_result rpl_dense_stream_nodes_dev(rpl_dense_stream* s, uint32_t apply_ascend,
+    const uint8_t* ascend_per_stream /* nullable, [n_streams], host */, rpl_node_hq* nodes, uint64_t capacity_nodes,
+    uint64_t* node_offsets, uint32_t* node_counts, uint32_t* status, uint64_t* total_nodes, void* stream);
+rpl_result rpl_dense_stream_nodes(rpl_dense_stream* s, uint32_t apply_ascend, const uint8_t* ascend_per_stream,
+    rpl_node_hq* nodes, uint64_t capacity_nodes, uint64_t* node_offsets, uint32_t* node_counts, uint32_t* status,
+    uint64_t* total_nodes);
+rpl_result rpl_normal_stream_nodes_dev(rpl_normal_stream* s, uint32_t apply_ascend,
+    const uint8_t* ascend_per_stream /* nullable, [n_streams], host */, rpl_node_hq* nodes, uint64_t capacity_nodes,
+    uint64_t* node_offsets, uint32_t* node_counts, uint32_t* status, uint64_t* total_nodes, void* stream);
+rpl_result rpl_normal_stream_nodes(rpl_normal_stream* s, uint32_t apply_ascend, const uint8_t* ascend_per_stream,
+    rpl_node_hq* nodes, uint64_t capacity_nodes, uint64_t* node_offsets, uint32_t* node_counts, uint32_t* status,
+    uint64_t* total_nodes);
+
 /* Session messages: the serialised sensor_msgs/LaserScan and PointCloud2 (XCDR1, as rpl_*_cdr_batch_dev below) of
  * every scan the session's last successful push published, packed back to back, each ready for
  * rclcpp::SerializedMessage (INTEGRATION.md 4c) -- what scan_pub_->publish (src/rplidar_node.cpp:679) hands the RMW
@@ -778,7 +830,8 @@ rpl_result rpl_normal_stream_cloud_msgs(rpl_normal_stream* s, const rpl_cloud_pa
  *            settings[s].is_new_protocol; before the first set_lidars: RPL_RESULT_INVALID_DATA.
  *   Changes between pushes apply to everything the next push decodes and publishes; a scan-begin stamp a push already
  *   computed (of a revolution still open) keeps its value.  Cloud and message calls read the table as it is when they
- *   are made.  apply_ascend stays a call parameter: it moves only unmeasured nodes, which no session output keeps. */
+ *   are made.  apply_ascend stays a call parameter: it moves only unmeasured nodes, which the session nodes
+ *   (rpl_*_stream_nodes*, below) alone keep, and they take it per call or per stream. */
 typedef struct rpl_lidar_settings {
   uint8_t is_new_protocol; /* as rpl_scan_params */
   uint8_t scan_processing; /* 1 Mode A, 0 Mode B */

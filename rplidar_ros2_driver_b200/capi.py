@@ -62,7 +62,8 @@ EXPORTS = [
     "rpl_capsule_stream_cloud", "rpl_capsule_stream_cloud_dev", "rpl_dense_stream_cloud", "rpl_dense_stream_cloud_dev",
     "rpl_normal_stream_cloud", "rpl_normal_stream_cloud_dev",
     *[f"rpl_{kind}_stream_{fn}" for kind in ("capsule", "dense", "normal")
-      for fn in ("set_frames", "set_lidars", "laserscan_msgs", "laserscan_msgs_dev", "cloud_msgs", "cloud_msgs_dev")],
+      for fn in ("set_frames", "set_lidars", "laserscan_msgs", "laserscan_msgs_dev", "cloud_msgs", "cloud_msgs_dev",
+                 "nodes", "nodes_dev")],
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -250,6 +251,8 @@ def lib() -> C.CDLL:
         sig[f"rpl_{kind}_stream_laserscan_msgs_dev"] = ([vp, PSP, C.c_int64, vp, u64, vp, vp, vp, vp], u32)
         sig[f"rpl_{kind}_stream_cloud_msgs"] = ([vp, PCP, C.c_int64, vp, u64, vp, vp, vp], u32)
         sig[f"rpl_{kind}_stream_cloud_msgs_dev"] = ([vp, PCP, C.c_int64, vp, u64, vp, vp, vp, vp], u32)
+        sig[f"rpl_{kind}_stream_nodes"] = ([vp, u32, vp, vp, u64, vp, vp, vp, vp], u32)
+        sig[f"rpl_{kind}_stream_nodes_dev"] = ([vp, u32, vp, vp, u64, vp, vp, vp, vp, vp], u32)
     for name, (args, res) in sig.items():
         fn = getattr(L, name)  # AttributeError here = the library does not export the ABI
         fn.argtypes = args
@@ -781,6 +784,41 @@ class CapsuleStreamSession:
         self._ctx._check(self._fn("cloud_msgs_dev")(self._h, C.byref(params), int(clock_offset_ns), _p(msgs),
                                                      int(capacity), _p(msg_offsets), _p(msg_sizes), _p(total_bytes),
                                                      _p(stream)))
+
+    def nodes(self, apply_ascend=True, per_stream=None, packed=False, nodes=None):
+        """The node buffers RealLidarDriver::grab_scan_data would return for every scan the last push published: per
+        slot (n_streams * max_scans) an array of NODE_DTYPE (empty for an unused slot), ascended when apply_ascend, or,
+        with per_stream ([n_streams] flags), where the stream's flag is set.  nodes: the host buffer to pack into
+        (None: one that always fits).  packed: return {"nodes", "node_offsets", "node_counts", "status",
+        "total_nodes", "result"} instead, with result RESULT_INSUFFICIENT_MEMORY rather than an exception when nodes is
+        too small; otherwise (buffers, status)."""
+        ns = self.n_streams * self.max_scans
+        if nodes is None:
+            nodes = np.zeros(ns * self.max_nodes, NODE_DTYPE)
+        assert nodes.dtype == NODE_DTYPE and nodes.flags.c_contiguous
+        m = None if per_stream is None else np.ascontiguousarray(per_stream, dtype=np.uint8)
+        assert m is None or m.shape == (self.n_streams,)
+        offs, counts, status = np.zeros(ns, np.uint64), np.zeros(ns, np.uint32), np.zeros(ns, np.uint32)
+        total = np.zeros(1, np.uint64)
+        rc = self._fn("nodes")(self._h, int(bool(apply_ascend)), _p(m), _p(nodes), nodes.size, _p(offs), _p(counts),
+                               _p(status), _p(total))
+        if not packed or rc != RESULT_INSUFFICIENT_MEMORY:
+            self._ctx._check(rc)
+        if packed:
+            return dict(nodes=nodes, node_offsets=offs, node_counts=counts, status=status, total_nodes=int(total[0]),
+                        result=rc)
+        return [nodes[o: o + n] for o, n in zip(offs.tolist(), counts.tolist())], status
+
+    def nodes_dev(self, nodes, capacity_nodes, node_offsets, node_counts, status, total_nodes, apply_ascend=True,
+                  per_stream=None, stream=None):
+        """Device addresses (nodes [capacity_nodes] 8-byte nodes, node_offsets [n_streams * max_scans] uint64,
+        node_counts and status uint32, total_nodes one uint64; per_stream a host array), asynchronous on `stream`
+        (None: the context's stream)."""
+        m = None if per_stream is None else np.ascontiguousarray(per_stream, dtype=np.uint8)
+        assert m is None or m.shape == (self.n_streams,)
+        self._ctx._check(self._fn("nodes_dev")(self._h, int(bool(apply_ascend)), _p(m), _p(nodes), int(capacity_nodes),
+                                               _p(node_offsets), _p(node_counts), _p(status), _p(total_nodes),
+                                               _p(stream)))
 
     def reset(self, mask=None):
         """Drops the held capsule, the decoder state and the open revolution of the streams where mask is true

@@ -18,6 +18,7 @@
 #include "cdr_args.h"
 #include "decode_args.h"
 #include "scan_args.h"
+#include "session_nodes_args.h"
 
 namespace rpl {
 cudaError_t launch_synth(uint64_t first_scan_id, uint32_t n_scans, uint32_t n, uint32_t stride,
@@ -1236,6 +1237,7 @@ struct rpl_capsule_stream {
   rpl::LidarSettings* lidars = nullptr;         // [n_streams] device
   std::vector<rpl::LidarSettings> lidars_host;
   uint32_t lidar_modes = 0;                     // LidarTable::modes of the table
+  unsigned char* node_work = nullptr;           // the tables of a nodes call (NodeWork)
 };
 
 static_assert(sizeof(rpl::LidarSettings) == sizeof(rpl_lidar_settings) &&
@@ -1511,6 +1513,24 @@ rpl_result push_host(rpl_ctx* c, const HostWire& h, uint32_t n_streams, uint32_t
   return run_chunks(c, n_streams, chunk, run_chunk);
 }
 
+// The tables of a nodes call (rpl_*_stream_nodes*), the session's own: every slot's place for the kernels, the
+// per-stream ascend flags, and the host form's directory, which the device form writes into the caller's arrays.
+struct NodeWork {
+  unsigned long long *place, *offsets, *total;
+  uint32_t *counts, *status;
+  uint8_t* ascend;
+};
+NodeWork node_work_layout(const rpl_capsule_stream* cs, Carve& k) {
+  const size_t NS = (size_t)cs->n_streams * cs->max_scans;
+  return NodeWork{k.take<unsigned long long>(NS), k.take<unsigned long long>(NS), k.take<unsigned long long>(1),
+                  k.take<uint32_t>(NS), k.take<uint32_t>(NS), k.take<uint8_t>(cs->n_streams)};
+}
+size_t node_work_bytes(const rpl_capsule_stream* cs) {
+  Carve k;
+  node_work_layout(cs, k);
+  return k.bytes;
+}
+
 // a call with RPL_FLAG_PER_STREAM / RPL_CLOUD_PER_STREAM needs the table
 bool lidars_ok(rpl_capsule_stream* cs) {
   if (!cs->lidars_host.empty()) return true;
@@ -1648,7 +1668,8 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint
       !cuda_ok(c, dev_alloc(&cs->views, n * max_scans), "cudaMalloc") ||
       !cuda_ok(c, dev_alloc(&cs->slot_begin, n * max_scans), "cudaMalloc") ||
       !cuda_ok(c, dev_alloc(&cs->slot_end, n * max_scans), "cudaMalloc") ||
-      !cuda_ok(c, dev_alloc(&cs->msg_hdr, n), "cudaMalloc"))
+      !cuda_ok(c, dev_alloc(&cs->msg_hdr, n), "cudaMalloc") ||
+      !cuda_ok(c, dev_alloc(&cs->node_work, node_work_bytes(cs)), "cudaMalloc"))
     return fail(oom);
   // the reference's defaults: frame_id "laser_frame" (rplidar_node.cpp:80), range_max 12 m (rplidar_node.hpp:328)
   cs->msg_hdr_host.assign(n, msg_header("laser_frame", 11, 12.0f));
@@ -2228,6 +2249,186 @@ rpl_result stream_msgs(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* pa
   return run_chunks(c, cs->n_streams, chunk, run_chunk);
 }
 
+// ---- grabbed node buffers of the last push (DESIGN.md 5.7.1 "Session nodes") -------------------------------------
+// Per call: the directory over every slot (counts, packed offsets, each slot's place), then per chunk of the push the
+// shared-memory EMIT kernel with the general kernel behind it for the ascended slots, writing each revolution at its
+// place, and the gather for the others.  The device form places into the caller's buffer; the host form reads the
+// directory back first and then places and copies chunk by chunk over the lanes, each chunk's buffers being one
+// stretch of the packed buffer, so that only node bytes cross the link.
+
+bool stream_nodes_args_ok(rpl_capsule_stream* cs, const void* nodes, const void* offsets, const void* counts,
+                          const void* status, const void* total, bool dev) {
+  rpl_ctx* c = cs->c;
+  if (!nodes || !offsets || !counts || !status || !total) {
+    c->err = "null nodes, node_offsets, node_counts, status or total_nodes";
+    return false;
+  }
+  auto mis4 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3u) != 0; };
+  if (dev && ((reinterpret_cast<uintptr_t>(nodes) & 15u) || misaligned8(offsets) || misaligned8(total) || mis4(counts) ||
+              mis4(status))) {
+    c->err = "nodes must be 16-byte aligned, node_offsets and total_nodes 8-byte, node_counts and status 4-byte aligned";
+    return false;
+  }
+  if (cs->cloud_chunk == 0) {
+    c->err = "no nodes to take: the session has not pushed yet, or its last push failed";
+    return false;
+  }
+  return true;
+}
+
+// which kernels a nodes call needs: the scan kernels (some stream is ascended), the gather (some stream is not)
+struct NodeKinds {
+  bool ascended, passed;
+};
+NodeKinds node_kinds(const rpl_capsule_stream* cs, uint32_t apply_ascend, const uint8_t* per_stream) {
+  if (!per_stream) return NodeKinds{apply_ascend != 0, apply_ascend == 0};
+  NodeKinds k{false, false};
+  for (uint32_t s = 0; s < cs->n_streams; ++s) (per_stream[s] ? k.ascended : k.passed) = true;
+  return k;
+}
+
+// on `st`, after the last push: the per-stream flags to the device, then the directory of every slot
+rpl_result nodes_prepare(rpl_capsule_stream* cs, const NodeWork& w, uint32_t apply_ascend, const uint8_t* per_stream,
+                         unsigned long long capacity, unsigned long long* offsets, uint32_t* counts, uint32_t* status,
+                         unsigned long long* total, bool rebase, cudaStream_t st) {
+  rpl_ctx* c = cs->c;
+  if (per_stream)
+    RPL_CUDA(c, cudaMemcpyAsync(w.ascend, per_stream, cs->n_streams, cudaMemcpyHostToDevice, st), RPL_RESULT_OPERATION_FAIL);
+  rpl::NodeDirArgs a{};
+  a.views = reinterpret_cast<const uint2*>(cs->views);
+  a.n_slots = cs->n_streams * cs->max_scans;
+  a.max_scans = cs->max_scans;
+  a.chunk_slots = cs->cloud_chunk * cs->max_scans;
+  a.rebase = rebase ? 1u : 0u;
+  a.ascend = per_stream ? w.ascend : nullptr;
+  a.ascend_all = apply_ascend;
+  a.capacity = capacity;
+  a.offsets = offsets;
+  a.counts = counts;
+  a.status = status;
+  a.total = total;
+  a.place = w.place;
+  RPL_CUDA(c, rpl::launch_node_directory(a, st), RPL_RESULT_OPERATION_FAIL);
+  c->launches++;
+  return RPL_RESULT_OK;
+}
+
+// The buffers of the scans of streams [s0, s0 + ns), one chunk of the last push (its views count from node 0 of stream
+// s0 in the push's arena), placed behind `out`; status points at the chunk's first slot.  One EMIT instantiation
+// serves every ascended slot: the ascended buffer does not depend on the LaserScan mode, and no LaserScan is computed.
+rpl_result stream_nodes_chunk(rpl_capsule_stream* cs, Lane& l, uint32_t s0, uint32_t ns, NodeKinds kinds,
+                              const unsigned long long* place, rpl_node_hq* out, uint32_t* status, cudaStream_t st) {
+  rpl_ctx* c = cs->c;
+  const size_t so = (size_t)s0 * cs->max_scans;
+  rpl::ScanBatchArgs a{};
+  a.nodes = reinterpret_cast<const uint2*>(cs->arena[cs->cloud_arena] + (size_t)s0 * cs->stride_nodes);
+  a.views = reinterpret_cast<const uint2*>(cs->views + so);
+  a.counts = reinterpret_cast<const uint32_t*>(a.views);
+  a.nodes_total = (unsigned long long)ns * cs->stride_nodes;
+  a.n_scans = ns * cs->max_scans;
+  a.stride = cs->max_nodes;
+  a.nodes_out = reinterpret_cast<uint2*>(out);
+  a.out_first = place + so;
+  a.status = status;
+  a.apply_ascend = 1;
+  a.fallback_list = l.fallback_list;
+  a.fallback_count = l.fallback_count;
+  if (kinds.ascended) {
+    rpl_result r = scratch_enter(c, l, st);
+    if (r == RPL_RESULT_OK) r = enqueue_args(c, l, a, 0u, st);
+    if (r == RPL_RESULT_OK) r = scratch_leave(c, l, st);
+    if (r != RPL_RESULT_OK) return r;
+  }
+  if (kinds.passed) {
+    const rpl::NodeGatherArgs g{a.nodes, a.views, a.out_first, a.n_scans, a.nodes_out};
+    RPL_CUDA(c, rpl::launch_node_gather(g, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+    c->launches++;
+  }
+  return RPL_RESULT_OK;
+}
+
+rpl_result stream_nodes_dev(rpl_capsule_stream* cs, uint32_t apply_ascend, const uint8_t* per_stream, rpl_node_hq* nodes,
+                            uint64_t capacity, uint64_t* node_offsets, uint32_t* node_counts, uint32_t* status,
+                            uint64_t* total_nodes, void* stream) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!stream_nodes_args_ok(cs, nodes, node_offsets, node_counts, status, total_nodes, true)) return RPL_RESULT_INVALID_DATA;
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
+  Carve k{cs->node_work};
+  const NodeWork w = node_work_layout(cs, k);
+  // the last push's kernels (and an earlier nodes call's, which read the same tables) are done before these; the next
+  // push waits for these
+  RPL_CUDA(c, cudaStreamWaitEvent(st, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
+  rpl_result r = nodes_prepare(cs, w, apply_ascend, per_stream, capacity, reinterpret_cast<unsigned long long*>(node_offsets),
+                               node_counts, status, reinterpret_cast<unsigned long long*>(total_nodes), false, st);
+  const NodeKinds kinds = node_kinds(cs, apply_ascend, per_stream);
+  for (uint32_t s0 = 0; s0 < cs->n_streams && r == RPL_RESULT_OK; s0 += cs->cloud_chunk)
+    r = stream_nodes_chunk(cs, c->lane[0], s0, std::min(cs->cloud_chunk, cs->n_streams - s0), kinds, w.place, nodes,
+                           status + (size_t)s0 * cs->max_scans, st);
+  RPL_CUDA(c, cudaEventRecord(cs->done, st), RPL_RESULT_OPERATION_FAIL);
+  return r;
+}
+
+rpl_result stream_nodes(rpl_capsule_stream* cs, uint32_t apply_ascend, const uint8_t* per_stream, rpl_node_hq* nodes,
+                        uint64_t capacity, uint64_t* node_offsets, uint32_t* node_counts, uint32_t* status,
+                        uint64_t* total_nodes) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!stream_nodes_args_ok(cs, nodes, node_offsets, node_counts, status, total_nodes, false)) return RPL_RESULT_INVALID_DATA;
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  Carve k{cs->node_work};
+  const NodeWork w = node_work_layout(cs, k);
+  const uint32_t NS = cs->n_streams * cs->max_scans;
+  cudaStream_t st = c->lane[0].stream;
+  for (int i = 0; i < kLanes; ++i) RPL_CUDA(c, cudaStreamWaitEvent(c->lane[i].stream, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
+  const rpl_result p = nodes_prepare(cs, w, apply_ascend, per_stream, capacity, w.offsets, w.counts, w.status, w.total, true, st);
+  if (p != RPL_RESULT_OK) {
+    cudaStreamSynchronize(st);
+    return p;
+  }
+  const cudaMemcpyKind d2h = cudaMemcpyDeviceToHost;
+  RPL_CUDA(c, cudaMemcpyAsync(node_offsets, w.offsets, (size_t)NS * 8, d2h, st), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaMemcpyAsync(node_counts, w.counts, (size_t)NS * 4, d2h, st), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaMemcpyAsync(status, w.status, (size_t)NS * 4, d2h, st), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaMemcpyAsync(total_nodes, w.total, 8, d2h, st), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);
+  const uint64_t total = *total_nodes;
+  if (total > capacity) {
+    c->err = "the buffers need more than capacity_nodes nodes (total_nodes tells how many)";
+    return RPL_RESULT_INSUFFICIENT_MEMORY;
+  }
+  // the chunks of the last push: each one's buffers are one stretch [lo, hi) of the packed buffer, in nodes
+  const uint32_t chunk = cs->cloud_chunk;
+  auto stretch = [&](uint32_t s0, uint32_t ns) {
+    const uint32_t i0 = s0 * cs->max_scans, i1 = (s0 + ns) * cs->max_scans;
+    const uint64_t hi = i1 < NS ? std::min<uint64_t>(node_offsets[i1], total) : total;
+    return std::make_pair(std::min<uint64_t>(node_offsets[i0], hi), hi);
+  };
+  size_t most = 0;
+  for (uint32_t s0 = 0; s0 < cs->n_streams; s0 += chunk) {
+    const auto [lo, hi] = stretch(s0, std::min(chunk, cs->n_streams - s0));
+    most = std::max<size_t>(most, hi - lo);
+  }
+  if (const rpl_result g = grow_stage(c, kLanes, [&](Carve& s) { s.take<rpl_node_hq>(most); }); g != RPL_RESULT_OK) return g;
+  const NodeKinds kinds = node_kinds(cs, apply_ascend, per_stream);
+  auto run_chunk = [&](Lane& l, uint32_t s0, uint32_t ns) -> rpl_result {
+    const auto [lo, hi] = stretch(s0, ns);
+    if (hi == lo) return RPL_RESULT_OK;  // no buffer in this chunk: the directory's statuses stand
+    const size_t so = (size_t)s0 * cs->max_scans;
+    RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);  // the lane's previous chunk has left
+    rpl_node_hq* stage = reinterpret_cast<rpl_node_hq*>(l.stage);
+    const rpl_result r = stream_nodes_chunk(cs, l, s0, ns, kinds, w.place, stage, w.status + so, l.stream);
+    if (r != RPL_RESULT_OK) return r;
+    RPL_CUDA(c, cudaMemcpyAsync(nodes + lo, stage, (hi - lo) * sizeof(rpl_node_hq), d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
+    if (kinds.ascended)
+      RPL_CUDA(c, cudaMemcpyAsync(status + so, w.status + so, (size_t)ns * cs->max_scans * 4, d2h, l.stream),
+               RPL_RESULT_OPERATION_FAIL);
+    return RPL_RESULT_OK;
+  };
+  return run_chunks(c, cs->n_streams, chunk, run_chunk);
+}
+
 }  // namespace
 
 extern "C" {
@@ -2329,6 +2530,7 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   cudaFree(cs->slot_end);
   cudaFree(cs->msg_hdr);
   cudaFree(cs->msg_work);
+  cudaFree(cs->node_work);
   cudaFree(cs->lidars);
   if (cs->done) cudaEventDestroy(cs->done);
   delete cs;
@@ -2604,6 +2806,42 @@ rpl_result rpl_normal_stream_state(rpl_normal_stream* ns, uint32_t* open_nodes, 
 }
 
 // ---- session clouds: the PointCloud2 chain over the scans the last push published, read in place ----
+rpl_result rpl_capsule_stream_nodes_dev(rpl_capsule_stream* cs, uint32_t apply_ascend, const uint8_t* ascend_per_stream,
+                                        rpl_node_hq* nodes, uint64_t capacity_nodes, uint64_t* node_offsets,
+                                        uint32_t* node_counts, uint32_t* status, uint64_t* total_nodes, void* stream) {
+  return stream_nodes_dev(cs, apply_ascend, ascend_per_stream, nodes, capacity_nodes, node_offsets, node_counts, status,
+                          total_nodes, stream);
+}
+rpl_result rpl_capsule_stream_nodes(rpl_capsule_stream* cs, uint32_t apply_ascend, const uint8_t* ascend_per_stream,
+                                    rpl_node_hq* nodes, uint64_t capacity_nodes, uint64_t* node_offsets,
+                                    uint32_t* node_counts, uint32_t* status, uint64_t* total_nodes) {
+  return stream_nodes(cs, apply_ascend, ascend_per_stream, nodes, capacity_nodes, node_offsets, node_counts, status,
+                      total_nodes);
+}
+rpl_result rpl_dense_stream_nodes_dev(rpl_dense_stream* ds, uint32_t apply_ascend, const uint8_t* ascend_per_stream,
+                                        rpl_node_hq* nodes, uint64_t capacity_nodes, uint64_t* node_offsets,
+                                        uint32_t* node_counts, uint32_t* status, uint64_t* total_nodes, void* stream) {
+  return stream_nodes_dev(capsule_session(ds), apply_ascend, ascend_per_stream, nodes, capacity_nodes, node_offsets, node_counts, status,
+                          total_nodes, stream);
+}
+rpl_result rpl_dense_stream_nodes(rpl_dense_stream* ds, uint32_t apply_ascend, const uint8_t* ascend_per_stream,
+                                    rpl_node_hq* nodes, uint64_t capacity_nodes, uint64_t* node_offsets,
+                                    uint32_t* node_counts, uint32_t* status, uint64_t* total_nodes) {
+  return stream_nodes(capsule_session(ds), apply_ascend, ascend_per_stream, nodes, capacity_nodes, node_offsets, node_counts, status,
+                      total_nodes);
+}
+rpl_result rpl_normal_stream_nodes_dev(rpl_normal_stream* ns, uint32_t apply_ascend, const uint8_t* ascend_per_stream,
+                                        rpl_node_hq* nodes, uint64_t capacity_nodes, uint64_t* node_offsets,
+                                        uint32_t* node_counts, uint32_t* status, uint64_t* total_nodes, void* stream) {
+  return stream_nodes_dev(capsule_session(ns), apply_ascend, ascend_per_stream, nodes, capacity_nodes, node_offsets, node_counts, status,
+                          total_nodes, stream);
+}
+rpl_result rpl_normal_stream_nodes(rpl_normal_stream* ns, uint32_t apply_ascend, const uint8_t* ascend_per_stream,
+                                    rpl_node_hq* nodes, uint64_t capacity_nodes, uint64_t* node_offsets,
+                                    uint32_t* node_counts, uint32_t* status, uint64_t* total_nodes) {
+  return stream_nodes(capsule_session(ns), apply_ascend, ascend_per_stream, nodes, capacity_nodes, node_offsets, node_counts, status,
+                      total_nodes);
+}
 rpl_result rpl_capsule_stream_cloud_dev(rpl_capsule_stream* cs, const rpl_cloud_params* params, float* xyzi,
                                         uint32_t* point_counts, void* stream) {
   return stream_cloud_dev(cs, params, xyzi, point_counts, stream);

@@ -44,7 +44,13 @@ struct ScanBatchArgs {
   // takes every scan's mode from the table.
   const LidarSettings* lidars;
   uint32_t lidar_scans, lidar_modes;
+  // placed ascended buffers (session nodes, nullable; the shared-memory EMIT kernels and the general kernel): scan s
+  // writes its buffer at nodes_out + out_first[s] instead of nodes_out + s * stride.  An entry with kOutSkip set is
+  // not this launch's scan: the kernels leave it before they read its nodes and write nothing for it, status included.
+  // (The last member: the argument offsets of the kernels that do not read it stay what they were.)
+  const unsigned long long* out_first;
 };
+constexpr unsigned long long kOutSkip = 1ull << 63;
 
 // per-CTA global workspace of the general kernel, sized for max_nodes
 struct GeneralWorkspace {

@@ -24,6 +24,14 @@ __device__ __forceinline__ void write_outcome(const ScanBatchArgs& a, uint32_t s
 __device__ __forceinline__ void write_outcome_empty(const ScanBatchArgs& a, uint32_t s) {
   write_outcome(a, s, a.apply_ascend ? kResultOperationFail : kResultOk, 0u, 0.0f);
 }
+// where scan s's ascended buffer goes: its row, or its placed position (ScanBatchArgs::out_first)
+__device__ __forceinline__ uint2* nodes_out_of(const ScanBatchArgs& a, uint32_t s) {
+  return a.nodes_out + (a.out_first ? (size_t)a.out_first[s] : (size_t)s * a.stride);
+}
+// a placed launch's scan that is another kernel's (or nobody's): nothing is read or written for it
+__device__ __forceinline__ bool out_skipped(const ScanBatchArgs& a, uint32_t s) {
+  return a.out_first && (a.out_first[s] & kOutSkip) != 0;
+}
 // scan s goes to the general kernel, which runs after this one and follows the stable tie rule
 __device__ __forceinline__ void hand_to_general(const ScanBatchArgs& a, uint32_t s) {
   a.fallback_list[atomicAdd(a.fallback_count, 1u)] = s;

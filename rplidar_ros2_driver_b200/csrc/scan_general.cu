@@ -121,6 +121,7 @@ __global__ void __launch_bounds__(GT, 1)
   const uint32_t n_work = all_scans ? a.n_scans : *a.fallback_count;
   for (uint32_t work = blockIdx.x; work < n_work; work += gridDim.x) {
     const uint32_t s = all_scans ? work : a.fallback_list[work];
+    if (a.out_first && (a.out_first[s] & kOutSkip) != 0) continue;  // a placed launch: not a scan of the scan kernels
     if (a.lidars) {  // the scan's stream's settings (the hand-off list mixes the modes of both shared-memory launches)
       const LidarSettings& ls = a.lidars[s / a.lidar_scans];
       new_proto = ls.is_new_protocol != 0;
@@ -129,7 +130,8 @@ __global__ void __launch_bounds__(GT, 1)
     }
     const uint32_t n = a.views ? a.views[s].y : a.counts[s];
     const uint2* base = a.views ? a.nodes + a.views[s].x : a.nodes + (size_t)s * a.stride;
-    uint2* nodes_out = a.nodes_out ? a.nodes_out + (size_t)s * a.stride : nullptr;
+    uint2* nodes_out =
+        a.nodes_out ? a.nodes_out + (a.out_first ? (size_t)a.out_first[s] : (size_t)s * a.stride) : nullptr;
 
     if (n > a.stride || n > ws.max_nodes) {  // caller error: report, touch nothing
       if (tid == 0) {

@@ -323,6 +323,7 @@ __global__ void __launch_bounds__(TS, POST ? 2 : (EMIT ? 4 : (MODE == 0 ? 5 : 1)
   uint32_t parity = 0;
 
   for (uint32_t s = blockIdx.x; s < a.n_scans; s += gridDim.x) {
+    if (EMIT && out_skipped(a, s)) continue;
     bool new_proto = a.is_new_protocol != 0, inverted = a.inverted != 0;
     if (a.lidars) {  // the scan's stream's settings; a LaserScan scan of the other mode is the other launch's
       const LidarSettings& ls = a.lidars[s / a.lidar_scans];
@@ -453,7 +454,7 @@ __global__ void __launch_bounds__(TS, POST ? 2 : (EMIT ? 4 : (MODE == 0 ? 5 : 1)
     if (M == 0) {
       if (tid == 0) write_outcome_empty(a, s);
       if (EMIT) {
-        uint2* out = a.nodes_out + (size_t)s * a.stride;
+        uint2* out = nodes_out_of(a, s);
         for (uint32_t i = tid; i < n; i += TS) out[i] = tile[i];
       }
       __syncthreads();
@@ -582,7 +583,7 @@ __global__ void __launch_bounds__(TS, POST ? 2 : (EMIT ? 4 : (MODE == 0 ? 5 : 1)
     float* ranges = want_scan ? a.ranges + (size_t)s * a.stride : nullptr;
     float* intens = want_scan ? a.intensities + (size_t)s * a.stride : nullptr;
     float4* cloud = CLOUD ? a.xyzi + (size_t)s * a.stride : nullptr;
-    uint2* nodes_out = EMIT ? a.nodes_out + (size_t)s * a.stride : nullptr;
+    uint2* nodes_out = EMIT ? nodes_out_of(a, s) : nullptr;
     const float inc = angle_increment(M, MODE_A);
     const ModeBOut mode_b(ranges, intens, M, inverted);
     // (two instances: revolutions with shared final keys are rare and must not slow the loop of the others down)

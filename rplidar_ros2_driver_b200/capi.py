@@ -50,20 +50,15 @@ EXPORTS = [
     "rpl_decode_dense_batch_dev", "rpl_decode_dense", "rpl_assemble_scans_dev", "rpl_assemble_scan_views_dev",
     "rpl_scan_views_dev", "rpl_chain_dense_laserscan", "rpl_decode_dense_batch_starts_dev",
     "rpl_assemble_scan_views_starts_dev",
-    "rpl_dense_stream_create", "rpl_dense_stream_destroy", "rpl_dense_stream_push", "rpl_dense_stream_push_dev",
-    "rpl_dense_stream_reset", "rpl_dense_stream_state", "rpl_dense_stream_push_ts", "rpl_dense_stream_push_ts_dev",
     "rpl_capsule_stream_create", "rpl_capsule_stream_destroy", "rpl_capsule_stream_push", "rpl_capsule_stream_push_dev",
     "rpl_capsule_stream_reset", "rpl_capsule_stream_state", "rpl_capsule_stream_push_ts",
     "rpl_capsule_stream_push_ts_dev",
     "rpl_capsule_stream_create_bytes", "rpl_capsule_stream_push_bytes", "rpl_capsule_stream_push_bytes_dev",
-    "rpl_capsule_stream_push_bytes_ts", "rpl_capsule_stream_push_bytes_ts_dev", "rpl_capsule_stream_state_bytes",
-    "rpl_normal_stream_create", "rpl_normal_stream_destroy", "rpl_normal_stream_push", "rpl_normal_stream_push_dev",
-    "rpl_normal_stream_reset", "rpl_normal_stream_state", "rpl_normal_stream_push_ts", "rpl_normal_stream_push_ts_dev",
-    "rpl_capsule_stream_cloud", "rpl_capsule_stream_cloud_dev", "rpl_dense_stream_cloud", "rpl_dense_stream_cloud_dev",
-    "rpl_normal_stream_cloud", "rpl_normal_stream_cloud_dev",
-    *[f"rpl_{kind}_stream_{fn}" for kind in ("capsule", "dense", "normal")
-      for fn in ("set_frames", "set_lidars", "laserscan_msgs", "laserscan_msgs_dev", "cloud_msgs", "cloud_msgs_dev",
-                 "nodes", "nodes_dev")],
+    "rpl_capsule_stream_push_bytes_ts", "rpl_capsule_stream_push_bytes_ts_dev",
+    "rpl_capsule_stream_cloud", "rpl_capsule_stream_cloud_dev", "rpl_capsule_stream_set_frames",
+    "rpl_capsule_stream_set_lidars", "rpl_capsule_stream_laserscan_msgs", "rpl_capsule_stream_laserscan_msgs_dev",
+    "rpl_capsule_stream_cloud_msgs", "rpl_capsule_stream_cloud_msgs_dev", "rpl_capsule_stream_nodes",
+    "rpl_capsule_stream_nodes_dev",
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -211,48 +206,30 @@ def lib() -> C.CDLL:
         "rpl_chain_dense_laserscan": ([vp, vp, vp, u32, u32, u32, PSP, u32, u32, vp, vp, vp, vp, vp], u32),
         "rpl_decode_dense_batch_starts_dev": ([vp, vp, vp, u32, u32, u32, vp, vp, vp, vp, vp, vp, vp, u32, vp, vp], u32),
         "rpl_assemble_scan_views_starts_dev": ([vp, vp, vp, u32, u32, vp, vp, vp, u32, vp, u32, vp, u32, u32, vp, vp, vp, vp, vp, vp], u32),
-        "rpl_dense_stream_create": ([vp, u32, u32, u32, u32, C.POINTER(vp)], u32),
-        "rpl_dense_stream_destroy": ([vp], None),
-        "rpl_dense_stream_push": ([vp, vp, vp, u32, PSP, vp, vp, vp, vp, vp], u32),
-        "rpl_dense_stream_push_dev": ([vp, vp, vp, u32, PSP, vp, vp, vp, vp, vp, vp], u32),
-        "rpl_dense_stream_reset": ([vp, vp], u32),
-        "rpl_dense_stream_state": ([vp, vp, vp], u32),
         "rpl_capsule_stream_create": ([vp, u32, u32, u32, u32, u32, C.POINTER(vp)], u32),
         "rpl_capsule_stream_destroy": ([vp], None),
         "rpl_capsule_stream_push": ([vp, vp, vp, u32, PSP, vp, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_push_dev": ([vp, vp, vp, u32, PSP, vp, vp, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_reset": ([vp, vp], u32),
-        "rpl_capsule_stream_state": ([vp, vp, vp], u32),
-        "rpl_normal_stream_create": ([vp, u32, u32, u32, u32, C.POINTER(vp)], u32),
-        "rpl_normal_stream_destroy": ([vp], None),
-        "rpl_normal_stream_push": ([vp, vp, vp, PSP, vp, vp, vp, vp, vp], u32),
-        "rpl_normal_stream_push_dev": ([vp, vp, vp, PSP, vp, vp, vp, vp, vp, vp], u32),
-        "rpl_normal_stream_reset": ([vp, vp], u32),
-        "rpl_normal_stream_state": ([vp, vp, vp], u32),
+        "rpl_capsule_stream_state": ([vp, vp, vp, vp], u32),
         "rpl_capsule_stream_push_ts": ([vp, vp, vp, PT, vp, PSP, vp, vp, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_push_ts_dev": ([vp, vp, vp, PT, vp, PSP, vp, vp, vp, vp, vp, vp, vp], u32),
-        "rpl_dense_stream_push_ts": ([vp, vp, vp, PT, vp, PSP, vp, vp, vp, vp, vp, vp], u32),
-        "rpl_dense_stream_push_ts_dev": ([vp, vp, vp, PT, vp, PSP, vp, vp, vp, vp, vp, vp, vp], u32),
-        "rpl_normal_stream_push_ts": ([vp, vp, vp, PT, u32, vp, PSP, vp, vp, vp, vp, vp, vp], u32),
-        "rpl_normal_stream_push_ts_dev": ([vp, vp, vp, PT, u32, vp, PSP, vp, vp, vp, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_create_bytes": ([vp, u32, u32, u32, u32, u32, C.POINTER(vp)], u32),
         "rpl_capsule_stream_push_bytes": ([vp, vp, vp, u32, PSP, vp, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_push_bytes_dev": ([vp, vp, vp, u32, PSP, vp, vp, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_push_bytes_ts": ([vp, vp, vp, PT, u32, vp, PSP, vp, vp, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_push_bytes_ts_dev": ([vp, vp, vp, PT, u32, vp, PSP, vp, vp, vp, vp, vp, vp, vp], u32),
-        "rpl_capsule_stream_state_bytes": ([vp, vp, vp, vp], u32),
+        "rpl_capsule_stream_cloud": ([vp, PCP, vp, vp], u32),
+        "rpl_capsule_stream_cloud_dev": ([vp, PCP, vp, vp, vp], u32),
+        "rpl_capsule_stream_set_frames": ([vp, vp, vp], u32),
+        "rpl_capsule_stream_set_lidars": ([vp, vp, vp], u32),
+        "rpl_capsule_stream_laserscan_msgs": ([vp, PSP, C.c_int64, vp, u64, vp, vp, vp], u32),
+        "rpl_capsule_stream_laserscan_msgs_dev": ([vp, PSP, C.c_int64, vp, u64, vp, vp, vp, vp], u32),
+        "rpl_capsule_stream_cloud_msgs": ([vp, PCP, C.c_int64, vp, u64, vp, vp, vp], u32),
+        "rpl_capsule_stream_cloud_msgs_dev": ([vp, PCP, C.c_int64, vp, u64, vp, vp, vp, vp], u32),
+        "rpl_capsule_stream_nodes": ([vp, u32, vp, vp, u64, vp, vp, vp, vp], u32),
+        "rpl_capsule_stream_nodes_dev": ([vp, u32, vp, vp, u64, vp, vp, vp, vp, vp], u32),
     }
-    for kind in ("capsule", "dense", "normal"):
-        sig[f"rpl_{kind}_stream_cloud"] = ([vp, PCP, vp, vp], u32)
-        sig[f"rpl_{kind}_stream_cloud_dev"] = ([vp, PCP, vp, vp, vp], u32)
-        sig[f"rpl_{kind}_stream_set_frames"] = ([vp, vp, vp], u32)
-        sig[f"rpl_{kind}_stream_set_lidars"] = ([vp, vp, vp], u32)
-        sig[f"rpl_{kind}_stream_laserscan_msgs"] = ([vp, PSP, C.c_int64, vp, u64, vp, vp, vp], u32)
-        sig[f"rpl_{kind}_stream_laserscan_msgs_dev"] = ([vp, PSP, C.c_int64, vp, u64, vp, vp, vp, vp], u32)
-        sig[f"rpl_{kind}_stream_cloud_msgs"] = ([vp, PCP, C.c_int64, vp, u64, vp, vp, vp], u32)
-        sig[f"rpl_{kind}_stream_cloud_msgs_dev"] = ([vp, PCP, C.c_int64, vp, u64, vp, vp, vp, vp], u32)
-        sig[f"rpl_{kind}_stream_nodes"] = ([vp, u32, vp, vp, u64, vp, vp, vp, vp], u32)
-        sig[f"rpl_{kind}_stream_nodes_dev"] = ([vp, u32, vp, vp, u64, vp, vp, vp, vp, vp], u32)
     for name, (args, res) in sig.items():
         fn = getattr(L, name)  # AttributeError here = the library does not export the ABI
         fn.argtypes = args
@@ -619,8 +596,6 @@ class CapsuleStreamSession:
     ultra-dense) pushed in pieces, scans published as the whole stream would publish them.  Borrows `ctx`; close it
     before the context."""
 
-    _sym = "rpl_capsule_stream"
-
     def __init__(self, ctx: Context, ans_type: int, n_streams: int, stride_capsules: int, max_nodes: int, max_scans: int):
         self._init(ctx, ans_type, n_streams, stride_capsules, max_nodes, max_scans,
                    lambda h: ctx._L.rpl_capsule_stream_create(ctx._h, ans_type, n_streams, stride_capsules, max_nodes,
@@ -635,7 +610,7 @@ class CapsuleStreamSession:
         self.n_streams, self.stride_capsules, self.max_nodes, self.max_scans = n_streams, stride_capsules, max_nodes, max_scans
 
     def _fn(self, name):
-        return getattr(self._L, f"{self._sym}_{name}")
+        return getattr(self._L, f"rpl_capsule_stream_{name}")
 
     def close(self):
         if getattr(self, "_h", None):
@@ -831,84 +806,23 @@ class CapsuleStreamSession:
         """(open_nodes, held_capsule): nodes in each stream's open revolution, 1 where a valid capsule is held."""
         open_nodes = np.zeros(self.n_streams, np.uint32)
         held = np.zeros(self.n_streams, np.uint32)
-        self._ctx._check(self._fn("state")(self._h, _p(open_nodes), _p(held)))
+        self._ctx._check(self._fn("state")(self._h, _p(open_nodes), _p(held), None))
         return open_nodes, held
 
 
 class DenseStreamSession(CapsuleStreamSession):
-    """rpl_dense_stream wrapper: the capsule session fixed to dense capsules (0x85, 84 bytes)."""
-
-    _sym = "rpl_dense_stream"
+    """The capsule session fixed to dense capsules (0x85, 84 bytes)."""
 
     def __init__(self, ctx: Context, n_streams: int, stride_capsules: int, max_nodes: int, max_scans: int):
-        self._init(ctx, 0x85, n_streams, stride_capsules, max_nodes, max_scans,
-                   lambda h: ctx._L.rpl_dense_stream_create(ctx._h, n_streams, stride_capsules, max_nodes, max_scans,
-                                                             C.byref(h)))
-
-
-class NormalStreamSession(CapsuleStreamSession):
-    """rpl_normal_stream wrapper: raw 0x81 standard-node byte streams pushed in any pieces, scans published as the
-    whole stream would publish them.  close, reset and state are the capsule session's; state() returns
-    (open_nodes, held_bytes), held_bytes = bytes of the unfinished record held for the next push (0..4)."""
-
-    _sym = "rpl_normal_stream"
-
-    def __init__(self, ctx: Context, n_streams: int, stride_bytes: int, max_nodes: int, max_scans: int):
-        self._L, self._ctx = ctx._L, ctx
-        h = C.c_void_p()
-        ctx._check(ctx._L.rpl_normal_stream_create(ctx._h, n_streams, stride_bytes, max_nodes, max_scans, C.byref(h)))
-        self._h = h
-        self.ans_type = 0x81
-        self.n_streams, self.stride_bytes, self.max_nodes, self.max_scans = n_streams, stride_bytes, max_nodes, max_scans
-
-    def push(self, stream_bytes, byte_counts, params: ScanParams, out=None, chunk_bytes=None, chunk_rx_us=None,
-             timing: "Timing | None" = None):
-        """Host buffers: stream_bytes [n_streams, stride_bytes] uint8 -> the dict of CapsuleStreamSession.push.  With
-        chunk_bytes, chunk_rx_us ([n_streams, ceil(stride_bytes / chunk_bytes)]: receive time of each chunk_bytes piece
-        of this push) and timing, a stamped push: the dict also holds scan_begin_ts_us."""
-        assert stream_bytes.dtype == np.uint8 and stream_bytes.shape == (self.n_streams, self.stride_bytes)
-        assert stream_bytes.flags.c_contiguous
-        bc = np.ascontiguousarray(byte_counts, dtype=np.uint32)
-        assert bc.shape == (self.n_streams,)
-        if chunk_bytes is None and chunk_rx_us is None and timing is None:
-            out = self._outputs(out)
-            self._ctx._check(self._fn("push")(
-                self._h, _p(stream_bytes), _p(bc), C.byref(params), _p(out["ranges"]), _p(out["intensities"]),
-                _p(out["beam_counts"]), _p(out["angle_increment"]), _p(out["scans_per_stream"])))
-            return out
-        assert chunk_bytes is not None and chunk_rx_us is not None and (timing is not None or params.flags & FLAG_PER_STREAM), \
-            "a stamped push takes chunk_bytes, chunk_rx_us and timing (timing may be None with FLAG_PER_STREAM)"
-        rx = np.ascontiguousarray(chunk_rx_us, dtype=np.uint64)
-        assert chunk_bytes == 0 or rx.shape == (self.n_streams, -(-self.stride_bytes // chunk_bytes))
-        out = self._stamped_outputs(out)
-        self._ctx._check(self._fn("push_ts")(
-            self._h, _p(stream_bytes), _p(bc), _timing(timing), chunk_bytes, _p(rx), C.byref(params),
-            _p(out["ranges"]), _p(out["intensities"]), _p(out["beam_counts"]), _p(out["angle_increment"]),
-            _p(out["scans_per_stream"]), _p(out["scan_begin_ts_us"])))
-        return out
-
-    def push_dev(self, stream_bytes, byte_counts, params: ScanParams, ranges, intensities, beam_counts,
-                 angle_increment, scans_per_stream, stream=None, chunk_bytes=None, chunk_rx_us=None,
-                 timing: "Timing | None" = None, scan_begin_ts_us=None):
-        """Device addresses (the layouts of push), asynchronous on `stream` (None: the context's stream).  With
-        chunk_bytes, chunk_rx_us, timing and scan_begin_ts_us, a stamped push."""
-        if chunk_bytes is None and chunk_rx_us is None and timing is None and scan_begin_ts_us is None:
-            self._ctx._check(self._fn("push_dev")(
-                self._h, _p(stream_bytes), _p(byte_counts), C.byref(params), _p(ranges), _p(intensities),
-                _p(beam_counts), _p(angle_increment), _p(scans_per_stream), _p(stream)))
-            return
-        self._ctx._check(self._fn("push_ts_dev")(
-            self._h, _p(stream_bytes), _p(byte_counts), C.byref(timing) if timing is not None else None,
-            chunk_bytes or 0, _p(chunk_rx_us), C.byref(params), _p(ranges), _p(intensities), _p(beam_counts),
-            _p(angle_increment), _p(scans_per_stream), _p(scan_begin_ts_us), _p(stream)))
+        super().__init__(ctx, 0x85, n_streams, stride_capsules, max_nodes, max_scans)
 
 
 class CapsuleByteStreamSession(CapsuleStreamSession):
-    """rpl_capsule_stream byte session (rpl_capsule_stream_create_bytes): the raw serial bytes of a capsule answer type
-    (0x82..0x86, after the answer descriptor) pushed in any pieces, with the unpackers' search for the sync bytes carried
-    across pushes; scans published as the whole stream would publish them.  close and reset are the capsule session's;
-    state() returns (open_nodes, held_capsule, held_bytes), held_bytes = bytes of the unfinished frame held for the next
-    push."""
+    """rpl_capsule_stream byte session (rpl_capsule_stream_create_bytes): the raw serial bytes of a measurement answer
+    type (0x81..0x86, after the answer descriptor) pushed in any pieces, with the unpackers' search for the sync bytes
+    (0x81: the unfinished record) carried across pushes; scans published as the whole stream would publish them.  close
+    and reset are the capsule session's; state() returns (open_nodes, held_capsule, held_bytes), held_bytes = bytes of
+    the unfinished frame (0x81: record) held for the next push."""
 
     def __init__(self, ctx: Context, ans_type: int, n_streams: int, stride_bytes: int, max_nodes: int, max_scans: int):
         self._init(ctx, ans_type, n_streams, 0, max_nodes, max_scans,
@@ -962,8 +876,32 @@ class CapsuleByteStreamSession(CapsuleStreamSession):
     def state(self):
         """(open_nodes, held_capsule, held_bytes)"""
         open_nodes, held, held_bytes = (np.zeros(self.n_streams, np.uint32) for _ in range(3))
-        self._ctx._check(self._L.rpl_capsule_stream_state_bytes(self._h, _p(open_nodes), _p(held), _p(held_bytes)))
+        self._ctx._check(self._fn("state")(self._h, _p(open_nodes), _p(held), _p(held_bytes)))
         return open_nodes, held, held_bytes
+
+
+class NormalStreamSession(CapsuleByteStreamSession):
+    """The byte session on raw 0x81 standard-node byte streams, whose decoder takes no sample duration.  state()
+    returns (open_nodes, held_bytes), held_bytes = bytes of the unfinished record held for the next push (0..4)."""
+
+    def __init__(self, ctx: Context, n_streams: int, stride_bytes: int, max_nodes: int, max_scans: int):
+        super().__init__(ctx, 0x81, n_streams, stride_bytes, max_nodes, max_scans)
+
+    def push(self, stream_bytes, byte_counts, params: ScanParams, out=None, chunk_bytes=None, chunk_rx_us=None,
+             timing: "Timing | None" = None):
+        return super().push(stream_bytes, byte_counts, params, 0, out, chunk_bytes, chunk_rx_us, timing)
+
+    def push_dev(self, stream_bytes, byte_counts, params: ScanParams, ranges, intensities, beam_counts,
+                 angle_increment, scans_per_stream, stream=None, chunk_bytes=None, chunk_rx_us=None,
+                 timing: "Timing | None" = None, scan_begin_ts_us=None):
+        super().push_dev(stream_bytes, byte_counts, params, ranges, intensities, beam_counts, angle_increment,
+                         scans_per_stream, 0, stream, chunk_bytes, chunk_rx_us, timing, scan_begin_ts_us)
+
+    def state(self):
+        """(open_nodes, held_bytes)"""
+        open_nodes, held_bytes = (np.zeros(self.n_streams, np.uint32) for _ in range(2))
+        self._ctx._check(self._fn("state")(self._h, _p(open_nodes), None, _p(held_bytes)))
+        return open_nodes, held_bytes
 
 
 EXCHANGE_NCCL, EXCHANGE_COPY = 0, 1

@@ -8,6 +8,7 @@
 #include <algorithm>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
 #include <new>
 #include <string>
 #include <utility>
@@ -1188,20 +1189,26 @@ rpl_result rpl_scan_views_dev(rpl_ctx* c, const rpl_node_hq* nodes, uint64_t nod
 // contiguous view.  Each stream's region of an arena is [max_nodes carry slots][nodes per capsule * stride_capsules new
 // nodes]; push t decodes into arena t % 2 and its assembler writes the new open revolution into the carry slots of the
 // other arena, because the scans push t closes are read from this arena's carry slots by the scan kernels after the
-// assembler.  rpl_dense_stream is this session fixed to 0x85.  rpl_normal_stream is this session on 0x81 standard-node
-// bytes: a push's input counts bytes instead of capsules (cap_bytes 1), the held record keeps the byte machine, and
-// there are no capsule reports (the standard unpacker requests no scan resets).
-// A stamped push (rpl_*_stream_push_ts*) runs the stamped decoder (0x81) and assembler instead; they keep, beside the
-// carry, the open revolution's stamp (open_ts, per arena like carry_len) and, for express and ultra, the held capsule's
-// receive time (held_rx).  An unstamped push leaves both stale, so the next stamped push counts them as unknown.
-// A byte session (rpl_capsule_stream_create_bytes) takes the raw bytes of the serial stream instead of framed capsules:
-// each push is framed first (frame.cu's session instantiation, the search carried in the framer record) into the
-// session's own capsule slots, which the decoder then reads as a framed session's push; stride_capsules counts those
-// slots, and a stamped push's capsule receive times come out of the framer.
+// assembler.
+// A stamped push (rpl_capsule_stream_push*_ts*) runs the stamped decoder (0x81) and assembler instead; they keep,
+// beside the carry, the open revolution's stamp (open_ts, per arena like carry_len) and, for express and ultra, the
+// held capsule's receive time (held_rx).  An unstamped push leaves both stale, so the next stamped push counts them as
+// unknown.
+// A byte session (rpl_capsule_stream_create_bytes) takes the raw bytes of the serial stream instead of framed capsules.
+// On a capsule answer type each push is framed first (frame.cu's session instantiation, the search carried in the
+// framer record) into the session's own capsule slots, which the decoder then reads as a framed session's push;
+// stride_capsules counts those slots, and a stamped push's capsule receive times come out of the framer.  On 0x81
+// standard nodes the decoder reads the pushed bytes itself: the held record keeps the byte machine, stride_capsules
+// counts bytes (cap_bytes 1), and there are no capsule reports (the standard unpacker requests no scan resets).
 struct rpl_capsule_stream {
   rpl_ctx* c = nullptr;
   uint32_t ans_type = 0, cap_bytes = 0;    // answer type, bytes per capsule (0x81: 1)
   uint32_t n_streams = 0, stride_capsules = 0, max_nodes = 0, max_scans = 0;  // stride_capsules: 0x81, bytes
+  // what a push takes, fixed at create: bytes (a byte session) or framed capsules; per stream at most stride_in of
+  // them (bytes or capsules), in_stream bytes of input
+  bool bytes = false;
+  uint32_t stride_in = 0;
+  size_t in_stream = 0;
   uint32_t stride_nodes = 0, starts_stride = 0;
   uint32_t chunk_dev = 0, chunk_host = 0;  // streams per scan launch (context's max_scans), per host-push chunk
   uint32_t parity = 0;                     // arena of the next push
@@ -1217,23 +1224,23 @@ struct rpl_capsule_stream {
   unsigned long long* held_rx = nullptr;        // [n_streams] express, ultra: receive time of the held capsule
   uint32_t* scan_ends = nullptr;                // 0x81: [n_streams][new nodes] end bytes of the scan-start records
   bool prev_stamped = true;                     // the last push had receive times (a fresh session holds nothing)
-  uint32_t stride_bytes = 0;                    // byte session: most bytes per stream in one push (0: framed capsules)
-  uint32_t* framer = nullptr;                   // byte session: [n_streams][kFramerWords]
-  uint8_t* framed = nullptr;                    // byte session: [n_streams][stride_capsules][cap_bytes] this push's
-  uint32_t* framed_counts = nullptr;            // byte session: [n_streams]
-  unsigned long long* framed_rx = nullptr;      // byte session: [n_streams][stride_capsules] (stamped pushes)
+  // a byte session of a capsule answer type (else null): the framer records, this push's framed capsules
+  uint32_t* framer = nullptr;                   // [n_streams][kFramerWords]
+  uint8_t* framed = nullptr;                    // [n_streams][stride_capsules][cap_bytes]
+  uint32_t* framed_counts = nullptr;            // [n_streams]
+  unsigned long long* framed_rx = nullptr;      // [n_streams][stride_capsules] (stamped pushes)
   // the last push, as the cloud calls replay it: its views count from the first stream of their chunk
   uint32_t cloud_chunk = 0;                     // streams per chunk (chunk_host or chunk_dev); 0: no push, or it failed
   uint32_t cloud_arena = 0;                     // the arena its views point into
-  // the messages of the last push (rpl_*_stream_*_msgs*): a stamped push's slot stamps, the per-stream settings
+  // the messages of the last push (rpl_capsule_stream_*_msgs*): a stamped push's slot stamps, the per-stream settings
   unsigned long long* slot_begin = nullptr;     // [n_streams * max_scans] scan-begin stamps (0: unused, unknown)
   unsigned long long* slot_end = nullptr;       // [n_streams * max_scans] the closing scan-start node's stamp
   rpl::StreamMsgHeader* msg_hdr = nullptr;      // [n_streams] device
   std::vector<rpl::StreamMsgHeader> msg_hdr_host;
   unsigned char* msg_work = nullptr;            // the scan kernels' outputs and the tables of a messages call
   size_t msg_work_bytes = 0;
-  // the per-stream lidar settings (rpl_*_stream_set_lidars) that calls with RPL_FLAG_PER_STREAM / RPL_CLOUD_PER_STREAM
-  // read; empty until the first call sets every stream
+  // the per-stream lidar settings (rpl_capsule_stream_set_lidars) that calls with RPL_FLAG_PER_STREAM /
+  // RPL_CLOUD_PER_STREAM read; empty until the first call sets every stream
   rpl::LidarSettings* lidars = nullptr;         // [n_streams] device
   std::vector<rpl::LidarSettings> lidars_host;
   uint32_t lidar_modes = 0;                     // LidarTable::modes of the table
@@ -1249,15 +1256,11 @@ static_assert(sizeof(rpl::LidarSettings) == sizeof(rpl_lidar_settings) &&
 
 namespace {
 
-// the dense and standard-node sessions' handles are a capsule session's
-rpl_capsule_stream* capsule_session(rpl_dense_stream* ds) { return reinterpret_cast<rpl_capsule_stream*>(ds); }
-rpl_capsule_stream* capsule_session(rpl_normal_stream* ns) { return reinterpret_cast<rpl_capsule_stream*>(ns); }
-
 // a stamped push's receive times and stamp output (rx, scan_ts: of the first stream of the call they are passed to)
 struct StampPush {
   rpl::TimingDesc timing;
-  const unsigned long long* rx;         // capsule_rx_us [.][stride_capsules], 0x81: chunk_rx_us [.][stride_chunks]
-  uint32_t chunk_bytes, stride_chunks;  // 0x81
+  const unsigned long long* rx;         // capsule_rx_us [.][stride_capsules], byte pushes: chunk_rx_us [.][stride_chunks]
+  uint32_t chunk_bytes, stride_chunks;  // a framed push's chunk_bytes is 1; stride_chunks: ceil(stride_in / chunk_bytes)
   unsigned long long* scan_ts;          // scan_begin_ts_us [.][max_scans]
 };
 
@@ -1322,7 +1325,7 @@ WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0, bool per_stre
   w.slot_end = cs->slot_end + so;
   w.prev_stamped = cs->prev_stamped;
   if (cs->framer) {
-    w.stride_bytes = cs->stride_bytes;
+    w.stride_bytes = cs->stride_in;
     w.framer = cs->framer + (size_t)s0 * rpl::kFramerWords;
     w.framed = cs->framed + (size_t)s0 * sc * cs->cap_bytes;
     w.framed_counts = cs->framed_counts + s0;
@@ -1513,7 +1516,7 @@ rpl_result push_host(rpl_ctx* c, const HostWire& h, uint32_t n_streams, uint32_t
   return run_chunks(c, n_streams, chunk, run_chunk);
 }
 
-// The tables of a nodes call (rpl_*_stream_nodes*), the session's own: every slot's place for the kernels, the
+// The tables of a nodes call (rpl_capsule_stream_nodes*), the session's own: every slot's place for the kernels, the
 // per-stream ascend flags, and the host form's directory, which the device form writes into the caller's arrays.
 struct NodeWork {
   unsigned long long *place, *offsets, *total;
@@ -1560,7 +1563,7 @@ bool capsule_stream_args_ok(rpl_capsule_stream* cs, const uint8_t* capsules, con
   }
   // the alignment rule of rpl_decode_capsules_batch_dev: only dense capsules are read in 4-byte words (a byte session's
   // bytes have any alignment: its decoder reads the session's own capsule slots)
-  if (cs->ans_type == 0x85 && !cs->framer && (reinterpret_cast<uintptr_t>(capsules) & 3u) != 0) {
+  if (cs->ans_type == 0x85 && !cs->bytes && (reinterpret_cast<uintptr_t>(capsules) & 3u) != 0) {
     c->err = "capsule buffer must be 4-byte aligned";
     return false;
   }
@@ -1581,20 +1584,20 @@ rpl::StreamMsgHeader msg_header(const char* frame_id, size_t len, float range_ma
   return h;
 }
 
-// a session of a capsule answer type or of 0x81 standard nodes (the caller has checked ans_type); stride_capsules
-// counts bytes for 0x81.  stride_bytes != 0: a byte session of a capsule answer type (stride_capsules is ignored)
-rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint32_t stride_capsules,
-                         uint32_t max_nodes, uint32_t max_scans, rpl_capsule_stream** out, uint32_t stride_bytes = 0) {
-  const bool normal = ans_type == RPL_ANS_MEASUREMENT, bytes = stride_bytes != 0;
+// a session of answer type ans_type (the caller has checked it) whose pushes take, per stream, at most stride_in framed
+// capsules, or with `bytes` at most stride_in bytes of the serial stream (a capsule answer type's are framed first)
+rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, bool bytes, uint32_t n_streams, uint32_t stride_in,
+                         uint32_t max_nodes, uint32_t max_scans, rpl_capsule_stream** out) {
+  const bool normal = ans_type == RPL_ANS_MEASUREMENT, framing = bytes && !normal;
   const uint32_t cap_bytes = normal ? 1u : rpl_capsule_bytes(ans_type);
   // a byte push completes at most `frames` frames with the up to cap_bytes - 1 bytes held before it, each behind at most
   // one all-zero capsule (none for HQ, whose skipped bytes are no loss)
-  const unsigned long long frames = bytes ? ((unsigned long long)stride_bytes + cap_bytes - 1) / cap_bytes : stride_capsules;
-  if (bytes) stride_capsules = (uint32_t)(ans_type == 0x83 ? frames : 2 * frames);
+  const unsigned long long frames = framing ? ((unsigned long long)stride_in + cap_bytes - 1) / cap_bytes : stride_in;
+  const uint32_t stride_capsules = framing ? (uint32_t)(ans_type == 0x83 ? frames : 2 * frames) : stride_in;
   if (n_streams == 0 || stride_capsules == 0 || max_scans == 0 || max_nodes == 0 || max_nodes > rpl::kSmallMaxNodes ||
       (max_nodes & 1u)) {
-    c->err = normal || bytes ? "need n_streams > 0, stride_bytes > 0, max_scans > 0 and an even max_nodes in [2, 8192]"
-                             : "need n_streams > 0, stride_capsules > 0, max_scans > 0 and an even max_nodes in [2, 8192]";
+    c->err = bytes ? "need n_streams > 0, stride_bytes > 0, max_scans > 0 and an even max_nodes in [2, 8192]"
+                   : "need n_streams > 0, stride_capsules > 0, max_scans > 0 and an even max_nodes in [2, 8192]";
     return RPL_RESULT_INVALID_DATA;
   }
   if (max_scans > c->max_scans) {
@@ -1609,10 +1612,10 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint
   if (stride_nodes * n_streams > 0xFFFFFFFFull) {
     c->err = normal ? "n_streams * (max_nodes + (stride_bytes + 4) / 5 rounded up to even) must stay below 2^32 "
                       "(32-bit scan views)"
-                    : bytes ? "n_streams * (max_nodes + nodes per capsule * ceil(stride_bytes / capsule bytes)) must stay "
-                              "below 2^32 (32-bit scan views)"
-                            : "n_streams * (max_nodes + nodes per capsule * stride_capsules) must stay below 2^32 (32-bit "
-                              "scan views)";
+                    : framing ? "n_streams * (max_nodes + nodes per capsule * ceil(stride_bytes / capsule bytes)) must "
+                                "stay below 2^32 (32-bit scan views)"
+                              : "n_streams * (max_nodes + nodes per capsule * stride_capsules) must stay below 2^32 "
+                                "(32-bit scan views)";
     return RPL_RESULT_INVALID_DATA;
   }
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
@@ -1628,10 +1631,11 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint
   cs->stride_nodes = (uint32_t)stride_nodes;  // even: every region starts 16-byte aligned
   cs->starts_stride = 2 * max_scans + 64;     // scan starts per stream the decoder may list (as in the chain)
   cs->chunk_dev = std::min(n_streams, c->max_scans / max_scans);
-  cs->stride_bytes = stride_bytes;
+  cs->bytes = bytes;
+  cs->stride_in = stride_in;
+  cs->in_stream = bytes ? (size_t)stride_in : (size_t)stride_in * cap_bytes;
   // host pushes: about 16 MiB of capsules (a byte session: bytes) per chunk, whole streams (as in the chain)
-  const size_t cap_bytes_stream = bytes ? (size_t)stride_bytes : (size_t)stride_capsules * cap_bytes;
-  cs->chunk_host = std::min<uint32_t>(cs->chunk_dev, (uint32_t)std::max<size_t>(1, ((size_t)16 << 20) / cap_bytes_stream));
+  cs->chunk_host = std::min<uint32_t>(cs->chunk_dev, (uint32_t)std::max<size_t>(1, ((size_t)16 << 20) / cs->in_stream));
   const size_t n = n_streams, ncap = n * stride_capsules;
   const rpl_result oom = RPL_RESULT_INSUFFICIENT_MEMORY;
   auto fail = [&](rpl_result r) {
@@ -1655,11 +1659,11 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint
   if (!normal && (!cuda_ok(c, dev_alloc(&cs->status, ncap), "cudaMalloc") ||
                   !cuda_ok(c, dev_alloc(&cs->offsets, ncap), "cudaMalloc")))
     return fail(oom);
-  if (bytes && (!cuda_ok(c, dev_alloc(&cs->framer, n * rpl::kFramerWords), "cudaMalloc") ||
-                !cuda_ok(c, cudaMemset(cs->framer, 0, n * rpl::kFramerWords * 4), "cudaMemset") ||
-                !cuda_ok(c, dev_alloc(&cs->framed, ncap * cap_bytes), "cudaMalloc") ||
-                !cuda_ok(c, dev_alloc(&cs->framed_counts, n), "cudaMalloc") ||
-                !cuda_ok(c, dev_alloc(&cs->framed_rx, ncap), "cudaMalloc")))
+  if (framing && (!cuda_ok(c, dev_alloc(&cs->framer, n * rpl::kFramerWords), "cudaMalloc") ||
+                  !cuda_ok(c, cudaMemset(cs->framer, 0, n * rpl::kFramerWords * 4), "cudaMemset") ||
+                  !cuda_ok(c, dev_alloc(&cs->framed, ncap * cap_bytes), "cudaMalloc") ||
+                  !cuda_ok(c, dev_alloc(&cs->framed_counts, n), "cudaMalloc") ||
+                  !cuda_ok(c, dev_alloc(&cs->framed_rx, ncap), "cudaMalloc")))
     return fail(oom);
   if (!cuda_ok(c, dev_alloc(&cs->held, n * rpl::kHeldWords), "cudaMalloc") ||
       !cuda_ok(c, cudaMemset(cs->held, 0, n * rpl::kHeldWords * 4), "cudaMemset") ||
@@ -1682,7 +1686,7 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint
   return RPL_RESULT_OK;
 }
 
-// the stamped pushes' own arguments (chunk_bytes: 0x81 only, 1 for the capsule formats) into *sp; with
+// the stamped pushes' own arguments (chunk_bytes: the byte pushes', 1 for a framed push) into *sp; with
 // RPL_FLAG_PER_STREAM the table's timing serves and `timing` may be null
 bool stamp_args_ok(rpl_capsule_stream* cs, const rpl_scan_params* params, const rpl_timing* timing, const uint64_t* rx,
                    uint32_t chunk_bytes, uint64_t* scan_begin_ts_us, StampPush* sp) {
@@ -1706,98 +1710,72 @@ bool stamp_args_ok(rpl_capsule_stream* cs, const rpl_scan_params* params, const 
                                  timing->native_interface_type};
   sp->rx = reinterpret_cast<const unsigned long long*>(rx);
   sp->chunk_bytes = chunk_bytes;
-  const uint32_t stride_in = cs->framer ? cs->stride_bytes : cs->stride_capsules;  // bytes, or capsules
-  sp->stride_chunks = (uint32_t)(((unsigned long long)stride_in + chunk_bytes - 1) / chunk_bytes);
+  sp->stride_chunks = (uint32_t)(((unsigned long long)cs->stride_in + chunk_bytes - 1) / chunk_bytes);
   sp->scan_ts = reinterpret_cast<unsigned long long*>(scan_begin_ts_us);
   return true;
 }
 
 // a byte push on a framed session or a framed push on a byte session
 bool push_kind_ok(rpl_capsule_stream* cs, bool bytes) {
-  if ((cs->framer != nullptr) == bytes) return true;
+  if (cs->bytes == bytes) return true;
   cs->c->err = bytes ? "a byte push needs a session made by rpl_capsule_stream_create_bytes"
                      : "a session made by rpl_capsule_stream_create_bytes takes byte pushes (rpl_capsule_stream_push_bytes*)";
   return false;
 }
 
-// a host push; sp: a stamped one (its rx and scan_ts are host arrays of all streams)
-rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* capsules, const uint32_t* capsule_counts,
-                       uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges, float* intensities,
-                       uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
-                       const StampPush* sp, bool bytes = false) {
+// A push of the kind the entry point takes (bytes: a byte push); sp: a stamped one.  Host arrays (dev false, stream
+// unused) run in the session's host chunks round-robin over the lanes, device arrays in its device chunks on `stream`.
+// The arrays, sp's rx and scan_ts included, hold every stream.
+rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t* counts, uint32_t sample_duration_us,
+                       const rpl_scan_params* params, float* ranges, float* intensities, uint32_t* beam_counts,
+                       float* angle_increment, uint32_t* scans_per_stream, const StampPush* sp, bool bytes, bool dev,
+                       void* stream) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
   rpl_ctx* c = cs->c;
   cs->cloud_chunk = 0;
   if (!push_kind_ok(cs, bytes)) return RPL_RESULT_INVALID_DATA;
-  if (!capsule_stream_args_ok(cs, capsules, capsule_counts, sample_duration_us, params, ranges, intensities,
-                              beam_counts, scans_per_stream))
+  if (!capsule_stream_args_ok(cs, in, counts, sample_duration_us, params, ranges, intensities, beam_counts,
+                              scans_per_stream))
     return RPL_RESULT_INVALID_DATA;
-  const uint32_t stride_in = bytes ? cs->stride_bytes : cs->stride_capsules;
-  for (uint32_t s = 0; s < cs->n_streams; ++s)
-    if (capsule_counts[s] > stride_in) {
-      c->err = cs->ans_type == RPL_ANS_MEASUREMENT || bytes ? "byte_counts[s] exceeds stride_bytes"
-                                                            : "capsule_counts[s] exceeds stride_capsules";
-      return RPL_RESULT_INVALID_DATA;
-    }
-  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  for (int i = 0; i < kLanes; ++i) RPL_CUDA(c, cudaStreamWaitEvent(c->lane[i].stream, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
-  // receive times per stream of a stamped push: one per capsule, 0x81 and byte pushes one per chunk_bytes piece
-  const size_t rx_stream = sp ? (cs->status && !bytes ? cs->stride_capsules : sp->stride_chunks) : 0;
-  const size_t in_stream = bytes ? (size_t)cs->stride_bytes : (size_t)cs->stride_capsules * cs->cap_bytes;
-  const HostWire h{capsules, capsule_counts, in_stream, sample_duration_us,
-                   cs->max_nodes, cs->max_scans, params, ranges, intensities, angle_increment, beam_counts,
-                   scans_per_stream, sp, rx_stream};
   const bool per_stream = (params->flags & RPL_FLAG_PER_STREAM) != 0;
-  const rpl_result r = push_host(c, h, cs->n_streams, cs->chunk_host,
-                                 [&](Carve&, uint32_t s0) { return session_chunk(cs, s0, per_stream); });
-  cs->parity ^= 1u;
-  cs->prev_stamped = sp != nullptr;
-  if (r == RPL_RESULT_OK) {
-    cs->cloud_chunk = cs->chunk_host;
-    cs->cloud_arena = cs->parity ^ 1u;
-  }
-  return r;
-}
-
-// a device push; sp: a stamped one (its rx and scan_ts are device arrays of all streams)
-rpl_result stream_push_dev(rpl_capsule_stream* cs, const uint8_t* capsules, const uint32_t* capsule_counts,
-                           uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
-                           float* intensities, uint32_t* beam_counts, float* angle_increment,
-                           uint32_t* scans_per_stream, void* stream, const StampPush* sp, bool bytes = false) {
-  if (!cs) return RPL_RESULT_INVALID_DATA;
-  rpl_ctx* c = cs->c;
-  cs->cloud_chunk = 0;
-  if (!push_kind_ok(cs, bytes)) return RPL_RESULT_INVALID_DATA;
-  if (!capsule_stream_args_ok(cs, capsules, capsule_counts, sample_duration_us, params, ranges, intensities,
-                              beam_counts, scans_per_stream))
-    return RPL_RESULT_INVALID_DATA;
-  cudaStream_t st;
-  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
-  RPL_CUDA(c, cudaStreamWaitEvent(st, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
-  const size_t row = (size_t)cs->max_scans * cs->max_nodes;
+  const uint32_t chunk = dev ? cs->chunk_dev : cs->chunk_host;
+  cudaStream_t st = nullptr;
   rpl_result r = RPL_RESULT_OK;
-  for (uint32_t s0 = 0; s0 < cs->n_streams && r == RPL_RESULT_OK; s0 += cs->chunk_dev) {
-    const uint32_t ns = std::min(cs->chunk_dev, cs->n_streams - s0);
-    const size_t so = (size_t)s0 * cs->max_scans;
-    StampPush chunk_sp{};
-    if (sp) {
-      chunk_sp = *sp;
-      chunk_sp.rx += (size_t)s0 * (cs->status && !bytes ? cs->stride_capsules : sp->stride_chunks);
-      chunk_sp.scan_ts += so;
+  if (dev) {
+    if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
+    RPL_CUDA(c, cudaStreamWaitEvent(st, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
+    const size_t row = (size_t)cs->max_scans * cs->max_nodes;
+    for (uint32_t s0 = 0; s0 < cs->n_streams && r == RPL_RESULT_OK; s0 += chunk) {
+      const size_t so = (size_t)s0 * cs->max_scans;
+      StampPush chunk_sp{};
+      if (sp) {
+        chunk_sp = *sp;
+        chunk_sp.rx += (size_t)s0 * sp->stride_chunks;
+        chunk_sp.scan_ts += so;
+      }
+      r = capsule_stream_chunk(c, c->lane[0], st, session_chunk(cs, s0, per_stream),
+                               std::min(chunk, cs->n_streams - s0), in + s0 * cs->in_stream, counts + s0,
+                               sample_duration_us, params, ranges + s0 * row, intensities + s0 * row, beam_counts + so,
+                               angle_increment ? angle_increment + so : nullptr, scans_per_stream + s0,
+                               sp ? &chunk_sp : nullptr);
     }
-    r = capsule_stream_chunk(c, c->lane[0], st, session_chunk(cs, s0, (params->flags & RPL_FLAG_PER_STREAM) != 0), ns,
-                             capsules + (size_t)s0 * (bytes ? cs->stride_bytes : cs->stride_capsules * cs->cap_bytes),
-                             capsule_counts + s0,
-                             sample_duration_us, params, ranges + (size_t)s0 * row, intensities + (size_t)s0 * row,
-                             beam_counts + so,
-                             angle_increment ? angle_increment + so : nullptr, scans_per_stream + s0,
-                             sp ? &chunk_sp : nullptr);
+  } else {
+    for (uint32_t s = 0; s < cs->n_streams; ++s)
+      if (counts[s] > cs->stride_in) {
+        c->err = bytes ? "byte_counts[s] exceeds stride_bytes" : "capsule_counts[s] exceeds stride_capsules";
+        return RPL_RESULT_INVALID_DATA;
+      }
+    RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+    for (int i = 0; i < kLanes; ++i) RPL_CUDA(c, cudaStreamWaitEvent(c->lane[i].stream, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
+    const HostWire h{in, counts, cs->in_stream, sample_duration_us, cs->max_nodes, cs->max_scans, params, ranges,
+                     intensities, angle_increment, beam_counts, scans_per_stream, sp, sp ? sp->stride_chunks : 0u};
+    r = push_host(c, h, cs->n_streams, chunk, [&](Carve&, uint32_t s0) { return session_chunk(cs, s0, per_stream); });
   }
   cs->parity ^= 1u;
   cs->prev_stamped = sp != nullptr;
-  RPL_CUDA(c, cudaEventRecord(cs->done, st), RPL_RESULT_OPERATION_FAIL);
+  if (dev) RPL_CUDA(c, cudaEventRecord(cs->done, st), RPL_RESULT_OPERATION_FAIL);
   if (r == RPL_RESULT_OK) {
-    cs->cloud_chunk = cs->chunk_dev;
+    cs->cloud_chunk = chunk;
     cs->cloud_arena = cs->parity ^ 1u;
   }
   return r;
@@ -1816,14 +1794,10 @@ bool cloud_params_ok(rpl_ctx* c, const rpl_cloud_params* p) {
   return true;
 }
 
-// The cloud chain over the scans of streams [s0, s0 + ns) of the session's last push, one chunk of that push: its
-// views count from node 0 of stream s0 in the push's arena.  xyzi / point_counts point at the chunk's first slot.
-// Flags 0: the shared-memory kernel with SOR / voxel grid fused, its arrays sized for at most kSmallPostMaxNodes nodes
-// (a longer view goes to the general kernel, then to the post passes restricted to the hand-off list);
-// RPL_CLOUD_NO_FUSED: the shared-memory kernel's window + xyz, then the post passes over every scan.
-rpl_result stream_cloud_chunk(rpl_capsule_stream* cs, Lane& l, uint32_t s0, uint32_t ns, const rpl_cloud_params* p,
-                              float* xyzi, uint32_t* point_counts, cudaStream_t st) {
-  rpl_ctx* c = cs->c;
+// The scans of streams [s0, s0 + ns) of the session's last push, one chunk of that push, as the scan kernels read
+// them: the chunk's region of the push's arena, its slots' views (which count from node 0 of stream s0 there) and
+// the holder's capacity as the stride.
+rpl::ScanBatchArgs last_push_scans(const rpl_capsule_stream* cs, uint32_t s0, uint32_t ns) {
   rpl::ScanBatchArgs a{};
   a.nodes = reinterpret_cast<const uint2*>(cs->arena[cs->cloud_arena] + (size_t)s0 * cs->stride_nodes);
   a.views = reinterpret_cast<const uint2*>(cs->views + (size_t)s0 * cs->max_scans);
@@ -1831,6 +1805,18 @@ rpl_result stream_cloud_chunk(rpl_capsule_stream* cs, Lane& l, uint32_t s0, uint
   a.nodes_total = (unsigned long long)ns * cs->stride_nodes;
   a.n_scans = ns * cs->max_scans;
   a.stride = cs->max_nodes;
+  return a;
+}
+
+// The cloud chain over the scans of one chunk of the session's last push (last_push_scans); xyzi / point_counts point
+// at the chunk's first slot.
+// Flags 0: the shared-memory kernel with SOR / voxel grid fused, its arrays sized for at most kSmallPostMaxNodes nodes
+// (a longer view goes to the general kernel, then to the post passes restricted to the hand-off list);
+// RPL_CLOUD_NO_FUSED: the shared-memory kernel's window + xyz, then the post passes over every scan.
+rpl_result stream_cloud_chunk(rpl_capsule_stream* cs, Lane& l, uint32_t s0, uint32_t ns, const rpl_cloud_params* p,
+                              float* xyzi, uint32_t* point_counts, cudaStream_t st) {
+  rpl_ctx* c = cs->c;
+  rpl::ScanBatchArgs a = last_push_scans(cs, s0, ns);
   a.beam_counts = point_counts;
   a.fallback_list = l.fallback_list;
   a.fallback_count = l.fallback_count;
@@ -1880,22 +1866,46 @@ bool stream_cloud_args_ok(rpl_capsule_stream* cs, const rpl_cloud_params* params
   return true;
 }
 
+// grows the session's message work block (an earlier messages call, on any stream, may still read it)
+rpl_result grow_msg_work(rpl_capsule_stream* cs, size_t bytes) {
+  rpl_ctx* c = cs->c;
+  if (cs->msg_work_bytes >= bytes) return RPL_RESULT_OK;
+  RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);
+  cudaFree(cs->msg_work);
+  cs->msg_work = nullptr;
+  cs->msg_work_bytes = 0;
+  RPL_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&cs->msg_work), bytes), RPL_RESULT_INSUFFICIENT_MEMORY);
+  cs->msg_work_bytes = bytes;
+  return RPL_RESULT_OK;
+}
+
+// The device form of a call on the last push: once the device is entered and the message work block has grown to
+// msg_work bytes (0: the call uses none), fn(st) enqueues the call on `stream` (NULL: lane 0's) behind the last push's
+// kernels, which are done before it reads the push's arena and views; the session's next push waits for it.
+template <class F>
+rpl_result last_push_dev(rpl_capsule_stream* cs, void* stream, size_t msg_work, F fn) {
+  rpl_ctx* c = cs->c;
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
+  if (const rpl_result r = grow_msg_work(cs, msg_work); r != RPL_RESULT_OK) return r;
+  RPL_CUDA(c, cudaStreamWaitEvent(st, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
+  const rpl_result r = fn(st);
+  RPL_CUDA(c, cudaEventRecord(cs->done, st), RPL_RESULT_OPERATION_FAIL);
+  return r;
+}
+
 rpl_result stream_cloud_dev(rpl_capsule_stream* cs, const rpl_cloud_params* params, float* xyzi,
                             uint32_t* point_counts, void* stream) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
-  rpl_ctx* c = cs->c;
   if (!stream_cloud_args_ok(cs, params, xyzi, point_counts)) return RPL_RESULT_INVALID_DATA;
-  cudaStream_t st;
-  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
-  // the last push's kernels are done before these read its arena and views; the next push waits for these
-  RPL_CUDA(c, cudaStreamWaitEvent(st, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
   const size_t row = (size_t)cs->max_scans * cs->max_nodes * 4;
-  rpl_result r = RPL_RESULT_OK;
-  for (uint32_t s0 = 0; s0 < cs->n_streams && r == RPL_RESULT_OK; s0 += cs->cloud_chunk)
-    r = stream_cloud_chunk(cs, c->lane[0], s0, std::min(cs->cloud_chunk, cs->n_streams - s0), params,
-                           xyzi + (size_t)s0 * row, point_counts + (size_t)s0 * cs->max_scans, st);
-  RPL_CUDA(c, cudaEventRecord(cs->done, st), RPL_RESULT_OPERATION_FAIL);
-  return r;
+  return last_push_dev(cs, stream, 0, [&](cudaStream_t st) -> rpl_result {
+    rpl_result r = RPL_RESULT_OK;
+    for (uint32_t s0 = 0; s0 < cs->n_streams && r == RPL_RESULT_OK; s0 += cs->cloud_chunk)
+      r = stream_cloud_chunk(cs, cs->c->lane[0], s0, std::min(cs->cloud_chunk, cs->n_streams - s0), params,
+                             xyzi + (size_t)s0 * row, point_counts + (size_t)s0 * cs->max_scans, st);
+    return r;
+  });
 }
 
 // the host variant: the last push's chunks round-robin over the lanes, each lane's clouds staged in its block and
@@ -2075,19 +2085,6 @@ bool stream_msgs_args_ok(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* 
   return true;
 }
 
-// grows the session's work block (an earlier messages call, on any stream, may still read it)
-rpl_result grow_msg_work(rpl_capsule_stream* cs, size_t bytes) {
-  rpl_ctx* c = cs->c;
-  if (cs->msg_work_bytes >= bytes) return RPL_RESULT_OK;
-  RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);
-  cudaFree(cs->msg_work);
-  cs->msg_work = nullptr;
-  cs->msg_work_bytes = 0;
-  RPL_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&cs->msg_work), bytes), RPL_RESULT_INSUFFICIENT_MEMORY);
-  cs->msg_work_bytes = bytes;
-  return RPL_RESULT_OK;
-}
-
 // on `st`, after the last push: the scan kernels or the cloud chain of every slot into w, then the tables
 rpl_result msgs_prepare(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* params, const MsgWork& w,
                         unsigned long long capacity, unsigned long long* offsets, uint32_t* sizes,
@@ -2100,10 +2097,10 @@ rpl_result msgs_prepare(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* p
     const size_t so = (size_t)s0 * cs->max_scans;
     if (kind == rpl::MsgKind::kLaserScan) {
       const auto* p = static_cast<const rpl_scan_params*>(params);
-      r = enqueue_scan(c, c->lane[0], cs->arena[cs->cloud_arena] + (size_t)s0 * cs->stride_nodes, cs->scan_len + so,
-                       ns * cs->max_scans, cs->max_nodes, p, nullptr, w.data + so * row, w.data + (NS + so) * row,
-                       w.counts + so, w.inc + so, nullptr, nullptr, st, reinterpret_cast<const uint2*>(cs->views + so),
-                       (unsigned long long)ns * cs->stride_nodes,
+      const rpl::ScanBatchArgs a = last_push_scans(cs, s0, ns);
+      r = enqueue_scan(c, c->lane[0], reinterpret_cast<const rpl_node_hq*>(a.nodes), cs->scan_len + so, a.n_scans,
+                       a.stride, p, nullptr, w.data + so * row, w.data + (NS + so) * row, w.counts + so, w.inc + so,
+                       nullptr, nullptr, st, a.views, a.nodes_total,
                        lidar_table(cs, (p->flags & RPL_FLAG_PER_STREAM) != 0, s0));
     } else {
       r = stream_cloud_chunk(cs, c->lane[0], s0, ns, static_cast<const rpl_cloud_params*>(params),
@@ -2171,25 +2168,86 @@ rpl_result stream_msgs_dev(rpl_capsule_stream* cs, rpl::MsgKind kind, const void
                            uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
                            uint64_t* total_bytes, void* stream) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
-  rpl_ctx* c = cs->c;
   if (!stream_msgs_args_ok(cs, kind, params, msgs, msg_offsets, msg_sizes, total_bytes, true))
     return RPL_RESULT_INVALID_DATA;
-  cudaStream_t st;
-  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   Carve k;
   msg_work_layout(cs, kind, false, k);
-  if (const rpl_result r = grow_msg_work(cs, k.bytes); r != RPL_RESULT_OK) return r;
-  Carve kw{cs->msg_work};
-  const MsgWork w = msg_work_layout(cs, kind, false, kw);
-  auto* offs = reinterpret_cast<unsigned long long*>(msg_offsets);
-  // the last push's kernels are done before these read its arena and views; the next push waits for these
-  RPL_CUDA(c, cudaStreamWaitEvent(st, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
-  rpl_result r = msgs_prepare(cs, kind, params, w, capacity, offs, msg_sizes,
-                              reinterpret_cast<unsigned long long*>(total_bytes), st);
-  if (r == RPL_RESULT_OK)
-    r = msgs_write(cs, kind, params, clock_offset_ns, w, offs, msg_sizes, 0, cs->n_streams * cs->max_scans, msgs, 0, st);
-  RPL_CUDA(c, cudaEventRecord(cs->done, st), RPL_RESULT_OPERATION_FAIL);
-  return r;
+  return last_push_dev(cs, stream, k.bytes, [&](cudaStream_t st) -> rpl_result {
+    Carve kw{cs->msg_work};
+    const MsgWork w = msg_work_layout(cs, kind, false, kw);
+    auto* offs = reinterpret_cast<unsigned long long*>(msg_offsets);
+    rpl_result r = msgs_prepare(cs, kind, params, w, capacity, offs, msg_sizes,
+                                reinterpret_cast<unsigned long long*>(total_bytes), st);
+    if (r == RPL_RESULT_OK)
+      r = msgs_write(cs, kind, params, clock_offset_ns, w, offs, msg_sizes, 0, cs->n_streams * cs->max_scans, msgs, 0,
+                     st);
+    return r;
+  });
+}
+
+// a per-slot uint32 table of a packed call: the caller's host array and the device table behind it
+struct SlotTable {
+  uint32_t* host;
+  const uint32_t* dev;
+};
+
+// The host form of a packed call (messages, nodes), once the caller has set the device and laid out its device tables:
+// prepare(st) enqueues them on lane 0 behind the last push; the packed offsets, `tables` and the total are read back;
+// when the total, in elements of elem bytes, fits capacity, each chunk of the last push -- one stretch [lo, hi) of the
+// packed buffer -- is written by write(lane, s0, ns, lo) into the lane's stage and copied to out, followed by the
+// chunk's slots of `rewritten` (nullable host), a table that write changes.
+template <class Prepare, class Write>
+rpl_result packed_host(rpl_capsule_stream* cs, Prepare prepare, uint64_t* offsets, const unsigned long long* offsets_dev,
+                       std::initializer_list<SlotTable> tables, uint64_t* total, const unsigned long long* total_dev,
+                       uint64_t capacity, const char* too_small, size_t elem, uint8_t* out, SlotTable rewritten,
+                       Write write) {
+  rpl_ctx* c = cs->c;
+  const uint32_t NS = cs->n_streams * cs->max_scans;
+  cudaStream_t st = c->lane[0].stream;
+  for (int i = 0; i < kLanes; ++i) RPL_CUDA(c, cudaStreamWaitEvent(c->lane[i].stream, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
+  if (const rpl_result r = prepare(st); r != RPL_RESULT_OK) {
+    cudaStreamSynchronize(st);
+    return r;
+  }
+  const cudaMemcpyKind d2h = cudaMemcpyDeviceToHost;
+  RPL_CUDA(c, cudaMemcpyAsync(offsets, offsets_dev, (size_t)NS * 8, d2h, st), RPL_RESULT_OPERATION_FAIL);
+  for (const SlotTable& t : tables)
+    RPL_CUDA(c, cudaMemcpyAsync(t.host, t.dev, (size_t)NS * 4, d2h, st), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaMemcpyAsync(total, total_dev, 8, d2h, st), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);
+  const uint64_t end = *total;
+  if (end > capacity) {
+    c->err = too_small;
+    return RPL_RESULT_INSUFFICIENT_MEMORY;
+  }
+  const uint32_t chunk = cs->cloud_chunk;
+  auto stretch = [&](uint32_t s0, uint32_t ns) {
+    const uint32_t i0 = s0 * cs->max_scans, i1 = (s0 + ns) * cs->max_scans;
+    const uint64_t hi = i1 < NS ? std::min<uint64_t>(offsets[i1], end) : end;
+    return std::make_pair(std::min<uint64_t>(offsets[i0], hi), hi);
+  };
+  size_t most = 0;
+  for (uint32_t s0 = 0; s0 < cs->n_streams; s0 += chunk) {
+    const auto [lo, hi] = stretch(s0, std::min(chunk, cs->n_streams - s0));
+    most = std::max<size_t>(most, hi - lo);
+  }
+  if (const rpl_result g = grow_stage(c, kLanes, [&](Carve& k) { k.take<uint8_t>(most * elem); }); g != RPL_RESULT_OK)
+    return g;
+  auto run_chunk = [&](Lane& l, uint32_t s0, uint32_t ns) -> rpl_result {
+    const auto [lo, hi] = stretch(s0, ns);
+    if (hi == lo) return RPL_RESULT_OK;  // nothing of this chunk is packed: the tables read back stand
+    RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);  // the lane's previous chunk has left
+    const rpl_result r = write(l, s0, ns, lo);
+    if (r != RPL_RESULT_OK) return r;
+    RPL_CUDA(c, cudaMemcpyAsync(out + lo * elem, l.stage, (hi - lo) * elem, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
+    if (rewritten.host) {
+      const size_t so = (size_t)s0 * cs->max_scans;
+      RPL_CUDA(c, cudaMemcpyAsync(rewritten.host + so, rewritten.dev + so, (size_t)ns * cs->max_scans * 4, d2h, l.stream),
+               RPL_RESULT_OPERATION_FAIL);
+    }
+    return RPL_RESULT_OK;
+  };
+  return run_chunks(c, cs->n_streams, chunk, run_chunk);
 }
 
 rpl_result stream_msgs(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* params, int64_t clock_offset_ns,
@@ -2205,48 +2263,14 @@ rpl_result stream_msgs(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* pa
   if (const rpl_result r = grow_msg_work(cs, k.bytes); r != RPL_RESULT_OK) return r;
   Carve kw{cs->msg_work};
   const MsgWork w = msg_work_layout(cs, kind, true, kw);
-  const uint32_t NS = cs->n_streams * cs->max_scans;
-  cudaStream_t st = c->lane[0].stream;
-  for (int i = 0; i < kLanes; ++i) RPL_CUDA(c, cudaStreamWaitEvent(c->lane[i].stream, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
-  rpl_result r = msgs_prepare(cs, kind, params, w, capacity, w.offsets, w.sizes, w.total, st);
-  if (r != RPL_RESULT_OK) {
-    cudaStreamSynchronize(st);
-    return r;
-  }
-  const cudaMemcpyKind d2h = cudaMemcpyDeviceToHost;
-  RPL_CUDA(c, cudaMemcpyAsync(msg_offsets, w.offsets, (size_t)NS * 8, d2h, st), RPL_RESULT_OPERATION_FAIL);
-  RPL_CUDA(c, cudaMemcpyAsync(msg_sizes, w.sizes, (size_t)NS * 4, d2h, st), RPL_RESULT_OPERATION_FAIL);
-  RPL_CUDA(c, cudaMemcpyAsync(total_bytes, w.total, 8, d2h, st), RPL_RESULT_OPERATION_FAIL);
-  RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);
-  const uint64_t total = *total_bytes;
-  if (total > capacity) {
-    c->err = "the messages need more than capacity bytes (total_bytes tells how many)";
-    return RPL_RESULT_INSUFFICIENT_MEMORY;
-  }
-  // the chunks of the last push: each one's messages are one stretch [lo, hi) of the packed buffer
-  const uint32_t chunk = cs->cloud_chunk;
-  auto stretch = [&](uint32_t s0, uint32_t ns) {
-    const uint32_t i0 = s0 * cs->max_scans, i1 = (s0 + ns) * cs->max_scans;
-    const uint64_t hi = i1 < NS ? std::min<uint64_t>(msg_offsets[i1], total) : total;
-    return std::make_pair(std::min<uint64_t>(msg_offsets[i0], hi), hi);
-  };
-  size_t most = 0;
-  for (uint32_t s0 = 0; s0 < cs->n_streams; s0 += chunk) {
-    const auto [lo, hi] = stretch(s0, std::min(chunk, cs->n_streams - s0));
-    most = std::max<size_t>(most, hi - lo);
-  }
-  if (const rpl_result g = grow_stage(c, kLanes, [&](Carve& k) { k.take<uint8_t>(most); }); g != RPL_RESULT_OK) return g;
-  auto run_chunk = [&](Lane& l, uint32_t s0, uint32_t ns) -> rpl_result {
-    const auto [lo, hi] = stretch(s0, ns);
-    if (hi == lo) return RPL_RESULT_OK;
-    RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);  // the lane's previous chunk has left
-    const rpl_result wr = msgs_write(cs, kind, params, clock_offset_ns, w, w.offsets, w.sizes, s0 * cs->max_scans,
-                                     ns * cs->max_scans, l.stage, lo, l.stream);
-    if (wr != RPL_RESULT_OK) return wr;
-    RPL_CUDA(c, cudaMemcpyAsync(msgs + lo, l.stage, hi - lo, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
-    return RPL_RESULT_OK;
-  };
-  return run_chunks(c, cs->n_streams, chunk, run_chunk);
+  return packed_host(
+      cs, [&](cudaStream_t st) { return msgs_prepare(cs, kind, params, w, capacity, w.offsets, w.sizes, w.total, st); },
+      msg_offsets, w.offsets, {{msg_sizes, w.sizes}}, total_bytes, w.total, capacity,
+      "the messages need more than capacity bytes (total_bytes tells how many)", 1, msgs, SlotTable{},
+      [&](Lane& l, uint32_t s0, uint32_t ns, uint64_t lo) {
+        return msgs_write(cs, kind, params, clock_offset_ns, w, w.offsets, w.sizes, s0 * cs->max_scans,
+                          ns * cs->max_scans, l.stage, lo, l.stream);
+      });
 }
 
 // ---- grabbed node buffers of the last push (DESIGN.md 5.7.1 "Session nodes") -------------------------------------
@@ -2313,22 +2337,15 @@ rpl_result nodes_prepare(rpl_capsule_stream* cs, const NodeWork& w, uint32_t app
   return RPL_RESULT_OK;
 }
 
-// The buffers of the scans of streams [s0, s0 + ns), one chunk of the last push (its views count from node 0 of stream
-// s0 in the push's arena), placed behind `out`; status points at the chunk's first slot.  One EMIT instantiation
+// The buffers of the scans of one chunk of the last push (last_push_scans), placed behind `out`; status points at the
+// chunk's first slot.  One EMIT instantiation
 // serves every ascended slot: the ascended buffer does not depend on the LaserScan mode, and no LaserScan is computed.
 rpl_result stream_nodes_chunk(rpl_capsule_stream* cs, Lane& l, uint32_t s0, uint32_t ns, NodeKinds kinds,
                               const unsigned long long* place, rpl_node_hq* out, uint32_t* status, cudaStream_t st) {
   rpl_ctx* c = cs->c;
-  const size_t so = (size_t)s0 * cs->max_scans;
-  rpl::ScanBatchArgs a{};
-  a.nodes = reinterpret_cast<const uint2*>(cs->arena[cs->cloud_arena] + (size_t)s0 * cs->stride_nodes);
-  a.views = reinterpret_cast<const uint2*>(cs->views + so);
-  a.counts = reinterpret_cast<const uint32_t*>(a.views);
-  a.nodes_total = (unsigned long long)ns * cs->stride_nodes;
-  a.n_scans = ns * cs->max_scans;
-  a.stride = cs->max_nodes;
+  rpl::ScanBatchArgs a = last_push_scans(cs, s0, ns);
   a.nodes_out = reinterpret_cast<uint2*>(out);
-  a.out_first = place + so;
+  a.out_first = place + (size_t)s0 * cs->max_scans;
   a.status = status;
   a.apply_ascend = 1;
   a.fallback_list = l.fallback_list;
@@ -2351,23 +2368,20 @@ rpl_result stream_nodes_dev(rpl_capsule_stream* cs, uint32_t apply_ascend, const
                             uint64_t capacity, uint64_t* node_offsets, uint32_t* node_counts, uint32_t* status,
                             uint64_t* total_nodes, void* stream) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
-  rpl_ctx* c = cs->c;
   if (!stream_nodes_args_ok(cs, nodes, node_offsets, node_counts, status, total_nodes, true)) return RPL_RESULT_INVALID_DATA;
-  cudaStream_t st;
-  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   Carve k{cs->node_work};
   const NodeWork w = node_work_layout(cs, k);
-  // the last push's kernels (and an earlier nodes call's, which read the same tables) are done before these; the next
-  // push waits for these
-  RPL_CUDA(c, cudaStreamWaitEvent(st, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
-  rpl_result r = nodes_prepare(cs, w, apply_ascend, per_stream, capacity, reinterpret_cast<unsigned long long*>(node_offsets),
-                               node_counts, status, reinterpret_cast<unsigned long long*>(total_nodes), false, st);
-  const NodeKinds kinds = node_kinds(cs, apply_ascend, per_stream);
-  for (uint32_t s0 = 0; s0 < cs->n_streams && r == RPL_RESULT_OK; s0 += cs->cloud_chunk)
-    r = stream_nodes_chunk(cs, c->lane[0], s0, std::min(cs->cloud_chunk, cs->n_streams - s0), kinds, w.place, nodes,
-                           status + (size_t)s0 * cs->max_scans, st);
-  RPL_CUDA(c, cudaEventRecord(cs->done, st), RPL_RESULT_OPERATION_FAIL);
-  return r;
+  // (an earlier nodes call reads the same tables: behind the last push, it is done before these too)
+  return last_push_dev(cs, stream, 0, [&](cudaStream_t st) -> rpl_result {
+    rpl_result r = nodes_prepare(cs, w, apply_ascend, per_stream, capacity,
+                                 reinterpret_cast<unsigned long long*>(node_offsets), node_counts, status,
+                                 reinterpret_cast<unsigned long long*>(total_nodes), false, st);
+    const NodeKinds kinds = node_kinds(cs, apply_ascend, per_stream);
+    for (uint32_t s0 = 0; s0 < cs->n_streams && r == RPL_RESULT_OK; s0 += cs->cloud_chunk)
+      r = stream_nodes_chunk(cs, cs->c->lane[0], s0, std::min(cs->cloud_chunk, cs->n_streams - s0), kinds, w.place,
+                             nodes, status + (size_t)s0 * cs->max_scans, st);
+    return r;
+  });
 }
 
 rpl_result stream_nodes(rpl_capsule_stream* cs, uint32_t apply_ascend, const uint8_t* per_stream, rpl_node_hq* nodes,
@@ -2379,54 +2393,20 @@ rpl_result stream_nodes(rpl_capsule_stream* cs, uint32_t apply_ascend, const uin
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
   Carve k{cs->node_work};
   const NodeWork w = node_work_layout(cs, k);
-  const uint32_t NS = cs->n_streams * cs->max_scans;
-  cudaStream_t st = c->lane[0].stream;
-  for (int i = 0; i < kLanes; ++i) RPL_CUDA(c, cudaStreamWaitEvent(c->lane[i].stream, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
-  const rpl_result p = nodes_prepare(cs, w, apply_ascend, per_stream, capacity, w.offsets, w.counts, w.status, w.total, true, st);
-  if (p != RPL_RESULT_OK) {
-    cudaStreamSynchronize(st);
-    return p;
-  }
-  const cudaMemcpyKind d2h = cudaMemcpyDeviceToHost;
-  RPL_CUDA(c, cudaMemcpyAsync(node_offsets, w.offsets, (size_t)NS * 8, d2h, st), RPL_RESULT_OPERATION_FAIL);
-  RPL_CUDA(c, cudaMemcpyAsync(node_counts, w.counts, (size_t)NS * 4, d2h, st), RPL_RESULT_OPERATION_FAIL);
-  RPL_CUDA(c, cudaMemcpyAsync(status, w.status, (size_t)NS * 4, d2h, st), RPL_RESULT_OPERATION_FAIL);
-  RPL_CUDA(c, cudaMemcpyAsync(total_nodes, w.total, 8, d2h, st), RPL_RESULT_OPERATION_FAIL);
-  RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);
-  const uint64_t total = *total_nodes;
-  if (total > capacity) {
-    c->err = "the buffers need more than capacity_nodes nodes (total_nodes tells how many)";
-    return RPL_RESULT_INSUFFICIENT_MEMORY;
-  }
-  // the chunks of the last push: each one's buffers are one stretch [lo, hi) of the packed buffer, in nodes
-  const uint32_t chunk = cs->cloud_chunk;
-  auto stretch = [&](uint32_t s0, uint32_t ns) {
-    const uint32_t i0 = s0 * cs->max_scans, i1 = (s0 + ns) * cs->max_scans;
-    const uint64_t hi = i1 < NS ? std::min<uint64_t>(node_offsets[i1], total) : total;
-    return std::make_pair(std::min<uint64_t>(node_offsets[i0], hi), hi);
-  };
-  size_t most = 0;
-  for (uint32_t s0 = 0; s0 < cs->n_streams; s0 += chunk) {
-    const auto [lo, hi] = stretch(s0, std::min(chunk, cs->n_streams - s0));
-    most = std::max<size_t>(most, hi - lo);
-  }
-  if (const rpl_result g = grow_stage(c, kLanes, [&](Carve& s) { s.take<rpl_node_hq>(most); }); g != RPL_RESULT_OK) return g;
   const NodeKinds kinds = node_kinds(cs, apply_ascend, per_stream);
-  auto run_chunk = [&](Lane& l, uint32_t s0, uint32_t ns) -> rpl_result {
-    const auto [lo, hi] = stretch(s0, ns);
-    if (hi == lo) return RPL_RESULT_OK;  // no buffer in this chunk: the directory's statuses stand
-    const size_t so = (size_t)s0 * cs->max_scans;
-    RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);  // the lane's previous chunk has left
-    rpl_node_hq* stage = reinterpret_cast<rpl_node_hq*>(l.stage);
-    const rpl_result r = stream_nodes_chunk(cs, l, s0, ns, kinds, w.place, stage, w.status + so, l.stream);
-    if (r != RPL_RESULT_OK) return r;
-    RPL_CUDA(c, cudaMemcpyAsync(nodes + lo, stage, (hi - lo) * sizeof(rpl_node_hq), d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
-    if (kinds.ascended)
-      RPL_CUDA(c, cudaMemcpyAsync(status + so, w.status + so, (size_t)ns * cs->max_scans * 4, d2h, l.stream),
-               RPL_RESULT_OPERATION_FAIL);
-    return RPL_RESULT_OK;
-  };
-  return run_chunks(c, cs->n_streams, chunk, run_chunk);
+  // an ascended chunk's kernels rewrite its statuses
+  return packed_host(
+      cs,
+      [&](cudaStream_t st) {
+        return nodes_prepare(cs, w, apply_ascend, per_stream, capacity, w.offsets, w.counts, w.status, w.total, true, st);
+      },
+      node_offsets, w.offsets, {{node_counts, w.counts}, {status, w.status}}, total_nodes, w.total, capacity,
+      "the buffers need more than capacity_nodes nodes (total_nodes tells how many)", sizeof(rpl_node_hq),
+      reinterpret_cast<uint8_t*>(nodes), SlotTable{kinds.ascended ? status : nullptr, w.status},
+      [&](Lane& l, uint32_t s0, uint32_t ns, uint64_t) {
+        return stream_nodes_chunk(cs, l, s0, ns, kinds, w.place, reinterpret_cast<rpl_node_hq*>(l.stage),
+                                  w.status + (size_t)s0 * cs->max_scans, l.stream);
+      });
 }
 
 }  // namespace
@@ -2496,10 +2476,11 @@ rpl_result rpl_capsule_stream_create(rpl_ctx* c, uint32_t ans_type, uint32_t n_s
   if (!c || !out) return RPL_RESULT_INVALID_DATA;
   *out = nullptr;
   if (rpl_capsule_bytes(ans_type) == 0) {
-    c->err = "a stream session takes the capsule answer types 0x82..0x86 (0x81 standard nodes are no capsules)";
+    c->err = "a stream session takes the capsule answer types 0x82..0x86 (0x81 standard-node bytes: "
+             "rpl_capsule_stream_create_bytes)";
     return RPL_RESULT_INVALID_DATA;
   }
-  return stream_create(c, ans_type, n_streams, stride_capsules, max_nodes, max_scans, out);
+  return stream_create(c, ans_type, false, n_streams, stride_capsules, max_nodes, max_scans, out);
 }
 
 void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
@@ -2541,15 +2522,15 @@ rpl_result rpl_capsule_stream_push(rpl_capsule_stream* cs, const uint8_t* capsul
                                    float* intensities, uint32_t* beam_counts, float* angle_increment,
                                    uint32_t* scans_per_stream) {
   return stream_push(cs, capsules, capsule_counts, sample_duration_us, params, ranges, intensities, beam_counts,
-                     angle_increment, scans_per_stream, nullptr);
+                     angle_increment, scans_per_stream, nullptr, false, false, nullptr);
 }
 
 rpl_result rpl_capsule_stream_push_dev(rpl_capsule_stream* cs, const uint8_t* capsules, const uint32_t* capsule_counts,
                                        uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
                                        float* intensities, uint32_t* beam_counts, float* angle_increment,
                                        uint32_t* scans_per_stream, void* stream) {
-  return stream_push_dev(cs, capsules, capsule_counts, sample_duration_us, params, ranges, intensities, beam_counts,
-                         angle_increment, scans_per_stream, stream, nullptr);
+  return stream_push(cs, capsules, capsule_counts, sample_duration_us, params, ranges, intensities, beam_counts,
+                     angle_increment, scans_per_stream, nullptr, false, true, stream);
 }
 
 rpl_result rpl_capsule_stream_push_ts(rpl_capsule_stream* cs, const uint8_t* capsules, const uint32_t* capsule_counts,
@@ -2560,7 +2541,7 @@ rpl_result rpl_capsule_stream_push_ts(rpl_capsule_stream* cs, const uint8_t* cap
   StampPush sp{};
   if (!stamp_args_ok(cs, params, timing, capsule_rx_us, 1, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
   return stream_push(cs, capsules, capsule_counts, timing ? timing->sample_duration_us : 0u, params, ranges, intensities,
-                     beam_counts, angle_increment, scans_per_stream, &sp);
+                     beam_counts, angle_increment, scans_per_stream, &sp, false, false, nullptr);
 }
 
 rpl_result rpl_capsule_stream_push_ts_dev(rpl_capsule_stream* cs, const uint8_t* capsules,
@@ -2570,8 +2551,8 @@ rpl_result rpl_capsule_stream_push_ts_dev(rpl_capsule_stream* cs, const uint8_t*
                                           uint32_t* scans_per_stream, uint64_t* scan_begin_ts_us, void* stream) {
   StampPush sp{};
   if (!stamp_args_ok(cs, params, timing, capsule_rx_us, 1, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
-  return stream_push_dev(cs, capsules, capsule_counts, timing ? timing->sample_duration_us : 0u, params, ranges, intensities,
-                         beam_counts, angle_increment, scans_per_stream, stream, &sp);
+  return stream_push(cs, capsules, capsule_counts, timing ? timing->sample_duration_us : 0u, params, ranges, intensities,
+                     beam_counts, angle_increment, scans_per_stream, &sp, false, true, stream);
 }
 
 rpl_result rpl_capsule_stream_reset(rpl_capsule_stream* cs, const uint8_t* stream_mask) {
@@ -2602,53 +2583,47 @@ rpl_result rpl_capsule_stream_reset(rpl_capsule_stream* cs, const uint8_t* strea
   return RPL_RESULT_OK;
 }
 
-rpl_result rpl_capsule_stream_state(rpl_capsule_stream* cs, uint32_t* open_nodes, uint32_t* held_capsule) {
-  return rpl_capsule_stream_state_bytes(cs, open_nodes, held_capsule, nullptr);
-}
-
-rpl_result rpl_capsule_stream_state_bytes(rpl_capsule_stream* cs, uint32_t* open_nodes, uint32_t* held_capsule,
-                                          uint32_t* held_bytes) {
+rpl_result rpl_capsule_stream_state(rpl_capsule_stream* cs, uint32_t* open_nodes, uint32_t* held_capsule,
+                                    uint32_t* held_bytes) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
   rpl_ctx* c = cs->c;
+  const bool normal = cs->ans_type == RPL_ANS_MEASUREMENT;
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
   RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);
   if (open_nodes)
     RPL_CUDA(c, cudaMemcpy(open_nodes, cs->carry_len[cs->parity], (size_t)cs->n_streams * 4, cudaMemcpyDeviceToHost),
              RPL_RESULT_OPERATION_FAIL);
-  std::vector<uint32_t> fr;  // a byte session's framer records
+  std::vector<uint32_t> fr;  // a capsule byte session's framer records
   if (cs->framer && (held_capsule || held_bytes)) {
     fr.resize((size_t)cs->n_streams * rpl::kFramerWords);
     RPL_CUDA(c, cudaMemcpy(fr.data(), cs->framer, fr.size() * 4, cudaMemcpyDeviceToHost), RPL_RESULT_OPERATION_FAIL);
   }
-  if (held_capsule) {  // HQ: the record stays zero; 0x81: the byte machine's state, 0..4 bytes held
-    std::vector<uint32_t> h((size_t)cs->n_streams * rpl::kHeldWords);
+  // the held records: HQ's stays zero; 0x81's holds the byte machine's state, 0..4 bytes held
+  std::vector<uint32_t> h;
+  if (held_capsule || (held_bytes && normal)) {
+    h.resize((size_t)cs->n_streams * rpl::kHeldWords);
     RPL_CUDA(c, cudaMemcpy(h.data(), cs->held, h.size() * 4, cudaMemcpyDeviceToHost), RPL_RESULT_OPERATION_FAIL);
-    for (uint32_t s = 0; s < cs->n_streams; ++s) {
-      held_capsule[s] = h[(size_t)s * rpl::kHeldWords + rpl::kHeldOk];
-      // skipped bytes waiting to be reported: the next frame releases nothing (the SDK cleared its ready flag)
-      if (!fr.empty() && fr[(size_t)s * rpl::kFramerWords + rpl::kFramerLost]) held_capsule[s] = 0;
-    }
   }
-  if (held_bytes)
-    for (uint32_t s = 0; s < cs->n_streams; ++s)
-      held_bytes[s] = fr.empty() ? 0u : fr[(size_t)s * rpl::kFramerWords + rpl::kFramerPos];
+  for (uint32_t s = 0; s < cs->n_streams; ++s) {
+    const uint32_t ok = h.empty() ? 0u : h[(size_t)s * rpl::kHeldWords + rpl::kHeldOk];
+    const uint32_t* f = fr.empty() ? nullptr : fr.data() + (size_t)s * rpl::kFramerWords;
+    // skipped bytes waiting to be reported: the next frame releases nothing (the SDK cleared its ready flag)
+    if (held_capsule) held_capsule[s] = normal || (f && f[rpl::kFramerLost]) ? 0u : ok;
+    if (held_bytes) held_bytes[s] = normal ? ok : f ? f[rpl::kFramerPos] : 0u;
+  }
   return RPL_RESULT_OK;
 }
 
-// ---- byte sessions: the capsule session fed the raw serial stream ----
+// ---- byte sessions: the session fed the raw serial stream (0x81: the standard-node session) ----
 rpl_result rpl_capsule_stream_create_bytes(rpl_ctx* c, uint32_t ans_type, uint32_t n_streams, uint32_t stride_bytes,
                                            uint32_t max_nodes, uint32_t max_scans, rpl_capsule_stream** out) {
   if (!c || !out) return RPL_RESULT_INVALID_DATA;
   *out = nullptr;
-  if (rpl_capsule_bytes(ans_type) == 0) {
-    c->err = "a byte session takes the capsule answer types 0x82..0x86 (0x81 standard-node bytes: rpl_normal_stream)";
+  if (ans_type != RPL_ANS_MEASUREMENT && rpl_capsule_bytes(ans_type) == 0) {
+    c->err = "a byte session takes the measurement answer types 0x81..0x86";
     return RPL_RESULT_INVALID_DATA;
   }
-  if (stride_bytes == 0) {
-    c->err = "need n_streams > 0, stride_bytes > 0, max_scans > 0 and an even max_nodes in [2, 8192]";
-    return RPL_RESULT_INVALID_DATA;
-  }
-  return stream_create(c, ans_type, n_streams, 0, max_nodes, max_scans, out, stride_bytes);
+  return stream_create(c, ans_type, true, n_streams, stride_bytes, max_nodes, max_scans, out);
 }
 
 rpl_result rpl_capsule_stream_push_bytes(rpl_capsule_stream* cs, const uint8_t* bytes, const uint32_t* byte_counts,
@@ -2656,15 +2631,15 @@ rpl_result rpl_capsule_stream_push_bytes(rpl_capsule_stream* cs, const uint8_t* 
                                          float* intensities, uint32_t* beam_counts, float* angle_increment,
                                          uint32_t* scans_per_stream) {
   return stream_push(cs, bytes, byte_counts, sample_duration_us, params, ranges, intensities, beam_counts,
-                     angle_increment, scans_per_stream, nullptr, true);
+                     angle_increment, scans_per_stream, nullptr, true, false, nullptr);
 }
 
 rpl_result rpl_capsule_stream_push_bytes_dev(rpl_capsule_stream* cs, const uint8_t* bytes, const uint32_t* byte_counts,
                                              uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
                                              float* intensities, uint32_t* beam_counts, float* angle_increment,
                                              uint32_t* scans_per_stream, void* stream) {
-  return stream_push_dev(cs, bytes, byte_counts, sample_duration_us, params, ranges, intensities, beam_counts,
-                         angle_increment, scans_per_stream, stream, nullptr, true);
+  return stream_push(cs, bytes, byte_counts, sample_duration_us, params, ranges, intensities, beam_counts,
+                     angle_increment, scans_per_stream, nullptr, true, true, stream);
 }
 
 rpl_result rpl_capsule_stream_push_bytes_ts(rpl_capsule_stream* cs, const uint8_t* bytes, const uint32_t* byte_counts,
@@ -2675,7 +2650,7 @@ rpl_result rpl_capsule_stream_push_bytes_ts(rpl_capsule_stream* cs, const uint8_
   StampPush sp{};
   if (!stamp_args_ok(cs, params, timing, chunk_rx_us, chunk_bytes, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
   return stream_push(cs, bytes, byte_counts, timing ? timing->sample_duration_us : 0u, params, ranges, intensities, beam_counts,
-                     angle_increment, scans_per_stream, &sp, true);
+                     angle_increment, scans_per_stream, &sp, true, false, nullptr);
 }
 
 rpl_result rpl_capsule_stream_push_bytes_ts_dev(rpl_capsule_stream* cs, const uint8_t* bytes,
@@ -2686,123 +2661,8 @@ rpl_result rpl_capsule_stream_push_bytes_ts_dev(rpl_capsule_stream* cs, const ui
                                                 uint32_t* scans_per_stream, uint64_t* scan_begin_ts_us, void* stream) {
   StampPush sp{};
   if (!stamp_args_ok(cs, params, timing, chunk_rx_us, chunk_bytes, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
-  return stream_push_dev(cs, bytes, byte_counts, timing ? timing->sample_duration_us : 0u, params, ranges, intensities, beam_counts,
-                         angle_increment, scans_per_stream, stream, &sp, true);
-}
-
-// ---- the dense session: the capsule session fixed to 0x85 ----
-rpl_result rpl_dense_stream_create(rpl_ctx* c, uint32_t n_streams, uint32_t stride_capsules, uint32_t max_nodes,
-                                   uint32_t max_scans, rpl_dense_stream** out) {
-  if (!c || !out) return RPL_RESULT_INVALID_DATA;
-  rpl_capsule_stream* cs = nullptr;
-  const rpl_result r = rpl_capsule_stream_create(c, 0x85, n_streams, stride_capsules, max_nodes, max_scans, &cs);
-  *out = reinterpret_cast<rpl_dense_stream*>(cs);
-  return r;
-}
-
-void rpl_dense_stream_destroy(rpl_dense_stream* ds) { rpl_capsule_stream_destroy(capsule_session(ds)); }
-
-rpl_result rpl_dense_stream_push(rpl_dense_stream* ds, const uint8_t* capsules, const uint32_t* capsule_counts,
-                                 uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
-                                 float* intensities, uint32_t* beam_counts, float* angle_increment,
-                                 uint32_t* scans_per_stream) {
-  return rpl_capsule_stream_push(capsule_session(ds), capsules, capsule_counts, sample_duration_us, params, ranges,
-                                 intensities, beam_counts, angle_increment, scans_per_stream);
-}
-
-rpl_result rpl_dense_stream_push_dev(rpl_dense_stream* ds, const uint8_t* capsules, const uint32_t* capsule_counts,
-                                     uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
-                                     float* intensities, uint32_t* beam_counts, float* angle_increment,
-                                     uint32_t* scans_per_stream, void* stream) {
-  return rpl_capsule_stream_push_dev(capsule_session(ds), capsules, capsule_counts, sample_duration_us, params, ranges,
-                                     intensities, beam_counts, angle_increment, scans_per_stream, stream);
-}
-
-rpl_result rpl_dense_stream_push_ts(rpl_dense_stream* ds, const uint8_t* capsules, const uint32_t* capsule_counts,
-                                    const rpl_timing* timing, const uint64_t* capsule_rx_us,
-                                    const rpl_scan_params* params, float* ranges, float* intensities,
-                                    uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
-                                    uint64_t* scan_begin_ts_us) {
-  return rpl_capsule_stream_push_ts(capsule_session(ds), capsules, capsule_counts, timing, capsule_rx_us, params,
-                                    ranges, intensities, beam_counts, angle_increment, scans_per_stream,
-                                    scan_begin_ts_us);
-}
-
-rpl_result rpl_dense_stream_push_ts_dev(rpl_dense_stream* ds, const uint8_t* capsules, const uint32_t* capsule_counts,
-                                        const rpl_timing* timing, const uint64_t* capsule_rx_us,
-                                        const rpl_scan_params* params, float* ranges, float* intensities,
-                                        uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
-                                        uint64_t* scan_begin_ts_us, void* stream) {
-  return rpl_capsule_stream_push_ts_dev(capsule_session(ds), capsules, capsule_counts, timing, capsule_rx_us, params,
-                                        ranges, intensities, beam_counts, angle_increment, scans_per_stream,
-                                        scan_begin_ts_us, stream);
-}
-
-rpl_result rpl_dense_stream_reset(rpl_dense_stream* ds, const uint8_t* stream_mask) {
-  return rpl_capsule_stream_reset(capsule_session(ds), stream_mask);
-}
-
-rpl_result rpl_dense_stream_state(rpl_dense_stream* ds, uint32_t* open_nodes, uint32_t* held_capsule) {
-  return rpl_capsule_stream_state(capsule_session(ds), open_nodes, held_capsule);
-}
-
-// ---- the standard-node session: the capsule session on 0x81 bytes ----
-rpl_result rpl_normal_stream_create(rpl_ctx* c, uint32_t n_streams, uint32_t stride_bytes, uint32_t max_nodes,
-                                    uint32_t max_scans, rpl_normal_stream** out) {
-  if (!c || !out) return RPL_RESULT_INVALID_DATA;
-  rpl_capsule_stream* cs = nullptr;
-  const rpl_result r = stream_create(c, RPL_ANS_MEASUREMENT, n_streams, stride_bytes, max_nodes, max_scans, &cs);
-  *out = reinterpret_cast<rpl_normal_stream*>(cs);
-  return r;
-}
-
-void rpl_normal_stream_destroy(rpl_normal_stream* ns) { rpl_capsule_stream_destroy(capsule_session(ns)); }
-
-rpl_result rpl_normal_stream_push(rpl_normal_stream* ns, const uint8_t* bytes, const uint32_t* byte_counts,
-                                  const rpl_scan_params* params, float* ranges, float* intensities,
-                                  uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream) {
-  return rpl_capsule_stream_push(capsule_session(ns), bytes, byte_counts, 0, params, ranges, intensities, beam_counts,
-                                 angle_increment, scans_per_stream);
-}
-
-rpl_result rpl_normal_stream_push_dev(rpl_normal_stream* ns, const uint8_t* bytes, const uint32_t* byte_counts,
-                                      const rpl_scan_params* params, float* ranges, float* intensities,
-                                      uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
-                                      void* stream) {
-  return rpl_capsule_stream_push_dev(capsule_session(ns), bytes, byte_counts, 0, params, ranges, intensities,
-                                     beam_counts, angle_increment, scans_per_stream, stream);
-}
-
-rpl_result rpl_normal_stream_push_ts(rpl_normal_stream* ns, const uint8_t* bytes, const uint32_t* byte_counts,
-                                     const rpl_timing* timing, uint32_t chunk_bytes, const uint64_t* chunk_rx_us,
-                                     const rpl_scan_params* params, float* ranges, float* intensities,
-                                     uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
-                                     uint64_t* scan_begin_ts_us) {
-  rpl_capsule_stream* cs = capsule_session(ns);
-  StampPush sp{};
-  if (!stamp_args_ok(cs, params, timing, chunk_rx_us, chunk_bytes, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
-  return stream_push(cs, bytes, byte_counts, 0, params, ranges, intensities, beam_counts, angle_increment,
-                     scans_per_stream, &sp);
-}
-
-rpl_result rpl_normal_stream_push_ts_dev(rpl_normal_stream* ns, const uint8_t* bytes, const uint32_t* byte_counts,
-                                         const rpl_timing* timing, uint32_t chunk_bytes, const uint64_t* chunk_rx_us,
-                                         const rpl_scan_params* params, float* ranges, float* intensities,
-                                         uint32_t* beam_counts, float* angle_increment, uint32_t* scans_per_stream,
-                                         uint64_t* scan_begin_ts_us, void* stream) {
-  rpl_capsule_stream* cs = capsule_session(ns);
-  StampPush sp{};
-  if (!stamp_args_ok(cs, params, timing, chunk_rx_us, chunk_bytes, scan_begin_ts_us, &sp)) return RPL_RESULT_INVALID_DATA;
-  return stream_push_dev(cs, bytes, byte_counts, 0, params, ranges, intensities, beam_counts, angle_increment,
-                         scans_per_stream, stream, &sp);
-}
-
-rpl_result rpl_normal_stream_reset(rpl_normal_stream* ns, const uint8_t* stream_mask) {
-  return rpl_capsule_stream_reset(capsule_session(ns), stream_mask);
-}
-
-rpl_result rpl_normal_stream_state(rpl_normal_stream* ns, uint32_t* open_nodes, uint32_t* held_bytes) {
-  return rpl_capsule_stream_state(capsule_session(ns), open_nodes, held_bytes);
+  return stream_push(cs, bytes, byte_counts, timing ? timing->sample_duration_us : 0u, params, ranges, intensities, beam_counts,
+                     angle_increment, scans_per_stream, &sp, true, true, stream);
 }
 
 // ---- session clouds: the PointCloud2 chain over the scans the last push published, read in place ----
@@ -2818,30 +2678,6 @@ rpl_result rpl_capsule_stream_nodes(rpl_capsule_stream* cs, uint32_t apply_ascen
   return stream_nodes(cs, apply_ascend, ascend_per_stream, nodes, capacity_nodes, node_offsets, node_counts, status,
                       total_nodes);
 }
-rpl_result rpl_dense_stream_nodes_dev(rpl_dense_stream* ds, uint32_t apply_ascend, const uint8_t* ascend_per_stream,
-                                        rpl_node_hq* nodes, uint64_t capacity_nodes, uint64_t* node_offsets,
-                                        uint32_t* node_counts, uint32_t* status, uint64_t* total_nodes, void* stream) {
-  return stream_nodes_dev(capsule_session(ds), apply_ascend, ascend_per_stream, nodes, capacity_nodes, node_offsets, node_counts, status,
-                          total_nodes, stream);
-}
-rpl_result rpl_dense_stream_nodes(rpl_dense_stream* ds, uint32_t apply_ascend, const uint8_t* ascend_per_stream,
-                                    rpl_node_hq* nodes, uint64_t capacity_nodes, uint64_t* node_offsets,
-                                    uint32_t* node_counts, uint32_t* status, uint64_t* total_nodes) {
-  return stream_nodes(capsule_session(ds), apply_ascend, ascend_per_stream, nodes, capacity_nodes, node_offsets, node_counts, status,
-                      total_nodes);
-}
-rpl_result rpl_normal_stream_nodes_dev(rpl_normal_stream* ns, uint32_t apply_ascend, const uint8_t* ascend_per_stream,
-                                        rpl_node_hq* nodes, uint64_t capacity_nodes, uint64_t* node_offsets,
-                                        uint32_t* node_counts, uint32_t* status, uint64_t* total_nodes, void* stream) {
-  return stream_nodes_dev(capsule_session(ns), apply_ascend, ascend_per_stream, nodes, capacity_nodes, node_offsets, node_counts, status,
-                          total_nodes, stream);
-}
-rpl_result rpl_normal_stream_nodes(rpl_normal_stream* ns, uint32_t apply_ascend, const uint8_t* ascend_per_stream,
-                                    rpl_node_hq* nodes, uint64_t capacity_nodes, uint64_t* node_offsets,
-                                    uint32_t* node_counts, uint32_t* status, uint64_t* total_nodes) {
-  return stream_nodes(capsule_session(ns), apply_ascend, ascend_per_stream, nodes, capacity_nodes, node_offsets, node_counts, status,
-                      total_nodes);
-}
 rpl_result rpl_capsule_stream_cloud_dev(rpl_capsule_stream* cs, const rpl_cloud_params* params, float* xyzi,
                                         uint32_t* point_counts, void* stream) {
   return stream_cloud_dev(cs, params, xyzi, point_counts, stream);
@@ -2852,62 +2688,45 @@ rpl_result rpl_capsule_stream_cloud(rpl_capsule_stream* cs, const rpl_cloud_para
   return stream_cloud(cs, params, xyzi, point_counts);
 }
 
-rpl_result rpl_dense_stream_cloud_dev(rpl_dense_stream* ds, const rpl_cloud_params* params, float* xyzi,
-                                      uint32_t* point_counts, void* stream) {
-  return stream_cloud_dev(capsule_session(ds), params, xyzi, point_counts, stream);
+// ---- per-stream settings and packed messages of the last push ----------------------------------------------------
+rpl_result rpl_capsule_stream_set_frames(rpl_capsule_stream* s, const char* const* frame_ids, const float* range_max) {
+  return stream_set_frames(s, frame_ids, range_max);
 }
 
-rpl_result rpl_dense_stream_cloud(rpl_dense_stream* ds, const rpl_cloud_params* params, float* xyzi,
-                                  uint32_t* point_counts) {
-  return stream_cloud(capsule_session(ds), params, xyzi, point_counts);
+rpl_result rpl_capsule_stream_set_lidars(rpl_capsule_stream* s, const rpl_lidar_settings* settings,
+                                         const uint8_t* stream_mask) {
+  return stream_set_lidars(s, settings, stream_mask);
 }
 
-rpl_result rpl_normal_stream_cloud_dev(rpl_normal_stream* ns, const rpl_cloud_params* params, float* xyzi,
-                                       uint32_t* point_counts, void* stream) {
-  return stream_cloud_dev(capsule_session(ns), params, xyzi, point_counts, stream);
+rpl_result rpl_capsule_stream_laserscan_msgs_dev(rpl_capsule_stream* s, const rpl_scan_params* params,
+                                                 int64_t clock_offset_ns, uint8_t* msgs, uint64_t capacity,
+                                                 uint64_t* msg_offsets, uint32_t* msg_sizes, uint64_t* total_bytes,
+                                                 void* stream) {
+  return stream_msgs_dev(s, rpl::MsgKind::kLaserScan, params, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
+                         total_bytes, stream);
 }
 
-rpl_result rpl_normal_stream_cloud(rpl_normal_stream* ns, const rpl_cloud_params* params, float* xyzi,
-                                   uint32_t* point_counts) {
-  return stream_cloud(capsule_session(ns), params, xyzi, point_counts);
+rpl_result rpl_capsule_stream_laserscan_msgs(rpl_capsule_stream* s, const rpl_scan_params* params,
+                                             int64_t clock_offset_ns, uint8_t* msgs, uint64_t capacity,
+                                             uint64_t* msg_offsets, uint32_t* msg_sizes, uint64_t* total_bytes) {
+  return stream_msgs(s, rpl::MsgKind::kLaserScan, params, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
+                     total_bytes);
 }
 
-// ---- per-stream settings and packed messages of the last push, one set per session handle type ---------------------
-#define RPL_STREAM_MSGS(KIND, T, SESSION)                                                                              \
-  rpl_result rpl_##KIND##_stream_set_frames(T* s, const char* const* frame_ids, const float* range_max) {             \
-    return stream_set_frames(SESSION, frame_ids, range_max);                                                         \
-  }                                                                                                                  \
-  rpl_result rpl_##KIND##_stream_set_lidars(T* s, const rpl_lidar_settings* settings, const uint8_t* stream_mask) {  \
-    return stream_set_lidars(SESSION, settings, stream_mask);                                                        \
-  }                                                                                                                  \
-  rpl_result rpl_##KIND##_stream_laserscan_msgs_dev(T* s, const rpl_scan_params* params, int64_t clock_offset_ns,    \
-                                                    uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,         \
-                                                    uint32_t* msg_sizes, uint64_t* total_bytes, void* stream) {      \
-    return stream_msgs_dev(SESSION, rpl::MsgKind::kLaserScan, params, clock_offset_ns, msgs, capacity, msg_offsets,  \
-                           msg_sizes, total_bytes, stream);                                                          \
-  }                                                                                                                  \
-  rpl_result rpl_##KIND##_stream_laserscan_msgs(T* s, const rpl_scan_params* params, int64_t clock_offset_ns,        \
-                                                uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,             \
-                                                uint32_t* msg_sizes, uint64_t* total_bytes) {                        \
-    return stream_msgs(SESSION, rpl::MsgKind::kLaserScan, params, clock_offset_ns, msgs, capacity, msg_offsets,      \
-                       msg_sizes, total_bytes);                                                                      \
-  }                                                                                                                  \
-  rpl_result rpl_##KIND##_stream_cloud_msgs_dev(T* s, const rpl_cloud_params* params, int64_t clock_offset_ns,       \
-                                                uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,             \
-                                                uint32_t* msg_sizes, uint64_t* total_bytes, void* stream) {          \
-    return stream_msgs_dev(SESSION, rpl::MsgKind::kPointCloud2, params, clock_offset_ns, msgs, capacity,             \
-                           msg_offsets, msg_sizes, total_bytes, stream);                                             \
-  }                                                                                                                  \
-  rpl_result rpl_##KIND##_stream_cloud_msgs(T* s, const rpl_cloud_params* params, int64_t clock_offset_ns,           \
-                                            uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,                 \
-                                            uint32_t* msg_sizes, uint64_t* total_bytes) {                            \
-    return stream_msgs(SESSION, rpl::MsgKind::kPointCloud2, params, clock_offset_ns, msgs, capacity, msg_offsets,    \
-                       msg_sizes, total_bytes);                                                                      \
-  }
-RPL_STREAM_MSGS(capsule, rpl_capsule_stream, s)
-RPL_STREAM_MSGS(dense, rpl_dense_stream, capsule_session(s))
-RPL_STREAM_MSGS(normal, rpl_normal_stream, capsule_session(s))
-#undef RPL_STREAM_MSGS
+rpl_result rpl_capsule_stream_cloud_msgs_dev(rpl_capsule_stream* s, const rpl_cloud_params* params,
+                                             int64_t clock_offset_ns, uint8_t* msgs, uint64_t capacity,
+                                             uint64_t* msg_offsets, uint32_t* msg_sizes, uint64_t* total_bytes,
+                                             void* stream) {
+  return stream_msgs_dev(s, rpl::MsgKind::kPointCloud2, params, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
+                         total_bytes, stream);
+}
+
+rpl_result rpl_capsule_stream_cloud_msgs(rpl_capsule_stream* s, const rpl_cloud_params* params, int64_t clock_offset_ns,
+                                         uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
+                                         uint64_t* total_bytes) {
+  return stream_msgs(s, rpl::MsgKind::kPointCloud2, params, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
+                     total_bytes);
+}
 
 // ---- LaserScan / PointCloud2 -> CDR (SURVEY.md 8(f) rank 3) -------------------------------------
 namespace {

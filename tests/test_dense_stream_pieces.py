@@ -1,7 +1,7 @@
 """The contract of the dense stream session, pinned on the CPU: the SDK's own unpacker fed a stream in pieces, then its
 own ScanDataHolder, publishes exactly the scans the restatement (oracle/decode_oracle.cpp) publishes from the whole
-stream in one call.  The session (rpl_dense_stream_*, tests/test_gpu_dense_stream.py) is held to the latter, so this
-is what makes "any split into pushes gives the whole stream's scans" the SDK's behaviour and not a new definition.
+stream in one call.  The session (rpl_capsule_stream_* on 0x85, tests/test_gpu_dense_stream.py) is held to the latter, so
+this is what makes "any split into pushes gives the whole stream's scans" the SDK's behaviour and not a new definition.
 Needs the compiled reference (oracle/_ref); skipped without it."""
 import numpy as np
 import pytest

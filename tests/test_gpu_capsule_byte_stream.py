@@ -290,12 +290,12 @@ def test_reset_mid_frame(R, oracle, ans):
     ctx.close()
 
 
-def test_argument_checks(R, oracle):
+def test_argument_checks_capsule_and_standard_node_bytes(R, oracle):
     import ctypes as C
 
     L = R.lib()
     ctx = R.Context(0, MAX_NODES, 4 * MAX_SCANS)
-    for ans in (0x81, 0x80, 0x87):
+    for ans in (0x80, 0x87):
         with pytest.raises(R.RplError) as e:
             R.CapsuleByteStreamSession(ctx, ans, 4, 1000, MAX_NODES, 8)
         assert e.value.code == R.RESULT_INVALID_DATA
@@ -337,4 +337,18 @@ def test_argument_checks(R, oracle):
         with R.CapsuleByteStreamSession(ctx, 0x85, 4, 1000, MAX_NODES, 8) as sess:
             res.append((_scans(_device_push(R, sess, buf, cnt + over, 4), 4, 8), [x.tolist() for x in sess.state()]))
     assert res[0] == res[1] and res[0][1][2] == [frame_stream(oracle, 0x85, raw)[2]] * 4
+    # 0x81 standard nodes come in no capsules: a framed session of them and a framed push on their byte session are
+    # refused, and state's held_bytes alone are the bytes of each stream's unfinished record
+    with pytest.raises(R.RplError) as e:
+        R.CapsuleStreamSession(ctx, 0x81, 4, 12, MAX_NODES, 8)
+    assert e.value.code == R.RESULT_INVALID_DATA and "create_bytes" in str(e.value)
+    with R.CapsuleByteStreamSession(ctx, 0x81, 4, 1000, MAX_NODES, 8) as ns:
+        assert L.rpl_capsule_stream_push(ns._h, R.capi._p(caps), R.capi._p(ccnt), 31, C.byref(params), *outs) == \
+            R.RESULT_INVALID_DATA
+        records = np.tile(np.array([0x01, 0x01, 0, 0, 0], np.uint8), 200)  # sync bit, check bit, distance 0
+        nbuf, _ = _pack([records] * 4, 1000)
+        ns.push(nbuf, np.array([0, 3, 7, 12], np.uint32), params, 0)
+        held = np.full(4, 99, np.uint32)
+        assert L.rpl_capsule_stream_state(ns._h, None, None, R.capi._p(held)) == R.RESULT_OK
+        assert held.tolist() == [0, 3, 2, 2]
     ctx.close()

@@ -1,8 +1,9 @@
-"""rpl_dense_stream_* (DenseStreamSession): dense capsules pushed in pieces publish exactly the scans of the whole
-stream -- the SDK's unpacker -> ScanDataHolder -> ascendScanData -> publish_scan on the concatenation (pinned on the
-CPU by tests/test_dense_stream_pieces.py).  Every comparison is bit for bit: against one push of the whole stream, and
-against the restatement (oracle dense_decode -> assemble_scans -> ascend -> publish, stable tie rule as in
-test_wire_bytes_to_laserscan_in_one_host_call) and, where oracle/_ref is built, the SDK's own decoder and holder."""
+"""The dense session (DenseStreamSession, rpl_capsule_stream_* on 0x85): dense capsules pushed in pieces publish exactly
+the scans of the whole stream -- the SDK's unpacker -> ScanDataHolder -> ascendScanData -> publish_scan on the
+concatenation (pinned on the CPU by tests/test_dense_stream_pieces.py).  Every comparison is bit for bit: against one
+push of the whole stream, and against the restatement (oracle dense_decode -> assemble_scans -> ascend -> publish,
+stable tie rule as in test_wire_bytes_to_laserscan_in_one_host_call) and, where oracle/_ref is built, the SDK's own
+decoder and holder."""
 import numpy as np
 import pytest
 

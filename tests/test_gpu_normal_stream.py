@@ -1,9 +1,9 @@
-"""rpl_normal_stream_* (NormalStreamSession): a raw 0x81 standard-node byte stream pushed in pieces publishes exactly
-the scans of the whole stream -- the SDK's UnpackerHandler_NormalNode -> ScanDataHolder -> ascendScanData ->
-publish_scan on the concatenation (pinned on the CPU by tests/test_normal_stream_pieces.py).  Every comparison is bit
-for bit on ranges, intensities, beam counts and angle increment: against one push of the whole stream, against the
-restatement (oracle decode_normal -> assemble_scans -> ascend -> publish, stable tie rule) and, where oracle/_ref is
-built, the SDK's own decoder and holder."""
+"""The standard-node session (NormalStreamSession, rpl_capsule_stream_*_bytes on 0x81): a raw 0x81 standard-node byte
+stream pushed in pieces publishes exactly the scans of the whole stream -- the SDK's UnpackerHandler_NormalNode ->
+ScanDataHolder -> ascendScanData -> publish_scan on the concatenation (pinned on the CPU by
+tests/test_normal_stream_pieces.py).  Every comparison is bit for bit on ranges, intensities, beam counts and angle
+increment: against one push of the whole stream, against the restatement (oracle decode_normal -> assemble_scans ->
+ascend -> publish, stable tie rule) and, where oracle/_ref is built, the SDK's own decoder and holder."""
 import numpy as np
 import pytest
 

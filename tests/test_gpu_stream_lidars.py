@@ -337,7 +337,7 @@ def test_reconfigure_between_pushes(R, oracle, kind, ans):
     ctx.close()
 
 
-def test_argument_checks(R, oracle):
+def test_argument_checks_on_the_session_handle(R, oracle):
     import ctypes as C
 
     O = oracle
@@ -364,8 +364,7 @@ def test_argument_checks(R, oracle):
     refused(lambda: d.sess.laserscan_msgs(per))
     refused(lambda: d.sess.cloud_msgs(cpp))
     # a null table, a first call that leaves a stream out, a zero sample duration: refused, the table unchanged
-    for name in ("rpl_capsule_stream_set_lidars", "rpl_dense_stream_set_lidars", "rpl_normal_stream_set_lidars"):
-        assert getattr(R.lib(), name)(d.sess._h, None, None) == R.RESULT_INVALID_DATA
+    assert R.lib().rpl_capsule_stream_set_lidars(d.sess._h, None, None) == R.RESULT_INVALID_DATA
     good = [(0, 0, 0, (31, 0, 0, 0)), (1, 1, 0, (63, 0, 0, 0)), (0, 1, 1, (31, 0, 9, 1)), (1, 0, 1, (90, 0, 0, 0))]
     refused(lambda: d.sess.set_lidars([lidar(R, st) for st in good], np.array([1, 1, 0, 1], np.uint8)))
     d.sess.set_lidars([lidar(R, st) for st in good])

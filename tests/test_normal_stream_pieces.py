@@ -1,10 +1,10 @@
 """The contract of the standard-node stream session (0x81), pinned on the CPU: the SDK's own unpacker
 (UnpackerHandler_NormalNode) fed a raw byte stream in pieces, then its own ScanDataHolder, publishes exactly the scans
-the restatement (oracle decode_normal + the holder restatement) publishes from the whole stream in one call.  The
-session (rpl_normal_stream_*, tests/test_gpu_normal_stream.py) is held to the latter, so this is what makes "any split
-of the bytes into pushes gives the whole stream's scans" the SDK's behaviour for 0x81 and not a new definition
-(tests/test_capsule_stream_pieces.py does the same for the capsule formats).  Needs the compiled reference
-(oracle/_ref); skipped without it.
+the restatement (oracle decode_normal + the holder restatement) publishes from the whole stream in one call.  The session
+(rpl_capsule_stream_*_bytes on 0x81, tests/test_gpu_normal_stream.py) is held to the latter, so this is what makes "any
+split of the bytes into pushes gives the whole stream's scans" the SDK's behaviour for 0x81 and not a new definition
+(tests/test_capsule_stream_pieces.py does the same for the capsule formats).  Needs the compiled reference (oracle/_ref);
+skipped without it.
 
 The stream builder here is shared with the GPU test."""
 import numpy as np

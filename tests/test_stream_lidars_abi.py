@@ -23,11 +23,10 @@ def _header():
     return re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
 
 
-def test_header_declares_the_calls_and_flags(capi):
+def test_header_declares_the_call_and_flags(capi):
     src = _header()
-    for kind in ("capsule", "dense", "normal"):
-        assert re.search(rf"rpl_result\s+rpl_{kind}_stream_set_lidars\s*\(\s*rpl_{kind}_stream\s*\*\s*\w+\s*,\s*"
-                         r"const\s+rpl_lidar_settings\s*\*\s*\w+\s*,\s*const\s+uint8_t\s*\*\s*\w+\s*\)\s*;", src), kind
+    assert re.search(r"rpl_result\s+rpl_capsule_stream_set_lidars\s*\(\s*rpl_capsule_stream\s*\*\s*\w+\s*,\s*"
+                     r"const\s+rpl_lidar_settings\s*\*\s*\w+\s*,\s*const\s+uint8_t\s*\*\s*\w+\s*\)\s*;", src)
     flags = dict(re.findall(r"#define\s+(RPL_\w+)\s+(\d+)u", src))
     assert int(flags["RPL_FLAG_PER_STREAM"]) == capi.FLAG_PER_STREAM == 8
     assert int(flags["RPL_CLOUD_PER_STREAM"]) == capi.CLOUD_PER_STREAM == 2

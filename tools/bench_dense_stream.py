@@ -1,6 +1,6 @@
 """Stream session timings on the GPU; prints one JSON line.
 
-With --format 0x85 (the default), the dense stream session (rpl_dense_stream_*):
+With --format 0x85 (the default), the dense stream session (rpl_capsule_stream_* on 0x85):
 
   * per-push latency of push (host buffers, synchronous) and push_dev (device buffers, CUDA events on a torch stream)
     for 512 streams x {8, 80, 800} capsules per push: a live aggregator's receive periods of ~2.5 ms, ~25 ms, ~250 ms
@@ -13,11 +13,11 @@ stateless device path on the same capsules (rpl_decode_capsules_batch_dev -> rpl
 rpl_scan_views_dev): a chain-like shape of 512 streams x about 163840 nodes per push (the chain's 4096 dense capsules
 x 40), revolutions of about 3200 nodes, max_nodes 4096, max_scans 56.
 
-With --format 0x81, the standard-node stream session (rpl_normal_stream_*) on raw byte streams: the same comparison
-against the stateless device path (rpl_decode_normal_batch_dev -> rpl_assemble_scan_views_dev -> rpl_scan_views_dev) on
-512 streams x 163840 five-byte records per push, revolutions of 3200 records, max_nodes 4096, max_scans 56; and the
-per-push latency of push and push_dev for 512 streams x {100, 1000, 10000} bytes (at 115200 baud a standard-mode lidar
-delivers about 11500 bytes per second).
+With --format 0x81, the standard-node stream session (rpl_capsule_stream_*_bytes on 0x81) on raw byte streams: the same
+comparison against the stateless device path (rpl_decode_normal_batch_dev -> rpl_assemble_scan_views_dev ->
+rpl_scan_views_dev) on 512 streams x 163840 five-byte records per push, revolutions of 3200 records, max_nodes 4096,
+max_scans 56; and the per-push latency of push and push_dev for 512 streams x {100, 1000, 10000} bytes (at 115200 baud a
+standard-mode lidar delivers about 11500 bytes per second).
 
 With --stamped (any --format), stamped pushes (rpl_*_stream_push_ts_dev, receive times in, scan-begin stamps out)
 against unstamped ones on the same data and shapes: the chain shape above for 0x85, the comparison shapes above for the

@@ -1,4 +1,4 @@
-"""What per-stream lidar settings (rpl_dense_stream_set_lidars + RPL_FLAG_PER_STREAM) cost a device push; prints one
+"""What per-stream lidar settings (rpl_capsule_stream_set_lidars + RPL_FLAG_PER_STREAM) cost a device push; prints one
 JSON line.
 
 Shape: the chain shape of bench.py, 512 dense-capsule streams (0x85) x 4096 capsules per push (about 51 revolutions of

@@ -1,4 +1,4 @@
-"""Packed LaserScan messages of a stream session (rpl_dense_stream_laserscan_msgs[_dev]) against the padded arrays of
+"""Packed LaserScan messages of a stream session (rpl_capsule_stream_laserscan_msgs[_dev]) against the padded arrays of
 the push; prints one JSON line.
 
 Shape: a multi-lidar aggregator of 256 dense-capsule streams (0x85), each push one receive period of 320 capsules per

@@ -1,4 +1,4 @@
-"""Session nodes (rpl_dense_stream_nodes_dev) behind the push that published the scans; prints one JSON line.
+"""Session nodes (rpl_capsule_stream_nodes_dev) behind the push that published the scans; prints one JSON line.
 
 Shapes: 512 dense-capsule streams (0x85), revolutions of about 3200 nodes:
   * the shape of bench.py --workload chain, 4096 capsules per stream and push, max_scans 56, at max_nodes 4096 and 8192;

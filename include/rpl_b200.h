@@ -524,6 +524,49 @@ rpl_result rpl_capsule_stream_reset(rpl_capsule_stream* s, const uint8_t* stream
 rpl_result rpl_capsule_stream_state(rpl_capsule_stream* s, uint32_t* open_nodes, uint32_t* held_capsule,
                                     uint32_t* held_bytes);
 
+/* Session counters: per stream, what the session decoded and what it had to throw away, accumulated on the device by
+ * the kernels every push already runs, from create on, over every push flavour (framed or bytes, host or _dev, stamped
+ * or not, with or without RPL_FLAG_PER_STREAM).  Every counter but scans_unreturned depends on the stream alone, not on
+ * how it is split into pushes: after any split it equals what one push of the whole stream counts, and what the SDK's
+ * unpacker and ScanDataHolder fed the same bytes in any pieces count.  An event is counted by the push whose input
+ * completes it (a discard: by the capsule that would have released the held one; an overwrite: by the node that
+ * overwrites).  A stream with a count of 0 in a push changes no counter; a push that returns an error may have counted
+ * part of its input.  rpl_capsule_stream_reset leaves the counters alone (a reconnect is not a new lidar); the bytes it
+ * drops from a held frame are counted nowhere.  On a byte session never reset, with held_bytes of
+ * rpl_capsule_stream_state: bytes_in == frames * frame size + skipped_bytes + held_bytes (0x81: 5 * frames + ...).
+ * References: src/sdk/src/dataunpacker/unpacker/handler_capsules.cpp (express :112-136,:170,:185; ultra :387,:402;
+ * dense :703,:717; ultra-dense :915,:929), handler_hqnode.cpp:95-172, handler_normalnode.cpp:92-113,
+ * dataunpacker.cpp:199-202, sl_lidar_driver.cpp:272-315 (ScanDataHolder), :1645-1653. */
+typedef struct rpl_stream_counters {
+  uint64_t bytes_in;           /* bytes taken from the caller's buffers (_dev: after the clamp); a framed session:
+                                  capsules x capsule size */
+  uint64_t frames;             /* frames the sync hunt completed (byte sessions), capsules pushed (framed sessions),
+                                  records decoded (0x81) */
+  uint64_t skipped_bytes;      /* bytes the unpacker's sync hunt skipped (handler_capsules.cpp:112-136 and siblings,
+                                  handler_hqnode.cpp:95-172, handler_normalnode.cpp:92-113), a first sync byte dropped
+                                  with a second that does not match included; 0 on a framed session */
+  uint64_t bad_frames;         /* capsules decoded as RPL_CAPSULE_BAD_FRAME: a byte session's all-zero capsule per run
+                                  of skipped bytes, a framed session's capsules with wrong sync nibbles; 0 on 0x81 */
+  uint64_t checksum_errors;    /* ERR_EVENT_ON_EXP_CHECKSUM_ERR (dataunpacker.h:52-65; HQ: CRC, handler_hqnode.cpp:162) */
+  uint64_t encoder_resets;     /* ERR_EVENT_ON_EXP_ENCODER_RESET (dataunpacker.h:52-65) */
+  uint64_t scan_resets;        /* onHQNodeScanResetReq calls (dataunpacker.cpp:199-202) */
+  uint64_t discarded_capsules; /* capsules whose nodes the angular-jump bound kept back (RPL_CAPSULE_DISCARD), under the
+                                  stream's own sample duration with RPL_FLAG_PER_STREAM */
+  uint64_t nodes;              /* onHQNodeDecoded calls (sl_lidar_driver.cpp:1645-1649) */
+  uint64_t nodes_unopened;     /* nodes the holder dropped because no scan was open (sl_lidar_driver.cpp:296-298) */
+  uint64_t nodes_overwritten;  /* nodes that replaced the last entry of a revolution longer than the session's max_nodes
+                                  (sl_lidar_driver.cpp:302-305) */
+  uint64_t scans_rewound;      /* scan resets that emptied a non-empty revolution in progress (sl_lidar_driver.cpp:312-315) */
+  uint64_t scans_published;    /* scans the holder completed (sl_lidar_driver.cpp:279-288) */
+  uint64_t scans_unreturned;   /* published scans a push could not return, beyond its max_scans (the sum over pushes of
+                                  scans_per_stream - max_scans where positive) */
+} rpl_stream_counters;
+/* Synchronous: waits for every push issued before it, on any CUDA stream, copies the n_streams records to out
+ * (nullable: no copy), then zeroes the records of the streams whose clear_mask entry is non-zero (nullable: none)
+ * before any later push runs.  Null session: RPL_RESULT_INVALID_DATA. */
+rpl_result rpl_capsule_stream_counters(rpl_capsule_stream* s, rpl_stream_counters* out /* [n_streams] */,
+                                       const uint8_t* clear_mask /* [n_streams] */);
+
 /* Byte session: the session fed the RAW serial stream after the answer descriptor, any number of bytes per push, a
  * push ending anywhere -- what the SDK's protocol codec hands LIDARSampleDataUnpacker::onSampleData.  Per stream the
  * device also keeps the unpacker's state between frames, so for ANY split of a stream's bytes into pushes the scans

@@ -52,7 +52,7 @@ EXPORTS = [
     "rpl_assemble_scan_views_starts_dev",
     "rpl_capsule_stream_create", "rpl_capsule_stream_destroy", "rpl_capsule_stream_push", "rpl_capsule_stream_push_dev",
     "rpl_capsule_stream_reset", "rpl_capsule_stream_state", "rpl_capsule_stream_push_ts",
-    "rpl_capsule_stream_push_ts_dev",
+    "rpl_capsule_stream_push_ts_dev", "rpl_capsule_stream_counters",
     "rpl_capsule_stream_create_bytes", "rpl_capsule_stream_push_bytes", "rpl_capsule_stream_push_bytes_dev",
     "rpl_capsule_stream_push_bytes_ts", "rpl_capsule_stream_push_bytes_ts_dev",
     "rpl_capsule_stream_cloud", "rpl_capsule_stream_cloud_dev", "rpl_capsule_stream_set_frames",
@@ -115,6 +115,13 @@ class CloudParams(C.Structure):
         ("flags", C.c_uint8),
         ("pad", C.c_uint8 * 2),
     ]
+
+
+# rpl_stream_counters: one stream session stream's counters (include/rpl_b200.h)
+STREAM_COUNTER_FIELDS = ("bytes_in", "frames", "skipped_bytes", "bad_frames", "checksum_errors", "encoder_resets",
+                         "scan_resets", "discarded_capsules", "nodes", "nodes_unopened", "nodes_overwritten",
+                         "scans_rewound", "scans_published", "scans_unreturned")
+STREAM_COUNTERS_DTYPE = np.dtype([(f, "<u8") for f in STREAM_COUNTER_FIELDS])
 
 
 class RplError(RuntimeError):
@@ -212,6 +219,7 @@ def lib() -> C.CDLL:
         "rpl_capsule_stream_push_dev": ([vp, vp, vp, u32, PSP, vp, vp, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_reset": ([vp, vp], u32),
         "rpl_capsule_stream_state": ([vp, vp, vp, vp], u32),
+        "rpl_capsule_stream_counters": ([vp, vp, vp], u32),
         "rpl_capsule_stream_push_ts": ([vp, vp, vp, PT, vp, PSP, vp, vp, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_push_ts_dev": ([vp, vp, vp, PT, vp, PSP, vp, vp, vp, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_create_bytes": ([vp, u32, u32, u32, u32, u32, C.POINTER(vp)], u32),
@@ -808,6 +816,16 @@ class CapsuleStreamSession:
         held = np.zeros(self.n_streams, np.uint32)
         self._ctx._check(self._fn("state")(self._h, _p(open_nodes), _p(held), None))
         return open_nodes, held
+
+    def counters(self, clear=None):
+        """Every stream's counters since create (or since its last clear), after every push issued before the call:
+        a STREAM_COUNTERS_DTYPE array [n_streams].  clear ([n_streams] flags, None: none): the streams whose counters
+        are zeroed after the copy."""
+        out = np.zeros(self.n_streams, STREAM_COUNTERS_DTYPE)
+        m = None if clear is None else np.ascontiguousarray(clear, dtype=np.uint8)
+        assert m is None or m.shape == (self.n_streams,)
+        self._ctx._check(self._fn("counters")(self._h, _p(out), _p(m)))
+        return out
 
 
 class DenseStreamSession(CapsuleStreamSession):

@@ -25,7 +25,14 @@ namespace {
 
 constexpr int AT = 512;
 constexpr uint32_t kListCap = 4096, kResetCap = 1024;  // scan starts per stream handled by the list path
-constexpr uint32_t kStSync = 2;
+constexpr uint32_t kStSync = 2, kStDiscard = 8, kStChecksum = 16, kStEncReset = 32, kStBadFrame = 64;
+
+// STREAM: the counters this push adds to a stream's StreamCounters (s_ct, summed over the CTA)
+enum : uint32_t { kCtChecksum, kCtEncReset, kCtDiscard, kCtBadFrame, kCtUnopened, kCtOverwritten, kCtN };
+__device__ __forceinline__ void block_count(uint32_t* s_ct, uint32_t i, uint32_t v) {
+  v = __reduce_add_sync(0xffffffffu, v);
+  if ((threadIdx.x & 31) == 0 && v) atomicAdd(s_ct + i, v);
+}
 
 __device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t* warp_tot, uint32_t* total) {
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -74,6 +81,7 @@ __device__ __forceinline__ void assemble_body(const AssembleArgs& a, const Assem
   __shared__ int s_last_sync;       // position of the latest scan-start node seen so far (-1: none)
   __shared__ uint32_t s_published;  // scans published so far
   __shared__ int s_open;            // STREAM: first node of the revolution left open (-1: none, or a reset emptied it)
+  __shared__ uint32_t s_ct[kCtN];   // STREAM: this push's counts (block_count)
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 
   for (uint32_t s = blockIdx.x; s < a.n_streams; s += gridDim.x) {
@@ -137,13 +145,29 @@ __device__ __forceinline__ void assemble_body(const AssembleArgs& a, const Assem
       s_last_sync = -1;
       s_published = 0;
     }
+    if constexpr (STREAM)
+      if (tid < kCtN) s_ct[tid] = 0;
     __syncthreads();
     // ---- flag pass: positions of the scan-start nodes and of the reset requests -----------------------
+    uint32_t n_chk = 0, n_enc = 0, n_disc = 0, n_bad = 0;  // STREAM: the capsule reports' events
     for (uint32_t j = tid; j < ncap; j += AT) {
-      if (cst[j] & kStSync) {
+      const uint32_t v = cst[j];
+      if (v & kStSync) {
         const uint32_t idx = atomicAdd(&s_rcnt, 1u);
         if (idx < kResetCap) s_rlist[idx] = coff[j] + L;
       }
+      if constexpr (STREAM) {
+        n_chk += (v & kStChecksum) ? 1u : 0u;
+        n_enc += (v & kStEncReset) ? 1u : 0u;
+        n_disc += (v & kStDiscard) ? 1u : 0u;
+        n_bad += (v & kStBadFrame) ? 1u : 0u;
+      }
+    }
+    if constexpr (STREAM) {
+      block_count(s_ct, kCtChecksum, n_chk);
+      block_count(s_ct, kCtEncReset, n_enc);
+      block_count(s_ct, kCtDiscard, n_disc);
+      block_count(s_ct, kCtBadFrame, n_bad);
     }
     // the decoder may have handed the scan-start positions over (rpl_decode_dense_batch_starts_dev): then the node
     // stream is not read again at all
@@ -214,6 +238,21 @@ __device__ __forceinline__ void assemble_body(const AssembleArgs& a, const Assem
         if (tid == 0) s_published += tot;
         __syncthreads();
       }
+      if constexpr (STREAM) {
+        // the holder's losses per revolution [start, end): the first reset after its start empties it, and the nodes
+        // from there to the next scan start find no scan open; the nodes it kept past max_nodes overwrote its last
+        // entry.  The nodes in front of the first scan start (none behind a carried revolution) find none either.
+        uint32_t unopened = (tid == 0) ? (K ? s_sorted[0] : n) : 0u, overwritten = 0;
+        for (uint32_t k = tid; k < K; k += AT) {
+          const uint32_t st = s_sorted[k], en = k + 1 < K ? s_sorted[k + 1] : n;
+          const uint32_t ri = resets_upto(st);
+          const uint32_t cut = ri < RK ? min(s_rsorted[ri], en) : en;
+          unopened += en - cut;
+          overwritten += cut - st > a.max_nodes ? cut - st - a.max_nodes : 0u;
+        }
+        block_count(s_ct, kCtUnopened, unopened);
+        block_count(s_ct, kCtOverwritten, overwritten);
+      }
       // the revolution after the last scan start stays open unless a reset follows its start
       if (STREAM && tid == 0) s_open = (K > 0 && resets_upto(s_sorted[K - 1]) == RK) ? (int)s_sorted[K - 1] : -1;
     } else {
@@ -257,6 +296,17 @@ __device__ __forceinline__ void assemble_body(const AssembleArgs& a, const Assem
         prev = max(prev, before);
         uint32_t publish = 0;
         if (sync && prev >= 0) publish = (resets_upto(i) == resets_upto((uint32_t)prev)) ? 1u : 0u;
+        if constexpr (STREAM) {
+          // the holder's losses node by node: a node finds no scan open when no scan start precedes it or a reset
+          // came after that start; one kept max_nodes or more behind its scan start overwrote the last entry
+          uint32_t unopened = 0, overwritten = 0;
+          if (i < n && !sync) {
+            if (prev < 0 || resets_upto(i) != resets_upto((uint32_t)prev)) unopened = 1;
+            else if (i - (uint32_t)prev >= a.max_nodes) overwritten = 1;
+          }
+          block_count(s_ct, kCtUnopened, unopened);
+          block_count(s_ct, kCtOverwritten, overwritten);
+        }
         uint32_t tot = 0;
         const uint32_t ex = block_excl_scan(publish, s_warp, &tot);  // syncs
         if (publish) {
@@ -280,6 +330,28 @@ __device__ __forceinline__ void assemble_body(const AssembleArgs& a, const Assem
     __syncthreads();
     const uint32_t total = s_published;
     if (tid == 0) a.scans_per_stream[s] = total;
+    if constexpr (STREAM) {
+      if (tid == 0) {
+        // K counts every scan start (the lists keep counting past their capacity): each closes the revolution before
+        // it, published unless a reset emptied it, and a reset after the last one empties the open revolution
+        StreamCounters& c = a.counters[s];
+        if (a.counted_capsule_bytes) {
+          c.frames += ncap;
+          c.bytes_in += (unsigned long long)ncap * a.counted_capsule_bytes;
+        }
+        c.bad_frames += s_ct[kCtBadFrame];
+        c.checksum_errors += s_ct[kCtChecksum];
+        c.encoder_resets += s_ct[kCtEncReset];
+        c.scan_resets += RK;
+        c.discarded_capsules += s_ct[kCtDiscard];
+        c.nodes += a.node_counts[s];
+        c.nodes_unopened += s_ct[kCtUnopened];
+        c.nodes_overwritten += s_ct[kCtOverwritten];
+        c.scans_rewound += K ? K - 1 - total + (s_open < 0 ? 1u : 0u) : 0u;
+        c.scans_published += total;
+        c.scans_unreturned += total > a.max_scans ? total - a.max_scans : 0u;
+      }
+    }
     // ---- copy the published scans (descriptors were written by this CTA: visible after the barrier) ---
     const uint32_t stored = min(total, a.max_scans);
     if (a.views_out) {

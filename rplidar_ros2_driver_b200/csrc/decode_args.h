@@ -49,6 +49,13 @@ struct CapsuleDecodeArgs {
 constexpr uint32_t kHeldCapsuleWords = 43, kHeldOk = 43, kHeldStart = 44, kHeldSync = 45, kHeldLast = 46,
                    kHeldWords = 48;
 
+// a stream session's counters of one stream (rpl_stream_counters byte for byte), accumulated by the kernels of every
+// push: the framer or the 0x81 decoder count the bytes, the assembler the capsule reports and the holder's losses
+struct StreamCounters {
+  unsigned long long bytes_in, frames, skipped_bytes, bad_frames, checksum_errors, encoder_resets, scan_resets,
+      discarded_capsules, nodes, nodes_unopened, nodes_overwritten, scans_rewound, scans_published, scans_unreturned;
+};
+
 // 5-byte standard nodes from raw byte streams
 struct NormalDecodeArgs {
   const uint8_t* bytes;           // [n_streams][stride_bytes]
@@ -64,6 +71,8 @@ struct NormalDecodeArgs {
   // (nullable, [n_streams][node_stride - node_first]) is written for the scan-start records only
   uint32_t* held;                 // [n_streams][kHeldWords], read and rewritten in place
   uint32_t node_stride, node_first;
+  // stream session only: each stream's counters, given bytes_in, frames (records) and skipped_bytes
+  StreamCounters* counters;       // [n_streams]
 };
 
 // per-sample timestamps (timestamps.cu; TimingDesc: lidar_args.h)
@@ -118,6 +127,10 @@ struct AssembleArgs {
   const uint32_t* carry_len;          // [n_streams]
   uint2* carry_out;                   // [n_streams][stride_nodes]
   uint32_t* carry_len_out;            // [n_streams]
+  // stream session only: each stream's counters, given the capsule reports' events, nodes and the holder's counters
+  // (and, when counted_capsule_bytes != 0 -- a framed session's push --, frames and bytes_in: capsules x that size)
+  StreamCounters* counters;           // [n_streams]
+  uint32_t counted_capsule_bytes;
 };
 
 // a stamped stream-session push (launch_assemble_stamped; AssembleArgs::scan_begin_ts_us is the output, every slot
@@ -173,6 +186,7 @@ struct FrameStreamArgs {
   const unsigned long long* chunk_rx_us;    // [n_streams][stride_chunks]
   uint32_t chunk_bytes, stride_chunks;
   unsigned long long* capsule_rx_out;       // [n_streams][stride_capsules] with chunk_rx_us: each capsule's
+  StreamCounters* counters;                 // [n_streams]: given bytes_in, frames and skipped_bytes
 };
 cudaError_t launch_frame_capsules(const FrameArgs& a, int grid, cudaStream_t stream);
 cudaError_t launch_frame_capsules_stream(const FrameArgs& a, const FrameStreamArgs& f, int grid, cudaStream_t stream);

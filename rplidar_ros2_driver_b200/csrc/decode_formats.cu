@@ -905,11 +905,13 @@ __device__ __forceinline__ void decode_normal_body(const NormalDecodeArgs& a) {
                         : a.nodes_out + (size_t)s * (a.stride_bytes / 5u);
     uint32_t* end_out = STARTS ? a.node_end + (size_t)s * (a.node_stride - a.node_first)
                         : (!STREAM && a.node_end) ? a.node_end + (size_t)s * (a.stride_bytes / 5u) : nullptr;
+    uint32_t held_in = 0;  // STREAM, thread 0: bytes of the unfinished record entering the push
     if constexpr (STREAM) {
       // all zero (a fresh stream): state 0, whose first record ends at byte 5 at the earliest, never reading the halo
       if (tid == 0) {
         const uint32_t* held = a.held + (size_t)s * kHeldWords;
-        sm.carry_state = held[kHeldOk];
+        held_in = held[kHeldOk];
+        sm.carry_state = held_in;
         sm.carry_nodes = 0;
         *reinterpret_cast<uint32_t*>(sm_bytes) = held[0];
       }
@@ -1063,6 +1065,11 @@ __device__ __forceinline__ void decode_normal_body(const NormalDecodeArgs& a) {
         uint32_t* held = a.held + (size_t)s * kHeldWords;
         held[kHeldOk] = sm.carry_state;
         held[0] = *reinterpret_cast<const uint32_t*>(sm_bytes);
+        // every byte entering (held + pushed) is in a decoded record, held for the next push, or skipped
+        StreamCounters& sc = a.counters[s];
+        sc.bytes_in += n;
+        sc.frames += sm.carry_nodes;
+        sc.skipped_bytes += held_in + n - 5u * sm.carry_nodes - sm.carry_state;
       } else {
         if (a.fsm_state_out) a.fsm_state_out[s] = sm.carry_state;
       }

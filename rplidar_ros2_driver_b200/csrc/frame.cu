@@ -67,6 +67,7 @@ __global__ void __launch_bounds__(FT) frame_capsules_kernel(FrameArgs a, FrameSt
     const unsigned long long* rx_in = STREAM && f.chunk_rx_us ? f.chunk_rx_us + (size_t)s * f.stride_chunks : nullptr;
     unsigned long long* rx_out = STREAM ? f.capsule_rx_out + (size_t)s * a.stride_capsules : nullptr;
     uint32_t pos = 0, count = 0, tile = 0;
+    uint32_t zeros = 0;  // STREAM, thread 0: all-zero capsules among the `count` emitted
     bool lost = STREAM ? rec[kFramerLost] != 0u : false, done = false;
     const uint8_t* t = sb;
     while (!done && pos < n) {
@@ -115,6 +116,7 @@ __global__ void __launch_bounds__(FT) frame_capsules_kernel(FrameArgs a, FrameSt
           for (uint32_t j = tid; j < kw; j += FT) rx_out[first + j] = rx_in[(pos + (j + 1) * cb - 1 - k) / f.chunk_bytes];
           if (lost && count < a.stride_capsules && tid == 0) rx_out[count] = rx_in[(pos + cb - 1 - k) / f.chunk_bytes];
         }
+        if (STREAM && lost) ++zeros;
         count = first + K;
         lost = false;
         pos += K * cb;
@@ -148,6 +150,7 @@ __global__ void __launch_bounds__(FT) frame_capsules_kernel(FrameArgs a, FrameSt
           if (l) {
             sm.entry[ne++] = kDummy;
             l = 0;
+            if (STREAM) ++zeros;
           }
           sm.entry[ne++] = q;
           q += cb;
@@ -187,6 +190,12 @@ __global__ void __launch_bounds__(FT) frame_capsules_kernel(FrameArgs a, FrameSt
       if (tid == 0) {
         rec[kFramerPos] = left;
         rec[kFramerLost] = lost ? 1u : 0u;
+        // every byte entering (held + pushed) is in a completed frame, held for the next push, or skipped
+        const uint32_t frames = count - zeros;
+        StreamCounters& sc = f.counters[s];
+        sc.bytes_in += n - k;
+        sc.frames += frames;
+        sc.skipped_bytes += n - left - frames * cb;
       }
     }
     if (tid == 0) {

@@ -1046,7 +1046,8 @@ rpl_result assemble_common(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t*
                                   uint64_t* scan_begin_ts_us, void* stream, const uint32_t* scan_starts = nullptr,
                                   uint32_t starts_stride = 0, const uint32_t* scan_start_counts = nullptr,
                                   const uint32_t* carry_len = nullptr, rpl_node_hq* carry_out = nullptr,
-                                  uint32_t* carry_len_out = nullptr, const rpl::AssembleStampArgs* stamp = nullptr) {
+                                  uint32_t* carry_len_out = nullptr, const rpl::AssembleStampArgs* stamp = nullptr,
+                                  rpl::StreamCounters* counters = nullptr, uint32_t counted_capsule_bytes = 0) {
   if (!c || !nodes || !node_counts || (!scans_out && !views_out) || !scan_len || !scans_per_stream) return RPL_RESULT_INVALID_DATA;
   if (views_out && (unsigned long long)n_streams * stride_nodes > 0xFFFFFFFFull) {
     c->err = "view mode addresses nodes with 32 bits: n_streams * stride_nodes must stay below 2^32";
@@ -1109,6 +1110,8 @@ rpl_result assemble_common(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t*
   a.carry_len = carry_len;
   a.carry_out = reinterpret_cast<uint2*>(carry_out);
   a.carry_len_out = carry_len_out;
+  a.counters = counters;
+  a.counted_capsule_bytes = counted_capsule_bytes;
   const int grid = (int)std::min<uint32_t>(n_streams, (uint32_t)c->num_sms * 4u);
   if (stamp)
     RPL_CUDA(c, rpl::launch_assemble_stamped(a, *stamp, grid, st), RPL_RESULT_OPERATION_FAIL);
@@ -1245,7 +1248,19 @@ struct rpl_capsule_stream {
   std::vector<rpl::LidarSettings> lidars_host;
   uint32_t lidar_modes = 0;                     // LidarTable::modes of the table
   unsigned char* node_work = nullptr;           // the tables of a nodes call (NodeWork)
+  // [n_streams] device, zeroed at create: what every push decoded and lost (rpl_capsule_stream_counters); a stream's
+  // record is written by the one CTA of each kernel that serves the stream
+  rpl::StreamCounters* counters = nullptr;
 };
+
+static_assert(sizeof(rpl::StreamCounters) == sizeof(rpl_stream_counters) &&
+                  offsetof(rpl::StreamCounters, bytes_in) == offsetof(rpl_stream_counters, bytes_in) &&
+                  offsetof(rpl::StreamCounters, skipped_bytes) == offsetof(rpl_stream_counters, skipped_bytes) &&
+                  offsetof(rpl::StreamCounters, scan_resets) == offsetof(rpl_stream_counters, scan_resets) &&
+                  offsetof(rpl::StreamCounters, nodes) == offsetof(rpl_stream_counters, nodes) &&
+                  offsetof(rpl::StreamCounters, scans_rewound) == offsetof(rpl_stream_counters, scans_rewound) &&
+                  offsetof(rpl::StreamCounters, scans_unreturned) == offsetof(rpl_stream_counters, scans_unreturned),
+              "rpl::StreamCounters must be rpl_stream_counters byte for byte");
 
 static_assert(sizeof(rpl::LidarSettings) == sizeof(rpl_lidar_settings) &&
                   offsetof(rpl::LidarSettings, mode_a) == offsetof(rpl_lidar_settings, scan_processing) &&
@@ -1291,6 +1306,10 @@ struct WireChunk {
   // a session push with RPL_FLAG_PER_STREAM: the chunk's first stream's entry of the session's table (else nullptr)
   const rpl::LidarSettings* lidars;
   uint32_t lidar_modes;
+  // a session's counters (the chain's: nullptr); a framed session's bytes per capsule, which the assembler counts in
+  // (a byte session's framer or 0x81 decoder counts the bytes)
+  rpl::StreamCounters* counters;
+  uint32_t counted_capsule_bytes;
 };
 
 // session cs's chunk from stream s0 in the push under way (arena cs->parity); per_stream: RPL_FLAG_PER_STREAM
@@ -1324,6 +1343,8 @@ WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0, bool per_stre
   w.slot_begin = cs->slot_begin + so;
   w.slot_end = cs->slot_end + so;
   w.prev_stamped = cs->prev_stamped;
+  w.counters = cs->counters + s0;
+  w.counted_capsule_bytes = cs->bytes ? 0u : cs->cap_bytes;
   if (cs->framer) {
     w.stride_bytes = cs->stride_in;
     w.framer = cs->framer + (size_t)s0 * rpl::kFramerWords;
@@ -1359,6 +1380,7 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
     a.capsule_counts_out = w.framed_counts;
     rpl::FrameStreamArgs f{};
     f.framer = w.framer;
+    f.counters = w.counters;
     if (sp) {  // the framer turns the chunk receive times into the capsule receive times the assembler reads
       f.chunk_rx_us = sp->rx;
       f.chunk_bytes = sp->chunk_bytes;
@@ -1387,6 +1409,7 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
     a.node_stride = w.node_stride;
     a.node_first = w.node_first;
     a.node_end = ends;
+    a.counters = w.counters;
     r = decode_normal_launch(c, a, st);
   } else {
     rpl::CapsuleDecodeArgs a{};
@@ -1435,7 +1458,7 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
                       w.status ? sc : 0u, w.max_nodes, w.max_scans, w.max_nodes, nullptr, w.views, w.scan_len,
                       scans_per_stream, nullptr, sp ? reinterpret_cast<uint64_t*>(sp->scan_ts) : nullptr, st, w.starts,
                       w.starts ? w.starts_stride : 0u, w.start_counts, w.carry_len, w.carry_out, w.carry_len_out,
-                      sp ? &t : nullptr);
+                      sp ? &t : nullptr, w.counters, w.counted_capsule_bytes);
   if (r != RPL_RESULT_OK) return r;
   RPL_CUDA(c, cudaEventRecord(c->asm_done, st), RPL_RESULT_OPERATION_FAIL);
   return enqueue_scan(c, l, w.nodes, w.scan_len, ns * w.max_scans, w.max_nodes, params, nullptr, ranges, intens, beams,
@@ -1673,6 +1696,8 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, bool bytes, uint32_t n_s
       !cuda_ok(c, dev_alloc(&cs->slot_begin, n * max_scans), "cudaMalloc") ||
       !cuda_ok(c, dev_alloc(&cs->slot_end, n * max_scans), "cudaMalloc") ||
       !cuda_ok(c, dev_alloc(&cs->msg_hdr, n), "cudaMalloc") ||
+      !cuda_ok(c, dev_alloc(&cs->counters, n), "cudaMalloc") ||
+      !cuda_ok(c, cudaMemset(cs->counters, 0, n * sizeof(rpl::StreamCounters)), "cudaMemset") ||
       !cuda_ok(c, dev_alloc(&cs->node_work, node_work_bytes(cs)), "cudaMalloc"))
     return fail(oom);
   // the reference's defaults: frame_id "laser_frame" (rplidar_node.cpp:80), range_max 12 m (rplidar_node.hpp:328)
@@ -2513,6 +2538,7 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   cudaFree(cs->msg_work);
   cudaFree(cs->node_work);
   cudaFree(cs->lidars);
+  cudaFree(cs->counters);
   if (cs->done) cudaEventDestroy(cs->done);
   delete cs;
 }
@@ -2611,6 +2637,31 @@ rpl_result rpl_capsule_stream_state(rpl_capsule_stream* cs, uint32_t* open_nodes
     if (held_capsule) held_capsule[s] = normal || (f && f[rpl::kFramerLost]) ? 0u : ok;
     if (held_bytes) held_bytes[s] = normal ? ok : f ? f[rpl::kFramerPos] : 0u;
   }
+  return RPL_RESULT_OK;
+}
+
+rpl_result rpl_capsule_stream_counters(rpl_capsule_stream* cs, rpl_stream_counters* out, const uint8_t* clear_mask) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);  // host pushes return synchronised
+  if (out)
+    RPL_CUDA(c, cudaMemcpy(out, cs->counters, (size_t)cs->n_streams * sizeof(rpl_stream_counters), cudaMemcpyDeviceToHost),
+             RPL_RESULT_OPERATION_FAIL);
+  if (!clear_mask) return RPL_RESULT_OK;
+  cudaStream_t st = c->lane[0].stream;
+  for (uint32_t s = 0; s < cs->n_streams;) {  // one clear per run of masked streams
+    if (!clear_mask[s]) {
+      ++s;
+      continue;
+    }
+    uint32_t e = s + 1;
+    while (e < cs->n_streams && clear_mask[e]) ++e;
+    RPL_CUDA(c, cudaMemsetAsync(cs->counters + s, 0, (size_t)(e - s) * sizeof(rpl::StreamCounters), st),
+             RPL_RESULT_OPERATION_FAIL);
+    s = e;
+  }
+  RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);  // cleared before any later push runs
   return RPL_RESULT_OK;
 }
 

@@ -415,8 +415,18 @@ __global__ void __launch_bounds__(kBlock, 2) scan_tma_kernel(ScanBatchArgs a, ui
 // chunks while this scan folds, exchanges and builds its rank table -- a stretch in which the SM would
 // otherwise have no load in flight.  The other slots are handed back in the place pass, which takes them
 // first, in ascending order, and then places the held chunks from registers.  Each filled slot still gets
-// exactly one arrive per consumer warp per scan: held slots in the mark pass, the others in the place pass
-// or, for a scan handed on or with nothing measured, right after the exchange.
+// exactly one arrive per consumer warp per scan: held slots when they are marked, the others in the place
+// pass, which hands them back without placing them for a scan handed on or with nothing measured.
+//
+// Pipeline: the consumer warps mark the cluster's next streamed scan s2 while they place scan s, so that the
+// stretch with no stores in flight is only the fold, the exchange and the rank table.  After each of s's slots
+// j >= kHeld is placed and handed back, a warp marks one chunk of s2: first its held chunks (slots the producer
+// refilled during s's fold and exchange), then its slot j - kMarkLag, whose refill was asked for kMarkLag places
+// ago.  Then s's held chunks are placed from registers and the rest of s2 is marked.  The byte map is free by then:
+// s's fold has turned it into bit-words, and it is cleared for s2 right after that fold, behind rank_table's
+// barriers and before the barrier that precedes the first mark of s2.  s2's measured count stays in a register
+// until its fold, as sm.red holds s's counts until rank_table has read them.  Both sets of held chunks are live
+// during the first places (96 registers per thread, no spills).
 //
 // Exchange: CTA r writes its words and count into the PEER's inbox with st.async, whose bytes complete on
 // the peer's inbox_full barrier; the peer arms that barrier for the scan with one arrive.expect_tx of
@@ -433,15 +443,24 @@ __global__ void __launch_bounds__(kBlock, 2) scan_tma_kernel(ScanBatchArgs a, ui
 //
 // Why this cannot deadlock: only the consumer threads touch the exchange barriers, and both CTAs walk
 // the same scans in the same order and take the same branches (every decision -- invalid, empty, no
-// measured node, duplicate key -- depends on counts[s] or on the exchanged totals, identical on both
-// sides).  In scan s a CTA publishes after its own mark pass, which waits only on its own producer.  To
-// fill a slot for scan s the producer waits only on its own consumers: for a held slot (j < kHeld), on
-// their mark pass of scan s - 1, which needs nothing from the peer; for any other slot, on their place
-// pass of scan s - 1 (or their early exit after its exchange), which in turn needs the peer's publish of
-// s - 1 and the peer's read of the inbox of s - 1 -- both done before the peer could start scan s.  The
-// producer fills scan by scan, so while it waits on a slot for scan s + 1 every slot of scan s is filled,
-// and the mark pass of scan s (held slots included) can finish.  The producer warp never takes part in a
-// cluster barrier while the loop runs;
+// measured node, duplicate key -- depends on counts[] or on the exchanged totals, identical on both
+// sides).  The waits, for consecutive streamed scans s - 1, s and s + 1 of the cluster:
+//   * The producer fills scan by scan and slot by slot and waits only on its own consumers' arrives: to load
+//     chunk j of scan s + 1 into a held slot it waits for their mark of slot j of scan s; into any other slot,
+//     for their place pass of scan s over slot j (a slot scan s does not use is free already).
+//   * In the place pass of scan s, a consumer warp waits on slot j of scan s + 1 only after it has itself handed
+//     back every slot of s up to j (held slots: all of them, at their mark; others: kMarkLag places before).
+//     Take the lowest slot any warp waits on: every waiting warp has handed it back, and a warp that waits on
+//     nothing runs on until it has handed back every slot of s -- no warp meets a barrier before it has marked
+//     all of s + 1, so none can hold another up there.  All 16 arrives for that slot come, the producer, which
+//     has filled every lower slot, fills it, and the wait ends.  By induction every mark of s + 1 ends.  There
+//     is no block barrier between a warp's arrive on a slot and its wait on that slot's refill.
+//   * The exchange of scan s + 1 comes after both CTAs have marked all of it, which needs nothing from the peer
+//     past the rank table of s.  A CTA's rank table of s needs the peer's words of s, which the peer sends once
+//     it has marked s (in its place pass of s - 1, or before its loop for the first scan), and the peer_free
+//     arrive for s - 1, which the peer made in its rank table of s - 1 before it marked s.  Neither waits on
+//     this CTA past the exchange of s - 1, which it has finished.  So no wait of either CTA closes a cycle.
+// The producer warp never takes part in a cluster barrier while the loop runs;
 // the whole cluster, producer warps included, meets in barrier.cluster exactly twice: after the barrier
 // init (no remote arrive may reach an uninitialised barrier) and before exit (no CTA may exit while the
 // peer can still store to its inbox or arrive on its barriers).
@@ -453,6 +472,10 @@ static_assert(kClusterMaxNodes <= kMaxFastNodes, "every scan the cluster kernel 
 // 0.784-0.791 ms at 64 / 80 / 88 / 95 / 96 / 96 registers per thread, no spills (DESIGN.md §5.1).
 constexpr int kHeld = 4;
 static_assert(kHeld >= 0 && kHeld <= kClusterSlots, "held slots are a prefix of the tile");
+// How many slots the next scan's mark trails the place front by, so that a slot's refill has landed by the time it
+// is marked.  Timed on an H100 SXM at 700 W (4096 x 32768-node Mode B launches, three runs each, alternately):
+// 2 / 4 / 6 slots take 0.744-0.745 / 0.744-0.745 / 0.752 ms (DESIGN.md §5.1).
+constexpr uint32_t kMarkLag = 4;
 
 struct __align__(128) ClusterSmem {
   uint8_t bytemap[kKeySpace];                // presence map of this CTA's nodes (swizzled)
@@ -535,77 +558,94 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
       if (lane == 0) mbar_arrive(&sm.empty[j]);
     };
 
-    for (uint32_t s = s0; s < a.n_scans; s += s_step) {
-      const uint32_t n = a.counts[s];
-      if (n > a.stride || n > max_nodes) {  // caller error: report, touch nothing
-        if (writer) write_outcome(a, s, kResultInvalidData, 0u, 0.0f);
-        continue;
+    // the first scan at or after s that runs through the tile; the writer reports the ones it passes over
+    auto next_streamed = [&](uint32_t s) {
+      for (; s < a.n_scans; s += s_step) {
+        const uint32_t n = a.counts[s];
+        if (scan_is_streamed(n, a.stride, max_nodes)) break;
+        if (writer) {
+          if (n == 0) write_outcome_empty(a, s);  // ascendScanData: OPERATION_FAIL; publish_scan: nodes.empty() -> return
+          else write_outcome(a, s, kResultInvalidData, 0u, 0.0f);  // caller error: report, touch nothing
+        }
       }
-      if (n == 0) {  // ascendScanData: OPERATION_FAIL; publish_scan: nodes.empty() -> return
-        if (writer) write_outcome_empty(a, s);
-        continue;
-      }
+      return s;
+    };
+    // this CTA's share of a streamed scan of n nodes (n = 0: no scan, no chunk)
+    struct Half {
+      uint32_t n, mine, mine_full, nheld;
+    };
+    auto half_of = [&](uint32_t n) {
       const uint32_t nch = (n + CH - 1) / CH, nfull = n / CH;
-      const uint32_t mine = (nch + 1u - rank) >> 1;
+      Half h;
+      h.n = n;
+      h.mine = (nch + 1u - rank) >> 1;  // chunks c < nch with c & 1 == rank
+      // the partial chunk (c == nfull < nch) is the last of this CTA's chunks if it is this CTA's at all
+      h.mine_full = nfull < nch && (nfull & 1u) == rank ? h.mine - 1u : h.mine;
+      h.nheld = min((uint32_t)kHeld, h.mine);
+      return h;
+    };
 
-      // ---- clear the presence map (while this scan's copies are still in flight) --------------
+    uint32_t cnt = 0;  // measured nodes this thread has marked of the scan being marked
+    uint8_t* const bmap = sm.bytemap;
+    auto fetch = [&](uint32_t j, uint2 (&v)[kRounds]) {
+      const uint2* slot = sm.tile[j];
+#pragma unroll
+      for (int r = 0; r < kRounds; ++r) v[r] = slot[r * TC + tid];
+    };
+    auto wait_and_fetch = [&](uint32_t j, uint2 (&v)[kRounds]) {
+      mbar_wait(&sm.full[j], (fph >> j) & 1u);
+      fph ^= 1u << j;
+      fetch(j, v);
+    };
+    auto mark_chunk = [&](auto checked, const uint2 (&v)[kRounds], uint32_t j, uint32_t n) {
+      const uint32_t c = 2u * j + rank;
+#pragma unroll
+      for (int r = 0; r < kRounds; ++r) {
+        const uint32_t dist = __funnelshift_r(v[r].x, v[r].y, 16);
+        bool valid = dist != 0;
+        if (decltype(checked)::value && c * CH + r * TC + tid >= n) valid = false;
+        if (valid) bmap[swz_x(v[r].x)] = 1;
+        cnt += valid ? 1u : 0u;
+      }
+    };
+    // held slot j: copied into registers, marked, and handed back at once (after the byte-map stores whose addresses
+    // depend on the slot's values).  Every held chunk takes the tail mask, which is a no-op on the full ones.
+    auto mark_held = [&](uint32_t j, const Half& h, uint2 (&v)[kRounds]) {
+      wait_and_fetch(j, v);
+      mark_chunk(Checked{}, v, j, h.n);
+      release(j);
+    };
+    // any other slot: marked and left in shared memory for the place pass
+    auto mark_resident = [&](uint32_t j, const Half& h) {
+      uint2 v[kRounds];
+      wait_and_fetch(j, v);
+      if (j < h.mine_full) mark_chunk(Unchecked{}, v, j, h.n);
+      else mark_chunk(Checked{}, v, j, h.n);
+    };
+
+    // The loop is software-pipelined over the cluster's streamed scans: an iteration starts with scan s marked
+    // (its held chunks in held[]), folds, exchanges and ranks it, and places it while it marks the next streamed
+    // scan s2 into the byte map, which is cleared right after s's fold.  Only constant indices into held[] and
+    // next_held[] (no local memory).
+    uint2 held[kHeld > 0 ? kHeld : 1][kRounds];
+    uint2 next_held[kHeld > 0 ? kHeld : 1][kRounds];
+    uint32_t s = next_streamed(s0);
+    Half cur = half_of(s < a.n_scans ? a.counts[s] : 0u);
+    if (s < a.n_scans) {  // the first scan is marked with no place pass to hide behind
       bytemap_clear(sm.bytemap, tid);
       consumer_sync();
-
-      // ---- mark this CTA's chunks ---------------------------------------------------------------
-      // Slots j < kHeld are copied into registers and handed back as soon as they are marked, so the producer
-      // loads the next scan into them during this scan's fold and exchange; the other slots stay in shared
-      // memory until the place pass.
-      uint2 held[kHeld > 0 ? kHeld : 1][kRounds];
-      uint32_t cnt = 0;
-      uint8_t* const bmap = sm.bytemap;
-      auto fetch = [&](uint32_t j, uint2 (&v)[kRounds]) {
-        const uint2* slot = sm.tile[j];
-#pragma unroll
-        for (int r = 0; r < kRounds; ++r) v[r] = slot[r * TC + tid];
-      };
-      auto wait_and_fetch = [&](uint32_t j, uint2 (&v)[kRounds]) {
-        mbar_wait(&sm.full[j], (fph >> j) & 1u);
-        fph ^= 1u << j;
-        fetch(j, v);
-      };
-      auto mark_chunk = [&](auto checked, const uint2 (&v)[kRounds], uint32_t j) {
-        const uint32_t c = 2u * j + rank;
-#pragma unroll
-        for (int r = 0; r < kRounds; ++r) {
-          const uint32_t dist = __funnelshift_r(v[r].x, v[r].y, 16);
-          bool valid = dist != 0;
-          if (decltype(checked)::value && c * CH + r * TC + tid >= n) valid = false;
-          if (valid) bmap[swz_x(v[r].x)] = 1;
-          cnt += valid ? 1u : 0u;
-        }
-      };
-      // the partial chunk (c == nfull < nch) is the last of this CTA's chunks if it is this CTA's at all
-      const bool tail = nfull < nch && (nfull & 1u) == rank;
-      const uint32_t mine_full = tail ? mine - 1u : mine;
-      const uint32_t nheld = min((uint32_t)kHeld, mine);
-      // held slots first: the producer fills them first.  Only constant indices into held[] (no local memory);
-      // every held chunk takes the tail mask, which is a no-op on the full ones.
 #pragma unroll
       for (int j = 0; j < kHeld; ++j) {
-        if (j < (int)mine) {
-          wait_and_fetch(j, held[j]);
-          mark_chunk(Checked{}, held[j], j);
-          release(j);  // after the byte-map stores whose addresses depend on the slot's values
-        }
+        if (j < (int)cur.nheld) mark_held(j, cur, held[j]);
       }
-      for (uint32_t j = nheld; j < mine_full; ++j) {
-        uint2 v[kRounds];
-        wait_and_fetch(j, v);
-        mark_chunk(Unchecked{}, v, j);
-      }
-      if (tail && mine_full >= nheld) {
-        uint2 v[kRounds];
-        wait_and_fetch(mine_full, v);
-        mark_chunk(Checked{}, v, mine_full);
-      }
+      for (uint32_t j = cur.nheld; j < cur.mine; ++j) mark_resident(j, cur);
+    }
+
+    while (s < a.n_scans) {
       cnt = warp_sum(cnt);
       if (lane == 0) sm.red[warp] = cnt;
+      // s2's counts stay in cnt until its fold: sm.red holds s's until rank_table has read them
+      cnt = 0;
       consumer_sync();
 
       // ---- fold, exchange with the peer, rank table -----------------------------------------
@@ -632,21 +672,27 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
         rank_table(sm, wv, tid, other);
         // every thread has used its inbox entry (rank_table's barriers): the peer may overwrite it
         if (tid == 0) mbar_arrive_remote(peer_peer_free);
+        // every thread has folded its row (rank_table's barriers), and the fold maps threads to bytes unlike the
+        // clear: clear the map for the next scan, whose first mark comes after the barrier below
+        bytemap_clear(sm.bytemap, tid);
       }
       consumer_sync();
       const uint32_t M = sm.valid_count;  // measured nodes of the whole scan, the same in both CTAs
 
-      if (M == 0 || sm.totV != M) {
-        if (writer) {
-          if (M == 0) write_outcome_empty(a, s);
-          else hand_to_general(a, s);  // duplicate keys, within a half or across the halves
-        }
-        for (uint32_t j = nheld; j < mine; ++j) release(j);  // the held slots went back in the mark pass
-        continue;
+      const bool placing = M != 0 && sm.totV == M;
+      if (writer && !placing) {
+        if (M == 0) write_outcome_empty(a, s);
+        else hand_to_general(a, s);  // duplicate keys, within a half or across the halves
       }
+      const uint32_t s2 = next_streamed(s + s_step);
+      const Half nx = half_of(s2 < a.n_scans ? a.counts[s2] : 0u);
 
-      // ---- place this CTA's chunks by rank: the slots still in shared memory first, handing each back, ----
-      // ---- so that the producer's next wait (on slot kHeld) is the first one met; then the held chunks ----
+      // ---- place this CTA's chunks of s by rank and mark those of s2 ----------------------------------------
+      // s's slots still in shared memory go first, in ascending order, each handed back once placed (or at once if
+      // s is not placed), so that the producer's next wait (on slot kHeld) is the first one met.  After each of
+      // them one chunk of s2 is marked: its held chunks first, which the producer loaded during s's fold and
+      // exchange, then its other chunks kMarkLag slots behind the place front, so that their refill has had time
+      // to land.  Then s's held chunks are placed from registers, and the rest of s2 is marked.
       const ModeBOut mode_b(a.ranges + (size_t)s * a.stride, a.intensities + (size_t)s * a.stride, M, inverted,
                             l2_policy_evict_normal());
       auto place_chunk = [&](auto checked, const uint2 (&v)[kRounds], uint32_t j) {
@@ -657,27 +703,46 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
           const uint32_t k = nd.x & 0xFFFFu;
           const uint32_t dist = __funnelshift_r(nd.x, nd.y, 16);
           uint32_t measured = dist != 0 ? 1u : 0u;
-          if (decltype(checked)::value && c * CH + r * TC + tid >= n) measured = 0;
+          if (decltype(checked)::value && c * CH + r * TC + tid >= cur.n) measured = 0;
           mode_b.store(rank_of(sm.rankV, k), dist_to_m(dist), intensity_of(nd.y), measured);
         }
       };
-      for (uint32_t j = nheld; j < mine_full; ++j) {
-        uint2 v[kRounds];
-        fetch(j, v);
-        place_chunk(Unchecked{}, v, j);
-        release(j);
-      }
-      if (tail && mine_full >= nheld) {
-        uint2 v[kRounds];
-        fetch(mine_full, v);
-        place_chunk(Checked{}, v, mine_full);
-        release(mine_full);
-      }
+      auto place_resident = [&](uint32_t j) {
+        if (placing) {
+          uint2 v[kRounds];
+          fetch(j, v);
+          if (j < cur.mine_full) place_chunk(Unchecked{}, v, j);
+          else place_chunk(Checked{}, v, j);
+        }
+        release(j);  // the held slots went back in the mark pass
+      };
+      uint32_t j = cur.nheld;  // s's next slot to place
 #pragma unroll
-      for (int j = 0; j < kHeld; ++j) {
-        if (j < (int)mine) place_chunk(Checked{}, held[j], j);
+      for (int h = 0; h < kHeld; ++h) {
+        if (j < cur.mine) place_resident(j++);
+        if (h < (int)nx.nheld) mark_held(h, nx, next_held[h]);
       }
-      if (writer) write_outcome(a, s, kResultOk, M, angle_increment(M, false));
+      uint32_t jm = nx.nheld;  // s2's next slot to mark
+      for (; j < cur.mine; ++j) {
+        place_resident(j);
+        if (jm + kMarkLag <= j && jm < nx.mine) mark_resident(jm++, nx);
+      }
+      if (placing) {
+#pragma unroll
+        for (int h = 0; h < kHeld; ++h) {
+          if (h < (int)cur.nheld) place_chunk(Checked{}, held[h], h);
+        }
+        if (writer) write_outcome(a, s, kResultOk, M, angle_increment(M, false));
+      }
+      for (; jm < nx.mine; ++jm) mark_resident(jm, nx);
+
+#pragma unroll
+      for (int h = 0; h < kHeld; ++h) {
+#pragma unroll
+        for (int r = 0; r < kRounds; ++r) held[h][r] = next_held[h][r];
+      }
+      cur = nx;
+      s = s2;
     }
   }
   cluster_sync_all();

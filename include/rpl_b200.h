@@ -629,6 +629,41 @@ rpl_result rpl_capsule_stream_push_bytes_ts_dev(rpl_capsule_stream* s, const uin
                                                 const rpl_scan_params* params, float* ranges, float* intensities,
                                                 uint32_t* beam_counts, float* angle_increment,
                                                 uint32_t* scans_per_stream, uint64_t* scan_begin_ts_us, void* stream);
+/* Mixed byte sessions: a byte session in which every stream has its own answer type, and a stream's type can change
+ * between pushes, as the node's scan_mode parameter restarts the scan in another mode (rplidar_node.cpp:737-767).
+ *   create_bytes_mixed: ans_types [n_streams] (host), each 0x81..0x86; stride_bytes, max_nodes, max_scans and the 2^32
+ *            node limit as for create_bytes.  Every stream's regions are sized for the largest of the six types, so
+ *            that any later switch fits without reallocating: with F(t) = ceil(stride_bytes / frame size of t) and
+ *            S(t) = 2 * F(t) capsule slots (F for HQ), two node arenas of n_streams * (max_nodes + 96 *
+ *            ceil(stride_bytes / 132)) nodes of 8 bytes (ultra completes the most nodes from a push), n_streams *
+ *            max_t(S(t) * frame size of t) bytes of framed capsules (rounded up to 16) and n_streams * S(0x82) reports
+ *            and receive times of 16 bytes, an 800-byte framer record, the 0x81 scan-end table of n_streams * (arena
+ *            stride - max_nodes) words and the dense scan-start list.  A null ans_types, a type outside 0x81..0x86 or
+ *            framed capsules of 2^32 bytes or more per stream (stride_bytes near 2^31): RPL_RESULT_INVALID_DATA.
+ *   set_answer_types: the masked streams (stream_mask nullable: all) take ans_types[s]; synchronous, it waits for the
+ *            session's device calls in flight.  A stream whose type changes is reset exactly as rpl_capsule_stream_reset
+ *            resets it (held frame and search, held record, open revolution and its stamp, held receive time: the
+ *            SDK's startScan* holder reset and unpacker enable, sl_lidar_driver.cpp:640-657) and decodes as the new
+ *            type from the next push on; a stream whose type does not change is left alone (the node skips an
+ *            unchanged scan_mode, :741-743).  Counters, lidar and frame settings are kept, and the last push's clouds,
+ *            nodes and messages do not change.  A null ans_types, a masked type outside 0x81..0x86 or a session not
+ *            made by create_bytes_mixed: RPL_RESULT_INVALID_DATA and no stream changes.
+ *   Every byte session call (push_bytes*, with or without RPL_FLAG_PER_STREAM, reset, state, counters, set_frames,
+ *            set_lidars, cloud*, nodes*, laserscan_msgs*, cloud_msgs*) takes a mixed session; state reports held_bytes
+ *            and held_capsule by each stream's own type.  Without RPL_FLAG_PER_STREAM a push's sample_duration_us
+ *            serves every capsule-type stream and is ignored for 0x81 streams (a session of 0x81 streams alone
+ *            checks none).  Framed pushes: RPL_RESULT_INVALID_DATA, as on any byte session.
+ *   Definition: for any split into pushes, stream s gives bit for bit what a one-stream create_bytes session of its
+ *            type gives when fed the same pieces with the same params, in every output of every call above.  Across a
+ *            switch the stream's outputs are two such sessions in a row: the old type's up to the switch, then a fresh
+ *            session of the new type fed only the bytes after it; its counters are the sum of the two sessions'.
+ *   Cost: each push runs the framer (capsule types), decoder and assembler once per answer type present in each
+ *            chunk, over that type's streams, and the scan kernels once per chunk. */
+rpl_result rpl_capsule_stream_create_bytes_mixed(rpl_ctx* ctx, const uint32_t* ans_types, uint32_t n_streams,
+                                                 uint32_t stride_bytes, uint32_t max_nodes, uint32_t max_scans,
+                                                 rpl_capsule_stream** out);
+rpl_result rpl_capsule_stream_set_answer_types(rpl_capsule_stream* s, const uint32_t* ans_types,
+                                               const uint8_t* stream_mask);
 /* Session clouds: the PointCloud2 chain of rpl_cloud_batch_dev over the scans the session's last successful push
  * published, read in place from the session's node arenas (no copy of the scans, no second decode).
  *   Which scans: xyzi [n_streams * max_scans][max_nodes][4] floats (the layout of rpl_cloud_batch_dev), point_counts

@@ -20,7 +20,9 @@ objs=()
 for s in "${SRCS[@]}"; do
   o="$OBJ/$(basename "${s%.cu}").o"
   objs+=("$o")
-  if [[ ! -f "$o" || "$s" -nt "$o" || "$NEWEST_HDR" -nt "$o" ]]; then
+  # decode_list.cu compiles decode_formats.cu a second time (its stream-list instantiations)
+  dep="$s"; [[ "$(basename "$s")" == decode_list.cu ]] && dep="$HERE/csrc/decode_formats.cu"
+  if [[ ! -f "$o" || "$s" -nt "$o" || "$dep" -nt "$o" || "$NEWEST_HDR" -nt "$o" ]]; then
     ( "$NVCC" "${CFLAGS[@]}" -c -o "$o.tmp" "$s" && mv "$o.tmp" "$o" ) &
     pids+=($!)
   fi

@@ -54,6 +54,7 @@ EXPORTS = [
     "rpl_capsule_stream_reset", "rpl_capsule_stream_state", "rpl_capsule_stream_push_ts",
     "rpl_capsule_stream_push_ts_dev", "rpl_capsule_stream_counters",
     "rpl_capsule_stream_create_bytes", "rpl_capsule_stream_push_bytes", "rpl_capsule_stream_push_bytes_dev",
+    "rpl_capsule_stream_create_bytes_mixed", "rpl_capsule_stream_set_answer_types",
     "rpl_capsule_stream_push_bytes_ts", "rpl_capsule_stream_push_bytes_ts_dev",
     "rpl_capsule_stream_cloud", "rpl_capsule_stream_cloud_dev", "rpl_capsule_stream_set_frames",
     "rpl_capsule_stream_set_lidars", "rpl_capsule_stream_laserscan_msgs", "rpl_capsule_stream_laserscan_msgs_dev",
@@ -223,6 +224,8 @@ def lib() -> C.CDLL:
         "rpl_capsule_stream_push_ts": ([vp, vp, vp, PT, vp, PSP, vp, vp, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_push_ts_dev": ([vp, vp, vp, PT, vp, PSP, vp, vp, vp, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_create_bytes": ([vp, u32, u32, u32, u32, u32, C.POINTER(vp)], u32),
+        "rpl_capsule_stream_create_bytes_mixed": ([vp, vp, u32, u32, u32, u32, C.POINTER(vp)], u32),
+        "rpl_capsule_stream_set_answer_types": ([vp, vp, vp], u32),
         "rpl_capsule_stream_push_bytes": ([vp, vp, vp, u32, PSP, vp, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_push_bytes_dev": ([vp, vp, vp, u32, PSP, vp, vp, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_push_bytes_ts": ([vp, vp, vp, PT, u32, vp, PSP, vp, vp, vp, vp, vp, vp], u32),
@@ -920,6 +923,31 @@ class NormalStreamSession(CapsuleByteStreamSession):
         open_nodes, held_bytes = (np.zeros(self.n_streams, np.uint32) for _ in range(2))
         self._ctx._check(self._fn("state")(self._h, _p(open_nodes), None, _p(held_bytes)))
         return open_nodes, held_bytes
+
+
+class MixedByteStreamSession(CapsuleByteStreamSession):
+    """A byte session in which every stream has its own answer type (rpl_capsule_stream_create_bytes_mixed): ans_types
+    [n_streams], each 0x81..0x86, switched between pushes by set_answer_types.  Pushes, state and every other call are
+    the byte session's; a push's sample_duration_us serves the capsule-type streams and is ignored for 0x81 ones."""
+
+    def __init__(self, ctx: Context, ans_types, stride_bytes: int, max_nodes: int, max_scans: int):
+        t = np.ascontiguousarray(ans_types, dtype=np.uint32)
+        self._init(ctx, 0, t.size, 0, max_nodes, max_scans,
+                   lambda h: ctx._L.rpl_capsule_stream_create_bytes_mixed(ctx._h, _p(t), t.size, stride_bytes,
+                                                                           max_nodes, max_scans, C.byref(h)))
+        self.stride_bytes = stride_bytes
+        self.ans_types = t.copy()
+
+    def set_answer_types(self, ans_types, mask=None):
+        """The masked streams (mask [n_streams] of bool, None: all) take ans_types[s]; a stream whose type changes is
+        reset as reset() resets it, the others are left alone."""
+        t = np.ascontiguousarray(ans_types, dtype=np.uint32)
+        assert t.shape == (self.n_streams,)
+        m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
+        assert m is None or m.shape == (self.n_streams,)
+        self._ctx._check(self._fn("set_answer_types")(self._h, _p(t), _p(m)))
+        sel = np.ones(self.n_streams, bool) if m is None else m.astype(bool)
+        self.ans_types = np.where(sel, t, self.ans_types)
 
 
 EXCHANGE_NCCL, EXCHANGE_COPY = 0, 1

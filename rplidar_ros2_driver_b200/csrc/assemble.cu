@@ -70,9 +70,12 @@ __device__ __forceinline__ void rank_sort(const uint32_t* in, uint32_t* out, uin
 // STAMPED (a stamped session push, STREAM only): also the stamp of every published scan's scan-start node and of the
 // open revolution's first node, computed for those nodes alone (sa, and the delay model m0 or, with a per-stream table,
 // the stream's own)
-template <bool STREAM, bool STAMPED>
-__device__ __forceinline__ void assemble_body(const AssembleArgs& a, const AssembleStampArgs& sa, const DelayModel& m0) {
+// LIST (a mixed byte session, STREAM only): CTA slot i serves stream list.streams[i] of the chunk
+template <bool STREAM, bool STAMPED, bool LIST>
+__device__ __forceinline__ void assemble_body(const AssembleArgs& a, const AssembleStampArgs& sa, const DelayModel& m0,
+                                              const StreamList& list) {
   static_assert(STREAM || !STAMPED, "stamps are a stream session's");
+  static_assert(STREAM || !LIST, "stream lists are a stream session's");
   __shared__ uint32_t s_list[kListCap], s_sorted[kListCap];      // scan-start positions
   __shared__ uint32_t s_rlist[kResetCap], s_rsorted[kResetCap];  // reset positions
   __shared__ uint32_t s_cnt, s_rcnt;
@@ -84,7 +87,8 @@ __device__ __forceinline__ void assemble_body(const AssembleArgs& a, const Assem
   __shared__ uint32_t s_ct[kCtN];   // STREAM: this push's counts (block_count)
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 
-  for (uint32_t s = blockIdx.x; s < a.n_streams; s += gridDim.x) {
+  for (uint32_t i = blockIdx.x; i < a.n_streams; i += gridDim.x) {
+    const uint32_t s = LIST ? list.streams[i] : i;
     DelayModel m = m0;
     if constexpr (STAMPED)
       if (sa.lidars) m = delay_model(sa.ans_type, sa.lidars[s].timing);
@@ -440,27 +444,39 @@ __device__ __forceinline__ void assemble_body(const AssembleArgs& a, const Assem
 
 template <bool STREAM>
 __global__ void __launch_bounds__(AT) assemble_kernel(AssembleArgs a) {
-  assemble_body<STREAM, false>(a, AssembleStampArgs{}, DelayModel{});
+  assemble_body<STREAM, false, false>(a, AssembleStampArgs{}, DelayModel{}, StreamList{});
 }
 
 __global__ void __launch_bounds__(AT) assemble_stamped_kernel(AssembleArgs a, AssembleStampArgs sa, DelayModel m) {
-  assemble_body<true, true>(a, sa, m);
+  assemble_body<true, true, false>(a, sa, m, StreamList{});
+}
+
+template <bool STAMPED>
+__global__ void __launch_bounds__(AT) assemble_list_kernel(AssembleArgs a, AssembleStampArgs sa, DelayModel m,
+                                                           StreamList l) {
+  assemble_body<true, STAMPED, true>(a, sa, m, l);
 }
 
 }  // namespace
 
-cudaError_t launch_assemble(const AssembleArgs& a, int grid, cudaStream_t stream) {
+cudaError_t launch_assemble(const AssembleArgs& a, int grid, cudaStream_t stream, const StreamList* list) {
   if (a.n_streams == 0) return cudaSuccess;
-  if (a.carry_len)
+  if (list)
+    assemble_list_kernel<false><<<grid, AT, 0, stream>>>(a, AssembleStampArgs{}, DelayModel{}, *list);
+  else if (a.carry_len)
     assemble_kernel<true><<<grid, AT, 0, stream>>>(a);
   else
     assemble_kernel<false><<<grid, AT, 0, stream>>>(a);
   return cudaGetLastError();
 }
 
-cudaError_t launch_assemble_stamped(const AssembleArgs& a, const AssembleStampArgs& sa, int grid, cudaStream_t stream) {
+cudaError_t launch_assemble_stamped(const AssembleArgs& a, const AssembleStampArgs& sa, int grid, cudaStream_t stream,
+                                    const StreamList* list) {
   if (a.n_streams == 0) return cudaSuccess;
-  assemble_stamped_kernel<<<grid, AT, 0, stream>>>(a, sa, delay_model(sa.ans_type, sa.timing));
+  if (list)
+    assemble_list_kernel<true><<<grid, AT, 0, stream>>>(a, sa, delay_model(sa.ans_type, sa.timing), *list);
+  else
+    assemble_stamped_kernel<<<grid, AT, 0, stream>>>(a, sa, delay_model(sa.ans_type, sa.timing));
   return cudaGetLastError();
 }
 

@@ -9,6 +9,15 @@
 
 namespace rpl {
 
+// A mixed byte session's launch over the streams of one answer type (rpl_capsule_stream_create_bytes_mixed): the
+// framer, decoder and assembler take their regions as for the whole chunk, n_streams is the length of the list, and CTA
+// slot i serves stream streams[i] of the chunk.  capsule_stride: bytes per stream of the framed capsules (the framer's
+// output, the capsule decoder's input), which every answer type's slots share.
+struct StreamList {
+  const uint32_t* streams;  // [n_streams] chunk-relative stream indices, device
+  uint32_t capsule_stride;
+};
+
 // the capsule formats (decode_formats.cu): 0x82 express, 0x83 HQ, 0x84 ultra, 0x85 dense, 0x86 ultra-dense
 struct CapsuleDecodeArgs {
   const uint8_t* capsules;        // [n_streams][stride_capsules][capsule bytes]
@@ -94,8 +103,11 @@ struct NormalTimestampArgs {
 cudaError_t launch_node_timestamps(uint32_t ans_type, const TimingDesc& t, const TimestampArgs& a, cudaStream_t stream);
 cudaError_t launch_normal_timestamps(const TimingDesc& t, const NormalTimestampArgs& a, cudaStream_t stream);
 
-cudaError_t launch_decode_capsules(uint32_t ans_type, const CapsuleDecodeArgs& a, int grid, cudaStream_t stream);
-cudaError_t launch_decode_normal(const NormalDecodeArgs& a, int grid, cudaStream_t stream);
+// list (nullable): a mixed byte session's streams of this answer type (stream session instantiations only)
+cudaError_t launch_decode_capsules(uint32_t ans_type, const CapsuleDecodeArgs& a, int grid, cudaStream_t stream,
+                                   const StreamList* list = nullptr);
+cudaError_t launch_decode_normal(const NormalDecodeArgs& a, int grid, cudaStream_t stream,
+                                 const StreamList* list = nullptr);
 cudaError_t decode_formats_configure();
 
 struct AssembleArgs {
@@ -189,8 +201,10 @@ struct FrameStreamArgs {
   StreamCounters* counters;                 // [n_streams]: given bytes_in, frames and skipped_bytes
 };
 cudaError_t launch_frame_capsules(const FrameArgs& a, int grid, cudaStream_t stream);
-cudaError_t launch_frame_capsules_stream(const FrameArgs& a, const FrameStreamArgs& f, int grid, cudaStream_t stream);
-cudaError_t launch_assemble(const AssembleArgs& a, int grid, cudaStream_t stream);
-cudaError_t launch_assemble_stamped(const AssembleArgs& a, const AssembleStampArgs& t, int grid, cudaStream_t stream);
+cudaError_t launch_frame_capsules_stream(const FrameArgs& a, const FrameStreamArgs& f, int grid, cudaStream_t stream,
+                                         const StreamList* list = nullptr);
+cudaError_t launch_assemble(const AssembleArgs& a, int grid, cudaStream_t stream, const StreamList* list = nullptr);
+cudaError_t launch_assemble_stamped(const AssembleArgs& a, const AssembleStampArgs& t, int grid, cudaStream_t stream,
+                                    const StreamList* list = nullptr);
 
 }  // namespace rpl

@@ -37,6 +37,28 @@
 
 namespace rpl {
 
+// The stream-list instantiations (a mixed byte session's launches over the streams of one answer type, StreamList) are
+// compiled from this file in a translation unit of their own, decode_list.cu, with RPL_DECODE_LIST defined: there every
+// stream session kernel takes a StreamList l too, CTA slot i serves stream l.streams[i] of the chunk, and the capsule
+// decoders read each stream's capsules l.capsule_stride bytes apart.  Spelled as macros, so that the kernels of this
+// translation unit stay token for token what they were and compile to the same code.
+#ifdef RPL_DECODE_LIST
+#define RPL_LIST_PARAM , StreamList l
+#define RPL_LIST_ARG , l
+#define RPL_FOR_STREAMS(s) \
+  for (uint32_t i_ = blockIdx.x; i_ < a.n_streams; i_ += gridDim.x) if (const uint32_t s = l.streams[i_]; true)
+#define RPL_STREAM_CAPSULES(s, cb) (size_t)s * l.capsule_stride
+#else
+#define RPL_LIST_PARAM
+#define RPL_LIST_ARG
+#define RPL_FOR_STREAMS(s) for (uint32_t s = blockIdx.x; s < a.n_streams; s += gridDim.x)
+#define RPL_STREAM_CAPSULES(s, cb) (size_t)s * a.stride_capsules * cb
+#endif
+cudaError_t launch_decode_capsules_list(uint32_t ans_type, const CapsuleDecodeArgs& a, const StreamList& l, int grid,
+                                        cudaStream_t stream);
+cudaError_t launch_decode_normal_list(const NormalDecodeArgs& a, const StreamList& l, int grid, cudaStream_t stream);
+cudaError_t decode_list_configure();
+
 namespace {
 
 // threads = capsules per tile: Fmt<F>::DT (smaller tiles where the per-capsule state is large: more CTAs per SM, so a
@@ -290,7 +312,7 @@ struct CapsuleSmem {
 // previous tile's last capsule and its state (sm.carry, okflag[0], start_q8[0], carry_sync, carry_last), so a push
 // boundary is decoded as a tile boundary is.
 template <int F, bool STREAM>
-__global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecodeArgs a) {
+__global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecodeArgs a RPL_LIST_PARAM) {
   using T = Fmt<F>;
   constexpr int CB = T::CB, NODES = T::NODES, DT = T::DT;
   constexpr bool DENSE = F == kDense;
@@ -306,11 +328,11 @@ __global__ void __launch_bounds__(Fmt<F>::DT) decode_capsule_kernel(CapsuleDecod
     __syncthreads();
   }
 
-  for (uint32_t s = blockIdx.x; s < a.n_streams; s += gridDim.x) {
+  RPL_FOR_STREAMS(s) {
     if constexpr (STREAM && T::JUMP_CABINS != 0)
       if (a.lidars) thr_q8 = (360 * 100 * T::JUMP_CABINS / (int)(1000000u / a.lidars[s].timing.sample_duration_us)) << 8;
     const uint32_t n = STREAM ? min(a.counts[s], a.stride_capsules) : a.counts[s];
-    const uint8_t* src = a.capsules + (size_t)s * a.stride_capsules * CB;
+    const uint8_t* src = a.capsules + RPL_STREAM_CAPSULES(s, CB);
     uint2* out = STREAM ? a.nodes_out + (size_t)s * a.node_stride + a.node_first
                         : a.nodes_out + (size_t)s * a.stride_capsules * NODES;
     uint32_t* st_out = a.capsule_status ? a.capsule_status + (size_t)s * a.stride_capsules : nullptr;
@@ -718,7 +740,7 @@ struct HqSmem {
 // STREAM: a stream session's instantiation.  HQ capsules carry nothing across capsules (handler_hqnode.cpp:93-172), so
 // it differs only in where the nodes go (behind the session's carry slots).
 template <bool STREAM>
-__global__ void __launch_bounds__(HT) decode_hq_kernel(CapsuleDecodeArgs a) {
+__global__ void __launch_bounds__(HT) decode_hq_kernel(CapsuleDecodeArgs a RPL_LIST_PARAM) {
   extern __shared__ __align__(16) unsigned char capsule_smem_raw[];
   HqSmem& sm = *reinterpret_cast<HqSmem*>(capsule_smem_raw);
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -743,9 +765,9 @@ __global__ void __launch_bounds__(HT) decode_hq_kernel(CapsuleDecodeArgs a) {
     return sm.advance[which][0][v & 0xFFu] ^ sm.advance[which][1][(v >> 8) & 0xFFu] ^ sm.advance[which][2][(v >> 16) & 0xFFu] ^
            sm.advance[which][3][v >> 24];
   };
-  for (uint32_t s = blockIdx.x; s < a.n_streams; s += gridDim.x) {
+  RPL_FOR_STREAMS(s) {
     const uint32_t n = STREAM ? min(a.counts[s], a.stride_capsules) : a.counts[s];
-    const uint8_t* src = a.capsules + (size_t)s * a.stride_capsules * kHqBytes;
+    const uint8_t* src = a.capsules + RPL_STREAM_CAPSULES(s, kHqBytes);
     uint2* out = STREAM ? a.nodes_out + (size_t)s * a.node_stride + a.node_first
                         : a.nodes_out + (size_t)s * a.stride_capsules * 96;
     uint32_t* st_out = a.capsule_status ? a.capsule_status + (size_t)s * a.stride_capsules : nullptr;
@@ -893,12 +915,12 @@ __device__ __forceinline__ uint32_t compose_map(uint32_t g, uint32_t f) {
 // STARTS (a stamped session push, STREAM only): node_end [n_streams][node_stride - node_first] gets the push-relative
 // index of the last byte of the scan-start records alone, at their node index (a few stores per revolution)
 template <bool STREAM, bool STARTS>
-__device__ __forceinline__ void decode_normal_body(const NormalDecodeArgs& a) {
+__device__ __forceinline__ void decode_normal_body(const NormalDecodeArgs& a RPL_LIST_PARAM) {
   static_assert(STREAM || !STARTS, "the scan-start ends are a stream session's");
   __shared__ __align__(16) NormalSmem sm;
   uint8_t* const sm_bytes = sm.raw + 12;  // bytes[0..3] = halo, bytes + 4 = the tile
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  for (uint32_t s = blockIdx.x; s < a.n_streams; s += gridDim.x) {
+  RPL_FOR_STREAMS(s) {
     const uint32_t n = STREAM ? min(a.byte_counts[s], a.stride_bytes) : a.byte_counts[s];
     const uint8_t* src = a.bytes + (size_t)s * a.stride_bytes;
     uint2* out = STREAM ? a.nodes_out + (size_t)s * a.node_stride + a.node_first
@@ -1079,63 +1101,16 @@ __device__ __forceinline__ void decode_normal_body(const NormalDecodeArgs& a) {
 }
 
 template <bool STREAM>
-__global__ void __launch_bounds__(NT, 5) decode_normal_kernel(NormalDecodeArgs a) {
-  decode_normal_body<STREAM, false>(a);
+__global__ void __launch_bounds__(NT, 5) decode_normal_kernel(NormalDecodeArgs a RPL_LIST_PARAM) {
+  decode_normal_body<STREAM, false>(a RPL_LIST_ARG);
 }
 
-__global__ void __launch_bounds__(NT, 5) decode_normal_starts_kernel(NormalDecodeArgs a) {
-  decode_normal_body<true, true>(a);
+__global__ void __launch_bounds__(NT, 5) decode_normal_starts_kernel(NormalDecodeArgs a RPL_LIST_PARAM) {
+  decode_normal_body<true, true>(a RPL_LIST_ARG);
 }
 
-template <int F>
-cudaError_t launch_fmt(const CapsuleDecodeArgs& a, int grid, cudaStream_t stream) {
-  if (a.node_stride)
-    decode_capsule_kernel<F, true><<<grid, Fmt<F>::DT, sizeof(CapsuleSmem<F>), stream>>>(a);
-  else
-    decode_capsule_kernel<F, false><<<grid, Fmt<F>::DT, sizeof(CapsuleSmem<F>), stream>>>(a);
-  return cudaGetLastError();
-}
-
-template <int F>
-cudaError_t configure_fmt() {
-  cudaError_t e = cudaFuncSetAttribute(decode_capsule_kernel<F, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)sizeof(CapsuleSmem<F>));
-  if (e != cudaSuccess) return e;
-  return cudaFuncSetAttribute(decode_capsule_kernel<F, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                              (int)sizeof(CapsuleSmem<F>));
-}
-
-}  // namespace
-
-cudaError_t launch_decode_capsules(uint32_t ans_type, const CapsuleDecodeArgs& a, int grid, cudaStream_t stream) {
-  if (a.n_streams == 0) return cudaSuccess;
-  switch (ans_type) {
-    case 0x82: return launch_fmt<kExpress>(a, grid, stream);
-    case 0x84: return launch_fmt<kUltra>(a, grid, stream);
-    case 0x85: return launch_fmt<kDense>(a, grid, stream);
-    case 0x86: return launch_fmt<kUltraDense>(a, grid, stream);
-    case 0x83:
-      if (a.node_stride)
-        decode_hq_kernel<true><<<grid, HT, sizeof(HqSmem), stream>>>(a);
-      else
-        decode_hq_kernel<false><<<grid, HT, sizeof(HqSmem), stream>>>(a);
-      return cudaGetLastError();
-    default: return cudaErrorInvalidValue;
-  }
-}
-
-cudaError_t launch_decode_normal(const NormalDecodeArgs& a, int grid, cudaStream_t stream) {
-  if (a.n_streams == 0) return cudaSuccess;
-  if (a.node_stride && a.node_end)
-    decode_normal_starts_kernel<<<grid, NT, 0, stream>>>(a);
-  else if (a.node_stride)
-    decode_normal_kernel<true><<<grid, NT, 0, stream>>>(a);
-  else
-    decode_normal_kernel<false><<<grid, NT, 0, stream>>>(a);
-  return cudaGetLastError();
-}
-
-cudaError_t decode_formats_configure() {
+// the decoders' tables, in this translation unit's device memory
+cudaError_t upload_tables() {
   cudaError_t e;
   {  // handler_capsules.cpp:546-556, evaluated exactly as written there (double arithmetic, truncation)
     int table[493];
@@ -1167,12 +1142,118 @@ cudaError_t decode_formats_configure() {
     e = cudaMemcpyToSymbol(g_hq_advance, adv, sizeof(adv));
     if (e != cudaSuccess) return e;
   }
+  return cudaSuccess;
+}
+
+#ifndef RPL_DECODE_LIST
+template <int F>
+cudaError_t launch_fmt(const CapsuleDecodeArgs& a, int grid, cudaStream_t stream) {
+  if (a.node_stride)
+    decode_capsule_kernel<F, true><<<grid, Fmt<F>::DT, sizeof(CapsuleSmem<F>), stream>>>(a);
+  else
+    decode_capsule_kernel<F, false><<<grid, Fmt<F>::DT, sizeof(CapsuleSmem<F>), stream>>>(a);
+  return cudaGetLastError();
+}
+
+template <int F>
+cudaError_t configure_fmt() {
+  cudaError_t e = cudaFuncSetAttribute(decode_capsule_kernel<F, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)sizeof(CapsuleSmem<F>));
+  if (e != cudaSuccess) return e;
+  return cudaFuncSetAttribute(decode_capsule_kernel<F, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              (int)sizeof(CapsuleSmem<F>));
+}
+
+}  // namespace
+
+cudaError_t launch_decode_capsules(uint32_t ans_type, const CapsuleDecodeArgs& a, int grid, cudaStream_t stream,
+                                   const StreamList* list) {
+  if (a.n_streams == 0) return cudaSuccess;
+  if (list) return launch_decode_capsules_list(ans_type, a, *list, grid, stream);
+  switch (ans_type) {
+    case 0x82: return launch_fmt<kExpress>(a, grid, stream);
+    case 0x84: return launch_fmt<kUltra>(a, grid, stream);
+    case 0x85: return launch_fmt<kDense>(a, grid, stream);
+    case 0x86: return launch_fmt<kUltraDense>(a, grid, stream);
+    case 0x83:
+      if (a.node_stride)
+        decode_hq_kernel<true><<<grid, HT, sizeof(HqSmem), stream>>>(a);
+      else
+        decode_hq_kernel<false><<<grid, HT, sizeof(HqSmem), stream>>>(a);
+      return cudaGetLastError();
+    default: return cudaErrorInvalidValue;
+  }
+}
+
+cudaError_t launch_decode_normal(const NormalDecodeArgs& a, int grid, cudaStream_t stream, const StreamList* list) {
+  if (a.n_streams == 0) return cudaSuccess;
+  if (list) return launch_decode_normal_list(a, *list, grid, stream);
+  if (a.node_stride && a.node_end)
+    decode_normal_starts_kernel<<<grid, NT, 0, stream>>>(a);
+  else if (a.node_stride)
+    decode_normal_kernel<true><<<grid, NT, 0, stream>>>(a);
+  else
+    decode_normal_kernel<false><<<grid, NT, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
+cudaError_t decode_formats_configure() {
+  cudaError_t e;
+  if ((e = upload_tables()) != cudaSuccess) return e;
   if ((e = configure_fmt<kExpress>()) != cudaSuccess || (e = configure_fmt<kUltra>()) != cudaSuccess ||
       (e = configure_fmt<kDense>()) != cudaSuccess || (e = configure_fmt<kUltraDense>()) != cudaSuccess)
     return e;
   e = cudaFuncSetAttribute(decode_hq_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HqSmem));
   if (e != cudaSuccess) return e;
+  e = cudaFuncSetAttribute(decode_hq_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HqSmem));
+  if (e != cudaSuccess) return e;
+  return decode_list_configure();
+}
+#else
+template <int F>
+cudaError_t launch_fmt(const CapsuleDecodeArgs& a, const StreamList& l, int grid, cudaStream_t stream) {
+  decode_capsule_kernel<F, true><<<grid, Fmt<F>::DT, sizeof(CapsuleSmem<F>), stream>>>(a, l);
+  return cudaGetLastError();
+}
+
+template <int F>
+cudaError_t configure_fmt() {
+  return cudaFuncSetAttribute(decode_capsule_kernel<F, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              (int)sizeof(CapsuleSmem<F>));
+}
+
+}  // namespace
+
+cudaError_t launch_decode_capsules_list(uint32_t ans_type, const CapsuleDecodeArgs& a, const StreamList& l, int grid,
+                                        cudaStream_t stream) {
+  switch (ans_type) {
+    case 0x82: return launch_fmt<kExpress>(a, l, grid, stream);
+    case 0x84: return launch_fmt<kUltra>(a, l, grid, stream);
+    case 0x85: return launch_fmt<kDense>(a, l, grid, stream);
+    case 0x86: return launch_fmt<kUltraDense>(a, l, grid, stream);
+    case 0x83:
+      decode_hq_kernel<true><<<grid, HT, sizeof(HqSmem), stream>>>(a, l);
+      return cudaGetLastError();
+    default: return cudaErrorInvalidValue;
+  }
+}
+
+cudaError_t launch_decode_normal_list(const NormalDecodeArgs& a, const StreamList& l, int grid, cudaStream_t stream) {
+  if (a.node_end)
+    decode_normal_starts_kernel<<<grid, NT, 0, stream>>>(a, l);
+  else
+    decode_normal_kernel<true><<<grid, NT, 0, stream>>>(a, l);
+  return cudaGetLastError();
+}
+
+cudaError_t decode_list_configure() {
+  cudaError_t e;
+  if ((e = upload_tables()) != cudaSuccess) return e;
+  if ((e = configure_fmt<kExpress>()) != cudaSuccess || (e = configure_fmt<kUltra>()) != cudaSuccess ||
+      (e = configure_fmt<kDense>()) != cudaSuccess || (e = configure_fmt<kUltraDense>()) != cudaSuccess)
+    return e;
   return cudaFuncSetAttribute(decode_hq_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(HqSmem));
 }
+#endif
 
 }  // namespace rpl

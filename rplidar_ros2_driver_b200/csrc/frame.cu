@@ -50,20 +50,24 @@ struct FrameSmem {
   uint32_t n_entries, new_pos, lost, done;
 };
 
-template <bool STREAM>
-__global__ void __launch_bounds__(FT) frame_capsules_kernel(FrameArgs a, FrameStreamArgs f) {
+// LIST (a mixed byte session, STREAM only): CTA slot i serves stream list.streams[i] of the chunk, whose framed
+// capsules start list.capsule_stride bytes apart
+template <bool STREAM, bool LIST>
+__device__ __forceinline__ void frame_capsules_body(FrameArgs a, FrameStreamArgs f, StreamList list) {
+  static_assert(STREAM || !LIST, "stream lists are a byte session's");
   __shared__ FrameSmem<STREAM> sm;
   const uint32_t tid = threadIdx.x;
   const uint32_t cb = a.capsule_bytes;
   const bool hq = STREAM && cb == kHqFrame;
   uint8_t* sb = reinterpret_cast<uint8_t*>(sm.words);
-  for (uint32_t s = blockIdx.x; s < a.n_streams; s += gridDim.x) {
+  for (uint32_t i = blockIdx.x; i < a.n_streams; i += gridDim.x) {
+    const uint32_t s = LIST ? list.streams[i] : i;
     // session: stream positions count from the first held byte; the push's byte i is position k + i
     uint32_t* rec = STREAM ? f.framer + (size_t)s * kFramerWords : nullptr;
     const uint32_t k = STREAM ? rec[kFramerPos] : 0u;
     const uint8_t* in = a.bytes + (size_t)s * a.stride_bytes;
     const uint32_t n = STREAM ? k + min(a.byte_counts[s], a.stride_bytes) : a.byte_counts[s];
-    uint8_t* out = a.capsules_out + (size_t)s * a.stride_capsules * cb;
+    uint8_t* out = a.capsules_out + (LIST ? (size_t)s * list.capsule_stride : (size_t)s * a.stride_capsules * cb);
     const unsigned long long* rx_in = STREAM && f.chunk_rx_us ? f.chunk_rx_us + (size_t)s * f.stride_chunks : nullptr;
     unsigned long long* rx_out = STREAM ? f.capsule_rx_out + (size_t)s * a.stride_capsules : nullptr;
     uint32_t pos = 0, count = 0, tile = 0;
@@ -206,6 +210,15 @@ __global__ void __launch_bounds__(FT) frame_capsules_kernel(FrameArgs a, FrameSt
   }
 }
 
+template <bool STREAM>
+__global__ void __launch_bounds__(FT) frame_capsules_kernel(FrameArgs a, FrameStreamArgs f) {
+  frame_capsules_body<STREAM, false>(a, f, StreamList{});
+}
+
+__global__ void __launch_bounds__(FT) frame_capsules_list_kernel(FrameArgs a, FrameStreamArgs f, StreamList l) {
+  frame_capsules_body<true, true>(a, f, l);
+}
+
 }  // namespace
 
 cudaError_t launch_frame_capsules(const FrameArgs& a, int grid, cudaStream_t stream) {
@@ -214,9 +227,13 @@ cudaError_t launch_frame_capsules(const FrameArgs& a, int grid, cudaStream_t str
   return cudaGetLastError();
 }
 
-cudaError_t launch_frame_capsules_stream(const FrameArgs& a, const FrameStreamArgs& f, int grid, cudaStream_t stream) {
+cudaError_t launch_frame_capsules_stream(const FrameArgs& a, const FrameStreamArgs& f, int grid, cudaStream_t stream,
+                                         const StreamList* list) {
   if (a.n_streams == 0) return cudaSuccess;
-  frame_capsules_kernel<true><<<grid, FT, 0, stream>>>(a, f);
+  if (list)
+    frame_capsules_list_kernel<<<grid, FT, 0, stream>>>(a, f, *list);
+  else
+    frame_capsules_kernel<true><<<grid, FT, 0, stream>>>(a, f);
   return cudaGetLastError();
 }
 

@@ -761,23 +761,26 @@ rpl_result rpl_scan(rpl_ctx* c, rpl_node_hq* nodes, size_t count, const rpl_scan
 // ---- dense-capsule decode (SURVEY.md 8(f) rank 1) ---------------------------------------------
 namespace {
 // one launch of the capsule decoder on arguments the entry point has checked (n_streams > 0)
-rpl_result decode_capsules_launch(rpl_ctx* c, uint32_t ans_type, const rpl::CapsuleDecodeArgs& a, void* stream) {
+// (list: a mixed byte session's streams of this type, a.n_streams of them)
+rpl_result decode_capsules_launch(rpl_ctx* c, uint32_t ans_type, const rpl::CapsuleDecodeArgs& a, void* stream,
+                                  const rpl::StreamList* list = nullptr) {
   cudaStream_t st;
   if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   // one CTA per stream, up to four (dense) or eight (the other formats) CTAs per SM; a CTA loops over the rest
   const uint32_t ctas_per_sm = ans_type == 0x85 ? 4u : 8u;
   const int grid = (int)std::min<uint32_t>(a.n_streams, (uint32_t)c->num_sms * ctas_per_sm);
-  RPL_CUDA(c, rpl::launch_decode_capsules(ans_type, a, grid, st), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, rpl::launch_decode_capsules(ans_type, a, grid, st, list), RPL_RESULT_OPERATION_FAIL);
   c->launches++;
   return RPL_RESULT_OK;
 }
 
 // one launch of the standard-node decoder on arguments the entry point has checked (n_streams > 0)
-rpl_result decode_normal_launch(rpl_ctx* c, const rpl::NormalDecodeArgs& a, void* stream) {
+rpl_result decode_normal_launch(rpl_ctx* c, const rpl::NormalDecodeArgs& a, void* stream,
+                                const rpl::StreamList* list = nullptr) {
   cudaStream_t st;
   if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   const int grid = (int)std::min<uint32_t>(a.n_streams, (uint32_t)c->num_sms * 8u);
-  RPL_CUDA(c, rpl::launch_decode_normal(a, grid, st), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, rpl::launch_decode_normal(a, grid, st, list), RPL_RESULT_OPERATION_FAIL);
   c->launches++;
   return RPL_RESULT_OK;
 }
@@ -1036,7 +1039,8 @@ rpl_result rpl_decode_normal(rpl_ctx* c, const uint8_t* bytes, uint32_t n_bytes,
 }  // extern "C"
 
 namespace {
-// copy mode (scans_out) or view mode (views_out + writable nodes)
+// copy mode (scans_out) or view mode (views_out + writable nodes); with `list` (a mixed byte session's launch over the
+// n_streams streams of one answer type) the regions are those of the list_span streams of the chunk
 rpl_result assemble_common(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t* node_counts,
                                   uint32_t n_streams, uint32_t stride_nodes, const uint32_t* capsule_status,
                                   const uint32_t* capsule_node_offset, const uint32_t* capsule_counts,
@@ -1047,9 +1051,11 @@ rpl_result assemble_common(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t*
                                   uint32_t starts_stride = 0, const uint32_t* scan_start_counts = nullptr,
                                   const uint32_t* carry_len = nullptr, rpl_node_hq* carry_out = nullptr,
                                   uint32_t* carry_len_out = nullptr, const rpl::AssembleStampArgs* stamp = nullptr,
-                                  rpl::StreamCounters* counters = nullptr, uint32_t counted_capsule_bytes = 0) {
+                                  rpl::StreamCounters* counters = nullptr, uint32_t counted_capsule_bytes = 0,
+                                  const rpl::StreamList* list = nullptr, uint32_t list_span = 0) {
   if (!c || !nodes || !node_counts || (!scans_out && !views_out) || !scan_len || !scans_per_stream) return RPL_RESULT_INVALID_DATA;
-  if (views_out && (unsigned long long)n_streams * stride_nodes > 0xFFFFFFFFull) {
+  const uint32_t span = list ? list_span : n_streams;
+  if (views_out && (unsigned long long)span * stride_nodes > 0xFFFFFFFFull) {
     c->err = "view mode addresses nodes with 32 bits: n_streams * stride_nodes must stay below 2^32";
     return RPL_RESULT_INVALID_DATA;
   }
@@ -1069,8 +1075,8 @@ rpl_result assemble_common(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t*
   if (n_streams == 0) return RPL_RESULT_OK;
   cudaStream_t st;
   if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
-  const size_t need_rp = (size_t)n_streams * std::max<uint32_t>(stride_capsules, 1u);
-  const size_t need_desc = (size_t)n_streams * max_scans;
+  const size_t need_rp = (size_t)span * std::max<uint32_t>(stride_capsules, 1u);
+  const size_t need_desc = (size_t)span * max_scans;
   if (need_rp > c->reset_prefix_cap) {
     cudaFree(c->d_reset_prefix);
     c->d_reset_prefix = nullptr;
@@ -1114,9 +1120,9 @@ rpl_result assemble_common(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t*
   a.counted_capsule_bytes = counted_capsule_bytes;
   const int grid = (int)std::min<uint32_t>(n_streams, (uint32_t)c->num_sms * 4u);
   if (stamp)
-    RPL_CUDA(c, rpl::launch_assemble_stamped(a, *stamp, grid, st), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, rpl::launch_assemble_stamped(a, *stamp, grid, st, list), RPL_RESULT_OPERATION_FAIL);
   else
-    RPL_CUDA(c, rpl::launch_assemble(a, grid, st), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, rpl::launch_assemble(a, grid, st, list), RPL_RESULT_OPERATION_FAIL);
   c->launches++;
   return RPL_RESULT_OK;
 }
@@ -1232,6 +1238,14 @@ struct rpl_capsule_stream {
   uint8_t* framed = nullptr;                    // [n_streams][stride_capsules][cap_bytes]
   uint32_t* framed_counts = nullptr;            // [n_streams]
   unsigned long long* framed_rx = nullptr;      // [n_streams][stride_capsules] (stamped pushes)
+  size_t framed_stride = 0;                     // bytes per stream of `framed`
+  // a mixed byte session (rpl_capsule_stream_create_bytes_mixed; ans_type 0): each stream's answer type, and for the
+  // host-push chunks (0) and the device-push chunks (1) the chunk-relative indices of every chunk's streams grouped by
+  // answer type (lists[k] + s0: the chunk from stream s0's), which list_begin[k] directs: entry 7 * chunk + t the first
+  // position of type 0x81 + t in that chunk's list (t = 6: its end)
+  std::vector<uint32_t> types;                  // [n_streams] host; empty: a single-type session
+  uint32_t* lists[2] = {nullptr, nullptr};     // [n_streams] device
+  std::vector<uint32_t> list_begin[2];
   // the last push, as the cloud calls replay it: its views count from the first stream of their chunk
   uint32_t cloud_chunk = 0;                     // streams per chunk (chunk_host or chunk_dev); 0: no push, or it failed
   uint32_t cloud_arena = 0;                     // the arena its views point into
@@ -1303,6 +1317,10 @@ struct WireChunk {
   uint32_t *framer, *framed_counts;
   uint8_t* framed;
   unsigned long long* framed_rx;
+  size_t framed_stride;
+  // a mixed byte session's: the chunk's streams by answer type (the session's lists and list_begin at this chunk)
+  const uint32_t* lists;
+  const uint32_t* list_begin;
   // a session push with RPL_FLAG_PER_STREAM: the chunk's first stream's entry of the session's table (else nullptr)
   const rpl::LidarSettings* lidars;
   uint32_t lidar_modes;
@@ -1312,8 +1330,9 @@ struct WireChunk {
   uint32_t counted_capsule_bytes;
 };
 
-// session cs's chunk from stream s0 in the push under way (arena cs->parity); per_stream: RPL_FLAG_PER_STREAM
-WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0, bool per_stream) {
+// session cs's chunk from stream s0 in the push under way (arena cs->parity); per_stream: RPL_FLAG_PER_STREAM; dev: a
+// device push's chunking (else a host push's)
+WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0, bool per_stream, bool dev) {
   const uint32_t p = cs->parity, sc = cs->stride_capsules;
   const size_t sn = (size_t)s0 * cs->stride_nodes, so = (size_t)s0 * cs->max_scans;
   WireChunk w{};
@@ -1348,9 +1367,15 @@ WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0, bool per_stre
   if (cs->framer) {
     w.stride_bytes = cs->stride_in;
     w.framer = cs->framer + (size_t)s0 * rpl::kFramerWords;
-    w.framed = cs->framed + (size_t)s0 * sc * cs->cap_bytes;
+    w.framed = cs->framed + (size_t)s0 * cs->framed_stride;
     w.framed_counts = cs->framed_counts + s0;
     w.framed_rx = cs->framed_rx + (size_t)s0 * sc;
+    w.framed_stride = cs->framed_stride;
+  }
+  if (!cs->types.empty()) {
+    const uint32_t chunk = dev ? cs->chunk_dev : cs->chunk_host;
+    w.lists = cs->lists[dev] + s0;
+    w.list_begin = cs->list_begin[dev].data() + (size_t)7 * (s0 / chunk);
   }
   if (per_stream) {
     w.lidars = cs->lidars + s0;
@@ -1359,22 +1384,33 @@ WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0, bool per_stre
   return w;
 }
 
-// (frame ->) decode -> assemble -> scan kernels for the ns streams of chunk w on `st`; capsules / counts / outputs / sp
-// point at the chunk's first stream's (a byte session's capsules / counts: the raw bytes and byte counts)
-rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const WireChunk& w, uint32_t ns,
-                                const uint8_t* capsules, const uint32_t* counts, uint32_t sample_duration_us,
-                                const rpl_scan_params* params, float* ranges, float* intens, uint32_t* beams,
-                                float* inc, uint32_t* scans_per_stream, const StampPush* sp = nullptr) {
-  const uint32_t sc = w.stride_capsules;
+// a mixed byte session's launch over the n streams of one answer type in a chunk
+struct ListLaunch {
+  rpl::StreamList l;
+  uint32_t n;
+};
+
+// (frame ->) decode -> assemble of the ns streams of chunk w on `st` as answer type ans_type, or with `list` (a mixed
+// byte session's) of the list->streams of that type alone; capsules / counts / sp as capsule_stream_chunk's
+rpl_result decode_assemble(rpl_ctx* c, cudaStream_t st, const WireChunk& w, uint32_t ans_type, uint32_t ns,
+                           const uint8_t* capsules, const uint32_t* counts, uint32_t sample_duration_us,
+                           uint32_t* scans_per_stream, const StampPush* sp, const ListLaunch* list) {
+  const uint32_t sc = w.stride_capsules, n = list ? list->n : ns;
+  const bool normal = ans_type == RPL_ANS_MEASUREMENT;
+  uint32_t* status = normal ? nullptr : w.status;  // the per-capsule reports
+  uint32_t* offsets = normal ? nullptr : w.offsets;
+  uint32_t* starts = ans_type == 0x85 ? w.starts : nullptr;
+  uint32_t* start_counts = ans_type == 0x85 ? w.start_counts : nullptr;
+  const rpl::StreamList* l = list ? &list->l : nullptr;
   uint32_t* ends = sp ? w.node_end : nullptr;
   StampPush framed_sp{};
-  if (w.framer) {
+  if (w.framer && !normal) {
     rpl::FrameArgs a{};
     a.bytes = capsules;
     a.byte_counts = counts;
-    a.n_streams = ns;
+    a.n_streams = n;
     a.stride_bytes = w.stride_bytes;
-    a.capsule_bytes = rpl_capsule_bytes(w.ans_type);
+    a.capsule_bytes = rpl_capsule_bytes(ans_type);
     a.capsules_out = w.framed;
     a.stride_capsules = sc;
     a.capsule_counts_out = w.framed_counts;
@@ -1390,19 +1426,19 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
       framed_sp.rx = w.framed_rx;
       sp = &framed_sp;
     }
-    const int grid = (int)std::min<uint32_t>(ns, (uint32_t)c->num_sms * 8u);
-    RPL_CUDA(c, rpl::launch_frame_capsules_stream(a, f, grid, st), RPL_RESULT_OPERATION_FAIL);
+    const int grid = (int)std::min<uint32_t>(n, (uint32_t)c->num_sms * 8u);
+    RPL_CUDA(c, rpl::launch_frame_capsules_stream(a, f, grid, st, l), RPL_RESULT_OPERATION_FAIL);
     c->launches++;
     capsules = w.framed;
     counts = w.framed_counts;
   }
   rpl_result r;
-  if (w.ans_type == RPL_ANS_MEASUREMENT) {
+  if (normal) {
     rpl::NormalDecodeArgs a{};
     a.bytes = capsules;
     a.byte_counts = counts;
-    a.n_streams = ns;
-    a.stride_bytes = sc;
+    a.n_streams = n;
+    a.stride_bytes = list ? w.stride_bytes : sc;
     a.nodes_out = reinterpret_cast<uint2*>(w.nodes);
     a.node_counts = w.node_counts;
     a.held = w.held;
@@ -1410,27 +1446,27 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
     a.node_first = w.node_first;
     a.node_end = ends;
     a.counters = w.counters;
-    r = decode_normal_launch(c, a, st);
+    r = decode_normal_launch(c, a, st, l);
   } else {
     rpl::CapsuleDecodeArgs a{};
     a.capsules = capsules;
     a.counts = counts;
-    a.n_streams = ns;
+    a.n_streams = n;
     a.stride_capsules = sc;
     a.sample_duration_us = sample_duration_us;
     a.state_words = 1;
     a.nodes_out = reinterpret_cast<uint2*>(w.nodes);
     a.node_counts = w.node_counts;
-    a.capsule_status = w.status;
-    a.capsule_node_offset = w.offsets;
-    a.scan_starts = w.starts;
-    a.scan_start_counts = w.start_counts;
+    a.capsule_status = status;
+    a.capsule_node_offset = offsets;
+    a.scan_starts = starts;
+    a.scan_start_counts = start_counts;
     a.starts_stride = w.starts_stride;
     a.held = w.held;
     a.node_stride = w.node_stride;
     a.node_first = w.node_first;
     a.lidars = w.lidars;
-    r = decode_capsules_launch(c, w.ans_type, a, st);
+    r = decode_capsules_launch(c, ans_type, a, st, l);
   }
   if (r != RPL_RESULT_OK) return r;
   // the assembler's scratch belongs to the context: one assemble kernel at a time, whatever lane or stream
@@ -1438,14 +1474,14 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
   RPL_CUDA(c, cudaStreamWaitEvent(st, c->asm_done, 0), RPL_RESULT_OPERATION_FAIL);
   rpl::AssembleStampArgs t{};
   if (sp) {
-    t.ans_type = w.ans_type;
+    t.ans_type = ans_type;
     t.timing = sp->timing;
-    t.capsule_rx_us = w.status ? sp->rx : nullptr;
+    t.capsule_rx_us = status ? sp->rx : nullptr;
     t.node_end = ends;
     t.stride_ends = w.stride_nodes - w.node_first;
     t.chunk_bytes = sp->chunk_bytes;
     t.stride_chunks = sp->stride_chunks;
-    t.chunk_rx_us = w.status ? nullptr : sp->rx;
+    t.chunk_rx_us = status ? nullptr : sp->rx;
     t.open_ts_in = w.open_ts_in;
     t.open_ts_out = w.open_ts_out;
     t.held_rx = w.held_rx;
@@ -1454,13 +1490,37 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
     t.slot_end_us = w.slot_end;
     t.lidars = w.lidars;
   }
-  r = assemble_common(c, w.nodes, w.node_counts, ns, w.stride_nodes, w.status, w.offsets, w.status ? counts : nullptr,
-                      w.status ? sc : 0u, w.max_nodes, w.max_scans, w.max_nodes, nullptr, w.views, w.scan_len,
-                      scans_per_stream, nullptr, sp ? reinterpret_cast<uint64_t*>(sp->scan_ts) : nullptr, st, w.starts,
-                      w.starts ? w.starts_stride : 0u, w.start_counts, w.carry_len, w.carry_out, w.carry_len_out,
-                      sp ? &t : nullptr, w.counters, w.counted_capsule_bytes);
+  r = assemble_common(c, w.nodes, w.node_counts, n, w.stride_nodes, status, offsets, status ? counts : nullptr,
+                      status ? sc : 0u, w.max_nodes, w.max_scans, w.max_nodes, nullptr, w.views, w.scan_len,
+                      scans_per_stream, nullptr, sp ? reinterpret_cast<uint64_t*>(sp->scan_ts) : nullptr, st, starts,
+                      starts ? w.starts_stride : 0u, start_counts, w.carry_len, w.carry_out, w.carry_len_out,
+                      sp ? &t : nullptr, w.counters, w.counted_capsule_bytes, l, ns);
   if (r != RPL_RESULT_OK) return r;
   RPL_CUDA(c, cudaEventRecord(c->asm_done, st), RPL_RESULT_OPERATION_FAIL);
+  return RPL_RESULT_OK;
+}
+
+// (frame ->) decode -> assemble -> scan kernels for the ns streams of chunk w on `st`; capsules / counts / outputs / sp
+// point at the chunk's first stream's (a byte session's capsules / counts: the raw bytes and byte counts).  A mixed
+// byte session's chunk runs the first three for each answer type present in it, over that type's streams, and the scan
+// kernels, which read the arenas whatever the type, once.
+rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const WireChunk& w, uint32_t ns,
+                                const uint8_t* capsules, const uint32_t* counts, uint32_t sample_duration_us,
+                                const rpl_scan_params* params, float* ranges, float* intens, uint32_t* beams,
+                                float* inc, uint32_t* scans_per_stream, const StampPush* sp = nullptr) {
+  rpl_result r = RPL_RESULT_OK;
+  if (!w.list_begin) {
+    r = decode_assemble(c, st, w, w.ans_type, ns, capsules, counts, sample_duration_us, scans_per_stream, sp, nullptr);
+  } else {
+    for (uint32_t t = 0; t < 6 && r == RPL_RESULT_OK; ++t) {
+      const uint32_t b = w.list_begin[t], e = w.list_begin[t + 1];
+      if (b == e) continue;
+      const ListLaunch list{{w.lists + b, (uint32_t)w.framed_stride}, e - b};
+      r = decode_assemble(c, st, w, RPL_ANS_MEASUREMENT + t, ns, capsules, counts, sample_duration_us,
+                          scans_per_stream, sp, &list);
+    }
+  }
+  if (r != RPL_RESULT_OK) return r;
   return enqueue_scan(c, l, w.nodes, w.scan_len, ns * w.max_scans, w.max_nodes, params, nullptr, ranges, intens, beams,
                       inc, nullptr, nullptr, st, reinterpret_cast<const uint2*>(w.views),
                       (unsigned long long)ns * w.stride_nodes, LidarTable{w.lidars, w.max_scans, w.lidar_modes});
@@ -1570,6 +1630,12 @@ LidarTable lidar_table(const rpl_capsule_stream* cs, bool per_stream, uint32_t s
   return LidarTable{cs->lidars + s0, cs->max_scans, cs->lidar_modes};
 }
 
+// a capsule answer type's decoder runs in the session's pushes (a mixed session's: any stream's)
+bool decodes_capsules(const rpl_capsule_stream* cs) {
+  if (cs->types.empty()) return cs->ans_type != RPL_ANS_MEASUREMENT;
+  return std::any_of(cs->types.begin(), cs->types.end(), [](uint32_t t) { return t != RPL_ANS_MEASUREMENT; });
+}
+
 bool capsule_stream_args_ok(rpl_capsule_stream* cs, const uint8_t* capsules, const uint32_t* capsule_counts,
                             uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
                             float* intensities, uint32_t* beam_counts, uint32_t* scans_per_stream) {
@@ -1580,7 +1646,7 @@ bool capsule_stream_args_ok(rpl_capsule_stream* cs, const uint8_t* capsules, con
   }
   if ((params->flags & RPL_FLAG_PER_STREAM) != 0) {  // every stream's sample duration comes from the table
     if (!lidars_ok(cs)) return false;
-  } else if (cs->ans_type != RPL_ANS_MEASUREMENT && !sample_duration_ok(c, sample_duration_us)) {
+  } else if (decodes_capsules(cs) && !sample_duration_ok(c, sample_duration_us)) {
     // (the standard decoder takes no sample duration: it tests no jump between capsules)
     return false;
   }
@@ -1607,16 +1673,84 @@ rpl::StreamMsgHeader msg_header(const char* frame_id, size_t len, float range_ma
   return h;
 }
 
-// a session of answer type ans_type (the caller has checked it) whose pushes take, per stream, at most stride_in framed
-// capsules, or with `bytes` at most stride_in bytes of the serial stream (a capsule answer type's are framed first)
-rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, bool bytes, uint32_t n_streams, uint32_t stride_in,
-                         uint32_t max_nodes, uint32_t max_scans, rpl_capsule_stream** out) {
+// a mixed byte session's answer types: each chunking's lists and directory, built from t and uploaded (synchronously:
+// no device call of the session may be in flight)
+rpl_result set_types(rpl_capsule_stream* cs, std::vector<uint32_t> t) {
+  rpl_ctx* c = cs->c;
+  std::vector<uint32_t> lists[2];
+  std::vector<uint32_t> begin[2];
+  for (int k = 0; k < 2; ++k) {
+    const uint32_t chunk = k ? cs->chunk_dev : cs->chunk_host;
+    lists[k].reserve(cs->n_streams);
+    for (uint32_t s0 = 0; s0 < cs->n_streams; s0 += chunk) {
+      const uint32_t ns = std::min(chunk, cs->n_streams - s0);
+      for (uint32_t y = 0; y < 6; ++y) {
+        begin[k].push_back((uint32_t)lists[k].size() - s0);
+        for (uint32_t i = 0; i < ns; ++i)
+          if (t[s0 + i] == RPL_ANS_MEASUREMENT + y) lists[k].push_back(i);
+      }
+      begin[k].push_back(ns);
+    }
+  }
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  cudaStream_t st = c->lane[0].stream;
+  for (int k = 0; k < 2; ++k)
+    RPL_CUDA(c, cudaMemcpyAsync(cs->lists[k], lists[k].data(), lists[k].size() * 4, cudaMemcpyHostToDevice, st),
+             RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);
+  for (int k = 0; k < 2; ++k) cs->list_begin[k] = std::move(begin[k]);
+  cs->types = std::move(t);
+  return RPL_RESULT_OK;
+}
+
+// The per-stream regions of a session of answer type ans_type whose pushes take at most stride_in framed capsules, or
+// with `bytes` at most stride_in bytes of the serial stream: capsule slots and the nodes one push may complete
+struct StreamSizes {
+  unsigned long long stride_capsules, new_nodes;
+};
+StreamSizes stream_sizes(uint32_t ans_type, bool bytes, uint32_t stride_in) {
   const bool normal = ans_type == RPL_ANS_MEASUREMENT, framing = bytes && !normal;
   const uint32_t cap_bytes = normal ? 1u : rpl_capsule_bytes(ans_type);
   // a byte push completes at most `frames` frames with the up to cap_bytes - 1 bytes held before it, each behind at most
   // one all-zero capsule (none for HQ, whose skipped bytes are no loss)
   const unsigned long long frames = framing ? ((unsigned long long)stride_in + cap_bytes - 1) / cap_bytes : stride_in;
-  const uint32_t stride_capsules = framing ? (uint32_t)(ans_type == 0x83 ? frames : 2 * frames) : stride_in;
+  const unsigned long long stride_capsules = framing ? (ans_type == 0x83 ? frames : 2 * frames) : stride_in;
+  // 0x81: a push of n bytes completes up to (n + 4) / 5 records with the up to 4 bytes held before it; rounded up to
+  // even, as every capsule format's node count is, so that every region stays 16-byte aligned
+  const unsigned long long new_nodes = normal ? ((stride_capsules + 4) / 5 + 1) & ~1ull
+                                              : (unsigned long long)rpl_capsule_nodes(ans_type) * frames;
+  return StreamSizes{stride_capsules, new_nodes};
+}
+
+// a session of answer type ans_type (the caller has checked it) whose pushes take, per stream, at most stride_in framed
+// capsules, or with `bytes` at most stride_in bytes of the serial stream (a capsule answer type's are framed first).
+// types (a mixed byte session, ans_type 0 and `bytes`): each stream's answer type, every region sized for the largest
+// any of the six types needs
+rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, bool bytes, uint32_t n_streams, uint32_t stride_in,
+                         uint32_t max_nodes, uint32_t max_scans, rpl_capsule_stream** out,
+                         const uint32_t* types = nullptr) {
+  const bool normal = ans_type == RPL_ANS_MEASUREMENT, framing = bytes && !normal;
+  const uint32_t cap_bytes = normal || types ? 1u : rpl_capsule_bytes(ans_type);
+  StreamSizes z{0, 0};
+  unsigned long long framed_stride = 0;
+  if (!types) {
+    z = stream_sizes(ans_type, bytes, stride_in);
+    framed_stride = framing ? z.stride_capsules * cap_bytes : 0;
+  } else {
+    for (uint32_t t = RPL_ANS_MEASUREMENT; t <= 0x86u; ++t) {
+      const StreamSizes y = stream_sizes(t, true, stride_in);
+      z.new_nodes = std::max(z.new_nodes, y.new_nodes);
+      if (t == RPL_ANS_MEASUREMENT) continue;  // its decoder reads the pushed bytes: no capsule slots
+      z.stride_capsules = std::max(z.stride_capsules, y.stride_capsules);
+      framed_stride = std::max(framed_stride, y.stride_capsules * rpl_capsule_bytes(t));
+    }
+    framed_stride = (framed_stride + 15) & ~15ull;  // every stream's capsules 16-byte aligned
+  }
+  if (types && framed_stride > 0xFFFFFFFFull) {  // StreamList::capsule_stride
+    c->err = "stride_bytes too large: a stream's framed capsules must stay below 2^32 bytes";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  const uint32_t stride_capsules = (uint32_t)z.stride_capsules;
   if (n_streams == 0 || stride_capsules == 0 || max_scans == 0 || max_nodes == 0 || max_nodes > rpl::kSmallMaxNodes ||
       (max_nodes & 1u)) {
     c->err = bytes ? "need n_streams > 0, stride_bytes > 0, max_scans > 0 and an even max_nodes in [2, 8192]"
@@ -1627,13 +1761,11 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, bool bytes, uint32_t n_s
     c->err = "the context's max_scans is smaller than max_scans of one stream";
     return RPL_RESULT_INVALID_DATA;
   }
-  // 0x81: a push of n bytes completes up to (n + 4) / 5 records with the up to 4 bytes held before it; rounded up to
-  // even, as every capsule format's node count is, so that every region stays 16-byte aligned
-  const unsigned long long new_nodes = normal ? (((unsigned long long)stride_capsules + 4) / 5 + 1) & ~1ull
-                                              : (unsigned long long)rpl_capsule_nodes(ans_type) * frames;
+  const unsigned long long new_nodes = z.new_nodes;
   const unsigned long long stride_nodes = (unsigned long long)max_nodes + new_nodes;
   if (stride_nodes * n_streams > 0xFFFFFFFFull) {
-    c->err = normal ? "n_streams * (max_nodes + (stride_bytes + 4) / 5 rounded up to even) must stay below 2^32 "
+    c->err = types ? "n_streams * (max_nodes + 96 * ceil(stride_bytes / 132)) must stay below 2^32 (32-bit scan views)"
+           : normal ? "n_streams * (max_nodes + (stride_bytes + 4) / 5 rounded up to even) must stay below 2^32 "
                       "(32-bit scan views)"
                     : framing ? "n_streams * (max_nodes + nodes per capsule * ceil(stride_bytes / capsule bytes)) must "
                                 "stay below 2^32 (32-bit scan views)"
@@ -1647,6 +1779,7 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, bool bytes, uint32_t n_s
   cs->c = c;
   cs->ans_type = ans_type;
   cs->cap_bytes = cap_bytes;
+  cs->framed_stride = (size_t)framed_stride;
   cs->n_streams = n_streams;
   cs->stride_capsules = stride_capsules;
   cs->max_nodes = max_nodes;
@@ -1675,8 +1808,8 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, bool bytes, uint32_t n_s
   if (!cuda_ok(c, dev_alloc(&cs->held_rx, n), "cudaMalloc") ||
       !cuda_ok(c, cudaMemset(cs->held_rx, 0, n * 8), "cudaMemset"))
     return fail(oom);
-  if (normal && !cuda_ok(c, dev_alloc(&cs->scan_ends, n * (size_t)new_nodes), "cudaMalloc")) return fail(oom);
-  if (ans_type == 0x85 && (!cuda_ok(c, dev_alloc(&cs->starts, n * cs->starts_stride), "cudaMalloc") ||
+  if ((normal || types) && !cuda_ok(c, dev_alloc(&cs->scan_ends, n * (size_t)new_nodes), "cudaMalloc")) return fail(oom);
+  if ((ans_type == 0x85 || types) && (!cuda_ok(c, dev_alloc(&cs->starts, n * cs->starts_stride), "cudaMalloc") ||
                            !cuda_ok(c, dev_alloc(&cs->start_counts, n), "cudaMalloc")))
     return fail(oom);
   if (!normal && (!cuda_ok(c, dev_alloc(&cs->status, ncap), "cudaMalloc") ||
@@ -1684,7 +1817,7 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, bool bytes, uint32_t n_s
     return fail(oom);
   if (framing && (!cuda_ok(c, dev_alloc(&cs->framer, n * rpl::kFramerWords), "cudaMalloc") ||
                   !cuda_ok(c, cudaMemset(cs->framer, 0, n * rpl::kFramerWords * 4), "cudaMemset") ||
-                  !cuda_ok(c, dev_alloc(&cs->framed, ncap * cap_bytes), "cudaMalloc") ||
+                  !cuda_ok(c, dev_alloc(&cs->framed, n * framed_stride), "cudaMalloc") ||
                   !cuda_ok(c, dev_alloc(&cs->framed_counts, n), "cudaMalloc") ||
                   !cuda_ok(c, dev_alloc(&cs->framed_rx, ncap), "cudaMalloc")))
     return fail(oom);
@@ -1707,6 +1840,12 @@ rpl_result stream_create(rpl_ctx* c, uint32_t ans_type, bool bytes, uint32_t n_s
       !cuda_ok(c, cudaEventCreateWithFlags(&cs->done, cudaEventDisableTiming), "cudaEventCreate") ||
       !cuda_ok(c, cudaDeviceSynchronize(), "cudaDeviceSynchronize"))  // the zeroed state is in place before any push
     return fail(oom);
+  if (types) {
+    for (int k = 0; k < 2; ++k)
+      if (!cuda_ok(c, dev_alloc(&cs->lists[k], n), "cudaMalloc")) return fail(oom);
+    if (const rpl_result r = set_types(cs, std::vector<uint32_t>(types, types + n_streams)); r != RPL_RESULT_OK)
+      return fail(r);
+  }
   *out = cs;
   return RPL_RESULT_OK;
 }
@@ -1778,7 +1917,7 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
         chunk_sp.rx += (size_t)s0 * sp->stride_chunks;
         chunk_sp.scan_ts += so;
       }
-      r = capsule_stream_chunk(c, c->lane[0], st, session_chunk(cs, s0, per_stream),
+      r = capsule_stream_chunk(c, c->lane[0], st, session_chunk(cs, s0, per_stream, true),
                                std::min(chunk, cs->n_streams - s0), in + s0 * cs->in_stream, counts + s0,
                                sample_duration_us, params, ranges + s0 * row, intensities + s0 * row, beam_counts + so,
                                angle_increment ? angle_increment + so : nullptr, scans_per_stream + s0,
@@ -1794,7 +1933,8 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
     for (int i = 0; i < kLanes; ++i) RPL_CUDA(c, cudaStreamWaitEvent(c->lane[i].stream, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
     const HostWire h{in, counts, cs->in_stream, sample_duration_us, cs->max_nodes, cs->max_scans, params, ranges,
                      intensities, angle_increment, beam_counts, scans_per_stream, sp, sp ? sp->stride_chunks : 0u};
-    r = push_host(c, h, cs->n_streams, chunk, [&](Carve&, uint32_t s0) { return session_chunk(cs, s0, per_stream); });
+    r = push_host(c, h, cs->n_streams, chunk,
+                  [&](Carve&, uint32_t s0) { return session_chunk(cs, s0, per_stream, false); });
   }
   cs->parity ^= 1u;
   cs->prev_stamped = sp != nullptr;
@@ -2532,6 +2672,8 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   cudaFree(cs->framed);
   cudaFree(cs->framed_counts);
   cudaFree(cs->framed_rx);
+  cudaFree(cs->lists[0]);
+  cudaFree(cs->lists[1]);
   cudaFree(cs->slot_begin);
   cudaFree(cs->slot_end);
   cudaFree(cs->msg_hdr);
@@ -2613,7 +2755,6 @@ rpl_result rpl_capsule_stream_state(rpl_capsule_stream* cs, uint32_t* open_nodes
                                     uint32_t* held_bytes) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
   rpl_ctx* c = cs->c;
-  const bool normal = cs->ans_type == RPL_ANS_MEASUREMENT;
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
   RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);
   if (open_nodes)
@@ -2626,13 +2767,14 @@ rpl_result rpl_capsule_stream_state(rpl_capsule_stream* cs, uint32_t* open_nodes
   }
   // the held records: HQ's stays zero; 0x81's holds the byte machine's state, 0..4 bytes held
   std::vector<uint32_t> h;
-  if (held_capsule || (held_bytes && normal)) {
+  if (held_capsule || held_bytes) {
     h.resize((size_t)cs->n_streams * rpl::kHeldWords);
     RPL_CUDA(c, cudaMemcpy(h.data(), cs->held, h.size() * 4, cudaMemcpyDeviceToHost), RPL_RESULT_OPERATION_FAIL);
   }
   for (uint32_t s = 0; s < cs->n_streams; ++s) {
+    const bool normal = (cs->types.empty() ? cs->ans_type : cs->types[s]) == RPL_ANS_MEASUREMENT;
     const uint32_t ok = h.empty() ? 0u : h[(size_t)s * rpl::kHeldWords + rpl::kHeldOk];
-    const uint32_t* f = fr.empty() ? nullptr : fr.data() + (size_t)s * rpl::kFramerWords;
+    const uint32_t* f = fr.empty() || normal ? nullptr : fr.data() + (size_t)s * rpl::kFramerWords;
     // skipped bytes waiting to be reported: the next frame releases nothing (the SDK cleared its ready flag)
     if (held_capsule) held_capsule[s] = normal || (f && f[rpl::kFramerLost]) ? 0u : ok;
     if (held_bytes) held_bytes[s] = normal ? ok : f ? f[rpl::kFramerPos] : 0u;
@@ -2675,6 +2817,57 @@ rpl_result rpl_capsule_stream_create_bytes(rpl_ctx* c, uint32_t ans_type, uint32
     return RPL_RESULT_INVALID_DATA;
   }
   return stream_create(c, ans_type, true, n_streams, stride_bytes, max_nodes, max_scans, out);
+}
+
+// ---- mixed byte sessions: an answer type per stream, switched between pushes ----
+namespace {
+bool answer_types_ok(rpl_ctx* c, const uint32_t* ans_types, uint32_t n_streams, const uint8_t* stream_mask) {
+  if (!ans_types) {
+    c->err = "null ans_types";
+    return false;
+  }
+  for (uint32_t s = 0; s < n_streams; ++s)
+    if ((!stream_mask || stream_mask[s]) && (ans_types[s] < RPL_ANS_MEASUREMENT || ans_types[s] > 0x86u)) {
+      c->err = "a byte session takes the measurement answer types 0x81..0x86";
+      return false;
+    }
+  return true;
+}
+}  // namespace
+
+rpl_result rpl_capsule_stream_create_bytes_mixed(rpl_ctx* c, const uint32_t* ans_types, uint32_t n_streams,
+                                                 uint32_t stride_bytes, uint32_t max_nodes, uint32_t max_scans,
+                                                 rpl_capsule_stream** out) {
+  if (!c || !out) return RPL_RESULT_INVALID_DATA;
+  *out = nullptr;
+  if (!answer_types_ok(c, ans_types, n_streams, nullptr)) return RPL_RESULT_INVALID_DATA;
+  return stream_create(c, 0, true, n_streams, stride_bytes, max_nodes, max_scans, out, ans_types);
+}
+
+rpl_result rpl_capsule_stream_set_answer_types(rpl_capsule_stream* cs, const uint32_t* ans_types,
+                                               const uint8_t* stream_mask) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (cs->types.empty()) {
+    c->err = "rpl_capsule_stream_set_answer_types needs a session made by rpl_capsule_stream_create_bytes_mixed";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  if (!answer_types_ok(c, ans_types, cs->n_streams, stream_mask)) return RPL_RESULT_INVALID_DATA;
+  // the streams whose type changes start over as the SDK's startScan leaves them: holder reset, unpacker enabled
+  std::vector<uint8_t> changed(cs->n_streams, 0);
+  std::vector<uint32_t> t = cs->types;
+  bool any = false;
+  for (uint32_t s = 0; s < cs->n_streams; ++s)
+    if ((!stream_mask || stream_mask[s]) && ans_types[s] != t[s]) {
+      changed[s] = 1;
+      t[s] = ans_types[s];
+      any = true;
+    }
+  if (!any) return RPL_RESULT_OK;
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);  // a push may still read the lists
+  if (const rpl_result r = rpl_capsule_stream_reset(cs, changed.data()); r != RPL_RESULT_OK) return r;
+  return set_types(cs, std::move(t));
 }
 
 rpl_result rpl_capsule_stream_push_bytes(rpl_capsule_stream* cs, const uint8_t* bytes, const uint32_t* byte_counts,

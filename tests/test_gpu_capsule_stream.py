@@ -379,7 +379,8 @@ def test_first_push_equals_the_stateless_path(R, oracle, ans, params):
 
 def test_two_formats_push_dev_and_many_streams(R, oracle):
     """an ultra and an ultra-dense session pushed alternately with push_dev on a caller's torch stream, on one context;
-    more streams than num_sms * 4 and than one chunk of the context's max_scans; both equal their host pushes"""
+    more streams than one chunk of the context's max_scans, so each push runs in several chunks; both equal their host
+    pushes (more streams than CTAs per launch: tests/test_gpu_fleet_scale.py)"""
     import torch
 
     dev = torch.device("cuda", 0)

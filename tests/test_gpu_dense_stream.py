@@ -285,7 +285,8 @@ def test_reset_mask(R, oracle):
 
 def test_two_sessions_push_dev_and_many_streams(R, oracle):
     """two sessions pushed alternately on one context; push_dev on a caller's non-default torch stream equals push;
-    more streams than num_sms * 4 and more than one host chunk"""
+    more streams than one chunk, so each push runs in several chunks (more streams than CTAs per launch:
+    tests/test_gpu_fleet_scale.py)"""
     import torch
 
     n_caps, max_nodes, max_scans = 240, 4096, 8

@@ -303,8 +303,8 @@ def test_first_push_equals_the_stateless_path(R, oracle, params):
 
 
 def test_push_dev_on_a_caller_stream_and_many_streams(R, oracle):
-    """push_dev on a caller's torch stream; more streams than the decoder's grid (num_sms * 8) and than one chunk of
-    the context's max_scans; equal to the host pushes"""
+    """push_dev on a caller's torch stream; more streams than one chunk of the context's max_scans, so each push runs
+    in several chunks; equal to the host pushes (more streams than CTAs per launch: tests/test_gpu_fleet_scale.py)"""
     import torch
 
     dev = torch.device("cuda", 0)

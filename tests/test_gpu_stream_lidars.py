@@ -72,14 +72,15 @@ def split(rng, streams, rev):
 class Drive:
     """one session of any kind, pushed host or device, stamped or not; outputs come back as host arrays"""
 
-    def __init__(self, R, ctx, kind, ans, n, stride, max_nodes=MAX_NODES):
+    def __init__(self, R, ctx, kind, ans, n, stride, max_nodes=MAX_NODES, max_scans=MS):
         self.R, self.kind, self.ans, self.n, self.stride, self.max_nodes = R, kind, ans, n, stride, max_nodes
+        self.ms = max_scans
         if kind == "normal":
-            self.sess = R.NormalStreamSession(ctx, n, stride, max_nodes, MS)
+            self.sess = R.NormalStreamSession(ctx, n, stride, max_nodes, max_scans)
         elif kind == "bytes":
-            self.sess = R.CapsuleByteStreamSession(ctx, ans, n, stride, max_nodes, MS)
+            self.sess = R.CapsuleByteStreamSession(ctx, ans, n, stride, max_nodes, max_scans)
         else:
-            self.sess = R.CapsuleStreamSession(ctx, ans, n, stride, max_nodes, MS)
+            self.sess = R.CapsuleStreamSession(ctx, ans, n, stride, max_nodes, max_scans)
 
     def push(self, units, params, flavour, timing=None, rx=None):
         """units: per stream the capsules (bytes); timing: R.Timing or None; rx: the stamped push's receive times"""
@@ -102,7 +103,7 @@ class Drive:
         import torch
 
         dev = torch.device("cuda", 0)
-        NS = n * MS
+        NS = n * self.ms
         d_buf, d_cnt = torch.from_numpy(buf).to(dev), torch.from_numpy(cnt.view(np.int32)).to(dev)
         r = torch.full((NS, self.max_nodes), -1.0, device=dev)
         it = torch.full((NS, self.max_nodes), -1.0, device=dev)
@@ -129,16 +130,16 @@ class Drive:
         self.sess.close()
 
 
-def slots(out, s):
-    """stream s's part of a push's outputs"""
+def slots(out, s, ms=MS):
+    """stream s's part of a push's outputs (ms: the session's max_scans)"""
     k = int(out["scans_per_stream"][s])
     res = [k]
-    for j in range(min(k, MS)):
-        i = s * MS + j
+    for j in range(min(k, ms)):
+        i = s * ms + j
         m = int(out["beam_counts"][i])
         res.append((m, bits(out["ranges"][i, :m]), bits(out["intensities"][i, :m]), bits(out["angle_increment"][i:i + 1])))
     if out["scan_begin_ts_us"] is not None:
-        res.append(out["scan_begin_ts_us"][s * MS:(s + 1) * MS].tolist())
+        res.append(out["scan_begin_ts_us"][s * ms:(s + 1) * ms].tolist())
     return res
 
 

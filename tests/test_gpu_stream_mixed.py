@@ -42,6 +42,7 @@ class MixedDrive(Drive):
 
     def __init__(self, R, ctx, types, stride):
         self.R, self.kind, self.ans, self.n, self.stride, self.max_nodes = R, "bytes", 0, len(types), stride, MAX_NODES
+        self.ms = MS
         self.sess = R.MixedByteStreamSession(ctx, types, stride, MAX_NODES, MS)
 
 

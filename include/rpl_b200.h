@@ -781,6 +781,62 @@ rpl_result rpl_capsule_stream_cloud_msgs(rpl_capsule_stream* s, const rpl_cloud_
                                          uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
                                          uint64_t* total_bytes);
 
+/* Messages from the push: one call that pushes `in` and returns the LaserScan messages of the scans it published,
+ * written by the push's own scan kernels straight into the packed messages.  No padded
+ * [n_streams * max_scans][max_nodes] row is allocated, computed into or copied.
+ *   in:      one descriptor for every push flavour; the session's kind decides how data is read (framed: capsules
+ *            [n_streams][stride_capsules][capsule bytes]; byte session: bytes [n_streams][stride_bytes]).  rx_us NULL:
+ *            an unstamped push with sample_duration_us (rpl_capsule_stream_push / _push_bytes).  Else a stamped push
+ *            with timing: capsule_rx_us (framed, rpl_capsule_stream_push_ts) or chunk_rx_us with chunk_bytes (byte
+ *            session, rpl_capsule_stream_push_bytes_ts).  chunk_bytes must be 0 on a framed session and on an
+ *            unstamped push.
+ *   Definition: with two sessions of the same history, A pushed with the entry point of in's kind and then
+ *            rpl_capsule_stream_laserscan_msgs[_dev] with params and clock_offset_ns, B with this call: for every slot
+ *            i = s * max_scans + k, scans_per_stream and msg_sizes are equal, message i's msg_sizes[i] bytes are equal,
+ *            and every later call returns on B what it returns on A (this call sets the last push as a push does).  A
+ *            call that fails its checks leaves the session as the push it stands for would.
+ *   Packing: the bound of slot i is rpl_laserscan_cdr_size(strlen(frame_id of s), n_i) rounded up to 16 for a
+ *            published slot (k < min(scans_per_stream[s], max_scans); n_i its scan's node count, the node_counts[i]
+ *            rpl_capsule_stream_nodes reports for the push), 0 for an unused one.  msg_offsets is the exclusive scan
+ *            of the bounds in slot order and *total_bytes their sum: every message starts 16-byte aligned, and the
+ *            bytes between a message's end and the next offset (8 per unmeasured node) are unspecified.  A message's
+ *            exact size is only known once its scan kernel has run; its bound is known before, when each chunk's
+ *            directory places its slots.
+ *   Capacity: message i is written iff msg_offsets[i] + bound_i <= capacity, else its size is 0; the push itself is
+ *            done either way.  Unlike laserscan_msgs this is not all or nothing: a device push's total is not known
+ *            on the host before its chunks run.  The host form returns RPL_RESULT_INSUFFICIENT_MEMORY when
+ *            *total_bytes > capacity, the _dev form reports it through *total_bytes only; in both cases
+ *            rpl_capsule_stream_laserscan_msgs on the same push returns every message.  Nothing at or past
+ *            msgs + min(*total_bytes, capacity) is written.
+ *   Errors:  a null descriptor, data, counts, params, output or scans_per_stream; a stamped push with bad timing;
+ *            misaligned device outputs; chunk_bytes where it does not belong; and the checks of the matching push
+ *            and message calls: RPL_RESULT_INVALID_DATA.
+ *   _dev:    data, counts, rx_us and the outputs are device memory (msgs 16-byte aligned, msg_offsets and total_bytes
+ *            8-byte, msg_sizes and scans_per_stream 4-byte aligned); the descriptor and timing are host memory.
+ *            Asynchronous on `stream` (NULL = the context's stream), ordered with the session's other calls as a
+ *            device push is.
+ *   host:    synchronous, host buffers.  Only the tables and the messages' stretch of msgs cross the link.
+ *   Cost:    the session keeps, from the first call, 24 bytes per slot of device tables; the host form stages one
+ *            chunk's bounded messages per lane instead of its padded rows. */
+typedef struct rpl_push_input {
+  const uint8_t* data;          /* framed session: capsules; byte session: bytes -- the session's kind decides */
+  const uint32_t* counts;       /* [n_streams] capsules or bytes (the rules of the matching push) */
+  const uint64_t* rx_us;        /* NULL: an unstamped push.  Else capsule_rx_us (framed) or chunk_rx_us (bytes), laid
+                                   out as for push_ts / push_bytes_ts */
+  const rpl_timing* timing;     /* stamped pushes (may be NULL with RPL_FLAG_PER_STREAM, as for push_ts) */
+  uint32_t sample_duration_us;  /* unstamped pushes, as rpl_capsule_stream_push */
+  uint32_t chunk_bytes;         /* stamped byte pushes, as rpl_capsule_stream_push_bytes_ts */
+} rpl_push_input;
+rpl_result rpl_capsule_stream_push_laserscan_msgs(rpl_capsule_stream* s, const rpl_push_input* in,
+                                                  const rpl_scan_params* params, int64_t clock_offset_ns, uint8_t* msgs,
+                                                  uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
+                                                  uint64_t* total_bytes, uint32_t* scans_per_stream);
+rpl_result rpl_capsule_stream_push_laserscan_msgs_dev(rpl_capsule_stream* s, const rpl_push_input* in,
+                                                      const rpl_scan_params* params, int64_t clock_offset_ns,
+                                                      uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,
+                                                      uint32_t* msg_sizes, uint64_t* total_bytes,
+                                                      uint32_t* scans_per_stream, void* stream);
+
 /* Per-stream lidar settings: each stream of a session is one lidar, the reference's one RPlidarNode, with its own
  * intensity protocol (RealLidarDriver::is_new_type(), src/lidar_driver_wrapper.cpp:303-305), scan_processing and
  * inverted parameters (src/rplidar_node.cpp:270, 278-279) and SlamtecLidarTimingDesc (which depends on the model, the

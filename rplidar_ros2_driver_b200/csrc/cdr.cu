@@ -19,6 +19,7 @@
 // follows the OMG CDR rules above and oracle/cdr_oracle.py restates it independently in numpy.
 #include "cdr_args.h"
 #include "rpl_device.cuh"
+#include "scan_args.h"
 
 namespace rpl {
 
@@ -164,10 +165,39 @@ __device__ __forceinline__ double msg_period(unsigned long long b, unsigned long
   return (double)(long long)((e - b) * 1000ull) / 1e9;
 }
 
-// the header words of the stream's settings, stamp words left to the caller (no two threads write one word)
+// the header words of the stream's settings, stamp words left to the caller (no two threads write one word); T threads
+template <int T = CT>
 __device__ __forceinline__ void put_header(uint8_t* msg, const StreamMsgHeader& h) {
-  for (uint32_t w = threadIdx.x; w < h.bytes / 4; w += CT)
+  for (uint32_t w = threadIdx.x; w < h.bytes / 4; w += T)
     if (w != 1 && w != 2) put32(msg + 4 * w, h.w[w]);
+}
+
+// LaserScan message i's fixed part -- header, stamp, the 7 floats, both sequence lengths -- for n beams, by the T threads
+// of a CTA; P = h.bytes + 32, where the ranges start
+template <int T>
+__device__ __forceinline__ void put_laserscan_fixed(const MsgWriteArgs& a, uint32_t i, uint32_t n, const StreamMsgHeader& h,
+                                                    uint32_t P, uint8_t* msg) {
+  put_header<T>(msg, h);
+  if (threadIdx.x == 0) {
+    const unsigned long long b = a.begin_us ? a.begin_us[i] : 0ull, e = a.end_us ? a.end_us[i] : 0ull;
+    uint32_t sec, nsec;
+    msg_stamp(b, a.clock_offset_ns, &sec, &nsec);
+    const double d = msg_period(b, e);
+    const bool mode_a = a.lidars ? a.lidars[i / a.max_scans].mode_a != 0 : a.mode_a != 0;
+    const double denom = mode_a ? (double)n : (double)(n > 1 ? n - 1 : 1);
+    put32(msg + 4, sec);
+    put32(msg + 8, nsec);
+    uint8_t* f = msg + h.bytes;
+    put32(f + 0, __float_as_uint(0.0f));                             // angle_min
+    put32(f + 4, __float_as_uint((float)(2.0 * 3.14159265358979323846)));  // angle_max
+    put32(f + 8, __float_as_uint(a.angle_increment[i]));
+    put32(f + 12, __float_as_uint(__double2float_rn(d / denom)));    // time_increment
+    put32(f + 16, __float_as_uint(__double2float_rn(d)));            // scan_time
+    put32(f + 20, __float_as_uint(0.15f));                           // range_min
+    put32(f + 24, __float_as_uint(h.range_max));
+    put32(f + 28, n);
+    put32(msg + P + 4 * (size_t)n, n);  // intensities count
+  }
 }
 
 __global__ void __launch_bounds__(CT) laserscan_msgs_kernel(MsgWriteArgs a) {
@@ -178,29 +208,7 @@ __global__ void __launch_bounds__(CT) laserscan_msgs_kernel(MsgWriteArgs a) {
   const StreamMsgHeader& h = a.hdr[i / a.max_scans];
   const uint32_t P = h.bytes + 32;  // the 7 floats and the ranges count follow the header
   uint8_t* msg = a.out + (a.offsets[i] - a.out_base);
-  if (blockIdx.x == 0) {
-    put_header(msg, h);
-    if (threadIdx.x == 0) {
-      const unsigned long long b = a.begin_us ? a.begin_us[i] : 0ull, e = a.end_us ? a.end_us[i] : 0ull;
-      uint32_t sec, nsec;
-      msg_stamp(b, a.clock_offset_ns, &sec, &nsec);
-      const double d = msg_period(b, e);
-      const bool mode_a = a.lidars ? a.lidars[i / a.max_scans].mode_a != 0 : a.mode_a != 0;
-      const double denom = mode_a ? (double)n : (double)(n > 1 ? n - 1 : 1);
-      put32(msg + 4, sec);
-      put32(msg + 8, nsec);
-      uint8_t* f = msg + h.bytes;
-      put32(f + 0, __float_as_uint(0.0f));                             // angle_min
-      put32(f + 4, __float_as_uint((float)(2.0 * 3.14159265358979323846)));  // angle_max
-      put32(f + 8, __float_as_uint(a.angle_increment[i]));
-      put32(f + 12, __float_as_uint(__double2float_rn(d / denom)));    // time_increment
-      put32(f + 16, __float_as_uint(__double2float_rn(d)));            // scan_time
-      put32(f + 20, __float_as_uint(0.15f));                           // range_min
-      put32(f + 24, __float_as_uint(h.range_max));
-      put32(f + 28, n);
-      put32(msg + P + 4 * (size_t)n, n);  // intensities count
-    }
-  }
+  if (blockIdx.x == 0) put_laserscan_fixed<CT>(a, i, n, h, P, msg);
   uint32_t* r_out = reinterpret_cast<uint32_t*>(msg + P);
   uint32_t* i_out = r_out + n + 1;
   const uint32_t* r_in = reinterpret_cast<const uint32_t*>(a.ranges + (size_t)i * a.stride);
@@ -220,7 +228,7 @@ __global__ void __launch_bounds__(CT) pointcloud2_msgs_kernel(MsgWriteArgs a, Cl
   const uint32_t P = h.bytes + t.bytes;  // ends with the data length
   uint8_t* msg = a.out + (a.offsets[i] - a.out_base);
   if (blockIdx.x == 0) {
-    put_header(msg, h);
+    put_header<CT>(msg, h);
     for (uint32_t w = threadIdx.x; w < t.bytes / 4; w += CT) {
       const uint32_t v = w == t.at_width ? n : (w == t.at_row_step || w == t.at_data) ? 16u * n : t.w[w];
       put32(msg + h.bytes + 4 * w, v);
@@ -244,7 +252,91 @@ __global__ void __launch_bounds__(CT) pointcloud2_msgs_kernel(MsgWriteArgs a, Cl
   }
 }
 
+// ---- LaserScan messages written by a push ------------------------------------------------------------------------
+// One CTA over the chunk's slots in tiles of MT, as msg_table_kernel, the carry passing from tile to tile and, through
+// *a.carry, from chunk to chunk: the chunks of a push run one after the other (one stream, or the host push's lanes
+// ordered by an event), so each reads the end the one before it wrote.
+__global__ void __launch_bounds__(MT) push_msg_dir_kernel(PushMsgDirArgs a) {
+  __shared__ unsigned long long s_warp[MT / 32];
+  __shared__ unsigned long long s_first, s_fit_end;
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  if (tid == 0) {
+    s_first = a.first ? 0ull : *a.carry;
+    s_fit_end = s_first;
+  }
+  __syncthreads();
+  const unsigned long long first = s_first, rel = a.rebase ? first : 0ull;
+  unsigned long long carry = first;
+  for (uint32_t t0 = 0; t0 < a.n_slots; t0 += MT) {
+    const uint32_t i = t0 + tid;
+    uint32_t bound = 0, hb = 0;
+    if (i < a.n_slots) {
+      const uint32_t s = i / a.max_scans, k = i - s * a.max_scans;
+      hb = a.hdr[s].bytes;
+      if (k < min(a.scans_per_stream[s], a.max_scans)) bound = (msg_bytes(MsgKind::kLaserScan, hb, a.views[i].y) + 15u) & ~15u;
+    }
+    const unsigned long long v = bound;
+    unsigned long long inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned long long u = __shfl_up_sync(0xffffffffu, inc, o);
+      if (lane >= (uint32_t)o) inc += u;
+    }
+    if (lane == 31) s_warp[warp] = inc;
+    __syncthreads();
+    unsigned long long base = 0, tile = 0;
+    for (uint32_t w = 0; w < MT / 32; ++w) {
+      const unsigned long long x = s_warp[w];
+      if (w < warp) base += x;
+      tile += x;
+    }
+    const unsigned long long off = carry + base + inc - v;
+    if (i < a.n_slots) {
+      const bool fits = bound != 0 && off + bound <= a.capacity;
+      a.offsets[i] = off;
+      a.place[i] = fits ? off - rel + hb + 32u : kOutSkip;
+      if (fits) atomicMax(&s_fit_end, off + bound);
+    }
+    carry += tile;
+    __syncthreads();  // s_warp is rewritten by the next tile
+  }
+  if (tid == 0) {
+    *a.carry = carry;
+    if (a.extent) {
+      a.extent[0] = first;
+      a.extent[1] = s_fit_end;
+      a.extent[2] = carry;
+    }
+    if (a.total) *a.total = carry;
+  }
+}
+
+// one CTA of 32 threads per slot: the arrays are the scan kernels'
+__global__ void __launch_bounds__(32) laserscan_placed_kernel(MsgWriteArgs a, const unsigned long long* place,
+                                                              uint32_t* sizes) {
+  const uint32_t i = blockIdx.x;
+  const unsigned long long pl = place[i];
+  const uint32_t n = (pl & kOutSkip) ? 0u : a.counts[i];
+  const StreamMsgHeader& h = a.hdr[i / a.max_scans];
+  if (threadIdx.x == 0) sizes[i] = n ? msg_bytes(MsgKind::kLaserScan, h.bytes, n) : 0u;
+  if (n == 0) return;
+  const uint32_t P = h.bytes + 32;
+  put_laserscan_fixed<32>(a, i, n, h, P, a.out + (pl - P));
+}
+
 }  // namespace
+
+cudaError_t launch_push_msg_dir(const PushMsgDirArgs& a, cudaStream_t stream) {
+  push_msg_dir_kernel<<<1, MT, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_laserscan_placed(const MsgWriteArgs& a, const unsigned long long* place, uint32_t* sizes,
+                                    cudaStream_t stream) {
+  if (a.n == 0) return cudaSuccess;
+  laserscan_placed_kernel<<<a.n, 32, 0, stream>>>(a, place, sizes);
+  return cudaGetLastError();
+}
 
 cudaError_t launch_msg_table(const MsgTableArgs& a, cudaStream_t stream) {
   if (a.n_slots == 0) return cudaSuccess;

@@ -100,6 +100,36 @@ struct MsgWriteArgs {
 
 cudaError_t launch_msg_table(const MsgTableArgs& a, cudaStream_t stream);
 cudaError_t launch_laserscan_msgs(const MsgWriteArgs& a, uint32_t max_beams, cudaStream_t stream);
+
+// ---- LaserScan messages written by a push (rpl_capsule_stream_push_laserscan_msgs*) ---------------------------------
+// The directory of one chunk of the push, one CTA, every pointer at the chunk's first slot (stream).  A published slot
+// (k < min(scans_per_stream[s], max_scans)) is bounded by its message at the view's node count, rounded up to 16; an
+// unused slot by 0.  offsets[i] = *carry (the previous chunk's end; 0 for the push's first chunk) + the exclusive scan
+// of the chunk's bounds; the chunk's end goes back to *carry.  A slot whose bounded message ends past `capacity` gets
+// no message.
+struct PushMsgDirArgs {
+  const uint2* views;               // [n_slots] the chunk's scans
+  const uint32_t* scans_per_stream; // [n_slots / max_scans]
+  const StreamMsgHeader* hdr;       // [n_slots / max_scans]
+  uint32_t n_slots, max_scans;
+  uint32_t first;                   // != 0: the push's first chunk (the carry is not read)
+  uint32_t rebase;                  // != 0: place[] counts from the chunk's first offset (else from 0)
+  unsigned long long capacity;
+  unsigned long long* carry;        // [1] in / out
+  unsigned long long* offsets;      // [n_slots] out
+  // [n_slots] out, ScanBatchArgs::msg_ranges: where the message's ranges start (message position + header + 32);
+  // kOutSkip for a slot without a message
+  unsigned long long* place;
+  unsigned long long* extent;       // [3] out, nullable: the chunk's first offset, the end of its last message that
+                                    // fits, the end of its bounds
+  unsigned long long* total;        // [1] out, nullable: the end of the chunk's bounds
+};
+cudaError_t launch_push_msg_dir(const PushMsgDirArgs& a, cudaStream_t stream);
+// The fixed part of every placed message of slots [0, a.n) once the scan kernels have written its arrays (a's hdr,
+// begin_us / end_us, counts, angle_increment, lidars at the chunk's first slot; its offsets, sizes, out_base unused):
+// message i at a.out + place[i] - header bytes - 32; sizes[i] its bytes, 0 for no message.
+cudaError_t launch_laserscan_placed(const MsgWriteArgs& a, const unsigned long long* place, uint32_t* sizes,
+                                    cudaStream_t stream);
 cudaError_t launch_pointcloud2_msgs(const MsgWriteArgs& a, const CloudTail& t, uint32_t max_points, cudaStream_t stream);
 
 }  // namespace rpl

@@ -93,7 +93,8 @@ enum class FastKernel { kNone, kSmall, kCluster, kTma, kFast };
 // the kernel-selection rule of every scan entry point, batches and single scans alike
 FastKernel pick_fast(const rpl::ScanBatchArgs& a, uint32_t flags) {
   // FORCE_GENERAL and status-only calls (no LaserScan, no ascended buffer) take the general kernel alone
-  if ((flags & RPL_FLAG_FORCE_GENERAL) != 0 || (!a.ranges && !a.nodes_out && !a.xyzi)) return FastKernel::kNone;
+  if ((flags & RPL_FLAG_FORCE_GENERAL) != 0 || (!a.ranges && !a.nodes_out && !a.xyzi && !a.msg_out))
+    return FastKernel::kNone;
   // revolutions that fit shared memory (what a lidar delivers) have their own kernels
   if (rpl::scan_small_applies(a.stride) && (flags & RPL_FLAG_NO_SMALL) == 0) return FastKernel::kSmall;
   // above that the TMA kernels need every scan base 16-byte aligned, and the PointCloud2 payload exists in the
@@ -195,8 +196,8 @@ rpl_result enqueue_args(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, uint32_t flag
     a.nodes_out = nullptr;
   }
   FastKernel k = pick_fast(a, flags);
-  // per-stream settings are read by the shared-memory kernels and the general kernel only
-  if (a.lidars && k != FastKernel::kSmall) k = FastKernel::kNone;
+  // per-stream settings and placed messages are read by the shared-memory kernels and the general kernel only
+  if ((a.lidars || a.msg_out) && k != FastKernel::kSmall) k = FastKernel::kNone;
   if (k != FastKernel::kNone) {
     RPL_CUDA(c, cudaMemsetAsync(l.fallback_count, 0, sizeof(uint32_t), stream), RPL_RESULT_OPERATION_FAIL);
     const rpl_result r = launch_fast(c, l, a, k, stream, cloud, post_fused, hand_off);
@@ -231,7 +232,8 @@ rpl_result enqueue_scan(rpl_ctx* c, Lane& l, const rpl_node_hq* nodes, const uin
                         uint32_t n_scans, uint32_t stride, const rpl_scan_params* p,
                         rpl_node_hq* nodes_out, float* ranges, float* intens, uint32_t* beams,
                         float* inc, uint32_t* status, uint32_t* path, cudaStream_t stream,
-                        const uint2* views = nullptr, unsigned long long nodes_total = 0, LidarTable lt = {}) {
+                        const uint2* views = nullptr, unsigned long long nodes_total = 0, LidarTable lt = {},
+                        uint8_t* msg_out = nullptr, const unsigned long long* msg_ranges = nullptr) {
   if (n_scans == 0) return RPL_RESULT_OK;
   if (!nodes || !counts || !p) {
     c->err = "null nodes/counts/params";
@@ -270,6 +272,8 @@ rpl_result enqueue_scan(rpl_ctx* c, Lane& l, const rpl_node_hq* nodes, const uin
   a.lidars = lt.at;
   a.lidar_scans = lt.per;
   a.lidar_modes = lt.modes;
+  a.msg_out = msg_out;
+  a.msg_ranges = msg_ranges;
   rpl_result r = scratch_enter(c, l, stream);
   if (r == RPL_RESULT_OK) r = enqueue_args(c, l, a, p->flags, stream);
   return r == RPL_RESULT_OK ? scratch_leave(c, l, stream) : r;
@@ -1265,6 +1269,11 @@ struct rpl_capsule_stream {
   // [n_streams] device, zeroed at create: what every push decoded and lost (rpl_capsule_stream_counters); a stream's
   // record is written by the one CTA of each kernel that serves the stream
   rpl::StreamCounters* counters = nullptr;
+  // message pushes (rpl_capsule_stream_push_laserscan_msgs*), made by the first: the device tables of the push's slots
+  // (PushMsgWork), the host form's pinned read-back of a chunk's extent, and the events that order its chunks
+  unsigned char* push_msg_work = nullptr;
+  unsigned long long* push_msg_extent = nullptr;
+  cudaEvent_t push_msg_extent_ready = nullptr, push_msg_dir_order = nullptr;
 };
 
 static_assert(sizeof(rpl::StreamCounters) == sizeof(rpl_stream_counters) &&
@@ -1500,14 +1509,33 @@ rpl_result decode_assemble(rpl_ctx* c, cudaStream_t st, const WireChunk& w, uint
   return RPL_RESULT_OK;
 }
 
+// A message push's chunk (rpl_capsule_stream_push_laserscan_msgs*): where its messages and tables go, every table at
+// the chunk's first slot (stream).
+struct ChunkMsgs {
+  uint8_t* out;                      // message i at out + place[i] - header - 32
+  bool first, rebase;                // PushMsgDirArgs::first, rebase
+  unsigned long long capacity;
+  unsigned long long *carry, *offsets, *place, *extent, *total;  // PushMsgDirArgs (extent, total nullable)
+  uint32_t* sizes;
+  const rpl::StreamMsgHeader* hdr;
+  long long clock_offset_ns;
+  // a host push's: the directory's extent read back (pinned, then extent_ready), and the order of the chunks' directories
+  // across the lanes (the previous chunk's directory recorded it)
+  unsigned long long* extent_host;
+  cudaEvent_t extent_ready, dir_order;
+};
+
 // (frame ->) decode -> assemble -> scan kernels for the ns streams of chunk w on `st`; capsules / counts / outputs / sp
 // point at the chunk's first stream's (a byte session's capsules / counts: the raw bytes and byte counts).  A mixed
 // byte session's chunk runs the first three for each answer type present in it, over that type's streams, and the scan
 // kernels, which read the arenas whatever the type, once.
+// m (a message push): the directory runs between the assembler and the scan kernels, which write into the placed
+// messages instead of ranges / intens (null), and the header writer behind them.
 rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const WireChunk& w, uint32_t ns,
                                 const uint8_t* capsules, const uint32_t* counts, uint32_t sample_duration_us,
                                 const rpl_scan_params* params, float* ranges, float* intens, uint32_t* beams,
-                                float* inc, uint32_t* scans_per_stream, const StampPush* sp = nullptr) {
+                                float* inc, uint32_t* scans_per_stream, const StampPush* sp = nullptr,
+                                const ChunkMsgs* m = nullptr) {
   rpl_result r = RPL_RESULT_OK;
   if (!w.list_begin) {
     r = decode_assemble(c, st, w, w.ans_type, ns, capsules, counts, sample_duration_us, scans_per_stream, sp, nullptr);
@@ -1521,10 +1549,56 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
     }
   }
   if (r != RPL_RESULT_OK) return r;
-  return enqueue_scan(c, l, w.nodes, w.scan_len, ns * w.max_scans, w.max_nodes, params, nullptr, ranges, intens, beams,
-                      inc, nullptr, nullptr, st, reinterpret_cast<const uint2*>(w.views),
-                      (unsigned long long)ns * w.stride_nodes, LidarTable{w.lidars, w.max_scans, w.lidar_modes});
+  const LidarTable lt{w.lidars, w.max_scans, w.lidar_modes};
+  const uint2* views = reinterpret_cast<const uint2*>(w.views);
+  if (!m)
+    return enqueue_scan(c, l, w.nodes, w.scan_len, ns * w.max_scans, w.max_nodes, params, nullptr, ranges, intens, beams,
+                        inc, nullptr, nullptr, st, views, (unsigned long long)ns * w.stride_nodes, lt);
+  rpl::PushMsgDirArgs d{};
+  d.views = views;
+  d.scans_per_stream = scans_per_stream;
+  d.hdr = m->hdr;
+  d.n_slots = ns * w.max_scans;
+  d.max_scans = w.max_scans;
+  d.first = m->first ? 1u : 0u;
+  d.rebase = m->rebase ? 1u : 0u;
+  d.capacity = m->capacity;
+  d.carry = m->carry;
+  d.offsets = m->offsets;
+  d.place = m->place;
+  d.extent = m->extent;
+  d.total = m->total;
+  if (m->dir_order) RPL_CUDA(c, cudaStreamWaitEvent(st, m->dir_order, 0), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, rpl::launch_push_msg_dir(d, st), RPL_RESULT_OPERATION_FAIL);
+  c->launches++;
+  if (m->dir_order) RPL_CUDA(c, cudaEventRecord(m->dir_order, st), RPL_RESULT_OPERATION_FAIL);
+  if (m->extent_host) {
+    RPL_CUDA(c, cudaMemcpyAsync(m->extent_host, m->extent, 3 * 8, cudaMemcpyDeviceToHost, st), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaEventRecord(m->extent_ready, st), RPL_RESULT_OPERATION_FAIL);
+  }
+  r = enqueue_scan(c, l, w.nodes, w.scan_len, ns * w.max_scans, w.max_nodes, params, nullptr, nullptr, nullptr, beams,
+                   inc, nullptr, nullptr, st, views, (unsigned long long)ns * w.stride_nodes, lt, m->out, m->place);
+  if (r != RPL_RESULT_OK) return r;
+  rpl::MsgWriteArgs a{};
+  a.hdr = m->hdr;
+  if (sp) {  // the slots' stamps, as the stamped assembler has just kept them
+    a.begin_us = w.slot_begin;
+    a.end_us = w.slot_end;
+  }
+  a.clock_offset_ns = m->clock_offset_ns;
+  a.counts = beams;
+  a.angle_increment = inc;
+  a.max_scans = w.max_scans;
+  a.mode_a = params->scan_processing ? 1u : 0u;
+  a.n = ns * w.max_scans;
+  a.out = m->out;
+  a.lidars = w.lidars;
+  RPL_CUDA(c, rpl::launch_laserscan_placed(a, m->place, m->sizes, st), RPL_RESULT_OPERATION_FAIL);
+  c->launches++;
+  return RPL_RESULT_OK;
 }
+
+struct HostMsgs;
 
 // A host call's wire input and LaserScan outputs: host arrays of all its streams (the chain's, a session's host push)
 struct HostWire {
@@ -1537,16 +1611,35 @@ struct HostWire {
   uint32_t *beam_counts, *scans_per_stream;
   const StampPush* sp;  // a stamped push: receive times in, scan stamps out
   size_t rx_stream;     // receive times per stream of a stamped push
+  const HostMsgs* msgs;  // a message push: its messages instead of the LaserScan rows (ranges etc. unused)
+};
+
+// A host message push's outputs (host arrays of every slot) and the session's device tables of its chunks
+struct HostMsgs {
+  uint8_t* msgs;
+  unsigned long long capacity;
+  uint64_t* offsets;
+  uint32_t* sizes;
+  uint64_t* total;
+  size_t chunk_bytes;  // staging for one chunk's messages: the bound of its slots at max_nodes
+  long long clock_offset_ns;
+  const rpl::StreamMsgHeader* hdr;  // the session's, [n_streams]
+  unsigned long long *carry, *place, *extent_host;
+  cudaEvent_t extent_ready, dir_order;
 };
 
 // Runs a host call's n_streams streams through capsule_stream_chunk, `chunk` streams at a time round-robin over the
-// lanes: H2D of a chunk's input (and receive times), its kernels, D2H of its LaserScans (and stamps).  A lane's
+// lanes: H2D of a chunk's input (and receive times), its kernels, D2H of its LaserScans (and stamps).  A message push
+// (h.msgs) stages the chunk's messages instead: once its directory's extent is read back (the chunk's scan kernels run
+// meanwhile), the stretch of the packed buffer the chunk fills is copied to msgs, with the chunk's tables.  A lane's
 // staging block holds one chunk's input and outputs, then whatever chunk_at(k, s0) carves off k for the device state
 // of the chunk from stream s0, which it returns (the chain's lives there; a session's in its arenas).
 template <class ChunkAt>
 rpl_result push_host(rpl_ctx* c, const HostWire& h, uint32_t n_streams, uint32_t chunk, ChunkAt chunk_at) {
   const size_t NS = (size_t)chunk * h.max_scans, row = (size_t)h.max_scans * h.max_nodes;
   using u64 = unsigned long long;
+  const HostMsgs* hm = h.msgs;
+  const size_t rows = hm ? 0 : NS * h.max_nodes;
   struct Regions {
     uint8_t* in;
     uint32_t* counts;
@@ -1554,13 +1647,18 @@ rpl_result push_host(rpl_ctx* c, const HostWire& h, uint32_t n_streams, uint32_t
     float *ranges, *intens, *inc;
     uint32_t *beams, *sps;
     u64* ts;
+    uint8_t* msgs;  // a message push's: the chunk's messages, offsets, sizes and extent
+    u64* offs;
+    uint32_t* sizes;
+    u64* extent;
     WireChunk w;
   };
   auto layout = [&](Carve& k, uint32_t s0) {
     return Regions{k.take<uint8_t>(chunk * h.in_stream), k.take<uint32_t>(chunk),
-                   k.take<u64>(h.sp ? chunk * h.rx_stream : 0), k.take<float>(NS * h.max_nodes),
-                   k.take<float>(NS * h.max_nodes), k.take<float>(NS), k.take<uint32_t>(NS), k.take<uint32_t>(chunk),
-                   k.take<u64>(h.sp ? NS : 0), chunk_at(k, s0)};
+                   k.take<u64>(h.sp ? chunk * h.rx_stream : 0), k.take<float>(rows), k.take<float>(rows),
+                   k.take<float>(NS), k.take<uint32_t>(NS), k.take<uint32_t>(chunk), k.take<u64>(h.sp ? NS : 0),
+                   k.take<uint8_t>(hm ? hm->chunk_bytes : 0), k.take<u64>(hm ? NS : 0), k.take<uint32_t>(hm ? NS : 0),
+                   k.take<u64>(hm ? 3 : 0), chunk_at(k, s0)};
   };
   if (const rpl_result r = grow_stage(c, kLanes, [&](Carve& k) { layout(k, 0); }); r != RPL_RESULT_OK) return r;
   const cudaMemcpyKind h2d = cudaMemcpyHostToDevice, d2h = cudaMemcpyDeviceToHost;
@@ -1580,9 +1678,40 @@ rpl_result push_host(rpl_ctx* c, const HostWire& h, uint32_t n_streams, uint32_t
       RPL_CUDA(c, cudaMemcpyAsync(d.rx, h.sp->rx + s0 * h.rx_stream, ns * h.rx_stream * 8, h2d, l.stream),
                RPL_RESULT_OPERATION_FAIL);
     }
+    ChunkMsgs m{};
+    if (hm) {
+      m.out = d.msgs;
+      m.first = s0 == 0;
+      m.rebase = true;
+      m.capacity = hm->capacity;
+      m.carry = hm->carry;
+      m.offsets = d.offs;
+      m.place = hm->place + so;
+      m.extent = d.extent;
+      m.sizes = d.sizes;
+      m.hdr = hm->hdr + s0;
+      m.clock_offset_ns = hm->clock_offset_ns;
+      m.extent_host = hm->extent_host;
+      m.extent_ready = hm->extent_ready;
+      m.dir_order = hm->dir_order;
+    }
     const rpl_result r = capsule_stream_chunk(c, l, l.stream, d.w, ns, d.in, d.counts, h.sample_duration_us, h.params,
-                                              d.ranges, d.intens, d.beams, d.inc, d.sps, h.sp ? &sp : nullptr);
+                                              d.ranges, d.intens, d.beams, d.inc, d.sps, h.sp ? &sp : nullptr,
+                                              hm ? &m : nullptr);
     if (r != RPL_RESULT_OK) return r;
+    if (hm) {
+      // the chunk's stretch [first offset, end of its last message that fits): known once its directory has run
+      RPL_CUDA(c, cudaEventSynchronize(hm->extent_ready), RPL_RESULT_OPERATION_FAIL);
+      const u64 lo = hm->extent_host[0], hi = hm->extent_host[1];
+      if (s0 + ns == n_streams) *hm->total = hm->extent_host[2];
+      if (hi > lo)
+        RPL_CUDA(c, cudaMemcpyAsync(hm->msgs + lo, d.msgs, hi - lo, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
+      RPL_CUDA(c, cudaMemcpyAsync(hm->offsets + so, d.offs, nsc * 8, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
+      RPL_CUDA(c, cudaMemcpyAsync(hm->sizes + so, d.sizes, nsc * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
+      RPL_CUDA(c, cudaMemcpyAsync(h.scans_per_stream + s0, d.sps, (size_t)ns * 4, d2h, l.stream),
+               RPL_RESULT_OPERATION_FAIL);
+      return RPL_RESULT_OK;
+    }
     if (h.sp)
       RPL_CUDA(c, cudaMemcpyAsync(h.sp->scan_ts + so, d.ts, nsc * 8, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
     RPL_CUDA(c, cudaMemcpyAsync(h.ranges + so * h.max_nodes, d.ranges, ns * row * 4, d2h, l.stream),
@@ -1636,11 +1765,13 @@ bool decodes_capsules(const rpl_capsule_stream* cs) {
   return std::any_of(cs->types.begin(), cs->types.end(), [](uint32_t t) { return t != RPL_ANS_MEASUREMENT; });
 }
 
+// msgs: a message push, which has no LaserScan rows
 bool capsule_stream_args_ok(rpl_capsule_stream* cs, const uint8_t* capsules, const uint32_t* capsule_counts,
                             uint32_t sample_duration_us, const rpl_scan_params* params, float* ranges,
-                            float* intensities, uint32_t* beam_counts, uint32_t* scans_per_stream) {
+                            float* intensities, uint32_t* beam_counts, uint32_t* scans_per_stream, bool msgs = false) {
   rpl_ctx* c = cs->c;
-  if (!capsules || !capsule_counts || !params || !ranges || !intensities || !beam_counts || !scans_per_stream) {
+  if (!capsules || !capsule_counts || !params || (!msgs && (!ranges || !intensities || !beam_counts)) ||
+      !scans_per_stream) {
     c->err = "null capsules, counts, params or output buffer";
     return false;
   }
@@ -1887,19 +2018,45 @@ bool push_kind_ok(rpl_capsule_stream* cs, bool bytes) {
   return false;
 }
 
+// The session's device tables of a message push, every slot's: the carry of the directories, each slot's place, the
+// scan kernels' beam counts and angle increments, and the stamped assembler's scan stamps
+struct PushMsgWork {
+  unsigned long long *carry, *place;
+  uint32_t* beams;
+  float* inc;
+  unsigned long long* ts;
+};
+PushMsgWork push_msg_work_layout(const rpl_capsule_stream* cs, Carve& k) {
+  const size_t NS = (size_t)cs->n_streams * cs->max_scans;
+  return PushMsgWork{k.take<unsigned long long>(1), k.take<unsigned long long>(NS), k.take<uint32_t>(NS),
+                     k.take<float>(NS), k.take<unsigned long long>(NS)};
+}
+
+// a message push's outputs (host or device arrays of every slot, as the push's)
+struct PushMsgs {
+  uint8_t* msgs;
+  unsigned long long capacity;
+  uint64_t* offsets;
+  uint32_t* sizes;
+  uint64_t* total;
+  long long clock_offset_ns;
+  PushMsgWork w;
+};
+
 // A push of the kind the entry point takes (bytes: a byte push); sp: a stamped one.  Host arrays (dev false, stream
 // unused) run in the session's host chunks round-robin over the lanes, device arrays in its device chunks on `stream`.
-// The arrays, sp's rx and scan_ts included, hold every stream.
+// The arrays, sp's rx and scan_ts included, hold every stream.  pm: a message push, whose scans go into its messages
+// (ranges, intensities, beam_counts and angle_increment unused).
 rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t* counts, uint32_t sample_duration_us,
                        const rpl_scan_params* params, float* ranges, float* intensities, uint32_t* beam_counts,
                        float* angle_increment, uint32_t* scans_per_stream, const StampPush* sp, bool bytes, bool dev,
-                       void* stream) {
+                       void* stream, const PushMsgs* pm = nullptr) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
   rpl_ctx* c = cs->c;
   cs->cloud_chunk = 0;
   if (!push_kind_ok(cs, bytes)) return RPL_RESULT_INVALID_DATA;
   if (!capsule_stream_args_ok(cs, in, counts, sample_duration_us, params, ranges, intensities, beam_counts,
-                              scans_per_stream))
+                              scans_per_stream, pm != nullptr))
     return RPL_RESULT_INVALID_DATA;
   const bool per_stream = (params->flags & RPL_FLAG_PER_STREAM) != 0;
   const uint32_t chunk = dev ? cs->chunk_dev : cs->chunk_host;
@@ -1917,11 +2074,25 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
         chunk_sp.rx += (size_t)s0 * sp->stride_chunks;
         chunk_sp.scan_ts += so;
       }
+      ChunkMsgs m{};
+      if (pm) {  // straight into the caller's buffer and tables, one chunk after the other on st
+        m.out = pm->msgs;
+        m.first = s0 == 0;
+        m.capacity = pm->capacity;
+        m.carry = pm->w.carry;
+        m.offsets = reinterpret_cast<unsigned long long*>(pm->offsets) + so;
+        m.place = pm->w.place + so;
+        m.total = reinterpret_cast<unsigned long long*>(pm->total);
+        m.sizes = pm->sizes + so;
+        m.hdr = cs->msg_hdr + s0;
+        m.clock_offset_ns = pm->clock_offset_ns;
+      }
       r = capsule_stream_chunk(c, c->lane[0], st, session_chunk(cs, s0, per_stream, true),
                                std::min(chunk, cs->n_streams - s0), in + s0 * cs->in_stream, counts + s0,
-                               sample_duration_us, params, ranges + s0 * row, intensities + s0 * row, beam_counts + so,
-                               angle_increment ? angle_increment + so : nullptr, scans_per_stream + s0,
-                               sp ? &chunk_sp : nullptr);
+                               sample_duration_us, params, pm ? nullptr : ranges + s0 * row,
+                               pm ? nullptr : intensities + s0 * row, pm ? pm->w.beams + so : beam_counts + so,
+                               pm ? pm->w.inc + so : angle_increment ? angle_increment + so : nullptr,
+                               scans_per_stream + s0, sp ? &chunk_sp : nullptr, pm ? &m : nullptr);
     }
   } else {
     for (uint32_t s = 0; s < cs->n_streams; ++s)
@@ -1931,8 +2102,18 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
       }
     RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
     for (int i = 0; i < kLanes; ++i) RPL_CUDA(c, cudaStreamWaitEvent(c->lane[i].stream, cs->done, 0), RPL_RESULT_OPERATION_FAIL);
+    HostMsgs hm{};
+    if (pm) {
+      uint32_t hdr_most = 0;
+      for (const rpl::StreamMsgHeader& e : cs->msg_hdr_host) hdr_most = std::max(hdr_most, e.bytes);
+      const size_t bound = ((size_t)hdr_most + 32 + 8 * (size_t)cs->max_nodes + 4 + 15) & ~(size_t)15;  // a message's
+      hm = HostMsgs{pm->msgs, pm->capacity, pm->offsets, pm->sizes, pm->total, (size_t)chunk * cs->max_scans * bound,
+                    pm->clock_offset_ns, cs->msg_hdr, pm->w.carry, pm->w.place, cs->push_msg_extent,
+                    cs->push_msg_extent_ready, cs->push_msg_dir_order};
+    }
     const HostWire h{in, counts, cs->in_stream, sample_duration_us, cs->max_nodes, cs->max_scans, params, ranges,
-                     intensities, angle_increment, beam_counts, scans_per_stream, sp, sp ? sp->stride_chunks : 0u};
+                     intensities, angle_increment, beam_counts, scans_per_stream, sp, sp ? sp->stride_chunks : 0u,
+                     pm ? &hm : nullptr};
     r = push_host(c, h, cs->n_streams, chunk,
                   [&](Carve&, uint32_t s0) { return session_chunk(cs, s0, per_stream, false); });
   }
@@ -2438,6 +2619,61 @@ rpl_result stream_msgs(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* pa
       });
 }
 
+// ---- LaserScan messages from the push itself (DESIGN.md 5.7.1 "Messages from the push") ---------------------------
+// The push of in's kind, each chunk's scans written straight into their messages: per chunk, after the assembler, the
+// directory places every slot behind the previous chunk's end; the scan kernels write each scan's arrays into its
+// message; the header writer fills in the rest.  The device form writes into the caller's buffer and tables; the host
+// form stages each chunk's messages on its lane and copies the stretch they fill.
+rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, const rpl_scan_params* params,
+                     int64_t clock_offset_ns, uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
+                     uint64_t* total_bytes, uint32_t* scans_per_stream, bool dev, void* stream) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  cs->cloud_chunk = 0;  // as a push that fails its checks
+  if (!in || !params || !msgs || !msg_offsets || !msg_sizes || !total_bytes || !scans_per_stream) {
+    c->err = "null input, params, msgs, msg_offsets, msg_sizes, total_bytes or scans_per_stream";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  if (in->chunk_bytes != 0 && (!cs->bytes || !in->rx_us)) {
+    c->err = cs->bytes ? "chunk_bytes is a stamped push's (rx_us set)"
+                       : "chunk_bytes is a byte push's: a framed session's receive times are per capsule";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  auto mis4 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3u) != 0; };
+  if (dev && ((reinterpret_cast<uintptr_t>(msgs) & 15u) || misaligned8(msg_offsets) || misaligned8(total_bytes) ||
+              mis4(msg_sizes) || mis4(scans_per_stream))) {
+    c->err = "msgs must be 16-byte aligned, msg_offsets and total_bytes 8-byte, msg_sizes and scans_per_stream 4-byte "
+             "aligned";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  if (!cs->push_msg_work) {  // the first message push: the session's tables, made once (their size is fixed)
+    RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+    Carve k;
+    push_msg_work_layout(cs, k);
+    RPL_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&cs->push_msg_work), k.bytes), RPL_RESULT_INSUFFICIENT_MEMORY);
+    RPL_CUDA(c, cudaMallocHost(reinterpret_cast<void**>(&cs->push_msg_extent), 3 * 8), RPL_RESULT_INSUFFICIENT_MEMORY);
+    RPL_CUDA(c, cudaEventCreateWithFlags(&cs->push_msg_extent_ready, cudaEventDisableTiming), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaEventCreateWithFlags(&cs->push_msg_dir_order, cudaEventDisableTiming), RPL_RESULT_OPERATION_FAIL);
+  }
+  Carve k{cs->push_msg_work};
+  const PushMsgs pm{msgs, capacity, msg_offsets, msg_sizes, total_bytes, clock_offset_ns, push_msg_work_layout(cs, k)};
+  StampPush sp{};
+  const bool stamped = in->rx_us != nullptr;
+  // (a stamped push's scan stamps stay on the device: the messages carry them)
+  if (stamped && !stamp_args_ok(cs, params, in->timing, in->rx_us, cs->bytes ? in->chunk_bytes : 1u,
+                                reinterpret_cast<uint64_t*>(pm.w.ts), &sp))
+    return RPL_RESULT_INVALID_DATA;
+  const uint32_t sample_duration_us = stamped ? (in->timing ? in->timing->sample_duration_us : 0u) : in->sample_duration_us;
+  const rpl_result r = stream_push(cs, in->data, in->counts, sample_duration_us, params, nullptr, nullptr, nullptr,
+                                   nullptr, scans_per_stream, stamped ? &sp : nullptr, cs->bytes, dev, stream, &pm);
+  if (r != RPL_RESULT_OK) return r;
+  if (!dev && *total_bytes > capacity) {
+    c->err = "the messages need more than capacity bytes (total_bytes tells how many; the push itself is done)";
+    return RPL_RESULT_INSUFFICIENT_MEMORY;
+  }
+  return RPL_RESULT_OK;
+}
+
 // ---- grabbed node buffers of the last push (DESIGN.md 5.7.1 "Session nodes") -------------------------------------
 // Per call: the directory over every slot (counts, packed offsets, each slot's place), then per chunk of the push the
 // shared-memory EMIT kernel with the general kernel behind it for the ascended slots, writing each revolution at its
@@ -2681,6 +2917,10 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   cudaFree(cs->node_work);
   cudaFree(cs->lidars);
   cudaFree(cs->counters);
+  cudaFree(cs->push_msg_work);
+  cudaFreeHost(cs->push_msg_extent);
+  if (cs->push_msg_extent_ready) cudaEventDestroy(cs->push_msg_extent_ready);
+  if (cs->push_msg_dir_order) cudaEventDestroy(cs->push_msg_dir_order);
   if (cs->done) cudaEventDestroy(cs->done);
   delete cs;
 }
@@ -2955,6 +3195,23 @@ rpl_result rpl_capsule_stream_laserscan_msgs(rpl_capsule_stream* s, const rpl_sc
                                              uint64_t* msg_offsets, uint32_t* msg_sizes, uint64_t* total_bytes) {
   return stream_msgs(s, rpl::MsgKind::kLaserScan, params, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
                      total_bytes);
+}
+
+rpl_result rpl_capsule_stream_push_laserscan_msgs(rpl_capsule_stream* s, const rpl_push_input* in,
+                                                  const rpl_scan_params* params, int64_t clock_offset_ns, uint8_t* msgs,
+                                                  uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
+                                                  uint64_t* total_bytes, uint32_t* scans_per_stream) {
+  return push_msgs(s, in, params, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes, total_bytes, scans_per_stream,
+                   false, nullptr);
+}
+
+rpl_result rpl_capsule_stream_push_laserscan_msgs_dev(rpl_capsule_stream* s, const rpl_push_input* in,
+                                                      const rpl_scan_params* params, int64_t clock_offset_ns,
+                                                      uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,
+                                                      uint32_t* msg_sizes, uint64_t* total_bytes,
+                                                      uint32_t* scans_per_stream, void* stream) {
+  return push_msgs(s, in, params, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes, total_bytes, scans_per_stream,
+                   true, stream);
 }
 
 rpl_result rpl_capsule_stream_cloud_msgs_dev(rpl_capsule_stream* s, const rpl_cloud_params* params,

@@ -49,6 +49,13 @@ struct ScanBatchArgs {
   // not this launch's scan: the kernels leave it before they read its nodes and write nothing for it, status included.
   // (The last member: the argument offsets of the kernels that do not read it stay what they were.)
   const unsigned long long* out_first;
+  // placed LaserScan messages (a push's messages, rpl_capsule_stream_push_laserscan_msgs*; nullable; the shared-memory
+  // MSG kernels and the general kernel): scan s writes its ranges at msg_out + msg_ranges[s] and its intensities 4 bytes
+  // behind its last range, where the header writer puts the intensities count.  The payload is only 4-byte aligned (the
+  // header's length follows the frame_id): the kernels store 4-byte words.  An entry with kOutSkip set has no message:
+  // the kernels leave it as they leave an out_first skip.  (Behind out_first, for the same reason.)
+  uint8_t* msg_out;
+  const unsigned long long* msg_ranges;
 };
 constexpr unsigned long long kOutSkip = 1ull << 63;
 

@@ -102,7 +102,7 @@ __global__ void __launch_bounds__(GT, 1)
   bool inverted = a.inverted != 0;
   const bool ascend = a.apply_ascend != 0;
   const bool cloud = a.xyzi != nullptr;  // PointCloud2 payload: window filter + polar->xyz
-  const bool want_scan = a.ranges != nullptr || cloud;
+  const bool want_scan = a.ranges != nullptr || cloud || a.msg_out != nullptr;
   auto kept = [&](uint2 nd) {
     const uint32_t d = node_dist(nd);
     if (d == 0) return false;
@@ -122,6 +122,7 @@ __global__ void __launch_bounds__(GT, 1)
   for (uint32_t work = blockIdx.x; work < n_work; work += gridDim.x) {
     const uint32_t s = all_scans ? work : a.fallback_list[work];
     if (a.out_first && (a.out_first[s] & kOutSkip) != 0) continue;  // a placed launch: not a scan of the scan kernels
+    if (a.msg_out && (a.msg_ranges[s] & kOutSkip) != 0) continue;  // a placed message that has no room
     if (a.lidars) {  // the scan's stream's settings (the hand-off list mixes the modes of both shared-memory launches)
       const LidarSettings& ls = a.lidars[s / a.lidar_scans];
       new_proto = ls.is_new_protocol != 0;
@@ -242,8 +243,9 @@ __global__ void __launch_bounds__(GT, 1)
       __syncthreads();
       continue;
     }
-    float* ranges = a.ranges + (size_t)s * a.stride;
-    float* intens = a.intensities + (size_t)s * a.stride;
+    // a placed message: ranges, the intensities count, intensities (ScanBatchArgs::msg_out)
+    float* ranges = a.msg_out ? reinterpret_cast<float*>(a.msg_out + a.msg_ranges[s]) : a.ranges + (size_t)s * a.stride;
+    float* intens = a.msg_out ? ranges + M + 1 : a.intensities + (size_t)s * a.stride;
     if (!mode_a) {  // Mode B (reference rplidar_node.cpp:661-677)
       for (uint32_t v = tid; v < M; v += GT) {
         const uint2 nd = base[vidx[v]];

@@ -264,14 +264,16 @@ __device__ __noinline__ void vdup_place_shared(const uint2* tile, const uint32_t
   }
 }
 
-template <int MODE, bool EMIT, bool POST, int TS>
-__global__ void __launch_bounds__(TS, POST ? 2 : (EMIT ? 4 : (MODE == 0 ? 5 : 1))) scan_small_kernel(ScanBatchArgs a, SmallArgs p) {
+// The body of every shared-memory kernel.  MSG (LaserScan, no ascended buffer): the ranges and intensities go into the
+// scan's placed message (ScanBatchArgs::msg_out) instead of its rows.
+template <int MODE, bool EMIT, bool POST, int TS, bool MSG>
+__device__ __forceinline__ void scan_small_body(const ScanBatchArgs& a, const SmallArgs& p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   constexpr bool MODE_A = (MODE == 1);
   constexpr bool CLOUD = (MODE == 2);
   constexpr int NW = TS / 32;
   constexpr uint32_t WPT = kWords / TS;  // bitmap words per thread in the prefix step
-  static_assert(!(EMIT && CLOUD) && !(POST && !CLOUD), "variant");
+  static_assert(!(EMIT && CLOUD) && !(POST && !CLOUD) && !(MSG && (EMIT || CLOUD)), "variant");
   static_assert(kWords % TS == 0 && WPT % 4 == 0, "prefix layout");
   SmallCtl& ctl = *reinterpret_cast<SmallCtl*>(smem_raw);
   const uint32_t cap = p.cap;
@@ -324,6 +326,7 @@ __global__ void __launch_bounds__(TS, POST ? 2 : (EMIT ? 4 : (MODE == 0 ? 5 : 1)
 
   for (uint32_t s = blockIdx.x; s < a.n_scans; s += gridDim.x) {
     if (EMIT && out_skipped(a, s)) continue;
+    if (MSG && (a.msg_ranges[s] & kOutSkip) != 0) continue;
     bool new_proto = a.is_new_protocol != 0, inverted = a.inverted != 0;
     if (a.lidars) {  // the scan's stream's settings; a LaserScan scan of the other mode is the other launch's
       const LidarSettings& ls = a.lidars[s / a.lidar_scans];
@@ -582,6 +585,10 @@ __global__ void __launch_bounds__(TS, POST ? 2 : (EMIT ? 4 : (MODE == 0 ? 5 : 1)
     // ---- place ------------------------------------------------------------------------------------------
     float* ranges = want_scan ? a.ranges + (size_t)s * a.stride : nullptr;
     float* intens = want_scan ? a.intensities + (size_t)s * a.stride : nullptr;
+    if constexpr (MSG) {  // the message's float32[] ranges, its intensities count, its float32[] intensities
+      ranges = reinterpret_cast<float*>(a.msg_out + a.msg_ranges[s]);
+      intens = ranges + M + 1;
+    }
     float4* cloud = CLOUD ? a.xyzi + (size_t)s * a.stride : nullptr;
     uint2* nodes_out = EMIT ? nodes_out_of(a, s) : nullptr;
     const float inc = angle_increment(M, MODE_A);
@@ -987,26 +994,47 @@ __global__ void __launch_bounds__(TS, POST ? 2 : (EMIT ? 4 : (MODE == 0 ? 5 : 1)
 }
 
 template <int MODE, bool EMIT, bool POST, int TS>
+__global__ void __launch_bounds__(TS, POST ? 2 : (EMIT ? 4 : (MODE == 0 ? 5 : 1))) scan_small_kernel(ScanBatchArgs a, SmallArgs p) {
+  scan_small_body<MODE, EMIT, POST, TS, false>(a, p);
+}
+
+constexpr int kSmallThreads = 256;      // LaserScan variants
+constexpr int kSmallPostThreads = 512;  // PointCloud2 chain
+
+// LaserScan Mode B (MODE 0) or Mode A (MODE 1) into placed messages: its own kernel, so that the others keep their code
+template <int MODE>
+__global__ void __launch_bounds__(kSmallThreads, MODE == 0 ? 5 : 1) scan_small_msg_kernel(ScanBatchArgs a, SmallArgs p) {
+  scan_small_body<MODE, false, false, kSmallThreads, true>(a, p);
+}
+
+template <class K>
+cudaError_t configure_kernel(K kernel) {
+  return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+}
+
+template <int MODE, bool EMIT, bool POST, int TS>
 cudaError_t configure_one() {
-  return cudaFuncSetAttribute(scan_small_kernel<MODE, EMIT, POST, TS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                              227 * 1024);
+  return configure_kernel(scan_small_kernel<MODE, EMIT, POST, TS>);
+}
+
+template <class K>
+cudaError_t launch_kernel(K kernel, int threads, const ScanBatchArgs& a, const SmallArgs& p, size_t smem, int num_sms,
+                          cudaStream_t stream) {
+  int occ = 0;
+  cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, threads, smem);
+  if (e != cudaSuccess) return e;
+  if (occ < 1) return cudaErrorLaunchOutOfResources;
+  const int grid = (int)std::min<uint32_t>((uint32_t)(occ * num_sms), a.n_scans);
+  kernel<<<grid, threads, smem, stream>>>(a, p);
+  return cudaGetLastError();
 }
 
 template <int MODE, bool EMIT, bool POST, int TS>
 cudaError_t launch_one(const ScanBatchArgs& a, const SmallArgs& p, size_t smem, int num_sms, cudaStream_t stream) {
-  int occ = 0;
-  cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, scan_small_kernel<MODE, EMIT, POST, TS>, TS, smem);
-  if (e != cudaSuccess) return e;
-  if (occ < 1) return cudaErrorLaunchOutOfResources;
-  const int grid = (int)std::min<uint32_t>((uint32_t)(occ * num_sms), a.n_scans);
-  scan_small_kernel<MODE, EMIT, POST, TS><<<grid, TS, smem, stream>>>(a, p);
-  return cudaGetLastError();
+  return launch_kernel(scan_small_kernel<MODE, EMIT, POST, TS>, TS, a, p, smem, num_sms, stream);
 }
 
 }  // namespace
-
-constexpr int kSmallThreads = 256;      // LaserScan variants
-constexpr int kSmallPostThreads = 512;  // PointCloud2 chain
 
 size_t scan_small_smem_bytes(uint32_t cap, int mode, bool emit, bool post) {
   size_t b = kCtl + (size_t)cap * 8 + 16;  // control block + tile (+ one node either side for unaligned views)
@@ -1028,6 +1056,8 @@ cudaError_t scan_small_configure() {
   if ((e = configure_one<1, false, false, kSmallThreads>()) != cudaSuccess) return e;
   if ((e = configure_one<1, true, false, kSmallThreads>()) != cudaSuccess) return e;
   if ((e = configure_one<2, false, false, kSmallThreads>()) != cudaSuccess) return e;
+  if ((e = configure_kernel(scan_small_msg_kernel<0>)) != cudaSuccess) return e;
+  if ((e = configure_kernel(scan_small_msg_kernel<1>)) != cudaSuccess) return e;
   return configure_one<2, false, true, kSmallPostThreads>();
 }
 
@@ -1050,6 +1080,10 @@ cudaError_t launch_scan_small(const ScanBatchArgs& a, uint32_t max_nodes, uint32
   }
   auto launch_mode = [&](int mode) {
     const size_t sh = scan_small_smem_bytes(p.cap, mode, emit, false);
+    if (a.msg_out) {
+      if (mode == 1) return launch_kernel(scan_small_msg_kernel<1>, kSmallThreads, a, p, sh, num_sms, stream);
+      return launch_kernel(scan_small_msg_kernel<0>, kSmallThreads, a, p, sh, num_sms, stream);
+    }
     if (mode == 1) {
       if (emit) return launch_one<1, true, false, kSmallThreads>(a, p, sh, num_sms, stream);
       return launch_one<1, false, false, kSmallThreads>(a, p, sh, num_sms, stream);

@@ -837,6 +837,49 @@ rpl_result rpl_capsule_stream_push_laserscan_msgs_dev(rpl_capsule_stream* s, con
                                                       uint32_t* msg_sizes, uint64_t* total_bytes,
                                                       uint32_t* scans_per_stream, void* stream);
 
+/* PointCloud2 messages from the push: one call that pushes `in` and returns the PointCloud2 messages of the scans it
+ * published.  Each chunk of the push runs its cloud chain over the views its assembler has just made, then sizes and
+ * packs the chunk's messages and writes them.  No LaserScan is computed, and no padded row of any kind crosses the link.
+ *   in:      as rpl_capsule_stream_push_laserscan_msgs.
+ *   params:  the cloud chain's, as rpl_capsule_stream_cloud_msgs.  With RPL_CLOUD_PER_STREAM the push decodes and stamps
+ *            stream s with settings[s], as a push with RPL_FLAG_PER_STREAM does (of rpl_scan_params only that flag
+ *            reaches the decoders, the assembler and the stamps), and its cloud takes settings[s].is_new_protocol.
+ *            Without it the push takes in's timing for every stream.
+ *   Definition: with two sessions of the same history, A pushed with the entry point of in's kind (RPL_FLAG_PER_STREAM
+ *            iff params has RPL_CLOUD_PER_STREAM) and then rpl_capsule_stream_cloud_msgs[_dev] with params and
+ *            clock_offset_ns, B with this call: when *total_bytes <= capacity, scans_per_stream, msg_offsets, msg_sizes,
+ *            *total_bytes and every message's bytes are equal, and every later call returns on B what it returns on A
+ *            (this call sets the last push as a push does).  A call that fails its checks leaves the session as the
+ *            push it stands for would.
+ *   Packing: exact, the packing of rpl_capsule_stream_cloud_msgs: slot i = s * max_scans + k of a published scan
+ *            (k < min(scans_per_stream[s], max_scans)) has its message at the cloud's point count, an empty cloud
+ *            included; an unused slot none.  msg_offsets is the exclusive scan of the sizes, each rounded up to 16, in
+ *            slot order, and *total_bytes the end of the last message.  Unlike push_laserscan_msgs no bound is needed:
+ *            each chunk sizes its messages after its cloud kernels have run, and a carry on the device continues the
+ *            offsets from chunk to chunk.
+ *   Capacity: message i is written iff msg_offsets[i] + its size <= capacity, else its size is 0: the written messages
+ *            are a prefix, and the push itself is done either way.  Unlike cloud_msgs this is not all or nothing: a
+ *            device push's total is not known on the host before its chunks run.  The host form returns
+ *            RPL_RESULT_INSUFFICIENT_MEMORY when *total_bytes > capacity, the _dev form reports it through *total_bytes
+ *            only; in both cases rpl_capsule_stream_cloud_msgs on the same push returns every message.  Nothing at or
+ *            past msgs + min(*total_bytes, capacity) is written.
+ *   Errors:  those of rpl_capsule_stream_push_laserscan_msgs, a params that fails the cloud chain's rules, and
+ *            RPL_CLOUD_PER_STREAM before the first rpl_capsule_stream_set_lidars: RPL_RESULT_INVALID_DATA.
+ *   _dev:    as rpl_capsule_stream_push_laserscan_msgs_dev.
+ *   host:    synchronous, host buffers.  Only the tables and the messages' stretch of msgs cross the link.
+ *   Cost:    the session keeps, from the first call, 24 bytes per slot of device tables.  The _dev form's clouds take a
+ *            block of one device chunk's slots at max_nodes (16 bytes per node; the session's message work block, which
+ *            cloud_msgs sizes for every slot); the host form stages one host chunk's clouds and messages per lane. */
+rpl_result rpl_capsule_stream_push_cloud_msgs(rpl_capsule_stream* s, const rpl_push_input* in,
+                                              const rpl_cloud_params* params, int64_t clock_offset_ns, uint8_t* msgs,
+                                              uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
+                                              uint64_t* total_bytes, uint32_t* scans_per_stream);
+rpl_result rpl_capsule_stream_push_cloud_msgs_dev(rpl_capsule_stream* s, const rpl_push_input* in,
+                                                  const rpl_cloud_params* params, int64_t clock_offset_ns,
+                                                  uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,
+                                                  uint32_t* msg_sizes, uint64_t* total_bytes,
+                                                  uint32_t* scans_per_stream, void* stream);
+
 /* Per-stream lidar settings: each stream of a session is one lidar, the reference's one RPlidarNode, with its own
  * intensity protocol (RealLidarDriver::is_new_type(), src/lidar_driver_wrapper.cpp:303-305), scan_processing and
  * inverted parameters (src/rplidar_node.cpp:270, 278-279) and SlamtecLidarTimingDesc (which depends on the model, the

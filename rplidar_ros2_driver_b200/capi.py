@@ -60,6 +60,7 @@ EXPORTS = [
     "rpl_capsule_stream_set_lidars", "rpl_capsule_stream_laserscan_msgs", "rpl_capsule_stream_laserscan_msgs_dev",
     "rpl_capsule_stream_cloud_msgs", "rpl_capsule_stream_cloud_msgs_dev", "rpl_capsule_stream_nodes",
     "rpl_capsule_stream_nodes_dev", "rpl_capsule_stream_push_laserscan_msgs", "rpl_capsule_stream_push_laserscan_msgs_dev",
+    "rpl_capsule_stream_push_cloud_msgs", "rpl_capsule_stream_push_cloud_msgs_dev",
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -126,7 +127,8 @@ STREAM_COUNTERS_DTYPE = np.dtype([(f, "<u8") for f in STREAM_COUNTER_FIELDS])
 
 
 class PushInput(C.Structure):
-    """rpl_push_input: one push of any flavour for rpl_capsule_stream_push_laserscan_msgs[_dev] (addresses as ints)."""
+    """rpl_push_input: one push of any flavour for rpl_capsule_stream_push_{laserscan,cloud}_msgs[_dev] (addresses as
+    ints)."""
     _fields_ = [("data", C.c_void_p), ("counts", C.c_void_p), ("rx_us", C.c_void_p), ("timing", C.POINTER(Timing)),
                 ("sample_duration_us", C.c_uint32), ("chunk_bytes", C.c_uint32)]
 
@@ -249,6 +251,9 @@ def lib() -> C.CDLL:
         "rpl_capsule_stream_push_laserscan_msgs": ([vp, C.POINTER(PushInput), PSP, C.c_int64, vp, u64, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_push_laserscan_msgs_dev":
             ([vp, C.POINTER(PushInput), PSP, C.c_int64, vp, u64, vp, vp, vp, vp, vp], u32),
+        "rpl_capsule_stream_push_cloud_msgs": ([vp, C.POINTER(PushInput), PCP, C.c_int64, vp, u64, vp, vp, vp, vp], u32),
+        "rpl_capsule_stream_push_cloud_msgs_dev":
+            ([vp, C.POINTER(PushInput), PCP, C.c_int64, vp, u64, vp, vp, vp, vp, vp], u32),
     }
     for name, (args, res) in sig.items():
         fn = getattr(L, name)  # AttributeError here = the library does not export the ABI
@@ -787,6 +792,28 @@ class CapsuleStreamSession:
         pi._keep = t
         return pi
 
+    def _push_msgs(self, name, data, counts, params, clock_offset_ns, sample_duration_us, rx_us, timing, chunk_bytes,
+                   msgs, packed):
+        assert isinstance(data, np.ndarray) and data.dtype == np.uint8 and data.flags.c_contiguous
+        cnt = np.ascontiguousarray(counts, dtype=np.uint32)
+        assert cnt.shape == (self.n_streams,)
+        rx = None if rx_us is None else np.ascontiguousarray(rx_us, dtype=np.uint64)
+        ns = self.n_streams * self.max_scans
+        if msgs is None:  # room for every slot's largest message
+            per = 288 + (32 + 8 * self.max_nodes + 4 if name == "push_laserscan_msgs" else 116 + 16 * self.max_nodes + 1)
+            msgs = np.zeros(ns * ((per + 15) // 16 * 16), np.uint8)
+        assert msgs.dtype == np.uint8 and msgs.flags.c_contiguous
+        offs, sizes, total = np.zeros(ns, np.uint64), np.zeros(ns, np.uint32), np.zeros(1, np.uint64)
+        sps = np.zeros(self.n_streams, np.uint32)
+        pi = self._push_input(data, cnt, sample_duration_us, rx, timing, chunk_bytes)
+        rc = self._fn(name)(self._h, C.byref(pi), C.byref(params), int(clock_offset_ns), _p(msgs), msgs.size, _p(offs),
+                            _p(sizes), _p(total), _p(sps))
+        if not packed or rc != RESULT_INSUFFICIENT_MEMORY:
+            self._ctx._check(rc)
+        if packed:
+            return dict(msgs=msgs, msg_offsets=offs, msg_sizes=sizes, total_bytes=int(total[0]), result=rc), sps
+        return [bytes(msgs[o: o + n]) if n else None for o, n in zip(offs.tolist(), sizes.tolist())], sps
+
     def push_laserscan_msgs(self, data, counts, params: ScanParams, clock_offset_ns=0, sample_duration_us=31,
                             rx_us=None, timing: "Timing | None" = None, chunk_bytes=None, msgs=None, packed=False):
         """One push (host buffers: data and counts as the push of the session's kind; rx_us -- capsule receive times on a
@@ -795,24 +822,8 @@ class CapsuleStreamSession:
         (messages, scans_per_stream): messages as laserscan_msgs returns them (per slot the bytes or None; packed: the
         dict, with the push's own bound-based offsets and result RESULT_INSUFFICIENT_MEMORY rather than an exception
         when msgs is too small -- the push is done either way).  msgs None: a buffer that always fits."""
-        assert isinstance(data, np.ndarray) and data.dtype == np.uint8 and data.flags.c_contiguous
-        cnt = np.ascontiguousarray(counts, dtype=np.uint32)
-        assert cnt.shape == (self.n_streams,)
-        rx = None if rx_us is None else np.ascontiguousarray(rx_us, dtype=np.uint64)
-        ns = self.n_streams * self.max_scans
-        if msgs is None:
-            msgs = np.zeros(ns * ((288 + 32 + 8 * self.max_nodes + 4 + 15) // 16 * 16), np.uint8)
-        assert msgs.dtype == np.uint8 and msgs.flags.c_contiguous
-        offs, sizes, total = np.zeros(ns, np.uint64), np.zeros(ns, np.uint32), np.zeros(1, np.uint64)
-        sps = np.zeros(self.n_streams, np.uint32)
-        pi = self._push_input(data, cnt, sample_duration_us, rx, timing, chunk_bytes)
-        rc = self._fn("push_laserscan_msgs")(self._h, C.byref(pi), C.byref(params), int(clock_offset_ns), _p(msgs),
-                                             msgs.size, _p(offs), _p(sizes), _p(total), _p(sps))
-        if not packed or rc != RESULT_INSUFFICIENT_MEMORY:
-            self._ctx._check(rc)
-        if packed:
-            return dict(msgs=msgs, msg_offsets=offs, msg_sizes=sizes, total_bytes=int(total[0]), result=rc), sps
-        return [bytes(msgs[o: o + n]) if n else None for o, n in zip(offs.tolist(), sizes.tolist())], sps
+        return self._push_msgs("push_laserscan_msgs", data, counts, params, clock_offset_ns, sample_duration_us, rx_us,
+                               timing, chunk_bytes, msgs, packed)
 
     def push_laserscan_msgs_dev(self, data, counts, params: ScanParams, clock_offset_ns, msgs, capacity, msg_offsets,
                                 msg_sizes, total_bytes, scans_per_stream, sample_duration_us=31, rx_us=None,
@@ -821,6 +832,25 @@ class CapsuleStreamSession:
         laserscan_msgs_dev), asynchronous on `stream` (None: the context's stream)."""
         pi = self._push_input(data, counts, sample_duration_us, rx_us, timing, chunk_bytes)
         self._ctx._check(self._fn("push_laserscan_msgs_dev")(
+            self._h, C.byref(pi), C.byref(params), int(clock_offset_ns), _p(msgs), int(capacity), _p(msg_offsets),
+            _p(msg_sizes), _p(total_bytes), _p(scans_per_stream), _p(stream)))
+
+    def push_cloud_msgs(self, data, counts, params: CloudParams, clock_offset_ns=0, sample_duration_us=31, rx_us=None,
+                        timing: "Timing | None" = None, chunk_bytes=None, msgs=None, packed=False):
+        """One push, as push_laserscan_msgs takes it, whose scans come back as their serialised sensor_msgs/PointCloud2:
+        each chunk of the push runs the cloud chain of params over its scans, then packs their messages exactly as
+        cloud_msgs does.  With CLOUD_PER_STREAM the push decodes and stamps each stream with its own lidar settings.
+        Returns (messages, scans_per_stream) as push_laserscan_msgs; capacity is per message (the written messages
+        are a prefix), and RESULT_INSUFFICIENT_MEMORY (packed) leaves the push done."""
+        return self._push_msgs("push_cloud_msgs", data, counts, params, clock_offset_ns, sample_duration_us, rx_us,
+                               timing, chunk_bytes, msgs, packed)
+
+    def push_cloud_msgs_dev(self, data, counts, params: CloudParams, clock_offset_ns, msgs, capacity, msg_offsets,
+                            msg_sizes, total_bytes, scans_per_stream, sample_duration_us=31, rx_us=None,
+                            timing: "Timing | None" = None, chunk_bytes=None, stream=None):
+        """Device addresses, as push_laserscan_msgs_dev."""
+        pi = self._push_input(data, counts, sample_duration_us, rx_us, timing, chunk_bytes)
+        self._ctx._check(self._fn("push_cloud_msgs_dev")(
             self._h, C.byref(pi), C.byref(params), int(clock_offset_ns), _p(msgs), int(capacity), _p(msg_offsets),
             _p(msg_sizes), _p(total_bytes), _p(scans_per_stream), _p(stream)))
 

@@ -252,30 +252,41 @@ __global__ void __launch_bounds__(CT) pointcloud2_msgs_kernel(MsgWriteArgs a, Cl
   }
 }
 
-// ---- LaserScan messages written by a push ------------------------------------------------------------------------
+// ---- messages written by a push --------------------------------------------------------------------------------
 // One CTA over the chunk's slots in tiles of MT, as msg_table_kernel, the carry passing from tile to tile and, through
 // *a.carry, from chunk to chunk: the chunks of a push run one after the other (one stream, or the host push's lanes
 // ordered by an event), so each reads the end the one before it wrote.
+// K = kLaserScan: a published slot's bound, its message at the view's node count rounded up to 16, places it before
+// the scan kernels run (place[i]); the end of the bounds is the total.
+// K = kPointCloud2: a published slot's exact size at its cloud's point count, once the cloud kernels have run, rounded
+// up to 16 for the offsets (msg_table_kernel's packing); sizes[i] is the size when the message fits capacity, else 0,
+// and the total is the end of the last message, carried in carry[1].
+template <MsgKind K>
 __global__ void __launch_bounds__(MT) push_msg_dir_kernel(PushMsgDirArgs a) {
+  constexpr bool kCloud = K == MsgKind::kPointCloud2;
   __shared__ unsigned long long s_warp[MT / 32];
-  __shared__ unsigned long long s_first, s_fit_end;
+  __shared__ unsigned long long s_first, s_fit_end, s_last_end;
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   if (tid == 0) {
     s_first = a.first ? 0ull : *a.carry;
     s_fit_end = s_first;
+    if constexpr (kCloud) s_last_end = a.first ? 0ull : a.carry[1];
   }
   __syncthreads();
   const unsigned long long first = s_first, rel = a.rebase ? first : 0ull;
   unsigned long long carry = first;
   for (uint32_t t0 = 0; t0 < a.n_slots; t0 += MT) {
     const uint32_t i = t0 + tid;
-    uint32_t bound = 0, hb = 0;
+    uint32_t bound = 0, hb = 0;  // PointCloud2: the exact size
     if (i < a.n_slots) {
       const uint32_t s = i / a.max_scans, k = i - s * a.max_scans;
       hb = a.hdr[s].bytes;
-      if (k < min(a.scans_per_stream[s], a.max_scans)) bound = (msg_bytes(MsgKind::kLaserScan, hb, a.views[i].y) + 15u) & ~15u;
+      if (k < min(a.scans_per_stream[s], a.max_scans)) {
+        if constexpr (kCloud) bound = msg_bytes(K, hb, a.counts[i]);
+        else bound = (msg_bytes(K, hb, a.views[i].y) + 15u) & ~15u;
+      }
     }
-    const unsigned long long v = bound;
+    const unsigned long long v = kCloud ? (bound + 15u) & ~15u : bound;
     unsigned long long inc = v;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
@@ -294,7 +305,12 @@ __global__ void __launch_bounds__(MT) push_msg_dir_kernel(PushMsgDirArgs a) {
     if (i < a.n_slots) {
       const bool fits = bound != 0 && off + bound <= a.capacity;
       a.offsets[i] = off;
-      a.place[i] = fits ? off - rel + hb + 32u : kOutSkip;
+      if constexpr (kCloud) {
+        a.sizes[i] = fits ? bound : 0u;
+        if (bound) atomicMax(&s_last_end, off + bound);
+      } else {
+        a.place[i] = fits ? off - rel + hb + 32u : kOutSkip;
+      }
       if (fits) atomicMax(&s_fit_end, off + bound);
     }
     carry += tile;
@@ -302,12 +318,14 @@ __global__ void __launch_bounds__(MT) push_msg_dir_kernel(PushMsgDirArgs a) {
   }
   if (tid == 0) {
     *a.carry = carry;
+    const unsigned long long end = kCloud ? s_last_end : carry;
+    if constexpr (kCloud) a.carry[1] = end;
     if (a.extent) {
       a.extent[0] = first;
       a.extent[1] = s_fit_end;
-      a.extent[2] = carry;
+      a.extent[2] = end;
     }
-    if (a.total) *a.total = carry;
+    if (a.total) *a.total = end;
   }
 }
 
@@ -326,8 +344,11 @@ __global__ void __launch_bounds__(32) laserscan_placed_kernel(MsgWriteArgs a, co
 
 }  // namespace
 
-cudaError_t launch_push_msg_dir(const PushMsgDirArgs& a, cudaStream_t stream) {
-  push_msg_dir_kernel<<<1, MT, 0, stream>>>(a);
+cudaError_t launch_push_msg_dir(const PushMsgDirArgs& a, MsgKind kind, cudaStream_t stream) {
+  if (kind == MsgKind::kLaserScan)
+    push_msg_dir_kernel<MsgKind::kLaserScan><<<1, MT, 0, stream>>>(a);
+  else
+    push_msg_dir_kernel<MsgKind::kPointCloud2><<<1, MT, 0, stream>>>(a);
   return cudaGetLastError();
 }
 

@@ -101,12 +101,13 @@ struct MsgWriteArgs {
 cudaError_t launch_msg_table(const MsgTableArgs& a, cudaStream_t stream);
 cudaError_t launch_laserscan_msgs(const MsgWriteArgs& a, uint32_t max_beams, cudaStream_t stream);
 
-// ---- LaserScan messages written by a push (rpl_capsule_stream_push_laserscan_msgs*) ---------------------------------
+// ---- messages written by a push (rpl_capsule_stream_push_{laserscan,cloud}_msgs*) -------------------------------
 // The directory of one chunk of the push, one CTA, every pointer at the chunk's first slot (stream).  A published slot
-// (k < min(scans_per_stream[s], max_scans)) is bounded by its message at the view's node count, rounded up to 16; an
-// unused slot by 0.  offsets[i] = *carry (the previous chunk's end; 0 for the push's first chunk) + the exclusive scan
-// of the chunk's bounds; the chunk's end goes back to *carry.  A slot whose bounded message ends past `capacity` gets
-// no message.
+// (k < min(scans_per_stream[s], max_scans)) takes, rounded up to 16, its LaserScan message at the view's node count (a
+// bound, known before the scan kernels run) or its PointCloud2 message at the cloud's point count (the exact size,
+// known once the cloud kernels have run); an unused slot 0.  offsets[i] = *carry (the previous chunk's end; 0 for the
+// push's first chunk) + the exclusive scan of the chunk's rounded sizes; the chunk's end goes back to *carry.  A slot
+// whose message ends past `capacity` gets no message.
 struct PushMsgDirArgs {
   const uint2* views;               // [n_slots] the chunk's scans
   const uint32_t* scans_per_stream; // [n_slots / max_scans]
@@ -115,16 +116,19 @@ struct PushMsgDirArgs {
   uint32_t first;                   // != 0: the push's first chunk (the carry is not read)
   uint32_t rebase;                  // != 0: place[] counts from the chunk's first offset (else from 0)
   unsigned long long capacity;
-  unsigned long long* carry;        // [1] in / out
+  unsigned long long* carry;        // [1] in / out; PointCloud2: [2], the end of the last message in carry[1]
   unsigned long long* offsets;      // [n_slots] out
-  // [n_slots] out, ScanBatchArgs::msg_ranges: where the message's ranges start (message position + header + 32);
-  // kOutSkip for a slot without a message
+  // [n_slots] out, LaserScan, ScanBatchArgs::msg_ranges: where the message's ranges start (message position + header
+  // + 32); kOutSkip for a slot without a message
   unsigned long long* place;
   unsigned long long* extent;       // [3] out, nullable: the chunk's first offset, the end of its last message that
-                                    // fits, the end of its bounds
-  unsigned long long* total;        // [1] out, nullable: the end of the chunk's bounds
+                                    // fits, the total so far
+  unsigned long long* total;        // [1] out, nullable: the total so far -- LaserScan: the end of the chunk's bounds;
+                                    // PointCloud2: the end of the last message (msg_table_kernel's total)
+  const uint32_t* counts;           // [n_slots] PointCloud2: the clouds' point counts
+  uint32_t* sizes;                  // [n_slots] out, PointCloud2: the message's bytes when it fits, else 0
 };
-cudaError_t launch_push_msg_dir(const PushMsgDirArgs& a, cudaStream_t stream);
+cudaError_t launch_push_msg_dir(const PushMsgDirArgs& a, MsgKind kind, cudaStream_t stream);
 // The fixed part of every placed message of slots [0, a.n) once the scan kernels have written its arrays (a's hdr,
 // begin_us / end_us, counts, angle_increment, lidars at the chunk's first slot; its offsets, sizes, out_base unused):
 // message i at a.out + place[i] - header bytes - 32; sizes[i] its bytes, 0 for no message.

@@ -1269,11 +1269,12 @@ struct rpl_capsule_stream {
   // [n_streams] device, zeroed at create: what every push decoded and lost (rpl_capsule_stream_counters); a stream's
   // record is written by the one CTA of each kernel that serves the stream
   rpl::StreamCounters* counters = nullptr;
-  // message pushes (rpl_capsule_stream_push_laserscan_msgs*), made by the first: the device tables of the push's slots
-  // (PushMsgWork), the host form's pinned read-back of a chunk's extent, and the events that order its chunks
+  // message pushes (rpl_capsule_stream_push_{laserscan,cloud}_msgs*), made by the first: the device tables of the push's
+  // slots (PushMsgWork), the host form's pinned read-back of each lane's chunk's extent ([kLanes][3]) with the events
+  // that tell it is there, and the event that orders the chunks' directories
   unsigned char* push_msg_work = nullptr;
   unsigned long long* push_msg_extent = nullptr;
-  cudaEvent_t push_msg_extent_ready = nullptr, push_msg_dir_order = nullptr;
+  cudaEvent_t push_msg_extent_ready[kLanes] = {}, push_msg_dir_order = nullptr;
 };
 
 static_assert(sizeof(rpl::StreamCounters) == sizeof(rpl_stream_counters) &&
@@ -1509,10 +1510,53 @@ rpl_result decode_assemble(rpl_ctx* c, cudaStream_t st, const WireChunk& w, uint
   return RPL_RESULT_OK;
 }
 
-// A message push's chunk (rpl_capsule_stream_push_laserscan_msgs*): where its messages and tables go, every table at
-// the chunk's first slot (stream).
+// The cloud chain over the scans `a` of one chunk: its nodes, views, counts, nodes_total, n_scans and stride set (a
+// push's chunk as its assembler left it, or last_push_scans); xyzi / point_counts point at the chunk's first slot;
+// lidars: RPL_CLOUD_PER_STREAM's table at the chunk's first stream, lidar_scans slots per stream (else nullptr).
+// Flags 0: the shared-memory kernel with SOR / voxel grid fused, its arrays sized for at most kSmallPostMaxNodes nodes
+// (a longer view goes to the general kernel, then to the post passes restricted to the hand-off list);
+// RPL_CLOUD_NO_FUSED: the shared-memory kernel's window + xyz, then the post passes over every scan.
+rpl_result stream_cloud_chunk(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, const rpl::LidarSettings* lidars,
+                              uint32_t lidar_scans, const rpl_cloud_params* p, float* xyzi, uint32_t* point_counts,
+                              cudaStream_t st) {
+  a.beam_counts = point_counts;
+  a.fallback_list = l.fallback_list;
+  a.fallback_count = l.fallback_count;
+  a.is_new_protocol = p->is_new_protocol;
+  a.xyzi = reinterpret_cast<float4*>(xyzi);
+  a.trig = c->lane[0].cws.trig;
+  a.angle = c->lane[0].cws.angle;
+  a.range_min = p->range_min;
+  a.range_max = p->range_max;
+  a.intensity_min = p->intensity_min;
+  if ((p->flags & RPL_CLOUD_PER_STREAM) != 0) {  // each stream's is_new_protocol (the window's intensity too)
+    a.lidars = lidars;
+    a.lidar_scans = lidar_scans;
+  }
+  const bool separate = (p->flags & RPL_CLOUD_NO_FUSED) != 0;
+  bool fused = false;
+  rpl_result r = scratch_enter(c, l, st);
+  if (r == RPL_RESULT_OK) r = enqueue_args(c, l, a, 0u, st, separate ? nullptr : p, &fused, true);
+  if (r != RPL_RESULT_OK) return r;
+  if (p->sor_k > 0 || p->voxel_size > 0.0f) {
+    // the post passes read lane l's fallback list and run on lane 0's cws: a lane-1 chunk takes lane 0's scratch too
+    Lane& post = c->lane[0];
+    if (&l != &post && (r = scratch_enter(c, post, st)) != RPL_RESULT_OK) return r;
+    int launched = 0;
+    RPL_CUDA(c, rpl::launch_cloud_post(a.xyzi, point_counts, a.n_scans, a.stride, p->sor_k, p->sor_alpha, p->voxel_size,
+                                       post.cws, fused ? a.fallback_list : nullptr, fused ? a.fallback_count : nullptr,
+                                       st, &launched),
+             RPL_RESULT_OPERATION_FAIL);
+    c->launches += launched;
+    if (&l != &post && (r = scratch_leave(c, post, st)) != RPL_RESULT_OK) return r;
+  }
+  return scratch_leave(c, l, st);
+}
+
+// A message push's chunk (rpl_capsule_stream_push_{laserscan,cloud}_msgs*): where its messages and tables go, every
+// table at the chunk's first slot (stream).
 struct ChunkMsgs {
-  uint8_t* out;                      // message i at out + place[i] - header - 32
+  uint8_t* out;                      // LaserScan message i at out + place[i] - header - 32
   bool first, rebase;                // PushMsgDirArgs::first, rebase
   unsigned long long capacity;
   unsigned long long *carry, *offsets, *place, *extent, *total;  // PushMsgDirArgs (extent, total nullable)
@@ -1523,14 +1567,50 @@ struct ChunkMsgs {
   // across the lanes (the previous chunk's directory recorded it)
   unsigned long long* extent_host;
   cudaEvent_t extent_ready, dir_order;
+  // a PointCloud2 push's: the cloud chain's parameters and its clouds and point counts of the chunk's slots; message i
+  // at out + offsets[i] - the base its writer is given (cloud_push_write)
+  const rpl_cloud_params* cloud;
+  float* xyzi;
+  uint32_t* points;
 };
+
+rpl::CloudTail cloud_tail();
+
+// A PointCloud2 push's messages of the chunk of ns streams m describes, once its directory has sized and placed them:
+// pointcloud2_msgs_kernel writes message i at m.out + m.offsets[i] - out_base, stamped with the slot stamps of the
+// stamped assembler (0 for an unstamped push), as msgs_write does for the last push's
+rpl_result cloud_push_write(rpl_ctx* c, const WireChunk& w, uint32_t ns, bool stamped, const ChunkMsgs& m,
+                            unsigned long long out_base, cudaStream_t st) {
+  rpl::MsgWriteArgs a{};
+  a.hdr = m.hdr;
+  if (stamped) {
+    a.begin_us = w.slot_begin;
+    a.end_us = w.slot_end;
+  }
+  a.clock_offset_ns = m.clock_offset_ns;
+  a.counts = m.points;
+  a.xyzi = m.xyzi;
+  a.stride = w.max_nodes;
+  a.max_scans = w.max_scans;
+  a.n = ns * w.max_scans;
+  a.offsets = m.offsets;
+  a.sizes = m.sizes;
+  a.out = m.out;
+  a.out_base = out_base;
+  static const rpl::CloudTail tail = cloud_tail();
+  RPL_CUDA(c, rpl::launch_pointcloud2_msgs(a, tail, w.max_nodes, st), RPL_RESULT_OPERATION_FAIL);
+  c->launches += (a.n + 65534) / 65535;
+  return RPL_RESULT_OK;
+}
 
 // (frame ->) decode -> assemble -> scan kernels for the ns streams of chunk w on `st`; capsules / counts / outputs / sp
 // point at the chunk's first stream's (a byte session's capsules / counts: the raw bytes and byte counts).  A mixed
 // byte session's chunk runs the first three for each answer type present in it, over that type's streams, and the scan
 // kernels, which read the arenas whatever the type, once.
 // m (a message push): the directory runs between the assembler and the scan kernels, which write into the placed
-// messages instead of ranges / intens (null), and the header writer behind them.
+// messages instead of ranges / intens (null), and the header writer behind them.  A PointCloud2 push (m->cloud) runs
+// the cloud chain over the chunk's fresh views instead of the scan kernels, then the directory, which sizes each
+// message by its cloud, then (the device form; the host form's waits for the extent, push_host) the writer.
 rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const WireChunk& w, uint32_t ns,
                                 const uint8_t* capsules, const uint32_t* counts, uint32_t sample_duration_us,
                                 const rpl_scan_params* params, float* ranges, float* intens, uint32_t* beams,
@@ -1554,6 +1634,18 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
   if (!m)
     return enqueue_scan(c, l, w.nodes, w.scan_len, ns * w.max_scans, w.max_nodes, params, nullptr, ranges, intens, beams,
                         inc, nullptr, nullptr, st, views, (unsigned long long)ns * w.stride_nodes, lt);
+  if (m->cloud) {  // the scans as last_push_scans will give them once the push is done
+    rpl::ScanBatchArgs a{};
+    a.nodes = reinterpret_cast<const uint2*>(w.nodes);
+    a.views = views;
+    a.counts = reinterpret_cast<const uint32_t*>(views);
+    a.nodes_total = (unsigned long long)ns * w.stride_nodes;
+    a.n_scans = ns * w.max_scans;
+    a.stride = w.max_nodes;
+    r = stream_cloud_chunk(c, l, a, w.lidars, w.max_scans, m->cloud, m->xyzi, m->points, st);
+    if (r != RPL_RESULT_OK) return r;
+  }
+  const rpl::MsgKind kind = m->cloud ? rpl::MsgKind::kPointCloud2 : rpl::MsgKind::kLaserScan;
   rpl::PushMsgDirArgs d{};
   d.views = views;
   d.scans_per_stream = scans_per_stream;
@@ -1568,14 +1660,17 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
   d.place = m->place;
   d.extent = m->extent;
   d.total = m->total;
+  d.counts = m->points;
+  d.sizes = m->cloud ? m->sizes : nullptr;
   if (m->dir_order) RPL_CUDA(c, cudaStreamWaitEvent(st, m->dir_order, 0), RPL_RESULT_OPERATION_FAIL);
-  RPL_CUDA(c, rpl::launch_push_msg_dir(d, st), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, rpl::launch_push_msg_dir(d, kind, st), RPL_RESULT_OPERATION_FAIL);
   c->launches++;
   if (m->dir_order) RPL_CUDA(c, cudaEventRecord(m->dir_order, st), RPL_RESULT_OPERATION_FAIL);
   if (m->extent_host) {
     RPL_CUDA(c, cudaMemcpyAsync(m->extent_host, m->extent, 3 * 8, cudaMemcpyDeviceToHost, st), RPL_RESULT_OPERATION_FAIL);
     RPL_CUDA(c, cudaEventRecord(m->extent_ready, st), RPL_RESULT_OPERATION_FAIL);
   }
+  if (m->cloud) return m->extent_host ? RPL_RESULT_OK : cloud_push_write(c, w, ns, sp != nullptr, *m, 0, st);
   r = enqueue_scan(c, l, w.nodes, w.scan_len, ns * w.max_scans, w.max_nodes, params, nullptr, nullptr, nullptr, beams,
                    inc, nullptr, nullptr, st, views, (unsigned long long)ns * w.stride_nodes, lt, m->out, m->place);
   if (r != RPL_RESULT_OK) return r;
@@ -1624,14 +1719,20 @@ struct HostMsgs {
   size_t chunk_bytes;  // staging for one chunk's messages: the bound of its slots at max_nodes
   long long clock_offset_ns;
   const rpl::StreamMsgHeader* hdr;  // the session's, [n_streams]
-  unsigned long long *carry, *place, *extent_host;
-  cudaEvent_t extent_ready, dir_order;
+  unsigned long long *carry, *place;
+  unsigned long long* extent_host;  // [kLanes][3] pinned, and extent_ready[kLanes]: each lane's chunk's
+  const cudaEvent_t* extent_ready;
+  cudaEvent_t dir_order;
+  const rpl_cloud_params* cloud;    // a PointCloud2 push
 };
 
 // Runs a host call's n_streams streams through capsule_stream_chunk, `chunk` streams at a time round-robin over the
 // lanes: H2D of a chunk's input (and receive times), its kernels, D2H of its LaserScans (and stamps).  A message push
 // (h.msgs) stages the chunk's messages instead: once its directory's extent is read back (the chunk's scan kernels run
-// meanwhile), the stretch of the packed buffer the chunk fills is copied to msgs, with the chunk's tables.  A lane's
+// meanwhile), the stretch of the packed buffer the chunk fills is copied to msgs, with the chunk's tables.  A
+// PointCloud2 push's directory follows the chunk's cloud kernels, so the host reads a chunk's extent only once the next
+// chunk is queued on the other lane (finish_cloud), then queues the writer, which packs the chunk's messages from the
+// stretch's first offset on, and the copies.  A lane's
 // staging block holds one chunk's input and outputs, then whatever chunk_at(k, s0) carves off k for the device state
 // of the chunk from stream s0, which it returns (the chain's lives there; a session's in its arenas).
 template <class ChunkAt>
@@ -1651,17 +1752,48 @@ rpl_result push_host(rpl_ctx* c, const HostWire& h, uint32_t n_streams, uint32_t
     u64* offs;
     uint32_t* sizes;
     u64* extent;
+    float* xyzi;  // a PointCloud2 push's: the chunk's clouds and point counts
+    uint32_t* points;
     WireChunk w;
   };
+  const bool cloud = hm && hm->cloud;
   auto layout = [&](Carve& k, uint32_t s0) {
     return Regions{k.take<uint8_t>(chunk * h.in_stream), k.take<uint32_t>(chunk),
                    k.take<u64>(h.sp ? chunk * h.rx_stream : 0), k.take<float>(rows), k.take<float>(rows),
                    k.take<float>(NS), k.take<uint32_t>(NS), k.take<uint32_t>(chunk), k.take<u64>(h.sp ? NS : 0),
                    k.take<uint8_t>(hm ? hm->chunk_bytes : 0), k.take<u64>(hm ? NS : 0), k.take<uint32_t>(hm ? NS : 0),
-                   k.take<u64>(hm ? 3 : 0), chunk_at(k, s0)};
+                   k.take<u64>(hm ? 3 : 0), k.take<float>(cloud ? NS * h.max_nodes * 4 : 0),
+                   k.take<uint32_t>(cloud ? NS : 0), chunk_at(k, s0)};
   };
   if (const rpl_result r = grow_stage(c, kLanes, [&](Carve& k) { layout(k, 0); }); r != RPL_RESULT_OK) return r;
   const cudaMemcpyKind h2d = cudaMemcpyHostToDevice, d2h = cudaMemcpyDeviceToHost;
+  // a PointCloud2 push's chunk whose kernels are queued and whose writer and copies are not
+  struct Queued {
+    Lane* l = nullptr;
+    uint32_t s0, ns;
+    Regions d;
+    ChunkMsgs m;
+  } queued;
+  auto finish_cloud = [&]() -> rpl_result {
+    if (!queued.l) return RPL_RESULT_OK;
+    const Queued q = queued;
+    queued.l = nullptr;
+    const int li = (int)(q.l - c->lane);
+    const size_t so = (size_t)q.s0 * h.max_scans, nsc = (size_t)q.ns * h.max_scans;
+    RPL_CUDA(c, cudaEventSynchronize(hm->extent_ready[li]), RPL_RESULT_OPERATION_FAIL);
+    const u64 lo = q.m.extent_host[0], hi = q.m.extent_host[1];
+    if (q.s0 + q.ns == n_streams) *hm->total = q.m.extent_host[2];
+    if (const rpl_result r = cloud_push_write(c, q.d.w, q.ns, h.sp != nullptr, q.m, lo, q.l->stream);
+        r != RPL_RESULT_OK)
+      return r;
+    if (hi > lo)
+      RPL_CUDA(c, cudaMemcpyAsync(hm->msgs + lo, q.d.msgs, hi - lo, d2h, q.l->stream), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(hm->offsets + so, q.d.offs, nsc * 8, d2h, q.l->stream), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(hm->sizes + so, q.d.sizes, nsc * 4, d2h, q.l->stream), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(h.scans_per_stream + q.s0, q.d.sps, (size_t)q.ns * 4, d2h, q.l->stream),
+             RPL_RESULT_OPERATION_FAIL);
+    return RPL_RESULT_OK;
+  };
   auto run_chunk = [&](Lane& l, uint32_t s0, uint32_t ns) -> rpl_result {
     Carve k{l.stage};
     const Regions d = layout(k, s0);
@@ -1691,19 +1823,28 @@ rpl_result push_host(rpl_ctx* c, const HostWire& h, uint32_t n_streams, uint32_t
       m.sizes = d.sizes;
       m.hdr = hm->hdr + s0;
       m.clock_offset_ns = hm->clock_offset_ns;
-      m.extent_host = hm->extent_host;
-      m.extent_ready = hm->extent_ready;
+      const int li = (int)(&l - c->lane);
+      m.extent_host = hm->extent_host + 3 * li;
+      m.extent_ready = hm->extent_ready[li];
       m.dir_order = hm->dir_order;
+      m.cloud = hm->cloud;
+      m.xyzi = d.xyzi;
+      m.points = d.points;
     }
     const rpl_result r = capsule_stream_chunk(c, l, l.stream, d.w, ns, d.in, d.counts, h.sample_duration_us, h.params,
                                               d.ranges, d.intens, d.beams, d.inc, d.sps, h.sp ? &sp : nullptr,
                                               hm ? &m : nullptr);
     if (r != RPL_RESULT_OK) return r;
+    if (cloud) {  // this chunk runs while the host waits for the previous one's extent
+      const rpl_result f = finish_cloud();
+      queued = Queued{&l, s0, ns, d, m};
+      return f;
+    }
     if (hm) {
       // the chunk's stretch [first offset, end of its last message that fits): known once its directory has run
-      RPL_CUDA(c, cudaEventSynchronize(hm->extent_ready), RPL_RESULT_OPERATION_FAIL);
-      const u64 lo = hm->extent_host[0], hi = hm->extent_host[1];
-      if (s0 + ns == n_streams) *hm->total = hm->extent_host[2];
+      RPL_CUDA(c, cudaEventSynchronize(m.extent_ready), RPL_RESULT_OPERATION_FAIL);
+      const u64 lo = m.extent_host[0], hi = m.extent_host[1];
+      if (s0 + ns == n_streams) *hm->total = m.extent_host[2];
       if (hi > lo)
         RPL_CUDA(c, cudaMemcpyAsync(hm->msgs + lo, d.msgs, hi - lo, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
       RPL_CUDA(c, cudaMemcpyAsync(hm->offsets + so, d.offs, nsc * 8, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
@@ -1725,7 +1866,15 @@ rpl_result push_host(rpl_ctx* c, const HostWire& h, uint32_t n_streams, uint32_t
              RPL_RESULT_OPERATION_FAIL);
     return RPL_RESULT_OK;
   };
-  return run_chunks(c, n_streams, chunk, run_chunk);
+  rpl_result r = run_chunks(c, n_streams, chunk, run_chunk);
+  if (r == RPL_RESULT_OK && queued.l) {  // the last chunk of a PointCloud2 push
+    r = finish_cloud();
+    const std::string why = c->err;
+    const rpl_result s = rpl_ctx_synchronize(c);
+    if (r == RPL_RESULT_OK) return s;
+    c->err = why;
+  }
+  return r;
 }
 
 // The tables of a nodes call (rpl_capsule_stream_nodes*), the session's own: every slot's place for the kernels, the
@@ -1757,6 +1906,11 @@ bool lidars_ok(rpl_capsule_stream* cs) {
 LidarTable lidar_table(const rpl_capsule_stream* cs, bool per_stream, uint32_t s0) {
   if (!per_stream) return LidarTable{};
   return LidarTable{cs->lidars + s0, cs->max_scans, cs->lidar_modes};
+}
+
+// the table's entry of stream s0, nullptr before the first set_lidars
+const rpl::LidarSettings* lidars_at(const rpl_capsule_stream* cs, uint32_t s0) {
+  return cs->lidars ? cs->lidars + s0 : nullptr;
 }
 
 // a capsule answer type's decoder runs in the session's pushes (a mixed session's: any stream's)
@@ -2018,8 +2172,9 @@ bool push_kind_ok(rpl_capsule_stream* cs, bool bytes) {
   return false;
 }
 
-// The session's device tables of a message push, every slot's: the carry of the directories, each slot's place, the
-// scan kernels' beam counts and angle increments, and the stamped assembler's scan stamps
+// The session's device tables of a message push, every slot's: the carry of the directories (a PointCloud2 push's: the
+// running offset and the end of the last message), each slot's place, the scan kernels' beam counts and angle
+// increments, and the stamped assembler's scan stamps
 struct PushMsgWork {
   unsigned long long *carry, *place;
   uint32_t* beams;
@@ -2028,7 +2183,7 @@ struct PushMsgWork {
 };
 PushMsgWork push_msg_work_layout(const rpl_capsule_stream* cs, Carve& k) {
   const size_t NS = (size_t)cs->n_streams * cs->max_scans;
-  return PushMsgWork{k.take<unsigned long long>(1), k.take<unsigned long long>(NS), k.take<uint32_t>(NS),
+  return PushMsgWork{k.take<unsigned long long>(2), k.take<unsigned long long>(NS), k.take<uint32_t>(NS),
                      k.take<float>(NS), k.take<unsigned long long>(NS)};
 }
 
@@ -2041,12 +2196,16 @@ struct PushMsgs {
   uint64_t* total;
   long long clock_offset_ns;
   PushMsgWork w;
+  // a PointCloud2 push's: the chain's parameters, and the device form's clouds and point counts of one chunk's slots
+  const rpl_cloud_params* cloud;
+  float* xyzi;
+  uint32_t* points;
 };
 
 // A push of the kind the entry point takes (bytes: a byte push); sp: a stamped one.  Host arrays (dev false, stream
 // unused) run in the session's host chunks round-robin over the lanes, device arrays in its device chunks on `stream`.
-// The arrays, sp's rx and scan_ts included, hold every stream.  pm: a message push, whose scans go into its messages
-// (ranges, intensities, beam_counts and angle_increment unused).
+// The arrays, sp's rx and scan_ts included, hold every stream.  pm: a message push, whose scans (pm->cloud: clouds) go
+// into its messages (ranges, intensities, beam_counts and angle_increment unused).
 rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t* counts, uint32_t sample_duration_us,
                        const rpl_scan_params* params, float* ranges, float* intensities, uint32_t* beam_counts,
                        float* angle_increment, uint32_t* scans_per_stream, const StampPush* sp, bool bytes, bool dev,
@@ -2086,6 +2245,9 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
         m.sizes = pm->sizes + so;
         m.hdr = cs->msg_hdr + s0;
         m.clock_offset_ns = pm->clock_offset_ns;
+        m.cloud = pm->cloud;
+        m.xyzi = pm->xyzi;
+        m.points = pm->points;
       }
       r = capsule_stream_chunk(c, c->lane[0], st, session_chunk(cs, s0, per_stream, true),
                                std::min(chunk, cs->n_streams - s0), in + s0 * cs->in_stream, counts + s0,
@@ -2106,10 +2268,12 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
     if (pm) {
       uint32_t hdr_most = 0;
       for (const rpl::StreamMsgHeader& e : cs->msg_hdr_host) hdr_most = std::max(hdr_most, e.bytes);
-      const size_t bound = ((size_t)hdr_most + 32 + 8 * (size_t)cs->max_nodes + 4 + 15) & ~(size_t)15;  // a message's
+      // a message's bytes at max_nodes, rounded up to 16 (PointCloud2: the tail, 16 B per point and is_dense)
+      const size_t n = cs->max_nodes, most = pm->cloud ? (size_t)hdr_most + 116 + 16 * n + 1 : hdr_most + 32 + 8 * n + 4;
+      const size_t bound = (most + 15) & ~(size_t)15;
       hm = HostMsgs{pm->msgs, pm->capacity, pm->offsets, pm->sizes, pm->total, (size_t)chunk * cs->max_scans * bound,
                     pm->clock_offset_ns, cs->msg_hdr, pm->w.carry, pm->w.place, cs->push_msg_extent,
-                    cs->push_msg_extent_ready, cs->push_msg_dir_order};
+                    cs->push_msg_extent_ready, cs->push_msg_dir_order, pm->cloud};
     }
     const HostWire h{in, counts, cs->in_stream, sample_duration_us, cs->max_nodes, cs->max_scans, params, ranges,
                      intensities, angle_increment, beam_counts, scans_per_stream, sp, sp ? sp->stride_chunks : 0u,
@@ -2152,49 +2316,6 @@ rpl::ScanBatchArgs last_push_scans(const rpl_capsule_stream* cs, uint32_t s0, ui
   a.n_scans = ns * cs->max_scans;
   a.stride = cs->max_nodes;
   return a;
-}
-
-// The cloud chain over the scans of one chunk of the session's last push (last_push_scans); xyzi / point_counts point
-// at the chunk's first slot.
-// Flags 0: the shared-memory kernel with SOR / voxel grid fused, its arrays sized for at most kSmallPostMaxNodes nodes
-// (a longer view goes to the general kernel, then to the post passes restricted to the hand-off list);
-// RPL_CLOUD_NO_FUSED: the shared-memory kernel's window + xyz, then the post passes over every scan.
-rpl_result stream_cloud_chunk(rpl_capsule_stream* cs, Lane& l, uint32_t s0, uint32_t ns, const rpl_cloud_params* p,
-                              float* xyzi, uint32_t* point_counts, cudaStream_t st) {
-  rpl_ctx* c = cs->c;
-  rpl::ScanBatchArgs a = last_push_scans(cs, s0, ns);
-  a.beam_counts = point_counts;
-  a.fallback_list = l.fallback_list;
-  a.fallback_count = l.fallback_count;
-  a.is_new_protocol = p->is_new_protocol;
-  a.xyzi = reinterpret_cast<float4*>(xyzi);
-  a.trig = c->lane[0].cws.trig;
-  a.angle = c->lane[0].cws.angle;
-  a.range_min = p->range_min;
-  a.range_max = p->range_max;
-  a.intensity_min = p->intensity_min;
-  if ((p->flags & RPL_CLOUD_PER_STREAM) != 0) {  // each stream's is_new_protocol (the window's intensity too)
-    a.lidars = cs->lidars + s0;
-    a.lidar_scans = cs->max_scans;
-  }
-  const bool separate = (p->flags & RPL_CLOUD_NO_FUSED) != 0;
-  bool fused = false;
-  rpl_result r = scratch_enter(c, l, st);
-  if (r == RPL_RESULT_OK) r = enqueue_args(c, l, a, 0u, st, separate ? nullptr : p, &fused, true);
-  if (r != RPL_RESULT_OK) return r;
-  if (p->sor_k > 0 || p->voxel_size > 0.0f) {
-    // the post passes read lane l's fallback list and run on lane 0's cws: a lane-1 chunk takes lane 0's scratch too
-    Lane& post = c->lane[0];
-    if (&l != &post && (r = scratch_enter(c, post, st)) != RPL_RESULT_OK) return r;
-    int launched = 0;
-    RPL_CUDA(c, rpl::launch_cloud_post(a.xyzi, point_counts, a.n_scans, a.stride, p->sor_k, p->sor_alpha, p->voxel_size,
-                                       post.cws, fused ? a.fallback_list : nullptr, fused ? a.fallback_count : nullptr,
-                                       st, &launched),
-             RPL_RESULT_OPERATION_FAIL);
-    c->launches += launched;
-    if (&l != &post && (r = scratch_leave(c, post, st)) != RPL_RESULT_OK) return r;
-  }
-  return scratch_leave(c, l, st);
 }
 
 bool stream_cloud_args_ok(rpl_capsule_stream* cs, const rpl_cloud_params* params, float* xyzi, uint32_t* point_counts) {
@@ -2248,8 +2369,9 @@ rpl_result stream_cloud_dev(rpl_capsule_stream* cs, const rpl_cloud_params* para
   return last_push_dev(cs, stream, 0, [&](cudaStream_t st) -> rpl_result {
     rpl_result r = RPL_RESULT_OK;
     for (uint32_t s0 = 0; s0 < cs->n_streams && r == RPL_RESULT_OK; s0 += cs->cloud_chunk)
-      r = stream_cloud_chunk(cs, cs->c->lane[0], s0, std::min(cs->cloud_chunk, cs->n_streams - s0), params,
-                             xyzi + (size_t)s0 * row, point_counts + (size_t)s0 * cs->max_scans, st);
+      r = stream_cloud_chunk(cs->c, cs->c->lane[0], last_push_scans(cs, s0, std::min(cs->cloud_chunk, cs->n_streams - s0)),
+                             lidars_at(cs, s0), cs->max_scans, params, xyzi + (size_t)s0 * row,
+                             point_counts + (size_t)s0 * cs->max_scans, st);
     return r;
   });
 }
@@ -2275,7 +2397,8 @@ rpl_result stream_cloud(rpl_capsule_stream* cs, const rpl_cloud_params* params, 
     Carve k{l.stage};
     const Regions d = layout(k);
     RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);  // the lane's previous chunk has left
-    const rpl_result r = stream_cloud_chunk(cs, l, s0, ns, params, d.xyzi, d.counts, l.stream);
+    const rpl_result r = stream_cloud_chunk(c, l, last_push_scans(cs, s0, ns), lidars_at(cs, s0), cs->max_scans, params,
+                                            d.xyzi, d.counts, l.stream);
     if (r != RPL_RESULT_OK) return r;
     RPL_CUDA(c, cudaMemcpyAsync(xyzi + (size_t)s0 * row, d.xyzi, ns * row * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
     RPL_CUDA(c, cudaMemcpyAsync(point_counts + (size_t)s0 * cs->max_scans, d.counts, (size_t)ns * cs->max_scans * 4, d2h,
@@ -2449,8 +2572,8 @@ rpl_result msgs_prepare(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* p
                        nullptr, nullptr, st, a.views, a.nodes_total,
                        lidar_table(cs, (p->flags & RPL_FLAG_PER_STREAM) != 0, s0));
     } else {
-      r = stream_cloud_chunk(cs, c->lane[0], s0, ns, static_cast<const rpl_cloud_params*>(params),
-                             w.data + so * row * 4, w.counts + so, st);
+      r = stream_cloud_chunk(c, c->lane[0], last_push_scans(cs, s0, ns), lidars_at(cs, s0), cs->max_scans,
+                             static_cast<const rpl_cloud_params*>(params), w.data + so * row * 4, w.counts + so, st);
     }
   }
   if (r != RPL_RESULT_OK) return r;
@@ -2619,12 +2742,17 @@ rpl_result stream_msgs(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* pa
       });
 }
 
-// ---- LaserScan messages from the push itself (DESIGN.md 5.7.1 "Messages from the push") ---------------------------
+// ---- messages from the push itself (DESIGN.md 5.7.1 "Messages from the push", "PointCloud2 messages from the push") --
 // The push of in's kind, each chunk's scans written straight into their messages: per chunk, after the assembler, the
 // directory places every slot behind the previous chunk's end; the scan kernels write each scan's arrays into its
 // message; the header writer fills in the rest.  The device form writes into the caller's buffer and tables; the host
 // form stages each chunk's messages on its lane and copies the stretch they fill.
-rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, const rpl_scan_params* params,
+// kind kPointCloud2 (params: rpl_cloud_params): per chunk, after the assembler, the cloud chain over the chunk's views
+// into a block of one chunk's clouds (the device form: the session's message work block; the host form: the lane's),
+// then the directory, which packs the messages exactly as msg_table_kernel does, then pointcloud2_msgs_kernel.  The
+// push decodes and stamps with RPL_FLAG_PER_STREAM when the cloud takes RPL_CLOUD_PER_STREAM: of rpl_scan_params only
+// that flag reaches the decoders, the assembler and the stamps.
+rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, rpl::MsgKind kind, const void* params,
                      int64_t clock_offset_ns, uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
                      uint64_t* total_bytes, uint32_t* scans_per_stream, bool dev, void* stream) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
@@ -2646,25 +2774,49 @@ rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, const rpl
              "aligned";
     return RPL_RESULT_INVALID_DATA;
   }
+  const bool cloud = kind == rpl::MsgKind::kPointCloud2;
+  const auto* cp = cloud ? static_cast<const rpl_cloud_params*>(params) : nullptr;
+  if (cloud && !cloud_params_ok(c, cp)) return RPL_RESULT_INVALID_DATA;
+  // a cloud push's: its decode, assemble and stamp settings (RPL_CLOUD_PER_STREAM before set_lidars fails the push's
+  // check of RPL_FLAG_PER_STREAM)
+  rpl_scan_params push_params{};
+  if (cloud && (cp->flags & RPL_CLOUD_PER_STREAM) != 0) push_params.flags = RPL_FLAG_PER_STREAM;
+  const auto* sp_params = cloud ? &push_params : static_cast<const rpl_scan_params*>(params);
   if (!cs->push_msg_work) {  // the first message push: the session's tables, made once (their size is fixed)
     RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
     Carve k;
     push_msg_work_layout(cs, k);
     RPL_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&cs->push_msg_work), k.bytes), RPL_RESULT_INSUFFICIENT_MEMORY);
-    RPL_CUDA(c, cudaMallocHost(reinterpret_cast<void**>(&cs->push_msg_extent), 3 * 8), RPL_RESULT_INSUFFICIENT_MEMORY);
-    RPL_CUDA(c, cudaEventCreateWithFlags(&cs->push_msg_extent_ready, cudaEventDisableTiming), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMallocHost(reinterpret_cast<void**>(&cs->push_msg_extent), kLanes * 3 * 8),
+             RPL_RESULT_INSUFFICIENT_MEMORY);
+    for (cudaEvent_t& e : cs->push_msg_extent_ready)
+      RPL_CUDA(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming), RPL_RESULT_OPERATION_FAIL);
     RPL_CUDA(c, cudaEventCreateWithFlags(&cs->push_msg_dir_order, cudaEventDisableTiming), RPL_RESULT_OPERATION_FAIL);
   }
   Carve k{cs->push_msg_work};
-  const PushMsgs pm{msgs, capacity, msg_offsets, msg_sizes, total_bytes, clock_offset_ns, push_msg_work_layout(cs, k)};
+  PushMsgs pm{msgs, capacity, msg_offsets, msg_sizes, total_bytes, clock_offset_ns, push_msg_work_layout(cs, k), cp,
+              nullptr, nullptr};
+  if (cloud && dev) {  // one chunk's clouds, in the session's message work block (cloud_msgs' when that is larger)
+    const size_t NS = (size_t)cs->chunk_dev * cs->max_scans;
+    auto layout = [&](Carve& kw) {
+      pm.xyzi = kw.take<float>(NS * cs->max_nodes * 4);
+      pm.points = kw.take<uint32_t>(NS);
+    };
+    Carve kb;
+    layout(kb);
+    RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+    if (const rpl_result r = grow_msg_work(cs, kb.bytes); r != RPL_RESULT_OK) return r;
+    Carve kw{cs->msg_work};
+    layout(kw);
+  }
   StampPush sp{};
   const bool stamped = in->rx_us != nullptr;
   // (a stamped push's scan stamps stay on the device: the messages carry them)
-  if (stamped && !stamp_args_ok(cs, params, in->timing, in->rx_us, cs->bytes ? in->chunk_bytes : 1u,
+  if (stamped && !stamp_args_ok(cs, sp_params, in->timing, in->rx_us, cs->bytes ? in->chunk_bytes : 1u,
                                 reinterpret_cast<uint64_t*>(pm.w.ts), &sp))
     return RPL_RESULT_INVALID_DATA;
   const uint32_t sample_duration_us = stamped ? (in->timing ? in->timing->sample_duration_us : 0u) : in->sample_duration_us;
-  const rpl_result r = stream_push(cs, in->data, in->counts, sample_duration_us, params, nullptr, nullptr, nullptr,
+  const rpl_result r = stream_push(cs, in->data, in->counts, sample_duration_us, sp_params, nullptr, nullptr, nullptr,
                                    nullptr, scans_per_stream, stamped ? &sp : nullptr, cs->bytes, dev, stream, &pm);
   if (r != RPL_RESULT_OK) return r;
   if (!dev && *total_bytes > capacity) {
@@ -2919,7 +3071,8 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   cudaFree(cs->counters);
   cudaFree(cs->push_msg_work);
   cudaFreeHost(cs->push_msg_extent);
-  if (cs->push_msg_extent_ready) cudaEventDestroy(cs->push_msg_extent_ready);
+  for (cudaEvent_t e : cs->push_msg_extent_ready)
+    if (e) cudaEventDestroy(e);
   if (cs->push_msg_dir_order) cudaEventDestroy(cs->push_msg_dir_order);
   if (cs->done) cudaEventDestroy(cs->done);
   delete cs;
@@ -3201,8 +3354,8 @@ rpl_result rpl_capsule_stream_push_laserscan_msgs(rpl_capsule_stream* s, const r
                                                   const rpl_scan_params* params, int64_t clock_offset_ns, uint8_t* msgs,
                                                   uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
                                                   uint64_t* total_bytes, uint32_t* scans_per_stream) {
-  return push_msgs(s, in, params, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes, total_bytes, scans_per_stream,
-                   false, nullptr);
+  return push_msgs(s, in, rpl::MsgKind::kLaserScan, params, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
+                   total_bytes, scans_per_stream, false, nullptr);
 }
 
 rpl_result rpl_capsule_stream_push_laserscan_msgs_dev(rpl_capsule_stream* s, const rpl_push_input* in,
@@ -3210,8 +3363,25 @@ rpl_result rpl_capsule_stream_push_laserscan_msgs_dev(rpl_capsule_stream* s, con
                                                       uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,
                                                       uint32_t* msg_sizes, uint64_t* total_bytes,
                                                       uint32_t* scans_per_stream, void* stream) {
-  return push_msgs(s, in, params, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes, total_bytes, scans_per_stream,
-                   true, stream);
+  return push_msgs(s, in, rpl::MsgKind::kLaserScan, params, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
+                   total_bytes, scans_per_stream, true, stream);
+}
+
+rpl_result rpl_capsule_stream_push_cloud_msgs(rpl_capsule_stream* s, const rpl_push_input* in,
+                                              const rpl_cloud_params* params, int64_t clock_offset_ns, uint8_t* msgs,
+                                              uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
+                                              uint64_t* total_bytes, uint32_t* scans_per_stream) {
+  return push_msgs(s, in, rpl::MsgKind::kPointCloud2, params, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
+                   total_bytes, scans_per_stream, false, nullptr);
+}
+
+rpl_result rpl_capsule_stream_push_cloud_msgs_dev(rpl_capsule_stream* s, const rpl_push_input* in,
+                                                  const rpl_cloud_params* params, int64_t clock_offset_ns,
+                                                  uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,
+                                                  uint32_t* msg_sizes, uint64_t* total_bytes,
+                                                  uint32_t* scans_per_stream, void* stream) {
+  return push_msgs(s, in, rpl::MsgKind::kPointCloud2, params, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
+                   total_bytes, scans_per_stream, true, stream);
 }
 
 rpl_result rpl_capsule_stream_cloud_msgs_dev(rpl_capsule_stream* s, const rpl_cloud_params* params,

@@ -129,6 +129,8 @@ typedef struct rpl_cloud_params {
                                  could fuse them (A/B measurements, second implementation for the tests) */
 #define RPL_CLOUD_PER_STREAM 2u /* stream sessions: every stream's own is_new_protocol (rpl_capsule_stream_set_lidars) for
                                    the intensity and the intensity_min window; other calls ignore it */
+#define RPL_CLOUD_PER_STREAM_CHAIN 4u /* stream sessions: every stream's own chain (rpl_capsule_stream_set_clouds) in
+                                         place of this struct's range_min .. sor_alpha; other calls ignore it */
 
 typedef struct rpl_ctx rpl_ctx;
 
@@ -910,6 +912,40 @@ typedef struct rpl_lidar_settings {
   rpl_timing timing;       /* sample_duration_us must be in [1, 1000000] */
 } rpl_lidar_settings;
 rpl_result rpl_capsule_stream_set_lidars(rpl_capsule_stream* s, const rpl_lidar_settings* settings /* [n_streams] */,
+                                         const uint8_t* stream_mask /* nullable: all */);
+
+/* Per-stream clouds: each stream's PointCloud2 chain as its own node would run it (the NodeAccel parameters
+ * publish_pointcloud, cloud_range_min / cloud_range_max, cloud_intensity_min, cloud_voxel_size, cloud_sor_k,
+ * cloud_sor_alpha; INTEGRATION.md 4e), so that one session serves a fleet that mixes lidar models and cloud settings.
+ *   set_clouds: synchronous (it waits for the session's device calls in flight).  Copies settings[s] for every stream
+ *            whose stream_mask entry is non-zero (NULL = all); the first call must set every stream.  A null settings,
+ *            a first call that leaves a stream out, or a masked entry that breaks the chain's rules (sor_k > 32; a
+ *            voxel grid with voxel_size < 1e-6 or range_max >= 1000): RPL_RESULT_INVALID_DATA, and the table is
+ *            unchanged.
+ *   range_max 0: the stream's range_max of rpl_capsule_stream_set_frames, as it is when a cloud call is made (a
+ *            set_frames in between moves the window).  A call whose resolved entry breaks the voxel rule:
+ *            RPL_RESULT_INVALID_DATA.
+ *   RPL_CLOUD_PER_STREAM_CHAIN in rpl_cloud_params.flags (cloud[_dev], cloud_msgs[_dev], push_cloud_msgs[_dev]): stream
+ *            s takes range_min, range_max, intensity_min, voxel_size, sor_k and sor_alpha from its entry, and the call's
+ *            own values of these six are ignored.  It combines with RPL_CLOUD_PER_STREAM (which still decides
+ *            is_new_protocol) and RPL_CLOUD_NO_FUSED.  Before the first set_clouds: RPL_RESULT_INVALID_DATA.
+ *   Definition: for an enabled stream every output of a flagged call -- point counts, xyzi rows, message sizes and
+ *            bytes -- is bit for bit what a session of that stream alone gives on the same pieces with uniform
+ *            rpl_cloud_params equal to its resolved entry.  A disabled stream (enabled 0) has point count 0 and its
+ *            rows are not written (cloud[_dev]), and no message, size 0, as an unused slot (the message calls); its
+ *            scans are not read.  A push still decodes, assembles and stamps it, so counters, carries and later calls
+ *            are unchanged. */
+typedef struct rpl_cloud_settings {
+  float range_min;
+  float range_max;      /* 0: the stream's range_max of rpl_capsule_stream_set_frames */
+  float intensity_min;
+  float voxel_size;     /* 0: no voxel grid */
+  uint32_t sor_k;       /* 0: no statistical outlier removal; <= 32 */
+  float sor_alpha;
+  uint8_t enabled;      /* 0: this stream publishes no cloud */
+  uint8_t pad[3];
+} rpl_cloud_settings;   /* 28 bytes; the first 24 are laid out as in rpl_cloud_params */
+rpl_result rpl_capsule_stream_set_clouds(rpl_capsule_stream* s, const rpl_cloud_settings* settings /* [n_streams] */,
                                          const uint8_t* stream_mask /* nullable: all */);
 
 /* ---- LaserScan / PointCloud2 -> wire (SURVEY.md 8(f) rank 3) ---------------------------- */

@@ -28,6 +28,7 @@ FLAG_NO_SMALL = 4
 FLAG_PER_STREAM = 8
 CLOUD_NO_FUSED = 1
 CLOUD_PER_STREAM = 2
+CLOUD_PER_STREAM_CHAIN = 4
 CAPSULE_OK, CAPSULE_SYNC, CAPSULE_EMIT, CAPSULE_DISCARD = 1, 2, 4, 8
 CAPSULE_CHECKSUM_ERR, CAPSULE_ENCODER_RESET_ERR, CAPSULE_BAD_FRAME = 16, 32, 64
 PATH_FAST, PATH_GENERAL = 0, 1
@@ -57,7 +58,7 @@ EXPORTS = [
     "rpl_capsule_stream_create_bytes_mixed", "rpl_capsule_stream_set_answer_types",
     "rpl_capsule_stream_push_bytes_ts", "rpl_capsule_stream_push_bytes_ts_dev",
     "rpl_capsule_stream_cloud", "rpl_capsule_stream_cloud_dev", "rpl_capsule_stream_set_frames",
-    "rpl_capsule_stream_set_lidars", "rpl_capsule_stream_laserscan_msgs", "rpl_capsule_stream_laserscan_msgs_dev",
+    "rpl_capsule_stream_set_lidars", "rpl_capsule_stream_set_clouds", "rpl_capsule_stream_laserscan_msgs", "rpl_capsule_stream_laserscan_msgs_dev",
     "rpl_capsule_stream_cloud_msgs", "rpl_capsule_stream_cloud_msgs_dev", "rpl_capsule_stream_nodes",
     "rpl_capsule_stream_nodes_dev", "rpl_capsule_stream_push_laserscan_msgs", "rpl_capsule_stream_push_laserscan_msgs_dev",
     "rpl_capsule_stream_push_cloud_msgs", "rpl_capsule_stream_push_cloud_msgs_dev",
@@ -116,6 +117,21 @@ class CloudParams(C.Structure):
         ("is_new_protocol", C.c_uint8),
         ("flags", C.c_uint8),
         ("pad", C.c_uint8 * 2),
+    ]
+
+
+class CloudSettings(C.Structure):
+    """rpl_cloud_settings: one stream's PointCloud2 chain (its node's publish_pointcloud and cloud_* parameters); the
+    first 24 bytes are laid out as in CloudParams."""
+    _fields_ = [
+        ("range_min", C.c_float),
+        ("range_max", C.c_float),
+        ("intensity_min", C.c_float),
+        ("voxel_size", C.c_float),
+        ("sor_k", C.c_uint32),
+        ("sor_alpha", C.c_float),
+        ("enabled", C.c_uint8),
+        ("pad", C.c_uint8 * 3),
     ]
 
 
@@ -242,6 +258,7 @@ def lib() -> C.CDLL:
         "rpl_capsule_stream_cloud_dev": ([vp, PCP, vp, vp, vp], u32),
         "rpl_capsule_stream_set_frames": ([vp, vp, vp], u32),
         "rpl_capsule_stream_set_lidars": ([vp, vp, vp], u32),
+        "rpl_capsule_stream_set_clouds": ([vp, vp, vp], u32),
         "rpl_capsule_stream_laserscan_msgs": ([vp, PSP, C.c_int64, vp, u64, vp, vp, vp], u32),
         "rpl_capsule_stream_laserscan_msgs_dev": ([vp, PSP, C.c_int64, vp, u64, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_cloud_msgs": ([vp, PCP, C.c_int64, vp, u64, vp, vp, vp], u32),
@@ -277,6 +294,13 @@ def cloud_params(range_min=0.15, range_max=40.0, intensity_min=0.0, voxel_size=0
                  sor_alpha=1.0, is_new_protocol=0, flags=0) -> CloudParams:
     return CloudParams(float(range_min), float(range_max), float(intensity_min), float(voxel_size),
                        int(sor_k), float(sor_alpha), int(is_new_protocol), int(flags), (C.c_uint8 * 2)(0, 0))
+
+
+def cloud_settings(range_min=0.15, range_max=0.0, intensity_min=0.0, voxel_size=0.0, sor_k=0, sor_alpha=1.0,
+                   enabled=True) -> CloudSettings:
+    """range_max 0: the stream's range_max of set_frames."""
+    return CloudSettings(float(range_min), float(range_max), float(intensity_min), float(voxel_size), int(sor_k),
+                         float(sor_alpha), int(bool(enabled)), (C.c_uint8 * 3)(0, 0, 0))
 
 
 def _timing(t):
@@ -743,6 +767,16 @@ class CapsuleStreamSession:
         m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
         assert m is None or m.shape == (self.n_streams,)
         self._ctx._check(self._fn("set_lidars")(self._h, C.cast(arr, C.c_void_p), _p(m)))
+
+    def set_clouds(self, settings, mask=None):
+        """Per stream the PointCloud2 chain (n_streams CloudSettings, see cloud_settings) that cloud calls with
+        CLOUD_PER_STREAM_CHAIN use instead of their params' window, SOR and voxel grid.  Only the entries where mask is
+        true are copied (None: all); the first call must set every stream."""
+        assert len(settings) == self.n_streams
+        arr = (CloudSettings * self.n_streams)(*settings)
+        m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
+        assert m is None or m.shape == (self.n_streams,)
+        self._ctx._check(self._fn("set_clouds")(self._h, C.cast(arr, C.c_void_p), _p(m)))
 
     def _msgs(self, name, params, clock_offset_ns, msgs, packed):
         ns = self.n_streams * self.max_scans

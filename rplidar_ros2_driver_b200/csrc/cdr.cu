@@ -111,7 +111,9 @@ __global__ void __launch_bounds__(MT) msg_table_kernel(MsgTableArgs a) {
   unsigned long long carry = 0;
   auto size_of = [&](uint32_t i) -> uint32_t {
     const uint32_t n = a.counts[i];
-    const bool has = a.kind == MsgKind::kLaserScan ? n > 0 : a.views[i].y > 0;
+    const bool has = a.kind == MsgKind::kLaserScan
+                         ? n > 0
+                         : a.views[i].y > 0 && !(a.clouds && a.clouds[i / a.max_scans].route == kCloudOff);
     return has ? msg_bytes(a.kind, a.hdr[i / a.max_scans].bytes, n) : 0u;
   };
   for (uint32_t t0 = 0; t0 < a.n_slots; t0 += MT) {
@@ -281,7 +283,8 @@ __global__ void __launch_bounds__(MT) push_msg_dir_kernel(PushMsgDirArgs a) {
     if (i < a.n_slots) {
       const uint32_t s = i / a.max_scans, k = i - s * a.max_scans;
       hb = a.hdr[s].bytes;
-      if (k < min(a.scans_per_stream[s], a.max_scans)) {
+      const bool off = kCloud && a.clouds && a.clouds[s].route == kCloudOff;  // a stream without a cloud
+      if (k < min(a.scans_per_stream[s], a.max_scans) && !off) {
         if constexpr (kCloud) bound = msg_bytes(K, hb, a.counts[i]);
         else bound = (msg_bytes(K, hb, a.views[i].y) + 15u) & ~15u;
       }

@@ -79,6 +79,7 @@ struct MsgTableArgs {
   unsigned long long* offsets;     // [n_slots] out: exclusive scan of the sizes rounded up to 16
   uint32_t* sizes;                 // [n_slots] out: message bytes, 0 for no message or when the total exceeds capacity
   unsigned long long* total;       // out: end of the last message
+  const CloudSettings* clouds;     // [n_slots / max_scans] nullable, PointCloud2: a kCloudOff stream's slots have none
 };
 
 // the writers, over slots [slot0, slot0 + n) (slot indices count from the first slot of the call)
@@ -127,6 +128,7 @@ struct PushMsgDirArgs {
                                     // PointCloud2: the end of the last message (msg_table_kernel's total)
   const uint32_t* counts;           // [n_slots] PointCloud2: the clouds' point counts
   uint32_t* sizes;                  // [n_slots] out, PointCloud2: the message's bytes when it fits, else 0
+  const CloudSettings* clouds;      // [n_slots / max_scans] nullable, PointCloud2: a kCloudOff stream's slots have none
 };
 cudaError_t launch_push_msg_dir(const PushMsgDirArgs& a, MsgKind kind, cudaStream_t stream);
 // The fixed part of every placed message of slots [0, a.n) once the scan kernels have written its arrays (a's hdr,

@@ -82,7 +82,8 @@ template <int K>
 __global__ void __launch_bounds__(CT) cloud_sor_kernel(float4* xyzi, uint32_t* point_counts, uint32_t n_scans,
                                                        uint32_t stride, uint32_t sor_k, float sor_alpha,
                                                        void* scratch, size_t per_cta, uint32_t max_nodes,
-                                                       const uint32_t* list, const uint32_t* list_count) {
+                                                       const uint32_t* list, const uint32_t* list_count,
+                                                       CloudTable tab) {
   __shared__ float2 s_xy[CT + 2 * kHalfWindow];
   __shared__ uint32_t s_warp[CT / 32];
   __shared__ long long s_s1[CT / 32];
@@ -94,6 +95,14 @@ __global__ void __launch_bounds__(CT) cloud_sor_kernel(float4* xyzi, uint32_t* p
   const uint32_t n_work = list ? min(*list_count, n_scans) : n_scans;
   for (uint32_t sj = blockIdx.x; sj < n_work; sj += gridDim.x) {
     const uint32_t s = list ? list[sj] : sj;
+    uint32_t sor_k_s = sor_k;
+    float alpha = sor_alpha;
+    if (tab.at) {  // per-stream clouds: the scans of this pass's route that have the step, with their own k and alpha
+      const CloudSettings& cl = tab.at[s / tab.per];
+      if (cloud_route(cl, tab.launches) != tab.route || cl.sor_k == 0) continue;
+      sor_k_s = cl.sor_k;
+      alpha = cl.sor_alpha;
+    }
     float4* pts = xyzi + (size_t)s * stride;
     const uint32_t m = point_counts[s];
     if (m < 2 || m > max_nodes) continue;  // fewer than 2 points keep everything
@@ -145,7 +154,7 @@ __global__ void __launch_bounds__(CT) cloud_sor_kernel(float4* xyzi, uint32_t* p
           add(s_xy[tid + kHalfWindow + o]);
         }
       }
-      const uint32_t k = min(sor_k, nd);
+      const uint32_t k = min(sor_k_s, nd);
       float sum = 0.0f;
 #pragma unroll
       for (int t = 0; t < K; ++t)
@@ -179,7 +188,7 @@ __global__ void __launch_bounds__(CT) cloud_sor_kernel(float4* xyzi, uint32_t* p
       const double sq = __ddiv_rn(__dmul_rn((double)t1, (double)t1), dn);
       double var = __ddiv_rn(__dsub_rn((double)t2, sq), __dsub_rn(dn, 1.0));
       if (!(var > 0.0)) var = 0.0;
-      s_thr = __dadd_rn(mean, __dmul_rn((double)sor_alpha, __dsqrt_rn(var)));
+      s_thr = __dadd_rn(mean, __dmul_rn((double)alpha, __dsqrt_rn(var)));
     }
     __syncthreads();
     const double thr = s_thr;
@@ -217,7 +226,7 @@ __global__ void cloud_table_init_kernel(void* scratch, size_t per_cta, uint32_t 
 __global__ void __launch_bounds__(CT) cloud_voxel_kernel(float4* xyzi, uint32_t* point_counts, uint32_t n_scans,
                                                          uint32_t stride, float voxel, void* scratch, size_t per_cta,
                                                          uint32_t max_nodes, const uint32_t* list,
-                                                         const uint32_t* list_count) {
+                                                         const uint32_t* list_count, CloudTable tab) {
   __shared__ uint32_t s_warp[CT / 32];
   // the whole table (>= 2 * max_nodes slots) is clean on entry; a scan uses a prefix sized to its own
   // point count so that the slots all resident CTAs touch stay inside the L2
@@ -226,6 +235,12 @@ __global__ void __launch_bounds__(CT) cloud_voxel_kernel(float4* xyzi, uint32_t*
   const uint32_t n_work = list ? min(*list_count, n_scans) : n_scans;
   for (uint32_t sj = blockIdx.x; sj < n_work; sj += gridDim.x) {
     const uint32_t s = list ? list[sj] : sj;
+    float vox = voxel;
+    if (tab.at) {  // per-stream clouds: the scans of this pass's route that have a voxel grid, with their own size
+      const CloudSettings& cl = tab.at[s / tab.per];
+      if (cloud_route(cl, tab.launches) != tab.route || !(cl.voxel > 0.0f)) continue;
+      vox = cl.voxel;
+    }
     float4* pts = xyzi + (size_t)s * stride;
     const uint32_t m = point_counts[s];
     if (m == 0 || m > max_nodes) continue;
@@ -243,8 +258,8 @@ __global__ void __launch_bounds__(CT) cloud_voxel_kernel(float4* xyzi, uint32_t*
         const uint4 r = ld_hint_v4(pts + i, l2_policy_evict_first());
         p = make_float4(__uint_as_float(r.x), __uint_as_float(r.y), __uint_as_float(r.z), __uint_as_float(r.w));
       }
-      const int ix = __float2int_rd(__fdiv_rn(p.x, voxel));  // floorf(x / voxel)
-      const int iy = __float2int_rd(__fdiv_rn(p.y, voxel));
+      const int ix = __float2int_rd(__fdiv_rn(p.x, vox));  // floorf(x / voxel)
+      const int iy = __float2int_rd(__fdiv_rn(p.y, vox));
       // lanes past the end get the key no cell can have
       const unsigned long long key = valid ? (((unsigned long long)(uint32_t)ix << 32) | (uint32_t)iy) : kVoxelEmpty;
       const unsigned long long key_prev = __shfl_up_sync(0xffffffffu, key, 1);
@@ -456,7 +471,8 @@ void cloud_workspace_free(CloudWorkspace& ws) {
 
 cudaError_t launch_cloud_post(float4* xyzi, uint32_t* point_counts, uint32_t n_scans, uint32_t stride,
                               uint32_t sor_k, float sor_alpha, float voxel, const CloudWorkspace& ws,
-                              const uint32_t* list, const uint32_t* list_count, cudaStream_t stream, int* launched) {
+                              const uint32_t* list, const uint32_t* list_count, cudaStream_t stream, int* launched,
+                              const CloudTable& tab) {
   // with a list the work is a handful of scans: a small grid finds out on the device
   const int grid = list ? (int)min((uint32_t)ws.ctas, min(n_scans, 64u)) : (int)min((uint32_t)ws.ctas, n_scans);
   if (sor_k > 0) {
@@ -465,12 +481,12 @@ cudaError_t launch_cloud_post(float4* xyzi, uint32_t* point_counts, uint32_t n_s
     else if (sor_k <= 8) k = cloud_sor_kernel<8>;
     else if (sor_k <= 16) k = cloud_sor_kernel<16>;
     k<<<grid, CT, 0, stream>>>(xyzi, point_counts, n_scans, stride, sor_k, sor_alpha, ws.scratch, ws.scratch_per_cta,
-                               ws.max_nodes, list, list_count);
+                               ws.max_nodes, list, list_count, tab);
     if (launched) ++*launched;
   }
   if (voxel > 0.0f) {
     cloud_voxel_kernel<<<grid, CT, 0, stream>>>(xyzi, point_counts, n_scans, stride, voxel, ws.scratch,
-                                                ws.scratch_per_cta, ws.max_nodes, list, list_count);
+                                                ws.scratch_per_cta, ws.max_nodes, list, list_count, tab);
     if (launched) ++*launched;
   }
   return cudaGetLastError();

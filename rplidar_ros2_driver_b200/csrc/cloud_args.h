@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "lidar_args.h"
+
 namespace rpl {
 
 struct CloudWorkspace {
@@ -17,12 +19,21 @@ struct CloudWorkspace {
 cudaError_t cloud_configure();
 cudaError_t cloud_workspace_alloc(CloudWorkspace& ws, int num_sms, uint32_t max_nodes);
 void cloud_workspace_free(CloudWorkspace& ws);
+// Per-stream clouds (ScanBatchArgs::clouds) in a post pass: scan s is served iff cloud_route(at[s / per], launches)
+// == route and its entry has the step, which then takes its sor_k / sor_alpha / voxel from there.  at == nullptr:
+// every scan, with the pass's own parameters.
+struct CloudTable {
+  const CloudSettings* at;
+  uint32_t per, launches, route;
+};
 // steps 4-5 (SOR, voxel grid) over per-scan clouds already in angle order, in place.  list / list_count
 // (device, nullable): restrict the pass to these scans (what the shared-memory kernel of scan_small.cu
-// handed to the general kernel); the general path for revolutions above 4096 nodes.
+// handed to the general kernel); the general path for revolutions above 4096 nodes.  With tab.at: sor_k > 0 runs
+// the SOR pass at compile-time bound sor_k (the largest of the table), voxel > 0 the voxel pass.
 cudaError_t launch_cloud_post(float4* xyzi, uint32_t* point_counts, uint32_t n_scans, uint32_t stride,
                               uint32_t sor_k, float sor_alpha, float voxel, const CloudWorkspace& ws,
-                              const uint32_t* list, const uint32_t* list_count, cudaStream_t stream, int* launched);
+                              const uint32_t* list, const uint32_t* list_count, cudaStream_t stream, int* launched,
+                              const CloudTable& tab = CloudTable{});
 // fuse + all-gather through peer memory (NVLink P2P, CUDA IPC)
 constexpr uint32_t kMaxPeers = 16;
 constexpr uint32_t kPeerHeaderBytes = 256;

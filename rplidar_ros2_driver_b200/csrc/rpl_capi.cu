@@ -128,6 +128,14 @@ rpl_result launch_fast(rpl_ctx* c, Lane& l, const rpl::ScanBatchArgs& a, FastKer
     // SOR / voxel grid run inside the kernel when the 32-bit cell keys and accumulators are exact:
     // |cell index| < 32768 and voxel <= 4 m (scan_small.cu); otherwise as separate passes
     const bool fits = rpl::scan_small_post_applies(a.stride);
+    if (a.xyzi && a.clouds) {  // per-stream clouds: the launches a.cloud_launches names (stream_cloud_chunk)
+      RPL_CUDA(c, rpl::launch_scan_small(a, l.fws.max_nodes, 0u, 0.0f, 0.0f, c->num_sms, stream,
+                                         fits ? 0u : rpl::kSmallPostMaxNodes),
+               RPL_RESULT_OPERATION_FAIL);
+      if (post_fused) *post_fused = (a.cloud_launches & 2u) != 0;
+      c->launches += __builtin_popcount(a.cloud_launches);
+      return RPL_RESULT_OK;
+    }
     bool fuse = false;
     if (a.xyzi && cloud && (cloud->sor_k > 0 || cloud->voxel_size > 0.0f) && (fits || (hand_off && a.views)))
       fuse = cloud->voxel_size == 0.0f || (cloud->voxel_size <= 4.0f && a.range_max / cloud->voxel_size < 32000.0f);
@@ -196,8 +204,9 @@ rpl_result enqueue_args(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, uint32_t flag
     a.nodes_out = nullptr;
   }
   FastKernel k = pick_fast(a, flags);
-  // per-stream settings and placed messages are read by the shared-memory kernels and the general kernel only
-  if ((a.lidars || a.msg_out) && k != FastKernel::kSmall) k = FastKernel::kNone;
+  // per-stream settings, per-stream clouds and placed messages are read by the shared-memory kernels and the general
+  // kernel only
+  if ((a.lidars || a.msg_out || a.clouds) && k != FastKernel::kSmall) k = FastKernel::kNone;
   if (k != FastKernel::kNone) {
     RPL_CUDA(c, cudaMemsetAsync(l.fallback_count, 0, sizeof(uint32_t), stream), RPL_RESULT_OPERATION_FAIL);
     const rpl_result r = launch_fast(c, l, a, k, stream, cloud, post_fused, hand_off);
@@ -1265,6 +1274,15 @@ struct rpl_capsule_stream {
   rpl::LidarSettings* lidars = nullptr;         // [n_streams] device
   std::vector<rpl::LidarSettings> lidars_host;
   uint32_t lidar_modes = 0;                     // LidarTable::modes of the table
+  // the per-stream clouds (rpl_capsule_stream_set_clouds) that calls with RPL_CLOUD_PER_STREAM_CHAIN read: the entries
+  // as set (empty until the first call sets every stream), and the table resolved against the frames' range_max
+  // (clouds_resolve): on the device, the routes present (bit per rpl::CloudRoute), the largest sor_k and whether a
+  // voxel grid runs, and why a flagged call fails (empty: it does not)
+  std::vector<rpl_cloud_settings> clouds_host;
+  rpl::CloudSettings* clouds = nullptr;         // [n_streams] device
+  uint32_t cloud_routes = 0, cloud_sor_k = 0;
+  bool cloud_voxel = false;
+  std::string clouds_bad;
   unsigned char* node_work = nullptr;           // the tables of a nodes call (NodeWork)
   // [n_streams] device, zeroed at create: what every push decoded and lost (rpl_capsule_stream_counters); a stream's
   // record is written by the one CTA of each kernel that serves the stream
@@ -1293,6 +1311,14 @@ static_assert(sizeof(rpl::LidarSettings) == sizeof(rpl_lidar_settings) &&
                   sizeof(rpl::TimingDesc) == sizeof(rpl_timing),
               "rpl::LidarSettings must be rpl_lidar_settings byte for byte");
 
+static_assert(sizeof(rpl::CloudSettings) == sizeof(rpl_cloud_settings) &&
+                  offsetof(rpl::CloudSettings, voxel) == offsetof(rpl_cloud_settings, voxel_size) &&
+                  offsetof(rpl::CloudSettings, sor_k) == offsetof(rpl_cloud_settings, sor_k) &&
+                  offsetof(rpl::CloudSettings, sor_alpha) == offsetof(rpl_cloud_settings, sor_alpha) &&
+                  offsetof(rpl::CloudSettings, route) == offsetof(rpl_cloud_settings, enabled) &&
+                  offsetof(rpl_cloud_settings, sor_alpha) == offsetof(rpl_cloud_params, sor_alpha),
+              "rpl::CloudSettings must be laid out as rpl_cloud_settings, and its first 24 bytes as rpl_cloud_params");
+
 namespace {
 
 // a stamped push's receive times and stamp output (rx, scan_ts: of the first stream of the call they are passed to)
@@ -1302,6 +1328,20 @@ struct StampPush {
   uint32_t chunk_bytes, stride_chunks;  // a framed push's chunk_bytes is 1; stride_chunks: ceil(stride_in / chunk_bytes)
   unsigned long long* scan_ts;          // scan_begin_ts_us [.][max_scans]
 };
+
+// A cloud call's per-stream chains (RPL_CLOUD_PER_STREAM_CHAIN): the session's resolved table at the chunk's first
+// stream (nullptr before the first set_clouds) and what the whole table holds
+struct CloudChains {
+  const rpl::CloudSettings* at;
+  uint32_t routes;  // bit r: some stream has rpl::CloudRoute r
+  uint32_t sor_k;   // the largest sor_k of the streams with SOR
+  bool voxel;       // some stream has a voxel grid
+};
+
+// the per-stream chains from stream s0 on (at: nullptr before the first set_clouds)
+CloudChains chains_at(const rpl_capsule_stream* cs, uint32_t s0) {
+  return CloudChains{cs->clouds ? cs->clouds + s0 : nullptr, cs->cloud_routes, cs->cloud_sor_k, cs->cloud_voxel};
+}
 
 // Where a chunk of streams lives on the device between the kernels of capsule_stream_chunk, every pointer at the
 // chunk's first stream.  A session's chunk decodes behind node_first carry slots per stream (node_stride != 0),
@@ -1338,6 +1378,8 @@ struct WireChunk {
   // (a byte session's framer or 0x81 decoder counts the bytes)
   rpl::StreamCounters* counters;
   uint32_t counted_capsule_bytes;
+  // the session's per-stream chains, which a PointCloud2 push with RPL_CLOUD_PER_STREAM_CHAIN reads
+  CloudChains clouds;
 };
 
 // session cs's chunk from stream s0 in the push under way (arena cs->parity); per_stream: RPL_FLAG_PER_STREAM; dev: a
@@ -1391,6 +1433,7 @@ WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0, bool per_stre
     w.lidars = cs->lidars + s0;
     w.lidar_modes = cs->lidar_modes;
   }
+  w.clouds = chains_at(cs, s0);
   return w;
 }
 
@@ -1510,15 +1553,58 @@ rpl_result decode_assemble(rpl_ctx* c, cudaStream_t st, const WireChunk& w, uint
   return RPL_RESULT_OK;
 }
 
+// stream_cloud_chunk with RPL_CLOUD_PER_STREAM_CHAIN, `a` set up but for the table
+rpl_result stream_chains_chunk(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, const CloudChains& chains, bool separate,
+                               uint32_t* point_counts, cudaStream_t st) {
+  using rpl::kCloudFused;
+  using rpl::kCloudSeparate;
+  using rpl::kCloudWindow;
+  a.clouds = chains.at;
+  // the fused kernel runs when the call may fuse (flags 0's rule: shared-memory kernels, a view longer than its arrays
+  // handed on) and some stream is fusable; the window-only kernel for the other routes, and for the streams without a
+  // cloud when the fused kernel does not run
+  const bool fused = !separate && rpl::scan_small_applies(a.stride) &&
+                     (rpl::scan_small_post_applies(a.stride) || a.views) && (chains.routes & (1u << kCloudFused)) != 0;
+  const uint32_t separate_routes = (1u << kCloudSeparate) | (fused ? 0u : 1u << kCloudFused);
+  a.cloud_launches = fused ? 2u : 0u;
+  if (!fused || (chains.routes & ((1u << kCloudWindow) | separate_routes)) != 0) a.cloud_launches |= 1u;
+  bool post_fused = false;
+  rpl_result r = scratch_enter(c, l, st);
+  if (r == RPL_RESULT_OK) r = enqueue_args(c, l, a, 0u, st, nullptr, &post_fused, true);
+  if (r != RPL_RESULT_OK) return r;
+  const bool full = (chains.routes & separate_routes) != 0;  // the separate route's scans: every scan's pass
+  if ((full || post_fused) && (chains.sor_k > 0 || chains.voxel)) {
+    // (lane 0's cws and scratch, as below)
+    Lane& post = c->lane[0];
+    if (&l != &post && (r = scratch_enter(c, post, st)) != RPL_RESULT_OK) return r;
+    for (int pass = 0; pass < 2; ++pass) {
+      if (pass == 0 ? !full : !post_fused) continue;
+      const rpl::CloudTable tab{chains.at, a.lidar_scans, a.cloud_launches, pass == 0 ? kCloudSeparate : kCloudFused};
+      int launched = 0;
+      RPL_CUDA(c, rpl::launch_cloud_post(a.xyzi, point_counts, a.n_scans, a.stride, chains.sor_k, 0.0f,
+                                         chains.voxel ? 1.0f : 0.0f, post.cws, pass ? a.fallback_list : nullptr,
+                                         pass ? a.fallback_count : nullptr, st, &launched, tab),
+               RPL_RESULT_OPERATION_FAIL);
+      c->launches += launched;
+    }
+    if (&l != &post && (r = scratch_leave(c, post, st)) != RPL_RESULT_OK) return r;
+  }
+  return scratch_leave(c, l, st);
+}
+
 // The cloud chain over the scans `a` of one chunk: its nodes, views, counts, nodes_total, n_scans and stride set (a
 // push's chunk as its assembler left it, or last_push_scans); xyzi / point_counts point at the chunk's first slot;
-// lidars: RPL_CLOUD_PER_STREAM's table at the chunk's first stream, lidar_scans slots per stream (else nullptr).
+// lidars: RPL_CLOUD_PER_STREAM's table at the chunk's first stream, lidar_scans slots per stream (else nullptr);
+// chains: RPL_CLOUD_PER_STREAM_CHAIN's.
 // Flags 0: the shared-memory kernel with SOR / voxel grid fused, its arrays sized for at most kSmallPostMaxNodes nodes
 // (a longer view goes to the general kernel, then to the post passes restricted to the hand-off list);
 // RPL_CLOUD_NO_FUSED: the shared-memory kernel's window + xyz, then the post passes over every scan.
+// RPL_CLOUD_PER_STREAM_CHAIN: the same per stream, by route -- the fused kernel for the fusable streams (when the call
+// may fuse), the window-only kernel for the others; the post passes over every scan for the separate route, and
+// restricted to the hand-off list for the fused route.  Each kernel and pass serves only its route's scans.
 rpl_result stream_cloud_chunk(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, const rpl::LidarSettings* lidars,
-                              uint32_t lidar_scans, const rpl_cloud_params* p, float* xyzi, uint32_t* point_counts,
-                              cudaStream_t st) {
+                              const CloudChains& chains, uint32_t lidar_scans, const rpl_cloud_params* p, float* xyzi,
+                              uint32_t* point_counts, cudaStream_t st) {
   a.beam_counts = point_counts;
   a.fallback_list = l.fallback_list;
   a.fallback_count = l.fallback_count;
@@ -1529,11 +1615,10 @@ rpl_result stream_cloud_chunk(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, const r
   a.range_min = p->range_min;
   a.range_max = p->range_max;
   a.intensity_min = p->intensity_min;
-  if ((p->flags & RPL_CLOUD_PER_STREAM) != 0) {  // each stream's is_new_protocol (the window's intensity too)
-    a.lidars = lidars;
-    a.lidar_scans = lidar_scans;
-  }
+  a.lidar_scans = lidar_scans;
+  if ((p->flags & RPL_CLOUD_PER_STREAM) != 0) a.lidars = lidars;  // each stream's is_new_protocol (the window's too)
   const bool separate = (p->flags & RPL_CLOUD_NO_FUSED) != 0;
+  if ((p->flags & RPL_CLOUD_PER_STREAM_CHAIN) != 0) return stream_chains_chunk(c, l, a, chains, separate, point_counts, st);
   bool fused = false;
   rpl_result r = scratch_enter(c, l, st);
   if (r == RPL_RESULT_OK) r = enqueue_args(c, l, a, 0u, st, separate ? nullptr : p, &fused, true);
@@ -1642,7 +1727,7 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
     a.nodes_total = (unsigned long long)ns * w.stride_nodes;
     a.n_scans = ns * w.max_scans;
     a.stride = w.max_nodes;
-    r = stream_cloud_chunk(c, l, a, w.lidars, w.max_scans, m->cloud, m->xyzi, m->points, st);
+    r = stream_cloud_chunk(c, l, a, w.lidars, w.clouds, w.max_scans, m->cloud, m->xyzi, m->points, st);
     if (r != RPL_RESULT_OK) return r;
   }
   const rpl::MsgKind kind = m->cloud ? rpl::MsgKind::kPointCloud2 : rpl::MsgKind::kLaserScan;
@@ -1662,6 +1747,7 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
   d.total = m->total;
   d.counts = m->points;
   d.sizes = m->cloud ? m->sizes : nullptr;
+  if (m->cloud && (m->cloud->flags & RPL_CLOUD_PER_STREAM_CHAIN) != 0) d.clouds = w.clouds.at;
   if (m->dir_order) RPL_CUDA(c, cudaStreamWaitEvent(st, m->dir_order, 0), RPL_RESULT_OPERATION_FAIL);
   RPL_CUDA(c, rpl::launch_push_msg_dir(d, kind, st), RPL_RESULT_OPERATION_FAIL);
   c->launches++;
@@ -2304,6 +2390,21 @@ bool cloud_params_ok(rpl_ctx* c, const rpl_cloud_params* p) {
   return true;
 }
 
+// a cloud call's chain rules: its params', or with RPL_CLOUD_PER_STREAM_CHAIN those of the session's resolved table
+bool cloud_call_ok(rpl_capsule_stream* cs, const rpl_cloud_params* p) {
+  rpl_ctx* c = cs->c;
+  if ((p->flags & RPL_CLOUD_PER_STREAM_CHAIN) == 0) return cloud_params_ok(c, p);
+  if (cs->clouds_host.empty()) {
+    c->err = "per-stream clouds requested before rpl_capsule_stream_set_clouds set every stream";
+    return false;
+  }
+  if (!cs->clouds_bad.empty()) {
+    c->err = cs->clouds_bad;
+    return false;
+  }
+  return true;
+}
+
 // The scans of streams [s0, s0 + ns) of the session's last push, one chunk of that push, as the scan kernels read
 // them: the chunk's region of the push's arena, its slots' views (which count from node 0 of stream s0 there) and
 // the holder's capacity as the stride.
@@ -2324,7 +2425,7 @@ bool stream_cloud_args_ok(rpl_capsule_stream* cs, const rpl_cloud_params* params
     c->err = "null params, xyzi or point_counts";
     return false;
   }
-  if (!cloud_params_ok(c, params)) return false;
+  if (!cloud_call_ok(cs, params)) return false;
   if ((params->flags & RPL_CLOUD_PER_STREAM) != 0 && !lidars_ok(cs)) return false;
   if (cs->cloud_chunk == 0) {
     c->err = "no clouds to take: the session has not pushed yet, or its last push failed";
@@ -2370,7 +2471,7 @@ rpl_result stream_cloud_dev(rpl_capsule_stream* cs, const rpl_cloud_params* para
     rpl_result r = RPL_RESULT_OK;
     for (uint32_t s0 = 0; s0 < cs->n_streams && r == RPL_RESULT_OK; s0 += cs->cloud_chunk)
       r = stream_cloud_chunk(cs->c, cs->c->lane[0], last_push_scans(cs, s0, std::min(cs->cloud_chunk, cs->n_streams - s0)),
-                             lidars_at(cs, s0), cs->max_scans, params, xyzi + (size_t)s0 * row,
+                             lidars_at(cs, s0), chains_at(cs, s0), cs->max_scans, params, xyzi + (size_t)s0 * row,
                              point_counts + (size_t)s0 * cs->max_scans, st);
     return r;
   });
@@ -2397,8 +2498,8 @@ rpl_result stream_cloud(rpl_capsule_stream* cs, const rpl_cloud_params* params, 
     Carve k{l.stage};
     const Regions d = layout(k);
     RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);  // the lane's previous chunk has left
-    const rpl_result r = stream_cloud_chunk(c, l, last_push_scans(cs, s0, ns), lidars_at(cs, s0), cs->max_scans, params,
-                                            d.xyzi, d.counts, l.stream);
+    const rpl_result r = stream_cloud_chunk(c, l, last_push_scans(cs, s0, ns), lidars_at(cs, s0), chains_at(cs, s0),
+                                            cs->max_scans, params, d.xyzi, d.counts, l.stream);
     if (r != RPL_RESULT_OK) return r;
     RPL_CUDA(c, cudaMemcpyAsync(xyzi + (size_t)s0 * row, d.xyzi, ns * row * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
     RPL_CUDA(c, cudaMemcpyAsync(point_counts + (size_t)s0 * cs->max_scans, d.counts, (size_t)ns * cs->max_scans * 4, d2h,
@@ -2414,6 +2515,47 @@ rpl_result stream_cloud(rpl_capsule_stream* cs, const rpl_cloud_params* params, 
 // session's work block, the sizes and offsets pass over every slot, then the writers.  The device form writes every
 // message into the caller's buffer; the host form reads the tables back first and then writes and copies the
 // messages chunk by chunk over the lanes, so that only message bytes cross the link.
+
+// The device table of the per-stream clouds from the entries as set and the frames' range_max, with its summary: each
+// stream's route (the fusion guard of launch_fast at its resolved range_max) and why a flagged call would fail.  The
+// caller has passed cs->done.
+rpl_result clouds_resolve(rpl_capsule_stream* cs) {
+  rpl_ctx* c = cs->c;
+  std::vector<rpl::CloudSettings> t(cs->n_streams);
+  uint32_t routes = 0, sor_k = 0;
+  bool voxel = false;
+  std::string bad;
+  for (uint32_t s = 0; s < cs->n_streams; ++s) {
+    const rpl_cloud_settings& e = cs->clouds_host[s];
+    rpl::CloudSettings& d = t[s];
+    d.range_min = e.range_min;
+    d.range_max = e.range_max != 0.0f ? e.range_max : cs->msg_hdr_host[s].range_max;
+    d.intensity_min = e.intensity_min;
+    d.voxel = e.voxel_size;
+    d.sor_k = e.sor_k;
+    d.sor_alpha = e.sor_alpha;
+    if (!e.enabled) {
+      d.route = rpl::kCloudOff;
+    } else if (e.sor_k == 0 && e.voxel_size == 0.0f) {
+      d.route = rpl::kCloudWindow;
+    } else {
+      if (e.voxel_size != 0.0f && !(d.range_max < 1000.0f) && bad.empty())
+        bad = "voxel grid: a stream's range_max, resolved against rpl_capsule_stream_set_frames, must be < 1000 m";
+      const bool fusable = e.voxel_size == 0.0f || (e.voxel_size <= 4.0f && d.range_max / e.voxel_size < 32000.0f);
+      d.route = fusable ? rpl::kCloudFused : rpl::kCloudSeparate;
+      sor_k = std::max(sor_k, e.sor_k);
+      voxel = voxel || e.voxel_size > 0.0f;
+    }
+    routes |= 1u << d.route;
+  }
+  RPL_CUDA(c, cudaMemcpy(cs->clouds, t.data(), t.size() * sizeof(rpl::CloudSettings), cudaMemcpyHostToDevice),
+           RPL_RESULT_OPERATION_FAIL);
+  cs->cloud_routes = routes;
+  cs->cloud_sor_k = sor_k;
+  cs->cloud_voxel = voxel;
+  cs->clouds_bad = bad;
+  return RPL_RESULT_OK;
+}
 
 rpl_result stream_set_frames(rpl_capsule_stream* cs, const char* const* frame_ids, const float* range_max) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
@@ -2437,7 +2579,7 @@ rpl_result stream_set_frames(rpl_capsule_stream* cs, const char* const* frame_id
   RPL_CUDA(c, cudaMemcpy(cs->msg_hdr, h.data(), h.size() * sizeof(rpl::StreamMsgHeader), cudaMemcpyHostToDevice),
            RPL_RESULT_OPERATION_FAIL);
   cs->msg_hdr_host = std::move(h);
-  return RPL_RESULT_OK;
+  return cs->clouds_host.empty() ? RPL_RESULT_OK : clouds_resolve(cs);  // a range_max of 0 follows the frames
 }
 
 // the per-stream lidar settings: the masked entries of `settings` replace the table's, all or none
@@ -2474,6 +2616,37 @@ rpl_result stream_set_lidars(rpl_capsule_stream* cs, const rpl_lidar_settings* s
   cs->lidars_host = std::move(t);
   cs->lidar_modes = modes;
   return RPL_RESULT_OK;
+}
+
+// the per-stream clouds: the masked entries of `settings` replace the table's, all or none
+rpl_result stream_set_clouds(rpl_capsule_stream* cs, const rpl_cloud_settings* settings, const uint8_t* stream_mask) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!settings) {
+    c->err = "null settings";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  std::vector<rpl_cloud_settings> t = cs->clouds_host;
+  if (t.empty()) {
+    for (uint32_t s = 0; s < cs->n_streams; ++s)
+      if (stream_mask && !stream_mask[s]) {
+        c->err = "the first rpl_capsule_stream_set_clouds call must set every stream";
+        return RPL_RESULT_INVALID_DATA;
+      }
+    t.resize(cs->n_streams);
+  }
+  for (uint32_t s = 0; s < cs->n_streams; ++s) {
+    if (stream_mask && !stream_mask[s]) continue;
+    rpl_cloud_params p{};
+    std::memcpy(&p, &settings[s], offsetof(rpl_cloud_params, is_new_protocol));  // the chain's six fields
+    if (!cloud_params_ok(c, &p)) return RPL_RESULT_INVALID_DATA;
+    t[s] = settings[s];
+  }
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  if (!cs->clouds) RPL_CUDA(c, dev_alloc(&cs->clouds, cs->n_streams), RPL_RESULT_INSUFFICIENT_MEMORY);
+  RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);  // a cloud or messages call may still read it
+  cs->clouds_host = std::move(t);
+  return clouds_resolve(cs);
 }
 
 // the PointCloud2 members between the header and the data: height 1, width, the fields x, y, z, intensity (float32,
@@ -2536,7 +2709,7 @@ bool stream_msgs_args_ok(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* 
     c->err = "null params, msgs, msg_offsets, msg_sizes or total_bytes";
     return false;
   }
-  if (kind == rpl::MsgKind::kPointCloud2 && !cloud_params_ok(c, static_cast<const rpl_cloud_params*>(params)))
+  if (kind == rpl::MsgKind::kPointCloud2 && !cloud_call_ok(cs, static_cast<const rpl_cloud_params*>(params)))
     return false;
   const bool per_stream = kind == rpl::MsgKind::kLaserScan
                               ? (static_cast<const rpl_scan_params*>(params)->flags & RPL_FLAG_PER_STREAM) != 0
@@ -2572,8 +2745,9 @@ rpl_result msgs_prepare(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* p
                        nullptr, nullptr, st, a.views, a.nodes_total,
                        lidar_table(cs, (p->flags & RPL_FLAG_PER_STREAM) != 0, s0));
     } else {
-      r = stream_cloud_chunk(c, c->lane[0], last_push_scans(cs, s0, ns), lidars_at(cs, s0), cs->max_scans,
-                             static_cast<const rpl_cloud_params*>(params), w.data + so * row * 4, w.counts + so, st);
+      r = stream_cloud_chunk(c, c->lane[0], last_push_scans(cs, s0, ns), lidars_at(cs, s0), chains_at(cs, s0),
+                             cs->max_scans, static_cast<const rpl_cloud_params*>(params), w.data + so * row * 4,
+                             w.counts + so, st);
     }
   }
   if (r != RPL_RESULT_OK) return r;
@@ -2588,6 +2762,9 @@ rpl_result msgs_prepare(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* p
   t.offsets = offsets;
   t.sizes = sizes;
   t.total = total;
+  if (kind == rpl::MsgKind::kPointCloud2 &&
+      (static_cast<const rpl_cloud_params*>(params)->flags & RPL_CLOUD_PER_STREAM_CHAIN) != 0)
+    t.clouds = cs->clouds;
   RPL_CUDA(c, rpl::launch_msg_table(t, st), RPL_RESULT_OPERATION_FAIL);
   c->launches++;
   return RPL_RESULT_OK;
@@ -2776,7 +2953,7 @@ rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, rpl::MsgK
   }
   const bool cloud = kind == rpl::MsgKind::kPointCloud2;
   const auto* cp = cloud ? static_cast<const rpl_cloud_params*>(params) : nullptr;
-  if (cloud && !cloud_params_ok(c, cp)) return RPL_RESULT_INVALID_DATA;
+  if (cloud && !cloud_call_ok(cs, cp)) return RPL_RESULT_INVALID_DATA;
   // a cloud push's: its decode, assemble and stamp settings (RPL_CLOUD_PER_STREAM before set_lidars fails the push's
   // check of RPL_FLAG_PER_STREAM)
   rpl_scan_params push_params{};
@@ -3068,6 +3245,7 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   cudaFree(cs->msg_work);
   cudaFree(cs->node_work);
   cudaFree(cs->lidars);
+  cudaFree(cs->clouds);
   cudaFree(cs->counters);
   cudaFree(cs->push_msg_work);
   cudaFreeHost(cs->push_msg_extent);
@@ -3333,6 +3511,11 @@ rpl_result rpl_capsule_stream_set_frames(rpl_capsule_stream* s, const char* cons
 rpl_result rpl_capsule_stream_set_lidars(rpl_capsule_stream* s, const rpl_lidar_settings* settings,
                                          const uint8_t* stream_mask) {
   return stream_set_lidars(s, settings, stream_mask);
+}
+
+rpl_result rpl_capsule_stream_set_clouds(rpl_capsule_stream* s, const rpl_cloud_settings* settings,
+                                         const uint8_t* stream_mask) {
+  return stream_set_clouds(s, settings, stream_mask);
 }
 
 rpl_result rpl_capsule_stream_laserscan_msgs_dev(rpl_capsule_stream* s, const rpl_scan_params* params,

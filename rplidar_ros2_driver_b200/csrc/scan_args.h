@@ -56,6 +56,14 @@ struct ScanBatchArgs {
   // the kernels leave it as they leave an out_first skip.  (Behind out_first, for the same reason.)
   uint8_t* msg_out;
   const unsigned long long* msg_ranges;
+  // per-stream clouds (RPL_CLOUD_PER_STREAM_CHAIN, nullable; the PointCloud2 payload of the shared-memory kernels and
+  // the general kernel): scan s takes its window, and the fused kernel its SOR / voxel grid, from
+  // clouds[s / lidar_scans] instead of the fields above and SmallArgs.  cloud_launches (bit 0 the window-only kernel,
+  // bit 1 the fused kernel) tells which shared-memory launches the call makes: each serves the scans of its route
+  // (cloud_route), a kCloudOff scan is the window-only launch's when it runs, else the fused one's, and is left with
+  // point count 0 before its nodes are read.  (Behind msg_ranges, for the same reason.)
+  const CloudSettings* clouds;
+  uint32_t cloud_launches;
 };
 constexpr unsigned long long kOutSkip = 1ull << 63;
 

@@ -103,12 +103,12 @@ __global__ void __launch_bounds__(GT, 1)
   const bool ascend = a.apply_ascend != 0;
   const bool cloud = a.xyzi != nullptr;  // PointCloud2 payload: window filter + polar->xyz
   const bool want_scan = a.ranges != nullptr || cloud || a.msg_out != nullptr;
+  float rmin = a.range_min, rmax = a.range_max, imin = a.intensity_min;  // the window (per-stream clouds: per scan)
   auto kept = [&](uint2 nd) {
     const uint32_t d = node_dist(nd);
     if (d == 0) return false;
     if (!cloud) return true;
-    return cloud_keep(dist_to_m(d), quality_to_intensity(node_quality(nd), new_proto), a.range_min, a.range_max,
-                      a.intensity_min);
+    return cloud_keep(dist_to_m(d), quality_to_intensity(node_quality(nd), new_proto), rmin, rmax, imin);
   };
 
   const size_t wo = (size_t)blockIdx.x * ws.max_nodes;
@@ -128,6 +128,16 @@ __global__ void __launch_bounds__(GT, 1)
       new_proto = ls.is_new_protocol != 0;
       mode_a = ls.mode_a != 0;
       inverted = ls.inverted != 0;
+    }
+    if (cloud && a.clouds) {  // the scan's stream's cloud (only every scan's launch meets one without a cloud)
+      const CloudSettings& cl = a.clouds[s / a.lidar_scans];
+      if (cl.route == kCloudOff) {
+        if (tid == 0 && a.beam_counts) a.beam_counts[s] = 0u;
+        continue;
+      }
+      rmin = cl.range_min;
+      rmax = cl.range_max;
+      imin = cl.intensity_min;
     }
     const uint32_t n = a.views ? a.views[s].y : a.counts[s];
     const uint2* base = a.views ? a.nodes + a.views[s].x : a.nodes + (size_t)s * a.stride;

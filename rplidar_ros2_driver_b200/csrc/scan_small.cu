@@ -45,6 +45,10 @@ struct SmallCtl {
   double thr;
   uint32_t red[3 * 32];
   uint32_t totV, totA, first_valid, front_key, fallback, count_out;
+  // PointCloud2: the scan's window and (fused kernel) SOR / voxel grid, staged by one thread (SmallArgs or its stream's
+  // ScanBatchArgs::clouds entry) so that they hold no register through the passes
+  float rmin, rmax, imin, sor_alpha, voxel;
+  uint32_t sor_k;
   union {
     uint32_t chunk_base[128];  // PointCloud2 chain, voxel ordering: per (chunk, warp) counts -> exclusive bases
     struct {                   // ascended buffer: the few nodes whose final key is already taken (see the place pass)
@@ -314,7 +318,6 @@ __device__ __forceinline__ void scan_small_body(const ScanBatchArgs& a, const Sm
 
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint64_t pol_stream = l2_policy_evict_first();
-  const float w_rmin = a.range_min, w_rmax = a.range_max, w_imin = a.intensity_min;
   const bool want_scan = CLOUD ? false : (EMIT ? (a.ranges != nullptr) : true);
 
   if (tid == 0) {
@@ -327,6 +330,15 @@ __device__ __forceinline__ void scan_small_body(const ScanBatchArgs& a, const Sm
   for (uint32_t s = blockIdx.x; s < a.n_scans; s += gridDim.x) {
     if (EMIT && out_skipped(a, s)) continue;
     if (MSG && (a.msg_ranges[s] & kOutSkip) != 0) continue;
+    if (CLOUD && a.clouds) {  // per-stream clouds: a scan of the other launch's route is not this launch's
+      const uint32_t route = cloud_route(a.clouds[s / a.lidar_scans], a.cloud_launches);
+      const bool mine = route == kCloudOff ? ((a.cloud_launches & 1u) != 0) != POST : (route == kCloudFused) == POST;
+      if (!mine) continue;
+      if (route == kCloudOff) {  // no cloud: point count 0, the nodes not read
+        if (tid == 0) write_outcome_empty(a, s);
+        continue;
+      }
+    }
     bool new_proto = a.is_new_protocol != 0, inverted = a.inverted != 0;
     if (a.lidars) {  // the scan's stream's settings; a LaserScan scan of the other mode is the other launch's
       const LidarSettings& ls = a.lidars[s / a.lidar_scans];
@@ -395,12 +407,36 @@ __device__ __forceinline__ void scan_small_body(const ScanBatchArgs& a, const Sm
           ctl.d.ndup = 0;
           ctl.d.ndupnode = 0;
         }
+        if (CLOUD) {
+          if (a.clouds) {
+            const CloudSettings& cl = a.clouds[s / a.lidar_scans];
+            ctl.rmin = cl.range_min;
+            ctl.rmax = cl.range_max;
+            ctl.imin = cl.intensity_min;
+            ctl.sor_k = cl.sor_k;
+            ctl.sor_alpha = cl.sor_alpha;
+            ctl.voxel = cl.voxel;
+          } else {
+            ctl.rmin = a.range_min;
+            ctl.rmax = a.range_max;
+            ctl.imin = a.intensity_min;
+            ctl.sor_k = p.sor_k;
+            ctl.sor_alpha = p.sor_alpha;
+            ctl.voxel = p.voxel;
+          }
+        }
       }
     }
     __syncthreads();
     if (bulk) {
       mbar_wait(&ctl.full, parity);
       parity ^= 1u;
+    }
+    float w_rmin = 0.0f, w_rmax = 0.0f, w_imin = 0.0f;
+    if (CLOUD) {
+      w_rmin = ctl.rmin;
+      w_rmax = ctl.rmax;
+      w_imin = ctl.imin;
     }
 
     // ---- mark: one shared-memory atomicOr per kept key -----------------------------------------------
@@ -727,19 +763,19 @@ __device__ __forceinline__ void scan_small_body(const ScanBatchArgs& a, const Sm
     if constexpr (POST) {
       uint32_t m = M;
       // ---- step 4: statistical outlier removal over the +-16 angular neighbours --------------------------
-      if (p.sor_k > 0 && m >= 2) {
+      if (ctl.sor_k > 0 && m >= 2) {
         unsigned long long* qv = reinterpret_cast<unsigned long long*>(acc);  // [cap] (rank table is dead)
         const bool all_others = (m - 1) <= 32u;
         long long s1 = 0;
         unsigned long long s2 = 0;
         for (uint32_t i = tid; i < m; i += TS) {
           float mean;
-          if (all_others || p.sor_k > 8u) {
-            mean = sor_mean_generic(px, m, i, p.sor_k, all_others);
+          if (all_others || ctl.sor_k > 8u) {
+            mean = sor_mean_generic(px, m, i, ctl.sor_k, all_others);
           } else if (__all_sync(__activemask(), i >= 16u && i + 16u < m)) {  // the whole warp is clear of both ends
-            mean = sor_mean_win8<false>(px, m, i, p.sor_k);
+            mean = sor_mean_win8<false>(px, m, i, ctl.sor_k);
           } else {
-            mean = sor_mean_win8<true>(px, m, i, p.sor_k);
+            mean = sor_mean_win8<true>(px, m, i, ctl.sor_k);
           }
           const long long qq = __float2ll_rn(__fmul_rn(mean, 65536.0f));  // llrintf
           qv[i] = (unsigned long long)qq;
@@ -768,7 +804,7 @@ __device__ __forceinline__ void scan_small_body(const ScanBatchArgs& a, const Sm
           const double sq = __ddiv_rn(__dmul_rn(t1, t1), dn);
           double var = __ddiv_rn(__dsub_rn(t2, sq), __dsub_rn(dn, 1.0));
           if (!(var > 0.0)) var = 0.0;
-          ctl.thr = __dadd_rn(mean, __dmul_rn((double)p.sor_alpha, __dsqrt_rn(var)));
+          ctl.thr = __dadd_rn(mean, __dmul_rn((double)ctl.sor_alpha, __dsqrt_rn(var)));
         }
         __syncthreads();
         const double thr = ctl.thr;
@@ -816,7 +852,7 @@ __device__ __forceinline__ void scan_small_body(const ScanBatchArgs& a, const Sm
       }
       m_out = m;
 
-      if (p.voxel > 0.0f && m > 0) {
+      if (ctl.voxel > 0.0f && m > 0) {
         // ---- step 5: voxel grid -------------------------------------------------------------------------
         // acc: key32[cap] | dx[cap] | dy[cap] | cs[cap]; table of cell leaders in the (dead) tile buffer
         uint32_t* key32 = reinterpret_cast<uint32_t*>(acc);
@@ -832,9 +868,9 @@ __device__ __forceinline__ void scan_small_body(const ScanBatchArgs& a, const Sm
           const uint4 e = make_uint4(kEmpty, kEmpty, kEmpty, kEmpty);
           for (uint32_t w = tid; w < nslots / 4; w += TS) t4[w] = e;
         }
-        const float rvoxel = __frcp_rn(p.voxel);
+        const float rvoxel = __frcp_rn(ctl.voxel);
         for (uint32_t i = tid; i < m; i += TS) {
-          key32[i] = cell_key(px[i], p.voxel, rvoxel);
+          key32[i] = cell_key(px[i], ctl.voxel, rvoxel);
           dxs[i] = 0;
           dys[i] = 0;
           cs[i] = 0;
@@ -1073,10 +1109,21 @@ cudaError_t launch_scan_small(const ScanBatchArgs& a, uint32_t max_nodes, uint32
   const bool cloud = a.xyzi != nullptr;
   const bool emit = !cloud && a.nodes_out != nullptr && a.apply_ascend != 0;
   const bool post = cloud && (sor_k > 0 || voxel > 0.0f);
-  if (cloud) {
-    const size_t sh = scan_small_smem_bytes(p.cap, 2, false, post);
-    if (post) return launch_one<2, false, true, kSmallPostThreads>(a, p, sh, num_sms, stream);
-    return launch_one<2, false, false, kSmallThreads>(a, p, sh, num_sms, stream);
+  auto launch_cloud = [&](bool fused, SmallArgs q) {
+    const size_t sh = scan_small_smem_bytes(q.cap, 2, false, fused);
+    if (fused) return launch_one<2, false, true, kSmallPostThreads>(a, q, sh, num_sms, stream);
+    return launch_one<2, false, false, kSmallThreads>(a, q, sh, num_sms, stream);
+  };
+  if (cloud && !a.clouds) return launch_cloud(post, p);
+  if (cloud) {  // per-stream clouds: the launches the call makes, each serving its routes' scans
+    cudaError_t e = cudaSuccess;
+    if (a.cloud_launches & 1u) {
+      SmallArgs q = p;
+      q.cap = (a.stride + 63u) & ~63u;
+      e = launch_cloud(false, q);
+    }
+    if (e == cudaSuccess && (a.cloud_launches & 2u)) e = launch_cloud(true, p);
+    return e;
   }
   auto launch_mode = [&](int mode) {
     const size_t sh = scan_small_smem_bytes(p.cap, mode, emit, false);

@@ -148,9 +148,11 @@ rpl_result rpl_host_alloc(size_t bytes, void** out);
 void rpl_host_free(void* p);
 /* Number of kernels this context has launched so far (bench.py's gpu_launches). */
 uint64_t rpl_ctx_launch_count(const rpl_ctx* ctx);
-/* Kernel timing for roofline reports: when enabled, every scan-kernel launch is bracketed by
- * CUDA events on the stream it is launched on.  rpl_ctx_profile_read synchronises, returns
- * the summed durations (ms) and launch counts since the last read, and clears them. */
+/* Kernel timing for roofline reports: when enabled, every scan-kernel launch is timed -- the
+ * LaserScan Mode B cluster kernel and the general kernel by the kernel itself (%globaltimer, from
+ * the first CTA's start to the last CTA's end, so without the launch latency), the others by
+ * CUDA events around the launch on its stream.  rpl_ctx_profile_read synchronises the device,
+ * returns the summed durations (ms) and launch counts since the last read, and clears them. */
 rpl_result rpl_ctx_profile(rpl_ctx* ctx, int enable);
 rpl_result rpl_ctx_profile_read(rpl_ctx* ctx, double* fast_ms, uint32_t* fast_launches,
                                 double* general_ms, uint32_t* general_launches);

@@ -90,6 +90,45 @@ rpl_result grow_stage(rpl_ctx* c, int lanes, Layout layout) {
 // kNone: the general kernel serves every scan.
 enum class FastKernel { kNone, kSmall, kCluster, kTma, kFast };
 
+// Sums every profiled launch queued so far into c->prof_ms / prof_n and resets the stamp records
+// (rpl_ctx::prof_stamps).  Synchronises the device.
+rpl_result prof_drain(rpl_ctx* c) {
+  RPL_CUDA(c, cudaDeviceSynchronize(), RPL_RESULT_OPERATION_FAIL);
+  std::vector<unsigned long long> st(2 * (size_t)c->prof_stamps_used);
+  if (!st.empty())
+    RPL_CUDA(c, cudaMemcpy(st.data(), c->prof_stamps, st.size() * 8, cudaMemcpyDeviceToHost), RPL_RESULT_OPERATION_FAIL);
+  auto sum = [&](std::vector<rpl_ctx::ProfLaunch>& v, int kind) {
+    for (const auto& pl : v) {
+      if (pl.stamp >= 0) {
+        const unsigned long long t0 = st[2 * pl.stamp], t1 = st[2 * pl.stamp + 1];
+        if (t1 > t0) c->prof_ms[kind] += (double)(t1 - t0) * 1e-6;
+      } else {
+        float t = 0.f;
+        if (cudaEventElapsedTime(&t, pl.e0, pl.e1) == cudaSuccess) c->prof_ms[kind] += t;
+        cudaEventDestroy(pl.e0);
+        cudaEventDestroy(pl.e1);
+      }
+      c->prof_n[kind]++;
+    }
+    v.clear();
+  };
+  sum(c->prof_fast, 0);
+  sum(c->prof_general, 1);
+  if (c->prof_stamps_used != 0) {  // {earliest start, latest end} = {all ones, 0}
+    RPL_CUDA(c, cudaMemset2D(c->prof_stamps, 16, 0xFF, 8, c->prof_stamps_used), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemset2D(c->prof_stamps + 1, 16, 0, 8, c->prof_stamps_used), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaDeviceSynchronize(), RPL_RESULT_OPERATION_FAIL);
+  }
+  c->prof_stamps_used = 0;
+  return RPL_RESULT_OK;
+}
+
+// the stamp record of one profiled launch (nullptr with c->err set on failure)
+unsigned long long* prof_take(rpl_ctx* c) {
+  if (c->prof_stamps_used == rpl_ctx::kProfStamps && prof_drain(c) != RPL_RESULT_OK) return nullptr;
+  return c->prof_stamps + 2 * (size_t)c->prof_stamps_used++;
+}
+
 // the kernel-selection rule of every scan entry point, batches and single scans alike
 FastKernel pick_fast(const rpl::ScanBatchArgs& a, uint32_t flags) {
   // FORCE_GENERAL and status-only calls (no LaserScan, no ascended buffer) take the general kernel alone
@@ -108,18 +147,25 @@ FastKernel pick_fast(const rpl::ScanBatchArgs& a, uint32_t flags) {
   return FastKernel::kTma;
 }
 
-// Launches fast kernel k on `stream` (k != kNone); the caller has zeroed a.fallback_count.  A PointCloud2 launch may
+// Launches fast kernel k on `stream` (k != kNone); a.fallback_count is zero when it starts.  A PointCloud2 launch may
 // fuse the SOR / voxel-grid passes of `cloud` (steps 4-5) into the shared-memory kernel: *post_fused tells.
 // hand_off (scan views): above kSmallPostMaxNodes, fuse all the same with the shared memory sized for that many nodes,
 // the longer views going to the general kernel like duplicate-key scans.
+// ticket (nullable, zero when the kernel starts): the cluster kernel hands out scans from it (scan_tma.cu); without
+// one, each cluster takes a fixed share.
 rpl_result launch_fast(rpl_ctx* c, Lane& l, const rpl::ScanBatchArgs& a, FastKernel k, cudaStream_t stream,
-                       const rpl_cloud_params* cloud = nullptr, bool* post_fused = nullptr, bool hand_off = false) {
+                       const rpl_cloud_params* cloud = nullptr, bool* post_fused = nullptr, bool hand_off = false,
+                       uint32_t* ticket = nullptr) {
   const int tma_grid = c->tma_grid[a.xyzi ? 2 : a.mode_a ? 1 : 0];
   const int grid = k == FastKernel::kCluster
                        ? 2 * (int)std::min<uint32_t>(a.n_scans, (uint32_t)c->tma_clusters)
                        : (int)std::min<uint32_t>(a.n_scans, (uint32_t)(k == FastKernel::kTma ? tma_grid : c->fast_grid));
+  // the cluster kernel times itself (its general kernel runs chained behind it), the others between two events
   cudaEvent_t e0 = nullptr, e1 = nullptr;
-  if (c->profile) {
+  unsigned long long* stamp = nullptr;
+  if (c->profile && k == FastKernel::kCluster) {
+    if (!(stamp = prof_take(c))) return RPL_RESULT_OPERATION_FAIL;
+  } else if (c->profile) {
     cudaEventCreate(&e0);
     cudaEventCreate(&e1);
     cudaEventRecord(e0, stream);
@@ -145,35 +191,32 @@ rpl_result launch_fast(rpl_ctx* c, Lane& l, const rpl::ScanBatchArgs& a, FastKer
              RPL_RESULT_OPERATION_FAIL);
     if (post_fused) *post_fused = fuse;
   } else if (k == FastKernel::kCluster) {
-    RPL_CUDA(c, rpl::launch_scan_tma_cluster(a, l.fws.max_nodes, grid, stream), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, rpl::launch_scan_tma_cluster(a, l.fws.max_nodes, grid, ticket, stamp, stream), RPL_RESULT_OPERATION_FAIL);
   } else if (k == FastKernel::kTma) {
     RPL_CUDA(c, rpl::launch_scan_tma(a, l.fws.max_nodes, grid, stream), RPL_RESULT_OPERATION_FAIL);
   } else {
     RPL_CUDA(c, rpl::launch_scan_fast(a, l.fws, grid, stream), RPL_RESULT_OPERATION_FAIL);
   }
   if (c->profile) {
-    cudaEventRecord(e1, stream);
-    c->prof_fast.emplace_back(e0, e1);
+    if (!stamp) cudaEventRecord(e1, stream);
+    c->prof_fast.push_back({e0, e1, stamp ? (int)((stamp - c->prof_stamps) / 2) : -1});
   }
   // a per-stream LaserScan launch of the shared-memory kernels is one launch per mode present
   c->launches += k == FastKernel::kSmall && a.lidars && !a.xyzi ? __builtin_popcount(a.lidar_modes) : 1;
   return RPL_RESULT_OK;
 }
 
-// launches scan_general_kernel on `stream` over every scan (all_scans) or over the scans in a.fallback_list
-rpl_result launch_general(rpl_ctx* c, Lane& l, const rpl::ScanBatchArgs& a, bool all_scans, cudaStream_t stream) {
+// launches scan_general_kernel on `stream` over every scan (all_scans) or over the scans in a.fallback_list; it zeroes
+// zero_next[0..1] (nullable) for the lane's next call.  chained: it directly follows the fast kernel that fills the list,
+// and is launched as that kernel's programmatic dependent, so that its launch overlaps the fast kernel's tail.
+rpl_result launch_general(rpl_ctx* c, Lane& l, const rpl::ScanBatchArgs& a, bool all_scans, cudaStream_t stream,
+                          uint32_t* zero_next = nullptr, bool chained = false) {
   const int grid = (int)std::min<uint32_t>(a.n_scans, (uint32_t)c->general_grid);
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  if (c->profile) {
-    cudaEventCreate(&e0);
-    cudaEventCreate(&e1);
-    cudaEventRecord(e0, stream);
-  }
-  RPL_CUDA(c, rpl::launch_scan_general(a, l.gws, grid, all_scans, stream), RPL_RESULT_OPERATION_FAIL);
-  if (c->profile) {
-    cudaEventRecord(e1, stream);
-    c->prof_general.emplace_back(e0, e1);
-  }
+  unsigned long long* stamp = nullptr;  // profiled: the kernel times itself, from the end of its wait on a chained start
+  if (c->profile && !(stamp = prof_take(c))) return RPL_RESULT_OPERATION_FAIL;
+  RPL_CUDA(c, rpl::launch_scan_general(a, l.gws, grid, all_scans, zero_next, chained, stamp, stream),
+           RPL_RESULT_OPERATION_FAIL);
+  if (c->profile) c->prof_general.push_back({nullptr, nullptr, (int)((stamp - c->prof_stamps) / 2)});
   c->launches++;
   return RPL_RESULT_OK;
 }
@@ -181,12 +224,16 @@ rpl_result launch_general(rpl_ctx* c, Lane& l, const rpl::ScanBatchArgs& a, bool
 // A lane's scan scratch (Lane::scratch_free) is taken by one section of kernels at a time: the device calls of every
 // stream run on lane 0's, the host calls' chunks on their lane's.  A section starts, on its stream, after the lane's
 // previous section has ended, and ends after its last kernel that reads the scratch.
-rpl_result scratch_enter(rpl_ctx* c, const Lane& l, cudaStream_t stream) {
+rpl_result scratch_enter(rpl_ctx* c, Lane& l, cudaStream_t stream) {
+  l.spare_queued = false;
   RPL_CUDA(c, cudaStreamWaitEvent(stream, l.scratch_free, 0), RPL_RESULT_OPERATION_FAIL);
   return RPL_RESULT_OK;
 }
-rpl_result scratch_leave(rpl_ctx* c, const Lane& l, cudaStream_t stream) {
+rpl_result scratch_leave(rpl_ctx* c, Lane& l, cudaStream_t stream) {
   RPL_CUDA(c, cudaEventRecord(l.scratch_free, stream), RPL_RESULT_OPERATION_FAIL);
+  // the next section, ordered behind this one, finds its hand-off counter zeroed by this section's general kernel
+  if (l.spare_queued) l.spare_zeroed = true;
+  l.spare_queued = false;
   return RPL_RESULT_OK;
 }
 
@@ -207,19 +254,28 @@ rpl_result enqueue_args(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, uint32_t flag
   // per-stream settings, per-stream clouds and placed messages are read by the shared-memory kernels and the general
   // kernel only
   if ((a.lidars || a.msg_out || a.clouds) && k != FastKernel::kSmall) k = FastKernel::kNone;
+  // this call's hand-off counter and scan ticket (Lane::fallback_count), and the lane's next call's pair, which the
+  // general kernel zeroes
+  l.count_parity ^= 1u;
+  a.fallback_count = l.hand_off_count();
+  const bool zeroed = l.spare_zeroed;
+  l.spare_zeroed = false;
   if (k != FastKernel::kNone) {
-    RPL_CUDA(c, cudaMemsetAsync(l.fallback_count, 0, sizeof(uint32_t), stream), RPL_RESULT_OPERATION_FAIL);
-    const rpl_result r = launch_fast(c, l, a, k, stream, cloud, post_fused, hand_off);
+    if (!zeroed)
+      RPL_CUDA(c, cudaMemsetAsync(a.fallback_count, 0, 2 * sizeof(uint32_t), stream), RPL_RESULT_OPERATION_FAIL);
+    const rpl_result r = launch_fast(c, l, a, k, stream, cloud, post_fused, hand_off, a.fallback_count + 1);
     if (r != RPL_RESULT_OK) return r;
   }
-  return launch_general(c, l, a, k == FastKernel::kNone, stream);
+  const rpl_result r = launch_general(c, l, a, k == FastKernel::kNone, stream,
+                                      l.fallback_count + 2 * (l.count_parity ^ 1u), k == FastKernel::kCluster);
+  if (r == RPL_RESULT_OK) l.spare_queued = true;
+  return r;
 }
 
 // the fields of a LaserScan launch that come from the parameters and the lane
 rpl::ScanBatchArgs scan_args(const rpl_scan_params* p, const Lane& l) {
   rpl::ScanBatchArgs a{};
   a.fallback_list = l.fallback_list;
-  a.fallback_count = l.fallback_count;
   a.is_new_protocol = p->is_new_protocol;
   a.mode_a = p->scan_processing;
   a.inverted = p->inverted;
@@ -387,7 +443,7 @@ rpl_result rpl_ctx_create(int device, uint32_t max_nodes, uint32_t max_scans, rp
     l.fws.max_nodes = max_nodes;
     l.gws.max_nodes = max_nodes;
     if (!cuda_ok(c, dev_alloc(&l.fallback_list, max_scans), "cudaMalloc") ||
-        !cuda_ok(c, dev_alloc(&l.fallback_count, 1), "cudaMalloc") ||
+        !cuda_ok(c, dev_alloc(&l.fallback_count, 4), "cudaMalloc") ||
         !cuda_ok(c, dev_alloc(&l.fws.group, fast_nodes), "cudaMalloc") ||
         !cuda_ok(c, dev_alloc(&l.gws.keyf, gen_nodes), "cudaMalloc") ||
         !cuda_ok(c, dev_alloc(&l.gws.idx0, gen_nodes), "cudaMalloc") ||
@@ -403,7 +459,7 @@ rpl_result rpl_ctx_create(int device, uint32_t max_nodes, uint32_t max_scans, rp
       l.cws.trig = c->lane[0].cws.trig;
       l.cws.angle = c->lane[0].cws.angle;
     }
-    if (!cuda_ok(c, cudaMemset(l.fallback_count, 0, sizeof(uint32_t)), "cudaMemset"))
+    if (!cuda_ok(c, cudaMemset(l.fallback_count, 0, 4 * sizeof(uint32_t)), "cudaMemset"))
       return fail(RPL_RESULT_OPERATION_FAIL);
   }
   if (!cuda_ok(c, cudaHostAlloc(reinterpret_cast<void**>(&c->h_counts), (size_t)max_scans * 4, cudaHostAllocDefault),
@@ -430,6 +486,7 @@ void rpl_ctx_destroy(rpl_ctx* c) {
     free_lane(c->lane[i]);
   }
   if (c->asm_done) cudaEventDestroy(c->asm_done);
+  cudaFree(c->prof_stamps);
   cudaFree(c->d_reset_prefix);
   cudaFree(c->d_desc);
   if (c->h_one) cudaFreeHost(c->h_one);
@@ -463,6 +520,14 @@ uint64_t rpl_ctx_launch_count(const rpl_ctx* c) { return c ? c->launches : 0; }
 
 rpl_result rpl_ctx_profile(rpl_ctx* c, int enable) {
   if (!c) return RPL_RESULT_INVALID_DATA;
+  if (enable && !c->prof_stamps) {
+    RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->prof_stamps), rpl_ctx::kProfStamps * 16),
+             RPL_RESULT_INSUFFICIENT_MEMORY);
+    c->prof_stamps_used = rpl_ctx::kProfStamps;  // the drain initialises every record
+    const rpl_result r = prof_drain(c);
+    if (r != RPL_RESULT_OK) return r;
+  }
   c->profile = enable != 0;
   return RPL_RESULT_OK;
 }
@@ -471,21 +536,14 @@ rpl_result rpl_ctx_profile_read(rpl_ctx* c, double* fast_ms, uint32_t* fast_laun
                                 double* general_ms, uint32_t* general_launches) {
   if (!c) return RPL_RESULT_INVALID_DATA;
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
-  auto drain = [&](std::vector<std::pair<cudaEvent_t, cudaEvent_t>>& v, double* ms, uint32_t* n) {
-    double sum = 0.0;
-    for (auto& pr : v) {
-      cudaEventSynchronize(pr.second);
-      float t = 0.f;
-      if (cudaEventElapsedTime(&t, pr.first, pr.second) == cudaSuccess) sum += t;
-      cudaEventDestroy(pr.first);
-      cudaEventDestroy(pr.second);
-    }
-    if (ms) *ms = sum;
-    if (n) *n = (uint32_t)v.size();
-    v.clear();
-  };
-  drain(c->prof_fast, fast_ms, fast_launches);
-  drain(c->prof_general, general_ms, general_launches);
+  const rpl_result r = prof_drain(c);
+  if (r != RPL_RESULT_OK) return r;
+  if (fast_ms) *fast_ms = c->prof_ms[0];
+  if (fast_launches) *fast_launches = c->prof_n[0];
+  if (general_ms) *general_ms = c->prof_ms[1];
+  if (general_launches) *general_launches = c->prof_n[1];
+  c->prof_ms[0] = c->prof_ms[1] = 0.0;
+  c->prof_n[0] = c->prof_n[1] = 0;
   return RPL_RESULT_OK;
 }
 
@@ -1583,7 +1641,7 @@ rpl_result stream_chains_chunk(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, const 
       int launched = 0;
       RPL_CUDA(c, rpl::launch_cloud_post(a.xyzi, point_counts, a.n_scans, a.stride, chains.sor_k, 0.0f,
                                          chains.voxel ? 1.0f : 0.0f, post.cws, pass ? a.fallback_list : nullptr,
-                                         pass ? a.fallback_count : nullptr, st, &launched, tab),
+                                         pass ? l.hand_off_count() : nullptr, st, &launched, tab),
                RPL_RESULT_OPERATION_FAIL);
       c->launches += launched;
     }
@@ -1607,7 +1665,6 @@ rpl_result stream_cloud_chunk(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, const r
                               uint32_t* point_counts, cudaStream_t st) {
   a.beam_counts = point_counts;
   a.fallback_list = l.fallback_list;
-  a.fallback_count = l.fallback_count;
   a.is_new_protocol = p->is_new_protocol;
   a.xyzi = reinterpret_cast<float4*>(xyzi);
   a.trig = c->lane[0].cws.trig;
@@ -1629,7 +1686,7 @@ rpl_result stream_cloud_chunk(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, const r
     if (&l != &post && (r = scratch_enter(c, post, st)) != RPL_RESULT_OK) return r;
     int launched = 0;
     RPL_CUDA(c, rpl::launch_cloud_post(a.xyzi, point_counts, a.n_scans, a.stride, p->sor_k, p->sor_alpha, p->voxel_size,
-                                       post.cws, fused ? a.fallback_list : nullptr, fused ? a.fallback_count : nullptr,
+                                       post.cws, fused ? a.fallback_list : nullptr, fused ? l.hand_off_count() : nullptr,
                                        st, &launched),
              RPL_RESULT_OPERATION_FAIL);
     c->launches += launched;
@@ -3079,7 +3136,6 @@ rpl_result stream_nodes_chunk(rpl_capsule_stream* cs, Lane& l, uint32_t s0, uint
   a.status = status;
   a.apply_ascend = 1;
   a.fallback_list = l.fallback_list;
-  a.fallback_count = l.fallback_count;
   if (kinds.ascended) {
     rpl_result r = scratch_enter(c, l, st);
     if (r == RPL_RESULT_OK) r = enqueue_args(c, l, a, 0u, st);
@@ -3806,7 +3862,6 @@ rpl_result rpl_cloud_batch_dev(rpl_ctx* c, const rpl_node_hq* nodes, const uint3
   a.stride = stride;
   a.beam_counts = point_counts;  // points kept per scan
   a.fallback_list = c->lane[0].fallback_list;
-  a.fallback_count = c->lane[0].fallback_count;
   a.is_new_protocol = params->is_new_protocol;
   a.xyzi = reinterpret_cast<float4*>(xyzi);
   a.trig = c->lane[0].cws.trig;
@@ -3826,7 +3881,7 @@ rpl_result rpl_cloud_batch_dev(rpl_ctx* c, const rpl_node_hq* nodes, const uint3
     int launched = 0;
     RPL_CUDA(c, rpl::launch_cloud_post(a.xyzi, point_counts, n_scans, stride, params->sor_k, params->sor_alpha,
                                        params->voxel_size, c->lane[0].cws, fused ? a.fallback_list : nullptr,
-                                       fused ? a.fallback_count : nullptr, st, &launched),
+                                       fused ? c->lane[0].hand_off_count() : nullptr, st, &launched),
              RPL_RESULT_OPERATION_FAIL);
     c->launches += launched;
   }

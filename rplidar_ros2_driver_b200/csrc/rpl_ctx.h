@@ -17,7 +17,15 @@ constexpr int kLanes = 2;  // host-buffer pipeline depth (copy/compute overlap; 
 struct Lane {
   cudaStream_t stream = nullptr;
   uint32_t* fallback_list = nullptr;
+  // [2][2]: per call parity, the hand-off counter and the cluster kernel's scan ticket.  enqueue_args gives each call
+  // the other pair than the lane's last call (count_parity), and that call's general kernel zeroes the pair the lane's
+  // next call takes, so that a call needs no memset of its own.  spare_zeroed: the next call's pair is known to be
+  // zero -- a general kernel that zeroes it was queued in a section that ended (spare_queued, scratch_leave); cleared
+  // by every enqueue_args.  When it is clear, enqueue_args zeroes the pair with a memset as before.
   uint32_t* fallback_count = nullptr;
+  uint32_t count_parity = 0;
+  bool spare_zeroed = true, spare_queued = false;
+  uint32_t* hand_off_count() const { return fallback_count + 2 * count_parity; }  // the current call's counter
   rpl::FastWorkspace fws{};
   rpl::GeneralWorkspace gws{};
   rpl::CloudWorkspace cws{};   // lane 0 owns the tables and the post-pass scratch; the others alias its tables
@@ -56,8 +64,22 @@ struct rpl_ctx {
   uint2* d_desc = nullptr;
   size_t reset_prefix_cap = 0, desc_cap = 0;
   cudaEvent_t asm_done = nullptr;   // the wire-to-LaserScan chunks of every lane and stream share the assemble scratch
+  // Profiling (rpl_ctx_profile): each profiled launch since the last rpl_ctx_profile_read is timed by an event pair
+  // around it, or (stamp >= 0) by the kernel itself -- the cluster kernel and the general kernel, which run chained
+  // with no room for an event between them: thread 0 of every CTA keeps the earliest CTA start in
+  // prof_stamps[2 stamp] and the latest CTA end in prof_stamps[2 stamp + 1] (%globaltimer, ns).  When the
+  // kProfStamps records run out, the finished launches are summed into prof_ms / prof_n (prof_drain).
   bool profile = false;
-  std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_fast, prof_general;
+  struct ProfLaunch {
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    int stamp = -1;
+  };
+  std::vector<ProfLaunch> prof_fast, prof_general;
+  static constexpr uint32_t kProfStamps = 4096;
+  unsigned long long* prof_stamps = nullptr;  // [kProfStamps][2], allocated when profiling is first enabled
+  uint32_t prof_stamps_used = 0;
+  double prof_ms[2] = {0.0, 0.0};  // fast, general
+  uint32_t prof_n[2] = {0, 0};
 };
 
 inline bool cuda_ok(rpl_ctx* c, cudaError_t e, const char* what) {

@@ -219,4 +219,18 @@ __device__ __forceinline__ uint2 ld_stream_v2(const void* p) {
   return r;
 }
 
+// Profiled launches (rpl_ctx::prof_stamps): thread 0 of every CTA folds its start and end into the launch's record
+// {earliest start, latest end} in %globaltimer nanoseconds.  rec == nullptr: not profiled.
+__device__ __forceinline__ unsigned long long global_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+__device__ __forceinline__ void stamp_start(unsigned long long* rec) {
+  if (rec && threadIdx.x == 0) atomicMin(rec, global_ns());
+}
+__device__ __forceinline__ void stamp_end(unsigned long long* rec) {
+  if (rec && threadIdx.x == 0) atomicMax(rec + 1, global_ns());
+}
+
 }  // namespace rpl

@@ -21,7 +21,7 @@ struct ScanBatchArgs {
   uint32_t* path;          // [n_scans] nullable
   // fast kernel -> general kernel hand-off (device side, no host round trip)
   uint32_t* fallback_list;   // [n_scans]
-  uint32_t* fallback_count;  // [1], zeroed before the fast kernel
+  uint32_t* fallback_count;  // [1], zero when the fast kernel starts
   uint8_t is_new_protocol;
   uint8_t mode_a;
   uint8_t inverted;
@@ -112,8 +112,11 @@ constexpr int kGeneralThreads = 128;
 
 cudaError_t launch_scan_fast(const ScanBatchArgs& a, const FastWorkspace& ws, int grid,
                              cudaStream_t stream);
-cudaError_t launch_scan_general(const ScanBatchArgs& a, const GeneralWorkspace& ws, int grid,
-                                bool all_scans, cudaStream_t stream);
+// zero_next (nullable): [2] set to 0 by the kernel (the lane's next hand-off counter and scan ticket).  chained: launched as the
+// programmatic dependent of the fast kernel before it on `stream`, which may trigger it early
+// (griddepcontrol.launch_dependents).  stamp (nullable): the launch's profiling record (rpl_device.cuh stamp_start)
+cudaError_t launch_scan_general(const ScanBatchArgs& a, const GeneralWorkspace& ws, int grid, bool all_scans,
+                                uint32_t* zero_next, bool chained, unsigned long long* stamp, cudaStream_t stream);
 size_t scan_fast_smem_bytes();
 size_t scan_general_smem_bytes();
 cudaError_t scan_fast_configure();     // opt-in dynamic shared memory, once per device
@@ -126,7 +129,10 @@ int scan_tma_max_ctas_per_sm(int mode);  // mode: 0 LaserScan Mode B, 1 Mode A, 
 // LaserScan Mode B without the ascended buffer for strides in (kSmallMaxNodes, 32768]: each scan staged whole
 // across a cluster of two CTAs (scan_tma.cu); 16-byte aligned scan bases, even grid of 2 x clusters
 bool scan_tma_cluster_applies(uint32_t stride);
-cudaError_t launch_scan_tma_cluster(const ScanBatchArgs& a, uint32_t max_nodes, int grid, cudaStream_t stream);
+// ticket (nullable): a counter at zero from which the clusters draw scans at run time; without one each cluster takes
+// a fixed share
+cudaError_t launch_scan_tma_cluster(const ScanBatchArgs& a, uint32_t max_nodes, int grid, uint32_t* ticket,
+                                    unsigned long long* stamp, cudaStream_t stream);
 int scan_tma_max_clusters();  // two-CTA clusters of that kernel resident at once on the current device
 
 }  // namespace rpl

@@ -93,7 +93,15 @@ __device__ void radix_pass(GeneralSmem& sm, const uint16_t* keyf, const uint32_t
 }
 
 __global__ void __launch_bounds__(GT, 1)
-    scan_general_kernel(ScanBatchArgs a, GeneralWorkspace ws, int all_scans) {
+    scan_general_kernel(ScanBatchArgs a, GeneralWorkspace ws, int all_scans, uint32_t* zero_next,
+                        unsigned long long* stamp) {
+  // Launched as the fast kernel's programmatic dependent (launch_scan_general, chained), this kernel may start before
+  // that kernel has finished: nothing it wrote -- the hand-off counter and list, the outputs -- is read before this
+  // wait, which returns once it has completed and its writes are visible.  A no-op in a plain launch.
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  stamp_start(stamp);
+  // the lane's next call's hand-off counter and scan ticket: no kernel of this call uses them (Lane::fallback_count)
+  if (zero_next && blockIdx.x == 0 && threadIdx.x < 2) zero_next[threadIdx.x] = 0u;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   GeneralSmem& sm = *reinterpret_cast<GeneralSmem*>(smem_raw);
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -289,16 +297,29 @@ __global__ void __launch_bounds__(GT, 1)
     }
     __syncthreads();
   }
+  if (stamp) {
+    __syncthreads();
+    stamp_end(stamp);
+  }
 }
 
 }  // namespace
 
 size_t scan_general_smem_bytes() { return sizeof(GeneralSmem); }
 
-cudaError_t launch_scan_general(const ScanBatchArgs& a, const GeneralWorkspace& ws, int grid,
-                                bool all_scans, cudaStream_t stream) {
-  scan_general_kernel<<<grid, GT, sizeof(GeneralSmem), stream>>>(a, ws, all_scans ? 1 : 0);
-  return cudaGetLastError();
+cudaError_t launch_scan_general(const ScanBatchArgs& a, const GeneralWorkspace& ws, int grid, bool all_scans,
+                                uint32_t* zero_next, bool chained, unsigned long long* stamp, cudaStream_t stream) {
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3((unsigned)grid);
+  cfg.blockDim = dim3(GT);
+  cfg.dynamicSmemBytes = sizeof(GeneralSmem);
+  cfg.stream = stream;
+  cfg.attrs = attr;
+  cfg.numAttrs = chained ? 1 : 0;
+  return cudaLaunchKernelEx(&cfg, scan_general_kernel, a, ws, all_scans ? 1 : 0, zero_next, stamp);
 }
 
 cudaError_t scan_general_configure() {

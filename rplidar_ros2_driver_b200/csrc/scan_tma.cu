@@ -442,9 +442,9 @@ __global__ void __launch_bounds__(kBlock, 2) scan_tma_kernel(ScanBatchArgs a, ui
 // warp for about 2 us per scan.  Both barriers complete one phase per streamed scan.
 //
 // Why this cannot deadlock: only the consumer threads touch the exchange barriers, and both CTAs walk
-// the same scans in the same order and take the same branches (every decision -- invalid, empty, no
-// measured node, duplicate key -- depends on counts[] or on the exchanged totals, identical on both
-// sides).  The waits, for consecutive streamed scans s - 1, s and s + 1 of the cluster:
+// the same scan sequence (see the comment above ClusterSmem; invalid and empty scans never enter it)
+// and take the same branches (no measured node, duplicate key -- decided on the exchanged totals,
+// identical on both sides).  The waits, for consecutive streamed scans s - 1, s and s + 1 of the cluster:
 //   * The producer fills scan by scan and slot by slot and waits only on its own consumers' arrives: to load
 //     chunk j of scan s + 1 into a held slot it waits for their mark of slot j of scan s; into any other slot,
 //     for their place pass of scan s over slot j (a slot scan s does not use is free already).
@@ -477,6 +477,25 @@ static_assert(kHeld >= 0 && kHeld <= kClusterSlots, "held slots are a prefix of 
 // 2 / 4 / 6 slots take 0.744-0.745 / 0.744-0.745 / 0.752 ms (DESIGN.md §5.1).
 constexpr uint32_t kMarkLag = 4;
 
+// The scan sequence of a cluster.  A static round robin (cluster c takes scans c, c + C, c + 2 C, ... of C clusters)
+// left the clusters ending up to 37 us apart on an H100 (DESIGN.md §5.1): clusters of the same work do not run at the
+// same rate.  So rank 0's producer draws the scans at run time: the cluster's first two candidates are static (c and
+// c + C), every later one comes from the call's ticket counter (2 C + atomicAdd(ticket, 1)), and without a ticket
+// (single scans) the round robin goes on.  It reports the scans that are not streamed as the consumers' writer did,
+// and keeps the streamed ones, in order, in a ring of kSeqSlots entries: seq[j % kSeqSlots] is the cluster's j-th
+// scan, kSeqEnd once there is none.  It draws entry j + 2 once it has issued every load of entry j, so that both
+// producers know each next scan while the current one still loads.  Rank 1 learns entries 0 and 1 from rank 0's ring
+// after the first cluster barrier, and entry k + 2 with the exchange of entry k (inbox_next), which its consumer
+// thread 0 then writes into its own ring.
+//   Ring reuse.  Rank 0: its producer writes entry j + 2 after loading entry j's chunk 0 into slot 0, which needed
+// every consumer warp's mark of entry j - 1's chunk 0, made after those threads had read entry j - 1 and so entry
+// j - 2, the entry that slot (j + 2) % kSeqSlots held: no consumer can still be reading it.  Rank 1: its consumers read
+// in order behind their own thread 0; its producer, which may run ahead through scans with no chunk of its own, frees
+// each entry on seq_empty, and thread 0 waits there before it overwrites the entry.  That producer never waits on
+// thread 0 for anything but entries already sent, so the wait ends.
+constexpr int kSeqSlots = 4;
+constexpr uint32_t kSeqEnd = 0xFFFFFFFFu;
+
 struct __align__(128) ClusterSmem {
   uint8_t bytemap[kKeySpace];                // presence map of this CTA's nodes (swizzled)
   uint2 tile[kClusterSlots][CH];             // this CTA's half of the scan: chunk 2 j + rank in slot j
@@ -486,17 +505,24 @@ struct __align__(128) ClusterSmem {
   unsigned long long empty[kClusterSlots];
   unsigned long long inbox_full;             // the peer wrote inbox and inbox_count
   unsigned long long peer_free;              // the peer read the words this CTA wrote into its inbox
+  unsigned long long seq_full[kSeqSlots];    // seq[j % kSeqSlots] holds the cluster's j-th scan
+  unsigned long long seq_empty[kSeqSlots];   // rank 1: its producer has read the entry (rank 0 needs none, below)
+  uint32_t seq[kSeqSlots];                   // the cluster's scan sequence (kSeqEnd after its last scan)
   uint32_t red[4 * kCWarps];
   uint32_t inbox_count;                      // the peer's measured-node count (written remotely)
+  uint32_t inbox_next;                       // rank 1: the scan two places ahead in the sequence (written remotely)
   uint32_t valid_count;
   uint32_t totV;
 };
 static_assert(sizeof(ClusterSmem) <= 232448, "one CTA per SM: at most 227 KB of dynamic shared memory");
-constexpr uint32_t kInboxBytes = sizeof(ClusterSmem::inbox) + sizeof(uint32_t);  // words + count per scan
+// words + count per scan; rank 1's inbox also takes the sequence entry rank 0 sends along
+constexpr uint32_t kInboxBytes = sizeof(ClusterSmem::inbox) + sizeof(uint32_t);
 
 // serves Mode B without the ascended buffer for strides in (kSmallMaxNodes, kClusterMaxNodes], 16-byte
 // aligned scan bases; launched with cluster dims (2, 1, 1) and an even grid
-__global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchArgs a, uint32_t max_nodes) {
+__global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchArgs a, uint32_t max_nodes,
+                                                                      uint32_t* ticket, unsigned long long* stamp) {
+  stamp_start(stamp);
   extern __shared__ __align__(128) unsigned char smem_raw[];
   ClusterSmem& sm = *reinterpret_cast<ClusterSmem*>(smem_raw);
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -510,19 +536,61 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
     }
     mbar_init(&sm.inbox_full, 1);        // this CTA's arrive.expect_tx per scan + the peer's st.async bytes
     mbar_init(&sm.peer_free, 1);         // one remote arrive by the peer per scan
+    for (int i = 0; i < kSeqSlots; ++i) {
+      mbar_init(&sm.seq_full[i], 1);     // the entry's writer
+      mbar_init(&sm.seq_empty[i], 1);    // rank 1's producer
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
+  // rank 0's producer: the next streamed scan of the cluster, or kSeqEnd; the others are reported here
+  uint32_t drawn = 0;
+  bool ended = false;
+  auto claim = [&]() -> uint32_t {
+    while (!ended) {
+      const uint32_t k = drawn++;
+      const uint32_t s = k < 2 || !ticket ? s0 + k * s_step : 2u * s_step + atomicAdd(ticket, 1u);
+      if (s >= a.n_scans) break;
+      const uint32_t n = a.counts[s];
+      if (scan_is_streamed(n, a.stride, max_nodes)) return s;
+      if (n == 0) write_outcome_empty(a, s);  // ascendScanData: OPERATION_FAIL; publish_scan: nodes.empty() -> return
+      else write_outcome(a, s, kResultInvalidData, 0u, 0.0f);  // caller error: report, touch nothing
+    }
+    ended = true;
+    return kSeqEnd;
+  };
+  auto seq_put = [&](uint32_t j, uint32_t v) {
+    sm.seq[j % kSeqSlots] = v;
+    mbar_arrive(&sm.seq_full[j % kSeqSlots]);
+  };
+  auto seq_get = [&](uint32_t j) {
+    mbar_wait(&sm.seq_full[j % kSeqSlots], (j / kSeqSlots) & 1u);
+    return *(volatile uint32_t*)&sm.seq[j % kSeqSlots];
+  };
+  if (rank == 0 && warp == kCWarps && lane == 0) {  // entries 0 and 1, published after the cluster barrier
+    sm.seq[0] = claim();
+    sm.seq[1] = claim();
+  }
   cluster_sync_all();
+  if (rank == 0 && warp == kCWarps && lane == 0) {
+    mbar_arrive(&sm.seq_full[0]);
+    mbar_arrive(&sm.seq_full[1]);
+  }
+  if (rank == 1 && tid == 0) {  // entries 0 and 1 from rank 0's ring (written before the cluster barrier)
+    seq_put(0, ld_peer_u32(peer_addr(&sm.seq[0], 0)));
+    seq_put(1, ld_peer_u32(peer_addr(&sm.seq[1], 0)));
+  }
 
   if (warp == kCWarps) {
     // =========================== producer warp =========================================
     if (lane == 0) {
       const uint64_t pol_load = l2_policy_evict_normal();  // (see the L2 policy note above the kernel)
       uint32_t eph = 0xFFFFFFFFu;  // empty-barrier parity per slot: the first fill passes at once
-      for (uint32_t s = s0; s < a.n_scans; s += s_step) {
+      for (uint32_t js = 0;; ++js) {
+        const uint32_t s = seq_get(js);
+        if (rank == 1) mbar_arrive(&sm.seq_empty[js % kSeqSlots]);
+        if (s == kSeqEnd) break;
         const uint32_t n = a.counts[s];
-        if (!scan_is_streamed(n, a.stride, max_nodes)) continue;
         const uint2* base = a.nodes + (size_t)s * a.stride;
         const uint32_t nch = (n + CH - 1) / CH;
         const uint32_t mine = (nch + 1u - rank) >> 1;  // chunks c < nch with c & 1 == rank
@@ -536,6 +604,7 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
           mbar_expect_tx(&sm.full[j], bytes);
           tma_load_1d(&sm.tile[j][0], base + (size_t)c * CH, bytes, &sm.full[j], pol_load);
         }
+        if (rank == 0) seq_put(js + 2, claim());
       }
     }
     __syncwarp();
@@ -548,6 +617,7 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
     const uint32_t peer_inbox = peer_addr(sm.inbox, peer);
     const uint32_t peer_count = peer_addr(&sm.inbox_count, peer);
     const uint32_t peer_inbox_full = peer_addr(&sm.inbox_full, peer);
+    const uint32_t peer_next = peer_addr(&sm.inbox_next, peer);
     const uint32_t peer_peer_free = peer_addr(&sm.peer_free, peer);
     uint32_t fph = 0;                         // full-barrier parity per slot
     uint32_t in_par = 0, free_par = 1;        // exchange barriers: peer_free's first wait passes at once
@@ -558,18 +628,6 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
       if (lane == 0) mbar_arrive(&sm.empty[j]);
     };
 
-    // the first scan at or after s that runs through the tile; the writer reports the ones it passes over
-    auto next_streamed = [&](uint32_t s) {
-      for (; s < a.n_scans; s += s_step) {
-        const uint32_t n = a.counts[s];
-        if (scan_is_streamed(n, a.stride, max_nodes)) break;
-        if (writer) {
-          if (n == 0) write_outcome_empty(a, s);  // ascendScanData: OPERATION_FAIL; publish_scan: nodes.empty() -> return
-          else write_outcome(a, s, kResultInvalidData, 0u, 0.0f);  // caller error: report, touch nothing
-        }
-      }
-      return s;
-    };
     // this CTA's share of a streamed scan of n nodes (n = 0: no scan, no chunk)
     struct Half {
       uint32_t n, mine, mine_full, nheld;
@@ -629,7 +687,8 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
     // next_held[] (no local memory).
     uint2 held[kHeld > 0 ? kHeld : 1][kRounds];
     uint2 next_held[kHeld > 0 ? kHeld : 1][kRounds];
-    uint32_t s = next_streamed(s0);
+    uint32_t js = 0;  // the sequence entry of s
+    uint32_t s = seq_get(js);
     Half cur = half_of(s < a.n_scans ? a.counts[s] : 0u);
     if (s < a.n_scans) {  // the first scan is marked with no place pass to hide behind
       bytemap_clear(sm.bytemap, tid);
@@ -653,18 +712,25 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
         uint32_t wv[kWordsPerThread];
         static_assert(kWordsPerThread == 4, "the exchange moves one uint4 of bit-words per thread");
         fold_row(sm.bytemap, tid, wv);
-        if (tid == 0) mbar_expect_tx(&sm.inbox_full, kInboxBytes);  // this scan's phase: the peer's words + count
+        // this scan's phase: the peer's words + count (+ rank 1: sequence entry js + 2)
+        if (tid == 0) mbar_expect_tx(&sm.inbox_full, kInboxBytes + (rank == 1 ? 4u : 0u));
         mbar_wait_cluster(&sm.peer_free, free_par);  // the peer has read what this CTA sent for the last scan
         free_par ^= 1u;
         st_async_v4(peer_inbox + tid * 16u, make_uint4(wv[0], wv[1], wv[2], wv[3]), peer_inbox_full);
         if (warp == 0) {
           const uint32_t own = warp_sum(lane < kCWarps ? sm.red[lane] : 0u);
           if (lane == 0) st_async_u32(peer_count, own, peer_inbox_full);
+          if (lane == 0 && rank == 0) st_async_u32(peer_next, seq_get(js + 2), peer_inbox_full);
         }
         mbar_wait_cluster(&sm.inbox_full, in_par);
         in_par ^= 1u;
         const uint4 pw = sm.inbox[tid];
         const uint32_t other = sm.inbox_count;
+        if (rank == 1 && tid == 0) {  // entry js + 2 into this CTA's ring, once its producer has read entry js - 2
+          const uint32_t jn = js + 2;
+          mbar_wait(&sm.seq_empty[jn % kSeqSlots], ((jn / kSeqSlots) & 1u) ^ 1u);
+          seq_put(jn, sm.inbox_next);
+        }
         wv[0] |= pw.x;
         wv[1] |= pw.y;
         wv[2] |= pw.z;
@@ -684,7 +750,7 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
         if (M == 0) write_outcome_empty(a, s);
         else hand_to_general(a, s);  // duplicate keys, within a half or across the halves
       }
-      const uint32_t s2 = next_streamed(s + s_step);
+      const uint32_t s2 = seq_get(js + 1);
       const Half nx = half_of(s2 < a.n_scans ? a.counts[s2] : 0u);
 
       // ---- place this CTA's chunks of s by rank and mark those of s2 ----------------------------------------
@@ -743,9 +809,14 @@ __global__ void __launch_bounds__(kBlock, 1) scan_tma_cluster_kernel(ScanBatchAr
       }
       cur = nx;
       s = s2;
+      ++js;
     }
   }
+  // this CTA has no scan left: the general kernel, launched as this kernel's programmatic dependent, may be scheduled
+  // onto the SMs the finished CTAs free (it waits for this whole kernel before it reads anything)
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   cluster_sync_all();
+  stamp_end(stamp);
 }
 
 }  // namespace
@@ -782,10 +853,11 @@ struct ClusterLaunch {
 };
 }  // namespace
 
-cudaError_t launch_scan_tma_cluster(const ScanBatchArgs& a, uint32_t max_nodes, int grid, cudaStream_t stream) {
+cudaError_t launch_scan_tma_cluster(const ScanBatchArgs& a, uint32_t max_nodes, int grid, uint32_t* ticket,
+                                    unsigned long long* stamp, cudaStream_t stream) {
   if (grid <= 0 || (grid & 1) != 0) return cudaErrorInvalidValue;
   ClusterLaunch l(grid, stream);
-  return cudaLaunchKernelEx(&l.cfg, scan_tma_cluster_kernel, a, max_nodes);
+  return cudaLaunchKernelEx(&l.cfg, scan_tma_cluster_kernel, a, max_nodes, ticket, stamp);
 }
 
 int scan_tma_max_clusters() {

@@ -97,6 +97,12 @@ __device__ __forceinline__ void st_async_u32(uint32_t addr, uint32_t v, uint32_t
 __device__ __forceinline__ void mbar_arrive_remote(uint32_t addr) {
   asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(addr) : "memory");
 }
+// plain load from the peer CTA's shared memory (ordered by a cluster barrier between the peer's store and it)
+__device__ __forceinline__ uint32_t ld_peer_u32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared::cluster.u32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
 // wait for a phase completed by the peer's remote arrive: acquire at cluster scope, so that the peer's
 // shared-memory accesses before its arrive are visible (or complete) here
 __device__ __forceinline__ void mbar_wait_cluster(void* bar, uint32_t parity) {

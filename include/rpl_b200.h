@@ -571,6 +571,51 @@ typedef struct rpl_stream_counters {
 rpl_result rpl_capsule_stream_counters(rpl_capsule_stream* s, rpl_stream_counters* out /* [n_streams] */,
                                        const uint8_t* clear_mask /* [n_streams] */);
 
+/* Moving streams between sessions: a stream's carried state out of one session and into another, of any n_streams,
+ * strides and max_scans, on any context or GPU, so that a fleet can outgrow its session or move lidars between GPUs
+ * without losing a revolution.  Both calls take host memory and are synchronous: each waits for the session's device
+ * calls in flight, and an import is in place before any later push runs.
+ *   What a record holds: the stream's carried state -- the held capsule (express, ultra, dense, ultra-dense) or the
+ *            0x81 byte machine's unfinished record, the decoder's scan-start flag and smoothed distance, a byte
+ *            session's sync-byte search and unfinished frame, the open revolution and its scan-begin stamp, the held
+ *            capsule's receive time -- and its counters.  Not its lidar, cloud or frame settings (the masked set_*
+ *            calls), and not the outputs of the last push.
+ *   export:  one record per listed stream streams[i] (< n_streams; a stream may be listed twice), record i at records +
+ *            record_offsets[i], the offsets the exclusive scan of the record sizes each rounded up to 16 (the packing
+ *            rule of the node and message calls), *total_bytes their sum.  If *total_bytes > capacity nothing is
+ *            written but record_offsets and *total_bytes, and the call returns RPL_RESULT_INSUFFICIENT_MEMORY (capacity
+ *            0, records NULL: a size query).  Export changes nothing in the session: it is a checkpoint.  To move a
+ *            stream, export it, import it elsewhere, then reset it (or destroy the session).
+ *   import:  replaces the carried state and counters of stream streams[i] with record i (at records +
+ *            record_offsets[i], within [0, total_bytes)).  Nothing else changes: not the stream's settings, not the
+ *            other streams, and not the last push's clouds, nodes and messages.  On a mixed byte session the stream
+ *            takes the record's answer type (no reset), as set_answer_types would set it.  The record's stamps count
+ *            at the destination's next stamped push whatever the destination's own last push was.
+ *   Definition: push P1..Pk of a stream into session A, export it, import the record into a session B of the same
+ *            kind (framed or byte) and max_nodes whose stream has the same settings, push P(k+1)..Pn into B: A's
+ *            outputs up to k followed by B's are bit for bit those of one session fed P1..Pn, in every output of every
+ *            call (scans, stamps, state, nodes, clouds, messages) and every counter but scans_unreturned.
+ *   Record:  little-endian bytes, version RPL_STREAM_RECORD_VERSION: a 32-byte header (uint32 magic "RPLM", version,
+ *            kind 0 framed / 1 byte session, answer type, max_nodes, open length L, stamp flags, 0), the 192-byte held
+ *            record, for a capsule answer type in a byte session the 800-byte framer record, the open revolution's
+ *            stamp and the held receive time (uint64; flag bits 1 and 2: known), the 14 uint64 counters
+ *            (rpl_stream_counters) and L nodes of 8 bytes.
+ *   Errors:  export: a null session, streams or record_offsets (n > 0), total_bytes, records with capacity > 0, or a
+ *            stream out of range: RPL_RESULT_INVALID_DATA.  import: RPL_RESULT_INVALID_DATA, and the session is bit for
+ *            bit unchanged, when any pointer is null (n > 0), a destination is out of range or listed twice, a record
+ *            offset is not a multiple of 16 or a record lies partly outside [0, total_bytes), or a record's magic or
+ *            version is wrong, its kind differs, its max_nodes differs, its answer type is not the session's (a
+ *            mixed session: not in 0x81..0x86), L > max_nodes, its framer position is not below the frame size or its
+ *            0x81 byte-machine state is not in 0..4.  Every record is checked before anything is written.
+ *   Cost:    352 bytes per record + 8 per open node (1152 + 8 per node for a capsule answer type in a byte session);
+ *            one small copy of the open lengths (export), one copy of the records each way and one kernel. */
+#define RPL_STREAM_RECORD_VERSION 1u
+rpl_result rpl_capsule_stream_export(rpl_capsule_stream* s, const uint32_t* streams, uint32_t n, uint8_t* records,
+                                     uint64_t capacity, uint64_t* record_offsets /* [n] */, uint64_t* total_bytes);
+rpl_result rpl_capsule_stream_import(rpl_capsule_stream* s, const uint32_t* streams, uint32_t n,
+                                     const uint8_t* records, const uint64_t* record_offsets /* [n] */,
+                                     uint64_t total_bytes);
+
 /* Byte session: the session fed the RAW serial stream after the answer descriptor, any number of bytes per push, a
  * push ending anywhere -- what the SDK's protocol codec hands LIDARSampleDataUnpacker::onSampleData.  Per stream the
  * device also keeps the unpacker's state between frames, so for ANY split of a stream's bytes into pushes the scans

@@ -54,6 +54,7 @@ EXPORTS = [
     "rpl_capsule_stream_create", "rpl_capsule_stream_destroy", "rpl_capsule_stream_push", "rpl_capsule_stream_push_dev",
     "rpl_capsule_stream_reset", "rpl_capsule_stream_state", "rpl_capsule_stream_push_ts",
     "rpl_capsule_stream_push_ts_dev", "rpl_capsule_stream_counters",
+    "rpl_capsule_stream_export", "rpl_capsule_stream_import",
     "rpl_capsule_stream_create_bytes", "rpl_capsule_stream_push_bytes", "rpl_capsule_stream_push_bytes_dev",
     "rpl_capsule_stream_create_bytes_mixed", "rpl_capsule_stream_set_answer_types",
     "rpl_capsule_stream_push_bytes_ts", "rpl_capsule_stream_push_bytes_ts_dev",
@@ -245,6 +246,8 @@ def lib() -> C.CDLL:
         "rpl_capsule_stream_reset": ([vp, vp], u32),
         "rpl_capsule_stream_state": ([vp, vp, vp, vp], u32),
         "rpl_capsule_stream_counters": ([vp, vp, vp], u32),
+        "rpl_capsule_stream_export": ([vp, vp, u32, vp, u64, vp, vp], u32),
+        "rpl_capsule_stream_import": ([vp, vp, u32, vp, vp, u64], u32),
         "rpl_capsule_stream_push_ts": ([vp, vp, vp, PT, vp, PSP, vp, vp, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_push_ts_dev": ([vp, vp, vp, PT, vp, PSP, vp, vp, vp, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_create_bytes": ([vp, u32, u32, u32, u32, u32, C.POINTER(vp)], u32),
@@ -946,6 +949,32 @@ class CapsuleStreamSession:
         assert m is None or m.shape == (self.n_streams,)
         self._ctx._check(self._fn("counters")(self._h, _p(out), _p(m)))
         return out
+
+    def export_streams(self, streams):
+        """The carried state and counters of the listed streams as records (rpl_capsule_stream_export): (records
+        uint8 [total_bytes], offsets uint64 [len(streams)]), record i at records[offsets[i]:].  The session is left as
+        it was; import_streams puts the records into any session of the same kind and max_nodes."""
+        s = np.ascontiguousarray(streams, dtype=np.uint32).reshape(-1)
+        offsets, total = np.zeros(s.size, np.uint64), np.zeros(1, np.uint64)
+        rc = self._fn("export")(self._h, _p(s), s.size, None, 0, _p(offsets), _p(total))
+        if rc != RESULT_INSUFFICIENT_MEMORY or s.size == 0:
+            self._ctx._check(rc)
+        records = np.zeros(int(total[0]), np.uint8)
+        self._ctx._check(self._fn("export")(self._h, _p(s), s.size, _p(records), records.size, _p(offsets), _p(total)))
+        return records, offsets
+
+    def import_streams(self, streams, records, offsets):
+        """Stream streams[i] takes record i of export_streams' (records, offsets) (rpl_capsule_stream_import); its
+        settings, the other streams and the last push's outputs are left alone.  A record that does not fit the
+        session raises RplError (RESULT_INVALID_DATA) and changes nothing."""
+        s = np.ascontiguousarray(streams, dtype=np.uint32).reshape(-1)
+        r = np.ascontiguousarray(records, dtype=np.uint8).reshape(-1)
+        o = np.ascontiguousarray(offsets, dtype=np.uint64).reshape(-1)
+        assert o.size == s.size
+        self._ctx._check(self._fn("import")(self._h, _p(s), s.size, _p(r) if r.size else None, _p(o), r.size))
+        if hasattr(self, "ans_types"):  # a mixed session's streams take their records' types
+            for i, off in zip(s.tolist(), o.tolist()):
+                self.ans_types[i] = int(r[off + 12: off + 16].view(np.uint32)[0])
 
 
 class DenseStreamSession(CapsuleStreamSession):

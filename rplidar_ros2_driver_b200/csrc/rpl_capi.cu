@@ -19,6 +19,7 @@
 #include "cdr_args.h"
 #include "decode_args.h"
 #include "scan_args.h"
+#include "session_migrate_args.h"
 #include "session_nodes_args.h"
 
 namespace rpl {
@@ -1273,7 +1274,8 @@ rpl_result rpl_scan_views_dev(rpl_ctx* c, const rpl_node_hq* nodes, uint64_t nod
 // A stamped push (rpl_capsule_stream_push*_ts*) runs the stamped decoder (0x81) and assembler instead; they keep,
 // beside the carry, the open revolution's stamp (open_ts, per arena like carry_len) and, for express and ultra, the
 // held capsule's receive time (held_rx).  An unstamped push leaves both stale, so the next stamped push counts them as
-// unknown.
+// unknown (carry_stamped false); an import folds that into every stream's own values first, open_ts 0 and held_rx
+// kRxUnknown, since the stream it writes keeps the stamps its record carries.
 // A byte session (rpl_capsule_stream_create_bytes) takes the raw bytes of the serial stream instead of framed capsules.
 // On a capsule answer type each push is framed first (frame.cu's session instantiation, the search carried in the
 // framer record) into the session's own capsule slots, which the decoder then reads as a framed session's push;
@@ -1304,6 +1306,7 @@ struct rpl_capsule_stream {
   unsigned long long* held_rx = nullptr;        // [n_streams] express, ultra: receive time of the held capsule
   uint32_t* scan_ends = nullptr;                // 0x81: [n_streams][new nodes] end bytes of the scan-start records
   bool prev_stamped = true;                     // the last push had receive times (a fresh session holds nothing)
+  bool carry_stamped = true;                    // open_ts[parity] and held_rx hold every stream's stamps (else none)
   // a byte session of a capsule answer type (else null): the framer records, this push's framed capsules
   uint32_t* framer = nullptr;                   // [n_streams][kFramerWords]
   uint8_t* framed = nullptr;                    // [n_streams][stride_capsules][cap_bytes]
@@ -1351,6 +1354,9 @@ struct rpl_capsule_stream {
   unsigned char* push_msg_work = nullptr;
   unsigned long long* push_msg_extent = nullptr;
   cudaEvent_t push_msg_extent_ready[kLanes] = {}, push_msg_dir_order = nullptr;
+  // export / import (rpl_capsule_stream_export, _import): the device staging of the records and their tables
+  unsigned char* migrate_work = nullptr;
+  size_t migrate_work_bytes = 0;
 };
 
 static_assert(sizeof(rpl::StreamCounters) == sizeof(rpl_stream_counters) &&
@@ -1471,7 +1477,7 @@ WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0, bool per_stre
   w.held_rx = cs->held_rx + s0;
   w.slot_begin = cs->slot_begin + so;
   w.slot_end = cs->slot_end + so;
-  w.prev_stamped = cs->prev_stamped;
+  w.prev_stamped = cs->carry_stamped;
   w.counters = cs->counters + s0;
   w.counted_capsule_bytes = cs->bytes ? 0u : cs->cap_bytes;
   if (cs->framer) {
@@ -2425,7 +2431,7 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
                   [&](Carve&, uint32_t s0) { return session_chunk(cs, s0, per_stream, false); });
   }
   cs->parity ^= 1u;
-  cs->prev_stamped = sp != nullptr;
+  cs->prev_stamped = cs->carry_stamped = sp != nullptr;
   if (dev) RPL_CUDA(c, cudaEventRecord(cs->done, st), RPL_RESULT_OPERATION_FAIL);
   if (r == RPL_RESULT_OK) {
     cs->cloud_chunk = chunk;
@@ -3304,6 +3310,7 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   cudaFree(cs->clouds);
   cudaFree(cs->counters);
   cudaFree(cs->push_msg_work);
+  cudaFree(cs->migrate_work);
   cudaFreeHost(cs->push_msg_extent);
   for (cudaEvent_t e : cs->push_msg_extent_ready)
     if (e) cudaEventDestroy(e);
@@ -3431,6 +3438,224 @@ rpl_result rpl_capsule_stream_counters(rpl_capsule_stream* cs, rpl_stream_counte
     s = e;
   }
   RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);  // cleared before any later push runs
+  return RPL_RESULT_OK;
+}
+
+// ---- moving streams between sessions (DESIGN.md 5.7.1): records of each stream's carried state ----
+}  // extern "C"
+
+namespace {
+
+static_assert(rpl::kRecVersion == RPL_STREAM_RECORD_VERSION && rpl::kRecCounterBytes == sizeof(rpl_stream_counters),
+              "the record of include/rpl_b200.h");
+
+// a record's bytes, rounded up to 16: its fixed part (with the framer record for a capsule answer type in a byte
+// session) and L nodes
+uint64_t record_bytes(bool bytes, uint32_t ans_type, uint32_t L) {
+  return ((uint64_t)rpl::record_fixed_bytes(bytes && ans_type != RPL_ANS_MEASUREMENT) + 8ull * L + 15ull) & ~15ull;
+}
+
+uint32_t stream_type(const rpl_capsule_stream* cs, uint32_t s) { return cs->types.empty() ? cs->ans_type : cs->types[s]; }
+
+// The device staging of n records, `bytes` in all, then their tables: offsets [n], streams [n], types [n] (uploaded as
+// one block from `tables`), in args a.  No device call of the session may be in flight.
+rpl_result migrate_stage(rpl_capsule_stream* cs, uint64_t bytes, uint32_t n, const std::vector<unsigned char>& tables,
+                         rpl::MigrateArgs* a) {
+  rpl_ctx* c = cs->c;
+  const size_t rec = (size_t)((bytes + 15) & ~15ull), need = rec + tables.size();
+  if (cs->migrate_work_bytes < need) {
+    cudaFree(cs->migrate_work);
+    cs->migrate_work = nullptr;
+    cs->migrate_work_bytes = 0;
+    RPL_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&cs->migrate_work), need), RPL_RESULT_INSUFFICIENT_MEMORY);
+    cs->migrate_work_bytes = need;
+  }
+  RPL_CUDA(c, cudaMemcpyAsync(cs->migrate_work + rec, tables.data(), tables.size(), cudaMemcpyHostToDevice,
+                              c->lane[0].stream),
+           RPL_RESULT_OPERATION_FAIL);
+  const uint32_t p = cs->parity;
+  a->records = cs->migrate_work;
+  a->offsets = reinterpret_cast<const unsigned long long*>(cs->migrate_work + rec);
+  a->streams = reinterpret_cast<const uint32_t*>(cs->migrate_work + rec + (size_t)8 * n);
+  a->types = reinterpret_cast<const uint32_t*>(cs->migrate_work + rec + (size_t)12 * n);
+  a->n = n;
+  a->arena = reinterpret_cast<uint2*>(cs->arena[p]);
+  a->stride_nodes = cs->stride_nodes;
+  a->max_nodes = cs->max_nodes;
+  a->carry_len = cs->carry_len[p];
+  a->open_ts = cs->open_ts[p];
+  a->held_rx = cs->held_rx;
+  a->held = cs->held;
+  a->framer = cs->framer;
+  a->counters = cs->counters;
+  a->kind = cs->bytes ? 1u : 0u;
+  return RPL_RESULT_OK;
+}
+
+// the tables of migrate_stage: offsets, streams and (export) each record's answer type
+std::vector<unsigned char> migrate_tables(const uint64_t* offsets, const uint32_t* streams, const uint32_t* types,
+                                          uint32_t n) {
+  std::vector<unsigned char> t((size_t)16 * n, 0);
+  std::memcpy(t.data(), offsets, (size_t)8 * n);
+  std::memcpy(t.data() + (size_t)8 * n, streams, (size_t)4 * n);
+  if (types) std::memcpy(t.data() + (size_t)12 * n, types, (size_t)4 * n);
+  return t;
+}
+
+// Record i of an import into session cs (bytes [off, off + its size) of `records`, total bytes in all): whether
+// every field the unpack kernel and the next push read as a length, an index or a state is in range for cs, and the
+// record's answer type and open length.  Records come from outside the program: nothing is trusted.
+bool record_ok(rpl_capsule_stream* cs, const uint8_t* records, uint64_t off, uint64_t total, uint32_t* type,
+               uint32_t* L) {
+  rpl_ctx* c = cs->c;
+  if ((off & 15u) != 0 || off > total || total - off < rpl::kRecHeaderBytes) {
+    c->err = "a record offset is not a multiple of 16, or its header lies outside [0, total_bytes)";
+    return false;
+  }
+  uint32_t h[8];
+  std::memcpy(h, records + off, sizeof h);
+  if (h[rpl::kRecWordMagic] != rpl::kRecMagic || h[rpl::kRecWordVersion] != rpl::kRecVersion) {
+    c->err = "not a stream record of this version (magic or version)";
+    return false;
+  }
+  if (h[rpl::kRecWordKind] != (cs->bytes ? 1u : 0u)) {
+    c->err = "a record of a framed session into a byte session, or the reverse";
+    return false;
+  }
+  const uint32_t t = h[rpl::kRecWordType];
+  if (cs->types.empty() ? t != cs->ans_type : (t < RPL_ANS_MEASUREMENT || t > 0x86u)) {
+    c->err = "the record's answer type is not one the destination stream decodes";
+    return false;
+  }
+  if (h[rpl::kRecWordMaxNodes] != cs->max_nodes) {
+    c->err = "the record's max_nodes differs from the session's";
+    return false;
+  }
+  if (h[rpl::kRecWordOpen] > cs->max_nodes || (h[rpl::kRecWordFlags] & ~(rpl::kRecOpenKnown | rpl::kRecRxKnown)) != 0 ||
+      h[rpl::kRecWordReserved] != 0) {
+    c->err = "the record's open revolution is longer than max_nodes, or its flags are unknown";
+    return false;
+  }
+  if (record_bytes(cs->bytes, t, h[rpl::kRecWordOpen]) > total - off) {
+    c->err = "a record lies partly outside [0, total_bytes)";
+    return false;
+  }
+  const uint8_t* held = records + off + rpl::kRecHeaderBytes;
+  if (t == RPL_ANS_MEASUREMENT) {  // the byte machine's state: bytes of the unfinished record
+    uint32_t state;
+    std::memcpy(&state, held + 4 * rpl::kHeldOk, 4);
+    if (state > 4) {
+      c->err = "the record's 0x81 byte-machine state is not in 0..4";
+      return false;
+    }
+  } else if (cs->bytes) {  // the framer's search position: bytes of the unfinished frame
+    uint32_t f[2];
+    std::memcpy(f, held + rpl::kRecHeldBytes + 4 * rpl::kFramerPos, sizeof f);
+    static_assert(rpl::kFramerLost == rpl::kFramerPos + 1, "framer words");
+    if (f[0] >= rpl_capsule_bytes(t) || f[1] > 1) {
+      c->err = "the record's framer position is not below the frame size, or its lost flag is not 0 or 1";
+      return false;
+    }
+  }
+  *type = t;
+  *L = h[rpl::kRecWordOpen];
+  return true;
+}
+
+}  // namespace
+
+extern "C" {
+
+rpl_result rpl_capsule_stream_export(rpl_capsule_stream* cs, const uint32_t* streams, uint32_t n, uint8_t* records,
+                                     uint64_t capacity, uint64_t* record_offsets, uint64_t* total_bytes) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if ((n && (!streams || !record_offsets)) || !total_bytes || (capacity && !records)) {
+    c->err = "null streams, records, record_offsets or total_bytes";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  for (uint32_t i = 0; i < n; ++i)
+    if (streams[i] >= cs->n_streams) {
+      c->err = "a listed stream is not below n_streams";
+      return RPL_RESULT_INVALID_DATA;
+    }
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);  // host pushes return synchronised
+  // the offsets need every listed stream's open length: read back as rpl_capsule_stream_state reads it
+  std::vector<uint32_t> open(cs->n_streams), types(n);
+  if (n)
+    RPL_CUDA(c, cudaMemcpy(open.data(), cs->carry_len[cs->parity], (size_t)cs->n_streams * 4, cudaMemcpyDeviceToHost),
+             RPL_RESULT_OPERATION_FAIL);
+  uint64_t total = 0;
+  for (uint32_t i = 0; i < n; ++i) {
+    types[i] = stream_type(cs, streams[i]);
+    record_offsets[i] = total;
+    total += record_bytes(cs->bytes, types[i], open[streams[i]]);
+  }
+  *total_bytes = total;
+  if (total > capacity) {
+    c->err = "capacity is smaller than total_bytes";
+    return RPL_RESULT_INSUFFICIENT_MEMORY;
+  }
+  if (n == 0) return RPL_RESULT_OK;
+  rpl::MigrateArgs a{};
+  if (const rpl_result r = migrate_stage(cs, total, n, migrate_tables(record_offsets, streams, types.data(), n), &a);
+      r != RPL_RESULT_OK)
+    return r;
+  a.stamps_known = cs->carry_stamped ? 1u : 0u;
+  cudaStream_t st = c->lane[0].stream;
+  RPL_CUDA(c, rpl::launch_stream_pack(a, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+  c->launches++;
+  RPL_CUDA(c, cudaMemcpyAsync(records, a.records, total, cudaMemcpyDeviceToHost, st), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);
+  return RPL_RESULT_OK;
+}
+
+rpl_result rpl_capsule_stream_import(rpl_capsule_stream* cs, const uint32_t* streams, uint32_t n, const uint8_t* records,
+                                     const uint64_t* record_offsets, uint64_t total_bytes) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (n && (!streams || !records || !record_offsets)) {
+    c->err = "null streams, records or record_offsets";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  // every record is checked before anything is written: a failure leaves the session as it was
+  std::vector<uint8_t> seen(cs->n_streams, 0);
+  std::vector<uint32_t> types = cs->types;
+  for (uint32_t i = 0; i < n; ++i) {
+    const uint32_t s = streams[i];
+    if (s >= cs->n_streams || seen[s]) {
+      c->err = "a destination stream is not below n_streams, or is listed twice";
+      return RPL_RESULT_INVALID_DATA;
+    }
+    seen[s] = 1;
+    uint32_t t = 0, L = 0;
+    if (!record_ok(cs, records, record_offsets[i], total_bytes, &t, &L)) return RPL_RESULT_INVALID_DATA;
+    if (!types.empty()) types[s] = t;
+  }
+  if (n == 0) return RPL_RESULT_OK;
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);
+  rpl::MigrateArgs a{};
+  if (const rpl_result r = migrate_stage(cs, total_bytes, n, migrate_tables(record_offsets, streams, nullptr, n), &a);
+      r != RPL_RESULT_OK)
+    return r;
+  cudaStream_t st = c->lane[0].stream;
+  RPL_CUDA(c, cudaMemcpyAsync(a.records, records, total_bytes, cudaMemcpyHostToDevice, st), RPL_RESULT_OPERATION_FAIL);
+  if (!cs->carry_stamped) {
+    // the last push kept no stamps, which made every stream's count as unknown: say so per stream, so that the
+    // imported streams' stamps count at the next stamped push and the others' still do not
+    RPL_CUDA(c, cudaMemsetAsync(cs->open_ts[cs->parity], 0, (size_t)cs->n_streams * 8, st), RPL_RESULT_OPERATION_FAIL);
+    static_assert(rpl::kRxUnknown == ~0ull, "held_rx's unknown is all ones");
+    RPL_CUDA(c, cudaMemsetAsync(cs->held_rx, 0xFF, (size_t)cs->n_streams * 8, st), RPL_RESULT_OPERATION_FAIL);
+    cs->carry_stamped = true;
+  }
+  // The unpack writes the next push's arena (parity) alone.  The last push's views, which its clouds, nodes and
+  // messages read, point into the arena it decoded into (cloud_arena, the other one), so they stay as they are.
+  RPL_CUDA(c, rpl::launch_stream_unpack(a, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+  c->launches++;
+  RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);  // in place before any later push runs
+  if (types != cs->types) return set_types(cs, std::move(types));     // a mixed session's streams take the record's type
   return RPL_RESULT_OK;
 }
 

@@ -109,6 +109,7 @@ typedef struct rpl_scan_params {
                                      revolutions of at most 8192 nodes; for A/B measurements */
 #define RPL_FLAG_PER_STREAM 8u    /* stream sessions: every stream's own rpl_lidar_settings (rpl_capsule_stream_set_lidars)
                                      instead of this struct's settings and the push's timing; other calls ignore it */
+/* RPL_FLAG_PER_STREAM_FILTERS 16u: stream sessions' LaserScan filters, defined with rpl_scan_filter_settings below */
 
 /* per-scan path report (optional output) */
 #define RPL_PATH_FAST 0u    /* tie-free scan: bitmap-rank kernel */
@@ -994,6 +995,58 @@ typedef struct rpl_cloud_settings {
 } rpl_cloud_settings;   /* 28 bytes; the first 24 are laid out as in rpl_cloud_params */
 rpl_result rpl_capsule_stream_set_clouds(rpl_capsule_stream* s, const rpl_cloud_settings* settings /* [n_streams] */,
                                          const uint8_t* stream_mask /* nullable: all */);
+
+/* LaserScan filters (DESIGN.md 5.7.1 "LaserScan filters"; INTEGRATION.md 4g): the chain a laser_filters node behind
+ * the driver runs, on the device, as a pure function F(settings, scan) of the published LaserScan (ranges,
+ * intensities, angle_increment; angle_min 0; Mode A / B and the inversion applied).  Stages, in order, each deciding
+ * every beam from the previous stage's whole output:
+ *   1. angular mask: beam i (angle fl(i * angle_increment)) inside a sector mask_lo[k] <= a <= mask_hi[k] (radians;
+ *      lo > hi: an unused sector; a sector through 0 is given as two);
+ *   2. range window: r < range_lo or r > range_hi;
+ *   3. intensity floor: intensity < intensity_min;
+ *   4. speckle (speckle_window > 0): fewer than speckle_min_neighbours beams within speckle_window beams (no wrap)
+ *      whose range differs from r by at most speckle_max_diff;
+ *   5. veiling points (shadow_window > 0): the far beam of a pair at most shadow_window beams apart whose segment
+ *      makes an angle below shadow_angle (radians) with the near beam's line of sight.
+ * A removed beam's range becomes the quiet NaN 0x7FC00000 (REP 117); intensities, beam counts, increments and message
+ * sizes never change, and a beam whose range is already non-finite is never tested.  oracle/scan_filter_oracle.py is
+ * the bit-exact definition.  Limits: windows <= 16, speckle_min_neighbours <= 2 * speckle_window, shadow_angle in
+ * (0, pi/2) when shadow_window > 0, range_lo <= range_hi, no NaN: otherwise RPL_RESULT_INVALID_DATA.  A disabled
+ * entry (enabled 0) leaves the scan as it is. */
+typedef struct rpl_scan_filter_settings {
+  float mask_lo[4];                /* offset 0 */
+  float mask_hi[4];                /* 16 */
+  float range_lo;                  /* 32 */
+  float range_hi;                  /* 36 */
+  float intensity_min;             /* 40 */
+  float speckle_max_diff;          /* 44: metres */
+  float shadow_angle;              /* 48: radians */
+  uint32_t speckle_window;         /* 52: 0 disables the speckle stage */
+  uint32_t speckle_min_neighbours; /* 56 */
+  uint32_t shadow_window;          /* 60: 0 disables the veiling stage */
+  uint8_t enabled;                 /* 64 */
+  uint8_t pad[3];
+} rpl_scan_filter_settings;        /* 68 bytes */
+/* Stateless: F(*settings, .) in place on n_scans rows laid out as rpl_scan_batch_dev writes them (device arrays):
+ * ranges / intensities [n_scans][stride], beam_counts and angle_increment [n_scans].  stride <= 8192.  Asynchronous on
+ * `stream` (NULL: the context's stream). */
+rpl_result rpl_scan_filter_batch_dev(rpl_ctx* c, const rpl_scan_filter_settings* settings, float* ranges,
+                                     const float* intensities, const uint32_t* beam_counts,
+                                     const float* angle_increment, uint32_t n_scans, uint32_t stride, void* stream);
+/* Per-stream filters of a stream session.
+ *   set_scan_filters: synchronous (it waits for the session's device calls in flight).  Copies settings[s] for every
+ *            stream whose stream_mask entry is non-zero (NULL = all); the first call must set every stream.  A null
+ *            settings, a first call that leaves a stream out, or a masked entry outside the limits:
+ *            RPL_RESULT_INVALID_DATA, and the table is unchanged.
+ *   RPL_FLAG_PER_STREAM_FILTERS in rpl_scan_params.flags (push, push_dev, push_ts*, push_bytes*, laserscan_msgs[_dev],
+ *            push_laserscan_msgs[_dev]): every scan of stream s is F(entry s, scan) of the scan the call without the
+ *            flag gives; a disabled stream's are those scans.  It combines with every other RPL_FLAG_*.  A device push
+ *            with the flag needs angle_increment.  Before the first set_scan_filters: RPL_RESULT_INVALID_DATA.  Cloud,
+ *            node and counter calls ignore it; export / import records do not carry the table. */
+#define RPL_FLAG_PER_STREAM_FILTERS 16u
+rpl_result rpl_capsule_stream_set_scan_filters(rpl_capsule_stream* s,
+                                               const rpl_scan_filter_settings* settings /* [n_streams] */,
+                                               const uint8_t* stream_mask /* nullable: all */);
 
 /* ---- LaserScan / PointCloud2 -> wire (SURVEY.md 8(f) rank 3) ---------------------------- */
 /* The serialised message the RMW layer would produce from the message the reference publishes

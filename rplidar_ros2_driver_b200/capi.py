@@ -26,6 +26,7 @@ FLAG_FORCE_GENERAL = 1
 FLAG_NO_TMA = 2
 FLAG_NO_SMALL = 4
 FLAG_PER_STREAM = 8
+FLAG_PER_STREAM_FILTERS = 16
 CLOUD_NO_FUSED = 1
 CLOUD_PER_STREAM = 2
 CLOUD_PER_STREAM_CHAIN = 4
@@ -63,6 +64,7 @@ EXPORTS = [
     "rpl_capsule_stream_cloud_msgs", "rpl_capsule_stream_cloud_msgs_dev", "rpl_capsule_stream_nodes",
     "rpl_capsule_stream_nodes_dev", "rpl_capsule_stream_push_laserscan_msgs", "rpl_capsule_stream_push_laserscan_msgs_dev",
     "rpl_capsule_stream_push_cloud_msgs", "rpl_capsule_stream_push_cloud_msgs_dev",
+    "rpl_scan_filter_batch_dev", "rpl_capsule_stream_set_scan_filters",
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -131,6 +133,25 @@ class CloudSettings(C.Structure):
         ("voxel_size", C.c_float),
         ("sor_k", C.c_uint32),
         ("sor_alpha", C.c_float),
+        ("enabled", C.c_uint8),
+        ("pad", C.c_uint8 * 3),
+    ]
+
+
+class ScanFilterSettings(C.Structure):
+    """rpl_scan_filter_settings: one LaserScan filter chain (angular mask, range window, intensity floor, speckle and
+    veiling-point removal; 68 bytes).  oracle/scan_filter_oracle.py defines what it does."""
+    _fields_ = [
+        ("mask_lo", C.c_float * 4),
+        ("mask_hi", C.c_float * 4),
+        ("range_lo", C.c_float),
+        ("range_hi", C.c_float),
+        ("intensity_min", C.c_float),
+        ("speckle_max_diff", C.c_float),
+        ("shadow_angle", C.c_float),
+        ("speckle_window", C.c_uint32),
+        ("speckle_min_neighbours", C.c_uint32),
+        ("shadow_window", C.c_uint32),
         ("enabled", C.c_uint8),
         ("pad", C.c_uint8 * 3),
     ]
@@ -262,6 +283,8 @@ def lib() -> C.CDLL:
         "rpl_capsule_stream_set_frames": ([vp, vp, vp], u32),
         "rpl_capsule_stream_set_lidars": ([vp, vp, vp], u32),
         "rpl_capsule_stream_set_clouds": ([vp, vp, vp], u32),
+        "rpl_capsule_stream_set_scan_filters": ([vp, vp, vp], u32),
+        "rpl_scan_filter_batch_dev": ([vp, C.POINTER(ScanFilterSettings), vp, vp, vp, vp, u32, u32, vp], u32),
         "rpl_capsule_stream_laserscan_msgs": ([vp, PSP, C.c_int64, vp, u64, vp, vp, vp], u32),
         "rpl_capsule_stream_laserscan_msgs_dev": ([vp, PSP, C.c_int64, vp, u64, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_cloud_msgs": ([vp, PCP, C.c_int64, vp, u64, vp, vp, vp], u32),
@@ -304,6 +327,19 @@ def cloud_settings(range_min=0.15, range_max=0.0, intensity_min=0.0, voxel_size=
     """range_max 0: the stream's range_max of set_frames."""
     return CloudSettings(float(range_min), float(range_max), float(intensity_min), float(voxel_size), int(sor_k),
                          float(sor_alpha), int(bool(enabled)), (C.c_uint8 * 3)(0, 0, 0))
+
+
+def scan_filter_settings(mask=(), range_lo=float("-inf"), range_hi=float("inf"), intensity_min=float("-inf"),
+                         speckle_window=0, speckle_min_neighbours=0, speckle_max_diff=0.0, shadow_window=0,
+                         shadow_angle=0.0, enabled=True) -> ScanFilterSettings:
+    """mask: up to four (lo, hi) sectors in radians (the others unused); the defaults remove nothing."""
+    assert len(mask) <= 4
+    lo = [float(a) for a, _ in mask] + [float("inf")] * (4 - len(mask))
+    hi = [float(b) for _, b in mask] + [float("-inf")] * (4 - len(mask))
+    return ScanFilterSettings((C.c_float * 4)(*lo), (C.c_float * 4)(*hi), float(range_lo), float(range_hi),
+                              float(intensity_min), float(speckle_max_diff), float(shadow_angle), int(speckle_window),
+                              int(speckle_min_neighbours), int(shadow_window), int(bool(enabled)),
+                              (C.c_uint8 * 3)(0, 0, 0))
 
 
 def _timing(t):
@@ -638,6 +674,13 @@ class Context:
             _p(out["scans_per_stream"])))
         return out
 
+    def scan_filter_batch_dev(self, settings: ScanFilterSettings, ranges, intensities, beam_counts, angle_increment,
+                              n_scans, stride, stream=None):
+        """The LaserScan filters in place on rows of rpl_scan_batch_dev's layout (device addresses)."""
+        self._check(self._L.rpl_scan_filter_batch_dev(self._h, C.byref(settings), _p(ranges), _p(intensities),
+                                                      _p(beam_counts), _p(angle_increment), n_scans, stride,
+                                                      _p(stream)))
+
     def cloud_fuse_dev(self, xyzi, point_counts, n_scans, stride, fused, offsets, total, stream=None):
         self._check(self._L.rpl_cloud_fuse_dev(self._h, _p(xyzi), _p(point_counts), n_scans, stride, _p(fused),
                                                _p(offsets), _p(total), _p(stream)))
@@ -780,6 +823,16 @@ class CapsuleStreamSession:
         m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
         assert m is None or m.shape == (self.n_streams,)
         self._ctx._check(self._fn("set_clouds")(self._h, C.cast(arr, C.c_void_p), _p(m)))
+
+    def set_scan_filters(self, settings, mask=None):
+        """Per stream the LaserScan filters (n_streams ScanFilterSettings, see scan_filter_settings) that pushes and
+        LaserScan message calls with FLAG_PER_STREAM_FILTERS apply.  Only the entries where mask is true are copied
+        (None: all); the first call must set every stream."""
+        assert len(settings) == self.n_streams
+        arr = (ScanFilterSettings * self.n_streams)(*settings)
+        m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
+        assert m is None or m.shape == (self.n_streams,)
+        self._ctx._check(self._fn("set_scan_filters")(self._h, C.cast(arr, C.c_void_p), _p(m)))
 
     def _msgs(self, name, params, clock_offset_ns, msgs, packed):
         ns = self.n_streams * self.max_scans

@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <initializer_list>
@@ -19,6 +20,7 @@
 #include "cdr_args.h"
 #include "decode_args.h"
 #include "scan_args.h"
+#include "scan_filter_args.h"
 #include "session_migrate_args.h"
 #include "session_nodes_args.h"
 
@@ -565,6 +567,72 @@ rpl_result rpl_scan_batch_dev(rpl_ctx* c, const rpl_node_hq* nodes, const uint32
   // through status[s] = RPL_RESULT_INVALID_DATA by the kernels (nothing else is written for it)
   return enqueue_scan(c, c->lane[0], nodes, counts, n_scans, stride, params, nodes_out, ranges,
                       intensities, beam_counts, angle_increment, status, path, st);
+}
+
+static_assert(sizeof(rpl_scan_filter_settings) == 68 && sizeof(rpl::ScanFilter) == sizeof(rpl_scan_filter_settings) &&
+                  offsetof(rpl_scan_filter_settings, range_lo) == offsetof(rpl::ScanFilter, range_lo) &&
+                  offsetof(rpl_scan_filter_settings, shadow_angle) == offsetof(rpl::ScanFilter, shadow_tan) &&
+                  offsetof(rpl_scan_filter_settings, speckle_window) == offsetof(rpl::ScanFilter, speckle_window) &&
+                  offsetof(rpl_scan_filter_settings, enabled) == 64,
+              "rpl::ScanFilter must be laid out as rpl_scan_filter_settings, tan(shadow_angle) for shadow_angle");
+
+namespace {
+
+// the limits of rpl_scan_filter_settings (oracle/scan_filter_oracle.py settings_ok)
+bool scan_filter_ok(rpl_ctx* c, const rpl_scan_filter_settings& e) {
+  bool nan = std::isnan(e.range_lo) || std::isnan(e.range_hi) || std::isnan(e.intensity_min) ||
+             std::isnan(e.speckle_max_diff) || std::isnan(e.shadow_angle);
+  for (int k = 0; k < 4; ++k) nan = nan || std::isnan(e.mask_lo[k]) || std::isnan(e.mask_hi[k]);
+  const char* why = nullptr;
+  if (nan) why = "a scan filter parameter is NaN";
+  else if (e.speckle_window > rpl::kScanFilterMaxWindow || e.shadow_window > rpl::kScanFilterMaxWindow)
+    why = "speckle_window and shadow_window must be <= 16";
+  else if (e.speckle_min_neighbours > 2 * e.speckle_window) why = "speckle_min_neighbours > 2 * speckle_window";
+  else if (!(e.range_lo <= e.range_hi)) why = "range_lo > range_hi";
+  else if (e.shadow_window > 0 && !((double)e.shadow_angle > 0.0 && (double)e.shadow_angle < M_PI / 2))
+    why = "shadow_angle must be in (0, pi/2)";
+  if (why) c->err = why;
+  return why == nullptr;
+}
+
+// an entry as the kernel reads it: tan(shadow_angle) in double, rounded to float, once
+rpl::ScanFilter scan_filter_entry(const rpl_scan_filter_settings& e) {
+  rpl::ScanFilter f{};
+  std::memcpy(&f, &e, offsetof(rpl_scan_filter_settings, enabled));
+  f.shadow_tan = (float)std::tan((double)e.shadow_angle);
+  f.enabled = e.enabled ? 1u : 0u;
+  return f;
+}
+
+}  // namespace
+
+rpl_result rpl_scan_filter_batch_dev(rpl_ctx* c, const rpl_scan_filter_settings* settings, float* ranges,
+                                     const float* intensities, const uint32_t* beam_counts,
+                                     const float* angle_increment, uint32_t n_scans, uint32_t stride, void* stream) {
+  if (!c) return RPL_RESULT_INVALID_DATA;
+  if (!settings || !ranges || !intensities || !beam_counts || !angle_increment) {
+    c->err = "null settings, ranges, intensities, beam_counts or angle_increment";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  if (n_scans != 0 && (stride == 0 || stride > rpl::kScanFilterMaxBeams)) {
+    c->err = "stride must be in [1, 8192]";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  if (!scan_filter_ok(c, *settings)) return RPL_RESULT_INVALID_DATA;
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
+  if (!settings->enabled || n_scans == 0) return RPL_RESULT_OK;
+  rpl::ScanFilterArgs a{};
+  a.one = scan_filter_entry(*settings);
+  a.ranges = ranges;
+  a.intensities = intensities;
+  a.stride = stride;
+  a.beam_counts = beam_counts;
+  a.angle_increment = angle_increment;
+  a.n_scans = n_scans;
+  RPL_CUDA(c, rpl::launch_scan_filter(a, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+  c->launches++;
+  return RPL_RESULT_OK;
 }
 
 // ---- host-buffer batch: chunked over the two lanes so that the H2D copy of chunk i+1, the
@@ -1344,6 +1412,10 @@ struct rpl_capsule_stream {
   uint32_t cloud_routes = 0, cloud_sor_k = 0;
   bool cloud_voxel = false;
   std::string clouds_bad;
+  // the per-stream LaserScan filters (rpl_capsule_stream_set_scan_filters) that calls with RPL_FLAG_PER_STREAM_FILTERS
+  // read: the entries as set (empty until the first call sets every stream) and as the kernel reads them
+  std::vector<rpl_scan_filter_settings> filters_host;
+  rpl::ScanFilter* filters = nullptr;           // [n_streams] device
   unsigned char* node_work = nullptr;           // the tables of a nodes call (NodeWork)
   // [n_streams] device, zeroed at create: what every push decoded and lost (rpl_capsule_stream_counters); a stream's
   // record is written by the one CTA of each kernel that serves the stream
@@ -1444,11 +1516,46 @@ struct WireChunk {
   uint32_t counted_capsule_bytes;
   // the session's per-stream chains, which a PointCloud2 push with RPL_CLOUD_PER_STREAM_CHAIN reads
   CloudChains clouds;
+  // a LaserScan push with RPL_FLAG_PER_STREAM_FILTERS: the chunk's first stream's entry of the session's filters, when
+  // some stream of the chunk has its filters enabled (else nullptr: no filter launch)
+  const rpl::ScanFilter* filters;
 };
 
-// session cs's chunk from stream s0 in the push under way (arena cs->parity); per_stream: RPL_FLAG_PER_STREAM; dev: a
-// device push's chunking (else a host push's)
-WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0, bool per_stream, bool dev) {
+// the filters of a call with RPL_FLAG_PER_STREAM_FILTERS over streams [s0, s0 + ns): the table at s0, or nullptr when
+// the call has no flag or no stream of the range is enabled
+const rpl::ScanFilter* filters_at(const rpl_capsule_stream* cs, const rpl_scan_params* p, uint32_t s0, uint32_t ns) {
+  if ((p->flags & RPL_FLAG_PER_STREAM_FILTERS) == 0 || cs->filters_host.empty()) return nullptr;
+  const uint32_t e = std::min(cs->n_streams, s0 + ns);
+  for (uint32_t s = s0; s < e; ++s)
+    if (cs->filters_host[s].enabled) return cs->filters + s0;
+  return nullptr;
+}
+
+// the filters at `filters` over n scan slots, per slots per entry: rows (ranges / intens at stride) or, with msg_out,
+// the placed messages of `place`; beams and inc the scan kernels' beam counts and angle increments of the slots
+rpl_result filter_scans(rpl_ctx* c, const rpl::ScanFilter* filters, uint32_t per, uint32_t n, float* ranges,
+                        const float* intens, uint32_t stride, uint8_t* msg_out, const unsigned long long* place,
+                        const uint32_t* beams, const float* inc, cudaStream_t st) {
+  rpl::ScanFilterArgs a{};
+  a.filters = filters;
+  a.per_filter = per;
+  a.ranges = ranges;
+  a.intensities = intens;
+  a.stride = stride;
+  a.msg_out = msg_out;
+  a.place = place;
+  a.beam_counts = beams;
+  a.angle_increment = inc;
+  a.n_scans = n;
+  RPL_CUDA(c, rpl::launch_scan_filter(a, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+  c->launches++;
+  return RPL_RESULT_OK;
+}
+
+// session cs's chunk from stream s0 in the push under way (arena cs->parity) with params' flags (RPL_FLAG_PER_STREAM,
+// RPL_FLAG_PER_STREAM_FILTERS); dev: a device push's chunking (else a host push's)
+WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0, const rpl_scan_params* params, bool dev) {
+  const bool per_stream = (params->flags & RPL_FLAG_PER_STREAM) != 0;
   const uint32_t p = cs->parity, sc = cs->stride_capsules;
   const size_t sn = (size_t)s0 * cs->stride_nodes, so = (size_t)s0 * cs->max_scans;
   WireChunk w{};
@@ -1498,6 +1605,7 @@ WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0, bool per_stre
     w.lidar_modes = cs->lidar_modes;
   }
   w.clouds = chains_at(cs, s0);
+  w.filters = filters_at(cs, params, s0, dev ? cs->chunk_dev : cs->chunk_host);
   return w;
 }
 
@@ -1779,9 +1887,13 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
   if (r != RPL_RESULT_OK) return r;
   const LidarTable lt{w.lidars, w.max_scans, w.lidar_modes};
   const uint2* views = reinterpret_cast<const uint2*>(w.views);
-  if (!m)
-    return enqueue_scan(c, l, w.nodes, w.scan_len, ns * w.max_scans, w.max_nodes, params, nullptr, ranges, intens, beams,
-                        inc, nullptr, nullptr, st, views, (unsigned long long)ns * w.stride_nodes, lt);
+  if (!m) {
+    r = enqueue_scan(c, l, w.nodes, w.scan_len, ns * w.max_scans, w.max_nodes, params, nullptr, ranges, intens, beams,
+                     inc, nullptr, nullptr, st, views, (unsigned long long)ns * w.stride_nodes, lt);
+    if (r != RPL_RESULT_OK || !w.filters) return r;
+    return filter_scans(c, w.filters, w.max_scans, ns * w.max_scans, ranges, intens, w.max_nodes, nullptr, nullptr,
+                        beams, inc, st);
+  }
   if (m->cloud) {  // the scans as last_push_scans will give them once the push is done
     rpl::ScanBatchArgs a{};
     a.nodes = reinterpret_cast<const uint2*>(w.nodes);
@@ -1822,6 +1934,8 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
   if (m->cloud) return m->extent_host ? RPL_RESULT_OK : cloud_push_write(c, w, ns, sp != nullptr, *m, 0, st);
   r = enqueue_scan(c, l, w.nodes, w.scan_len, ns * w.max_scans, w.max_nodes, params, nullptr, nullptr, nullptr, beams,
                    inc, nullptr, nullptr, st, views, (unsigned long long)ns * w.stride_nodes, lt, m->out, m->place);
+  if (r == RPL_RESULT_OK && w.filters)  // in place in the messages, before the header writer and the copies behind it
+    r = filter_scans(c, w.filters, w.max_scans, ns * w.max_scans, nullptr, nullptr, 0, m->out, m->place, beams, inc, st);
   if (r != RPL_RESULT_OK) return r;
   rpl::MsgWriteArgs a{};
   a.hdr = m->hdr;
@@ -2051,6 +2165,13 @@ bool lidars_ok(rpl_capsule_stream* cs) {
   return false;
 }
 
+// a call with RPL_FLAG_PER_STREAM_FILTERS needs the table
+bool filters_ok(rpl_capsule_stream* cs) {
+  if (!cs->filters_host.empty()) return true;
+  cs->c->err = "per-stream scan filters requested before rpl_capsule_stream_set_scan_filters set every stream";
+  return false;
+}
+
 // the table of a session call: the stream s0's entry on, when per_stream
 LidarTable lidar_table(const rpl_capsule_stream* cs, bool per_stream, uint32_t s0) {
   if (!per_stream) return LidarTable{};
@@ -2078,6 +2199,7 @@ bool capsule_stream_args_ok(rpl_capsule_stream* cs, const uint8_t* capsules, con
     c->err = "null capsules, counts, params or output buffer";
     return false;
   }
+  if ((params->flags & RPL_FLAG_PER_STREAM_FILTERS) != 0 && !filters_ok(cs)) return false;
   if ((params->flags & RPL_FLAG_PER_STREAM) != 0) {  // every stream's sample duration comes from the table
     if (!lidars_ok(cs)) return false;
   } else if (decodes_capsules(cs) && !sample_duration_ok(c, sample_duration_us)) {
@@ -2366,7 +2488,10 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
   if (!capsule_stream_args_ok(cs, in, counts, sample_duration_us, params, ranges, intensities, beam_counts,
                               scans_per_stream, pm != nullptr))
     return RPL_RESULT_INVALID_DATA;
-  const bool per_stream = (params->flags & RPL_FLAG_PER_STREAM) != 0;
+  if (dev && !pm && !angle_increment && (params->flags & RPL_FLAG_PER_STREAM_FILTERS) != 0) {
+    c->err = "a device push with RPL_FLAG_PER_STREAM_FILTERS needs angle_increment";
+    return RPL_RESULT_INVALID_DATA;
+  }
   const uint32_t chunk = dev ? cs->chunk_dev : cs->chunk_host;
   cudaStream_t st = nullptr;
   rpl_result r = RPL_RESULT_OK;
@@ -2398,7 +2523,7 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
         m.xyzi = pm->xyzi;
         m.points = pm->points;
       }
-      r = capsule_stream_chunk(c, c->lane[0], st, session_chunk(cs, s0, per_stream, true),
+      r = capsule_stream_chunk(c, c->lane[0], st, session_chunk(cs, s0, params, true),
                                std::min(chunk, cs->n_streams - s0), in + s0 * cs->in_stream, counts + s0,
                                sample_duration_us, params, pm ? nullptr : ranges + s0 * row,
                                pm ? nullptr : intensities + s0 * row, pm ? pm->w.beams + so : beam_counts + so,
@@ -2428,7 +2553,7 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
                      intensities, angle_increment, beam_counts, scans_per_stream, sp, sp ? sp->stride_chunks : 0u,
                      pm ? &hm : nullptr};
     r = push_host(c, h, cs->n_streams, chunk,
-                  [&](Carve&, uint32_t s0) { return session_chunk(cs, s0, per_stream, false); });
+                  [&](Carve&, uint32_t s0) { return session_chunk(cs, s0, params, false); });
   }
   cs->parity ^= 1u;
   cs->prev_stamped = cs->carry_stamped = sp != nullptr;
@@ -2712,6 +2837,40 @@ rpl_result stream_set_clouds(rpl_capsule_stream* cs, const rpl_cloud_settings* s
   return clouds_resolve(cs);
 }
 
+// the per-stream LaserScan filters: the masked entries of `settings` replace the table's, all or none
+rpl_result stream_set_scan_filters(rpl_capsule_stream* cs, const rpl_scan_filter_settings* settings,
+                                   const uint8_t* stream_mask) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!settings) {
+    c->err = "null settings";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  std::vector<rpl_scan_filter_settings> t = cs->filters_host;
+  if (t.empty()) {
+    for (uint32_t s = 0; s < cs->n_streams; ++s)
+      if (stream_mask && !stream_mask[s]) {
+        c->err = "the first rpl_capsule_stream_set_scan_filters call must set every stream";
+        return RPL_RESULT_INVALID_DATA;
+      }
+    t.resize(cs->n_streams);
+  }
+  for (uint32_t s = 0; s < cs->n_streams; ++s) {
+    if (stream_mask && !stream_mask[s]) continue;
+    if (!scan_filter_ok(c, settings[s])) return RPL_RESULT_INVALID_DATA;
+    t[s] = settings[s];
+  }
+  std::vector<rpl::ScanFilter> d(cs->n_streams);
+  for (uint32_t s = 0; s < cs->n_streams; ++s) d[s] = scan_filter_entry(t[s]);
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  if (!cs->filters) RPL_CUDA(c, dev_alloc(&cs->filters, cs->n_streams), RPL_RESULT_INSUFFICIENT_MEMORY);
+  RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);  // a push or messages call may still read it
+  RPL_CUDA(c, cudaMemcpy(cs->filters, d.data(), d.size() * sizeof(rpl::ScanFilter), cudaMemcpyHostToDevice),
+           RPL_RESULT_OPERATION_FAIL);
+  cs->filters_host = std::move(t);
+  return RPL_RESULT_OK;
+}
+
 // the PointCloud2 members between the header and the data: height 1, width, the fields x, y, z, intensity (float32,
 // count 1), is_bigendian 0, point_step 16, row_step, data length
 rpl::CloudTail cloud_tail() {
@@ -2778,6 +2937,9 @@ bool stream_msgs_args_ok(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* 
                               ? (static_cast<const rpl_scan_params*>(params)->flags & RPL_FLAG_PER_STREAM) != 0
                               : (static_cast<const rpl_cloud_params*>(params)->flags & RPL_CLOUD_PER_STREAM) != 0;
   if (per_stream && !lidars_ok(cs)) return false;
+  if (kind == rpl::MsgKind::kLaserScan &&
+      (static_cast<const rpl_scan_params*>(params)->flags & RPL_FLAG_PER_STREAM_FILTERS) != 0 && !filters_ok(cs))
+    return false;
   if (dev && ((reinterpret_cast<uintptr_t>(msgs) & 15u) || misaligned8(offsets) || misaligned8(total) ||
               (reinterpret_cast<uintptr_t>(sizes) & 3u))) {
     c->err = "msgs must be 16-byte aligned, msg_offsets and total_bytes 8-byte, msg_sizes 4-byte aligned";
@@ -2807,6 +2969,9 @@ rpl_result msgs_prepare(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* p
                        a.stride, p, nullptr, w.data + so * row, w.data + (NS + so) * row, w.counts + so, w.inc + so,
                        nullptr, nullptr, st, a.views, a.nodes_total,
                        lidar_table(cs, (p->flags & RPL_FLAG_PER_STREAM) != 0, s0));
+      if (const rpl::ScanFilter* f = filters_at(cs, p, s0, ns); r == RPL_RESULT_OK && f)
+        r = filter_scans(cs->c, f, cs->max_scans, a.n_scans, w.data + so * row, w.data + (NS + so) * row, cs->max_nodes,
+                         nullptr, nullptr, w.counts + so, w.inc + so, st);
     } else {
       r = stream_cloud_chunk(c, c->lane[0], last_push_scans(cs, s0, ns), lidars_at(cs, s0), chains_at(cs, s0),
                              cs->max_scans, static_cast<const rpl_cloud_params*>(params), w.data + so * row * 4,
@@ -3308,6 +3473,7 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   cudaFree(cs->node_work);
   cudaFree(cs->lidars);
   cudaFree(cs->clouds);
+  cudaFree(cs->filters);
   cudaFree(cs->counters);
   cudaFree(cs->push_msg_work);
   cudaFree(cs->migrate_work);
@@ -3797,6 +3963,11 @@ rpl_result rpl_capsule_stream_set_lidars(rpl_capsule_stream* s, const rpl_lidar_
 rpl_result rpl_capsule_stream_set_clouds(rpl_capsule_stream* s, const rpl_cloud_settings* settings,
                                          const uint8_t* stream_mask) {
   return stream_set_clouds(s, settings, stream_mask);
+}
+
+rpl_result rpl_capsule_stream_set_scan_filters(rpl_capsule_stream* s, const rpl_scan_filter_settings* settings,
+                                               const uint8_t* stream_mask) {
+  return stream_set_scan_filters(s, settings, stream_mask);
 }
 
 rpl_result rpl_capsule_stream_laserscan_msgs_dev(rpl_capsule_stream* s, const rpl_scan_params* params,

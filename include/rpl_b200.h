@@ -1008,9 +1008,11 @@ rpl_result rpl_capsule_stream_set_clouds(rpl_capsule_stream* s, const rpl_cloud_
  *      whose range differs from r by at most speckle_max_diff;
  *   5. veiling points (shadow_window > 0): the far beam of a pair at most shadow_window beams apart whose segment
  *      makes an angle below shadow_angle (radians) with the near beam's line of sight.
+ * With a footprint (rpl_scan_footprint below) its polygons run beside stages 1-3, deciding from the same input: the
+ * beams whose points lie inside a polygon (or outside an inverted one) are removed before speckle and veiling.
  * A removed beam's range becomes the quiet NaN 0x7FC00000 (REP 117); intensities, beam counts, increments and message
- * sizes never change, and a beam whose range is already non-finite is never tested.  oracle/scan_filter_oracle.py is
- * the bit-exact definition.  Limits: windows <= 16, speckle_min_neighbours <= 2 * speckle_window, shadow_angle in
+ * sizes never change, and a beam whose range is already non-finite is never tested.  oracle/scan_filter_oracle.py and
+ * oracle/scan_footprint_oracle.py are the bit-exact definition.  Limits: windows <= 16, speckle_min_neighbours <= 2 * speckle_window, shadow_angle in
  * (0, pi/2) when shadow_window > 0, range_lo <= range_hi, no NaN: otherwise RPL_RESULT_INVALID_DATA.  A disabled
  * entry (enabled 0) leaves the scan as it is. */
 typedef struct rpl_scan_filter_settings {
@@ -1047,6 +1049,40 @@ rpl_result rpl_scan_filter_batch_dev(rpl_ctx* c, const rpl_scan_filter_settings*
 rpl_result rpl_capsule_stream_set_scan_filters(rpl_capsule_stream* s,
                                                const rpl_scan_filter_settings* settings /* [n_streams] */,
                                                const uint8_t* stream_mask /* nullable: all */);
+/* The footprint stage of the filters (LaserScanPolygonFilter / LaserScanBoxFilter, INTEGRATION.md 4g): up to four
+ * polygons of 3..16 vertices (n_vertices 0: unused) in the footprint frame (base_link), and the pose (pose_x, pose_y,
+ * pose_yaw) of the published LaserScan frame in that frame.  A finite beam is removed when its point
+ * (fl(r * cos), fl(r * sin) of i * angle_increment) is inside a polygon whose invert is 0, or outside one whose invert
+ * is non-zero (a region of interest); the crossing-number rule decides, and a point on an edge is inside or outside as
+ * it decides.  The vertices are moved into the scan frame once, when the footprint is given, in double with libm's
+ * cos / sin of pose_yaw, and rounded to float.  A box is one 4-vertex polygon (its z bounds do not apply to a planar
+ * scan); polygon_padding is applied by the caller to the vertices.  Limits: n_vertices 0 or 3..16, every used vertex
+ * and the pose finite, |x|, |y|, |pose_x|, |pose_y| <= 1000 (metres): otherwise RPL_RESULT_INVALID_DATA.
+ * Offsets: x 0, y 256, n_vertices 512, invert 528, pose_x 532, pose_y 536, pose_yaw 540; 544 bytes. */
+typedef struct rpl_scan_footprint {
+  float x[4][16];          /* offset 0: metres, footprint frame */
+  float y[4][16];          /* 256 */
+  uint32_t n_vertices[4];  /* 512: 0 (unused) or 3..16 */
+  uint8_t invert[4];       /* 528: 0 removes inside, non-zero removes outside */
+  float pose_x;            /* 532: the LaserScan frame's origin in the footprint frame, metres */
+  float pose_y;            /* 536 */
+  float pose_yaw;          /* 540: radians */
+} rpl_scan_footprint;      /* 544 bytes */
+/* Stateless: rpl_scan_filter_batch_dev with a footprint; a NULL footprint is exactly rpl_scan_filter_batch_dev. */
+rpl_result rpl_scan_filter_footprint_batch_dev(rpl_ctx* c, const rpl_scan_filter_settings* settings,
+                                               const rpl_scan_footprint* footprint /* nullable: none */,
+                                               float* ranges, const float* intensities, const uint32_t* beam_counts,
+                                               const float* angle_increment, uint32_t n_scans, uint32_t stride,
+                                               void* stream);
+/*   set_scan_footprints: the footprint of every stream, with the rules of set_scan_filters: synchronous, masked
+ *            (NULL = all), the first call sets every stream, a null footprints or a masked entry outside the limits is
+ *            RPL_RESULT_INVALID_DATA and leaves the table unchanged.  Calls with RPL_FLAG_PER_STREAM_FILTERS apply
+ *            stream s's footprint as a stage of its filters (a stream whose filter entry is disabled is published as
+ *            it is); until the first call no stream has a footprint.  Cloud, node and counter calls ignore it;
+ *            export / import records do not carry the table. */
+rpl_result rpl_capsule_stream_set_scan_footprints(rpl_capsule_stream* s,
+                                                  const rpl_scan_footprint* footprints /* [n_streams] */,
+                                                  const uint8_t* stream_mask /* nullable: all */);
 
 /* ---- LaserScan / PointCloud2 -> wire (SURVEY.md 8(f) rank 3) ---------------------------- */
 /* The serialised message the RMW layer would produce from the message the reference publishes

@@ -65,6 +65,7 @@ EXPORTS = [
     "rpl_capsule_stream_nodes_dev", "rpl_capsule_stream_push_laserscan_msgs", "rpl_capsule_stream_push_laserscan_msgs_dev",
     "rpl_capsule_stream_push_cloud_msgs", "rpl_capsule_stream_push_cloud_msgs_dev",
     "rpl_scan_filter_batch_dev", "rpl_capsule_stream_set_scan_filters",
+    "rpl_scan_filter_footprint_batch_dev", "rpl_capsule_stream_set_scan_footprints",
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -154,6 +155,20 @@ class ScanFilterSettings(C.Structure):
         ("shadow_window", C.c_uint32),
         ("enabled", C.c_uint8),
         ("pad", C.c_uint8 * 3),
+    ]
+
+
+class ScanFootprint(C.Structure):
+    """rpl_scan_footprint: one stream's footprint, up to four polygons in the footprint frame with their invert bits and
+    the pose of the LaserScan frame in that frame (544 bytes).  oracle/scan_footprint_oracle.py defines what it does."""
+    _fields_ = [
+        ("x", (C.c_float * 16) * 4),
+        ("y", (C.c_float * 16) * 4),
+        ("n_vertices", C.c_uint32 * 4),
+        ("invert", C.c_uint8 * 4),
+        ("pose_x", C.c_float),
+        ("pose_y", C.c_float),
+        ("pose_yaw", C.c_float),
     ]
 
 
@@ -285,6 +300,9 @@ def lib() -> C.CDLL:
         "rpl_capsule_stream_set_clouds": ([vp, vp, vp], u32),
         "rpl_capsule_stream_set_scan_filters": ([vp, vp, vp], u32),
         "rpl_scan_filter_batch_dev": ([vp, C.POINTER(ScanFilterSettings), vp, vp, vp, vp, u32, u32, vp], u32),
+        "rpl_capsule_stream_set_scan_footprints": ([vp, vp, vp], u32),
+        "rpl_scan_filter_footprint_batch_dev":
+            ([vp, C.POINTER(ScanFilterSettings), C.POINTER(ScanFootprint), vp, vp, vp, vp, u32, u32, vp], u32),
         "rpl_capsule_stream_laserscan_msgs": ([vp, PSP, C.c_int64, vp, u64, vp, vp, vp], u32),
         "rpl_capsule_stream_laserscan_msgs_dev": ([vp, PSP, C.c_int64, vp, u64, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_cloud_msgs": ([vp, PCP, C.c_int64, vp, u64, vp, vp, vp], u32),
@@ -340,6 +358,22 @@ def scan_filter_settings(mask=(), range_lo=float("-inf"), range_hi=float("inf"),
                               float(intensity_min), float(speckle_max_diff), float(shadow_angle), int(speckle_window),
                               int(speckle_min_neighbours), int(shadow_window), int(bool(enabled)),
                               (C.c_uint8 * 3)(0, 0, 0))
+
+
+def scan_footprint(polygons=(), invert=(), pose=(0.0, 0.0, 0.0)) -> ScanFootprint:
+    """polygons: up to four vertex lists [(x, y), ...] (3..16 vertices each, metres in the footprint frame); invert: a
+    bit per polygon (missing: 0), set to remove what lies outside it; pose: (x, y, yaw) of the LaserScan frame in the
+    footprint frame.  The defaults remove nothing."""
+    assert len(polygons) <= 4 and len(invert) <= 4
+    f = ScanFootprint()
+    for p, poly in enumerate(polygons):
+        f.n_vertices[p] = len(poly)
+        for k, (x, y) in enumerate(poly):
+            f.x[p][k], f.y[p][k] = float(x), float(y)
+    for p, b in enumerate(invert):
+        f.invert[p] = int(bool(b))
+    f.pose_x, f.pose_y, f.pose_yaw = (float(v) for v in pose)
+    return f
 
 
 def _timing(t):
@@ -681,6 +715,13 @@ class Context:
                                                       _p(beam_counts), _p(angle_increment), n_scans, stride,
                                                       _p(stream)))
 
+    def scan_filter_footprint_batch_dev(self, settings: ScanFilterSettings, footprint: "ScanFootprint | None", ranges,
+                                        intensities, beam_counts, angle_increment, n_scans, stride, stream=None):
+        """scan_filter_batch_dev with a footprint (None: none)."""
+        self._check(self._L.rpl_scan_filter_footprint_batch_dev(
+            self._h, C.byref(settings), C.byref(footprint) if footprint is not None else None, _p(ranges),
+            _p(intensities), _p(beam_counts), _p(angle_increment), n_scans, stride, _p(stream)))
+
     def cloud_fuse_dev(self, xyzi, point_counts, n_scans, stride, fused, offsets, total, stream=None):
         self._check(self._L.rpl_cloud_fuse_dev(self._h, _p(xyzi), _p(point_counts), n_scans, stride, _p(fused),
                                                _p(offsets), _p(total), _p(stream)))
@@ -833,6 +874,16 @@ class CapsuleStreamSession:
         m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
         assert m is None or m.shape == (self.n_streams,)
         self._ctx._check(self._fn("set_scan_filters")(self._h, C.cast(arr, C.c_void_p), _p(m)))
+
+    def set_scan_footprints(self, footprints, mask=None):
+        """Per stream the footprint (n_streams ScanFootprint, see scan_footprint) that the filters of calls with
+        FLAG_PER_STREAM_FILTERS apply as one of their stages.  Only the entries where mask is true are copied (None:
+        all); the first call must set every stream."""
+        assert len(footprints) == self.n_streams
+        arr = (ScanFootprint * self.n_streams)(*footprints)
+        m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
+        assert m is None or m.shape == (self.n_streams,)
+        self._ctx._check(self._fn("set_scan_footprints")(self._h, C.cast(arr, C.c_void_p), _p(m)))
 
     def _msgs(self, name, params, clock_offset_ns, msgs, packed):
         ns = self.n_streams * self.max_scans

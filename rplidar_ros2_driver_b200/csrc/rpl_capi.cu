@@ -575,6 +575,11 @@ static_assert(sizeof(rpl_scan_filter_settings) == 68 && sizeof(rpl::ScanFilter) 
                   offsetof(rpl_scan_filter_settings, speckle_window) == offsetof(rpl::ScanFilter, speckle_window) &&
                   offsetof(rpl_scan_filter_settings, enabled) == 64,
               "rpl::ScanFilter must be laid out as rpl_scan_filter_settings, tan(shadow_angle) for shadow_angle");
+static_assert(sizeof(rpl_scan_footprint) == 544 && offsetof(rpl_scan_footprint, y) == 256 &&
+                  offsetof(rpl_scan_footprint, n_vertices) == 512 && offsetof(rpl_scan_footprint, invert) == 528 &&
+                  offsetof(rpl_scan_footprint, pose_x) == 532 && offsetof(rpl_scan_footprint, pose_y) == 536 &&
+                  offsetof(rpl_scan_footprint, pose_yaw) == 540,
+              "rpl_scan_footprint's layout is the header's");
 
 namespace {
 
@@ -604,11 +609,65 @@ rpl::ScanFilter scan_filter_entry(const rpl_scan_filter_settings& e) {
   return f;
 }
 
+// the limits of rpl_scan_footprint (oracle/scan_footprint_oracle.py footprint_ok)
+bool scan_footprint_ok(rpl_ctx* c, const rpl_scan_footprint& e) {
+  constexpr float kMax = 1000.0f;
+  const char* why = nullptr;
+  if (!std::isfinite(e.pose_x) || !std::isfinite(e.pose_y) || !std::isfinite(e.pose_yaw))
+    why = "a footprint pose is not finite";
+  else if (std::fabs(e.pose_x) > kMax || std::fabs(e.pose_y) > kMax)
+    why = "a footprint pose coordinate is beyond 1000 m";
+  for (uint32_t p = 0; p < rpl::kFootprintMaxPolygons && !why; ++p) {
+    const uint32_t n = e.n_vertices[p];
+    if (n != 0 && (n < 3 || n > rpl::kFootprintMaxVertices)) {
+      why = "a footprint polygon's n_vertices must be 0 or 3..16";
+      break;
+    }
+    for (uint32_t k = 0; k < n; ++k)
+      if (!(std::fabs(e.x[p][k]) <= kMax && std::fabs(e.y[p][k]) <= kMax)) {
+        why = "a footprint vertex is not finite or beyond 1000 m";
+        break;
+      }
+  }
+  if (why) c->err = why;
+  return why == nullptr;
+}
+
+// a footprint as the kernel reads it: the used polygons first, each vertex moved into the scan frame in double (every
+// operation rounded as written) and rounded to float once
+rpl::ScanFootprint scan_footprint_entry(const rpl_scan_footprint& e) {
+  rpl::ScanFootprint f{};
+  const double c = std::cos((double)e.pose_yaw), s = std::sin((double)e.pose_yaw);
+  const double px = e.pose_x, py = e.pose_y;
+  for (uint32_t p = 0; p < rpl::kFootprintMaxPolygons; ++p) {
+    const uint32_t n = e.n_vertices[p];
+    if (n == 0) continue;
+    const uint32_t q = f.n_polygons++;
+    for (uint32_t k = 0; k < n; ++k) {
+      const double dx = (double)e.x[p][k] - px, dy = (double)e.y[p][k] - py;
+      f.x[q][k] = (float)(c * dx + s * dy);
+      f.y[q][k] = (float)(-s * dx + c * dy);
+    }
+    f.n_vertices[q] = n;
+    f.invert[q] = e.invert[p] ? 1u : 0u;
+  }
+  return f;
+}
+
 }  // namespace
 
 rpl_result rpl_scan_filter_batch_dev(rpl_ctx* c, const rpl_scan_filter_settings* settings, float* ranges,
                                      const float* intensities, const uint32_t* beam_counts,
                                      const float* angle_increment, uint32_t n_scans, uint32_t stride, void* stream) {
+  return rpl_scan_filter_footprint_batch_dev(c, settings, nullptr, ranges, intensities, beam_counts, angle_increment,
+                                             n_scans, stride, stream);
+}
+
+rpl_result rpl_scan_filter_footprint_batch_dev(rpl_ctx* c, const rpl_scan_filter_settings* settings,
+                                               const rpl_scan_footprint* footprint, float* ranges,
+                                               const float* intensities, const uint32_t* beam_counts,
+                                               const float* angle_increment, uint32_t n_scans, uint32_t stride,
+                                               void* stream) {
   if (!c) return RPL_RESULT_INVALID_DATA;
   if (!settings || !ranges || !intensities || !beam_counts || !angle_increment) {
     c->err = "null settings, ranges, intensities, beam_counts or angle_increment";
@@ -619,11 +678,13 @@ rpl_result rpl_scan_filter_batch_dev(rpl_ctx* c, const rpl_scan_filter_settings*
     return RPL_RESULT_INVALID_DATA;
   }
   if (!scan_filter_ok(c, *settings)) return RPL_RESULT_INVALID_DATA;
+  if (footprint && !scan_footprint_ok(c, *footprint)) return RPL_RESULT_INVALID_DATA;
   cudaStream_t st;
   if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
   if (!settings->enabled || n_scans == 0) return RPL_RESULT_OK;
   rpl::ScanFilterArgs a{};
   a.one = scan_filter_entry(*settings);
+  if (footprint) a.one_footprint = scan_footprint_entry(*footprint);
   a.ranges = ranges;
   a.intensities = intensities;
   a.stride = stride;
@@ -1416,6 +1477,10 @@ struct rpl_capsule_stream {
   // read: the entries as set (empty until the first call sets every stream) and as the kernel reads them
   std::vector<rpl_scan_filter_settings> filters_host;
   rpl::ScanFilter* filters = nullptr;           // [n_streams] device
+  // their footprints (rpl_capsule_stream_set_scan_footprints): as set (empty until the first call sets every stream)
+  // and as the kernel reads them (nullptr until then: no stream has a footprint)
+  std::vector<rpl_scan_footprint> footprints_host;
+  rpl::ScanFootprint* footprints = nullptr;     // [n_streams] device
   unsigned char* node_work = nullptr;           // the tables of a nodes call (NodeWork)
   // [n_streams] device, zeroed at create: what every push decoded and lost (rpl_capsule_stream_counters); a stream's
   // record is written by the one CTA of each kernel that serves the stream
@@ -1519,6 +1584,7 @@ struct WireChunk {
   // a LaserScan push with RPL_FLAG_PER_STREAM_FILTERS: the chunk's first stream's entry of the session's filters, when
   // some stream of the chunk has its filters enabled (else nullptr: no filter launch)
   const rpl::ScanFilter* filters;
+  const rpl::ScanFootprint* footprints;  // with filters: the chunk's first stream's footprint (nullptr: none)
 };
 
 // the filters of a call with RPL_FLAG_PER_STREAM_FILTERS over streams [s0, s0 + ns): the table at s0, or nullptr when
@@ -1531,13 +1597,20 @@ const rpl::ScanFilter* filters_at(const rpl_capsule_stream* cs, const rpl_scan_p
   return nullptr;
 }
 
-// the filters at `filters` over n scan slots, per slots per entry: rows (ranges / intens at stride) or, with msg_out,
-// the placed messages of `place`; beams and inc the scan kernels' beam counts and angle increments of the slots
-rpl_result filter_scans(rpl_ctx* c, const rpl::ScanFilter* filters, uint32_t per, uint32_t n, float* ranges,
-                        const float* intens, uint32_t stride, uint8_t* msg_out, const unsigned long long* place,
-                        const uint32_t* beams, const float* inc, cudaStream_t st) {
+// the footprints of stream s0 on (nullptr before the first set_scan_footprints)
+const rpl::ScanFootprint* footprints_at(const rpl_capsule_stream* cs, uint32_t s0) {
+  return cs->footprints ? cs->footprints + s0 : nullptr;
+}
+
+// the filters at `filters` with the footprints at `footprints` (nullptr: none) over n scan slots, per slots per entry:
+// rows (ranges / intens at stride) or, with msg_out, the placed messages of `place`; beams and inc the scan kernels'
+// beam counts and angle increments of the slots
+rpl_result filter_scans(rpl_ctx* c, const rpl::ScanFilter* filters, const rpl::ScanFootprint* footprints, uint32_t per,
+                        uint32_t n, float* ranges, const float* intens, uint32_t stride, uint8_t* msg_out,
+                        const unsigned long long* place, const uint32_t* beams, const float* inc, cudaStream_t st) {
   rpl::ScanFilterArgs a{};
   a.filters = filters;
+  a.footprints = footprints;
   a.per_filter = per;
   a.ranges = ranges;
   a.intensities = intens;
@@ -1606,6 +1679,7 @@ WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0, const rpl_sca
   }
   w.clouds = chains_at(cs, s0);
   w.filters = filters_at(cs, params, s0, dev ? cs->chunk_dev : cs->chunk_host);
+  w.footprints = w.filters ? footprints_at(cs, s0) : nullptr;
   return w;
 }
 
@@ -1891,8 +1965,8 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
     r = enqueue_scan(c, l, w.nodes, w.scan_len, ns * w.max_scans, w.max_nodes, params, nullptr, ranges, intens, beams,
                      inc, nullptr, nullptr, st, views, (unsigned long long)ns * w.stride_nodes, lt);
     if (r != RPL_RESULT_OK || !w.filters) return r;
-    return filter_scans(c, w.filters, w.max_scans, ns * w.max_scans, ranges, intens, w.max_nodes, nullptr, nullptr,
-                        beams, inc, st);
+    return filter_scans(c, w.filters, w.footprints, w.max_scans, ns * w.max_scans, ranges, intens, w.max_nodes,
+                        nullptr, nullptr, beams, inc, st);
   }
   if (m->cloud) {  // the scans as last_push_scans will give them once the push is done
     rpl::ScanBatchArgs a{};
@@ -1935,7 +2009,8 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
   r = enqueue_scan(c, l, w.nodes, w.scan_len, ns * w.max_scans, w.max_nodes, params, nullptr, nullptr, nullptr, beams,
                    inc, nullptr, nullptr, st, views, (unsigned long long)ns * w.stride_nodes, lt, m->out, m->place);
   if (r == RPL_RESULT_OK && w.filters)  // in place in the messages, before the header writer and the copies behind it
-    r = filter_scans(c, w.filters, w.max_scans, ns * w.max_scans, nullptr, nullptr, 0, m->out, m->place, beams, inc, st);
+    r = filter_scans(c, w.filters, w.footprints, w.max_scans, ns * w.max_scans, nullptr, nullptr, 0, m->out, m->place,
+                     beams, inc, st);
   if (r != RPL_RESULT_OK) return r;
   rpl::MsgWriteArgs a{};
   a.hdr = m->hdr;
@@ -2871,6 +2946,40 @@ rpl_result stream_set_scan_filters(rpl_capsule_stream* cs, const rpl_scan_filter
   return RPL_RESULT_OK;
 }
 
+// the per-stream footprints: the masked entries of `footprints` replace the table's, all or none
+rpl_result stream_set_scan_footprints(rpl_capsule_stream* cs, const rpl_scan_footprint* footprints,
+                                      const uint8_t* stream_mask) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!footprints) {
+    c->err = "null footprints";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  std::vector<rpl_scan_footprint> t = cs->footprints_host;
+  if (t.empty()) {
+    for (uint32_t s = 0; s < cs->n_streams; ++s)
+      if (stream_mask && !stream_mask[s]) {
+        c->err = "the first rpl_capsule_stream_set_scan_footprints call must set every stream";
+        return RPL_RESULT_INVALID_DATA;
+      }
+    t.resize(cs->n_streams);
+  }
+  for (uint32_t s = 0; s < cs->n_streams; ++s) {
+    if (stream_mask && !stream_mask[s]) continue;
+    if (!scan_footprint_ok(c, footprints[s])) return RPL_RESULT_INVALID_DATA;
+    t[s] = footprints[s];
+  }
+  std::vector<rpl::ScanFootprint> d(cs->n_streams);
+  for (uint32_t s = 0; s < cs->n_streams; ++s) d[s] = scan_footprint_entry(t[s]);
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  if (!cs->footprints) RPL_CUDA(c, dev_alloc(&cs->footprints, cs->n_streams), RPL_RESULT_INSUFFICIENT_MEMORY);
+  RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);  // a push or messages call may still read it
+  RPL_CUDA(c, cudaMemcpy(cs->footprints, d.data(), d.size() * sizeof(rpl::ScanFootprint), cudaMemcpyHostToDevice),
+           RPL_RESULT_OPERATION_FAIL);
+  cs->footprints_host = std::move(t);
+  return RPL_RESULT_OK;
+}
+
 // the PointCloud2 members between the header and the data: height 1, width, the fields x, y, z, intensity (float32,
 // count 1), is_bigendian 0, point_step 16, row_step, data length
 rpl::CloudTail cloud_tail() {
@@ -2970,8 +3079,8 @@ rpl_result msgs_prepare(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* p
                        nullptr, nullptr, st, a.views, a.nodes_total,
                        lidar_table(cs, (p->flags & RPL_FLAG_PER_STREAM) != 0, s0));
       if (const rpl::ScanFilter* f = filters_at(cs, p, s0, ns); r == RPL_RESULT_OK && f)
-        r = filter_scans(cs->c, f, cs->max_scans, a.n_scans, w.data + so * row, w.data + (NS + so) * row, cs->max_nodes,
-                         nullptr, nullptr, w.counts + so, w.inc + so, st);
+        r = filter_scans(cs->c, f, footprints_at(cs, s0), cs->max_scans, a.n_scans, w.data + so * row,
+                         w.data + (NS + so) * row, cs->max_nodes, nullptr, nullptr, w.counts + so, w.inc + so, st);
     } else {
       r = stream_cloud_chunk(c, c->lane[0], last_push_scans(cs, s0, ns), lidars_at(cs, s0), chains_at(cs, s0),
                              cs->max_scans, static_cast<const rpl_cloud_params*>(params), w.data + so * row * 4,
@@ -3474,6 +3583,7 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   cudaFree(cs->lidars);
   cudaFree(cs->clouds);
   cudaFree(cs->filters);
+  cudaFree(cs->footprints);
   cudaFree(cs->counters);
   cudaFree(cs->push_msg_work);
   cudaFree(cs->migrate_work);
@@ -3968,6 +4078,11 @@ rpl_result rpl_capsule_stream_set_clouds(rpl_capsule_stream* s, const rpl_cloud_
 rpl_result rpl_capsule_stream_set_scan_filters(rpl_capsule_stream* s, const rpl_scan_filter_settings* settings,
                                                const uint8_t* stream_mask) {
   return stream_set_scan_filters(s, settings, stream_mask);
+}
+
+rpl_result rpl_capsule_stream_set_scan_footprints(rpl_capsule_stream* s, const rpl_scan_footprint* footprints,
+                                                  const uint8_t* stream_mask) {
+  return stream_set_scan_footprints(s, footprints, stream_mask);
 }
 
 rpl_result rpl_capsule_stream_laserscan_msgs_dev(rpl_capsule_stream* s, const rpl_scan_params* params,

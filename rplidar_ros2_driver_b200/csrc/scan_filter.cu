@@ -6,7 +6,10 @@
 // stages applied on the way in; the speckle and veiling stages each decide every beam from the staged ranges into a
 // bitmap (one ballot word per warp), then mark the removed beams NaN; the ranges go back at the end.  A scan's
 // (sin, cos) table of k * angle_increment, k <= 16, comes from a double polynomial with every operation rounded as
-// written, so that the decisions are the restatement's bit for bit.
+// written, so that the decisions are the restatement's bit for bit.  The footprint stage
+// (oracle/scan_footprint_oracle.py) runs beside the three per-beam stages: a scan with polygons stages them in shared
+// memory, and every beam still finite after the other per-beam stages takes its point from the same double polynomial
+// and is tested against each polygon.
 #include <algorithm>
 
 #include "scan_args.h"
@@ -51,7 +54,31 @@ struct FilterSmem {
   float r[kScanFilterMaxBeams];
   uint32_t removed[kScanFilterMaxBeams / 32];
   float sk[kScanFilterMaxWindow + 1], ck[kScanFilterMaxWindow + 1];
+  ScanFootprint fp;
 };
+
+// the footprint stage: the point of beam i at range r (finite) is inside a polygon whose invert is 0, or outside one
+// whose invert is 1 (the crossing-number rule, every float operation rounded as written)
+__device__ __forceinline__ bool footprint(const ScanFootprint& fp, uint32_t np, uint32_t i, float r, float inc) {
+  double sn, cs;
+  sincos_f64(__dmul_rn((double)i, (double)inc), &sn, &cs);
+  const float x = __fmul_rn(r, __double2float_rn(cs)), y = __fmul_rn(r, __double2float_rn(sn));
+  for (uint32_t p = 0; p < np; ++p) {
+    const uint32_t n = fp.n_vertices[p];
+    float xa = fp.x[p][n - 1], ya = fp.y[p][n - 1];
+    bool in = false;
+    for (uint32_t k = 0; k < n; ++k) {
+      const float xb = fp.x[p][k], yb = fp.y[p][k];
+      if ((ya > y) != (yb > y) &&
+          x < __fadd_rn(xa, __fdiv_rn(__fmul_rn(__fsub_rn(xb, xa), __fsub_rn(y, ya)), __fsub_rn(yb, ya))))
+        in = !in;
+      xa = xb;
+      ya = yb;
+    }
+    if (in != (fp.invert[p] != 0)) return true;
+  }
+  return false;
+}
 
 // speckle: a finite beam with fewer than n neighbours within w beams and max_diff of its range
 __device__ __forceinline__ bool speckle(const float* r, uint32_t i, uint32_t M, uint32_t w, uint32_t n, float max_diff) {
@@ -103,7 +130,8 @@ __device__ __forceinline__ void decide(FilterSmem& sm, uint32_t M, Decide fn) {
   __syncthreads();
 }
 
-__global__ void __launch_bounds__(FT) scan_filter_kernel(ScanFilterArgs a) {
+// a grid constant: `one_footprint` is read in place in the parameter space by address, without a local copy
+__global__ void __launch_bounds__(FT) scan_filter_kernel(const __grid_constant__ ScanFilterArgs a) {
   __shared__ FilterSmem sm;
   for (uint32_t s = blockIdx.x; s < a.n_scans; s += gridDim.x) {
     const ScanFilter& f = a.filters ? a.filters[s / a.per_filter] : a.one;
@@ -129,7 +157,15 @@ __global__ void __launch_bounds__(FT) scan_filter_kernel(ScanFilterArgs a) {
       sm.sk[threadIdx.x] = __double2float_rn(sn);
       sm.ck[threadIdx.x] = __double2float_rn(cs);
     }
-    // stages 1-3: angular mask, range window, intensity floor
+    const ScanFootprint* fp = a.footprints ? a.footprints + s / a.per_filter : &a.one_footprint;
+    const uint32_t np = fp->n_polygons;
+    if (np) {
+      const uint32_t* src = reinterpret_cast<const uint32_t*>(fp);
+      uint32_t* dst = reinterpret_cast<uint32_t*>(&sm.fp);
+      for (uint32_t w = threadIdx.x; w < sizeof(ScanFootprint) / 4; w += FT) dst[w] = src[w];
+      __syncthreads();
+    }
+    // stages 1-3 and the footprint: angular mask, range window, intensity floor, polygons
     for (uint32_t i = threadIdx.x; i < M; i += FT) {
       float v = rg[i];
       if (isfinite(v)) {
@@ -137,6 +173,7 @@ __global__ void __launch_bounds__(FT) scan_filter_kernel(ScanFilterArgs a) {
         bool rm = v < f.range_lo || v > f.range_hi || ig[i] < f.intensity_min;
 #pragma unroll
         for (int k = 0; k < 4; ++k) rm = rm || (f.mask_lo[k] <= ang && ang <= f.mask_hi[k]);
+        rm = rm || (np && footprint(sm.fp, np, i, v, inc));
         if (rm) v = __uint_as_float(kNanBits);
       }
       sm.r[i] = v;

@@ -132,6 +132,7 @@ typedef struct rpl_cloud_params {
                                    the intensity and the intensity_min window; other calls ignore it */
 #define RPL_CLOUD_PER_STREAM_CHAIN 4u /* stream sessions: every stream's own chain (rpl_capsule_stream_set_clouds) in
                                          place of this struct's range_min .. sor_alpha; other calls ignore it */
+/* RPL_CLOUD_PER_STREAM_FOOTPRINTS 8u: stream sessions' footprints on their clouds, defined with rpl_scan_footprint */
 
 typedef struct rpl_ctx rpl_ctx;
 
@@ -1044,7 +1045,8 @@ rpl_result rpl_scan_filter_batch_dev(rpl_ctx* c, const rpl_scan_filter_settings*
  *            push_laserscan_msgs[_dev]): every scan of stream s is F(entry s, scan) of the scan the call without the
  *            flag gives; a disabled stream's are those scans.  It combines with every other RPL_FLAG_*.  A device push
  *            with the flag needs angle_increment.  Before the first set_scan_filters: RPL_RESULT_INVALID_DATA.  Cloud,
- *            node and counter calls ignore it; export / import records do not carry the table. */
+ *            node and counter calls ignore it (a cloud call with RPL_CLOUD_PER_STREAM_FOOTPRINTS applies the footprints
+ *            whatever the filter entry says); export / import records do not carry the table. */
 #define RPL_FLAG_PER_STREAM_FILTERS 16u
 rpl_result rpl_capsule_stream_set_scan_filters(rpl_capsule_stream* s,
                                                const rpl_scan_filter_settings* settings /* [n_streams] */,
@@ -1078,11 +1080,39 @@ rpl_result rpl_scan_filter_footprint_batch_dev(rpl_ctx* c, const rpl_scan_filter
  *            (NULL = all), the first call sets every stream, a null footprints or a masked entry outside the limits is
  *            RPL_RESULT_INVALID_DATA and leaves the table unchanged.  Calls with RPL_FLAG_PER_STREAM_FILTERS apply
  *            stream s's footprint as a stage of its filters (a stream whose filter entry is disabled is published as
- *            it is); until the first call no stream has a footprint.  Cloud, node and counter calls ignore it;
- *            export / import records do not carry the table. */
+ *            it is); until the first call no stream has a footprint.  Cloud calls without
+ *            RPL_CLOUD_PER_STREAM_FOOTPRINTS, node and counter calls ignore it; export / import records do not carry
+ *            the table. */
 rpl_result rpl_capsule_stream_set_scan_footprints(rpl_capsule_stream* s,
                                                   const rpl_scan_footprint* footprints /* [n_streams] */,
                                                   const uint8_t* stream_mask /* nullable: all */);
+/* Footprints in the clouds (DESIGN.md 5.7.1 "Footprints in the clouds"): the same polygons remove the robot's body
+ * from the PointCloud2 chain.  The stage runs on each scan's points after the window and polar -> xyz (step 3 of
+ * oracle/cloud_oracle.cpp) and before SOR and the voxel grid: a point (x, y) = (fl(r * c_key), fl(r * s_key)), exactly
+ * what the cloud would publish without SOR or a voxel grid, is removed when the crossing-number rule of
+ * oracle/scan_footprint_oracle.py puts it inside a polygon whose invert is 0, or outside one whose invert is non-zero.
+ * SOR and the voxel grid then run unchanged on the points left.  Equivalently: the cloud of the nodes with every
+ * removed point's node given dist_mm_q2 = 0.
+ *   Frames: the vertices are those set_scan_footprints moved into the LaserScan frame (u, v).  The cloud is not
+ *            mirrored for an inverted lidar as the LaserScan is, so an inverted stream's points are tested against
+ *            (u, -v) -- the same physical body.  "Inverted" is the stream's rpl_lidar_settings.inverted in a call with
+ *            RPL_CLOUD_PER_STREAM; without that flag nothing is mirrored (a cloud call has no inversion of its own), so
+ *            inverted lidars need rpl_capsule_stream_set_lidars and RPL_CLOUD_PER_STREAM.  A Mode B LaserScan beam sits
+ *            at i * angle_increment and a cloud point at its node's angle, so the two outputs may disagree about a
+ *            return within a fraction of a beam of a polygon edge.
+ *   RPL_CLOUD_PER_STREAM_FOOTPRINTS in rpl_cloud_params.flags (cloud[_dev], cloud_msgs[_dev], push_cloud_msgs[_dev]):
+ *            stream s's clouds take stream s's footprint; it does not depend on the stream's LaserScan filter entry.
+ *            It combines with RPL_CLOUD_PER_STREAM, RPL_CLOUD_PER_STREAM_CHAIN and RPL_CLOUD_NO_FUSED; a stream with
+ *            polygons runs SOR and the voxel grid as separate passes (bit for bit the fused kernel's output).  Before
+ *            the first set_scan_footprints: RPL_RESULT_INVALID_DATA.  Node and counter calls ignore it. */
+#define RPL_CLOUD_PER_STREAM_FOOTPRINTS 8u
+/* Stateless: rpl_cloud_batch_dev with one footprint for every scan, its pose the pose of the cloud's frame in the
+ * footprint frame (nothing mirrored), with the limits of rpl_scan_footprint.  A NULL footprint, or one without
+ * polygons, is exactly rpl_cloud_batch_dev. */
+rpl_result rpl_cloud_footprint_batch_dev(rpl_ctx* ctx, const rpl_node_hq* nodes, const uint32_t* counts,
+                                         uint32_t n_scans, uint32_t stride, const rpl_cloud_params* params,
+                                         const rpl_scan_footprint* footprint /* nullable: none */, float* xyzi,
+                                         uint32_t* point_counts, void* stream);
 
 /* ---- LaserScan / PointCloud2 -> wire (SURVEY.md 8(f) rank 3) ---------------------------- */
 /* The serialised message the RMW layer would produce from the message the reference publishes

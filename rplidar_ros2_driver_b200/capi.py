@@ -30,6 +30,7 @@ FLAG_PER_STREAM_FILTERS = 16
 CLOUD_NO_FUSED = 1
 CLOUD_PER_STREAM = 2
 CLOUD_PER_STREAM_CHAIN = 4
+CLOUD_PER_STREAM_FOOTPRINTS = 8
 CAPSULE_OK, CAPSULE_SYNC, CAPSULE_EMIT, CAPSULE_DISCARD = 1, 2, 4, 8
 CAPSULE_CHECKSUM_ERR, CAPSULE_ENCODER_RESET_ERR, CAPSULE_BAD_FRAME = 16, 32, 64
 PATH_FAST, PATH_GENERAL = 0, 1
@@ -65,7 +66,7 @@ EXPORTS = [
     "rpl_capsule_stream_nodes_dev", "rpl_capsule_stream_push_laserscan_msgs", "rpl_capsule_stream_push_laserscan_msgs_dev",
     "rpl_capsule_stream_push_cloud_msgs", "rpl_capsule_stream_push_cloud_msgs_dev",
     "rpl_scan_filter_batch_dev", "rpl_capsule_stream_set_scan_filters",
-    "rpl_scan_filter_footprint_batch_dev", "rpl_capsule_stream_set_scan_footprints",
+    "rpl_scan_filter_footprint_batch_dev", "rpl_capsule_stream_set_scan_footprints", "rpl_cloud_footprint_batch_dev",
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -237,6 +238,7 @@ def lib() -> C.CDLL:
         "rpl_laserscan_batch": ([vp, vp, vp, u32, u32, PSP, vp, vp, vp, vp], u32),
         "rpl_scan_batch_dev": ([vp, vp, vp, u32, u32, PSP, vp, vp, vp, vp, vp, vp, vp, vp], u32),
         "rpl_cloud_batch_dev": ([vp, vp, vp, u32, u32, PCP, vp, vp, vp], u32),
+        "rpl_cloud_footprint_batch_dev": ([vp, vp, vp, u32, u32, PCP, C.POINTER(ScanFootprint), vp, vp, vp], u32),
         "rpl_cloud_batch": ([vp, vp, vp, u32, u32, PCP, vp, vp], u32),
         "rpl_cloud_fuse_dev": ([vp, vp, vp, u32, u32, vp, vp, vp, vp], u32),
         "rpl_synth_batch_dev": ([vp, u64, u32, u32, u32, i32, vp, vp, vp], u32),
@@ -509,6 +511,14 @@ class Context:
     def cloud_batch_dev(self, nodes, counts, n_scans, stride, params: CloudParams, xyzi, point_counts, stream=None):
         self._check(self._L.rpl_cloud_batch_dev(self._h, _p(nodes), _p(counts), n_scans, stride, C.byref(params),
                                                 _p(xyzi), _p(point_counts), _p(stream)))
+
+    def cloud_footprint_batch_dev(self, nodes, counts, n_scans, stride, params: CloudParams,
+                                  footprint: "ScanFootprint | None", xyzi, point_counts, stream=None):
+        """cloud_batch_dev with one footprint (None: none) removing points before SOR and the voxel grid; its pose is
+        the pose of the cloud's frame, nothing is mirrored."""
+        self._check(self._L.rpl_cloud_footprint_batch_dev(
+            self._h, _p(nodes), _p(counts), n_scans, stride, C.byref(params),
+            C.byref(footprint) if footprint is not None else None, _p(xyzi), _p(point_counts), _p(stream)))
 
     def cloud_batch(self, nodes: np.ndarray, counts, params: CloudParams):
         assert nodes.dtype == NODE_DTYPE and nodes.ndim == 2 and nodes.flags.c_contiguous
@@ -877,8 +887,9 @@ class CapsuleStreamSession:
 
     def set_scan_footprints(self, footprints, mask=None):
         """Per stream the footprint (n_streams ScanFootprint, see scan_footprint) that the filters of calls with
-        FLAG_PER_STREAM_FILTERS apply as one of their stages.  Only the entries where mask is true are copied (None:
-        all); the first call must set every stream."""
+        FLAG_PER_STREAM_FILTERS apply as one of their stages, and cloud calls with CLOUD_PER_STREAM_FOOTPRINTS before
+        SOR and the voxel grid (an inverted stream's cloud, with CLOUD_PER_STREAM, against the mirrored polygons).
+        Only the entries where mask is true are copied (None: all); the first call must set every stream."""
         assert len(footprints) == self.n_streams
         arr = (ScanFootprint * self.n_streams)(*footprints)
         m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)

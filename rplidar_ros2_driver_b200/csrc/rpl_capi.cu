@@ -17,6 +17,7 @@
 
 #include "../../include/rpl_b200.h"
 #include "cloud_args.h"
+#include "cloud_footprint_args.h"
 #include "cdr_args.h"
 #include "decode_args.h"
 #include "scan_args.h"
@@ -1471,6 +1472,10 @@ struct rpl_capsule_stream {
   std::vector<rpl_cloud_settings> clouds_host;
   rpl::CloudSettings* clouds = nullptr;         // [n_streams] device
   uint32_t cloud_routes = 0, cloud_sor_k = 0;
+  // the same table for calls with RPL_CLOUD_PER_STREAM_FOOTPRINTS: a stream with footprint polygons takes the separate
+  // passes where it would have been fused, so that the footprint pass runs between xyz and SOR (clouds_resolve)
+  rpl::CloudSettings* clouds_fp = nullptr;      // [n_streams] device
+  uint32_t cloud_routes_fp = 0;
   bool cloud_voxel = false;
   std::string clouds_bad;
   // the per-stream LaserScan filters (rpl_capsule_stream_set_scan_filters) that calls with RPL_FLAG_PER_STREAM_FILTERS
@@ -1539,9 +1544,29 @@ struct CloudChains {
   bool voxel;       // some stream has a voxel grid
 };
 
-// the per-stream chains from stream s0 on (at: nullptr before the first set_clouds)
-CloudChains chains_at(const rpl_capsule_stream* cs, uint32_t s0) {
+// the per-stream chains from stream s0 on (at: nullptr before the first set_clouds); fp: the table of a chunk that runs
+// the footprint pass
+CloudChains chains_at(const rpl_capsule_stream* cs, uint32_t s0, bool fp = false) {
+  if (fp) return CloudChains{cs->clouds ? cs->clouds_fp + s0 : nullptr, cs->cloud_routes_fp, cs->cloud_sor_k, cs->cloud_voxel};
   return CloudChains{cs->clouds ? cs->clouds + s0 : nullptr, cs->cloud_routes, cs->cloud_sor_k, cs->cloud_voxel};
+}
+
+// a footprint with at least one polygon
+bool has_polygons(const rpl_scan_footprint& e) {
+  for (uint32_t n : e.n_vertices)
+    if (n != 0) return true;
+  return false;
+}
+
+// the footprints of a cloud call with RPL_CLOUD_PER_STREAM_FOOTPRINTS over streams [s0, s0 + ns): the table at s0, or
+// nullptr when the call has no flag or no stream of the range has a polygon (no footprint pass)
+const rpl::ScanFootprint* cloud_footprints_at(const rpl_capsule_stream* cs, const rpl_cloud_params* p, uint32_t s0,
+                                              uint32_t ns) {
+  if (!p || (p->flags & RPL_CLOUD_PER_STREAM_FOOTPRINTS) == 0 || cs->footprints_host.empty()) return nullptr;
+  const uint32_t e = std::min(cs->n_streams, s0 + ns);
+  for (uint32_t s = s0; s < e; ++s)
+    if (has_polygons(cs->footprints_host[s])) return cs->footprints + s0;
+  return nullptr;
 }
 
 // Where a chunk of streams lives on the device between the kernels of capsule_stream_chunk, every pointer at the
@@ -1579,8 +1604,11 @@ struct WireChunk {
   // (a byte session's framer or 0x81 decoder counts the bytes)
   rpl::StreamCounters* counters;
   uint32_t counted_capsule_bytes;
-  // the session's per-stream chains, which a PointCloud2 push with RPL_CLOUD_PER_STREAM_CHAIN reads
+  // the session's per-stream chains, which a PointCloud2 push with RPL_CLOUD_PER_STREAM_CHAIN reads, and with
+  // RPL_CLOUD_PER_STREAM_FOOTPRINTS the chunk's first stream's footprint when some stream of the chunk has a polygon
+  // (else nullptr: no footprint pass)
   CloudChains clouds;
+  const rpl::ScanFootprint* cloud_footprints;
   // a LaserScan push with RPL_FLAG_PER_STREAM_FILTERS: the chunk's first stream's entry of the session's filters, when
   // some stream of the chunk has its filters enabled (else nullptr: no filter launch)
   const rpl::ScanFilter* filters;
@@ -1626,8 +1654,10 @@ rpl_result filter_scans(rpl_ctx* c, const rpl::ScanFilter* filters, const rpl::S
 }
 
 // session cs's chunk from stream s0 in the push under way (arena cs->parity) with params' flags (RPL_FLAG_PER_STREAM,
-// RPL_FLAG_PER_STREAM_FILTERS); dev: a device push's chunking (else a host push's)
-WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0, const rpl_scan_params* params, bool dev) {
+// RPL_FLAG_PER_STREAM_FILTERS) and a PointCloud2 push's cloud params (nullable); dev: a device push's chunking (else a
+// host push's)
+WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0, const rpl_scan_params* params, bool dev,
+                        const rpl_cloud_params* cloud = nullptr) {
   const bool per_stream = (params->flags & RPL_FLAG_PER_STREAM) != 0;
   const uint32_t p = cs->parity, sc = cs->stride_capsules;
   const size_t sn = (size_t)s0 * cs->stride_nodes, so = (size_t)s0 * cs->max_scans;
@@ -1677,7 +1707,8 @@ WireChunk session_chunk(const rpl_capsule_stream* cs, uint32_t s0, const rpl_sca
     w.lidars = cs->lidars + s0;
     w.lidar_modes = cs->lidar_modes;
   }
-  w.clouds = chains_at(cs, s0);
+  w.cloud_footprints = cloud_footprints_at(cs, cloud, s0, dev ? cs->chunk_dev : cs->chunk_host);
+  w.clouds = chains_at(cs, s0, w.cloud_footprints != nullptr);
   w.filters = filters_at(cs, params, s0, dev ? cs->chunk_dev : cs->chunk_host);
   w.footprints = w.filters ? footprints_at(cs, s0) : nullptr;
   return w;
@@ -1799,9 +1830,27 @@ rpl_result decode_assemble(rpl_ctx* c, cudaStream_t st, const WireChunk& w, uint
   return RPL_RESULT_OK;
 }
 
+// the footprint pass (cloud_footprint.cu) over the a.n_scans clouds of `a` (steps 1-3 done), scan s taking
+// footprints[s / a.lidar_scans] (nullptr: `one`), mirrored where a.lidars says the stream is inverted
+rpl_result footprint_clouds(rpl_ctx* c, const rpl::ScanBatchArgs& a, const rpl::ScanFootprint* footprints,
+                            const rpl::ScanFootprint& one, uint32_t* point_counts, cudaStream_t st) {
+  rpl::CloudFootprintArgs f{};
+  f.xyzi = a.xyzi;
+  f.point_counts = point_counts;
+  f.n_scans = a.n_scans;
+  f.stride = a.stride;
+  f.footprints = footprints;
+  f.lidars = a.lidars;
+  f.per = a.lidar_scans ? a.lidar_scans : 1u;
+  f.one = one;
+  RPL_CUDA(c, rpl::launch_cloud_footprint(f, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+  c->launches++;
+  return RPL_RESULT_OK;
+}
+
 // stream_cloud_chunk with RPL_CLOUD_PER_STREAM_CHAIN, `a` set up but for the table
 rpl_result stream_chains_chunk(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, const CloudChains& chains, bool separate,
-                               uint32_t* point_counts, cudaStream_t st) {
+                               const rpl::ScanFootprint* footprints, uint32_t* point_counts, cudaStream_t st) {
   using rpl::kCloudFused;
   using rpl::kCloudSeparate;
   using rpl::kCloudWindow;
@@ -1817,6 +1866,7 @@ rpl_result stream_chains_chunk(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, const 
   bool post_fused = false;
   rpl_result r = scratch_enter(c, l, st);
   if (r == RPL_RESULT_OK) r = enqueue_args(c, l, a, 0u, st, nullptr, &post_fused, true);
+  if (r == RPL_RESULT_OK && footprints) r = footprint_clouds(c, a, footprints, rpl::ScanFootprint{}, point_counts, st);
   if (r != RPL_RESULT_OK) return r;
   const bool full = (chains.routes & separate_routes) != 0;  // the separate route's scans: every scan's pass
   if ((full || post_fused) && (chains.sor_k > 0 || chains.voxel)) {
@@ -1841,16 +1891,20 @@ rpl_result stream_chains_chunk(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, const 
 // The cloud chain over the scans `a` of one chunk: its nodes, views, counts, nodes_total, n_scans and stride set (a
 // push's chunk as its assembler left it, or last_push_scans); xyzi / point_counts point at the chunk's first slot;
 // lidars: RPL_CLOUD_PER_STREAM's table at the chunk's first stream, lidar_scans slots per stream (else nullptr);
-// chains: RPL_CLOUD_PER_STREAM_CHAIN's.
+// chains: RPL_CLOUD_PER_STREAM_CHAIN's (the footprint table, chains_at(.., true), when footprints is set);
+// footprints: RPL_CLOUD_PER_STREAM_FOOTPRINTS's table at the chunk's first stream (cloud_footprints_at; nullptr: no
+// footprint pass).
 // Flags 0: the shared-memory kernel with SOR / voxel grid fused, its arrays sized for at most kSmallPostMaxNodes nodes
 // (a longer view goes to the general kernel, then to the post passes restricted to the hand-off list);
 // RPL_CLOUD_NO_FUSED: the shared-memory kernel's window + xyz, then the post passes over every scan.
 // RPL_CLOUD_PER_STREAM_CHAIN: the same per stream, by route -- the fused kernel for the fusable streams (when the call
 // may fuse), the window-only kernel for the others; the post passes over every scan for the separate route, and
 // restricted to the hand-off list for the fused route.  Each kernel and pass serves only its route's scans.
+// With footprints, the footprint pass runs behind the scan kernels and before the post passes: without the chain flag
+// the chunk runs as RPL_CLOUD_NO_FUSED, with it the footprint table routes every stream with a polygon separately.
 rpl_result stream_cloud_chunk(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, const rpl::LidarSettings* lidars,
                               const CloudChains& chains, uint32_t lidar_scans, const rpl_cloud_params* p, float* xyzi,
-                              uint32_t* point_counts, cudaStream_t st) {
+                              uint32_t* point_counts, cudaStream_t st, const rpl::ScanFootprint* footprints) {
   a.beam_counts = point_counts;
   a.fallback_list = l.fallback_list;
   a.is_new_protocol = p->is_new_protocol;
@@ -1862,11 +1916,13 @@ rpl_result stream_cloud_chunk(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, const r
   a.intensity_min = p->intensity_min;
   a.lidar_scans = lidar_scans;
   if ((p->flags & RPL_CLOUD_PER_STREAM) != 0) a.lidars = lidars;  // each stream's is_new_protocol (the window's too)
-  const bool separate = (p->flags & RPL_CLOUD_NO_FUSED) != 0;
-  if ((p->flags & RPL_CLOUD_PER_STREAM_CHAIN) != 0) return stream_chains_chunk(c, l, a, chains, separate, point_counts, st);
+  if ((p->flags & RPL_CLOUD_PER_STREAM_CHAIN) != 0)
+    return stream_chains_chunk(c, l, a, chains, (p->flags & RPL_CLOUD_NO_FUSED) != 0, footprints, point_counts, st);
+  const bool separate = (p->flags & RPL_CLOUD_NO_FUSED) != 0 || footprints;
   bool fused = false;
   rpl_result r = scratch_enter(c, l, st);
   if (r == RPL_RESULT_OK) r = enqueue_args(c, l, a, 0u, st, separate ? nullptr : p, &fused, true);
+  if (r == RPL_RESULT_OK && footprints) r = footprint_clouds(c, a, footprints, rpl::ScanFootprint{}, point_counts, st);
   if (r != RPL_RESULT_OK) return r;
   if (p->sor_k > 0 || p->voxel_size > 0.0f) {
     // the post passes read lane l's fallback list and run on lane 0's cws: a lane-1 chunk takes lane 0's scratch too
@@ -1976,7 +2032,8 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
     a.nodes_total = (unsigned long long)ns * w.stride_nodes;
     a.n_scans = ns * w.max_scans;
     a.stride = w.max_nodes;
-    r = stream_cloud_chunk(c, l, a, w.lidars, w.clouds, w.max_scans, m->cloud, m->xyzi, m->points, st);
+    r = stream_cloud_chunk(c, l, a, w.lidars, w.clouds, w.max_scans, m->cloud, m->xyzi, m->points, st,
+                           w.cloud_footprints);
     if (r != RPL_RESULT_OK) return r;
   }
   const rpl::MsgKind kind = m->cloud ? rpl::MsgKind::kPointCloud2 : rpl::MsgKind::kLaserScan;
@@ -2598,7 +2655,7 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
         m.xyzi = pm->xyzi;
         m.points = pm->points;
       }
-      r = capsule_stream_chunk(c, c->lane[0], st, session_chunk(cs, s0, params, true),
+      r = capsule_stream_chunk(c, c->lane[0], st, session_chunk(cs, s0, params, true, pm ? pm->cloud : nullptr),
                                std::min(chunk, cs->n_streams - s0), in + s0 * cs->in_stream, counts + s0,
                                sample_duration_us, params, pm ? nullptr : ranges + s0 * row,
                                pm ? nullptr : intensities + s0 * row, pm ? pm->w.beams + so : beam_counts + so,
@@ -2628,7 +2685,7 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
                      intensities, angle_increment, beam_counts, scans_per_stream, sp, sp ? sp->stride_chunks : 0u,
                      pm ? &hm : nullptr};
     r = push_host(c, h, cs->n_streams, chunk,
-                  [&](Carve&, uint32_t s0) { return session_chunk(cs, s0, params, false); });
+                  [&](Carve&, uint32_t s0) { return session_chunk(cs, s0, params, false, pm ? pm->cloud : nullptr); });
   }
   cs->parity ^= 1u;
   cs->prev_stamped = cs->carry_stamped = sp != nullptr;
@@ -2656,6 +2713,10 @@ bool cloud_params_ok(rpl_ctx* c, const rpl_cloud_params* p) {
 // a cloud call's chain rules: its params', or with RPL_CLOUD_PER_STREAM_CHAIN those of the session's resolved table
 bool cloud_call_ok(rpl_capsule_stream* cs, const rpl_cloud_params* p) {
   rpl_ctx* c = cs->c;
+  if ((p->flags & RPL_CLOUD_PER_STREAM_FOOTPRINTS) != 0 && cs->footprints_host.empty()) {
+    c->err = "per-stream cloud footprints requested before rpl_capsule_stream_set_scan_footprints set every stream";
+    return false;
+  }
   if ((p->flags & RPL_CLOUD_PER_STREAM_CHAIN) == 0) return cloud_params_ok(c, p);
   if (cs->clouds_host.empty()) {
     c->err = "per-stream clouds requested before rpl_capsule_stream_set_clouds set every stream";
@@ -2732,10 +2793,13 @@ rpl_result stream_cloud_dev(rpl_capsule_stream* cs, const rpl_cloud_params* para
   const size_t row = (size_t)cs->max_scans * cs->max_nodes * 4;
   return last_push_dev(cs, stream, 0, [&](cudaStream_t st) -> rpl_result {
     rpl_result r = RPL_RESULT_OK;
-    for (uint32_t s0 = 0; s0 < cs->n_streams && r == RPL_RESULT_OK; s0 += cs->cloud_chunk)
-      r = stream_cloud_chunk(cs->c, cs->c->lane[0], last_push_scans(cs, s0, std::min(cs->cloud_chunk, cs->n_streams - s0)),
-                             lidars_at(cs, s0), chains_at(cs, s0), cs->max_scans, params, xyzi + (size_t)s0 * row,
-                             point_counts + (size_t)s0 * cs->max_scans, st);
+    for (uint32_t s0 = 0; s0 < cs->n_streams && r == RPL_RESULT_OK; s0 += cs->cloud_chunk) {
+      const uint32_t ns = std::min(cs->cloud_chunk, cs->n_streams - s0);
+      const rpl::ScanFootprint* fp = cloud_footprints_at(cs, params, s0, ns);
+      r = stream_cloud_chunk(cs->c, cs->c->lane[0], last_push_scans(cs, s0, ns), lidars_at(cs, s0),
+                             chains_at(cs, s0, fp != nullptr), cs->max_scans, params, xyzi + (size_t)s0 * row,
+                             point_counts + (size_t)s0 * cs->max_scans, st, fp);
+    }
     return r;
   });
 }
@@ -2761,8 +2825,10 @@ rpl_result stream_cloud(rpl_capsule_stream* cs, const rpl_cloud_params* params, 
     Carve k{l.stage};
     const Regions d = layout(k);
     RPL_CUDA(c, cudaStreamSynchronize(l.stream), RPL_RESULT_OPERATION_FAIL);  // the lane's previous chunk has left
-    const rpl_result r = stream_cloud_chunk(c, l, last_push_scans(cs, s0, ns), lidars_at(cs, s0), chains_at(cs, s0),
-                                            cs->max_scans, params, d.xyzi, d.counts, l.stream);
+    const rpl::ScanFootprint* fp = cloud_footprints_at(cs, params, s0, ns);
+    const rpl_result r = stream_cloud_chunk(c, l, last_push_scans(cs, s0, ns), lidars_at(cs, s0),
+                                            chains_at(cs, s0, fp != nullptr), cs->max_scans, params, d.xyzi, d.counts,
+                                            l.stream, fp);
     if (r != RPL_RESULT_OK) return r;
     RPL_CUDA(c, cudaMemcpyAsync(xyzi + (size_t)s0 * row, d.xyzi, ns * row * 4, d2h, l.stream), RPL_RESULT_OPERATION_FAIL);
     RPL_CUDA(c, cudaMemcpyAsync(point_counts + (size_t)s0 * cs->max_scans, d.counts, (size_t)ns * cs->max_scans * 4, d2h,
@@ -2782,8 +2848,9 @@ rpl_result stream_cloud(rpl_capsule_stream* cs, const rpl_cloud_params* params, 
 // The device table of the per-stream clouds from the entries as set and the frames' range_max, with its summary: each
 // stream's route (the fusion guard of launch_fast at its resolved range_max) and why a flagged call would fail.  The
 // caller has passed cs->done.
-rpl_result clouds_resolve(rpl_capsule_stream* cs) {
+rpl_result clouds_resolve(rpl_capsule_stream* cs, const std::vector<rpl_scan_footprint>* footprints = nullptr) {
   rpl_ctx* c = cs->c;
+  const std::vector<rpl_scan_footprint>& fps = footprints ? *footprints : cs->footprints_host;
   std::vector<rpl::CloudSettings> t(cs->n_streams);
   uint32_t routes = 0, sor_k = 0;
   bool voxel = false;
@@ -2813,6 +2880,15 @@ rpl_result clouds_resolve(rpl_capsule_stream* cs) {
   }
   RPL_CUDA(c, cudaMemcpy(cs->clouds, t.data(), t.size() * sizeof(rpl::CloudSettings), cudaMemcpyHostToDevice),
            RPL_RESULT_OPERATION_FAIL);
+  // the footprint table: a stream with a polygon is never fused (its SOR / voxel grid run behind the footprint pass)
+  uint32_t routes_fp = 0;
+  for (uint32_t s = 0; s < cs->n_streams; ++s) {
+    if (t[s].route == rpl::kCloudFused && !fps.empty() && has_polygons(fps[s])) t[s].route = rpl::kCloudSeparate;
+    routes_fp |= 1u << t[s].route;
+  }
+  RPL_CUDA(c, cudaMemcpy(cs->clouds_fp, t.data(), t.size() * sizeof(rpl::CloudSettings), cudaMemcpyHostToDevice),
+           RPL_RESULT_OPERATION_FAIL);
+  cs->cloud_routes_fp = routes_fp;
   cs->cloud_routes = routes;
   cs->cloud_sor_k = sor_k;
   cs->cloud_voxel = voxel;
@@ -2907,6 +2983,7 @@ rpl_result stream_set_clouds(rpl_capsule_stream* cs, const rpl_cloud_settings* s
   }
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
   if (!cs->clouds) RPL_CUDA(c, dev_alloc(&cs->clouds, cs->n_streams), RPL_RESULT_INSUFFICIENT_MEMORY);
+  if (!cs->clouds_fp) RPL_CUDA(c, dev_alloc(&cs->clouds_fp, cs->n_streams), RPL_RESULT_INSUFFICIENT_MEMORY);
   RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);  // a cloud or messages call may still read it
   cs->clouds_host = std::move(t);
   return clouds_resolve(cs);
@@ -2974,6 +3051,9 @@ rpl_result stream_set_scan_footprints(rpl_capsule_stream* cs, const rpl_scan_foo
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
   if (!cs->footprints) RPL_CUDA(c, dev_alloc(&cs->footprints, cs->n_streams), RPL_RESULT_INSUFFICIENT_MEMORY);
   RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);  // a push or messages call may still read it
+  // the clouds' footprint route table follows the new footprints (every allocation is made before the tables change)
+  if (!cs->clouds_host.empty())
+    if (const rpl_result r = clouds_resolve(cs, &t); r != RPL_RESULT_OK) return r;
   RPL_CUDA(c, cudaMemcpy(cs->footprints, d.data(), d.size() * sizeof(rpl::ScanFootprint), cudaMemcpyHostToDevice),
            RPL_RESULT_OPERATION_FAIL);
   cs->footprints_host = std::move(t);
@@ -3082,9 +3162,11 @@ rpl_result msgs_prepare(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* p
         r = filter_scans(cs->c, f, footprints_at(cs, s0), cs->max_scans, a.n_scans, w.data + so * row,
                          w.data + (NS + so) * row, cs->max_nodes, nullptr, nullptr, w.counts + so, w.inc + so, st);
     } else {
-      r = stream_cloud_chunk(c, c->lane[0], last_push_scans(cs, s0, ns), lidars_at(cs, s0), chains_at(cs, s0),
-                             cs->max_scans, static_cast<const rpl_cloud_params*>(params), w.data + so * row * 4,
-                             w.counts + so, st);
+      const auto* p = static_cast<const rpl_cloud_params*>(params);
+      const rpl::ScanFootprint* fp = cloud_footprints_at(cs, p, s0, ns);
+      r = stream_cloud_chunk(c, c->lane[0], last_push_scans(cs, s0, ns), lidars_at(cs, s0),
+                             chains_at(cs, s0, fp != nullptr), cs->max_scans, p, w.data + so * row * 4, w.counts + so,
+                             st, fp);
     }
   }
   if (r != RPL_RESULT_OK) return r;
@@ -3582,6 +3664,7 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   cudaFree(cs->node_work);
   cudaFree(cs->lidars);
   cudaFree(cs->clouds);
+  cudaFree(cs->clouds_fp);
   cudaFree(cs->filters);
   cudaFree(cs->footprints);
   cudaFree(cs->counters);
@@ -4357,7 +4440,15 @@ rpl_result rpl_synth_batch_dev(rpl_ctx* c, uint64_t first_scan_id, uint32_t n_sc
 rpl_result rpl_cloud_batch_dev(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t* counts,
                                uint32_t n_scans, uint32_t stride, const rpl_cloud_params* params,
                                float* xyzi, uint32_t* point_counts, void* stream) {
+  return rpl_cloud_footprint_batch_dev(c, nodes, counts, n_scans, stride, params, nullptr, xyzi, point_counts, stream);
+}
+
+rpl_result rpl_cloud_footprint_batch_dev(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t* counts,
+                                         uint32_t n_scans, uint32_t stride, const rpl_cloud_params* params,
+                                         const rpl_scan_footprint* footprint, float* xyzi, uint32_t* point_counts,
+                                         void* stream) {
   if (!c || !nodes || !counts || !params || !xyzi || !point_counts) return RPL_RESULT_INVALID_DATA;
+  if (footprint && !scan_footprint_ok(c, *footprint)) return RPL_RESULT_INVALID_DATA;
   if (n_scans == 0) return RPL_RESULT_OK;
   if (n_scans > c->max_scans) {
     c->err = "n_scans exceeds max_scans";
@@ -4383,10 +4474,15 @@ rpl_result rpl_cloud_batch_dev(rpl_ctx* c, const rpl_node_hq* nodes, const uint3
   // Revolutions of at most 4096 nodes: the whole chain (window, xyz, SOR, voxel grid) in one kernel, in shared
   // memory (scan_small.cu); the separate in-place post passes then only see the duplicate-key scans that kernel
   // handed to the general kernel.  Larger revolutions: steps 1-3 inside the scan kernels, steps 4-5 as post passes.
+  // A footprint with polygons: steps 1-3 in the scan kernels, the footprint pass, then steps 4-5 over every scan.
+  rpl::ScanFootprint one{};
+  if (footprint) one = scan_footprint_entry(*footprint);
+  const bool fp = one.n_polygons != 0;
   bool fused = false;
   const uint32_t flags = (params->flags & RPL_CLOUD_NO_FUSED) ? RPL_FLAG_NO_SMALL : 0u;
   rpl_result r = scratch_enter(c, c->lane[0], st);
-  if (r == RPL_RESULT_OK) r = enqueue_args(c, c->lane[0], a, flags, st, params, &fused);
+  if (r == RPL_RESULT_OK) r = enqueue_args(c, c->lane[0], a, flags, st, fp ? nullptr : params, &fused);
+  if (r == RPL_RESULT_OK && fp) r = footprint_clouds(c, a, nullptr, one, point_counts, st);
   if (r != RPL_RESULT_OK) return r;
   if (params->sor_k > 0 || params->voxel_size > 0.0f) {
     int launched = 0;

@@ -12,6 +12,7 @@
 // and is tested against each polygon.
 #include <algorithm>
 
+#include "footprint_rule.cuh"
 #include "scan_args.h"
 #include "scan_filter_args.h"
 
@@ -58,26 +59,14 @@ struct FilterSmem {
 };
 
 // the footprint stage: the point of beam i at range r (finite) is inside a polygon whose invert is 0, or outside one
-// whose invert is 1 (the crossing-number rule, every float operation rounded as written)
+// whose invert is 1 (footprint_rule.cuh)
 __device__ __forceinline__ bool footprint(const ScanFootprint& fp, uint32_t np, uint32_t i, float r, float inc) {
-  double sn, cs;
-  sincos_f64(__dmul_rn((double)i, (double)inc), &sn, &cs);
-  const float x = __fmul_rn(r, __double2float_rn(cs)), y = __fmul_rn(r, __double2float_rn(sn));
-  for (uint32_t p = 0; p < np; ++p) {
-    const uint32_t n = fp.n_vertices[p];
-    float xa = fp.x[p][n - 1], ya = fp.y[p][n - 1];
-    bool in = false;
-    for (uint32_t k = 0; k < n; ++k) {
-      const float xb = fp.x[p][k], yb = fp.y[p][k];
-      if ((ya > y) != (yb > y) &&
-          x < __fadd_rn(xa, __fdiv_rn(__fmul_rn(__fsub_rn(xb, xa), __fsub_rn(y, ya)), __fsub_rn(yb, ya))))
-        in = !in;
-      xa = xb;
-      ya = yb;
-    }
-    if (in != (fp.invert[p] != 0)) return true;
-  }
-  return false;
+  return footprint_removes(fp, np, [&](float* x, float* y) {
+    double sn, cs;
+    sincos_f64(__dmul_rn((double)i, (double)inc), &sn, &cs);
+    *x = __fmul_rn(r, __double2float_rn(cs));
+    *y = __fmul_rn(r, __double2float_rn(sn));
+  });
 }
 
 // speckle: a finite beam with fewer than n neighbours within w beams and max_diff of its range

@@ -1114,6 +1114,59 @@ rpl_result rpl_cloud_footprint_batch_dev(rpl_ctx* ctx, const rpl_node_hq* nodes,
                                          const rpl_scan_footprint* footprint /* nullable: none */, float* xyzi,
                                          uint32_t* point_counts, void* stream);
 
+/* Clouds projected from the LaserScans (DESIGN.md 5.7.1 "Clouds projected from the LaserScans"; INTEGRATION.md 4h):
+ * laser_geometry's LaserProjection::projectLaser of each published LaserScan, on the device, so the cloud agrees with
+ * the filtered, footprinted scan by construction.  P(params, scan) is a pure function of one LaserScan (ranges,
+ * intensities, angle_increment, time_increment, range_min, range_max; angle_min 0), defined bit for bit by
+ * oracle/scan_cloud_oracle.py:
+ *   kept:    beam i iff range_min <= r_i < cutoff, cutoff = range_cutoff when >= 0, else the scan's range_max (NaN and
+ *            +inf beams are never kept); the kept beams in beam order.
+ *   point:   x = fl(r_i * c_i), y = fl(r_i * s_i), z = 0 -- the point the footprint stage of the filters tests.
+ *   fields:  x, y, z (FLOAT32), then per channel bit, in this order: intensity (FLOAT32, intensities[i]), index (INT32,
+ *            i), distances (FLOAT32, r_i), stamps (FLOAT32, fl((float)i * time_increment)); offsets 0, 4, 8, ...;
+ *            point_step = 12 + 4 * popcount(channels).  Any other bit (laser_geometry's viewpoint 0x10 included):
+ *            RPL_RESULT_INVALID_DATA.
+ *   message: the LaserScan's stamp and frame_id, height 1, width the kept count, is_bigendian 0, row_step point_step *
+ *            width, is_dense 1.
+ * Offsets: channels 0, range_cutoff 4; 8 bytes. */
+typedef struct rpl_scan_cloud_params {
+  uint32_t channels;   /* RPL_SCAN_CLOUD_* bits; laser_geometry's default is INTENSITY | INDEX */
+  float range_cutoff;  /* < 0: each scan's range_max; NaN: RPL_RESULT_INVALID_DATA */
+} rpl_scan_cloud_params;
+#define RPL_SCAN_CLOUD_INTENSITY 0x01u
+#define RPL_SCAN_CLOUD_INDEX 0x02u
+#define RPL_SCAN_CLOUD_DISTANCE 0x04u
+#define RPL_SCAN_CLOUD_TIMESTAMP 0x08u
+/* Stateless: P(*params, scan s) of n_scans rows laid out as rpl_scan_batch_dev writes them (device arrays): ranges /
+ * intensities [n_scans][stride], beam_counts and angle_increment [n_scans]; time_increment [n_scans] (nullable: 0);
+ * range_min and range_max every scan's.  stride <= the context's max_nodes.  Scan s's point_step-byte records at
+ * points + s * stride * point_step (4-byte aligned), its kept count at point_counts[s].  Asynchronous on `stream`
+ * (NULL: the context's stream). */
+rpl_result rpl_scan_cloud_batch_dev(rpl_ctx* ctx, const rpl_scan_cloud_params* params, const float* ranges,
+                                    const float* intensities, const uint32_t* beam_counts,
+                                    const float* angle_increment, const float* time_increment /* nullable: 0 */,
+                                    float range_min, float range_max, uint32_t n_scans, uint32_t stride, void* points,
+                                    uint32_t* point_counts, void* stream);
+/* The session form: one PointCloud2 message per LaserScan message.
+ *   Definition: slot i has a message iff rpl_capsule_stream_laserscan_msgs with the same scan_params gives it one (so
+ *            RPL_FLAG_PER_STREAM and RPL_FLAG_PER_STREAM_FILTERS, footprints included, apply as they do there), and that
+ *            message is P(*cloud_params, that LaserScan message).  A scan whose beams are all removed has a message of
+ *            width 0.
+ *   Packing, capacity, alignment, _dev and host: those of rpl_capsule_stream_laserscan_msgs[_dev], with exact sizes:
+ *            msg_offsets the exclusive scan of the sizes rounded up to 16, all or nothing.
+ *   Errors:  a null argument, an unknown channel bit, a NaN range_cutoff, misaligned device outputs, and the checks of
+ *            laserscan_msgs with scan_params (its flags before set_lidars / set_scan_filters): RPL_RESULT_INVALID_DATA.
+ *   Cost:    the session's message work block holds every slot's LaserScan (8 bytes per node of max_nodes) and 4 bytes
+ *            per slot for the kept counts.  No state is kept between calls. */
+rpl_result rpl_capsule_stream_scan_cloud_msgs_dev(rpl_capsule_stream* s, const rpl_scan_params* scan_params,
+                                                  const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
+                                                  uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,
+                                                  uint32_t* msg_sizes, uint64_t* total_bytes, void* stream);
+rpl_result rpl_capsule_stream_scan_cloud_msgs(rpl_capsule_stream* s, const rpl_scan_params* scan_params,
+                                              const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
+                                              uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,
+                                              uint32_t* msg_sizes, uint64_t* total_bytes);
+
 /* ---- LaserScan / PointCloud2 -> wire (SURVEY.md 8(f) rank 3) ---------------------------- */
 /* The serialised message the RMW layer would produce from the message the reference publishes
  * (scan_pub_->publish, reference src/rplidar_node.cpp:679): XCDR1 little endian, 4-byte

@@ -31,6 +31,8 @@ CLOUD_NO_FUSED = 1
 CLOUD_PER_STREAM = 2
 CLOUD_PER_STREAM_CHAIN = 4
 CLOUD_PER_STREAM_FOOTPRINTS = 8
+# rpl_scan_cloud_params.channels (laser_geometry ChannelOption)
+SCAN_CLOUD_INTENSITY, SCAN_CLOUD_INDEX, SCAN_CLOUD_DISTANCE, SCAN_CLOUD_TIMESTAMP = 1, 2, 4, 8
 CAPSULE_OK, CAPSULE_SYNC, CAPSULE_EMIT, CAPSULE_DISCARD = 1, 2, 4, 8
 CAPSULE_CHECKSUM_ERR, CAPSULE_ENCODER_RESET_ERR, CAPSULE_BAD_FRAME = 16, 32, 64
 PATH_FAST, PATH_GENERAL = 0, 1
@@ -67,6 +69,7 @@ EXPORTS = [
     "rpl_capsule_stream_push_cloud_msgs", "rpl_capsule_stream_push_cloud_msgs_dev",
     "rpl_scan_filter_batch_dev", "rpl_capsule_stream_set_scan_filters",
     "rpl_scan_filter_footprint_batch_dev", "rpl_capsule_stream_set_scan_footprints", "rpl_cloud_footprint_batch_dev",
+    "rpl_scan_cloud_batch_dev", "rpl_capsule_stream_scan_cloud_msgs", "rpl_capsule_stream_scan_cloud_msgs_dev",
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -171,6 +174,12 @@ class ScanFootprint(C.Structure):
         ("pose_y", C.c_float),
         ("pose_yaw", C.c_float),
     ]
+
+
+class ScanCloudParams(C.Structure):
+    """rpl_scan_cloud_params: the projection of LaserScans into PointCloud2 (laser_geometry's projectLaser; 8 bytes).
+    oracle/scan_cloud_oracle.py defines what it does."""
+    _fields_ = [("channels", C.c_uint32), ("range_cutoff", C.c_float)]
 
 
 # rpl_stream_counters: one stream session stream's counters (include/rpl_b200.h)
@@ -305,6 +314,12 @@ def lib() -> C.CDLL:
         "rpl_capsule_stream_set_scan_footprints": ([vp, vp, vp], u32),
         "rpl_scan_filter_footprint_batch_dev":
             ([vp, C.POINTER(ScanFilterSettings), C.POINTER(ScanFootprint), vp, vp, vp, vp, u32, u32, vp], u32),
+        "rpl_scan_cloud_batch_dev": ([vp, C.POINTER(ScanCloudParams), vp, vp, vp, vp, vp, C.c_float, C.c_float, u32, u32,
+                                      vp, vp, vp], u32),
+        "rpl_capsule_stream_scan_cloud_msgs":
+            ([vp, PSP, C.POINTER(ScanCloudParams), C.c_int64, vp, u64, vp, vp, vp], u32),
+        "rpl_capsule_stream_scan_cloud_msgs_dev":
+            ([vp, PSP, C.POINTER(ScanCloudParams), C.c_int64, vp, u64, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_laserscan_msgs": ([vp, PSP, C.c_int64, vp, u64, vp, vp, vp], u32),
         "rpl_capsule_stream_laserscan_msgs_dev": ([vp, PSP, C.c_int64, vp, u64, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_cloud_msgs": ([vp, PCP, C.c_int64, vp, u64, vp, vp, vp], u32),
@@ -376,6 +391,16 @@ def scan_footprint(polygons=(), invert=(), pose=(0.0, 0.0, 0.0)) -> ScanFootprin
         f.invert[p] = int(bool(b))
     f.pose_x, f.pose_y, f.pose_yaw = (float(v) for v in pose)
     return f
+
+
+def scan_cloud_params(channels=SCAN_CLOUD_INTENSITY | SCAN_CLOUD_INDEX, range_cutoff=-1.0) -> ScanCloudParams:
+    """laser_geometry's defaults: the intensity and index channels, range_cutoff -1 (each scan's range_max)."""
+    return ScanCloudParams(int(channels), float(range_cutoff))
+
+
+def scan_cloud_point_step(channels) -> int:
+    """the bytes of one record: x, y, z and 4 per channel bit"""
+    return 12 + 4 * bin(int(channels) & 0xF).count("1")
 
 
 def _timing(t):
@@ -732,6 +757,15 @@ class Context:
             self._h, C.byref(settings), C.byref(footprint) if footprint is not None else None, _p(ranges),
             _p(intensities), _p(beam_counts), _p(angle_increment), n_scans, stride, _p(stream)))
 
+    def scan_cloud_batch_dev(self, params: ScanCloudParams, ranges, intensities, beam_counts, angle_increment,
+                             time_increment, range_min, range_max, n_scans, stride, points, point_counts, stream=None):
+        """The projection of rows of rpl_scan_batch_dev's layout (device addresses; time_increment None: 0): scan s's
+        point_step-byte records at points + s * stride * point_step, its kept count at point_counts[s]."""
+        self._check(self._L.rpl_scan_cloud_batch_dev(
+            self._h, C.byref(params), _p(ranges), _p(intensities), _p(beam_counts), _p(angle_increment),
+            _p(time_increment), float(range_min), float(range_max), n_scans, stride, _p(points), _p(point_counts),
+            _p(stream)))
+
     def cloud_fuse_dev(self, xyzi, point_counts, n_scans, stride, fused, offsets, total, stream=None):
         self._check(self._L.rpl_cloud_fuse_dev(self._h, _p(xyzi), _p(point_counts), n_scans, stride, _p(fused),
                                                _p(offsets), _p(total), _p(stream)))
@@ -896,15 +930,21 @@ class CapsuleStreamSession:
         assert m is None or m.shape == (self.n_streams,)
         self._ctx._check(self._fn("set_scan_footprints")(self._h, C.cast(arr, C.c_void_p), _p(m)))
 
-    def _msgs(self, name, params, clock_offset_ns, msgs, packed):
+    def _msgs(self, name, params, clock_offset_ns, msgs, packed, cloud_params=None):
         ns = self.n_streams * self.max_scans
         if msgs is None:  # room for every slot's largest message
-            per = 288 + (32 + 8 * self.max_nodes + 4 if name == "laserscan_msgs" else 116 + 16 * self.max_nodes + 1)
+            if name == "laserscan_msgs":
+                per = 288 + 32 + 8 * self.max_nodes + 4
+            elif name == "scan_cloud_msgs":
+                per = 288 + 192 + scan_cloud_point_step(cloud_params.channels) * self.max_nodes + 1
+            else:
+                per = 288 + 116 + 16 * self.max_nodes + 1
             msgs = np.zeros(ns * ((per + 15) // 16 * 16), np.uint8)
         assert msgs.dtype == np.uint8 and msgs.flags.c_contiguous
         offs, sizes, total = np.zeros(ns, np.uint64), np.zeros(ns, np.uint32), np.zeros(1, np.uint64)
-        rc = self._fn(name)(self._h, C.byref(params), int(clock_offset_ns), _p(msgs), msgs.size, _p(offs), _p(sizes),
-                            _p(total))
+        extra = () if cloud_params is None else (C.byref(cloud_params),)
+        rc = self._fn(name)(self._h, C.byref(params), *extra, int(clock_offset_ns), _p(msgs), msgs.size, _p(offs),
+                            _p(sizes), _p(total))
         if not packed or rc != RESULT_INSUFFICIENT_MEMORY:
             self._ctx._check(rc)
         if packed:
@@ -921,6 +961,19 @@ class CapsuleStreamSession:
     def cloud_msgs(self, params: CloudParams, clock_offset_ns=0, msgs=None, packed=False):
         """The serialised sensor_msgs/PointCloud2 of every published slot, as laserscan_msgs."""
         return self._msgs("cloud_msgs", params, clock_offset_ns, msgs, packed)
+
+    def scan_cloud_msgs(self, params: ScanParams, cloud_params: ScanCloudParams, clock_offset_ns=0, msgs=None,
+                        packed=False):
+        """The serialised sensor_msgs/PointCloud2 projected from every LaserScan message laserscan_msgs(params) gives
+        (laser_geometry's projectLaser with cloud_params), as laserscan_msgs returns them."""
+        return self._msgs("scan_cloud_msgs", params, clock_offset_ns, msgs, packed, cloud_params)
+
+    def scan_cloud_msgs_dev(self, params: ScanParams, cloud_params: ScanCloudParams, clock_offset_ns, msgs, capacity,
+                            msg_offsets, msg_sizes, total_bytes, stream=None):
+        """Device addresses, as laserscan_msgs_dev."""
+        self._ctx._check(self._fn("scan_cloud_msgs_dev")(
+            self._h, C.byref(params), C.byref(cloud_params), int(clock_offset_ns), _p(msgs), int(capacity),
+            _p(msg_offsets), _p(msg_sizes), _p(total_bytes), _p(stream)))
 
     def laserscan_msgs_dev(self, params: ScanParams, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
                            total_bytes, stream=None):

@@ -18,6 +18,7 @@
 // PARITY UNPINNED: the reference holds no serialiser (it lives in the RMW dependency); the format
 // follows the OMG CDR rules above and oracle/cdr_oracle.py restates it independently in numpy.
 #include "cdr_args.h"
+#include "msg_fixed.cuh"
 #include "rpl_device.cuh"
 #include "scan_args.h"
 
@@ -26,8 +27,6 @@ namespace rpl {
 namespace {
 
 constexpr int CT = 256;
-
-__device__ __forceinline__ void put32(uint8_t* p, uint32_t v) { *reinterpret_cast<uint32_t*>(p) = v; }
 
 __global__ void __launch_bounds__(CT) laserscan_cdr_kernel(LaserScanCdrArgs a, CdrTemplate t) {
   const uint32_t s = blockIdx.y;
@@ -111,6 +110,8 @@ __global__ void __launch_bounds__(MT) msg_table_kernel(MsgTableArgs a) {
   unsigned long long carry = 0;
   auto size_of = [&](uint32_t i) -> uint32_t {
     const uint32_t n = a.counts[i];
+    if (a.kind == MsgKind::kScanCloud)
+      return a.beams[i] > 0 ? a.hdr[i / a.max_scans].bytes + a.tail_bytes + a.point_step * n + 1 : 0u;
     const bool has = a.kind == MsgKind::kLaserScan
                          ? n > 0
                          : a.views[i].y > 0 && !(a.clouds && a.clouds[i / a.max_scans].route == kCloudOff);
@@ -148,32 +149,6 @@ __global__ void __launch_bounds__(MT) msg_table_kernel(MsgTableArgs a) {
   if (tid == 0) *a.total = total;
 }
 
-// header.stamp of a scan-begin stamp b (SDK us) on the caller's clock: {0, 0} when unknown or not representable
-__device__ __forceinline__ void msg_stamp(unsigned long long b, long long offset_ns, uint32_t* sec, uint32_t* nanosec) {
-  *sec = 0;
-  *nanosec = 0;
-  if (b == 0) return;
-  const long long t = (long long)(b * 1000ull + (unsigned long long)offset_ns);  // int64 ns, two's complement
-  if (t < 0) return;
-  const long long s = t / 1000000000ll;
-  if (s > 2147483647ll) return;
-  *sec = (uint32_t)s;
-  *nanosec = (uint32_t)(t - s * 1000000000ll);
-}
-
-// rclcpp's Duration::seconds() of the stamp-to-stamp period (0 when either stamp is unknown or the period is not > 0)
-__device__ __forceinline__ double msg_period(unsigned long long b, unsigned long long e) {
-  if (b == 0 || e == 0 || e <= b) return 0.0;
-  return (double)(long long)((e - b) * 1000ull) / 1e9;
-}
-
-// the header words of the stream's settings, stamp words left to the caller (no two threads write one word); T threads
-template <int T = CT>
-__device__ __forceinline__ void put_header(uint8_t* msg, const StreamMsgHeader& h) {
-  for (uint32_t w = threadIdx.x; w < h.bytes / 4; w += T)
-    if (w != 1 && w != 2) put32(msg + 4 * w, h.w[w]);
-}
-
 // LaserScan message i's fixed part -- header, stamp, the 7 floats, both sequence lengths -- for n beams, by the T threads
 // of a CTA; P = h.bytes + 32, where the ranges start
 template <int T>
@@ -186,16 +161,15 @@ __device__ __forceinline__ void put_laserscan_fixed(const MsgWriteArgs& a, uint3
     msg_stamp(b, a.clock_offset_ns, &sec, &nsec);
     const double d = msg_period(b, e);
     const bool mode_a = a.lidars ? a.lidars[i / a.max_scans].mode_a != 0 : a.mode_a != 0;
-    const double denom = mode_a ? (double)n : (double)(n > 1 ? n - 1 : 1);
     put32(msg + 4, sec);
     put32(msg + 8, nsec);
     uint8_t* f = msg + h.bytes;
     put32(f + 0, __float_as_uint(0.0f));                             // angle_min
     put32(f + 4, __float_as_uint((float)(2.0 * 3.14159265358979323846)));  // angle_max
     put32(f + 8, __float_as_uint(a.angle_increment[i]));
-    put32(f + 12, __float_as_uint(__double2float_rn(d / denom)));    // time_increment
+    put32(f + 12, __float_as_uint(msg_time_increment(d, mode_a, n)));
     put32(f + 16, __float_as_uint(__double2float_rn(d)));            // scan_time
-    put32(f + 20, __float_as_uint(0.15f));                           // range_min
+    put32(f + 20, __float_as_uint(kLaserScanRangeMin));
     put32(f + 24, __float_as_uint(h.range_max));
     put32(f + 28, n);
     put32(msg + P + 4 * (size_t)n, n);  // intensities count

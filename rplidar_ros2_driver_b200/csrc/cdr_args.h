@@ -66,7 +66,8 @@ struct CloudTail {
   uint32_t at_width, at_row_step, at_data;  // word indices patched per message
 };
 
-enum class MsgKind : uint32_t { kLaserScan, kPointCloud2 };
+// kScanCloud: the projection of each slot's LaserScan (scan_cloud.cu), a PointCloud2 of point_step-byte records
+enum class MsgKind : uint32_t { kLaserScan, kPointCloud2, kScanCloud };
 
 // sizes and offsets pass: one CTA over every slot
 struct MsgTableArgs {
@@ -80,6 +81,10 @@ struct MsgTableArgs {
   uint32_t* sizes;                 // [n_slots] out: message bytes, 0 for no message or when the total exceeds capacity
   unsigned long long* total;       // out: end of the last message
   const CloudSettings* clouds;     // [n_slots / max_scans] nullable, PointCloud2: a kCloudOff stream's slots have none
+  // kScanCloud: a slot has a message iff its LaserScan has beams (beams[i] > 0), of header + tail_bytes + point_step *
+  // counts[i] + 1 (is_dense) bytes
+  const uint32_t* beams;
+  uint32_t tail_bytes, point_step;
 };
 
 // the writers, over slots [slot0, slot0 + n) (slot indices count from the first slot of the call)

@@ -21,6 +21,7 @@
 #include "cdr_args.h"
 #include "decode_args.h"
 #include "scan_args.h"
+#include "scan_cloud_args.h"
 #include "scan_filter_args.h"
 #include "session_migrate_args.h"
 #include "session_nodes_args.h"
@@ -693,6 +694,132 @@ rpl_result rpl_scan_filter_footprint_batch_dev(rpl_ctx* c, const rpl_scan_filter
   a.angle_increment = angle_increment;
   a.n_scans = n_scans;
   RPL_CUDA(c, rpl::launch_scan_filter(a, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+  c->launches++;
+  return RPL_RESULT_OK;
+}
+
+static_assert(sizeof(rpl_scan_cloud_params) == 8 && offsetof(rpl_scan_cloud_params, range_cutoff) == 4 &&
+                  RPL_SCAN_CLOUD_INTENSITY == rpl::kScanCloudIntensity && RPL_SCAN_CLOUD_INDEX == rpl::kScanCloudIndex &&
+                  RPL_SCAN_CLOUD_DISTANCE == rpl::kScanCloudDistance &&
+                  RPL_SCAN_CLOUD_TIMESTAMP == rpl::kScanCloudTimestamp,
+              "rpl_scan_cloud_params and its channel bits are the header's");
+
+namespace {
+
+// the rules of rpl_scan_cloud_params (oracle/scan_cloud_oracle.py params_ok)
+bool scan_cloud_ok(rpl_ctx* c, const rpl_scan_cloud_params& p) {
+  const char* why = nullptr;
+  if (p.channels & ~rpl::kScanCloudChannels) why = "unknown scan cloud channel bits (only 0x01, 0x02, 0x04, 0x08)";
+  else if (std::isnan(p.range_cutoff)) why = "range_cutoff is NaN";
+  if (why) c->err = why;
+  return why == nullptr;
+}
+
+uint32_t scan_cloud_point_step(uint32_t channels) { return 12u + 4u * (uint32_t)__builtin_popcount(channels); }
+
+// The PointCloud2 members between the header and the data of fields names[0..nf) (datatypes types[], count 1, offsets
+// 4 bytes apart from 0): height 1, width, the fields, is_bigendian 0, point_step, row_step, data length
+extern "C++" template <class Tail>
+Tail pointcloud2_tail(const char* const* names, const uint8_t* types, uint32_t nf, uint32_t point_step) {
+  Tail t{};
+  uint8_t* b = reinterpret_cast<uint8_t*>(t.w);
+  uint32_t n = 0;
+  auto u32 = [&](uint32_t v) {
+    n = (n + 3) & ~3u;
+    std::memcpy(b + n, &v, 4);
+    n += 4;
+  };
+  u32(1);
+  t.at_width = n / 4;
+  u32(0);
+  u32(nf);
+  for (uint32_t f = 0; f < nf; ++f) {
+    const uint32_t L = (uint32_t)std::strlen(names[f]);
+    u32(L + 1);
+    std::memcpy(b + n, names[f], L + 1);
+    n += L + 1;
+    u32(4 * f);
+    b[n++] = types[f];
+    u32(1);
+  }
+  b[n++] = 0;  // is_bigendian
+  u32(point_step);
+  t.at_row_step = (n + 3) / 4;
+  u32(0);
+  t.at_data = n / 4;
+  u32(0);
+  t.bytes = n;
+  return t;
+}
+
+// the tail of a channel set: x, y, z, then laser_geometry's channels in bit order
+const rpl::ScanCloudTail& scan_cloud_tail(uint32_t channels) {
+  static const std::vector<rpl::ScanCloudTail> tails = [] {
+    std::vector<rpl::ScanCloudTail> v(rpl::kScanCloudChannels + 1);
+    const char* const channel_names[4] = {"intensity", "index", "distances", "stamps"};
+    const uint8_t channel_types[4] = {7, 5, 7, 7};  // FLOAT32, INT32, FLOAT32, FLOAT32
+    for (uint32_t ch = 0; ch <= rpl::kScanCloudChannels; ++ch) {
+      const char* names[7] = {"x", "y", "z"};
+      uint8_t types[7] = {7, 7, 7};
+      uint32_t nf = 3;
+      for (uint32_t k = 0; k < 4; ++k)
+        if (ch & (1u << k)) {
+          names[nf] = channel_names[k];
+          types[nf++] = channel_types[k];
+        }
+      v[ch] = pointcloud2_tail<rpl::ScanCloudTail>(names, types, nf, scan_cloud_point_step(ch));
+    }
+    return v;
+  }();
+  return tails[channels];
+}
+
+// the settings of params into a
+void scan_cloud_setup(rpl::ScanCloudArgs& a, const rpl_scan_cloud_params& p) {
+  a.channels = p.channels;
+  a.point_step = scan_cloud_point_step(p.channels);
+  a.range_cutoff = p.range_cutoff;
+  a.tail = scan_cloud_tail(p.channels);
+}
+
+}  // namespace
+
+rpl_result rpl_scan_cloud_batch_dev(rpl_ctx* c, const rpl_scan_cloud_params* params, const float* ranges,
+                                    const float* intensities, const uint32_t* beam_counts,
+                                    const float* angle_increment, const float* time_increment, float range_min,
+                                    float range_max, uint32_t n_scans, uint32_t stride, void* points,
+                                    uint32_t* point_counts, void* stream) {
+  if (!c) return RPL_RESULT_INVALID_DATA;
+  if (!params || !ranges || !intensities || !beam_counts || !angle_increment || !points || !point_counts) {
+    c->err = "null params, ranges, intensities, beam_counts, angle_increment, points or point_counts";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  if (!scan_cloud_ok(c, *params)) return RPL_RESULT_INVALID_DATA;
+  if (n_scans != 0 && (stride == 0 || stride > c->max_nodes)) {
+    c->err = "stride must be in [1, the context's max_nodes]";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  if (reinterpret_cast<uintptr_t>(points) & 3u) {
+    c->err = "points must be 4-byte aligned";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
+  if (n_scans == 0) return RPL_RESULT_OK;
+  rpl::ScanCloudArgs a{};
+  scan_cloud_setup(a, *params);
+  a.m.counts = beam_counts;
+  a.m.ranges = ranges;
+  a.m.intensities = intensities;
+  a.m.angle_increment = angle_increment;
+  a.m.stride = stride;
+  a.m.n = n_scans;
+  a.range_min = range_min;
+  a.range_max = range_max;
+  a.time_increment = time_increment;
+  a.kept = point_counts;
+  a.points = static_cast<float*>(points);
+  RPL_CUDA(c, rpl::launch_scan_cloud(a, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
   c->launches++;
   return RPL_RESULT_OK;
 }
@@ -3060,39 +3187,11 @@ rpl_result stream_set_scan_footprints(rpl_capsule_stream* cs, const rpl_scan_foo
   return RPL_RESULT_OK;
 }
 
-// the PointCloud2 members between the header and the data: height 1, width, the fields x, y, z, intensity (float32,
-// count 1), is_bigendian 0, point_step 16, row_step, data length
+// the PointCloud2 members between the header and the data: the fields x, y, z, intensity (float32), point_step 16
 rpl::CloudTail cloud_tail() {
-  rpl::CloudTail t{};
-  uint8_t* b = reinterpret_cast<uint8_t*>(t.w);
-  uint32_t n = 0;
-  auto u32 = [&](uint32_t v) {
-    n = (n + 3) & ~3u;
-    std::memcpy(b + n, &v, 4);
-    n += 4;
-  };
-  u32(1);
-  t.at_width = n / 4;
-  u32(0);
-  u32(4);
   const char* names[4] = {"x", "y", "z", "intensity"};
-  for (uint32_t f = 0; f < 4; ++f) {
-    const uint32_t L = (uint32_t)std::strlen(names[f]);
-    u32(L + 1);
-    std::memcpy(b + n, names[f], L + 1);
-    n += L + 1;
-    u32(4 * f);
-    b[n++] = 7;  // FLOAT32
-    u32(1);
-  }
-  b[n++] = 0;  // is_bigendian
-  u32(16);     // point_step
-  t.at_row_step = (n + 3) / 4;
-  u32(0);
-  t.at_data = n / 4;
-  u32(0);
-  t.bytes = n;
-  return t;
+  const uint8_t types[4] = {7, 7, 7, 7};  // FLOAT32
+  return pointcloud2_tail<rpl::CloudTail>(names, types, 4, 16);
 }
 
 // the work block of a messages call: scan outputs of every slot (LaserScan ranges then intensities, or xyzi), their
@@ -3104,13 +3203,27 @@ struct MsgWork {
   unsigned long long* offsets;
   uint32_t* sizes;
   unsigned long long* total;
+  uint32_t* kept;  // kScanCloud: the projections' point counts
 };
 MsgWork msg_work_layout(const rpl_capsule_stream* cs, rpl::MsgKind kind, bool tables, Carve& k) {
   const size_t NS = (size_t)cs->n_streams * cs->max_scans;
-  const size_t floats = NS * cs->max_nodes * (kind == rpl::MsgKind::kLaserScan ? 2 : 4);
+  const size_t floats = NS * cs->max_nodes * (kind == rpl::MsgKind::kPointCloud2 ? 4 : 2);
   return MsgWork{k.take<float>(floats), k.take<uint32_t>(NS), k.take<float>(NS),
                  k.take<unsigned long long>(tables ? NS : 0), k.take<uint32_t>(tables ? NS : 0),
-                 k.take<unsigned long long>(tables ? 1 : 0)};
+                 k.take<unsigned long long>(tables ? 1 : 0), k.take<uint32_t>(kind == rpl::MsgKind::kScanCloud ? NS : 0)};
+}
+
+// the params of a kScanCloud messages call
+struct ScanCloudCall {
+  const rpl_scan_params* scan;
+  const rpl_scan_cloud_params* cloud;
+};
+
+// the LaserScan params of a messages call (kLaserScan, kScanCloud), nullptr for kPointCloud2
+const rpl_scan_params* msgs_scan_params(rpl::MsgKind kind, const void* params) {
+  if (kind == rpl::MsgKind::kLaserScan) return static_cast<const rpl_scan_params*>(params);
+  if (kind == rpl::MsgKind::kScanCloud) return static_cast<const ScanCloudCall*>(params)->scan;
+  return nullptr;
 }
 
 bool stream_msgs_args_ok(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* params, const void* msgs,
@@ -3122,13 +3235,19 @@ bool stream_msgs_args_ok(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* 
   }
   if (kind == rpl::MsgKind::kPointCloud2 && !cloud_call_ok(cs, static_cast<const rpl_cloud_params*>(params)))
     return false;
-  const bool per_stream = kind == rpl::MsgKind::kLaserScan
-                              ? (static_cast<const rpl_scan_params*>(params)->flags & RPL_FLAG_PER_STREAM) != 0
-                              : (static_cast<const rpl_cloud_params*>(params)->flags & RPL_CLOUD_PER_STREAM) != 0;
+  if (kind == rpl::MsgKind::kScanCloud) {
+    const auto* q = static_cast<const ScanCloudCall*>(params);
+    if (!q->scan || !q->cloud) {
+      c->err = "null scan_params or cloud_params";
+      return false;
+    }
+    if (!scan_cloud_ok(c, *q->cloud)) return false;
+  }
+  const rpl_scan_params* sp = msgs_scan_params(kind, params);
+  const bool per_stream = sp ? (sp->flags & RPL_FLAG_PER_STREAM) != 0
+                             : (static_cast<const rpl_cloud_params*>(params)->flags & RPL_CLOUD_PER_STREAM) != 0;
   if (per_stream && !lidars_ok(cs)) return false;
-  if (kind == rpl::MsgKind::kLaserScan &&
-      (static_cast<const rpl_scan_params*>(params)->flags & RPL_FLAG_PER_STREAM_FILTERS) != 0 && !filters_ok(cs))
-    return false;
+  if (sp && (sp->flags & RPL_FLAG_PER_STREAM_FILTERS) != 0 && !filters_ok(cs)) return false;
   if (dev && ((reinterpret_cast<uintptr_t>(msgs) & 15u) || misaligned8(offsets) || misaligned8(total) ||
               (reinterpret_cast<uintptr_t>(sizes) & 3u))) {
     c->err = "msgs must be 16-byte aligned, msg_offsets and total_bytes 8-byte, msg_sizes 4-byte aligned";
@@ -3141,6 +3260,27 @@ bool stream_msgs_args_ok(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* 
   return true;
 }
 
+// the projection of every slot's LaserScan in w (kScanCloud): the count pass's arguments over all slots (msgs_write
+// adds the placement)
+rpl::ScanCloudArgs scan_cloud_msg_args(const rpl_capsule_stream* cs, const void* params, const MsgWork& w) {
+  const auto* q = static_cast<const ScanCloudCall*>(params);
+  const size_t NS = (size_t)cs->n_streams * cs->max_scans;
+  rpl::ScanCloudArgs a{};
+  scan_cloud_setup(a, *q->cloud);
+  a.m.hdr = cs->msg_hdr;
+  a.m.counts = w.counts;
+  a.m.ranges = w.data;
+  a.m.intensities = w.data + NS * cs->max_nodes;
+  a.m.angle_increment = w.inc;
+  a.m.stride = cs->max_nodes;
+  a.m.max_scans = cs->max_scans;
+  a.m.n = (uint32_t)NS;
+  a.m.mode_a = q->scan->scan_processing ? 1u : 0u;
+  if ((q->scan->flags & RPL_FLAG_PER_STREAM) != 0) a.m.lidars = cs->lidars;
+  a.kept = w.kept;
+  return a;
+}
+
 // on `st`, after the last push: the scan kernels or the cloud chain of every slot into w, then the tables
 rpl_result msgs_prepare(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* params, const MsgWork& w,
                         unsigned long long capacity, unsigned long long* offsets, uint32_t* sizes,
@@ -3148,11 +3288,12 @@ rpl_result msgs_prepare(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* p
   rpl_ctx* c = cs->c;
   const size_t NS = (size_t)cs->n_streams * cs->max_scans, row = cs->max_nodes;
   rpl_result r = RPL_RESULT_OK;
+  const rpl_scan_params* scan = msgs_scan_params(kind, params);
   for (uint32_t s0 = 0; s0 < cs->n_streams && r == RPL_RESULT_OK; s0 += cs->cloud_chunk) {
     const uint32_t ns = std::min(cs->cloud_chunk, cs->n_streams - s0);
     const size_t so = (size_t)s0 * cs->max_scans;
-    if (kind == rpl::MsgKind::kLaserScan) {
-      const auto* p = static_cast<const rpl_scan_params*>(params);
+    if (scan) {
+      const rpl_scan_params* p = scan;
       const rpl::ScanBatchArgs a = last_push_scans(cs, s0, ns);
       r = enqueue_scan(c, c->lane[0], reinterpret_cast<const rpl_node_hq*>(a.nodes), cs->scan_len + so, a.n_scans,
                        a.stride, p, nullptr, w.data + so * row, w.data + (NS + so) * row, w.counts + so, w.inc + so,
@@ -3171,9 +3312,17 @@ rpl_result msgs_prepare(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* p
   }
   if (r != RPL_RESULT_OK) return r;
   rpl::MsgTableArgs t{};
+  if (kind == rpl::MsgKind::kScanCloud) {  // the kept counts size the messages
+    const rpl::ScanCloudArgs a = scan_cloud_msg_args(cs, params, w);
+    RPL_CUDA(c, rpl::launch_scan_cloud_count(a, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+    c->launches++;
+    t.beams = w.counts;
+    t.tail_bytes = a.tail.bytes;
+    t.point_step = a.point_step;
+  }
   t.kind = kind;
   t.hdr = cs->msg_hdr;
-  t.counts = w.counts;
+  t.counts = kind == rpl::MsgKind::kScanCloud ? w.kept : w.counts;
   t.views = reinterpret_cast<const uint2*>(cs->views);
   t.n_slots = (uint32_t)NS;
   t.max_scans = cs->max_scans;
@@ -3212,6 +3361,21 @@ rpl_result msgs_write(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* par
   a.sizes = sizes;
   a.out = out;
   a.out_base = out_base;
+  if (kind == rpl::MsgKind::kScanCloud) {  // the count pass's LaserScans and settings, with a's stamps and placement
+    rpl::ScanCloudArgs sa = scan_cloud_msg_args(cs, params, w);
+    sa.m.slot0 = slot0;
+    sa.m.n = n;
+    sa.m.begin_us = a.begin_us;
+    sa.m.end_us = a.end_us;
+    sa.m.clock_offset_ns = clock_offset_ns;
+    sa.m.offsets = offsets;
+    sa.m.sizes = sizes;
+    sa.m.out = out;
+    sa.m.out_base = out_base;
+    RPL_CUDA(c, rpl::launch_scan_cloud(sa, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+    c->launches++;
+    return RPL_RESULT_OK;
+  }
   if (kind == rpl::MsgKind::kLaserScan) {
     a.ranges = w.data;
     a.intensities = w.data + NS * cs->max_nodes;
@@ -4229,6 +4393,24 @@ rpl_result rpl_capsule_stream_cloud_msgs(rpl_capsule_stream* s, const rpl_cloud_
                                          uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
                                          uint64_t* total_bytes) {
   return stream_msgs(s, rpl::MsgKind::kPointCloud2, params, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
+                     total_bytes);
+}
+
+rpl_result rpl_capsule_stream_scan_cloud_msgs_dev(rpl_capsule_stream* s, const rpl_scan_params* scan_params,
+                                                  const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
+                                                  uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,
+                                                  uint32_t* msg_sizes, uint64_t* total_bytes, void* stream) {
+  const ScanCloudCall q{scan_params, cloud_params};
+  return stream_msgs_dev(s, rpl::MsgKind::kScanCloud, &q, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
+                         total_bytes, stream);
+}
+
+rpl_result rpl_capsule_stream_scan_cloud_msgs(rpl_capsule_stream* s, const rpl_scan_params* scan_params,
+                                              const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
+                                              uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,
+                                              uint32_t* msg_sizes, uint64_t* total_bytes) {
+  const ScanCloudCall q{scan_params, cloud_params};
+  return stream_msgs(s, rpl::MsgKind::kScanCloud, &q, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
                      total_bytes);
 }
 

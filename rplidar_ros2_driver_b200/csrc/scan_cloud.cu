@@ -1,0 +1,150 @@
+// scan_cloud.cu -- the projection of published LaserScans into PointCloud2 (DESIGN.md 5.7.1 "Clouds projected from the
+// LaserScans"), laser_geometry's LaserProjection::projectLaser, whose definition and CPU restatement is
+// oracle/scan_cloud_oracle.py: beam i is kept iff range_min <= r_i < cutoff, and becomes the record x, y, z = 0 and the
+// chosen channels, the kept beams in beam order.  x, y is beam_point.cuh's point, the one the footprint stage of the
+// filters tests.
+//
+// One CTA per scan slot over a persistent grid.  The count pass gives each slot's kept count, from which msg_table_kernel
+// (cdr.cu) places a session's messages exactly; the write pass decides every beam again, compacts the kept ones chunk by
+// chunk (a warp ballot for the lane's place, the warps' counts in shared memory for the block's) and writes each record
+// straight into its row or into its message's data, and a message's fixed part from the stream's header and the call's
+// tail.  Both passes read the ranges only once per beam; no state is kept.
+#include <algorithm>
+
+#include "beam_point.cuh"
+#include "msg_fixed.cuh"
+#include "scan_cloud_args.h"
+
+namespace rpl {
+namespace {
+
+constexpr int ST = 256;
+
+__device__ __forceinline__ bool keep_beam(float r, float range_min, float cutoff) {
+  return r >= range_min && r < cutoff;  // NaN never, +inf never (cutoff <= +inf)
+}
+
+// the window of slot i: a session's LaserScan range_min and its stream's range_max, or the call's; the cutoff
+__device__ __forceinline__ void slot_window(const ScanCloudArgs& a, uint32_t i, float* lo, float* cut) {
+  const float hi = a.m.hdr ? a.m.hdr[i / a.m.max_scans].range_max : a.range_max;
+  *lo = a.m.hdr ? kLaserScanRangeMin : a.range_min;
+  *cut = a.range_cutoff >= 0.0f ? a.range_cutoff : hi;
+}
+
+__global__ void __launch_bounds__(ST) scan_cloud_count_kernel(const __grid_constant__ ScanCloudArgs a) {
+  for (uint32_t s = blockIdx.x; s < a.m.n; s += gridDim.x) {
+    const uint32_t i = a.m.slot0 + s;
+    const uint32_t M = min(a.m.counts[i], a.m.stride);
+    const float* rg = a.m.ranges + (size_t)i * a.m.stride;
+    float lo, cut;
+    slot_window(a, i, &lo, &cut);
+    uint32_t n = 0;
+    for (uint32_t b0 = 0; b0 < M; b0 += ST) {
+      const uint32_t j = b0 + threadIdx.x;
+      n += __syncthreads_count(j < M && keep_beam(rg[j], lo, cut));
+    }
+    if (threadIdx.x == 0) a.kept[i] = n;
+  }
+}
+
+__global__ void __launch_bounds__(ST) scan_cloud_kernel(const __grid_constant__ ScanCloudArgs a) {
+  __shared__ uint32_t s_warp[ST / 32];
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t words = a.point_step / 4, ch = a.channels;
+  for (uint32_t s = blockIdx.x; s < a.m.n; s += gridDim.x) {
+    const uint32_t i = a.m.slot0 + s;
+    const uint32_t M = min(a.m.counts[i], a.m.stride);
+    float ti;
+    uint32_t* data;
+    if (a.m.out) {
+      if (a.m.sizes[i] == 0) continue;  // no message, or the messages do not fit
+      const StreamMsgHeader& h = a.m.hdr[i / a.m.max_scans];
+      uint8_t* msg = a.m.out + (a.m.offsets[i] - a.m.out_base);
+      const uint32_t P = h.bytes + a.tail.bytes, n = a.kept[i];
+      put_header<ST>(msg, h);
+      for (uint32_t w = tid; w < a.tail.bytes / 4; w += ST) {
+        const uint32_t v = w == a.tail.at_width ? n
+                           : (w == a.tail.at_row_step || w == a.tail.at_data) ? a.point_step * n
+                                                                               : a.tail.w[w];
+        put32(msg + h.bytes + 4 * w, v);
+      }
+      const unsigned long long b = a.m.begin_us ? a.m.begin_us[i] : 0ull, e = a.m.end_us ? a.m.end_us[i] : 0ull;
+      if (tid == 0) {
+        uint32_t sec, nsec;
+        msg_stamp(b, a.m.clock_offset_ns, &sec, &nsec);
+        put32(msg + 4, sec);
+        put32(msg + 8, nsec);
+        msg[P + (size_t)a.point_step * n] = 1;  // is_dense: every kept point is finite
+      }
+      const bool mode_a = a.m.lidars ? a.m.lidars[i / a.m.max_scans].mode_a != 0 : a.m.mode_a != 0;
+      ti = msg_time_increment(msg_period(b, e), mode_a, M);  // the LaserScan message's time_increment
+      data = reinterpret_cast<uint32_t*>(msg + P);
+    } else {
+      ti = a.time_increment ? a.time_increment[i] : 0.0f;
+      data = reinterpret_cast<uint32_t*>(a.points) + (size_t)s * a.m.stride * words;
+    }
+    const float* rg = a.m.ranges + (size_t)i * a.m.stride;
+    const float* ig = a.m.intensities + (size_t)i * a.m.stride;
+    const float inc = M ? a.m.angle_increment[i] : 0.0f;
+    float lo, cut;
+    slot_window(a, i, &lo, &cut);
+    uint32_t done = 0;
+    for (uint32_t b0 = 0; b0 < M; b0 += ST) {
+      const uint32_t j = b0 + tid;
+      const float r = j < M ? rg[j] : 0.0f;
+      const bool keep = j < M && keep_beam(r, lo, cut);
+      const uint32_t bal = __ballot_sync(0xFFFFFFFFu, keep);
+      if (lane == 0) s_warp[warp] = __popc(bal);
+      __syncthreads();
+      uint32_t base = 0, tot = 0;
+#pragma unroll
+      for (int v = 0; v < ST / 32; ++v) {
+        const uint32_t t = s_warp[v];
+        if ((uint32_t)v < warp) base += t;
+        tot += t;
+      }
+      __syncthreads();  // s_warp is rewritten by the next chunk
+      if (keep) {
+        uint32_t* p = data + (size_t)(done + base + __popc(bal & ((1u << lane) - 1u))) * words;
+        float x, y;
+        beam_point(j, inc, r, &x, &y);
+        p[0] = __float_as_uint(x);
+        p[1] = __float_as_uint(y);
+        p[2] = 0u;
+        uint32_t k = 3;
+        if (ch & kScanCloudIntensity) p[k++] = __float_as_uint(ig[j]);
+        if (ch & kScanCloudIndex) p[k++] = j;
+        if (ch & kScanCloudDistance) p[k++] = __float_as_uint(r);
+        if (ch & kScanCloudTimestamp) p[k++] = __float_as_uint(__fmul_rn((float)j, ti));
+      }
+      done += tot;
+    }
+    if (!a.m.out && tid == 0) a.kept[i] = done;
+  }
+}
+
+// a persistent grid: as many CTAs as can be resident at once (the kernel's occupancy, asked once)
+template <class K>
+int per_sm(K kernel) {
+  int n = 0;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, ST, 0);
+  return std::max(n, 1);
+}
+
+}  // namespace
+
+cudaError_t launch_scan_cloud_count(const ScanCloudArgs& a, int num_sms, cudaStream_t stream) {
+  if (a.m.n == 0) return cudaSuccess;
+  static const int k = per_sm(scan_cloud_count_kernel);
+  scan_cloud_count_kernel<<<(int)std::min<uint32_t>(a.m.n, (uint32_t)(num_sms * k)), ST, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_scan_cloud(const ScanCloudArgs& a, int num_sms, cudaStream_t stream) {
+  if (a.m.n == 0) return cudaSuccess;
+  static const int k = per_sm(scan_cloud_kernel);
+  scan_cloud_kernel<<<(int)std::min<uint32_t>(a.m.n, (uint32_t)(num_sms * k)), ST, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
+}  // namespace rpl

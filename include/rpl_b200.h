@@ -1167,6 +1167,59 @@ rpl_result rpl_capsule_stream_scan_cloud_msgs(rpl_capsule_stream* s, const rpl_s
                                               uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,
                                               uint32_t* msg_sizes, uint64_t* total_bytes);
 
+/* LaserScans and their projected clouds from the push (DESIGN.md 5.7.1 "LaserScans and their projected clouds from the
+ * push"): one call that pushes `in` and returns both the LaserScan messages of the scans it published and the
+ * PointCloud2 projection of each.  Each chunk of the push runs the push_laserscan_msgs chunk (decode, assemble, the
+ * LaserScan directory, the scan kernels and filters writing into the placed messages, their fixed parts), then
+ * projects every LaserScan message where it lies: a count pass, the clouds' directory, the write pass.  The scan
+ * kernels run once per scan; the message calls of the last push replay it.
+ *   in, scan_params: as rpl_capsule_stream_push_laserscan_msgs (every RPL_FLAG_*, per-stream lidars and per-stream
+ *            filters with their footprints included).  cloud_params: as rpl_capsule_stream_scan_cloud_msgs.
+ *   Definition: with two sessions of the same history, A pushed with rpl_capsule_stream_push_laserscan_msgs[_dev]
+ *            (in, scan_params) and then took rpl_capsule_stream_scan_cloud_msgs[_dev] (scan_params, cloud_params, the
+ *            same clock_offset_ns), B with this call: scans and scans_per_stream equal A's push output in every case,
+ *            capacity cases included (offsets, sizes, total, every written message's bytes); when both totals fit
+ *            their capacities, clouds equals A's scan_cloud_msgs output (offsets, sizes, total, every message's
+ *            bytes); every later call returns on B what it returns on A (this call sets the last push as a push does).
+ *            A call that fails its checks leaves the session as the push it stands for would.
+ *   Packing: scans, the bound-based packing of push_laserscan_msgs.  clouds, the exact packing of scan_cloud_msgs:
+ *            msg_offsets the exclusive scan of the sizes, each rounded up to 16, carried from chunk to chunk on the
+ *            device; slot i has a cloud message iff its LaserScan message was written (scans->msg_sizes[i] > 0), one
+ *            of width 0 when the filters removed every beam.
+ *   Capacity: per message in both sets.  A LaserScan message that does not fit is not written, so its cloud has no
+ *            source and no message (size 0, no room in the cloud offsets).  A cloud message is written iff its offset
+ *            + size <= clouds->capacity: the written clouds are a prefix.  The host form returns
+ *            RPL_RESULT_INSUFFICIENT_MEMORY when either total exceeds its capacity, the _dev form reports it through the
+ *            totals only; the push itself is done either way, and laserscan_msgs / scan_cloud_msgs on the same push
+ *            return every message.  Nothing at or past msgs + min(*total_bytes, capacity) is written, in either buffer.
+ *   Errors:  a null scans, clouds or cloud_params, a null member of either, and the checks of push_laserscan_msgs and
+ *            scan_cloud_msgs (an unknown channel bit, a NaN range_cutoff, flags before set_lidars / set_scan_filters,
+ *            chunk_bytes where it does not belong): RPL_RESULT_INVALID_DATA.
+ *   _dev:    as rpl_capsule_stream_push_laserscan_msgs_dev, both sets in device memory with its alignment (msgs 16-byte,
+ *            msg_offsets and total_bytes 8-byte, msg_sizes 4-byte).
+ *   host:    synchronous, host buffers.  Only the tables and the two sets' stretches cross the link.
+ *   Cost:    beyond push_laserscan_msgs' 24 bytes per slot, the first call of this kind keeps 4 bytes per slot (the
+ *            kept counts) and 16 bytes (the clouds' carry) of device tables and 48 bytes of pinned host memory; the
+ *            host form's lanes also stage one host chunk's clouds (their bound at max_nodes) and their tables. */
+typedef struct rpl_msgs_out { /* one packed message buffer and its tables; 40 bytes */
+  uint8_t* msgs;
+  uint64_t capacity;
+  uint64_t* msg_offsets; /* [n_streams * max_scans] */
+  uint32_t* msg_sizes;   /* [n_streams * max_scans] */
+  uint64_t* total_bytes; /* [1] */
+} rpl_msgs_out;
+rpl_result rpl_capsule_stream_push_scan_cloud_msgs(rpl_capsule_stream* s, const rpl_push_input* in,
+                                                   const rpl_scan_params* scan_params,
+                                                   const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
+                                                   const rpl_msgs_out* scans, const rpl_msgs_out* clouds,
+                                                   uint32_t* scans_per_stream);
+rpl_result rpl_capsule_stream_push_scan_cloud_msgs_dev(rpl_capsule_stream* s, const rpl_push_input* in,
+                                                       const rpl_scan_params* scan_params,
+                                                       const rpl_scan_cloud_params* cloud_params,
+                                                       int64_t clock_offset_ns, const rpl_msgs_out* scans,
+                                                       const rpl_msgs_out* clouds, uint32_t* scans_per_stream,
+                                                       void* stream);
+
 /* ---- LaserScan / PointCloud2 -> wire (SURVEY.md 8(f) rank 3) ---------------------------- */
 /* The serialised message the RMW layer would produce from the message the reference publishes
  * (scan_pub_->publish, reference src/rplidar_node.cpp:679): XCDR1 little endian, 4-byte

@@ -70,6 +70,7 @@ EXPORTS = [
     "rpl_scan_filter_batch_dev", "rpl_capsule_stream_set_scan_filters",
     "rpl_scan_filter_footprint_batch_dev", "rpl_capsule_stream_set_scan_footprints", "rpl_cloud_footprint_batch_dev",
     "rpl_scan_cloud_batch_dev", "rpl_capsule_stream_scan_cloud_msgs", "rpl_capsule_stream_scan_cloud_msgs_dev",
+    "rpl_capsule_stream_push_scan_cloud_msgs", "rpl_capsule_stream_push_scan_cloud_msgs_dev",
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -194,6 +195,12 @@ class PushInput(C.Structure):
     ints)."""
     _fields_ = [("data", C.c_void_p), ("counts", C.c_void_p), ("rx_us", C.c_void_p), ("timing", C.POINTER(Timing)),
                 ("sample_duration_us", C.c_uint32), ("chunk_bytes", C.c_uint32)]
+
+
+class MsgsOut(C.Structure):
+    """rpl_msgs_out: one packed message buffer and its tables (addresses as ints; 40 bytes)."""
+    _fields_ = [("msgs", C.c_void_p), ("capacity", C.c_uint64), ("msg_offsets", C.c_void_p),
+                ("msg_sizes", C.c_void_p), ("total_bytes", C.c_void_p)]
 
 
 class RplError(RuntimeError):
@@ -332,6 +339,12 @@ def lib() -> C.CDLL:
         "rpl_capsule_stream_push_cloud_msgs": ([vp, C.POINTER(PushInput), PCP, C.c_int64, vp, u64, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_push_cloud_msgs_dev":
             ([vp, C.POINTER(PushInput), PCP, C.c_int64, vp, u64, vp, vp, vp, vp, vp], u32),
+        "rpl_capsule_stream_push_scan_cloud_msgs":
+            ([vp, C.POINTER(PushInput), PSP, C.POINTER(ScanCloudParams), C.c_int64, C.POINTER(MsgsOut),
+              C.POINTER(MsgsOut), vp], u32),
+        "rpl_capsule_stream_push_scan_cloud_msgs_dev":
+            ([vp, C.POINTER(PushInput), PSP, C.POINTER(ScanCloudParams), C.c_int64, C.POINTER(MsgsOut),
+              C.POINTER(MsgsOut), vp, vp], u32),
     }
     for name, (args, res) in sig.items():
         fn = getattr(L, name)  # AttributeError here = the library does not export the ABI
@@ -1058,6 +1071,56 @@ class CapsuleStreamSession:
         self._ctx._check(self._fn("push_cloud_msgs_dev")(
             self._h, C.byref(pi), C.byref(params), int(clock_offset_ns), _p(msgs), int(capacity), _p(msg_offsets),
             _p(msg_sizes), _p(total_bytes), _p(scans_per_stream), _p(stream)))
+
+    def push_scan_cloud_msgs(self, data, counts, params: ScanParams, cloud_params: ScanCloudParams, clock_offset_ns=0,
+                             sample_duration_us=31, rx_us=None, timing: "Timing | None" = None, chunk_bytes=None,
+                             msgs=None, cloud_msgs=None):
+        """One push, as push_laserscan_msgs takes it, whose scans come back both as their serialised
+        sensor_msgs/LaserScan and as the PointCloud2 each projects to (laser_geometry's projectLaser with
+        cloud_params), from one run of the scan kernels.  msgs / cloud_msgs: the host buffers to pack into (their sizes
+        are the capacities; None: ones that always fit).  Returns (scans, clouds, scans_per_stream): scans and clouds
+        as the packed dicts of push_laserscan_msgs(packed=True), each with the call's result, which is
+        RESULT_INSUFFICIENT_MEMORY rather than an exception when either buffer is too small (the push is done)."""
+        assert isinstance(data, np.ndarray) and data.dtype == np.uint8 and data.flags.c_contiguous
+        cnt = np.ascontiguousarray(counts, dtype=np.uint32)
+        assert cnt.shape == (self.n_streams,)
+        rx = None if rx_us is None else np.ascontiguousarray(rx_us, dtype=np.uint64)
+        ns = self.n_streams * self.max_scans
+        if msgs is None:
+            msgs = np.zeros(ns * ((288 + 32 + 8 * self.max_nodes + 4 + 15) // 16 * 16), np.uint8)
+        if cloud_msgs is None:
+            per = 288 + 192 + scan_cloud_point_step(cloud_params.channels) * self.max_nodes + 1
+            cloud_msgs = np.zeros(ns * ((per + 15) // 16 * 16), np.uint8)
+        out = []
+        for buf in (msgs, cloud_msgs):
+            assert buf.dtype == np.uint8 and buf.flags.c_contiguous
+            t = dict(msgs=buf, msg_offsets=np.zeros(ns, np.uint64), msg_sizes=np.zeros(ns, np.uint32),
+                     total=np.zeros(1, np.uint64))
+            t["out"] = MsgsOut(_p(buf).value, buf.size, _p(t["msg_offsets"]).value, _p(t["msg_sizes"]).value,
+                               _p(t["total"]).value)
+            out.append(t)
+        sps = np.zeros(self.n_streams, np.uint32)
+        pi = self._push_input(data, cnt, sample_duration_us, rx, timing, chunk_bytes)
+        rc = self._fn("push_scan_cloud_msgs")(self._h, C.byref(pi), C.byref(params), C.byref(cloud_params),
+                                              int(clock_offset_ns), C.byref(out[0]["out"]), C.byref(out[1]["out"]),
+                                              _p(sps))
+        if rc != RESULT_INSUFFICIENT_MEMORY:
+            self._ctx._check(rc)
+        res = [dict(msgs=t["msgs"], msg_offsets=t["msg_offsets"], msg_sizes=t["msg_sizes"],
+                    total_bytes=int(t["total"][0]), result=rc) for t in out]
+        return res[0], res[1], sps
+
+    def push_scan_cloud_msgs_dev(self, data, counts, params: ScanParams, cloud_params: ScanCloudParams,
+                                 clock_offset_ns, scans: MsgsOut, clouds: MsgsOut, scans_per_stream,
+                                 sample_duration_us=31, rx_us=None, timing: "Timing | None" = None, chunk_bytes=None,
+                                 stream=None):
+        """Device addresses (data, counts, rx_us and scans_per_stream as for push_laserscan_msgs_dev; scans and clouds
+        MsgsOut of device buffers laid out as for laserscan_msgs_dev), asynchronous on `stream` (None: the context's
+        stream)."""
+        pi = self._push_input(data, counts, sample_duration_us, rx_us, timing, chunk_bytes)
+        self._ctx._check(self._fn("push_scan_cloud_msgs_dev")(
+            self._h, C.byref(pi), C.byref(params), C.byref(cloud_params), int(clock_offset_ns), C.byref(scans),
+            C.byref(clouds), _p(scans_per_stream), _p(stream)))
 
     def nodes(self, apply_ascend=True, per_stream=None, packed=False, nodes=None):
         """The node buffers RealLidarDriver::grab_scan_data would return for every scan the last push published: per

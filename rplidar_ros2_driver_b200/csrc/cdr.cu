@@ -237,9 +237,11 @@ __global__ void __launch_bounds__(CT) pointcloud2_msgs_kernel(MsgWriteArgs a, Cl
 // K = kPointCloud2: a published slot's exact size at its cloud's point count, once the cloud kernels have run, rounded
 // up to 16 for the offsets (msg_table_kernel's packing); sizes[i] is the size when the message fits capacity, else 0,
 // and the total is the end of the last message, carried in carry[1].
+// K = kScanCloud: as kPointCloud2, a slot's exact size at its projection's kept count, for a slot whose LaserScan
+// message the push wrote.
 template <MsgKind K>
 __global__ void __launch_bounds__(MT) push_msg_dir_kernel(PushMsgDirArgs a) {
-  constexpr bool kCloud = K == MsgKind::kPointCloud2;
+  constexpr bool kCloud = K != MsgKind::kLaserScan;
   __shared__ unsigned long long s_warp[MT / 32];
   __shared__ unsigned long long s_first, s_fit_end, s_last_end;
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -257,10 +259,14 @@ __global__ void __launch_bounds__(MT) push_msg_dir_kernel(PushMsgDirArgs a) {
     if (i < a.n_slots) {
       const uint32_t s = i / a.max_scans, k = i - s * a.max_scans;
       hb = a.hdr[s].bytes;
-      const bool off = kCloud && a.clouds && a.clouds[s].route == kCloudOff;  // a stream without a cloud
-      if (k < min(a.scans_per_stream[s], a.max_scans) && !off) {
-        if constexpr (kCloud) bound = msg_bytes(K, hb, a.counts[i]);
-        else bound = (msg_bytes(K, hb, a.views[i].y) + 15u) & ~15u;
+      if constexpr (K == MsgKind::kScanCloud) {
+        if (a.scan_sizes[i] > 0) bound = hb + a.tail_bytes + a.point_step * a.counts[i] + 1u;
+      } else {
+        const bool off = kCloud && a.clouds && a.clouds[s].route == kCloudOff;  // a stream without a cloud
+        if (k < min(a.scans_per_stream[s], a.max_scans) && !off) {
+          if constexpr (kCloud) bound = msg_bytes(K, hb, a.counts[i]);
+          else bound = (msg_bytes(K, hb, a.views[i].y) + 15u) & ~15u;
+        }
       }
     }
     const unsigned long long v = kCloud ? (bound + 15u) & ~15u : bound;
@@ -324,8 +330,10 @@ __global__ void __launch_bounds__(32) laserscan_placed_kernel(MsgWriteArgs a, co
 cudaError_t launch_push_msg_dir(const PushMsgDirArgs& a, MsgKind kind, cudaStream_t stream) {
   if (kind == MsgKind::kLaserScan)
     push_msg_dir_kernel<MsgKind::kLaserScan><<<1, MT, 0, stream>>>(a);
-  else
+  else if (kind == MsgKind::kPointCloud2)
     push_msg_dir_kernel<MsgKind::kPointCloud2><<<1, MT, 0, stream>>>(a);
+  else
+    push_msg_dir_kernel<MsgKind::kScanCloud><<<1, MT, 0, stream>>>(a);
   return cudaGetLastError();
 }
 

@@ -134,6 +134,10 @@ struct PushMsgDirArgs {
   const uint32_t* counts;           // [n_slots] PointCloud2: the clouds' point counts
   uint32_t* sizes;                  // [n_slots] out, PointCloud2: the message's bytes when it fits, else 0
   const CloudSettings* clouds;      // [n_slots / max_scans] nullable, PointCloud2: a kCloudOff stream's slots have none
+  // kScanCloud (sizes, total and carry [2] as PointCloud2): slot i has a message iff its LaserScan message was written
+  // (scan_sizes[i] > 0), of header + tail_bytes + point_step * counts[i] (the kept beams) + 1 (is_dense) bytes
+  const uint32_t* scan_sizes;
+  uint32_t tail_bytes, point_step;
 };
 cudaError_t launch_push_msg_dir(const PushMsgDirArgs& a, MsgKind kind, cudaStream_t stream);
 // The fixed part of every placed message of slots [0, a.n) once the scan kernels have written its arrays (a's hdr,

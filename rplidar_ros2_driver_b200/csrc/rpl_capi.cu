@@ -703,6 +703,10 @@ static_assert(sizeof(rpl_scan_cloud_params) == 8 && offsetof(rpl_scan_cloud_para
                   RPL_SCAN_CLOUD_DISTANCE == rpl::kScanCloudDistance &&
                   RPL_SCAN_CLOUD_TIMESTAMP == rpl::kScanCloudTimestamp,
               "rpl_scan_cloud_params and its channel bits are the header's");
+static_assert(sizeof(rpl_msgs_out) == 40 && offsetof(rpl_msgs_out, capacity) == 8 &&
+                  offsetof(rpl_msgs_out, msg_offsets) == 16 && offsetof(rpl_msgs_out, msg_sizes) == 24 &&
+                  offsetof(rpl_msgs_out, total_bytes) == 32,
+              "rpl_msgs_out is the header's");
 
 namespace {
 
@@ -1623,6 +1627,13 @@ struct rpl_capsule_stream {
   unsigned char* push_msg_work = nullptr;
   unsigned long long* push_msg_extent = nullptr;
   cudaEvent_t push_msg_extent_ready[kLanes] = {}, push_msg_dir_order = nullptr;
+  // pushes that also project their LaserScans (rpl_capsule_stream_push_scan_cloud_msgs*), made by the first: the
+  // clouds' directory carry and every slot's kept count (ScanCloudWork), the host form's pinned read-back of each
+  // lane's chunk's cloud extent ([kLanes][3]; push_msg_extent_ready tells it is there) and the order of the chunks'
+  // cloud directories
+  unsigned char* push_scan_cloud_work = nullptr;
+  unsigned long long* push_scan_cloud_extent = nullptr;
+  cudaEvent_t push_scan_cloud_dir_order = nullptr;
   // export / import (rpl_capsule_stream_export, _import): the device staging of the records and their tables
   unsigned char* migrate_work = nullptr;
   size_t migrate_work_bytes = 0;
@@ -2066,8 +2077,22 @@ rpl_result stream_cloud_chunk(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, const r
   return scratch_leave(c, l, st);
 }
 
-// A message push's chunk (rpl_capsule_stream_push_{laserscan,cloud}_msgs*): where its messages and tables go, every
-// table at the chunk's first slot (stream).
+// The projection of a LaserScan push's chunk (rpl_capsule_stream_push_scan_cloud_msgs*): its parameters (nullptr: none),
+// the kept counts, and the clouds' messages and directory as a PointCloud2 push's (carry [2]; extent, total,
+// extent_host and dir_order as ChunkMsgs'), every table at the chunk's first slot
+struct ChunkScanClouds {
+  const rpl_scan_cloud_params* params;
+  uint32_t* kept;
+  uint8_t* out;
+  unsigned long long capacity;
+  unsigned long long *carry, *offsets, *extent, *total;
+  uint32_t* sizes;
+  unsigned long long* extent_host;
+  cudaEvent_t dir_order;
+};
+
+// A message push's chunk (rpl_capsule_stream_push_{laserscan,cloud,scan_cloud}_msgs*): where its messages and tables
+// go, every table at the chunk's first slot (stream).
 struct ChunkMsgs {
   uint8_t* out;                      // LaserScan message i at out + place[i] - header - 32
   bool first, rebase;                // PushMsgDirArgs::first, rebase
@@ -2085,9 +2110,49 @@ struct ChunkMsgs {
   const rpl_cloud_params* cloud;
   float* xyzi;
   uint32_t* points;
+  ChunkScanClouds proj;  // a LaserScan push's projected clouds
 };
 
 rpl::CloudTail cloud_tail();
+
+// The projection of the LaserScan messages of the chunk of ns streams m describes, read where the push's scan kernels
+// wrote them (m.out at m.place, m.sizes), with the header, stamps and timing laserscan_placed_kernel gave them: the
+// count pass's arguments (the write pass adds the clouds' placement, scan_cloud_push_write)
+rpl::ScanCloudArgs scan_cloud_push_args(const WireChunk& w, uint32_t ns, bool stamped, const rpl_scan_params* params,
+                                        const ChunkMsgs& m, const uint32_t* beams, const float* inc) {
+  rpl::ScanCloudArgs a{};
+  scan_cloud_setup(a, *m.proj.params);
+  a.m.hdr = m.hdr;
+  if (stamped) {
+    a.m.begin_us = w.slot_begin;
+    a.m.end_us = w.slot_end;
+  }
+  a.m.clock_offset_ns = m.clock_offset_ns;
+  a.m.counts = beams;
+  a.m.angle_increment = inc;
+  a.m.stride = w.max_nodes;
+  a.m.max_scans = w.max_scans;
+  a.m.mode_a = params->scan_processing ? 1u : 0u;
+  a.m.lidars = w.lidars;
+  a.m.n = ns * w.max_scans;
+  a.kept = m.proj.kept;
+  a.scan_msgs = m.out;
+  a.place = m.place;
+  a.scan_sizes = m.sizes;
+  return a;
+}
+
+// the write pass of those clouds, once their directory has placed them: message i at m.proj.out + offsets[i] - out_base
+rpl_result scan_cloud_push_write(rpl_ctx* c, rpl::ScanCloudArgs a, const ChunkScanClouds& p, unsigned long long out_base,
+                                 cudaStream_t st) {
+  a.m.offsets = p.offsets;
+  a.m.sizes = p.sizes;
+  a.m.out = p.out;
+  a.m.out_base = out_base;
+  RPL_CUDA(c, rpl::launch_scan_cloud(a, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+  c->launches++;
+  return RPL_RESULT_OK;
+}
 
 // A PointCloud2 push's messages of the chunk of ns streams m describes, once its directory has sized and placed them:
 // pointcloud2_msgs_kernel writes message i at m.out + m.offsets[i] - out_base, stamped with the slot stamps of the
@@ -2123,7 +2188,9 @@ rpl_result cloud_push_write(rpl_ctx* c, const WireChunk& w, uint32_t ns, bool st
 // m (a message push): the directory runs between the assembler and the scan kernels, which write into the placed
 // messages instead of ranges / intens (null), and the header writer behind them.  A PointCloud2 push (m->cloud) runs
 // the cloud chain over the chunk's fresh views instead of the scan kernels, then the directory, which sizes each
-// message by its cloud, then (the device form; the host form's waits for the extent, push_host) the writer.
+// message by its cloud, then (the device form; the host form's waits for the extent, push_host) the writer.  A LaserScan
+// push with m->proj.params then projects the messages its header writer has finished: the count pass, the clouds'
+// directory, and the write pass in the same way.
 rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const WireChunk& w, uint32_t ns,
                                 const uint8_t* capsules, const uint32_t* counts, uint32_t sample_duration_us,
                                 const rpl_scan_params* params, float* ranges, float* intens, uint32_t* beams,
@@ -2181,14 +2248,20 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
   d.counts = m->points;
   d.sizes = m->cloud ? m->sizes : nullptr;
   if (m->cloud && (m->cloud->flags & RPL_CLOUD_PER_STREAM_CHAIN) != 0) d.clouds = w.clouds.at;
-  if (m->dir_order) RPL_CUDA(c, cudaStreamWaitEvent(st, m->dir_order, 0), RPL_RESULT_OPERATION_FAIL);
-  RPL_CUDA(c, rpl::launch_push_msg_dir(d, kind, st), RPL_RESULT_OPERATION_FAIL);
-  c->launches++;
-  if (m->dir_order) RPL_CUDA(c, cudaEventRecord(m->dir_order, st), RPL_RESULT_OPERATION_FAIL);
-  if (m->extent_host) {
-    RPL_CUDA(c, cudaMemcpyAsync(m->extent_host, m->extent, 3 * 8, cudaMemcpyDeviceToHost, st), RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaEventRecord(m->extent_ready, st), RPL_RESULT_OPERATION_FAIL);
-  }
+  // a directory behind the previous chunk's of its kind (a host push's order across the lanes), and its extent read back
+  auto directory = [&](const rpl::PushMsgDirArgs& a, rpl::MsgKind k, cudaEvent_t order,
+                       unsigned long long* extent_host) -> rpl_result {
+    if (order) RPL_CUDA(c, cudaStreamWaitEvent(st, order, 0), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, rpl::launch_push_msg_dir(a, k, st), RPL_RESULT_OPERATION_FAIL);
+    c->launches++;
+    if (order) RPL_CUDA(c, cudaEventRecord(order, st), RPL_RESULT_OPERATION_FAIL);
+    if (extent_host) {
+      RPL_CUDA(c, cudaMemcpyAsync(extent_host, a.extent, 3 * 8, cudaMemcpyDeviceToHost, st), RPL_RESULT_OPERATION_FAIL);
+      RPL_CUDA(c, cudaEventRecord(m->extent_ready, st), RPL_RESULT_OPERATION_FAIL);
+    }
+    return RPL_RESULT_OK;
+  };
+  if (const rpl_result e = directory(d, kind, m->dir_order, m->extent_host); e != RPL_RESULT_OK) return e;
   if (m->cloud) return m->extent_host ? RPL_RESULT_OK : cloud_push_write(c, w, ns, sp != nullptr, *m, 0, st);
   r = enqueue_scan(c, l, w.nodes, w.scan_len, ns * w.max_scans, w.max_nodes, params, nullptr, nullptr, nullptr, beams,
                    inc, nullptr, nullptr, st, views, (unsigned long long)ns * w.stride_nodes, lt, m->out, m->place);
@@ -2212,7 +2285,26 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
   a.lidars = w.lidars;
   RPL_CUDA(c, rpl::launch_laserscan_placed(a, m->place, m->sizes, st), RPL_RESULT_OPERATION_FAIL);
   c->launches++;
-  return RPL_RESULT_OK;
+  if (!m->proj.params) return RPL_RESULT_OK;
+  // the projection of the messages just finished: the kept counts, the clouds' directory, which sizes each message
+  // exactly, then (the device form; the host form's waits for both extents, push_host) the write pass
+  const rpl::ScanCloudArgs sa = scan_cloud_push_args(w, ns, sp != nullptr, params, *m, beams, inc);
+  RPL_CUDA(c, rpl::launch_scan_cloud_count(sa, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+  c->launches++;
+  d.capacity = m->proj.capacity;
+  d.carry = m->proj.carry;
+  d.offsets = m->proj.offsets;
+  d.place = nullptr;
+  d.extent = m->proj.extent;
+  d.total = m->proj.total;
+  d.counts = m->proj.kept;
+  d.sizes = m->proj.sizes;
+  d.scan_sizes = m->sizes;
+  d.tail_bytes = sa.tail.bytes;
+  d.point_step = sa.point_step;
+  r = directory(d, rpl::MsgKind::kScanCloud, m->proj.dir_order, m->proj.extent_host);
+  if (r != RPL_RESULT_OK || m->extent_host) return r;
+  return scan_cloud_push_write(c, sa, m->proj, 0, st);
 }
 
 struct HostMsgs;
@@ -2246,6 +2338,15 @@ struct HostMsgs {
   const cudaEvent_t* extent_ready;
   cudaEvent_t dir_order;
   const rpl_cloud_params* cloud;    // a PointCloud2 push
+  // a LaserScan push that also projects its scans: the projection's parameters, the clouds' outputs, the staging for
+  // one chunk's clouds (their bound at max_nodes), the session's cloud carry and kept counts, each lane's cloud extent
+  // (pinned [kLanes][3], ready with extent_ready) and the order of the cloud directories
+  const rpl_scan_cloud_params* proj;
+  const rpl_msgs_out* clouds;
+  size_t proj_chunk_bytes;
+  unsigned long long *proj_carry, *proj_extent_host;
+  uint32_t* kept;
+  cudaEvent_t proj_dir_order;
 };
 
 // Runs a host call's n_streams streams through capsule_stream_chunk, `chunk` streams at a time round-robin over the
@@ -2254,9 +2355,11 @@ struct HostMsgs {
 // meanwhile), the stretch of the packed buffer the chunk fills is copied to msgs, with the chunk's tables.  A
 // PointCloud2 push's directory follows the chunk's cloud kernels, so the host reads a chunk's extent only once the next
 // chunk is queued on the other lane (finish_cloud), then queues the writer, which packs the chunk's messages from the
-// stretch's first offset on, and the copies.  A lane's
-// staging block holds one chunk's input and outputs, then whatever chunk_at(k, s0) carves off k for the device state
-// of the chunk from stream s0, which it returns (the chain's lives there; a session's in its arenas).
+// stretch's first offset on, and the copies.  A projecting push (hm->proj) does the same for its clouds, whose
+// directory follows the chunk's scan kernels: both extents are read once the next chunk is queued, then the clouds'
+// write pass and both stretches and tables are queued.  A lane's staging block holds one chunk's input and outputs,
+// then whatever chunk_at(k, s0) carves off k for the device state of the chunk from stream s0, which it returns (the
+// chain's lives there; a session's in its arenas).
 template <class ChunkAt>
 rpl_result push_host(rpl_ctx* c, const HostWire& h, uint32_t n_streams, uint32_t chunk, ChunkAt chunk_at) {
   const size_t NS = (size_t)chunk * h.max_scans, row = (size_t)h.max_scans * h.max_nodes;
@@ -2276,20 +2379,26 @@ rpl_result push_host(rpl_ctx* c, const HostWire& h, uint32_t n_streams, uint32_t
     u64* extent;
     float* xyzi;  // a PointCloud2 push's: the chunk's clouds and point counts
     uint32_t* points;
+    uint8_t* pmsgs;  // a projecting push's: the chunk's projected clouds, their offsets, sizes and extent
+    u64* poffs;
+    uint32_t* psizes;
+    u64* pextent;
     WireChunk w;
   };
-  const bool cloud = hm && hm->cloud;
+  const bool cloud = hm && hm->cloud, proj = hm && hm->proj;
   auto layout = [&](Carve& k, uint32_t s0) {
     return Regions{k.take<uint8_t>(chunk * h.in_stream), k.take<uint32_t>(chunk),
                    k.take<u64>(h.sp ? chunk * h.rx_stream : 0), k.take<float>(rows), k.take<float>(rows),
                    k.take<float>(NS), k.take<uint32_t>(NS), k.take<uint32_t>(chunk), k.take<u64>(h.sp ? NS : 0),
                    k.take<uint8_t>(hm ? hm->chunk_bytes : 0), k.take<u64>(hm ? NS : 0), k.take<uint32_t>(hm ? NS : 0),
                    k.take<u64>(hm ? 3 : 0), k.take<float>(cloud ? NS * h.max_nodes * 4 : 0),
-                   k.take<uint32_t>(cloud ? NS : 0), chunk_at(k, s0)};
+                   k.take<uint32_t>(cloud ? NS : 0), k.take<uint8_t>(proj ? hm->proj_chunk_bytes : 0),
+                   k.take<u64>(proj ? NS : 0), k.take<uint32_t>(proj ? NS : 0), k.take<u64>(proj ? 3 : 0),
+                   chunk_at(k, s0)};
   };
   if (const rpl_result r = grow_stage(c, kLanes, [&](Carve& k) { layout(k, 0); }); r != RPL_RESULT_OK) return r;
   const cudaMemcpyKind h2d = cudaMemcpyHostToDevice, d2h = cudaMemcpyDeviceToHost;
-  // a PointCloud2 push's chunk whose kernels are queued and whose writer and copies are not
+  // a PointCloud2 or projecting push's chunk whose kernels are queued and whose writer and copies are not
   struct Queued {
     Lane* l = nullptr;
     uint32_t s0, ns;
@@ -2302,17 +2411,28 @@ rpl_result push_host(rpl_ctx* c, const HostWire& h, uint32_t n_streams, uint32_t
     queued.l = nullptr;
     const int li = (int)(q.l - c->lane);
     const size_t so = (size_t)q.s0 * h.max_scans, nsc = (size_t)q.ns * h.max_scans;
+    const bool last = q.s0 + q.ns == n_streams;
+    cudaStream_t st = q.l->stream;
     RPL_CUDA(c, cudaEventSynchronize(hm->extent_ready[li]), RPL_RESULT_OPERATION_FAIL);
     const u64 lo = q.m.extent_host[0], hi = q.m.extent_host[1];
-    if (q.s0 + q.ns == n_streams) *hm->total = q.m.extent_host[2];
-    if (const rpl_result r = cloud_push_write(c, q.d.w, q.ns, h.sp != nullptr, q.m, lo, q.l->stream);
-        r != RPL_RESULT_OK)
-      return r;
-    if (hi > lo)
-      RPL_CUDA(c, cudaMemcpyAsync(hm->msgs + lo, q.d.msgs, hi - lo, d2h, q.l->stream), RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(hm->offsets + so, q.d.offs, nsc * 8, d2h, q.l->stream), RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(hm->sizes + so, q.d.sizes, nsc * 4, d2h, q.l->stream), RPL_RESULT_OPERATION_FAIL);
-    RPL_CUDA(c, cudaMemcpyAsync(h.scans_per_stream + q.s0, q.d.sps, (size_t)q.ns * 4, d2h, q.l->stream),
+    if (last) *hm->total = q.m.extent_host[2];
+    if (cloud)
+      if (const rpl_result r = cloud_push_write(c, q.d.w, q.ns, h.sp != nullptr, q.m, lo, st); r != RPL_RESULT_OK)
+        return r;
+    if (proj) {  // the clouds' stretch [first offset, end of the last that fits), written from its first offset on
+      const u64 plo = q.m.proj.extent_host[0], phi = q.m.proj.extent_host[1];
+      if (last) *hm->clouds->total_bytes = q.m.proj.extent_host[2];
+      const rpl::ScanCloudArgs a = scan_cloud_push_args(q.d.w, q.ns, h.sp != nullptr, h.params, q.m, q.d.beams, q.d.inc);
+      if (const rpl_result r = scan_cloud_push_write(c, a, q.m.proj, plo, st); r != RPL_RESULT_OK) return r;
+      if (phi > plo)
+        RPL_CUDA(c, cudaMemcpyAsync(hm->clouds->msgs + plo, q.d.pmsgs, phi - plo, d2h, st), RPL_RESULT_OPERATION_FAIL);
+      RPL_CUDA(c, cudaMemcpyAsync(hm->clouds->msg_offsets + so, q.d.poffs, nsc * 8, d2h, st), RPL_RESULT_OPERATION_FAIL);
+      RPL_CUDA(c, cudaMemcpyAsync(hm->clouds->msg_sizes + so, q.d.psizes, nsc * 4, d2h, st), RPL_RESULT_OPERATION_FAIL);
+    }
+    if (hi > lo) RPL_CUDA(c, cudaMemcpyAsync(hm->msgs + lo, q.d.msgs, hi - lo, d2h, st), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(hm->offsets + so, q.d.offs, nsc * 8, d2h, st), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(hm->sizes + so, q.d.sizes, nsc * 4, d2h, st), RPL_RESULT_OPERATION_FAIL);
+    RPL_CUDA(c, cudaMemcpyAsync(h.scans_per_stream + q.s0, q.d.sps, (size_t)q.ns * 4, d2h, st),
              RPL_RESULT_OPERATION_FAIL);
     return RPL_RESULT_OK;
   };
@@ -2352,12 +2472,15 @@ rpl_result push_host(rpl_ctx* c, const HostWire& h, uint32_t n_streams, uint32_t
       m.cloud = hm->cloud;
       m.xyzi = d.xyzi;
       m.points = d.points;
+      if (proj)
+        m.proj = ChunkScanClouds{hm->proj, hm->kept + so, d.pmsgs, hm->clouds->capacity, hm->proj_carry, d.poffs,
+                                 d.pextent, nullptr, d.psizes, hm->proj_extent_host + 3 * li, hm->proj_dir_order};
     }
     const rpl_result r = capsule_stream_chunk(c, l, l.stream, d.w, ns, d.in, d.counts, h.sample_duration_us, h.params,
                                               d.ranges, d.intens, d.beams, d.inc, d.sps, h.sp ? &sp : nullptr,
                                               hm ? &m : nullptr);
     if (r != RPL_RESULT_OK) return r;
-    if (cloud) {  // this chunk runs while the host waits for the previous one's extent
+    if (cloud || proj) {  // this chunk runs while the host waits for the previous one's extent
       const rpl_result f = finish_cloud();
       queued = Queued{&l, s0, ns, d, m};
       return f;
@@ -2389,7 +2512,7 @@ rpl_result push_host(rpl_ctx* c, const HostWire& h, uint32_t n_streams, uint32_t
     return RPL_RESULT_OK;
   };
   rpl_result r = run_chunks(c, n_streams, chunk, run_chunk);
-  if (r == RPL_RESULT_OK && queued.l) {  // the last chunk of a PointCloud2 push
+  if (r == RPL_RESULT_OK && queued.l) {  // the last chunk of a PointCloud2 or projecting push
     r = finish_cloud();
     const std::string why = c->err;
     const rpl_result s = rpl_ctx_synchronize(c);
@@ -2717,6 +2840,16 @@ PushMsgWork push_msg_work_layout(const rpl_capsule_stream* cs, Carve& k) {
                      k.take<float>(NS), k.take<unsigned long long>(NS)};
 }
 
+// The session's device tables of a projecting push: the clouds' directory carry (the running offset and the end of
+// the last message) and every slot's kept count
+struct ScanCloudWork {
+  unsigned long long* carry;
+  uint32_t* kept;
+};
+ScanCloudWork scan_cloud_work_layout(const rpl_capsule_stream* cs, Carve& k) {
+  return ScanCloudWork{k.take<unsigned long long>(2), k.take<uint32_t>((size_t)cs->n_streams * cs->max_scans)};
+}
+
 // a message push's outputs (host or device arrays of every slot, as the push's)
 struct PushMsgs {
   uint8_t* msgs;
@@ -2730,6 +2863,12 @@ struct PushMsgs {
   const rpl_cloud_params* cloud;
   float* xyzi;
   uint32_t* points;
+  // a LaserScan push that also projects its scans: the projection's parameters, the clouds' outputs, and the session's
+  // tables of the projection (ScanCloudWork)
+  const rpl_scan_cloud_params* proj;
+  const rpl_msgs_out* clouds;
+  unsigned long long* proj_carry;
+  uint32_t* kept;
 };
 
 // A push of the kind the entry point takes (bytes: a byte push); sp: a stamped one.  Host arrays (dev false, stream
@@ -2781,6 +2920,11 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
         m.cloud = pm->cloud;
         m.xyzi = pm->xyzi;
         m.points = pm->points;
+        if (pm->proj)
+          m.proj = ChunkScanClouds{pm->proj, pm->kept + so, pm->clouds->msgs, pm->clouds->capacity, pm->proj_carry,
+                                   reinterpret_cast<unsigned long long*>(pm->clouds->msg_offsets) + so, nullptr,
+                                   reinterpret_cast<unsigned long long*>(pm->clouds->total_bytes),
+                                   pm->clouds->msg_sizes + so, nullptr, nullptr};
       }
       r = capsule_stream_chunk(c, c->lane[0], st, session_chunk(cs, s0, params, true, pm ? pm->cloud : nullptr),
                                std::min(chunk, cs->n_streams - s0), in + s0 * cs->in_stream, counts + s0,
@@ -2807,6 +2951,17 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
       hm = HostMsgs{pm->msgs, pm->capacity, pm->offsets, pm->sizes, pm->total, (size_t)chunk * cs->max_scans * bound,
                     pm->clock_offset_ns, cs->msg_hdr, pm->w.carry, pm->w.place, cs->push_msg_extent,
                     cs->push_msg_extent_ready, cs->push_msg_dir_order, pm->cloud};
+      if (pm->proj) {  // a projected cloud's bound: its message at max_nodes kept beams, rounded up to 16
+        const size_t pmost = (size_t)hdr_most + scan_cloud_tail(pm->proj->channels).bytes +
+                             (size_t)scan_cloud_point_step(pm->proj->channels) * n + 1;
+        hm.proj = pm->proj;
+        hm.clouds = pm->clouds;
+        hm.proj_chunk_bytes = (size_t)chunk * cs->max_scans * ((pmost + 15) & ~(size_t)15);
+        hm.proj_carry = pm->proj_carry;
+        hm.proj_extent_host = cs->push_scan_cloud_extent;
+        hm.kept = pm->kept;
+        hm.proj_dir_order = cs->push_scan_cloud_dir_order;
+      }
     }
     const HostWire h{in, counts, cs->in_stream, sample_duration_us, cs->max_nodes, cs->max_scans, params, ranges,
                      intensities, angle_increment, beam_counts, scans_per_stream, sp, sp ? sp->stride_chunks : 0u,
@@ -3512,15 +3667,30 @@ rpl_result stream_msgs(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* pa
 // then the directory, which packs the messages exactly as msg_table_kernel does, then pointcloud2_msgs_kernel.  The
 // push decodes and stamps with RPL_FLAG_PER_STREAM when the cloud takes RPL_CLOUD_PER_STREAM: of rpl_scan_params only
 // that flag reaches the decoders, the assembler and the stamps.
+// proj (kind kLaserScan, rpl_capsule_stream_push_scan_cloud_msgs*): each chunk also projects its LaserScan messages
+// where they lie, into clouds (DESIGN.md 5.7.1 "LaserScans and their projected clouds from the push").
 rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, rpl::MsgKind kind, const void* params,
                      int64_t clock_offset_ns, uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
-                     uint64_t* total_bytes, uint32_t* scans_per_stream, bool dev, void* stream) {
+                     uint64_t* total_bytes, uint32_t* scans_per_stream, bool dev, void* stream,
+                     const rpl_scan_cloud_params* proj = nullptr, const rpl_msgs_out* clouds = nullptr) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
   rpl_ctx* c = cs->c;
   cs->cloud_chunk = 0;  // as a push that fails its checks
   if (!in || !params || !msgs || !msg_offsets || !msg_sizes || !total_bytes || !scans_per_stream) {
     c->err = "null input, params, msgs, msg_offsets, msg_sizes, total_bytes or scans_per_stream";
     return RPL_RESULT_INVALID_DATA;
+  }
+  if (proj) {
+    if (!clouds->msgs || !clouds->msg_offsets || !clouds->msg_sizes || !clouds->total_bytes) {
+      c->err = "null clouds->msgs, msg_offsets, msg_sizes or total_bytes";
+      return RPL_RESULT_INVALID_DATA;
+    }
+    if (!scan_cloud_ok(c, *proj)) return RPL_RESULT_INVALID_DATA;
+    if (dev && ((reinterpret_cast<uintptr_t>(clouds->msgs) & 15u) || misaligned8(clouds->msg_offsets) ||
+                misaligned8(clouds->total_bytes) || (reinterpret_cast<uintptr_t>(clouds->msg_sizes) & 3u))) {
+      c->err = "clouds: msgs must be 16-byte aligned, msg_offsets and total_bytes 8-byte, msg_sizes 4-byte aligned";
+      return RPL_RESULT_INVALID_DATA;
+    }
   }
   if (in->chunk_bytes != 0 && (!cs->bytes || !in->rx_us)) {
     c->err = cs->bytes ? "chunk_bytes is a stamped push's (rx_us set)"
@@ -3553,9 +3723,28 @@ rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, rpl::MsgK
       RPL_CUDA(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming), RPL_RESULT_OPERATION_FAIL);
     RPL_CUDA(c, cudaEventCreateWithFlags(&cs->push_msg_dir_order, cudaEventDisableTiming), RPL_RESULT_OPERATION_FAIL);
   }
+  if (proj && !cs->push_scan_cloud_work) {  // the first projecting push: its tables, made once
+    RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+    Carve k;
+    scan_cloud_work_layout(cs, k);
+    RPL_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&cs->push_scan_cloud_work), k.bytes),
+             RPL_RESULT_INSUFFICIENT_MEMORY);
+    RPL_CUDA(c, cudaMallocHost(reinterpret_cast<void**>(&cs->push_scan_cloud_extent), kLanes * 3 * 8),
+             RPL_RESULT_INSUFFICIENT_MEMORY);
+    RPL_CUDA(c, cudaEventCreateWithFlags(&cs->push_scan_cloud_dir_order, cudaEventDisableTiming),
+             RPL_RESULT_OPERATION_FAIL);
+  }
   Carve k{cs->push_msg_work};
   PushMsgs pm{msgs, capacity, msg_offsets, msg_sizes, total_bytes, clock_offset_ns, push_msg_work_layout(cs, k), cp,
               nullptr, nullptr};
+  if (proj) {
+    Carve kp{cs->push_scan_cloud_work};
+    const ScanCloudWork sw = scan_cloud_work_layout(cs, kp);
+    pm.proj = proj;
+    pm.clouds = clouds;
+    pm.proj_carry = sw.carry;
+    pm.kept = sw.kept;
+  }
   if (cloud && dev) {  // one chunk's clouds, in the session's message work block (cloud_msgs' when that is larger)
     const size_t NS = (size_t)cs->chunk_dev * cs->max_scans;
     auto layout = [&](Carve& kw) {
@@ -3579,11 +3768,26 @@ rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, rpl::MsgK
   const rpl_result r = stream_push(cs, in->data, in->counts, sample_duration_us, sp_params, nullptr, nullptr, nullptr,
                                    nullptr, scans_per_stream, stamped ? &sp : nullptr, cs->bytes, dev, stream, &pm);
   if (r != RPL_RESULT_OK) return r;
-  if (!dev && *total_bytes > capacity) {
+  if (!dev && (*total_bytes > capacity || (proj && *clouds->total_bytes > clouds->capacity))) {
     c->err = "the messages need more than capacity bytes (total_bytes tells how many; the push itself is done)";
     return RPL_RESULT_INSUFFICIENT_MEMORY;
   }
   return RPL_RESULT_OK;
+}
+
+rpl_result push_scan_cloud_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, const rpl_scan_params* scan_params,
+                                const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
+                                const rpl_msgs_out* scans, const rpl_msgs_out* clouds, uint32_t* scans_per_stream,
+                                bool dev, void* stream) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  if (!scans || !clouds || !cloud_params) {
+    cs->cloud_chunk = 0;  // as a push that fails its checks
+    cs->c->err = "null scans, clouds or cloud_params";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  return push_msgs(cs, in, rpl::MsgKind::kLaserScan, scan_params, clock_offset_ns, scans->msgs, scans->capacity,
+                   scans->msg_offsets, scans->msg_sizes, scans->total_bytes, scans_per_stream, dev, stream,
+                   cloud_params, clouds);
 }
 
 // ---- grabbed node buffers of the last push (DESIGN.md 5.7.1 "Session nodes") -------------------------------------
@@ -3838,6 +4042,9 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   for (cudaEvent_t e : cs->push_msg_extent_ready)
     if (e) cudaEventDestroy(e);
   if (cs->push_msg_dir_order) cudaEventDestroy(cs->push_msg_dir_order);
+  cudaFree(cs->push_scan_cloud_work);
+  cudaFreeHost(cs->push_scan_cloud_extent);
+  if (cs->push_scan_cloud_dir_order) cudaEventDestroy(cs->push_scan_cloud_dir_order);
   if (cs->done) cudaEventDestroy(cs->done);
   delete cs;
 }
@@ -4379,6 +4586,25 @@ rpl_result rpl_capsule_stream_push_cloud_msgs_dev(rpl_capsule_stream* s, const r
                                                   uint32_t* scans_per_stream, void* stream) {
   return push_msgs(s, in, rpl::MsgKind::kPointCloud2, params, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
                    total_bytes, scans_per_stream, true, stream);
+}
+
+rpl_result rpl_capsule_stream_push_scan_cloud_msgs(rpl_capsule_stream* s, const rpl_push_input* in,
+                                                   const rpl_scan_params* scan_params,
+                                                   const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
+                                                   const rpl_msgs_out* scans, const rpl_msgs_out* clouds,
+                                                   uint32_t* scans_per_stream) {
+  return push_scan_cloud_msgs(s, in, scan_params, cloud_params, clock_offset_ns, scans, clouds, scans_per_stream, false,
+                              nullptr);
+}
+
+rpl_result rpl_capsule_stream_push_scan_cloud_msgs_dev(rpl_capsule_stream* s, const rpl_push_input* in,
+                                                       const rpl_scan_params* scan_params,
+                                                       const rpl_scan_cloud_params* cloud_params,
+                                                       int64_t clock_offset_ns, const rpl_msgs_out* scans,
+                                                       const rpl_msgs_out* clouds, uint32_t* scans_per_stream,
+                                                       void* stream) {
+  return push_scan_cloud_msgs(s, in, scan_params, cloud_params, clock_offset_ns, scans, clouds, scans_per_stream, true,
+                              stream);
 }
 
 rpl_result rpl_capsule_stream_cloud_msgs_dev(rpl_capsule_stream* s, const rpl_cloud_params* params,

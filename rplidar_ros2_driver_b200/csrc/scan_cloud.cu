@@ -8,7 +8,8 @@
 // (cdr.cu) places a session's messages exactly; the write pass decides every beam again, compacts the kept ones chunk by
 // chunk (a warp ballot for the lane's place, the warps' counts in shared memory for the block's) and writes each record
 // straight into its row or into its message's data, and a message's fixed part from the stream's header and the call's
-// tail.  Both passes read the ranges only once per beam; no state is kept.
+// tail.  Both passes read the ranges only once per beam; no state is kept.  A slot's beams are its row, or, in a push
+// that returns both messages (push_scan_cloud_msgs), its LaserScan message where the push's scan kernels placed it.
 #include <algorithm>
 
 #include "beam_point.cuh"
@@ -31,11 +32,27 @@ __device__ __forceinline__ void slot_window(const ScanCloudArgs& a, uint32_t i, 
   *cut = a.range_cutoff >= 0.0f ? a.range_cutoff : hi;
 }
 
+// slot i's beams: its row, or its placed LaserScan message (a push's, 4-byte aligned: the loads stay 4-byte)
+struct SlotBeams {
+  uint32_t M;
+  const float *rg, *ig;
+};
+__device__ __forceinline__ SlotBeams slot_beams(const ScanCloudArgs& a, uint32_t i) {
+  if (!a.scan_msgs)
+    return SlotBeams{min(a.m.counts[i], a.m.stride), a.m.ranges + (size_t)i * a.m.stride,
+                     a.m.intensities + (size_t)i * a.m.stride};
+  if (a.scan_sizes[i] == 0) return SlotBeams{0u, nullptr, nullptr};
+  const uint32_t M = a.m.counts[i];
+  const float* rg = reinterpret_cast<const float*>(a.scan_msgs + a.place[i]);
+  return SlotBeams{M, rg, rg + M + 1};  // the intensities follow the ranges and their count
+}
+
 __global__ void __launch_bounds__(ST) scan_cloud_count_kernel(const __grid_constant__ ScanCloudArgs a) {
   for (uint32_t s = blockIdx.x; s < a.m.n; s += gridDim.x) {
     const uint32_t i = a.m.slot0 + s;
-    const uint32_t M = min(a.m.counts[i], a.m.stride);
-    const float* rg = a.m.ranges + (size_t)i * a.m.stride;
+    const SlotBeams sb = slot_beams(a, i);
+    const uint32_t M = sb.M;
+    const float* rg = sb.rg;
     float lo, cut;
     slot_window(a, i, &lo, &cut);
     uint32_t n = 0;
@@ -47,13 +64,16 @@ __global__ void __launch_bounds__(ST) scan_cloud_count_kernel(const __grid_const
   }
 }
 
-__global__ void __launch_bounds__(ST) scan_cloud_kernel(const __grid_constant__ ScanCloudArgs a) {
+// 8 CTAs per SM: left to itself the compiler takes 40 registers for the two sources and the persistent grid loses a
+// quarter of its CTAs, which costs the row path 8-10 %; at 32 nothing spills
+__global__ void __launch_bounds__(ST, 8) scan_cloud_kernel(const __grid_constant__ ScanCloudArgs a) {
   __shared__ uint32_t s_warp[ST / 32];
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t words = a.point_step / 4, ch = a.channels;
   for (uint32_t s = blockIdx.x; s < a.m.n; s += gridDim.x) {
     const uint32_t i = a.m.slot0 + s;
-    const uint32_t M = min(a.m.counts[i], a.m.stride);
+    const SlotBeams sb = slot_beams(a, i);
+    const uint32_t M = sb.M;
     float ti;
     uint32_t* data;
     if (a.m.out) {
@@ -83,8 +103,7 @@ __global__ void __launch_bounds__(ST) scan_cloud_kernel(const __grid_constant__ 
       ti = a.time_increment ? a.time_increment[i] : 0.0f;
       data = reinterpret_cast<uint32_t*>(a.points) + (size_t)s * a.m.stride * words;
     }
-    const float* rg = a.m.ranges + (size_t)i * a.m.stride;
-    const float* ig = a.m.intensities + (size_t)i * a.m.stride;
+    const float *rg = sb.rg, *ig = sb.ig;
     const float inc = M ? a.m.angle_increment[i] : 0.0f;
     float lo, cut;
     slot_window(a, i, &lo, &cut);

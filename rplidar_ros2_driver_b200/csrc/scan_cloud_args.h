@@ -33,6 +33,12 @@ struct ScanCloudArgs {
   uint32_t* kept;                    // [n_slots] the kept counts: the count pass writes them (rows: the write pass)
   float* points;                     // rows: scan s's records at points + s * m.stride * point_step / 4
   ScanCloudTail tail;                // messages
+  // A push's LaserScans, read where its scan kernels wrote them (scan_msgs non-null; m.ranges, m.intensities unused):
+  // slot i's ranges at scan_msgs + place[i], its intensities m.counts[i] + 1 floats later; a slot whose scan_sizes[i]
+  // is 0 has no LaserScan message and no beams
+  const uint8_t* scan_msgs;
+  const unsigned long long* place;
+  const uint32_t* scan_sizes;
 };
 
 // the count pass: kept[i] of every slot [m.slot0, m.slot0 + m.n) (0 for a slot without beams)

@@ -1125,7 +1125,7 @@ rpl_result rpl_cloud_footprint_batch_dev(rpl_ctx* ctx, const rpl_node_hq* nodes,
  *   fields:  x, y, z (FLOAT32), then per channel bit, in this order: intensity (FLOAT32, intensities[i]), index (INT32,
  *            i), distances (FLOAT32, r_i), stamps (FLOAT32, fl((float)i * time_increment)); offsets 0, 4, 8, ...;
  *            point_step = 12 + 4 * popcount(channels).  Any other bit (laser_geometry's viewpoint 0x10 included):
- *            RPL_RESULT_INVALID_DATA.
+ *            RPL_RESULT_INVALID_DATA, except where "Clouds in a target frame" below accepts it.
  *   message: the LaserScan's stamp and frame_id, height 1, width the kept count, is_bigendian 0, row_step point_step *
  *            width, is_dense 1.
  * Offsets: channels 0, range_cutoff 4; 8 bytes. */
@@ -1219,6 +1219,57 @@ rpl_result rpl_capsule_stream_push_scan_cloud_msgs_dev(rpl_capsule_stream* s, co
                                                        int64_t clock_offset_ns, const rpl_msgs_out* scans,
                                                        const rpl_msgs_out* clouds, uint32_t* scans_per_stream,
                                                        void* stream);
+
+/* Clouds in a target frame (DESIGN.md 5.7.1 "Projected clouds in a target frame"; INTEGRATION.md 4i): laser_geometry's
+ * transformLaserScanToPointCloud with a static transform, i.e. P(params, scan) with the points moved into the robot's
+ * frame on the device, defined bit for bit by tests/scan_cloud_transform_oracle.py.
+ *   Entry:   a geometry_msgs/Transform of the published LaserScan frame in the target frame and the target frame_id;
+ *            p_target = R p_scan + t.  R comes from the quaternion (x, y, z, w) on the host, once, in double, as tf2's
+ *            Matrix3x3::setRotation (d = x^2 + y^2 + z^2 + w^2, s = 2 / d), and each entry is rounded to float once; so
+ *            is t.  The LaserScan frame of an inverted lidar is already mirrored: its transform is that frame's pose.
+ *   Point:   for k = 0, 1, 2: X_k = fl(fl(fl(R_k0 * x_i) + fl(R_k1 * y_i)) + t_k), from the untransformed point (x_i, y_i,
+ *            0) of P; no FMA.  The keep rule, beam order, the channels, the stamp, height and is_dense are P's; the
+ *            message's frame_id is the target frame.
+ *   Viewpoint (RPL_SCAN_CLOUD_VIEWPOINT): three FLOAT32 fields vp_x, vp_y, vp_z after every other field, each t_k --
+ *            the sensor origin in the target frame; point_step = 12 + 4 * popcount(channels & 0x0F) + 12.
+ *   Disabled (enabled 0): P exactly -- the LaserScan's frame, no transform, viewpoint 0, 0, 0 (the origin in that
+ *            frame).  Its transform and target frame are not read (target_frames[s] may be NULL).
+ *   Limits:  every value finite, |d - 1| <= 1e-3, |t_k| <= 1000 (metres), target frame_id at most 255 characters;
+ *            otherwise RPL_RESULT_INVALID_DATA.
+ * Offsets: translation 0, rotation 24, enabled 56; 64 bytes. */
+typedef struct rpl_scan_cloud_transform {
+  double translation[3]; /* offset 0: t, metres, target frame */
+  double rotation[4];    /* 24: quaternion x, y, z, w */
+  uint8_t enabled;       /* 56: 0: no transform */
+  uint8_t pad[7];        /* 57 */
+} rpl_scan_cloud_transform; /* 64 bytes */
+/* RPL_SCAN_CLOUD_VIEWPOINT, a channel: accepted with RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS, or by
+ * rpl_scan_cloud_transform_batch_dev with a non-NULL transform; refused everywhere else. */
+#define RPL_SCAN_CLOUD_VIEWPOINT 0x10u
+/* RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS, an option in rpl_scan_cloud_params.channels (it adds no field): stream s's
+ * clouds take stream s's transform entry and target frame.  Accepted by scan_cloud_msgs[_dev] and
+ * push_scan_cloud_msgs[_dev] after the first set_scan_cloud_transforms; everywhere else, and before that call,
+ * RPL_RESULT_INVALID_DATA.  Sizes, packing and capacity are those of the call without it, with the target frame's
+ * header. */
+#define RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS 0x100u
+/*   set_scan_cloud_transforms: the transform and target frame of every stream, with the rules of set_scan_filters:
+ *            synchronous, masked (NULL = all), the first call sets every stream; a null transforms or target_frames, or
+ *            a masked enabled entry outside the limits (a null frame included), is RPL_RESULT_INVALID_DATA and leaves
+ *            the table unchanged.  rpl_capsule_stream_set_frames keeps its effect on disabled entries (their header is
+ *            the LaserScan's).  Export / import records do not carry the table. */
+rpl_result rpl_capsule_stream_set_scan_cloud_transforms(rpl_capsule_stream* s,
+                                                        const rpl_scan_cloud_transform* transforms /* [n_streams] */,
+                                                        const char* const* target_frames /* [n_streams] */,
+                                                        const uint8_t* stream_mask /* nullable: all */);
+/* Stateless: rpl_scan_cloud_batch_dev with one transform for every scan (the records only: rows carry no frame).  A
+ * NULL transform is exactly rpl_scan_cloud_batch_dev. */
+rpl_result rpl_scan_cloud_transform_batch_dev(rpl_ctx* ctx, const rpl_scan_cloud_params* params,
+                                              const rpl_scan_cloud_transform* transform /* nullable: none */,
+                                              const float* ranges, const float* intensities,
+                                              const uint32_t* beam_counts, const float* angle_increment,
+                                              const float* time_increment /* nullable: 0 */, float range_min,
+                                              float range_max, uint32_t n_scans, uint32_t stride, void* points,
+                                              uint32_t* point_counts, void* stream);
 
 /* ---- LaserScan / PointCloud2 -> wire (SURVEY.md 8(f) rank 3) ---------------------------- */
 /* The serialised message the RMW layer would produce from the message the reference publishes

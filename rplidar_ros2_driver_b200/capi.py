@@ -33,6 +33,8 @@ CLOUD_PER_STREAM_CHAIN = 4
 CLOUD_PER_STREAM_FOOTPRINTS = 8
 # rpl_scan_cloud_params.channels (laser_geometry ChannelOption)
 SCAN_CLOUD_INTENSITY, SCAN_CLOUD_INDEX, SCAN_CLOUD_DISTANCE, SCAN_CLOUD_TIMESTAMP = 1, 2, 4, 8
+# with a transform: the viewpoint channel, and the option that takes each stream's transform
+SCAN_CLOUD_VIEWPOINT, SCAN_CLOUD_PER_STREAM_TRANSFORMS = 0x10, 0x100
 CAPSULE_OK, CAPSULE_SYNC, CAPSULE_EMIT, CAPSULE_DISCARD = 1, 2, 4, 8
 CAPSULE_CHECKSUM_ERR, CAPSULE_ENCODER_RESET_ERR, CAPSULE_BAD_FRAME = 16, 32, 64
 PATH_FAST, PATH_GENERAL = 0, 1
@@ -71,6 +73,7 @@ EXPORTS = [
     "rpl_scan_filter_footprint_batch_dev", "rpl_capsule_stream_set_scan_footprints", "rpl_cloud_footprint_batch_dev",
     "rpl_scan_cloud_batch_dev", "rpl_capsule_stream_scan_cloud_msgs", "rpl_capsule_stream_scan_cloud_msgs_dev",
     "rpl_capsule_stream_push_scan_cloud_msgs", "rpl_capsule_stream_push_scan_cloud_msgs_dev",
+    "rpl_capsule_stream_set_scan_cloud_transforms", "rpl_scan_cloud_transform_batch_dev",
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -181,6 +184,14 @@ class ScanCloudParams(C.Structure):
     """rpl_scan_cloud_params: the projection of LaserScans into PointCloud2 (laser_geometry's projectLaser; 8 bytes).
     oracle/scan_cloud_oracle.py defines what it does."""
     _fields_ = [("channels", C.c_uint32), ("range_cutoff", C.c_float)]
+
+
+class ScanCloudTransform(C.Structure):
+    """rpl_scan_cloud_transform: the pose of a published LaserScan frame in a target frame (geometry_msgs/Transform:
+    translation, quaternion x, y, z, w) and whether it applies (64 bytes).  tests/scan_cloud_transform_oracle.py
+    defines what it does."""
+    _fields_ = [("translation", C.c_double * 3), ("rotation", C.c_double * 4), ("enabled", C.c_uint8),
+                ("pad", C.c_uint8 * 7)]
 
 
 # rpl_stream_counters: one stream session stream's counters (include/rpl_b200.h)
@@ -323,6 +334,10 @@ def lib() -> C.CDLL:
             ([vp, C.POINTER(ScanFilterSettings), C.POINTER(ScanFootprint), vp, vp, vp, vp, u32, u32, vp], u32),
         "rpl_scan_cloud_batch_dev": ([vp, C.POINTER(ScanCloudParams), vp, vp, vp, vp, vp, C.c_float, C.c_float, u32, u32,
                                       vp, vp, vp], u32),
+        "rpl_scan_cloud_transform_batch_dev":
+            ([vp, C.POINTER(ScanCloudParams), C.POINTER(ScanCloudTransform), vp, vp, vp, vp, vp, C.c_float, C.c_float,
+              u32, u32, vp, vp, vp], u32),
+        "rpl_capsule_stream_set_scan_cloud_transforms": ([vp, vp, vp, vp], u32),
         "rpl_capsule_stream_scan_cloud_msgs":
             ([vp, PSP, C.POINTER(ScanCloudParams), C.c_int64, vp, u64, vp, vp, vp], u32),
         "rpl_capsule_stream_scan_cloud_msgs_dev":
@@ -412,8 +427,22 @@ def scan_cloud_params(channels=SCAN_CLOUD_INTENSITY | SCAN_CLOUD_INDEX, range_cu
 
 
 def scan_cloud_point_step(channels) -> int:
-    """the bytes of one record: x, y, z and 4 per channel bit"""
-    return 12 + 4 * bin(int(channels) & 0xF).count("1")
+    """the bytes of one record: x, y, z, 4 per channel bit and 12 for the viewpoint"""
+    return 12 + 4 * bin(int(channels) & 0xF).count("1") + (12 if int(channels) & SCAN_CLOUD_VIEWPOINT else 0)
+
+
+def _scan_cloud_bound(channels, max_nodes) -> int:
+    """the largest projected cloud message: the longest header (288), the tail (192; 264 with the viewpoint), the
+    records of max_nodes beams and is_dense"""
+    return 288 + (264 if int(channels) & SCAN_CLOUD_VIEWPOINT else 192) + scan_cloud_point_step(channels) * max_nodes + 1
+
+
+def scan_cloud_transform(translation=(0.0, 0.0, 0.0), rotation=(0.0, 0.0, 0.0, 1.0), enabled=True) -> ScanCloudTransform:
+    """translation (x, y, z) in metres and the quaternion rotation (x, y, z, w) of the LaserScan frame in the target
+    frame; enabled False: no transform (P as without one)."""
+    return ScanCloudTransform((C.c_double * 3)(*(float(v) for v in translation)),
+                              (C.c_double * 4)(*(float(v) for v in rotation)), int(bool(enabled)),
+                              (C.c_uint8 * 7)())
 
 
 def _timing(t):
@@ -779,6 +808,15 @@ class Context:
             _p(time_increment), float(range_min), float(range_max), n_scans, stride, _p(points), _p(point_counts),
             _p(stream)))
 
+    def scan_cloud_transform_batch_dev(self, params: ScanCloudParams, transform: "ScanCloudTransform | None", ranges,
+                                       intensities, beam_counts, angle_increment, time_increment, range_min,
+                                       range_max, n_scans, stride, points, point_counts, stream=None):
+        """scan_cloud_batch_dev with every scan's points moved by one transform (None: none)."""
+        self._check(self._L.rpl_scan_cloud_transform_batch_dev(
+            self._h, C.byref(params), C.byref(transform) if transform is not None else None, _p(ranges),
+            _p(intensities), _p(beam_counts), _p(angle_increment), _p(time_increment), float(range_min),
+            float(range_max), n_scans, stride, _p(points), _p(point_counts), _p(stream)))
+
     def cloud_fuse_dev(self, xyzi, point_counts, n_scans, stride, fused, offsets, total, stream=None):
         self._check(self._L.rpl_cloud_fuse_dev(self._h, _p(xyzi), _p(point_counts), n_scans, stride, _p(fused),
                                                _p(offsets), _p(total), _p(stream)))
@@ -943,13 +981,25 @@ class CapsuleStreamSession:
         assert m is None or m.shape == (self.n_streams,)
         self._ctx._check(self._fn("set_scan_footprints")(self._h, C.cast(arr, C.c_void_p), _p(m)))
 
+    def set_scan_cloud_transforms(self, transforms, target_frames, mask=None):
+        """Per stream the transform (n_streams ScanCloudTransform, see scan_cloud_transform) and target frame (str; None
+        for a disabled entry) of the clouds that projecting calls with SCAN_CLOUD_PER_STREAM_TRANSFORMS publish.  Only
+        the entries where mask is true are copied (None: all); the first call must set every stream."""
+        assert len(transforms) == self.n_streams and len(target_frames) == self.n_streams
+        arr = (ScanCloudTransform * self.n_streams)(*transforms)
+        names = (C.c_char_p * self.n_streams)(*(None if f is None else f.encode() for f in target_frames))
+        m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
+        assert m is None or m.shape == (self.n_streams,)
+        self._ctx._check(self._fn("set_scan_cloud_transforms")(self._h, C.cast(arr, C.c_void_p),
+                                                                C.cast(names, C.c_void_p), _p(m)))
+
     def _msgs(self, name, params, clock_offset_ns, msgs, packed, cloud_params=None):
         ns = self.n_streams * self.max_scans
         if msgs is None:  # room for every slot's largest message
             if name == "laserscan_msgs":
                 per = 288 + 32 + 8 * self.max_nodes + 4
             elif name == "scan_cloud_msgs":
-                per = 288 + 192 + scan_cloud_point_step(cloud_params.channels) * self.max_nodes + 1
+                per = _scan_cloud_bound(cloud_params.channels, self.max_nodes)
             else:
                 per = 288 + 116 + 16 * self.max_nodes + 1
             msgs = np.zeros(ns * ((per + 15) // 16 * 16), np.uint8)
@@ -1089,7 +1139,7 @@ class CapsuleStreamSession:
         if msgs is None:
             msgs = np.zeros(ns * ((288 + 32 + 8 * self.max_nodes + 4 + 15) // 16 * 16), np.uint8)
         if cloud_msgs is None:
-            per = 288 + 192 + scan_cloud_point_step(cloud_params.channels) * self.max_nodes + 1
+            per = _scan_cloud_bound(cloud_params.channels, self.max_nodes)
             cloud_msgs = np.zeros(ns * ((per + 15) // 16 * 16), np.uint8)
         out = []
         for buf in (msgs, cloud_msgs):

@@ -703,6 +703,11 @@ static_assert(sizeof(rpl_scan_cloud_params) == 8 && offsetof(rpl_scan_cloud_para
                   RPL_SCAN_CLOUD_DISTANCE == rpl::kScanCloudDistance &&
                   RPL_SCAN_CLOUD_TIMESTAMP == rpl::kScanCloudTimestamp,
               "rpl_scan_cloud_params and its channel bits are the header's");
+static_assert(sizeof(rpl_scan_cloud_transform) == 64 && offsetof(rpl_scan_cloud_transform, rotation) == 24 &&
+                  offsetof(rpl_scan_cloud_transform, enabled) == 56 &&
+                  RPL_SCAN_CLOUD_VIEWPOINT == rpl::kScanCloudViewpoint &&
+                  RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS == rpl::kScanCloudPerStreamTransforms,
+              "rpl_scan_cloud_transform and the transform bits are the header's");
 static_assert(sizeof(rpl_msgs_out) == 40 && offsetof(rpl_msgs_out, capacity) == 8 &&
                   offsetof(rpl_msgs_out, msg_offsets) == 16 && offsetof(rpl_msgs_out, msg_sizes) == 24 &&
                   offsetof(rpl_msgs_out, total_bytes) == 32,
@@ -710,16 +715,22 @@ static_assert(sizeof(rpl_msgs_out) == 40 && offsetof(rpl_msgs_out, capacity) == 
 
 namespace {
 
-// the rules of rpl_scan_cloud_params (oracle/scan_cloud_oracle.py params_ok)
-bool scan_cloud_ok(rpl_ctx* c, const rpl_scan_cloud_params& p) {
+// the rules of rpl_scan_cloud_params (oracle/scan_cloud_oracle.py params_ok); `extra`: the bits beyond the four
+// channels the call accepts (the viewpoint and the per-stream transforms, where a transform applies)
+bool scan_cloud_ok(rpl_ctx* c, const rpl_scan_cloud_params& p, uint32_t extra = 0) {
   const char* why = nullptr;
-  if (p.channels & ~rpl::kScanCloudChannels) why = "unknown scan cloud channel bits (only 0x01, 0x02, 0x04, 0x08)";
+  if (p.channels & ~(rpl::kScanCloudChannels | extra))
+    why = extra ? "unknown scan cloud channel bits, or RPL_SCAN_CLOUD_VIEWPOINT without a transform"
+                : "unknown scan cloud channel bits (only 0x01, 0x02, 0x04, 0x08)";
   else if (std::isnan(p.range_cutoff)) why = "range_cutoff is NaN";
   if (why) c->err = why;
   return why == nullptr;
 }
 
-uint32_t scan_cloud_point_step(uint32_t channels) { return 12u + 4u * (uint32_t)__builtin_popcount(channels); }
+uint32_t scan_cloud_point_step(uint32_t channels) {
+  return 12u + 4u * (uint32_t)__builtin_popcount(channels & rpl::kScanCloudChannels) +
+         ((channels & rpl::kScanCloudViewpoint) ? 12u : 0u);
+}
 
 // The PointCloud2 members between the header and the data of fields names[0..nf) (datatypes types[], count 1, offsets
 // 4 bytes apart from 0): height 1, width, the fields, is_bigendian 0, point_step, row_step, data length
@@ -756,49 +767,113 @@ Tail pointcloud2_tail(const char* const* names, const uint8_t* types, uint32_t n
   return t;
 }
 
-// the tail of a channel set: x, y, z, then laser_geometry's channels in bit order
+// the tails of the channel sets below `sets`: x, y, z, then laser_geometry's channels in bit order, then the viewpoint's
+// three fields
+extern "C++" template <class Tail>
+std::vector<Tail> scan_cloud_tails(uint32_t sets) {
+  std::vector<Tail> v(sets);
+  const char* const channel_names[7] = {"intensity", "index", "distances", "stamps", "vp_x", "vp_y", "vp_z"};
+  const uint8_t channel_types[7] = {7, 5, 7, 7, 7, 7, 7};  // FLOAT32, INT32, FLOAT32 ...
+  for (uint32_t ch = 0; ch < sets; ++ch) {
+    const char* names[10] = {"x", "y", "z"};
+    uint8_t types[10] = {7, 7, 7};
+    uint32_t nf = 3;
+    for (uint32_t k = 0; k < 7; ++k)
+      if (ch & (1u << (k < 4 ? k : 4))) {
+        names[nf] = channel_names[k];
+        types[nf++] = channel_types[k];
+      }
+    v[ch] = pointcloud2_tail<Tail>(names, types, nf, scan_cloud_point_step(ch));
+  }
+  return v;
+}
 const rpl::ScanCloudTail& scan_cloud_tail(uint32_t channels) {
-  static const std::vector<rpl::ScanCloudTail> tails = [] {
-    std::vector<rpl::ScanCloudTail> v(rpl::kScanCloudChannels + 1);
-    const char* const channel_names[4] = {"intensity", "index", "distances", "stamps"};
-    const uint8_t channel_types[4] = {7, 5, 7, 7};  // FLOAT32, INT32, FLOAT32, FLOAT32
-    for (uint32_t ch = 0; ch <= rpl::kScanCloudChannels; ++ch) {
-      const char* names[7] = {"x", "y", "z"};
-      uint8_t types[7] = {7, 7, 7};
-      uint32_t nf = 3;
-      for (uint32_t k = 0; k < 4; ++k)
-        if (ch & (1u << k)) {
-          names[nf] = channel_names[k];
-          types[nf++] = channel_types[k];
-        }
-      v[ch] = pointcloud2_tail<rpl::ScanCloudTail>(names, types, nf, scan_cloud_point_step(ch));
-    }
-    return v;
-  }();
+  static const std::vector<rpl::ScanCloudTail> tails = scan_cloud_tails<rpl::ScanCloudTail>(rpl::kScanCloudChannels + 1);
   return tails[channels];
 }
+// a transforming call's: every channel set with or without the viewpoint
+const rpl::ScanCloudTailXf& scan_cloud_tail_xf(uint32_t channels) {
+  static const std::vector<rpl::ScanCloudTailXf> tails =
+      scan_cloud_tails<rpl::ScanCloudTailXf>(2 * rpl::kScanCloudViewpoint);
+  return tails[channels & (rpl::kScanCloudChannels | rpl::kScanCloudViewpoint)];
+}
+// its tail's bytes
+uint32_t scan_cloud_tail_bytes(uint32_t channels) {
+  return (channels & rpl::kScanCloudPerStreamTransforms) ? scan_cloud_tail_xf(channels).bytes
+                                                         : scan_cloud_tail(channels).bytes;
+}
 
-// the settings of params into a
+// the settings of params into a (a call with RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS: the transforming kernel's tail; the
+// caller gives it the tables)
 void scan_cloud_setup(rpl::ScanCloudArgs& a, const rpl_scan_cloud_params& p) {
   a.channels = p.channels;
   a.point_step = scan_cloud_point_step(p.channels);
   a.range_cutoff = p.range_cutoff;
-  a.tail = scan_cloud_tail(p.channels);
+  if (p.channels & rpl::kScanCloudPerStreamTransforms) {
+    a.transform = 1;
+    a.tail_xf = scan_cloud_tail_xf(p.channels);
+  } else {
+    a.tail = scan_cloud_tail(p.channels);
+  }
+}
+
+// The limits of one transform entry (tests/scan_cloud_transform_oracle.py transform_ok); frame: its target frame, or
+// nullptr where none is given (the stateless call)
+bool scan_cloud_transform_ok(rpl_ctx* c, const rpl_scan_cloud_transform& e, const char* frame, bool framed) {
+  const char* why = nullptr;
+  const double* q = e.rotation;
+  bool finite = true;
+  for (int k = 0; k < 3; ++k) finite = finite && std::isfinite(e.translation[k]);
+  for (int k = 0; k < 4; ++k) finite = finite && std::isfinite(q[k]);
+  if (!finite) why = "a transform's translation and rotation must be finite";
+  else if (!(std::fabs(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] - 1.0) <= 1e-3))
+    why = "a transform's quaternion must be of norm 1 (|x^2 + y^2 + z^2 + w^2 - 1| <= 1e-3)";
+  else if (!(std::fabs(e.translation[0]) <= 1000.0 && std::fabs(e.translation[1]) <= 1000.0 &&
+             std::fabs(e.translation[2]) <= 1000.0))
+    why = "a transform's translation must be within 1000 m";
+  else if (framed && !frame) why = "null target_frames[s] of an enabled entry";
+  if (why) {
+    c->err = why;
+    return false;
+  }
+  return !framed || frame_id_length_ok(c, std::strlen(frame));
+}
+
+// The rows {R_k0, R_k1, t_k, on} of a transform entry (scan_cloud_kernel<true>): R from the quaternion in double as
+// tf2's Matrix3x3::setRotation, each entry and t rounded to float once; a disabled entry's are zero (on 0: no
+// transform)
+void scan_cloud_rows(const rpl_scan_cloud_transform& e, float4 rows[3]) {
+  if (!e.enabled) {
+    for (int k = 0; k < 3; ++k) rows[k] = float4{0.0f, 0.0f, 0.0f, 0.0f};
+    return;
+  }
+  const double x = e.rotation[0], y = e.rotation[1], z = e.rotation[2], w = e.rotation[3];
+  const double d = x * x + y * y + z * z + w * w, s = 2.0 / d;
+  const double xs = x * s, ys = y * s, zs = z * s;
+  const double wx = w * xs, wy = w * ys, wz = w * zs;
+  const double xx = x * xs, xy = x * ys, xz = x * zs;
+  const double yy = y * ys, yz = y * zs, zz = z * zs;
+  const double R[3][2] = {{1.0 - (yy + zz), xy - wz}, {xy + wz, 1.0 - (xx + zz)}, {xz - wy, yz + wx}};
+  for (int k = 0; k < 3; ++k)
+    rows[k] = float4{(float)R[k][0], (float)R[k][1], (float)e.translation[k], 1.0f};
 }
 
 }  // namespace
 
-rpl_result rpl_scan_cloud_batch_dev(rpl_ctx* c, const rpl_scan_cloud_params* params, const float* ranges,
-                                    const float* intensities, const uint32_t* beam_counts,
-                                    const float* angle_increment, const float* time_increment, float range_min,
-                                    float range_max, uint32_t n_scans, uint32_t stride, void* points,
-                                    uint32_t* point_counts, void* stream) {
+rpl_result rpl_scan_cloud_transform_batch_dev(rpl_ctx* c, const rpl_scan_cloud_params* params,
+                                              const rpl_scan_cloud_transform* transform, const float* ranges,
+                                              const float* intensities, const uint32_t* beam_counts,
+                                              const float* angle_increment, const float* time_increment,
+                                              float range_min, float range_max, uint32_t n_scans, uint32_t stride,
+                                              void* points, uint32_t* point_counts, void* stream) {
   if (!c) return RPL_RESULT_INVALID_DATA;
   if (!params || !ranges || !intensities || !beam_counts || !angle_increment || !points || !point_counts) {
     c->err = "null params, ranges, intensities, beam_counts, angle_increment, points or point_counts";
     return RPL_RESULT_INVALID_DATA;
   }
-  if (!scan_cloud_ok(c, *params)) return RPL_RESULT_INVALID_DATA;
+  if (!scan_cloud_ok(c, *params, transform ? rpl::kScanCloudViewpoint : 0u)) return RPL_RESULT_INVALID_DATA;
+  if (transform && transform->enabled && !scan_cloud_transform_ok(c, *transform, nullptr, false))
+    return RPL_RESULT_INVALID_DATA;
   if (n_scans != 0 && (stride == 0 || stride > c->max_nodes)) {
     c->err = "stride must be in [1, the context's max_nodes]";
     return RPL_RESULT_INVALID_DATA;
@@ -823,9 +898,23 @@ rpl_result rpl_scan_cloud_batch_dev(rpl_ctx* c, const rpl_scan_cloud_params* par
   a.time_increment = time_increment;
   a.kept = point_counts;
   a.points = static_cast<float*>(points);
+  if (transform) {
+    a.transform = 1;
+    scan_cloud_rows(*transform, a.xf_one);
+  }
   RPL_CUDA(c, rpl::launch_scan_cloud(a, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
   c->launches++;
   return RPL_RESULT_OK;
+}
+
+rpl_result rpl_scan_cloud_batch_dev(rpl_ctx* c, const rpl_scan_cloud_params* params, const float* ranges,
+                                    const float* intensities, const uint32_t* beam_counts,
+                                    const float* angle_increment, const float* time_increment, float range_min,
+                                    float range_max, uint32_t n_scans, uint32_t stride, void* points,
+                                    uint32_t* point_counts, void* stream) {
+  return rpl_scan_cloud_transform_batch_dev(c, params, nullptr, ranges, intensities, beam_counts, angle_increment,
+                                            time_increment, range_min, range_max, n_scans, stride, points,
+                                            point_counts, stream);
 }
 
 // ---- host-buffer batch: chunked over the two lanes so that the H2D copy of chunk i+1, the
@@ -1617,6 +1706,15 @@ struct rpl_capsule_stream {
   // and as the kernel reads them (nullptr until then: no stream has a footprint)
   std::vector<rpl_scan_footprint> footprints_host;
   rpl::ScanFootprint* footprints = nullptr;     // [n_streams] device
+  // the transforms of the projected clouds (rpl_capsule_stream_set_scan_cloud_transforms) that calls with
+  // RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS read: the entries and target frames as set (empty until the first call sets
+  // every stream), their rows (scan_cloud_rows) and each stream's resolved message header -- the target frame's, a
+  // disabled entry's the LaserScan's -- rebuilt by set_frames as well (transforms_resolve)
+  std::vector<rpl_scan_cloud_transform> xf_host;
+  std::vector<std::string> xf_frames;
+  float4* xf = nullptr;                         // [n_streams][3] device
+  rpl::StreamMsgHeader* xf_hdr = nullptr;       // [n_streams] device
+  std::vector<rpl::StreamMsgHeader> xf_hdr_host;
   unsigned char* node_work = nullptr;           // the tables of a nodes call (NodeWork)
   // [n_streams] device, zeroed at create: what every push decoded and lost (rpl_capsule_stream_counters); a stream's
   // record is written by the one CTA of each kernel that serves the stream
@@ -2089,6 +2187,9 @@ struct ChunkScanClouds {
   uint32_t* sizes;
   unsigned long long* extent_host;
   cudaEvent_t dir_order;
+  // RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS: the session's resolved headers and rows at the chunk's first stream
+  const rpl::StreamMsgHeader* hdr;
+  const float4* xf;
 };
 
 // A message push's chunk (rpl_capsule_stream_push_{laserscan,cloud,scan_cloud}_msgs*): where its messages and tables
@@ -2139,6 +2240,8 @@ rpl::ScanCloudArgs scan_cloud_push_args(const WireChunk& w, uint32_t ns, bool st
   a.scan_msgs = m.out;
   a.place = m.place;
   a.scan_sizes = m.sizes;
+  a.cloud_hdr = m.proj.hdr;
+  a.xf = m.proj.xf;
   return a;
 }
 
@@ -2300,7 +2403,8 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
   d.counts = m->proj.kept;
   d.sizes = m->proj.sizes;
   d.scan_sizes = m->sizes;
-  d.tail_bytes = sa.tail.bytes;
+  if (sa.transform) d.hdr = m->proj.hdr;  // the target frames' headers size the messages
+  d.tail_bytes = sa.transform ? sa.tail_xf.bytes : sa.tail.bytes;
   d.point_step = sa.point_step;
   r = directory(d, rpl::MsgKind::kScanCloud, m->proj.dir_order, m->proj.extent_host);
   if (r != RPL_RESULT_OK || m->extent_host) return r;
@@ -2347,6 +2451,8 @@ struct HostMsgs {
   unsigned long long *proj_carry, *proj_extent_host;
   uint32_t* kept;
   cudaEvent_t proj_dir_order;
+  const rpl::StreamMsgHeader* proj_hdr;  // RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS: the session's resolved headers, rows
+  const float4* proj_xf;
 };
 
 // Runs a host call's n_streams streams through capsule_stream_chunk, `chunk` streams at a time round-robin over the
@@ -2474,7 +2580,8 @@ rpl_result push_host(rpl_ctx* c, const HostWire& h, uint32_t n_streams, uint32_t
       m.points = d.points;
       if (proj)
         m.proj = ChunkScanClouds{hm->proj, hm->kept + so, d.pmsgs, hm->clouds->capacity, hm->proj_carry, d.poffs,
-                                 d.pextent, nullptr, d.psizes, hm->proj_extent_host + 3 * li, hm->proj_dir_order};
+                                 d.pextent, nullptr, d.psizes, hm->proj_extent_host + 3 * li, hm->proj_dir_order,
+                                 hm->proj_hdr ? hm->proj_hdr + s0 : nullptr, hm->proj_xf ? hm->proj_xf + 3 * s0 : nullptr};
     }
     const rpl_result r = capsule_stream_chunk(c, l, l.stream, d.w, ns, d.in, d.counts, h.sample_duration_us, h.params,
                                               d.ranges, d.intens, d.beams, d.inc, d.sps, h.sp ? &sp : nullptr,
@@ -2869,6 +2976,8 @@ struct PushMsgs {
   const rpl_msgs_out* clouds;
   unsigned long long* proj_carry;
   uint32_t* kept;
+  const rpl::StreamMsgHeader* proj_hdr;  // RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS: the session's resolved headers, rows
+  const float4* proj_xf;
 };
 
 // A push of the kind the entry point takes (bytes: a byte push); sp: a stamped one.  Host arrays (dev false, stream
@@ -2924,7 +3033,8 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
           m.proj = ChunkScanClouds{pm->proj, pm->kept + so, pm->clouds->msgs, pm->clouds->capacity, pm->proj_carry,
                                    reinterpret_cast<unsigned long long*>(pm->clouds->msg_offsets) + so, nullptr,
                                    reinterpret_cast<unsigned long long*>(pm->clouds->total_bytes),
-                                   pm->clouds->msg_sizes + so, nullptr, nullptr};
+                                   pm->clouds->msg_sizes + so, nullptr, nullptr, pm->proj_hdr ? pm->proj_hdr + s0 : nullptr,
+                                   pm->proj_xf ? pm->proj_xf + 3 * s0 : nullptr};
       }
       r = capsule_stream_chunk(c, c->lane[0], st, session_chunk(cs, s0, params, true, pm ? pm->cloud : nullptr),
                                std::min(chunk, cs->n_streams - s0), in + s0 * cs->in_stream, counts + s0,
@@ -2952,7 +3062,12 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
                     pm->clock_offset_ns, cs->msg_hdr, pm->w.carry, pm->w.place, cs->push_msg_extent,
                     cs->push_msg_extent_ready, cs->push_msg_dir_order, pm->cloud};
       if (pm->proj) {  // a projected cloud's bound: its message at max_nodes kept beams, rounded up to 16
-        const size_t pmost = (size_t)hdr_most + scan_cloud_tail(pm->proj->channels).bytes +
+        uint32_t proj_hdr_most = hdr_most;  // with transforms: the longest resolved header
+        if (pm->proj_hdr) {
+          proj_hdr_most = 0;
+          for (const rpl::StreamMsgHeader& e : cs->xf_hdr_host) proj_hdr_most = std::max(proj_hdr_most, e.bytes);
+        }
+        const size_t pmost = (size_t)proj_hdr_most + scan_cloud_tail_bytes(pm->proj->channels) +
                              (size_t)scan_cloud_point_step(pm->proj->channels) * n + 1;
         hm.proj = pm->proj;
         hm.clouds = pm->clouds;
@@ -2961,6 +3076,8 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
         hm.proj_extent_host = cs->push_scan_cloud_extent;
         hm.kept = pm->kept;
         hm.proj_dir_order = cs->push_scan_cloud_dir_order;
+        hm.proj_hdr = pm->proj_hdr;
+        hm.proj_xf = pm->proj_xf;
       }
     }
     const HostWire h{in, counts, cs->in_stream, sample_duration_us, cs->max_nodes, cs->max_scans, params, ranges,
@@ -3178,6 +3295,62 @@ rpl_result clouds_resolve(rpl_capsule_stream* cs, const std::vector<rpl_scan_foo
   return RPL_RESULT_OK;
 }
 
+// The device tables of the per-stream transforms from entries t and target frames f: each stream's rows and its
+// clouds' header (a disabled entry's the LaserScan's).  The caller has passed cs->done and made the tables.
+rpl_result transforms_resolve(rpl_capsule_stream* cs, const std::vector<rpl_scan_cloud_transform>& t,
+                              const std::vector<std::string>& f) {
+  rpl_ctx* c = cs->c;
+  std::vector<float4> rows(3 * (size_t)cs->n_streams);
+  std::vector<rpl::StreamMsgHeader> h(cs->n_streams);
+  for (uint32_t s = 0; s < cs->n_streams; ++s) {
+    scan_cloud_rows(t[s], &rows[3 * (size_t)s]);
+    h[s] = t[s].enabled ? msg_header(f[s].data(), f[s].size(), cs->msg_hdr_host[s].range_max) : cs->msg_hdr_host[s];
+  }
+  RPL_CUDA(c, cudaMemcpy(cs->xf, rows.data(), rows.size() * sizeof(float4), cudaMemcpyHostToDevice),
+           RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaMemcpy(cs->xf_hdr, h.data(), h.size() * sizeof(rpl::StreamMsgHeader), cudaMemcpyHostToDevice),
+           RPL_RESULT_OPERATION_FAIL);
+  cs->xf_hdr_host = std::move(h);
+  return RPL_RESULT_OK;
+}
+
+// the transforms of the projected clouds: the masked entries and target frames replace the table's, all or none
+rpl_result stream_set_scan_cloud_transforms(rpl_capsule_stream* cs, const rpl_scan_cloud_transform* transforms,
+                                            const char* const* target_frames, const uint8_t* stream_mask) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!transforms || !target_frames) {
+    c->err = "null transforms or target_frames";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  std::vector<rpl_scan_cloud_transform> t = cs->xf_host;
+  std::vector<std::string> f = cs->xf_frames;
+  if (t.empty()) {
+    for (uint32_t s = 0; s < cs->n_streams; ++s)
+      if (stream_mask && !stream_mask[s]) {
+        c->err = "the first rpl_capsule_stream_set_scan_cloud_transforms call must set every stream";
+        return RPL_RESULT_INVALID_DATA;
+      }
+    t.resize(cs->n_streams);
+    f.resize(cs->n_streams);
+  }
+  for (uint32_t s = 0; s < cs->n_streams; ++s) {
+    if (stream_mask && !stream_mask[s]) continue;
+    const bool on = transforms[s].enabled != 0;
+    if (on && !scan_cloud_transform_ok(c, transforms[s], target_frames[s], true)) return RPL_RESULT_INVALID_DATA;
+    t[s] = transforms[s];
+    f[s] = on ? std::string(target_frames[s]) : std::string();
+  }
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  if (!cs->xf) RPL_CUDA(c, dev_alloc(&cs->xf, 3 * (size_t)cs->n_streams), RPL_RESULT_INSUFFICIENT_MEMORY);
+  if (!cs->xf_hdr) RPL_CUDA(c, dev_alloc(&cs->xf_hdr, cs->n_streams), RPL_RESULT_INSUFFICIENT_MEMORY);
+  RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);  // a messages call may still read them
+  if (const rpl_result r = transforms_resolve(cs, t, f); r != RPL_RESULT_OK) return r;
+  cs->xf_host = std::move(t);
+  cs->xf_frames = std::move(f);
+  return RPL_RESULT_OK;
+}
+
 rpl_result stream_set_frames(rpl_capsule_stream* cs, const char* const* frame_ids, const float* range_max) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
   rpl_ctx* c = cs->c;
@@ -3200,6 +3373,8 @@ rpl_result stream_set_frames(rpl_capsule_stream* cs, const char* const* frame_id
   RPL_CUDA(c, cudaMemcpy(cs->msg_hdr, h.data(), h.size() * sizeof(rpl::StreamMsgHeader), cudaMemcpyHostToDevice),
            RPL_RESULT_OPERATION_FAIL);
   cs->msg_hdr_host = std::move(h);
+  if (!cs->xf_host.empty())  // a disabled transform entry's header follows the frames
+    if (const rpl_result r = transforms_resolve(cs, cs->xf_host, cs->xf_frames); r != RPL_RESULT_OK) return r;
   return cs->clouds_host.empty() ? RPL_RESULT_OK : clouds_resolve(cs);  // a range_max of 0 follows the frames
 }
 
@@ -3374,11 +3549,28 @@ struct ScanCloudCall {
   const rpl_scan_cloud_params* cloud;
 };
 
+// a kScanCloud messages call with RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS
+bool scan_cloud_transforms(const void* params) {
+  return (static_cast<const ScanCloudCall*>(params)->cloud->channels & rpl::kScanCloudPerStreamTransforms) != 0;
+}
+
 // the LaserScan params of a messages call (kLaserScan, kScanCloud), nullptr for kPointCloud2
 const rpl_scan_params* msgs_scan_params(rpl::MsgKind kind, const void* params) {
   if (kind == rpl::MsgKind::kLaserScan) return static_cast<const rpl_scan_params*>(params);
   if (kind == rpl::MsgKind::kScanCloud) return static_cast<const ScanCloudCall*>(params)->scan;
   return nullptr;
+}
+
+// the rules of a session projection's params: the channels, and RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS (with which the
+// viewpoint is accepted) only after the first set_scan_cloud_transforms
+bool scan_cloud_call_ok(rpl_capsule_stream* cs, const rpl_scan_cloud_params& p) {
+  const bool xf = (p.channels & rpl::kScanCloudPerStreamTransforms) != 0;
+  if (!scan_cloud_ok(cs->c, p, rpl::kScanCloudPerStreamTransforms | (xf ? rpl::kScanCloudViewpoint : 0u))) return false;
+  if (xf && cs->xf_host.empty()) {
+    cs->c->err = "RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS before the first rpl_capsule_stream_set_scan_cloud_transforms";
+    return false;
+  }
+  return true;
 }
 
 bool stream_msgs_args_ok(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* params, const void* msgs,
@@ -3396,7 +3588,7 @@ bool stream_msgs_args_ok(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* 
       c->err = "null scan_params or cloud_params";
       return false;
     }
-    if (!scan_cloud_ok(c, *q->cloud)) return false;
+    if (!scan_cloud_call_ok(cs, *q->cloud)) return false;
   }
   const rpl_scan_params* sp = msgs_scan_params(kind, params);
   const bool per_stream = sp ? (sp->flags & RPL_FLAG_PER_STREAM) != 0
@@ -3433,6 +3625,10 @@ rpl::ScanCloudArgs scan_cloud_msg_args(const rpl_capsule_stream* cs, const void*
   a.m.mode_a = q->scan->scan_processing ? 1u : 0u;
   if ((q->scan->flags & RPL_FLAG_PER_STREAM) != 0) a.m.lidars = cs->lidars;
   a.kept = w.kept;
+  if (a.transform) {
+    a.cloud_hdr = cs->xf_hdr;
+    a.xf = cs->xf;
+  }
   return a;
 }
 
@@ -3472,11 +3668,11 @@ rpl_result msgs_prepare(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* p
     RPL_CUDA(c, rpl::launch_scan_cloud_count(a, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
     c->launches++;
     t.beams = w.counts;
-    t.tail_bytes = a.tail.bytes;
+    t.tail_bytes = a.transform ? a.tail_xf.bytes : a.tail.bytes;
     t.point_step = a.point_step;
   }
   t.kind = kind;
-  t.hdr = cs->msg_hdr;
+  t.hdr = kind == rpl::MsgKind::kScanCloud && scan_cloud_transforms(params) ? cs->xf_hdr : cs->msg_hdr;
   t.counts = kind == rpl::MsgKind::kScanCloud ? w.kept : w.counts;
   t.views = reinterpret_cast<const uint2*>(cs->views);
   t.n_slots = (uint32_t)NS;
@@ -3685,7 +3881,7 @@ rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, rpl::MsgK
       c->err = "null clouds->msgs, msg_offsets, msg_sizes or total_bytes";
       return RPL_RESULT_INVALID_DATA;
     }
-    if (!scan_cloud_ok(c, *proj)) return RPL_RESULT_INVALID_DATA;
+    if (!scan_cloud_call_ok(cs, *proj)) return RPL_RESULT_INVALID_DATA;
     if (dev && ((reinterpret_cast<uintptr_t>(clouds->msgs) & 15u) || misaligned8(clouds->msg_offsets) ||
                 misaligned8(clouds->total_bytes) || (reinterpret_cast<uintptr_t>(clouds->msg_sizes) & 3u))) {
       c->err = "clouds: msgs must be 16-byte aligned, msg_offsets and total_bytes 8-byte, msg_sizes 4-byte aligned";
@@ -3744,6 +3940,10 @@ rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, rpl::MsgK
     pm.clouds = clouds;
     pm.proj_carry = sw.carry;
     pm.kept = sw.kept;
+    if (proj->channels & rpl::kScanCloudPerStreamTransforms) {
+      pm.proj_hdr = cs->xf_hdr;
+      pm.proj_xf = cs->xf;
+    }
   }
   if (cloud && dev) {  // one chunk's clouds, in the session's message work block (cloud_msgs' when that is larger)
     const size_t NS = (size_t)cs->chunk_dev * cs->max_scans;
@@ -4043,6 +4243,8 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
     if (e) cudaEventDestroy(e);
   if (cs->push_msg_dir_order) cudaEventDestroy(cs->push_msg_dir_order);
   cudaFree(cs->push_scan_cloud_work);
+  cudaFree(cs->xf);
+  cudaFree(cs->xf_hdr);
   cudaFreeHost(cs->push_scan_cloud_extent);
   if (cs->push_scan_cloud_dir_order) cudaEventDestroy(cs->push_scan_cloud_dir_order);
   if (cs->done) cudaEventDestroy(cs->done);
@@ -4532,6 +4734,12 @@ rpl_result rpl_capsule_stream_set_clouds(rpl_capsule_stream* s, const rpl_cloud_
 rpl_result rpl_capsule_stream_set_scan_filters(rpl_capsule_stream* s, const rpl_scan_filter_settings* settings,
                                                const uint8_t* stream_mask) {
   return stream_set_scan_filters(s, settings, stream_mask);
+}
+
+rpl_result rpl_capsule_stream_set_scan_cloud_transforms(rpl_capsule_stream* s,
+                                                        const rpl_scan_cloud_transform* transforms,
+                                                        const char* const* target_frames, const uint8_t* stream_mask) {
+  return stream_set_scan_cloud_transforms(s, transforms, target_frames, stream_mask);
 }
 
 rpl_result rpl_capsule_stream_set_scan_footprints(rpl_capsule_stream* s, const rpl_scan_footprint* footprints,

@@ -1271,6 +1271,76 @@ rpl_result rpl_scan_cloud_transform_batch_dev(rpl_ctx* ctx, const rpl_scan_cloud
                                               float range_max, uint32_t n_scans, uint32_t stride, void* points,
                                               uint32_t* point_counts, void* stream);
 
+/* LaserScans re-gridded from the projected clouds (DESIGN.md 5.7.1 "LaserScans re-gridded from the projected clouds";
+ * INTEGRATION.md 4j): pointcloud_to_laserscan's cloudCallback on the device, over the clouds the projection above
+ * publishes -- filtered, footprinted, projected and transformed -- so that the scan agrees with that cloud by
+ * construction and has the same beam count for a stream in every revolution.  Q(settings, cloud) is a pure function
+ * of one cloud's x, y, z, defined bit for bit by oracle/rescan_oracle.py:
+ *   grid:    ranges_size = ceil(fl32(fl32(angle_max - angle_min) / angle_increment)) (float arithmetic); every beam
+ *            starts at +inf (use_inf) or fl32(range_max + inf_epsilon) (the sum in double).
+ *   point:   in record order, (X, Y, Z) is skipped when Z > max_height or Z < min_height; range = sqrt(X*X + Y*Y) in
+ *            double (exact products, one rounded sum, a correctly rounded sqrt), skipped outside [range_min,
+ *            range_max]; angle = fdlibm's atan2(Y, X) with every double operation rounded as written, skipped outside
+ *            [angle_min, angle_max]; index = (int)((angle - angle_min) / angle_increment) in double, skipped when
+ *            >= ranges_size; ranges[index] = min(ranges[index], fl32(range)).
+ *   message: sensor_msgs/LaserScan: the LaserScan's stamp; the stream's target frame when the call has
+ *            RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS and the stream's transform entry is enabled, else the LaserScan's
+ *            frame; angle_min, angle_max, angle_increment, scan_time, range_min, range_max the entry's;
+ *            time_increment 0; ranges_size ranges; no intensities.  A cloud of width 0 gives every beam its start.
+ *   Limits:  every float finite, angle_increment > 0, angle_min < angle_max, 1 <= ranges_size <= 8192,
+ *            0 <= range_min <= range_max, min_height <= max_height, inf_epsilon >= 0; otherwise
+ *            RPL_RESULT_INVALID_DATA.  A disabled entry (enabled 0) is not read; its slots have no message.
+ * Offsets: angle_min 0, angle_max 4, angle_increment 8, range_min 12, range_max 16, min_height 20, max_height 24,
+ *          inf_epsilon 28, scan_time 32, use_inf 36, enabled 37; 40 bytes. */
+typedef struct rpl_rescan_settings {
+  float angle_min;        /* offset 0: radians, in the cloud's frame */
+  float angle_max;        /* 4 */
+  float angle_increment;  /* 8 */
+  float range_min;        /* 12: metres */
+  float range_max;        /* 16 */
+  float min_height;       /* 20: metres, z in the cloud's frame */
+  float max_height;       /* 24 */
+  float inf_epsilon;      /* 28: without use_inf, every beam starts at range_max + inf_epsilon */
+  float scan_time;        /* 32: seconds, published as is */
+  uint8_t use_inf;        /* 36: != 0: every beam starts at +inf */
+  uint8_t enabled;        /* 37: 0: the stream has no re-gridded scans */
+  uint8_t pad[2];         /* 38 */
+} rpl_rescan_settings;   /* 40 bytes */
+/* Stateless: Q(*settings, the cloud rpl_scan_cloud_transform_batch_dev(cloud_params, transform, ...) gives row s) of
+ * n_scans rows laid out as rpl_scan_batch_dev writes them (device arrays: ranges [n_scans][stride], beam_counts and
+ * angle_increment [n_scans]; intensities is not read and may be NULL), with the arguments and refusals of that call;
+ * settings->enabled is not read.  Row s's ranges_size floats at out_ranges + s * ranges_size.  Asynchronous on
+ * `stream` (NULL: the context's stream). */
+rpl_result rpl_rescan_batch_dev(rpl_ctx* ctx, const rpl_rescan_settings* settings,
+                                const rpl_scan_cloud_params* cloud_params,
+                                const rpl_scan_cloud_transform* transform /* nullable: none */, const float* ranges,
+                                const float* intensities /* nullable */, const uint32_t* beam_counts,
+                                const float* angle_increment, float range_min, float range_max, uint32_t n_scans,
+                                uint32_t stride, float* out_ranges /* [n_scans][ranges_size] */, void* stream);
+/*   set_rescans: the entry of every stream, with the rules of set_scan_filters: synchronous, masked (NULL = all), the
+ *            first call sets every stream; a null settings, or a masked enabled entry outside the limits, is
+ *            RPL_RESULT_INVALID_DATA and leaves the table unchanged.  Export / import records do not carry the table. */
+rpl_result rpl_capsule_stream_set_rescans(rpl_capsule_stream* s, const rpl_rescan_settings* settings /* [n_streams] */,
+                                          const uint8_t* stream_mask /* nullable: all */);
+/* The session form: one re-gridded LaserScan per projected cloud.
+ *   Definition: slot i has a message iff rpl_capsule_stream_laserscan_msgs with the same scan_params gives it one and
+ *            stream s's entry is enabled; that message is Q(entry s, the cloud rpl_capsule_stream_scan_cloud_msgs
+ *            (scan_params, cloud_params) gives slot i).  cloud_params is checked as scan_cloud_msgs checks it; its
+ *            channel bits do not change the result, RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS does.
+ *   Packing, capacity, alignment, _dev and host: those of rpl_capsule_stream_scan_cloud_msgs[_dev], exact and all or
+ *            nothing; a stream's message size is fixed by its entry and its header: header + 36 + 4 * ranges_size.
+ *   Errors:  the errors of scan_cloud_msgs, and a call before the first set_rescans: RPL_RESULT_INVALID_DATA.
+ *   Cost:    the session's message work block holds every slot's LaserScan (8 bytes per node of max_nodes).  Each slot's
+ *            grid is built in 32 KB of shared memory.  No state is kept between calls. */
+rpl_result rpl_capsule_stream_rescan_msgs_dev(rpl_capsule_stream* s, const rpl_scan_params* scan_params,
+                                              const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
+                                              uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,
+                                              uint32_t* msg_sizes, uint64_t* total_bytes, void* stream);
+rpl_result rpl_capsule_stream_rescan_msgs(rpl_capsule_stream* s, const rpl_scan_params* scan_params,
+                                          const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
+                                          uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
+                                          uint64_t* total_bytes);
+
 /* ---- LaserScan / PointCloud2 -> wire (SURVEY.md 8(f) rank 3) ---------------------------- */
 /* The serialised message the RMW layer would produce from the message the reference publishes
  * (scan_pub_->publish, reference src/rplidar_node.cpp:679): XCDR1 little endian, 4-byte

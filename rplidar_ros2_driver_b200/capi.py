@@ -8,6 +8,7 @@ There is no CPU path.
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 import subprocess
 
@@ -74,6 +75,8 @@ EXPORTS = [
     "rpl_scan_cloud_batch_dev", "rpl_capsule_stream_scan_cloud_msgs", "rpl_capsule_stream_scan_cloud_msgs_dev",
     "rpl_capsule_stream_push_scan_cloud_msgs", "rpl_capsule_stream_push_scan_cloud_msgs_dev",
     "rpl_capsule_stream_set_scan_cloud_transforms", "rpl_scan_cloud_transform_batch_dev",
+    "rpl_rescan_batch_dev", "rpl_capsule_stream_set_rescans", "rpl_capsule_stream_rescan_msgs",
+    "rpl_capsule_stream_rescan_msgs_dev",
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -192,6 +195,15 @@ class ScanCloudTransform(C.Structure):
     defines what it does."""
     _fields_ = [("translation", C.c_double * 3), ("rotation", C.c_double * 4), ("enabled", C.c_uint8),
                 ("pad", C.c_uint8 * 7)]
+
+
+class RescanSettings(C.Structure):
+    """rpl_rescan_settings: one stream's re-gridded LaserScan, pointcloud_to_laserscan's parameters (40 bytes).
+    oracle/rescan_oracle.py defines what it does."""
+    _fields_ = [("angle_min", C.c_float), ("angle_max", C.c_float), ("angle_increment", C.c_float),
+                ("range_min", C.c_float), ("range_max", C.c_float), ("min_height", C.c_float),
+                ("max_height", C.c_float), ("inf_epsilon", C.c_float), ("scan_time", C.c_float),
+                ("use_inf", C.c_uint8), ("enabled", C.c_uint8), ("pad", C.c_uint8 * 2)]
 
 
 # rpl_stream_counters: one stream session stream's counters (include/rpl_b200.h)
@@ -338,6 +350,14 @@ def lib() -> C.CDLL:
             ([vp, C.POINTER(ScanCloudParams), C.POINTER(ScanCloudTransform), vp, vp, vp, vp, vp, C.c_float, C.c_float,
               u32, u32, vp, vp, vp], u32),
         "rpl_capsule_stream_set_scan_cloud_transforms": ([vp, vp, vp, vp], u32),
+        "rpl_rescan_batch_dev":
+            ([vp, C.POINTER(RescanSettings), C.POINTER(ScanCloudParams), C.POINTER(ScanCloudTransform), vp, vp, vp, vp,
+              C.c_float, C.c_float, u32, u32, vp, vp], u32),
+        "rpl_capsule_stream_set_rescans": ([vp, vp, vp], u32),
+        "rpl_capsule_stream_rescan_msgs":
+            ([vp, PSP, C.POINTER(ScanCloudParams), C.c_int64, vp, u64, vp, vp, vp], u32),
+        "rpl_capsule_stream_rescan_msgs_dev":
+            ([vp, PSP, C.POINTER(ScanCloudParams), C.c_int64, vp, u64, vp, vp, vp, vp], u32),
         "rpl_capsule_stream_scan_cloud_msgs":
             ([vp, PSP, C.POINTER(ScanCloudParams), C.c_int64, vp, u64, vp, vp, vp], u32),
         "rpl_capsule_stream_scan_cloud_msgs_dev":
@@ -443,6 +463,28 @@ def scan_cloud_transform(translation=(0.0, 0.0, 0.0), rotation=(0.0, 0.0, 0.0, 1
     return ScanCloudTransform((C.c_double * 3)(*(float(v) for v in translation)),
                               (C.c_double * 4)(*(float(v) for v in rotation)), int(bool(enabled)),
                               (C.c_uint8 * 7)())
+
+
+FLT_MAX = float(np.finfo(np.float32).max)
+RESCAN_MAX_BINS = 8192
+
+
+def rescan_settings(angle_min=-math.pi, angle_max=math.pi, angle_increment=math.pi / 180.0, range_min=0.0,
+                    range_max=FLT_MAX, min_height=-FLT_MAX, max_height=FLT_MAX, use_inf=True, inf_epsilon=1.0,
+                    scan_time=1.0 / 30.0, enabled=True) -> RescanSettings:
+    """pointcloud_to_laserscan's defaults for the angular grid, use_inf, inf_epsilon and scan_time; the range window
+    and the height band default to everything a float holds (the package's double limits do not fit a float)."""
+    return RescanSettings(float(angle_min), float(angle_max), float(angle_increment), float(range_min),
+                          float(range_max), float(min_height), float(max_height), float(inf_epsilon),
+                          float(scan_time), int(bool(use_inf)), int(bool(enabled)), (C.c_uint8 * 2)())
+
+
+def rescan_ranges_size(settings: RescanSettings) -> int:
+    """ranges_size of an entry: ceil(fl32(fl32(angle_max - angle_min) / angle_increment)) (0 outside [1, 8192])"""
+    f = np.float32
+    with np.errstate(all="ignore"):
+        q = np.ceil(f(f(f(settings.angle_max) - f(settings.angle_min)) / f(settings.angle_increment)))
+    return int(q) if 1 <= q <= RESCAN_MAX_BINS else 0
 
 
 def _timing(t):
@@ -817,6 +859,16 @@ class Context:
             _p(intensities), _p(beam_counts), _p(angle_increment), _p(time_increment), float(range_min),
             float(range_max), n_scans, stride, _p(points), _p(point_counts), _p(stream)))
 
+    def rescan_batch_dev(self, settings: RescanSettings, cloud_params: ScanCloudParams,
+                         transform: "ScanCloudTransform | None", ranges, intensities, beam_counts, angle_increment,
+                         range_min, range_max, n_scans, stride, out_ranges, stream=None):
+        """The LaserScan re-gridded from the cloud scan_cloud_transform_batch_dev gives each row (device addresses;
+        out_ranges [n_scans][rescan_ranges_size(settings)] float32; intensities may be None)."""
+        self._check(self._L.rpl_rescan_batch_dev(
+            self._h, C.byref(settings), C.byref(cloud_params), C.byref(transform) if transform is not None else None,
+            _p(ranges), _p(intensities), _p(beam_counts), _p(angle_increment), float(range_min), float(range_max),
+            n_scans, stride, _p(out_ranges), _p(stream)))
+
     def cloud_fuse_dev(self, xyzi, point_counts, n_scans, stride, fused, offsets, total, stream=None):
         self._check(self._L.rpl_cloud_fuse_dev(self._h, _p(xyzi), _p(point_counts), n_scans, stride, _p(fused),
                                                _p(offsets), _p(total), _p(stream)))
@@ -993,6 +1045,15 @@ class CapsuleStreamSession:
         self._ctx._check(self._fn("set_scan_cloud_transforms")(self._h, C.cast(arr, C.c_void_p),
                                                                 C.cast(names, C.c_void_p), _p(m)))
 
+    def set_rescans(self, settings, mask=None):
+        """Per stream the re-gridded LaserScan (n_streams RescanSettings, see rescan_settings) that rescan_msgs[_dev]
+        publish.  Only the entries where mask is true are copied (None: all); the first call must set every stream."""
+        assert len(settings) == self.n_streams
+        arr = (RescanSettings * self.n_streams)(*settings)
+        m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
+        assert m is None or m.shape == (self.n_streams,)
+        self._ctx._check(self._fn("set_rescans")(self._h, C.cast(arr, C.c_void_p), _p(m)))
+
     def _msgs(self, name, params, clock_offset_ns, msgs, packed, cloud_params=None):
         ns = self.n_streams * self.max_scans
         if msgs is None:  # room for every slot's largest message
@@ -1000,6 +1061,8 @@ class CapsuleStreamSession:
                 per = 288 + 32 + 8 * self.max_nodes + 4
             elif name == "scan_cloud_msgs":
                 per = _scan_cloud_bound(cloud_params.channels, self.max_nodes)
+            elif name == "rescan_msgs":
+                per = 288 + 36 + 4 * RESCAN_MAX_BINS
             else:
                 per = 288 + 116 + 16 * self.max_nodes + 1
             msgs = np.zeros(ns * ((per + 15) // 16 * 16), np.uint8)
@@ -1035,6 +1098,19 @@ class CapsuleStreamSession:
                             msg_offsets, msg_sizes, total_bytes, stream=None):
         """Device addresses, as laserscan_msgs_dev."""
         self._ctx._check(self._fn("scan_cloud_msgs_dev")(
+            self._h, C.byref(params), C.byref(cloud_params), int(clock_offset_ns), _p(msgs), int(capacity),
+            _p(msg_offsets), _p(msg_sizes), _p(total_bytes), _p(stream)))
+
+    def rescan_msgs(self, params: ScanParams, cloud_params: ScanCloudParams, clock_offset_ns=0, msgs=None,
+                    packed=False):
+        """The serialised sensor_msgs/LaserScan re-gridded (pointcloud_to_laserscan, with each stream's set_rescans
+        entry) from every cloud scan_cloud_msgs(params, cloud_params) gives, as laserscan_msgs returns them."""
+        return self._msgs("rescan_msgs", params, clock_offset_ns, msgs, packed, cloud_params)
+
+    def rescan_msgs_dev(self, params: ScanParams, cloud_params: ScanCloudParams, clock_offset_ns, msgs, capacity,
+                        msg_offsets, msg_sizes, total_bytes, stream=None):
+        """Device addresses, as laserscan_msgs_dev."""
+        self._ctx._check(self._fn("rescan_msgs_dev")(
             self._h, C.byref(params), C.byref(cloud_params), int(clock_offset_ns), _p(msgs), int(capacity),
             _p(msg_offsets), _p(msg_sizes), _p(total_bytes), _p(stream)))
 

@@ -112,6 +112,10 @@ __global__ void __launch_bounds__(MT) msg_table_kernel(MsgTableArgs a) {
     const uint32_t n = a.counts[i];
     if (a.kind == MsgKind::kScanCloud)
       return a.beams[i] > 0 ? a.hdr[i / a.max_scans].bytes + a.tail_bytes + a.point_step * n + 1 : 0u;
+    if (a.kind == MsgKind::kRescan) {
+      const uint32_t b = a.bins[i / a.max_scans];
+      return n > 0 && b > 0 ? a.hdr[i / a.max_scans].bytes + 36 + 4 * b : 0u;
+    }
     const bool has = a.kind == MsgKind::kLaserScan
                          ? n > 0
                          : a.views[i].y > 0 && !(a.clouds && a.clouds[i / a.max_scans].route == kCloudOff);

@@ -66,8 +66,9 @@ struct CloudTail {
   uint32_t at_width, at_row_step, at_data;  // word indices patched per message
 };
 
-// kScanCloud: the projection of each slot's LaserScan (scan_cloud.cu), a PointCloud2 of point_step-byte records
-enum class MsgKind : uint32_t { kLaserScan, kPointCloud2, kScanCloud };
+// kScanCloud: the projection of each slot's LaserScan (scan_cloud.cu), a PointCloud2 of point_step-byte records;
+// kRescan: the LaserScan re-gridded from that projection (rescan.cu), of its stream's fixed beam count
+enum class MsgKind : uint32_t { kLaserScan, kPointCloud2, kScanCloud, kRescan };
 
 // sizes and offsets pass: one CTA over every slot
 struct MsgTableArgs {
@@ -85,6 +86,9 @@ struct MsgTableArgs {
   // counts[i] + 1 (is_dense) bytes
   const uint32_t* beams;
   uint32_t tail_bytes, point_step;
+  // kRescan (counts: the LaserScans' beams): a slot has a message iff its LaserScan has beams and its stream's bins[s]
+  // (the entry's ranges_size, 0 for a disabled entry) is > 0, of header + 36 + 4 * bins[s] bytes
+  const uint32_t* bins;
 };
 
 // the writers, over slots [slot0, slot0 + n) (slot indices count from the first slot of the call)

@@ -20,6 +20,7 @@
 #include "cloud_footprint_args.h"
 #include "cdr_args.h"
 #include "decode_args.h"
+#include "rescan_args.h"
 #include "scan_args.h"
 #include "scan_cloud_args.h"
 #include "scan_filter_args.h"
@@ -708,6 +709,13 @@ static_assert(sizeof(rpl_scan_cloud_transform) == 64 && offsetof(rpl_scan_cloud_
                   RPL_SCAN_CLOUD_VIEWPOINT == rpl::kScanCloudViewpoint &&
                   RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS == rpl::kScanCloudPerStreamTransforms,
               "rpl_scan_cloud_transform and the transform bits are the header's");
+static_assert(sizeof(rpl_rescan_settings) == 40 && offsetof(rpl_rescan_settings, angle_max) == 4 &&
+                  offsetof(rpl_rescan_settings, angle_increment) == 8 && offsetof(rpl_rescan_settings, range_min) == 12 &&
+                  offsetof(rpl_rescan_settings, range_max) == 16 && offsetof(rpl_rescan_settings, min_height) == 20 &&
+                  offsetof(rpl_rescan_settings, max_height) == 24 && offsetof(rpl_rescan_settings, inf_epsilon) == 28 &&
+                  offsetof(rpl_rescan_settings, scan_time) == 32 && offsetof(rpl_rescan_settings, use_inf) == 36 &&
+                  offsetof(rpl_rescan_settings, enabled) == 37,
+              "rpl_rescan_settings is the header's");
 static_assert(sizeof(rpl_msgs_out) == 40 && offsetof(rpl_msgs_out, capacity) == 8 &&
                   offsetof(rpl_msgs_out, msg_offsets) == 16 && offsetof(rpl_msgs_out, msg_sizes) == 24 &&
                   offsetof(rpl_msgs_out, total_bytes) == 32,
@@ -915,6 +923,97 @@ rpl_result rpl_scan_cloud_batch_dev(rpl_ctx* c, const rpl_scan_cloud_params* par
   return rpl_scan_cloud_transform_batch_dev(c, params, nullptr, ranges, intensities, beam_counts, angle_increment,
                                             time_increment, range_min, range_max, n_scans, stride, points,
                                             point_counts, stream);
+}
+
+namespace {
+
+// ranges_size of an entry: ceil(fl32(fl32(angle_max - angle_min) / angle_increment)), the package's float arithmetic
+// (oracle/rescan_oracle.py ranges_size); 0 when it is not a count
+uint32_t rescan_bins(const rpl_rescan_settings& e) {
+  const float q = std::ceil((e.angle_max - e.angle_min) / e.angle_increment);
+  return q >= 1.0f && q <= (float)rpl::kRescanMaxBins ? (uint32_t)q : 0u;
+}
+
+// the limits of an entry (oracle/rescan_oracle.py settings_ok)
+bool rescan_ok(rpl_ctx* c, const rpl_rescan_settings& e) {
+  const float v[9] = {e.angle_min, e.angle_max, e.angle_increment, e.range_min, e.range_max,
+                      e.min_height, e.max_height, e.inf_epsilon, e.scan_time};
+  const char* why = nullptr;
+  if (!std::all_of(v, v + 9, [](float f) { return std::isfinite(f); })) why = "a rescan entry's floats must be finite";
+  else if (!(e.angle_increment > 0.0f) || !(e.angle_min < e.angle_max))
+    why = "a rescan entry needs angle_increment > 0 and angle_min < angle_max";
+  else if (rescan_bins(e) == 0) why = "a rescan entry's ranges_size must be in [1, 8192]";
+  else if (!(0.0f <= e.range_min && e.range_min <= e.range_max)) why = "a rescan entry needs 0 <= range_min <= range_max";
+  else if (!(e.min_height <= e.max_height)) why = "a rescan entry needs min_height <= max_height";
+  else if (!(e.inf_epsilon >= 0.0f)) why = "a rescan entry needs inf_epsilon >= 0";
+  if (why) c->err = why;
+  return why == nullptr;
+}
+
+// an entry as rescan_kernel reads it (a disabled one: no bins, no message)
+rpl::RescanGrid rescan_grid(const rpl_rescan_settings& e, bool use_enabled) {
+  rpl::RescanGrid g{};
+  if (use_enabled && !e.enabled) return g;
+  g.angle_min = e.angle_min;
+  g.angle_max = e.angle_max;
+  g.angle_increment = e.angle_increment;
+  g.range_min = e.range_min;
+  g.range_max = e.range_max;
+  g.min_height = e.min_height;
+  g.max_height = e.max_height;
+  g.scan_time = e.scan_time;
+  const float seed = e.use_inf ? INFINITY : (float)((double)e.range_max + (double)e.inf_epsilon);
+  std::memcpy(&g.seed, &seed, 4);
+  g.bins = rescan_bins(e);
+  return g;
+}
+
+}  // namespace
+
+rpl_result rpl_rescan_batch_dev(rpl_ctx* c, const rpl_rescan_settings* settings,
+                                const rpl_scan_cloud_params* cloud_params, const rpl_scan_cloud_transform* transform,
+                                const float* ranges, const float* intensities, const uint32_t* beam_counts,
+                                const float* angle_increment, float range_min, float range_max, uint32_t n_scans,
+                                uint32_t stride, float* out_ranges, void* stream) {
+  if (!c) return RPL_RESULT_INVALID_DATA;
+  if (!settings || !cloud_params || !ranges || !beam_counts || !angle_increment || !out_ranges) {
+    c->err = "null settings, cloud_params, ranges, beam_counts, angle_increment or out_ranges";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  if (!rescan_ok(c, *settings)) return RPL_RESULT_INVALID_DATA;
+  if (!scan_cloud_ok(c, *cloud_params, transform ? rpl::kScanCloudViewpoint : 0u)) return RPL_RESULT_INVALID_DATA;
+  if (transform && transform->enabled && !scan_cloud_transform_ok(c, *transform, nullptr, false))
+    return RPL_RESULT_INVALID_DATA;
+  if (n_scans != 0 && (stride == 0 || stride > c->max_nodes)) {
+    c->err = "stride must be in [1, the context's max_nodes]";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  if (reinterpret_cast<uintptr_t>(out_ranges) & 3u) {
+    c->err = "out_ranges must be 4-byte aligned";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
+  if (n_scans == 0) return RPL_RESULT_OK;
+  rpl::RescanArgs a{};
+  a.c.channels = cloud_params->channels;
+  a.c.range_cutoff = cloud_params->range_cutoff;
+  a.c.m.counts = beam_counts;
+  a.c.m.ranges = ranges;
+  a.c.m.angle_increment = angle_increment;
+  a.c.m.stride = stride;
+  a.c.m.n = n_scans;
+  a.c.range_min = range_min;
+  a.c.range_max = range_max;
+  if (transform) {
+    a.c.transform = 1;
+    scan_cloud_rows(*transform, a.c.xf_one);
+  }
+  a.grid_one = rescan_grid(*settings, false);
+  a.out = out_ranges;
+  RPL_CUDA(c, rpl::launch_rescan(a, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+  c->launches++;
+  return RPL_RESULT_OK;
 }
 
 // ---- host-buffer batch: chunked over the two lanes so that the H2D copy of chunk i+1, the
@@ -1715,6 +1814,11 @@ struct rpl_capsule_stream {
   float4* xf = nullptr;                         // [n_streams][3] device
   rpl::StreamMsgHeader* xf_hdr = nullptr;       // [n_streams] device
   std::vector<rpl::StreamMsgHeader> xf_hdr_host;
+  // the re-gridded scans' entries (rpl_capsule_stream_set_rescans) as set (empty until the first call sets every
+  // stream), as rescan_kernel reads them, and their ranges_size (0: disabled), which sizes the messages
+  std::vector<rpl_rescan_settings> rescan_host;
+  rpl::RescanGrid* rescan = nullptr;            // [n_streams] device
+  uint32_t* rescan_bins = nullptr;              // [n_streams] device
   unsigned char* node_work = nullptr;           // the tables of a nodes call (NodeWork)
   // [n_streams] device, zeroed at create: what every push decoded and lost (rpl_capsule_stream_counters); a stream's
   // record is written by the one CTA of each kernel that serves the stream
@@ -3351,6 +3455,46 @@ rpl_result stream_set_scan_cloud_transforms(rpl_capsule_stream* cs, const rpl_sc
   return RPL_RESULT_OK;
 }
 
+// the re-gridded scans' entries: the masked entries of `settings` replace the table's, all or none
+rpl_result stream_set_rescans(rpl_capsule_stream* cs, const rpl_rescan_settings* settings, const uint8_t* stream_mask) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!settings) {
+    c->err = "null settings";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  std::vector<rpl_rescan_settings> t = cs->rescan_host;
+  if (t.empty()) {
+    for (uint32_t s = 0; s < cs->n_streams; ++s)
+      if (stream_mask && !stream_mask[s]) {
+        c->err = "the first rpl_capsule_stream_set_rescans call must set every stream";
+        return RPL_RESULT_INVALID_DATA;
+      }
+    t.resize(cs->n_streams);
+  }
+  for (uint32_t s = 0; s < cs->n_streams; ++s) {
+    if (stream_mask && !stream_mask[s]) continue;
+    if (settings[s].enabled && !rescan_ok(c, settings[s])) return RPL_RESULT_INVALID_DATA;
+    t[s] = settings[s];
+  }
+  std::vector<rpl::RescanGrid> g(cs->n_streams);
+  std::vector<uint32_t> bins(cs->n_streams);
+  for (uint32_t s = 0; s < cs->n_streams; ++s) {
+    g[s] = rescan_grid(t[s], true);
+    bins[s] = g[s].bins;
+  }
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  if (!cs->rescan) RPL_CUDA(c, dev_alloc(&cs->rescan, cs->n_streams), RPL_RESULT_INSUFFICIENT_MEMORY);
+  if (!cs->rescan_bins) RPL_CUDA(c, dev_alloc(&cs->rescan_bins, cs->n_streams), RPL_RESULT_INSUFFICIENT_MEMORY);
+  RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);  // a messages call may still read them
+  RPL_CUDA(c, cudaMemcpy(cs->rescan, g.data(), g.size() * sizeof(rpl::RescanGrid), cudaMemcpyHostToDevice),
+           RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaMemcpy(cs->rescan_bins, bins.data(), bins.size() * 4, cudaMemcpyHostToDevice),
+           RPL_RESULT_OPERATION_FAIL);
+  cs->rescan_host = std::move(t);
+  return RPL_RESULT_OK;
+}
+
 rpl_result stream_set_frames(rpl_capsule_stream* cs, const char* const* frame_ids, const float* range_max) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
   rpl_ctx* c = cs->c;
@@ -3543,21 +3687,22 @@ MsgWork msg_work_layout(const rpl_capsule_stream* cs, rpl::MsgKind kind, bool ta
                  k.take<unsigned long long>(tables ? 1 : 0), k.take<uint32_t>(kind == rpl::MsgKind::kScanCloud ? NS : 0)};
 }
 
-// the params of a kScanCloud messages call
+// the params of a kScanCloud or kRescan messages call
 struct ScanCloudCall {
   const rpl_scan_params* scan;
   const rpl_scan_cloud_params* cloud;
 };
 
-// a kScanCloud messages call with RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS
+// a kScanCloud or kRescan messages call with RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS
 bool scan_cloud_transforms(const void* params) {
   return (static_cast<const ScanCloudCall*>(params)->cloud->channels & rpl::kScanCloudPerStreamTransforms) != 0;
 }
 
-// the LaserScan params of a messages call (kLaserScan, kScanCloud), nullptr for kPointCloud2
+// the LaserScan params of a messages call (kLaserScan, kScanCloud, kRescan), nullptr for kPointCloud2
 const rpl_scan_params* msgs_scan_params(rpl::MsgKind kind, const void* params) {
   if (kind == rpl::MsgKind::kLaserScan) return static_cast<const rpl_scan_params*>(params);
-  if (kind == rpl::MsgKind::kScanCloud) return static_cast<const ScanCloudCall*>(params)->scan;
+  if (kind == rpl::MsgKind::kScanCloud || kind == rpl::MsgKind::kRescan)
+    return static_cast<const ScanCloudCall*>(params)->scan;
   return nullptr;
 }
 
@@ -3582,13 +3727,17 @@ bool stream_msgs_args_ok(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* 
   }
   if (kind == rpl::MsgKind::kPointCloud2 && !cloud_call_ok(cs, static_cast<const rpl_cloud_params*>(params)))
     return false;
-  if (kind == rpl::MsgKind::kScanCloud) {
+  if (kind == rpl::MsgKind::kScanCloud || kind == rpl::MsgKind::kRescan) {
     const auto* q = static_cast<const ScanCloudCall*>(params);
     if (!q->scan || !q->cloud) {
       c->err = "null scan_params or cloud_params";
       return false;
     }
     if (!scan_cloud_call_ok(cs, *q->cloud)) return false;
+    if (kind == rpl::MsgKind::kRescan && cs->rescan_host.empty()) {
+      c->err = "rescan_msgs before the first rpl_capsule_stream_set_rescans";
+      return false;
+    }
   }
   const rpl_scan_params* sp = msgs_scan_params(kind, params);
   const bool per_stream = sp ? (sp->flags & RPL_FLAG_PER_STREAM) != 0
@@ -3607,8 +3756,8 @@ bool stream_msgs_args_ok(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* 
   return true;
 }
 
-// the projection of every slot's LaserScan in w (kScanCloud): the count pass's arguments over all slots (msgs_write
-// adds the placement)
+// the projection of every slot's LaserScan in w (kScanCloud, kRescan): the count pass's arguments over all slots
+// (msgs_write adds the placement)
 rpl::ScanCloudArgs scan_cloud_msg_args(const rpl_capsule_stream* cs, const void* params, const MsgWork& w) {
   const auto* q = static_cast<const ScanCloudCall*>(params);
   const size_t NS = (size_t)cs->n_streams * cs->max_scans;
@@ -3671,8 +3820,11 @@ rpl_result msgs_prepare(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* p
     t.tail_bytes = a.transform ? a.tail_xf.bytes : a.tail.bytes;
     t.point_step = a.point_step;
   }
+  if (kind == rpl::MsgKind::kRescan) t.bins = cs->rescan_bins;  // the LaserScans' beams and the entries size them
   t.kind = kind;
-  t.hdr = kind == rpl::MsgKind::kScanCloud && scan_cloud_transforms(params) ? cs->xf_hdr : cs->msg_hdr;
+  t.hdr = (kind == rpl::MsgKind::kScanCloud || kind == rpl::MsgKind::kRescan) && scan_cloud_transforms(params)
+              ? cs->xf_hdr
+              : cs->msg_hdr;
   t.counts = kind == rpl::MsgKind::kScanCloud ? w.kept : w.counts;
   t.views = reinterpret_cast<const uint2*>(cs->views);
   t.n_slots = (uint32_t)NS;
@@ -3712,6 +3864,22 @@ rpl_result msgs_write(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* par
   a.sizes = sizes;
   a.out = out;
   a.out_base = out_base;
+  if (kind == rpl::MsgKind::kRescan) {  // the projection's LaserScans, transforms and window, with a's stamps and placement
+    rpl::RescanArgs ra{};
+    ra.c = scan_cloud_msg_args(cs, params, w);
+    ra.c.m.slot0 = slot0;
+    ra.c.m.n = n;
+    ra.c.m.begin_us = a.begin_us;
+    ra.c.m.clock_offset_ns = clock_offset_ns;
+    ra.c.m.offsets = offsets;
+    ra.c.m.sizes = sizes;
+    ra.c.m.out = out;
+    ra.c.m.out_base = out_base;
+    ra.grid = cs->rescan;
+    RPL_CUDA(c, rpl::launch_rescan(ra, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+    c->launches++;
+    return RPL_RESULT_OK;
+  }
   if (kind == rpl::MsgKind::kScanCloud) {  // the count pass's LaserScans and settings, with a's stamps and placement
     rpl::ScanCloudArgs sa = scan_cloud_msg_args(cs, params, w);
     sa.m.slot0 = slot0;
@@ -4245,6 +4413,8 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   cudaFree(cs->push_scan_cloud_work);
   cudaFree(cs->xf);
   cudaFree(cs->xf_hdr);
+  cudaFree(cs->rescan);
+  cudaFree(cs->rescan_bins);
   cudaFreeHost(cs->push_scan_cloud_extent);
   if (cs->push_scan_cloud_dir_order) cudaEventDestroy(cs->push_scan_cloud_dir_order);
   if (cs->done) cudaEventDestroy(cs->done);
@@ -4845,6 +5015,29 @@ rpl_result rpl_capsule_stream_scan_cloud_msgs(rpl_capsule_stream* s, const rpl_s
                                               uint32_t* msg_sizes, uint64_t* total_bytes) {
   const ScanCloudCall q{scan_params, cloud_params};
   return stream_msgs(s, rpl::MsgKind::kScanCloud, &q, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
+                     total_bytes);
+}
+
+rpl_result rpl_capsule_stream_set_rescans(rpl_capsule_stream* s, const rpl_rescan_settings* settings,
+                                          const uint8_t* stream_mask) {
+  return stream_set_rescans(s, settings, stream_mask);
+}
+
+rpl_result rpl_capsule_stream_rescan_msgs_dev(rpl_capsule_stream* s, const rpl_scan_params* scan_params,
+                                              const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
+                                              uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,
+                                              uint32_t* msg_sizes, uint64_t* total_bytes, void* stream) {
+  const ScanCloudCall q{scan_params, cloud_params};
+  return stream_msgs_dev(s, rpl::MsgKind::kRescan, &q, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
+                         total_bytes, stream);
+}
+
+rpl_result rpl_capsule_stream_rescan_msgs(rpl_capsule_stream* s, const rpl_scan_params* scan_params,
+                                          const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
+                                          uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
+                                          uint64_t* total_bytes) {
+  const ScanCloudCall q{scan_params, cloud_params};
+  return stream_msgs(s, rpl::MsgKind::kRescan, &q, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
                      total_bytes);
 }
 

@@ -17,37 +17,12 @@
 #include "beam_point.cuh"
 #include "msg_fixed.cuh"
 #include "scan_cloud_args.h"
+#include "scan_cloud_point.cuh"
 
 namespace rpl {
 namespace {
 
 constexpr int ST = 256;
-
-__device__ __forceinline__ bool keep_beam(float r, float range_min, float cutoff) {
-  return r >= range_min && r < cutoff;  // NaN never, +inf never (cutoff <= +inf)
-}
-
-// the window of slot i: a session's LaserScan range_min and its stream's range_max, or the call's; the cutoff
-__device__ __forceinline__ void slot_window(const ScanCloudArgs& a, uint32_t i, float* lo, float* cut) {
-  const float hi = a.m.hdr ? a.m.hdr[i / a.m.max_scans].range_max : a.range_max;
-  *lo = a.m.hdr ? kLaserScanRangeMin : a.range_min;
-  *cut = a.range_cutoff >= 0.0f ? a.range_cutoff : hi;
-}
-
-// slot i's beams: its row, or its placed LaserScan message (a push's, 4-byte aligned: the loads stay 4-byte)
-struct SlotBeams {
-  uint32_t M;
-  const float *rg, *ig;
-};
-__device__ __forceinline__ SlotBeams slot_beams(const ScanCloudArgs& a, uint32_t i) {
-  if (!a.scan_msgs)
-    return SlotBeams{min(a.m.counts[i], a.m.stride), a.m.ranges + (size_t)i * a.m.stride,
-                     a.m.intensities + (size_t)i * a.m.stride};
-  if (a.scan_sizes[i] == 0) return SlotBeams{0u, nullptr, nullptr};
-  const uint32_t M = a.m.counts[i];
-  const float* rg = reinterpret_cast<const float*>(a.scan_msgs + a.place[i]);
-  return SlotBeams{M, rg, rg + M + 1};  // the intensities follow the ranges and their count
-}
 
 __global__ void __launch_bounds__(ST) scan_cloud_count_kernel(const __grid_constant__ ScanCloudArgs a) {
   for (uint32_t s = blockIdx.x; s < a.m.n; s += gridDim.x) {
@@ -154,11 +129,9 @@ __global__ void __launch_bounds__(ST, kXf ? kXfBlocks : 8) scan_cloud_kernel(con
         float x, y;
         beam_point(j, inc, r, &x, &y);
         if constexpr (kXf) {
-          if (xr[0].w != 0.0f) {  // p_target = R p + t, z = 0: no R_k2 term, no FMA
+          if (xr[0].w != 0.0f) {
             float X[3];
-#pragma unroll
-            for (int k = 0; k < 3; ++k)
-              X[k] = __fadd_rn(__fadd_rn(__fmul_rn(xr[k].x, x), __fmul_rn(xr[k].y, y)), xr[k].z);
+            target_point(xr, x, y, X);
             p[0] = __float_as_uint(X[0]);
             p[1] = __float_as_uint(X[1]);
             p[2] = __float_as_uint(X[2]);

@@ -596,7 +596,9 @@ rpl_result rpl_capsule_stream_counters(rpl_capsule_stream* s, rpl_stream_counter
  *   Definition: push P1..Pk of a stream into session A, export it, import the record into a session B of the same
  *            kind (framed or byte) and max_nodes whose stream has the same settings, push P(k+1)..Pn into B: A's
  *            outputs up to k followed by B's are bit for bit those of one session fed P1..Pn, in every output of every
- *            call (scans, stamps, state, nodes, clouds, messages) and every counter but scans_unreturned.
+ *            call (scans, stamps, state, nodes, clouds, messages) and every counter but scans_unreturned -- with one
+ *            exception: records do not carry the windows over the re-gridded scans, so the outputs of
+ *            push_rescan_msgs[_dev] on a stream with observations >= 2 restart their window at the import.
  *   Record:  little-endian bytes, version RPL_STREAM_RECORD_VERSION: a 32-byte header (uint32 magic "RPLM", version,
  *            kind 0 framed / 1 byte session, answer type, max_nodes, open length L, stamp flags, 0), the 192-byte held
  *            record, for a capsule answer type in a byte session the 800-byte framer record, the open revolution's
@@ -1331,7 +1333,8 @@ rpl_result rpl_capsule_stream_set_rescans(rpl_capsule_stream* s, const rpl_resca
  *            nothing; a stream's message size is fixed by its entry and its header: header + 36 + 4 * ranges_size.
  *   Errors:  the errors of scan_cloud_msgs, and a call before the first set_rescans: RPL_RESULT_INVALID_DATA.
  *   Cost:    the session's message work block holds every slot's LaserScan (8 bytes per node of max_nodes).  Each slot's
- *            grid is built in 32 KB of shared memory.  No state is kept between calls. */
+ *            grid is built in 32 KB of shared memory.  No state is kept between calls: the windows below belong to the
+ *            push form alone. */
 rpl_result rpl_capsule_stream_rescan_msgs_dev(rpl_capsule_stream* s, const rpl_scan_params* scan_params,
                                               const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
                                               uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets,
@@ -1340,6 +1343,86 @@ rpl_result rpl_capsule_stream_rescan_msgs(rpl_capsule_stream* s, const rpl_scan_
                                           const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
                                           uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
                                           uint64_t* total_bytes);
+
+/* Windows over the re-gridded scans (DESIGN.md 5.7.1 "Windows over the re-gridded scans"; INTEGRATION.md 4k):
+ * laser_filters' LaserArrayFilter behind the re-grid -- a per-bin median or mean of a stream's last `observations`
+ * re-gridded scans, which removes flicker and single-revolution dropouts -- kept on the device per stream.  W(window,
+ * xs), over the rows xs of one stream's grid oldest first (n = len(xs) <= observations), is defined bit for bit by
+ * oracle/rescan_window_oracle.py:
+ *   median:  per bin, the value of rank (n - 1) / 2 of the n values in ascending order (the lower median for even n).
+ *   mean:    per bin, the float sum from +0.0, oldest to newest, rounded at each step, then fl32(sum / n).
+ *   Re-grid values are never NaN or -0 (finite, +inf, or the entry's seed), so the median is one of the values.
+ *   Limits:  1 <= observations <= 16 (1: no window, the message is Q's), statistic RPL_RESCAN_WINDOW_MEDIAN or
+ *            RPL_RESCAN_WINDOW_MEAN; otherwise RPL_RESULT_INVALID_DATA.
+ * Offsets: observations 0, statistic 4; 8 bytes. */
+#define RPL_RESCAN_WINDOW_MEDIAN 0u
+#define RPL_RESCAN_WINDOW_MEAN 1u
+typedef struct rpl_rescan_window {
+  uint32_t observations; /* offset 0: LaserArrayFilter's number_of_observations, 1..16 */
+  uint32_t statistic;    /* 4: RPL_RESCAN_WINDOW_MEDIAN (MultiChannelMedianFilterFloat) or _MEAN (...MeanFilterFloat) */
+} rpl_rescan_window;     /* 8 bytes */
+/* Stateless: row t of out is W(*window, rows max(0, t - observations + 1) .. t of in), a window that starts empty at row
+ * 0; in and out device arrays [n_scans][bins], 4-byte aligned, 1 <= bins <= 8192.  A null ctx, window, in or out, or a
+ * window or bins outside the limits: RPL_RESULT_INVALID_DATA.  Asynchronous on `stream` (NULL: the context's stream). */
+rpl_result rpl_rescan_window_batch_dev(rpl_ctx* ctx, const rpl_rescan_window* window, const float* in, uint32_t n_scans,
+                                       uint32_t bins, float* out, void* stream);
+/*   set_rescan_windows: the window of every stream, with the rules of set_rescans: synchronous, masked (NULL = all); a
+ *            null windows or a masked entry outside the limits is RPL_RESULT_INVALID_DATA and leaves the table and every
+ *            window unchanged.  Until the first call every stream has observations 1.
+ *   Stream window: stream s's window is the sequence of its raw re-gridded scans (Q's ranges) that qualify, newest
+ *            last.  A revolution qualifies when a push_rescan_msgs[_dev] call returned it, its LaserScan message was
+ *            written (scans->msg_sizes[i] > 0) and s's re-grid entry is enabled.  Nothing else advances it: a revolution
+ *            whose re-grid message did not fit rescans->capacity still enters it, while revolutions other push calls
+ *            return, revolutions beyond max_scans and LaserScans that did not fit scans->capacity are not seen -- a
+ *            downstream filter does not see a dropped message either.  So the window is a function of the input
+ *            history and of which LaserScans the caller received.
+ *   Emptied: stream s's window, by session create; set_rescans or set_rescan_windows with s masked in (the grid may have
+ *            changed, as LaserArrayFilter reconfigures when the range count does); rpl_capsule_stream_reset with s
+ *            masked in; rpl_capsule_stream_import into s (records do not carry windows: the outputs of the push form on
+ *            a stream with observations >= 2 restart their window at the import); and a switch of s's answer type by
+ *            set_answer_types (a fresh session).  A refused set call, or a push that fails its checks, leaves every
+ *            window bit for bit unchanged.
+ *   Memory:  the device ring holds (observations - 1) * ranges_size floats per enabled stream with a window, laid out
+ *            from both tables by either set call, plus a count and a head per stream; the windows of the streams a set
+ *            call does not mask in survive the new layout.  Running out of device memory: RPL_RESULT_INSUFFICIENT_MEMORY,
+ *            and nothing changes. */
+rpl_result rpl_capsule_stream_set_rescan_windows(rpl_capsule_stream* s, const rpl_rescan_window* windows /* [n_streams] */,
+                                                 const uint8_t* stream_mask /* nullable: all */);
+/* LaserScans and their re-gridded scans from the push: one call that pushes `in` and returns the LaserScan messages of
+ * the scans it published and the re-gridded scan of each, windowed per stream.  Each chunk runs the push_laserscan_msgs
+ * chunk, then re-grids every LaserScan message where it lies: the re-grid directory, then rescan_kernel for the streams
+ * with observations 1 and one CTA per stream for the others, which go through the stream's slots in revolution order.
+ *   in, scan_params, cloud_params, clock_offset_ns: as rpl_capsule_stream_push_scan_cloud_msgs.
+ *   Definition: with two sessions of the same history (set calls included), A pushed with push_laserscan_msgs[_dev]
+ *            (in, scan_params) and then took rescan_msgs[_dev] (scan_params, cloud_params, the same clock_offset_ns), B
+ *            with this call: scans and scans_per_stream equal A's push output in every case, capacity cases included;
+ *            slot i has a re-grid message iff its LaserScan message was written and stream s's entry is enabled, of
+ *            header + 36 + 4 * ranges_size bytes; when both totals fit, rescans equals A's rescan_msgs output for every
+ *            stream with observations 1, and for the others every byte but the ranges, which are W(window s, the last
+ *            min(observations, k) entries of s's window) with revolution k the newest -- the message keeps Q's header,
+ *            the newest revolution's stamp, angles and sizes, as LaserArrayFilter republishes its input.  Every later
+ *            call returns on B what it returns on A (this call sets the last push as a push does; rescan_msgs replays
+ *            Q, without windows).  A call that fails its checks leaves the session, windows included, as it was.
+ *   Packing: scans, the bound-based packing of push_laserscan_msgs; rescans, exact, msg_offsets the exclusive scan of
+ *            the sizes each rounded up to 16, carried from chunk to chunk on the device.  A re-grid message is written
+ *            iff its offset + size <= rescans->capacity: the written messages are a prefix.  The host form returns
+ *            RPL_RESULT_INSUFFICIENT_MEMORY when either total exceeds its capacity, the _dev form reports it through the
+ *            totals only; the push itself is done and the windows have advanced either way.
+ *   Errors:  the errors of push_scan_cloud_msgs, and a call before the first set_rescans: RPL_RESULT_INVALID_DATA.
+ *   Cost:    the first call of this kind, or of push_scan_cloud_msgs, keeps 4 bytes per slot and 16 bytes of device
+ *            tables and 48 bytes of pinned host memory, shared by the two; the host form's lanes also stage one host
+ *            chunk's re-grid messages (their bound at the longest header and the largest ranges_size).  A chunk with no
+ *            enabled entry launches no re-grid kernel, and one with no window launches no window kernel. */
+rpl_result rpl_capsule_stream_push_rescan_msgs(rpl_capsule_stream* s, const rpl_push_input* in,
+                                               const rpl_scan_params* scan_params,
+                                               const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
+                                               const rpl_msgs_out* scans, const rpl_msgs_out* rescans,
+                                               uint32_t* scans_per_stream);
+rpl_result rpl_capsule_stream_push_rescan_msgs_dev(rpl_capsule_stream* s, const rpl_push_input* in,
+                                                   const rpl_scan_params* scan_params,
+                                                   const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
+                                                   const rpl_msgs_out* scans, const rpl_msgs_out* rescans,
+                                                   uint32_t* scans_per_stream, void* stream);
 
 /* ---- LaserScan / PointCloud2 -> wire (SURVEY.md 8(f) rank 3) ---------------------------- */
 /* The serialised message the RMW layer would produce from the message the reference publishes

@@ -77,6 +77,8 @@ EXPORTS = [
     "rpl_capsule_stream_set_scan_cloud_transforms", "rpl_scan_cloud_transform_batch_dev",
     "rpl_rescan_batch_dev", "rpl_capsule_stream_set_rescans", "rpl_capsule_stream_rescan_msgs",
     "rpl_capsule_stream_rescan_msgs_dev",
+    "rpl_rescan_window_batch_dev", "rpl_capsule_stream_set_rescan_windows", "rpl_capsule_stream_push_rescan_msgs",
+    "rpl_capsule_stream_push_rescan_msgs_dev",
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -204,6 +206,12 @@ class RescanSettings(C.Structure):
                 ("range_min", C.c_float), ("range_max", C.c_float), ("min_height", C.c_float),
                 ("max_height", C.c_float), ("inf_epsilon", C.c_float), ("scan_time", C.c_float),
                 ("use_inf", C.c_uint8), ("enabled", C.c_uint8), ("pad", C.c_uint8 * 2)]
+
+
+class RescanWindow(C.Structure):
+    """rpl_rescan_window: one stream's window over its re-gridded LaserScans, laser_filters' LaserArrayFilter (8 bytes).
+    oracle/rescan_window_oracle.py defines what it does."""
+    _fields_ = [("observations", C.c_uint32), ("statistic", C.c_uint32)]
 
 
 # rpl_stream_counters: one stream session stream's counters (include/rpl_b200.h)
@@ -380,6 +388,14 @@ def lib() -> C.CDLL:
         "rpl_capsule_stream_push_scan_cloud_msgs_dev":
             ([vp, C.POINTER(PushInput), PSP, C.POINTER(ScanCloudParams), C.c_int64, C.POINTER(MsgsOut),
               C.POINTER(MsgsOut), vp, vp], u32),
+        "rpl_rescan_window_batch_dev": ([vp, C.POINTER(RescanWindow), vp, u32, u32, vp, vp], u32),
+        "rpl_capsule_stream_set_rescan_windows": ([vp, vp, vp], u32),
+        "rpl_capsule_stream_push_rescan_msgs":
+            ([vp, C.POINTER(PushInput), PSP, C.POINTER(ScanCloudParams), C.c_int64, C.POINTER(MsgsOut),
+              C.POINTER(MsgsOut), vp], u32),
+        "rpl_capsule_stream_push_rescan_msgs_dev":
+            ([vp, C.POINTER(PushInput), PSP, C.POINTER(ScanCloudParams), C.c_int64, C.POINTER(MsgsOut),
+              C.POINTER(MsgsOut), vp, vp], u32),
     }
     for name, (args, res) in sig.items():
         fn = getattr(L, name)  # AttributeError here = the library does not export the ABI
@@ -485,6 +501,17 @@ def rescan_ranges_size(settings: RescanSettings) -> int:
     with np.errstate(all="ignore"):
         q = np.ceil(f(f(f(settings.angle_max) - f(settings.angle_min)) / f(settings.angle_increment)))
     return int(q) if 1 <= q <= RESCAN_MAX_BINS else 0
+
+
+RESCAN_WINDOW_MEDIAN, RESCAN_WINDOW_MEAN = 0, 1
+RESCAN_WINDOW_MAX = 16
+
+
+def rescan_window(observations=1, statistic="median") -> RescanWindow:
+    """LaserArrayFilter's number_of_observations and its filter: "median" (MultiChannelMedianFilterFloat) or "mean"
+    (MultiChannelMeanFilterFloat); observations 1 is no window."""
+    stat = {"median": RESCAN_WINDOW_MEDIAN, "mean": RESCAN_WINDOW_MEAN}.get(statistic, statistic)
+    return RescanWindow(int(observations), int(stat))
 
 
 def _timing(t):
@@ -869,6 +896,12 @@ class Context:
             _p(ranges), _p(intensities), _p(beam_counts), _p(angle_increment), float(range_min), float(range_max),
             n_scans, stride, _p(out_ranges), _p(stream)))
 
+    def rescan_window_batch_dev(self, window: RescanWindow, in_ranges, n_scans, bins, out_ranges, stream=None):
+        """Row t of out_ranges is the window's statistic over rows max(0, t - observations + 1) .. t of in_ranges
+        (device addresses, [n_scans][bins] float32 each)."""
+        self._check(self._L.rpl_rescan_window_batch_dev(self._h, C.byref(window), _p(in_ranges), n_scans, bins,
+                                                        _p(out_ranges), _p(stream)))
+
     def cloud_fuse_dev(self, xyzi, point_counts, n_scans, stride, fused, offsets, total, stream=None):
         self._check(self._L.rpl_cloud_fuse_dev(self._h, _p(xyzi), _p(point_counts), n_scans, stride, _p(fused),
                                                _p(offsets), _p(total), _p(stream)))
@@ -1054,6 +1087,16 @@ class CapsuleStreamSession:
         assert m is None or m.shape == (self.n_streams,)
         self._ctx._check(self._fn("set_rescans")(self._h, C.cast(arr, C.c_void_p), _p(m)))
 
+    def set_rescan_windows(self, windows, mask=None):
+        """Per stream the window over the re-gridded LaserScans push_rescan_msgs[_dev] publish (n_streams RescanWindow,
+        see rescan_window).  Only the entries where mask is true are copied (None: all), and their windows start
+        over; until the first call every stream has observations 1."""
+        assert len(windows) == self.n_streams
+        arr = (RescanWindow * self.n_streams)(*windows)
+        m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
+        assert m is None or m.shape == (self.n_streams,)
+        self._ctx._check(self._fn("set_rescan_windows")(self._h, C.cast(arr, C.c_void_p), _p(m)))
+
     def _msgs(self, name, params, clock_offset_ns, msgs, packed, cloud_params=None):
         ns = self.n_streams * self.max_scans
         if msgs is None:  # room for every slot's largest message
@@ -1198,6 +1241,37 @@ class CapsuleStreamSession:
             self._h, C.byref(pi), C.byref(params), int(clock_offset_ns), _p(msgs), int(capacity), _p(msg_offsets),
             _p(msg_sizes), _p(total_bytes), _p(scans_per_stream), _p(stream)))
 
+    def _push_msgs_pair(self, name, second_bytes, data, counts, params, cloud_params, clock_offset_ns,
+                        sample_duration_us, rx_us, timing, chunk_bytes, msgs, second_msgs):
+        """A push returning two packed message sets (entry point `name`): the LaserScans into msgs, the second set into
+        second_msgs; None: a buffer that always fits, second_bytes per slot for the second set."""
+        assert isinstance(data, np.ndarray) and data.dtype == np.uint8 and data.flags.c_contiguous
+        cnt = np.ascontiguousarray(counts, dtype=np.uint32)
+        assert cnt.shape == (self.n_streams,)
+        rx = None if rx_us is None else np.ascontiguousarray(rx_us, dtype=np.uint64)
+        ns = self.n_streams * self.max_scans
+        if msgs is None:
+            msgs = np.zeros(ns * ((288 + 32 + 8 * self.max_nodes + 4 + 15) // 16 * 16), np.uint8)
+        if second_msgs is None:
+            second_msgs = np.zeros(ns * ((second_bytes + 15) // 16 * 16), np.uint8)
+        out = []
+        for buf in (msgs, second_msgs):
+            assert buf.dtype == np.uint8 and buf.flags.c_contiguous
+            t = dict(msgs=buf, msg_offsets=np.zeros(ns, np.uint64), msg_sizes=np.zeros(ns, np.uint32),
+                     total=np.zeros(1, np.uint64))
+            t["out"] = MsgsOut(_p(buf).value, buf.size, _p(t["msg_offsets"]).value, _p(t["msg_sizes"]).value,
+                               _p(t["total"]).value)
+            out.append(t)
+        sps = np.zeros(self.n_streams, np.uint32)
+        pi = self._push_input(data, cnt, sample_duration_us, rx, timing, chunk_bytes)
+        rc = self._fn(name)(self._h, C.byref(pi), C.byref(params), C.byref(cloud_params), int(clock_offset_ns),
+                            C.byref(out[0]["out"]), C.byref(out[1]["out"]), _p(sps))
+        if rc != RESULT_INSUFFICIENT_MEMORY:
+            self._ctx._check(rc)
+        res = [dict(msgs=t["msgs"], msg_offsets=t["msg_offsets"], msg_sizes=t["msg_sizes"],
+                    total_bytes=int(t["total"][0]), result=rc) for t in out]
+        return res[0], res[1], sps
+
     def push_scan_cloud_msgs(self, data, counts, params: ScanParams, cloud_params: ScanCloudParams, clock_offset_ns=0,
                              sample_duration_us=31, rx_us=None, timing: "Timing | None" = None, chunk_bytes=None,
                              msgs=None, cloud_msgs=None):
@@ -1207,34 +1281,9 @@ class CapsuleStreamSession:
         are the capacities; None: ones that always fit).  Returns (scans, clouds, scans_per_stream): scans and clouds
         as the packed dicts of push_laserscan_msgs(packed=True), each with the call's result, which is
         RESULT_INSUFFICIENT_MEMORY rather than an exception when either buffer is too small (the push is done)."""
-        assert isinstance(data, np.ndarray) and data.dtype == np.uint8 and data.flags.c_contiguous
-        cnt = np.ascontiguousarray(counts, dtype=np.uint32)
-        assert cnt.shape == (self.n_streams,)
-        rx = None if rx_us is None else np.ascontiguousarray(rx_us, dtype=np.uint64)
-        ns = self.n_streams * self.max_scans
-        if msgs is None:
-            msgs = np.zeros(ns * ((288 + 32 + 8 * self.max_nodes + 4 + 15) // 16 * 16), np.uint8)
-        if cloud_msgs is None:
-            per = _scan_cloud_bound(cloud_params.channels, self.max_nodes)
-            cloud_msgs = np.zeros(ns * ((per + 15) // 16 * 16), np.uint8)
-        out = []
-        for buf in (msgs, cloud_msgs):
-            assert buf.dtype == np.uint8 and buf.flags.c_contiguous
-            t = dict(msgs=buf, msg_offsets=np.zeros(ns, np.uint64), msg_sizes=np.zeros(ns, np.uint32),
-                     total=np.zeros(1, np.uint64))
-            t["out"] = MsgsOut(_p(buf).value, buf.size, _p(t["msg_offsets"]).value, _p(t["msg_sizes"]).value,
-                               _p(t["total"]).value)
-            out.append(t)
-        sps = np.zeros(self.n_streams, np.uint32)
-        pi = self._push_input(data, cnt, sample_duration_us, rx, timing, chunk_bytes)
-        rc = self._fn("push_scan_cloud_msgs")(self._h, C.byref(pi), C.byref(params), C.byref(cloud_params),
-                                              int(clock_offset_ns), C.byref(out[0]["out"]), C.byref(out[1]["out"]),
-                                              _p(sps))
-        if rc != RESULT_INSUFFICIENT_MEMORY:
-            self._ctx._check(rc)
-        res = [dict(msgs=t["msgs"], msg_offsets=t["msg_offsets"], msg_sizes=t["msg_sizes"],
-                    total_bytes=int(t["total"][0]), result=rc) for t in out]
-        return res[0], res[1], sps
+        return self._push_msgs_pair("push_scan_cloud_msgs", _scan_cloud_bound(cloud_params.channels, self.max_nodes),
+                                    data, counts, params, cloud_params, clock_offset_ns, sample_duration_us, rx_us,
+                                    timing, chunk_bytes, msgs, cloud_msgs)
 
     def push_scan_cloud_msgs_dev(self, data, counts, params: ScanParams, cloud_params: ScanCloudParams,
                                  clock_offset_ns, scans: MsgsOut, clouds: MsgsOut, scans_per_stream,
@@ -1247,6 +1296,26 @@ class CapsuleStreamSession:
         self._ctx._check(self._fn("push_scan_cloud_msgs_dev")(
             self._h, C.byref(pi), C.byref(params), C.byref(cloud_params), int(clock_offset_ns), C.byref(scans),
             C.byref(clouds), _p(scans_per_stream), _p(stream)))
+
+    def push_rescan_msgs(self, data, counts, params: ScanParams, cloud_params: ScanCloudParams, clock_offset_ns=0,
+                         sample_duration_us=31, rx_us=None, timing: "Timing | None" = None, chunk_bytes=None,
+                         msgs=None, rescan_msgs=None):
+        """One push, as push_laserscan_msgs takes it, whose scans come back both as their serialised
+        sensor_msgs/LaserScan and as the LaserScan each re-grids to (rescan_msgs with cloud_params), windowed per
+        stream by set_rescan_windows.  Buffers and returns (scans, rescans, scans_per_stream) as
+        push_scan_cloud_msgs."""
+        return self._push_msgs_pair("push_rescan_msgs", 288 + 36 + 4 * RESCAN_MAX_BINS, data, counts, params,
+                                    cloud_params, clock_offset_ns, sample_duration_us, rx_us, timing, chunk_bytes, msgs,
+                                    rescan_msgs)
+
+    def push_rescan_msgs_dev(self, data, counts, params: ScanParams, cloud_params: ScanCloudParams, clock_offset_ns,
+                             scans: MsgsOut, rescans: MsgsOut, scans_per_stream, sample_duration_us=31, rx_us=None,
+                             timing: "Timing | None" = None, chunk_bytes=None, stream=None):
+        """Device addresses, as push_scan_cloud_msgs_dev."""
+        pi = self._push_input(data, counts, sample_duration_us, rx_us, timing, chunk_bytes)
+        self._ctx._check(self._fn("push_rescan_msgs_dev")(
+            self._h, C.byref(pi), C.byref(params), C.byref(cloud_params), int(clock_offset_ns), C.byref(scans),
+            C.byref(rescans), _p(scans_per_stream), _p(stream)))
 
     def nodes(self, apply_ascend=True, per_stream=None, packed=False, nodes=None):
         """The node buffers RealLidarDriver::grab_scan_data would return for every scan the last push published: per

@@ -243,6 +243,7 @@ __global__ void __launch_bounds__(CT) pointcloud2_msgs_kernel(MsgWriteArgs a, Cl
 // and the total is the end of the last message, carried in carry[1].
 // K = kScanCloud: as kPointCloud2, a slot's exact size at its projection's kept count, for a slot whose LaserScan
 // message the push wrote.
+// K = kRescan: as kScanCloud, a slot's re-gridded message at its stream's fixed bin count.
 template <MsgKind K>
 __global__ void __launch_bounds__(MT) push_msg_dir_kernel(PushMsgDirArgs a) {
   constexpr bool kCloud = K != MsgKind::kLaserScan;
@@ -265,6 +266,8 @@ __global__ void __launch_bounds__(MT) push_msg_dir_kernel(PushMsgDirArgs a) {
       hb = a.hdr[s].bytes;
       if constexpr (K == MsgKind::kScanCloud) {
         if (a.scan_sizes[i] > 0) bound = hb + a.tail_bytes + a.point_step * a.counts[i] + 1u;
+      } else if constexpr (K == MsgKind::kRescan) {
+        if (a.scan_sizes[i] > 0 && a.counts[s] > 0) bound = hb + 36u + 4u * a.counts[s];
       } else {
         const bool off = kCloud && a.clouds && a.clouds[s].route == kCloudOff;  // a stream without a cloud
         if (k < min(a.scans_per_stream[s], a.max_scans) && !off) {
@@ -336,8 +339,10 @@ cudaError_t launch_push_msg_dir(const PushMsgDirArgs& a, MsgKind kind, cudaStrea
     push_msg_dir_kernel<MsgKind::kLaserScan><<<1, MT, 0, stream>>>(a);
   else if (kind == MsgKind::kPointCloud2)
     push_msg_dir_kernel<MsgKind::kPointCloud2><<<1, MT, 0, stream>>>(a);
-  else
+  else if (kind == MsgKind::kScanCloud)
     push_msg_dir_kernel<MsgKind::kScanCloud><<<1, MT, 0, stream>>>(a);
+  else
+    push_msg_dir_kernel<MsgKind::kRescan><<<1, MT, 0, stream>>>(a);
   return cudaGetLastError();
 }
 

@@ -142,6 +142,9 @@ struct PushMsgDirArgs {
   // (scan_sizes[i] > 0), of header + tail_bytes + point_step * counts[i] (the kept beams) + 1 (is_dense) bytes
   const uint32_t* scan_sizes;
   uint32_t tail_bytes, point_step;
+  // kRescan (sizes, total and carry [2] as PointCloud2): counts is [n_slots / max_scans], each stream's entry's
+  // ranges_size (0 for a disabled entry); slot i has a message iff its LaserScan message was written (scan_sizes[i] >
+  // 0) and counts[s] > 0, of header + 36 + 4 * counts[s] bytes
 };
 cudaError_t launch_push_msg_dir(const PushMsgDirArgs& a, MsgKind kind, cudaStream_t stream);
 // The fixed part of every placed message of slots [0, a.n) once the scan kernels have written its arrays (a's hdr,

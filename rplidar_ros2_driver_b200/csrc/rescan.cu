@@ -8,6 +8,12 @@
 // >= 0, so an integer atomicMin is the float min, and the result does not depend on the order of the points.  The grid
 // is written straight into the slot's placed LaserScan message (msg_table_kernel sizes it from the stream's entry), or
 // into its row.  No state is kept.
+//
+// rescan_window_kernel (DESIGN.md 5.7.1 "Windows over the re-gridded scans"), the push form's streams with a window:
+// laser_filters' LaserArrayFilter over the same grids, a per-bin median or mean of each stream's last revolutions, whose
+// definition and CPU restatement is oracle/rescan_window_oracle.py.  It runs behind rescan_kernel, reads each grid from
+// the message rescan_kernel wrote (or builds it with the same loop, rescan_slot_grid, when the message did not fit),
+// writes W over it, and keeps the last observations - 1 grids of the stream in a ring in device memory.
 #include <algorithm>
 
 #include "beam_point.cuh"
@@ -20,6 +26,50 @@ namespace {
 
 constexpr int RT = 256;
 
+// Slot i's grid in s_bins, by the RT threads of the CTA: every bin seeded, then the least range of the points that land
+// in it; s_bins is complete when this returns
+__device__ __forceinline__ void rescan_slot_grid(const ScanCloudArgs& c, uint32_t i, const RescanGrid& g,
+                                                 uint32_t* s_bins) {
+  const uint32_t tid = threadIdx.x;
+  for (uint32_t b = tid; b < g.bins; b += RT) s_bins[b] = g.seed;
+  __syncthreads();
+  const SlotBeams sb = slot_beams(c, i);
+  const float inc = sb.M ? c.m.angle_increment[i] : 0.0f;
+  float lo, cut;
+  slot_window(c, i, &lo, &cut);
+  float4 xr[3] = {};  // the stream's rows {R_k0, R_k1, t_k, on}; on 0: no transform
+  if (c.transform) {
+    const float4* rows = c.xf ? c.xf + 3 * (i / c.m.max_scans) : c.xf_one;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) xr[k] = rows[k];
+  }
+  const double amin = g.angle_min, amax = g.angle_max, ainc = g.angle_increment;
+  for (uint32_t j = tid; j < sb.M; j += RT) {
+    const float r = sb.rg[j];
+    if (!keep_beam(r, lo, cut)) continue;
+    float x, y, p[3];
+    beam_point(j, inc, r, &x, &y);
+    if (xr[0].w != 0.0f) {
+      target_point(xr, x, y, p);
+    } else {
+      p[0] = x;
+      p[1] = y;
+      p[2] = 0.0f;
+    }
+    if (p[2] > g.max_height || p[2] < g.min_height) continue;
+    const double X = p[0], Y = p[1];
+    // the products of floats are exact in double; the sum is rounded once and sqrt correctly
+    const double range = __dsqrt_rn(__dadd_rn(__dmul_rn(X, X), __dmul_rn(Y, Y)));
+    if (range < (double)g.range_min || range > (double)g.range_max) continue;
+    const double angle = atan2_f64(Y, X);
+    if (angle < amin || angle > amax) continue;
+    const int index = __double2int_rz(__ddiv_rn(__dsub_rn(angle, amin), ainc));  // >= 0
+    if (index >= (int)g.bins) continue;  // the package would write past its grid here
+    atomicMin(&s_bins[index], __float_as_uint(__double2float_rn(range)));
+  }
+  __syncthreads();
+}
+
 __global__ void __launch_bounds__(RT) rescan_kernel(const __grid_constant__ RescanArgs a) {
   __shared__ uint32_t s_bins[kRescanMaxBins];
   const ScanCloudArgs& c = a.c;
@@ -28,43 +78,7 @@ __global__ void __launch_bounds__(RT) rescan_kernel(const __grid_constant__ Resc
     const uint32_t i = c.m.slot0 + s;
     if (c.m.out && c.m.sizes[i] == 0) continue;  // no message, or the messages do not fit
     const RescanGrid& g = a.grid ? a.grid[i / c.m.max_scans] : a.grid_one;
-    for (uint32_t b = tid; b < g.bins; b += RT) s_bins[b] = g.seed;
-    __syncthreads();
-    const SlotBeams sb = slot_beams(c, i);
-    const float inc = sb.M ? c.m.angle_increment[i] : 0.0f;
-    float lo, cut;
-    slot_window(c, i, &lo, &cut);
-    float4 xr[3] = {};  // the stream's rows {R_k0, R_k1, t_k, on}; on 0: no transform
-    if (c.transform) {
-      const float4* rows = c.xf ? c.xf + 3 * (i / c.m.max_scans) : c.xf_one;
-#pragma unroll
-      for (int k = 0; k < 3; ++k) xr[k] = rows[k];
-    }
-    const double amin = g.angle_min, amax = g.angle_max, ainc = g.angle_increment;
-    for (uint32_t j = tid; j < sb.M; j += RT) {
-      const float r = sb.rg[j];
-      if (!keep_beam(r, lo, cut)) continue;
-      float x, y, p[3];
-      beam_point(j, inc, r, &x, &y);
-      if (xr[0].w != 0.0f) {
-        target_point(xr, x, y, p);
-      } else {
-        p[0] = x;
-        p[1] = y;
-        p[2] = 0.0f;
-      }
-      if (p[2] > g.max_height || p[2] < g.min_height) continue;
-      const double X = p[0], Y = p[1];
-      // the products of floats are exact in double; the sum is rounded once and sqrt correctly
-      const double range = __dsqrt_rn(__dadd_rn(__dmul_rn(X, X), __dmul_rn(Y, Y)));
-      if (range < (double)g.range_min || range > (double)g.range_max) continue;
-      const double angle = atan2_f64(Y, X);
-      if (angle < amin || angle > amax) continue;
-      const int index = __double2int_rz(__ddiv_rn(__dsub_rn(angle, amin), ainc));  // >= 0
-      if (index >= (int)g.bins) continue;  // the package would write past its grid here
-      atomicMin(&s_bins[index], __float_as_uint(__double2float_rn(range)));
-    }
-    __syncthreads();
+    rescan_slot_grid(c, i, g, s_bins);
     if (c.m.out) {
       const StreamMsgHeader& h = c.transform ? c.cloud_hdr[i / c.m.max_scans] : c.m.hdr[i / c.m.max_scans];
       uint8_t* msg = c.m.out + (c.m.offsets[i] - c.m.out_base);
@@ -92,6 +106,101 @@ __global__ void __launch_bounds__(RT) rescan_kernel(const __grid_constant__ Resc
   }
 }
 
+// W (oracle/rescan_window_oracle.py) of the n values v[0 .. n) of one bin, oldest first, 1 <= n <= kRescanWindowMax;
+// v[j] for j >= n is not read.  Median: the value v[j] with at most k = (n - 1) / 2 values below it and more than k at
+// or below it -- a value itself, whatever the ties -- in n * n comparisons.  Mean: the float sum from +0 oldest first,
+// over n.  The loops are unrolled and leave at n (the same for every thread of the CTA), so every index is a constant
+// and v stays in registers.
+__device__ __forceinline__ float window_stat(const float (&v)[kRescanWindowMax], uint32_t n, uint32_t statistic) {
+  if (statistic == kRescanWindowMean) {
+    float sum = 0.0f;
+#pragma unroll
+    for (uint32_t j = 0; j < kRescanWindowMax; ++j) {
+      if (j >= n) break;
+      sum = __fadd_rn(sum, v[j]);
+    }
+    return __fdiv_rn(sum, (float)n);
+  }
+  const uint32_t k = (n - 1) / 2;
+  float m = v[0];
+#pragma unroll
+  for (uint32_t j = 0; j < kRescanWindowMax; ++j) {
+    if (j >= n) break;
+    uint32_t lt = 0, le = 0;
+#pragma unroll
+    for (uint32_t q = 0; q < kRescanWindowMax; ++q) {
+      if (q >= n) break;
+      lt += v[q] < v[j] ? 1u : 0u;
+      le += v[q] <= v[j] ? 1u : 0u;
+    }
+    if (lt <= k && k < le) m = v[j];
+  }
+  return m;
+}
+
+// One CTA per stream with a window (RescanWindowArgs), its slots in revolution order; each thread keeps the same bins
+// from the grid through the ring to the message, so the ring needs no barrier of its own
+__global__ void __launch_bounds__(RT) rescan_window_kernel(const __grid_constant__ RescanWindowArgs a) {
+  __shared__ uint32_t s_bins[kRescanMaxBins];
+  const ScanCloudArgs& c = a.r.c;
+  const uint32_t tid = threadIdx.x;
+  for (uint32_t q = blockIdx.x; q < a.n; q += gridDim.x) {
+    const uint32_t s = a.streams[q] - a.stream0;
+    const RescanGrid& g = a.r.grid[s];
+    const RescanWindow w = a.win[s];
+    const uint32_t R = w.observations - 1, bins = g.bins;
+    float* ring = a.ring + w.ring;
+    uint2 st = a.state[s];  // {held, next row}
+    for (uint32_t k = 0; k < c.m.max_scans; ++k) {
+      const uint32_t i = s * c.m.max_scans + k;
+      if (c.scan_sizes[i] == 0) continue;  // no LaserScan message: not a revolution of the window
+      // the message rescan_kernel has just written holds the grid; one that did not fit is built here
+      uint8_t* ranges = nullptr;
+      if (c.m.sizes[i]) {
+        const StreamMsgHeader& h = c.transform ? c.cloud_hdr[i / c.m.max_scans] : c.m.hdr[i / c.m.max_scans];
+        ranges = c.m.out + (c.m.offsets[i] - c.m.out_base) + h.bytes + 32;
+      } else {
+        rescan_slot_grid(c, i, g, s_bins);
+      }
+      const uint32_t n = st.x + 1;
+      uint32_t row[kRescanWindowMax - 1];  // the held values' rows, oldest first
+#pragma unroll
+      for (uint32_t j = 0; j + 1 < kRescanWindowMax; ++j) row[j] = (st.y + R - st.x + j) % R;
+      for (uint32_t b = tid; b < bins; b += RT) {
+        const float x = __uint_as_float(ranges ? *reinterpret_cast<const uint32_t*>(ranges + 4 * b) : s_bins[b]);
+        float v[kRescanWindowMax];
+#pragma unroll
+        for (uint32_t j = 0; j < kRescanWindowMax; ++j)
+          v[j] = j < st.x ? ring[(size_t)row[j < kRescanWindowMax - 1 ? j : 0] * bins + b]
+                 : x;  // v[st.x], the newest; entries past it are not read
+        if (ranges) put32(ranges + 4 * b, __float_as_uint(window_stat(v, n, w.statistic)));
+        ring[(size_t)st.y * bins + b] = x;
+      }
+      st.x = min(st.x + 1, R);
+      st.y = st.y + 1 == R ? 0u : st.y + 1;
+      __syncthreads();  // s_bins is seeded again for the next slot
+    }
+    if (tid == 0) a.state[s] = st;
+  }
+}
+
+// one thread per (row, bin) of the stateless form
+__global__ void __launch_bounds__(RT) rescan_window_batch_kernel(const float* __restrict__ in, uint32_t n_scans,
+                                                                 uint32_t bins, uint32_t observations,
+                                                                 uint32_t statistic, float* __restrict__ out) {
+  const unsigned long long total = (unsigned long long)n_scans * bins;
+  for (unsigned long long e = blockIdx.x * (unsigned long long)RT + threadIdx.x; e < total;
+       e += (unsigned long long)gridDim.x * RT) {
+    const uint32_t t = (uint32_t)(e / bins), b = (uint32_t)(e - (unsigned long long)t * bins);
+    const uint32_t n = min(observations, t + 1), first = t + 1 - n;
+    float v[kRescanWindowMax];
+#pragma unroll
+    for (uint32_t j = 0; j < kRescanWindowMax; ++j)
+      v[j] = j < n ? __ldg(in + (size_t)(first + j) * bins + b) : 0.0f;  // past n: not read
+    out[e] = window_stat(v, n, statistic);
+  }
+}
+
 }  // namespace
 
 cudaError_t launch_rescan(const RescanArgs& a, int num_sms, cudaStream_t stream) {
@@ -102,6 +211,26 @@ cudaError_t launch_rescan(const RescanArgs& a, int num_sms, cudaStream_t stream)
     return std::max(n, 1);
   }();
   rescan_kernel<<<(int)std::min<uint32_t>(a.c.m.n, (uint32_t)(num_sms * k)), RT, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_rescan_window(const RescanWindowArgs& a, int num_sms, cudaStream_t stream) {
+  if (a.n == 0) return cudaSuccess;
+  static const int k = [] {
+    int n = 0;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, rescan_window_kernel, RT, 0);
+    return std::max(n, 1);
+  }();
+  rescan_window_kernel<<<(int)std::min<uint32_t>(a.n, (uint32_t)(num_sms * k)), RT, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_rescan_window_batch(const float* in, uint32_t n_scans, uint32_t bins, uint32_t observations,
+                                       uint32_t statistic, float* out, int num_sms, cudaStream_t stream) {
+  const unsigned long long total = (unsigned long long)n_scans * bins;
+  if (total == 0) return cudaSuccess;
+  const unsigned long long blocks = std::min<unsigned long long>((total + RT - 1) / RT, (unsigned long long)num_sms * 8);
+  rescan_window_batch_kernel<<<(unsigned)blocks, RT, 0, stream>>>(in, n_scans, bins, observations, statistic, out);
   return cudaGetLastError();
 }
 

@@ -716,6 +716,10 @@ static_assert(sizeof(rpl_rescan_settings) == 40 && offsetof(rpl_rescan_settings,
                   offsetof(rpl_rescan_settings, scan_time) == 32 && offsetof(rpl_rescan_settings, use_inf) == 36 &&
                   offsetof(rpl_rescan_settings, enabled) == 37,
               "rpl_rescan_settings is the header's");
+static_assert(sizeof(rpl_rescan_window) == 8 && offsetof(rpl_rescan_window, observations) == 0 &&
+                  offsetof(rpl_rescan_window, statistic) == 4 && RPL_RESCAN_WINDOW_MEDIAN == rpl::kRescanWindowMedian &&
+                  RPL_RESCAN_WINDOW_MEAN == rpl::kRescanWindowMean,
+              "rpl_rescan_window is the header's");
 static_assert(sizeof(rpl_msgs_out) == 40 && offsetof(rpl_msgs_out, capacity) == 8 &&
                   offsetof(rpl_msgs_out, msg_offsets) == 16 && offsetof(rpl_msgs_out, msg_sizes) == 24 &&
                   offsetof(rpl_msgs_out, total_bytes) == 32,
@@ -1012,6 +1016,45 @@ rpl_result rpl_rescan_batch_dev(rpl_ctx* c, const rpl_rescan_settings* settings,
   a.grid_one = rescan_grid(*settings, false);
   a.out = out_ranges;
   RPL_CUDA(c, rpl::launch_rescan(a, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+  c->launches++;
+  return RPL_RESULT_OK;
+}
+
+namespace {
+
+// the limits of a window (oracle/rescan_window_oracle.py window_ok)
+bool rescan_window_ok(rpl_ctx* c, const rpl_rescan_window& w) {
+  if (w.observations >= 1 && w.observations <= rpl::kRescanWindowMax &&
+      (w.statistic == RPL_RESCAN_WINDOW_MEDIAN || w.statistic == RPL_RESCAN_WINDOW_MEAN))
+    return true;
+  c->err = "a rescan window needs observations in [1, 16] and statistic RPL_RESCAN_WINDOW_MEDIAN or _MEAN";
+  return false;
+}
+
+}  // namespace
+
+rpl_result rpl_rescan_window_batch_dev(rpl_ctx* c, const rpl_rescan_window* window, const float* in, uint32_t n_scans,
+                                       uint32_t bins, float* out, void* stream) {
+  if (!c) return RPL_RESULT_INVALID_DATA;
+  if (!window || !in || !out) {
+    c->err = "null window, in or out";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  if (!rescan_window_ok(c, *window)) return RPL_RESULT_INVALID_DATA;
+  if (bins == 0 || bins > rpl::kRescanMaxBins) {
+    c->err = "bins must be in [1, 8192]";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  if ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out)) & 3u) {
+    c->err = "in and out must be 4-byte aligned";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
+  if (n_scans == 0) return RPL_RESULT_OK;
+  RPL_CUDA(c, rpl::launch_rescan_window_batch(in, n_scans, bins, window->observations, window->statistic, out,
+                                              c->num_sms, st),
+           RPL_RESULT_OPERATION_FAIL);
   c->launches++;
   return RPL_RESULT_OK;
 }
@@ -1819,6 +1862,16 @@ struct rpl_capsule_stream {
   std::vector<rpl_rescan_settings> rescan_host;
   rpl::RescanGrid* rescan = nullptr;            // [n_streams] device
   uint32_t* rescan_bins = nullptr;              // [n_streams] device
+  // the windows over them (rpl_capsule_stream_set_rescan_windows): the entries as set (empty until the first call: every
+  // stream's observations is 1) and, laid out from both tables by either set call (windows_layout), each stream's
+  // window as the kernel reads it, its {count, head}, the ring, and the enabled streams with a window (ascending)
+  std::vector<rpl_rescan_window> win_host;
+  rpl::RescanWindow* win = nullptr;             // [n_streams] device
+  uint2* win_state = nullptr;                   // [n_streams] device, zeroed at the first call
+  float* win_ring = nullptr;
+  uint32_t* win_streams = nullptr;              // [n_streams] device, win_streams_host.size() used
+  std::vector<uint32_t> win_streams_host;
+  std::vector<rpl::RescanWindow> win_layout_host;  // as win
   unsigned char* node_work = nullptr;           // the tables of a nodes call (NodeWork)
   // [n_streams] device, zeroed at create: what every push decoded and lost (rpl_capsule_stream_counters); a stream's
   // record is written by the one CTA of each kernel that serves the stream
@@ -2279,9 +2332,41 @@ rpl_result stream_cloud_chunk(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, const r
   return scratch_leave(c, l, st);
 }
 
+// The re-grid of a LaserScan push's chunk (rpl_capsule_stream_push_rescan_msgs*), the session's tables at the chunk's
+// first stream: the entries and their bins, and the chunk's streams with a window and their windows
+struct ChunkRescans {
+  const rpl::RescanGrid* grid;  // nullptr: not a re-gridding push
+  const uint32_t* bins;
+  bool any;                     // an enabled entry in the chunk: rescan_kernel runs
+  const uint32_t* streams;      // [n_win] session indices, from stream0 on
+  uint32_t n_win, stream0;
+  const rpl::RescanWindow* win;
+  uint2* state;
+  float* ring;
+};
+
+ChunkRescans rescan_chunk(const rpl_capsule_stream* cs, uint32_t s0, uint32_t ns) {
+  ChunkRescans r{};
+  r.grid = cs->rescan + s0;
+  r.bins = cs->rescan_bins + s0;
+  for (uint32_t s = s0; s < s0 + ns && !r.any; ++s) r.any = cs->rescan_host[s].enabled != 0;
+  const std::vector<uint32_t>& ws = cs->win_streams_host;
+  const auto lo = std::lower_bound(ws.begin(), ws.end(), s0), hi = std::lower_bound(ws.begin(), ws.end(), s0 + ns);
+  r.n_win = (uint32_t)(hi - lo);
+  if (r.n_win) {
+    r.streams = cs->win_streams + (lo - ws.begin());
+    r.stream0 = s0;
+    r.win = cs->win + s0;
+    r.state = cs->win_state + s0;
+    r.ring = cs->win_ring;
+  }
+  return r;
+}
+
 // The projection of a LaserScan push's chunk (rpl_capsule_stream_push_scan_cloud_msgs*): its parameters (nullptr: none),
 // the kept counts, and the clouds' messages and directory as a PointCloud2 push's (carry [2]; extent, total,
-// extent_host and dir_order as ChunkMsgs'), every table at the chunk's first slot
+// extent_host and dir_order as ChunkMsgs'), every table at the chunk's first slot.  A re-gridding push
+// (rescan.grid) takes the same members for its re-grid messages, and its own projection (the re-grid's points).
 struct ChunkScanClouds {
   const rpl_scan_cloud_params* params;
   uint32_t* kept;
@@ -2294,6 +2379,7 @@ struct ChunkScanClouds {
   // RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS: the session's resolved headers and rows at the chunk's first stream
   const rpl::StreamMsgHeader* hdr;
   const float4* xf;
+  ChunkRescans rescan;
 };
 
 // A message push's chunk (rpl_capsule_stream_push_{laserscan,cloud,scan_cloud}_msgs*): where its messages and tables
@@ -2349,13 +2435,36 @@ rpl::ScanCloudArgs scan_cloud_push_args(const WireChunk& w, uint32_t ns, bool st
   return a;
 }
 
-// the write pass of those clouds, once their directory has placed them: message i at m.proj.out + offsets[i] - out_base
+// the write pass of those clouds (a re-gridding push: of the re-grid messages), once their directory has placed them:
+// message i at m.proj.out + offsets[i] - out_base
 rpl_result scan_cloud_push_write(rpl_ctx* c, rpl::ScanCloudArgs a, const ChunkScanClouds& p, unsigned long long out_base,
                                  cudaStream_t st) {
   a.m.offsets = p.offsets;
   a.m.sizes = p.sizes;
   a.m.out = p.out;
   a.m.out_base = out_base;
+  if (const ChunkRescans& q = p.rescan; q.grid) {
+    rpl::RescanArgs ra{};
+    ra.c = a;
+    ra.grid = q.grid;
+    if (q.any) {  // every message, as the replay re-grids it
+      RPL_CUDA(c, rpl::launch_rescan(ra, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+      c->launches++;
+    }
+    if (q.n_win) {  // then the windows, over those grids (or their own, for a message that did not fit)
+      rpl::RescanWindowArgs wa{};
+      wa.r = ra;
+      wa.streams = q.streams;
+      wa.n = q.n_win;
+      wa.stream0 = q.stream0;
+      wa.win = q.win;
+      wa.state = q.state;
+      wa.ring = q.ring;
+      RPL_CUDA(c, rpl::launch_rescan_window(wa, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+      c->launches++;
+    }
+    return RPL_RESULT_OK;
+  }
   RPL_CUDA(c, rpl::launch_scan_cloud(a, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
   c->launches++;
   return RPL_RESULT_OK;
@@ -2494,10 +2603,14 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
   c->launches++;
   if (!m->proj.params) return RPL_RESULT_OK;
   // the projection of the messages just finished: the kept counts, the clouds' directory, which sizes each message
-  // exactly, then (the device form; the host form's waits for both extents, push_host) the write pass
+  // exactly, then (the device form; the host form's waits for both extents, push_host) the write pass.  A re-gridding
+  // push's directory sizes each re-grid message by its stream's entry: no count pass.
+  const bool rescan = m->proj.rescan.grid != nullptr;
   const rpl::ScanCloudArgs sa = scan_cloud_push_args(w, ns, sp != nullptr, params, *m, beams, inc);
-  RPL_CUDA(c, rpl::launch_scan_cloud_count(sa, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
-  c->launches++;
+  if (!rescan) {
+    RPL_CUDA(c, rpl::launch_scan_cloud_count(sa, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+    c->launches++;
+  }
   d.capacity = m->proj.capacity;
   d.carry = m->proj.carry;
   d.offsets = m->proj.offsets;
@@ -2510,7 +2623,8 @@ rpl_result capsule_stream_chunk(rpl_ctx* c, Lane& l, cudaStream_t st, const Wire
   if (sa.transform) d.hdr = m->proj.hdr;  // the target frames' headers size the messages
   d.tail_bytes = sa.transform ? sa.tail_xf.bytes : sa.tail.bytes;
   d.point_step = sa.point_step;
-  r = directory(d, rpl::MsgKind::kScanCloud, m->proj.dir_order, m->proj.extent_host);
+  if (rescan) d.counts = m->proj.rescan.bins;
+  r = directory(d, rescan ? rpl::MsgKind::kRescan : rpl::MsgKind::kScanCloud, m->proj.dir_order, m->proj.extent_host);
   if (r != RPL_RESULT_OK || m->extent_host) return r;
   return scan_cloud_push_write(c, sa, m->proj, 0, st);
 }
@@ -2557,6 +2671,8 @@ struct HostMsgs {
   cudaEvent_t proj_dir_order;
   const rpl::StreamMsgHeader* proj_hdr;  // RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS: the session's resolved headers, rows
   const float4* proj_xf;
+  // a re-gridding push: its session (rescan_chunk), whose re-grid messages take the projection's members above
+  const rpl_capsule_stream* rescan;
 };
 
 // Runs a host call's n_streams streams through capsule_stream_chunk, `chunk` streams at a time round-robin over the
@@ -2686,6 +2802,7 @@ rpl_result push_host(rpl_ctx* c, const HostWire& h, uint32_t n_streams, uint32_t
         m.proj = ChunkScanClouds{hm->proj, hm->kept + so, d.pmsgs, hm->clouds->capacity, hm->proj_carry, d.poffs,
                                  d.pextent, nullptr, d.psizes, hm->proj_extent_host + 3 * li, hm->proj_dir_order,
                                  hm->proj_hdr ? hm->proj_hdr + s0 : nullptr, hm->proj_xf ? hm->proj_xf + 3 * s0 : nullptr};
+      if (proj && hm->rescan) m.proj.rescan = rescan_chunk(hm->rescan, s0, ns);
     }
     const rpl_result r = capsule_stream_chunk(c, l, l.stream, d.w, ns, d.in, d.counts, h.sample_duration_us, h.params,
                                               d.ranges, d.intens, d.beams, d.inc, d.sps, h.sp ? &sp : nullptr,
@@ -3082,6 +3199,7 @@ struct PushMsgs {
   uint32_t* kept;
   const rpl::StreamMsgHeader* proj_hdr;  // RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS: the session's resolved headers, rows
   const float4* proj_xf;
+  bool rescan;  // a re-gridding push: clouds are its re-grid messages (ChunkScanClouds::rescan)
 };
 
 // A push of the kind the entry point takes (bytes: a byte push); sp: a stamped one.  Host arrays (dev false, stream
@@ -3139,6 +3257,8 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
                                    reinterpret_cast<unsigned long long*>(pm->clouds->total_bytes),
                                    pm->clouds->msg_sizes + so, nullptr, nullptr, pm->proj_hdr ? pm->proj_hdr + s0 : nullptr,
                                    pm->proj_xf ? pm->proj_xf + 3 * s0 : nullptr};
+        if (pm->proj && pm->rescan)
+          m.proj.rescan = rescan_chunk(cs, s0, std::min(chunk, cs->n_streams - s0));
       }
       r = capsule_stream_chunk(c, c->lane[0], st, session_chunk(cs, s0, params, true, pm ? pm->cloud : nullptr),
                                std::min(chunk, cs->n_streams - s0), in + s0 * cs->in_stream, counts + s0,
@@ -3171,8 +3291,12 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
           proj_hdr_most = 0;
           for (const rpl::StreamMsgHeader& e : cs->xf_hdr_host) proj_hdr_most = std::max(proj_hdr_most, e.bytes);
         }
-        const size_t pmost = (size_t)proj_hdr_most + scan_cloud_tail_bytes(pm->proj->channels) +
-                             (size_t)scan_cloud_point_step(pm->proj->channels) * n + 1;
+        uint32_t bins_most = 0;  // a re-gridding push's: the largest ranges_size
+        for (const rpl_rescan_settings& e : cs->rescan_host)
+          if (pm->rescan && e.enabled) bins_most = std::max(bins_most, rescan_bins(e));
+        const size_t pmost = pm->rescan ? (size_t)proj_hdr_most + 36 + 4 * (size_t)bins_most
+                                        : (size_t)proj_hdr_most + scan_cloud_tail_bytes(pm->proj->channels) +
+                                              (size_t)scan_cloud_point_step(pm->proj->channels) * n + 1;
         hm.proj = pm->proj;
         hm.clouds = pm->clouds;
         hm.proj_chunk_bytes = (size_t)chunk * cs->max_scans * ((pmost + 15) & ~(size_t)15);
@@ -3182,6 +3306,7 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
         hm.proj_dir_order = cs->push_scan_cloud_dir_order;
         hm.proj_hdr = pm->proj_hdr;
         hm.proj_xf = pm->proj_xf;
+        if (pm->rescan) hm.rescan = cs;
       }
     }
     const HostWire h{in, counts, cs->in_stream, sample_duration_us, cs->max_nodes, cs->max_scans, params, ranges,
@@ -3455,6 +3580,106 @@ rpl_result stream_set_scan_cloud_transforms(rpl_capsule_stream* cs, const rpl_sc
   return RPL_RESULT_OK;
 }
 
+// Empties the windows of the streams `mask` takes in (nullptr: all), on `st`: one clear per run of them
+rpl_result windows_empty(rpl_capsule_stream* cs, const uint8_t* mask, cudaStream_t st) {
+  for (uint32_t s = 0; s < cs->n_streams;) {
+    if (mask && !mask[s]) {
+      ++s;
+      continue;
+    }
+    uint32_t e = s + 1;
+    while (e < cs->n_streams && (!mask || mask[e])) ++e;
+    RPL_CUDA(cs->c, cudaMemsetAsync(cs->win_state + s, 0, (size_t)(e - s) * sizeof(uint2), st), RPL_RESULT_OPERATION_FAIL);
+    s = e;
+  }
+  return RPL_RESULT_OK;
+}
+
+// Lays the windows out from the re-grid entries t and the windows w as the set call will leave them, once cs->done has
+// passed: each enabled stream with observations >= 2 gets (observations - 1) * ranges_size floats of a new ring.  The
+// streams `mask` leaves out (their entries and so their sizes unchanged) keep their window, copied; the others start
+// empty.  Running out of memory changes nothing.
+rpl_result windows_layout(rpl_capsule_stream* cs, const std::vector<rpl_rescan_settings>& t,
+                          const std::vector<rpl_rescan_window>& w, const uint8_t* mask) {
+  rpl_ctx* c = cs->c;
+  const uint32_t n = cs->n_streams;
+  std::vector<rpl::RescanWindow> win(n);
+  std::vector<uint32_t> streams;
+  unsigned long long total = 0;
+  for (uint32_t s = 0; s < n; ++s) {
+    const uint32_t bins = t.empty() || !t[s].enabled ? 0u : rescan_bins(t[s]);
+    const bool windowed = bins > 0 && w[s].observations > 1;
+    win[s] = rpl::RescanWindow{total, w[s].observations, w[s].statistic};
+    if (windowed) {
+      streams.push_back(s);
+      total += (unsigned long long)(w[s].observations - 1) * bins;
+    }
+  }
+  if (!cs->win) {  // the first call: the per-stream tables, every window empty; all three or none
+    rpl::RescanWindow* win = nullptr;
+    uint32_t* streams_d = nullptr;
+    uint2* state = nullptr;
+    cudaError_t e = dev_alloc(&win, n);
+    if (e == cudaSuccess) e = dev_alloc(&streams_d, n);
+    if (e == cudaSuccess) e = dev_alloc(&state, n);
+    if (e == cudaSuccess) e = cudaMemset(state, 0, (size_t)n * sizeof(uint2));
+    if (e != cudaSuccess) {
+      cudaFree(win);
+      cudaFree(streams_d);
+      cudaFree(state);
+      RPL_CUDA(c, e, e == cudaErrorMemoryAllocation ? RPL_RESULT_INSUFFICIENT_MEMORY : RPL_RESULT_OPERATION_FAIL);
+    }
+    cs->win = win;
+    cs->win_streams = streams_d;
+    cs->win_state = state;
+  }
+  float* ring = nullptr;
+  if (total) RPL_CUDA(c, dev_alloc(&ring, total), RPL_RESULT_INSUFFICIENT_MEMORY);
+  std::vector<uint8_t> kept(n, 0);  // a stream with a window in both layouts that the call leaves out
+  for (uint32_t s : cs->win_streams_host) kept[s] = mask && !mask[s] ? 1 : 0;
+  cudaError_t e = cudaSuccess;
+  for (uint32_t s : streams)
+    if (kept[s] && e == cudaSuccess)
+      e = cudaMemcpy(ring + win[s].ring, cs->win_ring + cs->win_layout_host[s].ring,
+                     (size_t)(w[s].observations - 1) * rescan_bins(t[s]) * 4, cudaMemcpyDeviceToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(cs->win, win.data(), (size_t)n * sizeof(rpl::RescanWindow), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && !streams.empty())
+    e = cudaMemcpy(cs->win_streams, streams.data(), streams.size() * 4, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    cudaFree(ring);
+    RPL_CUDA(c, e, RPL_RESULT_OPERATION_FAIL);
+  }
+  if (const rpl_result r = windows_empty(cs, mask, c->lane[0].stream); r != RPL_RESULT_OK) return r;
+  RPL_CUDA(c, cudaStreamSynchronize(c->lane[0].stream), RPL_RESULT_OPERATION_FAIL);
+  cudaFree(cs->win_ring);
+  cs->win_ring = ring;
+  cs->win_layout_host = std::move(win);
+  cs->win_streams_host = std::move(streams);
+  return RPL_RESULT_OK;
+}
+
+// the windows over the re-gridded scans: the masked entries of `windows` replace the table's, all or none
+rpl_result stream_set_rescan_windows(rpl_capsule_stream* cs, const rpl_rescan_window* windows, const uint8_t* stream_mask) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!windows) {
+    c->err = "null windows";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  std::vector<rpl_rescan_window> w = cs->win_host;
+  if (w.empty()) w.assign(cs->n_streams, rpl_rescan_window{1u, RPL_RESCAN_WINDOW_MEDIAN});
+  for (uint32_t s = 0; s < cs->n_streams; ++s) {
+    if (stream_mask && !stream_mask[s]) continue;
+    if (!rescan_window_ok(c, windows[s])) return RPL_RESULT_INVALID_DATA;
+    w[s] = windows[s];
+  }
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);  // a push may still read them
+  if (const rpl_result r = windows_layout(cs, cs->rescan_host, w, stream_mask); r != RPL_RESULT_OK) return r;
+  cs->win_host = std::move(w);
+  return RPL_RESULT_OK;
+}
+
 // the re-gridded scans' entries: the masked entries of `settings` replace the table's, all or none
 rpl_result stream_set_rescans(rpl_capsule_stream* cs, const rpl_rescan_settings* settings, const uint8_t* stream_mask) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
@@ -3487,6 +3712,8 @@ rpl_result stream_set_rescans(rpl_capsule_stream* cs, const rpl_rescan_settings*
   if (!cs->rescan) RPL_CUDA(c, dev_alloc(&cs->rescan, cs->n_streams), RPL_RESULT_INSUFFICIENT_MEMORY);
   if (!cs->rescan_bins) RPL_CUDA(c, dev_alloc(&cs->rescan_bins, cs->n_streams), RPL_RESULT_INSUFFICIENT_MEMORY);
   RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);  // a messages call may still read them
+  if (!cs->win_host.empty())  // the masked streams' grids may change: their windows start over
+    if (const rpl_result r = windows_layout(cs, t, cs->win_host, stream_mask); r != RPL_RESULT_OK) return r;
   RPL_CUDA(c, cudaMemcpy(cs->rescan, g.data(), g.size() * sizeof(rpl::RescanGrid), cudaMemcpyHostToDevice),
            RPL_RESULT_OPERATION_FAIL);
   RPL_CUDA(c, cudaMemcpy(cs->rescan_bins, bins.data(), bins.size() * 4, cudaMemcpyHostToDevice),
@@ -4036,7 +4263,8 @@ rpl_result stream_msgs(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* pa
 rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, rpl::MsgKind kind, const void* params,
                      int64_t clock_offset_ns, uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
                      uint64_t* total_bytes, uint32_t* scans_per_stream, bool dev, void* stream,
-                     const rpl_scan_cloud_params* proj = nullptr, const rpl_msgs_out* clouds = nullptr) {
+                     const rpl_scan_cloud_params* proj = nullptr, const rpl_msgs_out* clouds = nullptr,
+                     bool rescan = false) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
   rpl_ctx* c = cs->c;
   cs->cloud_chunk = 0;  // as a push that fails its checks
@@ -4050,6 +4278,10 @@ rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, rpl::MsgK
       return RPL_RESULT_INVALID_DATA;
     }
     if (!scan_cloud_call_ok(cs, *proj)) return RPL_RESULT_INVALID_DATA;
+    if (rescan && cs->rescan_host.empty()) {
+      c->err = "push_rescan_msgs before the first rpl_capsule_stream_set_rescans";
+      return RPL_RESULT_INVALID_DATA;
+    }
     if (dev && ((reinterpret_cast<uintptr_t>(clouds->msgs) & 15u) || misaligned8(clouds->msg_offsets) ||
                 misaligned8(clouds->total_bytes) || (reinterpret_cast<uintptr_t>(clouds->msg_sizes) & 3u))) {
       c->err = "clouds: msgs must be 16-byte aligned, msg_offsets and total_bytes 8-byte, msg_sizes 4-byte aligned";
@@ -4087,7 +4319,8 @@ rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, rpl::MsgK
       RPL_CUDA(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming), RPL_RESULT_OPERATION_FAIL);
     RPL_CUDA(c, cudaEventCreateWithFlags(&cs->push_msg_dir_order, cudaEventDisableTiming), RPL_RESULT_OPERATION_FAIL);
   }
-  if (proj && !cs->push_scan_cloud_work) {  // the first projecting push: its tables, made once
+  // the first projecting or re-gridding push: its tables, made once (a re-gridding push uses the carry alone)
+  if (proj && !cs->push_scan_cloud_work) {
     RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
     Carve k;
     scan_cloud_work_layout(cs, k);
@@ -4108,6 +4341,7 @@ rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, rpl::MsgK
     pm.clouds = clouds;
     pm.proj_carry = sw.carry;
     pm.kept = sw.kept;
+    pm.rescan = rescan;
     if (proj->channels & rpl::kScanCloudPerStreamTransforms) {
       pm.proj_hdr = cs->xf_hdr;
       pm.proj_xf = cs->xf;
@@ -4136,26 +4370,27 @@ rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, rpl::MsgK
   const rpl_result r = stream_push(cs, in->data, in->counts, sample_duration_us, sp_params, nullptr, nullptr, nullptr,
                                    nullptr, scans_per_stream, stamped ? &sp : nullptr, cs->bytes, dev, stream, &pm);
   if (r != RPL_RESULT_OK) return r;
-  if (!dev && (*total_bytes > capacity || (proj && *clouds->total_bytes > clouds->capacity))) {
+  if (!dev && (*total_bytes > capacity || (proj && *clouds->total_bytes > clouds->capacity))) {  // windows advanced
     c->err = "the messages need more than capacity bytes (total_bytes tells how many; the push itself is done)";
     return RPL_RESULT_INSUFFICIENT_MEMORY;
   }
   return RPL_RESULT_OK;
 }
 
+// rescan: rpl_capsule_stream_push_rescan_msgs*, whose `clouds` are the re-grid messages
 rpl_result push_scan_cloud_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, const rpl_scan_params* scan_params,
                                 const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
                                 const rpl_msgs_out* scans, const rpl_msgs_out* clouds, uint32_t* scans_per_stream,
-                                bool dev, void* stream) {
+                                bool dev, void* stream, bool rescan = false) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
   if (!scans || !clouds || !cloud_params) {
     cs->cloud_chunk = 0;  // as a push that fails its checks
-    cs->c->err = "null scans, clouds or cloud_params";
+    cs->c->err = rescan ? "null scans, rescans or cloud_params" : "null scans, clouds or cloud_params";
     return RPL_RESULT_INVALID_DATA;
   }
   return push_msgs(cs, in, rpl::MsgKind::kLaserScan, scan_params, clock_offset_ns, scans->msgs, scans->capacity,
                    scans->msg_offsets, scans->msg_sizes, scans->total_bytes, scans_per_stream, dev, stream,
-                   cloud_params, clouds);
+                   cloud_params, clouds, rescan);
 }
 
 // ---- grabbed node buffers of the last push (DESIGN.md 5.7.1 "Session nodes") -------------------------------------
@@ -4415,6 +4650,10 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   cudaFree(cs->xf_hdr);
   cudaFree(cs->rescan);
   cudaFree(cs->rescan_bins);
+  cudaFree(cs->win);
+  cudaFree(cs->win_state);
+  cudaFree(cs->win_ring);
+  cudaFree(cs->win_streams);
   cudaFreeHost(cs->push_scan_cloud_extent);
   if (cs->push_scan_cloud_dir_order) cudaEventDestroy(cs->push_scan_cloud_dir_order);
   if (cs->done) cudaEventDestroy(cs->done);
@@ -4481,6 +4720,8 @@ rpl_result rpl_capsule_stream_reset(rpl_capsule_stream* cs, const uint8_t* strea
     if (cs->framer)  // the handlers' reset: _cached_scan_node_buf_pos = 0, _is_previous_capsuledataRdy = false
       RPL_CUDA(c, cudaMemsetAsync(cs->framer + (size_t)s * rpl::kFramerWords, 0, (size_t)(e - s) * rpl::kFramerWords * 4, st),
                RPL_RESULT_OPERATION_FAIL);
+    if (cs->win_state)  // the windows over the re-gridded scans start over
+      RPL_CUDA(c, cudaMemsetAsync(cs->win_state + s, 0, (size_t)(e - s) * sizeof(uint2), st), RPL_RESULT_OPERATION_FAIL);
     s = e;
   }
   RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);
@@ -4756,6 +4997,9 @@ rpl_result rpl_capsule_stream_import(rpl_capsule_stream* cs, const uint32_t* str
   // messages read, point into the arena it decoded into (cloud_arena, the other one), so they stay as they are.
   RPL_CUDA(c, rpl::launch_stream_unpack(a, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
   c->launches++;
+  // records do not carry the windows over the re-gridded scans: the destinations' start over
+  if (cs->win_state)
+    if (const rpl_result r = windows_empty(cs, seen.data(), st); r != RPL_RESULT_OK) return r;
   RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);  // in place before any later push runs
   if (types != cs->types) return set_types(cs, std::move(types));     // a mixed session's streams take the record's type
   return RPL_RESULT_OK;
@@ -5016,6 +5260,29 @@ rpl_result rpl_capsule_stream_scan_cloud_msgs(rpl_capsule_stream* s, const rpl_s
   const ScanCloudCall q{scan_params, cloud_params};
   return stream_msgs(s, rpl::MsgKind::kScanCloud, &q, clock_offset_ns, msgs, capacity, msg_offsets, msg_sizes,
                      total_bytes);
+}
+
+rpl_result rpl_capsule_stream_set_rescan_windows(rpl_capsule_stream* s, const rpl_rescan_window* windows,
+                                                 const uint8_t* stream_mask) {
+  return stream_set_rescan_windows(s, windows, stream_mask);
+}
+
+rpl_result rpl_capsule_stream_push_rescan_msgs(rpl_capsule_stream* s, const rpl_push_input* in,
+                                               const rpl_scan_params* scan_params,
+                                               const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
+                                               const rpl_msgs_out* scans, const rpl_msgs_out* rescans,
+                                               uint32_t* scans_per_stream) {
+  return push_scan_cloud_msgs(s, in, scan_params, cloud_params, clock_offset_ns, scans, rescans, scans_per_stream, false,
+                              nullptr, true);
+}
+
+rpl_result rpl_capsule_stream_push_rescan_msgs_dev(rpl_capsule_stream* s, const rpl_push_input* in,
+                                                   const rpl_scan_params* scan_params,
+                                                   const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
+                                                   const rpl_msgs_out* scans, const rpl_msgs_out* rescans,
+                                                   uint32_t* scans_per_stream, void* stream) {
+  return push_scan_cloud_msgs(s, in, scan_params, cloud_params, clock_offset_ns, scans, rescans, scans_per_stream, true,
+                              stream, true);
 }
 
 rpl_result rpl_capsule_stream_set_rescans(rpl_capsule_stream* s, const rpl_rescan_settings* settings,

@@ -597,8 +597,9 @@ rpl_result rpl_capsule_stream_counters(rpl_capsule_stream* s, rpl_stream_counter
  *            kind (framed or byte) and max_nodes whose stream has the same settings, push P(k+1)..Pn into B: A's
  *            outputs up to k followed by B's are bit for bit those of one session fed P1..Pn, in every output of every
  *            call (scans, stamps, state, nodes, clouds, messages) and every counter but scans_unreturned -- with one
- *            exception: records do not carry the windows over the re-gridded scans, so the outputs of
- *            push_rescan_msgs[_dev] on a stream with observations >= 2 restart their window at the import.
+ *            exception: records do not carry the windows over the re-gridded scans, nor the held grids of the merge
+ *            groups, so the outputs of push_rescan_msgs[_dev] on a stream with observations >= 2 restart their window
+ *            at the import, and push_rescan_merge_msgs[_dev] merges nothing of the stream until it publishes again.
  *   Record:  little-endian bytes, version RPL_STREAM_RECORD_VERSION: a 32-byte header (uint32 magic "RPLM", version,
  *            kind 0 framed / 1 byte session, answer type, max_nodes, open length L, stamp flags, 0), the 192-byte held
  *            record, for a capsule answer type in a byte session the 800-byte framer record, the open revolution's
@@ -1423,6 +1424,83 @@ rpl_result rpl_capsule_stream_push_rescan_msgs_dev(rpl_capsule_stream* s, const 
                                                    const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
                                                    const rpl_msgs_out* scans, const rpl_msgs_out* rescans,
                                                    uint32_t* scans_per_stream, void* stream);
+
+/* Merged scans from the push (DESIGN.md 5.7.1 "Merged scans from the push"; INTEGRATION.md 4l): a scan merger
+ * (ira_laser_tools' laserscan_multi_merger and its ports) over the re-gridded scans -- one LaserScan per group of
+ * streams, such as a robot's front and rear lidars, in the frame and on the grid its members share.  When the members
+ * share one rpl_rescan_settings entry and one target frame, pointcloud_to_laserscan over the concatenated clouds is the
+ * per-bin minimum of the members' grids, bit for bit, whatever the point order.  oracle/rescan_merge_oracle.py defines:
+ *   M(settings, grids): per bin, the least of the entry's seed (+inf with use_inf, else fl32(range_max + inf_epsilon))
+ *            and the grids' values.  Re-grid values are never NaN or -0, so the minimum does not depend on the order.
+ *            M(settings, [Q(settings, c1), ..., Q(settings, cn)]) == Q(settings, c1 ++ ... ++ cn).
+ * RPL_RESCAN_MERGE_NONE marks a stream in no group and a row of no group. */
+#define RPL_RESCAN_MERGE_NONE 0xFFFFFFFFu
+/* Stateless: out[g] ([n_groups][ranges_size], row g at out + g * ranges_size) is M(*settings, the rows r of in
+ * ([n_rows][ranges_size]) with row_group[r] == g); a group with no rows is all seed, a row whose group is not below
+ * n_groups (RPL_RESCAN_MERGE_NONE, say) is not read.  settings->enabled is not read.  Device arrays, 4-byte aligned.  A
+ * null ctx, settings or out, a null in or row_group with n_rows > 0, an entry outside the limits of set_rescans, or a
+ * misaligned array: RPL_RESULT_INVALID_DATA, and nothing is written.  Asynchronous on `stream` (NULL: the context's
+ * stream). */
+rpl_result rpl_rescan_merge_batch_dev(rpl_ctx* ctx, const rpl_rescan_settings* settings,
+                                      const float* in /* [n_rows][ranges_size] */,
+                                      const uint32_t* row_group /* [n_rows], RPL_RESCAN_MERGE_NONE: ignored */,
+                                      uint32_t n_rows, uint32_t n_groups, float* out /* [n_groups][ranges_size] */,
+                                      void* stream);
+/*   set_rescan_merges: the groups, replaced whole (synchronous, not masked): stream s goes into group
+ *            group_of_stream[s] < n_groups, or into none (RPL_RESCAN_MERGE_NONE); group g keeps a member's grid for
+ *            max_age[g] merge pushes.  n_groups 0 removes every group.  A null group_of_stream (or max_age with
+ *            n_groups > 0), a group index neither below n_groups nor RPL_RESCAN_MERGE_NONE, a group without a member,
+ *            n_groups > n_streams or a max_age > 65535: RPL_RESULT_INVALID_DATA, and nothing changes.  Out of device
+ *            memory: RPL_RESULT_INSUFFICIENT_MEMORY, and nothing changes.
+ *   Held grid: a grouped stream s holds the ranges of the newest re-grid message of s that a merge push wrote (size >
+ *            0: it fit rescans->capacity), as published (a window's output where s has one), with that message's
+ *            stamp and the number of the merge push.  A merge push that wrote no re-grid message of s leaves it as it
+ *            was.  Unlike a window, which takes a re-grid that did not fit, a held grid is what a merger downstream
+ *            would have received.
+ *   Emptied: stream s's held grid, by session create; every set_rescan_merges call; set_rescans,
+ *            set_rescan_windows or set_scan_cloud_transforms with s masked in; set_frames; rpl_capsule_stream_reset
+ *            with s masked in; rpl_capsule_stream_import into s; a switch of s's answer type.  A refused call of any
+ *            kind changes no held grid and no push count.
+ *   Cost:    one device block per layout: 20 bytes per stream, 16 per group, and a row of 8192 floats (32 KB) per
+ *            grouped stream, so that a later set_rescans never lays the rows out again. */
+rpl_result rpl_capsule_stream_set_rescan_merges(rpl_capsule_stream* s, const uint32_t* group_of_stream /* [n_streams] */,
+                                                const uint32_t* max_age /* [n_groups] */, uint32_t n_groups);
+/* The push form: push_rescan_msgs, plus one merged LaserScan per group that has news.
+ *   scans, rescans: exactly what push_rescan_msgs[_dev] returns on a session with the same history (windows advance
+ *            alike).  Other calls, push_rescan_msgs and rescan_msgs among them, neither read nor advance held grids.
+ *   Checks:  at call time, since set_rescans, set_scan_cloud_transforms and set_frames can change them after the groups
+ *            were set: every member of a group has an enabled rpl_rescan_settings entry, all byte for byte equal but
+ *            for pad, and every member's re-grid message carries one frame_id (the resolved target frame under
+ *            RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS, else the LaserScan frame).  A call that fails them, or comes before
+ *            the first set_rescans or the first set_rescan_merges, is RPL_RESULT_INVALID_DATA and changes nothing.
+ *   Publish: with seq the number of this call among the merge pushes that succeeded, group g publishes one message iff
+ *            a member's held grid is from this call.  Its contributors are the members whose held grid is from within
+ *            max_age[g] calls (seq - held seq <= max_age; 0: this call only), so a stopped or dead lidar drops out.  The
+ *            message is the re-grid message of the contributor with the newest stamp ((sec, nanosec); a tie goes to the
+ *            lowest stream index) with M over the contributors' held grids as its ranges.
+ *   Rate:    one merged scan per group per call, not per revolution: revolutions of different streams within one push
+ *            have no order the call can observe.  For one merged scan per revolution, push at the revolution cadence.
+ *   merged:  an rpl_msgs_out indexed by group (msg_sizes[g] 0: no message this call), packed as rescans: msg_offsets
+ *            the exclusive scan of the sizes rounded up to 16, a message written iff offset + size <= capacity, so the
+ *            written messages are a prefix; total_bytes the end of the last.  Its alignment rules in the _dev form are
+ *            those of rescans.  The host form returns RPL_RESULT_INSUFFICIENT_MEMORY when any of the three totals
+ *            exceeds its capacity; the push is done and windows and held grids have advanced either way.
+ *   Cost:    per chunk with a grouped stream, one hold launch of one CTA per grouped stream (none elsewhere); at the
+ *            end, the groups' directory and one CTA per message.  The host form stages the merged messages in a
+ *            session buffer of n_groups * (the longest header + 36 + 4 * the largest ranges_size) bytes and copies them
+ *            back once, behind the directory. */
+rpl_result rpl_capsule_stream_push_rescan_merge_msgs(rpl_capsule_stream* s, const rpl_push_input* in,
+                                                     const rpl_scan_params* scan_params,
+                                                     const rpl_scan_cloud_params* cloud_params,
+                                                     int64_t clock_offset_ns, const rpl_msgs_out* scans,
+                                                     const rpl_msgs_out* rescans, const rpl_msgs_out* merged,
+                                                     uint32_t* scans_per_stream);
+rpl_result rpl_capsule_stream_push_rescan_merge_msgs_dev(rpl_capsule_stream* s, const rpl_push_input* in,
+                                                         const rpl_scan_params* scan_params,
+                                                         const rpl_scan_cloud_params* cloud_params,
+                                                         int64_t clock_offset_ns, const rpl_msgs_out* scans,
+                                                         const rpl_msgs_out* rescans, const rpl_msgs_out* merged,
+                                                         uint32_t* scans_per_stream, void* stream);
 
 /* ---- LaserScan / PointCloud2 -> wire (SURVEY.md 8(f) rank 3) ---------------------------- */
 /* The serialised message the RMW layer would produce from the message the reference publishes

@@ -15,5 +15,6 @@ from .capi import (  # noqa: F401
     ScanFootprint, scan_footprint, ScanCloudParams, scan_cloud_params, SCAN_CLOUD_INTENSITY, SCAN_CLOUD_INDEX,
     SCAN_CLOUD_DISTANCE, SCAN_CLOUD_TIMESTAMP, MsgsOut, ScanCloudTransform, scan_cloud_transform, SCAN_CLOUD_VIEWPOINT,
     SCAN_CLOUD_PER_STREAM_TRANSFORMS, RescanSettings, rescan_settings, rescan_ranges_size, RescanWindow, rescan_window,
+    RESCAN_MERGE_NONE,
     FLAG_FORCE_GENERAL, FLAG_NO_TMA, FLAG_NO_SMALL, CLOUD_NO_FUSED, PATH_FAST, PATH_GENERAL, RESULT_OK, RESULT_OPERATION_FAIL, RESULT_INVALID_DATA,
 )

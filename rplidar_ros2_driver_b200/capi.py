@@ -79,6 +79,8 @@ EXPORTS = [
     "rpl_capsule_stream_rescan_msgs_dev",
     "rpl_rescan_window_batch_dev", "rpl_capsule_stream_set_rescan_windows", "rpl_capsule_stream_push_rescan_msgs",
     "rpl_capsule_stream_push_rescan_msgs_dev",
+    "rpl_rescan_merge_batch_dev", "rpl_capsule_stream_set_rescan_merges", "rpl_capsule_stream_push_rescan_merge_msgs",
+    "rpl_capsule_stream_push_rescan_merge_msgs_dev",
     "rpl_capsule_bytes", "rpl_capsule_nodes", "rpl_decode_capsules_batch_dev", "rpl_decode_capsules",
     "rpl_decode_normal_batch_dev", "rpl_decode_normal", "rpl_frame_capsules_dev", "rpl_node_timestamps_dev", "rpl_normal_timestamps_dev",
     "rpl_peer_gather_bytes", "rpl_peer_alloc", "rpl_peer_open", "rpl_peer_close", "rpl_peer_free",
@@ -396,6 +398,14 @@ def lib() -> C.CDLL:
         "rpl_capsule_stream_push_rescan_msgs_dev":
             ([vp, C.POINTER(PushInput), PSP, C.POINTER(ScanCloudParams), C.c_int64, C.POINTER(MsgsOut),
               C.POINTER(MsgsOut), vp, vp], u32),
+        "rpl_rescan_merge_batch_dev": ([vp, C.POINTER(RescanSettings), vp, vp, u32, u32, vp, vp], u32),
+        "rpl_capsule_stream_set_rescan_merges": ([vp, vp, vp, u32], u32),
+        "rpl_capsule_stream_push_rescan_merge_msgs":
+            ([vp, C.POINTER(PushInput), PSP, C.POINTER(ScanCloudParams), C.c_int64, C.POINTER(MsgsOut),
+              C.POINTER(MsgsOut), C.POINTER(MsgsOut), vp], u32),
+        "rpl_capsule_stream_push_rescan_merge_msgs_dev":
+            ([vp, C.POINTER(PushInput), PSP, C.POINTER(ScanCloudParams), C.c_int64, C.POINTER(MsgsOut),
+              C.POINTER(MsgsOut), C.POINTER(MsgsOut), vp, vp], u32),
     }
     for name, (args, res) in sig.items():
         fn = getattr(L, name)  # AttributeError here = the library does not export the ABI
@@ -504,6 +514,7 @@ def rescan_ranges_size(settings: RescanSettings) -> int:
 
 
 RESCAN_WINDOW_MEDIAN, RESCAN_WINDOW_MEAN = 0, 1
+RESCAN_MERGE_NONE = 0xFFFFFFFF
 RESCAN_WINDOW_MAX = 16
 
 
@@ -902,6 +913,13 @@ class Context:
         self._check(self._L.rpl_rescan_window_batch_dev(self._h, C.byref(window), _p(in_ranges), n_scans, bins,
                                                         _p(out_ranges), _p(stream)))
 
+    def rescan_merge_batch_dev(self, settings: RescanSettings, in_ranges, row_group, n_rows, n_groups, out_ranges,
+                               stream=None):
+        """Row g of out_ranges ([n_groups][ranges_size]) is the per-bin minimum, from the entry's seed, of the rows r of
+        in_ranges ([n_rows][ranges_size]) with row_group[r] == g (device addresses; RESCAN_MERGE_NONE: no group)."""
+        self._check(self._L.rpl_rescan_merge_batch_dev(self._h, C.byref(settings), _p(in_ranges), _p(row_group),
+                                                       n_rows, n_groups, _p(out_ranges), _p(stream)))
+
     def cloud_fuse_dev(self, xyzi, point_counts, n_scans, stride, fused, offsets, total, stream=None):
         self._check(self._L.rpl_cloud_fuse_dev(self._h, _p(xyzi), _p(point_counts), n_scans, stride, _p(fused),
                                                _p(offsets), _p(total), _p(stream)))
@@ -1097,6 +1115,15 @@ class CapsuleStreamSession:
         assert m is None or m.shape == (self.n_streams,)
         self._ctx._check(self._fn("set_rescan_windows")(self._h, C.cast(arr, C.c_void_p), _p(m)))
 
+    def set_rescan_merges(self, group_of_stream, max_age):
+        """The groups whose re-gridded scans push_rescan_merge_msgs[_dev] merge into one LaserScan each: per stream its
+        group (< len(max_age)) or RESCAN_MERGE_NONE, and per group how many merge pushes a member's grid is kept for.
+        Replaces every group; every held grid starts empty."""
+        g = np.ascontiguousarray(group_of_stream, dtype=np.uint32)
+        assert g.shape == (self.n_streams,)
+        a = np.ascontiguousarray(max_age, dtype=np.uint32).reshape(-1)
+        self._ctx._check(self._fn("set_rescan_merges")(self._h, _p(g), _p(a) if a.size else None, int(a.size)))
+
     def _msgs(self, name, params, clock_offset_ns, msgs, packed, cloud_params=None):
         ns = self.n_streams * self.max_scans
         if msgs is None:  # room for every slot's largest message
@@ -1241,10 +1268,11 @@ class CapsuleStreamSession:
             self._h, C.byref(pi), C.byref(params), int(clock_offset_ns), _p(msgs), int(capacity), _p(msg_offsets),
             _p(msg_sizes), _p(total_bytes), _p(scans_per_stream), _p(stream)))
 
-    def _push_msgs_pair(self, name, second_bytes, data, counts, params, cloud_params, clock_offset_ns,
-                        sample_duration_us, rx_us, timing, chunk_bytes, msgs, second_msgs):
-        """A push returning two packed message sets (entry point `name`): the LaserScans into msgs, the second set into
-        second_msgs; None: a buffer that always fits, second_bytes per slot for the second set."""
+    def _push_msgs_sets(self, name, second_bytes, data, counts, params, cloud_params, clock_offset_ns,
+                        sample_duration_us, rx_us, timing, chunk_bytes, msgs, second_msgs, merged=None, n_groups=None):
+        """A push returning packed message sets (entry point `name`): the LaserScans into msgs, the second set into
+        second_msgs; None: a buffer that always fits, second_bytes per slot for the second set.  With n_groups (a merge
+        push) a third set, by group, into merged (None: one that always fits)."""
         assert isinstance(data, np.ndarray) and data.dtype == np.uint8 and data.flags.c_contiguous
         cnt = np.ascontiguousarray(counts, dtype=np.uint32)
         assert cnt.shape == (self.n_streams,)
@@ -1254,10 +1282,15 @@ class CapsuleStreamSession:
             msgs = np.zeros(ns * ((288 + 32 + 8 * self.max_nodes + 4 + 15) // 16 * 16), np.uint8)
         if second_msgs is None:
             second_msgs = np.zeros(ns * ((second_bytes + 15) // 16 * 16), np.uint8)
+        bufs = [(msgs, ns), (second_msgs, ns)]
+        if n_groups is not None:
+            if merged is None:
+                merged = np.zeros(max(n_groups, 1) * ((second_bytes + 15) // 16 * 16), np.uint8)
+            bufs.append((merged, n_groups))
         out = []
-        for buf in (msgs, second_msgs):
+        for buf, n in bufs:
             assert buf.dtype == np.uint8 and buf.flags.c_contiguous
-            t = dict(msgs=buf, msg_offsets=np.zeros(ns, np.uint64), msg_sizes=np.zeros(ns, np.uint32),
+            t = dict(msgs=buf, msg_offsets=np.zeros(n, np.uint64), msg_sizes=np.zeros(n, np.uint32),
                      total=np.zeros(1, np.uint64))
             t["out"] = MsgsOut(_p(buf).value, buf.size, _p(t["msg_offsets"]).value, _p(t["msg_sizes"]).value,
                                _p(t["total"]).value)
@@ -1265,12 +1298,12 @@ class CapsuleStreamSession:
         sps = np.zeros(self.n_streams, np.uint32)
         pi = self._push_input(data, cnt, sample_duration_us, rx, timing, chunk_bytes)
         rc = self._fn(name)(self._h, C.byref(pi), C.byref(params), C.byref(cloud_params), int(clock_offset_ns),
-                            C.byref(out[0]["out"]), C.byref(out[1]["out"]), _p(sps))
+                            *[C.byref(t["out"]) for t in out], _p(sps))
         if rc != RESULT_INSUFFICIENT_MEMORY:
             self._ctx._check(rc)
         res = [dict(msgs=t["msgs"], msg_offsets=t["msg_offsets"], msg_sizes=t["msg_sizes"],
                     total_bytes=int(t["total"][0]), result=rc) for t in out]
-        return res[0], res[1], sps
+        return (*res, sps)
 
     def push_scan_cloud_msgs(self, data, counts, params: ScanParams, cloud_params: ScanCloudParams, clock_offset_ns=0,
                              sample_duration_us=31, rx_us=None, timing: "Timing | None" = None, chunk_bytes=None,
@@ -1281,7 +1314,7 @@ class CapsuleStreamSession:
         are the capacities; None: ones that always fit).  Returns (scans, clouds, scans_per_stream): scans and clouds
         as the packed dicts of push_laserscan_msgs(packed=True), each with the call's result, which is
         RESULT_INSUFFICIENT_MEMORY rather than an exception when either buffer is too small (the push is done)."""
-        return self._push_msgs_pair("push_scan_cloud_msgs", _scan_cloud_bound(cloud_params.channels, self.max_nodes),
+        return self._push_msgs_sets("push_scan_cloud_msgs", _scan_cloud_bound(cloud_params.channels, self.max_nodes),
                                     data, counts, params, cloud_params, clock_offset_ns, sample_duration_us, rx_us,
                                     timing, chunk_bytes, msgs, cloud_msgs)
 
@@ -1304,7 +1337,7 @@ class CapsuleStreamSession:
         sensor_msgs/LaserScan and as the LaserScan each re-grids to (rescan_msgs with cloud_params), windowed per
         stream by set_rescan_windows.  Buffers and returns (scans, rescans, scans_per_stream) as
         push_scan_cloud_msgs."""
-        return self._push_msgs_pair("push_rescan_msgs", 288 + 36 + 4 * RESCAN_MAX_BINS, data, counts, params,
+        return self._push_msgs_sets("push_rescan_msgs", 288 + 36 + 4 * RESCAN_MAX_BINS, data, counts, params,
                                     cloud_params, clock_offset_ns, sample_duration_us, rx_us, timing, chunk_bytes, msgs,
                                     rescan_msgs)
 
@@ -1316,6 +1349,26 @@ class CapsuleStreamSession:
         self._ctx._check(self._fn("push_rescan_msgs_dev")(
             self._h, C.byref(pi), C.byref(params), C.byref(cloud_params), int(clock_offset_ns), C.byref(scans),
             C.byref(rescans), _p(scans_per_stream), _p(stream)))
+
+    def push_rescan_merge_msgs(self, data, counts, params: ScanParams, cloud_params: ScanCloudParams, n_groups,
+                               clock_offset_ns=0, sample_duration_us=31, rx_us=None, timing: "Timing | None" = None,
+                               chunk_bytes=None, msgs=None, rescan_msgs=None, merged_msgs=None):
+        """push_rescan_msgs, plus one merged LaserScan per group of set_rescan_merges (n_groups of them) that has news:
+        the per-bin minimum of the members' held grids.  Returns (scans, rescans, merged, scans_per_stream), merged
+        packed by group as the others by slot."""
+        return self._push_msgs_sets("push_rescan_merge_msgs", 288 + 36 + 4 * RESCAN_MAX_BINS, data, counts, params,
+                                    cloud_params, clock_offset_ns, sample_duration_us, rx_us, timing, chunk_bytes, msgs,
+                                    rescan_msgs, merged_msgs, n_groups)
+
+    def push_rescan_merge_msgs_dev(self, data, counts, params: ScanParams, cloud_params: ScanCloudParams,
+                                   clock_offset_ns, scans: MsgsOut, rescans: MsgsOut, merged: MsgsOut,
+                                   scans_per_stream, sample_duration_us=31, rx_us=None,
+                                   timing: "Timing | None" = None, chunk_bytes=None, stream=None):
+        """Device addresses, as push_rescan_msgs_dev; merged is indexed by group."""
+        pi = self._push_input(data, counts, sample_duration_us, rx_us, timing, chunk_bytes)
+        self._ctx._check(self._fn("push_rescan_merge_msgs_dev")(
+            self._h, C.byref(pi), C.byref(params), C.byref(cloud_params), int(clock_offset_ns), C.byref(scans),
+            C.byref(rescans), C.byref(merged), _p(scans_per_stream), _p(stream)))
 
     def nodes(self, apply_ascend=True, per_stream=None, packed=False, nodes=None):
         """The node buffers RealLidarDriver::grab_scan_data would return for every scan the last push published: per

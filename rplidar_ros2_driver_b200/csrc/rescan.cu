@@ -14,6 +14,12 @@
 // definition and CPU restatement is oracle/rescan_window_oracle.py.  It runs behind rescan_kernel, reads each grid from
 // the message rescan_kernel wrote (or builds it with the same loop, rescan_slot_grid, when the message did not fit),
 // writes W over it, and keeps the last observations - 1 grids of the stream in a ring in device memory.
+//
+// The merged scans (DESIGN.md 5.7.1 "Merged scans from the push"), a scan merger over the same grids, whose definition
+// and CPU restatement is oracle/rescan_merge_oracle.py: rescan_hold_kernel keeps each grouped stream's newest written
+// re-grid message's ranges and stamp in its held row, per chunk behind the window kernel; at the end of the push
+// rescan_merge_dir_kernel places one message per group that has news and rescan_merge_kernel writes it, the per-bin
+// minimum of the contributors' held rows (merge_bins, shared with the stateless rescan_merge_batch_kernel).
 #include <algorithm>
 
 #include "beam_point.cuh"
@@ -70,6 +76,17 @@ __device__ __forceinline__ void rescan_slot_grid(const ScanCloudArgs& c, uint32_
   __syncthreads();
 }
 
+// The re-grid message's members behind its header, by threads 0 .. 7: angle_min, angle_max, angle_increment,
+// time_increment 0, scan_time, range_min, range_max, the ranges' count
+__device__ __forceinline__ void put_rescan_fields(uint8_t* body, const RescanGrid& g) {
+  const uint32_t tid = threadIdx.x;
+  if (tid < 8) {
+    const float f = tid == 0 ? g.angle_min : tid == 1 ? g.angle_max : tid == 2 ? g.angle_increment
+                    : tid == 4 ? g.scan_time : tid == 5 ? g.range_min : tid == 6 ? g.range_max : 0.0f;
+    put32(body + 4 * tid, tid == 7 ? g.bins : __float_as_uint(f));
+  }
+}
+
 __global__ void __launch_bounds__(RT) rescan_kernel(const __grid_constant__ RescanArgs a) {
   __shared__ uint32_t s_bins[kRescanMaxBins];
   const ScanCloudArgs& c = a.c;
@@ -91,12 +108,7 @@ __global__ void __launch_bounds__(RT) rescan_kernel(const __grid_constant__ Resc
         put32(msg + 8, nsec);
         put32(body + 32 + 4 * g.bins, 0u);  // intensities: none
       }
-      if (tid < 8) {  // angle_min, angle_max, angle_increment, time_increment 0, scan_time, range_min, range_max, ranges'
-                      // count
-        const float f = tid == 0 ? g.angle_min : tid == 1 ? g.angle_max : tid == 2 ? g.angle_increment
-                        : tid == 4 ? g.scan_time : tid == 5 ? g.range_min : tid == 6 ? g.range_max : 0.0f;
-        put32(body + 4 * tid, tid == 7 ? g.bins : __float_as_uint(f));
-      }
+      put_rescan_fields(body, g);
       for (uint32_t b = tid; b < g.bins; b += RT) put32(body + 32 + 4 * b, s_bins[b]);
     } else {
       uint32_t* row = reinterpret_cast<uint32_t*>(a.out) + (size_t)i * g.bins;
@@ -201,6 +213,151 @@ __global__ void __launch_bounds__(RT) rescan_window_batch_kernel(const float* __
   }
 }
 
+// M (oracle/rescan_merge_oracle.py) at bin b: the least of the bits m and bin b of every row row(j), j < n, that is not
+// null.  Re-grid values are >= +0 and never NaN, so the unsigned min of the bits is the float min, in any order.
+template <class Row>
+__device__ __forceinline__ uint32_t merge_bins(uint32_t m, uint32_t n, uint32_t b, Row row) {
+  for (uint32_t j = 0; j < n; ++j)
+    if (const float* r = row(j)) m = min(m, __float_as_uint(r[b]));
+  return m;
+}
+
+// One CTA per grouped stream of the chunk (RescanHoldArgs)
+__global__ void __launch_bounds__(RT) rescan_hold_kernel(const __grid_constant__ RescanHoldArgs a) {
+  const ScanCloudArgs& c = a.r.c;
+  const uint32_t tid = threadIdx.x;
+  for (uint32_t q = blockIdx.x; q < a.n; q += gridDim.x) {
+    const uint32_t s = a.streams[q] - a.stream0;
+    uint32_t i = kRescanMergeNone;  // the newest slot whose re-grid message was written
+    for (uint32_t k = c.m.max_scans; k-- > 0;)
+      if (c.m.sizes[s * c.m.max_scans + k]) {
+        i = s * c.m.max_scans + k;
+        break;
+      }
+    if (i == kRescanMergeNone) continue;  // the held grid stays as it was
+    const StreamMsgHeader& h = c.transform ? c.cloud_hdr[s] : c.m.hdr[s];
+    const uint8_t* msg = c.m.out + (c.m.offsets[i] - c.m.out_base);
+    const uint32_t* ranges = reinterpret_cast<const uint32_t*>(msg + h.bytes + 32);
+    float* row = a.rows + (size_t)a.row[s] * kRescanMaxBins;
+    for (uint32_t b = tid; b < a.r.grid[s].bins; b += RT) row[b] = __uint_as_float(ranges[b]);
+    if (tid == 0)
+      a.held[s] = RescanHeld{*reinterpret_cast<const uint32_t*>(msg + 4), *reinterpret_cast<const uint32_t*>(msg + 8),
+                             a.seq, c.transform ? kHeldTargetHdr : kHeldScanHdr};
+  }
+}
+
+__device__ __forceinline__ bool contributes(const RescanMergeArgs& a, const RescanHeld& h, uint32_t g) {
+  return h.hdr && a.seq - h.seq <= a.max_age[g];
+}
+
+// the header stream s's held grid's message took
+__device__ __forceinline__ const StreamMsgHeader& held_header(const RescanMergeArgs& a, uint32_t s) {
+  return (a.held[s].hdr == kHeldTargetHdr ? a.hdr_target : a.hdr_scan)[s];
+}
+
+// One CTA over the groups in tiles of RT, as push_msg_dir_kernel over slots
+__global__ void __launch_bounds__(RT) rescan_merge_dir_kernel(const __grid_constant__ RescanMergeArgs a) {
+  __shared__ unsigned long long s_warp[RT / 32];
+  __shared__ unsigned long long s_fit_end, s_last_end;
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  if (tid == 0) s_fit_end = s_last_end = 0;
+  __syncthreads();
+  unsigned long long carry = 0;
+  for (uint32_t g0 = 0; g0 < a.n_groups; g0 += RT) {
+    const uint32_t g = g0 + tid;
+    uint32_t size = 0;
+    if (g < a.n_groups) {
+      bool publish = false;
+      uint32_t pick = kRescanMergeNone, sec = 0, nsec = 0;
+      for (uint32_t j = a.begin[g]; j < a.begin[g + 1]; ++j) {  // ascending: a tie keeps the lowest index
+        const uint32_t s = a.members[j];
+        const RescanHeld h = a.held[s];
+        if (!contributes(a, h, g)) continue;
+        publish |= h.seq == a.seq;
+        if (pick == kRescanMergeNone || h.sec > sec || (h.sec == sec && h.nanosec > nsec)) {
+          pick = s;
+          sec = h.sec;
+          nsec = h.nanosec;
+        }
+      }
+      if (!publish) pick = kRescanMergeNone;
+      else size = held_header(a, pick).bytes + 36u + 4u * a.grid[pick].bins;
+      a.pick[g] = pick;
+    }
+    const unsigned long long v = (size + 15u) & ~15u;
+    unsigned long long inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned long long u = __shfl_up_sync(0xffffffffu, inc, o);
+      if (lane >= (uint32_t)o) inc += u;
+    }
+    if (lane == 31) s_warp[warp] = inc;
+    __syncthreads();
+    unsigned long long base = 0, tile = 0;
+    for (uint32_t w = 0; w < RT / 32; ++w) {
+      const unsigned long long x = s_warp[w];
+      if (w < warp) base += x;
+      tile += x;
+    }
+    const unsigned long long off = carry + base + inc - v;
+    if (g < a.n_groups) {
+      const bool fits = size != 0 && off + size <= a.capacity;
+      a.offsets[g] = off;
+      a.sizes[g] = fits ? size : 0u;
+      if (size) atomicMax(&s_last_end, off + size);
+      if (fits) atomicMax(&s_fit_end, off + size);
+    }
+    carry += tile;
+    __syncthreads();  // s_warp is rewritten by the next tile
+  }
+  if (tid == 0) {
+    *a.total = s_last_end;
+    if (a.fit_end) *a.fit_end = s_fit_end;
+  }
+}
+
+// One CTA per group whose message the directory placed and that fits
+__global__ void __launch_bounds__(RT) rescan_merge_kernel(const __grid_constant__ RescanMergeArgs a) {
+  const uint32_t tid = threadIdx.x;
+  for (uint32_t g = blockIdx.x; g < a.n_groups; g += gridDim.x) {
+    if (a.sizes[g] == 0) continue;
+    const uint32_t p = a.pick[g];
+    const StreamMsgHeader& h = held_header(a, p);
+    const RescanGrid& gr = a.grid[p];
+    uint8_t* msg = a.out + a.offsets[g];
+    put_header<RT>(msg, h);
+    uint8_t* body = msg + h.bytes;
+    if (tid == 0) {
+      const RescanHeld x = a.held[p];
+      put32(msg + 4, x.sec);
+      put32(msg + 8, x.nanosec);
+      put32(body + 32 + 4 * gr.bins, 0u);  // intensities: none
+    }
+    put_rescan_fields(body, gr);
+    const uint32_t j0 = a.begin[g], n = a.begin[g + 1] - j0;
+    for (uint32_t b = tid; b < gr.bins; b += RT)
+      put32(body + 32 + 4 * b, merge_bins(gr.seed, n, b, [&](uint32_t j) -> const float* {
+              const uint32_t s = a.members[j0 + j];
+              return contributes(a, a.held[s], g) ? a.rows + (size_t)a.row[s] * kRescanMaxBins : nullptr;
+            }));
+  }
+}
+
+// one thread per (group, bin) of the stateless form
+__global__ void __launch_bounds__(RT) rescan_merge_batch_kernel(const float* __restrict__ in,
+                                                                const uint32_t* __restrict__ row_group, uint32_t n_rows,
+                                                                uint32_t n_groups, uint32_t bins, uint32_t seed,
+                                                                float* __restrict__ out) {
+  const unsigned long long total = (unsigned long long)n_groups * bins;
+  for (unsigned long long e = blockIdx.x * (unsigned long long)RT + threadIdx.x; e < total;
+       e += (unsigned long long)gridDim.x * RT) {
+    const uint32_t g = (uint32_t)(e / bins), b = (uint32_t)(e - (unsigned long long)g * bins);
+    out[e] = __uint_as_float(merge_bins(seed, n_rows, b, [&](uint32_t r) -> const float* {
+      return __ldg(row_group + r) == g ? in + (size_t)r * bins : nullptr;
+    }));
+  }
+}
+
 }  // namespace
 
 cudaError_t launch_rescan(const RescanArgs& a, int num_sms, cudaStream_t stream) {
@@ -231,6 +388,27 @@ cudaError_t launch_rescan_window_batch(const float* in, uint32_t n_scans, uint32
   if (total == 0) return cudaSuccess;
   const unsigned long long blocks = std::min<unsigned long long>((total + RT - 1) / RT, (unsigned long long)num_sms * 8);
   rescan_window_batch_kernel<<<(unsigned)blocks, RT, 0, stream>>>(in, n_scans, bins, observations, statistic, out);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_rescan_hold(const RescanHoldArgs& a, int num_sms, cudaStream_t stream) {
+  if (a.n == 0) return cudaSuccess;
+  rescan_hold_kernel<<<(int)std::min<uint32_t>(a.n, (uint32_t)num_sms * 8u), RT, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_rescan_merge(const RescanMergeArgs& a, int num_sms, cudaStream_t stream) {
+  rescan_merge_dir_kernel<<<1, RT, 0, stream>>>(a);
+  if (a.n_groups) rescan_merge_kernel<<<(int)std::min<uint32_t>(a.n_groups, (uint32_t)num_sms * 8u), RT, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_rescan_merge_batch(const float* in, const uint32_t* row_group, uint32_t n_rows, uint32_t n_groups,
+                                      uint32_t bins, uint32_t seed, float* out, int num_sms, cudaStream_t stream) {
+  const unsigned long long total = (unsigned long long)n_groups * bins;
+  if (total == 0) return cudaSuccess;
+  const unsigned long long blocks = std::min<unsigned long long>((total + RT - 1) / RT, (unsigned long long)num_sms * 8);
+  rescan_merge_batch_kernel<<<(unsigned)blocks, RT, 0, stream>>>(in, row_group, n_rows, n_groups, bins, seed, out);
   return cudaGetLastError();
 }
 

@@ -59,4 +59,58 @@ cudaError_t launch_rescan_window(const RescanWindowArgs& a, int num_sms, cudaStr
 cudaError_t launch_rescan_window_batch(const float* in, uint32_t n_scans, uint32_t bins, uint32_t observations,
                                        uint32_t statistic, float* out, int num_sms, cudaStream_t stream);
 
+// ---- merged scans from the push (oracle/rescan_merge_oracle.py M; a scan merger over the re-gridded scans) ----------
+constexpr uint32_t kRescanMergeNone = 0xFFFFFFFFu;  // a stream in no group, a row of no group
+
+// A stream's held grid as the kernels keep it: its ranges in a row of kRescanMaxBins floats, the stamp of the re-grid
+// message they came from, the merge push that wrote it (seq >= 1) and the header table that message took: hdr 0,
+// nothing held; 1, the LaserScan frame's; 2, the target frame's (RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS).  The set calls
+// that change either table empty the held grids, so the message is rebuilt byte for byte.
+constexpr uint32_t kHeldScanHdr = 1, kHeldTargetHdr = 2;
+struct RescanHeld {
+  uint32_t sec, nanosec, seq, hdr;
+};
+
+// A push's held grids over the chunk's grouped streams, one CTA per stream, behind rescan_kernel and the window kernel:
+// r as theirs (r.c.m.out / offsets / sizes / out_base: the re-grid messages as this chunk wrote them).  The newest slot
+// of the stream whose re-grid message was written (size > 0) gives the held row its ranges and stamp.
+struct RescanHoldArgs {
+  RescanArgs r;
+  const uint32_t* streams;  // [n] the session indices of the chunk's grouped streams
+  uint32_t n, stream0;      // stream0: the chunk's first stream
+  const uint32_t* row;      // [streams] at the chunk's first stream: the stream's held row
+  RescanHeld* held;         // [streams] at the chunk's first stream
+  float* rows;              // [held rows][kRescanMaxBins]
+  uint32_t seq;             // this merge push's number
+};
+cudaError_t launch_rescan_hold(const RescanHoldArgs& a, int num_sms, cudaStream_t stream);
+
+// The end of a merge push, over the session's groups: the directory (one CTA) decides each group's message, then the
+// merge kernel (one CTA per message) writes it.  Group g's members are members[begin[g] .. begin[g + 1]) (session
+// indices, ascending); a member contributes when it holds a grid of a push within max_age[g] of this one (seq -
+// held.seq <= max_age[g]); the group publishes when a member's grid is from this push.  The message is the re-grid
+// message of the contributor with the newest stamp (lowest index on a tie) -- the header its held grid took
+// (hdr_scan or hdr_target, as RescanHeld::hdr says) with that stamp, then its entry's fields -- with M over the
+// contributors' rows in place of its ranges.  Packed as the re-grid messages: offsets the exclusive scan of the sizes
+// rounded up to 16, sizes[g] the size when it fits capacity (else 0), *total the end of the last.
+struct RescanMergeArgs {
+  const uint32_t *members, *begin, *max_age;
+  uint32_t n_groups, seq;
+  const uint32_t* row;                 // [n_streams]
+  const RescanHeld* held;              // [n_streams]
+  const float* rows;
+  const StreamMsgHeader *hdr_scan, *hdr_target;  // [n_streams] each (hdr_target nullable: no transforms set)
+  const RescanGrid* grid;              // [n_streams]
+  uint32_t* pick;                      // [n_groups] the directory's choice for the merge kernel (kRescanMergeNone: none)
+  unsigned long long capacity;
+  unsigned long long *offsets, *total;  // offsets [n_groups]
+  uint32_t* sizes;                      // [n_groups]
+  unsigned long long* fit_end;          // nullable: the end of the last message that fits
+  uint8_t* out;
+};
+cudaError_t launch_rescan_merge(const RescanMergeArgs& a, int num_sms, cudaStream_t stream);
+// stateless: out[g] ([n_groups][bins]) is M over the rows r of in ([n_rows][bins]) with row_group[r] == g, from `seed`
+cudaError_t launch_rescan_merge_batch(const float* in, const uint32_t* row_group, uint32_t n_rows, uint32_t n_groups,
+                                      uint32_t bins, uint32_t seed, float* out, int num_sms, cudaStream_t stream);
+
 }  // namespace rpl

@@ -1059,6 +1059,29 @@ rpl_result rpl_rescan_window_batch_dev(rpl_ctx* c, const rpl_rescan_window* wind
   return RPL_RESULT_OK;
 }
 
+rpl_result rpl_rescan_merge_batch_dev(rpl_ctx* c, const rpl_rescan_settings* settings, const float* in,
+                                      const uint32_t* row_group, uint32_t n_rows, uint32_t n_groups, float* out,
+                                      void* stream) {
+  if (!c) return RPL_RESULT_INVALID_DATA;
+  if (!settings || !out || (n_rows && (!in || !row_group))) {
+    c->err = "null settings, in, row_group or out";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  if (!rescan_ok(c, *settings)) return RPL_RESULT_INVALID_DATA;
+  if ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(row_group) | reinterpret_cast<uintptr_t>(out)) & 3u) {
+    c->err = "in, row_group and out must be 4-byte aligned";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  cudaStream_t st;
+  if (!enter_device(c, stream, &st)) return RPL_RESULT_OPERATION_FAIL;
+  const rpl::RescanGrid g = rescan_grid(*settings, false);
+  if ((unsigned long long)n_groups * g.bins == 0) return RPL_RESULT_OK;
+  RPL_CUDA(c, rpl::launch_rescan_merge_batch(in, row_group, n_rows, n_groups, g.bins, g.seed, out, c->num_sms, st),
+           RPL_RESULT_OPERATION_FAIL);
+  c->launches++;
+  return RPL_RESULT_OK;
+}
+
 // ---- host-buffer batch: chunked over the two lanes so that the H2D copy of chunk i+1, the
 // kernels of chunk i and the D2H copy of chunk i-1 overlap ---------------------------------
 rpl_result rpl_scan_batch(rpl_ctx* c, const rpl_node_hq* nodes, const uint32_t* counts,
@@ -1872,6 +1895,16 @@ struct rpl_capsule_stream {
   uint32_t* win_streams = nullptr;              // [n_streams] device, win_streams_host.size() used
   std::vector<uint32_t> win_streams_host;
   std::vector<rpl::RescanWindow> win_layout_host;  // as win
+  // the groups merged into one scan each (rpl_capsule_stream_set_rescan_merges; mg_set false until the first call), in
+  // one device block (MergeTables): each group's members ascending by group (mg_begin), the grouped streams ascending
+  // (mg_streams_host; a chunk's hold launch takes its run of them), and the merge pushes that succeeded (mg_seq).  The
+  // host form stages its merged messages and their directory in mg_stage.
+  bool mg_set = false;
+  uint32_t mg_groups = 0, mg_seq = 0;
+  std::vector<uint32_t> mg_members_host, mg_begin_host, mg_streams_host;
+  unsigned char* mg_block = nullptr;
+  unsigned char* mg_stage = nullptr;
+  size_t mg_stage_bytes = 0;
   unsigned char* node_work = nullptr;           // the tables of a nodes call (NodeWork)
   // [n_streams] device, zeroed at create: what every push decoded and lost (rpl_capsule_stream_counters); a stream's
   // record is written by the one CTA of each kernel that serves the stream
@@ -2332,8 +2365,28 @@ rpl_result stream_cloud_chunk(rpl_ctx* c, Lane& l, rpl::ScanBatchArgs a, const r
   return scratch_leave(c, l, st);
 }
 
+// The device tables of the merge groups (rpl_capsule_stream_set_rescan_merges), carved from the session's mg_block:
+// each stream's held row (kRescanMergeNone: in no group) and held grid, the grouped streams ascending, the members by
+// group with each group's first member, the groups' max_age, the directory's choices, and the held rows
+struct MergeTables {
+  uint32_t* row;
+  rpl::RescanHeld* held;
+  uint32_t *streams, *members, *begin, *max_age, *pick;
+  float* rows;
+};
+MergeTables merge_tables_layout(Carve& k, uint32_t n_streams, uint32_t n_grouped, uint32_t n_groups) {
+  return MergeTables{k.take<uint32_t>(n_streams), k.take<rpl::RescanHeld>(n_streams), k.take<uint32_t>(n_grouped),
+                     k.take<uint32_t>(n_grouped), k.take<uint32_t>(n_groups + 1), k.take<uint32_t>(n_groups),
+                     k.take<uint32_t>(n_groups), k.take<float>((size_t)n_grouped * rpl::kRescanMaxBins)};
+}
+MergeTables merge_tables(const rpl_capsule_stream* cs) {
+  Carve k{cs->mg_block};
+  return merge_tables_layout(k, cs->n_streams, (uint32_t)cs->mg_streams_host.size(), cs->mg_groups);
+}
+
 // The re-grid of a LaserScan push's chunk (rpl_capsule_stream_push_rescan_msgs*), the session's tables at the chunk's
-// first stream: the entries and their bins, and the chunk's streams with a window and their windows
+// first stream: the entries and their bins, the chunk's streams with a window and their windows, and for a merge push
+// (rpl_capsule_stream_push_rescan_merge_msgs*) its grouped streams and their held grids
 struct ChunkRescans {
   const rpl::RescanGrid* grid;  // nullptr: not a re-gridding push
   const uint32_t* bins;
@@ -2343,10 +2396,29 @@ struct ChunkRescans {
   const rpl::RescanWindow* win;
   uint2* state;
   float* ring;
+  const uint32_t* hold_streams;  // [n_hold] session indices
+  uint32_t n_hold, seq;          // seq: the merge push's number
+  const uint32_t* hold_row;
+  rpl::RescanHeld* held;
+  float* held_rows;
 };
 
-ChunkRescans rescan_chunk(const rpl_capsule_stream* cs, uint32_t s0, uint32_t ns) {
+ChunkRescans rescan_chunk(const rpl_capsule_stream* cs, uint32_t s0, uint32_t ns, bool merge = false) {
   ChunkRescans r{};
+  r.stream0 = s0;
+  if (merge) {
+    const std::vector<uint32_t>& gs = cs->mg_streams_host;
+    const auto lo = std::lower_bound(gs.begin(), gs.end(), s0), hi = std::lower_bound(gs.begin(), gs.end(), s0 + ns);
+    r.n_hold = (uint32_t)(hi - lo);
+    if (r.n_hold) {
+      const MergeTables t = merge_tables(cs);
+      r.hold_streams = t.streams + (lo - gs.begin());
+      r.seq = cs->mg_seq + 1;
+      r.hold_row = t.row + s0;
+      r.held = t.held + s0;
+      r.held_rows = t.rows;
+    }
+  }
   r.grid = cs->rescan + s0;
   r.bins = cs->rescan_bins + s0;
   for (uint32_t s = s0; s < s0 + ns && !r.any; ++s) r.any = cs->rescan_host[s].enabled != 0;
@@ -2355,7 +2427,6 @@ ChunkRescans rescan_chunk(const rpl_capsule_stream* cs, uint32_t s0, uint32_t ns
   r.n_win = (uint32_t)(hi - lo);
   if (r.n_win) {
     r.streams = cs->win_streams + (lo - ws.begin());
-    r.stream0 = s0;
     r.win = cs->win + s0;
     r.state = cs->win_state + s0;
     r.ring = cs->win_ring;
@@ -2461,6 +2532,19 @@ rpl_result scan_cloud_push_write(rpl_ctx* c, rpl::ScanCloudArgs a, const ChunkSc
       wa.state = q.state;
       wa.ring = q.ring;
       RPL_CUDA(c, rpl::launch_rescan_window(wa, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+      c->launches++;
+    }
+    if (q.n_hold) {  // then the held grids, from the messages as published
+      rpl::RescanHoldArgs ha{};
+      ha.r = ra;
+      ha.streams = q.hold_streams;
+      ha.n = q.n_hold;
+      ha.stream0 = q.stream0;
+      ha.row = q.hold_row;
+      ha.held = q.held;
+      ha.rows = q.held_rows;
+      ha.seq = q.seq;
+      RPL_CUDA(c, rpl::launch_rescan_hold(ha, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
       c->launches++;
     }
     return RPL_RESULT_OK;
@@ -2671,8 +2755,10 @@ struct HostMsgs {
   cudaEvent_t proj_dir_order;
   const rpl::StreamMsgHeader* proj_hdr;  // RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS: the session's resolved headers, rows
   const float4* proj_xf;
-  // a re-gridding push: its session (rescan_chunk), whose re-grid messages take the projection's members above
+  // a re-gridding push: its session (rescan_chunk), whose re-grid messages take the projection's members above; merge:
+  // a merge push, which holds the grouped streams' grids
   const rpl_capsule_stream* rescan;
+  bool merge;
 };
 
 // Runs a host call's n_streams streams through capsule_stream_chunk, `chunk` streams at a time round-robin over the
@@ -2802,7 +2888,7 @@ rpl_result push_host(rpl_ctx* c, const HostWire& h, uint32_t n_streams, uint32_t
         m.proj = ChunkScanClouds{hm->proj, hm->kept + so, d.pmsgs, hm->clouds->capacity, hm->proj_carry, d.poffs,
                                  d.pextent, nullptr, d.psizes, hm->proj_extent_host + 3 * li, hm->proj_dir_order,
                                  hm->proj_hdr ? hm->proj_hdr + s0 : nullptr, hm->proj_xf ? hm->proj_xf + 3 * s0 : nullptr};
-      if (proj && hm->rescan) m.proj.rescan = rescan_chunk(hm->rescan, s0, ns);
+      if (proj && hm->rescan) m.proj.rescan = rescan_chunk(hm->rescan, s0, ns, hm->merge);
     }
     const rpl_result r = capsule_stream_chunk(c, l, l.stream, d.w, ns, d.in, d.counts, h.sample_duration_us, h.params,
                                               d.ranges, d.intens, d.beams, d.inc, d.sps, h.sp ? &sp : nullptr,
@@ -3200,7 +3286,71 @@ struct PushMsgs {
   const rpl::StreamMsgHeader* proj_hdr;  // RPL_SCAN_CLOUD_PER_STREAM_TRANSFORMS: the session's resolved headers, rows
   const float4* proj_xf;
   bool rescan;  // a re-gridding push: clouds are its re-grid messages (ChunkScanClouds::rescan)
+  const rpl_msgs_out* merged;  // a merge push's merged scans, by group (nullptr: not a merge push)
 };
+
+// The host form's staging of a merge push (the session's mg_stage): the directory {fit end, total}, offsets and sizes,
+// then the merged messages
+struct MergeStage {
+  unsigned long long *dir, *offsets;
+  uint32_t* sizes;
+  uint8_t* msgs;
+};
+MergeStage merge_stage_layout(Carve& k, uint32_t n_groups) {
+  return MergeStage{k.take<unsigned long long>(2), k.take<unsigned long long>(n_groups), k.take<uint32_t>(n_groups),
+                    k.take<uint8_t>(0)};
+}
+
+// The end of a merge push, once every chunk has held its grouped streams' grids (on st; the host form's lanes are
+// drained): the directory over the groups and the merged messages, into the caller's arrays (dev) or staged in the
+// session's mg_stage and copied back (the directory, then the messages that fit)
+rpl_result rescan_merge_end(rpl_capsule_stream* cs, const PushMsgs& pm, bool dev, cudaStream_t st) {
+  rpl_ctx* c = cs->c;
+  const rpl_msgs_out& o = *pm.merged;
+  const MergeTables t = merge_tables(cs);
+  const uint32_t G = cs->mg_groups;
+  rpl::RescanMergeArgs a{};
+  a.members = t.members;
+  a.begin = t.begin;
+  a.max_age = t.max_age;
+  a.n_groups = G;
+  a.seq = cs->mg_seq + 1;
+  a.row = t.row;
+  a.held = t.held;
+  a.rows = t.rows;
+  a.hdr_scan = cs->msg_hdr;
+  a.hdr_target = cs->xf_hdr;
+  a.grid = cs->rescan;
+  a.pick = t.pick;
+  a.capacity = o.capacity;
+  using u64 = unsigned long long;
+  if (dev) {
+    a.offsets = reinterpret_cast<u64*>(o.msg_offsets);
+    a.sizes = o.msg_sizes;
+    a.total = reinterpret_cast<u64*>(o.total_bytes);
+    a.out = o.msgs;
+  } else {
+    Carve k{cs->mg_stage};
+    const MergeStage m = merge_stage_layout(k, G);
+    a.fit_end = m.dir;
+    a.total = m.dir + 1;
+    a.offsets = m.offsets;
+    a.sizes = m.sizes;
+    a.out = m.msgs;
+  }
+  RPL_CUDA(c, rpl::launch_rescan_merge(a, c->num_sms, st), RPL_RESULT_OPERATION_FAIL);
+  c->launches += G ? 2 : 1;
+  if (dev) return RPL_RESULT_OK;
+  u64 dir[2];  // {the end of the last message that fits, the total}
+  RPL_CUDA(c, cudaMemcpyAsync(dir, a.fit_end, 16, cudaMemcpyDeviceToHost, st), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaMemcpyAsync(o.msg_offsets, a.offsets, (size_t)G * 8, cudaMemcpyDeviceToHost, st),
+           RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaMemcpyAsync(o.msg_sizes, a.sizes, (size_t)G * 4, cudaMemcpyDeviceToHost, st), RPL_RESULT_OPERATION_FAIL);
+  RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);
+  *o.total_bytes = dir[1];
+  if (dir[0]) RPL_CUDA(c, cudaMemcpy(o.msgs, a.out, dir[0], cudaMemcpyDeviceToHost), RPL_RESULT_OPERATION_FAIL);
+  return RPL_RESULT_OK;
+}
 
 // A push of the kind the entry point takes (bytes: a byte push); sp: a stamped one.  Host arrays (dev false, stream
 // unused) run in the session's host chunks round-robin over the lanes, device arrays in its device chunks on `stream`.
@@ -3258,7 +3408,7 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
                                    pm->clouds->msg_sizes + so, nullptr, nullptr, pm->proj_hdr ? pm->proj_hdr + s0 : nullptr,
                                    pm->proj_xf ? pm->proj_xf + 3 * s0 : nullptr};
         if (pm->proj && pm->rescan)
-          m.proj.rescan = rescan_chunk(cs, s0, std::min(chunk, cs->n_streams - s0));
+          m.proj.rescan = rescan_chunk(cs, s0, std::min(chunk, cs->n_streams - s0), pm->merged != nullptr);
       }
       r = capsule_stream_chunk(c, c->lane[0], st, session_chunk(cs, s0, params, true, pm ? pm->cloud : nullptr),
                                std::min(chunk, cs->n_streams - s0), in + s0 * cs->in_stream, counts + s0,
@@ -3267,6 +3417,7 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
                                pm ? pm->w.inc + so : angle_increment ? angle_increment + so : nullptr,
                                scans_per_stream + s0, sp ? &chunk_sp : nullptr, pm ? &m : nullptr);
     }
+    if (r == RPL_RESULT_OK && pm && pm->merged) r = rescan_merge_end(cs, *pm, true, st);
   } else {
     for (uint32_t s = 0; s < cs->n_streams; ++s)
       if (counts[s] > cs->stride_in) {
@@ -3307,6 +3458,7 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
         hm.proj_hdr = pm->proj_hdr;
         hm.proj_xf = pm->proj_xf;
         if (pm->rescan) hm.rescan = cs;
+        hm.merge = pm->merged != nullptr;
       }
     }
     const HostWire h{in, counts, cs->in_stream, sample_duration_us, cs->max_nodes, cs->max_scans, params, ranges,
@@ -3314,6 +3466,7 @@ rpl_result stream_push(rpl_capsule_stream* cs, const uint8_t* in, const uint32_t
                      pm ? &hm : nullptr};
     r = push_host(c, h, cs->n_streams, chunk,
                   [&](Carve&, uint32_t s0) { return session_chunk(cs, s0, params, false, pm ? pm->cloud : nullptr); });
+    if (r == RPL_RESULT_OK && pm && pm->merged) r = rescan_merge_end(cs, *pm, false, c->lane[0].stream);
   }
   cs->parity ^= 1u;
   cs->prev_stamped = cs->carry_stamped = sp != nullptr;
@@ -3543,6 +3696,24 @@ rpl_result transforms_resolve(rpl_capsule_stream* cs, const std::vector<rpl_scan
   return RPL_RESULT_OK;
 }
 
+// Empties the held grids of the merge groups' streams `mask` takes in (nullptr: all), on `st`, when there are groups
+rpl_result merges_empty(rpl_capsule_stream* cs, const uint8_t* mask, cudaStream_t st) {
+  if (!cs->mg_block) return RPL_RESULT_OK;
+  rpl::RescanHeld* held = merge_tables(cs).held;
+  for (uint32_t s = 0; s < cs->n_streams;) {
+    if (mask && !mask[s]) {
+      ++s;
+      continue;
+    }
+    uint32_t e = s + 1;
+    while (e < cs->n_streams && (!mask || mask[e])) ++e;
+    RPL_CUDA(cs->c, cudaMemsetAsync(held + s, 0, (size_t)(e - s) * sizeof(rpl::RescanHeld), st),
+             RPL_RESULT_OPERATION_FAIL);
+    s = e;
+  }
+  return RPL_RESULT_OK;
+}
+
 // the transforms of the projected clouds: the masked entries and target frames replace the table's, all or none
 rpl_result stream_set_scan_cloud_transforms(rpl_capsule_stream* cs, const rpl_scan_cloud_transform* transforms,
                                             const char* const* target_frames, const uint8_t* stream_mask) {
@@ -3575,6 +3746,8 @@ rpl_result stream_set_scan_cloud_transforms(rpl_capsule_stream* cs, const rpl_sc
   if (!cs->xf_hdr) RPL_CUDA(c, dev_alloc(&cs->xf_hdr, cs->n_streams), RPL_RESULT_INSUFFICIENT_MEMORY);
   RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);  // a messages call may still read them
   if (const rpl_result r = transforms_resolve(cs, t, f); r != RPL_RESULT_OK) return r;
+  if (const rpl_result r = merges_empty(cs, stream_mask, c->lane[0].stream); r != RPL_RESULT_OK) return r;
+  RPL_CUDA(c, cudaStreamSynchronize(c->lane[0].stream), RPL_RESULT_OPERATION_FAIL);
   cs->xf_host = std::move(t);
   cs->xf_frames = std::move(f);
   return RPL_RESULT_OK;
@@ -3676,7 +3849,77 @@ rpl_result stream_set_rescan_windows(rpl_capsule_stream* cs, const rpl_rescan_wi
   RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
   RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);  // a push may still read them
   if (const rpl_result r = windows_layout(cs, cs->rescan_host, w, stream_mask); r != RPL_RESULT_OK) return r;
+  if (const rpl_result r = merges_empty(cs, stream_mask, c->lane[0].stream); r != RPL_RESULT_OK) return r;
+  RPL_CUDA(c, cudaStreamSynchronize(c->lane[0].stream), RPL_RESULT_OPERATION_FAIL);
   cs->win_host = std::move(w);
+  return RPL_RESULT_OK;
+}
+
+// the merge groups: a new layout replaces the old whole, every held grid empty, all or none
+rpl_result stream_set_rescan_merges(rpl_capsule_stream* cs, const uint32_t* group_of_stream, const uint32_t* max_age,
+                                    uint32_t n_groups) {
+  if (!cs) return RPL_RESULT_INVALID_DATA;
+  rpl_ctx* c = cs->c;
+  if (!group_of_stream || (n_groups && !max_age)) {
+    c->err = "null group_of_stream or max_age";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  if (n_groups > cs->n_streams) {
+    c->err = "n_groups exceeds n_streams";
+    return RPL_RESULT_INVALID_DATA;
+  }
+  std::vector<uint32_t> count(n_groups, 0), streams, row(cs->n_streams, rpl::kRescanMergeNone);
+  for (uint32_t s = 0; s < cs->n_streams; ++s) {
+    const uint32_t g = group_of_stream[s];
+    if (g == rpl::kRescanMergeNone) continue;
+    if (g >= n_groups) {
+      c->err = "a group index must be below n_groups or RPL_RESCAN_MERGE_NONE";
+      return RPL_RESULT_INVALID_DATA;
+    }
+    count[g]++;
+    row[s] = (uint32_t)streams.size();
+    streams.push_back(s);
+  }
+  for (uint32_t g = 0; g < n_groups; ++g) {
+    if (count[g] == 0) {
+      c->err = "every merge group needs a member";
+      return RPL_RESULT_INVALID_DATA;
+    }
+    if (max_age[g] > 65535) {
+      c->err = "max_age must be at most 65535";
+      return RPL_RESULT_INVALID_DATA;
+    }
+  }
+  std::vector<uint32_t> begin(n_groups + 1, 0), members(streams.size());
+  for (uint32_t g = 0; g < n_groups; ++g) begin[g + 1] = begin[g] + count[g];
+  std::vector<uint32_t> at(begin.begin(), begin.end() - 1);
+  for (uint32_t s : streams) members[at[group_of_stream[s]]++] = s;  // ascending within each group
+  const uint32_t ng = (uint32_t)streams.size();
+  Carve k;
+  merge_tables_layout(k, cs->n_streams, ng, n_groups);
+  RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+  unsigned char* block = nullptr;
+  RPL_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&block), k.bytes), RPL_RESULT_INSUFFICIENT_MEMORY);
+  Carve kb{block};
+  const MergeTables t = merge_tables_layout(kb, cs->n_streams, ng, n_groups);
+  cudaError_t e = cudaMemcpy(t.row, row.data(), row.size() * 4, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemset(t.held, 0, (size_t)cs->n_streams * sizeof(rpl::RescanHeld));
+  if (e == cudaSuccess && ng) e = cudaMemcpy(t.streams, streams.data(), (size_t)ng * 4, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && ng) e = cudaMemcpy(t.members, members.data(), (size_t)ng * 4, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(t.begin, begin.data(), begin.size() * 4, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && n_groups) e = cudaMemcpy(t.max_age, max_age, (size_t)n_groups * 4, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    cudaFree(block);
+    RPL_CUDA(c, e, RPL_RESULT_OPERATION_FAIL);
+  }
+  RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);  // a push may still read the old block
+  cudaFree(cs->mg_block);
+  cs->mg_block = block;
+  cs->mg_set = true;
+  cs->mg_groups = n_groups;
+  cs->mg_members_host = std::move(members);
+  cs->mg_begin_host = std::move(begin);
+  cs->mg_streams_host = std::move(streams);
   return RPL_RESULT_OK;
 }
 
@@ -3714,6 +3957,8 @@ rpl_result stream_set_rescans(rpl_capsule_stream* cs, const rpl_rescan_settings*
   RPL_CUDA(c, cudaEventSynchronize(cs->done), RPL_RESULT_OPERATION_FAIL);  // a messages call may still read them
   if (!cs->win_host.empty())  // the masked streams' grids may change: their windows start over
     if (const rpl_result r = windows_layout(cs, t, cs->win_host, stream_mask); r != RPL_RESULT_OK) return r;
+  if (const rpl_result r = merges_empty(cs, stream_mask, c->lane[0].stream); r != RPL_RESULT_OK) return r;
+  RPL_CUDA(c, cudaStreamSynchronize(c->lane[0].stream), RPL_RESULT_OPERATION_FAIL);
   RPL_CUDA(c, cudaMemcpy(cs->rescan, g.data(), g.size() * sizeof(rpl::RescanGrid), cudaMemcpyHostToDevice),
            RPL_RESULT_OPERATION_FAIL);
   RPL_CUDA(c, cudaMemcpy(cs->rescan_bins, bins.data(), bins.size() * 4, cudaMemcpyHostToDevice),
@@ -3744,6 +3989,8 @@ rpl_result stream_set_frames(rpl_capsule_stream* cs, const char* const* frame_id
   RPL_CUDA(c, cudaMemcpy(cs->msg_hdr, h.data(), h.size() * sizeof(rpl::StreamMsgHeader), cudaMemcpyHostToDevice),
            RPL_RESULT_OPERATION_FAIL);
   cs->msg_hdr_host = std::move(h);
+  if (const rpl_result r = merges_empty(cs, nullptr, c->lane[0].stream); r != RPL_RESULT_OK) return r;
+  RPL_CUDA(c, cudaStreamSynchronize(c->lane[0].stream), RPL_RESULT_OPERATION_FAIL);
   if (!cs->xf_host.empty())  // a disabled transform entry's header follows the frames
     if (const rpl_result r = transforms_resolve(cs, cs->xf_host, cs->xf_frames); r != RPL_RESULT_OK) return r;
   return cs->clouds_host.empty() ? RPL_RESULT_OK : clouds_resolve(cs);  // a range_max of 0 follows the frames
@@ -4260,11 +4507,54 @@ rpl_result stream_msgs(rpl_capsule_stream* cs, rpl::MsgKind kind, const void* pa
 // that flag reaches the decoders, the assembler and the stamps.
 // proj (kind kLaserScan, rpl_capsule_stream_push_scan_cloud_msgs*): each chunk also projects its LaserScan messages
 // where they lie, into clouds (DESIGN.md 5.7.1 "LaserScans and their projected clouds from the push").
+// The checks of a merge push that the set calls cannot make once for all: every group's members have equal enabled
+// re-grid entries (pad aside) and equal re-grid headers under the push's cloud_params, and the merged outputs are there
+bool merges_ok(rpl_capsule_stream* cs, const rpl_scan_cloud_params& proj, const rpl_msgs_out& merged, bool dev) {
+  rpl_ctx* c = cs->c;
+  if (!cs->mg_set) {
+    c->err = "push_rescan_merge_msgs before the first rpl_capsule_stream_set_rescan_merges";
+    return false;
+  }
+  if (!merged.msgs || !merged.msg_offsets || !merged.msg_sizes || !merged.total_bytes) {
+    c->err = "null merged->msgs, msg_offsets, msg_sizes or total_bytes";
+    return false;
+  }
+  if (dev && ((reinterpret_cast<uintptr_t>(merged.msgs) & 15u) || misaligned8(merged.msg_offsets) ||
+              misaligned8(merged.total_bytes) || (reinterpret_cast<uintptr_t>(merged.msg_sizes) & 3u))) {
+    c->err = "merged: msgs must be 16-byte aligned, msg_offsets and total_bytes 8-byte, msg_sizes 4-byte aligned";
+    return false;
+  }
+  const std::vector<rpl::StreamMsgHeader>& hs =
+      (proj.channels & rpl::kScanCloudPerStreamTransforms) ? cs->xf_hdr_host : cs->msg_hdr_host;
+  for (uint32_t g = 0; g < cs->mg_groups; ++g) {
+    const uint32_t b = cs->mg_begin_host[g], e = cs->mg_begin_host[g + 1];
+    if (b == e) {
+      c->err = "a merge group has no member";
+      return false;
+    }
+    const uint32_t f = cs->mg_members_host[b];
+    const rpl_rescan_settings& t0 = cs->rescan_host[f];
+    const rpl::StreamMsgHeader& h0 = hs[f];
+    for (uint32_t j = b; j < e; ++j) {
+      const uint32_t s = cs->mg_members_host[j];
+      if (!cs->rescan_host[s].enabled || std::memcmp(&cs->rescan_host[s], &t0, offsetof(rpl_rescan_settings, pad))) {
+        c->err = "a merge group's members need equal enabled rpl_rescan_settings entries";
+        return false;
+      }
+      if (hs[s].bytes != h0.bytes || std::memcmp(hs[s].w, h0.w, h0.bytes)) {
+        c->err = "a merge group's re-grid messages need one frame_id";
+        return false;
+      }
+    }
+  }
+  return true;
+}
+
 rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, rpl::MsgKind kind, const void* params,
                      int64_t clock_offset_ns, uint8_t* msgs, uint64_t capacity, uint64_t* msg_offsets, uint32_t* msg_sizes,
                      uint64_t* total_bytes, uint32_t* scans_per_stream, bool dev, void* stream,
                      const rpl_scan_cloud_params* proj = nullptr, const rpl_msgs_out* clouds = nullptr,
-                     bool rescan = false) {
+                     bool rescan = false, const rpl_msgs_out* merged = nullptr) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
   rpl_ctx* c = cs->c;
   cs->cloud_chunk = 0;  // as a push that fails its checks
@@ -4282,6 +4572,7 @@ rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, rpl::MsgK
       c->err = "push_rescan_msgs before the first rpl_capsule_stream_set_rescans";
       return RPL_RESULT_INVALID_DATA;
     }
+    if (merged && !merges_ok(cs, *proj, *merged, dev)) return RPL_RESULT_INVALID_DATA;
     if (dev && ((reinterpret_cast<uintptr_t>(clouds->msgs) & 15u) || misaligned8(clouds->msg_offsets) ||
                 misaligned8(clouds->total_bytes) || (reinterpret_cast<uintptr_t>(clouds->msg_sizes) & 3u))) {
       c->err = "clouds: msgs must be 16-byte aligned, msg_offsets and total_bytes 8-byte, msg_sizes 4-byte aligned";
@@ -4347,6 +4638,26 @@ rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, rpl::MsgK
       pm.proj_xf = cs->xf;
     }
   }
+  if (merged && !dev) {  // the host form's staging: the groups' directory and their messages' bound
+    uint32_t hdr_most = 0, bins_most = 0;  // a held grid's message may have taken either header
+    for (uint32_t s : cs->mg_streams_host) {
+      hdr_most = std::max(hdr_most, cs->msg_hdr_host[s].bytes);
+      if (!cs->xf_hdr_host.empty()) hdr_most = std::max(hdr_most, cs->xf_hdr_host[s].bytes);
+      bins_most = std::max(bins_most, rescan_bins(cs->rescan_host[s]));
+    }
+    Carve kd;
+    merge_stage_layout(kd, cs->mg_groups);
+    const size_t bytes = kd.bytes + (size_t)cs->mg_groups * ((hdr_most + 36 + 4 * (size_t)bins_most + 15) & ~(size_t)15);
+    if (bytes > cs->mg_stage_bytes) {
+      RPL_CUDA(c, cudaSetDevice(c->device), RPL_RESULT_OPERATION_FAIL);
+      unsigned char* b = nullptr;
+      RPL_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&b), bytes), RPL_RESULT_INSUFFICIENT_MEMORY);
+      cudaFree(cs->mg_stage);  // its last user, a host push, has synchronised
+      cs->mg_stage = b;
+      cs->mg_stage_bytes = bytes;
+    }
+  }
+  pm.merged = merged;
   if (cloud && dev) {  // one chunk's clouds, in the session's message work block (cloud_msgs' when that is larger)
     const size_t NS = (size_t)cs->chunk_dev * cs->max_scans;
     auto layout = [&](Carve& kw) {
@@ -4370,27 +4681,33 @@ rpl_result push_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, rpl::MsgK
   const rpl_result r = stream_push(cs, in->data, in->counts, sample_duration_us, sp_params, nullptr, nullptr, nullptr,
                                    nullptr, scans_per_stream, stamped ? &sp : nullptr, cs->bytes, dev, stream, &pm);
   if (r != RPL_RESULT_OK) return r;
-  if (!dev && (*total_bytes > capacity || (proj && *clouds->total_bytes > clouds->capacity))) {  // windows advanced
+  if (merged) cs->mg_seq++;
+  if (!dev && (*total_bytes > capacity || (proj && *clouds->total_bytes > clouds->capacity) ||
+               (merged && *merged->total_bytes > merged->capacity))) {  // windows and held grids advanced
     c->err = "the messages need more than capacity bytes (total_bytes tells how many; the push itself is done)";
     return RPL_RESULT_INSUFFICIENT_MEMORY;
   }
   return RPL_RESULT_OK;
 }
 
-// rescan: rpl_capsule_stream_push_rescan_msgs*, whose `clouds` are the re-grid messages
+// rescan: rpl_capsule_stream_push_rescan_msgs*, whose `clouds` are the re-grid messages; merge: a merge push
+// (rpl_capsule_stream_push_rescan_merge_msgs*), whose merged scans go into `merged`
 rpl_result push_scan_cloud_msgs(rpl_capsule_stream* cs, const rpl_push_input* in, const rpl_scan_params* scan_params,
                                 const rpl_scan_cloud_params* cloud_params, int64_t clock_offset_ns,
                                 const rpl_msgs_out* scans, const rpl_msgs_out* clouds, uint32_t* scans_per_stream,
-                                bool dev, void* stream, bool rescan = false) {
+                                bool dev, void* stream, bool rescan = false, bool merge = false,
+                                const rpl_msgs_out* merged = nullptr) {
   if (!cs) return RPL_RESULT_INVALID_DATA;
-  if (!scans || !clouds || !cloud_params) {
+  if (!scans || !clouds || !cloud_params || (merge && !merged)) {
     cs->cloud_chunk = 0;  // as a push that fails its checks
-    cs->c->err = rescan ? "null scans, rescans or cloud_params" : "null scans, clouds or cloud_params";
+    cs->c->err = merge    ? "null scans, rescans, merged or cloud_params"
+                 : rescan ? "null scans, rescans or cloud_params"
+                          : "null scans, clouds or cloud_params";
     return RPL_RESULT_INVALID_DATA;
   }
   return push_msgs(cs, in, rpl::MsgKind::kLaserScan, scan_params, clock_offset_ns, scans->msgs, scans->capacity,
                    scans->msg_offsets, scans->msg_sizes, scans->total_bytes, scans_per_stream, dev, stream,
-                   cloud_params, clouds, rescan);
+                   cloud_params, clouds, rescan, merged);
 }
 
 // ---- grabbed node buffers of the last push (DESIGN.md 5.7.1 "Session nodes") -------------------------------------
@@ -4654,6 +4971,8 @@ void rpl_capsule_stream_destroy(rpl_capsule_stream* cs) {
   cudaFree(cs->win_state);
   cudaFree(cs->win_ring);
   cudaFree(cs->win_streams);
+  cudaFree(cs->mg_block);
+  cudaFree(cs->mg_stage);
   cudaFreeHost(cs->push_scan_cloud_extent);
   if (cs->push_scan_cloud_dir_order) cudaEventDestroy(cs->push_scan_cloud_dir_order);
   if (cs->done) cudaEventDestroy(cs->done);
@@ -4724,6 +5043,7 @@ rpl_result rpl_capsule_stream_reset(rpl_capsule_stream* cs, const uint8_t* strea
       RPL_CUDA(c, cudaMemsetAsync(cs->win_state + s, 0, (size_t)(e - s) * sizeof(uint2), st), RPL_RESULT_OPERATION_FAIL);
     s = e;
   }
+  if (const rpl_result r = merges_empty(cs, stream_mask, st); r != RPL_RESULT_OK) return r;  // and the held grids
   RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);
   return RPL_RESULT_OK;
 }
@@ -5000,6 +5320,7 @@ rpl_result rpl_capsule_stream_import(rpl_capsule_stream* cs, const uint32_t* str
   // records do not carry the windows over the re-gridded scans: the destinations' start over
   if (cs->win_state)
     if (const rpl_result r = windows_empty(cs, seen.data(), st); r != RPL_RESULT_OK) return r;
+  if (const rpl_result r = merges_empty(cs, seen.data(), st); r != RPL_RESULT_OK) return r;  // nor the held grids
   RPL_CUDA(c, cudaStreamSynchronize(st), RPL_RESULT_OPERATION_FAIL);  // in place before any later push runs
   if (types != cs->types) return set_types(cs, std::move(types));     // a mixed session's streams take the record's type
   return RPL_RESULT_OK;
@@ -5283,6 +5604,31 @@ rpl_result rpl_capsule_stream_push_rescan_msgs_dev(rpl_capsule_stream* s, const 
                                                    uint32_t* scans_per_stream, void* stream) {
   return push_scan_cloud_msgs(s, in, scan_params, cloud_params, clock_offset_ns, scans, rescans, scans_per_stream, true,
                               stream, true);
+}
+
+rpl_result rpl_capsule_stream_set_rescan_merges(rpl_capsule_stream* s, const uint32_t* group_of_stream,
+                                                const uint32_t* max_age, uint32_t n_groups) {
+  return stream_set_rescan_merges(s, group_of_stream, max_age, n_groups);
+}
+
+rpl_result rpl_capsule_stream_push_rescan_merge_msgs(rpl_capsule_stream* s, const rpl_push_input* in,
+                                                     const rpl_scan_params* scan_params,
+                                                     const rpl_scan_cloud_params* cloud_params,
+                                                     int64_t clock_offset_ns, const rpl_msgs_out* scans,
+                                                     const rpl_msgs_out* rescans, const rpl_msgs_out* merged,
+                                                     uint32_t* scans_per_stream) {
+  return push_scan_cloud_msgs(s, in, scan_params, cloud_params, clock_offset_ns, scans, rescans, scans_per_stream, false,
+                              nullptr, true, true, merged);
+}
+
+rpl_result rpl_capsule_stream_push_rescan_merge_msgs_dev(rpl_capsule_stream* s, const rpl_push_input* in,
+                                                         const rpl_scan_params* scan_params,
+                                                         const rpl_scan_cloud_params* cloud_params,
+                                                         int64_t clock_offset_ns, const rpl_msgs_out* scans,
+                                                         const rpl_msgs_out* rescans, const rpl_msgs_out* merged,
+                                                         uint32_t* scans_per_stream, void* stream) {
+  return push_scan_cloud_msgs(s, in, scan_params, cloud_params, clock_offset_ns, scans, rescans, scans_per_stream, true,
+                              stream, true, true, merged);
 }
 
 rpl_result rpl_capsule_stream_set_rescans(rpl_capsule_stream* s, const rpl_rescan_settings* settings,
